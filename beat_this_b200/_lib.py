@@ -1,7 +1,7 @@
-"""ctypes binding of libbeatthis_sm100.so (C ABI in include/beatthis.h).
+"""ctypes binding of libbeatthis_sm90.so (C ABI in include/beatthis.h).
 
 The library is built in-tree by ``__graft_entry__.build()`` / ``beat_this_b200._lib.build()``
-(nvcc, sm_100a).  There is no fallback: if the shared object is missing or no sm_100 GPU is
+(nvcc, sm_90a).  There is no fallback: if the shared object is missing or no sm_90 GPU is
 present, loading / ``bt_create`` fails loudly.
 """
 from __future__ import annotations
@@ -14,7 +14,7 @@ from ctypes import POINTER, c_char_p, c_double, c_float, c_int, c_int32, c_int64
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 # BT_LIB_PATH: an instrumented build of the same sources (e.g. build(extra_flags=("-DBT_FF_PROF",), out_path=...))
-LIB_PATH = os.environ.get("BT_LIB_PATH") or os.path.join(HERE, "libbeatthis_sm100.so")
+LIB_PATH = os.environ.get("BT_LIB_PATH") or os.path.join(HERE, "libbeatthis_sm90.so")
 SOURCES = ["bt_api.cu", "kernels_simt.cu", "kernels_misc.cu", "kernels_gemm.cu", "kernels_attn.cu", "kernels_fused.cu", "dbn_host.cpp", "host_stage.cpp"]
 HEADERS = ["common.cuh", "epilogue.cuh", "tc_common.cuh", "bt_kernels.h", os.path.join("..", "..", "include", "beatthis.h")]
 
@@ -102,7 +102,8 @@ _lib = None
 
 
 OBJ_DIR = os.path.join(CSRC, "_obj")
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = [*ARCH, "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC"]
 
 
 def _nvcc() -> str:
@@ -123,7 +124,7 @@ def needs_build() -> bool:
 
 
 def build(force: bool = False, verbose: bool = False, extra_flags: tuple = (), out_path: str = LIB_PATH) -> str:
-    """Compile the CUDA library for sm_100a (cross-compiles without a GPU): one nvcc -c per source, in parallel,
+    """Compile the CUDA library for sm_90a (cross-compiles without a GPU): one nvcc -c per source, in parallel,
     objects cached under csrc/_obj (keyed by flags), then one link step."""
     from concurrent.futures import ThreadPoolExecutor
 
@@ -151,7 +152,7 @@ def build(force: bool = False, verbose: bool = False, extra_flags: tuple = (), o
     if errors:
         raise RuntimeError("nvcc failed:\n" + "\n".join(errors))
     tmp = out_path + f".tmp{os.getpid()}"
-    cmd = [_nvcc(), "-shared", "-gencode", "arch=compute_100a,code=sm_100a", *[o for o, _ in results], "-o", tmp]
+    cmd = [_nvcc(), "-shared", *ARCH, *[o for o, _ in results], "-o", tmp]
     res = subprocess.run(cmd, capture_output=True, text=True)
     if res.returncode != 0:
         raise RuntimeError(f"nvcc link failed:\n{res.stdout}\n{res.stderr}")
@@ -166,7 +167,7 @@ def load() -> ctypes.CDLL:
         return _lib
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
-            f"{LIB_PATH} is missing: the sm_100a CUDA library has not been built. Run "
+            f"{LIB_PATH} is missing: the sm_90a CUDA library has not been built. Run "
             "`python -c 'import __graft_entry__ as g; g.build()'` (or beat_this_b200._lib.build()). "
             "There is no CPU or PyTorch fallback."
         )

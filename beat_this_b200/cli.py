@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""``beat_this`` command line tool on the B200 engine (reference beat_this/cli.py:22-191: same options, same
+"""``beat_this`` command line tool on the H100 engine (reference beat_this/cli.py:22-191: same options, same
 output naming, same ``.beats`` / ``.npy`` files), re-organised around the batched device path: the work list is
 built first, then ``--batch`` files at a time are claimed and handed to ``File2Beats.batch`` (native WAV decode on
 host threads -> pinned ring -> device, groups of one sample rate share launches, decode of the next group overlaps
@@ -23,7 +23,7 @@ from .utils import save_beat_tsv
 
 
 def build_parser() -> argparse.ArgumentParser:
-    ap = argparse.ArgumentParser(prog="beat_this_b200", description="Beat and downbeat times for audio files (Beat This! model on the B200 engine).")
+    ap = argparse.ArgumentParser(prog="beat_this_b200", description="Beat and downbeat times for audio files (Beat This! model on the H100 engine).")
     add = ap.add_argument
     add("inputs", nargs="+", help="audio files and/or directories that are searched recursively")
     add("--model", default="final0", help="checkpoint name or path [%(default)s]")

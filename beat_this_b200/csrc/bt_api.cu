@@ -1,6 +1,6 @@
 // C ABI (include/beatthis.h): context, packed-parameter registry, chunk planner, workspace
 // and the per-wave schedule of the BeatThis forward pass (reference
-// beat_this/model/beat_tracker.py:188-192, math restated in SURVEY.md App. A.3).
+// beat_this/model/beat_tracker.py:188-192).
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -627,7 +627,7 @@ int run_wave(bt_ctx* c, const float* spect, const Wave& wv, float* beat, float* 
 struct HostChunk { ChunkSrc s; int len; };
 
 // upload the chunk table and run the forward pass in waves of up to ws_wave chunks, longest first.  A wave is padded
-// to its longest chunk: a shorter chunk costs its padded share of one wave (<= 0.35 ms on B200) instead of ~90
+// to its longest chunk: a shorter chunk costs its padded share of one wave (a fraction of a millisecond) instead of ~90
 // launches of its own (~0.7 ms of fixed cost), so chunks of all lengths share waves
 int run_chunks(bt_ctx* c, const float* spect_dev, std::vector<HostChunk>& all, float* beat_dev, float* downbeat_dev,
                cudaStream_t st) {
@@ -718,8 +718,8 @@ int bt_create(bt_ctx** out, int device_ordinal, const bt_hparams* hp, int comput
     return fail(nullptr, BT_ERR_CUDA, "cudaSetDevice: %s", cudaGetErrorString(e));
   cudaDeviceProp prop;
   cudaGetDeviceProperties(&prop, device_ordinal);
-  if (prop.major != 10)
-    return fail(nullptr, BT_ERR_CUDA, "bt_create: device is sm_%d%d; this library is built for sm_100a only",
+  if (prop.major != 9 || prop.minor != 0)
+    return fail(nullptr, BT_ERR_CUDA, "bt_create: device is sm_%d%d; this library is built for sm_90a only",
                 prop.major, prop.minor);
   bt_ctx* c = new bt_ctx();
   c->device = device_ordinal;
@@ -1207,8 +1207,6 @@ int bt_debug_attention_time(bt_ctx* c, int32_t seqs, int32_t L, int32_t heads, i
   if (!p) rc = fail(c, BT_ERR_CUDA, "%s", err);
   else {
     if (variant >= 0) attn_set_variant(variant);
-    unsigned long long prof[40];
-    attn_prof_read(prof, true);
     cudaEvent_t e0, e1;
     cudaEventCreate(&e0); cudaEventCreate(&e1);
     for (int i = 0; i < 2 && rc == BT_OK; ++i)
@@ -1221,16 +1219,6 @@ int bt_debug_attention_time(bt_ctx* c, int32_t seqs, int32_t L, int32_t heads, i
     float ms = 0.f;
     cudaEventElapsedTime(&ms, e0, e1);
     *ms_per_launch = ms / iters;
-    if (variant >= 0 && (variant & 64)) {
-      attn_prof_read(prof, true);
-      for (int w = 0; w < 4; ++w) {
-        const unsigned long long* q = prof + 8 * w;
-        const double n = static_cast<double>(q[6] ? q[6] : 1);  // warp-tiles
-        fprintf(stderr, "attention phases, warp %d, cycles per tile: wait S %.0f | ld S %.0f | max %.0f | exp %.0f | wait PV %.0f | st P %.0f\n",
-                w, q[0] / n, q[1] / n, q[2] / n, q[3] / n, q[4] / n, q[5] / n);
-      }
-      if (prof[34]) fprintf(stderr, "issuer warp, cycles per tile: wait P %.0f | rest %.0f\n", prof[32] / double(prof[34]), prof[33] / double(prof[34]));
-    }
     cudaEventDestroy(e0); cudaEventDestroy(e1);
     tc_attn_plan_destroy(p);
     if (variant >= 0) attn_set_variant(-1);

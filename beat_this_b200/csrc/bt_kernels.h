@@ -1,4 +1,4 @@
-// Internal kernel-launcher interface shared by the .cu files of libbeatthis_sm100.so.
+// Internal kernel-launcher interface shared by the .cu files of libbeatthis_sm90.so.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -25,7 +25,7 @@ struct GemmShape {
   int lda;
 };
 
-// Epilogue description (shared by the fp32 CUDA-core GEMM and the 16-bit tcgen05 GEMM).
+// Epilogue description (shared by the fp32 CUDA-core GEMM and the 16-bit wgmma GEMM).
 struct EpiParams {
   int kind;            // 0 generic, 1 qkv (RoPE + q scaling), 2 attention gates:
                        //   out_f32[m*heads + n] = sigmoid(acc + bias[n]) for n < heads (N padded to 32)
@@ -100,7 +100,7 @@ void launch_h16_to_f32(const void* in, float* out, int64_t n, cudaStream_t st);
 void launch_pack_qkv_test(const float* q, const float* k, const float* v, void* qkv, int seqs, int L,
                           int heads, float qscale, int act_h16, cudaStream_t st);
 
-// ---- 16-bit (fp16 or bf16 operands) tcgen05 path ------------------------------------------------------------------------
+// ---- 16-bit (fp16 or bf16 operands) tensor-core path (wgmma GEMM, mma.sync attention) ---------------------------------
 struct TcGemmPlan;  // cached tensor maps + launch geometry
 TcGemmPlan* tc_gemm_plan_create(const void* A_h16, const void* W_h16, const GemmShape& g,
                                 int planes_in, char* err, int errlen);
@@ -110,8 +110,7 @@ int launch_gemm_tc(const TcGemmPlan* plan, const EpiParams& e, cudaStream_t st);
 struct TcAttnPlan;
 TcAttnPlan* tc_attn_plan_create(const void* qkv_h16, int seqs, int L, int heads, char* err, int errlen);
 void tc_attn_plan_destroy(TcAttnPlan*);
-void attn_prof_read(unsigned long long* out40, bool reset);  // debug: phase cycle counters of variant bit 64
-void attn_set_variant(int v);  // debug: template parameter V of attn_tc48_kernel (kernels_attn.cu)
+void attn_set_variant(int v);  // debug: template parameter V of attn_time_kernel (kernels_attn.cu)
 int launch_attn_time_tc(const TcAttnPlan* plan, const float* gates, void* out_h16, cudaStream_t st,
                         const ChunkSrc* chunks = nullptr, int seqs_per_chunk = 1);
 

@@ -1,5 +1,5 @@
-// Shared device helpers for the sm_100a kernels: mbarrier, TMA, tcgen05 / TMEM wrappers
-// (inline PTX), small math helpers.  No torch, no CUTLASS.
+// Shared device helpers for the sm_90a kernels: mbarrier and TMA wrappers (inline PTX), small math helpers.
+// No torch, no CUTLASS.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -12,7 +12,7 @@ namespace bt {
 // 16-bit operand type of the tensor-core path (BT_DTYPE_H16).  Default: IEEE fp16 -- the dtype the reference's
 // float16=True autocasts to on CUDA (beat_this/inference.py:245-246); every operand on this path is RMS-normalised,
 // a folded weight, a softmax probability <= 2^8 or a GELU output, all far inside fp16 range, and its 11-bit
-// significand cuts the logit error of the bf16 build ~8x at the same tcgen05 rate.  -DBT_ACT_BF16 builds bf16.
+// significand cuts the logit error of the bf16 build ~8x at the same tensor-core rate.  -DBT_ACT_BF16 builds bf16.
 #if defined(BT_ACT_BF16)
 typedef __nv_bfloat16 h16;
 #define BT_H16_IS_F16 0
@@ -153,9 +153,6 @@ __device__ __forceinline__ void mbar_wait_a(uint32_t bar, uint32_t parity) {
     }
   }
 }
-__device__ __forceinline__ void umma_commit_a(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
 __device__ __forceinline__ void tma_load_3d_a(uint32_t smem_dst, const void* tmap, uint32_t bar, int32_t c0, int32_t c1,
                                               int32_t c2) {
   asm volatile(
@@ -201,86 +198,9 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const void* tmap, ui
       "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
-// generic-proxy smem writes -> visible to the async proxy (TMA / tcgen05.mma operand reads)
+// generic-proxy smem writes -> visible to the async proxy (TMA / wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
-
-// ----------------------------------------------------------------------------- PTX: tcgen05
-template <int COLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_result)),
-               "n"(COLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int COLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(COLS)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]; h16 x h16 -> fp32, issued by ONE thread.
-__device__ __forceinline__ void umma_h16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                          uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// mbarrier arrives once all previously issued tcgen05.mma of this thread have completed
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-          smem_u32(bar))
-      : "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns: thread i of the warp gets row (lane base + i).
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]),
-        "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]),
-        "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// UMMA shared-memory matrix descriptor, K-major operand, swizzled canonical layout
-// (rows of SWIZZLE_BYTES bytes, 8-row groups SBO apart):
-//   bits [0,14) start>>4 | [16,30) LBO>>4 (=1, unused for swizzled K-major) |
-//   [32,46) SBO>>4 | [46,48) version=1 | [61,64) layout (2 = 128B swizzle, 4 = 64B swizzle)
-template <int SWIZZLE_BYTES>
-__device__ __forceinline__ uint64_t make_kmajor_desc(uint32_t smem_addr) {
-  static_assert(SWIZZLE_BYTES == 128 || SWIZZLE_BYTES == 64, "swizzle");
-  constexpr uint64_t layout = SWIZZLE_BYTES == 128 ? 2 : 4;
-  constexpr uint64_t sbo = (8 * SWIZZLE_BYTES) >> 4;
-  return static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4) | (1ull << 16) | (sbo << 32) |
-         (1ull << 46) | (layout << 61);
-}
-// tcgen05 instruction descriptor, kind::f16: h16 A/B (K-major both), fp32 accumulate.
-//   bits [4,6) D format (1 = f32) | [7,10) A format, [10,13) B format (0 = f16, 1 = bf16) | [15] A MN-major |
-//   [16] B MN-major | [17,23) N >> 3 | [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc_h16(int M, int N) {
-  constexpr uint32_t fmt = BT_H16_IS_F16 ? 0u : 1u;
-  return (1u << 4) | (fmt << 7) | (fmt << 10) | (static_cast<uint32_t>(N >> 3) << 17) |
-         (static_cast<uint32_t>(M >> 4) << 24);
 }
 
 }  // namespace bt

@@ -1,6 +1,6 @@
-// tcgen05 flash attention for head_dim 32 over sequences of up to 1500 frames: the time-direction
+// Tensor-core flash attention for head_dim 32 over sequences of up to 1500 frames: the time-direction
 // attention of the three frontend blocks and of the 6 main layers (reference roformer.py:73-80 SDPA,
-// called from roformer.py:114-132 / beat_tracker.py:290-301).  P and O live in tensor memory.
+// called from roformer.py:114-132 / beat_tracker.py:290-301).
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -9,102 +9,47 @@
 
 namespace bt {
 
+// CTA = 128 queries of one (sequence, head): 8 MMA warps of 16 query rows each + 1 producer warp.  The producer
+// TMA-loads Q once and the K / V tiles of 64 keys through an AT_NST-deep ring of mbarriers (64-byte swizzled rows,
+// the layout ldmatrix reads without bank conflicts).  Each MMA warp keeps S, P and O in registers
+// (mma.sync m16n8k16, fp32 accumulate): S = Q K^T -> online softmax in log2 units (q carries scale * log2 e) ->
+// P packed to 16 bits straight from the S accumulator layout -> O += P V.  With head_dim 32 there are only 128
+// tensor FLOPs per exponential: the exponentials (MUFU.EX2, 16 /clk/SM) bound the kernel, so a share of them can
+// run as a polynomial on the FMA pipe instead (template parameter V).
 constexpr int AT_BQ = 128;
-constexpr int AT_SQ = 8192;
-constexpr float AT_TAU = 8.0f;  // log2 units: rescale O only when the row maximum grew by more than this
-
-constexpr int AT_THREADS = 160;  // 4 softmax warps (one thread per query row) + 1 issuer warp
+constexpr int AT_BKV = 64;
+constexpr int AT_NST = 4;
+constexpr int AT_WARPS = 8;
+constexpr int AT_THREADS = 32 * (AT_WARPS + 1);
+constexpr int AT_SQ = AT_BQ * 64;    // 128 query rows x 32 dims x 2 bytes
+constexpr int AT_SKV = AT_BKV * 64;  // 64 key rows x 32 dims x 2 bytes
+constexpr int AT_SMEM = 1024 + AT_SQ + AT_NST * 2 * AT_SKV + 128;
 
 // which of every 8 score pairs take the polynomial exp2 (spread out so that MUFU and FMA work interleave)
 __host__ __device__ constexpr uint32_t attn_poly_mask(int pp) {
   return pp == 0 ? 0x00u : pp == 1 ? 0x08u : pp == 2 ? 0x44u : pp == 3 ? 0x52u : pp == 4 ? 0xAAu : pp == 5 ? 0xB5u : pp == 6 ? 0xBBu : 0xFFu;
 }
 
-// V & 64: cycles per softmax phase, [warp 0..3][phase 0..5, tiles, -] + [32..] issuer warp: wait P, rest, tiles
-__device__ unsigned long long g_attn_prof[40];
-
-// ---------------------------------------------------------------------------------------------------------------------
-// CTA = 128 queries of one (sequence, head): 4 softmax warps (ONE thread per query row: no partial-maximum
-// exchange) + 1 issuer warp; FOUR CTAs per SM (128 TMEM columns, 92 registers, 33 KB shared memory each), i.e. four
-// softmax warps per SM sub-partition, each from a different CTA.  Keys come in tiles of 48:
-//   TMEM  S0|P0 [0,48) | S1|P1 [48,96) | O [96,128)        (P_j, 24 columns of fp16 pairs, is written over S_j by the
-//                                                           warp that has just read those lanes)
-//   issuer, per tile:  wait "all P_j stored"  ->  PV_j (3 MMAs, P from tensor memory)  ->  S_{j+2} (2 MMAs) queued right
-//                      behind it: tcgen05.mma executes in issue order, so S_{j+2} overwrites the buffer of P_j only after
-//                      PV_j has read it -- one wake-up of the issuer per tile, S ready a whole tile before it is needed
-//   softmax, per tile: wait S_j -> tcgen05.ld -> row max -> lazy rescale -> exp2 -> tcgen05.st P_j -> arrive
-// With head_dim 32 there are only 128 tensor FLOPs per exponential: the kernel is bound by MUFU.EX2 (16 /clk/SM), the
-// tensor pipe is 20 % busy.  What the round-2 measurements showed (profiles/r2_notes.md, tools/attn_ubench.py,
-// tools/ubench_mufu_warps.cu):
-//   * one warp per sub-partition reaches 47 % of the MUFU rate with the instruction order ptxas emits (pack / sum
-//     right behind their two MUFU.EX2), two warps 88 %, three 97 %: every cycle in which fewer than three of the
-//     four softmax warps of a sub-partition are inside their exponential section costs MUFU time;
-//   * 3 of every 8 score pairs therefore take a Cody-Waite + degree-3 polynomial on packed fp32 (FFMA2): -8 % time;
-//     it pays only now that the kernel has registers to spare (64-key tiles: 96 registers and spills, slower);
-//   * 48-key tiles + the ordering above: -2.4 % against 64-key tiles with one S buffer (S_{j+1} after all four warps
-//     had read S_j, P_j stored only after PV_{j-1});
-//   * measured and dropped: exponentials before the row maximum with a redo when the maximum grew (slower: the redo
-//     path's second tcgen05.ld and the longer live ranges), P stores completed one tile later (slower), early
-//     non-blocking probe of the S barrier (no change), 16 exponentials issued back to back before any pack
-//     (slower: the MUFU burst holds up the other warps' tcgen05.ld / st / mbarrier instructions in the same queue).
-constexpr int A4_BKV = 48, A4_NST = 4;
-constexpr int A4_SK = A4_BKV * 64, A4_SV = A4_BKV * 64;
-constexpr int A4_SMEM = AT_SQ + A4_NST * (A4_SK + A4_SV) + 1024 + 128;
-constexpr uint32_t A4_TM_O = 96;
-
-__device__ __forceinline__ void mbar_wait_q(uint32_t bar, uint32_t parity) {  // bounded spin, trap without printf: no call in the hot loop
-  uint32_t spins = 0;
-  for (;;) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(bar), "r"(parity)
-        : "memory");
-    if (ok) break;
-    if (++spins > (1u << 26)) __trap();
-  }
-}
-
-// P = exp2(S - m) for score pairs [Q0, Q1) of a row: packed fp32 subtract / row-sum (FADD2), two MUFU.EX2, one pack
-template <int Q0, int Q1, bool NOEXP, uint32_t POLY = 0u>
-__device__ __forceinline__ void softmax_pairs(const float (&s)[A4_BKV], uint64_t m2, uint32_t (&pk)[A4_BKV / 2], uint64_t (&ls2)[2]) {
-#pragma unroll
-  for (int q = Q0; q < Q1; ++q) {
-    const uint64_t x2 = sub_f32x2(pack_f32x2(s[2 * q], s[2 * q + 1]), m2);
-    float p0, p1;
-    if (!NOEXP && ((POLY >> (q & 7)) & 1u)) {
-      unpack_f32x2(ex2_poly_f32x2(x2), p0, p1);
-    } else {
-      unpack_f32x2(x2, p0, p1);
-      if (!NOEXP) { p0 = ex2_approx(p0); p1 = ex2_approx(p1); }
-    }
-    pk[q] = pack_h16x2(p0, p1);
-    ls2[q & 1] = add_f32x2(ls2[q & 1], pack_f32x2(p0, p1));
-  }
+// byte offset of 16-byte chunk c of row r in a tile of 64-byte rows written by TMA with CU_TENSOR_MAP_SWIZZLE_64B
+__device__ __forceinline__ uint32_t sw64_off(int r, int c) {
+  return static_cast<uint32_t>(r * 64 + ((c ^ ((r >> 1) & 3)) << 4));
 }
 
 // V: bits 0, 2, 3 = how many of every 8 score pairs take the polynomial (1 + 2 + 4) | bit 1 = timing ablation without
-// exponentials (wrong results) | bit 5 = S_{j+2} queued right behind PV_j (else only after PV_j has completed) |
-// bit 6 = phase cycle counters (g_attn_prof)
+// exponentials (wrong results)
 template <int V>
-__global__ void __launch_bounds__(AT_THREADS, 4)
-attn_tc48_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
+__global__ void __launch_bounds__(AT_THREADS, 2)
+attn_time_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
                  const float* __restrict__ gates, h16* __restrict__ out, int L, int heads,
                  const ChunkSrc* __restrict__ chunks, int seqs_per_chunk) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t sQ = sbase;
-  const uint32_t sK = sQ + AT_SQ;             // [A4_NST] 48 keys x 32 dims, SW64 K-major
-  const uint32_t sV = sK + A4_NST * A4_SK;    // [A4_NST] 48 keys x 32 dims, used as MN-major B operand
-  const uint32_t bar_q = sV + A4_NST * A4_SV;
-  const uint32_t bar_kv = bar_q + 8;          // [A4_NST]
-  const uint32_t bar_s = bar_kv + 8 * A4_NST; // [2] S_j complete (buffer j & 1)
-  const uint32_t bar_p = bar_s + 16;          // [2] all 128 rows of P_j stored
-  const uint32_t bar_pv = bar_p + 16;         // [2] PV_j complete: O holds tiles 0..j, buffer j & 1 and K/V stage j are free
-  const uint32_t tmem_slot = bar_pv + 16;
+  const uint32_t sK = sQ + AT_SQ;              // [AT_NST] key tiles
+  const uint32_t sV = sK + AT_NST * AT_SKV;    // [AT_NST] value tiles
+  const uint32_t bar_q = sV + AT_NST * AT_SKV;
+  const uint32_t full = bar_q + 8;             // [AT_NST] K and V of a tile landed
+  const uint32_t empty = full + 8 * AT_NST;    // [AT_NST] every MMA warp is done with the stage
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int q0 = blockIdx.x * AT_BQ;
@@ -113,231 +58,140 @@ attn_tc48_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
   const int C = heads * 32;
   // keys that exist for this sequence: the whole plane, or (waves of chunks of different lengths) its chunk's frames
   const int Lk = chunks ? chunks[seq / seqs_per_chunk].len : L;
-  const int nkv = ceil_div(Lk, A4_BKV);
-  constexpr int MMA_WARP = 4;
-  constexpr int NSOFT = 128;
-  // pairs (mod 8) whose exp2 runs as a polynomial on the FMA pipe: V bits 0, 2, 3 = how many of every 8
+  const int nkv = ceil_div(Lk, AT_BKV);
   constexpr uint32_t PM = attn_poly_mask((V & 1) + ((V & 4) ? 2 : 0) + ((V & 8) ? 4 : 0));
+  constexpr bool NOEXP = (V & 2) != 0;
 
-  if (warp == MMA_WARP && lane == 0) {
-    tma_prefetch_desc(&tmQ);
-    tma_prefetch_desc(&tmKV);
-    auto init = [](uint32_t bar, uint32_t count) {
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-    };
-    init(bar_q, 1);
-    for (int i = 0; i < A4_NST; ++i) init(bar_kv + 8 * i, 1);
-    init(bar_s, 1); init(bar_s + 8, 1);
-    init(bar_p, NSOFT); init(bar_p + 8, NSOFT);
-    init(bar_pv, 1); init(bar_pv + 8, 1);
+  if (threadIdx.x == 0) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar_q), "r"(1));
+    for (int i = 0; i < AT_NST; ++i) {
+      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(full + 8 * i), "r"(1));
+      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(empty + 8 * i), "r"(AT_WARPS));
+    }
     fence_barrier_init();
   }
-  if (warp == MMA_WARP) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "n"(128) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot) : "memory");
 
-  if (warp == MMA_WARP) {
-    const uint32_t on = elect_one() ? 1u : 0u;  // converged issuer warp: single-lane instructions are predicated
-    constexpr uint32_t idesc_s = make_idesc_h16(128, A4_BKV);
-    constexpr uint32_t idesc_o = make_idesc_h16(128, 32) | (1u << 16);  // bit 16: B is MN-major
-    auto load_kv = [&](int j) {
-      const int st = j % A4_NST;
-      mbar_expect_tx_p(on, bar_kv + 8 * st, A4_SK + A4_SV);
-      tma_load_3d_p(on, sK + st * A4_SK, &tmKV, bar_kv + 8 * st, C + h * 32, j * A4_BKV, seq);
-      tma_load_3d_p(on, sV + st * A4_SV, &tmKV, bar_kv + 8 * st, 2 * C + h * 32, j * A4_BKV, seq);
-    };
-    auto issue_s = [&](int j) {
-      mbar_wait_q(bar_kv + 8 * (j % A4_NST), (j / A4_NST) & 1);
-      tc_fence_after();
-      const uint32_t kb = sK + (j % A4_NST) * A4_SK;
-#pragma unroll
-      for (int k = 0; k < 2; ++k)
-        umma_h16_p(on, tmem_base + (j & 1) * A4_BKV, make_kmajor_desc<64>(sQ + k * 32), make_kmajor_desc<64>(kb + k * 32),
-                    idesc_s, k != 0 ? 1u : 0u);
-      umma_commit_p(on, bar_s + 8 * (j & 1));
-    };
-    mbar_expect_tx_p(on, bar_q, AT_SQ);
-    tma_load_3d_p(on, sQ, &tmQ, bar_q, h * 32, q0, seq);
-    for (int j = 0; j < A4_NST && j < nkv; ++j) load_kv(j);
-    mbar_wait_q(bar_q, 0);
-    issue_s(0);
-    if (nkv > 1) issue_s(1);
-    long long tw = 0, tr = 0, tm0 = (V & 64) ? clock64() : 0;
-    for (int j = 0; j < nkv; ++j) {
-      if ((V & 32) && j >= 1 && j - 1 + A4_NST < nkv) {  // PV_{j-1} finished long ago: refill its K/V stage
-        mbar_wait_q(bar_pv + 8 * ((j - 1) & 1), ((j - 1) >> 1) & 1);
-        load_kv(j - 1 + A4_NST);
-      }
-      if (V & 64) { const long long t_ = clock64(); tr += t_ - tm0; tm0 = t_; }
-      mbar_wait_q(bar_p + 8 * (j & 1), (j >> 1) & 1);
-      tc_fence_after();
-      if (V & 64) { const long long t_ = clock64(); tw += t_ - tm0; tm0 = t_; }
-      const uint32_t vb = sV + (j % A4_NST) * A4_SV;
-#pragma unroll
-      for (int k = 0; k < A4_BKV / 16; ++k)  // 16 keys = 8 TMEM columns of P per MMA
-        umma_h16_ts_p(on, tmem_base + A4_TM_O, tmem_base + (j & 1) * A4_BKV + k * 8, make_mnmajor_desc_sw64(vb + k * 1024, 0),
-                       idesc_o, (j != 0 || k != 0) ? 1u : 0u);
-      umma_commit_p(on, bar_pv + 8 * (j & 1));
-      if (V & 32) {
-        // tcgen05.mma instructions execute in issue order: S_{j+2}, which overwrites the buffer of P_j, is queued right
-        // behind PV_j -- one wake-up of this warp per tile, and S is ready a whole tile before it is needed
-        if (j + 2 < nkv) issue_s(j + 2);
-      } else if (j + 2 < nkv) {
-        mbar_wait_q(bar_pv + 8 * (j & 1), (j >> 1) & 1);  // PV_j done: its S/P buffer and its K/V stage are free
-        if (j + A4_NST < nkv) load_kv(j + A4_NST);
-        issue_s(j + 2);
-      }
-    }
-    if ((V & 64) && lane == 0) {
-      atomicAdd(&g_attn_prof[32], static_cast<unsigned long long>(tw));
-      atomicAdd(&g_attn_prof[33], static_cast<unsigned long long>(tr));
-      atomicAdd(&g_attn_prof[34], static_cast<unsigned long long>(nkv));
-    }
-  } else {
-    const int row = warp * 32 + lane;
-    const uint32_t lane_base = static_cast<uint32_t>(warp * 32) << 16;
-    float m_ref = -INFINITY, l = 0.f;
-    const uint32_t o_tmem = tmem_base + lane_base + A4_TM_O;
-    const bool dead = q0 + warp * 32 >= L;  // all 32 rows are padding: keep the barrier protocol only
-    if (dead) {
+  if (warp == AT_WARPS) {  // producer
+    if (lane == 0) {
+      tma_prefetch_desc(&tmQ);
+      tma_prefetch_desc(&tmKV);
+      mbar_expect_tx_a(bar_q, AT_SQ);
+      tma_load_3d_a(sQ, &tmQ, bar_q, h * 32, q0, seq);
       for (int j = 0; j < nkv; ++j) {
-        mbar_wait_q(bar_s + 8 * (j & 1), (j >> 1) & 1);
-        mbar_arrive_a(bar_p + 8 * (j & 1));
+        const int st = j % AT_NST;
+        if (j >= AT_NST) mbar_wait_a(empty + 8 * st, ((j / AT_NST) - 1) & 1);
+        mbar_expect_tx_a(full + 8 * st, 2 * AT_SKV);
+        tma_load_3d_a(sK + st * AT_SKV, &tmKV, full + 8 * st, C + h * 32, j * AT_BKV, seq);
+        tma_load_3d_a(sV + st * AT_SKV, &tmKV, full + 8 * st, 2 * C + h * 32, j * AT_BKV, seq);
       }
     }
-    long long tp[6] = {0, 0, 0, 0, 0, 0}, tc0 = 0;
-#define BT_TICK(i_) if (V & 64) { const long long t_ = clock64(); tp[i_] += t_ - tc0; tc0 = t_; }
-    if (V & 64) tc0 = clock64();
-    for (int j = 0; j < (dead ? 0 : nkv); ++j) {
-      const uint32_t sp_tmem = tmem_base + lane_base + (j & 1) * A4_BKV;  // S_j, then P_j
-      mbar_wait_q(bar_s + 8 * (j & 1), (j >> 1) & 1);
-      tc_fence_after();
-      if (j == 0) { BT_TICK(4) } else { BT_TICK(0) }  // slot 4: start-up until S_0 is there
-      float s[A4_BKV];
-      int lim = A4_BKV;
-      auto load_s = [&]() {
-        uint32_t r0[32], r1[16];
-        tmem_ld_32x32b_x32(sp_tmem, r0);
-        tmem_ld_32x32b_x16(sp_tmem + 32, r1);
-        tmem_ld_wait();
+    return;
+  }
+
+  const int r0 = warp * 16;  // this warp's query rows [r0, r0 + 16) of the tile; the thread holds rows lane/4 and +8
+  mbar_wait_a(bar_q, 0);
+  uint32_t qa[2][4];
 #pragma unroll
-        for (int i = 0; i < 32; ++i) s[i] = __uint_as_float(r0[i]);
+  for (int ks = 0; ks < 2; ++ks) ldmatrix_x4(sQ + sw64_off(r0 + (lane & 15), 2 * ks + (lane >> 4)), qa[ks]);
+
+  float o[4][4];
 #pragma unroll
-        for (int i = 0; i < 16; ++i) s[32 + i] = __uint_as_float(r1[i]);
-        if (j == nkv - 1) {
-          lim = Lk - j * A4_BKV;  // keys >= lim are padding
+  for (int d = 0; d < 4; ++d) o[d][0] = o[d][1] = o[d][2] = o[d][3] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  for (int j = 0; j < nkv; ++j) {
+    const int st = j % AT_NST;
+    mbar_wait_a(full + 8 * st, (j / AT_NST) & 1);
+    const uint32_t kb = sK + st * AT_SKV, vb = sV + st * AT_SKV;
+    float s[8][4];
 #pragma unroll
-          for (int i = 0; i < A4_BKV; ++i)
-            if (i >= lim) s[i] = -INFINITY;
-        }
-      };
-      load_s();
-      BT_TICK(1)
-      auto rowmax = [&]() {  // four independent chains of 3-input maxima (FMNMX3, ALU pipe)
-        float mq[4];
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          float m = max3f(s[12 * k], s[12 * k + 1], s[12 * k + 2]);
-#pragma unroll
-          for (int i = 3; i < 11; i += 2) m = max3f(m, s[12 * k + i], s[12 * k + i + 1]);
-          mq[k] = fmaxf(m, s[12 * k + 11]);
-        }
-        return fmaxf(max3f(mq[0], mq[1], mq[2]), mq[3]);
-      };
-      // P = exp2(S - m_ref): with head_dim 32 there are only 128 tensor FLOPs per exponential, the kernel is bound by
-      // MUFU.EX2 (16 /clk/SM).  Thirds of the tile without any existing key are skipped (warp-uniform).
-      uint32_t pk[A4_BKV / 2];
-      uint64_t ls2[2];
-      auto exps = [&](float mref) {
-        const uint64_t m2 = pack_f32x2(mref, mref);
-        ls2[0] = ls2[1] = 0ull;
-        softmax_pairs<0, 8, (V & 2) != 0, PM>(s, m2, pk, ls2);
-        if (lim > 16) softmax_pairs<8, 16, (V & 2) != 0, PM>(s, m2, pk, ls2);
-        else {
-#pragma unroll
-          for (int q = 8; q < 16; ++q) pk[q] = 0u;
-        }
-        if (lim > 32) softmax_pairs<16, 24, (V & 2) != 0, PM>(s, m2, pk, ls2);
-        else {
-#pragma unroll
-          for (int q = 16; q < 24; ++q) pk[q] = 0u;
-        }
-      };
-      constexpr bool redo = true;
-      if (redo) {  // always at j = 0 (m_ref = -inf); rare afterwards
-        const float mx = rowmax();
-        const bool need = mx > m_ref + AT_TAU;
-        const float a_corr = (need && j > 0) ? ex2_approx(m_ref - mx) : 1.0f;
-        if (need) { m_ref = mx; l *= a_corr; }
-        exps(m_ref);
-        if (j >= 1 && __any_sync(0xffffffffu, need)) {  // O holds tiles 0..j-1 once PV_{j-1} is done
-          if (V & 64) tp[4] += 1000000;  // (counted in the "wait PV" slot: one million per rescaled tile)
-          mbar_wait_q(bar_pv + 8 * ((j - 1) & 1), ((j - 1) >> 1) & 1);
-          tc_fence_after();
-          uint32_t r[32];
-          tmem_ld_32x32b_x32(o_tmem, r);
-          tmem_ld_wait();
-#pragma unroll
-          for (int d = 0; d < 32; ++d) r[d] = __float_as_uint(__uint_as_float(r[d]) * a_corr);
-          tmem_st_32x32b_x16(o_tmem, *reinterpret_cast<uint32_t (*)[16]>(&r[0]));
-          tmem_st_32x32b_x16(o_tmem + 16, *reinterpret_cast<uint32_t (*)[16]>(&r[16]));
-        }
-      }
-      {
-        float a0, a1;
-        unpack_f32x2(add_f32x2(ls2[0], ls2[1]), a0, a1);
-        l += a0 + a1;
-      }
-      BT_TICK(3)
-      tmem_st_32x32b_x16(sp_tmem, *reinterpret_cast<uint32_t (*)[16]>(&pk[0]));
-      tmem_st_32x32b_x8(sp_tmem + 16, *reinterpret_cast<uint32_t (*)[8]>(&pk[16]));
-      tmem_st_wait();
-      tc_fence_before();
-      mbar_arrive_a(bar_p + 8 * (j & 1));
-      BT_TICK(5)
+    for (int nb = 0; nb < 8; ++nb) {  // keys [8 nb, 8 nb + 8)
+      s[nb][0] = s[nb][1] = s[nb][2] = s[nb][3] = 0.f;
+      uint32_t kf[4];
+      ldmatrix_x4(kb + sw64_off(nb * 8 + (lane & 7), lane >> 3), kf);
+      mma_16816(s[nb], qa[0], kf[0], kf[1]);
+      mma_16816(s[nb], qa[1], kf[2], kf[3]);
     }
-    if ((V & 64) && lane == 0 && !dead) {
+    if (j == nkv - 1) {  // keys >= Lk are padding
+      const int lim = Lk - j * AT_BKV;
 #pragma unroll
-      for (int i = 0; i < 6; ++i) atomicAdd(&g_attn_prof[warp * 8 + i], static_cast<unsigned long long>(tp[i]));
-      atomicAdd(&g_attn_prof[warp * 8 + 6], static_cast<unsigned long long>(nkv));
-    }
-#undef BT_TICK
-    if (!dead) {
-      const int so = (nkv - 1) & 1;
-      mbar_wait_q(bar_pv + 8 * so, ((nkv - 1) >> 1) & 1);
-      tc_fence_after();
-      uint32_t r[32];
-      tmem_ld_32x32b_x32(o_tmem, r);
-      tmem_ld_wait();
-      const int q = q0 + row;
-      if (q < L) {
-        const int64_t m = static_cast<int64_t>(seq) * L + q;
-        const float gsc = gates[m * heads + h] / l;
-        uint4 u[4];
-        uint32_t* w = reinterpret_cast<uint32_t*>(u);
-#pragma unroll
-        for (int d = 0; d < 16; ++d)
-          w[d] = pack_h16x2(__uint_as_float(r[2 * d]) * gsc, __uint_as_float(r[2 * d + 1]) * gsc);
-        uint4* dst = reinterpret_cast<uint4*>(out + m * C + h * 32);
-#pragma unroll
-        for (int d = 0; d < 4; ++d) dst[d] = u[d];
+      for (int nb = 0; nb < 8; ++nb) {
+        const int key = nb * 8 + 2 * (lane & 3);
+        if (key >= lim) s[nb][0] = s[nb][2] = -INFINITY;
+        if (key + 1 >= lim) s[nb][1] = s[nb][3] = -INFINITY;
       }
+    }
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int nb = 0; nb < 8; ++nb) {
+      mx[0] = fmaxf(mx[0], fmaxf(s[nb][0], s[nb][1]));
+      mx[1] = fmaxf(mx[1], fmaxf(s[nb][2], s[nb][3]));
+    }
+    float mref[2], alpha[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+      mref[r] = fmaxf(m_run[r], mx[r]);  // finite: the first tile holds key 0 of every row
+      alpha[r] = ex2_approx(m_run[r] - mref[r]);
+      m_run[r] = mref[r];
+      l_run[r] *= alpha[r];
+    }
+#pragma unroll
+    for (int d = 0; d < 4; ++d) {
+      o[d][0] *= alpha[0]; o[d][1] *= alpha[0];
+      o[d][2] *= alpha[1]; o[d][3] *= alpha[1];
+    }
+    uint32_t pa[4][4];  // P as the A operand of P V: 16 keys per k-step
+#pragma unroll
+    for (int nb = 0; nb < 8; ++nb) {
+      float p[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const float x = s[nb][i] - mref[i >> 1];
+        p[i] = NOEXP ? x : (((PM >> nb) & 1u) ? ex2_poly(x) : ex2_approx(x));
+      }
+      l_run[0] += p[0] + p[1];
+      l_run[1] += p[2] + p[3];
+      pa[nb >> 1][(nb & 1) * 2] = pack_h16x2(p[0], p[1]);
+      pa[nb >> 1][(nb & 1) * 2 + 1] = pack_h16x2(p[2], p[3]);
+    }
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      const int key = kk * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;
+#pragma unroll
+      for (int dp = 0; dp < 2; ++dp) {  // dims [16 dp, 16 dp + 16)
+        uint32_t vf[4];
+        ldmatrix_x4_trans(vb + sw64_off(key, 2 * dp + (lane >> 4)), vf);
+        mma_16816(o[2 * dp], pa[kk], vf[0], vf[1]);
+        mma_16816(o[2 * dp + 1], pa[kk], vf[2], vf[3]);
+      }
+    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive_a(empty + 8 * st);
+  }
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 1);
+    l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 2);
+  }
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int q = q0 + r0 + (lane >> 2) + 8 * r;
+    if (q < L) {
+      const int64_t m = static_cast<int64_t>(seq) * L + q;
+      const float gsc = gates[m * heads + h] / l_run[r];
+      h16* dst = out + m * C + h * 32 + 2 * (lane & 3);
+#pragma unroll
+      for (int d = 0; d < 4; ++d)
+        *reinterpret_cast<uint32_t*>(dst + 8 * d) = pack_h16x2(o[d][2 * r] * gsc, o[d][2 * r + 1] * gsc);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == MMA_WARP) tmem_dealloc<128>(tmem_base);
 }
 
 struct TcAttnPlan {
   CUtensorMap tmQ;   // [seqs, L, 3C] 16-bit, boxes of 128 rows x 32 columns (one head's queries)
-  CUtensorMap tmKV;  // same tensor, boxes of 48 rows (one key / value tile)
+  CUtensorMap tmKV;  // same tensor, boxes of 64 rows (one key / value tile)
   int seqs, L, heads;
 };
 
@@ -348,7 +202,7 @@ TcAttnPlan* tc_attn_plan_create(const void* qkv, int seqs, int L, int heads, cha
   const uint64_t dims[3] = {static_cast<uint64_t>(3 * C), static_cast<uint64_t>(L), static_cast<uint64_t>(seqs)};
   const uint64_t strides[2] = {static_cast<uint64_t>(3 * C) * 2, static_cast<uint64_t>(L) * 3 * C * 2};
   const uint32_t box_q[3] = {32, AT_BQ, 1};
-  const uint32_t box_kv[3] = {32, A4_BKV, 1};
+  const uint32_t box_kv[3] = {32, AT_BKV, 1};
   if (!make_tmap(&p->tmQ, qkv, 3, dims, strides, box_q, 64, err, errlen) ||
       !make_tmap(&p->tmKV, qkv, 3, dims, strides, box_kv, 64, err, errlen)) {
     delete p;
@@ -358,54 +212,40 @@ TcAttnPlan* tc_attn_plan_create(const void* qkv, int seqs, int L, int heads, cha
 }
 void tc_attn_plan_destroy(TcAttnPlan* p) { delete p; }
 
-// Kernel variant (template parameter V of attn_tc48_kernel).  The product runs A4_DEFAULT_V; the others are the
-// experiments of profiles/r2_notes.md, reachable through BT_ATTN_VARIANT / bt_debug_attention_time.
-constexpr int A4_DEFAULT_V = 32 | 5;  // S_{j+2} queued behind PV_j, 3 of 8 score pairs on the polynomial
+// Kernel variant (template parameter V of attn_time_kernel), reachable through BT_ATTN_VARIANT /
+// bt_debug_attention_time.  The product runs AT_DEFAULT_V.
+constexpr int AT_DEFAULT_V = 37;  // 3 of 8 score pairs on the polynomial
 static int g_attn_variant = -1;
 void attn_set_variant(int v) { g_attn_variant = v; }
-void attn_prof_read(unsigned long long* out40, bool reset) {
-  cudaMemcpyFromSymbol(out40, g_attn_prof, 320);
-  if (reset) { unsigned long long z[40] = {}; cudaMemcpyToSymbol(g_attn_prof, z, 320); }
-}
 
-static void attn_prof_print(cudaStream_t st) {  // variant 101 inside the real pipeline (BT_ATTN_PROF_PRINT=1)
-  cudaStreamSynchronize(st);
-  unsigned long long h[40];
-  attn_prof_read(h, true);
-  const double n = h[6] ? double(h[6]) : 1.0;
-  fprintf(stderr, "attention warp 0, cycles per tile: wait S %.0f | ld S %.0f | max+rescale %.0f | exp %.0f | st P %.0f | rescaled tiles %.1f %%\n",
-          h[0] / n, h[1] / n, h[2] / n, h[3] / n, h[5] / n, 100.0 * (h[4] / 1000000) / n);
-}
-
-//   37 default | 32, 33, 36, 40, 41: 0, 1, 2, 4, 5 of 8 pairs on the polynomial | 5: S_{j+2} only after PV_j has
-//   completed | 39, 34: without exponentials (timing ablation, wrong results) | 101: phase cycle counters
-#define BT_A4_VARIANTS(X) X(37) X(32) X(33) X(36) X(40) X(41) X(5) X(39) X(34) X(101)
+//   37 default | 32, 33, 36, 40, 41: 0, 1, 2, 4, 5 of 8 pairs on the polynomial | 39, 34: without exponentials
+//   (timing ablation, wrong results)
+#define BT_AT_VARIANTS(X) X(37) X(32) X(33) X(36) X(40) X(41) X(39) X(34)
 
 int launch_attn_time_tc(const TcAttnPlan* p, const float* gates, void* out, cudaStream_t st, const ChunkSrc* chunks,
                         int seqs_per_chunk) {
   dim3 grid(ceil_div(p->L, AT_BQ), p->heads, p->seqs);
-  if (g_attn_variant < 0) g_attn_variant = getenv("BT_ATTN_VARIANT") ? atoi(getenv("BT_ATTN_VARIANT")) : A4_DEFAULT_V;
+  if (g_attn_variant < 0) g_attn_variant = getenv("BT_ATTN_VARIANT") ? atoi(getenv("BT_ATTN_VARIANT")) : AT_DEFAULT_V;
   h16* o = reinterpret_cast<h16*>(out);
-#define BT_A4_L(V_)                                                                                                  \
+#define BT_AT_L(V_)                                                                                                  \
   if (g_attn_variant == (V_)) {                                                                                      \
-    attn_tc48_kernel<V_><<<grid, AT_THREADS, A4_SMEM, st>>>(p->tmQ, p->tmKV, gates, o, p->L, p->heads, chunks,        \
+    attn_time_kernel<V_><<<grid, AT_THREADS, AT_SMEM, st>>>(p->tmQ, p->tmKV, gates, o, p->L, p->heads, chunks,        \
                                                             seqs_per_chunk);                                         \
-    if (((V_) & 64) && getenv("BT_ATTN_PROF_PRINT")) attn_prof_print(st);                                            \
     return 0;                                                                                                        \
   }
-  BT_A4_VARIANTS(BT_A4_L)
-#undef BT_A4_L
+  BT_AT_VARIANTS(BT_AT_L)
+#undef BT_AT_L
   return -3;
 }
 
 int tc_init_attn(char* err, int errlen) {
   cudaError_t r = cudaSuccess;
-#define BT_A4_A(V_) \
-  if (r == cudaSuccess) r = cudaFuncSetAttribute(attn_tc48_kernel<V_>, cudaFuncAttributeMaxDynamicSharedMemorySize, A4_SMEM);
-  BT_A4_VARIANTS(BT_A4_A)
-#undef BT_A4_A
+#define BT_AT_A(V_) \
+  if (r == cudaSuccess) r = cudaFuncSetAttribute(attn_time_kernel<V_>, cudaFuncAttributeMaxDynamicSharedMemorySize, AT_SMEM);
+  BT_AT_VARIANTS(BT_AT_A)
+#undef BT_AT_A
   if (r != cudaSuccess) {
-    snprintf(err, errlen, "cudaFuncSetAttribute(attn_tc48_kernel) failed: %s", cudaGetErrorString(r));
+    snprintf(err, errlen, "cudaFuncSetAttribute(attn_time_kernel) failed: %s", cudaGetErrorString(r));
     return -1;
   }
   return 0;

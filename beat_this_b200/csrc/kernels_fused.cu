@@ -1,6 +1,13 @@
 // Persistent fused kernels for the narrow frontend sub-blocks (C = 32 / 64): [out-projection +] RMSNorm + FFN +
 // residual (fused_ff_kernel) and RMSNorm + gates + QKV + RoPE (fused_qkv_kernel); reference
 // roformer.py:38-61,114-128 as called by PartialFTTransformer, beat_tracker.py:290-301.
+//
+// Every weight matrix of the block is staged once per CTA into shared memory (rows padded by 16 bytes, so that the
+// B-fragment reads of a warp hit 32 different banks).  A warp then owns 16 token rows at a time and does the whole
+// block in registers with mma.sync m16n8k16 (16-bit operands, fp32 accumulate): each thread loads the fp32 values of
+// its two rows in the order of the MMA fragments, so the row it normalises is also the A operand, and for C <= 64 the
+// accumulator of an N = C product holds exactly the columns the thread loaded.  Unfused, the FFN streams 32 bytes per
+// element through HBM (norm 6 + ff1 10 + ff2 16); fused it is 8 (+2 for the out-projection input, +2 for the 16-bit copy).
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -9,431 +16,255 @@
 
 namespace bt {
 
-// ==================================================================== fused frontend FFN
-// x += W2 gelu(W1 rmsnorm(x) + b1) + b2 for the narrow frontend FFNs (C = 32 / 64, hidden 4C) in ONE
-// kernel (reference roformer.py:38-61): the hidden activations never leave the SM.  Unfused, this
-// block streams 32 bytes per element through HBM (norm 6 + ff1 10 + ff2 16); fused it is 8.
-// CTA = 128 tokens; warps 0-3: one token row per thread (RMSNorm, bias+GELU, output), for C = 64 warps 4-7 share those
-// rows and take half of every GELU epilogue, the last warp (converged, one elected lane issues): TMA (weights) +
-// tcgen05.mma.  Hidden units are processed in chunks of 128:
-//   H_h = Xn W1_h^T (N=128, K=C) -> TMEM cols [0,128) -> bias+GELU -> h16 tile in smem ->
-//   OUT += H_h W2_h^T (N=C, K=128) -> TMEM cols [128,128+C), which start from the residual x (written there by the
-//   row's thread): the tensor core adds the residual, the row does not stay in registers.
-constexpr int FF_THREADS = 160;   // fused_qkv_kernel: 4 row warps + issuer
-// fused_ff_kernel: 4 row warps [+ 4 helper warps for C = 64] + issuer.  (C = 32 runs three CTAs per SM: nine warps each
-// would leave 72 registers per thread -- measured slower than four row warps with the next tile's rows prefetched.)
-template <int C> __host__ __device__ constexpr int ffn_threads() { return C == 64 ? 288 : 160; }
+constexpr int FU_WARPS = 8;
+constexpr int FU_THREADS = 32 * FU_WARPS;
 
-#ifdef BT_FF_PROF  // -DBT_FF_PROF: cycles per phase of the row warps (lane 0), printed after every launch
-__device__ unsigned long long g_ff_prof[16];
-#define FF_TICK(i_) { const long long t_ = clock64(); tp[i_] += t_ - tc0; tc0 = t_; }
-#else
-#define FF_TICK(i_)
-#endif
-template <int C>
-struct FfCfg {
-  static constexpr int NH = 4 * C / 128;            // hidden chunks
-  static constexpr int A_BYTES = 128 * C * 2;       // normalised tokens, K-major
-  static constexpr int W1_BYTES = 4 * C * C * 2;    // all chunks resident
-  static constexpr int W2C_BYTES = C * 128 * 2;     // one K-chunk of W2
-  static constexpr int H_BYTES = 128 * 128 * 2;
-  static constexpr int WO_BYTES = C * C * 2;       // attention out-projection weight (fused_ff_kernel<C, true>)
-  static constexpr int SMEM = A_BYTES + W1_BYTES + W2C_BYTES + H_BYTES + WO_BYTES + 5 * C * 4 + 1024 + 128;
-  static constexpr int SWZ_A = C * 2 < 128 ? C * 2 : 128;  // 64-byte rows for C=32, 128 for C=64
-  // TMEM: H accumulator [0,128) and OUT accumulator.  With a single hidden chunk (C = 32) OUT reuses the H
-  // columns (every thread has read H before MMA2 is issued) -> 128 columns, 3 CTAs/SM instead of 2.
-  static constexpr int OUT_COL = NH == 1 ? 0 : 128;
-  static constexpr int TCOLS = NH == 1 ? 128 : 256;
-  static constexpr int CTAS = NH == 1 ? 3 : 2;
-  // accumulator of the optional out-projection prologue (O Wo^T): columns that are dead at that point
-  static constexpr int D0_COL = NH == 1 ? 64 : 0;
-};
-
-// OP = true: the attention out-projection is fused in front (reference roformer.py:134-140 followed by
-// roformer.py:38-61): x' = x + O Wo^T is computed per tile by one more MMA (the gated attention output O is
-// TMA-loaded into the A-tile buffer, which the normalised x' overwrites afterwards), then the FFN runs on x'.
-// Saves the separate out-projection GEMM: one fp32 read + write of the residual stream per element.
-template <int C, bool OP>
-__global__ void __launch_bounds__(ffn_threads<C>(), FfCfg<C>::CTAS)
-fused_ff_kernel(const __grid_constant__ CUtensorMap tmW1, const __grid_constant__ CUtensorMap tmW2,
-                const __grid_constant__ CUtensorMap tmO, const __grid_constant__ CUtensorMap tmWo,
-                const __grid_constant__ CUtensorMap tmXst, const __grid_constant__ CUtensorMap tmXb,
-                float* __restrict__ X, const float* __restrict__ b1, const float* __restrict__ b2,
-                h16* __restrict__ xb_out, int64_t M) {
-  // PERSISTENT: each CTA walks over token tiles (stride gridDim.x); W1 (and W2 when it is a single chunk) are
-  // fetched once per CTA, barriers / TMEM / bias staging are set up once.  (The one-tile-per-CTA form spent
-  // more time on set-up and on re-fetching 16-64 KB of weights per CTA than on its tile.)
-  using Cfg = FfCfg<C>;
-  constexpr int NH = Cfg::NH;
-  constexpr bool HELP = C == 64;
-  constexpr int FFN_THREADS = ffn_threads<C>();
-  constexpr int FFN_ISSUER = HELP ? 8 : 4;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t sA = sbase;
-  const uint32_t sW1 = sA + Cfg::A_BYTES;
-  const uint32_t sW2 = sW1 + Cfg::W1_BYTES;
-  const uint32_t sH = sW2 + Cfg::W2C_BYTES;
-  const uint32_t sWo = sH + Cfg::H_BYTES;
-  const uint32_t sB = sWo + Cfg::WO_BYTES;        // b1[4C] | b2[C] fp32
-  const uint32_t bar_w1 = sB + 5 * C * 4;
-  const uint32_t bar_w2 = bar_w1 + 8;
-  const uint32_t bar_a = bar_w2 + 8;
-  const uint32_t bar_h = bar_a + 8;
-  const uint32_t bar_h2 = bar_h + 8;
-  const uint32_t bar_o = bar_h2 + 8;
-  const uint32_t bar_of = bar_o + 8;              // O tile landed in the A buffer (OP)
-  const uint32_t bar_d0 = bar_of + 8;             // O Wo^T accumulated (OP)
-  const uint32_t tmem_slot = bar_d0 + 8;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int ntiles = static_cast<int>((M + 127) / 128);
-
-  if (warp == FFN_ISSUER && lane == 0) {
-    tma_prefetch_desc(&tmW1);
-    tma_prefetch_desc(&tmW2);
-    auto init = [](uint32_t bar, uint32_t count) {
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-    };
-    init(bar_w1, 1); init(bar_w2, 1); init(bar_a, 128); init(bar_h, 1); init(bar_h2, HELP ? 256 : 128); init(bar_o, 1);
-    init(bar_of, 1); init(bar_d0, 1);
-    fence_barrier_init();
+// W [rows][cols] 16-bit row-major (global) -> shared memory with row stride cols + 8 elements
+__device__ __forceinline__ void stage_weight(h16* dst, const h16* __restrict__ src, int rows, int cols) {
+  const int vpr = cols / 8;  // 16-byte vectors per row
+  for (int i = threadIdx.x; i < rows * vpr; i += blockDim.x) {
+    const int r = i / vpr, v = i - r * vpr;
+    *reinterpret_cast<uint4*>(dst + r * (cols + 8) + v * 8) = __ldg(reinterpret_cast<const uint4*>(src + static_cast<int64_t>(r) * cols) + v);
   }
-  if (warp == FFN_ISSUER) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "n"(Cfg::TCOLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  for (int i = threadIdx.x; i < 5 * C; i += FFN_THREADS)
-    st_shared_f32(sB + 4 * i, i < 4 * C ? __ldg(b1 + i) : __ldg(b2 + i - 4 * C));
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot) : "memory");
-
-  if (warp == FFN_ISSUER) {
-    const uint32_t on = elect_one() ? 1u : 0u;  // converged issuer warp, predicated single-lane TMA / MMA (see umma_h16_p)
-    constexpr uint32_t idesc1 = make_idesc_h16(128, 128);
-    constexpr uint32_t idesc2 = make_idesc_h16(128, C);
-    // weights: W1 [4C, C] all chunks (boxes of 128 rows), W2 [C, 4C] one K-chunk at a time (two 64-wide boxes)
-    mbar_expect_tx_p(on, bar_w1, Cfg::W1_BYTES + (OP ? Cfg::WO_BYTES : 0));
-    for (int h = 0; h < NH; ++h) tma_load_2d_p(on, sW1 + h * (128 * C * 2), &tmW1, bar_w1, 0, h * 128);
-    if constexpr (OP) tma_load_2d_p(on, sWo, &tmWo, bar_w1, 0, 0);
-    auto load_o = [&](int tile) {  // gated attention output rows of a tile -> the A buffer (same box / swizzle)
-      mbar_expect_tx_p(on, bar_of, Cfg::A_BYTES);
-      tma_load_2d_p(on, sA, &tmO, bar_of, 0, tile * 128);
-    };
-    if constexpr (OP) {
-      if (static_cast<int>(blockIdx.x) < ntiles) load_o(blockIdx.x);
-    }
-    auto load_w2 = [&](int h) {
-      mbar_expect_tx_p(on, bar_w2, Cfg::W2C_BYTES);
-      for (int a = 0; a < 2; ++a) tma_load_2d_p(on, sW2 + a * (C * 128), &tmW2, bar_w2, h * 128 + a * 64, 0);
-    };
-    load_w2(0);
-    auto issue_mma1 = [&](int h) {
-#pragma unroll
-      for (int k = 0; k < C / 16; ++k)
-        umma_h16_p(on, tmem_base, make_kmajor_desc<Cfg::SWZ_A>(sA + k * 32),
-                    make_kmajor_desc<Cfg::SWZ_A>(sW1 + h * (128 * C * 2) + k * 32), idesc1, k != 0 ? 1u : 0u);
-      umma_commit_p(on, bar_h);
-    };
-    mbar_wait_a(bar_w1, 0);
-    int idx = 0;      // chunk counter over all tiles of this CTA: parity of bar_h / bar_h2 / bar_o
-    int w2_loads = 0; // completed-or-in-flight W2 chunk loads minus one: parity of bar_w2
-    int it = 0;
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-      if constexpr (OP) {  // D0 = O Wo^T into columns that nobody reads at this point
-        constexpr uint32_t idesc0 = make_idesc_h16(128, C);
-        mbar_wait_a(bar_of, it & 1);
-        tc_fence_after();
-#pragma unroll
-        for (int k = 0; k < C / 16; ++k)
-          umma_h16_p(on, tmem_base + Cfg::D0_COL, make_kmajor_desc<Cfg::SWZ_A>(sA + k * 32),
-                      make_kmajor_desc<Cfg::SWZ_A>(sWo + k * 32), idesc0, k != 0 ? 1u : 0u);
-        umma_commit_p(on, bar_d0);
-      }
-      mbar_wait_a(bar_a, it & 1);  // normalised tile in smem (and every thread is done with the previous tile's TMEM)
-      tc_fence_after();
-      issue_mma1(0);
-      for (int h = 0; h < NH; ++h, ++idx) {
-        mbar_wait_a(bar_h2, idx & 1);  // h16 H_h tile written, accumulator H consumed
-        tc_fence_after();
-        if (h + 1 < NH) issue_mma1(h + 1);
-        if constexpr (OP) {  // the last MMA1 of this tile has completed (its H was read): the A buffer is free
-          if (h == NH - 1 && tile + static_cast<int>(gridDim.x) < ntiles) load_o(tile + gridDim.x);
-        }
-        if (NH > 1 || idx == 0) mbar_wait_a(bar_w2, w2_loads & 1);
-        tc_fence_after();
-#pragma unroll
-        for (int k = 0; k < 8; ++k)
-          umma_h16_p(on, tmem_base + Cfg::OUT_COL, make_kmajor_desc<128>(sH + (k >> 2) * 16384 + (k & 3) * 32),
-                      make_kmajor_desc<128>(sW2 + (k >> 2) * (C * 128) + (k & 3) * 32), idesc2, 1u);  // OUT starts from the residual x
-        umma_commit_p(on, bar_o);
-        if (NH > 1 && (h + 1 < NH || tile + static_cast<int>(gridDim.x) < ntiles)) {
-          mbar_wait_a(bar_o, idx & 1);  // MMA2 finished reading this W2 chunk (and the H tile)
-          load_w2((h + 1) % NH);
-          ++w2_loads;
-        }
-      }
-    }
-  } else {
-    // warps 0-3 own one token row per thread (load, RMSNorm, residual, stores); warps 4-7 share the same rows
-    // (TMEM lane quarter warp & 3) and take the upper half of every hidden chunk's bias + GELU epilogue -- the longest
-    // stretch of per-thread work in a tile, whose latency bounds a kernel with only 2-3 CTAs per SM
-    const int wq = warp & 3;
-    const bool helper = warp >= 4;
-    const int row = wq * 32 + lane;
-    const uint32_t lane_base = static_cast<uint32_t>(wq * 32) << 16;
-    const uint32_t hrow = sH + row * 128;
-    const uint32_t hsw = static_cast<uint32_t>(row & 7) << 4;
-    int idx = 0, it = 0;
-    const int c4_lo = helper ? 2 : 0;  // this thread's 64 of the 128 hidden units of a chunk (HELP)
-    constexpr int c4_n = HELP ? 2 : 4;
-    if (helper) {
-      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-        for (int h = 0; h < NH; ++h, ++idx) {
-          mbar_wait_a(bar_h, idx & 1);
-          tc_fence_after();
-          if (h >= 1) {
-            mbar_wait_a(bar_o, (idx - 1) & 1);
-            tc_fence_after();
-          }
-          #pragma unroll
-        for (int c4 = c4_lo; c4 < c4_lo + c4_n; ++c4) {
-          uint32_t r[32];
-          tmem_ld_32x32b_x32(tmem_base + lane_base + c4 * 32, r);
-          tmem_ld_wait();
-#pragma unroll
-          for (int c = 0; c < 4; ++c) {  // 4 chunks of 8 hidden units, bias + GELU on packed fp32 pairs
-            const float4 ba = ld_shared_v4_f32(sB + 4 * (h * 128 + c4 * 32 + 8 * c));
-            const float4 bb = ld_shared_v4_f32(sB + 4 * (h * 128 + c4 * 32 + 8 * c + 4));
-            const uint64_t bq[4] = {pack_f32x2(ba.x, ba.y), pack_f32x2(ba.z, ba.w), pack_f32x2(bb.x, bb.y), pack_f32x2(bb.z, bb.w)};
-            uint32_t w[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const uint64_t g = gelu_tanh_f32x2(add_f32x2(pack_f32x2(__uint_as_float(r[8 * c + 2 * i]), __uint_as_float(r[8 * c + 2 * i + 1])), bq[i]));
-              float g0, g1;
-              unpack_f32x2(g, g0, g1);
-              w[i] = pack_h16x2(g0, g1);
-            }
-            const int cc = c4 * 4 + c;  // 16-byte chunk index inside the 128-wide row: atom = cc >> 3
-            st_shared_v4(hrow + (cc >> 3) * 16384 + (((cc & 7) << 4) ^ hsw), w[0], w[1], w[2], w[3]);
-          }
-        }
-          fence_proxy_async_smem();
-          tc_fence_before();
-          mbar_arrive_a(bar_h2);
-        }
-      }
-    }
-    constexpr bool PREFETCH = C == 32;  // next tile's row requested while this tile is in the MMAs (register budget: C = 32 only)
-    float4 xn[PREFETCH ? C / 4 : 1];
-    auto load_x = [&](int tile, float4* dst) {
-      const int64_t mm = static_cast<int64_t>(tile) * 128 + row;
-      const float4* xr = reinterpret_cast<const float4*>(X + (mm < M ? mm : 0) * C);
-#pragma unroll
-      for (int i = 0; i < C / 4; ++i) dst[i] = mm < M ? xr[i] : make_float4(0.f, 0.f, 0.f, 0.f);
-    };
-    if constexpr (PREFETCH) {
-      if (static_cast<int>(blockIdx.x) < ntiles) load_x(blockIdx.x, xn);
-    }
-#ifdef BT_FF_PROF
-    long long tp[8] = {0, 0, 0, 0, 0, 0, 0, 0}, tc0 = clock64();
-#endif
-    for (int tile = blockIdx.x; tile < (helper ? 0 : ntiles); tile += gridDim.x, ++it) {
-      const int64_t m = static_cast<int64_t>(tile) * 128 + row;
-      const bool valid = m < M;
-      // ---- RMSNorm of this token.  The residual is added by the tensor core: x is written into the OUT accumulator
-      // columns and MMA2 accumulates on top of it, so the row does not stay in registers for the whole tile ----
-      float x[C];
-      {
-        float4 xq[C / 4];
-        if constexpr (PREFETCH) {
-#pragma unroll
-          for (int i = 0; i < C / 4; ++i) xq[i] = xn[i];
-        } else {
-          load_x(tile, xq);
-        }
-#pragma unroll
-        for (int i = 0; i < C / 4; ++i) {
-          const float4 q = xq[i];
-          x[4 * i] = q.x; x[4 * i + 1] = q.y; x[4 * i + 2] = q.z; x[4 * i + 3] = q.w;
-        }
-        FF_TICK(0)  // x loaded
-        if constexpr (OP) {  // x' = x + O Wo^T (attention residual)
-          mbar_wait_a(bar_d0, it & 1);
-          tc_fence_after();
-#pragma unroll
-          for (int c4 = 0; c4 < C / 32; ++c4) {
-            uint32_t r[32];
-            tmem_ld_32x32b_x32(tmem_base + lane_base + Cfg::D0_COL + c4 * 32, r);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) x[c4 * 32 + i] += __uint_as_float(r[i]);
-          }
-        }
-        FF_TICK(1)  // out-projection result added
-        float ss = 0.f;
-#pragma unroll
-        for (int i = 0; i < C; ++i) ss = fmaf(x[i], x[i], ss);
-        const float inv = 1.0f / fmaxf(sqrtf(ss), 1e-12f);
-        constexpr int RB = C * 2;  // bytes per A row
-        const uint32_t arow = sA + row * RB;
-        const uint32_t sw = C == 32 ? (static_cast<uint32_t>((row >> 1) & 3) << 4) : (static_cast<uint32_t>(row & 7) << 4);
-        // the A tile is free: the last MMA1 of the previous tile completed before its bar_h was observed
-#pragma unroll
-        for (int c = 0; c < C / 8; ++c)
-          st_shared_v4(arow + ((c << 4) ^ sw), pack_h16x2(x[8 * c] * inv, x[8 * c + 1] * inv),
-                       pack_h16x2(x[8 * c + 2] * inv, x[8 * c + 3] * inv), pack_h16x2(x[8 * c + 4] * inv, x[8 * c + 5] * inv),
-                       pack_h16x2(x[8 * c + 6] * inv, x[8 * c + 7] * inv));
-        if constexpr (NH > 1) {  // OUT has columns of its own: free since this thread read the previous tile's result
-          auto xr = reinterpret_cast<uint32_t (*)[16]>(x);
-#pragma unroll
-          for (int c = 0; c < C / 16; ++c) tmem_st_32x32b_x16(tmem_base + lane_base + Cfg::OUT_COL + 16 * c, xr[c]);
-          tmem_st_wait();
-        }
-        fence_proxy_async_smem();
-        tc_fence_before();  // this thread's TMEM reads of the previous tile are ordered before the next MMAs
-        // this warp's rows of the H tile staged the previous tile's results: the TMA stores must be done reading them
-        // before ANY warp (the helpers too) writes the next hidden activations, i.e. before MMA1 can be issued
-        if (lane == 0) bulk_wait_read<0>();
-        __syncwarp();
-        mbar_arrive_a(bar_a);
-        FF_TICK(2)  // norm, A tile, x into OUT
-        if constexpr (!PREFETCH) {  // no registers for the next tile's row: at least pull its lines into L2 now
-          const int64_t mn = m + static_cast<int64_t>(gridDim.x) * 128;
-          if (mn < M) {
-#pragma unroll
-            for (int i = 0; i < C * 4 / 128; ++i)
-              asm volatile("prefetch.global.L2 [%0];" ::"l"(X + mn * C + i * 32));
-          }
-        }
-        if constexpr (PREFETCH) {
-          if (tile + static_cast<int>(gridDim.x) < ntiles) load_x(tile + gridDim.x, xn);
-        }
-      }
-      for (int h = 0; h < NH; ++h, ++idx) {
-        mbar_wait_a(bar_h, idx & 1);
-        tc_fence_after();
-        if (h >= 1) {  // the single H tile is free once MMA2_{h-1} has completed (h == 0: waited at the end of the last tile)
-          mbar_wait_a(bar_o, (idx - 1) & 1);
-          tc_fence_after();
-        }
-        FF_TICK(3)  // waited for MMA1 (and MMA2 of the previous chunk)
-#pragma unroll
-        for (int c4 = c4_lo; c4 < c4_lo + c4_n; ++c4) {
-          uint32_t r[32];
-          tmem_ld_32x32b_x32(tmem_base + lane_base + c4 * 32, r);
-          tmem_ld_wait();
-          if (NH == 1 && c4 == 0) {  // OUT shares the H columns: this thread has read [0,32), x goes there now
-            auto xr = reinterpret_cast<uint32_t (*)[16]>(x);
-#pragma unroll
-            for (int c = 0; c < C / 16; ++c) tmem_st_32x32b_x16(tmem_base + lane_base + Cfg::OUT_COL + 16 * c, xr[c]);
-          }
-#pragma unroll
-          for (int c = 0; c < 4; ++c) {  // 4 chunks of 8 hidden units, bias + GELU on packed fp32 pairs
-            const float4 ba = ld_shared_v4_f32(sB + 4 * (h * 128 + c4 * 32 + 8 * c));
-            const float4 bb = ld_shared_v4_f32(sB + 4 * (h * 128 + c4 * 32 + 8 * c + 4));
-            const uint64_t bq[4] = {pack_f32x2(ba.x, ba.y), pack_f32x2(ba.z, ba.w), pack_f32x2(bb.x, bb.y), pack_f32x2(bb.z, bb.w)};
-            uint32_t w[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const uint64_t g = gelu_tanh_f32x2(add_f32x2(pack_f32x2(__uint_as_float(r[8 * c + 2 * i]), __uint_as_float(r[8 * c + 2 * i + 1])), bq[i]));
-              float g0, g1;
-              unpack_f32x2(g, g0, g1);
-              w[i] = pack_h16x2(g0, g1);
-            }
-            const int cc = c4 * 4 + c;  // 16-byte chunk index inside the 128-wide row: atom = cc >> 3
-            st_shared_v4(hrow + (cc >> 3) * 16384 + (((cc & 7) << 4) ^ hsw), w[0], w[1], w[2], w[3]);
-          }
-        }
-        if (NH == 1) tmem_st_wait();
-        fence_proxy_async_smem();
-        tc_fence_before();
-        mbar_arrive_a(bar_h2);
-        FF_TICK(4)  // H epilogue
-      }
-      mbar_wait_a(bar_o, (idx - 1) & 1);
-      tc_fence_after();
-      FF_TICK(5)  // waited for the last MMA2
-      // Results leave through TMA stores staged in this warp's rows of the H tile buffer (free from here until the
-      // next tile's hidden activations are written): with one row per lane, st.global touched 32 lines per
-      // instruction and the L1 data pipe bounded the kernel (ncu: lsu wavefronts 80 %, DRAM 35 %).
-      const uint32_t stg = sH + wq * 4096;  // + c4 * 16384: [32 rows][128 B] SW128 fp32 box of 32 columns
-      const uint32_t sw128 = static_cast<uint32_t>(lane & 7) << 4, sw64 = static_cast<uint32_t>((lane >> 1) & 3) << 4;
-      uint32_t xbp[C / 2];  // the 16-bit copy of the row (for the following convolution), packed
-#pragma unroll
-      for (int c4 = 0; c4 < C / 32; ++c4) {
-        uint32_t r[32];
-        tmem_ld_32x32b_x32(tmem_base + lane_base + Cfg::OUT_COL + c4 * 32, r);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const float4 bq = ld_shared_v4_f32(sB + 4 * (4 * C + c4 * 32 + 4 * i));
-          const float v0 = __uint_as_float(r[4 * i]) + bq.x;
-          const float v1 = __uint_as_float(r[4 * i + 1]) + bq.y;
-          const float v2 = __uint_as_float(r[4 * i + 2]) + bq.z;
-          const float v3 = __uint_as_float(r[4 * i + 3]) + bq.w;
-          asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(stg + c4 * 16384 + lane * 128 + ((static_cast<uint32_t>(i) << 4) ^ sw128)),
-                       "f"(v0), "f"(v1), "f"(v2), "f"(v3) : "memory");
-          xbp[c4 * 16 + 2 * i] = pack_h16x2(v0, v1);
-          xbp[c4 * 16 + 2 * i + 1] = pack_h16x2(v2, v3);
-        }
-      }
-      if (C == 32 && xb_out) {  // room for the 16-bit tile next to the fp32 one (second half of this warp's H rows)
-#pragma unroll
-        for (int i = 0; i < 4; ++i)
-          st_shared_v4(stg + 16384 + lane * 64 + ((static_cast<uint32_t>(i) << 4) ^ sw64), xbp[4 * i], xbp[4 * i + 1], xbp[4 * i + 2], xbp[4 * i + 3]);
-      }
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) {
-#pragma unroll
-        for (int c4 = 0; c4 < C / 32; ++c4) tma_store_2d(&tmXst, stg + c4 * 16384, c4 * 32, tile * 128 + wq * 32);
-        if (C == 32 && xb_out) tma_store_2d(&tmXb, stg + 16384, 0, tile * 128 + wq * 32);
-        bulk_commit();
-      }
-      if (C == 64 && xb_out) {  // no spare room: the 16-bit tiles reuse the staging area once the fp32 stores have read it
-        if (lane == 0) bulk_wait_read<0>();
-        __syncwarp();
-#pragma unroll
-        for (int c4 = 0; c4 < C / 32; ++c4)
-#pragma unroll
-          for (int i = 0; i < 4; ++i)
-            st_shared_v4(stg + c4 * 16384 + lane * 64 + ((static_cast<uint32_t>(i) << 4) ^ sw64), xbp[c4 * 16 + 4 * i],
-                         xbp[c4 * 16 + 4 * i + 1], xbp[c4 * 16 + 4 * i + 2], xbp[c4 * 16 + 4 * i + 3]);
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) {
-#pragma unroll
-          for (int c4 = 0; c4 < C / 32; ++c4) tma_store_2d(&tmXb, stg + c4 * 16384, c4 * 32, tile * 128 + wq * 32);
-          bulk_commit();
-        }
-      }
-      FF_TICK(6)  // out epilogue, staging, TMA stores
-    }
-    if (!helper && lane == 0) bulk_wait_read<0>();
-    __syncwarp();
-#ifdef BT_FF_PROF
-    if (!helper && lane == 0) {
-      for (int i = 0; i < 8; ++i) atomicAdd(&g_ff_prof[i], static_cast<unsigned long long>(tp[i]));
-      atomicAdd(&g_ff_prof[8], static_cast<unsigned long long>(it));
-    }
-#endif
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == FFN_ISSUER) tmem_dealloc<Cfg::TCOLS>(tmem_base);
+}
+__device__ __forceinline__ uint32_t lds32(const h16* p) { return *reinterpret_cast<const uint32_t*>(p); }
+// B fragment of out = A W^T for output columns [8 nb, 8 nb + 8) and K [16 ks, 16 ks + 16): W staged with row stride LD
+template <int LD>
+__device__ __forceinline__ void b_frag(const h16* sW, int nb, int ks, int lane, uint32_t& b0, uint32_t& b1) {
+  const h16* p = sW + (nb * 8 + (lane >> 2)) * LD + ks * 16 + 2 * (lane & 3);
+  b0 = lds32(p);
+  b1 = lds32(p + 8);
 }
 
+// ==================================================================== fused frontend QKV projection
+// gates = sigmoid(wg . rmsnorm(x) + bg) in fp32, qkv = RoPE(rmsnorm(x) Wqkv^T) (q also scaled) -> 16-bit.  HBM: 4 bytes
+// in, 6 bytes out per element.
+template <int C>
+__global__ void __launch_bounds__(FU_THREADS, C == 32 ? 4 : 2)
+fused_qkv_kernel(const h16* __restrict__ wqkv, const float* __restrict__ X, const float* __restrict__ wg,
+                 const float* __restrict__ bg, const float* __restrict__ rope_cos, const float* __restrict__ rope_sin,
+                 h16* __restrict__ qkv, float* __restrict__ gates, int64_t M, int L, int F, int posmode, float qscale) {
+  constexpr int LD = C + 8, KS = C / 16, NB = 3 * C / 8, heads = C / 32;
+  extern __shared__ uint4 fu_smem[];
+  h16* sW = reinterpret_cast<h16*>(fu_smem);
+  stage_weight(sW, wqkv, 3 * C, C);
+  __syncthreads();
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, q = lane & 3;
+  const int64_t ngroups = (M + 15) / 16;
+  for (int64_t g = static_cast<int64_t>(blockIdx.x) * FU_WARPS + warp; g < ngroups; g += static_cast<int64_t>(gridDim.x) * FU_WARPS) {
+    int64_t m[2];
+    bool ok[2];
+    float xs[2][C / 4];  // xs[r][4 ks + 2 h + e] = x[row r][16 ks + 8 h + 2 q + e]
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      m[r] = g * 16 + (lane >> 2) + 8 * r;
+      ok[r] = m[r] < M;
+#pragma unroll
+      for (int j = 0; j < C / 4; j += 2) {
+        const float2 v = ok[r] ? *reinterpret_cast<const float2*>(X + m[r] * C + 16 * (j >> 2) + 8 * ((j >> 1) & 1) + 2 * q)
+                               : make_float2(0.f, 0.f);
+        xs[r][j] = v.x;
+        xs[r][j + 1] = v.y;
+      }
+    }
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {  // RMSNorm without gamma (folded into the weights); the quad holds the whole row
+      float ss = 0.f;
+#pragma unroll
+      for (int j = 0; j < C / 4; ++j) ss = fmaf(xs[r][j], xs[r][j], ss);
+      ss += __shfl_xor_sync(0xffffffffu, ss, 1);
+      ss += __shfl_xor_sync(0xffffffffu, ss, 2);
+      const float inv = 1.0f / fmaxf(sqrtf(ss), 1e-12f);
+#pragma unroll
+      for (int j = 0; j < C / 4; ++j) xs[r][j] *= inv;
+    }
+#pragma unroll
+    for (int h = 0; h < heads; ++h) {  // gates = sigmoid(to_gates(x_normed)) (gamma * sqrt(C) folded into wg)
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        float a = 0.f;
+#pragma unroll
+        for (int j = 0; j < C / 4; j += 2) {
+          const float2 w = __ldg(reinterpret_cast<const float2*>(wg + h * C + 16 * (j >> 2) + 8 * ((j >> 1) & 1) + 2 * q));
+          a = fmaf(xs[r][j], w.x, fmaf(xs[r][j + 1], w.y, a));
+        }
+        a += __shfl_xor_sync(0xffffffffu, a, 1);
+        a += __shfl_xor_sync(0xffffffffu, a, 2);
+        if (q == 0 && ok[r]) gates[m[r] * heads + h] = sigmoidf_(a + __ldg(bg + h));
+      }
+    }
+    uint32_t a[KS][4];
+#pragma unroll
+    for (int ks = 0; ks < KS; ++ks) {
+      a[ks][0] = pack_h16x2(xs[0][4 * ks], xs[0][4 * ks + 1]);
+      a[ks][1] = pack_h16x2(xs[1][4 * ks], xs[1][4 * ks + 1]);
+      a[ks][2] = pack_h16x2(xs[0][4 * ks + 2], xs[0][4 * ks + 3]);
+      a[ks][3] = pack_h16x2(xs[1][4 * ks + 2], xs[1][4 * ks + 3]);
+    }
+    const float* cs[2];
+    const float* sn[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {  // RoPE position of the row (interleaved pairs, rotary_embedding_torch semantics)
+      const int pos = ok[r] ? (posmode == 0 ? static_cast<int>(m[r] % L) : static_cast<int>((m[r] / L) % F)) : 0;
+      cs[r] = rope_cos + pos * 16;
+      sn[r] = rope_sin + pos * 16;
+    }
+#pragma unroll
+    for (int nb = 0; nb < NB; ++nb) {
+      float acc[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+      for (int ks = 0; ks < KS; ++ks) {
+        uint32_t b0, b1;
+        b_frag<LD>(sW, nb, ks, lane, b0, b1);
+        mma_16816(acc, a[ks], b0, b1);
+      }
+      const int n = nb * 8 + 2 * q;
+      const int which = (nb * 8) / C;  // 0 q, 1 k, 2 v (a block of 8 columns never straddles them)
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        float v0 = acc[2 * r], v1 = acc[2 * r + 1];
+        if (which < 2) {
+          const float sc = which == 0 ? qscale : 1.0f;
+          const int i = ((n - which * C) & 31) >> 1;
+          const float co = __ldg(cs[r] + i), si = __ldg(sn[r] + i);
+          const float x0 = v0, x1 = v1;
+          v0 = (x0 * co - x1 * si) * sc;
+          v1 = (x1 * co + x0 * si) * sc;
+        }
+        if (ok[r]) *reinterpret_cast<uint32_t*>(qkv + m[r] * (3 * C) + n) = pack_h16x2(v0, v1);
+      }
+    }
+  }
+}
+
+// ==================================================================== fused frontend FFN
+// x += W2 gelu(W1 rmsnorm(x) + b1) + b2; with OP the preceding attention's out-projection runs in front
+// (x' = x + O Wo^T, reference roformer.py:134-140, then the FFN on x').  The accumulator of the N = C products starts
+// from the residual row, so the tensor core adds it.  Hidden units go 16 at a time: two 8-column blocks of
+// rmsnorm(x') W1^T -> bias + GELU -> packed straight from the accumulator layout into the A operand of the W2
+// product: the hidden activations never leave the registers.
+template <int C, bool OP>
+__global__ void __launch_bounds__(FU_THREADS, C == 32 ? 3 : 2)
+fused_ff_kernel(const h16* __restrict__ w1, const h16* __restrict__ w2, const h16* __restrict__ wo,
+                const h16* __restrict__ O, float* __restrict__ X, const float* __restrict__ b1,
+                const float* __restrict__ b2, h16* __restrict__ xb_out, int64_t M) {
+  constexpr int HID = 4 * C, LD1 = C + 8, LD2 = HID + 8, KS = C / 16, NB = C / 8, HS = HID / 16;
+  extern __shared__ uint4 fu_smem[];
+  h16* sW1 = reinterpret_cast<h16*>(fu_smem);  // [4C][C + 8]
+  h16* sW2 = sW1 + HID * LD1;                   // [C][4C + 8]
+  h16* sWo = sW2 + C * LD2;                     // [C][C + 8] (OP)
+  stage_weight(sW1, w1, HID, C);
+  stage_weight(sW2, w2, C, HID);
+  if constexpr (OP) stage_weight(sWo, wo, C, C);
+  __syncthreads();
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, q = lane & 3;
+  const int64_t ngroups = (M + 15) / 16;
+  for (int64_t g = static_cast<int64_t>(blockIdx.x) * FU_WARPS + warp; g < ngroups; g += static_cast<int64_t>(gridDim.x) * FU_WARPS) {
+    int64_t m[2];
+    bool ok[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      m[r] = g * 16 + (lane >> 2) + 8 * r;
+      ok[r] = m[r] < M;
+    }
+    float acc[NB][4];  // columns 8 nb + 2 q + {0, 1} of rows r0 (acc[nb][0..1]) and r0 + 8 (acc[nb][2..3])
+#pragma unroll
+    for (int nb = 0; nb < NB; ++nb)
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        const float2 v = ok[r] ? *reinterpret_cast<const float2*>(X + m[r] * C + nb * 8 + 2 * q) : make_float2(0.f, 0.f);
+        acc[nb][2 * r] = v.x;
+        acc[nb][2 * r + 1] = v.y;
+      }
+    if constexpr (OP) {  // x' = x + O Wo^T, O (gated attention output, 16-bit) loaded in A-fragment order
+      uint32_t ao[KS][4];
+#pragma unroll
+      for (int ks = 0; ks < KS; ++ks)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const int r = i & 1;
+          ao[ks][i] = ok[r] ? *reinterpret_cast<const uint32_t*>(O + m[r] * C + ks * 16 + 8 * (i >> 1) + 2 * q) : 0u;
+        }
+#pragma unroll
+      for (int nb = 0; nb < NB; ++nb)
+#pragma unroll
+        for (int ks = 0; ks < KS; ++ks) {
+          uint32_t b0, b1;
+          b_frag<LD1>(sWo, nb, ks, lane, b0, b1);
+          mma_16816(acc[nb], ao[ks], b0, b1);
+        }
+    }
+    float inv[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      float ss = 0.f;
+#pragma unroll
+      for (int nb = 0; nb < NB; ++nb) ss = fmaf(acc[nb][2 * r], acc[nb][2 * r], fmaf(acc[nb][2 * r + 1], acc[nb][2 * r + 1], ss));
+      ss += __shfl_xor_sync(0xffffffffu, ss, 1);
+      ss += __shfl_xor_sync(0xffffffffu, ss, 2);
+      inv[r] = 1.0f / fmaxf(sqrtf(ss), 1e-12f);
+    }
+    uint32_t a[KS][4];  // rmsnorm(x') as the A operand: k-step ks covers accumulator blocks 2 ks and 2 ks + 1
+#pragma unroll
+    for (int ks = 0; ks < KS; ++ks) {
+      a[ks][0] = pack_h16x2(acc[2 * ks][0] * inv[0], acc[2 * ks][1] * inv[0]);
+      a[ks][1] = pack_h16x2(acc[2 * ks][2] * inv[1], acc[2 * ks][3] * inv[1]);
+      a[ks][2] = pack_h16x2(acc[2 * ks + 1][0] * inv[0], acc[2 * ks + 1][1] * inv[0]);
+      a[ks][3] = pack_h16x2(acc[2 * ks + 1][2] * inv[1], acc[2 * ks + 1][3] * inv[1]);
+    }
+#pragma unroll
+    for (int nb = 0; nb < NB; ++nb) {  // + b2: the result accumulates on top of x' + b2
+      const float2 b = __ldg(reinterpret_cast<const float2*>(b2 + nb * 8 + 2 * q));
+      acc[nb][0] += b.x; acc[nb][1] += b.y;
+      acc[nb][2] += b.x; acc[nb][3] += b.y;
+    }
+#pragma unroll 2
+    for (int j = 0; j < HS; ++j) {  // hidden units [16 j, 16 j + 16)
+      float hh[2][4];
+#pragma unroll
+      for (int t = 0; t < 2; ++t) {
+        hh[t][0] = hh[t][1] = hh[t][2] = hh[t][3] = 0.f;
+#pragma unroll
+        for (int ks = 0; ks < KS; ++ks) {
+          uint32_t b0, b1;
+          b_frag<LD1>(sW1, 2 * j + t, ks, lane, b0, b1);
+          mma_16816(hh[t], a[ks], b0, b1);
+        }
+        const float2 b = __ldg(reinterpret_cast<const float2*>(b1 + (2 * j + t) * 8 + 2 * q));
+        hh[t][0] = gelu_tanh_fast(hh[t][0] + b.x); hh[t][1] = gelu_tanh_fast(hh[t][1] + b.y);
+        hh[t][2] = gelu_tanh_fast(hh[t][2] + b.x); hh[t][3] = gelu_tanh_fast(hh[t][3] + b.y);
+      }
+      const uint32_t ah[4] = {pack_h16x2(hh[0][0], hh[0][1]), pack_h16x2(hh[0][2], hh[0][3]), pack_h16x2(hh[1][0], hh[1][1]),
+                              pack_h16x2(hh[1][2], hh[1][3])};
+#pragma unroll
+      for (int nb = 0; nb < NB; ++nb) {
+        uint32_t b0, b1;
+        b_frag<LD2>(sW2, nb, j, lane, b0, b1);
+        mma_16816(acc[nb], ah, b0, b1);
+      }
+    }
+#pragma unroll
+    for (int nb = 0; nb < NB; ++nb)
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        if (!ok[r]) continue;
+        const int64_t o = m[r] * C + nb * 8 + 2 * q;
+        *reinterpret_cast<float2*>(X + o) = make_float2(acc[nb][2 * r], acc[nb][2 * r + 1]);
+        if (xb_out) *reinterpret_cast<uint32_t*>(xb_out + o) = pack_h16x2(acc[nb][2 * r], acc[nb][2 * r + 1]);
+      }
+  }
+}
+
+template <int C> constexpr int ff_smem(bool op) { return (4 * C * (C + 8) + C * (4 * C + 8) + (op ? C * (C + 8) : 0)) * 2; }
+template <int C> constexpr int qkv_smem() { return 3 * C * (C + 8) * 2; }
+template <int C> constexpr int ff_ctas() { return C == 32 ? 3 : 2; }
+template <int C> constexpr int qkv_ctas() { return C == 32 ? 4 : 2; }
+
 struct TcFfPlan {
-  CUtensorMap tmW1, tmW2, tmO, tmWo;
+  const void *w1, *w2, *o, *wo;
   int C;
   int64_t M;
   bool outproj;
-  // result tensor maps, (re)encoded when a launch names other buffers (a call site always passes the same ones)
-  mutable CUtensorMap tmXst, tmXb;
-  mutable const void *k_x = nullptr, *k_xb = nullptr;
 };
 
 // o_h16 / wout_h16 != nullptr: plan for the variant with the attention out-projection fused in front
@@ -442,318 +273,66 @@ TcFfPlan* tc_ff_plan_create(const void* w1_h16, const void* w2_h16, int C, int64
                             const void* wout_h16, char* err, int errlen) {
   if (C != 32 && C != 64) { snprintf(err, errlen, "fused ff: C must be 32 or 64"); return nullptr; }
   TcFfPlan* p = new TcFfPlan();
+  p->w1 = w1_h16; p->w2 = w2_h16; p->o = o_h16; p->wo = wout_h16;
   p->C = C; p->M = M; p->outproj = o_h16 != nullptr && wout_h16 != nullptr;
-  const uint32_t swz_a = C * 2 < 128 ? C * 2 : 128;
-  {  // W1 [4C, C] row-major: box = {C, 128 rows}
-    const uint64_t dims[2] = {static_cast<uint64_t>(C), static_cast<uint64_t>(4 * C)};
-    const uint64_t strides[1] = {static_cast<uint64_t>(C) * 2};
-    const uint32_t box[2] = {static_cast<uint32_t>(C), 128};
-    if (!make_tmap(&p->tmW1, w1_h16, 2, dims, strides, box, swz_a, err, errlen)) { delete p; return nullptr; }
-  }
-  {  // W2 [C, 4C] row-major: box = {64 K, C rows}
-    const uint64_t dims[2] = {static_cast<uint64_t>(4 * C), static_cast<uint64_t>(C)};
-    const uint64_t strides[1] = {static_cast<uint64_t>(4 * C) * 2};
-    const uint32_t box[2] = {64, static_cast<uint32_t>(C)};
-    if (!make_tmap(&p->tmW2, w2_h16, 2, dims, strides, box, 128, err, errlen)) { delete p; return nullptr; }
-  }
-  if (p->outproj) {
-    {  // O [M, C] row-major: box = {C, 128 tokens}, same swizzle as the hand-written A tile
-      const uint64_t dims[2] = {static_cast<uint64_t>(C), static_cast<uint64_t>(M)};
-      const uint64_t strides[1] = {static_cast<uint64_t>(C) * 2};
-      const uint32_t box[2] = {static_cast<uint32_t>(C), 128};
-      if (!make_tmap(&p->tmO, o_h16, 2, dims, strides, box, swz_a, err, errlen)) { delete p; return nullptr; }
-    }
-    {  // Wo [C, C] row-major
-      const uint64_t dims[2] = {static_cast<uint64_t>(C), static_cast<uint64_t>(C)};
-      const uint64_t strides[1] = {static_cast<uint64_t>(C) * 2};
-      const uint32_t box[2] = {static_cast<uint32_t>(C), static_cast<uint32_t>(C)};
-      if (!make_tmap(&p->tmWo, wout_h16, 2, dims, strides, box, swz_a, err, errlen)) { delete p; return nullptr; }
-    }
-  } else {
-    p->tmO = p->tmW1;  // never dereferenced
-    p->tmWo = p->tmW1;
-  }
   return p;
 }
 void tc_ff_plan_destroy(TcFfPlan* p) { delete p; }
 
+static unsigned fused_grid(int64_t M, int ctas_per_sm) {
+  const int64_t ctas = ((M + 15) / 16 + FU_WARPS - 1) / FU_WARPS;
+  const int64_t slots = static_cast<int64_t>(g_num_sms) * ctas_per_sm;  // persistent CTAs: weights staged once each
+  return static_cast<unsigned>(ctas < slots ? ctas : slots);
+}
+
 int launch_fused_ff(const TcFfPlan* p, float* X, const float* b1, const float* b2, void* xb_out, cudaStream_t st) {
-  if (p->k_x != X || p->k_xb != xb_out) {
-    char err[256];
-    const uint32_t box[2] = {32, 32};
-    const uint64_t dx[2] = {static_cast<uint64_t>(p->C), static_cast<uint64_t>(p->M)};
-    const uint64_t sx[1] = {static_cast<uint64_t>(p->C) * 4};
-    const uint64_t sb[1] = {static_cast<uint64_t>(p->C) * 2};
-    if (!make_tmap_f32(&p->tmXst, X, 2, dx, sx, box, 128, err, sizeof(err))) return -1;
-    if (xb_out) { if (!make_tmap(&p->tmXb, xb_out, 2, dx, sb, box, 64, err, sizeof(err))) return -1; }
-    else p->tmXb = p->tmXst;  // never dereferenced
-    p->k_x = X; p->k_xb = xb_out;
-  }
-  const unsigned ntiles = static_cast<unsigned>((p->M + 127) / 128);
-  const unsigned slots = static_cast<unsigned>(g_num_sms) * (p->C == 32 ? FfCfg<32>::CTAS : FfCfg<64>::CTAS);
-  const unsigned grid = ntiles < slots ? ntiles : slots;  // persistent CTAs
-  h16* xb = reinterpret_cast<h16*>(xb_out);
-#define BT_FF_L(CC, OPP)                                                                                          \
-  fused_ff_kernel<CC, OPP><<<grid, ffn_threads<CC>(), FfCfg<CC>::SMEM, st>>>(p->tmW1, p->tmW2, p->tmO, p->tmWo, p->tmXst, p->tmXb, X, \
-                                                                      b1, b2, xb, p->M)
+  const h16* w1 = static_cast<const h16*>(p->w1);
+  const h16* w2 = static_cast<const h16*>(p->w2);
+  const h16* wo = static_cast<const h16*>(p->wo);
+  const h16* o = static_cast<const h16*>(p->o);
+  h16* xb = static_cast<h16*>(xb_out);
+#define BT_FF_L(CC, OPP)                                                                                            \
+  fused_ff_kernel<CC, OPP><<<fused_grid(p->M, ff_ctas<CC>()), FU_THREADS, ff_smem<CC>(OPP), st>>>(w1, w2, wo, o, X, b1, \
+                                                                                                  b2, xb, p->M)
   if (p->C == 32) { if (p->outproj) BT_FF_L(32, true); else BT_FF_L(32, false); }
   else { if (p->outproj) BT_FF_L(64, true); else BT_FF_L(64, false); }
 #undef BT_FF_L
-#ifdef BT_FF_PROF
-  {
-    cudaStreamSynchronize(st);
-    unsigned long long h[16], z[16] = {};
-    cudaMemcpyFromSymbol(h, g_ff_prof, sizeof(h));
-    cudaMemcpyToSymbol(g_ff_prof, z, sizeof(z));
-    const double n = h[8] ? double(h[8]) : 1.0;
-    fprintf(stderr, "fused_ff C=%d op=%d cycles/tile: load %.0f | d0 %.0f | norm %.0f | wait mma1 %.0f | H epi %.0f | wait mma2 %.0f | out %.0f\n", p->C,
-            int(p->outproj), h[0] / n, h[1] / n, h[2] / n, h[3] / n, h[4] / n, h[5] / n, h[6] / n);
-  }
-#endif
   return 0;
 }
 
-// ================================================================ fused frontend QKV projection
-// RMSNorm -> gates -> to_qkv GEMM -> RoPE (+ q scaling) for the narrow frontend attentions (C = 32 /
-// 64) in one kernel (reference roformer.py:114-123,127-128): replaces norm_kernel + the QKV GEMM
-// (16 bytes/element through HBM) by 4 in + 6 out.  CTA = 128 tokens; warps 0-3 one token row per
-// thread, warp 4 (converged) TMA (weights) + tcgen05.mma.  N = 3C fits one MMA and 128/256 TMEM columns.
-template <int C>
-struct QkvCfg {
-  static constexpr int A_BYTES = 128 * C * 2;
-  static constexpr int W_BYTES = 3 * C * C * 2;
-  // per warp: the fp32 rows of its 32 tokens (TMA-loaded, C/32 boxes of 32 rows x 128 B) + four rotating 32 x 32
-  // 16-bit output tiles (TMA-stored).  Threads never issue ld/st.global for the activations: with one row per lane
-  // every 16-byte access touched 32 different lines and the L1 data pipe, not HBM, bounded the kernel (ncu:
-  // l1tex lsu wavefronts 80-85 %, DRAM 37 %; profiles/r2_notes.md).
-  static constexpr int XW_BYTES = 32 * C * 4;
-  static constexpr int WARP_BYTES = XW_BYTES + 4 * 2048;
-  static constexpr int SMEM = A_BYTES + W_BYTES + 4 * WARP_BYTES + 1024 + 128;
-  static constexpr int TCOLS = 3 * C <= 128 ? 128 : 256;
-  static constexpr int SWZ = C * 2 < 128 ? C * 2 : 128;
-};
-
-template <int C>
-__global__ void __launch_bounds__(FF_THREADS, (C == 32 ? 3 : 2))
-fused_qkv_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmX,
-                 const __grid_constant__ CUtensorMap tmQ, const float* __restrict__ wg,
-                 const float* __restrict__ bg, const float* __restrict__ rope_cos, const float* __restrict__ rope_sin,
-                 float* __restrict__ gates, int64_t M, int L, int F, int posmode, float qscale) {
-  using Cfg = QkvCfg<C>;
-  constexpr int heads = C / 32;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t sA = sbase;
-  const uint32_t sW = sA + Cfg::A_BYTES;
-  const uint32_t sWarp = sW + Cfg::W_BYTES;  // A_BYTES and W_BYTES are multiples of 1024
-  const uint32_t bar_w = sWarp + 4 * Cfg::WARP_BYTES;
-  const uint32_t bar_a = bar_w + 8;
-  const uint32_t bar_d = bar_a + 8;
-  const uint32_t bar_x = bar_d + 8;  // [4] one per token warp
-  const uint32_t tmem_slot = bar_x + 32;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int ntiles = static_cast<int>((M + 127) / 128);  // PERSISTENT: tiles blockIdx.x, +gridDim.x, ... (W fetched once)
-
-  if (warp == 4 && lane == 0) {
-    tma_prefetch_desc(&tmW);
-    tma_prefetch_desc(&tmX);
-    tma_prefetch_desc(&tmQ);
-    auto init = [](uint32_t bar, uint32_t count) {
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-    };
-    init(bar_w, 1); init(bar_a, 128); init(bar_d, 1);
-    for (int i = 0; i < 4; ++i) init(bar_x + 8 * i, 1);
-    fence_barrier_init();
-  }
-  if (warp == 4) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "n"(Cfg::TCOLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot) : "memory");
-
-  if (warp == 4) {
-    const uint32_t on = elect_one() ? 1u : 0u;  // converged issuer warp (see umma_h16_p)
-    constexpr uint32_t idesc = make_idesc_h16(128, 3 * C);
-    mbar_expect_tx_p(on, bar_w, Cfg::W_BYTES);
-    tma_load_2d_p(on, sW, &tmW, bar_w, 0, 0);
-    mbar_wait_a(bar_w, 0);
-    int it = 0;
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-      mbar_wait_a(bar_a, it & 1);  // normalised tile in smem, previous accumulator read by every thread
-      tc_fence_after();
-#pragma unroll
-      for (int k = 0; k < C / 16; ++k)
-        umma_h16_p(on, tmem_base, make_kmajor_desc<Cfg::SWZ>(sA + k * 32), make_kmajor_desc<Cfg::SWZ>(sW + k * 32), idesc,
-                   k != 0 ? 1u : 0u);
-      umma_commit_p(on, bar_d);
-    }
-  } else {
-    const int row = warp * 32 + lane;
-    const uint32_t lane_base = static_cast<uint32_t>(warp * 32) << 16;
-    const uint32_t xbuf = sWarp + warp * Cfg::WARP_BYTES;  // [C/32 boxes][32 rows][128 B], SW128
-    const uint32_t qbuf = xbuf + Cfg::XW_BYTES;            // 4 x [32 rows][64 B], SW64
-    const uint32_t xbar = bar_x + 8 * warp;
-    const uint32_t sw128 = static_cast<uint32_t>(lane & 7) << 4, sw64 = static_cast<uint32_t>((lane >> 1) & 3) << 4;
-    auto load_x = [&](int tile) {  // this warp's 32 token rows of `tile` (rows beyond M arrive as zeros)
-      if (lane == 0) {
-        mbar_expect_tx_a(xbar, Cfg::XW_BYTES);
-#pragma unroll
-        for (int b = 0; b < C / 32; ++b) tma_load_2d_a(xbuf + b * 4096, &tmX, xbar, b * 32, tile * 128 + warp * 32);
-      }
-    };
-    if (static_cast<int>(blockIdx.x) < ntiles) load_x(blockIdx.x);
-    int it = 0, ck = 0;
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-      const int64_t m = static_cast<int64_t>(tile) * 128 + row;
-      const bool valid = m < M;
-      {
-        float x[C];
-        float ss = 0.f;
-        mbar_wait_a(xbar, it & 1);
-#pragma unroll
-        for (int i = 0; i < C / 4; ++i) {
-          const float4 q = ld_shared_v4_f32(xbuf + (i >> 3) * 4096 + lane * 128 + ((static_cast<uint32_t>(i & 7) << 4) ^ sw128));
-          x[4 * i] = q.x; x[4 * i + 1] = q.y; x[4 * i + 2] = q.z; x[4 * i + 3] = q.w;
-          ss = fmaf(q.x, q.x, ss); ss = fmaf(q.y, q.y, ss); ss = fmaf(q.z, q.z, ss); ss = fmaf(q.w, q.w, ss);
-        }
-        __syncwarp();  // every lane has its row in registers: the buffer can take the next tile's rows
-        if (tile + static_cast<int>(gridDim.x) < ntiles) load_x(tile + gridDim.x);
-        const float inv = 1.0f / fmaxf(sqrtf(ss), 1e-12f);
-#pragma unroll
-        for (int i = 0; i < C; ++i) x[i] *= inv;
-        // gates = sigmoid(to_gates(x_normed)) (gamma*sqrt(C) folded into wg)
-#pragma unroll
-        for (int h = 0; h < heads; ++h) {
-          const float4* w4 = reinterpret_cast<const float4*>(wg + h * C);
-          float a = 0.f;
-#pragma unroll
-          for (int i = 0; i < C / 4; ++i) {
-            const float4 w = __ldg(w4 + i);
-            a = fmaf(x[4 * i], w.x, a); a = fmaf(x[4 * i + 1], w.y, a); a = fmaf(x[4 * i + 2], w.z, a); a = fmaf(x[4 * i + 3], w.w, a);
-          }
-          if (valid) gates[m * heads + h] = sigmoidf_(a + __ldg(bg + h));
-        }
-        constexpr int RB = C * 2;
-        const uint32_t arow = sA + row * RB;
-        const uint32_t sw = C == 32 ? sw64 : sw128;
-#pragma unroll
-        for (int c = 0; c < C / 8; ++c)
-          st_shared_v4(arow + ((c << 4) ^ sw), pack_h16x2(x[8 * c], x[8 * c + 1]), pack_h16x2(x[8 * c + 2], x[8 * c + 3]),
-                       pack_h16x2(x[8 * c + 4], x[8 * c + 5]), pack_h16x2(x[8 * c + 6], x[8 * c + 7]));
-        fence_proxy_async_smem();
-        tc_fence_before();  // TMEM reads of the previous tile are ordered before the next MMA
-        mbar_arrive_a(bar_a);
-      }
-      // RoPE row of this token (interleaved pairs, rotary_embedding_torch semantics)
-      float cs[16], sn[16];
-      {
-        const int pos = valid ? (posmode == 0 ? static_cast<int>(m % L) : static_cast<int>((m / L) % F)) : 0;
-        const float4* c4 = reinterpret_cast<const float4*>(rope_cos + pos * 16);
-        const float4* s4 = reinterpret_cast<const float4*>(rope_sin + pos * 16);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const float4 a = __ldg(c4 + i), b = __ldg(s4 + i);
-          cs[4 * i] = a.x; cs[4 * i + 1] = a.y; cs[4 * i + 2] = a.z; cs[4 * i + 3] = a.w;
-          sn[4 * i] = b.x; sn[4 * i + 1] = b.y; sn[4 * i + 2] = b.z; sn[4 * i + 3] = b.w;
-        }
-      }
-      mbar_wait_a(bar_d, it & 1);
-      tc_fence_after();
-#pragma unroll
-      for (int c = 0; c < 3 * C / 32; ++c, ++ck) {
-        uint32_t r[32];
-        tmem_ld_32x32b_x32(tmem_base + lane_base + c * 32, r);
-        const uint32_t qb = qbuf + 2048u * (ck & 3);
-        if (lane == 0) bulk_wait_read<3>();  // the store that last read this output tile (four chunks ago) is done
-        __syncwarp();
-        tmem_ld_wait();
-        float v[32];
-#pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-        const int which = (c * 32) / C;  // 0 q, 1 k, 2 v (compile-time after unrolling)
-        if (which < 2) {
-          const float sc = which == 0 ? qscale : 1.0f;
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            const float x0 = v[2 * i], x1 = v[2 * i + 1];
-            v[2 * i] = (x0 * cs[i] - x1 * sn[i]) * sc;
-            v[2 * i + 1] = (x1 * cs[i] + x0 * sn[i]) * sc;
-          }
-        }
-#pragma unroll
-        for (int i = 0; i < 4; ++i)
-          st_shared_v4(qb + lane * 64 + ((static_cast<uint32_t>(i) << 4) ^ sw64), pack_h16x2(v[8 * i], v[8 * i + 1]),
-                       pack_h16x2(v[8 * i + 2], v[8 * i + 3]), pack_h16x2(v[8 * i + 4], v[8 * i + 5]),
-                       pack_h16x2(v[8 * i + 6], v[8 * i + 7]));
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) {
-          tma_store_2d(&tmQ, qb, c * 32, tile * 128 + warp * 32);  // rows beyond M are clipped
-          bulk_commit();
-        }
-      }
-    }  // tile loop
-    if (lane == 0) bulk_wait_read<0>();
-    __syncwarp();
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) tmem_dealloc<Cfg::TCOLS>(tmem_base);
-}
-
 struct TcQkvPlan {
-  CUtensorMap tmW;
+  const void* w;
   int C;
   int64_t M;
-  // activation tensor maps, (re)encoded when a launch names other buffers (a call site always passes the same ones)
-  mutable CUtensorMap tmX, tmQ;
-  mutable const void *k_x = nullptr, *k_q = nullptr;
 };
 TcQkvPlan* tc_qkv_plan_create(const void* wqkv_h16, int C, int64_t M, char* err, int errlen) {
   if (C != 32 && C != 64) { snprintf(err, errlen, "fused qkv: C must be 32 or 64"); return nullptr; }
   TcQkvPlan* p = new TcQkvPlan();
-  p->C = C; p->M = M;
-  const uint64_t dims[2] = {static_cast<uint64_t>(C), static_cast<uint64_t>(3 * C)};
-  const uint64_t strides[1] = {static_cast<uint64_t>(C) * 2};
-  const uint32_t box[2] = {static_cast<uint32_t>(C), static_cast<uint32_t>(3 * C)};
-  if (!make_tmap(&p->tmW, wqkv_h16, 2, dims, strides, box, C * 2 < 128 ? C * 2 : 128, err, errlen)) { delete p; return nullptr; }
+  p->w = wqkv_h16; p->C = C; p->M = M;
   return p;
 }
 void tc_qkv_plan_destroy(TcQkvPlan* p) { delete p; }
 int launch_fused_qkv(const TcQkvPlan* p, const float* X, const float* wg, const float* bg, const float* rope_cos,
                      const float* rope_sin, void* qkv, float* gates, int L, int F, int posmode, float qscale,
                      cudaStream_t st) {
-  if (p->k_x != X || p->k_q != qkv) {
-    char err[256];
-    const uint32_t box[2] = {32, 32};
-    const uint64_t dx[2] = {static_cast<uint64_t>(p->C), static_cast<uint64_t>(p->M)};
-    const uint64_t sx[1] = {static_cast<uint64_t>(p->C) * 4};
-    const uint64_t dq[2] = {static_cast<uint64_t>(3 * p->C), static_cast<uint64_t>(p->M)};
-    const uint64_t sq[1] = {static_cast<uint64_t>(3 * p->C) * 2};
-    if (!make_tmap_f32(&p->tmX, X, 2, dx, sx, box, 128, err, sizeof(err)) || !make_tmap(&p->tmQ, qkv, 2, dq, sq, box, 64, err, sizeof(err)))
-      return -1;
-    p->k_x = X; p->k_q = qkv;
-  }
-  const unsigned ntiles = static_cast<unsigned>((p->M + 127) / 128);
-  const unsigned slots = static_cast<unsigned>(g_num_sms) * (p->C == 32 ? 3u : 2u);
-  const unsigned grid = ntiles < slots ? ntiles : slots;  // persistent CTAs
+  const h16* w = static_cast<const h16*>(p->w);
+  h16* out = static_cast<h16*>(qkv);
   if (p->C == 32)
-    fused_qkv_kernel<32><<<grid, FF_THREADS, QkvCfg<32>::SMEM, st>>>(p->tmW, p->tmX, p->tmQ, wg, bg, rope_cos, rope_sin, gates, p->M, L, F, posmode, qscale);
+    fused_qkv_kernel<32><<<fused_grid(p->M, qkv_ctas<32>()), FU_THREADS, qkv_smem<32>(), st>>>(w, X, wg, bg, rope_cos, rope_sin, out,
+                                                                                             gates, p->M, L, F, posmode, qscale);
   else
-    fused_qkv_kernel<64><<<grid, FF_THREADS, QkvCfg<64>::SMEM, st>>>(p->tmW, p->tmX, p->tmQ, wg, bg, rope_cos, rope_sin, gates, p->M, L, F, posmode, qscale);
+    fused_qkv_kernel<64><<<fused_grid(p->M, qkv_ctas<64>()), FU_THREADS, qkv_smem<64>(), st>>>(w, X, wg, bg, rope_cos, rope_sin, out,
+                                                                                             gates, p->M, L, F, posmode, qscale);
   return 0;
 }
+
 int tc_init_fused(char* err, int errlen) {
-  cudaError_t r = cudaFuncSetAttribute(fused_ff_kernel<32, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, FfCfg<32>::SMEM);
-  if (r == cudaSuccess) r = cudaFuncSetAttribute(fused_ff_kernel<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, FfCfg<64>::SMEM);
-  if (r == cudaSuccess) r = cudaFuncSetAttribute(fused_ff_kernel<32, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, FfCfg<32>::SMEM);
-  if (r == cudaSuccess) r = cudaFuncSetAttribute(fused_ff_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, FfCfg<64>::SMEM);
-  if (r == cudaSuccess) r = cudaFuncSetAttribute(fused_qkv_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, QkvCfg<32>::SMEM);
-  if (r == cudaSuccess) r = cudaFuncSetAttribute(fused_qkv_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, QkvCfg<64>::SMEM);
+  cudaError_t r = cudaFuncSetAttribute(fused_ff_kernel<32, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, ff_smem<32>(false));
+  if (r == cudaSuccess) r = cudaFuncSetAttribute(fused_ff_kernel<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, ff_smem<64>(false));
+  if (r == cudaSuccess) r = cudaFuncSetAttribute(fused_ff_kernel<32, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, ff_smem<32>(true));
+  if (r == cudaSuccess) r = cudaFuncSetAttribute(fused_ff_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, ff_smem<64>(true));
+  if (r == cudaSuccess) r = cudaFuncSetAttribute(fused_qkv_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, qkv_smem<32>());
+  if (r == cudaSuccess) r = cudaFuncSetAttribute(fused_qkv_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, qkv_smem<64>());
   if (r != cudaSuccess) {
     snprintf(err, errlen, "cudaFuncSetAttribute(fused_ff_kernel / fused_qkv_kernel) failed: %s", cudaGetErrorString(r));
     return -1;

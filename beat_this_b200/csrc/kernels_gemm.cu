@@ -1,7 +1,7 @@
-// 16-bit tensor-core GEMM for sm_100a: D = A * W^T over "planes" with shifted slabs (linear layers, the
-// k(2,3) frontend convolutions as implicit GEMM, frontend.linear), tcgen05.mma with TMEM accumulators,
+// 16-bit tensor-core GEMM for sm_90a: D = A * W^T over "planes" with shifted slabs (linear layers, the
+// k(2,3) frontend convolutions as implicit GEMM, frontend.linear), wgmma with register accumulators,
 // TMA (cp.async.bulk.tensor) operand staging through an mbarrier ring, persistent over output tiles,
-// warp-specialised roles, fused epilogues (epilogue.cuh).  Reference call sites: every nn.Linear /
+// warp-specialised roles (one producer warp, two consumer warpgroups), fused epilogues (epilogue.cuh).  Reference call sites: every nn.Linear /
 // Conv2d of beat_this/model/roformer.py:53-61,103-111 and beat_tracker.py:77,155-166.
 #include <cstdio>
 #include <cstdlib>
@@ -17,7 +17,7 @@ typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_
                                     const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                     CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 static PFN_encodeTiled g_encode = nullptr;
-int g_num_sms = 148;
+int g_num_sms = 132;
 
 static bool make_tmap_any(CUtensorMap* tm, CUtensorMapDataType dt, const void* base, int rank, const uint64_t* dims,
                           const uint64_t* strides_bytes /* rank-1 */, const uint32_t* box, int swizzle_bytes,
@@ -48,419 +48,126 @@ bool make_tmap(CUtensorMap* tm, const void* base, int rank, const uint64_t* dims
   return make_tmap_any(tm, BT_H16_IS_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, base, rank,
                        dims, strides_bytes, box, swizzle_bytes, err, errlen);
 }
-bool make_tmap_f32(CUtensorMap* tm, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                   const uint32_t* box, int swizzle_bytes, char* err, int errlen) {
-  return make_tmap_any(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, base, rank, dims, strides_bytes, box, swizzle_bytes, err, errlen);
-}
 
 // =============================================================================== GEMM
+// CTA = 128 output rows x BN columns, persistent over tiles (stride gridDim.x).  Warp 0 (one elected lane) streams
+// the A and W k-blocks through a STAGES-deep TMA ring; warpgroups 1 and 2 own rows [0, 64) and [64, 128) of the
+// tile and issue wgmma m64nNCk16 over NC-column slices of it (NC = 64, or 32 when BN is not a multiple of 64).  The
+// accumulators stay in registers and go through epilogue_pair straight to global memory.
 constexpr int TG_BM = 128;
-constexpr int TG_EPI_WARPS = 8;
-constexpr int TG_THREADS = 64 + 32 * TG_EPI_WARPS;  // warp0 TMA, warp1 MMA, 8 epilogue warps
+constexpr int TG_THREADS = 384;  // warpgroup 0: producer (warp 0), warpgroups 1-2: MMA + epilogue
 
-// TE = epilogue through TMA in both directions (BN >= 128): every epilogue warp owns a staging area
-//   [fp32 tile 0: 32 rows x 128 B][fp32 tile 1][optional 16-bit tile: 32 rows x 64 B][bias of the warp's columns]
-// the fp32 residual tile is TMA-loaded into a staging tile (the next chunk's tile is in flight while the current one
-// is processed), the result overwrites it in place and is TMA-stored from there; 16-bit outputs rotate through the
-// same area as 2 KB tiles.  Threads never touch global memory: the row-per-lane ld/st.global of the direct epilogue
-// (32 sectors per warp instruction) kept the LSU queue full and the next tcgen05.ld waiting on the registers of
-// stores still queued (ncu source view, profiles/r2_notes.md).
-template <int BN, int BK, bool TE>
+template <int BN, int BK>
 struct TgCfg {
   static constexpr int A_BYTES = TG_BM * BK * 2;
   static constexpr int W_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + W_BYTES;
-  static constexpr int EPI_H16_EXTRA = (TE && BN <= 192) ? 2048 : 0;   // third staging tile: fp32 + 16-bit outputs together
-  static constexpr int EPI_WARP = TE ? 8192 + EPI_H16_EXTRA : 0;      // staging tiles of one warp (multiple of 1024)
-  // bias: TE: 512 B slice per warp (the warp's <= 128 columns of the current tile); direct epilogue: whole vector
-  static constexpr int BIAS_BYTES = TE ? TG_EPI_WARPS * 512 : 16384;
-  static constexpr int FIXED = 1024 /*align*/ + 512 /*barriers*/ + BIAS_BYTES + TG_EPI_WARPS * EPI_WARP;
+  static constexpr int FIXED = 1024 /*align*/ + 256 /*barriers*/;
   static constexpr int STAGES_FIT = (232448 - FIXED) / STAGE_BYTES;
-  static constexpr int STAGES = STAGES_FIT > 8 ? 8 : STAGES_FIT;
-  static constexpr int TCOLS = 2 * BN <= 32 ? 32 : 2 * BN <= 64 ? 64 : 2 * BN <= 128 ? 128 : 2 * BN <= 256 ? 256 : 512;
+  static constexpr int STAGES = STAGES_FIT > 6 ? 6 : STAGES_FIT;
   static constexpr int SMEM = STAGES * STAGE_BYTES + FIXED;
   static constexpr int SWZ = BK * 2;  // 128 or 64 byte rows
+  static constexpr int NC = BN % 64 == 0 ? 64 : 32;
+  static constexpr int NCH = BN / NC;
 };
 
-// EM: 0 direct epilogue (epilogue.cuh, any EpiParams); TMA epilogues: EM_QKV RoPE + q scale -> 16-bit; EM_ACT bias +
-// GELU -> 16-bit; EM_RESID [bias +] fp32 residual -> fp32 in place [+ 16-bit copy]; EM_F32 bias [+ GELU] -> fp32
-enum { EM_DIRECT = 0, EM_QKV = 1, EM_ACT = 2, EM_RESID = 3, EM_F32 = 4 };
-
-template <int BN, int BK, int EM>
+template <int BN, int BK>
 __global__ void __launch_bounds__(TG_THREADS, 1)
-gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW,
-               const __grid_constant__ CUtensorMap tmOutAct, const __grid_constant__ CUtensorMap tmOutF32,
-               const __grid_constant__ CUtensorMap tmResid, const GemmShape g, const EpiParams e, int num_tiles,
-               int t_tiles, int n_tiles, int m_tiles) {
-  constexpr bool TE = EM != EM_DIRECT;
-  using Cfg = TgCfg<BN, BK, TE>;
+gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW, const GemmShape g,
+               const EpiParams e, int num_tiles, int t_tiles, int n_tiles, int m_tiles) {
+  using Cfg = TgCfg<BN, BK>;
   constexpr int STAGES = Cfg::STAGES;
+  constexpr int NC = Cfg::NC;
+  constexpr int NCH = Cfg::NCH;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sA = smem;
-  uint8_t* sW = smem + STAGES * Cfg::A_BYTES;
-  uint8_t* sEpi = smem + STAGES * Cfg::STAGE_BYTES;  // 1024-aligned (STAGE_BYTES % 1024 == 0): TE staging tiles
-  uint64_t* full = reinterpret_cast<uint64_t*>(sEpi + TG_EPI_WARPS * Cfg::EPI_WARP);
-  uint64_t* empty = full + STAGES;
-  uint64_t* tfull = empty + STAGES;
-  uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tempty + 2);
-  uint64_t* rbar = tempty + 4;  // TE: [TG_EPI_WARPS][2] residual-tile barriers
-  float* sBias = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(full) + 512);
+  const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t sA = sbase;
+  const uint32_t sW = sbase + STAGES * Cfg::A_BYTES;
+  const uint32_t full = sbase + STAGES * Cfg::STAGE_BYTES;  // [STAGES] k-block landed
+  const uint32_t empty = full + 8 * STAGES;                  // [STAGES] both consumer warpgroups done with it
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const bool stage_bias = !TE && e.kind == 0 && e.bias != nullptr && g.N <= Cfg::BIAS_BYTES / 4;
-  if (stage_bias)
-    for (int i = threadIdx.x; i < g.N; i += TG_THREADS) sBias[i] = __ldg(e.bias + i);
-  const uint32_t bias_smem = stage_bias ? smem_u32(sBias) : 0u;
-
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmW);
-    if constexpr (TE) {
-      if (e.out_act) tma_prefetch_desc(&tmOutAct);
-      if (e.out_f32) tma_prefetch_desc(&tmOutF32);
-      if (e.resid) tma_prefetch_desc(&tmResid);
+    for (int i = 0; i < STAGES; ++i) {
+      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(full + 8 * i), "r"(1));
+      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(empty + 8 * i), "r"(2));
     }
-  }
-  if (warp == 1 && lane == 0) {
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&tfull[i], 1); mbar_init(&tempty[i], BN <= 64 ? TG_EPI_WARPS / 2 : TG_EPI_WARPS); }
-    if constexpr (TE)
-      for (int i = 0; i < 2 * TG_EPI_WARPS; ++i) mbar_init(&rbar[i], 1);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<Cfg::TCOLS>(tmem_ptr);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
   const int kb_per_slab = g.Kslab / BK;
   const int num_kb = g.nslab * kb_per_slab;
 
   if (warp == 0) {
-    // producer and MMA warps run CONVERGED with predicated single-lane TMA / MMA / commit instructions
-    // (see umma_h16_p): in a divergent `if (lane == 0)` block every tcgen05.mma costs ~85 issue cycles.
-    const uint32_t on = elect_one() ? 1u : 0u;
+    if (lane == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const int mt = tile / n_tiles, nt = tile % n_tiles;
+        const int p_out = mt / t_tiles;
+        const int t0 = (mt - p_out * t_tiles) * TG_BM;
+        for (int kb = 0; kb < num_kb; ++kb) {
+          const int s = kb / kb_per_slab;
+          const int k0 = (kb - s * kb_per_slab) * BK;
+          mbar_wait_a(empty + 8 * stage, phase ^ 1);
+          const uint32_t fb = full + 8 * stage;
+          mbar_expect_tx_a(fb, Cfg::STAGE_BYTES);
+          // A rows outside [0, L) of the plane (conv time shifts, the last tile of a plane) arrive as zeros
+          tma_load_3d_a(sA + stage * Cfg::A_BYTES, &tmA, fb, k0, t0 + g.t_shift[s], p_out * g.plane_mul + g.plane_add[s]);
+          tma_load_2d_a(sW + stage * Cfg::W_BYTES, &tmW, fb, s * g.Kslab + k0, nt * BN);
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        }
+      }
+    }
+  } else if (warp >= 4) {
+    const int wg = (warp >> 2) - 1;   // 0: tile rows [0, 64), 1: [64, 128)
+    const int wq = warp & 3;          // warp inside the warpgroup: 16 rows each
+    const uint32_t a_off = static_cast<uint32_t>(wg * 64 * BK * 2);
     int stage = 0;
     uint32_t phase = 0;
+    float acc[NCH][NC / 2];
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int mt = tile / n_tiles, nt = tile % n_tiles;
       const int p_out = mt / t_tiles;
-      const int t0 = (mt - p_out * t_tiles) * TG_BM;
       for (int kb = 0; kb < num_kb; ++kb) {
-        const int s = kb / kb_per_slab;
-        const int k0 = (kb - s * kb_per_slab) * BK;
-        mbar_wait(&empty[stage], phase ^ 1);
-        const uint32_t fb = smem_u32(&full[stage]);
-        mbar_expect_tx_p(on, fb, Cfg::STAGE_BYTES);
-        tma_load_3d_p(on, smem_u32(sA + stage * Cfg::A_BYTES), &tmA, fb, k0, t0 + g.t_shift[s],
-                      p_out * g.plane_mul + g.plane_add[s]);
-        tma_load_2d_p(on, smem_u32(sW + stage * Cfg::W_BYTES), &tmW, fb, s * g.Kslab + k0, nt * BN);
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else if (warp == 1) {
-    const uint32_t on = elect_one() ? 1u : 0u;
-    constexpr uint32_t idesc = make_idesc_h16(TG_BM, BN);
-    int stage = 0;
-    uint32_t phase = 0;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      mbar_wait(&tempty[acc], acc_phase ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + acc * BN;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full[stage], phase);
-        tc_fence_after();
-        const uint32_t a_base = smem_u32(sA + stage * Cfg::A_BYTES);
-        const uint32_t b_base = smem_u32(sW + stage * Cfg::W_BYTES);
+        mbar_wait_a(full + 8 * stage, phase);
+        const uint32_t a_base = sA + stage * Cfg::A_BYTES + a_off;
+        const uint32_t b_base = sW + stage * Cfg::W_BYTES;
+        wgmma_fence();
 #pragma unroll
         for (int k = 0; k < BK / 16; ++k) {
-          umma_h16_p(on, d_tmem, make_kmajor_desc<Cfg::SWZ>(a_base + k * 32), make_kmajor_desc<Cfg::SWZ>(b_base + k * 32),
-                     idesc, (kb | k) != 0 ? 1u : 0u);
+          const uint64_t da = make_wgmma_desc<Cfg::SWZ>(a_base + k * 32);
+#pragma unroll
+          for (int c = 0; c < NCH; ++c)
+            wgmma_n<NC>(acc[c], da, make_wgmma_desc<Cfg::SWZ>(b_base + c * NC * BK * 2 + k * 32), (kb | k) != 0 ? 1u : 0u);
         }
-        umma_commit_p(on, smem_u32(&empty[stage]));
-        if (kb == num_kb - 1) umma_commit_p(on, smem_u32(&tfull[acc]));
+        wgmma_commit();
+        wgmma_wait<0>();
+        if ((threadIdx.x & 127) == 0) mbar_arrive_a(empty + 8 * stage);
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
-    }
-  } else if constexpr (TE) {
-    // TMA epilogue (see TgCfg), specialised at compile time by EM (what the call site needs) so that the chunk loop
-    // is straight-line code on packed fp32 pairs.  Warp (quarter, half): TMEM lanes / tile rows [32*quarter, +32),
-    // columns [half*BN/2, +BN/2) in chunks of 32; thread = one output row of the chunk.  The accumulator chunk k+1
-    // is requested (tcgen05.ld) before chunk k is processed.
-    const int ew = warp - 2;
-    const int quarter = warp & 3;
-    const int half = ew >> 2;
-    constexpr int NCH = BN / 32;
-    constexpr int SPLIT = (NCH + 1) / 2;
-    const int c_begin = half == 0 ? 0 : SPLIT;
-    const int nch = half == 0 ? SPLIT : NCH - SPLIT;
-    const uint32_t ebase = smem_u32(sEpi) + static_cast<uint32_t>(ew) * Cfg::EPI_WARP;
-    const uint32_t bias_w = smem_u32(sBias) + 512u * ew;  // this warp's bias slice
-    const uint32_t rb0 = smem_u32(&rbar[2 * ew]);
-    const uint32_t tm_lane = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16);
-    constexpr bool RESID = EM == EM_RESID;
-    constexpr bool F32_OUT = EM == EM_RESID || EM == EM_F32;
-    constexpr bool ACT_ONLY = EM == EM_QKV || EM == EM_ACT;
-    const bool has_bias = EM != EM_QKV && e.bias != nullptr;
-    const bool do_gelu = EM == EM_ACT || (EM == EM_F32 && e.gelu);
-    const bool act_copy = RESID && e.out_act != nullptr;  // 16-bit copy next to the fp32 result (frontend block 2 -> conv)
-    const uint32_t sw64 = static_cast<uint32_t>((lane >> 1) & 3) << 4;
-    const uint32_t sw128 = static_cast<uint32_t>(lane & 7) << 4;
-    const uint32_t frow = static_cast<uint32_t>(lane) * 128u, hrow = static_cast<uint32_t>(lane) * 64u;
-    uint32_t rphase = 0;   // bit b: parity of residual barrier b
-    int ck = 0;            // running chunk counter of this warp (staging tile rotation continues across tiles)
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const int mt = tile / n_tiles, nt = tile % n_tiles;
-      const int p_out = mt / t_tiles;
-      const int trow0 = (mt - p_out * t_tiles) * TG_BM + quarter * 32;  // first row of this warp inside the plane
-      const int t = trow0 + lane;
-      const int col_w = nt * BN + c_begin * 32;  // first column of this warp
-      if (has_bias) {  // bias of the warp's columns -> shared memory (broadcast reads in the chunk loop)
-        if (4 * lane < nch * 32) {
-          const float4 b4 = __ldg(reinterpret_cast<const float4*>(e.bias + col_w) + lane);
-          asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(bias_w + 16u * lane), "f"(b4.x), "f"(b4.y), "f"(b4.z), "f"(b4.w) : "memory");
-        }
-        __syncwarp();
-      }
-      float cs[EM == EM_QKV ? 16 : 1], sn[EM == EM_QKV ? 16 : 1];  // cos | sin of this row's position (every q / k head)
-      if constexpr (EM == EM_QKV) {
-        const int tt = t < g.L ? t : 0;
-        const int pos = e.posmode == 0 ? tt : static_cast<int>(p_out % e.F);
-        const float4* c4 = reinterpret_cast<const float4*>(e.rope_cos + pos * 16);
-        const float4* s4 = reinterpret_cast<const float4*>(e.rope_sin + pos * 16);
+      // epilogue: this thread's rows t and t + 8, columns 8j + 2 (lane % 4) + {0, 1} of every slice
+      const int tr = (mt - p_out * t_tiles) * TG_BM + wg * 64 + wq * 16 + (lane >> 2);
+      const int col0 = nt * BN + 2 * (lane & 3);
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const float4 a = __ldg(c4 + i), b = __ldg(s4 + i);
-          cs[4 * i] = a.x; cs[4 * i + 1] = a.y; cs[4 * i + 2] = a.z; cs[4 * i + 3] = a.w;
-          sn[4 * i] = b.x; sn[4 * i + 1] = b.y; sn[4 * i + 2] = b.z; sn[4 * i + 3] = b.w;
+      for (int h = 0; h < 2; ++h) {
+        const int t = tr + 8 * h;
+        if (t < g.L && mt < m_tiles) {
+          const int64_t m = static_cast<int64_t>(p_out) * g.L + t;
+          const int pos = e.kind != 1 ? 0 : e.posmode == 0 ? t : p_out % e.F;
+#pragma unroll
+          for (int c = 0; c < NCH; ++c)
+#pragma unroll
+            for (int j = 0; j < NC / 8; ++j)
+              epilogue_pair<h16>(e, m, pos, col0 + c * NC + 8 * j, acc[c][4 * j + 2 * h], acc[c][4 * j + 2 * h + 1]);
         }
       }
-      if constexpr (RESID) {  // residual tile of the first chunk (its staging tile was released two chunks ago)
-        const int b = ck & 1;
-        if (lane == 0) {
-          bulk_wait_read<1>();
-          mbar_expect_tx_a(rb0 + 8 * b, 4096);
-          tma_load_3d_a(ebase + 4096 * b, &tmResid, rb0 + 8 * b, col_w, trow0, p_out);
-        }
-        __syncwarp();
-      }
-      mbar_wait(&tfull[acc], acc_phase);
-      tc_fence_after();
-      uint32_t ra[32], rb[32];
-      tmem_ld_32x32b_x32(tm_lane + acc * BN + c_begin * 32, ra);
-      tmem_ld_wait();
-#pragma unroll
-      for (int k = 0; k < SPLIT; ++k) {
-        if (k < nch) {
-          uint32_t (&r)[32] = (k & 1) ? rb : ra;
-          uint32_t (&rn)[32] = (k & 1) ? ra : rb;
-          if (k + 1 < nch) tmem_ld_32x32b_x32(tm_lane + acc * BN + (c_begin + k + 1) * 32, rn);  // in flight during chunk k
-          const int n0 = col_w + k * 32;
-          const int b = ck & 1;
-          const uint32_t fbuf = ebase + 4096 * b;                                   // fp32 staging tile of this chunk
-          const uint32_t hbuf = ACT_ONLY ? ebase + 2048 * (ck & 3) : ebase + 8192;  // 16-bit staging tile
-          if (lane == 0) {  // staging tiles about to be (re)written must have been read by their last TMA store
-            if constexpr (RESID) {
-              // next chunk's residual tile goes into the other fp32 tile, last stored one chunk ago; the 16-bit copy
-              // (single extra tile) was last stored one chunk ago as well
-              if (k + 1 < nch || act_copy) bulk_wait_read<0>();
-              if (k + 1 < nch) {
-                mbar_expect_tx_a(rb0 + 8 * (b ^ 1), 4096);
-                tma_load_3d_a(ebase + 4096 * (b ^ 1), &tmResid, rb0 + 8 * (b ^ 1), n0 + 32, trow0, p_out);
-              }
-            } else if constexpr (ACT_ONLY) {
-              bulk_wait_read<3>();
-            } else {
-              bulk_wait_read<1>();
-            }
-          }
-          __syncwarp();
-          uint64_t v[16];  // 32 accumulator columns as fp32 pairs
-#pragma unroll
-          for (int i = 0; i < 16; ++i) v[i] = pack_f32x2(__uint_as_float(r[2 * i]), __uint_as_float(r[2 * i + 1]));
-          if constexpr (EM == EM_QKV) {
-            // RoPE on interleaved pairs (rotary_embedding_torch semantics, roformer.py:121-123) + q scaling
-            const int which = n0 / e.C;  // 0 q, 1 k, 2 v: a 32-column chunk is one head of one of them
-            if (which < 2) {
-              const float sc = which == 0 ? e.qscale : 1.0f;
-#pragma unroll
-              for (int i = 0; i < 16; ++i) {
-                float x0, x1;
-                unpack_f32x2(v[i], x0, x1);
-                const float co = cs[i] * sc, si = sn[i] * sc;
-                v[i] = pack_f32x2(fmaf(-x1, si, x0 * co), fmaf(x0, si, x1 * co));
-              }
-            }
-          } else {
-            if (has_bias) {
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                const float4 q = ld_shared_v4_f32(bias_w + static_cast<uint32_t>(k * 32 + 4 * i) * 4u);
-                v[2 * i] = add_f32x2(v[2 * i], pack_f32x2(q.x, q.y));
-                v[2 * i + 1] = add_f32x2(v[2 * i + 1], pack_f32x2(q.z, q.w));
-              }
-            }
-            if (do_gelu) {
-#pragma unroll
-              for (int i = 0; i < 16; ++i) v[i] = gelu_tanh_f32x2(v[i]);
-            }
-            if constexpr (RESID) {
-              mbar_wait_a(rb0 + 8 * b, (rphase >> b) & 1u);
-              rphase ^= 1u << b;
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                const float4 q = ld_shared_v4_f32(fbuf + frow + ((static_cast<uint32_t>(i) << 4) ^ sw128));
-                v[2 * i] = add_f32x2(v[2 * i], pack_f32x2(q.x, q.y));
-                v[2 * i + 1] = add_f32x2(v[2 * i + 1], pack_f32x2(q.z, q.w));
-              }
-            }
-          }
-          if constexpr (F32_OUT) {
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              float a0, a1, a2, a3;
-              unpack_f32x2(v[2 * i], a0, a1);
-              unpack_f32x2(v[2 * i + 1], a2, a3);
-              asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(fbuf + frow + ((static_cast<uint32_t>(i) << 4) ^ sw128)),
-                           "f"(a0), "f"(a1), "f"(a2), "f"(a3) : "memory");
-            }
-          }
-          const bool h16_tile = ACT_ONLY || (act_copy && Cfg::EPI_H16_EXTRA != 0);
-          if (h16_tile) {
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              uint32_t w[4];
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                float a0, a1;
-                unpack_f32x2(v[4 * i + j], a0, a1);
-                w[j] = pack_h16x2(a0, a1);
-              }
-              st_shared_v4(hbuf + hrow + ((static_cast<uint32_t>(i) << 4) ^ sw64), w[0], w[1], w[2], w[3]);
-            }
-          } else if (act_copy) {  // no room for a third staging tile (BN = 256): direct row store of the 16-bit copy
-            if (t < g.L) {
-              float f[32];
-#pragma unroll
-              for (int i = 0; i < 16; ++i) unpack_f32x2(v[i], f[2 * i], f[2 * i + 1]);
-              store_act<h16, 32>(reinterpret_cast<h16*>(e.out_act) + (static_cast<int64_t>(p_out) * g.L + t) * e.ldo_act + n0, f);
-            }
-          }
-          fence_proxy_async_smem();
-          __syncwarp();
-          if (lane == 0) {
-            if constexpr (F32_OUT) tma_store_3d(&tmOutF32, fbuf, n0, trow0, p_out);
-            if (h16_tile) tma_store_3d(&tmOutAct, hbuf, n0, trow0, p_out);
-            bulk_commit();
-          }
-          ++ck;
-          if (k + 1 < nch) tmem_ld_wait();
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty[acc]);
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
-    }
-    if (lane == 0) bulk_wait_read<0>();  // shared memory must outlive the last stores' reads
-    __syncwarp();
-  } else {
-    // Epilogue warps.  A warp may only touch TMEM lanes [32*(warp%4), +32); thread = one output row.
-    //  BN >= 96: the 8 warps split the columns of every tile (2 warps per lane quarter);
-    //  BN <= 64: warps 2-5 take the even tiles of this CTA and warps 6-9 the odd ones.
-    // The residual rows of the NEXT 32-column chunk are requested before the current chunk is
-    // processed (software pipelining: the epilogue is latency-bound on those loads otherwise,
-    // ncu long_scoreboard 64% -- profiles/r1_notes.md).
-    const int ew = warp - 2;
-    const int quarter = warp & 3;
-    const int half = ew >> 2;
-    constexpr int NCH = BN / 32;
-    constexpr bool TILE_SPLIT = NCH <= 2;
-    constexpr int SPLIT = (NCH + 1) / 2;
-    constexpr int MAXC = TILE_SPLIT ? NCH : SPLIT;
-    const int c_begin = TILE_SPLIT ? 0 : (half == 0 ? 0 : SPLIT);
-    const int nch = TILE_SPLIT ? NCH : (half == 0 ? SPLIT : NCH - SPLIT);
-    const int row = quarter * 32 + lane;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    int iter = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++iter) {
-      if (TILE_SPLIT && (iter & 1) != half) {
-        acc ^= 1;
-        if (acc == 0) acc_phase ^= 1;
-        continue;
-      }
-      const int mt = tile / n_tiles, nt = tile % n_tiles;
-      const int p_out = mt / t_tiles;
-      const int t = (mt - p_out * t_tiles) * TG_BM + row;
-      const bool valid = t < g.L && mt < m_tiles;
-      const int64_t m = static_cast<int64_t>(p_out) * g.L + t;
-      float ra[32], rb[32];
-      const bool has_resid = e.kind == 0 && e.resid != nullptr && valid;
-      const bool has_rope = e.kind == 1 && valid;
-      auto load_resid = [&](int c, float (&dst)[32]) {
-        const float4* r4 = reinterpret_cast<const float4*>(e.resid + m * e.ldr + nt * BN + c * 32);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const float4 q = r4[i];
-          dst[4 * i] = q.x; dst[4 * i + 1] = q.y; dst[4 * i + 2] = q.z; dst[4 * i + 3] = q.w;
-        }
-      };
-      if (has_rope) {  // cos[16] | sin[16] of this row's position, reused by every q/k head of the row
-        const int pos = e.posmode == 0 ? t : static_cast<int>((m / g.L) % e.F);
-        const float4* c4 = reinterpret_cast<const float4*>(e.rope_cos + pos * 16);
-        const float4* s4 = reinterpret_cast<const float4*>(e.rope_sin + pos * 16);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const float4 a = __ldg(c4 + i), b = __ldg(s4 + i);
-          ra[4 * i] = a.x; ra[4 * i + 1] = a.y; ra[4 * i + 2] = a.z; ra[4 * i + 3] = a.w;
-          ra[16 + 4 * i] = b.x; ra[16 + 4 * i + 1] = b.y; ra[16 + 4 * i + 2] = b.z; ra[16 + 4 * i + 3] = b.w;
-        }
-#pragma unroll
-        for (int i = 0; i < 32; ++i) rb[i] = ra[i];  // either buffer may be handed to the epilogue
-      }
-      if (has_resid) load_resid(c_begin, ra);  // in flight while we wait for the accumulator
-      mbar_wait(&tfull[acc], acc_phase);
-      tc_fence_after();
-#pragma unroll
-      for (int k = 0; k < MAXC; ++k) {
-        if (k < nch) {
-          const int c = c_begin + k;
-          float (&cur)[32] = (k & 1) ? rb : ra;
-          float (&nxt)[32] = (k & 1) ? ra : rb;
-          if (has_resid && k + 1 < nch) load_resid(c + 1, nxt);
-          uint32_t r[32];
-          tmem_ld_32x32b_x32(tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc * BN + c * 32, r);
-          tmem_ld_wait();
-          if (valid) {
-            float v[32];
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-            epilogue_apply<h16, 32>(e, g.L, m, nt * BN + c * 32, v, cur, has_rope || has_resid, bias_smem);
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty[acc]);
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<Cfg::TCOLS>(tmem_base);
 }
 
 struct TcGemmPlan {
@@ -468,65 +175,29 @@ struct TcGemmPlan {
   GemmShape g;
   int BN, BK;
   int num_tiles, t_tiles, n_tiles, m_tiles, grid;
-  // TMA epilogue: output / residual tensor maps, (re)encoded when the epilogue targets of a launch change (a call
-  // site always passes the same ones, so this happens once)
-  mutable CUtensorMap tmOutAct, tmOutF32, tmResid;
-  mutable const void *k_act = nullptr, *k_f32 = nullptr, *k_res = nullptr;
-  mutable int k_lda = 0, k_ldf = 0, k_ldr = 0;
-  mutable bool epi_ok = false;
 };
 
+// BN = 256 would need 128 accumulator registers per thread and spills at the 168-register limit of 384 threads
 static int pick_bn(int N) {
-  const int cands[6] = {256, 192, 128, 96, 64, 32};
-  for (int i = 0; i < 6; ++i)
+  const int cands[5] = {192, 128, 96, 64, 32};
+  for (int i = 0; i < 5; ++i)
     if (N % cands[i] == 0) return cands[i];
   return 0;
 }
 
-template <int BN, int BK, int EM>
+template <int BN, int BK>
 static int gemm_tc_launch(const TcGemmPlan* p, const EpiParams& e, cudaStream_t st) {
-  using Cfg = TgCfg<BN, BK, EM != EM_DIRECT>;
+  using Cfg = TgCfg<BN, BK>;
   static_assert(Cfg::STAGES >= 2, "pipeline too shallow");
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t r = cudaFuncSetAttribute(gemm_tc_kernel<BN, BK, EM>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
+    cudaError_t r = cudaFuncSetAttribute(gemm_tc_kernel<BN, BK>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
     if (r != cudaSuccess) return -1;
     attr_set = true;
   }
-  gemm_tc_kernel<BN, BK, EM><<<p->grid, TG_THREADS, Cfg::SMEM, st>>>(p->tmA, p->tmW, p->tmOutAct, p->tmOutF32, p->tmResid, p->g,
-                                                                       e, p->num_tiles, p->t_tiles, p->n_tiles, p->m_tiles);
+  gemm_tc_kernel<BN, BK><<<p->grid, TG_THREADS, Cfg::SMEM, st>>>(p->tmA, p->tmW, p->g, e, p->num_tiles, p->t_tiles,
+                                                                  p->n_tiles, p->m_tiles);
   return 0;
-}
-
-// tensor maps of the epilogue targets: [planes_out, L, ld] row-major views with 32-row x 32-column boxes, so that
-// the rows a tile has beyond the end of its plane (L is not a multiple of 128) are clipped / zero-filled by TMA
-static bool prepare_tma_epilogue(const TcGemmPlan* p, const EpiParams& e) {
-  if (p->k_act == e.out_act && p->k_f32 == e.out_f32 && p->k_res == e.resid && p->k_lda == e.ldo_act && p->k_ldf == e.ldo_f32 &&
-      p->k_ldr == e.ldr)
-    return p->epi_ok;
-  p->k_act = e.out_act; p->k_f32 = e.out_f32; p->k_res = e.resid;
-  p->k_lda = e.ldo_act; p->k_ldf = e.ldo_f32; p->k_ldr = e.ldr;
-  char err[256];
-  const GemmShape& g = p->g;
-  bool ok = true;
-  auto enc = [&](CUtensorMap* tm, const void* base, int ld, bool f32) {
-    const uint64_t es = f32 ? 4 : 2;
-    const uint64_t dims[3] = {static_cast<uint64_t>(ld), static_cast<uint64_t>(g.L), static_cast<uint64_t>(g.planes_out)};
-    const uint64_t strides[2] = {static_cast<uint64_t>(ld) * es, static_cast<uint64_t>(g.L) * ld * es};
-    const uint32_t box[3] = {32, 32, 1};
-    return f32 ? make_tmap_f32(tm, base, 3, dims, strides, box, 128, err, sizeof(err))
-               : make_tmap(tm, base, 3, dims, strides, box, 64, err, sizeof(err));
-  };
-  // TMA needs 16-byte aligned bases and row pitches
-  auto aligned = [](const void* q, int ld, int es) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0 && (static_cast<int64_t>(ld) * es) % 16 == 0; };
-  if (e.out_act) ok = ok && aligned(e.out_act, e.ldo_act, 2) && enc(&p->tmOutAct, e.out_act, e.ldo_act, false);
-  if (e.out_f32) ok = ok && aligned(e.out_f32, e.ldo_f32, 4) && enc(&p->tmOutF32, e.out_f32, e.ldo_f32, true);
-  if (e.resid) ok = ok && aligned(e.resid, e.ldr, 4) && enc(&p->tmResid, e.resid, e.ldr, true);
-  if (!e.out_act) p->tmOutAct = p->tmA;  // never dereferenced
-  if (!e.out_f32) p->tmOutF32 = p->tmA;
-  if (!e.resid) p->tmResid = p->tmA;
-  p->epi_ok = ok;
-  return ok;
 }
 
 TcGemmPlan* tc_gemm_plan_create(const void* A, const void* W, const GemmShape& g, int planes_in, char* err,
@@ -565,31 +236,9 @@ TcGemmPlan* tc_gemm_plan_create(const void* A, const void* W, const GemmShape& g
 void tc_gemm_plan_destroy(TcGemmPlan* p) { delete p; }
 
 int launch_gemm_tc(const TcGemmPlan* p, const EpiParams& e, cudaStream_t st) {
-  // BT_GEMM_TMA_EPI=0: direct (row-per-lane ld/st.global) epilogue everywhere, for A/B measurements
-  static const bool te_enabled = !(getenv("BT_GEMM_TMA_EPI") && getenv("BT_GEMM_TMA_EPI")[0] == '0');
-  const bool te = te_enabled && p->BN >= 128 && p->BK == 64 && e.kind != 2 && (e.out_act || e.out_f32) &&
-                  (e.kind == 0 || e.C % 32 == 0) && prepare_tma_epilogue(p, e);
-  if (te) {
-    // which specialised epilogue covers this call site (anything else takes the direct epilogue)
-    int em = EM_DIRECT;
-    if (e.kind == 1 && e.out_act && !e.out_f32) em = EM_QKV;
-    else if (e.kind == 0 && e.out_act && !e.out_f32 && !e.resid && e.bias && e.gelu) em = EM_ACT;
-    else if (e.kind == 0 && e.resid && e.out_f32 && !e.gelu) em = EM_RESID;
-    else if (e.kind == 0 && !e.resid && e.out_f32 && !e.out_act && e.bias) em = EM_F32;
-#define BT_TE_CASE(bn) \
-    if (p->BN == bn) { \
-      if (em == EM_QKV) return gemm_tc_launch<bn, 64, EM_QKV>(p, e, st); \
-      if (em == EM_ACT) return gemm_tc_launch<bn, 64, EM_ACT>(p, e, st); \
-      if (em == EM_RESID) return gemm_tc_launch<bn, 64, EM_RESID>(p, e, st); \
-      if (em == EM_F32) return gemm_tc_launch<bn, 64, EM_F32>(p, e, st); \
-    }
-    BT_TE_CASE(256) BT_TE_CASE(192) BT_TE_CASE(128)
-#undef BT_TE_CASE
-  }
-  if (!p->epi_ok) { p->tmOutAct = p->tmA; p->tmOutF32 = p->tmA; p->tmResid = p->tmA; }
 #define BT_TG_CASE(bn, bk) \
-  if (p->BN == bn && p->BK == bk) return gemm_tc_launch<bn, bk, EM_DIRECT>(p, e, st);
-  BT_TG_CASE(256, 64) BT_TG_CASE(192, 64) BT_TG_CASE(128, 64) BT_TG_CASE(96, 64) BT_TG_CASE(64, 64)
+  if (p->BN == bn && p->BK == bk) return gemm_tc_launch<bn, bk>(p, e, st);
+  BT_TG_CASE(192, 64) BT_TG_CASE(128, 64) BT_TG_CASE(96, 64) BT_TG_CASE(64, 64)
   BT_TG_CASE(32, 64) BT_TG_CASE(128, 32) BT_TG_CASE(96, 32) BT_TG_CASE(64, 32) BT_TG_CASE(32, 32)
 #undef BT_TG_CASE
   return -2;

@@ -1,6 +1,6 @@
 // fp32 CUDA-core path (BT_DTYPE_F32): tiled GEMM with the shared epilogues and a
 // flash-style time-direction attention.  This is the exact-numerics path (the reference's
-// float16=False behaviour); the 16-bit tcgen05 path lives in kernels_gemm.cu, kernels_attn.cu, kernels_fused.cu.
+// float16=False behaviour); the 16-bit tensor-core path lives in kernels_gemm.cu, kernels_attn.cu, kernels_fused.cu.
 #include "epilogue.cuh"
 
 namespace bt {

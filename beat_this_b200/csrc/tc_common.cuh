@@ -1,6 +1,6 @@
-// Device helpers shared by the tensor-core kernel files (kernels_gemm.cu, kernels_attn.cu,
-// kernels_fused.cu): predicated single-lane issue forms for converged issuer warps, tcgen05.ld/st
-// shapes, operand descriptors, and the host-side tensor-map encoder.
+// Device helpers shared by the tensor-core kernel files (kernels_gemm.cu, kernels_attn.cu, kernels_fused.cu):
+// warpgroup MMA (wgmma) wrappers and shared-memory matrix descriptors, warp-level mma.sync / ldmatrix, TMA issue
+// forms, small math helpers, and the host-side tensor-map encoder.
 #pragma once
 #include <cuda.h>
 
@@ -8,197 +8,15 @@
 
 namespace bt {
 
-// Predicated forms for a CONVERGED issuer warp: every lane executes the asm block with warp-uniform
-// operands, only the lane with `on != 0` (picked once with elect.sync) performs the operation.
-// Keeping the warp converged lets ptxas keep descriptors in uniform registers instead of wrapping
-// every tcgen05.mma of a divergent `if (lane == 0)` region in a vote loop (measured: ~85 cycles
-// per MMA issue in the divergent form).
-__device__ __forceinline__ void umma_h16_p(uint32_t on, uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                            uint32_t accumulate) {
+__device__ __forceinline__ void tma_load_2d_a(uint32_t smem_dst, const void* tmap, uint32_t bar, int32_t c0, int32_t c1) {
   asm volatile(
-      "{\n\t.reg .pred p, q;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\tsetp.ne.b32 q, %5, 0;\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate), "r"(on)
-      : "memory");
-}
-__device__ __forceinline__ void umma_h16_ts_p(uint32_t on, uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                                               uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p, q;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\tsetp.ne.b32 q, %5, 0;\n\t"
-      "@q tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate), "r"(on)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_p(uint32_t on, uint32_t bar) {
-  asm volatile(
-      "{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %1, 0;\n\t"
-      "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}" ::"r"(bar), "r"(on)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_3d_p(uint32_t on, uint32_t smem_dst, const void* tmap, uint32_t bar, int32_t c0,
-                                              int32_t c1, int32_t c2) {
-  asm volatile(
-      "{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %6, 0;\n\t"
-      "@q cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5}], [%2];\n\t}" ::"r"(smem_dst),
-      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(on)
-      : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx_p(uint32_t on, uint32_t bar, uint32_t bytes) {
-  asm volatile(
-      "{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %2, 0;\n\t"
-      "@q mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n\t}" ::"r"(bar), "r"(bytes), "r"(on)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_p(uint32_t on, uint32_t smem_dst, const void* tmap, uint32_t bar, int32_t c0,
-                                              int32_t c1) {
-  asm volatile(
-      "{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %5, 0;\n\t"
-      "@q cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];\n\t}" ::"r"(smem_dst),
-      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar), "r"(c0), "r"(c1), "r"(on)
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes"
+      " [%0], [%1, {%3, %4}], [%2];" ::"r"(smem_dst),
+      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar), "r"(c0), "r"(c1)
       : "memory");
 }
 
-
-__device__ __forceinline__ float ex2_approx(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-// ---- packed fp32 pairs (sm_100: FADD2 / FMUL2 / FFMA2 take one issue slot for two lanes' worth of work) ----
-__device__ __forceinline__ uint64_t pack_f32x2(float lo, float hi) {
-  uint64_t r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ void unpack_f32x2(uint64_t v, float& lo, float& hi) {
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
-}
-__device__ __forceinline__ uint64_t add_f32x2(uint64_t a, uint64_t b) {
-  uint64_t r;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
-__device__ __forceinline__ uint64_t sub_f32x2(uint64_t a, uint64_t b) {
-  uint64_t r;
-  asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
-__device__ __forceinline__ uint64_t fma_f32x2(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-  return r;
-}
-__device__ __forceinline__ uint64_t mul_f32x2(uint64_t a, uint64_t b) {
-  uint64_t r;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
-// tanh-form GELU (epilogue.cuh gelu_tanh_fast) for two values: 5 packed FMA-pipe instructions + 2 MUFU.TANH
-__device__ __forceinline__ uint64_t gelu_tanh_f32x2(uint64_t x) {
-  const uint64_t w = fma_f32x2(mul_f32x2(x, x), pack_f32x2(0.0356774081f, 0.0356774081f), pack_f32x2(0.7978845608f, 0.7978845608f));
-  float u0, u1, t0, t1;
-  unpack_f32x2(mul_f32x2(x, w), u0, u1);
-  asm("tanh.approx.f32 %0, %1;" : "=f"(t0) : "f"(u0));
-  asm("tanh.approx.f32 %0, %1;" : "=f"(t1) : "f"(u1));
-  const uint64_t hx = mul_f32x2(x, pack_f32x2(0.5f, 0.5f));
-  return fma_f32x2(hx, pack_f32x2(t0, t1), hx);
-}
-__device__ __forceinline__ float max3f(float a, float b, float c) {  // FMNMX3
-  float r;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c));
-  return r;
-}
-// 2^x for a pair of scores on the FMA / ALU pipes: Cody-Waite split (n = round(x) through the 1.5 * 2^23 trick,
-// r = x - n in [-0.5, 0.5]) + degree-3 minimax polynomial (relative error 8e-5, a fifth of an fp16 ulp of the
-// probability it produces) + exponent insertion by an integer shift-add.  Inputs below -120 (masked keys are -inf)
-// are clamped; the result underflows to 0 in the 16-bit pack either way.
-__device__ __forceinline__ uint64_t ex2_poly_f32x2(uint64_t x2) {
-  float x0, x1;
-  unpack_f32x2(x2, x0, x1);
-  const uint64_t x = pack_f32x2(fmaxf(x0, -120.0f), fmaxf(x1, -120.0f));
-  const uint64_t magic = pack_f32x2(12582912.0f, 12582912.0f);
-  const uint64_t t = add_f32x2(x, magic);
-  const uint64_t r = sub_f32x2(x, sub_f32x2(t, magic));
-  uint64_t p = fma_f32x2(pack_f32x2(0.05508868f, 0.05508868f), r, pack_f32x2(0.24260405f, 0.24260405f));
-  p = fma_f32x2(p, r, pack_f32x2(0.69327623f, 0.69327623f));
-  p = fma_f32x2(p, r, pack_f32x2(0.99992895f, 0.99992895f));
-  float t0, t1, p0, p1;
-  unpack_f32x2(t, t0, t1);
-  unpack_f32x2(p, p0, p1);
-  int y0, y1;  // p * 2^n: n sits in the low mantissa bits of t
-  asm("mad.lo.s32 %0, %1, 8388608, %2;" : "=r"(y0) : "r"(__float_as_int(t0)), "r"(__float_as_int(p0)));
-  asm("mad.lo.s32 %0, %1, 8388608, %2;" : "=r"(y1) : "r"(__float_as_int(t1)), "r"(__float_as_int(p1)));
-  return pack_f32x2(__int_as_float(y0), __int_as_float(y1));
-}
-__device__ __forceinline__ uint32_t tmem_ld_32x32b_x1(uint32_t taddr) {
-  uint32_t r;
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x1.b32 {%0}, [%1];" : "=r"(r) : "r"(taddr) : "memory");
-  return r;
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x32b_x1(uint32_t taddr, uint32_t r) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x1.b32 [%0], {%1};" ::"r"(taddr), "r"(r) : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x32b_x16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-        "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x8(uint32_t taddr, uint32_t (&r)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x32b_x8(uint32_t taddr, const uint32_t (&r)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr), "r"(r[0]),
-               "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-template <int N> __device__ __forceinline__ void tmem_ld_n(uint32_t taddr, uint32_t (&r)[N]);
-template <> __device__ __forceinline__ void tmem_ld_n<8>(uint32_t taddr, uint32_t (&r)[8]) { tmem_ld_32x32b_x8(taddr, r); }
-template <> __device__ __forceinline__ void tmem_ld_n<16>(uint32_t taddr, uint32_t (&r)[16]) { tmem_ld_32x32b_x16(taddr, r); }
-template <int N> __device__ __forceinline__ void tmem_st_n(uint32_t taddr, const uint32_t (&r)[N]);
-template <> __device__ __forceinline__ void tmem_st_n<8>(uint32_t taddr, const uint32_t (&r)[8]) { tmem_st_32x32b_x8(taddr, r); }
-template <> __device__ __forceinline__ void tmem_st_n<16>(uint32_t taddr, const uint32_t (&r)[16]) { tmem_st_32x32b_x16(taddr, r); }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-// D[tmem] (+)= A[tmem] * B[smem]: A is read from tensor memory (lane = row, one 32-bit column
-// per two K elements), kind::f16 with h16 operands.
-__device__ __forceinline__ void umma_h16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
-// B operand in MN-major form (N contiguous): rows of 64 B (32 h16), SWIZZLE_64B, 8-row groups
-// 512 B apart (SBO); a second 32-column block of N lives `lbo_bytes` after the first (LBO).
-__device__ __forceinline__ uint64_t make_mnmajor_desc_sw64(uint32_t smem_addr, uint32_t lbo_bytes) {
-  return static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4) | (static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16) |
-         (static_cast<uint64_t>(512 >> 4) << 32) | (1ull << 46) | (4ull << 61);
-}
-
-// ---- TMA stores (shared -> global, bulk async groups of the issuing thread) and address-form loads ----
+// ---- TMA stores (shared -> global, bulk async groups of the issuing thread) ----
 __device__ __forceinline__ void tma_store_3d(const void* tmap, uint32_t smem_src, int32_t c0, int32_t c1, int32_t c2) {
   asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(
                    reinterpret_cast<uint64_t>(tmap)),
@@ -211,18 +29,101 @@ __device__ __forceinline__ void bulk_wait_read() {  // at most N of this thread'
   asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
 }
 
-__device__ __forceinline__ void tma_store_2d(const void* tmap, uint32_t smem_src, int32_t c0, int32_t c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
-                   reinterpret_cast<uint64_t>(tmap)),
-               "r"(smem_src), "r"(c0), "r"(c1)
+__device__ __forceinline__ float ex2_approx(float x) {
+  float y;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+  return y;
+}
+// 2^x on the FMA / ALU pipes: Cody-Waite split (n = round(x) through the 1.5 * 2^23 trick, r = x - n in
+// [-0.5, 0.5]) + degree-3 minimax polynomial (relative error 8e-5, a fifth of an fp16 ulp of the probability it
+// produces) + exponent insertion by an integer shift-add.  Inputs below -120 (masked keys are -inf) are clamped;
+// the result underflows to 0 in the 16-bit pack either way.
+__device__ __forceinline__ float ex2_poly(float x) {
+  x = fmaxf(x, -120.0f);
+  const float magic = 12582912.0f;
+  const float t = x + magic;
+  const float r = x - (t - magic);
+  float p = fmaf(0.05508868f, r, 0.24260405f);
+  p = fmaf(p, r, 0.69327623f);
+  p = fmaf(p, r, 0.99992895f);
+  int y;  // p * 2^n: n sits in the low mantissa bits of t
+  asm("mad.lo.s32 %0, %1, 8388608, %2;" : "=r"(y) : "r"(__float_as_int(t)), "r"(__float_as_int(p)));
+  return __int_as_float(y);
+}
+
+// ---------------------------------------------------------------------------------------------- wgmma (sm_90a)
+// Shared-memory matrix descriptor of a K-major operand in the swizzled canonical layout that TMA writes with
+// CU_TENSOR_MAP_SWIZZLE_{128,64}B (rows of SW bytes, 8-row groups SW * 8 bytes apart):
+//   bits [0,14) start >> 4 | [16,30) LBO >> 4 (unused for swizzled K-major, 1) | [32,46) SBO >> 4 |
+//   [62,64) layout (1 = 128B swizzle, 2 = 64B swizzle)
+// Advancing K by 16 elements inside a swizzled row is a +32 byte offset of the start address.
+template <int SW>
+__device__ __forceinline__ uint64_t make_wgmma_desc(uint32_t smem_addr) {
+  static_assert(SW == 128 || SW == 64, "swizzle");
+  constexpr uint64_t layout = SW == 128 ? 1 : 2;
+  constexpr uint64_t sbo = (8 * SW) >> 4;
+  return static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4) | (1ull << 16) | (sbo << 32) | (layout << 62);
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// D[64 x 64] (+)= A[64 x 16] * B[64 x 16]^T, both operands K-major in shared memory, fp32 accumulators in
+// registers: thread (warp w, lane l) of the warpgroup holds rows 16w + l/4 (d[4j], d[4j+1]) and 16w + l/4 + 8
+// (d[4j+2], d[4j+3]) of columns 8j + 2(l%4) + {0, 1}.
+__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32." BT_H16_MMA_SYNC " "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "%32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate)
+      : "memory");
+}
+// the same for 32 output columns (tiles whose width is not a multiple of 64)
+__device__ __forceinline__ void wgmma_m64n32k16(float (&d)[16], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32." BT_H16_MMA_SYNC " "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+      "%16, %17, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate)
+      : "memory");
+}
+template <int NC>
+__device__ __forceinline__ void wgmma_n(float (&d)[NC / 2], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+  if constexpr (NC == 64) wgmma_m64n64k16(d, a_desc, b_desc, accumulate);
+  else wgmma_m64n32k16(d, a_desc, b_desc, accumulate);
+}
+
+// ------------------------------------------------- warp-level MMA (attention, fused frontend kernels)
+// D[16 x 8] += A[16 x 16] * B[16 x 8], 16-bit operands, fp32 accumulate
+__device__ __forceinline__ void mma_16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32." BT_H16_MMA_SYNC ".f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+               "{%0, %1, %2, %3};"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+__device__ __forceinline__ void ldmatrix_x4(uint32_t addr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(addr)
                : "memory");
 }
-__device__ __forceinline__ void tma_load_2d_a(uint32_t smem_dst, const void* tmap, uint32_t bar, int32_t c0, int32_t c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];" ::"r"(smem_dst),
-      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar), "r"(c0), "r"(c1)
-      : "memory");
+__device__ __forceinline__ void ldmatrix_x4_trans(uint32_t addr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(addr)
+               : "memory");
 }
 
 // --------------------------------------------------------------------------- host side (kernels_gemm.cu)
@@ -231,9 +132,6 @@ extern int g_num_sms;
 // dims 1.., box per dim, swizzle 0 / 32 / 64 / 128 bytes
 bool make_tmap(CUtensorMap* tm, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                const uint32_t* box, int swizzle_bytes, char* err, int errlen);
-// fp32 tensor map (residual stream tiles moved by TMA in the GEMM epilogues)
-bool make_tmap_f32(CUtensorMap* tm, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                   const uint32_t* box, int swizzle_bytes, char* err, int errlen);
 int tc_init_attn(char* err, int errlen);
 int tc_init_fused(char* err, int errlen);
 

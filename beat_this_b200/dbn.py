@@ -5,7 +5,7 @@ transition_lambda=100; madmom defaults observation_lambda=16, threshold=0.05, co
 madmom is a third-party package that is not installable offline, so this is a RESTATEMENT of its published
 algorithm (F. Krebs, S. Boeck, G. Widmer, "An Efficient State-Space Model for Joint Tempo and Meter Tracking",
 ISMIR 2015; S. Boeck et al., "Joint Beat and Downbeat Tracking with Recurrent Neural Networks", ISMIR 2016):
-parity with madmom is UNPINNED (SURVEY.md section 8(c)); tests check the Viterbi decoder against a brute-force
+parity with madmom is UNPINNED (madmom is not installable offline); tests check the Viterbi decoder against a brute-force
 dense decoder and the tracker on synthetic activations.
 
 State space: for every beat of the bar and every tempo (beat interval of i frames, i = round(60 fps / max_bpm) ..

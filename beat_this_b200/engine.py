@@ -16,7 +16,7 @@ def _cuda_device(device) -> torch.device:
     dev = torch.device(device)
     if dev.type != "cuda":
         raise RuntimeError(
-            f"beat_this_b200 runs on an sm_100a CUDA device only (got device={device!r}); "
+            f"beat_this_b200 runs on an sm_90a (H100) CUDA device only (got device={device!r}); "
             "there is no CPU fallback"
         )
     if dev.index is None:
@@ -45,7 +45,7 @@ class Engine:
     def __init__(self, packed: dict | None, hparams: dict | None, device="cuda", half: bool = False, wave_chunks: int | None = None):
         self.lib = _lib.load()
         self.device = _cuda_device(device)
-        self.half = bool(half)  # 16-bit tcgen05 path (fp16 operands; see bt_act_dtype) instead of fp32 CUDA cores
+        self.half = bool(half)  # 16-bit tensor-core path (fp16 operands; see bt_act_dtype) instead of fp32 CUDA cores
         self.act_dtype = self.lib.bt_act_dtype().decode() if half else "f32"
         hp = hparams or {}
         self.hparams = dict(hp)

@@ -1,11 +1,11 @@
 """Drop-in mirror of the reference ``beat_this.inference`` API (reference beat_this/inference.py:16-315): same
 function and class names, constructor and call signatures, return types and exceptions -- with everything between
-"audio samples" and "beat timestamps" executed by the sm_100a CUDA library.
+"audio samples" and "beat timestamps" executed by the sm_90a CUDA library.
 
 Differences a user can observe:
 * ``device`` must be a CUDA device (default ``"cuda"``); ``device="cpu"`` raises.
 * ``float16=False`` -> fp32 CUDA-core kernels (reference-exact numerics, <=1e-3 on logits);
-  ``float16=True`` -> fp16-operand tcgen05 tensor-core kernels with fp32 accumulation and an fp32 residual stream
+  ``float16=True`` -> fp16-operand tensor-core kernels with fp32 accumulation and an fp32 residual stream
   (the reference autocasts to fp16 here as well, inference.py:245-246).
 * every class has a ``batch(...)`` method that processes many clips per call through the host/device pipeline of
   ``beat_this_b200.pipeline`` (the reference is strictly one clip, one chunk at a time: inference.py:215).

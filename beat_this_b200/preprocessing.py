@@ -1,7 +1,7 @@
 """Audio loading and the log-mel frontend (mirror of reference beat_this/preprocessing.py).
 
 ``LogMelSpect`` keeps the reference's constructor defaults and call signature
-(preprocessing.py:27-59) but runs the fused sm_100a kernel (frame -> Hann -> 1024-point FFT
+(preprocessing.py:27-59) but runs the fused sm_90a kernel (frame -> Hann -> 1024-point FFT
 -> |.| -> 128-band slaney mel -> log1p(1000 x)) through ``bt_logmel``.
 ``load_audio`` (preprocessing.py:6-24) walks the reference's decoder chain (torchaudio, soundfile, madmom -- whichever
 is installed) and then two dependency-free WAV readers; the batched File2Beats path reads WAV files natively
@@ -223,7 +223,7 @@ class LogMelSpect(torch.nn.Module):
         super().__init__()
         given = (sample_rate, n_fft, hop_length, f_min, f_max, n_mels, mel_scale, normalized, power, log_multiplier)
         if given != (22050, 1024, 441, 30, 11000, 128, "slaney", "frame_length", 1, 1000):
-            raise NotImplementedError("the sm_100a log-mel kernel implements the reference defaults only")
+            raise NotImplementedError("the log-mel kernel implements the reference defaults only")
         from .engine import Engine
 
         self.engine = _engine if _engine is not None else Engine.mel_only(device)

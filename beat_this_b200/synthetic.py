@@ -3,7 +3,7 @@
 There is no network in the build/bench environment, so the published checkpoints
 ("final0", "small0", reference beat_this/inference.py:13,38-48) cannot be fetched.
 This module writes checkpoints in the *exact* ``.ckpt`` layout the reference loads
-(reference inference.py:56-87, key list in SURVEY.md App. B): a ``torch.save``d dict
+(reference inference.py:56-87): a ``torch.save``d dict
 with ``state_dict`` (keys prefixed ``model.``) and ``hyper_parameters``.
 
 Conv2d weights follow the reference initialiser (beat_tracker.py:170-186, kaiming-normal
@@ -151,7 +151,7 @@ def write_checkpoint(path: str, name: str = "final0", seed: int = 0) -> str:
 
 def synth_clip(index: int, seconds: float = 30.0, sr: int = SAMPLE_RATE) -> np.ndarray:
     """Seeded synthetic mono clip: low noise plus decaying click/sine bursts on a per-clip
-    tempo grid (60-180 BPM) so that the activations are not degenerate (SURVEY.md 8d)."""
+    tempo grid (60-180 BPM) so that the activations are not degenerate."""
     rng = np.random.default_rng(1000 + index)
     n = int(round(seconds * sr))
     x = 0.004 * rng.standard_normal(n)

@@ -1,9 +1,9 @@
 """Checkpoint tensors -> packed parameters of libbeatthis_sm100.so.
 
-Input is the reference's state_dict layout (SURVEY.md App. B; reference
+Input is the reference's state_dict layout (reference
 beat_this/inference.py:56-87 strips the ``model.`` prefix).  Output is a dict
 ``name -> contiguous float32 numpy array`` uploaded with ``bt_set_param``.  Folds done here
-(all exact re-associations of the reference math, SURVEY.md App. A.3):
+(all exact re-associations of the reference math):
 
 * eval-mode BatchNorm2d after a bias-free conv (beat_tracker.py:115-123,155-165) -> conv
   weight scale + bias.  BatchNorm1d of the stem (``:113``) is kept as an explicit

@@ -1,10 +1,11 @@
 #!/usr/bin/env python
-"""bench.py -- clips/sec for 30 s audio -> beats (final0-shaped checkpoint) on N B200 GPUs.
+"""bench.py -- clips/sec for 30 s audio -> beats (final0-shaped checkpoint) on N H100 GPUs.
 
     python bench.py --gpus 1 --steps K --warmup W            # our CUDA path, BASELINE config 2 (default)
-    python bench.py --impl reference --gpus 1 --steps K ...  # the UNMODIFIED reference (baseline/_ref) on host cores
+    python bench.py --impl reference --gpus 1 --steps K ...  # the UNMODIFIED reference (oracle/_ref) on host cores
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
     python bench.py --config 3|4|5 ...                       # the other BASELINE configs (files / --dbn / ragged)
+    python bench.py ... --dump-outputs DIR                   # also write the last timed step's results as DIR/*.npy
 
 One "step" = one pass of the hot path over one batch of `--batch` synthetic 30 s clips per GPU (BASELINE config 2:
 Audio2Frames final0, batch 64; the minimal peak picker is included so that the step is audio -> beats).  Prints ONE
@@ -14,10 +15,10 @@ value    : device-resident throughput (audio already in HBM; CUDA events; max ov
 e2e      : the reference-signature call -- Audio2Beats.batch(list of float64 numpy arrays as load_audio returns
            them) -- for steps*batch clips: threaded mono-mix/cast into pinned memory, H2D copy, all kernels, D2H of
            the timestamp arrays, every step, staging of step i+1 overlapping the kernels of step i.
-roofline : the dominant kernel (time-direction flash attention, tcgen05) -- algorithmic FLOPs / CUDA-event time,
+roofline : the dominant kernel (time-direction flash attention, mma.sync) -- algorithmic FLOPs / CUDA-event time,
            measured live in a second timed pass with one event per launch (bt_profile_*).
 parity   : the GPU results of the timed path checked against the CPU run of the cpu_baseline leg on the same clips.
-cpu_baseline: the unmodified reference (kind "reference") -- or the oracle port when baseline/_ref is absent --
+cpu_baseline: the unmodified reference (kind "reference") -- or the oracle port when oracle/_ref is absent --
            timed on this box's host cores.
 """
 from __future__ import annotations
@@ -51,7 +52,7 @@ import torch
 SR = 22050
 METRIC = "clips/sec (30 s audio->beats, final0)"
 CACHE = os.environ.get("BT_TEST_CACHE", "/tmp/beat_this_b200_cache")
-REF_DIR = os.path.join(ROOT, "baseline", "_ref")
+REF_DIR = os.path.join(ROOT, "oracle", "_ref")
 
 
 def load_peaks():
@@ -60,7 +61,8 @@ def load_peaks():
         with open(p) as f:
             d = json.load(f)
         return d, "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+    # NVIDIA H100 SXM data sheet (700 W): HBM3 bandwidth, dense BF16 / FP16 tensor rate.  Not measured.
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "data-sheet"
 
 
 class ClockSampler:
@@ -133,9 +135,9 @@ def synth_clips(n_clips: int, seconds: float, seed0: int):
 
 # ================================================================================== reference arm
 def import_reference():
-    """(beat_this.inference module of the UNMODIFIED reference, kind).  baseline/_ref = `pip install --no-deps
-    --target baseline/_ref /root/reference`; the two third-party packages it imports that are not installable
-    offline (rotary_embedding_torch, soxr) come from oracle/shims.  None when baseline/_ref is absent."""
+    """(beat_this.inference module of the UNMODIFIED reference, kind).  oracle/_ref = `pip install --no-deps
+    --target oracle/_ref <beat_this source tree>` (oracle/install_reference.py, run by build()); the two third-party packages it imports that are not installable
+    offline (rotary_embedding_torch, soxr) come from oracle/shims.  None when oracle/_ref is absent."""
     if not os.path.isdir(os.path.join(REF_DIR, "beat_this")):
         return None
     for p in (os.path.join(ROOT, "oracle", "shims"), REF_DIR):
@@ -154,7 +156,7 @@ def import_reference():
 
 class CpuArm:
     """The reference's CPU path: Audio2Beats(ckpt, "cpu", float16=False)(signal, sr) per clip, chunk by chunk, as
-    it really runs (inference.py:215) -- through baseline/_ref when present, else the oracle port."""
+    it really runs (inference.py:215) -- through oracle/_ref when present, else the oracle port."""
 
     def __init__(self, seconds: float):
         from beat_this_b200 import synthetic
@@ -164,7 +166,7 @@ class CpuArm:
         if self.ref is not None:
             self.kind = "reference"
             self.a2b = self.ref.Audio2Beats(self.ckpt, "cpu", False, False)
-            self.what = "UNMODIFIED reference beat_this.inference.Audio2Beats (baseline/_ref, fp32, torch CPU)"
+            self.what = "UNMODIFIED reference beat_this.inference.Audio2Beats (oracle/_ref, fp32, torch CPU)"
         else:
             from oracle import beat_this_oracle as O
 
@@ -192,8 +194,8 @@ class CpuArm:
         from beat_this_b200 import synthetic
 
         n = host_cores()
-        # more than ~32 threads only slows torch's CPU kernels down on these shapes (measured on the 128-CPU bench
-        # box: 64 threads 1.6-1.9 s per clip, 128 threads 22 s, 16 threads 0.33-0.47 s), so the sweep stops at 32
+        # more than ~32 threads only slows torch's CPU kernels down on these shapes (on a 128-CPU host: 64 threads
+        # 1.6-1.9 s per clip, 128 threads 22 s, 16 threads 0.33-0.47 s), so the sweep stops at 32
         cands = sorted({c for c in (min(n, 32), 24, 16, 12, 8) if 1 <= c <= n}, reverse=True)
         x = synthetic.synth_clip(999, self.seconds)
         best, best_t, table = cands[-1], float("inf"), {}
@@ -301,7 +303,7 @@ def cpu_baseline_and_parity(args, gpu_run, budget_s: float = 25.0):
 
 
 def gpu_reference_arm(args, dev, n_clips=8):
-    """The unmodified reference on the SAME GPU (eager PyTorch, float16=True autocast): the 'existing Blackwell path'."""
+    """The unmodified reference on the SAME GPU (eager PyTorch, float16=True autocast): the existing GPU path."""
     ref = import_reference()
     if ref is None:
         return None
@@ -325,6 +327,37 @@ def gpu_reference_arm(args, dev, n_clips=8):
 
 
 # ================================================================================== our arm
+DUMP_CAP_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir: str, beat, down, times) -> None:
+    """The arrays a caller of the timed path receives, for output-for-output comparison of two builds (the inputs are
+    seeded): frame logits of all clips concatenated (float32), beat / downbeat times of all clips concatenated
+    (float64) with the number of each per clip (float64).  When the whole set would exceed 64 MB, the logits are
+    replaced by a fixed sample of frames (seed 0, sorted indices, the same for both arrays) stored with its indices."""
+    os.makedirs(out_dir, exist_ok=True)
+    beat_np, down_np = beat.float().cpu().numpy(), down.float().cpu().numpy()
+    times_bytes = 8 * sum(len(b) + len(d) + 2 for b, d in times)
+    sample = None
+    if 2 * beat_np.nbytes + times_bytes > DUMP_CAP_BYTES:
+        n_keep = max(1, (DUMP_CAP_BYTES - times_bytes) // 16)  # two float32 logits + one float64 index per frame
+        sample = np.sort(np.random.default_rng(0).choice(beat_np.size, size=min(n_keep, beat_np.size), replace=False))
+        beat_np, down_np = beat_np[sample], down_np[sample]
+    arrays = {
+        "beat_logits": beat_np,
+        "downbeat_logits": down_np,
+        "beat_times": np.concatenate([b for b, _ in times]).astype(np.float64),
+        "downbeat_times": np.concatenate([d for _, d in times]).astype(np.float64),
+        "beat_counts": np.array([len(b) for b, _ in times], dtype=np.float64),
+        "downbeat_counts": np.array([len(d) for _, d in times], dtype=np.float64),
+    }
+    if sample is not None:
+        arrays["logit_frame_indices"] = sample.astype(np.float64)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+    print(f"dumped {', '.join(arrays)} to {out_dir} ({sum(a.nbytes for a in arrays.values()) / 1e6:.1f} MB)", file=sys.stderr)
+
+
 def make_model(args, dev, rank):
     from beat_this_b200 import synthetic
     from beat_this_b200.distributed import load_model_distributed
@@ -380,9 +413,11 @@ def run_ours(args, rank, world, local):
             dist.barrier()
         torch.cuda.synchronize(dev)
 
+    last = [None]  # what the most recent step computed: (beat logits, downbeat logits, per-clip timestamps)
+
     def step_device():
         beat, down, f = eng.audio2frames_cat(audio_dev, so)
-        return eng.peakpick_cat(beat, down, f)
+        last[0] = (beat, down, eng.peakpick_cat(beat, down, f))
 
     def timed_device_steps():
         barrier()
@@ -403,6 +438,8 @@ def run_ours(args, rank, world, local):
     ms = timed_device_steps()
     launches = eng.launches - l0
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, *last[0])
     # ---- second timed pass with one CUDA event per launch: per-kernel times for the roofline ---------------
     eng.profile_reset()
     eng.profile_enable(True)
@@ -444,7 +481,7 @@ def run_ours(args, rank, world, local):
     attn_flops = 4.0 * Lc * Lc * 32 * headseqs_per_chunk * n_chunks * args.steps
     key = "attn_time_tc" if half else "attn_time_simt"
     a_ms, a_n = prof.get(key, (0.0, 0))
-    peak_tf = float(peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops", 1400.0)))
+    peak_tf = float(peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops", 989.0)))
     traffic, traffic_src = None, None
     tpath = os.path.join(ROOT, "profiles", "attn_traffic.json")
     if half and os.path.exists(tpath) and args.batch == 64 and args.seconds == 30.0:
@@ -452,7 +489,7 @@ def run_ours(args, rank, world, local):
             tj = json.load(f)
         traffic, traffic_src = tj.get("dram_bytes_per_launch_mean"), tj.get("source")
     roof = {"bound": "tensor", "kernel": key, "achieved": (attn_flops / (a_ms / 1000.0) / 1e12) if a_ms > 0 else None,
-            "peak": peak_tf, "peak_source": f"{peak_src} bf16_tflops_sustained (fp16 and bf16 tcgen05 run at the same rate; kernel timed inside a long step)",
+            "peak": peak_tf, "peak_source": f"{peak_src} bf16_tflops (fp16 and bf16 run at the same tensor-core rate; kernel timed inside a long step)",
             "unit": "TFLOP/s", "traffic": traffic, "traffic_source": traffic_src, "launches": a_n, "avg_launch_ms": (a_ms / a_n) if a_n else None,
             "algorithmic_flops_per_launch": attn_flops / a_n if a_n else None,
             "timed_in": f"second timed pass of {args.steps} steps with one CUDA event per launch ({ms_prof / args.steps:.2f} ms/step vs {ms / args.steps:.2f} without)"}
@@ -468,7 +505,7 @@ def run_ours(args, rank, world, local):
                                f"@22.05 kHz mono per GPU ({n_chunks} chunks of {Lc} frames, {args.batch} distinct clips), log-mel + BeatThis forward + minimal peak picking",
                    "batch_per_gpu": args.batch, "global_batch": total_clips, "parallelism": f"dp{world} (clips sharded, weights broadcast once over NCCL)",
                    "wave_chunks": args.wave, "l2_policy": f"inputs larger than L2: {so[-1] * 4 / 1e6:.0f} MB audio per step per GPU; activations stream through HBM",
-                   "operands": f"{act} tcgen05 operands, fp32 accumulate, fp32 residual stream" if half else "fp32 CUDA cores"},
+                   "operands": f"{act} tensor-core operands, fp32 accumulate, fp32 residual stream" if half else "fp32 CUDA cores"},
         "roofline": roof, "kernel_time_shares": shares,
         "e2e": {"value": e2e_value, "unit": "clips/s", "h2d_bytes_per_step": int(h2d), "d2h_bytes_per_step": int(d2h),
                 "ms_per_step": e2e_ms / args.steps,
@@ -620,11 +657,17 @@ def main():
     ap.add_argument("--batch", type=int, default=64, help="clips per GPU per step")
     ap.add_argument("--seconds", type=float, default=30.0)
     ap.add_argument("--wave", type=int, default=128, help="chunks per wave (one wave = one launch of every kernel)")
-    ap.add_argument("--float32", action="store_true", help="fp32 CUDA-core path instead of the 16-bit tcgen05 path")
+    ap.add_argument("--float32", action="store_true", help="fp32 CUDA-core path instead of the 16-bit tensor-core path")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-gpu-reference", action="store_true")
     ap.add_argument("--ref-clips-per-step", type=int, default=2)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="config 2: write what the last timed step computed (frame logits, beat / downbeat times) as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
+    if args.dump_outputs and (args.impl != "ours" or args.config != 2):
+        ap.error("--dump-outputs applies to the default workload (--impl ours --config 2)")
     from beat_this_b200.distributed import init_from_env
 
     if args.impl == "reference":

@@ -1,5 +1,5 @@
 /*
- * beatthis.h -- C ABI of libbeatthis_sm100.so, the B200 (sm_100a) implementation of the
+ * beatthis.h -- C ABI of libbeatthis_sm90.so, the H100 (sm_90a) implementation of the
  * CPJKU/beat_this Audio -> Frames -> Beats inference path.
  *
  * The reference has no FFI: its boundary is the Python API of beat_this/inference.py
@@ -38,7 +38,7 @@ extern "C" {
 #define BT_ERR_FORMAT (-6) /* not a RIFF/WAVE file this library decodes (caller falls back to another decoder) */
 
 #define BT_DTYPE_F32 0  /* fp32 CUDA-core kernels: the reference's float16=False numerics   */
-#define BT_DTYPE_H16 1 /* 16-bit tcgen05 tensor-core kernels, fp32 accumulate + fp32 residual stream.  Operand type
+#define BT_DTYPE_H16 1 /* 16-bit tensor-core kernels (wgmma GEMMs, mma.sync attention), fp32 accumulate + fp32 residual stream.  Operand type
                         * fp16 (what the reference's float16=True autocasts to on CUDA, inference.py:245-246);
                         * bt_act_dtype() names it ("f16", or "bf16" for a -DBT_ACT_BF16 build) */
 

@@ -4,14 +4,14 @@ TEST INFRASTRUCTURE ONLY.  Nothing in the product package (beat_this_b200/) impo
 file; it is used by tests/, __graft_entry__.smoke() and the cpu_baseline / reference legs
 of bench.py as the *checker* and the timed CPU baseline.
 
-Every function cites the reference file:line (relative to /root/reference) it restates.
+Every function cites the reference file:line (relative to the reference's source tree) it restates.
 Floating point (fp32 by default, like the reference's CPU path); plain torch CPU ops.
 
 Pinning: oracle/make_golden.py imports the UNMODIFIED reference (through the import shims
 in oracle/shims/) and checks this restatement against it on seeded inputs and synthetic
 checkpoints, then writes tests/golden/*.npz from the reference's own outputs.  The
 reference's own tests hold no golden vectors (tests/test_inference.py asserts types only).
-Third-party arithmetic not under /root/reference and not installed here stays
+Third-party arithmetic not in the reference's source tree and not installed here stays
 "parity unpinned": rotary_embedding_torch 0.6.4 (RoPE; restated from its published
 semantics, see oracle/shims/rotary_embedding_torch.py), soxr 0.3.7 (resampler; not
 exercised: all inputs are 22.05 kHz), madmom (DBN; host, optional).
@@ -134,7 +134,7 @@ def aggregate(pred_chunks, starts, T, chunk=CHUNK, border=BORDER):
 
 
 # --------------------------------------------------------------------------------------
-# model  (beat_this/model/beat_tracker.py, roformer.py; math in SURVEY.md App. A.3)
+# model  (beat_this/model/beat_tracker.py, roformer.py)
 # --------------------------------------------------------------------------------------
 
 

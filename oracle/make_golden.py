@@ -1,8 +1,9 @@
-"""Generate tests/golden/*.npz by running the UNMODIFIED reference (/root/reference).
+"""Generate tests/golden/*.npz by running the UNMODIFIED reference (a beat_this source tree).
 
-Run HERE (the build container; /root/reference does not exist on the GPU box):
+    BEAT_THIS_REFERENCE=<beat_this source tree> python oracle/make_golden.py [live]
 
-    python oracle/make_golden.py
+(`live`: only tests/golden/live_reference.npz, the reference model's forward on a random batch and its chunk
+planner.)
 
 It (1) imports the reference through the two import shims in oracle/shims/ (packages absent
 offline: rotary_embedding_torch, soxr), (2) checks the oracle restatement
@@ -21,7 +22,9 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 sys.path.insert(0, os.path.join(HERE, "shims"))
-sys.path.insert(0, "/root/reference")
+if not os.environ.get("BEAT_THIS_REFERENCE"):
+    sys.exit("usage: BEAT_THIS_REFERENCE=<beat_this source tree> python oracle/make_golden.py [live]")
+sys.path.insert(0, os.environ["BEAT_THIS_REFERENCE"])
 sys.path.insert(0, ROOT)
 
 import numpy as np
@@ -247,5 +250,25 @@ def main():
             f.write(line + "\n")
 
 
+def write_live_reference(tmpdir="/tmp/bt_golden"):
+    """The reference model (small0) on a seeded random [2, 100, 128] batch, and its chunk starts for a few lengths:
+    what tests/test_cpu_oracle.py::test_oracle_against_reference_forward compares the oracle with."""
+    _, model, sd = ref_model_from("small0", 0, tmpdir)
+    torch.manual_seed(4)
+    x = torch.rand(2, 100, 128) * 7
+    with torch.inference_mode():
+        ref = model(x)
+    gold = {"small0_ckpt_sum": np.float64(synthetic.tensor_checksum(sd)), "beat": ref["beat"].numpy(),
+            "downbeat": ref["downbeat"].numpy(), "Ts": np.array([1, 1488, 1489, 3001], dtype=np.int64)}
+    for T in gold["Ts"]:
+        _, starts = ref_inf.split_piece(torch.zeros(int(T), 1), 1500, 6, True)
+        gold[f"starts_{T}"] = np.asarray(starts, dtype=np.int64)
+    np.savez_compressed(os.path.join(GOLD, "live_reference.npz"), **gold)
+
+
 if __name__ == "__main__":
-    main()
+    if sys.argv[1:] == ["live"]:
+        write_live_reference()
+    else:
+        main()
+        write_live_reference()

@@ -1,6 +1,6 @@
 """Generate tests/golden/cli_beats.npz: the `.beats` files the UNMODIFIED reference writes for int16 WAV material.
 
-Run HERE (the build container; /root/reference does not exist on the GPU box):
+Needs the reference's source tree, given by BEAT_THIS_REFERENCE:
 
     python oracle/make_golden_cli.py
 
@@ -22,7 +22,9 @@ import tempfile
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 sys.path.insert(0, os.path.join(HERE, "shims"))
-sys.path.insert(0, "/root/reference")
+if not os.environ.get("BEAT_THIS_REFERENCE"):
+    sys.exit("usage: BEAT_THIS_REFERENCE=<beat_this source tree> python oracle/make_golden_cli.py")
+sys.path.insert(0, os.environ["BEAT_THIS_REFERENCE"])
 sys.path.insert(0, ROOT)
 
 import numpy as np

@@ -1,4 +1,4 @@
-"""Import shim so the UNMODIFIED reference (/root/reference) can be imported in this
+"""Import shim so the UNMODIFIED reference can be imported in this
 container, where `rotary_embedding_torch` (pinned 0.6.4 in the reference's
 requirements.txt:6) is not installed and there is no network.
 
@@ -13,7 +13,7 @@ constructor the reference uses (`RotaryEmbedding(head_dim)`, beat_tracker.py:52)
            interleaved pairs;  pos = arange(seq_len) along dim -2; fp32 math.
 
 PARITY UNPINNED for this third-party piece: the package itself is absent, so the
-restatement cannot be executed against it here (SURVEY.md section 8c).
+restatement cannot be executed against it here.
 """
 import torch
 from torch import nn

@@ -16,7 +16,7 @@ def pytest_configure(config):
     import torch
 
     torch.set_num_threads(min(16, os.cpu_count() or 1))
-    config.addinivalue_line("markers", "gpu: needs a CUDA (sm_100a) device; run with -m gpu on the B200 box")
+    config.addinivalue_line("markers", "gpu: needs a CUDA (sm_90a, H100) device; run with -m gpu")
 
 
 def ckpt_path(name: str, seed: int = 0) -> str:

@@ -92,7 +92,7 @@ def test_checkpoint_layout_roundtrip(small0_ckpt):
     assert set(ck) >= {"state_dict", "hyper_parameters"}
     assert all(k.startswith("model.") for k in ck["state_dict"])
     assert len(ck["state_dict"]) == 166
-    assert sum(v.numel() for v in ck["state_dict"].values()) == 2101357  # SURVEY.md App. B (small0)
+    assert sum(v.numel() for v in ck["state_dict"].values()) == 2101357  # parameters of the small0 configuration
     with pytest.raises(ValueError):
         load_checkpoint("/nonexistent/dir/nothing-here")  # falls through to the URL path, no network -> ValueError
 

@@ -13,7 +13,6 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 VARIANTS = [
     {"BT_ATTN_VARIANT": "32"},                        # attention: every exponential on MUFU
     {"BT_ATTN_VARIANT": "40"},                        # ... 4 of every 8 score pairs on the packed FMA-pipe polynomial
-    {"BT_ATTN_VARIANT": "5"},                         # ... S(j+2) issued only after PV(j) has completed
     {"BT_ATTN_FREQ_SIMT": "1"},                       # CUDA-core frequency attention
     {"BT_FUSE_FF": "0"},                              # unfused frontend blocks (norm + GEMMs)
     {"BT_FUSE_OUTPROJ": "0"},                         # separate attention out-projection GEMM in front of the fused FFN
