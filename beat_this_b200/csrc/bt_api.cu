@@ -481,8 +481,8 @@ int build_plans(bt_ctx* c, int nb, int L, WavePlans** out) {
   }
   WavePlans* w = new WavePlans();
   char err[512] = "";
-  auto mk = [&](const void* A, const Param* W, const GemmShape& g, int planes_in) -> TcGemmPlan* {
-    return tc_gemm_plan_create(A, W->b16, g, planes_in, err, sizeof(err));
+  auto mk = [&](const void* A, const Param* W, const GemmShape& g, int planes_in, bool resid = false) -> TcGemmPlan* {
+    return tc_gemm_plan_create(A, W->b16, g, planes_in, resid, err, sizeof(err));
   };
   auto mk_attn = [&](AttnPlans& a, const AttnW& aw, int planes, int C, bool freq) -> bool {
     if (c->fuse_ff && (C == 32 || C == 64)) {
@@ -490,7 +490,7 @@ int build_plans(bt_ctx* c, int nb, int L, WavePlans** out) {
       if (!a.fqkv) return false;
     }
     a.qkv = mk(c->XN, aw.wqkv, plain_shape(planes, L, 3 * C, C, C), planes);
-    a.out = mk(c->O, aw.wout, plain_shape(planes, L, C, C, C), planes);
+    a.out = mk(c->O, aw.wout, plain_shape(planes, L, C, C, C), planes, true);
     a.gates = mk(c->XN, aw.wg, plain_shape(planes, L, 32, C, C), planes);
     if (!a.qkv || !a.out || !a.gates) return false;
     if (!freq) {
@@ -507,7 +507,7 @@ int build_plans(bt_ctx* c, int nb, int L, WavePlans** out) {
       return f.fused != nullptr && (!(wout && c->fuse_outproj) || f.fused_op != nullptr);
     }
     f.ff1 = mk(c->XN, fw.w1, plain_shape(planes, L, mult * C, C, C), planes);
-    f.ff2 = mk(c->H, fw.w2, plain_shape(planes, L, C, mult * C, mult * C), planes);
+    f.ff2 = mk(c->H, fw.w2, plain_shape(planes, L, C, mult * C, mult * C), planes, true);
     return f.ff1 && f.ff2;
   };
   bool ok = true;
@@ -1124,7 +1124,7 @@ int bt_debug_gemm(bt_ctx* c, const float* a_dev, const float* w_dev, float* d_de
     launch_f32_to_h16(a_dev, ab, static_cast<int64_t>(M) * K, st);
     launch_f32_to_h16(w_dev, wb, static_cast<int64_t>(N) * K, st);
     char err[512] = "";
-    TcGemmPlan* p = tc_gemm_plan_create(ab, wb, g, 1, err, sizeof(err));
+    TcGemmPlan* p = tc_gemm_plan_create(ab, wb, g, 1, false, err, sizeof(err));
     int rc = BT_OK;
     if (!p) rc = fail(c, BT_ERR_CUDA, "%s", err);
     else if (launch_gemm_tc(p, e, st) != 0) rc = fail(c, BT_ERR_CUDA, "tc gemm launch failed");

@@ -102,8 +102,9 @@ void launch_pack_qkv_test(const float* q, const float* k, const float* v, void* 
 
 // ---- 16-bit (fp16 or bf16 operands) tensor-core path (wgmma GEMM, mma.sync attention) ---------------------------------
 struct TcGemmPlan;  // cached tensor maps + launch geometry
+// resid_epilogue: the launches of this plan add the fp32 residual in the epilogue (tile width policy, kernels_gemm.cu)
 TcGemmPlan* tc_gemm_plan_create(const void* A_h16, const void* W_h16, const GemmShape& g,
-                                int planes_in, char* err, int errlen);
+                                int planes_in, bool resid_epilogue, char* err, int errlen);
 void tc_gemm_plan_destroy(TcGemmPlan*);
 int launch_gemm_tc(const TcGemmPlan* plan, const EpiParams& e, cudaStream_t st);
 

@@ -135,6 +135,8 @@ __device__ __forceinline__ void mbar_arrive_a(uint32_t bar) {
 __device__ __forceinline__ void mbar_expect_tx_a(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
+// Bounded spin that traps without a printf: a call (printf is one) in a kernel that issues wgmma makes ptxas
+// serialise every wgmma of that kernel (C7510).  The trap still ends a broken pipeline in a launch error.
 __device__ __forceinline__ void mbar_wait_a(uint32_t bar, uint32_t parity) {
   uint32_t spins = 0;
   for (;;) {
@@ -147,10 +149,7 @@ __device__ __forceinline__ void mbar_wait_a(uint32_t bar, uint32_t parity) {
         : "r"(bar), "r"(parity)
         : "memory");
     if (ok) break;
-    if (++spins > (1u << 26)) {
-      printf("bt: mbarrier timeout block (%d,%d,%d) thread %d\n", blockIdx.x, blockIdx.y, blockIdx.z, threadIdx.x);
-      __trap();
-    }
+    if (++spins > (1u << 26)) __trap();
   }
 }
 __device__ __forceinline__ void tma_load_3d_a(uint32_t smem_dst, const void* tmap, uint32_t bar, int32_t c0, int32_t c1,

@@ -163,11 +163,13 @@ __device__ __forceinline__ void epilogue_apply(const EpiParams& e, int L, int64_
 }
 
 // The same operations for the column pair (n, n + 1), n even, of output row m: the pair a thread of a wgmma
-// accumulator fragment holds.  For kind 1 the pair is one interleaved RoPE pair and pos the row's RoPE position
-// (m % L for posmode 0, (m / L) % F for posmode 1), computed once per row by the caller.
-template <typename TAct>
-__device__ __forceinline__ void epilogue_pair(const EpiParams& e, int64_t m, int pos, int n, float v0, float v1) {
-  if (e.kind == 0) {
+// accumulator fragment holds.  For kind 1 the pair is one interleaved RoPE pair and (co, si) its rotation at the
+// row's position, read once per row by the caller.  KIND is e.kind as a template argument: only the gates
+// instantiation (KIND 2) contains the IEEE division of sigmoidf_, whose slow path is a function call.
+template <typename TAct, int KIND>
+__device__ __forceinline__ void epilogue_pair(const EpiParams& e, int64_t m, int n, float v0, float v1, float co = 0.f,
+                                              float si = 0.f) {
+  if constexpr (KIND == 0) {
     if (e.bias) {
       const float2 b = __ldg(reinterpret_cast<const float2*>(e.bias + n));
       v0 += b.x; v1 += b.y;
@@ -179,15 +181,13 @@ __device__ __forceinline__ void epilogue_pair(const EpiParams& e, int64_t m, int
     }
     if (e.out_f32) *reinterpret_cast<float2*>(e.out_f32 + m * e.ldo_f32 + n) = make_float2(v0, v1);
     if (e.out_act) *reinterpret_cast<uint32_t*>(reinterpret_cast<TAct*>(e.out_act) + m * e.ldo_act + n) = pack_h16x2(v0, v1);
-  } else if (e.kind == 2) {
+  } else if constexpr (KIND == 2) {
     if (n < e.heads) e.out_f32[m * e.heads + n] = sigmoidf_(v0 + __ldg(e.bias + n));
     if (n + 1 < e.heads) e.out_f32[m * e.heads + n + 1] = sigmoidf_(v1 + __ldg(e.bias + n + 1));
   } else {
     const int which = n / e.C;  // 0 q, 1 k, 2 v
     if (which < 2) {
       const float sc = which == 0 ? e.qscale : 1.0f;
-      const int i = ((n - which * e.C) & 31) >> 1;
-      const float co = __ldg(e.rope_cos + pos * 16 + i), si = __ldg(e.rope_sin + pos * 16 + i);
       const float x0 = v0, x1 = v1;
       v0 = (x0 * co - x1 * si) * sc;
       v1 = (x1 * co + x0 * si) * sc;

@@ -52,8 +52,10 @@ bool make_tmap(CUtensorMap* tm, const void* base, int rank, const uint64_t* dims
 // =============================================================================== GEMM
 // CTA = 128 output rows x BN columns, persistent over tiles (stride gridDim.x).  Warp 0 (one elected lane) streams
 // the A and W k-blocks through a STAGES-deep TMA ring; warpgroups 1 and 2 own rows [0, 64) and [64, 128) of the
-// tile and issue wgmma m64nNCk16 over NC-column slices of it (NC = 64, or 32 when BN is not a multiple of 64).  The
-// accumulators stay in registers and go through epilogue_pair straight to global memory.
+// tile and issue one wgmma m64nBNk16 per k16 step, keeping one k-block's MMAs in flight while the next is issued.
+// At BN = 256 the producer warpgroup hands registers to the consumers (setmaxnreg 40 / 232), which is what lets the
+// 128 fp32 accumulators per thread live in registers.  Narrower tiles fit the 168 registers of 384 threads and skip
+// it: with it, the fp32-residual GEMMs at BN = 128 measured 10-15 % slower on H100.  They go through epilogue_pair straight to global memory.
 constexpr int TG_BM = 128;
 constexpr int TG_THREADS = 384;  // warpgroup 0: producer (warp 0), warpgroups 1-2: MMA + epilogue
 
@@ -67,18 +69,14 @@ struct TgCfg {
   static constexpr int STAGES = STAGES_FIT > 6 ? 6 : STAGES_FIT;
   static constexpr int SMEM = STAGES * STAGE_BYTES + FIXED;
   static constexpr int SWZ = BK * 2;  // 128 or 64 byte rows
-  static constexpr int NC = BN % 64 == 0 ? 64 : 32;
-  static constexpr int NCH = BN / NC;
 };
 
-template <int BN, int BK>
+template <int BN, int BK, int KIND>
 __global__ void __launch_bounds__(TG_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW, const GemmShape g,
                const EpiParams e, int num_tiles, int t_tiles, int n_tiles, int m_tiles) {
   using Cfg = TgCfg<BN, BK>;
   constexpr int STAGES = Cfg::STAGES;
-  constexpr int NC = Cfg::NC;
-  constexpr int NCH = Cfg::NCH;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t sA = sbase;
@@ -102,8 +100,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   const int kb_per_slab = g.Kslab / BK;
   const int num_kb = g.nslab * kb_per_slab;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp < 4) {
+    if constexpr (BN == 256) setmaxnreg_dec<40>();
+    if (warp == 0 && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
@@ -123,34 +122,37 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
       }
     }
-  } else if (warp >= 4) {
+  } else {
+    if constexpr (BN == 256) setmaxnreg_inc<232>();
     const int wg = (warp >> 2) - 1;   // 0: tile rows [0, 64), 1: [64, 128)
     const int wq = warp & 3;          // warp inside the warpgroup: 16 rows each
+    const bool leader = (threadIdx.x & 127) == 0;
     const uint32_t a_off = static_cast<uint32_t>(wg * 64 * BK * 2);
     int stage = 0;
     uint32_t phase = 0;
-    float acc[NCH][NC / 2];
+    float acc[BN / 2];
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int mt = tile / n_tiles, nt = tile % n_tiles;
       const int p_out = mt / t_tiles;
+      int prev = -1;  // stage of the k-block whose MMAs are still in flight
       for (int kb = 0; kb < num_kb; ++kb) {
         mbar_wait_a(full + 8 * stage, phase);
         const uint32_t a_base = sA + stage * Cfg::A_BYTES + a_off;
         const uint32_t b_base = sW + stage * Cfg::W_BYTES;
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < BK / 16; ++k) {
-          const uint64_t da = make_wgmma_desc<Cfg::SWZ>(a_base + k * 32);
-#pragma unroll
-          for (int c = 0; c < NCH; ++c)
-            wgmma_n<NC>(acc[c], da, make_wgmma_desc<Cfg::SWZ>(b_base + c * NC * BK * 2 + k * 32), (kb | k) != 0 ? 1u : 0u);
-        }
+        for (int k = 0; k < BK / 16; ++k)
+          wgmma_m64k16<BN>(acc, make_wgmma_desc<Cfg::SWZ>(a_base + k * 32), make_wgmma_desc<Cfg::SWZ>(b_base + k * 32),
+                           (kb | k) != 0 ? 1u : 0u);
         wgmma_commit();
-        wgmma_wait<0>();
-        if ((threadIdx.x & 127) == 0) mbar_arrive_a(empty + 8 * stage);
+        wgmma_wait<1>();  // the previous k-block's MMAs are done: its stage goes back to the producer
+        if (leader && prev >= 0) mbar_arrive_a(empty + 8 * prev);
+        prev = stage;
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
-      // epilogue: this thread's rows t and t + 8, columns 8j + 2 (lane % 4) + {0, 1} of every slice
+      wgmma_wait<0>();
+      if (leader) mbar_arrive_a(empty + 8 * prev);
+      // epilogue: this thread's rows t and t + 8, columns 8j + 2 (lane % 4) + {0, 1} of the tile
       const int tr = (mt - p_out * t_tiles) * TG_BM + wg * 64 + wq * 16 + (lane >> 2);
       const int col0 = nt * BN + 2 * (lane & 3);
 #pragma unroll
@@ -158,12 +160,27 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         const int t = tr + 8 * h;
         if (t < g.L && mt < m_tiles) {
           const int64_t m = static_cast<int64_t>(p_out) * g.L + t;
-          const int pos = e.kind != 1 ? 0 : e.posmode == 0 ? t : p_out % e.F;
+          if constexpr (KIND == 1) {
+            // BN and C (heads of 32) are multiples of 32, so column 8j + 2 (lane % 4) of the tile is RoPE pair
+            // (lane % 4) + 4 (j % 4) of its head: four rotations per row and thread, none for a tile of v columns
+            static_assert(BN % 32 == 0, "RoPE pairs of a column need BN % 32 == 0");
+            const int pos = e.posmode == 0 ? t : p_out % e.F;
+            float co[4] = {}, si[4] = {};
+            if (nt * BN < 2 * e.C) {
 #pragma unroll
-          for (int c = 0; c < NCH; ++c)
+              for (int q = 0; q < 4; ++q) {
+                co[q] = __ldg(e.rope_cos + pos * 16 + 4 * q + (lane & 3));
+                si[q] = __ldg(e.rope_sin + pos * 16 + 4 * q + (lane & 3));
+              }
+            }
 #pragma unroll
-            for (int j = 0; j < NC / 8; ++j)
-              epilogue_pair<h16>(e, m, pos, col0 + c * NC + 8 * j, acc[c][4 * j + 2 * h], acc[c][4 * j + 2 * h + 1]);
+            for (int j = 0; j < BN / 8; ++j)
+              epilogue_pair<h16, 1>(e, m, col0 + 8 * j, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], co[j & 3], si[j & 3]);
+          } else {
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j)
+              epilogue_pair<h16, KIND>(e, m, col0 + 8 * j, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+          }
         }
       }
     }
@@ -177,36 +194,39 @@ struct TcGemmPlan {
   int num_tiles, t_tiles, n_tiles, m_tiles, grid;
 };
 
-// BN = 256 would need 128 accumulator registers per thread and spills at the 168-register limit of 384 threads
-static int pick_bn(int N) {
-  const int cands[5] = {192, 128, 96, 64, 32};
+// Widest tile that divides N and is at most max_bn.  BK = 32 tiles stay at BN <= 128.  A GEMM whose epilogue reads the
+// fp32 residual stays at BN <= 128 as well: its epilogue runs straight from the accumulator registers (8-byte residual
+// loads and stores, 8 rows per warp instruction) and measured no faster at BN = 256 (H100 80GB HBM3 at 400 W, per bench
+// step: attention-out 6.7 ms against 6.0 ms at BN = 128, FFN-down 9.6 ms at both).
+static int pick_bn(int N, int max_bn) {
+  const int cands[5] = {256, 192, 128, 64, 32};
   for (int i = 0; i < 5; ++i)
-    if (N % cands[i] == 0) return cands[i];
+    if (cands[i] <= max_bn && N % cands[i] == 0) return cands[i];
   return 0;
 }
 
-template <int BN, int BK>
+template <int BN, int BK, int KIND>
 static int gemm_tc_launch(const TcGemmPlan* p, const EpiParams& e, cudaStream_t st) {
   using Cfg = TgCfg<BN, BK>;
   static_assert(Cfg::STAGES >= 2, "pipeline too shallow");
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t r = cudaFuncSetAttribute(gemm_tc_kernel<BN, BK>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
+    cudaError_t r = cudaFuncSetAttribute(gemm_tc_kernel<BN, BK, KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
     if (r != cudaSuccess) return -1;
     attr_set = true;
   }
-  gemm_tc_kernel<BN, BK><<<p->grid, TG_THREADS, Cfg::SMEM, st>>>(p->tmA, p->tmW, p->g, e, p->num_tiles, p->t_tiles,
+  gemm_tc_kernel<BN, BK, KIND><<<p->grid, TG_THREADS, Cfg::SMEM, st>>>(p->tmA, p->tmW, p->g, e, p->num_tiles, p->t_tiles,
                                                                   p->n_tiles, p->m_tiles);
   return 0;
 }
 
-TcGemmPlan* tc_gemm_plan_create(const void* A, const void* W, const GemmShape& g, int planes_in, char* err,
-                                int errlen) {
+TcGemmPlan* tc_gemm_plan_create(const void* A, const void* W, const GemmShape& g, int planes_in, bool resid_epilogue,
+                                char* err, int errlen) {
   TcGemmPlan* p = new TcGemmPlan();
   p->g = g;
   p->BK = (g.Kslab % 64 == 0) ? 64 : 32;
-  p->BN = pick_bn(g.N);
-  if (p->BN == 0 || g.Kslab % 32 != 0 || (p->BK == 32 && p->BN > 128)) {
+  p->BN = pick_bn(g.N, p->BK == 32 || resid_epilogue ? 128 : 256);
+  if (p->BN == 0 || g.Kslab % 32 != 0) {
     snprintf(err, errlen, "tc gemm: unsupported shape N=%d Kslab=%d", g.N, g.Kslab);
     delete p;
     return nullptr;
@@ -236,10 +256,17 @@ TcGemmPlan* tc_gemm_plan_create(const void* A, const void* W, const GemmShape& g
 void tc_gemm_plan_destroy(TcGemmPlan* p) { delete p; }
 
 int launch_gemm_tc(const TcGemmPlan* p, const EpiParams& e, cudaStream_t st) {
-#define BT_TG_CASE(bn, bk) \
-  if (p->BN == bn && p->BK == bk) return gemm_tc_launch<bn, bk>(p, e, st);
-  BT_TG_CASE(192, 64) BT_TG_CASE(128, 64) BT_TG_CASE(96, 64) BT_TG_CASE(64, 64)
-  BT_TG_CASE(32, 64) BT_TG_CASE(128, 32) BT_TG_CASE(96, 32) BT_TG_CASE(64, 32) BT_TG_CASE(32, 32)
+  // the gates GEMM (kind 2) is N = 32 wide
+  if (e.kind == 2) {
+    if (p->BN == 32 && p->BK == 64) return gemm_tc_launch<32, 64, 2>(p, e, st);
+    if (p->BN == 32 && p->BK == 32) return gemm_tc_launch<32, 32, 2>(p, e, st);
+    return -2;
+  }
+#define BT_TG_CASE(bn, bk)                                                      \
+  if (p->BN == bn && p->BK == bk)                                               \
+    return e.kind == 1 ? gemm_tc_launch<bn, bk, 1>(p, e, st) : gemm_tc_launch<bn, bk, 0>(p, e, st);
+  BT_TG_CASE(256, 64) BT_TG_CASE(192, 64) BT_TG_CASE(128, 64) BT_TG_CASE(64, 64) BT_TG_CASE(32, 64)
+  BT_TG_CASE(128, 32) BT_TG_CASE(64, 32) BT_TG_CASE(32, 32)
 #undef BT_TG_CASE
   return -2;
 }
