@@ -46,6 +46,29 @@ class bt_hparams(ctypes.Structure):
     ]
 
 
+class bt_debug_gemm_desc(ctypes.Structure):
+    _fields_ = [
+        ("planes_out", c_int32),
+        ("planes_in", c_int32),
+        ("L", c_int32),
+        ("N", c_int32),
+        ("Kslab", c_int32),
+        ("nslab", c_int32),
+        ("plane_mul", c_int32),
+        ("lda", c_int32),
+        ("plane_add", c_int32 * 6),
+        ("t_shift", c_int32 * 6),
+        ("resid_epilogue", c_int32),
+        ("kind", c_int32),
+        ("gelu", c_int32),
+        ("C", c_int32),
+        ("heads", c_int32),
+        ("posmode", c_int32),
+        ("F", c_int32),
+        ("qscale", c_float),
+    ]
+
+
 # every symbol include/beatthis.h declares: name -> (restype, argtypes)
 PROTOTYPES = {
     "bt_version": (c_int, []),
@@ -93,9 +116,20 @@ PROTOTYPES = {
     "bt_profile_get": (c_int, [c_void_p, c_int, c_char_p, c_int, POINTER(c_double), POINTER(c_int64)]),
     "bt_debug_request_tap": (c_int, [c_void_p, c_char_p, c_void_p, c_int64]),
     "bt_debug_tap_count": (c_int64, [c_void_p]),
-    "bt_debug_gemm": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p]),
+    "bt_debug_gemm": (
+        c_int,
+        [c_void_p, POINTER(bt_debug_gemm_desc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64,
+         c_void_p, c_void_p, POINTER(c_int32), c_void_p],
+    ),
     "bt_debug_attention_time": (c_int, [c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p]),
-    "bt_debug_attention": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p]),
+    "bt_debug_attention": (
+        c_int,
+        [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, POINTER(c_int32), c_int32,
+         c_void_p],
+    ),
+    "bt_debug_attention_freq": (
+        c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p],
+    ),
 }
 
 _lib = None

@@ -1110,73 +1110,136 @@ int bt_peakpick(bt_ctx* c, const float* beat_dev, const float* downbeat_dev, con
   return BT_OK;
 }
 
-int bt_debug_gemm(bt_ctx* c, const float* a_dev, const float* w_dev, float* d_dev, int32_t M, int32_t N, int32_t K,
+int bt_debug_gemm(bt_ctx* c, const bt_debug_gemm_desc* d, const float* a_dev, const float* w_dev,
+                  const float* bias_dev, const float* resid_dev, float* out_f32_dev, float* out_act_dev,
+                  int64_t out_act_count, const float* rope_cos_dev, const float* rope_sin_dev, int32_t* tile_out,
                   void* stream) {
-  if (!c) return BT_ERR_ARG;
+  if (!c || !d || !a_dev || !w_dev) return fail(c, BT_ERR_ARG, "bt_debug_gemm: null argument");
+  if (d->nslab < 1 || d->nslab > kMaxSlabs || d->planes_out < 1 || d->L < 1 || d->N % 4 != 0 || d->Kslab % 16 != 0 ||
+      d->lda % 4 != 0 || (out_act_dev && out_act_count < static_cast<int64_t>(d->planes_out) * d->L * d->N))
+    return fail(c, BT_ERR_ARG, "bt_debug_gemm: unsupported shape");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   BT_CUDA(c, cudaSetDevice(c->device));
-  GemmShape g = plain_shape(1, M, N, K, K);
-  EpiParams e = epi_generic(nullptr, 0, nullptr, 0, d_dev, N, nullptr, 0);
-  if (c->dtype == BT_DTYPE_H16) {
-    void *ab = nullptr, *wb = nullptr;
-    BT_CUDA(c, cudaMalloc(&ab, static_cast<size_t>(M) * K * 2));
-    BT_CUDA(c, cudaMalloc(&wb, static_cast<size_t>(N) * K * 2));
-    launch_f32_to_h16(a_dev, ab, static_cast<int64_t>(M) * K, st);
-    launch_f32_to_h16(w_dev, wb, static_cast<int64_t>(N) * K, st);
-    char err[512] = "";
-    TcGemmPlan* p = tc_gemm_plan_create(ab, wb, g, 1, false, err, sizeof(err));
-    int rc = BT_OK;
+  GemmShape g{};
+  g.planes_out = d->planes_out; g.L = d->L; g.N = d->N; g.Kslab = d->Kslab; g.nslab = d->nslab;
+  g.plane_mul = d->plane_mul; g.lda = d->lda;
+  for (int s = 0; s < kMaxSlabs; ++s) { g.plane_add[s] = d->plane_add[s]; g.t_shift[s] = d->t_shift[s]; }
+  EpiParams e{};
+  e.kind = d->kind; e.bias = bias_dev; e.gelu = d->gelu;
+  e.resid = resid_dev; e.ldr = d->N;
+  e.out_f32 = out_f32_dev; e.ldo_f32 = d->N;
+  e.out_act = out_act_dev; e.ldo_act = d->N;
+  e.rope_cos = rope_cos_dev; e.rope_sin = rope_sin_dev;
+  e.C = d->C; e.heads = d->heads; e.posmode = d->posmode; e.F = d->F; e.qscale = d->qscale;
+  if (tile_out) tile_out[0] = tile_out[1] = 0;
+  if (c->dtype != BT_DTYPE_H16) {
+    launch_gemm_simt(a_dev, w_dev, g, e, st);
+    BT_LAUNCHED(c, "debug_gemm", st);
+    BT_CUDA(c, cudaStreamSynchronize(st));
+    return BT_OK;
+  }
+  const int64_t a_n = static_cast<int64_t>(d->planes_in) * d->L * d->lda;
+  const int64_t w_n = static_cast<int64_t>(d->N) * d->Kslab * d->nslab;
+  void *ab = nullptr, *wb = nullptr, *ob = nullptr;
+  TcGemmPlan* p = nullptr;
+  int rc = BT_OK;
+  char err[512] = "";
+  if (cudaMalloc(&ab, a_n * 2) != cudaSuccess || cudaMalloc(&wb, w_n * 2) != cudaSuccess ||
+      (out_act_dev && cudaMalloc(&ob, out_act_count * 2) != cudaSuccess)) {
+    rc = fail(c, BT_ERR_CUDA, "bt_debug_gemm: out of device memory");
+  } else {
+    launch_f32_to_h16(a_dev, ab, a_n, st);
+    launch_f32_to_h16(w_dev, wb, w_n, st);
+    if (ob) launch_f32_to_h16(out_act_dev, ob, out_act_count, st);
+    e.out_act = ob;
+    p = tc_gemm_plan_create(ab, wb, g, d->planes_in, d->resid_epilogue != 0, err, sizeof(err));
     if (!p) rc = fail(c, BT_ERR_CUDA, "%s", err);
     else if (launch_gemm_tc(p, e, st) != 0) rc = fail(c, BT_ERR_CUDA, "tc gemm launch failed");
-    cudaError_t se = cudaStreamSynchronize(st);
-    if (rc == BT_OK && se != cudaSuccess) rc = fail(c, BT_ERR_CUDA, "tc gemm: %s", cudaGetErrorString(se));
-    if (p) tc_gemm_plan_destroy(p);
-    cudaFree(ab); cudaFree(wb);
-    c->launches++;
-    return rc;
+    else if (ob) launch_h16_to_f32(ob, out_act_dev, out_act_count, st);
+    if (p && tile_out) tc_gemm_plan_tile(p, &tile_out[0], &tile_out[1]);
   }
-  launch_gemm_simt(a_dev, w_dev, g, e, st);
-  BT_LAUNCHED(c, "debug_gemm", st);
-  return BT_OK;
+  cudaError_t se = cudaStreamSynchronize(st);
+  if (rc == BT_OK && se != cudaSuccess) rc = fail(c, BT_ERR_CUDA, "tc gemm: %s", cudaGetErrorString(se));
+  if (p) tc_gemm_plan_destroy(p);
+  cudaFree(ab); cudaFree(wb); cudaFree(ob);
+  c->launches++;
+  return rc;
 }
 
-int bt_debug_attention(bt_ctx* c, const float* q_dev, const float* k_dev, const float* v_dev, float* o_dev,
-                       int32_t seqs, int32_t L, int32_t heads, void* stream) {
-  if (!c) return BT_ERR_ARG;
+int bt_debug_attention(bt_ctx* c, const float* q_dev, const float* k_dev, const float* v_dev, const float* gates_dev,
+                       float* o_dev, int32_t seqs, int32_t L, int32_t heads, const int32_t* key_lens_host,
+                       int32_t seqs_per_chunk, void* stream) {
+  if (!c || !q_dev || !k_dev || !v_dev || !gates_dev || !o_dev) return fail(c, BT_ERR_ARG, "bt_debug_attention: null argument");
+  if (seqs < 1 || L < 1 || heads < 1 || (key_lens_host && (seqs_per_chunk < 1 || seqs % seqs_per_chunk != 0)))
+    return fail(c, BT_ERR_ARG, "bt_debug_attention: bad geometry");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   BT_CUDA(c, cudaSetDevice(c->device));
   const int C = heads * 32;
   const int64_t M = static_cast<int64_t>(seqs) * L;
   const bool tc = c->dtype == BT_DTYPE_H16;
   const size_t act = tc ? 2 : 4;
+  // per-chunk key counts travel in the ChunkSrc table the forward pass hands the kernels (only .len is read)
+  std::vector<ChunkSrc> chunks;
+  if (key_lens_host) {
+    chunks.assign(seqs / seqs_per_chunk, ChunkSrc{});
+    for (size_t i = 0; i < chunks.size(); ++i) {
+      if (key_lens_host[i] < 1 || key_lens_host[i] > L) return fail(c, BT_ERR_ARG, "bt_debug_attention: key length out of [1, L]");
+      chunks[i].len = key_lens_host[i];
+    }
+  }
   void *qkv = nullptr, *o = nullptr;
-  float* gates = nullptr;
+  ChunkSrc* chunks_dev = nullptr;
   BT_CUDA(c, cudaMalloc(&qkv, M * 3 * C * act));
   BT_CUDA(c, cudaMalloc(&o, M * C * act));
-  BT_CUDA(c, cudaMalloc(&gates, M * heads * 4));
-  std::vector<float> ones(M * heads, 1.0f);
-  BT_CUDA(c, cudaMemcpyAsync(gates, ones.data(), M * heads * 4, cudaMemcpyHostToDevice, st));
+  if (key_lens_host) {
+    BT_CUDA(c, cudaMalloc(&chunks_dev, chunks.size() * sizeof(ChunkSrc)));
+    BT_CUDA(c, cudaMemcpyAsync(chunks_dev, chunks.data(), chunks.size() * sizeof(ChunkSrc), cudaMemcpyHostToDevice, st));
+  }
   int rc = BT_OK;
   if (tc) {
     launch_pack_qkv_test(q_dev, k_dev, v_dev, qkv, seqs, L, heads, 0.17677669529663687f * 1.4426950408889634f, 1, st);
     char err[512] = "";
     TcAttnPlan* p = tc_attn_plan_create(qkv, seqs, L, heads, err, sizeof(err));
     if (!p) rc = fail(c, BT_ERR_CUDA, "%s", err);
-    else {
-      launch_attn_time_tc(p, gates, o, st);
-      launch_h16_to_f32(o, o_dev, M * C, st);
-    }
+    else if (launch_attn_time_tc(p, gates_dev, o, st, chunks_dev, seqs_per_chunk) != 0) rc = fail(c, BT_ERR_CUDA, "tc attention launch failed");
+    else launch_h16_to_f32(o, o_dev, M * C, st);
     cudaError_t se = cudaStreamSynchronize(st);
     if (rc == BT_OK && se != cudaSuccess) rc = fail(c, BT_ERR_CUDA, "tc attention: %s", cudaGetErrorString(se));
     if (p) tc_attn_plan_destroy(p);
   } else {
     launch_pack_qkv_test(q_dev, k_dev, v_dev, qkv, seqs, L, heads, 1.0f, 0, st);
-    launch_attn_time_simt(static_cast<const float*>(qkv), gates, o_dev, seqs, L, heads, st);
+    launch_attn_time_simt(static_cast<const float*>(qkv), gates_dev, o_dev, seqs, L, heads, st, chunks_dev, seqs_per_chunk);
     cudaError_t se = cudaStreamSynchronize(st);
     if (se != cudaSuccess) rc = fail(c, BT_ERR_CUDA, "simt attention: %s", cudaGetErrorString(se));
   }
   c->launches += 2;
-  cudaFree(qkv); cudaFree(o); cudaFree(gates);
+  cudaFree(qkv); cudaFree(o); cudaFree(chunks_dev);
+  return rc;
+}
+
+int bt_debug_attention_freq(bt_ctx* c, const float* q_dev, const float* k_dev, const float* v_dev,
+                            const float* gates_dev, float* o_dev, int32_t B, int32_t F, int32_t L, int32_t heads,
+                            void* stream) {
+  if (!c || !q_dev || !k_dev || !v_dev || !gates_dev || !o_dev) return fail(c, BT_ERR_ARG, "bt_debug_attention_freq: null argument");
+  if (B < 1 || L < 1 || heads < 1 || (F != 8 && F != 16 && F != 32))
+    return fail(c, BT_ERR_ARG, "bt_debug_attention_freq: need B, L, heads >= 1 and F in {8, 16, 32}");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  BT_CUDA(c, cudaSetDevice(c->device));
+  const int C = heads * 32;
+  const int64_t M = static_cast<int64_t>(B) * F * L;
+  const bool tc = c->dtype == BT_DTYPE_H16;
+  const size_t act = tc ? 2 : 4;
+  void *qkv = nullptr, *o = nullptr;
+  BT_CUDA(c, cudaMalloc(&qkv, M * 3 * C * act));
+  if (tc) BT_CUDA(c, cudaMalloc(&o, M * C * act));
+  launch_pack_qkv_test(q_dev, k_dev, v_dev, qkv, B * F, L, heads, 1.0f, tc ? 1 : 0, st);
+  launch_attn_freq(qkv, gates_dev, tc ? o : static_cast<void*>(o_dev), B, F, L, heads, 0.17677669529663687f, tc ? 1 : 0, st);
+  if (tc) launch_h16_to_f32(o, o_dev, M * C, st);
+  int rc = BT_OK;
+  cudaError_t se = cudaStreamSynchronize(st);
+  if (se != cudaSuccess) rc = fail(c, BT_ERR_CUDA, "frequency attention: %s", cudaGetErrorString(se));
+  c->launches += 2;
+  cudaFree(qkv); cudaFree(o);
   return rc;
 }
 

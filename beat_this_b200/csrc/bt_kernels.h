@@ -96,7 +96,7 @@ void launch_peakpick(const float* beat, const float* down, const int64_t* frame_
 void launch_f32_to_h16(const float* in, void* out, int64_t n, cudaStream_t st);
 void launch_h16_to_f32(const void* in, float* out, int64_t n, cudaStream_t st);
 // [seqs, L, heads*32] fp32 q,k,v -> packed qkv buffer [seqs*L, 3C] of the activation dtype
-// (test hook for bt_debug_attention)
+// (test hooks bt_debug_attention and bt_debug_attention_freq)
 void launch_pack_qkv_test(const float* q, const float* k, const float* v, void* qkv, int seqs, int L,
                           int heads, float qscale, int act_h16, cudaStream_t st);
 
@@ -106,6 +106,7 @@ struct TcGemmPlan;  // cached tensor maps + launch geometry
 TcGemmPlan* tc_gemm_plan_create(const void* A_h16, const void* W_h16, const GemmShape& g,
                                 int planes_in, bool resid_epilogue, char* err, int errlen);
 void tc_gemm_plan_destroy(TcGemmPlan*);
+void tc_gemm_plan_tile(const TcGemmPlan*, int* bn, int* bk);  // the (BN, BK) tile the plan launches
 int launch_gemm_tc(const TcGemmPlan* plan, const EpiParams& e, cudaStream_t st);
 
 struct TcAttnPlan;

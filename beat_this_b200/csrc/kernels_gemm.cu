@@ -254,6 +254,7 @@ TcGemmPlan* tc_gemm_plan_create(const void* A, const void* W, const GemmShape& g
   return p;
 }
 void tc_gemm_plan_destroy(TcGemmPlan* p) { delete p; }
+void tc_gemm_plan_tile(const TcGemmPlan* p, int* bn, int* bk) { *bn = p->BN; *bk = p->BK; }
 
 int launch_gemm_tc(const TcGemmPlan* p, const EpiParams& e, cudaStream_t st) {
   // the gates GEMM (kind 2) is N = 32 wide

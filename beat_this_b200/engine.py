@@ -284,17 +284,60 @@ class Engine:
         return buf[:n], out
 
     def debug_gemm(self, a: torch.Tensor, w: torch.Tensor):
+        """D[M, N] = A[M, K] W[N, K]^T (fp32 device tensors) through the ctx's GEMM, no epilogue."""
         M, K = a.shape
         N = w.shape[0]
         d = torch.empty((M, N), dtype=torch.float32, device=self.device)
-        code = self.lib.bt_debug_gemm(self.ctx, c_void_p(a.data_ptr()), c_void_p(w.data_ptr()), c_void_p(d.data_ptr()), M, N, K, self._stream())
-        _lib.check(self.lib, self.ctx, code)
+        shape = dict(planes_out=1, planes_in=1, L=M, N=N, Kslab=K, nslab=1, plane_mul=1, lda=K, plane_add=[0], t_shift=[0])
+        self.debug_gemm_full(shape, a.contiguous(), w.contiguous(), out_f32=d)
         return d
 
-    def debug_attention(self, q, k, v):
+    def debug_gemm_full(self, shape: dict, a, w, bias=None, resid=None, out_f32=None, out_act=None, rope_cos=None,
+                        rope_sin=None, resid_epilogue=False, kind=0, gelu=False, C=0, heads=0, posmode=0, F=1, qscale=1.0):
+        """One GEMM through bt_debug_gemm.  shape: the GemmShape fields (planes_out, planes_in, L, N, Kslab, nslab,
+        plane_mul, lda, plane_add, t_shift); tensors are fp32 on this device and are passed through as they are (the
+        outputs are written in place, resid may be out_f32).  Returns the (BN, BK) tile of the 16-bit plan."""
+        def ptr(t):
+            if t is None:
+                return None
+            assert t.is_cuda and t.dtype == torch.float32 and t.is_contiguous()
+            return c_void_p(t.data_ptr())
+
+        d = _lib.bt_debug_gemm_desc()
+        for f in ("planes_out", "planes_in", "L", "N", "Kslab", "nslab", "plane_mul", "lda"):
+            setattr(d, f, int(shape[f]))
+        for s in range(6):
+            d.plane_add[s] = int(shape["plane_add"][s]) if s < len(shape["plane_add"]) else 0
+            d.t_shift[s] = int(shape["t_shift"][s]) if s < len(shape["t_shift"]) else 0
+        d.resid_epilogue, d.kind, d.gelu, d.C, d.heads, d.posmode, d.F = int(resid_epilogue), kind, int(gelu), C, heads, posmode, F
+        d.qscale = float(qscale)
+        tile = (ctypes.c_int32 * 2)()
+        code = self.lib.bt_debug_gemm(self.ctx, ctypes.byref(d), ptr(a), ptr(w), ptr(bias), ptr(resid), ptr(out_f32), ptr(out_act),
+                                      out_act.numel() if out_act is not None else 0, ptr(rope_cos), ptr(rope_sin), tile,
+                                      self._stream())
+        _lib.check(self.lib, self.ctx, code)
+        return int(tile[0]), int(tile[1])
+
+    def debug_attention(self, q, k, v, gates=None, key_lens=None, seqs_per_chunk=1):
+        """gates * SDPA through the time-direction attention kernel; q/k/v [seqs, L, heads*32], gates [seqs*L, heads]
+        (None: ones); key_lens: keys per chunk of seqs_per_chunk sequences (None: all L)."""
         seqs, L, C = q.shape
+        if gates is None:
+            gates = torch.ones(seqs * L, C // 32, dtype=torch.float32, device=self.device)
         o = torch.empty_like(q)
+        lens = (ctypes.c_int32 * len(key_lens))(*[int(x) for x in key_lens]) if key_lens is not None else None
         code = self.lib.bt_debug_attention(self.ctx, c_void_p(q.data_ptr()), c_void_p(k.data_ptr()), c_void_p(v.data_ptr()),
-                                           c_void_p(o.data_ptr()), seqs, L, C // 32, self._stream())
+                                           c_void_p(gates.data_ptr()), c_void_p(o.data_ptr()), seqs, L, C // 32, lens,
+                                           seqs_per_chunk, self._stream())
+        _lib.check(self.lib, self.ctx, code)
+        return o
+
+    def debug_attention_freq(self, q, k, v, gates, B, F):
+        """gates * softmax over the F planes of each (chunk, frame, head); q/k/v [B*F*L, heads*32], gates [B*F*L, heads]."""
+        M, C = q.shape
+        o = torch.empty_like(q)
+        code = self.lib.bt_debug_attention_freq(self.ctx, c_void_p(q.data_ptr()), c_void_p(k.data_ptr()), c_void_p(v.data_ptr()),
+                                                c_void_p(gates.data_ptr()), c_void_p(o.data_ptr()), B, F, M // (B * F), C // 32,
+                                                self._stream())
         _lib.check(self.lib, self.ctx, code)
         return o

@@ -241,20 +241,53 @@ int bt_profile_get(const bt_ctx* ctx, int index, char* name, int name_cap, doubl
 int bt_debug_request_tap(bt_ctx* ctx, const char* tap, float* out_dev, int64_t cap);
 int64_t bt_debug_tap_count(const bt_ctx* ctx);
 
-/* Test hook: D[M,N] = A[M,K] * W[N,K]^T through the ctx's GEMM for its compute dtype
- * (fp32 inputs on device; the 16-bit path rounds A and W to its operand type first). */
-int bt_debug_gemm(bt_ctx* ctx, const float* a_dev, const float* w_dev, float* d_dev,
-                  int32_t M, int32_t N, int32_t K, void* stream);
+/* Shape and epilogue of one bt_debug_gemm call: the GEMM the forward pass runs for a linear layer, a k(2,3)
+ * convolution or frontend.linear (csrc/bt_kernels.h GemmShape / EpiParams).  Output row m = p_out * L + t of N
+ * columns; slab s reads plane p_out * plane_mul + plane_add[s] at time t + t_shift[s] (zeros outside [0, L)),
+ * columns [0, Kslab) of a row-major [planes_in * L, lda] A.  W is [N, nslab * Kslab].
+ * kind 0: (+ bias) (-> GELU) (+ resid) into out_f32 and/or out_act, both [M, N];  kind 1: q|k|v columns of C each,
+ * RoPE on q and k at position t (posmode 0) or p_out % F (posmode 1), q scaled by qscale, into out_act [M, N];
+ * kind 2: sigmoid(acc + bias) of columns n < heads into out_f32 [M, heads].
+ * resid_epilogue: the tile-width policy of a GEMM whose epilogue adds the fp32 residual. */
+typedef struct bt_debug_gemm_desc {
+  int32_t planes_out, planes_in, L, N, Kslab, nslab, plane_mul, lda;
+  int32_t plane_add[6];
+  int32_t t_shift[6];
+  int32_t resid_epilogue;
+  int32_t kind, gelu, C, heads, posmode, F;
+  float qscale;
+} bt_debug_gemm_desc;
 
-/* Test hook: softmax(Q K^T / sqrt(32)) V for `seqs` sequences of length L and `heads`
- * heads of dim 32 through the ctx's time-direction attention kernel.  q/k/v/o_dev are
- * [seqs, L, heads*32] fp32. */
+/* Test hook: one GEMM of shape and epilogue `desc` through the ctx's GEMM kernel (16-bit: gemm_tc_kernel, fp32:
+ * gemm_simt_kernel).  Every *_dev pointer is fp32 on the device (bias, resid, out_f32, out_act, rope tables may be
+ * NULL) and is passed through unchanged, so resid may alias out_f32.  The 16-bit context rounds A and W to its
+ * operand type and runs out_act (all out_act_count elements of the buffer, so values the kernel does not store
+ * survive) through its activation type around the launch.  tile_out[2] (optional) receives the (BN, BK) tile of the
+ * 16-bit plan, (0, 0) in the fp32 context.  Synchronises the stream. */
+int bt_debug_gemm(bt_ctx* ctx, const bt_debug_gemm_desc* desc, const float* a_dev, const float* w_dev,
+                  const float* bias_dev, const float* resid_dev, float* out_f32_dev, float* out_act_dev,
+                  int64_t out_act_count, const float* rope_cos_dev, const float* rope_sin_dev, int32_t* tile_out,
+                  void* stream);
+
+/* Test hook: gates * softmax(Q K^T / sqrt(32)) V for `seqs` sequences of length L and `heads` heads of dim 32
+ * through the ctx's time-direction attention kernel.  q/k/v/o_dev are [seqs, L, heads*32] fp32, gates_dev
+ * [seqs * L, heads] fp32.  key_lens_host (optional): sequence s belongs to chunk s / seqs_per_chunk and attends to
+ * the first key_lens_host[chunk] keys only (1 <= len <= L), as in a wave of chunks of different lengths.
+ * Synchronises the stream. */
 int bt_debug_attention(bt_ctx* ctx, const float* q_dev, const float* k_dev, const float* v_dev,
-                       float* o_dev, int32_t seqs, int32_t L, int32_t heads, void* stream);
+                       const float* gates_dev, float* o_dev, int32_t seqs, int32_t L, int32_t heads,
+                       const int32_t* key_lens_host, int32_t seqs_per_chunk, void* stream);
 
-/* Profiling hook (tools/attn_ubench.py): time `iters` launches of the 16-bit time-direction attention kernel on
- * synthetic q|k|v of [seqs, L, heads*32]; variant < 0 keeps the default kernel, otherwise the template parameter V
- * of attn_tc48_kernel (kernels_attn.cu lists the compiled ones).  *ms_per_launch from CUDA events. */
+/* Test hook: the frequency-direction attention of B chunks of F planes of L frames: token m = (b * F + f) * L + t
+ * attends over the F tokens of its (b, t), gates * softmax(q k^T / sqrt(32)) v per head.  q/k/v/o_dev are
+ * [B * F * L, heads * 32] fp32, gates_dev [B * F * L, heads]; F in {8, 16, 32}.  Synchronises the stream. */
+int bt_debug_attention_freq(bt_ctx* ctx, const float* q_dev, const float* k_dev, const float* v_dev,
+                            const float* gates_dev, float* o_dev, int32_t B, int32_t F, int32_t L, int32_t heads,
+                            void* stream);
+
+/* Profiling hook: time `iters` launches of the 16-bit time-direction attention kernel on synthetic q|k|v of
+ * [seqs, L, heads*32]; variant < 0 keeps the default kernel, otherwise the template parameter V of attn_time_kernel
+ * (kernels_attn.cu lists the compiled ones).  *ms_per_launch from CUDA events. */
 int bt_debug_attention_time(bt_ctx* ctx, int32_t seqs, int32_t L, int32_t heads, int32_t variant,
                             int32_t iters, float* ms_per_launch);
 
