@@ -15,8 +15,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 # BT_LIB_PATH: an instrumented build of the same sources (e.g. build(extra_flags=("-DBT_FF_PROF",), out_path=...))
 LIB_PATH = os.environ.get("BT_LIB_PATH") or os.path.join(HERE, "libbeatthis_sm90.so")
-SOURCES = ["bt_api.cu", "kernels_simt.cu", "kernels_misc.cu", "kernels_gemm.cu", "kernels_attn.cu", "kernels_fused.cu", "dbn_host.cpp", "host_stage.cpp"]
-HEADERS = ["common.cuh", "epilogue.cuh", "tc_common.cuh", "bt_kernels.h", os.path.join("..", "..", "include", "beatthis.h")]
+SOURCES = ["bt_api.cu", "kernels_simt.cu", "kernels_misc.cu", "kernels_gemm.cu", "kernels_attn.cu", "kernels_fused.cu", "kernels_dbn.cu", "dbn_host.cpp", "host_stage.cpp"]
+HEADERS = ["common.cuh", "epilogue.cuh", "tc_common.cuh", "bt_kernels.h", "dbn_model.h", os.path.join("..", "..", "include", "beatthis.h")]
 
 BT_DTYPE_F32 = 0
 BT_DTYPE_H16 = 1
@@ -96,6 +96,15 @@ PROTOTYPES = {
     "bt_dbn_viterbi": (
         c_int,
         [c_void_p, c_int64, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
+    ),
+    "bt_dbn_track_device": (
+        c_int,
+        [c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int64), c_int32, c_void_p, c_int32, c_double, c_double, c_int32,
+         c_double, c_double, c_double, c_int32, c_double, c_void_p, c_void_p, c_void_p, c_void_p],
+    ),
+    "bt_debug_dbn_viterbi": (
+        c_int,
+        [c_void_p, c_void_p, c_int64, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
     ),
     "bt_spect2frames": (c_int, [c_void_p, c_void_p, POINTER(c_int64), c_int32, c_void_p, c_void_p, c_void_p]),
     "bt_forward_chunks": (c_int, [c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_void_p]),

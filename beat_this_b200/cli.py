@@ -33,7 +33,10 @@ def build_parser() -> argparse.ArgumentParser:
     add("--skip-existing", action="store_true", help="leave results that already exist untouched")
     add("--touch-first", action="store_true", help="create the (empty) result file before working on it: with --skip-existing, "
                                                    "several processes can split one directory between them")
-    add("--dbn", default=False, action=argparse.BooleanOptionalAction, help="DBN post-processing on the host instead of peak picking")
+    add("--dbn", default=False, action=argparse.BooleanOptionalAction, help="DBN post-processing instead of peak picking")
+    add("--dbn-impl", default="auto", choices=["auto", "madmom", "native", "device"],
+        help="DBN decoder: madmom if installed else the host C++ tracker (auto), madmom, the host C++ tracker (native) "
+             "or the same tracker on the GPU (device) [%(default)s]")
     add("--gpu", type=int, default=None, help="CUDA device index [LOCAL_RANK or 0]; a GPU is required")
     add("--float16", action="store_true", help="fp16 tensor-core kernels (fast path) instead of fp32")
     add("--activations", action="store_true", help="also write the frame activations as <result>.npy (2 x frames)")
@@ -98,7 +101,7 @@ def _release(dst: Path, touch_first: bool) -> None:
 
 
 def run(inputs, model="final0", output=None, suffix=".beats", append=False, skip_existing=False, touch_first=False,
-        dbn=False, gpu=None, float16=False, activations=False, batch=256) -> int:
+        dbn=False, gpu=None, float16=False, activations=False, batch=256, dbn_impl="auto") -> int:
     from .inference import File2Beats
     from .preprocessing import load_audio
 
@@ -109,7 +112,7 @@ def run(inputs, model="final0", output=None, suffix=".beats", append=False, skip
         raise SystemExit("beat_this_b200 has no CPU path: --gpu must name a CUDA device")
     tasks, single = collect_tasks(inputs, output, suffix, append, skip_existing)
     tasks = tasks[rank::world]
-    f2b = File2Beats(model, f"cuda:{gpu}", float16, dbn)
+    f2b = File2Beats(model, f"cuda:{gpu}", float16, dbn, dbn_impl=dbn_impl)
     failed = 0
 
     def fail(src, dst, why=""):

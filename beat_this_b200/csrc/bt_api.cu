@@ -17,6 +17,7 @@
 
 #include "../../include/beatthis.h"
 #include "bt_kernels.h"
+#include "dbn_model.h"
 
 using namespace bt;
 
@@ -88,6 +89,12 @@ struct bt_ctx {
   // spectrogram scratch for bt_audio2frames
   float* spect_ws = nullptr;
   int64_t spect_cap = 0;
+  // DBN scratch for bt_dbn_track_device / bt_debug_dbn_viterbi (grows on demand): activations, densities, windows,
+  // per-model results and path codes; back pointers
+  void* dbn_ws = nullptr;
+  size_t dbn_ws_cap = 0;
+  void* dbn_bp = nullptr;
+  size_t dbn_bp_cap = 0;
   // pinned staging + device tables
   StageSlot stage[kStageSlots];
   int stage_next = 0;
@@ -854,6 +861,8 @@ void bt_destroy(bt_ctx* c) {
     if (kv.second.i32) cudaFree(kv.second.i32);
   }
   if (c->spect_ws) cudaFree(c->spect_ws);
+  if (c->dbn_ws) cudaFree(c->dbn_ws);
+  if (c->dbn_bp) cudaFree(c->dbn_bp);
   for (auto& sl : c->stage) {
     if (sl.host) cudaFreeHost(sl.host);
     if (sl.dev) cudaFree(sl.dev);
@@ -1107,6 +1116,247 @@ int bt_peakpick(bt_ctx* c, const float* beat_dev, const float* downbeat_dev, con
   launch_peakpick(beat_dev, downbeat_dev, static_cast<const int64_t*>(sl->dev), n_clips, beat_times_dev,
                   n_beats_dev, down_times_dev, n_down_dev, max_peaks, st);
   BT_LAUNCHED(c, "peakpick", st);
+  return BT_OK;
+}
+
+namespace {
+
+// One bar model as the device decodes it: the tables of DbnModelDev, checked, with the kernel's shared-memory need.
+struct DbnHostModel {
+  int32_t beats = 0, n_int = 0, per_beat = 0;
+  std::vector<int32_t> intervals, first, nrun;
+  std::vector<double> log_tempo;
+  double init = 0.0;
+  size_t smem = 0;
+};
+
+constexpr size_t kDbnStaticSmem = 512;  // dbn_viterbi_kernel's block reduction
+
+int dbn_host_model(bt_ctx* c, const char* fn, int32_t beats, int32_t n_int, const int32_t* intervals,
+                   const double* log_tempo, const int32_t* pointers, DbnHostModel& m) {
+  if (n_int < 1 || n_int > 255)
+    return fail(c, BT_ERR_ARG, "%s: %d tempi; the device decoder stores back pointers as bytes and takes 1..255 tempi", fn, n_int);
+  if (beats < 1 || beats > 127) return fail(c, BT_ERR_ARG, "%s: %d beats per bar; the device decoder takes 1..127", fn, beats);
+  if (beats * n_int > 1024)
+    return fail(c, BT_ERR_ARG, "%s: %d beats x %d tempi; the device decoder runs one thread per (beat, tempo), at most 1024",
+                fn, beats, n_int);
+  m.beats = beats;
+  m.n_int = n_int;
+  m.intervals.assign(intervals, intervals + n_int);
+  m.first.resize(n_int);
+  int64_t per_beat = 0;
+  for (int k = 0; k < n_int; ++k) {
+    if (intervals[k] <= 0) return fail(c, BT_ERR_ARG, "%s: beat intervals must be positive", fn);
+    m.first[k] = static_cast<int32_t>(per_beat);
+    per_beat += intervals[k];
+  }
+  const int64_t S = per_beat * beats;
+  m.smem = dbn_viterbi_smem(beats, n_int, static_cast<int>(std::min<int64_t>(per_beat, INT32_MAX / 256)));
+  int optin = 0;
+  BT_CUDA(c, cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, c->device));
+  if (per_beat > INT32_MAX / 256 || m.smem + kDbnStaticSmem > static_cast<size_t>(optin))
+    return fail(c, BT_ERR_ARG, "%s: a %d-beat model with %d tempi has %lld states and needs %zu bytes of shared memory; the "
+                "device allows %d per block", fn, beats, n_int, static_cast<long long>(S), m.smem + kDbnStaticSmem, optin);
+  m.per_beat = static_cast<int32_t>(per_beat);
+  // the ring form needs every (beat, tempo) to observe the (down)beat density on a leading run of positions and the
+  // "no beat" density on the rest (what BarModel::build produces)
+  m.nrun.resize(static_cast<size_t>(beats) * n_int);
+  for (int b = 0; b < beats; ++b)
+    for (int k = 0; k < n_int; ++k) {
+      const int32_t* pt = pointers + static_cast<int64_t>(b) * per_beat + m.first[k];
+      const int32_t lead = b == 0 ? 2 : 1;
+      int32_t n = 0;
+      while (n < intervals[k] && pt[n] == lead) ++n;
+      bool ok = n > 0;
+      for (int32_t p = n; p < intervals[k]; ++p) ok = ok && pt[p] == 0;
+      if (!ok)
+        return fail(c, BT_ERR_ARG, "%s: beat %d, tempo %d: the pointers are not a leading run of %d followed by 0 (the only "
+                    "form the device decoder handles)", fn, b, k, lead);
+      m.nrun[static_cast<size_t>(b) * n_int + k] = n;
+    }
+  m.log_tempo.assign(log_tempo, log_tempo + static_cast<size_t>(n_int) * n_int);
+  m.init = -std::log(static_cast<double>(S));
+  return BT_OK;
+}
+
+int dbn_grow(bt_ctx* c, void** buf, size_t* cap, size_t need) {
+  if (need <= *cap) return BT_OK;
+  if (*buf) cudaFree(*buf);  // only when the buffer grows, as spect_ws
+  *buf = nullptr;
+  *cap = 0;
+  const size_t n = need + need / 4;
+  BT_CUDA(c, cudaMalloc(buf, n));
+  *cap = n;
+  return BT_OK;
+}
+
+inline size_t align16(size_t v) { return (v + 15) & ~static_cast<size_t>(15); }
+
+// Model tables, frame offsets and (optionally) the windows of the clips through one staging slot; device pointers
+// into the slot come back.  bp_base of model i: the back pointers of the models before it, `total` frames each.
+int dbn_stage(bt_ctx* c, const std::vector<DbnHostModel>& ms, const int64_t* fo, int32_t n_clips, int64_t total,
+              const int64_t* win_host, cudaStream_t st, const DbnModelDev** models_dev, const int64_t** fo_dev,
+              const int64_t** win_dev) {
+  const int nm = static_cast<int>(ms.size());
+  size_t off = align16(sizeof(DbnModelDev) * nm);
+  const size_t o_fo = off;
+  off = align16(off + sizeof(int64_t) * (n_clips + 1));
+  const size_t o_win = off;
+  if (win_host) off = align16(off + sizeof(int64_t) * 2 * n_clips);
+  std::vector<size_t> o_lt(nm), o_iv(nm), o_first(nm), o_nrun(nm);
+  for (int i = 0; i < nm; ++i) {
+    o_lt[i] = off; off = align16(off + sizeof(double) * ms[i].log_tempo.size());
+    o_iv[i] = off; off = align16(off + sizeof(int32_t) * ms[i].n_int);
+    o_first[i] = off; off = align16(off + sizeof(int32_t) * ms[i].n_int);
+    o_nrun[i] = off; off = align16(off + sizeof(int32_t) * ms[i].nrun.size());
+  }
+  StageSlot* sl = nullptr;
+  int r = acquire_stage(c, off, &sl);
+  if (r != BT_OK) return r;
+  char* h = static_cast<char*>(sl->host);
+  char* d = static_cast<char*>(sl->dev);
+  int64_t bp_base = 0;
+  for (int i = 0; i < nm; ++i) {
+    const DbnHostModel& m = ms[i];
+    DbnModelDev md{};
+    md.intervals = reinterpret_cast<const int32_t*>(d + o_iv[i]);
+    md.first = reinterpret_cast<const int32_t*>(d + o_first[i]);
+    md.nrun = reinterpret_cast<const int32_t*>(d + o_nrun[i]);
+    md.log_tempo = reinterpret_cast<const double*>(d + o_lt[i]);
+    md.init = m.init;
+    md.bp_base = bp_base;
+    md.beats = m.beats; md.n_int = m.n_int; md.per_beat = m.per_beat;
+    bp_base += static_cast<int64_t>(m.beats) * m.n_int * total;
+    memcpy(h + sizeof(DbnModelDev) * i, &md, sizeof(md));
+    memcpy(h + o_lt[i], m.log_tempo.data(), sizeof(double) * m.log_tempo.size());
+    memcpy(h + o_iv[i], m.intervals.data(), sizeof(int32_t) * m.n_int);
+    memcpy(h + o_first[i], m.first.data(), sizeof(int32_t) * m.n_int);
+    memcpy(h + o_nrun[i], m.nrun.data(), sizeof(int32_t) * m.nrun.size());
+  }
+  memcpy(h + o_fo, fo, sizeof(int64_t) * (n_clips + 1));
+  if (win_host) memcpy(h + o_win, win_host, sizeof(int64_t) * 2 * n_clips);
+  if ((r = upload_stage(c, sl, off, st)) != BT_OK) return r;
+  *models_dev = reinterpret_cast<const DbnModelDev*>(d);
+  *fo_dev = reinterpret_cast<const int64_t*>(d + o_fo);
+  if (win_dev) *win_dev = win_host ? reinterpret_cast<const int64_t*>(d + o_win) : nullptr;
+  return BT_OK;
+}
+
+void dbn_launch_shape(const std::vector<DbnHostModel>& ms, int* threads, size_t* smem, size_t* bp_per_frame) {
+  int bn = 0;
+  *smem = 0;
+  *bp_per_frame = 0;
+  for (const auto& m : ms) {
+    bn = std::max(bn, m.beats * m.n_int);
+    *smem = std::max(*smem, m.smem);
+    *bp_per_frame += static_cast<size_t>(m.beats) * m.n_int;
+  }
+  *threads = (bn + 31) / 32 * 32;
+}
+
+}  // namespace
+
+int bt_dbn_track_device(bt_ctx* c, const float* beat_logits_dev, const float* downbeat_logits_dev,
+                        const double* activations_dev, const int64_t* frame_offsets_host, int32_t n_clips,
+                        const int32_t* beats_per_bar, int32_t n_bar_lengths, double min_bpm, double max_bpm,
+                        int32_t num_tempi, double transition_lambda, double observation_lambda, double threshold,
+                        int32_t correct, double fps, double* times_dev, int32_t* numbers_dev, int64_t* counts_dev,
+                        void* stream) {
+  if (!c) return BT_ERR_ARG;
+  const char* fn = "bt_dbn_track_device";
+  const bool logits = beat_logits_dev || downbeat_logits_dev;
+  if (logits == (activations_dev != nullptr) || (logits && !(beat_logits_dev && downbeat_logits_dev)))
+    return fail(c, BT_ERR_ARG, "%s: pass either both logit arrays or the activations", fn);
+  if (n_clips < 0 || !frame_offsets_host || !beats_per_bar || n_bar_lengths <= 0 || n_bar_lengths > 16 || !(min_bpm > 0) ||
+      !(max_bpm > min_bpm) || !(fps > 0) || !(observation_lambda > 1))
+    return fail(c, BT_ERR_ARG, "%s: bad model parameters (1..16 bar lengths, 0 < min_bpm < max_bpm, fps > 0, "
+                "observation_lambda > 1)", fn);
+  if (n_clips == 0) return BT_OK;
+  if (!times_dev || !numbers_dev || !counts_dev) return fail(c, BT_ERR_ARG, "%s: null output", fn);
+  if (frame_offsets_host[0] < 0) return fail(c, BT_ERR_ARG, "%s: negative frame offset", fn);
+  for (int i = 0; i < n_clips; ++i)
+    if (frame_offsets_host[i + 1] < frame_offsets_host[i]) return fail(c, BT_ERR_ARG, "%s: frame offsets must not decrease", fn);
+  std::vector<DbnHostModel> ms(n_bar_lengths);
+  for (int i = 0; i < n_bar_lengths; ++i) {
+    if (beats_per_bar[i] <= 0) return fail(c, BT_ERR_ARG, "%s: beats_per_bar must be positive", fn);
+    BarModel bm;
+    bm.build(beats_per_bar[i], 60.0 * fps / max_bpm, 60.0 * fps / min_bpm, num_tempi, transition_lambda, observation_lambda);
+    int r = dbn_host_model(c, fn, bm.beats, bm.n_int, bm.intervals.data(), bm.log_tempo.data(), bm.pointers.data(), ms[i]);
+    if (r != BT_OK) return r;
+  }
+  int threads;
+  size_t smem, bp_per_frame;
+  dbn_launch_shape(ms, &threads, &smem, &bp_per_frame);
+  const int64_t total = frame_offsets_host[n_clips];
+  const size_t nres = static_cast<size_t>(n_clips) * n_bar_lengths;
+  const size_t o_dens = align16(sizeof(double) * 2 * total);
+  const size_t o_win = align16(o_dens + sizeof(double) * 3 * total);
+  const size_t o_logp = align16(o_win + sizeof(int64_t) * 2 * n_clips);
+  const size_t o_state = align16(o_logp + sizeof(double) * nres);
+  const size_t o_codes = align16(o_state + sizeof(int64_t) * nres);
+  const size_t ws_bytes = o_codes + static_cast<size_t>(total);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  BT_CUDA(c, cudaSetDevice(c->device));
+  int r = dbn_grow(c, &c->dbn_ws, &c->dbn_ws_cap, ws_bytes);
+  if (r == BT_OK) r = dbn_grow(c, &c->dbn_bp, &c->dbn_bp_cap, std::max<size_t>(bp_per_frame * total, 1));
+  if (r != BT_OK) return r;
+  prof_mark(c, st);
+  const DbnModelDev* md = nullptr;
+  const int64_t* fo_dev = nullptr;
+  if ((r = dbn_stage(c, ms, frame_offsets_host, n_clips, total, nullptr, st, &md, &fo_dev, nullptr)) != BT_OK) return r;
+  char* ws = static_cast<char*>(c->dbn_ws);
+  double* act = reinterpret_cast<double*>(ws);
+  double* dens = reinterpret_cast<double*>(ws + o_dens);
+  int64_t* win = reinterpret_cast<int64_t*>(ws + o_win);
+  double* res_logp = reinterpret_cast<double*>(ws + o_logp);
+  int64_t* res_state = reinterpret_cast<int64_t*>(ws + o_state);
+  uint8_t* codes = reinterpret_cast<uint8_t*>(ws + o_codes);
+  uint8_t* bp = static_cast<uint8_t*>(c->dbn_bp);
+  launch_dbn_prep(beat_logits_dev, downbeat_logits_dev, activations_dev, fo_dev, n_clips, threshold, observation_lambda,
+                  act, dens, win, st);
+  BT_LAUNCHED(c, "dbn_prep", st);
+  if (const int e = launch_dbn_viterbi(md, n_bar_lengths, threads, smem, dens, fo_dev, win, n_clips, bp, res_logp,
+                                       res_state, st))
+    return fail(c, BT_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(static_cast<cudaError_t>(e)));
+  BT_LAUNCHED(c, "dbn_viterbi", st);
+  launch_dbn_backtrace(md, n_bar_lengths, fo_dev, win, n_clips, bp, res_logp, res_state, act, codes, correct != 0, fps,
+                       times_dev, numbers_dev, counts_dev, nullptr, nullptr, st);
+  BT_LAUNCHED(c, "dbn_backtrace", st);
+  return BT_OK;
+}
+
+int bt_debug_dbn_viterbi(bt_ctx* c, const double* log_dens_dev, int64_t T, int32_t beats, int32_t n_int,
+                         const int32_t* intervals, const double* log_tempo, const int32_t* pointers, int64_t* path_dev,
+                         double* logp_dev, void* stream) {
+  if (!c) return BT_ERR_ARG;
+  const char* fn = "bt_debug_dbn_viterbi";
+  if (!log_dens_dev || !intervals || !log_tempo || !pointers || !path_dev || !logp_dev || T <= 0)
+    return fail(c, BT_ERR_ARG, "%s: null argument or T <= 0", fn);
+  std::vector<DbnHostModel> ms(1);
+  int r = dbn_host_model(c, fn, beats, n_int, intervals, log_tempo, pointers, ms[0]);
+  if (r != BT_OK) return r;
+  int threads;
+  size_t smem, bp_per_frame;
+  dbn_launch_shape(ms, &threads, &smem, &bp_per_frame);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  BT_CUDA(c, cudaSetDevice(c->device));
+  r = dbn_grow(c, &c->dbn_ws, &c->dbn_ws_cap, 2 * sizeof(double));
+  if (r == BT_OK) r = dbn_grow(c, &c->dbn_bp, &c->dbn_bp_cap, bp_per_frame * T);
+  if (r != BT_OK) return r;
+  prof_mark(c, st);
+  const int64_t fo[2] = {0, T}, win_h[2] = {0, T};
+  const DbnModelDev* md = nullptr;
+  const int64_t *fo_dev = nullptr, *win = nullptr;
+  if ((r = dbn_stage(c, ms, fo, 1, T, win_h, st, &md, &fo_dev, &win)) != BT_OK) return r;
+  double* res_logp = static_cast<double*>(c->dbn_ws);
+  int64_t* res_state = reinterpret_cast<int64_t*>(res_logp + 1);
+  uint8_t* bp = static_cast<uint8_t*>(c->dbn_bp);
+  if (const int e = launch_dbn_viterbi(md, 1, threads, smem, log_dens_dev, fo_dev, win, 1, bp, res_logp, res_state, st))
+    return fail(c, BT_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(static_cast<cudaError_t>(e)));
+  BT_LAUNCHED(c, "dbn_viterbi", st);
+  launch_dbn_backtrace(md, 1, fo_dev, win, 1, bp, res_logp, res_state, nullptr, nullptr, 0, 1.0, nullptr, nullptr, nullptr,
+                       path_dev, logp_dev, st);
+  BT_LAUNCHED(c, "dbn_backtrace", st);
   return BT_OK;
 }
 

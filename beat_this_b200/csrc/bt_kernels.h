@@ -93,6 +93,41 @@ void launch_logmel(const float* audio, const int64_t* sample_off_dev, const int6
 void launch_peakpick(const float* beat, const float* down, const int64_t* frame_off_dev, int n_clips,
                      double* beat_t, int32_t* n_beat, double* down_t, int32_t* n_down,
                      int max_peaks, cudaStream_t st);
+// ---- DBN post-processor on the device (kernels_dbn.cu) ---------------------------------------------------------
+// One bar model of the bar-pointer HMM (dbn_model.h BarModel), tables on the device.  State s = b * per_beat +
+// first[k] + p (beat b, tempo k, position p < intervals[k]); positions p < nrun[b * n_int + k] observe the (down)beat
+// density, all others the "no beat" one.
+struct DbnModelDev {
+  const int32_t* intervals;  // [n_int]
+  const int32_t* first;      // [n_int]
+  const int32_t* nrun;       // [beats * n_int]
+  const double* log_tempo;   // [n_int * n_int], row = previous tempo
+  double init;               // initial value of every state, -log(S) as the host computes it
+  int64_t bp_base;           // this model's back pointers: bp[bp_base + frame * beats * n_int + b * n_int + k]
+  int32_t beats, n_int, per_beat, pad_;
+};
+// Per clip (frame offsets fo_dev): act [frames][2] float64 activations (from the fp32 logit pair, or copied from
+// act_in when it is non-null), dens [frames][3] log densities (no beat, beat, downbeat), win[clip] = {first frame,
+// frames to decode} of the threshold window (0 frames: no beats).
+void launch_dbn_prep(const float* beat, const float* down, const double* act_in, const int64_t* fo_dev, int n_clips,
+                     double threshold, double observation_lambda, double* act, double* dens, int64_t* win,
+                     cudaStream_t st);
+// dynamic shared memory of dbn_viterbi for one model
+size_t dbn_viterbi_smem(int beats, int n_int, int per_beat);
+// Viterbi of every (clip, model): back pointers into bp, res_logp / res_state [clip * n_models + model] = log-probability
+// and final state of the best path.  threads >= max beats * n_int (multiple of 32), smem >= max dbn_viterbi_smem.
+// Returns a cudaError_t.
+int launch_dbn_viterbi(const DbnModelDev* models_dev, int n_models, int threads, size_t smem, const double* dens,
+                       const int64_t* fo_dev, const int64_t* win, int n_clips, uint8_t* bp, double* res_logp,
+                       int64_t* res_state, cudaStream_t st);
+// Best model, backtrace and beats of every clip: (time, number) pairs at times / numbers + fo[clip], counts[clip]
+// (codes: one byte per frame of scratch).  With path_out non-null (one clip, one model) it writes the state path and
+// *logp_out instead.
+void launch_dbn_backtrace(const DbnModelDev* models_dev, int n_models, const int64_t* fo_dev, const int64_t* win,
+                          int n_clips, const uint8_t* bp, const double* res_logp, const int64_t* res_state,
+                          const double* act, uint8_t* codes, int correct, double fps, double* times, int32_t* numbers,
+                          int64_t* counts, int64_t* path_out, double* logp_out, cudaStream_t st);
+
 void launch_f32_to_h16(const float* in, void* out, int64_t n, cudaStream_t st);
 void launch_h16_to_f32(const void* in, float* out, int64_t n, cudaStream_t st);
 // [seqs, L, heads*32] fp32 q,k,v -> packed qkv buffer [seqs*L, 3C] of the activation dtype

@@ -150,6 +150,11 @@ class DBNDownBeatTracker:
         self.models = [_BarModel(b, min_interval, max_interval, num_tempi, transition_lambda, observation_lambda)
                        for b in np.atleast_1d(beats_per_bar)]
 
+    @property
+    def track_params(self) -> dict:
+        """Every tracker parameter of bt_dbn_track / bt_dbn_track_device: `params` plus threshold, correct and fps."""
+        return dict(self.params, threshold=float(self.threshold or 0.0), correct=bool(self.correct), fps=self.fps)
+
     def __call__(self, activations):
         """activations [T, 2] = (beat-but-not-downbeat, downbeat) probabilities -> [[time_s, beat_number], ...]."""
         if _native() is not None:
@@ -181,10 +186,10 @@ class DBNDownBeatTracker:
         numbers = np.empty(total, dtype=np.int32)
         counts = np.zeros(max(n, 1), dtype=np.int64)
         bpb = np.asarray(self.params["beats_per_bar"], dtype=np.int32)
-        p = self.params
+        p = self.track_params
         code = lib.bt_dbn_track(cat.ctypes.data, fo.ctypes.data, n, bpb.ctypes.data, len(bpb), p["min_bpm"], p["max_bpm"],
-                                p["num_tempi"], p["transition_lambda"], p["observation_lambda"], float(self.threshold or 0.0),
-                                int(bool(self.correct)), self.fps, int(n_threads), times.ctypes.data, numbers.ctypes.data,
+                                p["num_tempi"], p["transition_lambda"], p["observation_lambda"], p["threshold"],
+                                int(p["correct"]), p["fps"], int(n_threads), times.ctypes.data, numbers.ctypes.data,
                                 counts.ctypes.data)
         if code != 0:
             raise RuntimeError(f"bt_dbn_track failed ({code})")

@@ -41,6 +41,29 @@ class _PeakHandle:
         return self.slot["times_h"].numel() * 8 + self.slot["cnt_h"].numel() * 4
 
 
+class _DbnHandle:
+    def __init__(self, slot, frame_offsets):
+        self.slot, self.fo = slot, frame_offsets
+
+    def result(self):
+        self.slot["event"].synchronize()
+        n = len(self.fo) - 1
+        cnt = self.slot["counts_h"].numpy()
+        times = self.slot["times_h"].numpy()
+        numbers = self.slot["numbers_h"].numpy()
+        out = []
+        for i in range(n):  # as Postprocessor.batch_host splits the tracker's [n, 2] result
+            a, k = self.fo[i], int(cnt[i])
+            t = times[a : a + k].copy()
+            out.append((t, t[numbers[a : a + k] == 1]))
+        self.slot["keep"] = None
+        return out
+
+    @property
+    def d2h_bytes(self):
+        return (len(self.fo) - 1) * 8 + (self.fo[-1] if self.fo else 0) * 12
+
+
 class Engine:
     def __init__(self, packed: dict | None, hparams: dict | None, device="cuda", half: bool = False, wave_chunks: int | None = None):
         self.lib = _lib.load()
@@ -252,6 +275,72 @@ class Engine:
         slot["event"].record(torch.cuda.current_stream(self.device))
         slot["keep"] = (beat, down)  # keep the logits alive until the kernels have run
         return _PeakHandle(slot, n)
+
+    def _dbn_enqueue(self, beat, down, act, frame_offsets, params: dict, times, numbers, counts):
+        bpb = np.ascontiguousarray(params["beats_per_bar"], dtype=np.int32)
+        ptr = lambda t: None if t is None else c_void_p(t.data_ptr())  # noqa: E731
+        code = self.lib.bt_dbn_track_device(
+            self.ctx, ptr(beat), ptr(down), ptr(act), i64_array(frame_offsets), len(frame_offsets) - 1,
+            c_void_p(bpb.ctypes.data), len(bpb), float(params["min_bpm"]), float(params["max_bpm"]), int(params["num_tempi"]),
+            float(params["transition_lambda"]), float(params["observation_lambda"]), float(params["threshold"]),
+            int(bool(params["correct"])), float(params["fps"]), ptr(times), ptr(numbers), ptr(counts), self._stream())
+        _lib.check(self.lib, self.ctx, code)
+
+    def dbn_async(self, beat: torch.Tensor | None, down: torch.Tensor | None, frame_offsets, slot: dict | None = None,
+                  params: dict | None = None, activations: torch.Tensor | None = None):
+        """Postprocessor("dbn") on the device (bt_dbn_track_device) for concatenated fp32 logits -- or, with
+        `activations`, a [total, 2] float64 device tensor of (beat-but-not-downbeat, downbeat) probabilities -- without
+        a host synchronisation: (time, beat number) pairs and counts are copied to pinned host memory on the current
+        stream.  params: the tracker parameters (dbn.DBNDownBeatTracker.track_params).  ``.result()`` on the handle
+        gives a list of (beat_times, downbeat_times)."""
+        n = len(frame_offsets) - 1
+        total = int(frame_offsets[-1]) if n > 0 else 0
+        slot = slot if slot is not None else {}
+        cap = max(total, 1)
+        if slot.get("cap", -1) < cap or slot.get("n", -1) < n:
+            cap = max(cap, slot.get("cap", 0))
+            nn = max(n, slot.get("n", 0), 1)
+            slot["cap"], slot["n"] = cap, nn
+            slot["times"] = torch.empty(cap, dtype=torch.float64, device=self.device)
+            slot["numbers"] = torch.empty(cap, dtype=torch.int32, device=self.device)
+            slot["counts"] = torch.zeros(nn, dtype=torch.int64, device=self.device)
+            slot["times_h"] = torch.empty(cap, dtype=torch.float64).pin_memory()
+            slot["numbers_h"] = torch.empty(cap, dtype=torch.int32).pin_memory()
+            slot["counts_h"] = torch.empty(nn, dtype=torch.int64).pin_memory()
+            slot["event"] = torch.cuda.Event()
+        if activations is not None:
+            assert activations.is_cuda and activations.dtype == torch.float64 and activations.is_contiguous()
+        else:
+            assert beat.is_cuda and beat.dtype == torch.float32 and beat.is_contiguous()
+            assert down.is_cuda and down.dtype == torch.float32 and down.is_contiguous()
+        self._dbn_enqueue(beat, down, activations, frame_offsets, params, slot["times"], slot["numbers"], slot["counts"])
+        if n > 0:
+            slot["times_h"][:total].copy_(slot["times"][:total], non_blocking=True)
+            slot["numbers_h"][:total].copy_(slot["numbers"][:total], non_blocking=True)
+            slot["counts_h"][:n].copy_(slot["counts"][:n], non_blocking=True)
+        slot["event"].record(torch.cuda.current_stream(self.device))
+        slot["keep"] = (beat, down, activations)  # keep the inputs alive until the kernels have run
+        return _DbnHandle(slot, [int(v) for v in frame_offsets])
+
+    def dbn_cat(self, beat, down, frame_offsets, params: dict, activations=None):
+        """Synchronous dbn_async: list of (beat_times, downbeat_times) float64 numpy arrays, one pair per clip."""
+        return self.dbn_async(beat, down, frame_offsets, None, params, activations).result()
+
+    def debug_dbn_viterbi(self, log_dens: torch.Tensor, beats: int, intervals, log_tempo, pointers):
+        """bt_debug_dbn_viterbi: the device Viterbi of one bar model on float64 log densities [T, 3] (device tensor);
+        model tables as bt_dbn_viterbi takes them (host arrays).  Returns (path int64 numpy array, logp float)."""
+        assert log_dens.is_cuda and log_dens.dtype == torch.float64 and log_dens.is_contiguous()
+        T = log_dens.shape[0]
+        iv = np.ascontiguousarray(intervals, dtype=np.int32)
+        lt = np.ascontiguousarray(log_tempo, dtype=np.float64)
+        pt = np.ascontiguousarray(pointers, dtype=np.int32)
+        path = torch.empty(max(T, 1), dtype=torch.int64, device=self.device)
+        logp = torch.empty(1, dtype=torch.float64, device=self.device)
+        code = self.lib.bt_debug_dbn_viterbi(self.ctx, c_void_p(log_dens.data_ptr()), T, int(beats), len(iv),
+                                             c_void_p(iv.ctypes.data), c_void_p(lt.ctypes.data), c_void_p(pt.ctypes.data),
+                                             c_void_p(path.data_ptr()), c_void_p(logp.data_ptr()), self._stream())
+        _lib.check(self.lib, self.ctx, code)
+        return path[:T].cpu().numpy(), float(logp.item())
 
     # ---- per-kernel-class timing (bench.py roofline) -------------------------------------------
     def profile_enable(self, on: bool = True):

@@ -318,19 +318,22 @@ class Audio2Beats(Audio2Frames):
     """Beat / downbeat positions in seconds from an audio signal (reference
     inference.py:284-303)."""
 
-    def __init__(self, checkpoint_path="final0", device="cuda", float16=False, dbn=False, resampler="device"):
+    def __init__(self, checkpoint_path="final0", device="cuda", float16=False, dbn=False, resampler="device",
+                 dbn_impl="auto"):
         super().__init__(checkpoint_path, device, float16, resampler)
-        self._init_post(dbn)
+        self._init_post(dbn, dbn_impl)
 
-    def _init_post(self, dbn=False):
-        self.frames2beats = Postprocessor(type="dbn" if dbn else "minimal", engine=self.model.engine)
+    def _init_post(self, dbn=False, dbn_impl="auto"):
+        """dbn_impl (with dbn=True): "auto" (madmom if installed, else the host C++ tracker), "madmom", "native" (the
+        host C++ tracker) or "device" (the same tracker on the GPU, see Postprocessor)."""
+        self.frames2beats = Postprocessor(type="dbn" if dbn else "minimal", engine=self.model.engine, dbn_impl=dbn_impl)
 
     def __call__(self, signal, sr):
         return Audio2Beats.batch(self, [signal], sr)[0]
 
     def _finish(self, res):
         """pipeline result of one group -> list of (beat_times, downbeat_times)."""
-        if self.frames2beats.type == "minimal":
+        if self.frames2beats.type == "minimal" or self.frames2beats.on_device:
             return res
         import time
 
@@ -342,16 +345,26 @@ class Audio2Beats(Audio2Frames):
         return out
 
     @property
+    def pipeline(self) -> BeatPipeline:
+        pipe = super().pipeline
+        if self.frames2beats.on_device:
+            pipe.dbn_params = self.frames2beats.dbn_params
+        return pipe
+
+    @property
     def _want_beats(self):
-        return "beats" if self.frames2beats.type == "minimal" else "logits_host"
+        if self.frames2beats.type == "minimal":
+            return "beats"
+        return "dbn_device" if self.frames2beats.on_device else "logits_host"
 
     def batch(self, signals, sr=22050):
-        """list of signals -> list of (beat_times, downbeat_times) numpy float64 arrays.  With the DBN, the host
-        Viterbi of group g runs while the GPU works on group g+1."""
+        """list of signals -> list of (beat_times, downbeat_times) numpy float64 arrays.  With the host DBN, the host
+        Viterbi of group g runs while the GPU works on group g+1; the device DBN runs on the compute stream after the
+        forward pass of its group, like the peak picker."""
         arrays, sr = self._prepare(signals, sr)
         out = [None] * len(arrays)
-        if self.frames2beats.type == "minimal":
-            for lo, hi, res in self._run_groups(arrays, sr, "beats"):
+        if self.frames2beats.type == "minimal" or self.frames2beats.on_device:
+            for lo, hi, res in self._run_groups(arrays, sr, self._want_beats):
                 out[lo:hi] = res
             return out
         # DBN: the host Viterbi of a group runs on a worker thread (numpy and the C++ tracker release the GIL), so the

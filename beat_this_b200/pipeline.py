@@ -7,7 +7,8 @@ one pass of every kernel); for every group
   host threads   mono mix + fp32 cast of all clips straight into a pinned ring slot (``bt_stage_audio`` /
                  ``bt_stage_wav_files``: C++, GIL released)
   copy stream    one H2D copy of the slot
-  compute stream log-mel -> BeatThis forward -> (peak picking -> D2H of the timestamps | D2H of the logits for the DBN)
+  compute stream log-mel -> BeatThis forward -> (peak picking | device DBN -> D2H of the timestamps
+                 | D2H of the logits for the host DBN)
 
 and group g+1 is staged and copied while the kernels of group g run; results are collected in order.  Nothing in the
 enqueue path waits for the GPU (the C library keeps its small tables in a ring of pinned slots), so the device queue
@@ -68,6 +69,7 @@ class _Slot:
         self.dev = None       # device copy
         self.copied = None
         self.peak = {}        # reusable buffers of Engine.peakpick_async
+        self.dbn = {}         # reusable buffers of Engine.dbn_async
         self.logits_h = None  # pinned logits (DBN path)
         self.done = None
         self.t0 = None        # events around the group's kernels (stats: GPU busy time)
@@ -101,6 +103,7 @@ class BeatPipeline:
         self.host_threads = int(host_threads)
         self.h2d_bytes = 0
         self.d2h_bytes = 0
+        self.dbn_params = None  # tracker parameters of want="dbn_device" (Postprocessor.dbn_params)
         # host seconds spent staging (mono mix / decode into pinned memory), enqueueing and waiting for results
         self.stats = {"stage_s": 0.0, "enqueue_s": 0.0, "collect_wait_s": 0.0, "gpu_busy_s": 0.0, "groups": 0}
 
@@ -152,6 +155,12 @@ class BeatPipeline:
             beat, down, fo = eng.audio2frames_cat(audio, offs)
             if want == "beats":
                 handle = eng.peakpick_async(beat, down, fo, s.peak)
+                self.d2h_bytes += handle.d2h_bytes
+                payload = ("beats", handle)
+            elif want == "dbn_device":  # the DBN on the compute stream: no logits leave the device, no host thread
+                if self.dbn_params is None:
+                    raise RuntimeError('want="dbn_device" needs BeatPipeline.dbn_params')
+                handle = eng.dbn_async(beat, down, fo, s.dbn, self.dbn_params)
                 self.d2h_bytes += handle.d2h_bytes
                 payload = ("beats", handle)
             elif want == "logits_host":
@@ -219,7 +228,7 @@ class BeatPipeline:
 
     # ---- results ----------------------------------------------------------------------------------
     def collect(self):
-        """Oldest group: list of (beat_times, downbeat_times) ["beats"], (beat, down, fo) host arrays
+        """Oldest group: list of (beat_times, downbeat_times) ["beats", "dbn_device"], (beat, down, fo) host arrays
         ["logits_host"] or device tensors ["frames"]."""
         idx, (kind, p) = self.inflight.popleft()
         t0 = time.perf_counter()

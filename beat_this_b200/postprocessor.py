@@ -5,7 +5,9 @@ downbeat snapping and ``np.unique`` all run in one device kernel (``bt_peakpick`
 final timestamp arrays come back to the host.  ``type="dbn"``: the DBN stays on the host as in the
 reference (postprocessor.py:138-173): madmom's ``DBNDownBeatTrackingProcessor`` when madmom is
 installed (exactly the reference's object), otherwise the restatement of its published algorithm in
-``beat_this_b200/dbn.py`` (parity with madmom unpinned); ``dbn_impl`` forces one of the two.
+``beat_this_b200/dbn.py`` (parity with madmom unpinned); ``dbn_impl`` forces one of the two ("madmom", "native").
+``dbn_impl="device"`` decodes on the GPU instead (``bt_dbn_track_device``: sigmoid, clamps, Viterbi and beat
+correction in three kernels, pinned to the host C++ tracker); only the beat times come back to the host.
 """
 from __future__ import annotations
 
@@ -18,8 +20,9 @@ import torch
 class Postprocessor:
     def __init__(self, type: str = "minimal", fps: int = 50, engine=None, device="cuda", dbn_impl: str = "auto"):
         assert type in ["minimal", "dbn"]
-        assert dbn_impl in ["auto", "madmom", "native"]
+        assert dbn_impl in ["auto", "madmom", "native", "device"]
         self.type = type
+        self.dbn_impl = dbn_impl
         self.fps = fps
         if fps != 50:
             raise NotImplementedError("the device peak picker is built for the reference's 50 fps")
@@ -77,13 +80,32 @@ class Postprocessor:
             return self.engine.peakpick_cat(beat, downbeat, frame_offsets)
         return self._postp_dbn(beat, downbeat, frame_offsets)
 
+    @property
+    def on_device(self) -> bool:
+        """True when the DBN runs on the GPU (dbn_impl="device")."""
+        return self.type == "dbn" and self.dbn_impl == "device"
+
+    @property
+    def dbn_params(self) -> dict:
+        """Tracker parameters of the device DBN (dbn.DBNDownBeatTracker.track_params)."""
+        return self.dbn.track_params
+
     def _postp_dbn(self, beat, downbeat, frame_offsets):
+        if self.on_device:
+            beat = beat.to(self.engine.device, torch.float32).contiguous()
+            downbeat = downbeat.to(self.engine.device, torch.float32).contiguous()
+            return self.engine.dbn_cat(beat, downbeat, frame_offsets, self.dbn_params)
         return self.batch_host(beat.float().cpu().numpy(), downbeat.float().cpu().numpy(), frame_offsets)
 
     def batch_host(self, beat_logits: np.ndarray, downbeat_logits: np.ndarray, frame_offsets):
         """DBN post-processing of concatenated host logits (reference postprocessor.py:138-173, float64 on the host):
         list of (beat_times, downbeat_times)."""
         assert self.type == "dbn"
+        if self.on_device:  # fp32 logits, as the model produces them
+            dev = self.engine.device
+            beat = torch.as_tensor(np.ascontiguousarray(beat_logits), dtype=torch.float32).to(dev)
+            down = torch.as_tensor(np.ascontiguousarray(downbeat_logits), dtype=torch.float32).to(dev)
+            return self.engine.dbn_cat(beat, down, frame_offsets, self.dbn_params)
         eps = 1e-5
         # beat.double().sigmoid() with the reference's own torch op (postprocessor.py:139-140) -- on ONE thread: a
         # 100 k element op gains nothing from torch's intra-op pool, and waking a 128-thread pool costs tens of ms

@@ -213,6 +213,28 @@ int bt_peakpick(bt_ctx* ctx, const float* beat_dev, const float* downbeat_dev,
                 int32_t* n_beats_dev, double* down_times_dev, int32_t* n_down_dev,
                 int32_t max_peaks, void* stream);
 
+/* Postprocessor("dbn") (model/postprocessor.py:138-173) on the device: the decoder of bt_dbn_track, pinned to it (the
+ * same arithmetic, operation for operation, and the same tie-breaks), as three kernels (dbn_prep, dbn_viterbi,
+ * dbn_backtrace).  Input is either the fp32 logit pair (sigmoid and clamps of postprocessor.py:139-167 computed on the
+ * device in float64) or activations_dev [total][2] float64 as bt_dbn_track takes them; exactly one of the two forms
+ * is non-NULL.  Model parameters and the output layout as bt_dbn_track (times/numbers at frame_offsets[i],
+ * counts_dev[i]), all on the device.  BT_ERR_ARG, before anything is enqueued, for a model with more than 255 tempi or
+ * one whose state space does not fit in the device's shared memory (one CTA holds every state of one bar model).
+ * Works on a weight-less ctx.  Enqueues only: no synchronisation (a scratch buffer that has to grow is reallocated). */
+int bt_dbn_track_device(bt_ctx* ctx, const float* beat_logits_dev, const float* downbeat_logits_dev,
+                        const double* activations_dev, const int64_t* frame_offsets_host, int32_t n_clips,
+                        const int32_t* beats_per_bar, int32_t n_bar_lengths, double min_bpm, double max_bpm,
+                        int32_t num_tempi, double transition_lambda, double observation_lambda,
+                        double threshold, int32_t correct, double fps,
+                        double* times_dev, int32_t* numbers_dev, int64_t* counts_dev, void* stream);
+
+/* Test hook: the device Viterbi alone, same arguments and meaning as bt_dbn_viterbi (log_dens and the outputs on the
+ * device, the model tables on the host).  The pointer table must have the form BarModel builds: in every (beat, tempo)
+ * a leading run of 2 (first beat of the bar) or 1 (other beats) followed by 0; anything else is BT_ERR_ARG. */
+int bt_debug_dbn_viterbi(bt_ctx* ctx, const double* log_dens_dev, int64_t T, int32_t beats, int32_t n_int,
+                         const int32_t* intervals, const double* log_tempo, const int32_t* pointers,
+                         int64_t* path_dev, double* logp_dev, void* stream);
+
 /* ---- introspection / tuning ----------------------------------------------------------------- */
 
 /* Upper bound on the chunks processed per wave (default 128; one wave = one launch of every
