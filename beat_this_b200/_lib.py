@@ -130,7 +130,6 @@ PROTOTYPES = {
         [c_void_p, POINTER(bt_debug_gemm_desc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64,
          c_void_p, c_void_p, POINTER(c_int32), c_void_p],
     ),
-    "bt_debug_attention_time": (c_int, [c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p]),
     "bt_debug_attention": (
         c_int,
         [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, POINTER(c_int32), c_int32,

@@ -30,18 +30,18 @@ struct Param {
   int64_t n = 0;
 };
 
-struct AttnW { const Param *wqkv, *wg, *bg, *wout; };
-struct FfW { const Param *w1, *b1, *w2, *b2; };
-// every parameter the forward pass touches, resolved once in bt_finalize (no name lookups per launch)
-struct ModelW {
-  const Param *rope_cos = nullptr, *rope_sin = nullptr, *bn1_scale = nullptr, *bn1_shift = nullptr, *stem_w = nullptr,
-              *stem_b = nullptr, *lin_w = nullptr, *lin_b = nullptr, *head_w = nullptr, *head_b = nullptr;
-  AttnW fa[3]{}, ta[3]{};
-  FfW ff_f[3]{}, ff_t[3]{};
-  const Param *conv_w[3] = {nullptr, nullptr, nullptr}, *conv_b[3] = {nullptr, nullptr, nullptr};
-  std::vector<AttnW> la;
-  std::vector<FfW> lf;
+// One layer of the forward pass between the stem and the head.  bt_finalize builds the list from bt_hparams, in schedule
+// order: b{i}.attnF, b{i}.ffF, b{i}.attnT, b{i}.ffT (with partial transformers), b{i}.conv for i < 3, lin, then
+// l{l}.attn, l{l}.ff for every main layer.
+enum LayerKind { kAttnF, kAttnT, kAttn, kFf, kConv, kLin };  // kAttnF / kAttnT: frequency / time attention of a frontend block
+struct Layer {
+  LayerKind kind;
+  std::string name;  // parameter prefix, and the tap name of the layer's output (frontend.linear: "frontend")
+  int C, F;          // channels; frequency planes per chunk (1 in the main layers)
+  int mult;          // FFN hidden width multiplier
+  const Param* w[4]; // resolved weights, in the order of layer_params
 };
+
 // small host -> device tables (offsets, chunk descriptors) travel through a ring of pinned slots: a slot is only
 // waited for when it comes round again, kStageSlots uploads later, so no API call blocks on earlier GPU work
 constexpr int kStageSlots = 16;
@@ -53,16 +53,15 @@ struct StageSlot {
   bool pending = false;
 };
 
-// tensor-core plans for one (wave size, chunk length) geometry
-struct AttnPlans { TcGemmPlan *qkv = nullptr, *out = nullptr, *gates = nullptr; TcAttnPlan* attn = nullptr; TcQkvPlan* fqkv = nullptr; };
-struct FfPlans { TcGemmPlan *ff1 = nullptr, *ff2 = nullptr; TcFfPlan *fused = nullptr, *fused_op = nullptr; };
-struct WavePlans {
-  AttnPlans fa[3], ta[3];
-  FfPlans ff_f[3], ff_t[3];
-  TcGemmPlan* conv[3] = {nullptr, nullptr, nullptr};
-  TcGemmPlan* lin = nullptr;
-  std::vector<AttnPlans> la;
-  std::vector<FfPlans> lf;
+// Tensor-core plans of one layer for one (wave size, chunk length) geometry: what its launches use, nothing else.
+struct LayerPlans {
+  TcQkvPlan* fqkv = nullptr;                                    // attention, fused (C = 32 / 64)
+  TcGemmPlan *gates = nullptr, *qkv = nullptr, *out = nullptr;  // attention: gates and QKV unless fused; out-projection
+  TcAttnPlan* attn = nullptr;                                   // time attention
+  TcFreqPlan* freq = nullptr;                                   // frequency attention
+  TcFfPlan *ff = nullptr, *ff_op = nullptr;                     // FFN, fused; ff_op: after a frontend attention
+  TcGemmPlan *ff1 = nullptr, *ff2 = nullptr;                    // FFN, unfused
+  TcGemmPlan* gemm = nullptr;                                   // convolution, frontend.linear
 };
 
 char g_create_error[512] = "";
@@ -78,8 +77,6 @@ struct bt_ctx {
   mutable char err[1024] = "";
   int64_t launches = 0;
   bool sync_debug = false;
-  bool fuse_ff = true;  // BT_FUSE_FF=0 falls back to norm + two GEMMs for the narrow frontend FFNs
-  bool fuse_outproj = true;  // BT_FUSE_OUTPROJ=0: separate attention out-projection GEMM in front of the fused FFN
 
   // workspace: sized for ws_wave chunks of BT_CHUNK frames; grows on demand up to `wave`
   int wave = 128;
@@ -98,9 +95,12 @@ struct bt_ctx {
   // pinned staging + device tables
   StageSlot stage[kStageSlots];
   int stage_next = 0;
-  ModelW mw;
+  std::vector<Layer> layers;  // built by bt_finalize
+  // parameters outside the layer list, resolved in bt_finalize
+  const Param *rope_cos = nullptr, *rope_sin = nullptr, *bn1_scale = nullptr, *bn1_shift = nullptr, *stem_w = nullptr,
+              *stem_b = nullptr, *head_w = nullptr, *head_b = nullptr;
 
-  std::map<std::pair<int, int>, WavePlans*> plans;
+  std::map<std::pair<int, int>, std::vector<LayerPlans>> plans;  // parallel to `layers`
   std::vector<std::pair<int, int>> plan_order;  // insertion order: oldest geometry is evicted first
 
   // per-kernel-class device timing (bt_profile_*): one event after every launch; the
@@ -252,32 +252,21 @@ void free_ws(bt_ctx* c) {
   c->ws_wave = 0;
 }
 
-void destroy_wave_plans(WavePlans* w) {
-  auto fa = [](AttnPlans& a) {
-    if (a.qkv) tc_gemm_plan_destroy(a.qkv);
-    if (a.out) tc_gemm_plan_destroy(a.out);
-    if (a.gates) tc_gemm_plan_destroy(a.gates);
-    if (a.fqkv) tc_qkv_plan_destroy(a.fqkv);
-    if (a.attn) tc_attn_plan_destroy(a.attn);
-  };
-  auto ff = [](FfPlans& f) {
-    if (f.fused) tc_ff_plan_destroy(f.fused);
-    if (f.fused_op) tc_ff_plan_destroy(f.fused_op);
-    if (f.ff1) tc_gemm_plan_destroy(f.ff1);
-    if (f.ff2) tc_gemm_plan_destroy(f.ff2);
-  };
-  for (int i = 0; i < 3; ++i) {
-    fa(w->fa[i]); fa(w->ta[i]); ff(w->ff_f[i]); ff(w->ff_t[i]);
-    if (w->conv[i]) tc_gemm_plan_destroy(w->conv[i]);
+void destroy_plans(std::vector<LayerPlans>& v) {
+  for (LayerPlans& p : v) {
+    if (p.fqkv) tc_qkv_plan_destroy(p.fqkv);
+    for (TcGemmPlan* g : {p.gates, p.qkv, p.out, p.ff1, p.ff2, p.gemm})
+      if (g) tc_gemm_plan_destroy(g);
+    if (p.attn) tc_attn_plan_destroy(p.attn);
+    if (p.freq) tc_freq_plan_destroy(p.freq);
+    if (p.ff) tc_ff_plan_destroy(p.ff);
+    if (p.ff_op) tc_ff_plan_destroy(p.ff_op);
   }
-  if (w->lin) tc_gemm_plan_destroy(w->lin);
-  for (auto& a : w->la) fa(a);
-  for (auto& f : w->lf) ff(f);
-  delete w;
+  v.clear();
 }
 
 void free_plans(bt_ctx* c) {
-  for (auto& kv : c->plans) destroy_wave_plans(kv.second);
+  for (auto& kv : c->plans) destroy_plans(kv.second);
   c->plans.clear();
   c->plan_order.clear();
 }
@@ -364,75 +353,91 @@ EpiParams epi_generic(const Param* bias, int gelu, const float* resid, int ldr, 
   return e;
 }
 
-// x += attention(x) over `planes` planes of L tokens with dim C (reference roformer.py:114-132).
-// freq == true: sequences run over the F planes of each chunk (PartialFTTransformer attnF).
-// skip_out: the out-projection + residual are done by the following fused FFN kernel (fused_ff_kernel<C, true>).
-int attention_block(bt_ctx* c, float* X, int planes, int L, int C, int F, bool freq, const AttnW& w,
-                    AttnPlans* tp, int nb, cudaStream_t st, bool skip_out = false, const ChunkSrc* vl_chunks = nullptr) {
+bool is_attention(const Layer& l) { return l.kind == kAttnF || l.kind == kAttnT || l.kind == kAttn; }
+
+// sub-blocks of width C = 32 / 64 (the first two frontend blocks) run as one fused kernel each on the 16-bit path
+bool fused(const Layer& l) { return (l.C == 32 || l.C == 64) && (l.kind != kFf || l.mult == 4); }
+
+// The out-projection + residual of attention layer i run inside the fused FFN after it (fused_ff_kernel<C, true>),
+// unless a tap asks to see the residual stream between the two.
+bool outproj_in_ff(const bt_ctx* c, const std::vector<LayerPlans>* wp, size_t i) {
+  return wp && i + 1 < wp->size() && (*wp)[i + 1].ff_op && c->tap_name != c->layers[i].name;
+}
+
+// x += attention(x) over nb * F planes of L tokens with dim C (reference roformer.py:114-132).
+// kAttnF: sequences run over the F planes of each chunk (PartialFTTransformer attnF).
+int attention_block(bt_ctx* c, float* X, const Layer& l, const LayerPlans* tp, int nb, int L, bool out_in_ff,
+                    const ChunkSrc* vl_chunks, cudaStream_t st) {
   const bool tc = c->dtype == BT_DTYPE_H16;
-  const int heads = C / kHeadDim;
+  const bool freq = l.kind == kAttnF, front = l.F > 1;
+  const int C = l.C, F = l.F, heads = C / kHeadDim, planes = nb * F;
+  const Param *wqkv = l.w[0], *wg = l.w[1], *bg = l.w[2], *wout = l.w[3];
   const int64_t M = static_cast<int64_t>(planes) * L;
   const float inv_sqrt_d = 0.17677669529663687f;  // 1/sqrt(32): SDPA default scale (roformer.py:78-80)
-  const bool tc_time = tc && !freq;
-  const float qscale = tc_time ? inv_sqrt_d * 1.4426950408889634f : 1.0f;
+  const float qscale = tc && !freq ? inv_sqrt_d * 1.4426950408889634f : 1.0f;
   int r = BT_OK;
-  if (tc && tp && tp->fqkv) {  // narrow frontend attentions: norm + gates + QKV + RoPE in one kernel
-    if (launch_fused_qkv(tp->fqkv, X, w.wg->f32, w.bg->f32, c->mw.rope_cos->f32, c->mw.rope_sin->f32,
-                         c->QKV, c->GATES, L, F, freq ? 1 : 0, qscale, st) != 0)
+  if (tc && fused(l)) {  // norm + gates + QKV + RoPE in one kernel
+    if (launch_fused_qkv(tp->fqkv, X, wg->f32, bg->f32, c->rope_cos->f32, c->rope_sin->f32, c->QKV, c->GATES, L, F,
+                         freq ? 1 : 0, qscale, st) != 0)
       return fail(c, BT_ERR_CUDA, "fused qkv launch failed");
     BT_LAUNCHED(c, C == 32 ? "qkv_fused_c32" : "qkv_fused_c64", st);
   } else {
-    // heads 1/2 (unfused fallback of blocks 0/1): gates inside the norm kernel; heads >= 4: padded gates GEMM
-    static const int gin_max = getenv("BT_GATES_IN_NORM_MAX") ? atoi(getenv("BT_GATES_IN_NORM_MAX")) : 2;
-    const bool gates_in_norm = heads <= gin_max;
-    launch_norm(X, c->XN, M, C, tc, st, gates_in_norm ? c->GATES : nullptr, w.wg->f32, w.bg->f32, heads);
-    BT_LAUNCHED(c, gates_in_norm ? "norm_gates" : (F > 1 ? "norm_front" : "norm"), st);
+    // up to 2 heads (fp32 path only: the 16-bit path fuses those blocks): gates inside the norm kernel;
+    // otherwise from a padded gates GEMM
+    const bool gates_in_norm = heads <= 2;
+    launch_norm(X, c->XN, M, C, tc, st, gates_in_norm ? c->GATES : nullptr, wg->f32, bg->f32, heads);
+    BT_LAUNCHED(c, gates_in_norm ? "norm_gates" : (front ? "norm_front" : "norm"), st);
     if (!gates_in_norm) {  // gates = sigmoid(to_gates(x_normed)): a [heads -> 32 padded] x C GEMM on the same rows
       GemmShape gg = plain_shape(planes, L, 32, C, C);
       EpiParams eg{};
       eg.kind = 2;
-      eg.bias = w.bg->f32;
+      eg.bias = bg->f32;
       eg.heads = heads;
       eg.out_f32 = c->GATES;
-      int rg = run_gemm(c, c->XN, w.wg, tp ? tp->gates : nullptr, gg, eg, F > 1 ? "gemm_gates_front" : "gemm_gates", st);
+      int rg = run_gemm(c, c->XN, wg, tp ? tp->gates : nullptr, gg, eg, front ? "gemm_gates_front" : "gemm_gates", st);
       if (rg != BT_OK) return rg;
     }
     EpiParams e{};
     e.kind = 1;
     e.out_act = c->QKV; e.ldo_act = 3 * C;
-    e.rope_cos = c->mw.rope_cos->f32;
-    e.rope_sin = c->mw.rope_sin->f32;
+    e.rope_cos = c->rope_cos->f32;
+    e.rope_sin = c->rope_sin->f32;
     e.C = C; e.heads = heads; e.posmode = freq ? 1 : 0; e.F = F;
     e.qscale = qscale;
     GemmShape g = plain_shape(planes, L, 3 * C, C, C);
-    r = run_gemm(c, c->XN, w.wqkv, tp ? tp->qkv : nullptr, g, e, F > 1 ? "gemm_qkv_front" : "gemm_qkv", st);
+    r = run_gemm(c, c->XN, wqkv, tp ? tp->qkv : nullptr, g, e, front ? "gemm_qkv_front" : "gemm_qkv", st);
     if (r != BT_OK) return r;
   }
   if (freq) {
-    launch_attn_freq(c->QKV, c->GATES, c->O, nb, F, L, heads, inv_sqrt_d, tc, st);
+    if (tc) launch_attn_freq_tc(tp->freq, c->GATES, inv_sqrt_d, st);
+    else launch_attn_freq_simt(reinterpret_cast<const float*>(c->QKV), c->GATES, reinterpret_cast<float*>(c->O), nb, F, L,
+                               heads, inv_sqrt_d, st);
     BT_LAUNCHED(c, "attn_freq", st);
   } else if (tc) {
-    if (launch_attn_time_tc(tp->attn, c->GATES, c->O, st, vl_chunks, planes / nb) != 0) return fail(c, BT_ERR_CUDA, "attn tc launch failed");
+    launch_attn_time_tc(tp->attn, c->GATES, c->O, st, vl_chunks, F);
     BT_LAUNCHED(c, "attn_time_tc", st);
   } else {
     launch_attn_time_simt(reinterpret_cast<const float*>(c->QKV), c->GATES, reinterpret_cast<float*>(c->O),
-                          planes, L, heads, st, vl_chunks, planes / nb);
+                          planes, L, heads, st, vl_chunks, F);
     BT_LAUNCHED(c, "attn_time_simt", st);
   }
-  if (skip_out) return BT_OK;
+  if (out_in_ff) return BT_OK;
   GemmShape go = plain_shape(planes, L, C, C, C);
   EpiParams eo = epi_generic(nullptr, 0, X, C, X, C, nullptr, 0);
-  return run_gemm(c, c->O, w.wout, tp ? tp->out : nullptr, go, eo, F > 1 ? "gemm_attn_out_front" : "gemm_attn_out", st);
+  return run_gemm(c, c->O, wout, tp ? tp->out : nullptr, go, eo, front ? "gemm_attn_out_front" : "gemm_attn_out", st);
 }
 
-// x += ff(x) (reference roformer.py:38-61); optionally also writes a bf16 copy of the result.
-int ff_block(bt_ctx* c, float* X, int planes, int L, int C, int mult, const FfW& w, FfPlans* tp, void* copy_act,
-             cudaStream_t st, bool with_outproj = false, bool front = false) {
+// x += ff(x) (reference roformer.py:38-61); optionally also writes a 16-bit copy of the result.  with_outproj: the
+// fused kernel first adds the out-projection of the attention in front (LayerPlans::ff_op).
+int ff_block(bt_ctx* c, float* X, const Layer& l, const LayerPlans* tp, int nb, int L, bool with_outproj,
+             void* copy_act, cudaStream_t st) {
   const bool tc = c->dtype == BT_DTYPE_H16;
+  const bool front = l.F > 1;
+  const int C = l.C, mult = l.mult, planes = nb * l.F;
+  const Param *w1 = l.w[0], *b1 = l.w[1], *w2 = l.w[2], *b2 = l.w[3];
   const int64_t M = static_cast<int64_t>(planes) * L;
-  if (with_outproj && !(tc && tp && tp->fused_op)) return fail(c, BT_ERR_ARG, "fused out-projection requested without a plan");
-  if (tc && tp && tp->fused) {
-    if (launch_fused_ff(with_outproj ? tp->fused_op : tp->fused, X, w.b1->f32, w.b2->f32, copy_act, st) != 0)
+  if (tc && fused(l)) {
+    if (launch_fused_ff(with_outproj ? tp->ff_op : tp->ff, X, b1->f32, b2->f32, copy_act, st) != 0)
       return fail(c, BT_ERR_CUDA, "fused ff launch failed");
     BT_LAUNCHED(c, C == 32 ? "ff_fused_c32" : "ff_fused_c64", st);
     return BT_OK;
@@ -440,21 +445,12 @@ int ff_block(bt_ctx* c, float* X, int planes, int L, int C, int mult, const FfW&
   launch_norm(X, c->XN, M, C, tc, st);
   BT_LAUNCHED(c, front ? "norm_front" : "norm", st);
   GemmShape g1 = plain_shape(planes, L, mult * C, C, C);
-  EpiParams e1 = epi_generic(w.b1, 1, nullptr, 0, nullptr, 0, c->H, mult * C);
-  int r = run_gemm(c, c->XN, w.w1, tp ? tp->ff1 : nullptr, g1, e1, front ? "gemm_ff1_front" : "gemm_ff1", st);
+  EpiParams e1 = epi_generic(b1, 1, nullptr, 0, nullptr, 0, c->H, mult * C);
+  int r = run_gemm(c, c->XN, w1, tp ? tp->ff1 : nullptr, g1, e1, front ? "gemm_ff1_front" : "gemm_ff1", st);
   if (r != BT_OK) return r;
   GemmShape g2 = plain_shape(planes, L, C, mult * C, mult * C);
-  EpiParams e2 = epi_generic(w.b2, 0, X, C, X, C, copy_act, C);
-  return run_gemm(c, c->H, w.w2, tp ? tp->ff2 : nullptr, g2, e2, front ? "gemm_ff2_front" : "gemm_ff2", st);
-}
-
-AttnW attn_w(const bt_ctx* c, const std::string& p) {
-  return AttnW{find_param(c, p + ".wqkv"), find_param(c, p + ".wg"), find_param(c, p + ".bg"),
-               find_param(c, p + ".wout")};
-}
-FfW ff_w(const bt_ctx* c, const std::string& p) {
-  return FfW{find_param(c, p + ".w1"), find_param(c, p + ".b1"), find_param(c, p + ".w2"),
-             find_param(c, p + ".b2")};
+  EpiParams e2 = epi_generic(b2, 0, X, C, X, C, copy_act, C);
+  return run_gemm(c, c->H, w2, tp ? tp->ff2 : nullptr, g2, e2, front ? "gemm_ff2_front" : "gemm_ff2", st);
 }
 
 GemmShape conv_shape(int nb, int F, int L, int C) {
@@ -474,84 +470,69 @@ GemmShape lin_shape(int nb, int L, int D, int Fo, int Co) {
   return g;
 }
 
-int build_plans(bt_ctx* c, int nb, int L, WavePlans** out) {
+// the 16-bit plans of layer i for waves of nb chunks of L frames; false (message in err) when one cannot be made
+bool make_layer_plans(const bt_ctx* c, size_t i, int nb, int L, LayerPlans& p, char* err, int errlen) {
+  const Layer& l = c->layers[i];
+  const int C = l.C, planes = nb * l.F;
+  const int64_t M = static_cast<int64_t>(planes) * L;
+  auto gemm = [&](const void* A, const Param* W, const GemmShape& g, bool resid = false) {
+    return tc_gemm_plan_create(A, W->b16, g, planes, resid, err, errlen);
+  };
+  switch (l.kind) {
+    case kConv:
+      return (p.gemm = gemm(c->XB, l.w[0], conv_shape(nb, l.F, L, C))) != nullptr;
+    case kLin:
+      return (p.gemm = gemm(c->XN, l.w[0], lin_shape(nb, L, c->hp.transformer_dim, l.F, C))) != nullptr;
+    case kFf:
+      if (fused(l)) {
+        p.ff = tc_ff_plan_create(l.w[0]->b16, l.w[2]->b16, C, M, nullptr, nullptr, err, errlen);
+        const Layer& prev = c->layers[i - 1];
+        if (prev.kind == kAttnF || prev.kind == kAttnT)  // ... and with the out-projection of the frontend attention in front
+          p.ff_op = tc_ff_plan_create(l.w[0]->b16, l.w[2]->b16, C, M, c->O, prev.w[3]->b16, err, errlen);
+        return p.ff && (p.ff_op || prev.kind == kAttn);
+      }
+      p.ff1 = gemm(c->XN, l.w[0], plain_shape(planes, L, l.mult * C, C, C));
+      p.ff2 = gemm(c->H, l.w[2], plain_shape(planes, L, C, l.mult * C, l.mult * C), true);
+      return p.ff1 && p.ff2;
+    default:  // attention
+      if (fused(l)) {
+        if (!(p.fqkv = tc_qkv_plan_create(l.w[0]->b16, C, M, err, errlen))) return false;
+      } else {
+        p.gates = gemm(c->XN, l.w[1], plain_shape(planes, L, 32, C, C));
+        p.qkv = gemm(c->XN, l.w[0], plain_shape(planes, L, 3 * C, C, C));
+        if (!p.gates || !p.qkv) return false;
+      }
+      if (l.kind == kAttnF) {
+        if (!(p.freq = tc_freq_plan_create(c->QKV, c->O, nb, l.F, L, C / kHeadDim, err, errlen))) return false;
+      } else if (!(p.attn = tc_attn_plan_create(c->QKV, planes, L, C / kHeadDim, err, errlen))) {
+        return false;
+      }
+      return (p.out = gemm(c->O, l.w[3], plain_shape(planes, L, C, C, C), true)) != nullptr;
+  }
+}
+
+int build_plans(bt_ctx* c, int nb, int L, std::vector<LayerPlans>** out) {
   auto key = std::make_pair(nb, L);
   auto it = c->plans.find(key);
-  if (it != c->plans.end()) { *out = it->second; return BT_OK; }
+  if (it != c->plans.end()) { *out = &it->second; return BT_OK; }
   // bounded cache: tensor maps are copied into the kernel parameters at launch, so dropping the oldest geometry is
   // safe while its kernels are still in flight
   constexpr size_t kMaxPlans = 48;
   while (c->plans.size() >= kMaxPlans && !c->plan_order.empty()) {
     auto old = c->plans.find(c->plan_order.front());
-    if (old != c->plans.end()) { destroy_wave_plans(old->second); c->plans.erase(old); }
+    if (old != c->plans.end()) { destroy_plans(old->second); c->plans.erase(old); }
     c->plan_order.erase(c->plan_order.begin());
   }
-  WavePlans* w = new WavePlans();
+  std::vector<LayerPlans> v(c->layers.size());
   char err[512] = "";
-  auto mk = [&](const void* A, const Param* W, const GemmShape& g, int planes_in, bool resid = false) -> TcGemmPlan* {
-    return tc_gemm_plan_create(A, W->b16, g, planes_in, resid, err, sizeof(err));
-  };
-  auto mk_attn = [&](AttnPlans& a, const AttnW& aw, int planes, int C, bool freq) -> bool {
-    if (c->fuse_ff && (C == 32 || C == 64)) {
-      a.fqkv = tc_qkv_plan_create(aw.wqkv->b16, C, static_cast<int64_t>(planes) * L, err, sizeof(err));
-      if (!a.fqkv) return false;
+  for (size_t i = 0; i < v.size(); ++i) {
+    if (!make_layer_plans(c, i, nb, L, v[i], err, sizeof(err))) {  // never cache a half-built entry
+      destroy_plans(v);
+      return fail(c, BT_ERR_CUDA, "tensor-core plan creation failed (%s): %s", c->layers[i].name.c_str(), err);
     }
-    a.qkv = mk(c->XN, aw.wqkv, plain_shape(planes, L, 3 * C, C, C), planes);
-    a.out = mk(c->O, aw.wout, plain_shape(planes, L, C, C, C), planes, true);
-    a.gates = mk(c->XN, aw.wg, plain_shape(planes, L, 32, C, C), planes);
-    if (!a.qkv || !a.out || !a.gates) return false;
-    if (!freq) {
-      a.attn = tc_attn_plan_create(c->QKV, planes, L, C / 32, err, sizeof(err));
-      if (!a.attn) return false;
-    }
-    return true;
-  };
-  auto mk_ff = [&](FfPlans& f, const FfW& fw, int planes, int C, int mult, const Param* wout = nullptr) -> bool {
-    if (c->fuse_ff && mult == 4 && (C == 32 || C == 64)) {  // narrow frontend FFNs: one fused kernel
-      f.fused = tc_ff_plan_create(fw.w1->b16, fw.w2->b16, C, static_cast<int64_t>(planes) * L, nullptr, nullptr, err, sizeof(err));
-      if (f.fused && wout && c->fuse_outproj)  // ... and one with the preceding attention's out-projection in front
-        f.fused_op = tc_ff_plan_create(fw.w1->b16, fw.w2->b16, C, static_cast<int64_t>(planes) * L, c->O, wout->b16, err, sizeof(err));
-      return f.fused != nullptr && (!(wout && c->fuse_outproj) || f.fused_op != nullptr);
-    }
-    f.ff1 = mk(c->XN, fw.w1, plain_shape(planes, L, mult * C, C, C), planes);
-    f.ff2 = mk(c->H, fw.w2, plain_shape(planes, L, C, mult * C, mult * C), planes, true);
-    return f.ff1 && f.ff2;
-  };
-  bool ok = true;
-  int C = c->hp.stem_dim, F = c->hp.spect_dim / 4;
-  for (int i = 0; i < 3 && ok; ++i) {
-    const std::string p = "b" + std::to_string(i);
-    if (c->hp.partial_transformers) {
-      ok = ok && mk_attn(w->fa[i], c->mw.fa[i], nb * F, C, true);
-      ok = ok && mk_ff(w->ff_f[i], c->mw.ff_f[i], nb * F, C, 4, c->mw.fa[i].wout);
-      ok = ok && mk_attn(w->ta[i], c->mw.ta[i], nb * F, C, false);
-      ok = ok && mk_ff(w->ff_t[i], c->mw.ff_t[i], nb * F, C, 4, c->mw.ta[i].wout);
-    }
-    if (ok) {
-      w->conv[i] = mk(c->XB, c->mw.conv_w[i], conv_shape(nb, F, L, C), nb * F);
-      ok = w->conv[i] != nullptr;
-    }
-    C *= 2; F /= 2;
   }
-  const int D = c->hp.transformer_dim;
-  if (ok) {
-    w->lin = mk(c->XN, c->mw.lin_w, lin_shape(nb, L, D, F, C), nb * F);
-    ok = w->lin != nullptr;
-  }
-  w->la.resize(c->hp.n_layers);
-  w->lf.resize(c->hp.n_layers);
-  for (int l = 0; l < c->hp.n_layers && ok; ++l) {
-    const std::string p = "l" + std::to_string(l);
-    ok = ok && mk_attn(w->la[l], c->mw.la[l], nb, D, false);
-    ok = ok && mk_ff(w->lf[l], c->mw.lf[l], nb, D, c->hp.ff_mult);
-  }
-  if (!ok) {  // never cache a half-built entry
-    destroy_wave_plans(w);
-    return fail(c, BT_ERR_CUDA, "tensor-core plan creation failed: %s", err);
-  }
-  c->plans[key] = w;
   c->plan_order.push_back(key);
-  *out = w;
+  *out = &(c->plans[key] = std::move(v));
   return BT_OK;
 }
 
@@ -559,74 +540,64 @@ int build_plans(bt_ctx* c, int nb, int L, WavePlans** out) {
 int run_wave(bt_ctx* c, const float* spect, const Wave& wv, float* beat, float* down, cudaStream_t st) {
   const bool tc = c->dtype == BT_DTYPE_H16;
   const int nb = wv.nb, L = wv.L;
-  WavePlans* wp = nullptr;
-  if (tc) {
-    int r = build_plans(c, nb, L, &wp);
-    if (r != BT_OK) return r;
-  }
+  std::vector<LayerPlans>* wp = nullptr;
   int r;
+  if (tc && (r = build_plans(c, nb, L, &wp)) != BT_OK) return r;
   float* X = c->X0;
   float* Xalt = c->X1;
   // chunks shorter than the wave's padded length: the time attentions mask their missing keys and the convolutions
   // see zeros beyond their last frame (everything else works row by row, padding rows are never read back)
   const ChunkSrc* vl = wv.varlen ? wv.chunks_dev : nullptr;
-  int C = c->hp.stem_dim, F = c->hp.spect_dim / 4;
-  launch_stem(spect, wv.chunks_dev, nb, L, c->mw.bn1_scale->f32, c->mw.bn1_shift->f32, c->mw.stem_w->f32, c->mw.stem_b->f32, X, st);
+  launch_stem(spect, wv.chunks_dev, nb, L, c->bn1_scale->f32, c->bn1_shift->f32, c->stem_w->f32, c->stem_b->f32, X, st);
   BT_LAUNCHED(c, "stem", st);
-  if ((r = do_tap(c, "stem", X, static_cast<int64_t>(nb) * F * L * C, false, st)) != BT_OK) return r;
-  for (int i = 0; i < 3; ++i) {
-    const std::string p = "b" + std::to_string(i);
-    const int planes = nb * F;
-    const int64_t elems = static_cast<int64_t>(planes) * L * C;
-    void* copy_for_conv = tc ? c->XB : nullptr;
-    if (c->hp.partial_transformers) {
-      // out-projection + residual of an attention move into the following fused FFN kernel when there is a plan
-      // for it (C = 32 / 64) and nobody asked to see the intermediate residual stream (debug tap)
-      const bool op_f = wp && wp->ff_f[i].fused_op && (c->tap_name.empty() || c->tap_name != p + ".attnF");
-      const bool op_t = wp && wp->ff_t[i].fused_op && (c->tap_name.empty() || c->tap_name != p + ".attnT");
-      if ((r = attention_block(c, X, planes, L, C, F, true, c->mw.fa[i], wp ? &wp->fa[i] : nullptr, nb, st, op_f)) != BT_OK) return r;
-      if ((r = do_tap(c, (p + ".attnF").c_str(), X, elems, false, st)) != BT_OK) return r;
-      if ((r = ff_block(c, X, planes, L, C, 4, c->mw.ff_f[i], wp ? &wp->ff_f[i] : nullptr, nullptr, st, op_f, true)) != BT_OK) return r;
-      if ((r = do_tap(c, (p + ".ffF").c_str(), X, elems, false, st)) != BT_OK) return r;
-      if ((r = attention_block(c, X, planes, L, C, F, false, c->mw.ta[i], wp ? &wp->ta[i] : nullptr, nb, st, op_t, vl)) != BT_OK) return r;
-      if ((r = do_tap(c, (p + ".attnT").c_str(), X, elems, false, st)) != BT_OK) return r;
-      if ((r = ff_block(c, X, planes, L, C, 4, c->mw.ff_t[i], wp ? &wp->ff_t[i] : nullptr, copy_for_conv, st, op_t, true)) != BT_OK) return r;
-      if ((r = do_tap(c, (p + ".ffT").c_str(), X, elems, false, st)) != BT_OK) return r;
-    } else if (tc) {
-      launch_f32_to_h16(X, c->XB, elems, st);
-      BT_LAUNCHED(c, "f32_to_h16", st);
+  if ((r = do_tap(c, "stem", X, static_cast<int64_t>(nb) * (c->hp.spect_dim / 4) * L * c->hp.stem_dim, false, st)) != BT_OK)
+    return r;
+  const std::vector<Layer>& layers = c->layers;
+  for (size_t i = 0; i < layers.size(); ++i) {
+    const Layer& l = layers[i];
+    const LayerPlans* tp = wp ? &(*wp)[i] : nullptr;
+    const char* tap = l.name.c_str();
+    const void* out = X;  // the layer's output (tap)
+    bool out_act = false;
+    int64_t elems = static_cast<int64_t>(nb) * l.F * L * l.C;
+    if (is_attention(l)) {
+      r = attention_block(c, X, l, tp, nb, L, outproj_in_ff(c, wp, i), l.kind == kAttnF ? nullptr : vl, st);
+    } else if (l.kind == kFf) {
+      // the FFN in front of a convolution also writes the 16-bit copy the convolution reads
+      const bool before_conv = i + 1 < layers.size() && layers[i + 1].kind == kConv;
+      r = ff_block(c, X, l, tp, nb, L, outproj_in_ff(c, wp, i - 1), tc && before_conv ? c->XB : nullptr, st);
+    } else if (l.kind == kConv) {
+      if (tc && (i == 0 || layers[i - 1].kind != kFf)) {  // no FFN in front (no partial transformers)
+        launch_f32_to_h16(X, c->XB, elems, st);
+        BT_LAUNCHED(c, "f32_to_h16", st);
+      }
+      if (vl) {
+        launch_zero_tail(tc ? c->XB : static_cast<void*>(X), tc ? 2 : 4, vl, nb, l.F, L, l.C, st);
+        BT_LAUNCHED(c, "zero_tail", st);
+      }
+      // conv C -> 2C (+ folded BN2d + GELU); the last one feeds frontend.linear (activation dtype)
+      const bool last = layers[i + 1].kind == kLin;
+      EpiParams e = epi_generic(l.w[1], 1, nullptr, 0, last ? nullptr : Xalt, 2 * l.C, last ? c->XN : nullptr, 2 * l.C);
+      r = run_gemm(c, tc ? c->XB : static_cast<const void*>(X), l.w[0], tp ? tp->gemm : nullptr,
+                   conv_shape(nb, l.F, L, l.C), e, "gemm_conv", st);
+      if (last) {
+        out = c->XN;
+        out_act = true;
+      } else {
+        std::swap(X, Xalt);
+        out = X;
+      }
+    } else {  // kLin
+      const int D = c->hp.transformer_dim;
+      EpiParams e = epi_generic(l.w[1], 0, nullptr, 0, X, D, nullptr, 0);
+      r = run_gemm(c, c->XN, l.w[0], tp ? tp->gemm : nullptr, lin_shape(nb, L, D, l.F, l.C), e, "gemm_frontend_linear", st);
+      tap = "frontend";
+      elems = static_cast<int64_t>(nb) * L * D;
     }
-    if (vl) {
-      launch_zero_tail(tc ? c->XB : static_cast<void*>(X), tc ? 2 : 4, vl, nb, F, L, C, st);
-      BT_LAUNCHED(c, "zero_tail", st);
-    }
-    // conv C -> 2C (+ folded BN2d + GELU); the last block feeds frontend.linear (activation dtype)
-    GemmShape g = conv_shape(nb, F, L, C);
-    const bool last = i == 2;
-    EpiParams e = epi_generic(c->mw.conv_b[i], 1, nullptr, 0, last ? nullptr : Xalt, 2 * C,
-                              last ? c->XN : nullptr, 2 * C);
-    if ((r = run_gemm(c, tc ? c->XB : static_cast<const void*>(X), c->mw.conv_w[i],
-                      wp ? wp->conv[i] : nullptr, g, e, "gemm_conv", st)) != BT_OK) return r;
-    C *= 2; F /= 2;
-    if (!last) std::swap(X, Xalt);
-    if ((r = do_tap(c, (p + ".conv").c_str(), last ? c->XN : static_cast<const void*>(X),
-                    static_cast<int64_t>(nb) * F * L * C, last, st)) != BT_OK) return r;
+    if (r != BT_OK || (r = do_tap(c, tap, out, elems, out_act, st)) != BT_OK) return r;
   }
-  const int D = c->hp.transformer_dim;
-  {
-    GemmShape g = lin_shape(nb, L, D, F, C);
-    EpiParams e = epi_generic(c->mw.lin_b, 0, nullptr, 0, X, D, nullptr, 0);
-    if ((r = run_gemm(c, c->XN, c->mw.lin_w, wp ? wp->lin : nullptr, g, e, "gemm_frontend_linear", st)) != BT_OK) return r;
-    if ((r = do_tap(c, "frontend", X, static_cast<int64_t>(nb) * L * D, false, st)) != BT_OK) return r;
-  }
-  for (int l = 0; l < c->hp.n_layers; ++l) {
-    const std::string p = "l" + std::to_string(l);
-    if ((r = attention_block(c, X, nb, L, D, 1, false, c->mw.la[l], wp ? &wp->la[l] : nullptr, nb, st, false, vl)) != BT_OK) return r;
-    if ((r = do_tap(c, (p + ".attn").c_str(), X, static_cast<int64_t>(nb) * L * D, false, st)) != BT_OK) return r;
-    if ((r = ff_block(c, X, nb, L, D, c->hp.ff_mult, c->mw.lf[l], wp ? &wp->lf[l] : nullptr, nullptr, st)) != BT_OK) return r;
-    if ((r = do_tap(c, (p + ".ff").c_str(), X, static_cast<int64_t>(nb) * L * D, false, st)) != BT_OK) return r;
-  }
-  launch_head(X, D, c->mw.head_w->f32, c->mw.head_b->f32, wv.chunks_dev, nb, L, beat, down, c->hp.sum_head ? 1 : 0, st);
+  launch_head(X, c->hp.transformer_dim, c->head_w->f32, c->head_b->f32, wv.chunks_dev, nb, L, beat, down,
+              c->hp.sum_head ? 1 : 0, st);
   BT_LAUNCHED(c, "head", st);
   return BT_OK;
 }
@@ -659,25 +630,39 @@ int run_chunks(bt_ctx* c, const float* spect_dev, std::vector<HostChunk>& all, f
   return BT_OK;
 }
 
-std::vector<std::string> required_params(const bt_hparams& hp) {
-  std::vector<std::string> v = {"mel.window", "mel.twiddle", "mel.fb_start", "mel.fb_ptr", "mel.fb_w",
-                                "rope.cos", "rope.sin", "stem.bn1_scale", "stem.bn1_shift", "stem.w",
-                                "stem.bias", "lin.w", "lin.b", "head.w", "head.b"};
-  auto attn = [&](const std::string& p) { for (auto s : {".wqkv", ".wg", ".bg", ".wout"}) v.push_back(p + s); };
-  auto ff = [&](const std::string& p) { for (auto s : {".w1", ".b1", ".w2", ".b2"}) v.push_back(p + s); };
+std::vector<Layer> layer_list(const bt_hparams& hp) {
+  std::vector<Layer> v;
+  int C = hp.stem_dim, F = hp.spect_dim / 4;
   for (int i = 0; i < 3; ++i) {
-    const std::string p = "b" + std::to_string(i);
-    if (hp.partial_transformers) { attn(p + ".attnF"); ff(p + ".ffF"); attn(p + ".attnT"); ff(p + ".ffT"); }
-    v.push_back(p + ".conv.w");
-    v.push_back(p + ".conv.bias");
+    const std::string b = "b" + std::to_string(i);
+    if (hp.partial_transformers) {
+      v.push_back({kAttnF, b + ".attnF", C, F, 0, {}});
+      v.push_back({kFf, b + ".ffF", C, F, 4, {}});
+      v.push_back({kAttnT, b + ".attnT", C, F, 0, {}});
+      v.push_back({kFf, b + ".ffT", C, F, 4, {}});
+    }
+    v.push_back({kConv, b + ".conv", C, F, 0, {}});
+    C *= 2; F /= 2;
   }
-  for (int l = 0; l < hp.n_layers; ++l) { attn("l" + std::to_string(l) + ".attn"); ff("l" + std::to_string(l) + ".ff"); }
+  v.push_back({kLin, "lin", C, F, 0, {}});
+  for (int l = 0; l < hp.n_layers; ++l) {
+    v.push_back({kAttn, "l" + std::to_string(l) + ".attn", hp.transformer_dim, 1, 0, {}});
+    v.push_back({kFf, "l" + std::to_string(l) + ".ff", hp.transformer_dim, 1, hp.ff_mult, {}});
+  }
   return v;
 }
 
-bool is_gemm_weight(const std::string& n) {
-  auto ends = [&](const char* s) { size_t k = strlen(s); return n.size() >= k && n.compare(n.size() - k, k, s) == 0; };
-  return ends(".wqkv") || ends(".wout") || ends(".wg") || ends(".w1") || ends(".w2") || ends(".conv.w") || n == "lin.w";
+// the parameters of a layer in the order of Layer::w: name suffix, element count, and whether a GEMM reads it as
+// a 16-bit operand
+struct ParamSpec { const char* suffix; int64_t count; bool gemm; };
+std::vector<ParamSpec> layer_params(const Layer& l, int64_t D) {
+  const int64_t C = l.C, m = l.mult;
+  switch (l.kind) {
+    case kFf: return {{".w1", m * C * C, true}, {".b1", m * C, false}, {".w2", m * C * C, true}, {".b2", C, false}};
+    case kConv: return {{".w", 2 * C * 6 * C, true}, {".bias", 2 * C, false}};
+    case kLin: return {{".w", D * C * l.F, true}, {".b", D, false}};
+    default: return {{".wqkv", 3 * C * C, true}, {".wg", 32 * C, true}, {".bg", 32, false}, {".wout", C * C, true}};
+  }
 }
 
 }  // namespace
@@ -685,7 +670,7 @@ bool is_gemm_weight(const std::string& n) {
 // ================================================================================== C ABI
 extern "C" {
 
-int bt_version(void) { return 200; }
+int bt_version(void) { return 201; }
 
 const char* bt_act_dtype(void) {
 #if defined(BT_ACT_BF16)
@@ -734,10 +719,6 @@ int bt_create(bt_ctx** out, int device_ordinal, const bt_hparams* hp, int comput
   c->dtype = compute_dtype;
   const char* dbg = getenv("BT_SYNC_DEBUG");
   c->sync_debug = dbg && dbg[0] == '1';
-  const char* ffe = getenv("BT_FUSE_FF");
-  c->fuse_ff = !(ffe && ffe[0] == '0');
-  const char* foe = getenv("BT_FUSE_OUTPROJ");
-  c->fuse_outproj = !(foe && foe[0] == '0');
 
   if (compute_dtype == BT_DTYPE_H16) {
     char err[512];
@@ -775,75 +756,39 @@ int bt_finalize(bt_ctx* c) {
   if (!c) return BT_ERR_ARG;
   if (c->finalized) return BT_OK;
   BT_CUDA(c, cudaSetDevice(c->device));
-  const bt_hparams& hp = c->hp;
-  for (const auto& n : required_params(hp))
-    if (!find_param(c, n)) return fail(c, BT_ERR_PARAM, "bt_finalize: missing parameter '%s'", n.c_str());
-  // shape checks for the GEMM weights
-  auto expect = [&](const std::string& n, int64_t cnt) -> bool {
-    const Param* p = find_param(c, n);
-    if (!p || p->n != cnt) {
-      fail(c, BT_ERR_PARAM, "parameter '%s' has %lld elements, expected %lld", n.c_str(),
-           (long long)(p ? p->n : -1), (long long)cnt);
-      return false;
-    }
-    return true;
-  };
-  auto chk_attn = [&](const std::string& p, int64_t C) {
-    return expect(p + ".wqkv", 3 * C * C) && expect(p + ".wg", 32 * C) && expect(p + ".bg", 32) &&
-           expect(p + ".wout", C * C);
-  };
-  auto chk_ff = [&](const std::string& p, int64_t C, int64_t mult) {
-    return expect(p + ".w1", mult * C * C) && expect(p + ".b1", mult * C) && expect(p + ".w2", mult * C * C) &&
-           expect(p + ".b2", C);
-  };
-  int64_t C = hp.stem_dim;
-  for (int i = 0; i < 3; ++i) {
-    const std::string p = "b" + std::to_string(i);
-    if (hp.partial_transformers)
-      if (!chk_attn(p + ".attnF", C) || !chk_ff(p + ".ffF", C, 4) || !chk_attn(p + ".attnT", C) ||
-          !chk_ff(p + ".ffT", C, 4)) return BT_ERR_PARAM;
-    if (!expect(p + ".conv.w", 2 * C * 6 * C) || !expect(p + ".conv.bias", 2 * C)) return BT_ERR_PARAM;
-    C *= 2;
+  const int64_t D = c->hp.transformer_dim;
+  // every parameter the forward pass reads, with its element count (-1: not checked), resolved once here (no name
+  // lookups per launch)
+  struct Need { std::string name; int64_t count; const Param** dst; bool gemm; };
+  std::vector<Need> need = {
+      {"mel.window", 1024, nullptr, false}, {"mel.twiddle", 1024, nullptr, false}, {"mel.fb_start", 128, nullptr, false},
+      {"mel.fb_ptr", 129, nullptr, false}, {"mel.fb_w", -1, nullptr, false},
+      {"rope.cos", BT_CHUNK * 16, &c->rope_cos, false}, {"rope.sin", BT_CHUNK * 16, &c->rope_sin, false},
+      {"stem.bn1_scale", -1, &c->bn1_scale, false}, {"stem.bn1_shift", -1, &c->bn1_shift, false},
+      {"stem.w", 32 * 12, &c->stem_w, false}, {"stem.bias", -1, &c->stem_b, false},
+      {"head.w", 2 * D, &c->head_w, false}, {"head.b", 2, &c->head_b, false}};
+  c->layers = layer_list(c->hp);
+  for (Layer& l : c->layers) {
+    const std::vector<ParamSpec> specs = layer_params(l, D);
+    for (size_t k = 0; k < specs.size(); ++k) need.push_back({l.name + specs[k].suffix, specs[k].count, &l.w[k], specs[k].gemm});
   }
-  const int64_t D = hp.transformer_dim;
-  if (!expect("lin.w", D * C * (hp.spect_dim / 32)) || !expect("lin.b", D) || !expect("head.w", 2 * D) ||
-      !expect("head.b", 2) || !expect("stem.w", 32 * 12) || !expect("mel.window", 1024) ||
-      !expect("mel.twiddle", 1024) || !expect("mel.fb_start", 128) || !expect("mel.fb_ptr", 129) ||
-      !expect("rope.cos", (int64_t)BT_CHUNK * 16) || !expect("rope.sin", (int64_t)BT_CHUNK * 16))
-    return BT_ERR_PARAM;
-  for (int l = 0; l < hp.n_layers; ++l) {
-    const std::string p = "l" + std::to_string(l);
-    if (!chk_attn(p + ".attn", D) || !chk_ff(p + ".ff", D, hp.ff_mult)) return BT_ERR_PARAM;
+  for (const Need& n : need)
+    if (!find_param(c, n.name)) return fail(c, BT_ERR_PARAM, "bt_finalize: missing parameter '%s'", n.name.c_str());
+  for (const Need& n : need) {
+    const Param* p = find_param(c, n.name);
+    if (n.count >= 0 && p->n != n.count)
+      return fail(c, BT_ERR_PARAM, "parameter '%s' has %lld elements, expected %lld", n.name.c_str(), (long long)p->n,
+                  (long long)n.count);
+    if (n.dst) *n.dst = p;
   }
   if (c->dtype == BT_DTYPE_H16) {
-    for (auto& kv : c->params) {
-      if (!is_gemm_weight(kv.first)) continue;
-      BT_CUDA(c, cudaMalloc(&kv.second.b16, kv.second.n * 2));
-      launch_f32_to_h16(kv.second.f32, kv.second.b16, kv.second.n, nullptr);
+    for (const Need& n : need) {
+      if (!n.gemm) continue;
+      Param& p = c->params[n.name];
+      BT_CUDA(c, cudaMalloc(&p.b16, p.n * 2));
+      launch_f32_to_h16(p.f32, p.b16, p.n, nullptr);
     }
     BT_CUDA(c, cudaDeviceSynchronize());
-  }
-  {
-    ModelW& w = c->mw;
-    w.rope_cos = find_param(c, "rope.cos"); w.rope_sin = find_param(c, "rope.sin");
-    w.bn1_scale = find_param(c, "stem.bn1_scale"); w.bn1_shift = find_param(c, "stem.bn1_shift");
-    w.stem_w = find_param(c, "stem.w"); w.stem_b = find_param(c, "stem.bias");
-    w.lin_w = find_param(c, "lin.w"); w.lin_b = find_param(c, "lin.b");
-    w.head_w = find_param(c, "head.w"); w.head_b = find_param(c, "head.b");
-    for (int i = 0; i < 3; ++i) {
-      const std::string p = "b" + std::to_string(i);
-      if (hp.partial_transformers) {
-        w.fa[i] = attn_w(c, p + ".attnF"); w.ff_f[i] = ff_w(c, p + ".ffF");
-        w.ta[i] = attn_w(c, p + ".attnT"); w.ff_t[i] = ff_w(c, p + ".ffT");
-      }
-      w.conv_w[i] = find_param(c, p + ".conv.w");
-      w.conv_b[i] = find_param(c, p + ".conv.bias");
-    }
-    w.la.clear(); w.lf.clear();
-    for (int l = 0; l < hp.n_layers; ++l) {
-      w.la.push_back(attn_w(c, "l" + std::to_string(l) + ".attn"));
-      w.lf.push_back(ff_w(c, "l" + std::to_string(l) + ".ff"));
-    }
   }
   c->finalized = true;
   return BT_OK;
@@ -1451,8 +1396,10 @@ int bt_debug_attention(bt_ctx* c, const float* q_dev, const float* k_dev, const 
     char err[512] = "";
     TcAttnPlan* p = tc_attn_plan_create(qkv, seqs, L, heads, err, sizeof(err));
     if (!p) rc = fail(c, BT_ERR_CUDA, "%s", err);
-    else if (launch_attn_time_tc(p, gates_dev, o, st, chunks_dev, seqs_per_chunk) != 0) rc = fail(c, BT_ERR_CUDA, "tc attention launch failed");
-    else launch_h16_to_f32(o, o_dev, M * C, st);
+    else {
+      launch_attn_time_tc(p, gates_dev, o, st, chunks_dev, seqs_per_chunk);
+      launch_h16_to_f32(o, o_dev, M * C, st);
+    }
     cudaError_t se = cudaStreamSynchronize(st);
     if (rc == BT_OK && se != cudaSuccess) rc = fail(c, BT_ERR_CUDA, "tc attention: %s", cudaGetErrorString(se));
     if (p) tc_attn_plan_destroy(p);
@@ -1479,64 +1426,31 @@ int bt_debug_attention_freq(bt_ctx* c, const float* q_dev, const float* k_dev, c
   const int64_t M = static_cast<int64_t>(B) * F * L;
   const bool tc = c->dtype == BT_DTYPE_H16;
   const size_t act = tc ? 2 : 4;
+  const float inv_sqrt_d = 0.17677669529663687f;
   void *qkv = nullptr, *o = nullptr;
+  TcFreqPlan* p = nullptr;
   BT_CUDA(c, cudaMalloc(&qkv, M * 3 * C * act));
-  if (tc) BT_CUDA(c, cudaMalloc(&o, M * C * act));
+  if (tc) {
+    BT_CUDA(c, cudaMalloc(&o, M * C * act));
+    char err[512] = "";
+    if (!(p = tc_freq_plan_create(qkv, o, B, F, L, heads, err, sizeof(err)))) {
+      cudaFree(qkv); cudaFree(o);
+      return fail(c, BT_ERR_ARG, "bt_debug_attention_freq: %s", err);
+    }
+  }
   launch_pack_qkv_test(q_dev, k_dev, v_dev, qkv, B * F, L, heads, 1.0f, tc ? 1 : 0, st);
-  launch_attn_freq(qkv, gates_dev, tc ? o : static_cast<void*>(o_dev), B, F, L, heads, 0.17677669529663687f, tc ? 1 : 0, st);
-  if (tc) launch_h16_to_f32(o, o_dev, M * C, st);
+  if (tc) {
+    launch_attn_freq_tc(p, gates_dev, inv_sqrt_d, st);
+    launch_h16_to_f32(o, o_dev, M * C, st);
+  } else {
+    launch_attn_freq_simt(static_cast<const float*>(qkv), gates_dev, o_dev, B, F, L, heads, inv_sqrt_d, st);
+  }
   int rc = BT_OK;
   cudaError_t se = cudaStreamSynchronize(st);
   if (se != cudaSuccess) rc = fail(c, BT_ERR_CUDA, "frequency attention: %s", cudaGetErrorString(se));
   c->launches += 2;
+  if (p) tc_freq_plan_destroy(p);
   cudaFree(qkv); cudaFree(o);
-  return rc;
-}
-
-int bt_debug_attention_time(bt_ctx* c, int32_t seqs, int32_t L, int32_t heads, int32_t variant, int32_t iters,
-                            float* ms_per_launch) {
-  if (!c || !ms_per_launch || iters < 1) return BT_ERR_ARG;
-  if (c->dtype != BT_DTYPE_H16) return fail(c, BT_ERR_ARG, "bt_debug_attention_time needs the 16-bit context");
-  BT_CUDA(c, cudaSetDevice(c->device));
-  const int C = heads * 32;
-  const int64_t M = static_cast<int64_t>(seqs) * L;
-  void *qkv = nullptr, *o = nullptr;
-  float *gates = nullptr, *src = nullptr;
-  BT_CUDA(c, cudaMalloc(&qkv, M * 3 * C * 2));
-  BT_CUDA(c, cudaMalloc(&o, M * C * 2));
-  BT_CUDA(c, cudaMalloc(&gates, M * heads * 4));
-  BT_CUDA(c, cudaMalloc(&src, M * C * 4));
-  std::vector<float> h(M * C);
-  uint32_t x = 12345u;
-  for (auto& v : h) { x = x * 1664525u + 1013904223u; v = (static_cast<float>(x >> 8) / 8388608.0f - 1.0f) * 1.5f; }
-  BT_CUDA(c, cudaMemcpy(src, h.data(), M * C * 4, cudaMemcpyHostToDevice));
-  std::vector<float> ones(M * heads, 1.0f);
-  BT_CUDA(c, cudaMemcpy(gates, ones.data(), M * heads * 4, cudaMemcpyHostToDevice));
-  cudaStream_t st = nullptr;
-  launch_pack_qkv_test(src, src, src, qkv, seqs, L, heads, 0.17677669529663687f * 1.4426950408889634f, 1, st);
-  char err[512] = "";
-  TcAttnPlan* p = tc_attn_plan_create(qkv, seqs, L, heads, err, sizeof(err));
-  int rc = BT_OK;
-  if (!p) rc = fail(c, BT_ERR_CUDA, "%s", err);
-  else {
-    if (variant >= 0) attn_set_variant(variant);
-    cudaEvent_t e0, e1;
-    cudaEventCreate(&e0); cudaEventCreate(&e1);
-    for (int i = 0; i < 2 && rc == BT_OK; ++i)
-      if (launch_attn_time_tc(p, gates, o, st) != 0) rc = fail(c, BT_ERR_ARG, "unknown attention variant %d", variant);
-    cudaEventRecord(e0, st);
-    for (int i = 0; i < iters && rc == BT_OK; ++i) launch_attn_time_tc(p, gates, o, st);
-    cudaEventRecord(e1, st);
-    cudaError_t se = cudaStreamSynchronize(st);
-    if (rc == BT_OK && se != cudaSuccess) rc = fail(c, BT_ERR_CUDA, "attention: %s", cudaGetErrorString(se));
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, e0, e1);
-    *ms_per_launch = ms / iters;
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
-    tc_attn_plan_destroy(p);
-    if (variant >= 0) attn_set_variant(-1);
-  }
-  cudaFree(qkv); cudaFree(o); cudaFree(gates); cudaFree(src);
   return rc;
 }
 

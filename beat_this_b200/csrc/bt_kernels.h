@@ -56,14 +56,14 @@ void launch_gemm_simt(const float* A, const float* W, const GemmShape& g, const 
 // chunks != nullptr: sequence s belongs to chunk s / seqs_per_chunk and only its first chunks[..].len keys exist
 void launch_attn_time_simt(const float* qkv, const float* gates, float* out, int seqs, int L,
                            int heads, cudaStream_t st, const ChunkSrc* chunks = nullptr, int seqs_per_chunk = 1);
+// frequency-direction attention: tokens m = (b*F + f)*L + t, sequences over f (F in {8, 16, 32}).
+void launch_attn_freq_simt(const float* qkv, const float* gates, float* out, int B, int F, int L, int heads, float scale,
+                           cudaStream_t st);
 // rows [len_b, L) of every plane of chunk b <- 0 (the zero padding a k(2,3) convolution sees beyond the end of a
 // chunk that is shorter than the wave's padded length).  buf: [nchunks * F, L, C] of elem_bytes-sized elements.
 void launch_zero_tail(void* buf, int elem_bytes, const ChunkSrc* chunks, int nchunks, int F, int L, int C, cudaStream_t st);
 
 // ---- shared small kernels (templated on activation dtype inside) ---------------------------
-// frequency-direction attention: tokens m = (b*F + f)*L + t, sequences over f.
-void launch_attn_freq(const void* qkv, const float* gates, void* out, int B, int F, int L,
-                      int heads, float scale, int act_h16, cudaStream_t st);
 // RMSNorm without gamma (folded into the next weight); optionally also the attention gates
 // sigmoid(xn . wg[h] + bg[h]) for h < heads (used when heads <= 4; wg is [>=heads, C] fp32).
 void launch_norm(const float* x, void* xn, int64_t M, int C, int act_h16, cudaStream_t st, float* gates = nullptr,
@@ -147,9 +147,15 @@ int launch_gemm_tc(const TcGemmPlan* plan, const EpiParams& e, cudaStream_t st);
 struct TcAttnPlan;
 TcAttnPlan* tc_attn_plan_create(const void* qkv_h16, int seqs, int L, int heads, char* err, int errlen);
 void tc_attn_plan_destroy(TcAttnPlan*);
-void attn_set_variant(int v);  // debug: template parameter V of attn_time_kernel (kernels_attn.cu)
-int launch_attn_time_tc(const TcAttnPlan* plan, const float* gates, void* out_h16, cudaStream_t st,
-                        const ChunkSrc* chunks = nullptr, int seqs_per_chunk = 1);
+void launch_attn_time_tc(const TcAttnPlan* plan, const float* gates, void* out_h16, cudaStream_t st,
+                         const ChunkSrc* chunks = nullptr, int seqs_per_chunk = 1);
+
+// frequency-direction attention of the frontend blocks (F, heads) = (32, 1), (16, 2) or (8, 4): qkv [B * F * L, 3C] ->
+// out [B * F * L, C], the tokens of launch_attn_freq_simt.  Plan creation fails for any other pair.
+struct TcFreqPlan;
+TcFreqPlan* tc_freq_plan_create(const void* qkv_h16, void* out_h16, int B, int F, int L, int heads, char* err, int errlen);
+void tc_freq_plan_destroy(TcFreqPlan*);
+void launch_attn_freq_tc(const TcFreqPlan* plan, const float* gates, float scale, cudaStream_t st);
 
 // fused RMSNorm + FFN + residual for C in {32, 64} (frontend), x updated in place (+ optional 16-bit copy)
 struct TcFfPlan;

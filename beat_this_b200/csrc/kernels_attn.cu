@@ -2,8 +2,6 @@
 // attention of the three frontend blocks and of the 6 main layers (reference roformer.py:73-80 SDPA,
 // called from roformer.py:114-132 / beat_tracker.py:290-301).
 #include <cstdio>
-#include <cstdlib>
-#include <cstring>
 
 #include "tc_common.cuh"
 
@@ -15,7 +13,7 @@ namespace bt {
 // (mma.sync m16n8k16, fp32 accumulate): S = Q K^T -> online softmax in log2 units (q carries scale * log2 e) ->
 // P packed to 16 bits straight from the S accumulator layout -> O += P V.  With head_dim 32 there are only 128
 // tensor FLOPs per exponential: the exponentials (MUFU.EX2, 16 /clk/SM) bound the kernel, so a share of them can
-// run as a polynomial on the FMA pipe instead (template parameter V).
+// run as a polynomial on the FMA pipe instead: 3 of every 8 score pairs (AT_POLY_MASK).
 constexpr int AT_BQ = 128;
 constexpr int AT_BKV = 64;
 constexpr int AT_NST = 4;
@@ -26,18 +24,13 @@ constexpr int AT_SKV = AT_BKV * 64;  // 64 key rows x 32 dims x 2 bytes
 constexpr int AT_SMEM = 1024 + AT_SQ + AT_NST * 2 * AT_SKV + 128;
 
 // which of every 8 score pairs take the polynomial exp2 (spread out so that MUFU and FMA work interleave)
-__host__ __device__ constexpr uint32_t attn_poly_mask(int pp) {
-  return pp == 0 ? 0x00u : pp == 1 ? 0x08u : pp == 2 ? 0x44u : pp == 3 ? 0x52u : pp == 4 ? 0xAAu : pp == 5 ? 0xB5u : pp == 6 ? 0xBBu : 0xFFu;
-}
+constexpr uint32_t AT_POLY_MASK = 0x52u;
 
 // byte offset of 16-byte chunk c of row r in a tile of 64-byte rows written by TMA with CU_TENSOR_MAP_SWIZZLE_64B
 __device__ __forceinline__ uint32_t sw64_off(int r, int c) {
   return static_cast<uint32_t>(r * 64 + ((c ^ ((r >> 1) & 3)) << 4));
 }
 
-// V: bits 0, 2, 3 = how many of every 8 score pairs take the polynomial (1 + 2 + 4) | bit 1 = timing ablation without
-// exponentials (wrong results)
-template <int V>
 __global__ void __launch_bounds__(AT_THREADS, 2)
 attn_time_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
                  const float* __restrict__ gates, h16* __restrict__ out, int L, int heads,
@@ -59,8 +52,6 @@ attn_time_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
   // keys that exist for this sequence: the whole plane, or (waves of chunks of different lengths) its chunk's frames
   const int Lk = chunks ? chunks[seq / seqs_per_chunk].len : L;
   const int nkv = ceil_div(Lk, AT_BKV);
-  constexpr uint32_t PM = attn_poly_mask((V & 1) + ((V & 4) ? 2 : 0) + ((V & 8) ? 4 : 0));
-  constexpr bool NOEXP = (V & 2) != 0;
 
   if (threadIdx.x == 0) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar_q), "r"(1));
@@ -149,7 +140,7 @@ attn_time_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         const float x = s[nb][i] - mref[i >> 1];
-        p[i] = NOEXP ? x : (((PM >> nb) & 1u) ? ex2_poly(x) : ex2_approx(x));
+        p[i] = ((AT_POLY_MASK >> nb) & 1u) ? ex2_poly(x) : ex2_approx(x);
       }
       l_run[0] += p[0] + p[1];
       l_run[1] += p[2] + p[3];
@@ -212,38 +203,15 @@ TcAttnPlan* tc_attn_plan_create(const void* qkv, int seqs, int L, int heads, cha
 }
 void tc_attn_plan_destroy(TcAttnPlan* p) { delete p; }
 
-// Kernel variant (template parameter V of attn_time_kernel), reachable through BT_ATTN_VARIANT /
-// bt_debug_attention_time.  The product runs AT_DEFAULT_V.
-constexpr int AT_DEFAULT_V = 37;  // 3 of 8 score pairs on the polynomial
-static int g_attn_variant = -1;
-void attn_set_variant(int v) { g_attn_variant = v; }
-
-//   37 default | 32, 33, 36, 40, 41: 0, 1, 2, 4, 5 of 8 pairs on the polynomial | 39, 34: without exponentials
-//   (timing ablation, wrong results)
-#define BT_AT_VARIANTS(X) X(37) X(32) X(33) X(36) X(40) X(41) X(39) X(34)
-
-int launch_attn_time_tc(const TcAttnPlan* p, const float* gates, void* out, cudaStream_t st, const ChunkSrc* chunks,
-                        int seqs_per_chunk) {
+void launch_attn_time_tc(const TcAttnPlan* p, const float* gates, void* out, cudaStream_t st, const ChunkSrc* chunks,
+                         int seqs_per_chunk) {
   dim3 grid(ceil_div(p->L, AT_BQ), p->heads, p->seqs);
-  if (g_attn_variant < 0) g_attn_variant = getenv("BT_ATTN_VARIANT") ? atoi(getenv("BT_ATTN_VARIANT")) : AT_DEFAULT_V;
-  h16* o = reinterpret_cast<h16*>(out);
-#define BT_AT_L(V_)                                                                                                  \
-  if (g_attn_variant == (V_)) {                                                                                      \
-    attn_time_kernel<V_><<<grid, AT_THREADS, AT_SMEM, st>>>(p->tmQ, p->tmKV, gates, o, p->L, p->heads, chunks,        \
-                                                            seqs_per_chunk);                                         \
-    return 0;                                                                                                        \
-  }
-  BT_AT_VARIANTS(BT_AT_L)
-#undef BT_AT_L
-  return -3;
+  attn_time_kernel<<<grid, AT_THREADS, AT_SMEM, st>>>(p->tmQ, p->tmKV, gates, reinterpret_cast<h16*>(out), p->L, p->heads,
+                                                      chunks, seqs_per_chunk);
 }
 
 int tc_init_attn(char* err, int errlen) {
-  cudaError_t r = cudaSuccess;
-#define BT_AT_A(V_) \
-  if (r == cudaSuccess) r = cudaFuncSetAttribute(attn_time_kernel<V_>, cudaFuncAttributeMaxDynamicSharedMemorySize, AT_SMEM);
-  BT_AT_VARIANTS(BT_AT_A)
-#undef BT_AT_A
+  const cudaError_t r = cudaFuncSetAttribute(attn_time_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AT_SMEM);
   if (r != cudaSuccess) {
     snprintf(err, errlen, "cudaFuncSetAttribute(attn_time_kernel) failed: %s", cudaGetErrorString(r));
     return -1;

@@ -205,21 +205,6 @@ static int pick_bn(int N, int max_bn) {
   return 0;
 }
 
-template <int BN, int BK, int KIND>
-static int gemm_tc_launch(const TcGemmPlan* p, const EpiParams& e, cudaStream_t st) {
-  using Cfg = TgCfg<BN, BK>;
-  static_assert(Cfg::STAGES >= 2, "pipeline too shallow");
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t r = cudaFuncSetAttribute(gemm_tc_kernel<BN, BK, KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
-    if (r != cudaSuccess) return -1;
-    attr_set = true;
-  }
-  gemm_tc_kernel<BN, BK, KIND><<<p->grid, TG_THREADS, Cfg::SMEM, st>>>(p->tmA, p->tmW, p->g, e, p->num_tiles, p->t_tiles,
-                                                                  p->n_tiles, p->m_tiles);
-  return 0;
-}
-
 TcGemmPlan* tc_gemm_plan_create(const void* A, const void* W, const GemmShape& g, int planes_in, bool resid_epilogue,
                                 char* err, int errlen) {
   TcGemmPlan* p = new TcGemmPlan();
@@ -256,19 +241,24 @@ TcGemmPlan* tc_gemm_plan_create(const void* A, const void* W, const GemmShape& g
 void tc_gemm_plan_destroy(TcGemmPlan* p) { delete p; }
 void tc_gemm_plan_tile(const TcGemmPlan* p, int* bn, int* bk) { *bn = p->BN; *bk = p->BK; }
 
+// Every gemm_tc_kernel instantiation (BN, BK, epilogue kind): tc_init sets their shared-memory limits and
+// launch_gemm_tc dispatches over the same list.  The gates GEMM (kind 2) is N = 32 wide.
+#define BT_GEMM_TC_INSTANCES(X)                                                                                         \
+  X(256, 64, 0) X(256, 64, 1) X(192, 64, 0) X(192, 64, 1) X(128, 64, 0) X(128, 64, 1) X(64, 64, 0) X(64, 64, 1)       \
+  X(32, 64, 0) X(32, 64, 1) X(128, 32, 0) X(128, 32, 1) X(64, 32, 0) X(64, 32, 1) X(32, 32, 0) X(32, 32, 1)             \
+  X(32, 64, 2) X(32, 32, 2)
+
 int launch_gemm_tc(const TcGemmPlan* p, const EpiParams& e, cudaStream_t st) {
-  // the gates GEMM (kind 2) is N = 32 wide
-  if (e.kind == 2) {
-    if (p->BN == 32 && p->BK == 64) return gemm_tc_launch<32, 64, 2>(p, e, st);
-    if (p->BN == 32 && p->BK == 32) return gemm_tc_launch<32, 32, 2>(p, e, st);
-    return -2;
+  const int kind = e.kind == 1 || e.kind == 2 ? e.kind : 0;
+#define BT_TG_LAUNCH(bn, bk, kd)                                                                                       \
+  if (p->BN == bn && p->BK == bk && kind == kd) {                                                                      \
+    static_assert(TgCfg<bn, bk>::STAGES >= 2, "pipeline too shallow");                                               \
+    gemm_tc_kernel<bn, bk, kd><<<p->grid, TG_THREADS, TgCfg<bn, bk>::SMEM, st>>>(p->tmA, p->tmW, p->g, e, p->num_tiles, \
+                                                                                 p->t_tiles, p->n_tiles, p->m_tiles);  \
+    return 0;                                                                                                          \
   }
-#define BT_TG_CASE(bn, bk)                                                      \
-  if (p->BN == bn && p->BK == bk)                                               \
-    return e.kind == 1 ? gemm_tc_launch<bn, bk, 1>(p, e, st) : gemm_tc_launch<bn, bk, 0>(p, e, st);
-  BT_TG_CASE(256, 64) BT_TG_CASE(192, 64) BT_TG_CASE(128, 64) BT_TG_CASE(64, 64) BT_TG_CASE(32, 64)
-  BT_TG_CASE(128, 32) BT_TG_CASE(64, 32) BT_TG_CASE(32, 32)
-#undef BT_TG_CASE
+  BT_GEMM_TC_INSTANCES(BT_TG_LAUNCH)
+#undef BT_TG_LAUNCH
   return -2;
 }
 
@@ -286,7 +276,18 @@ int tc_init(char* err, int errlen) {
   int dev = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
+  cudaError_t r = cudaSuccess;
+#define BT_TG_ATTR(bn, bk, kd)                                                                                         \
+  if (r == cudaSuccess)                                                                                                \
+    r = cudaFuncSetAttribute(gemm_tc_kernel<bn, bk, kd>, cudaFuncAttributeMaxDynamicSharedMemorySize, TgCfg<bn, bk>::SMEM);
+  BT_GEMM_TC_INSTANCES(BT_TG_ATTR)
+#undef BT_TG_ATTR
+  if (r != cudaSuccess) {
+    snprintf(err, errlen, "cudaFuncSetAttribute(gemm_tc_kernel) failed: %s", cudaGetErrorString(r));
+    return -1;
+  }
   if (tc_init_attn(err, errlen) != 0) return -1;
+  if (tc_init_attn_freq(err, errlen) != 0) return -1;
   if (tc_init_fused(err, errlen) != 0) return -1;
   return 0;
 }

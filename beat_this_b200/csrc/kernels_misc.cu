@@ -2,7 +2,6 @@
 // frequency-direction attention, head + aggregation scatter, peak picking.
 #include <cuda_fp16.h>
 #include <cstdlib>
-#include <mutex>
 
 #include "bt_kernels.h"
 #include "common.cuh"
@@ -636,69 +635,77 @@ attn_freq_mma_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_cons
   }
 }
 
-template <int F>
-static int attn_freq_mma_launch(const void* qkv, const float* gates, void* out, int B, int L, float sl2, cudaStream_t st) {
-  constexpr int HEADS = 4 * (32 / F) / FT_TT;
-  constexpr int C = HEADS * 32;
-  constexpr int SMEM = 3 * HEADS * F * FT_TT * 64 + F * FT_TT * C * 2 + 1024 + 64;
-  // tensor maps over the activation buffers, cached per (buffers, geometry)
-  struct Key { const void *q, *o; int B, L; CUtensorMap in, outm; };
-  static Key cache[4];
-  static int n_cached = 0;
-  static std::mutex mu;
-  std::lock_guard<std::mutex> lock(mu);
-  Key* k = nullptr;
-  for (int i = 0; i < n_cached; ++i)
-    if (cache[i].q == qkv && cache[i].o == out && cache[i].B == B && cache[i].L == L) k = &cache[i];
-  if (!k) {
-    k = &cache[n_cached < 4 ? n_cached++ : 0];
-    char err[256];
-    // dimension order (channels, planes, frames): the plane stride is the larger one
-    const uint64_t din[3] = {static_cast<uint64_t>(3 * C), static_cast<uint64_t>(B) * F, static_cast<uint64_t>(L)};
-    const uint64_t sin_[2] = {static_cast<uint64_t>(L) * 3 * C * 2, static_cast<uint64_t>(3 * C) * 2};
-    const uint32_t bin[3] = {32, F, FT_TT};
-    const uint64_t dout[3] = {static_cast<uint64_t>(C), static_cast<uint64_t>(B) * F, static_cast<uint64_t>(L)};
-    const uint64_t sout[2] = {static_cast<uint64_t>(L) * C * 2, static_cast<uint64_t>(C) * 2};
-    const uint32_t bout[3] = {static_cast<uint32_t>(C), F, FT_TT};
-    if (!make_tmap(&k->in, qkv, 3, din, sin_, bin, 64, err, sizeof(err)) || !make_tmap(&k->outm, out, 3, dout, sout, bout, 0, err, sizeof(err))) {
-      fprintf(stderr, "bt: attn_freq tensor map: %s -- using the scalar kernel\n", err);  // never seen; loud if it happens
-      k->q = nullptr;
-      return -1;
-    }
-    k->q = qkv; k->o = out; k->B = B; k->L = L;
+// The (F, heads) pairs of the frontend blocks: the four warps of a CTA cover FT_TT frames x 32 / F heads.
+#define BT_FREQ_TC_INSTANCES(X) X(32) X(16) X(8)
+template <int F> constexpr int freq_tc_heads() { return 4 * (32 / F) / FT_TT; }
+template <int F> constexpr int freq_tc_smem() {
+  return 3 * freq_tc_heads<F>() * F * FT_TT * 64 + F * FT_TT * freq_tc_heads<F>() * 32 * 2 + 1024 + 64;
+}
+
+struct TcFreqPlan {
+  CUtensorMap tmIn;   // qkv [B * F planes, L, 3C], boxes of FT_TT frames x F planes x one head
+  CUtensorMap tmOut;  // out [B * F planes, L, C], boxes of FT_TT frames x F planes x C
+  int B, F, L;
+};
+
+TcFreqPlan* tc_freq_plan_create(const void* qkv, void* out, int B, int F, int L, int heads, char* err, int errlen) {
+  bool ok = false;
+#define BT_FREQ_OK(FF) ok = ok || (F == FF && heads == freq_tc_heads<FF>());
+  BT_FREQ_TC_INSTANCES(BT_FREQ_OK)
+#undef BT_FREQ_OK
+  if (!ok) {
+    snprintf(err, errlen, "frequency attention: no tensor-core kernel for F = %d with %d heads (F = 32, 16, 8 take 1, 2, 4 "
+             "heads)", F, heads);
+    return nullptr;
   }
-  static bool attr = false;
-  if (!attr) { cudaFuncSetAttribute(attn_freq_mma_kernel<F>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM); attr = true; }
-  dim3 grid(ceil_div(L, FT_TT), B);
-  attn_freq_mma_kernel<F><<<grid, 128, SMEM, st>>>(k->in, k->outm, gates, L, HEADS, sl2);
+  TcFreqPlan* p = new TcFreqPlan();
+  p->B = B; p->F = F; p->L = L;
+  const int C = heads * 32;
+  // dimension order (channels, planes, frames): the plane stride is the larger one
+  const uint64_t din[3] = {static_cast<uint64_t>(3 * C), static_cast<uint64_t>(B) * F, static_cast<uint64_t>(L)};
+  const uint64_t sin_[2] = {static_cast<uint64_t>(L) * 3 * C * 2, static_cast<uint64_t>(3 * C) * 2};
+  const uint32_t bin[3] = {32, static_cast<uint32_t>(F), FT_TT};
+  const uint64_t dout[3] = {static_cast<uint64_t>(C), static_cast<uint64_t>(B) * F, static_cast<uint64_t>(L)};
+  const uint64_t sout[2] = {static_cast<uint64_t>(L) * C * 2, static_cast<uint64_t>(C) * 2};
+  const uint32_t bout[3] = {static_cast<uint32_t>(C), static_cast<uint32_t>(F), FT_TT};
+  if (!make_tmap(&p->tmIn, qkv, 3, din, sin_, bin, 64, err, errlen) || !make_tmap(&p->tmOut, out, 3, dout, sout, bout, 0, err, errlen)) {
+    delete p;
+    return nullptr;
+  }
+  return p;
+}
+void tc_freq_plan_destroy(TcFreqPlan* p) { delete p; }
+
+void launch_attn_freq_tc(const TcFreqPlan* p, const float* gates, float scale, cudaStream_t st) {
+  const float sl2 = scale * 1.4426950408889634f;
+  const dim3 grid(ceil_div(p->L, FT_TT), p->B);
+#define BT_FREQ_LAUNCH(FF)                                                                                             \
+  if (p->F == FF)                                                                                                      \
+    attn_freq_mma_kernel<FF><<<grid, 128, freq_tc_smem<FF>(), st>>>(p->tmIn, p->tmOut, gates, p->L, freq_tc_heads<FF>(), sl2);
+  BT_FREQ_TC_INSTANCES(BT_FREQ_LAUNCH)
+#undef BT_FREQ_LAUNCH
+}
+
+int tc_init_attn_freq(char* err, int errlen) {
+  cudaError_t r = cudaSuccess;
+#define BT_FREQ_ATTR(FF) \
+  if (r == cudaSuccess) r = cudaFuncSetAttribute(attn_freq_mma_kernel<FF>, cudaFuncAttributeMaxDynamicSharedMemorySize, freq_tc_smem<FF>());
+  BT_FREQ_TC_INSTANCES(BT_FREQ_ATTR)
+#undef BT_FREQ_ATTR
+  if (r != cudaSuccess) {
+    snprintf(err, errlen, "cudaFuncSetAttribute(attn_freq_mma_kernel) failed: %s", cudaGetErrorString(r));
+    return -1;
+  }
   return 0;
 }
 
-template <typename TAct>
-static void attn_freq_dispatch(const void* qkv, const float* gates, void* out, int B, int F, int L, int heads,
-                               float scale, cudaStream_t st) {
+void launch_attn_freq_simt(const float* qkv, const float* gates, float* out, int B, int F, int L, int heads, float scale,
+                           cudaStream_t st) {
   const int64_t ngrp = static_cast<int64_t>(B) * L * heads;
-  const TAct* q = reinterpret_cast<const TAct*>(qkv);
-  TAct* o = reinterpret_cast<TAct*>(out);
   const unsigned grid = static_cast<unsigned>(ceil_div64(ngrp, 4 * (32 / F)));
-  if (F == 32) attn_freq_kernel<TAct, 32><<<grid, 128, 0, st>>>(q, gates, o, B, L, heads, scale);
-  else if (F == 16) attn_freq_kernel<TAct, 16><<<grid, 128, 0, st>>>(q, gates, o, B, L, heads, scale);
-  else attn_freq_kernel<TAct, 8><<<grid, 128, 0, st>>>(q, gates, o, B, L, heads, scale);
-}
-
-void launch_attn_freq(const void* qkv, const float* gates, void* out, int B, int F, int L, int heads,
-                      float scale, int act_h16, cudaStream_t st) {
-  static const bool simt = getenv("BT_ATTN_FREQ_SIMT") && atoi(getenv("BT_ATTN_FREQ_SIMT")) != 0;
-  if (act_h16 && !simt && (F == 32 || F == 16 || F == 8)) {
-    const float sl2 = scale * 1.4426950408889634f;
-    int rc = -1;
-    if (F == 32 && heads == 1) rc = attn_freq_mma_launch<32>(qkv, gates, out, B, L, sl2, st);
-    else if (F == 16 && heads == 2) rc = attn_freq_mma_launch<16>(qkv, gates, out, B, L, sl2, st);
-    else if (F == 8 && heads == 4) rc = attn_freq_mma_launch<8>(qkv, gates, out, B, L, sl2, st);
-    if (rc == 0) return;
-  }
-  if (act_h16) attn_freq_dispatch<h16>(qkv, gates, out, B, F, L, heads, scale, st);
-  else attn_freq_dispatch<float>(qkv, gates, out, B, F, L, heads, scale, st);
+  if (F == 32) attn_freq_kernel<float, 32><<<grid, 128, 0, st>>>(qkv, gates, out, B, L, heads, scale);
+  else if (F == 16) attn_freq_kernel<float, 16><<<grid, 128, 0, st>>>(qkv, gates, out, B, L, heads, scale);
+  else attn_freq_kernel<float, 8><<<grid, 128, 0, st>>>(qkv, gates, out, B, L, heads, scale);
 }
 
 // ------------------------------------------------------------------------------------------

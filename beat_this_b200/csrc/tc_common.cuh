@@ -199,6 +199,7 @@ extern int g_num_sms;
 bool make_tmap(CUtensorMap* tm, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                const uint32_t* box, int swizzle_bytes, char* err, int errlen);
 int tc_init_attn(char* err, int errlen);
+int tc_init_attn_freq(char* err, int errlen);
 int tc_init_fused(char* err, int errlen);
 
 }  // namespace bt

@@ -302,16 +302,12 @@ int bt_debug_attention(bt_ctx* ctx, const float* q_dev, const float* k_dev, cons
 
 /* Test hook: the frequency-direction attention of B chunks of F planes of L frames: token m = (b * F + f) * L + t
  * attends over the F tokens of its (b, t), gates * softmax(q k^T / sqrt(32)) v per head.  q/k/v/o_dev are
- * [B * F * L, heads * 32] fp32, gates_dev [B * F * L, heads]; F in {8, 16, 32}.  Synchronises the stream. */
+ * [B * F * L, heads * 32] fp32, gates_dev [B * F * L, heads]; F in {8, 16, 32}.  The 16-bit context runs the
+ * tensor-core kernel of the frontend blocks and returns BT_ERR_ARG for any pair other than (F, heads) = (32, 1),
+ * (16, 2), (8, 4).  Synchronises the stream. */
 int bt_debug_attention_freq(bt_ctx* ctx, const float* q_dev, const float* k_dev, const float* v_dev,
                             const float* gates_dev, float* o_dev, int32_t B, int32_t F, int32_t L, int32_t heads,
                             void* stream);
-
-/* Profiling hook: time `iters` launches of the 16-bit time-direction attention kernel on synthetic q|k|v of
- * [seqs, L, heads*32]; variant < 0 keeps the default kernel, otherwise the template parameter V of attn_time_kernel
- * (kernels_attn.cu lists the compiled ones).  *ms_per_launch from CUDA events. */
-int bt_debug_attention_time(bt_ctx* ctx, int32_t seqs, int32_t L, int32_t heads, int32_t variant,
-                            int32_t iters, float* ms_per_launch);
 
 #ifdef __cplusplus
 }
