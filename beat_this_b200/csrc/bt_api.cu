@@ -670,7 +670,7 @@ std::vector<ParamSpec> layer_params(const Layer& l, int64_t D) {
 // ================================================================================== C ABI
 extern "C" {
 
-int bt_version(void) { return 201; }
+int bt_version(void) { return 202; }
 
 const char* bt_act_dtype(void) {
 #if defined(BT_ACT_BF16)
@@ -1302,6 +1302,44 @@ int bt_debug_dbn_viterbi(bt_ctx* c, const double* log_dens_dev, int64_t T, int32
   launch_dbn_backtrace(md, 1, fo_dev, win, 1, bp, res_logp, res_state, nullptr, nullptr, 0, 1.0, nullptr, nullptr, nullptr,
                        path_dev, logp_dev, st);
   BT_LAUNCHED(c, "dbn_backtrace", st);
+  return BT_OK;
+}
+
+static_assert(BT_BEAT_METRIC_COLS == kBeatMetricCols, "bt_beat_metrics row width");
+
+int bt_beat_metrics(bt_ctx* c, const double* est_dev, const int64_t* est_offsets_host, const double* ref_dev,
+                    const int64_t* ref_offsets_host, int32_t n_sets, const bt_beat_metric_params* params, double* out_dev,
+                    void* stream) {
+  if (!c) return BT_ERR_ARG;
+  const char* fn = "bt_beat_metrics";
+  if (n_sets < 0 || !est_offsets_host || !ref_offsets_host || !params) return fail(c, BT_ERR_ARG, "%s: bad argument", fn);
+  const BeatMetricParams p{params->min_beat_time, params->f_window, params->cemgil_sigma, params->phase_threshold,
+                           params->period_threshold};
+  if (!std::isfinite(p.min_beat_time) || !std::isfinite(p.f_window) || !std::isfinite(p.cemgil_sigma) ||
+      !std::isfinite(p.phase_threshold) || !std::isfinite(p.period_threshold))
+    return fail(c, BT_ERR_ARG, "%s: parameters must be finite", fn);
+  for (const int64_t* off : {est_offsets_host, ref_offsets_host}) {
+    if (off[0] < 0) return fail(c, BT_ERR_ARG, "%s: negative offset", fn);
+    for (int i = 0; i < n_sets; ++i)
+      if (off[i + 1] < off[i]) return fail(c, BT_ERR_ARG, "%s: offsets must not decrease", fn);
+  }
+  if (n_sets == 0) return BT_OK;
+  if (!out_dev || (!est_dev && est_offsets_host[n_sets] > 0) || (!ref_dev && ref_offsets_host[n_sets] > 0))
+    return fail(c, BT_ERR_ARG, "%s: null device pointer", fn);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  BT_CUDA(c, cudaSetDevice(c->device));
+  prof_mark(c, st);
+  const size_t half = static_cast<size_t>(n_sets + 1) * sizeof(int64_t);
+  StageSlot* sl = nullptr;
+  int r = acquire_stage(c, 2 * half, &sl);
+  if (r != BT_OK) return r;
+  memcpy(sl->host, est_offsets_host, half);
+  memcpy(static_cast<char*>(sl->host) + half, ref_offsets_host, half);
+  if ((r = upload_stage(c, sl, 2 * half, st)) != BT_OK) return r;
+  const int64_t* off_dev = static_cast<const int64_t*>(sl->dev);
+  if (const int e = launch_beat_metrics(est_dev, off_dev, ref_dev, off_dev + n_sets + 1, n_sets, p, out_dev, st))
+    return fail(c, BT_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(static_cast<cudaError_t>(e)));
+  BT_LAUNCHED(c, "beat_metrics", st);
   return BT_OK;
 }
 

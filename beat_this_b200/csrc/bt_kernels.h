@@ -128,6 +128,17 @@ void launch_dbn_backtrace(const DbnModelDev* models_dev, int n_models, const int
                           const double* act, uint8_t* codes, int correct, double fps, double* times, int32_t* numbers,
                           int64_t* counts, int64_t* path_out, double* logp_out, cudaStream_t st);
 
+// ---- beat-tracking evaluation (kernels_eval.cu) ------------------------------------------------------------------
+// The parameters of bt_beat_metric_params (include/beatthis.h); one row of kBeatMetricCols float64 per set.
+struct BeatMetricParams {
+  double min_beat_time, f_window, cemgil_sigma, phase_threshold, period_threshold;
+};
+constexpr int kBeatMetricCols = 12;
+// Every set s: estimates est[est_off[s], est_off[s+1]), references ref[ref_off[s], ref_off[s+1]) (sorted, finite,
+// non-negative) -> out[s * 12 ..].  Returns a cudaError_t.
+int launch_beat_metrics(const double* est, const int64_t* est_off_dev, const double* ref, const int64_t* ref_off_dev,
+                        int n_sets, const BeatMetricParams& p, double* out, cudaStream_t st);
+
 void launch_f32_to_h16(const float* in, void* out, int64_t n, cudaStream_t st);
 void launch_h16_to_f32(const void* in, float* out, int64_t n, cudaStream_t st);
 // [seqs, L, heads*32] fp32 q,k,v -> packed qkv buffer [seqs*L, 3C] of the activation dtype

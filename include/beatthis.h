@@ -235,6 +235,44 @@ int bt_debug_dbn_viterbi(bt_ctx* ctx, const double* log_dens_dev, int64_t T, int
                          const int32_t* intervals, const double* log_tempo, const int32_t* pointers,
                          int64_t* path_dev, double* logp_dev, void* stream);
 
+/* ---- evaluation: Metrics of model/pl_module.py:320-339 (mir_eval.beat at its defaults) ------------------------- */
+
+typedef struct bt_beat_metric_params {
+  double min_beat_time;    /* trim_beats: times < this are dropped from both arrays (reference eval_trim_beats, 5 s) */
+  double f_window;         /* F-measure hit window [s] (0.07)                                                       */
+  double cemgil_sigma;     /* Cemgil Gaussian width [s] (0.04)                                                      */
+  double phase_threshold;  /* continuity phase threshold (0.175)                                                    */
+  double period_threshold; /* continuity period threshold (0.175)                                                   */
+} bt_beat_metric_params;
+
+#define BT_BEAT_METRIC_COLS 12
+
+/* Beat-tracking scores of n_sets event sets in one launch, one float64 row of BT_BEAT_METRIC_COLS per set at out_dev +
+ * 12 * i: n_ref, n_est (after trimming), matches, P, R, F, cemgil, cemgil_max, CMLc, CMLt, AMLc, AMLt.  Set i is the
+ * estimates est_dev[est_offsets_host[i], est_offsets_host[i+1]) against the references ref_dev[ref_offsets_host[i], ..).
+ * Inputs must be sorted, finite and non-negative (not checked on the device; beat_this_b200/evaluate.py checks).
+ * Contract, in float64, mirroring mir_eval.beat:
+ *  - trim: keep times >= min_beat_time in both arrays; if either is then empty, every score is 0;
+ *  - F-measure: a hit is est - w <= ref <= est + w; matches = size of a maximum matching of hits (greedy over sorted
+ *    refs, each taking the earliest unmatched estimate that holds it); P = matches / n_est, R = matches / n_ref,
+ *    F = 2PR / (P + R), 0 when P + R == 0;
+ *  - variations of the reference: original, off-beat (midpoints r[i] + 0.5 * (r[i+1] - r[i])), double tempo
+ *    (r0, m01, r1, ..., r_{n-1}), half tempo r[0::2], half tempo r[1::2];
+ *  - Cemgil per variation: sum over its beats of exp(-(d*d) / (2 sigma^2)), d = distance to the nearest estimate, over
+ *    0.5 * (n_est + n_variation); cemgil = original, cemgil_max = best of the five;
+ *  - continuity per variation: estimate m takes nearest = the lowest index at minimal |e_m - r| (np.argmin).  When
+ *    m == 0 or nearest == 0 the intervals are forward (r[k+1] - r[k], e[m+1] - e[m], backward at the last element;
+ *    both 0 for a one-element array, as Python's x[-1] makes them), otherwise backward.  m is a candidate when
+ *    |d / ref_int| < phase_threshold and |1 - est_int / ref_int| < period_threshold (a zero ref_int fails), and
+ *    succeeds when no earlier estimate with the same nearest was a candidate.  Over L = max(n_variation, n_est):
+ *    CMLc = longest run of successes / L, CMLt = successes / L on the original; AMLc, AMLt = maxima over the five.
+ *    A variation with no beats scores 0 (mir_eval raises there: argmin of an empty array).
+ * BT_ERR_ARG, before anything is enqueued, for n_sets < 0, null pointers, offsets that are negative or decrease, or
+ * non-finite parameters.  Works on a weight-less ctx.  Enqueues only: no synchronisation. */
+int bt_beat_metrics(bt_ctx* ctx, const double* est_dev, const int64_t* est_offsets_host, const double* ref_dev,
+                    const int64_t* ref_offsets_host, int32_t n_sets, const bt_beat_metric_params* params,
+                    double* out_dev, void* stream);
+
 /* ---- introspection / tuning ----------------------------------------------------------------- */
 
 /* Upper bound on the chunks processed per wave (default 128; one wave = one launch of every
