@@ -17,6 +17,7 @@
 
 #include "../../include/beatthis.h"
 #include "bt_kernels.h"
+#include "cuda_owned.h"
 #include "dbn_model.h"
 
 using namespace bt;
@@ -24,9 +25,9 @@ using namespace bt;
 namespace {
 
 struct Param {
-  float* f32 = nullptr;
-  void* b16 = nullptr;
-  int32_t* i32 = nullptr;
+  DeviceBuffer<float> f32;
+  DeviceBuffer<> b16;
+  DeviceBuffer<int32_t> i32;
   int64_t n = 0;
 };
 
@@ -46,22 +47,31 @@ struct Layer {
 // waited for when it comes round again, kStageSlots uploads later, so no API call blocks on earlier GPU work
 constexpr int kStageSlots = 16;
 struct StageSlot {
-  void* host = nullptr;
-  void* dev = nullptr;
-  size_t cap = 0;
-  cudaEvent_t ev = nullptr;
+  PinnedBuffer<char> host;
+  DeviceBuffer<char> dev;
+  Event ev;
   bool pending = false;
 };
 
 // Tensor-core plans of one layer for one (wave size, chunk length) geometry: what its launches use, nothing else.
 struct LayerPlans {
-  TcQkvPlan* fqkv = nullptr;                                    // attention, fused (C = 32 / 64)
-  TcGemmPlan *gates = nullptr, *qkv = nullptr, *out = nullptr;  // attention: gates and QKV unless fused; out-projection
-  TcAttnPlan* attn = nullptr;                                   // time attention
-  TcFreqPlan* freq = nullptr;                                   // frequency attention
-  TcFfPlan *ff = nullptr, *ff_op = nullptr;                     // FFN, fused; ff_op: after a frontend attention
-  TcGemmPlan *ff1 = nullptr, *ff2 = nullptr;                    // FFN, unfused
-  TcGemmPlan* gemm = nullptr;                                   // convolution, frontend.linear
+  QkvPlan fqkv;              // attention, fused (C = 32 / 64)
+  GemmPlan gates, qkv, out;  // attention: gates and QKV unless fused; out-projection
+  AttnPlan attn;             // time attention
+  FreqPlan freq;             // frequency attention
+  FfPlan ff, ff_op;          // FFN, fused; ff_op: after a frontend attention
+  GemmPlan ff1, ff2;         // FFN, unfused
+  GemmPlan gemm;             // convolution, frontend.linear
+};
+
+// The activations of a wave of up to `chunks` chunks of BT_CHUNK frames (XB only on the 16-bit path), and the
+// tensor-core plans made for them: their tensor maps hold workspace addresses, so the two are dropped together.
+struct Workspace {
+  int chunks = 0;
+  DeviceBuffer<float> X0, X1, GATES;
+  DeviceBuffer<> XB, XN, QKV, O, H;
+  std::map<std::pair<int, int>, std::vector<LayerPlans>> plans;  // per (nb, L) geometry, parallel to bt_ctx::layers
+  std::vector<std::pair<int, int>> plan_order;                   // insertion order: oldest geometry is evicted first
 };
 
 char g_create_error[512] = "";
@@ -78,20 +88,14 @@ struct bt_ctx {
   int64_t launches = 0;
   bool sync_debug = false;
 
-  // workspace: sized for ws_wave chunks of BT_CHUNK frames; grows on demand up to `wave`
-  int wave = 128;
-  int ws_wave = 0;
-  float *X0 = nullptr, *X1 = nullptr, *GATES = nullptr;
-  void *XB = nullptr, *XN = nullptr, *QKV = nullptr, *O = nullptr, *H = nullptr;
+  int wave = 128;  // the workspace grows on demand up to `wave` chunks
+  Workspace ws;
   // spectrogram scratch for bt_audio2frames
-  float* spect_ws = nullptr;
-  int64_t spect_cap = 0;
+  DeviceBuffer<float> spect_ws;
   // DBN scratch for bt_dbn_track_device / bt_debug_dbn_viterbi (grows on demand): activations, densities, windows,
   // per-model results and path codes; back pointers
-  void* dbn_ws = nullptr;
-  size_t dbn_ws_cap = 0;
-  void* dbn_bp = nullptr;
-  size_t dbn_bp_cap = 0;
+  DeviceBuffer<char> dbn_ws;
+  DeviceBuffer<uint8_t> dbn_bp;
   // pinned staging + device tables
   StageSlot stage[kStageSlots];
   int stage_next = 0;
@@ -100,13 +104,10 @@ struct bt_ctx {
   const Param *rope_cos = nullptr, *rope_sin = nullptr, *bn1_scale = nullptr, *bn1_shift = nullptr, *stem_w = nullptr,
               *stem_b = nullptr, *head_w = nullptr, *head_b = nullptr;
 
-  std::map<std::pair<int, int>, std::vector<LayerPlans>> plans;  // parallel to `layers`
-  std::vector<std::pair<int, int>> plan_order;  // insertion order: oldest geometry is evicted first
-
   // per-kernel-class device timing (bt_profile_*): one event after every launch; the
   // duration of a launch is the gap to the previous event on the same stream
   bool prof = false;
-  std::vector<cudaEvent_t> ev_pool;
+  std::vector<Event> ev_pool;
   size_t ev_used = 0;
   struct ProfRec { int kind; int ev; int prev; };
   std::vector<ProfRec> prof_recs;
@@ -145,10 +146,10 @@ int prof_event(bt_ctx* c, cudaStream_t st) {
   if (c->ev_used == c->ev_pool.size()) {
     cudaEvent_t ev;
     if (cudaEventCreate(&ev) != cudaSuccess) return -1;
-    c->ev_pool.push_back(ev);
+    c->ev_pool.emplace_back(ev);
   }
   const int idx = static_cast<int>(c->ev_used++);
-  cudaEventRecord(c->ev_pool[idx], st);
+  cudaEventRecord(c->ev_pool[idx].get(), st);
   return idx;
 }
 
@@ -217,58 +218,47 @@ int acquire_stage(bt_ctx* c, size_t bytes, StageSlot** out) {
   StageSlot* sl = &c->stage[c->stage_next];
   c->stage_next = (c->stage_next + 1) % kStageSlots;
   if (sl->pending) {  // kStageSlots uploads ago: long finished unless the caller is that far ahead of the GPU
-    BT_CUDA(c, cudaEventSynchronize(sl->ev));
+    BT_CUDA(c, cudaEventSynchronize(sl->ev.get()));
     sl->pending = false;
   }
-  if (!sl->ev) BT_CUDA(c, cudaEventCreateWithFlags(&sl->ev, cudaEventDisableTiming));
-  if (bytes > sl->cap) {
-    if (sl->host) cudaFreeHost(sl->host);
-    if (sl->dev) cudaFree(sl->dev);
-    sl->host = sl->dev = nullptr;
-    sl->cap = 0;
-    const size_t cap = std::max<size_t>(bytes * 2, 1 << 16);
-    BT_CUDA(c, cudaMallocHost(&sl->host, cap));
-    BT_CUDA(c, cudaMalloc(&sl->dev, cap));
-    sl->cap = cap;
+  if (!sl->ev) {
+    cudaEvent_t ev;
+    BT_CUDA(c, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+    sl->ev.reset(ev);
   }
+  const size_t cap = std::max<size_t>(bytes * 2, 1 << 16);
+  BT_CUDA(c, sl->host.reserve(bytes, cap));
+  BT_CUDA(c, sl->dev.reserve(bytes, cap));
   *out = sl;
   return BT_OK;
 }
 
 int upload_stage(bt_ctx* c, StageSlot* sl, size_t bytes, cudaStream_t st) {
-  BT_CUDA(c, cudaMemcpyAsync(sl->dev, sl->host, bytes, cudaMemcpyHostToDevice, st));
-  BT_CUDA(c, cudaEventRecord(sl->ev, st));
+  BT_CUDA(c, cudaMemcpyAsync(sl->dev.get(), sl->host.get(), bytes, cudaMemcpyHostToDevice, st));
+  BT_CUDA(c, cudaEventRecord(sl->ev.get(), st));
   sl->pending = true;
   return BT_OK;
 }
 
-void free_ws(bt_ctx* c) {
-  void** ptrs[] = {reinterpret_cast<void**>(&c->X0), reinterpret_cast<void**>(&c->X1),
-                   reinterpret_cast<void**>(&c->GATES), &c->XB, &c->XN, &c->QKV, &c->O, &c->H};
-  for (auto p : ptrs) {
-    if (*p) cudaFree(*p);
-    *p = nullptr;
-  }
-  c->ws_wave = 0;
-}
+inline size_t align16(size_t v) { return (v + 15) & ~static_cast<size_t>(15); }
 
-void destroy_plans(std::vector<LayerPlans>& v) {
-  for (LayerPlans& p : v) {
-    if (p.fqkv) tc_qkv_plan_destroy(p.fqkv);
-    for (TcGemmPlan* g : {p.gates, p.qkv, p.out, p.ff1, p.ff2, p.gemm})
-      if (g) tc_gemm_plan_destroy(g);
-    if (p.attn) tc_attn_plan_destroy(p.attn);
-    if (p.freq) tc_freq_plan_destroy(p.freq);
-    if (p.ff) tc_ff_plan_destroy(p.ff);
-    if (p.ff_op) tc_ff_plan_destroy(p.ff_op);
+// Copies a few host arrays of n[k] elements into the next ring slot, each at a 16-byte aligned offset, and uploads the
+// slot: dev[k] is array k on the device.
+template <class T>
+int stage(bt_ctx* c, cudaStream_t st, std::initializer_list<std::pair<const T*, size_t>> arrays, const T** dev) {
+  size_t bytes = 0;
+  for (const auto& a : arrays) bytes = align16(bytes) + sizeof(T) * a.second;
+  StageSlot* sl = nullptr;
+  const int r = acquire_stage(c, bytes, &sl);
+  if (r != BT_OK) return r;
+  size_t off = 0;
+  for (const auto& a : arrays) {
+    off = align16(off);
+    memcpy(sl->host.get() + off, a.first, sizeof(T) * a.second);
+    *dev++ = reinterpret_cast<const T*>(sl->dev.get() + off);
+    off += sizeof(T) * a.second;
   }
-  v.clear();
-}
-
-void free_plans(bt_ctx* c) {
-  for (auto& kv : c->plans) destroy_plans(kv.second);
-  c->plans.clear();
-  c->plan_order.clear();
+  return upload_stage(c, sl, bytes, st);
 }
 
 // elements per chunk of the largest frontend activation: F*L*C is the same for all blocks
@@ -276,31 +266,30 @@ int64_t front_elems(const bt_ctx* c) {
   return static_cast<int64_t>(c->hp.spect_dim / 4) * BT_CHUNK * c->hp.stem_dim;
 }
 
-int ensure_ws(bt_ctx* c, int need_chunks) {
+int ensure_ws(bt_ctx* c) {
   // sized once for a full wave (bt_set_wave_chunks; ~46 MB per 1500-frame chunk on the 16-bit path): growing later
-  // would mean cudaFree / cudaMalloc -- device-wide synchronisation -- in the middle of a stream of batches
-  (void)need_chunks;
+  // would mean freeing and allocating device memory -- device-wide synchronisation -- amid a stream of batches
   const int want = c->wave;
-  if (want <= c->ws_wave) return BT_OK;
-  free_ws(c);
-  free_plans(c);
+  if (want <= c->ws.chunks) return BT_OK;
+  c->ws = Workspace();  // the old blocks are freed before the new ones are allocated
   const int64_t G = want;
   const int64_t fe = front_elems(c);                                     // 1.536M
   const int64_t D = c->hp.transformer_dim;
   const int64_t me = static_cast<int64_t>(BT_CHUNK) * D;                 // main tokens * dim
   const int64_t xe = std::max(fe, me);
   const size_t act = c->dtype == BT_DTYPE_H16 ? 2 : 4;
-  BT_CUDA(c, cudaMalloc(&c->X0, G * xe * 4));
-  BT_CUDA(c, cudaMalloc(&c->X1, G * xe * 4));
-  BT_CUDA(c, cudaMalloc(&c->GATES, G * std::max<int64_t>(fe / 32, BT_CHUNK * (D / 32)) * 4));
-  BT_CUDA(c, cudaMalloc(&c->XN, G * xe * act));
-  BT_CUDA(c, cudaMalloc(&c->QKV, G * 3 * xe * act));
-  BT_CUDA(c, cudaMalloc(&c->O, G * xe * act));
-  BT_CUDA(c, cudaMalloc(&c->H, G * 4 * xe * act));
+  Workspace& ws = c->ws;
+  BT_CUDA(c, ws.X0.alloc(G * xe * 4));
+  BT_CUDA(c, ws.X1.alloc(G * xe * 4));
+  BT_CUDA(c, ws.GATES.alloc(G * std::max<int64_t>(fe / 32, BT_CHUNK * (D / 32)) * 4));
+  BT_CUDA(c, ws.XN.alloc(G * xe * act));
+  BT_CUDA(c, ws.QKV.alloc(G * 3 * xe * act));
+  BT_CUDA(c, ws.O.alloc(G * xe * act));
+  BT_CUDA(c, ws.H.alloc(G * 4 * xe * act));
   if (c->dtype == BT_DTYPE_H16) {
-    BT_CUDA(c, cudaMalloc(&c->XB, G * xe * 2));
+    BT_CUDA(c, ws.XB.alloc(G * xe * 2));
   }
-  c->ws_wave = want;
+  ws.chunks = want;
   return BT_OK;
 }
 
@@ -335,7 +324,7 @@ int run_gemm(bt_ctx* c, const void* A, const Param* W, TcGemmPlan* plan, const G
   if (c->dtype == BT_DTYPE_H16) {
     if (launch_gemm_tc(plan, e, st) != 0) return fail(c, BT_ERR_CUDA, "tc gemm launch %s failed", what);
   } else {
-    launch_gemm_simt(reinterpret_cast<const float*>(A), W->f32, g, e, st);
+    launch_gemm_simt(reinterpret_cast<const float*>(A), W->f32.get(), g, e, st);
   }
   BT_LAUNCHED(c, what, st);
   return BT_OK;
@@ -345,7 +334,7 @@ EpiParams epi_generic(const Param* bias, int gelu, const float* resid, int ldr, 
                       void* out_act, int ldoa) {
   EpiParams e{};
   e.kind = 0;
-  e.bias = bias ? bias->f32 : nullptr;
+  e.bias = bias ? bias->f32.get() : nullptr;
   e.gelu = gelu;
   e.resid = resid; e.ldr = ldr;
   e.out_f32 = out_f32; e.ldo_f32 = ldo32;
@@ -368,6 +357,7 @@ bool outproj_in_ff(const bt_ctx* c, const std::vector<LayerPlans>* wp, size_t i)
 // kAttnF: sequences run over the F planes of each chunk (PartialFTTransformer attnF).
 int attention_block(bt_ctx* c, float* X, const Layer& l, const LayerPlans* tp, int nb, int L, bool out_in_ff,
                     const ChunkSrc* vl_chunks, cudaStream_t st) {
+  const Workspace& ws = c->ws;
   const bool tc = c->dtype == BT_DTYPE_H16;
   const bool freq = l.kind == kAttnF, front = l.F > 1;
   const int C = l.C, F = l.F, heads = C / kHeadDim, planes = nb * F;
@@ -377,80 +367,83 @@ int attention_block(bt_ctx* c, float* X, const Layer& l, const LayerPlans* tp, i
   const float qscale = tc && !freq ? inv_sqrt_d * 1.4426950408889634f : 1.0f;
   int r = BT_OK;
   if (tc && fused(l)) {  // norm + gates + QKV + RoPE in one kernel
-    if (launch_fused_qkv(tp->fqkv, X, wg->f32, bg->f32, c->rope_cos->f32, c->rope_sin->f32, c->QKV, c->GATES, L, F,
-                         freq ? 1 : 0, qscale, st) != 0)
+    if (launch_fused_qkv(tp->fqkv.get(), X, wg->f32.get(), bg->f32.get(), c->rope_cos->f32.get(), c->rope_sin->f32.get(),
+                         ws.QKV.get(), ws.GATES.get(), L, F, freq ? 1 : 0, qscale, st) != 0)
       return fail(c, BT_ERR_CUDA, "fused qkv launch failed");
     BT_LAUNCHED(c, C == 32 ? "qkv_fused_c32" : "qkv_fused_c64", st);
   } else {
     // up to 2 heads (fp32 path only: the 16-bit path fuses those blocks): gates inside the norm kernel;
     // otherwise from a padded gates GEMM
     const bool gates_in_norm = heads <= 2;
-    launch_norm(X, c->XN, M, C, tc, st, gates_in_norm ? c->GATES : nullptr, wg->f32, bg->f32, heads);
+    launch_norm(X, ws.XN.get(), M, C, tc, st, gates_in_norm ? ws.GATES.get() : nullptr, wg->f32.get(), bg->f32.get(),
+                heads);
     BT_LAUNCHED(c, gates_in_norm ? "norm_gates" : (front ? "norm_front" : "norm"), st);
     if (!gates_in_norm) {  // gates = sigmoid(to_gates(x_normed)): a [heads -> 32 padded] x C GEMM on the same rows
       GemmShape gg = plain_shape(planes, L, 32, C, C);
       EpiParams eg{};
       eg.kind = 2;
-      eg.bias = bg->f32;
+      eg.bias = bg->f32.get();
       eg.heads = heads;
-      eg.out_f32 = c->GATES;
-      int rg = run_gemm(c, c->XN, wg, tp ? tp->gates : nullptr, gg, eg, front ? "gemm_gates_front" : "gemm_gates", st);
+      eg.out_f32 = ws.GATES.get();
+      int rg = run_gemm(c, ws.XN.get(), wg, tp->gates.get(), gg, eg, front ? "gemm_gates_front" : "gemm_gates", st);
       if (rg != BT_OK) return rg;
     }
     EpiParams e{};
     e.kind = 1;
-    e.out_act = c->QKV; e.ldo_act = 3 * C;
-    e.rope_cos = c->rope_cos->f32;
-    e.rope_sin = c->rope_sin->f32;
+    e.out_act = ws.QKV.get(); e.ldo_act = 3 * C;
+    e.rope_cos = c->rope_cos->f32.get();
+    e.rope_sin = c->rope_sin->f32.get();
     e.C = C; e.heads = heads; e.posmode = freq ? 1 : 0; e.F = F;
     e.qscale = qscale;
     GemmShape g = plain_shape(planes, L, 3 * C, C, C);
-    r = run_gemm(c, c->XN, wqkv, tp ? tp->qkv : nullptr, g, e, front ? "gemm_qkv_front" : "gemm_qkv", st);
+    r = run_gemm(c, ws.XN.get(), wqkv, tp->qkv.get(), g, e, front ? "gemm_qkv_front" : "gemm_qkv", st);
     if (r != BT_OK) return r;
   }
   if (freq) {
-    if (tc) launch_attn_freq_tc(tp->freq, c->GATES, inv_sqrt_d, st);
-    else launch_attn_freq_simt(reinterpret_cast<const float*>(c->QKV), c->GATES, reinterpret_cast<float*>(c->O), nb, F, L,
-                               heads, inv_sqrt_d, st);
+    if (tc) launch_attn_freq_tc(tp->freq.get(), ws.GATES.get(), inv_sqrt_d, st);
+    else launch_attn_freq_simt(static_cast<const float*>(ws.QKV.get()), ws.GATES.get(), static_cast<float*>(ws.O.get()),
+                               nb, F, L, heads, inv_sqrt_d, st);
     BT_LAUNCHED(c, "attn_freq", st);
   } else if (tc) {
-    launch_attn_time_tc(tp->attn, c->GATES, c->O, st, vl_chunks, F);
+    launch_attn_time_tc(tp->attn.get(), ws.GATES.get(), ws.O.get(), st, vl_chunks, F);
     BT_LAUNCHED(c, "attn_time_tc", st);
   } else {
-    launch_attn_time_simt(reinterpret_cast<const float*>(c->QKV), c->GATES, reinterpret_cast<float*>(c->O),
+    launch_attn_time_simt(static_cast<const float*>(ws.QKV.get()), ws.GATES.get(), static_cast<float*>(ws.O.get()),
                           planes, L, heads, st, vl_chunks, F);
     BT_LAUNCHED(c, "attn_time_simt", st);
   }
   if (out_in_ff) return BT_OK;
   GemmShape go = plain_shape(planes, L, C, C, C);
   EpiParams eo = epi_generic(nullptr, 0, X, C, X, C, nullptr, 0);
-  return run_gemm(c, c->O, wout, tp ? tp->out : nullptr, go, eo, front ? "gemm_attn_out_front" : "gemm_attn_out", st);
+  return run_gemm(c, ws.O.get(), wout, tp->out.get(), go, eo, front ? "gemm_attn_out_front" : "gemm_attn_out", st);
 }
 
 // x += ff(x) (reference roformer.py:38-61); optionally also writes a 16-bit copy of the result.  with_outproj: the
 // fused kernel first adds the out-projection of the attention in front (LayerPlans::ff_op).
 int ff_block(bt_ctx* c, float* X, const Layer& l, const LayerPlans* tp, int nb, int L, bool with_outproj,
              void* copy_act, cudaStream_t st) {
+  const Workspace& ws = c->ws;
   const bool tc = c->dtype == BT_DTYPE_H16;
   const bool front = l.F > 1;
   const int C = l.C, mult = l.mult, planes = nb * l.F;
   const Param *w1 = l.w[0], *b1 = l.w[1], *w2 = l.w[2], *b2 = l.w[3];
   const int64_t M = static_cast<int64_t>(planes) * L;
   if (tc && fused(l)) {
-    if (launch_fused_ff(with_outproj ? tp->ff_op : tp->ff, X, b1->f32, b2->f32, copy_act, st) != 0)
+    const TcFfPlan* plan = with_outproj ? tp->ff_op.get() : tp->ff.get();
+    if (launch_fused_ff(plan, X, b1->f32.get(), b2->f32.get(), copy_act, st) != 0)
       return fail(c, BT_ERR_CUDA, "fused ff launch failed");
     BT_LAUNCHED(c, C == 32 ? "ff_fused_c32" : "ff_fused_c64", st);
     return BT_OK;
   }
-  launch_norm(X, c->XN, M, C, tc, st);
+  launch_norm(X, ws.XN.get(), M, C, tc, st);
   BT_LAUNCHED(c, front ? "norm_front" : "norm", st);
   GemmShape g1 = plain_shape(planes, L, mult * C, C, C);
-  EpiParams e1 = epi_generic(b1, 1, nullptr, 0, nullptr, 0, c->H, mult * C);
-  int r = run_gemm(c, c->XN, w1, tp ? tp->ff1 : nullptr, g1, e1, front ? "gemm_ff1_front" : "gemm_ff1", st);
+  EpiParams e1 = epi_generic(b1, 1, nullptr, 0, nullptr, 0, ws.H.get(), mult * C);
+  int r = run_gemm(c, ws.XN.get(), w1, tp->ff1.get(), g1, e1, front ? "gemm_ff1_front" : "gemm_ff1", st);
   if (r != BT_OK) return r;
   GemmShape g2 = plain_shape(planes, L, C, mult * C, mult * C);
   EpiParams e2 = epi_generic(b2, 0, X, C, X, C, copy_act, C);
-  return run_gemm(c, c->H, w2, tp ? tp->ff2 : nullptr, g2, e2, front ? "gemm_ff2_front" : "gemm_ff2", st);
+  return run_gemm(c, ws.H.get(), w2, tp->ff2.get(), g2, e2, front ? "gemm_ff2_front" : "gemm_ff2", st);
 }
 
 GemmShape conv_shape(int nb, int F, int L, int C) {
@@ -473,89 +466,93 @@ GemmShape lin_shape(int nb, int L, int D, int Fo, int Co) {
 // the 16-bit plans of layer i for waves of nb chunks of L frames; false (message in err) when one cannot be made
 bool make_layer_plans(const bt_ctx* c, size_t i, int nb, int L, LayerPlans& p, char* err, int errlen) {
   const Layer& l = c->layers[i];
+  const Workspace& ws = c->ws;
   const int C = l.C, planes = nb * l.F;
   const int64_t M = static_cast<int64_t>(planes) * L;
   auto gemm = [&](const void* A, const Param* W, const GemmShape& g, bool resid = false) {
-    return tc_gemm_plan_create(A, W->b16, g, planes, resid, err, errlen);
+    return GemmPlan(tc_gemm_plan_create(A, W->b16.get(), g, planes, resid, err, errlen));
   };
   switch (l.kind) {
     case kConv:
-      return (p.gemm = gemm(c->XB, l.w[0], conv_shape(nb, l.F, L, C))) != nullptr;
+      return (p.gemm = gemm(ws.XB.get(), l.w[0], conv_shape(nb, l.F, L, C))) != nullptr;
     case kLin:
-      return (p.gemm = gemm(c->XN, l.w[0], lin_shape(nb, L, c->hp.transformer_dim, l.F, C))) != nullptr;
+      return (p.gemm = gemm(ws.XN.get(), l.w[0], lin_shape(nb, L, c->hp.transformer_dim, l.F, C))) != nullptr;
     case kFf:
       if (fused(l)) {
-        p.ff = tc_ff_plan_create(l.w[0]->b16, l.w[2]->b16, C, M, nullptr, nullptr, err, errlen);
+        const void *w1 = l.w[0]->b16.get(), *w2 = l.w[2]->b16.get();
+        p.ff.reset(tc_ff_plan_create(w1, w2, C, M, nullptr, nullptr, err, errlen));
         const Layer& prev = c->layers[i - 1];
         if (prev.kind == kAttnF || prev.kind == kAttnT)  // ... and with the out-projection of the frontend attention in front
-          p.ff_op = tc_ff_plan_create(l.w[0]->b16, l.w[2]->b16, C, M, c->O, prev.w[3]->b16, err, errlen);
+          p.ff_op.reset(tc_ff_plan_create(w1, w2, C, M, ws.O.get(), prev.w[3]->b16.get(), err, errlen));
         return p.ff && (p.ff_op || prev.kind == kAttn);
       }
-      p.ff1 = gemm(c->XN, l.w[0], plain_shape(planes, L, l.mult * C, C, C));
-      p.ff2 = gemm(c->H, l.w[2], plain_shape(planes, L, C, l.mult * C, l.mult * C), true);
+      p.ff1 = gemm(ws.XN.get(), l.w[0], plain_shape(planes, L, l.mult * C, C, C));
+      p.ff2 = gemm(ws.H.get(), l.w[2], plain_shape(planes, L, C, l.mult * C, l.mult * C), true);
       return p.ff1 && p.ff2;
     default:  // attention
       if (fused(l)) {
-        if (!(p.fqkv = tc_qkv_plan_create(l.w[0]->b16, C, M, err, errlen))) return false;
+        p.fqkv.reset(tc_qkv_plan_create(l.w[0]->b16.get(), C, M, err, errlen));
+        if (!p.fqkv) return false;
       } else {
-        p.gates = gemm(c->XN, l.w[1], plain_shape(planes, L, 32, C, C));
-        p.qkv = gemm(c->XN, l.w[0], plain_shape(planes, L, 3 * C, C, C));
+        p.gates = gemm(ws.XN.get(), l.w[1], plain_shape(planes, L, 32, C, C));
+        p.qkv = gemm(ws.XN.get(), l.w[0], plain_shape(planes, L, 3 * C, C, C));
         if (!p.gates || !p.qkv) return false;
       }
-      if (l.kind == kAttnF) {
-        if (!(p.freq = tc_freq_plan_create(c->QKV, c->O, nb, l.F, L, C / kHeadDim, err, errlen))) return false;
-      } else if (!(p.attn = tc_attn_plan_create(c->QKV, planes, L, C / kHeadDim, err, errlen))) {
-        return false;
-      }
-      return (p.out = gemm(c->O, l.w[3], plain_shape(planes, L, C, C, C), true)) != nullptr;
+      const int heads = C / kHeadDim;
+      if (l.kind == kAttnF) p.freq.reset(tc_freq_plan_create(ws.QKV.get(), ws.O.get(), nb, l.F, L, heads, err, errlen));
+      else p.attn.reset(tc_attn_plan_create(ws.QKV.get(), planes, L, heads, err, errlen));
+      if (!p.freq && !p.attn) return false;
+      return (p.out = gemm(ws.O.get(), l.w[3], plain_shape(planes, L, C, C, C), true)) != nullptr;
   }
 }
 
 int build_plans(bt_ctx* c, int nb, int L, std::vector<LayerPlans>** out) {
   auto key = std::make_pair(nb, L);
-  auto it = c->plans.find(key);
-  if (it != c->plans.end()) { *out = &it->second; return BT_OK; }
+  Workspace& ws = c->ws;
+  auto it = ws.plans.find(key);
+  if (it != ws.plans.end()) { *out = &it->second; return BT_OK; }
   // bounded cache: tensor maps are copied into the kernel parameters at launch, so dropping the oldest geometry is
   // safe while its kernels are still in flight
   constexpr size_t kMaxPlans = 48;
-  while (c->plans.size() >= kMaxPlans && !c->plan_order.empty()) {
-    auto old = c->plans.find(c->plan_order.front());
-    if (old != c->plans.end()) { destroy_plans(old->second); c->plans.erase(old); }
-    c->plan_order.erase(c->plan_order.begin());
+  while (ws.plans.size() >= kMaxPlans && !ws.plan_order.empty()) {
+    auto old = ws.plans.find(ws.plan_order.front());
+    if (old != ws.plans.end()) ws.plans.erase(old);
+    ws.plan_order.erase(ws.plan_order.begin());
   }
   std::vector<LayerPlans> v(c->layers.size());
   char err[512] = "";
   for (size_t i = 0; i < v.size(); ++i) {
-    if (!make_layer_plans(c, i, nb, L, v[i], err, sizeof(err))) {  // never cache a half-built entry
-      destroy_plans(v);
+    if (!make_layer_plans(c, i, nb, L, v[i], err, sizeof(err)))  // never cache a half-built entry
       return fail(c, BT_ERR_CUDA, "tensor-core plan creation failed (%s): %s", c->layers[i].name.c_str(), err);
-    }
   }
-  c->plan_order.push_back(key);
-  *out = &(c->plans[key] = std::move(v));
+  ws.plan_order.push_back(key);
+  *out = &(ws.plans[key] = std::move(v));
   return BT_OK;
 }
 
 // BeatThis.forward for one wave of nb equal-length chunks, scattering the head output.
 int run_wave(bt_ctx* c, const float* spect, const Wave& wv, float* beat, float* down, cudaStream_t st) {
   const bool tc = c->dtype == BT_DTYPE_H16;
+  const Workspace& ws = c->ws;
   const int nb = wv.nb, L = wv.L;
+  static const LayerPlans kNoPlans{};  // the fp32 path's launches take no plans
   std::vector<LayerPlans>* wp = nullptr;
   int r;
   if (tc && (r = build_plans(c, nb, L, &wp)) != BT_OK) return r;
-  float* X = c->X0;
-  float* Xalt = c->X1;
+  float* X = ws.X0.get();
+  float* Xalt = ws.X1.get();
   // chunks shorter than the wave's padded length: the time attentions mask their missing keys and the convolutions
   // see zeros beyond their last frame (everything else works row by row, padding rows are never read back)
   const ChunkSrc* vl = wv.varlen ? wv.chunks_dev : nullptr;
-  launch_stem(spect, wv.chunks_dev, nb, L, c->bn1_scale->f32, c->bn1_shift->f32, c->stem_w->f32, c->stem_b->f32, X, st);
+  launch_stem(spect, wv.chunks_dev, nb, L, c->bn1_scale->f32.get(), c->bn1_shift->f32.get(), c->stem_w->f32.get(),
+              c->stem_b->f32.get(), X, st);
   BT_LAUNCHED(c, "stem", st);
   if ((r = do_tap(c, "stem", X, static_cast<int64_t>(nb) * (c->hp.spect_dim / 4) * L * c->hp.stem_dim, false, st)) != BT_OK)
     return r;
   const std::vector<Layer>& layers = c->layers;
   for (size_t i = 0; i < layers.size(); ++i) {
     const Layer& l = layers[i];
-    const LayerPlans* tp = wp ? &(*wp)[i] : nullptr;
+    const LayerPlans* tp = wp ? &(*wp)[i] : &kNoPlans;
     const char* tap = l.name.c_str();
     const void* out = X;  // the layer's output (tap)
     bool out_act = false;
@@ -565,23 +562,24 @@ int run_wave(bt_ctx* c, const float* spect, const Wave& wv, float* beat, float* 
     } else if (l.kind == kFf) {
       // the FFN in front of a convolution also writes the 16-bit copy the convolution reads
       const bool before_conv = i + 1 < layers.size() && layers[i + 1].kind == kConv;
-      r = ff_block(c, X, l, tp, nb, L, outproj_in_ff(c, wp, i - 1), tc && before_conv ? c->XB : nullptr, st);
+      r = ff_block(c, X, l, tp, nb, L, outproj_in_ff(c, wp, i - 1), tc && before_conv ? ws.XB.get() : nullptr, st);
     } else if (l.kind == kConv) {
       if (tc && (i == 0 || layers[i - 1].kind != kFf)) {  // no FFN in front (no partial transformers)
-        launch_f32_to_h16(X, c->XB, elems, st);
+        launch_f32_to_h16(X, ws.XB.get(), elems, st);
         BT_LAUNCHED(c, "f32_to_h16", st);
       }
       if (vl) {
-        launch_zero_tail(tc ? c->XB : static_cast<void*>(X), tc ? 2 : 4, vl, nb, l.F, L, l.C, st);
+        launch_zero_tail(tc ? ws.XB.get() : static_cast<void*>(X), tc ? 2 : 4, vl, nb, l.F, L, l.C, st);
         BT_LAUNCHED(c, "zero_tail", st);
       }
       // conv C -> 2C (+ folded BN2d + GELU); the last one feeds frontend.linear (activation dtype)
       const bool last = layers[i + 1].kind == kLin;
-      EpiParams e = epi_generic(l.w[1], 1, nullptr, 0, last ? nullptr : Xalt, 2 * l.C, last ? c->XN : nullptr, 2 * l.C);
-      r = run_gemm(c, tc ? c->XB : static_cast<const void*>(X), l.w[0], tp ? tp->gemm : nullptr,
+      void* act_out = last ? ws.XN.get() : nullptr;
+      EpiParams e = epi_generic(l.w[1], 1, nullptr, 0, last ? nullptr : Xalt, 2 * l.C, act_out, 2 * l.C);
+      r = run_gemm(c, tc ? ws.XB.get() : static_cast<const void*>(X), l.w[0], tp->gemm.get(),
                    conv_shape(nb, l.F, L, l.C), e, "gemm_conv", st);
       if (last) {
-        out = c->XN;
+        out = ws.XN.get();
         out_act = true;
       } else {
         std::swap(X, Xalt);
@@ -590,39 +588,33 @@ int run_wave(bt_ctx* c, const float* spect, const Wave& wv, float* beat, float* 
     } else {  // kLin
       const int D = c->hp.transformer_dim;
       EpiParams e = epi_generic(l.w[1], 0, nullptr, 0, X, D, nullptr, 0);
-      r = run_gemm(c, c->XN, l.w[0], tp ? tp->gemm : nullptr, lin_shape(nb, L, D, l.F, l.C), e, "gemm_frontend_linear", st);
+      r = run_gemm(c, ws.XN.get(), l.w[0], tp->gemm.get(), lin_shape(nb, L, D, l.F, l.C), e, "gemm_frontend_linear",
+                   st);
       tap = "frontend";
       elems = static_cast<int64_t>(nb) * L * D;
     }
     if (r != BT_OK || (r = do_tap(c, tap, out, elems, out_act, st)) != BT_OK) return r;
   }
-  launch_head(X, c->hp.transformer_dim, c->head_w->f32, c->head_b->f32, wv.chunks_dev, nb, L, beat, down,
+  launch_head(X, c->hp.transformer_dim, c->head_w->f32.get(), c->head_b->f32.get(), wv.chunks_dev, nb, L, beat, down,
               c->hp.sum_head ? 1 : 0, st);
   BT_LAUNCHED(c, "head", st);
   return BT_OK;
 }
 
-struct HostChunk { ChunkSrc s; int len; };
-
-// upload the chunk table and run the forward pass in waves of up to ws_wave chunks, longest first.  A wave is padded
+// upload the chunk table and run the forward pass in waves of up to ws.chunks chunks, longest first.  A wave is padded
 // to its longest chunk: a shorter chunk costs its padded share of one wave (a fraction of a millisecond) instead of ~90
 // launches of its own (~0.7 ms of fixed cost), so chunks of all lengths share waves
-int run_chunks(bt_ctx* c, const float* spect_dev, std::vector<HostChunk>& all, float* beat_dev, float* downbeat_dev,
+int run_chunks(bt_ctx* c, const float* spect_dev, std::vector<ChunkSrc>& all, float* beat_dev, float* downbeat_dev,
                cudaStream_t st) {
   int r = BT_OK;
   if (all.empty()) return BT_OK;
-  if ((r = ensure_ws(c, static_cast<int>(all.size()))) != BT_OK) return r;
-  std::stable_sort(all.begin(), all.end(), [](const HostChunk& a, const HostChunk& b) { return a.len > b.len; });
-  const size_t bytes = all.size() * sizeof(ChunkSrc);
-  StageSlot* sl = nullptr;
-  if ((r = acquire_stage(c, bytes, &sl)) != BT_OK) return r;
-  ChunkSrc* hs = static_cast<ChunkSrc*>(sl->host);
-  for (size_t i = 0; i < all.size(); ++i) hs[i] = all[i].s;
-  if ((r = upload_stage(c, sl, bytes, st)) != BT_OK) return r;
-  const ChunkSrc* ds = static_cast<const ChunkSrc*>(sl->dev);
+  if ((r = ensure_ws(c)) != BT_OK) return r;
+  std::stable_sort(all.begin(), all.end(), [](const ChunkSrc& a, const ChunkSrc& b) { return a.len > b.len; });
+  const ChunkSrc* ds = nullptr;
+  if ((r = stage(c, st, {{all.data(), all.size()}}, &ds)) != BT_OK) return r;
   size_t i = 0;
   while (i < all.size()) {
-    const size_t j = std::min(all.size(), i + static_cast<size_t>(c->ws_wave));
+    const size_t j = std::min(all.size(), i + static_cast<size_t>(c->ws.chunks));
     Wave wv{ds + i, static_cast<int>(j - i), all[i].len, all[j - 1].len != all[i].len};
     if ((r = run_wave(c, spect_dev, wv, beat_dev, downbeat_dev, st)) != BT_OK) return r;
     i = j;
@@ -736,19 +728,17 @@ int bt_set_param(bt_ctx* c, const char* name, const float* data_host, int64_t co
   if (c->finalized) return fail(c, BT_ERR_STATE, "bt_set_param after bt_finalize");
   BT_CUDA(c, cudaSetDevice(c->device));
   Param& p = c->params[name];
-  if (p.f32) cudaFree(p.f32);
-  if (p.i32) cudaFree(p.i32);
   p = Param();
   p.n = count;
   const std::string n(name);
   if (n == "mel.fb_start" || n == "mel.fb_ptr") {
     std::vector<int32_t> tmp(count);
     for (int64_t i = 0; i < count; ++i) tmp[i] = static_cast<int32_t>(lrintf(data_host[i]));
-    BT_CUDA(c, cudaMalloc(&p.i32, count * 4));
-    BT_CUDA(c, cudaMemcpy(p.i32, tmp.data(), count * 4, cudaMemcpyHostToDevice));
+    BT_CUDA(c, p.i32.alloc(count * 4));
+    BT_CUDA(c, cudaMemcpy(p.i32.get(), tmp.data(), count * 4, cudaMemcpyHostToDevice));
   }
-  BT_CUDA(c, cudaMalloc(&p.f32, count * 4));
-  BT_CUDA(c, cudaMemcpy(p.f32, data_host, count * 4, cudaMemcpyHostToDevice));
+  BT_CUDA(c, p.f32.alloc(count * 4));
+  BT_CUDA(c, cudaMemcpy(p.f32.get(), data_host, count * 4, cudaMemcpyHostToDevice));
   return BT_OK;
 }
 
@@ -785,8 +775,8 @@ int bt_finalize(bt_ctx* c) {
     for (const Need& n : need) {
       if (!n.gemm) continue;
       Param& p = c->params[n.name];
-      BT_CUDA(c, cudaMalloc(&p.b16, p.n * 2));
-      launch_f32_to_h16(p.f32, p.b16, p.n, nullptr);
+      BT_CUDA(c, p.b16.alloc(p.n * 2));
+      launch_f32_to_h16(p.f32.get(), p.b16.get(), p.n, nullptr);
     }
     BT_CUDA(c, cudaDeviceSynchronize());
   }
@@ -798,33 +788,16 @@ void bt_destroy(bt_ctx* c) {
   if (!c) return;
   cudaSetDevice(c->device);
   cudaDeviceSynchronize();
-  free_plans(c);
-  free_ws(c);
-  for (auto& kv : c->params) {
-    if (kv.second.f32) cudaFree(kv.second.f32);
-    if (kv.second.b16) cudaFree(kv.second.b16);
-    if (kv.second.i32) cudaFree(kv.second.i32);
-  }
-  if (c->spect_ws) cudaFree(c->spect_ws);
-  if (c->dbn_ws) cudaFree(c->dbn_ws);
-  if (c->dbn_bp) cudaFree(c->dbn_bp);
-  for (auto& sl : c->stage) {
-    if (sl.host) cudaFreeHost(sl.host);
-    if (sl.dev) cudaFree(sl.dev);
-    if (sl.ev) cudaEventDestroy(sl.ev);
-  }
-  for (auto ev : c->ev_pool) cudaEventDestroy(ev);
   delete c;
 }
 
 int bt_set_wave_chunks(bt_ctx* c, int32_t chunks) {
   if (!c || chunks < 1 || chunks > 256) return fail(c, BT_ERR_ARG, "bt_set_wave_chunks: 1..256");
   c->wave = chunks;
-  if (c->ws_wave > chunks) {  // shrink: drop the workspace, it is re-created on the next call
+  if (c->ws.chunks > chunks) {  // shrink: drop the workspace, it is re-created on the next call
     cudaSetDevice(c->device);
     cudaDeviceSynchronize();
-    free_ws(c);
-    free_plans(c);
+    c->ws = Workspace();
   }
   return BT_OK;
 }
@@ -844,7 +817,7 @@ int bt_profile_collect(bt_ctx* c) {
   BT_CUDA(c, cudaDeviceSynchronize());
   for (const auto& r : c->prof_recs) {
     float ms = 0.f;
-    if (cudaEventElapsedTime(&ms, c->ev_pool[r.prev], c->ev_pool[r.ev]) == cudaSuccess) {
+    if (cudaEventElapsedTime(&ms, c->ev_pool[r.prev].get(), c->ev_pool[r.ev].get()) == cudaSuccess) {
       c->prof_ms[r.kind] += ms;
       c->prof_cnt[r.kind] += 1;
     }
@@ -902,24 +875,16 @@ int bt_logmel(bt_ctx* c, const float* audio_dev, const int64_t* sample_offsets_h
     if (frame_offsets_host[i + 1] - frame_offsets_host[i] != bt_num_frames(len))
       return fail(c, BT_ERR_ARG, "bt_logmel: frame_offsets do not match 1 + len/441 for clip %d", i);
   }
-  const size_t bytes = static_cast<size_t>(n_clips + 1) * 8 * 2;
-  StageSlot* sl = nullptr;
-  int r = acquire_stage(c, bytes, &sl);
+  const size_t n = n_clips + 1;
+  const int64_t* d[2];
+  const int r = stage(c, st, {{sample_offsets_host, n}, {frame_offsets_host, n}}, d);
   if (r != BT_OK) return r;
-  int64_t* h = static_cast<int64_t*>(sl->host);
-  memcpy(h, sample_offsets_host, (n_clips + 1) * 8);
-  memcpy(h + n_clips + 1, frame_offsets_host, (n_clips + 1) * 8);
-  if ((r = upload_stage(c, sl, bytes, st)) != BT_OK) return r;
-  const int64_t* d = static_cast<const int64_t*>(sl->dev);
-  const int64_t f0 = frame_offsets_host[0];
-  const int64_t total = frame_offsets_host[n_clips] - f0;
-  if (f0 != 0) return fail(c, BT_ERR_ARG, "bt_logmel: frame_offsets_host[0] must be 0");
+  if (frame_offsets_host[0] != 0) return fail(c, BT_ERR_ARG, "bt_logmel: frame_offsets_host[0] must be 0");
   int64_t max_frames = 0;
   for (int i = 0; i < n_clips; ++i) max_frames = std::max(max_frames, frame_offsets_host[i + 1] - frame_offsets_host[i]);
-  (void)total;
-  launch_logmel(audio_dev, d, d + n_clips + 1, n_clips, max_frames, find_param(c, "mel.window")->f32,
-                find_param(c, "mel.twiddle")->f32, find_param(c, "mel.fb_start")->i32,
-                find_param(c, "mel.fb_ptr")->i32, find_param(c, "mel.fb_w")->f32, spect_dev, st);
+  launch_logmel(audio_dev, d[0], d[1], n_clips, max_frames, find_param(c, "mel.window")->f32.get(),
+                find_param(c, "mel.twiddle")->f32.get(), find_param(c, "mel.fb_start")->i32.get(),
+                find_param(c, "mel.fb_ptr")->i32.get(), find_param(c, "mel.fb_w")->f32.get(), spect_dev, st);
   BT_LAUNCHED(c, "logmel", st);
   return BT_OK;
 }
@@ -941,16 +906,11 @@ int bt_resample(bt_ctx* c, const float* audio_in_dev, const int64_t* in_offsets_
       return fail(c, BT_ERR_ARG, "bt_resample: offsets must be non-decreasing");
     max_out = std::max(max_out, out_offsets_host[i + 1] - out_offsets_host[i]);
   }
-  const size_t bytes = static_cast<size_t>(n_clips + 1) * 8 * 2;
-  StageSlot* sl = nullptr;
-  int r = acquire_stage(c, bytes, &sl);
+  const size_t n = n_clips + 1;
+  const int64_t* d[2];
+  const int r = stage(c, st, {{in_offsets_host, n}, {out_offsets_host, n}}, d);
   if (r != BT_OK) return r;
-  int64_t* h = static_cast<int64_t*>(sl->host);
-  memcpy(h, in_offsets_host, (n_clips + 1) * 8);
-  memcpy(h + n_clips + 1, out_offsets_host, (n_clips + 1) * 8);
-  if ((r = upload_stage(c, sl, bytes, st)) != BT_OK) return r;
-  const int64_t* d = static_cast<const int64_t*>(sl->dev);
-  if (launch_resample(audio_in_dev, d, audio_out_dev, d + n_clips + 1, n_clips, max_out, coef_dev, L, M, K, st) != 0)
+  if (launch_resample(audio_in_dev, d[0], audio_out_dev, d[1], n_clips, max_out, coef_dev, L, M, K, st) != 0)
     return fail(c, BT_ERR_ARG, "bt_resample: ratio %d/%d with %d taps needs too much shared memory", L, M, K);
   BT_LAUNCHED(c, "resample", st);
   return BT_OK;
@@ -965,9 +925,8 @@ int bt_spect2frames(bt_ctx* c, const float* spect_dev, const int64_t* frame_offs
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   BT_CUDA(c, cudaSetDevice(c->device));
   prof_mark(c, st);
-  int r = BT_OK;
   // plan: all chunks of all clips, grouped by chunk length (1500 except for pieces <= 1488 frames)
-  std::vector<HostChunk> all;
+  std::vector<ChunkSrc> all;
   std::vector<int64_t> starts, lens;
   for (int i = 0; i < n_clips; ++i) {
     const int64_t T = frame_offsets_host[i + 1] - frame_offsets_host[i];
@@ -977,21 +936,19 @@ int bt_spect2frames(bt_ctx* c, const float* spect_dev, const int64_t* frame_offs
     starts.resize(n); lens.resize(n);
     chunks_for(T, starts.data(), lens.data(), n);
     for (int64_t j = 0; j < n; ++j) {
-      HostChunk hc;
-      hc.s.frame_base = frame_offsets_host[i];
-      hc.s.out_base = frame_offsets_host[i];
-      hc.s.T = static_cast<int32_t>(T);
-      hc.s.start = static_cast<int32_t>(starts[j]);
+      ChunkSrc s{};
+      s.frame_base = frame_offsets_host[i];
+      s.out_base = frame_offsets_host[i];
+      s.T = static_cast<int32_t>(T);
+      s.start = static_cast<int32_t>(starts[j]);
       // keep_first (inference.py:174-184): chunk j owns [start+6, start+len-6) minus what earlier chunks own
       int64_t lo = starts[j] + BT_BORDER;
       if (j > 0) lo = std::max(lo, starts[j - 1] + lens[j - 1] - BT_BORDER);
       const int64_t hi = starts[j] + lens[j] - BT_BORDER;
-      hc.s.write_lo = static_cast<int32_t>(lo - starts[j]);
-      hc.s.write_hi = static_cast<int32_t>(std::max(lo, hi) - starts[j]);
-      hc.s.len = static_cast<int32_t>(lens[j]);
-      hc.s.pad_ = 0;
-      hc.len = static_cast<int>(lens[j]);
-      all.push_back(hc);
+      s.write_lo = static_cast<int32_t>(lo - starts[j]);
+      s.write_hi = static_cast<int32_t>(std::max(lo, hi) - starts[j]);
+      s.len = static_cast<int32_t>(lens[j]);
+      all.push_back(s);
     }
   }
   return run_chunks(c, spect_dev, all, beat_dev, downbeat_dev, st);
@@ -1007,18 +964,17 @@ int bt_forward_chunks(bt_ctx* c, const float* chunks_dev, int32_t n_chunks, int3
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   BT_CUDA(c, cudaSetDevice(c->device));
   prof_mark(c, st);
-  std::vector<HostChunk> all(n_chunks);
+  std::vector<ChunkSrc> all(n_chunks);
   for (int i = 0; i < n_chunks; ++i) {
-    HostChunk& hc = all[i];
-    hc.s.frame_base = static_cast<int64_t>(i) * chunk_frames;
-    hc.s.out_base = hc.s.frame_base;
-    hc.s.T = chunk_frames;
-    hc.s.start = 0;
-    hc.s.write_lo = 0;
-    hc.s.write_hi = chunk_frames;
-    hc.s.len = chunk_frames;
-    hc.s.pad_ = 0;
-    hc.len = chunk_frames;
+    ChunkSrc& s = all[i];
+    s.frame_base = static_cast<int64_t>(i) * chunk_frames;
+    s.out_base = s.frame_base;
+    s.T = chunk_frames;
+    s.start = 0;
+    s.write_lo = 0;
+    s.write_hi = chunk_frames;
+    s.len = chunk_frames;
+    s.pad_ = 0;
   }
   return run_chunks(c, chunks_dev, all, beat_dev, downbeat_dev, st);
 }
@@ -1030,15 +986,11 @@ int bt_audio2frames(bt_ctx* c, const float* audio_dev, const int64_t* sample_off
   if (!frame_offsets_host) return fail(c, BT_ERR_ARG, "bt_audio2frames: null argument");
   BT_CUDA(c, cudaSetDevice(c->device));
   const int64_t total = frame_offsets_host[n_clips];
-  if (total * 128 > c->spect_cap) {
-    if (c->spect_ws) cudaFree(c->spect_ws);
-    c->spect_ws = nullptr;
-    c->spect_cap = total * 128 * 5 / 4;
-    BT_CUDA(c, cudaMalloc(&c->spect_ws, c->spect_cap * 4));
-  }
-  int r = bt_logmel(c, audio_dev, sample_offsets_host, n_clips, c->spect_ws, frame_offsets_host, stream);
+  const size_t need = total * 128 * 4;
+  BT_CUDA(c, c->spect_ws.reserve(need, need + need / 4));
+  int r = bt_logmel(c, audio_dev, sample_offsets_host, n_clips, c->spect_ws.get(), frame_offsets_host, stream);
   if (r != BT_OK) return r;
-  return bt_spect2frames(c, c->spect_ws, frame_offsets_host, n_clips, beat_dev, downbeat_dev, stream);
+  return bt_spect2frames(c, c->spect_ws.get(), frame_offsets_host, n_clips, beat_dev, downbeat_dev, stream);
 }
 
 int bt_peakpick(bt_ctx* c, const float* beat_dev, const float* downbeat_dev, const int64_t* frame_offsets_host,
@@ -1052,13 +1004,10 @@ int bt_peakpick(bt_ctx* c, const float* beat_dev, const float* downbeat_dev, con
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   BT_CUDA(c, cudaSetDevice(c->device));
   prof_mark(c, st);
-  const size_t bytes = static_cast<size_t>(n_clips + 1) * 8;
-  StageSlot* sl = nullptr;
-  int r = acquire_stage(c, bytes, &sl);
+  const int64_t* fo = nullptr;
+  const int r = stage(c, st, {{frame_offsets_host, static_cast<size_t>(n_clips + 1)}}, &fo);
   if (r != BT_OK) return r;
-  memcpy(sl->host, frame_offsets_host, bytes);
-  if ((r = upload_stage(c, sl, bytes, st)) != BT_OK) return r;
-  launch_peakpick(beat_dev, downbeat_dev, static_cast<const int64_t*>(sl->dev), n_clips, beat_times_dev,
+  launch_peakpick(beat_dev, downbeat_dev, fo, n_clips, beat_times_dev,
                   n_beats_dev, down_times_dev, n_down_dev, max_peaks, st);
   BT_LAUNCHED(c, "peakpick", st);
   return BT_OK;
@@ -1124,19 +1073,6 @@ int dbn_host_model(bt_ctx* c, const char* fn, int32_t beats, int32_t n_int, cons
   return BT_OK;
 }
 
-int dbn_grow(bt_ctx* c, void** buf, size_t* cap, size_t need) {
-  if (need <= *cap) return BT_OK;
-  if (*buf) cudaFree(*buf);  // only when the buffer grows, as spect_ws
-  *buf = nullptr;
-  *cap = 0;
-  const size_t n = need + need / 4;
-  BT_CUDA(c, cudaMalloc(buf, n));
-  *cap = n;
-  return BT_OK;
-}
-
-inline size_t align16(size_t v) { return (v + 15) & ~static_cast<size_t>(15); }
-
 // Model tables, frame offsets and (optionally) the windows of the clips through one staging slot; device pointers
 // into the slot come back.  bp_base of model i: the back pointers of the models before it, `total` frames each.
 int dbn_stage(bt_ctx* c, const std::vector<DbnHostModel>& ms, const int64_t* fo, int32_t n_clips, int64_t total,
@@ -1158,8 +1094,8 @@ int dbn_stage(bt_ctx* c, const std::vector<DbnHostModel>& ms, const int64_t* fo,
   StageSlot* sl = nullptr;
   int r = acquire_stage(c, off, &sl);
   if (r != BT_OK) return r;
-  char* h = static_cast<char*>(sl->host);
-  char* d = static_cast<char*>(sl->dev);
+  char* h = sl->host.get();
+  const char* d = sl->dev.get();
   int64_t bp_base = 0;
   for (int i = 0; i < nm; ++i) {
     const DbnHostModel& m = ms[i];
@@ -1242,21 +1178,22 @@ int bt_dbn_track_device(bt_ctx* c, const float* beat_logits_dev, const float* do
   const size_t ws_bytes = o_codes + static_cast<size_t>(total);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   BT_CUDA(c, cudaSetDevice(c->device));
-  int r = dbn_grow(c, &c->dbn_ws, &c->dbn_ws_cap, ws_bytes);
-  if (r == BT_OK) r = dbn_grow(c, &c->dbn_bp, &c->dbn_bp_cap, std::max<size_t>(bp_per_frame * total, 1));
-  if (r != BT_OK) return r;
+  const size_t bp_bytes = std::max<size_t>(bp_per_frame * total, 1);
+  BT_CUDA(c, c->dbn_ws.reserve(ws_bytes, ws_bytes + ws_bytes / 4));
+  BT_CUDA(c, c->dbn_bp.reserve(bp_bytes, bp_bytes + bp_bytes / 4));
   prof_mark(c, st);
   const DbnModelDev* md = nullptr;
   const int64_t* fo_dev = nullptr;
-  if ((r = dbn_stage(c, ms, frame_offsets_host, n_clips, total, nullptr, st, &md, &fo_dev, nullptr)) != BT_OK) return r;
-  char* ws = static_cast<char*>(c->dbn_ws);
+  const int r = dbn_stage(c, ms, frame_offsets_host, n_clips, total, nullptr, st, &md, &fo_dev, nullptr);
+  if (r != BT_OK) return r;
+  char* ws = c->dbn_ws.get();
   double* act = reinterpret_cast<double*>(ws);
   double* dens = reinterpret_cast<double*>(ws + o_dens);
   int64_t* win = reinterpret_cast<int64_t*>(ws + o_win);
   double* res_logp = reinterpret_cast<double*>(ws + o_logp);
   int64_t* res_state = reinterpret_cast<int64_t*>(ws + o_state);
   uint8_t* codes = reinterpret_cast<uint8_t*>(ws + o_codes);
-  uint8_t* bp = static_cast<uint8_t*>(c->dbn_bp);
+  uint8_t* bp = c->dbn_bp.get();
   launch_dbn_prep(beat_logits_dev, downbeat_logits_dev, activations_dev, fo_dev, n_clips, threshold, observation_lambda,
                   act, dens, win, st);
   BT_LAUNCHED(c, "dbn_prep", st);
@@ -1285,17 +1222,17 @@ int bt_debug_dbn_viterbi(bt_ctx* c, const double* log_dens_dev, int64_t T, int32
   dbn_launch_shape(ms, &threads, &smem, &bp_per_frame);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   BT_CUDA(c, cudaSetDevice(c->device));
-  r = dbn_grow(c, &c->dbn_ws, &c->dbn_ws_cap, 2 * sizeof(double));
-  if (r == BT_OK) r = dbn_grow(c, &c->dbn_bp, &c->dbn_bp_cap, bp_per_frame * T);
-  if (r != BT_OK) return r;
+  const size_t ws_bytes = 2 * sizeof(double), bp_bytes = bp_per_frame * T;
+  BT_CUDA(c, c->dbn_ws.reserve(ws_bytes, ws_bytes + ws_bytes / 4));
+  BT_CUDA(c, c->dbn_bp.reserve(bp_bytes, bp_bytes + bp_bytes / 4));
   prof_mark(c, st);
   const int64_t fo[2] = {0, T}, win_h[2] = {0, T};
   const DbnModelDev* md = nullptr;
   const int64_t *fo_dev = nullptr, *win = nullptr;
   if ((r = dbn_stage(c, ms, fo, 1, T, win_h, st, &md, &fo_dev, &win)) != BT_OK) return r;
-  double* res_logp = static_cast<double*>(c->dbn_ws);
+  double* res_logp = reinterpret_cast<double*>(c->dbn_ws.get());
   int64_t* res_state = reinterpret_cast<int64_t*>(res_logp + 1);
-  uint8_t* bp = static_cast<uint8_t*>(c->dbn_bp);
+  uint8_t* bp = c->dbn_bp.get();
   if (const int e = launch_dbn_viterbi(md, 1, threads, smem, log_dens_dev, fo_dev, win, 1, bp, res_logp, res_state, st))
     return fail(c, BT_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(static_cast<cudaError_t>(e)));
   BT_LAUNCHED(c, "dbn_viterbi", st);
@@ -1329,15 +1266,11 @@ int bt_beat_metrics(bt_ctx* c, const double* est_dev, const int64_t* est_offsets
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   BT_CUDA(c, cudaSetDevice(c->device));
   prof_mark(c, st);
-  const size_t half = static_cast<size_t>(n_sets + 1) * sizeof(int64_t);
-  StageSlot* sl = nullptr;
-  int r = acquire_stage(c, 2 * half, &sl);
+  const size_t n = n_sets + 1;
+  const int64_t* off_dev[2];
+  const int r = stage(c, st, {{est_offsets_host, n}, {ref_offsets_host, n}}, off_dev);
   if (r != BT_OK) return r;
-  memcpy(sl->host, est_offsets_host, half);
-  memcpy(static_cast<char*>(sl->host) + half, ref_offsets_host, half);
-  if ((r = upload_stage(c, sl, 2 * half, st)) != BT_OK) return r;
-  const int64_t* off_dev = static_cast<const int64_t*>(sl->dev);
-  if (const int e = launch_beat_metrics(est_dev, off_dev, ref_dev, off_dev + n_sets + 1, n_sets, p, out_dev, st))
+  if (const int e = launch_beat_metrics(est_dev, off_dev[0], ref_dev, off_dev[1], n_sets, p, out_dev, st))
     return fail(c, BT_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(static_cast<cudaError_t>(e)));
   BT_LAUNCHED(c, "beat_metrics", st);
   return BT_OK;
@@ -1373,28 +1306,23 @@ int bt_debug_gemm(bt_ctx* c, const bt_debug_gemm_desc* d, const float* a_dev, co
   }
   const int64_t a_n = static_cast<int64_t>(d->planes_in) * d->L * d->lda;
   const int64_t w_n = static_cast<int64_t>(d->N) * d->Kslab * d->nslab;
-  void *ab = nullptr, *wb = nullptr, *ob = nullptr;
-  TcGemmPlan* p = nullptr;
-  int rc = BT_OK;
+  DeviceBuffer<> ab, wb, ob;
+  if (ab.alloc(a_n * 2) != cudaSuccess || wb.alloc(w_n * 2) != cudaSuccess ||
+      (out_act_dev && ob.alloc(out_act_count * 2) != cudaSuccess))
+    return fail(c, BT_ERR_CUDA, "bt_debug_gemm: out of device memory");
+  launch_f32_to_h16(a_dev, ab.get(), a_n, st);
+  launch_f32_to_h16(w_dev, wb.get(), w_n, st);
+  if (out_act_dev) launch_f32_to_h16(out_act_dev, ob.get(), out_act_count, st);
+  e.out_act = ob.get();
   char err[512] = "";
-  if (cudaMalloc(&ab, a_n * 2) != cudaSuccess || cudaMalloc(&wb, w_n * 2) != cudaSuccess ||
-      (out_act_dev && cudaMalloc(&ob, out_act_count * 2) != cudaSuccess)) {
-    rc = fail(c, BT_ERR_CUDA, "bt_debug_gemm: out of device memory");
-  } else {
-    launch_f32_to_h16(a_dev, ab, a_n, st);
-    launch_f32_to_h16(w_dev, wb, w_n, st);
-    if (ob) launch_f32_to_h16(out_act_dev, ob, out_act_count, st);
-    e.out_act = ob;
-    p = tc_gemm_plan_create(ab, wb, g, d->planes_in, d->resid_epilogue != 0, err, sizeof(err));
-    if (!p) rc = fail(c, BT_ERR_CUDA, "%s", err);
-    else if (launch_gemm_tc(p, e, st) != 0) rc = fail(c, BT_ERR_CUDA, "tc gemm launch failed");
-    else if (ob) launch_h16_to_f32(ob, out_act_dev, out_act_count, st);
-    if (p && tile_out) tc_gemm_plan_tile(p, &tile_out[0], &tile_out[1]);
-  }
-  cudaError_t se = cudaStreamSynchronize(st);
+  const GemmPlan p(tc_gemm_plan_create(ab.get(), wb.get(), g, d->planes_in, d->resid_epilogue != 0, err, sizeof(err)));
+  int rc = BT_OK;
+  if (!p) rc = fail(c, BT_ERR_CUDA, "%s", err);
+  else if (launch_gemm_tc(p.get(), e, st) != 0) rc = fail(c, BT_ERR_CUDA, "tc gemm launch failed");
+  else if (out_act_dev) launch_h16_to_f32(ob.get(), out_act_dev, out_act_count, st);
+  if (p && tile_out) tc_gemm_plan_tile(p.get(), &tile_out[0], &tile_out[1]);
+  const cudaError_t se = cudaStreamSynchronize(st);
   if (rc == BT_OK && se != cudaSuccess) rc = fail(c, BT_ERR_CUDA, "tc gemm: %s", cudaGetErrorString(se));
-  if (p) tc_gemm_plan_destroy(p);
-  cudaFree(ab); cudaFree(wb); cudaFree(ob);
   c->launches++;
   return rc;
 }
@@ -1420,35 +1348,35 @@ int bt_debug_attention(bt_ctx* c, const float* q_dev, const float* k_dev, const 
       chunks[i].len = key_lens_host[i];
     }
   }
-  void *qkv = nullptr, *o = nullptr;
-  ChunkSrc* chunks_dev = nullptr;
-  BT_CUDA(c, cudaMalloc(&qkv, M * 3 * C * act));
-  BT_CUDA(c, cudaMalloc(&o, M * C * act));
+  DeviceBuffer<> qkv, o;
+  DeviceBuffer<ChunkSrc> chunks_dev;
+  BT_CUDA(c, qkv.alloc(M * 3 * C * act));
+  BT_CUDA(c, o.alloc(M * C * act));
   if (key_lens_host) {
-    BT_CUDA(c, cudaMalloc(&chunks_dev, chunks.size() * sizeof(ChunkSrc)));
-    BT_CUDA(c, cudaMemcpyAsync(chunks_dev, chunks.data(), chunks.size() * sizeof(ChunkSrc), cudaMemcpyHostToDevice, st));
+    const size_t bytes = chunks.size() * sizeof(ChunkSrc);
+    BT_CUDA(c, chunks_dev.alloc(bytes));
+    BT_CUDA(c, cudaMemcpyAsync(chunks_dev.get(), chunks.data(), bytes, cudaMemcpyHostToDevice, st));
   }
   int rc = BT_OK;
   if (tc) {
-    launch_pack_qkv_test(q_dev, k_dev, v_dev, qkv, seqs, L, heads, 0.17677669529663687f * 1.4426950408889634f, 1, st);
+    launch_pack_qkv_test(q_dev, k_dev, v_dev, qkv.get(), seqs, L, heads, 0.17677669529663687f * 1.4426950408889634f, 1, st);
     char err[512] = "";
-    TcAttnPlan* p = tc_attn_plan_create(qkv, seqs, L, heads, err, sizeof(err));
+    const AttnPlan p(tc_attn_plan_create(qkv.get(), seqs, L, heads, err, sizeof(err)));
     if (!p) rc = fail(c, BT_ERR_CUDA, "%s", err);
     else {
-      launch_attn_time_tc(p, gates_dev, o, st, chunks_dev, seqs_per_chunk);
-      launch_h16_to_f32(o, o_dev, M * C, st);
+      launch_attn_time_tc(p.get(), gates_dev, o.get(), st, chunks_dev.get(), seqs_per_chunk);
+      launch_h16_to_f32(o.get(), o_dev, M * C, st);
     }
-    cudaError_t se = cudaStreamSynchronize(st);
+    const cudaError_t se = cudaStreamSynchronize(st);
     if (rc == BT_OK && se != cudaSuccess) rc = fail(c, BT_ERR_CUDA, "tc attention: %s", cudaGetErrorString(se));
-    if (p) tc_attn_plan_destroy(p);
   } else {
-    launch_pack_qkv_test(q_dev, k_dev, v_dev, qkv, seqs, L, heads, 1.0f, 0, st);
-    launch_attn_time_simt(static_cast<const float*>(qkv), gates_dev, o_dev, seqs, L, heads, st, chunks_dev, seqs_per_chunk);
-    cudaError_t se = cudaStreamSynchronize(st);
+    launch_pack_qkv_test(q_dev, k_dev, v_dev, qkv.get(), seqs, L, heads, 1.0f, 0, st);
+    launch_attn_time_simt(static_cast<const float*>(qkv.get()), gates_dev, o_dev, seqs, L, heads, st, chunks_dev.get(),
+                          seqs_per_chunk);
+    const cudaError_t se = cudaStreamSynchronize(st);
     if (se != cudaSuccess) rc = fail(c, BT_ERR_CUDA, "simt attention: %s", cudaGetErrorString(se));
   }
   c->launches += 2;
-  cudaFree(qkv); cudaFree(o); cudaFree(chunks_dev);
   return rc;
 }
 
@@ -1465,30 +1393,26 @@ int bt_debug_attention_freq(bt_ctx* c, const float* q_dev, const float* k_dev, c
   const bool tc = c->dtype == BT_DTYPE_H16;
   const size_t act = tc ? 2 : 4;
   const float inv_sqrt_d = 0.17677669529663687f;
-  void *qkv = nullptr, *o = nullptr;
-  TcFreqPlan* p = nullptr;
-  BT_CUDA(c, cudaMalloc(&qkv, M * 3 * C * act));
+  DeviceBuffer<> qkv, o;
+  FreqPlan p;
+  BT_CUDA(c, qkv.alloc(M * 3 * C * act));
   if (tc) {
-    BT_CUDA(c, cudaMalloc(&o, M * C * act));
+    BT_CUDA(c, o.alloc(M * C * act));
     char err[512] = "";
-    if (!(p = tc_freq_plan_create(qkv, o, B, F, L, heads, err, sizeof(err)))) {
-      cudaFree(qkv); cudaFree(o);
-      return fail(c, BT_ERR_ARG, "bt_debug_attention_freq: %s", err);
-    }
+    p.reset(tc_freq_plan_create(qkv.get(), o.get(), B, F, L, heads, err, sizeof(err)));
+    if (!p) return fail(c, BT_ERR_ARG, "bt_debug_attention_freq: %s", err);
   }
-  launch_pack_qkv_test(q_dev, k_dev, v_dev, qkv, B * F, L, heads, 1.0f, tc ? 1 : 0, st);
+  launch_pack_qkv_test(q_dev, k_dev, v_dev, qkv.get(), B * F, L, heads, 1.0f, tc ? 1 : 0, st);
   if (tc) {
-    launch_attn_freq_tc(p, gates_dev, inv_sqrt_d, st);
-    launch_h16_to_f32(o, o_dev, M * C, st);
+    launch_attn_freq_tc(p.get(), gates_dev, inv_sqrt_d, st);
+    launch_h16_to_f32(o.get(), o_dev, M * C, st);
   } else {
-    launch_attn_freq_simt(static_cast<const float*>(qkv), gates_dev, o_dev, B, F, L, heads, inv_sqrt_d, st);
+    launch_attn_freq_simt(static_cast<const float*>(qkv.get()), gates_dev, o_dev, B, F, L, heads, inv_sqrt_d, st);
   }
   int rc = BT_OK;
   cudaError_t se = cudaStreamSynchronize(st);
   if (se != cudaSuccess) rc = fail(c, BT_ERR_CUDA, "frequency attention: %s", cudaGetErrorString(se));
   c->launches += 2;
-  if (p) tc_freq_plan_destroy(p);
-  cudaFree(qkv); cudaFree(o);
   return rc;
 }
 
