@@ -353,6 +353,28 @@ bool outproj_in_ff(const bt_ctx* c, const std::vector<LayerPlans>* wp, size_t i)
   return wp && i + 1 < wp->size() && (*wp)[i + 1].ff_op && c->tap_name != c->layers[i].name;
 }
 
+// the last convolution feeds frontend.linear in the activation dtype (XN) instead of the residual stream
+bool conv_feeds_linear(const bt_ctx* c, size_t i) {
+  return c->layers[i].kind == kConv && i + 1 < c->layers.size() && c->layers[i + 1].kind == kLin;
+}
+
+// The fp32 residual stream layer i reads and updates (other = false; i = layers.size(): what the head reads), and the
+// buffer a convolution writes its output to (other = true).  The stem writes X0; every convolution but the last moves
+// the stream to the other buffer.  The forward pass and its tensor-core plans (whose tensor maps hold these addresses)
+// both resolve the buffers here.
+float* residual_stream(const bt_ctx* c, size_t i, bool other = false) {
+  bool in_x1 = false;
+  for (size_t k = 0; k < i; ++k)
+    if (c->layers[k].kind == kConv && !conv_feeds_linear(c, k)) in_x1 = !in_x1;
+  return in_x1 != other ? c->ws.X1.get() : c->ws.X0.get();
+}
+
+// the 16-bit copy of its output that FFN layer i writes: the FFN in front of a convolution feeds it (16-bit path)
+void* ff_copy_act(const bt_ctx* c, size_t i) {
+  const bool before_conv = i + 1 < c->layers.size() && c->layers[i + 1].kind == kConv;
+  return c->dtype == BT_DTYPE_H16 && before_conv ? c->ws.XB.get() : nullptr;
+}
+
 // x += attention(x) over nb * F planes of L tokens with dim C (reference roformer.py:114-132).
 // kAttnF: sequences run over the F planes of each chunk (PartialFTTransformer attnF).
 int attention_block(bt_ctx* c, float* X, const Layer& l, const LayerPlans* tp, int nb, int L, bool out_in_ff,
@@ -469,14 +491,22 @@ bool make_layer_plans(const bt_ctx* c, size_t i, int nb, int L, LayerPlans& p, c
   const Workspace& ws = c->ws;
   const int C = l.C, planes = nb * l.F;
   const int64_t M = static_cast<int64_t>(planes) * L;
-  auto gemm = [&](const void* A, const Param* W, const GemmShape& g, bool resid = false) {
-    return GemmPlan(tc_gemm_plan_create(A, W->b16.get(), g, planes, resid, err, errlen));
+  float* X = residual_stream(c, i);
+  // the epilogue destinations each launch of attention_block / ff_block / run_wave passes (GemmDst)
+  auto gemm = [&](const void* A, const Param* W, const GemmShape& g, const GemmDst& dst, bool resid = false) {
+    return GemmPlan(tc_gemm_plan_create(A, W->b16.get(), g, planes, resid, dst, err, errlen));
   };
   switch (l.kind) {
-    case kConv:
-      return (p.gemm = gemm(ws.XB.get(), l.w[0], conv_shape(nb, l.F, L, C))) != nullptr;
-    case kLin:
-      return (p.gemm = gemm(ws.XN.get(), l.w[0], lin_shape(nb, L, c->hp.transformer_dim, l.F, C))) != nullptr;
+    case kConv: {
+      const GemmDst dst = conv_feeds_linear(c, i) ? GemmDst{nullptr, 0, nullptr, 0, ws.XN.get(), 2 * C}
+                                                  : GemmDst{nullptr, 0, residual_stream(c, i, true), 2 * C, nullptr, 0};
+      return (p.gemm = gemm(ws.XB.get(), l.w[0], conv_shape(nb, l.F, L, C), dst)) != nullptr;
+    }
+    case kLin: {
+      const int D = c->hp.transformer_dim;
+      return (p.gemm = gemm(ws.XN.get(), l.w[0], lin_shape(nb, L, D, l.F, C), GemmDst{nullptr, 0, X, D, nullptr, 0})) !=
+             nullptr;
+    }
     case kFf:
       if (fused(l)) {
         const void *w1 = l.w[0]->b16.get(), *w2 = l.w[2]->b16.get();
@@ -486,23 +516,27 @@ bool make_layer_plans(const bt_ctx* c, size_t i, int nb, int L, LayerPlans& p, c
           p.ff_op.reset(tc_ff_plan_create(w1, w2, C, M, ws.O.get(), prev.w[3]->b16.get(), err, errlen));
         return p.ff && (p.ff_op || prev.kind == kAttn);
       }
-      p.ff1 = gemm(ws.XN.get(), l.w[0], plain_shape(planes, L, l.mult * C, C, C));
-      p.ff2 = gemm(ws.H.get(), l.w[2], plain_shape(planes, L, C, l.mult * C, l.mult * C), true);
+      p.ff1 = gemm(ws.XN.get(), l.w[0], plain_shape(planes, L, l.mult * C, C, C),
+                   GemmDst{nullptr, 0, nullptr, 0, ws.H.get(), l.mult * C});
+      p.ff2 = gemm(ws.H.get(), l.w[2], plain_shape(planes, L, C, l.mult * C, l.mult * C),
+                   GemmDst{X, C, X, C, ff_copy_act(c, i), C}, true);
       return p.ff1 && p.ff2;
     default:  // attention
       if (fused(l)) {
         p.fqkv.reset(tc_qkv_plan_create(l.w[0]->b16.get(), C, M, err, errlen));
         if (!p.fqkv) return false;
       } else {
-        p.gates = gemm(ws.XN.get(), l.w[1], plain_shape(planes, L, 32, C, C));
-        p.qkv = gemm(ws.XN.get(), l.w[0], plain_shape(planes, L, 3 * C, C, C));
+        p.gates = gemm(ws.XN.get(), l.w[1], plain_shape(planes, L, 32, C, C), GemmDst{});
+        p.qkv = gemm(ws.XN.get(), l.w[0], plain_shape(planes, L, 3 * C, C, C),
+                     GemmDst{nullptr, 0, nullptr, 0, ws.QKV.get(), 3 * C});
         if (!p.gates || !p.qkv) return false;
       }
       const int heads = C / kHeadDim;
       if (l.kind == kAttnF) p.freq.reset(tc_freq_plan_create(ws.QKV.get(), ws.O.get(), nb, l.F, L, heads, err, errlen));
       else p.attn.reset(tc_attn_plan_create(ws.QKV.get(), planes, L, heads, err, errlen));
       if (!p.freq && !p.attn) return false;
-      return (p.out = gemm(ws.O.get(), l.w[3], plain_shape(planes, L, C, C, C), true)) != nullptr;
+      return (p.out = gemm(ws.O.get(), l.w[3], plain_shape(planes, L, C, C, C), GemmDst{X, C, X, C, nullptr, 0}, true)) !=
+             nullptr;
   }
 }
 
@@ -539,30 +573,27 @@ int run_wave(bt_ctx* c, const float* spect, const Wave& wv, float* beat, float* 
   std::vector<LayerPlans>* wp = nullptr;
   int r;
   if (tc && (r = build_plans(c, nb, L, &wp)) != BT_OK) return r;
-  float* X = ws.X0.get();
-  float* Xalt = ws.X1.get();
   // chunks shorter than the wave's padded length: the time attentions mask their missing keys and the convolutions
   // see zeros beyond their last frame (everything else works row by row, padding rows are never read back)
   const ChunkSrc* vl = wv.varlen ? wv.chunks_dev : nullptr;
   launch_stem(spect, wv.chunks_dev, nb, L, c->bn1_scale->f32.get(), c->bn1_shift->f32.get(), c->stem_w->f32.get(),
-              c->stem_b->f32.get(), X, st);
+              c->stem_b->f32.get(), residual_stream(c, 0), st);
   BT_LAUNCHED(c, "stem", st);
-  if ((r = do_tap(c, "stem", X, static_cast<int64_t>(nb) * (c->hp.spect_dim / 4) * L * c->hp.stem_dim, false, st)) != BT_OK)
+  if ((r = do_tap(c, "stem", residual_stream(c, 0), static_cast<int64_t>(nb) * (c->hp.spect_dim / 4) * L * c->hp.stem_dim, false, st)) != BT_OK)
     return r;
   const std::vector<Layer>& layers = c->layers;
   for (size_t i = 0; i < layers.size(); ++i) {
     const Layer& l = layers[i];
     const LayerPlans* tp = wp ? &(*wp)[i] : &kNoPlans;
     const char* tap = l.name.c_str();
+    float* X = residual_stream(c, i);
     const void* out = X;  // the layer's output (tap)
     bool out_act = false;
     int64_t elems = static_cast<int64_t>(nb) * l.F * L * l.C;
     if (is_attention(l)) {
       r = attention_block(c, X, l, tp, nb, L, outproj_in_ff(c, wp, i), l.kind == kAttnF ? nullptr : vl, st);
     } else if (l.kind == kFf) {
-      // the FFN in front of a convolution also writes the 16-bit copy the convolution reads
-      const bool before_conv = i + 1 < layers.size() && layers[i + 1].kind == kConv;
-      r = ff_block(c, X, l, tp, nb, L, outproj_in_ff(c, wp, i - 1), tc && before_conv ? ws.XB.get() : nullptr, st);
+      r = ff_block(c, X, l, tp, nb, L, outproj_in_ff(c, wp, i - 1), ff_copy_act(c, i), st);
     } else if (l.kind == kConv) {
       if (tc && (i == 0 || layers[i - 1].kind != kFf)) {  // no FFN in front (no partial transformers)
         launch_f32_to_h16(X, ws.XB.get(), elems, st);
@@ -573,7 +604,8 @@ int run_wave(bt_ctx* c, const float* spect, const Wave& wv, float* beat, float* 
         BT_LAUNCHED(c, "zero_tail", st);
       }
       // conv C -> 2C (+ folded BN2d + GELU); the last one feeds frontend.linear (activation dtype)
-      const bool last = layers[i + 1].kind == kLin;
+      const bool last = conv_feeds_linear(c, i);
+      float* Xalt = residual_stream(c, i, true);
       void* act_out = last ? ws.XN.get() : nullptr;
       EpiParams e = epi_generic(l.w[1], 1, nullptr, 0, last ? nullptr : Xalt, 2 * l.C, act_out, 2 * l.C);
       r = run_gemm(c, tc ? ws.XB.get() : static_cast<const void*>(X), l.w[0], tp->gemm.get(),
@@ -582,8 +614,7 @@ int run_wave(bt_ctx* c, const float* spect, const Wave& wv, float* beat, float* 
         out = ws.XN.get();
         out_act = true;
       } else {
-        std::swap(X, Xalt);
-        out = X;
+        out = Xalt;
       }
     } else {  // kLin
       const int D = c->hp.transformer_dim;
@@ -595,7 +626,7 @@ int run_wave(bt_ctx* c, const float* spect, const Wave& wv, float* beat, float* 
     }
     if (r != BT_OK || (r = do_tap(c, tap, out, elems, out_act, st)) != BT_OK) return r;
   }
-  launch_head(X, c->hp.transformer_dim, c->head_w->f32.get(), c->head_b->f32.get(), wv.chunks_dev, nb, L, beat, down,
+  launch_head(residual_stream(c, layers.size()), c->hp.transformer_dim, c->head_w->f32.get(), c->head_b->f32.get(), wv.chunks_dev, nb, L, beat, down,
               c->hp.sum_head ? 1 : 0, st);
   BT_LAUNCHED(c, "head", st);
   return BT_OK;
@@ -1314,8 +1345,9 @@ int bt_debug_gemm(bt_ctx* c, const bt_debug_gemm_desc* d, const float* a_dev, co
   launch_f32_to_h16(w_dev, wb.get(), w_n, st);
   if (out_act_dev) launch_f32_to_h16(out_act_dev, ob.get(), out_act_count, st);
   e.out_act = ob.get();
+  const GemmDst dst = e.kind == 2 ? GemmDst{} : GemmDst{e.resid, e.ldr, e.out_f32, e.ldo_f32, e.out_act, e.ldo_act};
   char err[512] = "";
-  const GemmPlan p(tc_gemm_plan_create(ab.get(), wb.get(), g, d->planes_in, d->resid_epilogue != 0, err, sizeof(err)));
+  const GemmPlan p(tc_gemm_plan_create(ab.get(), wb.get(), g, d->planes_in, d->resid_epilogue != 0, dst, err, sizeof(err)));
   int rc = BT_OK;
   if (!p) rc = fail(c, BT_ERR_CUDA, "%s", err);
   else if (launch_gemm_tc(p.get(), e, st) != 0) rc = fail(c, BT_ERR_CUDA, "tc gemm launch failed");

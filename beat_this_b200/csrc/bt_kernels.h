@@ -148,11 +148,23 @@ void launch_pack_qkv_test(const float* q, const float* k, const float* v, void* 
 
 // ---- 16-bit (fp16 or bf16 operands) tensor-core path (wgmma GEMM, mma.sync attention) ---------------------------------
 struct TcGemmPlan;  // cached tensor maps + launch geometry
+// Where the epilogue of kinds 0 and 1 reads the residual and writes its results ([planes_out * L] rows, leading
+// dimensions in elements, null = absent; EpiParams fields of the same names).  The plan encodes tensor maps of them,
+// and every launch of the plan must pass the same buffers.  The gates GEMM (kind 2) takes none.
+struct GemmDst {
+  const float* resid;
+  int ldr;
+  float* out_f32;
+  int ldo_f32;
+  void* out_act;
+  int ldo_act;
+};
 // resid_epilogue: the launches of this plan add the fp32 residual in the epilogue (tile width policy, kernels_gemm.cu)
-TcGemmPlan* tc_gemm_plan_create(const void* A_h16, const void* W_h16, const GemmShape& g,
-                                int planes_in, bool resid_epilogue, char* err, int errlen);
+TcGemmPlan* tc_gemm_plan_create(const void* A_h16, const void* W_h16, const GemmShape& g, int planes_in,
+                                bool resid_epilogue, const GemmDst& dst, char* err, int errlen);
 void tc_gemm_plan_destroy(TcGemmPlan*);
 void tc_gemm_plan_tile(const TcGemmPlan*, int* bn, int* bk);  // the (BN, BK) tile the plan launches
+// 0, -2 for a tile without a kernel, -3 when e names other epilogue buffers than the plan's GemmDst
 int launch_gemm_tc(const TcGemmPlan* plan, const EpiParams& e, cudaStream_t st);
 
 struct TcAttnPlan;

@@ -1,6 +1,6 @@
 // GEMM epilogues shared by the fp32 CUDA-core GEMM and the h16 wgmma GEMM.
 // epilogue_apply: a thread hands over CNT consecutive accumulator columns [n0, n0+CNT) of output row m;
-// epilogue_pair: two adjacent columns [n, n+1) of row m (the wgmma accumulator fragment).
+// epi_bias_gelu / epi_resid / epi_rope / epi_gates_pair: two adjacent columns [n, n+1) (the wgmma accumulator fragment).
 #pragma once
 #include "bt_kernels.h"
 #include <cuda_fp16.h>
@@ -162,38 +162,37 @@ __device__ __forceinline__ void epilogue_apply(const EpiParams& e, int L, int64_
   }
 }
 
-// The same operations for the column pair (n, n + 1), n even, of output row m: the pair a thread of a wgmma
-// accumulator fragment holds.  For kind 1 the pair is one interleaved RoPE pair and (co, si) its rotation at the
-// row's position, read once per row by the caller.  KIND is e.kind as a template argument: only the gates
-// instantiation (KIND 2) contains the IEEE division of sigmoidf_, whose slow path is a function call.
-template <typename TAct, int KIND>
-__device__ __forceinline__ void epilogue_pair(const EpiParams& e, int64_t m, int n, float v0, float v1, float co = 0.f,
-                                              float si = 0.f) {
-  if constexpr (KIND == 0) {
-    if (e.bias) {
-      const float2 b = __ldg(reinterpret_cast<const float2*>(e.bias + n));
-      v0 += b.x; v1 += b.y;
-    }
-    if (e.gelu) { v0 = gelu_for<TAct>(v0); v1 = gelu_for<TAct>(v1); }
-    if (e.resid) {
-      const float2 r = *reinterpret_cast<const float2*>(e.resid + m * e.ldr + n);
-      v0 += r.x; v1 += r.y;
-    }
-    if (e.out_f32) *reinterpret_cast<float2*>(e.out_f32 + m * e.ldo_f32 + n) = make_float2(v0, v1);
-    if (e.out_act) *reinterpret_cast<uint32_t*>(reinterpret_cast<TAct*>(e.out_act) + m * e.ldo_act + n) = pack_h16x2(v0, v1);
-  } else if constexpr (KIND == 2) {
-    if (n < e.heads) e.out_f32[m * e.heads + n] = sigmoidf_(v0 + __ldg(e.bias + n));
-    if (n + 1 < e.heads) e.out_f32[m * e.heads + n + 1] = sigmoidf_(v1 + __ldg(e.bias + n + 1));
-  } else {
-    const int which = n / e.C;  // 0 q, 1 k, 2 v
-    if (which < 2) {
-      const float sc = which == 0 ? e.qscale : 1.0f;
-      const float x0 = v0, x1 = v1;
-      v0 = (x0 * co - x1 * si) * sc;
-      v1 = (x1 * co + x0 * si) * sc;
-    }
-    *reinterpret_cast<uint32_t*>(reinterpret_cast<TAct*>(e.out_act) + m * e.ldo_act + n) = pack_h16x2(v0, v1);
+// The same operations for the column pair (n, n + 1), n even, the pair a thread of a wgmma accumulator fragment holds.
+// The 16-bit GEMM applies them to its accumulators in place; kinds 0 and 1 then stage the values through shared memory
+// (fp32 as they are, 16-bit through pack_h16x2), the gates (kind 2) store straight from registers.
+// Kind 0, in this order: bias, GELU, then the fp32 residual (epi_resid).
+template <typename TAct>
+__device__ __forceinline__ void epi_bias_gelu(const EpiParams& e, int n, float& v0, float& v1) {
+  if (e.bias) {
+    const float2 b = __ldg(reinterpret_cast<const float2*>(e.bias + n));
+    v0 += b.x; v1 += b.y;
   }
+  if (e.gelu) { v0 = gelu_for<TAct>(v0); v1 = gelu_for<TAct>(v1); }
+}
+__device__ __forceinline__ void epi_resid(float& v0, float& v1, float2 r) { v0 += r.x; v1 += r.y; }
+// Kind 1: the pair is one interleaved RoPE pair and (co, si) its rotation at the row's position, read once per row by
+// the caller; q columns are also scaled by qscale, v columns pass unchanged.
+__device__ __forceinline__ void epi_rope(const EpiParams& e, int n, float& v0, float& v1, float co, float si) {
+  const int which = n / e.C;  // 0 q, 1 k, 2 v
+  if (which < 2) {
+    const float sc = which == 0 ? e.qscale : 1.0f;
+    const float x0 = v0, x1 = v1;
+    // (x0 co - x1 si) sc and (x1 co + x0 si) sc with the fused multiply-adds written out: left to the compiler, which
+    // product gets fused changes with the surrounding code, and with it the last bit of q and k
+    v0 = fmaf(x0, co, -__fmul_rn(x1, si)) * sc;
+    v1 = fmaf(x1, co, __fmul_rn(x0, si)) * sc;
+  }
+}
+// Kind 2 (attention gates) of output row m, stored from registers.  Only the gates instantiation contains the IEEE
+// division of sigmoidf_, whose slow path is a function call.
+__device__ __forceinline__ void epi_gates_pair(const EpiParams& e, int64_t m, int n, float v0, float v1) {
+  if (n < e.heads) e.out_f32[m * e.heads + n] = sigmoidf_(v0 + __ldg(e.bias + n));
+  if (n + 1 < e.heads) e.out_f32[m * e.heads + n + 1] = sigmoidf_(v1 + __ldg(e.bias + n + 1));
 }
 
 }  // namespace bt

@@ -28,6 +28,25 @@ template <int N>
 __device__ __forceinline__ void bulk_wait_read() {  // at most N of this thread's bulk groups still read shared memory
   asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
 }
+// barrier `id` (1..15) over `count` threads of the CTA, leaving the others running
+__device__ __forceinline__ void named_bar_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+// four 8x8 16-bit matrices from the mma accumulator layout: register i of lane l holds row l / 4, columns 2 (l % 4)
+// and 2 (l % 4) + 1 of matrix i; lane l gives the shared address of row l % 8 of matrix l / 8
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1), "r"(r2),
+               "r"(r3)
+               : "memory");
+}
+__device__ __forceinline__ float2 ld_shared_v2_f32(uint32_t addr) {
+  float2 q;
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(q.x), "=f"(q.y) : "r"(addr) : "memory");
+  return q;
+}
+__device__ __forceinline__ void st_shared_v2_f32(uint32_t addr, float x, float y) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(x), "f"(y) : "memory");
+}
 
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
