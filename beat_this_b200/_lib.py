@@ -15,7 +15,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 # BT_LIB_PATH: an instrumented build of the same sources (e.g. build(extra_flags=("-DBT_FF_PROF",), out_path=...))
 LIB_PATH = os.environ.get("BT_LIB_PATH") or os.path.join(HERE, "libbeatthis_sm90.so")
-SOURCES = ["bt_api.cu", "kernels_simt.cu", "kernels_misc.cu", "kernels_gemm.cu", "kernels_attn.cu", "kernels_fused.cu", "kernels_dbn.cu", "kernels_eval.cu", "dbn_host.cpp", "host_stage.cpp"]
+SOURCES = ["bt_api.cu", "kernels_simt.cu", "kernels_misc.cu", "kernels_gemm.cu", "kernels_attn.cu", "kernels_fused.cu", "kernels_dbn.cu", "kernels_eval.cu", "kernels_loss.cu", "dbn_host.cpp", "host_stage.cpp"]
 HEADERS = ["common.cuh", "epilogue.cuh", "tc_common.cuh", "bt_kernels.h", "cuda_owned.h", "dbn_model.h", os.path.join("..", "..", "include", "beatthis.h")]
 
 BT_DTYPE_F32 = 0
@@ -79,6 +79,14 @@ class bt_beat_metric_params(ctypes.Structure):
     ]
 
 
+class bt_loss_params(ctypes.Structure):
+    _fields_ = [
+        ("kind", c_int32),
+        ("tolerance", c_int32),
+        ("pos_weight", c_float),
+    ]
+
+
 # every symbol include/beatthis.h declares: name -> (restype, argtypes)
 PROTOTYPES = {
     "bt_version": (c_int, []),
@@ -118,6 +126,14 @@ PROTOTYPES = {
     ),
     "bt_beat_metrics": (
         c_int, [c_void_p, c_void_p, POINTER(c_int64), c_void_p, POINTER(c_int64), c_int32, POINTER(bt_beat_metric_params),
+                c_void_p, c_void_p],
+    ),
+    "bt_beat_loss": (
+        c_int, [c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int64), c_int32, POINTER(bt_loss_params), c_void_p,
+                c_void_p, c_void_p],
+    ),
+    "bt_beat_loss_backward": (
+        c_int, [c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int64), c_int32, POINTER(bt_loss_params), c_void_p,
                 c_void_p, c_void_p],
     ),
     "bt_spect2frames": (c_int, [c_void_p, c_void_p, POINTER(c_int64), c_int32, c_void_p, c_void_p, c_void_p]),

@@ -96,6 +96,8 @@ struct bt_ctx {
   // per-model results and path codes; back pointers
   DeviceBuffer<char> dbn_ws;
   DeviceBuffer<uint8_t> dbn_bp;
+  // per-CTA partial sums of bt_beat_loss (grows on demand)
+  DeviceBuffer<double> loss_partials;
   // pinned staging + device tables
   StageSlot stage[kStageSlots];
   int stage_next = 0;
@@ -693,7 +695,7 @@ std::vector<ParamSpec> layer_params(const Layer& l, int64_t D) {
 // ================================================================================== C ABI
 extern "C" {
 
-int bt_version(void) { return 202; }
+int bt_version(void) { return 203; }
 
 const char* bt_act_dtype(void) {
 #if defined(BT_ACT_BF16)
@@ -1304,6 +1306,97 @@ int bt_beat_metrics(bt_ctx* c, const double* est_dev, const int64_t* est_offsets
   if (const int e = launch_beat_metrics(est_dev, off_dev[0], ref_dev, off_dev[1], n_sets, p, out_dev, st))
     return fail(c, BT_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(static_cast<cudaError_t>(e)));
   BT_LAUNCHED(c, "beat_metrics", st);
+  return BT_OK;
+}
+
+static_assert(BT_LOSS_MAX_TOLERANCE == kLossMaxTolerance, "bt_loss_params tolerance cap");
+
+namespace {
+
+// The checks bt_beat_loss and its backward share, before anything is enqueued: params, pointers, offsets.  Fills the
+// kernels' view of the params, the CTA prefix per row (forward or backward tiling) and the scored frames of all rows.
+int loss_prepare(bt_ctx* c, const char* fn, const float* preds, const float* targets, const float* mask,
+                 const int64_t* off, int32_t n_rows, const bt_loss_params* params, bool backward, LossParams* p,
+                 std::vector<int64_t>* tile_first, int64_t* n_scored) {
+  if (!params || !off || !preds || !targets) return fail(c, BT_ERR_ARG, "%s: null argument", fn);
+  *p = LossParams{params->kind, params->tolerance, params->pos_weight};
+  if (p->kind < BT_LOSS_MASKED_BCE || p->kind > BT_LOSS_SPLIT_SHIFT_TOLERANT)
+    return fail(c, BT_ERR_ARG, "%s: unknown loss kind %d", fn, p->kind);
+  if (p->tolerance < 0 || p->tolerance > BT_LOSS_MAX_TOLERANCE)
+    return fail(c, BT_ERR_ARG, "%s: tolerance %d outside [0, %d]", fn, p->tolerance, BT_LOSS_MAX_TOLERANCE);
+  if (!std::isfinite(p->pos_weight)) return fail(c, BT_ERR_ARG, "%s: pos_weight must be finite", fn);
+  if (p->kind == BT_LOSS_SPLIT_SHIFT_TOLERANT && !mask) return fail(c, BT_ERR_ARG, "%s: the split kind needs a mask", fn);
+  if (n_rows < 1 || off[0] != 0) return fail(c, BT_ERR_ARG, "%s: need n_rows >= 1 and offsets from 0", fn);
+  const int64_t min_len = p->kind == BT_LOSS_MASKED_BCE ? 1 : 4 * static_cast<int64_t>(p->tolerance) + 1;
+  tile_first->assign(1, 0);
+  *n_scored = 0;
+  for (int i = 0; i < n_rows; ++i) {
+    const int64_t len = off[i + 1] - off[i];
+    if (len < min_len) return fail(c, BT_ERR_ARG, "%s: row %d has %lld frames, fewer than %lld", fn, i,
+                                   static_cast<long long>(len), static_cast<long long>(min_len));
+    tile_first->push_back(tile_first->back() + loss_tiles(len, *p, backward));
+    *n_scored += p->kind == BT_LOSS_MASKED_BCE ? len : len - 4 * static_cast<int64_t>(p->tolerance);
+  }
+  if (tile_first->back() > 0x7fffffff) return fail(c, BT_ERR_ARG, "%s: too many frames", fn);
+  return BT_OK;
+}
+
+}  // namespace
+
+int bt_beat_loss(bt_ctx* c, const float* preds_dev, const float* targets_dev, const float* mask_dev,
+                 const int64_t* row_offsets_host, int32_t n_rows, const bt_loss_params* params, double* row_loss_dev,
+                 float* mean_dev, void* stream) {
+  if (!c) return BT_ERR_ARG;
+  const char* fn = "bt_beat_loss";
+  LossParams p;
+  std::vector<int64_t> tiles;
+  int64_t n_scored = 0;
+  int r = loss_prepare(c, fn, preds_dev, targets_dev, mask_dev, row_offsets_host, n_rows, params, false, &p, &tiles,
+                       &n_scored);
+  if (r != BT_OK) return r;
+  if (!row_loss_dev || !mean_dev) return fail(c, BT_ERR_ARG, "%s: null output", fn);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  BT_CUDA(c, cudaSetDevice(c->device));
+  prof_mark(c, st);
+  const int64_t n_tiles = tiles.back();
+  const size_t bytes = sizeof(double) * n_tiles;
+  BT_CUDA(c, c->loss_partials.reserve(bytes, bytes + bytes / 4));
+  const size_t n = static_cast<size_t>(n_rows) + 1;
+  const int64_t* dev[2];
+  if ((r = stage(c, st, {{row_offsets_host, n}, {tiles.data(), n}}, dev)) != BT_OK) return r;
+  if (const int e = launch_beat_loss(preds_dev, targets_dev, mask_dev, dev[0], dev[1], n_rows, n_tiles, p,
+                                     c->loss_partials.get(), st))
+    return fail(c, BT_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(static_cast<cudaError_t>(e)));
+  BT_LAUNCHED(c, "beat_loss", st);
+  if (const int e = launch_beat_loss_reduce(c->loss_partials.get(), dev[0], dev[1], n_rows, n_tiles, n_scored, p,
+                                            row_loss_dev, mean_dev, st))
+    return fail(c, BT_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(static_cast<cudaError_t>(e)));
+  BT_LAUNCHED(c, "beat_loss_reduce", st);
+  return BT_OK;
+}
+
+int bt_beat_loss_backward(bt_ctx* c, const float* preds_dev, const float* targets_dev, const float* mask_dev,
+                          const int64_t* row_offsets_host, int32_t n_rows, const bt_loss_params* params,
+                          const float* grad_mean_dev, float* grad_preds_dev, void* stream) {
+  if (!c) return BT_ERR_ARG;
+  const char* fn = "bt_beat_loss_backward";
+  LossParams p;
+  std::vector<int64_t> tiles;
+  int64_t n_scored = 0;
+  int r = loss_prepare(c, fn, preds_dev, targets_dev, mask_dev, row_offsets_host, n_rows, params, true, &p, &tiles,
+                       &n_scored);
+  if (r != BT_OK) return r;
+  if (!grad_mean_dev || !grad_preds_dev) return fail(c, BT_ERR_ARG, "%s: null gradient pointer", fn);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  BT_CUDA(c, cudaSetDevice(c->device));
+  prof_mark(c, st);
+  const size_t n = static_cast<size_t>(n_rows) + 1;
+  const int64_t* dev[2];
+  if ((r = stage(c, st, {{row_offsets_host, n}, {tiles.data(), n}}, dev)) != BT_OK) return r;
+  if (const int e = launch_beat_loss_backward(preds_dev, targets_dev, mask_dev, dev[0], dev[1], n_rows, tiles.back(),
+                                              n_scored, p, grad_mean_dev, grad_preds_dev, st))
+    return fail(c, BT_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(static_cast<cudaError_t>(e)));
+  BT_LAUNCHED(c, "beat_loss_backward", st);
   return BT_OK;
 }
 

@@ -139,6 +139,30 @@ constexpr int kBeatMetricCols = 12;
 int launch_beat_metrics(const double* est, const int64_t* est_off_dev, const double* ref, const int64_t* ref_off_dev,
                         int n_sets, const BeatMetricParams& p, double* out, cudaStream_t st);
 
+// ---- training losses (kernels_loss.cu) ----------------------------------------------------------------------------
+// The contract of bt_beat_loss (include/beatthis.h).  Rows are CSR over row_off_dev; tile_first_dev[i] is the first CTA
+// of row i ([n_rows + 1], prefix of the per-row tile counts the launchers' loss_tiles gives).
+constexpr int kLossTile = 256;
+constexpr int kLossMaxTolerance = 64;
+struct LossParams {
+  int kind, tolerance;
+  float pos_weight;
+};
+// CTAs row i needs: scored frames (forward) or frames (backward) over kLossTile
+int64_t loss_tiles(int64_t len, const LossParams& p, bool backward);
+// forward: one float64 partial per CTA into partials, then one CTA reduces them in a fixed order into row_loss and
+// *mean (n_scored: scored frames of all rows).  Each returns a cudaError_t.
+int launch_beat_loss(const float* x, const float* y, const float* m, const int64_t* row_off_dev,
+                     const int64_t* tile_first_dev, int n_rows, int64_t n_tiles, const LossParams& p, double* partials,
+                     cudaStream_t st);
+int launch_beat_loss_reduce(const double* partials, const int64_t* row_off_dev, const int64_t* tile_first_dev, int n_rows,
+                            int64_t n_tiles, int64_t n_scored, const LossParams& p, double* row_loss, float* mean,
+                            cudaStream_t st);
+// backward: grad[j] for every frame (gather over the windows covering j).  One launch; returns a cudaError_t.
+int launch_beat_loss_backward(const float* x, const float* y, const float* m, const int64_t* row_off_dev,
+                              const int64_t* tile_first_dev, int n_rows, int64_t n_tiles, int64_t n_scored,
+                              const LossParams& p, const float* grad_mean, float* grad, cudaStream_t st);
+
 void launch_f32_to_h16(const float* in, void* out, int64_t n, cudaStream_t st);
 void launch_h16_to_f32(const void* in, float* out, int64_t n, cudaStream_t st);
 // [seqs, L, heads*32] fp32 q,k,v -> packed qkv buffer [seqs*L, 3C] of the activation dtype

@@ -6,6 +6,7 @@
 * ``evaluate`` runs a model over annotated pieces (audio files or stored spectrograms) through the batched inference
   path, restricts the truth to the piece (``prepare_annotations``, dataset.py:536-547) and scores beats and downbeats
   in one metric launch.  Its summary keys are the reference's (``_compute_metrics_target``, pl_module.py:131-160).
+  With ``losses=True`` (``--losses``) it adds the test losses of the checkpoint's loss pair (``piece_losses``).
 * ``python -m beat_this_b200.evaluate`` is the command line counterpart of compute_paper_metrics.py.
 
     python -m beat_this_b200.evaluate --models final0.ckpt --data data          # prepared dataset layout
@@ -28,6 +29,7 @@ from . import _lib
 
 FIELDS = ("n_ref", "n_est", "matches", "P", "R", "F", "cemgil", "cemgil_max", "CMLc", "CMLt", "AMLc", "AMLt")
 SUMMARY_KEYS = tuple(f"{k}_{t}" for t in ("beat", "downbeat") for k in ("F-measure", "Cemgil", "CMLt", "AMLt"))
+LOSS_KEYS = ("test_loss_beat", "test_loss_downbeat", "test_loss")
 FPS = 50
 
 _engines = {}
@@ -148,11 +150,20 @@ def _frames_of_audio(runner, path) -> int:
     return 1 + n // 441
 
 
-def _predict(runner, pieces, group=64):
-    """(beats, downbeats) and spectrogram length of every piece through the batched inference path."""
-    preds, frames = [None] * len(pieces), [0] * len(pieces)
+def _predict(runner, pieces, group=64, logits=False):
+    """(beats, downbeats) and spectrogram length of every piece through the batched inference path; with `logits`,
+    also every piece's (beat, downbeat) logits on the device (audio then goes through the frames path and the
+    runner's post-processor, which gives the same beats), else None."""
+    preds, frames, frame_logits = [None] * len(pieces), [0] * len(pieces), [None] * len(pieces)
     audio = [i for i, p in enumerate(pieces) if p.audio is not None]
-    if audio:
+    if audio and logits:
+        out = runner.frames_batch([pieces[i].audio for i in audio])
+        fo = np.cumsum([0] + [len(b) for b, _ in out]).tolist()
+        beat = torch.cat([b for b, _ in out]).contiguous()
+        down = torch.cat([d for _, d in out]).contiguous()
+        for i, r, o in zip(audio, runner.frames2beats.batch_cat(beat, down, fo), out):
+            preds[i], frames[i], frame_logits[i] = r, len(o[0]), o
+    elif audio:
         res = runner.batch([pieces[i].audio for i in audio])
         for i, r in zip(audio, res):
             preds[i] = r
@@ -166,9 +177,41 @@ def _predict(runner, pieces, group=64):
             fo.append(fo[-1] + b.shape[0])
         beat = torch.cat([b for b, _ in out]).contiguous()
         down = torch.cat([d for _, d in out]).contiguous()
-        for i, r, a, b in zip(idx, runner.frames2beats.batch_cat(beat, down, fo), fo[:-1], fo[1:]):
+        for i, r, a, b, o in zip(idx, runner.frames2beats.batch_cat(beat, down, fo), fo[:-1], fo[1:], out):
             preds[i], frames[i] = r, b - a
-    return preds, frames
+            if logits:
+                frame_logits[i] = o
+    return preds, frames, frame_logits
+
+
+def framewise_truth(times, T: int) -> np.ndarray:
+    """prepare_annotations(item, 0, T, 50)'s framewise truth (reference dataset.py:512-534) as fp32: 1 at the frames
+    np.round(time * 50) (half to even) inside [0, T), 0 elsewhere."""
+    f = np.round(np.asarray(times, dtype=np.float64) * FPS).astype(np.int64)
+    out = np.zeros(T, dtype=np.float32)
+    out[f[(f >= 0) & (f < T)]] = 1
+    return out
+
+
+def piece_losses(runner, pieces, logits) -> dict:
+    """The reference's test losses (test_step, pl_module.py:99-114,224-229) of every piece: the checkpoint's loss pair
+    (loss_from_hparams) on the full-piece logits against the framewise truth, the downbeat mask 0 for pieces without
+    downbeat annotations.  All beat rows in one bt_beat_loss call, all downbeat rows in another."""
+    from .loss import beat_loss_rows, loss_from_hparams, loss_spec
+
+    dev = runner.model.device
+    fo = np.cumsum([0] + [len(b) for b, _ in logits]).tolist()
+    out = {}
+    for t, (target, module) in enumerate(zip(("beat", "downbeat"), loss_from_hparams(runner.model.checkpoint_hparams))):
+        x = torch.cat([lg[t] for lg in logits]).contiguous()
+        truth = [framewise_truth(p.beats if t == 0 else p.downbeats, len(lg[t])) for p, lg in zip(pieces, logits)]
+        y = torch.from_numpy(np.concatenate(truth)).to(dev)
+        keep = [1.0 if t == 0 or p.has_downbeats else 0.0 for p in pieces]
+        m = torch.from_numpy(np.repeat(np.asarray(keep, np.float32), np.diff(fo))).to(dev)
+        rows, _ = beat_loss_rows(x, y, m, fo, *loss_spec(module))
+        out[f"test_loss_{target}"] = rows.cpu().numpy()
+    out["test_loss"] = out["test_loss_beat"] + out["test_loss_downbeat"]
+    return out
 
 
 def make_runner(model, device="cuda", float16=True, dbn=False, dbn_impl="auto"):
@@ -180,18 +223,20 @@ def make_runner(model, device="cuda", float16=True, dbn=False, dbn_impl="auto"):
     return File2Beats.from_model(model, dbn=dbn, dbn_impl=dbn_impl)
 
 
-def evaluate(model_or_runner, items, min_beat_time=5.0, device="cuda", float16=True, dbn=False, dbn_impl="auto"):
+def evaluate(model_or_runner, items, min_beat_time=5.0, device="cuda", float16=True, dbn=False, dbn_impl="auto",
+             losses=False):
     """Predict every Piece of `items` with the model (a File2Beats / Audio2Beats runner, a BeatThisB200 or a checkpoint;
     float16 / dbn / dbn_impl apply when a runner has to be built) and score it against its annotations: truth cut to
     [0, T / 50) for a spectrogram of T frames, beats and downbeats of all pieces in one bt_beat_metrics launch.
     "Cemgil_<target>" is the reference's mean of mir_eval's (cemgil, cemgil_max) pair (pl_module.py:157-160); both
     parts stay available as cemgil_<target> and cemgil_max_<target>.  Pieces without downbeat annotations score 0 on
-    the downbeat keys, as in the reference."""
+    the downbeat keys, as in the reference.  With `losses`, metrics also hold every piece's test_loss_beat,
+    test_loss_downbeat and test_loss (piece_losses), and summary their means."""
     runner = model_or_runner
     if not hasattr(runner, "frames2beats"):
         runner = make_runner(runner, device, float16, dbn, dbn_impl)
     pieces = list(items)
-    preds, frames = _predict(runner, pieces)
+    preds, frames, logits = _predict(runner, pieces, logits=losses)
     est, ref = [], []
     for target in (0, 1):
         for p, pr, T in zip(pieces, preds, frames):
@@ -212,7 +257,11 @@ def evaluate(model_or_runner, items, min_beat_time=5.0, device="cuda", float16=T
         for j, f in enumerate(FIELDS):
             metrics[f"{f}_{target}"] = rows[t * n : (t + 1) * n, j]
     metrics = {k: metrics[k] for k in (*SUMMARY_KEYS, *[k for k in metrics if k not in SUMMARY_KEYS])}
-    summary = {k: float(np.mean(metrics[k])) if n else float("nan") for k in SUMMARY_KEYS}
+    keys = SUMMARY_KEYS
+    if losses and n:
+        metrics.update(piece_losses(runner, pieces, logits))
+        keys = (*SUMMARY_KEYS, *LOSS_KEYS)
+    summary = {k: float(np.mean(metrics[k])) if n else float("nan") for k in keys}
     return EvalResult(pieces, metrics, preds, summary)
 
 
@@ -302,6 +351,8 @@ def build_parser() -> argparse.ArgumentParser:
     add("--aggregation-type", default="mean-std", choices=["mean-std"],
         help="summary over several models [%(default)s]")
     add("--dump-predictions", metavar="FILENAME", default=None, help="write the predictions to this .npz file")
+    add("--losses", action="store_true",
+        help="also report the test losses of the checkpoint's loss_type (test_loss_beat, test_loss_downbeat, test_loss)")
     return ap
 
 
@@ -325,7 +376,7 @@ def _print_mean_std(summaries: list) -> None:
 
 
 def run(models, data=None, audio=None, annotations=None, items=None, gpu=0, eval_trim_beats=None, dbn=None,
-        dbn_impl="auto", float16=True, aggregation_type="mean-std", dump_predictions=None) -> int:
+        dbn_impl="auto", float16=True, aggregation_type="mean-std", dump_predictions=None, losses=False) -> int:
     from .inference import load_checkpoint
 
     if audio is not None and annotations is None:
@@ -343,7 +394,7 @@ def run(models, data=None, audio=None, annotations=None, items=None, gpu=0, eval
         trim = eval_trim_beats if eval_trim_beats is not None else float(hp.get("eval_trim_beats", 5))
         use_dbn = dbn if dbn is not None else bool(hp.get("use_dbn", False))
         runner = make_runner(ckpt, f"cuda:{gpu}", float16, use_dbn, dbn_impl)
-        result = evaluate(runner, pieces, min_beat_time=trim)
+        result = evaluate(runner, pieces, min_beat_time=trim, losses=losses)
         summaries.append(result.summary)
         if len(models) == 1:
             _print_single(result)

@@ -18,6 +18,7 @@ import math
 import numpy as np
 import torch
 
+from ._lib import bt_wav_info
 from .engine import Engine
 from .pipeline import BeatPipeline, as_signal_array, chunk_cost, plan_groups
 from .postprocessor import Postprocessor
@@ -61,6 +62,7 @@ class BeatThisB200:
     weights living on one GPU inside a ``bt_ctx``."""
 
     def __init__(self, hparams: dict, packed: dict, device, float16: bool = False, wave_chunks: int | None = None):
+        self.checkpoint_hparams = dict(hparams)  # all of them, the training ones (loss_type, pos_weights ...) included
         self.hparams = filter_hparams(hparams)
         self.engine = Engine(packed, self.hparams, device, half=float16, wave_chunks=wave_chunks)
         self.device = self.engine.device
@@ -95,9 +97,9 @@ def load_model(checkpoint_path: str | dict | None = "final0", device: str | torc
     if checkpoint_path is None:
         raise ValueError("beat_this_b200 needs a checkpoint (the reference's random-init BeatThis() has no use here)")
     checkpoint = checkpoint_path if isinstance(checkpoint_path, dict) else load_checkpoint(checkpoint_path, "cpu")
-    hparams = filter_hparams(checkpoint["hyper_parameters"])
+    hparams = checkpoint["hyper_parameters"]
     state_dict = replace_state_dict_key(dict(checkpoint["state_dict"]), "model.", "")
-    packed = pack_parameters(state_dict, hparams)
+    packed = pack_parameters(state_dict, filter_hparams(hparams))
     return BeatThisB200(hparams, packed, device, float16, wave_chunks)
 
 
@@ -459,6 +461,38 @@ class File2Beats(Audio2Beats):
                     except Exception:
                         res.append(None)
             for i, r in zip(idx, res):
+                out[i] = r
+        return out
+
+
+    def frames_batch(self, audio_paths):
+        """Framewise (beat, downbeat) logits of many files as device tensors, through the groups and kernels of batch()
+        up to the post-processor: frames2beats.batch_cat of them gives batch()'s beats.  Errors raise."""
+        paths = [str(p) for p in audio_paths]
+        out = [None] * len(paths)
+        infos, is_wav = self.probe(paths)
+        for i in range(len(paths)):
+            if is_wav[i] and infos[i].frames * 22050 // max(1, infos[i].sample_rate) <= 512:
+                raise ValueError(f'"{paths[i]}" is too short ({infos[i].frames} samples)')
+        pipe = self.pipeline
+        for sr in sorted({infos[i].sample_rate for i in range(len(paths)) if is_wav[i]}):
+            idx = [i for i in range(len(paths)) if is_wav[i] and infos[i].sample_rate == sr]
+            groups = plan_groups([chunk_cost(infos[i].frames, sr) for i in idx], GROUP_CHUNKS, GROUP_CLIPS)
+
+            def submit(g, idx=idx, groups=groups, sr=sr):
+                sel = idx[groups[g][0] : groups[g][1]]
+                pipe.submit_wavs([paths[i] for i in sel], (bt_wav_info * len(sel))(*[infos[i] for i in sel]), sr, "frames")
+
+            try:
+                for (lo, hi), (beat, down, fo) in zip(groups, pipe.run(len(groups), submit)):
+                    for j, k in enumerate(idx[lo:hi]):
+                        out[k] = (beat[fo[j] : fo[j + 1]], down[fo[j] : fo[j + 1]])
+            finally:
+                pipe.drain()
+        loaded = {i: load_audio(paths[i]) for i in range(len(paths)) if not is_wav[i]}
+        for sr in sorted({s for _, s in loaded.values()}):
+            idx = [i for i in loaded if loaded[i][1] == sr]
+            for i, r in zip(idx, Audio2Frames.batch(self, [loaded[i][0] for i in idx], sr)):
                 out[i] = r
         return out
 

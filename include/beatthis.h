@@ -273,6 +273,51 @@ int bt_beat_metrics(bt_ctx* ctx, const double* est_dev, const int64_t* est_offse
                     const int64_t* ref_offsets_host, int32_t n_sets, const bt_beat_metric_params* params,
                     double* out_dev, void* stream);
 
+/* ---- losses: model/loss.py of the reference (MaskedBCELoss, ShiftTolerantBCELoss, SplittedShiftTolerantBCELoss) ---- */
+
+#define BT_LOSS_MASKED_BCE 0           /* MaskedBCELoss, loss.py:9-35                 */
+#define BT_LOSS_SHIFT_TOLERANT 1       /* ShiftTolerantBCELoss, loss.py:38-92         */
+#define BT_LOSS_SPLIT_SHIFT_TOLERANT 2 /* SplittedShiftTolerantBCELoss, loss.py:95-160 */
+#define BT_LOSS_MAX_TOLERANCE 64
+
+typedef struct bt_loss_params {
+  int32_t kind;       /* BT_LOSS_*                                                                    */
+  int32_t tolerance;  /* t in [0, BT_LOSS_MAX_TOLERANCE]: predictions max-pooled by 2t+1, targets by 4t+1
+                       * (ignored by BT_LOSS_MASKED_BCE)                                              */
+  float pos_weight;   /* p: weight of positive targets (binary_cross_entropy_with_logits pos_weight) */
+} bt_loss_params;
+
+/* Beat tracker training losses over n_rows rows of frames: row i is preds_dev / targets_dev / mask_dev (fp32) at
+ * [row_offsets_host[i], row_offsets_host[i+1]).  mask_dev may be NULL (weight 1) except for the split kind.
+ * With softplus(z) = log1p(exp(-|z|)) + max(z, 0), the element loss is torch's binary_cross_entropy_with_logits with
+ * pos_weight: l(x, y) = (1 - y) x + (1 + (p - 1) y) softplus(-x).  Per kind, for the frames c of a row of length len:
+ *  - MASKED_BCE: every frame is scored; term m_c l(x_c, y_c).
+ *  - SHIFT_TOLERANT: frames c in [2t, len - 2t) are scored; xs_c = max_{|d|<=t} x_{c+d}, ys_c = max_{|d|<=2t} y_{c+d};
+ *    term (y_c + (1 - ys_c)) m_c l(xs_c, y_c).
+ *  - SPLIT_SHIFT_TOLERANT: the same frames, xs_c and ys_c; term y_c m_c l(xs_c, y_c) + (1 - ys_c) m_c l(xs_c, ys_c).
+ *    Equal to SHIFT_TOLERANT for binary targets, different for soft ones.
+ * A loss is the sum of its terms over its number of scored frames (zero-weight frames included, as in torch's mean).
+ * row_loss_dev[i] (float64) is the loss of row i alone (the reference's batch-size-1 test step, pl_module.py:99-114,
+ * 224-229); *mean_dev (fp32) is the terms of all rows over the scored frames of all rows (for rows of equal length, the
+ * reference module's batch mean).  Terms are computed in fp32 and summed in float64, one partial per CTA, the
+ * partials reduced in a fixed order by a second launch: results are bitwise repeatable.
+ * BT_ERR_ARG, before anything is enqueued, for an unknown kind, a tolerance outside [0, BT_LOSS_MAX_TOLERANCE], a
+ * non-finite pos_weight, n_rows < 1, offsets that do not start at 0 or decrease, a row shorter than 4t + 1 frames
+ * (1 for MASKED_BCE; torch's max_pool1d raises there), a null pointer, or the split kind without a mask.  Works on a
+ * weight-less ctx.  Enqueues only: no synchronisation (the scratch of per-CTA partials grows on demand). */
+int bt_beat_loss(bt_ctx* ctx, const float* preds_dev, const float* targets_dev, const float* mask_dev,
+                 const int64_t* row_offsets_host, int32_t n_rows, const bt_loss_params* params, double* row_loss_dev,
+                 float* mean_dev, void* stream);
+
+/* d(mean)/d(preds) of bt_beat_loss with the same arguments, times the upstream gradient *grad_mean_dev (fp32, read on
+ * the device), into grad_preds_dev (every frame written; frames outside the scored range and its pooling windows get
+ * 0).  Torch's form per scored frame: ((p y + 1 - y) sigmoid(xs) - p y) w g / N, the sum of the two parts for the split
+ * kind; the max-pool routes it to the lowest index that attains the window maximum (max_pool1d_with_indices), and
+ * each frame sums the windows it wins in ascending order.  One launch; errors as bt_beat_loss. */
+int bt_beat_loss_backward(bt_ctx* ctx, const float* preds_dev, const float* targets_dev, const float* mask_dev,
+                          const int64_t* row_offsets_host, int32_t n_rows, const bt_loss_params* params,
+                          const float* grad_mean_dev, float* grad_preds_dev, void* stream);
+
 /* ---- introspection / tuning ----------------------------------------------------------------- */
 
 /* Upper bound on the chunks processed per wave (default 128; one wave = one launch of every
