@@ -53,13 +53,14 @@ struct StageSlot {
   bool pending = false;
 };
 
-// Tensor-core plans of one layer for one (wave size, chunk length) geometry: what its launches use, nothing else.
+// Tensor-core plans of one layer for one (wave size, chunk length) geometry.  Each launch of the 16-bit path makes its
+// plan from its operands when the geometry first runs; later waves of the geometry reuse it.
 struct LayerPlans {
   QkvPlan fqkv;              // attention, fused (C = 32 / 64)
   GemmPlan gates, qkv, out;  // attention: gates and QKV unless fused; out-projection
   AttnPlan attn;             // time attention
   FreqPlan freq;             // frequency attention
-  FfPlan ff, ff_op;          // FFN, fused; ff_op: after a frontend attention
+  FfPlan ff, ff_op;          // FFN, fused; ff_op: with the attention's out-projection in front (outproj_in_ff)
   GemmPlan ff1, ff2;         // FFN, unfused
   GemmPlan gemm;             // convolution, frontend.linear
 };
@@ -321,10 +322,26 @@ GemmShape plain_shape(int planes, int L, int N, int K, int lda) {
   return g;
 }
 
-int run_gemm(bt_ctx* c, const void* A, const Param* W, TcGemmPlan* plan, const GemmShape& g,
+// Fills an empty plan slot of layer l: create(err, errlen) makes the plan from the operands of the launch that uses it.
+template <class Plan, class Create>
+int make_plan(bt_ctx* c, const Layer& l, std::unique_ptr<Plan, CudaDestroy>& slot, Create create) {
+  if (slot) return BT_OK;
+  char err[512] = "";
+  slot.reset(create(err, static_cast<int>(sizeof(err))));
+  if (!slot) return fail(c, BT_ERR_CUDA, "tensor-core plan creation failed (%s): %s", l.name.c_str(), err);
+  return BT_OK;
+}
+
+// A GEMM of layer l over a wave of nb chunks.  The GEMMs that add the residual (attention-out, FFN-down) are planned
+// with the tile width of a residual epilogue.
+int run_gemm(bt_ctx* c, const Layer& l, int nb, GemmPlan& plan, const void* A, const Param* W, const GemmShape& g,
              const EpiParams& e, const char* what, cudaStream_t st) {
   if (c->dtype == BT_DTYPE_H16) {
-    if (launch_gemm_tc(plan, e, st) != 0) return fail(c, BT_ERR_CUDA, "tc gemm launch %s failed", what);
+    const int r = make_plan(c, l, plan, [&](char* err, int errlen) {
+      return tc_gemm_plan_create(A, W->b16.get(), g, nb * l.F, e.resid != nullptr, e, err, errlen);
+    });
+    if (r != BT_OK) return r;
+    if (launch_gemm_tc(plan.get(), st) != 0) return fail(c, BT_ERR_CUDA, "tc gemm launch %s failed", what);
   } else {
     launch_gemm_simt(reinterpret_cast<const float*>(A), W->f32.get(), g, e, st);
   }
@@ -349,37 +366,17 @@ bool is_attention(const Layer& l) { return l.kind == kAttnF || l.kind == kAttnT 
 // sub-blocks of width C = 32 / 64 (the first two frontend blocks) run as one fused kernel each on the 16-bit path
 bool fused(const Layer& l) { return (l.C == 32 || l.C == 64) && (l.kind != kFf || l.mult == 4); }
 
-// The out-projection + residual of attention layer i run inside the fused FFN after it (fused_ff_kernel<C, true>),
-// unless a tap asks to see the residual stream between the two.
-bool outproj_in_ff(const bt_ctx* c, const std::vector<LayerPlans>* wp, size_t i) {
-  return wp && i + 1 < wp->size() && (*wp)[i + 1].ff_op && c->tap_name != c->layers[i].name;
-}
-
-// the last convolution feeds frontend.linear in the activation dtype (XN) instead of the residual stream
-bool conv_feeds_linear(const bt_ctx* c, size_t i) {
-  return c->layers[i].kind == kConv && i + 1 < c->layers.size() && c->layers[i + 1].kind == kLin;
-}
-
-// The fp32 residual stream layer i reads and updates (other = false; i = layers.size(): what the head reads), and the
-// buffer a convolution writes its output to (other = true).  The stem writes X0; every convolution but the last moves
-// the stream to the other buffer.  The forward pass and its tensor-core plans (whose tensor maps hold these addresses)
-// both resolve the buffers here.
-float* residual_stream(const bt_ctx* c, size_t i, bool other = false) {
-  bool in_x1 = false;
-  for (size_t k = 0; k < i; ++k)
-    if (c->layers[k].kind == kConv && !conv_feeds_linear(c, k)) in_x1 = !in_x1;
-  return in_x1 != other ? c->ws.X1.get() : c->ws.X0.get();
-}
-
-// the 16-bit copy of its output that FFN layer i writes: the FFN in front of a convolution feeds it (16-bit path)
-void* ff_copy_act(const bt_ctx* c, size_t i) {
-  const bool before_conv = i + 1 < c->layers.size() && c->layers[i + 1].kind == kConv;
-  return c->dtype == BT_DTYPE_H16 && before_conv ? c->ws.XB.get() : nullptr;
+// The out-projection + residual of attention layer i run inside the fused FFN after it (fused_ff_kernel<C, true>) on
+// the 16-bit path when the attention is a frontend one, unless a tap asks to see the residual stream between the two.
+bool outproj_in_ff(const bt_ctx* c, size_t i) {
+  const Layer& l = c->layers[i];
+  return c->dtype == BT_DTYPE_H16 && (l.kind == kAttnF || l.kind == kAttnT) && i + 1 < c->layers.size() &&
+         c->layers[i + 1].kind == kFf && fused(c->layers[i + 1]) && c->tap_name != l.name;
 }
 
 // x += attention(x) over nb * F planes of L tokens with dim C (reference roformer.py:114-132).
 // kAttnF: sequences run over the F planes of each chunk (PartialFTTransformer attnF).
-int attention_block(bt_ctx* c, float* X, const Layer& l, const LayerPlans* tp, int nb, int L, bool out_in_ff,
+int attention_block(bt_ctx* c, float* X, const Layer& l, LayerPlans& tp, int nb, int L, bool out_in_ff,
                     const ChunkSrc* vl_chunks, cudaStream_t st) {
   const Workspace& ws = c->ws;
   const bool tc = c->dtype == BT_DTYPE_H16;
@@ -391,9 +388,10 @@ int attention_block(bt_ctx* c, float* X, const Layer& l, const LayerPlans* tp, i
   const float qscale = tc && !freq ? inv_sqrt_d * 1.4426950408889634f : 1.0f;
   int r = BT_OK;
   if (tc && fused(l)) {  // norm + gates + QKV + RoPE in one kernel
-    if (launch_fused_qkv(tp->fqkv.get(), X, wg->f32.get(), bg->f32.get(), c->rope_cos->f32.get(), c->rope_sin->f32.get(),
-                         ws.QKV.get(), ws.GATES.get(), L, F, freq ? 1 : 0, qscale, st) != 0)
-      return fail(c, BT_ERR_CUDA, "fused qkv launch failed");
+    r = make_plan(c, l, tp.fqkv, [&](char* err, int n) { return tc_qkv_plan_create(wqkv->b16.get(), C, M, err, n); });
+    if (r != BT_OK) return r;
+    launch_fused_qkv(tp.fqkv.get(), X, wg->f32.get(), bg->f32.get(), c->rope_cos->f32.get(), c->rope_sin->f32.get(),
+                     ws.QKV.get(), ws.GATES.get(), L, F, freq ? 1 : 0, qscale, st);
     BT_LAUNCHED(c, C == 32 ? "qkv_fused_c32" : "qkv_fused_c64", st);
   } else {
     // up to 2 heads (fp32 path only: the 16-bit path fuses those blocks): gates inside the norm kernel;
@@ -409,7 +407,7 @@ int attention_block(bt_ctx* c, float* X, const Layer& l, const LayerPlans* tp, i
       eg.bias = bg->f32.get();
       eg.heads = heads;
       eg.out_f32 = ws.GATES.get();
-      int rg = run_gemm(c, ws.XN.get(), wg, tp->gates.get(), gg, eg, front ? "gemm_gates_front" : "gemm_gates", st);
+      int rg = run_gemm(c, l, nb, tp.gates, ws.XN.get(), wg, gg, eg, front ? "gemm_gates_front" : "gemm_gates", st);
       if (rg != BT_OK) return rg;
     }
     EpiParams e{};
@@ -420,16 +418,27 @@ int attention_block(bt_ctx* c, float* X, const Layer& l, const LayerPlans* tp, i
     e.C = C; e.heads = heads; e.posmode = freq ? 1 : 0; e.F = F;
     e.qscale = qscale;
     GemmShape g = plain_shape(planes, L, 3 * C, C, C);
-    r = run_gemm(c, ws.XN.get(), wqkv, tp->qkv.get(), g, e, front ? "gemm_qkv_front" : "gemm_qkv", st);
+    r = run_gemm(c, l, nb, tp.qkv, ws.XN.get(), wqkv, g, e, front ? "gemm_qkv_front" : "gemm_qkv", st);
     if (r != BT_OK) return r;
   }
   if (freq) {
-    if (tc) launch_attn_freq_tc(tp->freq.get(), ws.GATES.get(), inv_sqrt_d, st);
-    else launch_attn_freq_simt(static_cast<const float*>(ws.QKV.get()), ws.GATES.get(), static_cast<float*>(ws.O.get()),
-                               nb, F, L, heads, inv_sqrt_d, st);
+    if (tc) {
+      r = make_plan(c, l, tp.freq, [&](char* err, int n) {
+        return tc_freq_plan_create(ws.QKV.get(), ws.O.get(), nb, F, L, heads, err, n);
+      });
+      if (r != BT_OK) return r;
+      launch_attn_freq_tc(tp.freq.get(), ws.GATES.get(), inv_sqrt_d, st);
+    } else {
+      launch_attn_freq_simt(static_cast<const float*>(ws.QKV.get()), ws.GATES.get(), static_cast<float*>(ws.O.get()),
+                            nb, F, L, heads, inv_sqrt_d, st);
+    }
     BT_LAUNCHED(c, "attn_freq", st);
   } else if (tc) {
-    launch_attn_time_tc(tp->attn.get(), ws.GATES.get(), ws.O.get(), st, vl_chunks, F);
+    r = make_plan(c, l, tp.attn, [&](char* err, int n) {
+      return tc_attn_plan_create(ws.QKV.get(), planes, L, heads, err, n);
+    });
+    if (r != BT_OK) return r;
+    launch_attn_time_tc(tp.attn.get(), ws.GATES.get(), ws.O.get(), st, vl_chunks, F);
     BT_LAUNCHED(c, "attn_time_tc", st);
   } else {
     launch_attn_time_simt(static_cast<const float*>(ws.QKV.get()), ws.GATES.get(), static_cast<float*>(ws.O.get()),
@@ -439,13 +448,13 @@ int attention_block(bt_ctx* c, float* X, const Layer& l, const LayerPlans* tp, i
   if (out_in_ff) return BT_OK;
   GemmShape go = plain_shape(planes, L, C, C, C);
   EpiParams eo = epi_generic(nullptr, 0, X, C, X, C, nullptr, 0);
-  return run_gemm(c, ws.O.get(), wout, tp->out.get(), go, eo, front ? "gemm_attn_out_front" : "gemm_attn_out", st);
+  return run_gemm(c, l, nb, tp.out, ws.O.get(), wout, go, eo, front ? "gemm_attn_out_front" : "gemm_attn_out", st);
 }
 
-// x += ff(x) (reference roformer.py:38-61); optionally also writes a 16-bit copy of the result.  with_outproj: the
-// fused kernel first adds the out-projection of the attention in front (LayerPlans::ff_op).
-int ff_block(bt_ctx* c, float* X, const Layer& l, const LayerPlans* tp, int nb, int L, bool with_outproj,
-             void* copy_act, cudaStream_t st) {
+// x += ff(x) (reference roformer.py:38-61); optionally also writes a 16-bit copy of the result.  wout: the
+// out-projection weight of the attention in front, which the fused kernel first adds (outproj_in_ff), or null.
+int ff_block(bt_ctx* c, float* X, const Layer& l, LayerPlans& tp, int nb, int L, const Param* wout, void* copy_act,
+             cudaStream_t st) {
   const Workspace& ws = c->ws;
   const bool tc = c->dtype == BT_DTYPE_H16;
   const bool front = l.F > 1;
@@ -453,9 +462,13 @@ int ff_block(bt_ctx* c, float* X, const Layer& l, const LayerPlans* tp, int nb, 
   const Param *w1 = l.w[0], *b1 = l.w[1], *w2 = l.w[2], *b2 = l.w[3];
   const int64_t M = static_cast<int64_t>(planes) * L;
   if (tc && fused(l)) {
-    const TcFfPlan* plan = with_outproj ? tp->ff_op.get() : tp->ff.get();
-    if (launch_fused_ff(plan, X, b1->f32.get(), b2->f32.get(), copy_act, st) != 0)
-      return fail(c, BT_ERR_CUDA, "fused ff launch failed");
+    FfPlan& plan = wout ? tp.ff_op : tp.ff;
+    const int r = make_plan(c, l, plan, [&](char* err, int n) {
+      return tc_ff_plan_create(w1->b16.get(), w2->b16.get(), C, M, wout ? ws.O.get() : nullptr,
+                               wout ? wout->b16.get() : nullptr, err, n);
+    });
+    if (r != BT_OK) return r;
+    launch_fused_ff(plan.get(), X, b1->f32.get(), b2->f32.get(), copy_act, st);
     BT_LAUNCHED(c, C == 32 ? "ff_fused_c32" : "ff_fused_c64", st);
     return BT_OK;
   }
@@ -463,11 +476,11 @@ int ff_block(bt_ctx* c, float* X, const Layer& l, const LayerPlans* tp, int nb, 
   BT_LAUNCHED(c, front ? "norm_front" : "norm", st);
   GemmShape g1 = plain_shape(planes, L, mult * C, C, C);
   EpiParams e1 = epi_generic(b1, 1, nullptr, 0, nullptr, 0, ws.H.get(), mult * C);
-  int r = run_gemm(c, ws.XN.get(), w1, tp->ff1.get(), g1, e1, front ? "gemm_ff1_front" : "gemm_ff1", st);
+  int r = run_gemm(c, l, nb, tp.ff1, ws.XN.get(), w1, g1, e1, front ? "gemm_ff1_front" : "gemm_ff1", st);
   if (r != BT_OK) return r;
   GemmShape g2 = plain_shape(planes, L, C, mult * C, mult * C);
   EpiParams e2 = epi_generic(b2, 0, X, C, X, C, copy_act, C);
-  return run_gemm(c, ws.H.get(), w2, tp->ff2.get(), g2, e2, front ? "gemm_ff2_front" : "gemm_ff2", st);
+  return run_gemm(c, l, nb, tp.ff2, ws.H.get(), w2, g2, e2, front ? "gemm_ff2_front" : "gemm_ff2", st);
 }
 
 GemmShape conv_shape(int nb, int F, int L, int C) {
@@ -487,83 +500,22 @@ GemmShape lin_shape(int nb, int L, int D, int Fo, int Co) {
   return g;
 }
 
-// the 16-bit plans of layer i for waves of nb chunks of L frames; false (message in err) when one cannot be made
-bool make_layer_plans(const bt_ctx* c, size_t i, int nb, int L, LayerPlans& p, char* err, int errlen) {
-  const Layer& l = c->layers[i];
-  const Workspace& ws = c->ws;
-  const int C = l.C, planes = nb * l.F;
-  const int64_t M = static_cast<int64_t>(planes) * L;
-  float* X = residual_stream(c, i);
-  // the epilogue destinations each launch of attention_block / ff_block / run_wave passes (GemmDst)
-  auto gemm = [&](const void* A, const Param* W, const GemmShape& g, const GemmDst& dst, bool resid = false) {
-    return GemmPlan(tc_gemm_plan_create(A, W->b16.get(), g, planes, resid, dst, err, errlen));
-  };
-  switch (l.kind) {
-    case kConv: {
-      const GemmDst dst = conv_feeds_linear(c, i) ? GemmDst{nullptr, 0, nullptr, 0, ws.XN.get(), 2 * C}
-                                                  : GemmDst{nullptr, 0, residual_stream(c, i, true), 2 * C, nullptr, 0};
-      return (p.gemm = gemm(ws.XB.get(), l.w[0], conv_shape(nb, l.F, L, C), dst)) != nullptr;
-    }
-    case kLin: {
-      const int D = c->hp.transformer_dim;
-      return (p.gemm = gemm(ws.XN.get(), l.w[0], lin_shape(nb, L, D, l.F, C), GemmDst{nullptr, 0, X, D, nullptr, 0})) !=
-             nullptr;
-    }
-    case kFf:
-      if (fused(l)) {
-        const void *w1 = l.w[0]->b16.get(), *w2 = l.w[2]->b16.get();
-        p.ff.reset(tc_ff_plan_create(w1, w2, C, M, nullptr, nullptr, err, errlen));
-        const Layer& prev = c->layers[i - 1];
-        if (prev.kind == kAttnF || prev.kind == kAttnT)  // ... and with the out-projection of the frontend attention in front
-          p.ff_op.reset(tc_ff_plan_create(w1, w2, C, M, ws.O.get(), prev.w[3]->b16.get(), err, errlen));
-        return p.ff && (p.ff_op || prev.kind == kAttn);
-      }
-      p.ff1 = gemm(ws.XN.get(), l.w[0], plain_shape(planes, L, l.mult * C, C, C),
-                   GemmDst{nullptr, 0, nullptr, 0, ws.H.get(), l.mult * C});
-      p.ff2 = gemm(ws.H.get(), l.w[2], plain_shape(planes, L, C, l.mult * C, l.mult * C),
-                   GemmDst{X, C, X, C, ff_copy_act(c, i), C}, true);
-      return p.ff1 && p.ff2;
-    default:  // attention
-      if (fused(l)) {
-        p.fqkv.reset(tc_qkv_plan_create(l.w[0]->b16.get(), C, M, err, errlen));
-        if (!p.fqkv) return false;
-      } else {
-        p.gates = gemm(ws.XN.get(), l.w[1], plain_shape(planes, L, 32, C, C), GemmDst{});
-        p.qkv = gemm(ws.XN.get(), l.w[0], plain_shape(planes, L, 3 * C, C, C),
-                     GemmDst{nullptr, 0, nullptr, 0, ws.QKV.get(), 3 * C});
-        if (!p.gates || !p.qkv) return false;
-      }
-      const int heads = C / kHeadDim;
-      if (l.kind == kAttnF) p.freq.reset(tc_freq_plan_create(ws.QKV.get(), ws.O.get(), nb, l.F, L, heads, err, errlen));
-      else p.attn.reset(tc_attn_plan_create(ws.QKV.get(), planes, L, heads, err, errlen));
-      if (!p.freq && !p.attn) return false;
-      return (p.out = gemm(ws.O.get(), l.w[3], plain_shape(planes, L, C, C, C), GemmDst{X, C, X, C, nullptr, 0}, true)) !=
-             nullptr;
-  }
-}
-
-int build_plans(bt_ctx* c, int nb, int L, std::vector<LayerPlans>** out) {
+// The plans of the wave geometry (nb, L), one LayerPlans per layer, filled by the launches of its first wave (the fp32
+// path fills none).  Bounded cache: tensor maps are copied into the kernel parameters at launch, so dropping the oldest
+// geometry is safe while its kernels are still in flight.
+std::vector<LayerPlans>& geometry_plans(bt_ctx* c, int nb, int L) {
   auto key = std::make_pair(nb, L);
   Workspace& ws = c->ws;
   auto it = ws.plans.find(key);
-  if (it != ws.plans.end()) { *out = &it->second; return BT_OK; }
-  // bounded cache: tensor maps are copied into the kernel parameters at launch, so dropping the oldest geometry is
-  // safe while its kernels are still in flight
+  if (it != ws.plans.end()) return it->second;
   constexpr size_t kMaxPlans = 48;
   while (ws.plans.size() >= kMaxPlans && !ws.plan_order.empty()) {
     auto old = ws.plans.find(ws.plan_order.front());
     if (old != ws.plans.end()) ws.plans.erase(old);
     ws.plan_order.erase(ws.plan_order.begin());
   }
-  std::vector<LayerPlans> v(c->layers.size());
-  char err[512] = "";
-  for (size_t i = 0; i < v.size(); ++i) {
-    if (!make_layer_plans(c, i, nb, L, v[i], err, sizeof(err)))  // never cache a half-built entry
-      return fail(c, BT_ERR_CUDA, "tensor-core plan creation failed (%s): %s", c->layers[i].name.c_str(), err);
-  }
   ws.plan_order.push_back(key);
-  *out = &(ws.plans[key] = std::move(v));
-  return BT_OK;
+  return ws.plans[key] = std::vector<LayerPlans>(c->layers.size());
 }
 
 // BeatThis.forward for one wave of nb equal-length chunks, scattering the head output.
@@ -571,31 +523,32 @@ int run_wave(bt_ctx* c, const float* spect, const Wave& wv, float* beat, float* 
   const bool tc = c->dtype == BT_DTYPE_H16;
   const Workspace& ws = c->ws;
   const int nb = wv.nb, L = wv.L;
-  static const LayerPlans kNoPlans{};  // the fp32 path's launches take no plans
-  std::vector<LayerPlans>* wp = nullptr;
+  std::vector<LayerPlans>& plans = geometry_plans(c, nb, L);
   int r;
-  if (tc && (r = build_plans(c, nb, L, &wp)) != BT_OK) return r;
   // chunks shorter than the wave's padded length: the time attentions mask their missing keys and the convolutions
   // see zeros beyond their last frame (everything else works row by row, padding rows are never read back)
   const ChunkSrc* vl = wv.varlen ? wv.chunks_dev : nullptr;
+  // the fp32 residual stream: the stem writes X0, and every convolution but the last writes Xalt, which then carries it
+  float *X = ws.X0.get(), *Xalt = ws.X1.get();
   launch_stem(spect, wv.chunks_dev, nb, L, c->bn1_scale->f32.get(), c->bn1_shift->f32.get(), c->stem_w->f32.get(),
-              c->stem_b->f32.get(), residual_stream(c, 0), st);
+              c->stem_b->f32.get(), X, st);
   BT_LAUNCHED(c, "stem", st);
-  if ((r = do_tap(c, "stem", residual_stream(c, 0), static_cast<int64_t>(nb) * (c->hp.spect_dim / 4) * L * c->hp.stem_dim, false, st)) != BT_OK)
+  if ((r = do_tap(c, "stem", X, static_cast<int64_t>(nb) * (c->hp.spect_dim / 4) * L * c->hp.stem_dim, false, st)) != BT_OK)
     return r;
   const std::vector<Layer>& layers = c->layers;
   for (size_t i = 0; i < layers.size(); ++i) {
     const Layer& l = layers[i];
-    const LayerPlans* tp = wp ? &(*wp)[i] : &kNoPlans;
+    LayerPlans& tp = plans[i];
     const char* tap = l.name.c_str();
-    float* X = residual_stream(c, i);
     const void* out = X;  // the layer's output (tap)
     bool out_act = false;
     int64_t elems = static_cast<int64_t>(nb) * l.F * L * l.C;
     if (is_attention(l)) {
-      r = attention_block(c, X, l, tp, nb, L, outproj_in_ff(c, wp, i), l.kind == kAttnF ? nullptr : vl, st);
+      r = attention_block(c, X, l, tp, nb, L, outproj_in_ff(c, i), l.kind == kAttnF ? nullptr : vl, st);
     } else if (l.kind == kFf) {
-      r = ff_block(c, X, l, tp, nb, L, outproj_in_ff(c, wp, i - 1), ff_copy_act(c, i), st);
+      // the FFN in front of a convolution also writes the 16-bit copy the convolution reads (16-bit path)
+      void* copy_act = tc && i + 1 < layers.size() && layers[i + 1].kind == kConv ? ws.XB.get() : nullptr;
+      r = ff_block(c, X, l, tp, nb, L, i > 0 && outproj_in_ff(c, i - 1) ? layers[i - 1].w[3] : nullptr, copy_act, st);
     } else if (l.kind == kConv) {
       if (tc && (i == 0 || layers[i - 1].kind != kFf)) {  // no FFN in front (no partial transformers)
         launch_f32_to_h16(X, ws.XB.get(), elems, st);
@@ -605,30 +558,30 @@ int run_wave(bt_ctx* c, const float* spect, const Wave& wv, float* beat, float* 
         launch_zero_tail(tc ? ws.XB.get() : static_cast<void*>(X), tc ? 2 : 4, vl, nb, l.F, L, l.C, st);
         BT_LAUNCHED(c, "zero_tail", st);
       }
-      // conv C -> 2C (+ folded BN2d + GELU); the last one feeds frontend.linear (activation dtype)
-      const bool last = conv_feeds_linear(c, i);
-      float* Xalt = residual_stream(c, i, true);
+      // conv C -> 2C (+ folded BN2d + GELU); the last one feeds frontend.linear in the activation dtype (XN) instead
+      const bool last = i + 1 < layers.size() && layers[i + 1].kind == kLin;
       void* act_out = last ? ws.XN.get() : nullptr;
       EpiParams e = epi_generic(l.w[1], 1, nullptr, 0, last ? nullptr : Xalt, 2 * l.C, act_out, 2 * l.C);
-      r = run_gemm(c, tc ? ws.XB.get() : static_cast<const void*>(X), l.w[0], tp->gemm.get(),
+      r = run_gemm(c, l, nb, tp.gemm, tc ? ws.XB.get() : static_cast<const void*>(X), l.w[0],
                    conv_shape(nb, l.F, L, l.C), e, "gemm_conv", st);
       if (last) {
         out = ws.XN.get();
         out_act = true;
       } else {
         out = Xalt;
+        std::swap(X, Xalt);
       }
     } else {  // kLin
       const int D = c->hp.transformer_dim;
       EpiParams e = epi_generic(l.w[1], 0, nullptr, 0, X, D, nullptr, 0);
-      r = run_gemm(c, ws.XN.get(), l.w[0], tp->gemm.get(), lin_shape(nb, L, D, l.F, l.C), e, "gemm_frontend_linear",
+      r = run_gemm(c, l, nb, tp.gemm, ws.XN.get(), l.w[0], lin_shape(nb, L, D, l.F, l.C), e, "gemm_frontend_linear",
                    st);
       tap = "frontend";
       elems = static_cast<int64_t>(nb) * L * D;
     }
     if (r != BT_OK || (r = do_tap(c, tap, out, elems, out_act, st)) != BT_OK) return r;
   }
-  launch_head(residual_stream(c, layers.size()), c->hp.transformer_dim, c->head_w->f32.get(), c->head_b->f32.get(), wv.chunks_dev, nb, L, beat, down,
+  launch_head(X, c->hp.transformer_dim, c->head_w->f32.get(), c->head_b->f32.get(), wv.chunks_dev, nb, L, beat, down,
               c->hp.sum_head ? 1 : 0, st);
   BT_LAUNCHED(c, "head", st);
   return BT_OK;
@@ -1438,12 +1391,11 @@ int bt_debug_gemm(bt_ctx* c, const bt_debug_gemm_desc* d, const float* a_dev, co
   launch_f32_to_h16(w_dev, wb.get(), w_n, st);
   if (out_act_dev) launch_f32_to_h16(out_act_dev, ob.get(), out_act_count, st);
   e.out_act = ob.get();
-  const GemmDst dst = e.kind == 2 ? GemmDst{} : GemmDst{e.resid, e.ldr, e.out_f32, e.ldo_f32, e.out_act, e.ldo_act};
   char err[512] = "";
-  const GemmPlan p(tc_gemm_plan_create(ab.get(), wb.get(), g, d->planes_in, d->resid_epilogue != 0, dst, err, sizeof(err)));
+  const GemmPlan p(tc_gemm_plan_create(ab.get(), wb.get(), g, d->planes_in, d->resid_epilogue != 0, e, err, sizeof(err)));
   int rc = BT_OK;
   if (!p) rc = fail(c, BT_ERR_CUDA, "%s", err);
-  else if (launch_gemm_tc(p.get(), e, st) != 0) rc = fail(c, BT_ERR_CUDA, "tc gemm launch failed");
+  else if (launch_gemm_tc(p.get(), st) != 0) rc = fail(c, BT_ERR_CUDA, "tc gemm launch failed");
   else if (out_act_dev) launch_h16_to_f32(ob.get(), out_act_dev, out_act_count, st);
   if (p && tile_out) tc_gemm_plan_tile(p.get(), &tile_out[0], &tile_out[1]);
   const cudaError_t se = cudaStreamSynchronize(st);

@@ -171,25 +171,15 @@ void launch_pack_qkv_test(const float* q, const float* k, const float* v, void* 
                           int heads, float qscale, int act_h16, cudaStream_t st);
 
 // ---- 16-bit (fp16 or bf16 operands) tensor-core path (wgmma GEMM, mma.sync attention) ---------------------------------
-struct TcGemmPlan;  // cached tensor maps + launch geometry
-// Where the epilogue of kinds 0 and 1 reads the residual and writes its results ([planes_out * L] rows, leading
-// dimensions in elements, null = absent; EpiParams fields of the same names).  The plan encodes tensor maps of them,
-// and every launch of the plan must pass the same buffers.  The gates GEMM (kind 2) takes none.
-struct GemmDst {
-  const float* resid;
-  int ldr;
-  float* out_f32;
-  int ldo_f32;
-  void* out_act;
-  int ldo_act;
-};
-// resid_epilogue: the launches of this plan add the fp32 residual in the epilogue (tile width policy, kernels_gemm.cu)
+struct TcGemmPlan;  // one launch: its epilogue, tensor maps and launch geometry
+// The plan keeps e.  Kinds 0 and 1 read the residual and write their results ([planes_out * L] rows) through tensor
+// maps of e.resid / e.out_f32 / e.out_act that the plan encodes; the gates GEMM (kind 2) stores from registers.
+// resid_epilogue: the tile width policy of a GEMM that adds the fp32 residual (kernels_gemm.cu).
 TcGemmPlan* tc_gemm_plan_create(const void* A_h16, const void* W_h16, const GemmShape& g, int planes_in,
-                                bool resid_epilogue, const GemmDst& dst, char* err, int errlen);
+                                bool resid_epilogue, const EpiParams& e, char* err, int errlen);
 void tc_gemm_plan_destroy(TcGemmPlan*);
 void tc_gemm_plan_tile(const TcGemmPlan*, int* bn, int* bk);  // the (BN, BK) tile the plan launches
-// 0, -2 for a tile without a kernel, -3 when e names other epilogue buffers than the plan's GemmDst
-int launch_gemm_tc(const TcGemmPlan* plan, const EpiParams& e, cudaStream_t st);
+int launch_gemm_tc(const TcGemmPlan* plan, cudaStream_t st);  // 0, or -2 for a tile without a kernel
 
 struct TcAttnPlan;
 TcAttnPlan* tc_attn_plan_create(const void* qkv_h16, int seqs, int L, int heads, char* err, int errlen);
@@ -209,15 +199,15 @@ struct TcFfPlan;
 TcFfPlan* tc_ff_plan_create(const void* w1_h16, const void* w2_h16, int C, int64_t M, const void* o_h16,
                             const void* wout_h16, char* err, int errlen);
 void tc_ff_plan_destroy(TcFfPlan*);
-int launch_fused_ff(const TcFfPlan* plan, float* X, const float* b1, const float* b2, void* xb_out, cudaStream_t st);
+void launch_fused_ff(const TcFfPlan* plan, float* X, const float* b1, const float* b2, void* xb_out, cudaStream_t st);
 
 // fused RMSNorm + gates + QKV projection + RoPE for C in {32, 64} (frontend attentions)
 struct TcQkvPlan;
 TcQkvPlan* tc_qkv_plan_create(const void* wqkv_h16, int C, int64_t M, char* err, int errlen);
 void tc_qkv_plan_destroy(TcQkvPlan*);
-int launch_fused_qkv(const TcQkvPlan* plan, const float* X, const float* wg, const float* bg, const float* rope_cos,
-                     const float* rope_sin, void* qkv, float* gates, int L, int F, int posmode, float qscale,
-                     cudaStream_t st);
+void launch_fused_qkv(const TcQkvPlan* plan, const float* X, const float* wg, const float* bg, const float* rope_cos,
+                      const float* rope_sin, void* qkv, float* gates, int L, int F, int posmode, float qscale,
+                      cudaStream_t st);
 
 int tc_init(char* err, int errlen);  // resolves cuTensorMapEncodeTiled, sets smem attributes
 

@@ -285,7 +285,7 @@ static unsigned fused_grid(int64_t M, int ctas_per_sm) {
   return static_cast<unsigned>(ctas < slots ? ctas : slots);
 }
 
-int launch_fused_ff(const TcFfPlan* p, float* X, const float* b1, const float* b2, void* xb_out, cudaStream_t st) {
+void launch_fused_ff(const TcFfPlan* p, float* X, const float* b1, const float* b2, void* xb_out, cudaStream_t st) {
   const h16* w1 = static_cast<const h16*>(p->w1);
   const h16* w2 = static_cast<const h16*>(p->w2);
   const h16* wo = static_cast<const h16*>(p->wo);
@@ -297,7 +297,6 @@ int launch_fused_ff(const TcFfPlan* p, float* X, const float* b1, const float* b
   if (p->C == 32) { if (p->outproj) BT_FF_L(32, true); else BT_FF_L(32, false); }
   else { if (p->outproj) BT_FF_L(64, true); else BT_FF_L(64, false); }
 #undef BT_FF_L
-  return 0;
 }
 
 struct TcQkvPlan {
@@ -312,9 +311,9 @@ TcQkvPlan* tc_qkv_plan_create(const void* wqkv_h16, int C, int64_t M, char* err,
   return p;
 }
 void tc_qkv_plan_destroy(TcQkvPlan* p) { delete p; }
-int launch_fused_qkv(const TcQkvPlan* p, const float* X, const float* wg, const float* bg, const float* rope_cos,
-                     const float* rope_sin, void* qkv, float* gates, int L, int F, int posmode, float qscale,
-                     cudaStream_t st) {
+void launch_fused_qkv(const TcQkvPlan* p, const float* X, const float* wg, const float* bg, const float* rope_cos,
+                      const float* rope_sin, void* qkv, float* gates, int L, int F, int posmode, float qscale,
+                      cudaStream_t st) {
   const h16* w = static_cast<const h16*>(p->w);
   h16* out = static_cast<h16*>(qkv);
   if (p->C == 32)
@@ -323,7 +322,6 @@ int launch_fused_qkv(const TcQkvPlan* p, const float* X, const float* wg, const 
   else
     fused_qkv_kernel<64><<<fused_grid(p->M, qkv_ctas<64>()), FU_THREADS, qkv_smem<64>(), st>>>(w, X, wg, bg, rope_cos, rope_sin, out,
                                                                                              gates, p->M, L, F, posmode, qscale);
-  return 0;
 }
 
 int tc_init_fused(char* err, int errlen) {

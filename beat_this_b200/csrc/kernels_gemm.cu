@@ -315,9 +315,10 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 
 struct TcGemmPlan {
   CUtensorMap tmA, tmW;
-  CUtensorMap tmR, tmF, tmH;  // [planes_out, L, N] views of dst.resid, dst.out_f32, dst.out_act (when present)
-  GemmDst dst;
+  CUtensorMap tmR, tmF, tmH;  // [planes_out, L, N] views of e.resid, e.out_f32, e.out_act (kinds 0 and 1, when present)
+  EpiParams e;
   GemmShape g;
+  int kind;  // kernel instantiation: 0 generic, 1 qkv, 2 gates
   int BN, BK;
   int num_tiles, t_tiles, n_tiles, m_tiles, grid;
 };
@@ -350,10 +351,11 @@ static bool make_epi_tmap(CUtensorMap* tm, const void* base, int ld, int es, uin
 }
 
 TcGemmPlan* tc_gemm_plan_create(const void* A, const void* W, const GemmShape& g, int planes_in, bool resid_epilogue,
-                                const GemmDst& dst, char* err, int errlen) {
+                                const EpiParams& e, char* err, int errlen) {
   TcGemmPlan* p = new TcGemmPlan();
   p->g = g;
-  p->dst = dst;
+  p->e = e;
+  p->kind = e.kind == 1 || e.kind == 2 ? e.kind : 0;
   p->BK = (g.Kslab % 64 == 0) ? 64 : 32;
   p->BN = pick_bn(g.N, p->BK == 32 || resid_epilogue ? 128 : 256);
   if (p->BN == 0 || g.Kslab % 32 != 0) {
@@ -361,7 +363,12 @@ TcGemmPlan* tc_gemm_plan_create(const void* A, const void* W, const GemmShape& g
     delete p;
     return nullptr;
   }
-  if (dst.resid && (p->BN > 128 || !dst.out_f32)) {
+  if (p->kind == 1 && (e.resid || e.out_f32)) {
+    snprintf(err, errlen, "tc gemm: the qkv epilogue (kind 1) writes its 16-bit output only: no residual, no fp32 output");
+    delete p;
+    return nullptr;
+  }
+  if (p->kind != 2 && e.resid && (p->BN > 128 || !e.out_f32)) {
     snprintf(err, errlen, "tc gemm: a residual epilogue needs BN <= 128 (plan it with resid_epilogue) and an fp32 output");
     delete p;
     return nullptr;
@@ -382,9 +389,10 @@ TcGemmPlan* tc_gemm_plan_create(const void* A, const void* W, const GemmShape& g
     if (!make_tmap(&p->tmW, W, 2, dims, strides, box, swz, err, errlen)) { delete p; return nullptr; }
   }
   const uint32_t act_cols = p->BN < 64 ? p->BN : 64;
-  if ((dst.resid && !make_epi_tmap(&p->tmR, dst.resid, dst.ldr, 4, 32, TG_BM, g, "residual", err, errlen)) ||
-      (dst.out_f32 && !make_epi_tmap(&p->tmF, dst.out_f32, dst.ldo_f32, 4, 32, 64, g, "fp32 output", err, errlen)) ||
-      (dst.out_act && !make_epi_tmap(&p->tmH, dst.out_act, dst.ldo_act, 2, act_cols, 64, g, "16-bit output", err, errlen))) {
+  if (p->kind != 2 &&  // the gates GEMM stores from registers
+      ((e.resid && !make_epi_tmap(&p->tmR, e.resid, e.ldr, 4, 32, TG_BM, g, "residual", err, errlen)) ||
+       (e.out_f32 && !make_epi_tmap(&p->tmF, e.out_f32, e.ldo_f32, 4, 32, 64, g, "fp32 output", err, errlen)) ||
+       (e.out_act && !make_epi_tmap(&p->tmH, e.out_act, e.ldo_act, 2, act_cols, 64, g, "16-bit output", err, errlen)))) {
     delete p;
     return nullptr;
   }
@@ -405,18 +413,11 @@ void tc_gemm_plan_tile(const TcGemmPlan* p, int* bn, int* bk) { *bn = p->BN; *bk
   X(32, 64, 0) X(32, 64, 1) X(128, 32, 0) X(128, 32, 1) X(64, 32, 0) X(64, 32, 1) X(32, 32, 0) X(32, 32, 1)             \
   X(32, 64, 2) X(32, 32, 2)
 
-int launch_gemm_tc(const TcGemmPlan* p, const EpiParams& e, cudaStream_t st) {
-  const int kind = e.kind == 1 || e.kind == 2 ? e.kind : 0;
-  // the staged epilogues read and write through the plan's tensor maps: the launch must name the same buffers
-  const GemmDst& d = p->dst;
-  if (kind != 2 && (e.resid != d.resid || e.out_f32 != d.out_f32 || e.out_act != d.out_act || (e.resid && e.ldr != d.ldr) ||
-                    (e.out_f32 && e.ldo_f32 != d.ldo_f32) || (e.out_act && e.ldo_act != d.ldo_act)))
-    return -3;
-  if (kind == 1 && (e.resid || e.out_f32)) return -3;
+int launch_gemm_tc(const TcGemmPlan* p, cudaStream_t st) {
 #define BT_TG_LAUNCH(bn, bk, kd)                                                                                       \
-  if (p->BN == bn && p->BK == bk && kind == kd) {                                                                      \
+  if (p->BN == bn && p->BK == bk && p->kind == kd) {                                                                   \
     gemm_tc_kernel<bn, bk, kd><<<p->grid, TG_THREADS, TgCfg<bn, bk>::SMEM, st>>>(                                     \
-        p->tmA, p->tmW, p->tmR, p->tmF, p->tmH, p->g, e, p->num_tiles, p->t_tiles, p->n_tiles, p->m_tiles);           \
+        p->tmA, p->tmW, p->tmR, p->tmF, p->tmH, p->g, p->e, p->num_tiles, p->t_tiles, p->n_tiles, p->m_tiles);        \
     return 0;                                                                                                          \
   }
   BT_GEMM_TC_INSTANCES(BT_TG_LAUNCH)
