@@ -168,6 +168,19 @@ PROTOTYPES = {
     "bt_debug_attention_freq": (
         c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p],
     ),
+    "bt_debug_norm": (
+        c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_void_p, c_int32, c_void_p],
+    ),
+    "bt_debug_fused_qkv": (
+        c_int,
+        [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int32,
+         c_int32, c_int32, c_int32, c_float, c_void_p],
+    ),
+    "bt_debug_fused_ff": (
+        c_int,
+        [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int32,
+         c_void_p],
+    ),
 }
 
 _lib = None

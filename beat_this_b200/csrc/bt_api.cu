@@ -643,12 +643,22 @@ std::vector<ParamSpec> layer_params(const Layer& l, int64_t D) {
   }
 }
 
+bool aligned16(const void* p) { return reinterpret_cast<uintptr_t>(p) % 16 == 0; }
+
+// A test hook's 16-bit operand: the fp32 device array src of n elements rounded into buf on st (nothing for null src).
+cudaError_t to_h16_operand(DeviceBuffer<>& buf, const float* src, int64_t n, cudaStream_t st) {
+  if (!src) return cudaSuccess;
+  const cudaError_t e = buf.alloc(n * 2);
+  if (e == cudaSuccess) launch_f32_to_h16(src, buf.get(), n, st);
+  return e;
+}
+
 }  // namespace
 
 // ================================================================================== C ABI
 extern "C" {
 
-int bt_version(void) { return 203; }
+int bt_version(void) { return 204; }
 
 const char* bt_act_dtype(void) {
 #if defined(BT_ACT_BF16)
@@ -1490,6 +1500,91 @@ int bt_debug_attention_freq(bt_ctx* c, const float* q_dev, const float* k_dev, c
   cudaError_t se = cudaStreamSynchronize(st);
   if (se != cudaSuccess) rc = fail(c, BT_ERR_CUDA, "frequency attention: %s", cudaGetErrorString(se));
   c->launches += 2;
+  return rc;
+}
+
+int bt_debug_norm(bt_ctx* c, const float* x_dev, float* xn_dev, int64_t M, int32_t C, const float* wg_dev,
+                  const float* bg_dev, float* gates_dev, int32_t heads, void* stream) {
+  if (!c) return BT_ERR_ARG;
+  const char* fn = "bt_debug_norm";
+  const bool tc = c->dtype == BT_DTYPE_H16;
+  if (!x_dev || !xn_dev || !aligned16(x_dev) || (!tc && !aligned16(xn_dev)))  // the fp32 context stores xn directly
+    return fail(c, BT_ERR_ARG, "%s: need x and xn (16-byte aligned; xn only in the fp32 context)", fn);
+  if (M < 1 || (C != 32 && C != 64 && C != 128 && C != 256 && C != 512 && C != 1024))
+    return fail(c, BT_ERR_ARG, "%s: need M >= 1 and C in {32, 64, 128, 256, 512, 1024}", fn);
+  if (gates_dev ? (!wg_dev || !bg_dev || !aligned16(wg_dev) || heads < 1 || 32 * heads > C) : heads != 0)
+    return fail(c, BT_ERR_ARG, "%s: gates need wg (16-byte aligned), bg and 1 <= heads <= C / 32; no gates, heads 0", fn);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  BT_CUDA(c, cudaSetDevice(c->device));
+  const int64_t n = M * C;
+  DeviceBuffer<> xb;
+  if (tc) BT_CUDA(c, to_h16_operand(xb, xn_dev, n, st));  // elements the kernel does not store survive the round trip
+  launch_norm(x_dev, tc ? xb.get() : static_cast<void*>(xn_dev), M, C, tc ? 1 : 0, st, gates_dev, wg_dev, bg_dev, heads);
+  int rc = check_launch(c, "debug_norm", st);
+  if (rc == BT_OK && tc) launch_h16_to_f32(xb.get(), xn_dev, n, st);
+  const cudaError_t se = cudaStreamSynchronize(st);
+  if (rc == BT_OK && se != cudaSuccess) rc = fail(c, BT_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(se));
+  return rc;
+}
+
+int bt_debug_fused_qkv(bt_ctx* c, const float* x_dev, const float* wqkv_dev, const float* wg_dev, const float* bg_dev,
+                       const float* rope_cos_dev, const float* rope_sin_dev, float* qkv_dev, float* gates_dev, int64_t M,
+                       int32_t C, int32_t L, int32_t F, int32_t posmode, float qscale, void* stream) {
+  if (!c) return BT_ERR_ARG;
+  const char* fn = "bt_debug_fused_qkv";
+  if (c->dtype != BT_DTYPE_H16) return fail(c, BT_ERR_ARG, "%s: the fused kernel runs in the 16-bit context only", fn);
+  if (!x_dev || !wqkv_dev || !wg_dev || !bg_dev || !rope_cos_dev || !rope_sin_dev || !qkv_dev || !gates_dev ||
+      !aligned16(x_dev) || !aligned16(wg_dev))
+    return fail(c, BT_ERR_ARG, "%s: null argument, or x / wg not 16-byte aligned", fn);
+  if (M < 1 || (C != 32 && C != 64) || L < 1 || L > BT_CHUNK || (posmode != 0 && posmode != 1) ||
+      (posmode == 1 && (F < 1 || F > BT_CHUNK)))
+    return fail(c, BT_ERR_ARG, "%s: need M >= 1, C in {32, 64}, 1 <= L <= %d, posmode 0 or 1 (1: 1 <= F <= %d)", fn,
+                BT_CHUNK, BT_CHUNK);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  BT_CUDA(c, cudaSetDevice(c->device));
+  const int64_t n = M * 3 * C;
+  DeviceBuffer<> wb, ob;
+  BT_CUDA(c, to_h16_operand(wb, wqkv_dev, 3 * C * C, st));
+  BT_CUDA(c, to_h16_operand(ob, qkv_dev, n, st));
+  char err[512] = "";
+  const QkvPlan p(tc_qkv_plan_create(wb.get(), C, M, err, sizeof(err)));
+  if (!p) return fail(c, BT_ERR_CUDA, "%s: %s", fn, err);
+  launch_fused_qkv(p.get(), x_dev, wg_dev, bg_dev, rope_cos_dev, rope_sin_dev, ob.get(), gates_dev, L, F, posmode, qscale,
+                   st);
+  int rc = check_launch(c, "debug_fused_qkv", st);
+  if (rc == BT_OK) launch_h16_to_f32(ob.get(), qkv_dev, n, st);
+  const cudaError_t se = cudaStreamSynchronize(st);
+  if (rc == BT_OK && se != cudaSuccess) rc = fail(c, BT_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(se));
+  return rc;
+}
+
+int bt_debug_fused_ff(bt_ctx* c, float* x_dev, const float* w1_dev, const float* b1_dev, const float* w2_dev,
+                      const float* b2_dev, const float* o_dev, const float* wout_dev, float* xb_dev, int64_t M, int32_t C,
+                      void* stream) {
+  if (!c) return BT_ERR_ARG;
+  const char* fn = "bt_debug_fused_ff";
+  if (c->dtype != BT_DTYPE_H16) return fail(c, BT_ERR_ARG, "%s: the fused kernel runs in the 16-bit context only", fn);
+  if (!x_dev || !w1_dev || !b1_dev || !w2_dev || !b2_dev || !aligned16(x_dev) || !aligned16(b1_dev) ||
+      !aligned16(b2_dev) || !o_dev != !wout_dev)
+    return fail(c, BT_ERR_ARG, "%s: null argument, x / b1 / b2 not 16-byte aligned, or only one of o and wout", fn);
+  if (M < 1 || (C != 32 && C != 64)) return fail(c, BT_ERR_ARG, "%s: need M >= 1 and C in {32, 64}", fn);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  BT_CUDA(c, cudaSetDevice(c->device));
+  const int64_t n = M * C;
+  DeviceBuffer<> w1b, w2b, ob, woutb, xbb;
+  BT_CUDA(c, to_h16_operand(w1b, w1_dev, 4 * C * C, st));
+  BT_CUDA(c, to_h16_operand(w2b, w2_dev, 4 * C * C, st));
+  BT_CUDA(c, to_h16_operand(ob, o_dev, n, st));
+  BT_CUDA(c, to_h16_operand(woutb, wout_dev, C * C, st));
+  BT_CUDA(c, to_h16_operand(xbb, xb_dev, n, st));
+  char err[512] = "";
+  const FfPlan p(tc_ff_plan_create(w1b.get(), w2b.get(), C, M, ob.get(), woutb.get(), err, sizeof(err)));
+  if (!p) return fail(c, BT_ERR_CUDA, "%s: %s", fn, err);
+  launch_fused_ff(p.get(), x_dev, b1_dev, b2_dev, xbb.get(), st);
+  int rc = check_launch(c, "debug_fused_ff", st);
+  if (rc == BT_OK && xb_dev) launch_h16_to_f32(xbb.get(), xb_dev, n, st);
+  const cudaError_t se = cudaStreamSynchronize(st);
+  if (rc == BT_OK && se != cudaSuccess) rc = fail(c, BT_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(se));
   return rc;
 }
 

@@ -430,3 +430,36 @@ class Engine:
                                                 self._stream())
         _lib.check(self.lib, self.ctx, code)
         return o
+
+    # The row-kernel hooks take fp32 device tensors and write their outputs in place, so a caller can surround the
+    # M rows with sentinel values.  x and every output may have more than M rows; only the first M are the problem.
+    # The C hooks cannot see buffer sizes, so each tensor is checked here to hold at least the elements they touch.
+    def _dev_ptr(self, t, n: int = 0):
+        if t is None:
+            return None
+        assert t.is_cuda and t.dtype == torch.float32 and t.is_contiguous()
+        assert t.numel() >= n, f"tensor of {t.numel()} elements, the hook reads or writes {n}"
+        return c_void_p(t.data_ptr())
+
+    def debug_norm(self, x, xn_out, M: int, C: int, wg=None, bg=None, gates_out=None, heads: int = 0):
+        """bt_debug_norm: xn_out[:M] = rmsnorm(x[:M]) through norm_kernel (+ gates_out[:M] with heads > 0)."""
+        p, n = self._dev_ptr, max(M, 0)
+        code = self.lib.bt_debug_norm(self.ctx, p(x, n * C), p(xn_out, n * C), M, C, p(wg, heads * C), p(bg, heads),
+                                      p(gates_out, n * heads), heads, self._stream())
+        _lib.check(self.lib, self.ctx, code)
+
+    def debug_fused_qkv(self, x, wqkv, wg, bg, rope_cos, rope_sin, qkv_out, gates_out, M: int, C: int, L: int, F: int,
+                        posmode: int, qscale: float):
+        """bt_debug_fused_qkv: qkv_out[:M] (3C columns) and gates_out[:M] from x[:M] through fused_qkv_kernel<C>."""
+        p, n, heads, rows = self._dev_ptr, max(M, 0), C // 32, 1500  # RoPE tables: [BT_CHUNK, 16]
+        code = self.lib.bt_debug_fused_qkv(self.ctx, p(x, n * C), p(wqkv, 3 * C * C), p(wg, heads * C), p(bg, heads),
+                                           p(rope_cos, rows * 16), p(rope_sin, rows * 16), p(qkv_out, n * 3 * C),
+                                           p(gates_out, n * heads), M, C, L, F, posmode, float(qscale), self._stream())
+        _lib.check(self.lib, self.ctx, code)
+
+    def debug_fused_ff(self, x, w1, b1, w2, b2, M: int, C: int, o=None, wout=None, xb_out=None):
+        """bt_debug_fused_ff: x[:M] updated in place through fused_ff_kernel<C, o is not None> (+ xb_out[:M])."""
+        p, n = self._dev_ptr, max(M, 0)
+        code = self.lib.bt_debug_fused_ff(self.ctx, p(x, n * C), p(w1, 4 * C * C), p(b1, 4 * C), p(w2, 4 * C * C),
+                                          p(b2, C), p(o, n * C), p(wout, C * C), p(xb_out, n * C), M, C, self._stream())
+        _lib.check(self.lib, self.ctx, code)

@@ -392,6 +392,34 @@ int bt_debug_attention_freq(bt_ctx* ctx, const float* q_dev, const float* k_dev,
                             const float* gates_dev, float* o_dev, int32_t B, int32_t F, int32_t L, int32_t heads,
                             void* stream);
 
+/* Test hooks of the frontend's row kernels.  Every *_dev pointer is fp32 on the device; x, wg, b1 and b2 must be
+ * 16-byte aligned, and so must xn of bt_debug_norm in the fp32 context (the kernel stores it directly).  The 16-bit context rounds the 16-bit operands (wqkv, w1, w2, o, wout) to its activation type
+ * around the launch, and runs each 16-bit output (the whole [M, ...] buffer, so values the kernel does not store
+ * survive) through that type.  Each returns BT_ERR_ARG, before anything is enqueued, for a bad geometry or pointer,
+ * and synchronises the stream. */
+
+/* RMSNorm xn = x / max(||x||, 1e-12) of M rows of C in {32, 64, 128, 256, 512, 1024} through norm_kernel, in the
+ * ctx's activation type.  With gates_dev (then wg_dev [heads, C], bg_dev [heads], 1 <= heads <= C / 32) also
+ * gates [M, heads] = sigmoid(xn . wg[h] + bg[h]); without, heads is 0. */
+int bt_debug_norm(bt_ctx* ctx, const float* x_dev, float* xn_dev, int64_t M, int32_t C, const float* wg_dev,
+                  const float* bg_dev, float* gates_dev, int32_t heads, void* stream);
+
+/* The fused RMSNorm + gates + QKV + RoPE kernel of the frontend attentions (16-bit context only, C in {32, 64}):
+ * x [M, C] -> qkv [M, 3C] = rmsnorm(x) wqkv^T with RoPE on the q and k columns at position m % L (posmode 0) or
+ * (m / L) % F (posmode 1), q also scaled by qscale; gates [M, C / 32] as bt_debug_norm gives them.  wqkv [3C, C];
+ * wg [C / 32, C] or the padded [32, C]; bg likewise; rope tables [BT_CHUNK, 16]. */
+int bt_debug_fused_qkv(bt_ctx* ctx, const float* x_dev, const float* wqkv_dev, const float* wg_dev, const float* bg_dev,
+                       const float* rope_cos_dev, const float* rope_sin_dev, float* qkv_dev, float* gates_dev, int64_t M,
+                       int32_t C, int32_t L, int32_t F, int32_t posmode, float qscale, void* stream);
+
+/* The fused FFN of the frontend blocks (16-bit context only, C in {32, 64}), in place on x [M, C]:
+ * x' = x (+ o wout^T when o_dev and wout_dev are both set: the attention out-projection in front), then
+ * x = x' + w2 gelu(w1 rmsnorm(x') + b1) + b2.  w1 [4C, C], b1 [4C], w2 [C, 4C], b2 [C], o [M, C], wout [C, C].
+ * xb_dev (optional, [M, C]) receives the 16-bit copy of the result. */
+int bt_debug_fused_ff(bt_ctx* ctx, float* x_dev, const float* w1_dev, const float* b1_dev, const float* w2_dev,
+                      const float* b2_dev, const float* o_dev, const float* wout_dev, float* xb_dev, int64_t M, int32_t C,
+                      void* stream);
+
 #ifdef __cplusplus
 }
 #endif
