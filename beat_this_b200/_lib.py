@@ -79,6 +79,20 @@ class bt_beat_metric_params(ctypes.Structure):
     ]
 
 
+BT_CHUNK = 1500
+BT_KEEP_FIRST = 0
+BT_KEEP_LAST = 1
+OVERLAP_MODES = {"keep_first": BT_KEEP_FIRST, "keep_last": BT_KEEP_LAST}
+
+
+class bt_chunking(ctypes.Structure):
+    _fields_ = [
+        ("chunk_size", c_int32),
+        ("border", c_int32),
+        ("overlap_mode", c_int32),
+    ]
+
+
 class bt_loss_params(ctypes.Structure):
     _fields_ = [
         ("kind", c_int32),
@@ -98,6 +112,9 @@ PROTOTYPES = {
     "bt_last_error": (c_char_p, [c_void_p]),
     "bt_num_frames": (c_int64, [c_int64]),
     "bt_plan_chunks": (c_int64, [c_int64, POINTER(c_int64), POINTER(c_int64), c_int64]),
+    "bt_plan_chunking": (
+        c_int64, [c_int64, POINTER(bt_chunking), POINTER(c_int64), POINTER(c_int64), POINTER(c_int64), POINTER(c_int64), c_int64],
+    ),
     "bt_logmel": (c_int, [c_void_p, c_void_p, POINTER(c_int64), c_int32, c_void_p, POINTER(c_int64), c_void_p]),
     "bt_stage_audio": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_int32]),
     "bt_wav_probe": (c_int, [c_char_p, POINTER(bt_wav_info)]),
@@ -141,6 +158,13 @@ PROTOTYPES = {
     "bt_audio2frames": (
         c_int,
         [c_void_p, c_void_p, POINTER(c_int64), c_int32, c_void_p, c_void_p, POINTER(c_int64), c_void_p],
+    ),
+    "bt_spect2frames_chunked": (
+        c_int, [c_void_p, c_void_p, POINTER(c_int64), c_int32, c_void_p, c_void_p, POINTER(bt_chunking), c_void_p],
+    ),
+    "bt_audio2frames_chunked": (
+        c_int,
+        [c_void_p, c_void_p, POINTER(c_int64), c_int32, c_void_p, c_void_p, POINTER(c_int64), POINTER(bt_chunking), c_void_p],
     ),
     "bt_peakpick": (
         c_int,

@@ -194,25 +194,43 @@ const Param* find_param(const bt_ctx* c, const std::string& name) {
   return it == c->params.end() ? nullptr : &it->second;
 }
 
-int64_t chunks_for(int64_t T, int64_t* starts, int64_t* lens, int64_t cap) {
-  // split_piece (reference inference.py:119-125): starts = arange(-6, T-6, 1488); if T > 1488
-  // the last start is moved to T - 1494; chunk = frames [start, start+1500) clipped to the
-  // piece, zero padded by max(0,-start) on the left and max(0, min(6, start+1500-T)) on the right.
+constexpr bt_chunking kDefaultChunking{BT_CHUNK, BT_BORDER, BT_KEEP_FIRST};
+
+bool chunking_valid(const bt_chunking* ck) {
+  return ck && ck->chunk_size >= 1 && ck->chunk_size <= BT_CHUNK && ck->border >= 0 &&
+         2 * static_cast<int64_t>(ck->border) < ck->chunk_size &&
+         (ck->overlap_mode == BT_KEEP_FIRST || ck->overlap_mode == BT_KEEP_LAST);
+}
+
+// The chunk plan of bt_plan_chunking (contract and coverage argument in include/beatthis.h) for a valid chunking:
+// split_piece (reference inference.py:119-125) for the starts and lengths, aggregate_prediction (:174-184) for the
+// owned piece frames [own_lo, own_hi).  Chunks are visited in order, so keep_first cuts a chunk's range where the
+// previous one's ends and keep_last where the next one's begins.
+int64_t plan_chunks(int64_t T, const bt_chunking& ck, int64_t* starts, int64_t* lens, int64_t* own_lo, int64_t* own_hi,
+                    int64_t cap) {
   if (T <= 0) return 0;
-  const int64_t step = BT_CHUNK - 2 * BT_BORDER;
-  int64_t n = 0;
-  for (int64_t s = -BT_BORDER; s < T - BT_BORDER; s += step) ++n;
-  int64_t i = 0;
-  for (int64_t s = -BT_BORDER; s < T - BT_BORDER; s += step, ++i) {
-    int64_t st = s;
-    if (i == n - 1 && T > step) st = T - (BT_CHUNK - BT_BORDER);
-    const int64_t lo = std::max<int64_t>(st, 0), hi = std::min<int64_t>(st + BT_CHUNK, T);
-    const int64_t left = std::max<int64_t>(0, -st);
-    const int64_t right = std::max<int64_t>(0, std::min<int64_t>(BT_BORDER, st + BT_CHUNK - T));
-    if (i < cap) {
-      if (starts) starts[i] = st;
-      if (lens) lens[i] = (hi - lo) + left + right;
+  const int64_t c = ck.chunk_size, b = ck.border, step = c - 2 * b;
+  const int64_t n = (T + step - 1) / step;  // the length of arange(-b, T - b, step)
+  auto start = [&](int64_t i) { return i == n - 1 && T > step ? T - (c - b) : i * step - b; };
+  auto len = [&](int64_t s) {
+    const int64_t lo = std::max<int64_t>(s, 0), hi = std::min<int64_t>(s + c, T);
+    const int64_t left = std::max<int64_t>(0, -s);
+    const int64_t right = std::max<int64_t>(0, std::min<int64_t>(b, s + c - T));
+    return (hi - lo) + left + right;
+  };
+  for (int64_t i = 0; i < std::min(n, cap); ++i) {
+    const int64_t s = start(i), l = len(s);
+    int64_t lo = s + b, hi = s + l - b;
+    if (ck.overlap_mode == BT_KEEP_FIRST && i > 0) {
+      const int64_t sp = start(i - 1);
+      lo = std::max(lo, sp + len(sp) - b);
+    } else if (ck.overlap_mode == BT_KEEP_LAST && i < n - 1) {
+      hi = std::min(hi, start(i + 1) + b);
     }
+    if (starts) starts[i] = s;
+    if (lens) lens[i] = l;
+    if (own_lo) own_lo[i] = lo;
+    if (own_hi) own_hi[i] = std::max(lo, hi);
   }
   return n;
 }
@@ -658,7 +676,7 @@ cudaError_t to_h16_operand(DeviceBuffer<>& buf, const float* src, int64_t n, cud
 // ================================================================================== C ABI
 extern "C" {
 
-int bt_version(void) { return 204; }
+int bt_version(void) { return 205; }
 
 const char* bt_act_dtype(void) {
 #if defined(BT_ACT_BF16)
@@ -673,7 +691,13 @@ const char* bt_last_error(const bt_ctx* ctx) { return ctx ? ctx->err : g_create_
 int64_t bt_num_frames(int64_t n_samples) { return n_samples < 0 ? 0 : 1 + n_samples / BT_HOP; }
 
 int64_t bt_plan_chunks(int64_t T, int64_t* starts, int64_t* lens, int64_t cap) {
-  return chunks_for(T, starts, lens, cap);
+  return plan_chunks(T, kDefaultChunking, starts, lens, nullptr, nullptr, cap);
+}
+
+int64_t bt_plan_chunking(int64_t T, const bt_chunking* ck, int64_t* starts, int64_t* lens, int64_t* own_lo,
+                         int64_t* own_hi, int64_t cap) {
+  if (!chunking_valid(ck)) return BT_ERR_ARG;
+  return plan_chunks(T, *ck, starts, lens, own_lo, own_hi, cap);
 }
 
 int bt_create(bt_ctx** out, int device_ordinal, const bt_hparams* hp, int compute_dtype) {
@@ -912,42 +936,54 @@ int bt_resample(bt_ctx* c, const float* audio_in_dev, const int64_t* in_offsets_
   return BT_OK;
 }
 
-int bt_spect2frames(bt_ctx* c, const float* spect_dev, const int64_t* frame_offsets_host, int32_t n_clips,
-                    float* beat_dev, float* downbeat_dev, void* stream) {
-  if (!c || !c->finalized) return fail(c, BT_ERR_STATE, "bt_spect2frames: context not finalized");
+// bt_spect2frames(_chunked) under a chunking already checked by chunking_valid; `fn` names the entry point in errors
+static int spect2frames(bt_ctx* c, const float* spect_dev, const int64_t* frame_offsets_host, int32_t n_clips,
+                        float* beat_dev, float* downbeat_dev, const bt_chunking& ck, void* stream, const char* fn) {
   if (n_clips <= 0) return BT_OK;
-  if (!spect_dev || !frame_offsets_host || !beat_dev || !downbeat_dev)
-    return fail(c, BT_ERR_ARG, "bt_spect2frames: null argument");
+  if (!spect_dev || !frame_offsets_host || !beat_dev || !downbeat_dev) return fail(c, BT_ERR_ARG, "%s: null argument", fn);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   BT_CUDA(c, cudaSetDevice(c->device));
   prof_mark(c, st);
-  // plan: all chunks of all clips, grouped by chunk length (1500 except for pieces <= 1488 frames)
+  // plan: all chunks of all clips; run_chunks groups them by chunk length
   std::vector<ChunkSrc> all;
-  std::vector<int64_t> starts, lens;
+  std::vector<int64_t> starts, lens, own_lo, own_hi;
   for (int i = 0; i < n_clips; ++i) {
     const int64_t T = frame_offsets_host[i + 1] - frame_offsets_host[i];
-    if (T < 0) return fail(c, BT_ERR_ARG, "bt_spect2frames: negative clip length");
+    if (T < 0) return fail(c, BT_ERR_ARG, "%s: negative clip length", fn);
     if (T == 0) continue;
-    const int64_t n = chunks_for(T, nullptr, nullptr, 0);
-    starts.resize(n); lens.resize(n);
-    chunks_for(T, starts.data(), lens.data(), n);
+    const int64_t n = plan_chunks(T, ck, nullptr, nullptr, nullptr, nullptr, 0);
+    starts.resize(n); lens.resize(n); own_lo.resize(n); own_hi.resize(n);
+    plan_chunks(T, ck, starts.data(), lens.data(), own_lo.data(), own_hi.data(), n);
     for (int64_t j = 0; j < n; ++j) {
       ChunkSrc s{};
       s.frame_base = frame_offsets_host[i];
       s.out_base = frame_offsets_host[i];
       s.T = static_cast<int32_t>(T);
       s.start = static_cast<int32_t>(starts[j]);
-      // keep_first (inference.py:174-184): chunk j owns [start+6, start+len-6) minus what earlier chunks own
-      int64_t lo = starts[j] + BT_BORDER;
-      if (j > 0) lo = std::max(lo, starts[j - 1] + lens[j - 1] - BT_BORDER);
-      const int64_t hi = starts[j] + lens[j] - BT_BORDER;
-      s.write_lo = static_cast<int32_t>(lo - starts[j]);
-      s.write_hi = static_cast<int32_t>(std::max(lo, hi) - starts[j]);
+      s.write_lo = static_cast<int32_t>(own_lo[j] - starts[j]);
+      s.write_hi = static_cast<int32_t>(own_hi[j] - starts[j]);
       s.len = static_cast<int32_t>(lens[j]);
       all.push_back(s);
     }
   }
   return run_chunks(c, spect_dev, all, beat_dev, downbeat_dev, st);
+}
+
+int bt_spect2frames(bt_ctx* c, const float* spect_dev, const int64_t* frame_offsets_host, int32_t n_clips,
+                    float* beat_dev, float* downbeat_dev, void* stream) {
+  if (!c || !c->finalized) return fail(c, BT_ERR_STATE, "bt_spect2frames: context not finalized");
+  return spect2frames(c, spect_dev, frame_offsets_host, n_clips, beat_dev, downbeat_dev, kDefaultChunking, stream,
+                      "bt_spect2frames");
+}
+
+int bt_spect2frames_chunked(bt_ctx* c, const float* spect_dev, const int64_t* frame_offsets_host, int32_t n_clips,
+                            float* beat_dev, float* downbeat_dev, const bt_chunking* ck, void* stream) {
+  if (!c || !c->finalized) return fail(c, BT_ERR_STATE, "bt_spect2frames_chunked: context not finalized");
+  if (!chunking_valid(ck))
+    return fail(c, BT_ERR_ARG, "bt_spect2frames_chunked: need 1 <= chunk_size <= %d, 0 <= 2 * border < chunk_size "
+                "and overlap_mode BT_KEEP_FIRST or BT_KEEP_LAST", BT_CHUNK);
+  return spect2frames(c, spect_dev, frame_offsets_host, n_clips, beat_dev, downbeat_dev, *ck, stream,
+                      "bt_spect2frames_chunked");
 }
 
 int bt_forward_chunks(bt_ctx* c, const float* chunks_dev, int32_t n_chunks, int32_t chunk_frames, float* beat_dev,
@@ -975,18 +1011,37 @@ int bt_forward_chunks(bt_ctx* c, const float* chunks_dev, int32_t n_chunks, int3
   return run_chunks(c, chunks_dev, all, beat_dev, downbeat_dev, st);
 }
 
-int bt_audio2frames(bt_ctx* c, const float* audio_dev, const int64_t* sample_offsets_host, int32_t n_clips,
-                    float* beat_dev, float* downbeat_dev, const int64_t* frame_offsets_host, void* stream) {
-  if (!c || !c->finalized) return fail(c, BT_ERR_STATE, "bt_audio2frames: context not finalized");
+// bt_audio2frames(_chunked) under a chunking already checked by chunking_valid
+static int audio2frames(bt_ctx* c, const float* audio_dev, const int64_t* sample_offsets_host, int32_t n_clips,
+                        float* beat_dev, float* downbeat_dev, const int64_t* frame_offsets_host, const bt_chunking& ck,
+                        void* stream, const char* fn) {
   if (n_clips <= 0) return BT_OK;
-  if (!frame_offsets_host) return fail(c, BT_ERR_ARG, "bt_audio2frames: null argument");
+  if (!frame_offsets_host) return fail(c, BT_ERR_ARG, "%s: null argument", fn);
   BT_CUDA(c, cudaSetDevice(c->device));
   const int64_t total = frame_offsets_host[n_clips];
   const size_t need = total * 128 * 4;
   BT_CUDA(c, c->spect_ws.reserve(need, need + need / 4));
   int r = bt_logmel(c, audio_dev, sample_offsets_host, n_clips, c->spect_ws.get(), frame_offsets_host, stream);
   if (r != BT_OK) return r;
-  return bt_spect2frames(c, c->spect_ws.get(), frame_offsets_host, n_clips, beat_dev, downbeat_dev, stream);
+  return spect2frames(c, c->spect_ws.get(), frame_offsets_host, n_clips, beat_dev, downbeat_dev, ck, stream, fn);
+}
+
+int bt_audio2frames(bt_ctx* c, const float* audio_dev, const int64_t* sample_offsets_host, int32_t n_clips,
+                    float* beat_dev, float* downbeat_dev, const int64_t* frame_offsets_host, void* stream) {
+  if (!c || !c->finalized) return fail(c, BT_ERR_STATE, "bt_audio2frames: context not finalized");
+  return audio2frames(c, audio_dev, sample_offsets_host, n_clips, beat_dev, downbeat_dev, frame_offsets_host,
+                      kDefaultChunking, stream, "bt_audio2frames");
+}
+
+int bt_audio2frames_chunked(bt_ctx* c, const float* audio_dev, const int64_t* sample_offsets_host, int32_t n_clips,
+                            float* beat_dev, float* downbeat_dev, const int64_t* frame_offsets_host,
+                            const bt_chunking* ck, void* stream) {
+  if (!c || !c->finalized) return fail(c, BT_ERR_STATE, "bt_audio2frames_chunked: context not finalized");
+  if (!chunking_valid(ck))
+    return fail(c, BT_ERR_ARG, "bt_audio2frames_chunked: need 1 <= chunk_size <= %d, 0 <= 2 * border < chunk_size "
+                "and overlap_mode BT_KEEP_FIRST or BT_KEEP_LAST", BT_CHUNK);
+  return audio2frames(c, audio_dev, sample_offsets_host, n_clips, beat_dev, downbeat_dev, frame_offsets_host, *ck,
+                      stream, "bt_audio2frames_chunked");
 }
 
 int bt_peakpick(bt_ctx* c, const float* beat_dev, const float* downbeat_dev, const int64_t* frame_offsets_host,

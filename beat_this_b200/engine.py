@@ -24,6 +24,21 @@ def _cuda_device(device) -> torch.device:
     return dev
 
 
+def chunking_struct(chunk_size: int, border_size: int, overlap_mode: str) -> _lib.bt_chunking:
+    """split_predict_aggregate's (chunk_size, border_size, overlap_mode) as the C library takes it (bt_plan_chunking,
+    include/beatthis.h).  ``ValueError`` for what the library refuses: chunk_size outside [1, 1500] (the RoPE tables
+    and workspace are sized for 1500 frames), a negative border, 2 * border_size >= chunk_size or an overlap_mode other
+    than "keep_first" / "keep_last"."""
+    if overlap_mode not in _lib.OVERLAP_MODES:
+        raise ValueError("overlap_mode must be 'keep_first' or 'keep_last'")
+    chunk_size, border_size = int(chunk_size), int(border_size)
+    if not 1 <= chunk_size <= _lib.BT_CHUNK:
+        raise ValueError(f"chunk_size must be in [1, {_lib.BT_CHUNK}], got {chunk_size}")
+    if border_size < 0 or 2 * border_size >= chunk_size:
+        raise ValueError(f"border_size must satisfy 0 <= 2 * border_size < chunk_size, got {border_size} for {chunk_size}")
+    return _lib.bt_chunking(chunk_size, border_size, _lib.OVERLAP_MODES[overlap_mode])
+
+
 class _PeakHandle:
     def __init__(self, slot, n):
         self.slot, self.n = slot, n
@@ -182,14 +197,21 @@ class Engine:
         spect, fo = self.logmel_cat(torch.cat(sigs) if len(sigs) > 1 else sigs[0], so)
         return [spect[fo[i] : fo[i + 1]] for i in range(len(sigs))]
 
-    def spect2frames_cat(self, spect: torch.Tensor, frame_offsets):
+    def spect2frames_cat(self, spect: torch.Tensor, frame_offsets, chunking: tuple | None = None):
+        """Concatenated [total, 128] spectrograms -> (beat, downbeat) logits.  chunking: (chunk_size, border_size,
+        overlap_mode) of split_predict_aggregate, checked by chunking_struct; None is 1500 / 6 / keep_first."""
         assert self._model_ready, "model parameters not loaded"
         assert spect.is_cuda and spect.dtype == torch.float32 and spect.is_contiguous()
+        ck = None if chunking is None else chunking_struct(*chunking)
         total = int(frame_offsets[-1])
         beat = torch.empty(total, dtype=torch.float32, device=self.device)
         down = torch.empty(total, dtype=torch.float32, device=self.device)
-        code = self.lib.bt_spect2frames(self.ctx, c_void_p(spect.data_ptr()), i64_array(frame_offsets), len(frame_offsets) - 1,
-                                        c_void_p(beat.data_ptr()), c_void_p(down.data_ptr()), self._stream())
+        args = (self.ctx, c_void_p(spect.data_ptr()), i64_array(frame_offsets), len(frame_offsets) - 1,
+                c_void_p(beat.data_ptr()), c_void_p(down.data_ptr()))
+        if ck is None:
+            code = self.lib.bt_spect2frames(*args, self._stream())
+        else:
+            code = self.lib.bt_spect2frames_chunked(*args, ctypes.byref(ck), self._stream())
         _lib.check(self.lib, self.ctx, code)
         return beat, down
 
@@ -217,14 +239,20 @@ class Engine:
             self.lib.bt_debug_request_tap(self.ctx, b"", None, 0)
         return buf[:n], out
 
-    def audio2frames_cat(self, audio: torch.Tensor, sample_offsets):
+    def audio2frames_cat(self, audio: torch.Tensor, sample_offsets, chunking: tuple | None = None):
+        """Concatenated mono 22.05 kHz audio -> (beat, downbeat, frame offsets); chunking as in spect2frames_cat."""
         assert self._model_ready, "model parameters not loaded"
         assert audio.is_cuda and audio.dtype == torch.float32 and audio.is_contiguous()
+        ck = None if chunking is None else chunking_struct(*chunking)
         fo = self.frame_offsets(sample_offsets)
         beat = torch.empty(fo[-1], dtype=torch.float32, device=self.device)
         down = torch.empty(fo[-1], dtype=torch.float32, device=self.device)
-        code = self.lib.bt_audio2frames(self.ctx, c_void_p(audio.data_ptr()), i64_array(sample_offsets), len(sample_offsets) - 1,
-                                        c_void_p(beat.data_ptr()), c_void_p(down.data_ptr()), i64_array(fo), self._stream())
+        args = (self.ctx, c_void_p(audio.data_ptr()), i64_array(sample_offsets), len(sample_offsets) - 1,
+                c_void_p(beat.data_ptr()), c_void_p(down.data_ptr()), i64_array(fo))
+        if ck is None:
+            code = self.lib.bt_audio2frames(*args, self._stream())
+        else:
+            code = self.lib.bt_audio2frames_chunked(*args, ctypes.byref(ck), self._stream())
         _lib.check(self.lib, self.ctx, code)
         return beat, down, fo
 

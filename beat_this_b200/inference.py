@@ -19,7 +19,7 @@ import numpy as np
 import torch
 
 from ._lib import bt_wav_info
-from .engine import Engine
+from .engine import Engine, chunking_struct
 from .pipeline import BeatPipeline, as_signal_array, chunk_cost, plan_groups
 from .postprocessor import Postprocessor
 from .preprocessing import LogMelSpect, load_audio
@@ -104,9 +104,9 @@ def load_model(checkpoint_path: str | dict | None = "final0", device: str | torc
 
 
 # ------------------------------------------------------------------------------------------------------------
-# Chunking helpers of the reference API (inference.py:90-230).  The CUDA path never calls them -- bt_plan_chunks
+# Chunking helpers of the reference API (inference.py:90-230).  The CUDA path never calls them -- bt_plan_chunking
 # plans natively and the stem / head kernels gather and scatter in place -- they serve users of the reference's
-# function-level API and are pinned to the reference by tests/golden/chunking.npz.
+# function-level API and are pinned to the reference by tests/golden/chunking.npz and chunking_modes.npz.
 # ------------------------------------------------------------------------------------------------------------
 def chunk_starts(n_frames: int, chunk_size: int, border_size: int = 6, avoid_short_end: bool = True) -> np.ndarray:
     """First frame of every chunk: windows advance by chunk_size - 2*border_size from -border_size; with
@@ -171,14 +171,28 @@ def aggregate_prediction(pred_chunks: list, starts: list, full_size: int, chunk_
     return beat, downbeat
 
 
+DEFAULT_CHUNKING = (1500, 6, "keep_first")  # what Spect2Frames.spect2frames uses (reference inference.py:244-254)
+
+
+def engine_chunking(chunk_size: int, border_size: int, overlap_mode: str) -> tuple | None:
+    """The `chunking` argument of Engine.spect2frames_cat / audio2frames_cat for split_predict_aggregate's values:
+    None for 1500 / 6 / keep_first (the plain entry points), else the checked triple.  ``ValueError`` for values the
+    CUDA path cannot run (engine.chunking_struct)."""
+    chunking_struct(chunk_size, border_size, overlap_mode)
+    chunking = (int(chunk_size), int(border_size), overlap_mode)
+    return None if chunking == DEFAULT_CHUNKING else chunking
+
+
 def split_predict_aggregate(spect: torch.Tensor, chunk_size: int, border_size: int, overlap_mode: str,
                             model) -> dict:
     """Reference inference.py:188-230: chunk the piece, run `model` on every chunk, stitch.  A ``BeatThisB200`` model
-    with the standard 1500 / 6 / keep_first setting runs as ONE call of the CUDA path (all chunks batched, chunking
-    and stitching inside the kernels); anything else goes chunk by chunk through the functions above."""
-    if isinstance(model, BeatThisB200) and (chunk_size, border_size, overlap_mode) == (1500, 6, "keep_first"):
+    runs as ONE call of the CUDA path for every chunk_size <= 1500, border_size with 0 <= 2 * border_size < chunk_size
+    and overlap_mode (all chunks batched, chunking and stitching inside the kernels; other values raise
+    ``ValueError``); any other model goes chunk by chunk through the functions above."""
+    if isinstance(model, BeatThisB200):
+        chunking = engine_chunking(chunk_size, border_size, overlap_mode)
         spect = torch.as_tensor(spect, dtype=torch.float32, device=model.device).contiguous()
-        beat, down = model.engine.spect2frames_cat(spect, [0, spect.shape[0]])
+        beat, down = model.engine.spect2frames_cat(spect, [0, spect.shape[0]], chunking)
         return {"beat": beat, "downbeat": down}
     chunks, starts = split_piece(spect, chunk_size, border_size=border_size, avoid_short_end=True)
     preds = []
@@ -206,13 +220,15 @@ class Spect2Frames:
         beat, down = self.model.engine.spect2frames_cat(spect, [0, spect.shape[0]])
         return beat, down
 
-    def spects2frames(self, spects):
-        """Batched variant: list of [T_i,128] tensors -> list of (beat, downbeat)."""
+    def spects2frames(self, spects, chunk_size: int = 1500, border_size: int = 6, overlap_mode: str = "keep_first"):
+        """Batched variant: list of [T_i,128] tensors -> list of (beat, downbeat), every piece cut and stitched as
+        split_predict_aggregate(spect, chunk_size, border_size, overlap_mode, model) does, all in one call."""
+        chunking = engine_chunking(chunk_size, border_size, overlap_mode)
         spects = [torch.as_tensor(s, dtype=torch.float32, device=self.device) for s in spects]
         fo = [0]
         for s in spects:
             fo.append(fo[-1] + s.shape[0])
-        beat, down = self.model.engine.spect2frames_cat(torch.cat(spects).contiguous(), fo)
+        beat, down = self.model.engine.spect2frames_cat(torch.cat(spects).contiguous(), fo, chunking)
         return [(beat[fo[i] : fo[i + 1]], down[fo[i] : fo[i + 1]]) for i in range(len(spects))]
 
     def __call__(self, spect):
@@ -290,12 +306,13 @@ class Audio2Frames(Spect2Frames):
         return beat, down
 
     # ---- many clips ---------------------------------------------------------------------------------------
-    def _run_groups(self, arrays, sr, want):
+    def _run_groups(self, arrays, sr, want, chunking=None):
         """Generator over groups: (first index, last index + 1, pipeline result)."""
         pipe = self.pipeline
         groups = plan_groups([chunk_cost(a.shape[0], sr) for a in arrays], GROUP_CHUNKS, GROUP_CLIPS)
         try:
-            results = pipe.run(len(groups), lambda g: pipe.submit_signals(arrays[groups[g][0] : groups[g][1]], sr, want))
+            results = pipe.run(len(groups),
+                               lambda g: pipe.submit_signals(arrays[groups[g][0] : groups[g][1]], sr, want, chunking))
             for (lo, hi), res in zip(groups, results):
                 yield lo, hi, res
         finally:
@@ -304,9 +321,13 @@ class Audio2Frames(Spect2Frames):
     def batch(self, signals, sr=22050):
         """list of signals (1-D or (time, channels) arrays, `sr` Hz) -> list of (beat_logits, downbeat_logits) device
         tensors; staging, copies and kernels of consecutive groups of clips overlap."""
+        return self._frames_batch(signals, sr, None)
+
+    def _frames_batch(self, signals, sr, chunking):
+        """batch() with the `chunking` argument of Engine.audio2frames_cat."""
         arrays, sr = self._prepare(signals, sr)
         out = [None] * len(arrays)
-        for lo, hi, (beat, down, fo) in self._run_groups(arrays, sr, "frames"):
+        for lo, hi, (beat, down, fo) in self._run_groups(arrays, sr, "frames", chunking):
             for i in range(lo, hi):
                 out[i] = (beat[fo[i - lo] : fo[i - lo + 1]], down[fo[i - lo] : fo[i - lo + 1]])
         return out
@@ -465,9 +486,11 @@ class File2Beats(Audio2Beats):
         return out
 
 
-    def frames_batch(self, audio_paths):
+    def frames_batch(self, audio_paths, chunk_size: int = 1500, border_size: int = 6, overlap_mode: str = "keep_first"):
         """Framewise (beat, downbeat) logits of many files as device tensors, through the groups and kernels of batch()
-        up to the post-processor: frames2beats.batch_cat of them gives batch()'s beats.  Errors raise."""
+        up to the post-processor: frames2beats.batch_cat of them gives batch()'s beats.  Every piece is cut and
+        stitched as split_predict_aggregate(spect, chunk_size, border_size, overlap_mode, model) does.  Errors raise."""
+        chunking = engine_chunking(chunk_size, border_size, overlap_mode)
         paths = [str(p) for p in audio_paths]
         out = [None] * len(paths)
         infos, is_wav = self.probe(paths)
@@ -481,7 +504,8 @@ class File2Beats(Audio2Beats):
 
             def submit(g, idx=idx, groups=groups, sr=sr):
                 sel = idx[groups[g][0] : groups[g][1]]
-                pipe.submit_wavs([paths[i] for i in sel], (bt_wav_info * len(sel))(*[infos[i] for i in sel]), sr, "frames")
+                pipe.submit_wavs([paths[i] for i in sel], (bt_wav_info * len(sel))(*[infos[i] for i in sel]), sr, "frames",
+                                 chunking)
 
             try:
                 for (lo, hi), (beat, down, fo) in zip(groups, pipe.run(len(groups), submit)):
@@ -492,7 +516,7 @@ class File2Beats(Audio2Beats):
         loaded = {i: load_audio(paths[i]) for i in range(len(paths)) if not is_wav[i]}
         for sr in sorted({s for _, s in loaded.values()}):
             idx = [i for i in loaded if loaded[i][1] == sr]
-            for i, r in zip(idx, Audio2Frames.batch(self, [loaded[i][0] for i in idx], sr)):
+            for i, r in zip(idx, Audio2Frames._frames_batch(self, [loaded[i][0] for i in idx], sr, chunking)):
                 out[i] = r
         return out
 

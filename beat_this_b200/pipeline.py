@@ -63,6 +63,13 @@ def chunk_cost(n_samples: int, sr: int = 22050) -> int:
     return max(1, -(-frames // 1488))
 
 
+def _check_frames_route(want: str, chunking) -> None:
+    """Only framewise logits take another chunking than 1500 / 6 / keep_first: the beat routes keep the reference's
+    Audio2Beats, which always cuts that way (inference.py:244-254)."""
+    if chunking is not None and want != "frames":
+        raise ValueError(f'a chunking applies to want="frames" only, not want="{want}"')
+
+
 class _Slot:
     def __init__(self):
         self.host = None      # pinned fp32 staging buffer
@@ -137,7 +144,7 @@ class BeatPipeline:
             raise _lib.BTError(f"bt_stage_audio failed ({code}): bad signal array")
         return so
 
-    def _enqueue(self, idx, s, so, sr, want):
+    def _enqueue(self, idx, s, so, sr, want, chunking=None):
         n = so[-1]
         with torch.cuda.stream(self.copy_stream):
             s.dev[:n].copy_(s.host[:n], non_blocking=True)
@@ -152,7 +159,7 @@ class BeatPipeline:
             audio, offs = s.dev[:n], so
             if sr != 22050:
                 audio, offs = eng.resample_cat(audio, so, sr)
-            beat, down, fo = eng.audio2frames_cat(audio, offs)
+            beat, down, fo = eng.audio2frames_cat(audio, offs, chunking)
             if want == "beats":
                 handle = eng.peakpick_async(beat, down, fo, s.peak)
                 self.d2h_bytes += handle.d2h_bytes
@@ -180,13 +187,15 @@ class BeatPipeline:
             s.t1.record(self.compute_stream)
         self.inflight.append((idx, payload))
 
-    def submit_signals(self, arrays, sr: int = 22050, want: str = "beats"):
+    def submit_signals(self, arrays, sr: int = 22050, want: str = "beats", chunking: tuple | None = None):
+        """chunking (want="frames" only): (chunk_size, border_size, overlap_mode), see Engine.spect2frames_cat."""
+        _check_frames_route(want, chunking)
         idx, s = self._slot(sum(a.shape[0] for a in arrays))
         try:
             t0 = time.perf_counter()
             so = self.stage_signals(arrays, s.host)
             t1 = time.perf_counter()
-            self._enqueue(idx, s, so, int(sr), want)
+            self._enqueue(idx, s, so, int(sr), want, chunking)
             self.stats["stage_s"] += t1 - t0
             self.stats["enqueue_s"] += time.perf_counter() - t1
             self.stats["groups"] += 1
@@ -194,8 +203,10 @@ class BeatPipeline:
             self.free.append(idx)
             raise
 
-    def submit_wavs(self, paths, infos, sr: int, want: str = "beats"):
-        """paths: list of str; infos: ctypes array of bt_wav_info (all `sr` Hz) from bt_wav_probe."""
+    def submit_wavs(self, paths, infos, sr: int, want: str = "beats", chunking: tuple | None = None):
+        """paths: list of str; infos: ctypes array of bt_wav_info (all `sr` Hz) from bt_wav_probe; chunking as in
+        submit_signals."""
+        _check_frames_route(want, chunking)
         n = len(paths)
         so = [0]
         for i in range(n):
@@ -211,7 +222,7 @@ class BeatPipeline:
                 bad = [str(paths[i]) for i in range(n) if status[i] != 0]
                 raise RuntimeError(f"Could not load audio from {bad}")
             t1 = time.perf_counter()
-            self._enqueue(idx, s, so, int(sr), want)
+            self._enqueue(idx, s, so, int(sr), want, chunking)
             self.stats["stage_s"] += t1 - t0
             self.stats["enqueue_s"] += time.perf_counter() - t1
             self.stats["groups"] += 1

@@ -105,6 +105,37 @@ int64_t bt_num_frames(int64_t n_samples);
  * (or the count needed when cap is too small). */
 int64_t bt_plan_chunks(int64_t T, int64_t* starts, int64_t* lens, int64_t cap);
 
+/* How split_predict_aggregate (inference.py:188-230) cuts a piece and stitches it back: split_piece with
+ * avoid_short_end=True (:100-135), then aggregate_prediction (:138-185).  bt_plan_chunks, bt_spect2frames and
+ * bt_audio2frames use { BT_CHUNK, BT_BORDER, BT_KEEP_FIRST }; PLBeatThis.predict_step (model/pl_module.py:231-266) cuts
+ * a border of 2 * tolerance, 0 for the weighted_bce / bce checkpoints. */
+#define BT_KEEP_FIRST 0 /* a frame two chunks cover comes from the earlier one */
+#define BT_KEEP_LAST 1  /* ... from the later one                              */
+
+typedef struct bt_chunking {
+  int32_t chunk_size;   /* model frames per chunk, 1 <= chunk_size <= BT_CHUNK (the RoPE tables and workspace size) */
+  int32_t border;       /* frames cut from each side of a chunk's predictions, 0 <= 2 * border < chunk_size       */
+  int32_t overlap_mode; /* BT_KEEP_FIRST or BT_KEEP_LAST                                                       */
+} bt_chunking;
+
+/* The chunk plan of a piece of T frames under chunking `ck` (c = chunk_size, b = border, step = c - 2b):
+ *  - starts s_i = -b + i * step for i = 0 .. ceil(T / step) - 1 (numpy arange(-b, T - b, step)); when T > step the
+ *    last start is moved to T - (c - b);
+ *  - chunk i covers the piece rows [max(s_i, 0), min(s_i + c, T)), with max(0, -s_i) zero rows on its left and
+ *    max(0, min(b, s_i + c - T)) on its right; lens[i] is its length (<= c);
+ *  - its predictions lose b frames on each side; what remains lands on [s_i + b, s_i + lens[i] - b), which equals
+ *    [s_i + b, s_i + c - b) clipped to [0, T);
+ *  - a frame two chunks cover belongs to the earlier chunk (BT_KEEP_FIRST) or the later one (BT_KEEP_LAST):
+ *    chunk i owns [own_lo[i], own_hi[i]) in piece frames.
+ * No frame is left uncovered (the reference would leave -1000 there): s_0 + b = 0; starts increase and
+ * s_{i+1} + b <= s_i + c - b, with s_{i+1} + b < T, so each range reaches the next one's beginning; the last chunk's
+ * range ends at T (it starts at T - (c - b), or is the only chunk and T <= step).  Owned ranges are therefore
+ * consecutive, non-empty and tile [0, T) exactly.
+ * Writes up to `cap` entries of each non-NULL output array and returns the chunk count (the count needed when cap is
+ * too small; 0 for T <= 0), or BT_ERR_ARG when ck is NULL or outside the limits above.  Pure host: no ctx, no CUDA. */
+int64_t bt_plan_chunking(int64_t T, const bt_chunking* ck, int64_t* starts, int64_t* lens, int64_t* own_lo,
+                         int64_t* own_hi, int64_t cap);
+
 /* ---- host front door: Audio2Frames.signal2spect's host half (inference.py:269-276) ------------------ */
 
 #define BT_SIG_F32 0 /* float32 samples                                                         */
@@ -203,6 +234,16 @@ int bt_forward_chunks(bt_ctx* ctx, const float* chunks_dev, int32_t n_chunks, in
 int bt_audio2frames(bt_ctx* ctx, const float* audio_dev, const int64_t* sample_offsets_host,
                     int32_t n_clips, float* beat_dev, float* downbeat_dev,
                     const int64_t* frame_offsets_host, void* stream);
+
+/* bt_spect2frames / bt_audio2frames with the pieces cut and stitched by `ck` (see bt_plan_chunking) instead of
+ * 1500 / 6 / keep_first: split_predict_aggregate (inference.py:188-230) with any valid chunk_size, border_size and
+ * overlap_mode, every chunk of every clip batched into waves.  With { BT_CHUNK, BT_BORDER, BT_KEEP_FIRST } the results
+ * are bitwise those of the plain entry points.  BT_ERR_ARG, before anything is enqueued, for an invalid ck. */
+int bt_spect2frames_chunked(bt_ctx* ctx, const float* spect_dev, const int64_t* frame_offsets_host, int32_t n_clips,
+                            float* beat_dev, float* downbeat_dev, const bt_chunking* ck, void* stream);
+int bt_audio2frames_chunked(bt_ctx* ctx, const float* audio_dev, const int64_t* sample_offsets_host, int32_t n_clips,
+                            float* beat_dev, float* downbeat_dev, const int64_t* frame_offsets_host,
+                            const bt_chunking* ck, void* stream);
 
 /* Postprocessor("minimal") (model/postprocessor.py:85-136,176-197) on device.
  * Per clip i: beat_times_dev[i*max_peaks ..] (float64 seconds), n_beats_dev[i], same for
