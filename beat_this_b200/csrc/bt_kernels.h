@@ -65,7 +65,7 @@ void launch_zero_tail(void* buf, int elem_bytes, const ChunkSrc* chunks, int nch
 
 // ---- shared small kernels (templated on activation dtype inside) ---------------------------
 // RMSNorm without gamma (folded into the next weight); optionally also the attention gates
-// sigmoid(xn . wg[h] + bg[h]) for h < heads (used when heads <= 4; wg is [>=heads, C] fp32).
+// sigmoid(xn . wg[h] + bg[h]) for h < heads (used when heads <= 2; wg is [>=heads, C] fp32).
 void launch_norm(const float* x, void* xn, int64_t M, int C, int act_h16, cudaStream_t st, float* gates = nullptr,
                  const float* wg = nullptr, const float* bg = nullptr, int heads = 0);
 // per-chunk source description for the stem (chunk gather from per-clip spectrograms)

@@ -1,5 +1,5 @@
-// GEMM epilogues shared by the fp32 CUDA-core GEMM and the h16 wgmma GEMM.
-// epilogue_apply: a thread hands over CNT consecutive accumulator columns [n0, n0+CNT) of output row m;
+// GEMM epilogues of the fp32 CUDA-core GEMM and the h16 wgmma GEMM.
+// epilogue_apply (fp32 GEMM): a thread hands over four consecutive accumulator columns [n0, n0+4) of output row m;
 // epi_bias_gelu / epi_resid / epi_rope / epi_gates_pair: two adjacent columns [n, n+1) (the wgmma accumulator fragment).
 #pragma once
 #include "bt_kernels.h"
@@ -8,39 +8,6 @@
 #include "common.cuh"
 
 namespace bt {
-
-template <typename TAct, int CNT>
-__device__ __forceinline__ void store_act(TAct* p, const float (&v)[CNT]);
-
-template <>
-__device__ __forceinline__ void store_act<float, 4>(float* p, const float (&v)[4]) {
-  *reinterpret_cast<float4*>(p) = make_float4(v[0], v[1], v[2], v[3]);
-}
-template <>
-__device__ __forceinline__ void store_act<h16, 4>(h16* p, const float (&v)[4]) {
-  uint2 u;
-  u.x = pack_h16x2(v[0], v[1]);
-  u.y = pack_h16x2(v[2], v[3]);
-  *reinterpret_cast<uint2*>(p) = u;
-}
-template <>
-__device__ __forceinline__ void store_act<float, 32>(float* p, const float (&v)[32]) {
-#pragma unroll
-  for (int i = 0; i < 8; ++i)
-    reinterpret_cast<float4*>(p)[i] = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
-}
-template <>
-__device__ __forceinline__ void store_act<h16, 32>(h16* p, const float (&v)[32]) {
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    uint4 u;
-    u.x = pack_h16x2(v[8 * i + 0], v[8 * i + 1]);
-    u.y = pack_h16x2(v[8 * i + 2], v[8 * i + 3]);
-    u.z = pack_h16x2(v[8 * i + 4], v[8 * i + 5]);
-    u.w = pack_h16x2(v[8 * i + 6], v[8 * i + 7]);
-    reinterpret_cast<uint4*>(p)[i] = u;
-  }
-}
 
 // erf by Abramowitz-Stegun 7.1.26 (|error| <= 1.5e-7) on the MUFU/FMA pipes: the tensor-core
 // epilogue evaluates GELU for every FFN hidden element and erff()'s ~35 instructions made it
@@ -76,88 +43,53 @@ __device__ __forceinline__ float gelu_for(float x) {
   else return gelu_erf(x);
 }
 
-// CNT in {4, 32}; n0 % CNT == 0; for kind 1 a head (32 columns) is never split across a
-// q/k/v boundary because C % 32 == 0.
-template <typename TAct, int CNT>
-__device__ __forceinline__ void epilogue_apply(const EpiParams& e, int L, int64_t m, int n0,
-                                               float (&v)[CNT], const float (&pre)[CNT], bool use_pre,
-                                               uint32_t bias_smem = 0) {
+__device__ __forceinline__ void store_f32x4(float* p, const float (&v)[4]) {
+  *reinterpret_cast<float4*>(p) = make_float4(v[0], v[1], v[2], v[3]);
+}
+// n0 % 4 == 0; for kind 1 a head (32 columns) is never split across a q/k/v boundary because C % 32 == 0.
+__device__ __forceinline__ void epilogue_apply(const EpiParams& e, int L, int64_t m, int n0, float (&v)[4]) {
   if (e.kind == 0) {
     if (e.bias) {
-      if (bias_smem) {  // bias vector staged in shared memory by the caller (short-latency broadcast reads)
-#pragma unroll
-        for (int i = 0; i < CNT / 4; ++i) {
-          float4 q;
-          asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];"
-                       : "=f"(q.x), "=f"(q.y), "=f"(q.z), "=f"(q.w)
-                       : "r"(bias_smem + static_cast<uint32_t>(n0 + 4 * i) * 4u));
-          v[4 * i] += q.x; v[4 * i + 1] += q.y; v[4 * i + 2] += q.z; v[4 * i + 3] += q.w;
-        }
-      } else {
-        const float4* b4 = reinterpret_cast<const float4*>(e.bias + n0);
-#pragma unroll
-        for (int i = 0; i < CNT / 4; ++i) {
-          const float4 q = __ldg(b4 + i);
-          v[4 * i] += q.x; v[4 * i + 1] += q.y; v[4 * i + 2] += q.z; v[4 * i + 3] += q.w;
-        }
-      }
+      const float4 q = __ldg(reinterpret_cast<const float4*>(e.bias + n0));
+      v[0] += q.x; v[1] += q.y; v[2] += q.z; v[3] += q.w;
     }
     if (e.gelu) {
 #pragma unroll
-      for (int i = 0; i < CNT; ++i) v[i] = gelu_for<TAct>(v[i]);
+      for (int i = 0; i < 4; ++i) v[i] = gelu_erf(v[i]);
     }
-    if (use_pre) {  // residual prefetched by the caller (pipelined with the previous chunk)
-#pragma unroll
-      for (int i = 0; i < CNT; ++i) v[i] += pre[i];
-    } else if (e.resid) {
-      const float4* r = reinterpret_cast<const float4*>(e.resid + m * e.ldr + n0);
-#pragma unroll
-      for (int i = 0; i < CNT / 4; ++i) {
-        float4 q = r[i];
-        v[4 * i] += q.x;
-        v[4 * i + 1] += q.y;
-        v[4 * i + 2] += q.z;
-        v[4 * i + 3] += q.w;
-      }
+    if (e.resid) {
+      const float4 q = *reinterpret_cast<const float4*>(e.resid + m * e.ldr + n0);
+      v[0] += q.x; v[1] += q.y; v[2] += q.z; v[3] += q.w;
     }
-    if (e.out_f32) store_act<float, CNT>(e.out_f32 + m * e.ldo_f32 + n0, v);
-    if (e.out_act) store_act<TAct, CNT>(reinterpret_cast<TAct*>(e.out_act) + m * e.ldo_act + n0, v);
+    if (e.out_f32) store_f32x4(e.out_f32 + m * e.ldo_f32 + n0, v);
+    if (e.out_act) store_f32x4(reinterpret_cast<float*>(e.out_act) + m * e.ldo_act + n0, v);
   } else if (e.kind == 2) {
     // attention gates (reference roformer.py:127-128): sigmoid(to_gates(x_normed)), N padded to 32
 #pragma unroll
-    for (int i = 0; i < CNT; ++i)
+    for (int i = 0; i < 4; ++i)
       if (n0 + i < e.heads) e.out_f32[m * e.heads + n0 + i] = sigmoidf_(v[i] + __ldg(e.bias + n0 + i));
   } else {
     // qkv: RoPE on interleaved pairs (rotary_embedding_torch semantics, reference
     // roformer.py:121-123): out[2i] = x[2i] cos - x[2i+1] sin ; out[2i+1] = x[2i+1] cos + x[2i] sin
     const int which = n0 / e.C;          // 0 q, 1 k, 2 v
-    TAct* dst = reinterpret_cast<TAct*>(e.out_act) + m * e.ldo_act + n0;
+    float* dst = reinterpret_cast<float*>(e.out_act) + m * e.ldo_act + n0;
+    // the store sits in both branches: hoisted after them, it changes ptxas's register allocation of the whole GEMM
     if (which < 2) {
       const float sc = which == 0 ? e.qscale : 1.0f;
-      if (use_pre && CNT == 32) {  // cos[16] | sin[16] of this row's position, preloaded by the caller
+      const int c = n0 - which * e.C;
+      const int pos = e.posmode == 0 ? static_cast<int>(m % L) : static_cast<int>((m / L) % e.F);
+      const float* cs = e.rope_cos + pos * 16 + ((c & 31) >> 1);
+      const float* sn = e.rope_sin + pos * 16 + ((c & 31) >> 1);
 #pragma unroll
-        for (int i = 0; i < CNT / 2; ++i) {
-          const float co = pre[i % CNT], si = pre[(16 + i) % CNT];
-          const float x0 = v[2 * i], x1 = v[2 * i + 1];
-          v[2 * i] = (x0 * co - x1 * si) * sc;
-          v[2 * i + 1] = (x1 * co + x0 * si) * sc;
-        }
-      } else {
-        const int c = n0 - which * e.C;
-        const int pos = e.posmode == 0 ? static_cast<int>(m % L) : static_cast<int>((m / L) % e.F);
-        const float* cs = e.rope_cos + pos * 16 + ((c & 31) >> 1);
-        const float* sn = e.rope_sin + pos * 16 + ((c & 31) >> 1);
-#pragma unroll
-        for (int i = 0; i < CNT / 2; ++i) {
-          const float co = __ldg(cs + i), si = __ldg(sn + i);
-          const float x0 = v[2 * i], x1 = v[2 * i + 1];
-          v[2 * i] = (x0 * co - x1 * si) * sc;
-          v[2 * i + 1] = (x1 * co + x0 * si) * sc;
-        }
+      for (int i = 0; i < 2; ++i) {
+        const float co = __ldg(cs + i), si = __ldg(sn + i);
+        const float x0 = v[2 * i], x1 = v[2 * i + 1];
+        v[2 * i] = (x0 * co - x1 * si) * sc;
+        v[2 * i + 1] = (x1 * co + x0 * si) * sc;
       }
-      store_act<TAct, CNT>(dst, v);
+      store_f32x4(dst, v);
     } else {
-      store_act<TAct, CNT>(dst, v);
+      store_f32x4(dst, v);
     }
   }
 }

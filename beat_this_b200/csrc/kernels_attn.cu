@@ -54,10 +54,10 @@ attn_time_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
   const int nkv = ceil_div(Lk, AT_BKV);
 
   if (threadIdx.x == 0) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar_q), "r"(1));
+    mbar_init(bar_q, 1);
     for (int i = 0; i < AT_NST; ++i) {
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(full + 8 * i), "r"(1));
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(empty + 8 * i), "r"(AT_WARPS));
+      mbar_init(full + 8 * i, 1);
+      mbar_init(empty + 8 * i, AT_WARPS);
     }
     fence_barrier_init();
   }
@@ -67,21 +67,21 @@ attn_time_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     if (lane == 0) {
       tma_prefetch_desc(&tmQ);
       tma_prefetch_desc(&tmKV);
-      mbar_expect_tx_a(bar_q, AT_SQ);
-      tma_load_3d_a(sQ, &tmQ, bar_q, h * 32, q0, seq);
+      mbar_expect_tx(bar_q, AT_SQ);
+      tma_load_3d(sQ, &tmQ, bar_q, h * 32, q0, seq);
       for (int j = 0; j < nkv; ++j) {
         const int st = j % AT_NST;
-        if (j >= AT_NST) mbar_wait_a(empty + 8 * st, ((j / AT_NST) - 1) & 1);
-        mbar_expect_tx_a(full + 8 * st, 2 * AT_SKV);
-        tma_load_3d_a(sK + st * AT_SKV, &tmKV, full + 8 * st, C + h * 32, j * AT_BKV, seq);
-        tma_load_3d_a(sV + st * AT_SKV, &tmKV, full + 8 * st, 2 * C + h * 32, j * AT_BKV, seq);
+        if (j >= AT_NST) mbar_wait(empty + 8 * st, ((j / AT_NST) - 1) & 1);
+        mbar_expect_tx(full + 8 * st, 2 * AT_SKV);
+        tma_load_3d(sK + st * AT_SKV, &tmKV, full + 8 * st, C + h * 32, j * AT_BKV, seq);
+        tma_load_3d(sV + st * AT_SKV, &tmKV, full + 8 * st, 2 * C + h * 32, j * AT_BKV, seq);
       }
     }
     return;
   }
 
   const int r0 = warp * 16;  // this warp's query rows [r0, r0 + 16) of the tile; the thread holds rows lane/4 and +8
-  mbar_wait_a(bar_q, 0);
+  mbar_wait(bar_q, 0);
   uint32_t qa[2][4];
 #pragma unroll
   for (int ks = 0; ks < 2; ++ks) ldmatrix_x4(sQ + sw64_off(r0 + (lane & 15), 2 * ks + (lane >> 4)), qa[ks]);
@@ -92,7 +92,7 @@ attn_time_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
   float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
   for (int j = 0; j < nkv; ++j) {
     const int st = j % AT_NST;
-    mbar_wait_a(full + 8 * st, (j / AT_NST) & 1);
+    mbar_wait(full + 8 * st, (j / AT_NST) & 1);
     const uint32_t kb = sK + st * AT_SKV, vb = sV + st * AT_SKV;
     float s[8][4];
 #pragma unroll
@@ -159,7 +159,7 @@ attn_time_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
       }
     }
     __syncwarp();
-    if (lane == 0) mbar_arrive_a(empty + 8 * st);
+    if (lane == 0) mbar_arrive(empty + 8 * st);
   }
 #pragma unroll
   for (int r = 0; r < 2; ++r) {

@@ -125,11 +125,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     if (KIND == 0 && e.out_f32) tma_prefetch_desc(&tmF);
     if (KIND != 2 && e.out_act) tma_prefetch_desc(&tmH);
     for (int i = 0; i < STAGES; ++i) {
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(full + 8 * i), "r"(1));
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(empty + 8 * i), "r"(2));
+      mbar_init(full + 8 * i, 1);
+      mbar_init(empty + 8 * i, 2);
     }
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(rfull), "r"(1));
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(rempty), "r"(2));
+    mbar_init(rfull, 1);
+    mbar_init(rempty, 2);
     fence_barrier_init();
   }
   __syncthreads();
@@ -152,17 +152,17 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         for (int kb = 0; kb < num_kb; ++kb) {
           const int s = kb / kb_per_slab;
           const int k0 = (kb - s * kb_per_slab) * BK;
-          mbar_wait_a(empty + 8 * stage, phase ^ 1);
+          mbar_wait(empty + 8 * stage, phase ^ 1);
           const uint32_t fb = full + 8 * stage;
-          mbar_expect_tx_a(fb, Cfg::STAGE_BYTES);
+          mbar_expect_tx(fb, Cfg::STAGE_BYTES);
           // A rows outside [0, L) of the plane (conv time shifts, the last tile of a plane) arrive as zeros
-          tma_load_3d_a(sA + stage * Cfg::A_BYTES, &tmA, fb, k0, t0 + g.t_shift[s], p_out * g.plane_mul + g.plane_add[s]);
-          tma_load_2d_a(sW + stage * Cfg::W_BYTES, &tmW, fb, s * g.Kslab + k0, nt * BN);
+          tma_load_3d(sA + stage * Cfg::A_BYTES, &tmA, fb, k0, t0 + g.t_shift[s], p_out * g.plane_mul + g.plane_add[s]);
+          tma_load_2d(sW + stage * Cfg::W_BYTES, &tmW, fb, s * g.Kslab + k0, nt * BN);
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
           if (has_resid && kb == kb_resid) {
-            mbar_wait_a(rempty, rphase ^ 1);
-            mbar_expect_tx_a(rfull, TG_BM * BN * 4);
-            for (int u = 0; u < BN / 32; ++u) tma_load_3d_a(sE + u * TG_UNIT_BYTES, &tmR, rfull, nt * BN + 32 * u, t0, p_out);
+            mbar_wait(rempty, rphase ^ 1);
+            mbar_expect_tx(rfull, TG_BM * BN * 4);
+            for (int u = 0; u < BN / 32; ++u) tma_load_3d(sE + u * TG_UNIT_BYTES, &tmR, rfull, nt * BN + 32 * u, t0, p_out);
             rphase ^= 1;
           }
         }
@@ -186,7 +186,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       const int t0 = (mt - p_out * t_tiles) * TG_BM;
       int prev = -1;  // stage of the k-block whose MMAs are still in flight
       for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait_a(full + 8 * stage, phase);
+        mbar_wait(full + 8 * stage, phase);
         const uint32_t a_base = sA + stage * Cfg::A_BYTES + a_off;
         const uint32_t b_base = sW + stage * Cfg::W_BYTES;
         wgmma_fence();
@@ -199,15 +199,15 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           // while the first MMAs run: the previous tile's stores have read the staging units, which frees them and
           // the residual buffer
           bulk_wait_read<0>();
-          if (has_resid) mbar_arrive_a(rempty);
+          if (has_resid) mbar_arrive(rempty);
         }
         wgmma_wait<1>();  // the previous k-block's MMAs are done: its stage goes back to the producer
-        if (leader && prev >= 0) mbar_arrive_a(empty + 8 * prev);
+        if (leader && prev >= 0) mbar_arrive(empty + 8 * prev);
         prev = stage;
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
       wgmma_wait<0>();
-      if (leader) mbar_arrive_a(empty + 8 * prev);
+      if (leader) mbar_arrive(empty + 8 * prev);
       if constexpr (KIND == 2) {
         const int tr = t0 + wg * 64 + row_q;
 #pragma unroll
@@ -228,7 +228,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           for (int h = 0; h < 2; ++h) epi_bias_gelu<h16>(e, nt * BN + 8 * j + c0, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
       }
       if (has_resid) {
-        mbar_wait_a(rfull, rphase);
+        mbar_wait(rfull, rphase);
         rphase ^= 1;
       }
       named_bar_sync(1 + wg, 128);  // the leader's bulk_wait_read: every unit is free

@@ -1,6 +1,7 @@
 // HBM-bound kernels of the path: log-mel frontend, stem conv, RMSNorm(+gates),
 // frequency-direction attention, head + aggregation scatter, peak picking.
 #include <cuda_fp16.h>
+#include <cstdio>
 #include <cstdlib>
 
 #include "bt_kernels.h"
@@ -372,32 +373,19 @@ void launch_norm(const float* x, void* xn, int64_t M, int C, int act_h16, cudaSt
 // every (chunk, frame, head).  Token m = (b*F + f)*L + t.  A warp handles 32/F groups
 // (b,t,h) at once: lane -> (group g = lane / F, token f = lane % F).  Each lane loads its own
 // q/k/v rows with 16-byte loads, K/V are shared through padded shared memory (float4
-// broadcast reads).  HBM bytes: 3C in + C out per token (activation dtype).
+// broadcast reads).  HBM bytes: 3C in + C out per token (fp32).
 // ------------------------------------------------------------------------------------------
-template <typename TAct>
-__device__ __forceinline__ void load_row32(const TAct* p, float (&v)[32]);
-template <>
-__device__ __forceinline__ void load_row32<float>(const float* p, float (&v)[32]) {
+__device__ __forceinline__ void load_row32(const float* p, float (&v)[32]) {
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
     const float4 q = reinterpret_cast<const float4*>(p)[i];
     v[4 * i] = q.x; v[4 * i + 1] = q.y; v[4 * i + 2] = q.z; v[4 * i + 3] = q.w;
   }
 }
-template <>
-__device__ __forceinline__ void load_row32<h16>(const h16* p, float (&v)[32]) {
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const uint4 q = reinterpret_cast<const uint4*>(p)[i];
-    const uint32_t w[4] = {q.x, q.y, q.z, q.w};
-#pragma unroll
-    for (int j = 0; j < 4; ++j) unpack_h16x2(w[j], v[8 * i + 2 * j], v[8 * i + 2 * j + 1]);
-  }
-}
 
-template <typename TAct, int F>
+template <int F>
 __global__ void __launch_bounds__(128, 4)
-attn_freq_kernel(const TAct* __restrict__ qkv, const float* __restrict__ gates, TAct* __restrict__ out,
+attn_freq_kernel(const float* __restrict__ qkv, const float* __restrict__ gates, float* __restrict__ out,
                  int B, int L, int heads, float scale) {
   constexpr int GPW = 32 / F;
   constexpr int RS = 36;               // padded row stride (floats)
@@ -418,21 +406,21 @@ attn_freq_kernel(const TAct* __restrict__ qkv, const float* __restrict__ gates, 
   const int b = static_cast<int>(bt_ / L);
   const int C = heads * 32;
   const int64_t m = (static_cast<int64_t>(b) * F + f) * L + t;
-  const TAct* rp = qkv + m * 3 * C + h * 32;
+  const float* rp = qkv + m * 3 * C + h * 32;
   float q[32];
   {
     float kv[32];
-    load_row32<TAct>(rp + C, kv);
+    load_row32(rp + C, kv);
     float* kd = &Ks[wib][g * GS + f * RS];
 #pragma unroll
     for (int i = 0; i < 8; ++i)
       reinterpret_cast<float4*>(kd)[i] = make_float4(kv[4 * i], kv[4 * i + 1], kv[4 * i + 2], kv[4 * i + 3]);
-    load_row32<TAct>(rp + 2 * C, kv);
+    load_row32(rp + 2 * C, kv);
     float* vd = &Vs[wib][g * GS + f * RS];
 #pragma unroll
     for (int i = 0; i < 8; ++i)
       reinterpret_cast<float4*>(vd)[i] = make_float4(kv[4 * i], kv[4 * i + 1], kv[4 * i + 2], kv[4 * i + 3]);
-    load_row32<TAct>(rp, q);
+    load_row32(rp, q);
 #pragma unroll
     for (int d = 0; d < 32; ++d) q[d] *= scale;
   }
@@ -475,20 +463,10 @@ attn_freq_kernel(const TAct* __restrict__ qkv, const float* __restrict__ gates, 
   }
   if (act) {
     const float gsc = gates[m * heads + h] / l;
-    TAct* op = out + m * C + h * 32;
-    if constexpr (sizeof(TAct) == 4) {
+    float* op = out + m * C + h * 32;
 #pragma unroll
-      for (int i = 0; i < 8; ++i)
-        reinterpret_cast<float4*>(op)[i] = make_float4(o[4 * i] * gsc, o[4 * i + 1] * gsc, o[4 * i + 2] * gsc, o[4 * i + 3] * gsc);
-    } else {
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        uint4 u;
-        u.x = pack_h16x2(o[8 * i] * gsc, o[8 * i + 1] * gsc); u.y = pack_h16x2(o[8 * i + 2] * gsc, o[8 * i + 3] * gsc);
-        u.z = pack_h16x2(o[8 * i + 4] * gsc, o[8 * i + 5] * gsc); u.w = pack_h16x2(o[8 * i + 6] * gsc, o[8 * i + 7] * gsc);
-        reinterpret_cast<uint4*>(op)[i] = u;
-      }
-    }
+    for (int i = 0; i < 8; ++i)
+      reinterpret_cast<float4*>(op)[i] = make_float4(o[4 * i] * gsc, o[4 * i + 1] * gsc, o[4 * i + 2] * gsc, o[4 * i + 3] * gsc);
   }
 }
 
@@ -499,19 +477,6 @@ attn_freq_kernel(const TAct* __restrict__ qkv, const float* __restrict__ gates, 
 // P re-packed in registers as the A operand of P V (V through ldmatrix.trans).  F = 32: a tile sees
 // all 32 keys; F = 16: a tile is one group; F = 8: a tile holds two groups, the cross blocks are
 // masked.  ~40 tensor instructions per warp instead of ~4000 FMAs per lane.
-__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t (&r)[4]) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
-}
-__device__ __forceinline__ void ldsm_x4_trans(uint32_t addr, uint32_t (&r)[4]) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
-}
-__device__ __forceinline__ void mma_h16_16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32." BT_H16_MMA_SYNC ".f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
-               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
 
 // Tile = FT_TT consecutive frames of one chunk, all F frequency planes, all heads: ONE TMA box per (q|k|v, head)
 // brings [TT][F][32] fp16 into shared memory (SWIZZLE_64B; the tensor map lists the plane dimension before the frame
@@ -538,15 +503,15 @@ attn_freq_mma_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_cons
   const int wib = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int t0 = blockIdx.x * FT_TT, b = blockIdx.y;
   if (threadIdx.x == 0) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(1));
+    mbar_init(bar, 1);
     fence_barrier_init();
-    mbar_expect_tx_a(bar, 3 * HEADS * PH_BYTES);
+    mbar_expect_tx(bar, 3 * HEADS * PH_BYTES);
     for (int part = 0; part < 3; ++part)
       for (int h = 0; h < HEADS; ++h)
-        tma_load_3d_a(sIn + (part * HEADS + h) * PH_BYTES, &tmIn, bar, part * C + h * 32, b * F, t0);
+        tma_load_3d(sIn + (part * HEADS + h) * PH_BYTES, &tmIn, bar, part * C + h * 32, b * F, t0);
   }
   __syncthreads();
-  mbar_wait_a(bar, 0);
+  mbar_wait(bar, 0);
   // this warp's groups: head h, frames tt_base .. tt_base + GPW - 1; "staged row" r = gl * F + f as before
   const int h = (wib * GPW) / FT_TT;
   const int tt_base = (wib * GPW) % FT_TT;
@@ -562,15 +527,15 @@ attn_freq_mma_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_cons
     uint32_t qa[2][4];
 #pragma unroll
     for (int kk = 0; kk < 2; ++kk)
-      ldsm_x4(row_addr(sQ, 16 * mt + (lane & 7) + ((lane >> 3) & 1) * 8, kk * 2 + (lane >> 4)), qa[kk]);
+      ldmatrix_x4(row_addr(sQ, 16 * mt + (lane & 7) + ((lane >> 3) & 1) * 8, kk * 2 + (lane >> 4)), qa[kk]);
     float sc[NT][4];
 #pragma unroll
     for (int j = 0; j < NT; ++j) {
       sc[j][0] = sc[j][1] = sc[j][2] = sc[j][3] = 0.f;
       uint32_t kb[4];
-      ldsm_x4(row_addr(sK, key_base + 8 * j + (lane & 7), lane >> 3), kb);
-      mma_h16_16816(sc[j], qa[0], kb[0], kb[1]);
-      mma_h16_16816(sc[j], qa[1], kb[2], kb[3]);
+      ldmatrix_x4(row_addr(sK, key_base + 8 * j + (lane & 7), lane >> 3), kb);
+      mma_16816(sc[j], qa[0], kb[0], kb[1]);
+      mma_16816(sc[j], qa[1], kb[2], kb[3]);
     }
     if (F == 8) {  // rows 0-7 belong to the tile's first group (keys of tile 0), rows 8-15 to the second
       sc[1][0] = sc[1][1] = -INFINITY;
@@ -608,9 +573,9 @@ attn_freq_mma_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_cons
       for (int jd = 0; jd < 4; jd += 2) {
         uint32_t vb[4];
         const int q4 = lane >> 3;
-        ldsm_x4_trans(row_addr(sV, key_base + 16 * kk + (q4 & 1) * 8 + (lane & 7), jd + (q4 >> 1)), vb);
-        mma_h16_16816(o[jd], pa, vb[0], vb[1]);
-        mma_h16_16816(o[jd + 1], pa, vb[2], vb[3]);
+        ldmatrix_x4_trans(row_addr(sV, key_base + 16 * kk + (q4 & 1) * 8 + (lane & 7), jd + (q4 >> 1)), vb);
+        mma_16816(o[jd], pa, vb[0], vb[1]);
+        mma_16816(o[jd + 1], pa, vb[2], vb[3]);
       }
     }
 #pragma unroll
@@ -703,9 +668,9 @@ void launch_attn_freq_simt(const float* qkv, const float* gates, float* out, int
                            cudaStream_t st) {
   const int64_t ngrp = static_cast<int64_t>(B) * L * heads;
   const unsigned grid = static_cast<unsigned>(ceil_div64(ngrp, 4 * (32 / F)));
-  if (F == 32) attn_freq_kernel<float, 32><<<grid, 128, 0, st>>>(qkv, gates, out, B, L, heads, scale);
-  else if (F == 16) attn_freq_kernel<float, 16><<<grid, 128, 0, st>>>(qkv, gates, out, B, L, heads, scale);
-  else attn_freq_kernel<float, 8><<<grid, 128, 0, st>>>(qkv, gates, out, B, L, heads, scale);
+  if (F == 32) attn_freq_kernel<32><<<grid, 128, 0, st>>>(qkv, gates, out, B, L, heads, scale);
+  else if (F == 16) attn_freq_kernel<16><<<grid, 128, 0, st>>>(qkv, gates, out, B, L, heads, scale);
+  else attn_freq_kernel<8><<<grid, 128, 0, st>>>(qkv, gates, out, B, L, heads, scale);
 }
 
 // ------------------------------------------------------------------------------------------

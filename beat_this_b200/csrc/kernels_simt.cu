@@ -64,7 +64,7 @@ gemm_simt_kernel(const float* __restrict__ A, const float* __restrict__ W, GemmS
       const int t = t0 + ty * 4 + i;
       if (t < g.L) {
         const int64_t m = static_cast<int64_t>(p_out) * g.L + t;
-        epilogue_apply<float, 4>(e, g.L, m, n, acc[i], acc[i], false);
+        epilogue_apply(e, g.L, m, n, acc[i]);
       }
     }
   }

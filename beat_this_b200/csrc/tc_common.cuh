@@ -8,14 +8,6 @@
 
 namespace bt {
 
-__device__ __forceinline__ void tma_load_2d_a(uint32_t smem_dst, const void* tmap, uint32_t bar, int32_t c0, int32_t c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];" ::"r"(smem_dst),
-      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar), "r"(c0), "r"(c1)
-      : "memory");
-}
-
 // ---- TMA stores (shared -> global, bulk async groups of the issuing thread) ----
 __device__ __forceinline__ void tma_store_3d(const void* tmap, uint32_t smem_src, int32_t c0, int32_t c1, int32_t c2) {
   asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(
