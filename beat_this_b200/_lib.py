@@ -186,11 +186,12 @@ PROTOTYPES = {
     ),
     "bt_debug_attention": (
         c_int,
-        [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, POINTER(c_int32), c_int32,
-         c_void_p],
+        [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int32, c_int32, c_int32, POINTER(c_int32),
+         c_int32, c_void_p],
     ),
     "bt_debug_attention_freq": (
-        c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p],
+        c_int,
+        [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int32, c_int32, c_int32, c_int32, c_void_p],
     ),
     "bt_debug_norm": (
         c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_void_p, c_int32, c_void_p],

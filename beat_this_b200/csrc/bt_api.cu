@@ -676,7 +676,7 @@ cudaError_t to_h16_operand(DeviceBuffer<>& buf, const float* src, int64_t n, cud
 // ================================================================================== C ABI
 extern "C" {
 
-int bt_version(void) { return 205; }
+int bt_version(void) { return 206; }
 
 const char* bt_act_dtype(void) {
 #if defined(BT_ACT_BF16)
@@ -1470,17 +1470,15 @@ int bt_debug_gemm(bt_ctx* c, const bt_debug_gemm_desc* d, const float* a_dev, co
 }
 
 int bt_debug_attention(bt_ctx* c, const float* q_dev, const float* k_dev, const float* v_dev, const float* gates_dev,
-                       float* o_dev, int32_t seqs, int32_t L, int32_t heads, const int32_t* key_lens_host,
-                       int32_t seqs_per_chunk, void* stream) {
+                       float* o_dev, int64_t o_count, int32_t seqs, int32_t L, int32_t heads,
+                       const int32_t* key_lens_host, int32_t seqs_per_chunk, void* stream) {
   if (!c || !q_dev || !k_dev || !v_dev || !gates_dev || !o_dev) return fail(c, BT_ERR_ARG, "bt_debug_attention: null argument");
   if (seqs < 1 || L < 1 || heads < 1 || (key_lens_host && (seqs_per_chunk < 1 || seqs % seqs_per_chunk != 0)))
     return fail(c, BT_ERR_ARG, "bt_debug_attention: bad geometry");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  BT_CUDA(c, cudaSetDevice(c->device));
   const int C = heads * 32;
   const int64_t M = static_cast<int64_t>(seqs) * L;
-  const bool tc = c->dtype == BT_DTYPE_H16;
-  const size_t act = tc ? 2 : 4;
+  if (o_count < M * C) return fail(c, BT_ERR_ARG, "bt_debug_attention: o holds %lld elements, fewer than M * C",
+                                   static_cast<long long>(o_count));
   // per-chunk key counts travel in the ChunkSrc table the forward pass hands the kernels (only .len is read)
   std::vector<ChunkSrc> chunks;
   if (key_lens_host) {
@@ -1490,10 +1488,14 @@ int bt_debug_attention(bt_ctx* c, const float* q_dev, const float* k_dev, const 
       chunks[i].len = key_lens_host[i];
     }
   }
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  BT_CUDA(c, cudaSetDevice(c->device));
+  const bool tc = c->dtype == BT_DTYPE_H16;
+  const size_t act = tc ? 2 : 4;
   DeviceBuffer<> qkv, o;
   DeviceBuffer<ChunkSrc> chunks_dev;
   BT_CUDA(c, qkv.alloc(M * 3 * C * act));
-  BT_CUDA(c, o.alloc(M * C * act));
+  if (tc) BT_CUDA(c, to_h16_operand(o, o_dev, o_count, st));  // elements the kernel does not store survive the round trip
   if (key_lens_host) {
     const size_t bytes = chunks.size() * sizeof(ChunkSrc);
     BT_CUDA(c, chunks_dev.alloc(bytes));
@@ -1507,7 +1509,7 @@ int bt_debug_attention(bt_ctx* c, const float* q_dev, const float* k_dev, const 
     if (!p) rc = fail(c, BT_ERR_CUDA, "%s", err);
     else {
       launch_attn_time_tc(p.get(), gates_dev, o.get(), st, chunks_dev.get(), seqs_per_chunk);
-      launch_h16_to_f32(o.get(), o_dev, M * C, st);
+      launch_h16_to_f32(o.get(), o_dev, o_count, st);
     }
     const cudaError_t se = cudaStreamSynchronize(st);
     if (rc == BT_OK && se != cudaSuccess) rc = fail(c, BT_ERR_CUDA, "tc attention: %s", cudaGetErrorString(se));
@@ -1523,15 +1525,17 @@ int bt_debug_attention(bt_ctx* c, const float* q_dev, const float* k_dev, const 
 }
 
 int bt_debug_attention_freq(bt_ctx* c, const float* q_dev, const float* k_dev, const float* v_dev,
-                            const float* gates_dev, float* o_dev, int32_t B, int32_t F, int32_t L, int32_t heads,
-                            void* stream) {
+                            const float* gates_dev, float* o_dev, int64_t o_count, int32_t B, int32_t F, int32_t L,
+                            int32_t heads, void* stream) {
   if (!c || !q_dev || !k_dev || !v_dev || !gates_dev || !o_dev) return fail(c, BT_ERR_ARG, "bt_debug_attention_freq: null argument");
   if (B < 1 || L < 1 || heads < 1 || (F != 8 && F != 16 && F != 32))
     return fail(c, BT_ERR_ARG, "bt_debug_attention_freq: need B, L, heads >= 1 and F in {8, 16, 32}");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  BT_CUDA(c, cudaSetDevice(c->device));
   const int C = heads * 32;
   const int64_t M = static_cast<int64_t>(B) * F * L;
+  if (o_count < M * C) return fail(c, BT_ERR_ARG, "bt_debug_attention_freq: o holds %lld elements, fewer than M * C",
+                                   static_cast<long long>(o_count));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  BT_CUDA(c, cudaSetDevice(c->device));
   const bool tc = c->dtype == BT_DTYPE_H16;
   const size_t act = tc ? 2 : 4;
   const float inv_sqrt_d = 0.17677669529663687f;
@@ -1539,15 +1543,16 @@ int bt_debug_attention_freq(bt_ctx* c, const float* q_dev, const float* k_dev, c
   FreqPlan p;
   BT_CUDA(c, qkv.alloc(M * 3 * C * act));
   if (tc) {
-    BT_CUDA(c, o.alloc(M * C * act));
+    BT_CUDA(c, o.alloc(o_count * act));
     char err[512] = "";
     p.reset(tc_freq_plan_create(qkv.get(), o.get(), B, F, L, heads, err, sizeof(err)));
     if (!p) return fail(c, BT_ERR_ARG, "bt_debug_attention_freq: %s", err);
+    launch_f32_to_h16(o_dev, o.get(), o_count, st);  // elements the kernel does not store survive the round trip
   }
   launch_pack_qkv_test(q_dev, k_dev, v_dev, qkv.get(), B * F, L, heads, 1.0f, tc ? 1 : 0, st);
   if (tc) {
     launch_attn_freq_tc(p.get(), gates_dev, inv_sqrt_d, st);
-    launch_h16_to_f32(o.get(), o_dev, M * C, st);
+    launch_h16_to_f32(o.get(), o_dev, o_count, st);
   } else {
     launch_attn_freq_simt(static_cast<const float*>(qkv.get()), gates_dev, o_dev, B, F, L, heads, inv_sqrt_d, st);
   }

@@ -435,27 +435,31 @@ class Engine:
         _lib.check(self.lib, self.ctx, code)
         return int(tile[0]), int(tile[1])
 
-    def debug_attention(self, q, k, v, gates=None, key_lens=None, seqs_per_chunk=1):
+    def debug_attention(self, q, k, v, gates=None, key_lens=None, seqs_per_chunk=1, out=None):
         """gates * SDPA through the time-direction attention kernel; q/k/v [seqs, L, heads*32], gates [seqs*L, heads]
-        (None: ones); key_lens: keys per chunk of seqs_per_chunk sequences (None: all L)."""
+        (None: ones); key_lens: keys per chunk of seqs_per_chunk sequences (None: all L).  out: an fp32 device tensor
+        of at least seqs*L*heads*32 elements (None: a new one shaped like q), written in place: the first
+        seqs*L*heads*32 elements are the output, the rest keep their values.  Returns out."""
         seqs, L, C = q.shape
         if gates is None:
             gates = torch.ones(seqs * L, C // 32, dtype=torch.float32, device=self.device)
-        o = torch.empty_like(q)
+        o = torch.empty_like(q) if out is None else out
+        p = self._dev_ptr
         lens = (ctypes.c_int32 * len(key_lens))(*[int(x) for x in key_lens]) if key_lens is not None else None
-        code = self.lib.bt_debug_attention(self.ctx, c_void_p(q.data_ptr()), c_void_p(k.data_ptr()), c_void_p(v.data_ptr()),
-                                           c_void_p(gates.data_ptr()), c_void_p(o.data_ptr()), seqs, L, C // 32, lens,
-                                           seqs_per_chunk, self._stream())
+        code = self.lib.bt_debug_attention(self.ctx, p(q, q.numel()), p(k, q.numel()), p(v, q.numel()),
+                                           p(gates, seqs * L * (C // 32)), p(o, q.numel()), o.numel(), seqs, L, C // 32,
+                                           lens, seqs_per_chunk, self._stream())
         _lib.check(self.lib, self.ctx, code)
         return o
 
-    def debug_attention_freq(self, q, k, v, gates, B, F):
-        """gates * softmax over the F planes of each (chunk, frame, head); q/k/v [B*F*L, heads*32], gates [B*F*L, heads]."""
+    def debug_attention_freq(self, q, k, v, gates, B, F, out=None):
+        """gates * softmax over the F planes of each (chunk, frame, head); q/k/v [B*F*L, heads*32], gates [B*F*L, heads].
+        out as for debug_attention (None: a new tensor shaped like q).  Returns out."""
         M, C = q.shape
-        o = torch.empty_like(q)
-        code = self.lib.bt_debug_attention_freq(self.ctx, c_void_p(q.data_ptr()), c_void_p(k.data_ptr()), c_void_p(v.data_ptr()),
-                                                c_void_p(gates.data_ptr()), c_void_p(o.data_ptr()), B, F, M // (B * F), C // 32,
-                                                self._stream())
+        o = torch.empty_like(q) if out is None else out
+        p = self._dev_ptr
+        code = self.lib.bt_debug_attention_freq(self.ctx, p(q, M * C), p(k, M * C), p(v, M * C), p(gates, M * (C // 32)),
+                                                p(o, M * C), o.numel(), B, F, M // (B * F), C // 32, self._stream())
         _lib.check(self.lib, self.ctx, code)
         return o
 

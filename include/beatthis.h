@@ -416,22 +416,26 @@ int bt_debug_gemm(bt_ctx* ctx, const bt_debug_gemm_desc* desc, const float* a_de
                   void* stream);
 
 /* Test hook: gates * softmax(Q K^T / sqrt(32)) V for `seqs` sequences of length L and `heads` heads of dim 32
- * through the ctx's time-direction attention kernel.  q/k/v/o_dev are [seqs, L, heads*32] fp32, gates_dev
- * [seqs * L, heads] fp32.  key_lens_host (optional): sequence s belongs to chunk s / seqs_per_chunk and attends to
- * the first key_lens_host[chunk] keys only (1 <= len <= L), as in a wave of chunks of different lengths.
+ * through the ctx's time-direction attention kernel.  q/k/v_dev are [seqs, L, heads*32] fp32, gates_dev
+ * [seqs * L, heads] fp32.  o_dev holds o_count >= seqs * L * heads * 32 fp32 elements, the first seqs * L * heads * 32
+ * of them the output; the 16-bit context runs all o_count elements through its activation type around the launch,
+ * so values the kernel does not store survive.  key_lens_host (optional): sequence s belongs to chunk
+ * s / seqs_per_chunk and attends to the first key_lens_host[chunk] keys only (1 <= len <= L), as in a wave of chunks
+ * of different lengths.  Returns BT_ERR_ARG, before anything is enqueued, for a bad geometry or o_count.
  * Synchronises the stream. */
 int bt_debug_attention(bt_ctx* ctx, const float* q_dev, const float* k_dev, const float* v_dev,
-                       const float* gates_dev, float* o_dev, int32_t seqs, int32_t L, int32_t heads,
+                       const float* gates_dev, float* o_dev, int64_t o_count, int32_t seqs, int32_t L, int32_t heads,
                        const int32_t* key_lens_host, int32_t seqs_per_chunk, void* stream);
 
 /* Test hook: the frequency-direction attention of B chunks of F planes of L frames: token m = (b * F + f) * L + t
  * attends over the F tokens of its (b, t), gates * softmax(q k^T / sqrt(32)) v per head.  q/k/v/o_dev are
- * [B * F * L, heads * 32] fp32, gates_dev [B * F * L, heads]; F in {8, 16, 32}.  The 16-bit context runs the
- * tensor-core kernel of the frontend blocks and returns BT_ERR_ARG for any pair other than (F, heads) = (32, 1),
- * (16, 2), (8, 4).  Synchronises the stream. */
+ * [B * F * L, heads * 32] fp32, gates_dev [B * F * L, heads]; F in {8, 16, 32}.  o_dev holds o_count >= B * F * L *
+ * heads * 32 elements, as for bt_debug_attention.  The 16-bit context runs the tensor-core kernel of the frontend
+ * blocks and returns BT_ERR_ARG for any pair other than (F, heads) = (32, 1), (16, 2), (8, 4).  Synchronises the
+ * stream. */
 int bt_debug_attention_freq(bt_ctx* ctx, const float* q_dev, const float* k_dev, const float* v_dev,
-                            const float* gates_dev, float* o_dev, int32_t B, int32_t F, int32_t L, int32_t heads,
-                            void* stream);
+                            const float* gates_dev, float* o_dev, int64_t o_count, int32_t B, int32_t F, int32_t L,
+                            int32_t heads, void* stream);
 
 /* Test hooks of the frontend's row kernels.  Every *_dev pointer is fp32 on the device; x, wg, b1 and b2 must be
  * 16-byte aligned, and so must xn of bt_debug_norm in the fp32 context (the kernel stores it directly).  The 16-bit context rounds the 16-bit operands (wqkv, w1, w2, o, wout) to its activation type

@@ -155,8 +155,9 @@ def rope(t, freqs):
     return t * ang.cos() + rot * ang.sin()
 
 
-def attention(x, sd, p, heads, explicit=False):
-    """roformer.py:114-132 (+ Attend :73-80).  x [S, n, dim] -> [S, n, dim] (no residual)."""
+def pre_attention(x, sd, p, heads):
+    """roformer.py:114-125: the attention's inputs on x [S, n, dim]: roped q and k, v [S, h, n, d] and the gate
+    logits [S, n, h] (before the sigmoid)."""
     xn = rmsnorm(x, sd[p + ".norm.gamma"])
     qkv = xn @ sd[p + ".to_qkv.weight"].T
     S, n, _ = x.shape
@@ -167,12 +168,19 @@ def attention(x, sd, p, heads, explicit=False):
         d = q.shape[-1]
         freqs = 1.0 / (10000 ** (torch.arange(0, d, 2).float() / d))
     q, k = rope(q, freqs), rope(k, freqs)
+    gates = xn @ sd[p + ".to_gates.weight"].T + sd[p + ".to_gates.bias"]  # [S, n, h]
+    return q, k, v, gates
+
+
+def attention(x, sd, p, heads, explicit=False):
+    """roformer.py:114-132 (+ Attend :73-80).  x [S, n, dim] -> [S, n, dim] (no residual)."""
+    q, k, v, gates = pre_attention(x, sd, p, heads)
+    S, n, _ = x.shape
     if explicit:
         s = (q @ k.transpose(-1, -2)) / math.sqrt(q.shape[-1])
         out = torch.softmax(s, dim=-1) @ v
     else:
         out = F.scaled_dot_product_attention(q, k, v)
-    gates = xn @ sd[p + ".to_gates.weight"].T + sd[p + ".to_gates.bias"]  # [S, n, h]
     out = out * gates.permute(0, 2, 1).unsqueeze(-1).sigmoid()
     out = out.permute(0, 2, 1, 3).reshape(S, n, -1)
     return out @ sd[p + ".to_out.0.weight"].T

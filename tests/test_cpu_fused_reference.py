@@ -38,18 +38,14 @@ def _layer(packed, prefix, C):
 
 
 def _oracle_pre_attention(z, sd, p, heads):
-    """The part of oracle.attention in front of the softmax on z [S, n, C]: roped q and k, v [S, n, C] and the gates
-    [S, n, heads] (after the sigmoid)."""
+    """oracle.pre_attention on z [S, n, C]: roped q and k, v [S, n, C] and the gates [S, n, heads] (after the
+    sigmoid)."""
     from oracle import beat_this_oracle as O
 
-    xn = O.rmsnorm(z, sd[p + ".norm.gamma"])
     S, n, C = z.shape
-    qkv = (xn @ sd[p + ".to_qkv.weight"].T).view(S, n, 3, heads, -1).permute(2, 0, 3, 1, 4)
-    freqs = sd[p + ".rotary_embed.freqs"]
-    q, k, v = O.rope(qkv[0], freqs), O.rope(qkv[1], freqs), qkv[2]
+    q, k, v, gates = O.pre_attention(z, sd, p, heads)
     back = lambda t: t.permute(0, 2, 1, 3).reshape(S, n, C)
-    gates = torch.sigmoid(xn @ sd[p + ".to_gates.weight"].T + sd[p + ".to_gates.bias"])
-    return back(q), back(k), back(v), gates
+    return back(q), back(k), back(v), torch.sigmoid(gates)
 
 
 @pytest.mark.parametrize("name", ["small0", "final0"])

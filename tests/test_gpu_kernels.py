@@ -124,7 +124,8 @@ def test_peakpick_golden_bit_exact(lib_built, dev):
         assert np.array_equal(res[i][1], g[f"down_times_{i}"]), i
 
 
-# ------------------------------------------------------------------------------ GEMM / attention units
+# ------------------------------------------------------------------------------ GEMM units
+# (the attention kernels: tests/test_gpu_attention.py)
 # GEMM unit tolerances (bt_debug_gemm against the float64 reference of tests/gemm_reference.py, on the operands the
 # kernel multiplies: rounded to the 16-bit type in the 16-bit context):
 #   fp32 outputs  : fp32 accumulation over K <= 2048 of unit-scale products, |ref| ~ 1:
@@ -253,80 +254,6 @@ def _check_gemm_case(eng, half, case):
             check(f"{eng.act_dtype} out", got, ref16, _ulp(ref16, adt) + tol)
         else:
             check("act out (fp32)", got, ref, tol)
-
-
-ATTN_CASES = [
-    # (seqs, L, heads, keys per chunk or None, seqs_per_chunk, gated)
-    (3, 1500, 2, None, 1, False),
-    (2, 200, 1, None, 1, False),
-    (1, 13, 4, None, 1, False),
-    (2, 128, 1, None, 1, False),
-    (1, 129, 1, None, 1, False),
-    (2, 1500, 16, None, 1, True),                            # main layers: 16 heads of a 1500-frame chunk
-    (7, 1500, 16, [1, 13, 63, 64, 65, 150, 1500], 1, True),  # a wave of chunks of different lengths, main layers
-    (96, 150, 1, [150, 65, 13], 32, True),                   # frontend time attention: F = 32 planes per chunk
-    (64, 1500, 1, [1500, 64], 32, True),
-]
-MASKED_KV = 3e4  # keys / values a chunk does not have: large enough that any leak through the mask is visible
-
-
-@pytest.mark.parametrize("half", [False, True])
-def test_debug_attention(small_f32, small_h16, half):
-    """gates * SDPA (float64, key mask per chunk) through the time-direction attention kernel.  Every case runs and
-    prints its error; the failing ones are listed together at the end."""
-    eng = (small_h16 if half else small_f32).engine
-    failures = []
-    for case in ATTN_CASES:
-        try:
-            _check_attention_case(eng, half, case)
-        except AssertionError as e:
-            failures.append(f"{case}: {str(e).splitlines()[0]}")
-    assert not failures, f"{len(failures)} of {len(ATTN_CASES)} attention cases failed:\n" + "\n".join(failures)
-
-
-def _check_attention_case(eng, half, case):
-    seqs, L, heads, key_lens, spc, gated = case
-    g = torch.Generator(device="cpu").manual_seed(2)
-    q = torch.randn(seqs, L, heads * 32, generator=g) * 1.5
-    k = torch.randn(seqs, L, heads * 32, generator=g)
-    v = torch.randn(seqs, L, heads * 32, generator=g)
-    gates = torch.rand(seqs * L, heads, generator=g) if gated else torch.ones(seqs * L, heads)
-    lens = torch.tensor([key_lens[s // spc] for s in range(seqs)] if key_lens else [L] * seqs)
-    valid = torch.arange(L)[None, :] < lens[:, None]  # [seqs, L]: keys (and query rows) a chunk has
-    sign = torch.randint(0, 2, (seqs, L, heads * 32), generator=g) * 2 - 1
-    k = torch.where(valid[..., None], k, MASKED_KV * sign)
-    v = torch.where(valid[..., None], v, -MASKED_KV * sign)
-    sh = lambda t: t.view(seqs, L, heads, 32).permute(0, 2, 1, 3).double().cuda()
-    ref = torch.nn.functional.scaled_dot_product_attention(sh(q), sh(k), sh(v), attn_mask=valid[:, None, None, :].cuda())
-    ref = (ref.permute(0, 2, 1, 3) * gates.view(seqs, L, heads, 1).double().cuda()).reshape(seqs, L, -1)
-    o = eng.debug_attention(q.cuda(), k.cuda(), v.cuda(), gates.cuda(), key_lens, spc).double()
-    err = (o - ref).abs()[valid.cuda()].max().item()
-    print(f"attention half={half} seqs={seqs} L={L} heads={heads} keys={key_lens} per {spc} gated={gated}: "
-          f"max abs err {err:.3e}")
-    assert err < (5e-3 if half else 1e-4), f"max abs err {err:.3e}"
-
-
-@pytest.mark.parametrize("half", [False, True])
-def test_debug_attention_freq(small_f32, small_h16, half):
-    """gates * softmax over the F planes of each (chunk, frame, head) in float64 against the frequency attention: the
-    production (F, heads) pairs (tensor-core kernel in the 16-bit context), frame counts around its 4-frame tiles."""
-    eng = (small_h16 if half else small_f32).engine
-    g = torch.Generator(device="cpu").manual_seed(5)
-    for F, heads in ((32, 1), (16, 2), (8, 4)):
-        for L in (1, 3, 4, 5, 13, 1500):
-            for B in (1, 3):
-                M, C = B * F * L, heads * 32
-                q = torch.randn(M, C, generator=g) * 1.5
-                k = torch.randn(M, C, generator=g)
-                v = torch.randn(M, C, generator=g)
-                gates = torch.rand(M, heads, generator=g)
-                sh = lambda t: t.view(B, F, L, heads, 32).permute(0, 2, 3, 1, 4).double().cuda()  # [B, L, heads, F, 32]
-                ref = torch.nn.functional.scaled_dot_product_attention(sh(q), sh(k), sh(v)).permute(0, 3, 1, 2, 4)
-                ref = (ref * gates.view(B, F, L, heads, 1).double().cuda()).reshape(M, C)
-                o = eng.debug_attention_freq(q.cuda(), k.cuda(), v.cuda(), gates.cuda(), B, F).double()
-                err = (o - ref).abs().max().item()
-                print(f"attention_freq half={half} F={F} heads={heads} L={L} B={B}: max abs err {err:.3e}")
-                assert err < (5e-3 if half else 1e-4), (F, heads, L, B)
 
 
 @pytest.mark.parametrize("sr", [44100, 48000, 16000, 96000])
