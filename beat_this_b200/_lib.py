@@ -101,6 +101,22 @@ class bt_loss_params(ctypes.Structure):
     ]
 
 
+BT_MEL_NORM_NONE = 0
+BT_MEL_NORM_FRAME_LENGTH = 1
+BT_MEL_NORM_WINDOW = 2
+
+
+class bt_mel_config(ctypes.Structure):
+    _fields_ = [
+        ("n_fft", c_int32),
+        ("hop_length", c_int32),
+        ("n_mels", c_int32),
+        ("norm_mode", c_int32),
+        ("power", c_float),
+        ("log_multiplier", c_float),
+    ]
+
+
 # every symbol include/beatthis.h declares: name -> (restype, argtypes)
 PROTOTYPES = {
     "bt_version": (c_int, []),
@@ -116,6 +132,11 @@ PROTOTYPES = {
         c_int64, [c_int64, POINTER(bt_chunking), POINTER(c_int64), POINTER(c_int64), POINTER(c_int64), POINTER(c_int64), c_int64],
     ),
     "bt_logmel": (c_int, [c_void_p, c_void_p, POINTER(c_int64), c_int32, c_void_p, POINTER(c_int64), c_void_p]),
+    "bt_logmel_config": (
+        c_int,
+        [c_void_p, POINTER(bt_mel_config), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int64),
+         c_int32, c_void_p, POINTER(c_int64), c_void_p],
+    ),
     "bt_stage_audio": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_int32]),
     "bt_wav_probe": (c_int, [c_char_p, POINTER(bt_wav_info)]),
     "bt_stage_wav_files": (c_int, [c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_int32, c_void_p]),

@@ -909,6 +909,52 @@ int bt_logmel(bt_ctx* c, const float* audio_dev, const int64_t* sample_offsets_h
   return BT_OK;
 }
 
+int bt_logmel_config(bt_ctx* c, const bt_mel_config* cfg, const float* window_dev, const float* twiddle_dev,
+                     const int32_t* fb_start_dev, const int32_t* fb_ptr_dev, const float* fb_w_dev,
+                     const float* audio_dev, const int64_t* sample_offsets_host, int32_t n_clips,
+                     float* spect_dev, const int64_t* frame_offsets_host, void* stream) {
+  static const char* fn = "bt_logmel_config";
+  if (!c) return BT_ERR_ARG;
+  if (!cfg) return fail(c, BT_ERR_ARG, "%s: null config", fn);
+  int log2n = 6;
+  while (log2n < 13 && (1 << log2n) != cfg->n_fft) ++log2n;
+  if ((1 << log2n) != cfg->n_fft)
+    return fail(c, BT_ERR_ARG, "%s: n_fft %d is not a power of two in [64, 8192]", fn, cfg->n_fft);
+  if (cfg->hop_length < 1 || cfg->n_mels < 1 || cfg->n_mels > 1024)
+    return fail(c, BT_ERR_ARG, "%s: need hop_length >= 1 and 1 <= n_mels <= 1024", fn);
+  if (cfg->norm_mode < BT_MEL_NORM_NONE || cfg->norm_mode > BT_MEL_NORM_WINDOW)
+    return fail(c, BT_ERR_ARG, "%s: unknown norm_mode %d", fn, cfg->norm_mode);
+  if (!std::isfinite(cfg->power) || !(cfg->power > 0.f) || !std::isfinite(cfg->log_multiplier))
+    return fail(c, BT_ERR_ARG, "%s: need a finite power > 0 and a finite log_multiplier", fn);
+  if (n_clips < 0) return fail(c, BT_ERR_ARG, "%s: negative clip count", fn);
+  if (n_clips == 0) return BT_OK;
+  if (!window_dev || !twiddle_dev || !fb_start_dev || !fb_ptr_dev || !fb_w_dev || !audio_dev || !sample_offsets_host ||
+      !spect_dev || !frame_offsets_host)
+    return fail(c, BT_ERR_ARG, "%s: null argument", fn);
+  if (sample_offsets_host[0] < 0 || frame_offsets_host[0] != 0)
+    return fail(c, BT_ERR_ARG, "%s: sample offsets must start at >= 0 and frame offsets at 0", fn);
+  for (int i = 0; i < n_clips; ++i) {
+    const int64_t len = sample_offsets_host[i + 1] - sample_offsets_host[i];
+    if (len <= cfg->n_fft / 2)
+      return fail(c, BT_ERR_ARG, "%s: clip %d has %lld samples; reflect padding needs more than %d (torch.stft raises "
+                  "for such input as well)", fn, i, (long long)len, cfg->n_fft / 2);
+    if (frame_offsets_host[i + 1] - frame_offsets_host[i] != 1 + len / cfg->hop_length)
+      return fail(c, BT_ERR_ARG, "%s: frame_offsets do not match 1 + len/%d for clip %d", fn, cfg->hop_length, i);
+  }
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  BT_CUDA(c, cudaSetDevice(c->device));
+  prof_mark(c, st);
+  const size_t n = n_clips + 1;
+  const int64_t* d[2];
+  const int r = stage(c, st, {{sample_offsets_host, n}, {frame_offsets_host, n}}, d);
+  if (r != BT_OK) return r;
+  const MelConfigArgs args{window_dev, twiddle_dev, fb_start_dev, fb_ptr_dev, fb_w_dev, spect_dev,
+                           cfg->hop_length, cfg->n_mels, cfg->norm_mode, cfg->power, cfg->log_multiplier};
+  BT_CUDA(c, launch_logmel_config(log2n, audio_dev, d[0], d[1], n_clips, frame_offsets_host[n_clips], args, st));
+  BT_LAUNCHED(c, "logmel_config", st);
+  return BT_OK;
+}
+
 int bt_resample(bt_ctx* c, const float* audio_in_dev, const int64_t* in_offsets_host, int32_t n_clips,
                 const float* coef_dev, int32_t L, int32_t M, int32_t K, float* audio_out_dev,
                 const int64_t* out_offsets_host, void* stream) {

@@ -90,6 +90,20 @@ void launch_logmel(const float* audio, const int64_t* sample_off_dev, const int6
                    int n_clips, int64_t max_frames, const float* window, const float* twiddle,
                    const int32_t* fb_start, const int32_t* fb_ptr, const float* fb_w, float* spect,
                    cudaStream_t st);
+// bt_logmel_config's tables, output and scalars (kernels_misc.cu logmel_config_kernel); norm_mode as bt_mel_config
+struct MelConfigArgs {
+  const float* window;
+  const float* twiddle;
+  const int32_t* fb_start;
+  const int32_t* fb_ptr;
+  const float* fb_w;
+  float* spect;
+  int hop, n_mels, norm_mode;
+  float power, log_multiplier;
+};
+cudaError_t launch_logmel_config(int log2n, const float* audio, const int64_t* sample_off_dev,
+                                 const int64_t* frame_off_dev, int n_clips, int64_t total_frames,
+                                 const MelConfigArgs& p, cudaStream_t st);
 void launch_peakpick(const float* beat, const float* down, const int64_t* frame_off_dev, int n_clips,
                      double* beat_t, int32_t* n_beat, double* down_t, int32_t* n_down,
                      int max_peaks, cudaStream_t st);

@@ -1,6 +1,7 @@
 // HBM-bound kernels of the path: log-mel frontend, stem conv, RMSNorm(+gates),
 // frequency-direction attention, head + aggregation scatter, peak picking.
 #include <cuda_fp16.h>
+#include <algorithm>
 #include <cstdio>
 #include <cstdlib>
 
@@ -149,6 +150,217 @@ void launch_logmel(const float* audio, const int64_t* sample_off_dev, const int6
   dim3 grid(static_cast<unsigned>((max_frames + 1) / 2), static_cast<unsigned>(n_clips));
   logmel_kernel<<<grid, 128, 0, st>>>(audio, sample_off_dev, frame_off_dev, window,
                                       reinterpret_cast<const float2*>(twiddle), fb_start, fb_ptr, fb_w, spect);
+}
+
+// ------------------------------------------------------------------------------------------
+// General log-mel (bt_logmel_config, contract in include/beatthis.h): STFT with any power-of-two n_fft = N in
+// [64, 8192] and any hop -> |.|^power -> CSR mel filterbank -> log1p(log_multiplier x).
+// Algorithmic HBM bytes: hop new samples * 4 B read + n_mels * 4 B written per frame.
+//
+// As in logmel_kernel, the real N-point transform is one complex H = N/2-point FFT of z[n] = x[2n] + i x[2n+1] and the
+// untangling step.  The complex FFT is a Stockham autosort FFT: radix-8 passes while 8 divides what is left, then one
+// radix-4 or radix-2 pass.  The pass of radix R after the passes whose radices multiply to Ns has butterflies
+// j < H/R: read a[j + r H/R] (r < R), multiply by e^{-2 pi i (j mod Ns) r / (Ns R)}, take a DFT_R and write
+// a[(j - j mod Ns) R + j mod Ns + r Ns].  After the last pass Z is in natural order.  Every thread holds eight points
+// in registers per pass (one radix-8, two radix-4 or four radix-2 butterflies), so TPF = H/8 threads work on a frame
+// and one buffer suffices: a __syncthreads separates each pass's reads from its writes.  Buffer index i is stored at
+// i + i/8: the first pass writes with a stride of 8 points, which the padding spreads over all banks.
+// A CTA of max(256, TPF) threads transforms FPC = threads / TPF consecutive frames of the batch's frames flattened
+// over all clips (a frame finds its clip by binary search of frame_off; a CTA may span clips) and loops over frame
+// groups grid-stride.  Twiddles e^{-2 pi i j / N} (j < N/2) come from the caller's table through the read-only cache.
+// ------------------------------------------------------------------------------------------
+template <int LOG2N>
+struct MelGeom {
+  static constexpr int N = 1 << LOG2N, H = N / 2, TPF = H / 8;
+  static constexpr int THREADS = TPF > 256 ? TPF : 256, FPC = THREADS / TPF;
+  static constexpr int PITCH = H + H / 8;  // float2 per frame in the FFT buffer
+  static constexpr size_t SPEC_OFF = size_t(FPC) * PITCH * sizeof(float2);  // bytes; FPC x (H + 1) floats follow
+  static constexpr size_t RED_OFF = (SPEC_OFF + size_t(FPC) * (H + 1) * sizeof(float) + 7) / 8 * 8;  // 32 doubles
+  static constexpr size_t SMEM = RED_OFF + 32 * sizeof(double);
+};
+
+__device__ __forceinline__ int mel_pad(int i) { return i + (i >> 3); }
+
+template <int N>
+__device__ __forceinline__ float2 mel_tw(const float2* __restrict__ tw, int j) {  // e^{-2 pi i j / N}, 0 <= j <= N/2
+  const float2 w = __ldg(tw + (j & (N / 2 - 1)));
+  return (j & (N / 2)) ? make_float2(-w.x, -w.y) : w;
+}
+
+__device__ __forceinline__ void dft4(float2& a0, float2& a1, float2& a2, float2& a3) {
+  const float2 s0 = cadd(a0, a2), s1 = csub(a0, a2), s2 = cadd(a1, a3), s3 = cmul_mi(csub(a1, a3));
+  a0 = cadd(s0, s2); a2 = csub(s0, s2); a1 = cadd(s1, s3); a3 = csub(s1, s3);
+}
+
+// twiddles, DFT_R and stores of the thread's 8 / R butterflies j = lt + b TPF of the pass after Ns points
+template <int R, int LOG2N>
+__device__ __forceinline__ void mel_pass_store(float2* __restrict__ a, float2 (&v)[8], int lt, int Ns,
+                                               const float2* __restrict__ tw) {
+  using G = MelGeom<LOG2N>;
+#pragma unroll
+  for (int b = 0; b < 8 / R; ++b) {
+    const int j = lt + b * G::TPF, k = j & (Ns - 1);
+    const int step = G::N / (Ns * R);  // e^{-2 pi i k r / (Ns R)} = e^{-2 pi i k r step / N}
+#pragma unroll
+    for (int r = 1; r < R; ++r) v[b * R + r] = cmul(v[b * R + r], mel_tw<G::N>(tw, k * r * step));
+    if constexpr (R == 8) {
+      dft8(v);
+    } else if constexpr (R == 4) {
+      dft4(v[4 * b], v[4 * b + 1], v[4 * b + 2], v[4 * b + 3]);
+    } else {
+      const float2 t = v[2 * b];
+      v[2 * b] = cadd(t, v[2 * b + 1]);
+      v[2 * b + 1] = csub(t, v[2 * b + 1]);
+    }
+    const int d = (j - k) * R + k;
+#pragma unroll
+    for (int r = 0; r < R; ++r) a[mel_pad(d + r * Ns)] = v[b * R + r];
+  }
+}
+
+template <int R, int LOG2N>
+__device__ __forceinline__ void mel_pass_load(const float2* __restrict__ a, float2 (&v)[8], int lt) {
+  using G = MelGeom<LOG2N>;
+#pragma unroll
+  for (int b = 0; b < 8 / R; ++b)
+#pragma unroll
+    for (int r = 0; r < R; ++r) v[b * R + r] = a[mel_pad(lt + b * G::TPF + r * (G::H / R))];
+}
+
+template <int LOG2N>
+__global__ void __launch_bounds__(MelGeom<LOG2N>::THREADS)
+logmel_config_kernel(const float* __restrict__ audio, const int64_t* __restrict__ sample_off,
+                     const int64_t* __restrict__ frame_off, int n_clips, int64_t total_frames, MelConfigArgs p) {
+  using G = MelGeom<LOG2N>;
+  constexpr int N = G::N, H = G::H, TPF = G::TPF, FPC = G::FPC, THREADS = G::THREADS;
+  constexpr int LOG2H = LOG2N - 1, N8 = LOG2H / 3, REM = LOG2H % 3;
+  extern __shared__ float4 mel_smem4[];
+  unsigned char* const smem = reinterpret_cast<unsigned char*>(mel_smem4);
+  float2* const fft = reinterpret_cast<float2*>(smem);
+  float* const spec = reinterpret_cast<float*>(smem + G::SPEC_OFF);
+  double* const red = reinterpret_cast<double*>(smem + G::RED_OFF);
+  const float2* __restrict__ tw = reinterpret_cast<const float2*>(p.twiddle);
+  const int tid = threadIdx.x, fl = tid / TPF, lt = tid % TPF;
+
+  float scale = p.norm_mode == 1 ? rsqrtf(static_cast<float>(N)) : 1.f;
+  if (p.norm_mode == 2) {  // 1 / sqrt(sum window^2), summed in float64 in a fixed order
+    double s = 0.0;
+    for (int i = tid; i < N; i += THREADS) s += static_cast<double>(p.window[i]) * p.window[i];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if ((tid & 31) == 0) red[tid >> 5] = s;
+    __syncthreads();
+    s = 0.0;
+    for (int w = 0; w < THREADS / 32; ++w) s += red[w];
+    scale = static_cast<float>(1.0 / sqrt(s));
+  }
+
+  float2* const a = fft + fl * G::PITCH;
+  float* const sp = spec + fl * (H + 1);
+  for (int64_t g0 = static_cast<int64_t>(blockIdx.x) * FPC; g0 < total_frames; g0 += static_cast<int64_t>(gridDim.x) * FPC) {
+    const int64_t g = g0 + fl;
+    float2 v[8];
+    if (g < total_frames) {
+      int lo = 0, hi = n_clips;  // frame_off[lo] <= g < frame_off[hi]
+      while (hi - lo > 1) {
+        const int mid = (lo + hi) >> 1;
+        if (__ldg(frame_off + mid) <= g) lo = mid; else hi = mid;
+      }
+      const int64_t s0 = __ldg(sample_off + lo), len = __ldg(sample_off + lo + 1) - s0;
+      const int64_t base = (g - __ldg(frame_off + lo)) * p.hop - N / 2;
+#pragma unroll
+      for (int r = 0; r < 8; ++r) {  // first radix-8 pass: points z[lt + r H/8] straight from the clip
+        const int n = 2 * (lt + r * (H / 8));
+        float xs[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          int64_t i = base + n + e;
+          if (i < 0) i = -i;                    // reflect without repeating the edge, torch pad_mode="reflect";
+          if (i >= len) i = 2 * (len - 1) - i;  // len > N/2 makes one reflection enough
+          xs[e] = __ldg(audio + s0 + i) * __ldg(p.window + n + e);
+        }
+        v[r] = make_float2(xs[0], xs[1]);
+      }
+    } else {
+#pragma unroll
+      for (int r = 0; r < 8; ++r) v[r] = make_float2(0.f, 0.f);
+    }
+    mel_pass_store<8, LOG2N>(a, v, lt, 1, tw);
+    __syncthreads();
+#pragma unroll
+    for (int q = 1; q < N8; ++q) {
+      mel_pass_load<8, LOG2N>(a, v, lt);
+      __syncthreads();
+      mel_pass_store<8, LOG2N>(a, v, lt, 1 << (3 * q), tw);
+      __syncthreads();
+    }
+    if constexpr (REM != 0) {
+      constexpr int R = 1 << REM;
+      mel_pass_load<R, LOG2N>(a, v, lt);
+      __syncthreads();
+      mel_pass_store<R, LOG2N>(a, v, lt, 1 << (3 * N8), tw);
+      __syncthreads();
+    }
+    // untangle (as logmel_kernel): X[k] = E[k] + e^{-2 pi i k / N} O[k], bins 0..H, then (scale |X|)^power
+    for (int k = lt; k <= H; k += TPF) {
+      const float2 zk = a[mel_pad(k & (H - 1))], zc = a[mel_pad((H - k) & (H - 1))];
+      const float2 e = make_float2(0.5f * (zk.x + zc.x), 0.5f * (zk.y - zc.y));
+      const float2 o = make_float2(0.5f * (zk.y + zc.y), -0.5f * (zk.x - zc.x));
+      const float2 x = cadd(e, cmul(mel_tw<N>(tw, k), o));
+      const float m = sqrtf(x.x * x.x + x.y * x.y) * scale;
+      sp[k] = p.power == 1.f ? m : (p.power == 2.f ? m * m : powf(m, p.power));
+    }
+    __syncthreads();
+    // mel bands of the CTA's frames: consecutive threads write consecutive outputs
+    const int nm = p.n_mels;
+    for (int idx = tid; idx < FPC * nm; idx += THREADS) {
+      const int f = idx / nm, m = idx - f * nm;
+      if (g0 + f >= total_frames) break;
+      const int q0 = __ldg(p.fb_ptr + m), q1 = __ldg(p.fb_ptr + m + 1);
+      const float* s = spec + f * (H + 1) + __ldg(p.fb_start + m);
+      float acc = 0.f;
+      for (int q = q0; q < q1; ++q) acc = fmaf(s[q - q0], __ldg(p.fb_w + q), acc);
+      p.spect[(g0 + f) * nm + m] = log1pf(p.log_multiplier * acc);
+    }
+  }
+}
+
+template <int LOG2N>
+static cudaError_t launch_logmel_config_n(const float* audio, const int64_t* sample_off_dev, const int64_t* frame_off_dev,
+                                          int n_clips, int64_t total_frames, const MelConfigArgs& p, cudaStream_t st) {
+  using G = MelGeom<LOG2N>;
+  cudaError_t e = cudaFuncSetAttribute(logmel_config_kernel<LOG2N>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       static_cast<int>(G::SMEM));
+  if (e != cudaSuccess) return e;
+  static int max_ctas = 0;  // CTAs resident on the whole device at once: the grid-stride grid
+  if (max_ctas == 0) {
+    int dev = 0, sms = 0, per_sm = 0;
+    e = cudaGetDevice(&dev);
+    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    if (e == cudaSuccess)
+      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, logmel_config_kernel<LOG2N>, G::THREADS, G::SMEM);
+    if (e != cudaSuccess) return e;
+    max_ctas = std::max(1, sms * per_sm);
+  }
+  const int64_t groups = (total_frames + G::FPC - 1) / G::FPC;
+  const unsigned grid = static_cast<unsigned>(std::min<int64_t>(groups, max_ctas));
+  logmel_config_kernel<LOG2N><<<grid, G::THREADS, G::SMEM, st>>>(audio, sample_off_dev, frame_off_dev, n_clips,
+                                                                  total_frames, p);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_logmel_config(int log2n, const float* audio, const int64_t* sample_off_dev,
+                                 const int64_t* frame_off_dev, int n_clips, int64_t total_frames,
+                                 const MelConfigArgs& p, cudaStream_t st) {
+  if (n_clips <= 0 || total_frames <= 0) return cudaSuccess;
+  switch (log2n) {
+#define BT_MEL_CASE(L) \
+  case L: return launch_logmel_config_n<L>(audio, sample_off_dev, frame_off_dev, n_clips, total_frames, p, st);
+    BT_MEL_CASE(6) BT_MEL_CASE(7) BT_MEL_CASE(8) BT_MEL_CASE(9) BT_MEL_CASE(10) BT_MEL_CASE(11) BT_MEL_CASE(12)
+    BT_MEL_CASE(13)
+#undef BT_MEL_CASE
+    default: return cudaErrorInvalidValue;
+  }
 }
 
 // ------------------------------------------------------------------------------------------

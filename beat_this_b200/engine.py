@@ -152,10 +152,10 @@ class Engine:
 
     # ---- hot path ---------------------------------------------------------------------------
     @staticmethod
-    def frame_offsets(sample_offsets):
+    def frame_offsets(sample_offsets, hop: int = 441):
         fo = [0]
         for a, b in zip(sample_offsets[:-1], sample_offsets[1:]):
-            fo.append(fo[-1] + 1 + (int(b) - int(a)) // 441)
+            fo.append(fo[-1] + 1 + (int(b) - int(a)) // hop)
         return fo
 
     def resample_cat(self, audio: torch.Tensor, sample_offsets, sr: int, sr_out: int = 22050):
@@ -195,6 +195,29 @@ class Engine:
         for s in sigs:
             so.append(so[-1] + s.numel())
         spect, fo = self.logmel_cat(torch.cat(sigs) if len(sigs) > 1 else sigs[0], so)
+        return [spect[fo[i] : fo[i + 1]] for i in range(len(sigs))]
+
+    def logmel_config_cat(self, audio: torch.Tensor, sample_offsets, tables, device_tables: dict):
+        """bt_logmel_config on flat fp32 device audio for the analysis of ``tables`` (preprocessing.MelTables, whose
+        ``to(device)`` gave ``device_tables``): (spect [total_frames, n_mels], frame_offsets)."""
+        assert audio.is_cuda and audio.dtype == torch.float32 and audio.is_contiguous()
+        fo = self.frame_offsets(sample_offsets, tables.hop_length)
+        spect = torch.empty((fo[-1], tables.n_mels), dtype=torch.float32, device=self.device)
+        t = device_tables
+        code = self.lib.bt_logmel_config(
+            self.ctx, ctypes.byref(tables.config), c_void_p(t["window"].data_ptr()), c_void_p(t["twiddle"].data_ptr()),
+            c_void_p(t["fb_start"].data_ptr()), c_void_p(t["fb_ptr"].data_ptr()), c_void_p(t["fb_w"].data_ptr()),
+            c_void_p(audio.data_ptr()), i64_array(sample_offsets), len(sample_offsets) - 1, c_void_p(spect.data_ptr()),
+            i64_array(fo), self._stream())
+        _lib.check(self.lib, self.ctx, code)
+        return spect, fo
+
+    def logmel_config(self, signals, tables, device_tables: dict):
+        sigs = [torch.as_tensor(s, dtype=torch.float32, device=self.device).contiguous() for s in signals]
+        so = [0]
+        for s in sigs:
+            so.append(so[-1] + s.numel())
+        spect, fo = self.logmel_config_cat(torch.cat(sigs) if len(sigs) > 1 else sigs[0], so, tables, device_tables)
         return [spect[fo[i] : fo[i + 1]] for i in range(len(sigs))]
 
     def spect2frames_cat(self, spect: torch.Tensor, frame_offsets, chunking: tuple | None = None):

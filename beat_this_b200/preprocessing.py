@@ -1,8 +1,9 @@
 """Audio loading and the log-mel frontend (mirror of reference beat_this/preprocessing.py).
 
-``LogMelSpect`` keeps the reference's constructor defaults and call signature
-(preprocessing.py:27-59) but runs the fused sm_90a kernel (frame -> Hann -> 1024-point FFT
--> |.| -> 128-band slaney mel -> log1p(1000 x)) through ``bt_logmel``.
+``LogMelSpect`` keeps the reference's constructor and call signature (preprocessing.py:27-59).  At the
+reference defaults it runs the model path's fused sm_90a kernel (frame -> Hann -> 1024-point FFT -> |.| ->
+128-band slaney mel -> log1p(1000 x)) through ``bt_logmel``; any other analysis parameters run the general kernel
+through ``bt_logmel_config`` on the tables ``MelTables`` builds.
 ``load_audio`` (preprocessing.py:6-24) walks the reference's decoder chain (torchaudio, soundfile, madmom -- whichever
 is installed) and then two dependency-free WAV readers; the batched File2Beats path reads WAV files natively
 (``bt_stage_wav_files``) and only falls back to this function for other containers.
@@ -10,6 +11,7 @@ is installed) and then two dependency-free WAV readers; the batched File2Beats p
 from __future__ import annotations
 
 import math
+import numbers
 import wave
 
 import numpy as np
@@ -95,7 +97,9 @@ def load_audio(path, dtype="float64"):
 # ------------------------------------------------------------------------------------------
 
 
-def _hz_to_mel_slaney(freq: float) -> float:
+def _hz_to_mel(freq: float, mel_scale: str = "slaney") -> float:
+    if mel_scale == "htk":
+        return 2595.0 * math.log10(1.0 + (freq / 700.0))
     f_sp = 200.0 / 3
     mels = freq / f_sp
     min_log_hz = 1000.0
@@ -104,19 +108,26 @@ def _hz_to_mel_slaney(freq: float) -> float:
     return mels
 
 
-def mel_filterbank(n_freqs=N_FFT // 2 + 1, f_min=F_MIN, f_max=F_MAX, n_mels=N_MELS, sample_rate=SAMPLE_RATE):
-    """torchaudio.functional.melscale_fbanks(norm=None, mel_scale='slaney') restated with the
-    same fp32 torch ops so that the coefficients are bit-identical to what the reference's
-    MelSpectrogram holds (reference preprocessing.py:43-53)."""
+def mel_filterbank(n_freqs=N_FFT // 2 + 1, f_min=F_MIN, f_max=F_MAX, n_mels=N_MELS, sample_rate=SAMPLE_RATE,
+                   mel_scale="slaney"):
+    """torchaudio.functional.melscale_fbanks(norm=None) restated with the same fp32 torch ops, so that the
+    coefficients are bit-identical to what the reference's MelSpectrogram holds (reference preprocessing.py:43-53)
+    for either mel scale, any sample rate (the grid tops out at the integer ``sample_rate // 2``) and any band count.
+    ``ValueError`` for a mel_scale other than "slaney" / "htk", as torchaudio."""
+    if mel_scale not in ("slaney", "htk"):
+        raise ValueError('mel_scale should be one of "htk" or "slaney".')
     all_freqs = torch.linspace(0, sample_rate // 2, n_freqs)
-    m_pts = torch.linspace(_hz_to_mel_slaney(f_min), _hz_to_mel_slaney(f_max), n_mels + 2)
-    f_sp = 200.0 / 3
-    f_pts = f_sp * m_pts
-    min_log_hz = 1000.0
-    min_log_mel = min_log_hz / f_sp
-    logstep = math.log(6.4) / 27.0
-    log_t = m_pts >= min_log_mel
-    f_pts[log_t] = min_log_hz * torch.exp(logstep * (m_pts[log_t] - min_log_mel))
+    m_pts = torch.linspace(_hz_to_mel(f_min, mel_scale), _hz_to_mel(f_max, mel_scale), n_mels + 2)
+    if mel_scale == "htk":
+        f_pts = 700.0 * (10.0 ** (m_pts / 2595.0) - 1.0)
+    else:
+        f_sp = 200.0 / 3
+        f_pts = f_sp * m_pts
+        min_log_hz = 1000.0
+        min_log_mel = min_log_hz / f_sp
+        logstep = math.log(6.4) / 27.0
+        log_t = m_pts >= min_log_mel
+        f_pts[log_t] = min_log_hz * torch.exp(logstep * (m_pts[log_t] - min_log_mel))
     f_diff = f_pts[1:] - f_pts[:-1]
     slopes = f_pts.unsqueeze(0) - all_freqs.unsqueeze(1)
     down = (-1.0 * slopes[:, :-2]) / f_diff[:-1]
@@ -124,10 +135,10 @@ def mel_filterbank(n_freqs=N_FFT // 2 + 1, f_min=F_MIN, f_max=F_MAX, n_mels=N_ME
     return torch.max(torch.zeros(1), torch.min(down, up))  # [n_freqs, n_mels]
 
 
-def mel_constants() -> dict:
-    """Window, FFT twiddles and the filterbank in CSR form (each mel band is one contiguous
-    run of FFT bins) as packed parameters ``mel.*``."""
-    fb = mel_filterbank().numpy()  # [513, 128]
+def filterbank_csr(fb: np.ndarray):
+    """[n_freqs, n_mels] filterbank -> (start bin [n_mels], pointers [n_mels + 1], weights): band m is the run
+    w[ptr[m]:ptr[m+1]] on the bins from start[m] on, from its first to its last non-zero bin (an all-zero band is
+    an empty run at bin 0)."""
     starts, ptr, w = [], [0], []
     for m in range(fb.shape[1]):
         nz = np.nonzero(fb[:, m])[0]
@@ -138,15 +149,92 @@ def mel_constants() -> dict:
             starts.append(lo)
             w.extend(fb[lo:hi, m].tolist())
         ptr.append(len(w))
-    k = np.arange(512, dtype=np.float64)
-    tw = np.stack([np.cos(2 * np.pi * k / N_FFT), -np.sin(2 * np.pi * k / N_FFT)], axis=1)
+    return np.asarray(starts, np.int32), np.asarray(ptr, np.int32), np.asarray(w, np.float32)
+
+
+def fft_twiddles(n_fft: int) -> np.ndarray:
+    """e^{-2 pi i j / n_fft} for j < n_fft / 2 as interleaved (re, im) fp32, computed in float64."""
+    k = np.arange(n_fft // 2, dtype=np.float64)
+    tw = np.stack([np.cos(2 * np.pi * k / n_fft), -np.sin(2 * np.pi * k / n_fft)], axis=1)
+    return tw.astype(np.float32).reshape(-1)
+
+
+def mel_constants() -> dict:
+    """Window, FFT twiddles and the filterbank in CSR form (each mel band is one contiguous
+    run of FFT bins) as packed parameters ``mel.*``."""
+    starts, ptr, w = filterbank_csr(mel_filterbank().numpy())  # [513, 128]
     return {
         "mel.window": torch.hann_window(N_FFT, periodic=True).numpy(),
-        "mel.twiddle": tw.astype(np.float32).reshape(-1),
-        "mel.fb_start": np.asarray(starts, dtype=np.float32),
-        "mel.fb_ptr": np.asarray(ptr, dtype=np.float32),
-        "mel.fb_w": np.asarray(w, dtype=np.float32),
+        "mel.twiddle": fft_twiddles(N_FFT),
+        "mel.fb_start": starts.astype(np.float32),
+        "mel.fb_ptr": ptr.astype(np.float32),
+        "mel.fb_w": w,
     }
+
+
+MEL_N_FFT_RANGE = (64, 8192)
+MEL_MAX_BANDS = 1024
+
+
+def mel_norm_mode(normalized) -> int:
+    """torchaudio's `normalized` (_get_spec_norms) as bt_mel_config.norm_mode: "frame_length" scales the STFT by
+    n_fft^-1/2, True or "window" divides it by sqrt(sum window^2), False leaves it."""
+    from ._lib import BT_MEL_NORM_FRAME_LENGTH, BT_MEL_NORM_NONE, BT_MEL_NORM_WINDOW
+
+    if isinstance(normalized, str):
+        if normalized not in ("frame_length", "window"):
+            raise ValueError(f"Invalid normalized parameter: {normalized}")
+        return BT_MEL_NORM_FRAME_LENGTH if normalized == "frame_length" else BT_MEL_NORM_WINDOW
+    if isinstance(normalized, bool):
+        return BT_MEL_NORM_WINDOW if normalized else BT_MEL_NORM_NONE
+    raise TypeError("Input type not supported")
+
+
+class MelTables:
+    """Host-side constants of one bt_logmel_config analysis (include/beatthis.h): the config struct, the periodic
+    Hann window, the FFT twiddles and the filterbank in CSR form.  ``to(device)`` gives the device copies the call
+    takes.  Raises what the contract names for arguments outside it."""
+
+    def __init__(self, sample_rate, n_fft, hop_length, f_min, f_max, n_mels, mel_scale, normalized, power,
+                 log_multiplier):
+        from ._lib import bt_mel_config
+
+        norm_mode = mel_norm_mode(normalized)
+        if mel_scale not in ("slaney", "htk"):
+            raise ValueError('mel_scale should be one of "htk" or "slaney".')
+        if power is None:
+            raise NotImplementedError("complex output (power=None) is not implemented")
+        lo, hi = MEL_N_FFT_RANGE
+        n_fft_ok = isinstance(n_fft, numbers.Integral) and lo <= n_fft <= hi and n_fft & (n_fft - 1) == 0
+        if not (n_fft_ok and isinstance(hop_length, numbers.Integral) and hop_length >= 1
+                and isinstance(n_mels, numbers.Integral)
+                and 1 <= n_mels <= MEL_MAX_BANDS and math.isfinite(power) and power > 0
+                and math.isfinite(log_multiplier)):
+            raise NotImplementedError(
+                f"the log-mel kernels take a power-of-two n_fft in [{lo}, {hi}], hop_length >= 1, 1 <= n_mels <= "
+                f"{MEL_MAX_BANDS}, a finite power > 0 and a finite log_multiplier (got n_fft={n_fft}, "
+                f"hop_length={hop_length}, n_mels={n_mels}, power={power}, log_multiplier={log_multiplier})")
+        f_max = f_max if f_max is not None else float(sample_rate // 2)
+        if f_min > f_max:
+            raise ValueError(f"Require f_min: {f_min} <= f_max: {f_max}")
+        n_fft, hop_length, n_mels = int(n_fft), int(hop_length), int(n_mels)
+        self.n_fft, self.hop_length, self.n_mels = n_fft, hop_length, n_mels
+        self.config = bt_mel_config(n_fft, hop_length, n_mels, norm_mode, float(power), float(log_multiplier))
+        self.fb = mel_filterbank(n_fft // 2 + 1, f_min, f_max, n_mels, sample_rate, mel_scale)
+        self.fb_start, self.fb_ptr, self.fb_w = filterbank_csr(self.fb.numpy())
+        self.window = torch.hann_window(n_fft, periodic=True)
+        self.twiddle = fft_twiddles(n_fft)
+
+    def to(self, device) -> dict:
+        """Device tensors of the tables (fb_w holds at least one element, so that its pointer is never null)."""
+        fb_w = self.fb_w if len(self.fb_w) else np.zeros(1, np.float32)
+        return {
+            "window": self.window.to(device),
+            "twiddle": torch.from_numpy(self.twiddle).to(device),
+            "fb_start": torch.from_numpy(self.fb_start).to(device),
+            "fb_ptr": torch.from_numpy(self.fb_ptr).to(device),
+            "fb_w": torch.from_numpy(fb_w).to(device),
+        }
 
 
 # ------------------------------------------------------------------------------------------------
@@ -202,8 +290,12 @@ def resample_filter_bank(sr_in: int, sr_out: int = SAMPLE_RATE):
 
 
 class LogMelSpect(torch.nn.Module):
-    """Drop-in for the reference class (preprocessing.py:27-59).  Only the reference's
-    default analysis parameters are implemented in the kernel; anything else raises."""
+    """Drop-in for the reference class (preprocessing.py:27-59) with every one of its analysis parameters
+    (contract: ``bt_logmel_config`` in include/beatthis.h).  The reference defaults run the model path's fused
+    kernel (``bt_logmel``); any other parameters run the general kernel (``bt_logmel_config``) on tables built here.
+    ``_general=True`` sends the defaults through the general kernel too (for tests)."""
+
+    DEFAULTS = (22050, 1024, 441, 30, 11000, 128, "slaney", "frame_length", 1, 1000)
 
     def __init__(
         self,
@@ -219,16 +311,27 @@ class LogMelSpect(torch.nn.Module):
         log_multiplier=1000,
         device="cuda",
         _engine=None,
+        _general=False,
     ):
         super().__init__()
-        given = (sample_rate, n_fft, hop_length, f_min, f_max, n_mels, mel_scale, normalized, power, log_multiplier)
-        if given != (22050, 1024, 441, 30, 11000, 128, "slaney", "frame_length", 1, 1000):
-            raise NotImplementedError("the log-mel kernel implements the reference defaults only")
         from .engine import Engine
 
-        self.engine = _engine if _engine is not None else Engine.mel_only(device)
+        given = (sample_rate, n_fft, hop_length, f_min, f_max, n_mels, mel_scale, normalized, power, log_multiplier)
+        self.tables = MelTables(*given)
+        if given == self.DEFAULTS and not _general:
+            self.tables = None
+            self.engine = _engine if _engine is not None else Engine.mel_only(device)
+        else:
+            self.engine = _engine if _engine is not None else Engine(None, None, device)
+            self.device_tables = self.tables.to(self.engine.device)
 
     def forward(self, x):
         """Input is a waveform as a monodimensional array of shape T,
-        output is a 2D log mel spectrogram of shape (F,128)."""
-        return self.engine.logmel([x])[0]
+        output is a 2D log mel spectrogram of shape (F, n_mels)."""
+        return self.batch([x])[0]
+
+    def batch(self, signals):
+        """Many 1-D signals in one kernel launch: a list of [1 + len_i // hop_length, n_mels] spectrograms."""
+        if self.tables is None:
+            return self.engine.logmel(signals)
+        return self.engine.logmel_config(signals, self.tables, self.device_tables)

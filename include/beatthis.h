@@ -183,6 +183,45 @@ int bt_logmel(bt_ctx* ctx, const float* audio_dev, const int64_t* sample_offsets
               int32_t n_clips, float* spect_dev, const int64_t* frame_offsets_host,
               void* stream);
 
+/* LogMelSpect (preprocessing.py:27-59) with any analysis parameters: torchaudio 2.x MelSpectrogram as the reference
+ * constructs it, then log1p(log_multiplier * mel).  Contract, for a mono fp32 clip x of len samples:
+ *  - STFT: win_length = n_fft, the caller's window (a periodic Hann window for the reference), center=True with
+ *    pad_mode="reflect" (n_fft/2 samples mirrored at each end without repeating the edge), onesided: frame t covers
+ *    samples t*hop_length - n_fft/2 ..; T = 1 + len / hop_length frames of n_fft/2 + 1 bins X[t][k].
+ *  - normalisation (norm_mode; torchaudio's `normalized`): BT_MEL_NORM_FRAME_LENGTH ("frame_length") scales X by
+ *    n_fft^-1/2, BT_MEL_NORM_WINDOW (True or "window") divides it by sqrt(sum window^2), BT_MEL_NORM_NONE (False)
+ *    leaves it.  Any other string is a ValueError in Python (torchaudio's _get_spec_norms).
+ *  - power: S[t][k] = |X[t][k]|^power for a finite power > 0 (power = 1: the magnitude).  Complex output
+ *    (power=None) is not implemented.
+ *  - filterbank: torchaudio melscale_fbanks(n_fft/2 + 1, f_min, f_max, n_mels, sample_rate, norm=None, mel_scale) with
+ *    mel_scale "slaney" or "htk", frequency grid linspace(0, sample_rate // 2, n_fft/2 + 1) (integer floor: it
+ *    matters at odd rates such as 11025 Hz), f_max=None meaning float(sample_rate // 2); f_min > f_max is a
+ *    ValueError in Python.  The caller passes it in CSR form: band m has the weights fb_w_dev[fb_ptr_dev[m] ..
+ *    fb_ptr_dev[m+1]) on the bins from fb_start_dev[m] on (one contiguous run per band; an all-zero band is an empty
+ *    run and gives log1p(0) = 0, as torchaudio does after its warning).
+ *  - output: spect_dev [T_i][n_mels] fp32 at frame_offsets_host[i] = log1p(log_multiplier * sum_k S[t][k] fb[k][m]).
+ *  - tables (caller-owned, device): window_dev [n_fft], twiddle_dev [n_fft/2] complex fp32 (re, im) pairs
+ *    e^{-2 pi i j / n_fft} computed in float64 and rounded, as for bt_logmel's "mel.twiddle".
+ * Supported range: n_fft a power of two in [64, 8192], hop_length >= 1, 1 <= n_mels <= 1024, norm_mode one of the
+ * three, power finite and > 0, log_multiplier finite; anything else is BT_ERR_ARG (NotImplementedError in Python).
+ * Every clip needs more than n_fft/2 samples (torch's reflect padding fails below that); frame_offsets_host must start
+ * at 0 and give clip i exactly 1 + len_i / hop_length frames; sample offsets must not decrease.  All of this is
+ * checked, and BT_ERR_ARG returned, before anything is enqueued.  Needs no weights (a weight-less ctx is enough).
+ * Enqueues only: no synchronisation.  Kernel: logmel_config (profile name). */
+#define BT_MEL_NORM_NONE 0
+#define BT_MEL_NORM_FRAME_LENGTH 1
+#define BT_MEL_NORM_WINDOW 2
+
+typedef struct bt_mel_config {
+  int32_t n_fft, hop_length, n_mels, norm_mode;
+  float power, log_multiplier;
+} bt_mel_config;
+
+int bt_logmel_config(bt_ctx* ctx, const bt_mel_config* cfg, const float* window_dev, const float* twiddle_dev,
+                     const int32_t* fb_start_dev, const int32_t* fb_ptr_dev, const float* fb_w_dev,
+                     const float* audio_dev, const int64_t* sample_offsets_host, int32_t n_clips,
+                     float* spect_dev, const int64_t* frame_offsets_host, void* stream);
+
 /* Resample front door of Audio2Frames.signal2spect (inference.py:274-275:
  * `soxr.resample(signal, in_rate=sr, out_rate=22050)`), as a device polyphase FIR:
  *   out[n] = sum_k coef[(n*M) mod L][k] * in[floor(n*M/L) - K/2 + 1 + k]   (zeros outside a clip)
