@@ -80,6 +80,7 @@ class bt_beat_metric_params(ctypes.Structure):
 
 
 BT_CHUNK = 1500
+MAX_CHUNK_CAP = 256 * BT_CHUNK  # the longest maximum chunk bt_finalize accepts (RoPE tables of up to this many rows)
 BT_KEEP_FIRST = 0
 BT_KEEP_LAST = 1
 OVERLAP_MODES = {"keep_first": BT_KEEP_FIRST, "keep_last": BT_KEEP_LAST}
@@ -131,6 +132,12 @@ PROTOTYPES = {
     "bt_plan_chunking": (
         c_int64, [c_int64, POINTER(bt_chunking), POINTER(c_int64), POINTER(c_int64), POINTER(c_int64), POINTER(c_int64), c_int64],
     ),
+    "bt_plan_chunking_max": (
+        c_int64,
+        [c_int64, POINTER(bt_chunking), c_int32, POINTER(c_int64), POINTER(c_int64), POINTER(c_int64), POINTER(c_int64),
+         c_int64],
+    ),
+    "bt_max_chunk": (c_int32, [c_void_p]),
     "bt_logmel": (c_int, [c_void_p, c_void_p, POINTER(c_int64), c_int32, c_void_p, POINTER(c_int64), c_void_p]),
     "bt_logmel_config": (
         c_int,

@@ -65,10 +65,11 @@ struct LayerPlans {
   GemmPlan gemm;             // convolution, frontend.linear
 };
 
-// The activations of a wave of up to `chunks` chunks of BT_CHUNK frames (XB only on the 16-bit path), and the
+// The activations of a wave of up to `chunks` chunks and `frames` padded frames (XB only on the 16-bit path), and the
 // tensor-core plans made for them: their tensor maps hold workspace addresses, so the two are dropped together.
 struct Workspace {
   int chunks = 0;
+  int64_t frames = 0;
   DeviceBuffer<float> X0, X1, GATES;
   DeviceBuffer<> XB, XN, QKV, O, H;
   std::map<std::pair<int, int>, std::vector<LayerPlans>> plans;  // per (nb, L) geometry, parallel to bt_ctx::layers
@@ -90,6 +91,7 @@ struct bt_ctx {
   bool sync_debug = false;
 
   int wave = 128;  // the workspace grows on demand up to `wave` chunks
+  int max_chunk = BT_CHUNK;  // longest chunk the forward pass takes: the rows of the RoPE tables (bt_finalize)
   Workspace ws;
   // spectrogram scratch for bt_audio2frames
   DeviceBuffer<float> spect_ws;
@@ -195,9 +197,13 @@ const Param* find_param(const bt_ctx* c, const std::string& name) {
 }
 
 constexpr bt_chunking kDefaultChunking{BT_CHUNK, BT_BORDER, BT_KEEP_FIRST};
+constexpr int kMaxWaveChunks = 256;  // bt_set_wave_chunks
+// Longest chunk a ctx takes: the largest frame budget bt_set_wave_chunks allows, so that no wave holds more frames
+// than one of kMaxWaveChunks chunks of BT_CHUNK frames (the 32-bit element counts of the kernels stay within that)
+constexpr int64_t kMaxChunkCap = static_cast<int64_t>(kMaxWaveChunks) * BT_CHUNK;
 
-bool chunking_valid(const bt_chunking* ck) {
-  return ck && ck->chunk_size >= 1 && ck->chunk_size <= BT_CHUNK && ck->border >= 0 &&
+bool chunking_valid(const bt_chunking* ck, int64_t max_chunk) {
+  return ck && ck->chunk_size >= 1 && ck->chunk_size <= max_chunk && ck->border >= 0 &&
          2 * static_cast<int64_t>(ck->border) < ck->chunk_size &&
          (ck->overlap_mode == BT_KEEP_FIRST || ck->overlap_mode == BT_KEEP_LAST);
 }
@@ -282,35 +288,40 @@ int stage(bt_ctx* c, cudaStream_t st, std::initializer_list<std::pair<const T*, 
   return upload_stage(c, sl, bytes, st);
 }
 
-// elements per chunk of the largest frontend activation: F*L*C is the same for all blocks
+// elements per frame of the largest frontend activation: F*C is the same for all blocks
 int64_t front_elems(const bt_ctx* c) {
-  return static_cast<int64_t>(c->hp.spect_dim / 4) * BT_CHUNK * c->hp.stem_dim;
+  return static_cast<int64_t>(c->hp.spect_dim / 4) * c->hp.stem_dim;
+}
+
+// Padded frames a wave may hold: `wave` chunks of BT_CHUNK frames, or one chunk of the ctx's longest length
+int64_t wave_frames(const bt_ctx* c) {
+  return std::max<int64_t>(static_cast<int64_t>(c->wave) * BT_CHUNK, c->max_chunk);
 }
 
 int ensure_ws(bt_ctx* c) {
-  // sized once for a full wave (bt_set_wave_chunks; ~46 MB per 1500-frame chunk on the 16-bit path): growing later
+  // sized once for a full wave (bt_set_wave_chunks; ~46 MB per 1500 frames on the 16-bit path): growing later
   // would mean freeing and allocating device memory -- device-wide synchronisation -- amid a stream of batches
   const int want = c->wave;
-  if (want <= c->ws.chunks) return BT_OK;
+  const int64_t frames = wave_frames(c);
+  if (want <= c->ws.chunks && frames <= c->ws.frames) return BT_OK;
   c->ws = Workspace();  // the old blocks are freed before the new ones are allocated
-  const int64_t G = want;
-  const int64_t fe = front_elems(c);                                     // 1.536M
+  const int64_t fe = front_elems(c);                                     // 1024
   const int64_t D = c->hp.transformer_dim;
-  const int64_t me = static_cast<int64_t>(BT_CHUNK) * D;                 // main tokens * dim
-  const int64_t xe = std::max(fe, me);
+  const int64_t xe = frames * std::max(fe, D);                           // elements of the largest activation
   const size_t act = c->dtype == BT_DTYPE_H16 ? 2 : 4;
   Workspace& ws = c->ws;
-  BT_CUDA(c, ws.X0.alloc(G * xe * 4));
-  BT_CUDA(c, ws.X1.alloc(G * xe * 4));
-  BT_CUDA(c, ws.GATES.alloc(G * std::max<int64_t>(fe / 32, BT_CHUNK * (D / 32)) * 4));
-  BT_CUDA(c, ws.XN.alloc(G * xe * act));
-  BT_CUDA(c, ws.QKV.alloc(G * 3 * xe * act));
-  BT_CUDA(c, ws.O.alloc(G * xe * act));
-  BT_CUDA(c, ws.H.alloc(G * 4 * xe * act));
+  BT_CUDA(c, ws.X0.alloc(xe * 4));
+  BT_CUDA(c, ws.X1.alloc(xe * 4));
+  BT_CUDA(c, ws.GATES.alloc(frames * std::max(fe / 32, D / 32) * 4));
+  BT_CUDA(c, ws.XN.alloc(xe * act));
+  BT_CUDA(c, ws.QKV.alloc(3 * xe * act));
+  BT_CUDA(c, ws.O.alloc(xe * act));
+  BT_CUDA(c, ws.H.alloc(4 * xe * act));
   if (c->dtype == BT_DTYPE_H16) {
-    BT_CUDA(c, ws.XB.alloc(G * xe * 2));
+    BT_CUDA(c, ws.XB.alloc(xe * 2));
   }
   ws.chunks = want;
+  ws.frames = frames;
   return BT_OK;
 }
 
@@ -605,9 +616,10 @@ int run_wave(bt_ctx* c, const float* spect, const Wave& wv, float* beat, float* 
   return BT_OK;
 }
 
-// upload the chunk table and run the forward pass in waves of up to ws.chunks chunks, longest first.  A wave is padded
-// to its longest chunk: a shorter chunk costs its padded share of one wave (a fraction of a millisecond) instead of ~90
-// launches of its own (~0.7 ms of fixed cost), so chunks of all lengths share waves
+// upload the chunk table and run the forward pass in waves, longest first.  A wave is padded to its longest chunk and
+// closes before it would hold more than ws.chunks chunks or more than ws.frames padded frames (chunks of up to
+// BT_CHUNK frames never reach the frame budget).  A shorter chunk costs its padded share of one wave (a fraction of a
+// millisecond) instead of ~90 launches of its own (~0.7 ms of fixed cost), so chunks of all lengths share waves
 int run_chunks(bt_ctx* c, const float* spect_dev, std::vector<ChunkSrc>& all, float* beat_dev, float* downbeat_dev,
                cudaStream_t st) {
   int r = BT_OK;
@@ -618,7 +630,11 @@ int run_chunks(bt_ctx* c, const float* spect_dev, std::vector<ChunkSrc>& all, fl
   if ((r = stage(c, st, {{all.data(), all.size()}}, &ds)) != BT_OK) return r;
   size_t i = 0;
   while (i < all.size()) {
-    const size_t j = std::min(all.size(), i + static_cast<size_t>(c->ws.chunks));
+    const int64_t L = all[i].len;
+    size_t j = i + 1;  // a chunk alone fits: its length is at most max_chunk <= ws.frames
+    while (j < all.size() && j - i < static_cast<size_t>(c->ws.chunks) &&
+           static_cast<int64_t>(j - i + 1) * L <= c->ws.frames)
+      ++j;
     Wave wv{ds + i, static_cast<int>(j - i), all[i].len, all[j - 1].len != all[i].len};
     if ((r = run_wave(c, spect_dev, wv, beat_dev, downbeat_dev, st)) != BT_OK) return r;
     i = j;
@@ -676,7 +692,7 @@ cudaError_t to_h16_operand(DeviceBuffer<>& buf, const float* src, int64_t n, cud
 // ================================================================================== C ABI
 extern "C" {
 
-int bt_version(void) { return 206; }
+int bt_version(void) { return 207; }
 
 const char* bt_act_dtype(void) {
 #if defined(BT_ACT_BF16)
@@ -694,10 +710,15 @@ int64_t bt_plan_chunks(int64_t T, int64_t* starts, int64_t* lens, int64_t cap) {
   return plan_chunks(T, kDefaultChunking, starts, lens, nullptr, nullptr, cap);
 }
 
+int64_t bt_plan_chunking_max(int64_t T, const bt_chunking* ck, int32_t max_chunk, int64_t* starts, int64_t* lens,
+                             int64_t* own_lo, int64_t* own_hi, int64_t cap) {
+  if (!chunking_valid(ck, max_chunk)) return BT_ERR_ARG;
+  return plan_chunks(T, *ck, starts, lens, own_lo, own_hi, cap);
+}
+
 int64_t bt_plan_chunking(int64_t T, const bt_chunking* ck, int64_t* starts, int64_t* lens, int64_t* own_lo,
                          int64_t* own_hi, int64_t cap) {
-  if (!chunking_valid(ck)) return BT_ERR_ARG;
-  return plan_chunks(T, *ck, starts, lens, own_lo, own_hi, cap);
+  return bt_plan_chunking_max(T, ck, BT_CHUNK, starts, lens, own_lo, own_hi, cap);
 }
 
 int bt_create(bt_ctx** out, int device_ordinal, const bt_hparams* hp, int compute_dtype) {
@@ -773,7 +794,7 @@ int bt_finalize(bt_ctx* c) {
   std::vector<Need> need = {
       {"mel.window", 1024, nullptr, false}, {"mel.twiddle", 1024, nullptr, false}, {"mel.fb_start", 128, nullptr, false},
       {"mel.fb_ptr", 129, nullptr, false}, {"mel.fb_w", -1, nullptr, false},
-      {"rope.cos", BT_CHUNK * 16, &c->rope_cos, false}, {"rope.sin", BT_CHUNK * 16, &c->rope_sin, false},
+      {"rope.cos", -1, &c->rope_cos, false}, {"rope.sin", -1, &c->rope_sin, false},  // checked below
       {"stem.bn1_scale", -1, &c->bn1_scale, false}, {"stem.bn1_shift", -1, &c->bn1_shift, false},
       {"stem.w", 32 * 12, &c->stem_w, false}, {"stem.bias", -1, &c->stem_b, false},
       {"head.w", 2 * D, &c->head_w, false}, {"head.b", 2, &c->head_b, false}};
@@ -791,6 +812,12 @@ int bt_finalize(bt_ctx* c) {
                   (long long)n.count);
     if (n.dst) *n.dst = p;
   }
+  // the RoPE tables hold positions 0 .. P - 1, and P is the longest chunk this ctx takes
+  const int64_t rows = c->rope_cos->n / 16;
+  if (c->rope_cos->n % 16 != 0 || rows < BT_CHUNK || rows > kMaxChunkCap || c->rope_sin->n != c->rope_cos->n)
+    return fail(c, BT_ERR_PARAM, "parameters 'rope.cos' / 'rope.sin' have %lld / %lld elements; both need P x 16 with "
+                "%d <= P <= %lld", (long long)c->rope_cos->n, (long long)c->rope_sin->n, BT_CHUNK, (long long)kMaxChunkCap);
+  c->max_chunk = static_cast<int>(rows);
   if (c->dtype == BT_DTYPE_H16) {
     for (const Need& n : need) {
       if (!n.gemm) continue;
@@ -812,7 +839,7 @@ void bt_destroy(bt_ctx* c) {
 }
 
 int bt_set_wave_chunks(bt_ctx* c, int32_t chunks) {
-  if (!c || chunks < 1 || chunks > 256) return fail(c, BT_ERR_ARG, "bt_set_wave_chunks: 1..256");
+  if (!c || chunks < 1 || chunks > kMaxWaveChunks) return fail(c, BT_ERR_ARG, "bt_set_wave_chunks: 1..%d", kMaxWaveChunks);
   c->wave = chunks;
   if (c->ws.chunks > chunks) {  // shrink: drop the workspace, it is re-created on the next call
     cudaSetDevice(c->device);
@@ -821,6 +848,8 @@ int bt_set_wave_chunks(bt_ctx* c, int32_t chunks) {
   }
   return BT_OK;
 }
+
+int32_t bt_max_chunk(const bt_ctx* c) { return c ? c->max_chunk : BT_ERR_ARG; }
 
 int64_t bt_launch_count(const bt_ctx* c) { return c ? c->launches : 0; }
 
@@ -1025,9 +1054,9 @@ int bt_spect2frames(bt_ctx* c, const float* spect_dev, const int64_t* frame_offs
 int bt_spect2frames_chunked(bt_ctx* c, const float* spect_dev, const int64_t* frame_offsets_host, int32_t n_clips,
                             float* beat_dev, float* downbeat_dev, const bt_chunking* ck, void* stream) {
   if (!c || !c->finalized) return fail(c, BT_ERR_STATE, "bt_spect2frames_chunked: context not finalized");
-  if (!chunking_valid(ck))
-    return fail(c, BT_ERR_ARG, "bt_spect2frames_chunked: need 1 <= chunk_size <= %d, 0 <= 2 * border < chunk_size "
-                "and overlap_mode BT_KEEP_FIRST or BT_KEEP_LAST", BT_CHUNK);
+  if (!chunking_valid(ck, c->max_chunk))
+    return fail(c, BT_ERR_ARG, "bt_spect2frames_chunked: need 1 <= chunk_size <= %d (bt_max_chunk), 0 <= 2 * border < "
+                "chunk_size and overlap_mode BT_KEEP_FIRST or BT_KEEP_LAST", c->max_chunk);
   return spect2frames(c, spect_dev, frame_offsets_host, n_clips, beat_dev, downbeat_dev, *ck, stream,
                       "bt_spect2frames_chunked");
 }
@@ -1037,8 +1066,8 @@ int bt_forward_chunks(bt_ctx* c, const float* chunks_dev, int32_t n_chunks, int3
   if (!c || !c->finalized) return fail(c, BT_ERR_STATE, "bt_forward_chunks: context not finalized");
   if (n_chunks <= 0) return BT_OK;
   if (!chunks_dev || !beat_dev || !downbeat_dev) return fail(c, BT_ERR_ARG, "bt_forward_chunks: null argument");
-  if (chunk_frames < 1 || chunk_frames > BT_CHUNK)
-    return fail(c, BT_ERR_ARG, "bt_forward_chunks: chunk_frames must be in [1, %d]", BT_CHUNK);
+  if (chunk_frames < 1 || chunk_frames > c->max_chunk)
+    return fail(c, BT_ERR_ARG, "bt_forward_chunks: chunk_frames must be in [1, %d] (bt_max_chunk)", c->max_chunk);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   BT_CUDA(c, cudaSetDevice(c->device));
   prof_mark(c, st);
@@ -1083,9 +1112,9 @@ int bt_audio2frames_chunked(bt_ctx* c, const float* audio_dev, const int64_t* sa
                             float* beat_dev, float* downbeat_dev, const int64_t* frame_offsets_host,
                             const bt_chunking* ck, void* stream) {
   if (!c || !c->finalized) return fail(c, BT_ERR_STATE, "bt_audio2frames_chunked: context not finalized");
-  if (!chunking_valid(ck))
-    return fail(c, BT_ERR_ARG, "bt_audio2frames_chunked: need 1 <= chunk_size <= %d, 0 <= 2 * border < chunk_size "
-                "and overlap_mode BT_KEEP_FIRST or BT_KEEP_LAST", BT_CHUNK);
+  if (!chunking_valid(ck, c->max_chunk))
+    return fail(c, BT_ERR_ARG, "bt_audio2frames_chunked: need 1 <= chunk_size <= %d (bt_max_chunk), 0 <= 2 * border < "
+                "chunk_size and overlap_mode BT_KEEP_FIRST or BT_KEEP_LAST", c->max_chunk);
   return audio2frames(c, audio_dev, sample_offsets_host, n_clips, beat_dev, downbeat_dev, frame_offsets_host, *ck,
                       stream, "bt_audio2frames_chunked");
 }

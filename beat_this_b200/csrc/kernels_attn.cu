@@ -1,6 +1,7 @@
-// Tensor-core flash attention for head_dim 32 over sequences of up to 1500 frames: the time-direction
-// attention of the three frontend blocks and of the 6 main layers (reference roformer.py:73-80 SDPA,
-// called from roformer.py:114-132 / beat_tracker.py:290-301).
+// Tensor-core flash attention for head_dim 32 over sequences of any length (a ctx's chunks are at most bt_max_chunk
+// frames): the time-direction attention of the three frontend blocks and of the 6 main layers (reference
+// roformer.py:73-80 SDPA, called from roformer.py:114-132 / beat_tracker.py:290-301).  Row and tile indices are
+// 32-bit (L < 2^31); element offsets are 64-bit.
 #include <cstdio>
 
 #include "tc_common.cuh"

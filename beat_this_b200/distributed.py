@@ -75,18 +75,21 @@ def broadcast_packed(packed: dict | None, hparams: dict | None, device, src: int
     return packed_from_blob(t.cpu().numpy(), names, sizes), hparams
 
 
-def load_model_distributed(checkpoint_path, device, float16=False, wave_chunks=None):
-    """load_model for torchrun jobs: rank 0 loads + packs, one broadcast, every rank uploads."""
-    from .inference import BeatThisB200, load_checkpoint
+def load_model_distributed(checkpoint_path, device, float16=False, wave_chunks=None, max_chunk_size=1500):
+    """load_model for torchrun jobs: rank 0 loads + packs, one broadcast, every rank uploads.  The RoPE tables of
+    max_chunk_size rows travel in the blob, and every rank's model takes its maximum chunk length from them."""
+    from .inference import BeatThisB200, check_max_chunk_size, load_checkpoint
     from .utils import replace_state_dict_key
     from .weights import filter_hparams, pack_parameters
 
+    max_chunk_size = check_max_chunk_size(max_chunk_size)
     rank = dist.get_rank() if dist.is_initialized() else 0
     packed, hparams = None, None
     if rank == 0:
         ckpt = load_checkpoint(checkpoint_path, "cpu")
         hparams = filter_hparams(ckpt["hyper_parameters"])
-        packed = pack_parameters(replace_state_dict_key(dict(ckpt["state_dict"]), "model.", ""), hparams)
+        packed = pack_parameters(replace_state_dict_key(dict(ckpt["state_dict"]), "model.", ""), hparams,
+                                 rope_positions=max_chunk_size)
     packed, hparams = broadcast_packed(packed, hparams, device)
     return BeatThisB200(hparams, packed, device, float16, wave_chunks)
 

@@ -24,16 +24,18 @@ def _cuda_device(device) -> torch.device:
     return dev
 
 
-def chunking_struct(chunk_size: int, border_size: int, overlap_mode: str) -> _lib.bt_chunking:
-    """split_predict_aggregate's (chunk_size, border_size, overlap_mode) as the C library takes it (bt_plan_chunking,
-    include/beatthis.h).  ``ValueError`` for what the library refuses: chunk_size outside [1, 1500] (the RoPE tables
-    and workspace are sized for 1500 frames), a negative border, 2 * border_size >= chunk_size or an overlap_mode other
-    than "keep_first" / "keep_last"."""
+def chunking_struct(chunk_size: int, border_size: int, overlap_mode: str, max_chunk_size: int = _lib.BT_CHUNK
+                    ) -> _lib.bt_chunking:
+    """split_predict_aggregate's (chunk_size, border_size, overlap_mode) as the C library takes it
+    (bt_plan_chunking_max, include/beatthis.h).  ``ValueError`` for what the library refuses: chunk_size outside
+    [1, max_chunk_size] (the model's maximum chunk length: the rows of its RoPE tables, 1500 unless it was loaded with
+    a larger max_chunk_size), a negative border, 2 * border_size >= chunk_size or an overlap_mode other than
+    "keep_first" / "keep_last"."""
     if overlap_mode not in _lib.OVERLAP_MODES:
         raise ValueError("overlap_mode must be 'keep_first' or 'keep_last'")
     chunk_size, border_size = int(chunk_size), int(border_size)
-    if not 1 <= chunk_size <= _lib.BT_CHUNK:
-        raise ValueError(f"chunk_size must be in [1, {_lib.BT_CHUNK}], got {chunk_size}")
+    if not 1 <= chunk_size <= max_chunk_size:
+        raise ValueError(f"chunk_size must be in [1, {max_chunk_size}] (the model's max_chunk_size), got {chunk_size}")
     if border_size < 0 or 2 * border_size >= chunk_size:
         raise ValueError(f"border_size must satisfy 0 <= 2 * border_size < chunk_size, got {border_size} for {chunk_size}")
     return _lib.bt_chunking(chunk_size, border_size, _lib.OVERLAP_MODES[overlap_mode])
@@ -129,6 +131,11 @@ class Engine:
         _lib.check(self.lib, self.ctx, self.lib.bt_finalize(self.ctx))
         self._model_ready = True
 
+    @property
+    def max_chunk(self) -> int:
+        """The longest chunk this context runs (bt_max_chunk: the rows of its RoPE tables)."""
+        return int(self.lib.bt_max_chunk(self.ctx))
+
     def set_wave_chunks(self, n: int):
         _lib.check(self.lib, self.ctx, self.lib.bt_set_wave_chunks(self.ctx, int(n)))
 
@@ -222,10 +229,11 @@ class Engine:
 
     def spect2frames_cat(self, spect: torch.Tensor, frame_offsets, chunking: tuple | None = None):
         """Concatenated [total, 128] spectrograms -> (beat, downbeat) logits.  chunking: (chunk_size, border_size,
-        overlap_mode) of split_predict_aggregate, checked by chunking_struct; None is 1500 / 6 / keep_first."""
+        overlap_mode) of split_predict_aggregate, checked by chunking_struct against max_chunk; None is 1500 / 6 /
+        keep_first."""
         assert self._model_ready, "model parameters not loaded"
         assert spect.is_cuda and spect.dtype == torch.float32 and spect.is_contiguous()
-        ck = None if chunking is None else chunking_struct(*chunking)
+        ck = None if chunking is None else chunking_struct(*chunking, self.max_chunk)
         total = int(frame_offsets[-1])
         beat = torch.empty(total, dtype=torch.float32, device=self.device)
         down = torch.empty(total, dtype=torch.float32, device=self.device)
@@ -239,7 +247,7 @@ class Engine:
         return beat, down
 
     def forward_chunks(self, chunks: torch.Tensor):
-        """BeatThis.forward on [B, T<=1500, 128] chunks (no chunk planning, no borders cut): flat (beat, downbeat)."""
+        """BeatThis.forward on [B, T<=max_chunk, 128] chunks (no chunk planning, no borders cut): flat (beat, downbeat)."""
         assert self._model_ready, "model parameters not loaded"
         assert chunks.is_cuda and chunks.dtype == torch.float32 and chunks.is_contiguous() and chunks.ndim == 3
         B, T, _ = chunks.shape
@@ -266,7 +274,7 @@ class Engine:
         """Concatenated mono 22.05 kHz audio -> (beat, downbeat, frame offsets); chunking as in spect2frames_cat."""
         assert self._model_ready, "model parameters not loaded"
         assert audio.is_cuda and audio.dtype == torch.float32 and audio.is_contiguous()
-        ck = None if chunking is None else chunking_struct(*chunking)
+        ck = None if chunking is None else chunking_struct(*chunking, self.max_chunk)
         fo = self.frame_offsets(sample_offsets)
         beat = torch.empty(fo[-1], dtype=torch.float32, device=self.device)
         down = torch.empty(fo[-1], dtype=torch.float32, device=self.device)

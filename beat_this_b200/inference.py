@@ -18,9 +18,9 @@ import math
 import numpy as np
 import torch
 
-from ._lib import bt_wav_info
+from ._lib import BT_CHUNK, MAX_CHUNK_CAP, bt_wav_info
 from .engine import Engine, chunking_struct
-from .pipeline import BeatPipeline, as_signal_array, chunk_cost, plan_groups
+from .pipeline import BeatPipeline, as_signal_array, chunk_cost, padded_frames, plan_groups
 from .postprocessor import Postprocessor
 from .preprocessing import LogMelSpect, load_audio
 from .utils import replace_state_dict_key, save_beat_tsv
@@ -67,6 +67,8 @@ class BeatThisB200:
         self.engine = Engine(packed, self.hparams, device, half=float16, wave_chunks=wave_chunks)
         self.device = self.engine.device
         self.float16 = float16
+        # the longest chunk the model runs: the rows of the packed RoPE tables (load_model's max_chunk_size)
+        self.max_chunk_size = self.engine.max_chunk
 
     def eval(self):
         return self
@@ -78,28 +80,42 @@ class BeatThisB200:
 
     def __call__(self, spect: torch.Tensor) -> dict:
         """BeatThis.forward (reference beat_tracker.py:188-192) for a batch of equal-length spectrogram chunks
-        [B, T<=1500, 128]: every chunk runs as its own piece without borders being cut."""
-        if spect.ndim != 3 or spect.shape[2] != 128 or spect.shape[1] > 1500:
-            raise ValueError(f"Expected [B, T<=1500, 128] chunks, got {tuple(spect.shape)}")
+        [B, T<=max_chunk_size, 128]: every chunk runs as its own piece without borders being cut."""
+        if spect.ndim != 3 or spect.shape[2] != 128 or spect.shape[1] > self.max_chunk_size:
+            raise ValueError(f"Expected [B, T<={self.max_chunk_size}, 128] chunks (T up to the model's max_chunk_size), "
+                             f"got {tuple(spect.shape)}")
         B, T, _ = spect.shape
         beat, down = self.engine.forward_chunks(spect.to(self.device, torch.float32).contiguous())
         return {"beat": beat.view(B, T), "downbeat": down.view(B, T)}
 
 
+def check_max_chunk_size(max_chunk_size) -> int:
+    """The max_chunk_size keyword of load_model and the inference classes: an integer in [1500, 384000].  1500 is the
+    reference's inference chunk; a model trained on longer sequences (train.py --train-length) may run longer ones."""
+    if not isinstance(max_chunk_size, (int, np.integer)) or isinstance(max_chunk_size, bool) or \
+            not BT_CHUNK <= max_chunk_size <= MAX_CHUNK_CAP:
+        raise ValueError(f"max_chunk_size must be an integer in [{BT_CHUNK}, {MAX_CHUNK_CAP}], got {max_chunk_size!r}")
+    return int(max_chunk_size)
+
+
 def load_model(checkpoint_path: str | dict | None = "final0", device: str | torch.device = "cuda", float16: bool = False,
-               wave_chunks: int | None = None) -> BeatThisB200:
+               wave_chunks: int | None = None, max_chunk_size: int = BT_CHUNK) -> BeatThisB200:
     """Load a BeatThis model from a checkpoint (reference inference.py:56-87).  Accepts the
     reference ``.ckpt`` layout unchanged (``hyper_parameters`` + ``state_dict`` with the
-    ``model.`` prefix).  ``checkpoint_path`` may also be an already loaded checkpoint dict."""
+    ``model.`` prefix).  ``checkpoint_path`` may also be an already loaded checkpoint dict.
+    max_chunk_size: the longest chunk the model will run (its RoPE tables' length), 1500 by default; chunk sizes up
+    to it are accepted by split_predict_aggregate, spects2frames, frames_batch and the model call.  It is not read
+    from the checkpoint."""
     from .engine import _cuda_device
 
     _cuda_device(device)  # fail before touching the checkpoint: there is no CPU path
+    max_chunk_size = check_max_chunk_size(max_chunk_size)
     if checkpoint_path is None:
         raise ValueError("beat_this_b200 needs a checkpoint (the reference's random-init BeatThis() has no use here)")
     checkpoint = checkpoint_path if isinstance(checkpoint_path, dict) else load_checkpoint(checkpoint_path, "cpu")
     hparams = checkpoint["hyper_parameters"]
     state_dict = replace_state_dict_key(dict(checkpoint["state_dict"]), "model.", "")
-    packed = pack_parameters(state_dict, filter_hparams(hparams))
+    packed = pack_parameters(state_dict, filter_hparams(hparams), rope_positions=max_chunk_size)
     return BeatThisB200(hparams, packed, device, float16, wave_chunks)
 
 
@@ -174,23 +190,33 @@ def aggregate_prediction(pred_chunks: list, starts: list, full_size: int, chunk_
 DEFAULT_CHUNKING = (1500, 6, "keep_first")  # what Spect2Frames.spect2frames uses (reference inference.py:244-254)
 
 
-def engine_chunking(chunk_size: int, border_size: int, overlap_mode: str) -> tuple | None:
+def engine_chunking(chunk_size: int, border_size: int, overlap_mode: str, max_chunk_size: int = BT_CHUNK
+                    ) -> tuple | None:
     """The `chunking` argument of Engine.spect2frames_cat / audio2frames_cat for split_predict_aggregate's values:
     None for 1500 / 6 / keep_first (the plain entry points), else the checked triple.  ``ValueError`` for values the
-    CUDA path cannot run (engine.chunking_struct)."""
-    chunking_struct(chunk_size, border_size, overlap_mode)
+    CUDA path cannot run (engine.chunking_struct; chunk_size up to the model's max_chunk_size)."""
+    chunking_struct(chunk_size, border_size, overlap_mode, max_chunk_size)
     chunking = (int(chunk_size), int(border_size), overlap_mode)
     return None if chunking == DEFAULT_CHUNKING else chunking
+
+
+def _plan_groups(n_samples, sr: int, chunking: tuple | None):
+    """Groups of consecutive clips for the pipeline: GROUP_CHUNKS 1500-frame chunks, or with a chunking the padded
+    frames of as many, so that a group of long chunks fits one wave's frame budget (bt_set_wave_chunks)."""
+    if chunking is None:
+        return plan_groups([chunk_cost(n, sr) for n in n_samples], GROUP_CHUNKS, GROUP_CLIPS)
+    return plan_groups([padded_frames(n, sr, *chunking[:2]) for n in n_samples], GROUP_CHUNKS * BT_CHUNK, GROUP_CLIPS)
 
 
 def split_predict_aggregate(spect: torch.Tensor, chunk_size: int, border_size: int, overlap_mode: str,
                             model) -> dict:
     """Reference inference.py:188-230: chunk the piece, run `model` on every chunk, stitch.  A ``BeatThisB200`` model
-    runs as ONE call of the CUDA path for every chunk_size <= 1500, border_size with 0 <= 2 * border_size < chunk_size
-    and overlap_mode (all chunks batched, chunking and stitching inside the kernels; other values raise
-    ``ValueError``); any other model goes chunk by chunk through the functions above."""
+    runs as ONE call of the CUDA path for every chunk_size up to its max_chunk_size (1500 unless loaded with more),
+    border_size with 0 <= 2 * border_size < chunk_size and overlap_mode (all chunks batched, chunking and stitching
+    inside the kernels; other values raise ``ValueError``); any other model goes chunk by chunk through the functions
+    above.  With border_size 0 and chunk_size >= the piece's length the piece runs as one sequence."""
     if isinstance(model, BeatThisB200):
-        chunking = engine_chunking(chunk_size, border_size, overlap_mode)
+        chunking = engine_chunking(chunk_size, border_size, overlap_mode, model.max_chunk_size)
         spect = torch.as_tensor(spect, dtype=torch.float32, device=model.device).contiguous()
         beat, down = model.engine.spect2frames_cat(spect, [0, spect.shape[0]], chunking)
         return {"beat": beat, "downbeat": down}
@@ -206,11 +232,12 @@ def split_predict_aggregate(spect: torch.Tensor, chunk_size: int, border_size: i
 class Spect2Frames:
     """Framewise beat / downbeat logits from a spectrogram (reference inference.py:233-257)."""
 
-    def __init__(self, checkpoint_path="final0", device="cuda", float16=False):
+    def __init__(self, checkpoint_path="final0", device="cuda", float16=False, max_chunk_size=BT_CHUNK):
+        """max_chunk_size: the longest chunk_size spects2frames / frames_batch take (load_model)."""
         super().__init__()
         self.device = torch.device(device)
         self.float16 = float16
-        self.model = load_model(checkpoint_path, self.device, float16)
+        self.model = load_model(checkpoint_path, self.device, float16, max_chunk_size=max_chunk_size)
         self.device = self.model.device
 
     def spect2frames(self, spect):
@@ -223,7 +250,7 @@ class Spect2Frames:
     def spects2frames(self, spects, chunk_size: int = 1500, border_size: int = 6, overlap_mode: str = "keep_first"):
         """Batched variant: list of [T_i,128] tensors -> list of (beat, downbeat), every piece cut and stitched as
         split_predict_aggregate(spect, chunk_size, border_size, overlap_mode, model) does, all in one call."""
-        chunking = engine_chunking(chunk_size, border_size, overlap_mode)
+        chunking = engine_chunking(chunk_size, border_size, overlap_mode, self.model.max_chunk_size)
         spects = [torch.as_tensor(s, dtype=torch.float32, device=self.device) for s in spects]
         fo = [0]
         for s in spects:
@@ -253,8 +280,9 @@ class Audio2Frames(Spect2Frames):
 
     _want = "frames"
 
-    def __init__(self, checkpoint_path="final0", device="cuda", float16=False, resampler="device"):
-        super().__init__(checkpoint_path, device, float16)
+    def __init__(self, checkpoint_path="final0", device="cuda", float16=False, resampler="device",
+                 max_chunk_size=BT_CHUNK):
+        super().__init__(checkpoint_path, device, float16, max_chunk_size)
         self._init_front(resampler)
 
     def _init_front(self, resampler="device"):
@@ -309,7 +337,7 @@ class Audio2Frames(Spect2Frames):
     def _run_groups(self, arrays, sr, want, chunking=None):
         """Generator over groups: (first index, last index + 1, pipeline result)."""
         pipe = self.pipeline
-        groups = plan_groups([chunk_cost(a.shape[0], sr) for a in arrays], GROUP_CHUNKS, GROUP_CLIPS)
+        groups = _plan_groups([a.shape[0] for a in arrays], sr, chunking)
         try:
             results = pipe.run(len(groups),
                                lambda g: pipe.submit_signals(arrays[groups[g][0] : groups[g][1]], sr, want, chunking))
@@ -342,8 +370,8 @@ class Audio2Beats(Audio2Frames):
     inference.py:284-303)."""
 
     def __init__(self, checkpoint_path="final0", device="cuda", float16=False, dbn=False, resampler="device",
-                 dbn_impl="auto"):
-        super().__init__(checkpoint_path, device, float16, resampler)
+                 dbn_impl="auto", max_chunk_size=BT_CHUNK):
+        super().__init__(checkpoint_path, device, float16, resampler, max_chunk_size)
         self._init_post(dbn, dbn_impl)
 
     def _init_post(self, dbn=False, dbn_impl="auto"):
@@ -489,8 +517,9 @@ class File2Beats(Audio2Beats):
     def frames_batch(self, audio_paths, chunk_size: int = 1500, border_size: int = 6, overlap_mode: str = "keep_first"):
         """Framewise (beat, downbeat) logits of many files as device tensors, through the groups and kernels of batch()
         up to the post-processor: frames2beats.batch_cat of them gives batch()'s beats.  Every piece is cut and
-        stitched as split_predict_aggregate(spect, chunk_size, border_size, overlap_mode, model) does.  Errors raise."""
-        chunking = engine_chunking(chunk_size, border_size, overlap_mode)
+        stitched as split_predict_aggregate(spect, chunk_size, border_size, overlap_mode, model) does (chunk_size up to
+        the model's max_chunk_size).  Errors raise."""
+        chunking = engine_chunking(chunk_size, border_size, overlap_mode, self.model.max_chunk_size)
         paths = [str(p) for p in audio_paths]
         out = [None] * len(paths)
         infos, is_wav = self.probe(paths)
@@ -500,7 +529,7 @@ class File2Beats(Audio2Beats):
         pipe = self.pipeline
         for sr in sorted({infos[i].sample_rate for i in range(len(paths)) if is_wav[i]}):
             idx = [i for i in range(len(paths)) if is_wav[i] and infos[i].sample_rate == sr]
-            groups = plan_groups([chunk_cost(infos[i].frames, sr) for i in idx], GROUP_CHUNKS, GROUP_CLIPS)
+            groups = _plan_groups([infos[i].frames for i in idx], sr, chunking)
 
             def submit(g, idx=idx, groups=groups, sr=sr):
                 sel = idx[groups[g][0] : groups[g][1]]

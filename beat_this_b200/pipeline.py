@@ -63,6 +63,13 @@ def chunk_cost(n_samples: int, sr: int = 22050) -> int:
     return max(1, -(-frames // 1488))
 
 
+def padded_frames(n_samples: int, sr: int, chunk_size: int, border_size: int) -> int:
+    """Frames a clip of n_samples at `sr` Hz occupies in the waves of the C library under a chunking: its chunks
+    (split_piece, inference.py:119-125) times chunk_size, the most a chunk is padded to."""
+    frames = 1 + (int(n_samples) * 22050 // max(1, int(sr))) // 441
+    return max(1, -(-frames // (int(chunk_size) - 2 * int(border_size)))) * int(chunk_size)
+
+
 def _check_frames_route(want: str, chunking) -> None:
     """Only framewise logits take another chunking than 1500 / 6 / keep_first: the beat routes keep the reference's
     Audio2Beats, which always cuts that way (inference.py:244-254)."""

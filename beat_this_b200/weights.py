@@ -25,7 +25,7 @@ import torch
 from .preprocessing import mel_constants
 
 BN_EPS = 1e-5
-ROPE_POSITIONS = 1500  # chunk length (reference inference.py:247)
+ROPE_POSITIONS = 1500  # default maximum chunk length: the reference's inference chunk (inference.py:247)
 
 # BeatThis constructor signature (reference beat_tracker.py:39-49); load_model filters the
 # checkpoint's hyper_parameters to these names (inference.py:72-78).
@@ -93,7 +93,9 @@ def rope_tables(freqs: torch.Tensor, positions: int = ROPE_POSITIONS):
     return ang.cos(), ang.sin()
 
 
-def pack_parameters(state_dict: dict, hparams: dict) -> dict:
+def pack_parameters(state_dict: dict, hparams: dict, rope_positions: int = ROPE_POSITIONS) -> dict:
+    """rope_positions: rows of the RoPE tables, the longest chunk the loaded model will run (bt_max_chunk).  Rows
+    below 1500 do not depend on it."""
     sd = strip_prefixes(state_dict)
     hp = filter_hparams(hparams)
     out: dict = {}
@@ -105,7 +107,7 @@ def pack_parameters(state_dict: dict, hparams: dict) -> dict:
     else:  # checkpoints saved without the (constant) RoPE buffer
         d = hp["head_dim"]
         freqs = 1.0 / (10000 ** (torch.arange(0, d, 2).float() / d))
-    out["rope.cos"], out["rope.sin"] = rope_tables(freqs)
+    out["rope.cos"], out["rope.sin"] = rope_tables(freqs, rope_positions)
     # ---- stem ----------------------------------------------------------------------------------
     s1, b1 = _bn_fold(sd, "frontend.stem.bn1d")
     s2, b2 = _bn_fold(sd, "frontend.stem.bn2d")

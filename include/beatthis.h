@@ -85,8 +85,17 @@ int bt_create(bt_ctx** out, int device_ordinal, const bt_hparams* hp, int comput
 int bt_set_param(bt_ctx* ctx, const char* name, const float* data_host, int64_t count);
 
 /* Check that every parameter the model shape needs is present, build 16-bit operand copies and TMA
- * descriptors.  After this the weights are immutable.  (model.to(device).eval(), :87) */
+ * descriptors.  After this the weights are immutable.  (model.to(device).eval(), :87)
+ * "rope.cos" / "rope.sin" hold the RoPE rotation of positions 0 .. P - 1 ([P, 16] each, rotary_embedding_torch's
+ * fp32 cos / sin of pos * freqs); P sets the ctx's maximum chunk length (bt_max_chunk): BT_CHUNK for the reference's
+ * inference chunking, more for a model trained on longer sequences.  BT_ERR_PARAM unless both have P x 16 elements
+ * with BT_CHUNK <= P <= 256 * BT_CHUNK (the largest frame budget of a wave, bt_set_wave_chunks). */
 int bt_finalize(bt_ctx* ctx);
+
+/* The longest chunk this ctx runs (P of its RoPE tables; BT_CHUNK before bt_finalize): bt_spect2frames_chunked,
+ * bt_audio2frames_chunked and bt_forward_chunks refuse longer chunks with BT_ERR_ARG before anything is enqueued.
+ * BT_ERR_ARG for a NULL ctx. */
+int32_t bt_max_chunk(const bt_ctx* ctx);
 
 /* Free everything. */
 void bt_destroy(bt_ctx* ctx);
@@ -113,7 +122,7 @@ int64_t bt_plan_chunks(int64_t T, int64_t* starts, int64_t* lens, int64_t cap);
 #define BT_KEEP_LAST 1  /* ... from the later one                              */
 
 typedef struct bt_chunking {
-  int32_t chunk_size;   /* model frames per chunk, 1 <= chunk_size <= BT_CHUNK (the RoPE tables and workspace size) */
+  int32_t chunk_size;   /* model frames per chunk, 1 <= chunk_size <= the maximum chunk (BT_CHUNK, or bt_max_chunk)  */
   int32_t border;       /* frames cut from each side of a chunk's predictions, 0 <= 2 * border < chunk_size       */
   int32_t overlap_mode; /* BT_KEEP_FIRST or BT_KEEP_LAST                                                       */
 } bt_chunking;
@@ -132,9 +141,17 @@ typedef struct bt_chunking {
  * range ends at T (it starts at T - (c - b), or is the only chunk and T <= step).  Owned ranges are therefore
  * consecutive, non-empty and tile [0, T) exactly.
  * Writes up to `cap` entries of each non-NULL output array and returns the chunk count (the count needed when cap is
- * too small; 0 for T <= 0), or BT_ERR_ARG when ck is NULL or outside the limits above.  Pure host: no ctx, no CUDA. */
+ * too small; 0 for T <= 0), or BT_ERR_ARG when ck is NULL or outside the limits above with a maximum chunk of
+ * BT_CHUNK.  Pure host: no ctx, no CUDA. */
 int64_t bt_plan_chunking(int64_t T, const bt_chunking* ck, int64_t* starts, int64_t* lens, int64_t* own_lo,
                          int64_t* own_hi, int64_t cap);
+
+/* bt_plan_chunking with the maximum chunk `max_chunk` in place of BT_CHUNK (a ctx's bt_max_chunk): the same plan and
+ * outputs for 1 <= chunk_size <= max_chunk, BT_ERR_ARG otherwise.  bt_plan_chunking is this with max_chunk =
+ * BT_CHUNK.  A piece of T <= chunk_size - 2 * border frames is one chunk: with border 0 and chunk_size >= T the
+ * whole piece runs as one sequence, as in the reference. */
+int64_t bt_plan_chunking_max(int64_t T, const bt_chunking* ck, int32_t max_chunk, int64_t* starts, int64_t* lens,
+                             int64_t* own_lo, int64_t* own_hi, int64_t cap);
 
 /* ---- host front door: Audio2Frames.signal2spect's host half (inference.py:269-276) ------------------ */
 
@@ -262,7 +279,7 @@ int bt_dbn_track(const double* activations, const int64_t* frame_offsets, int32_
 int bt_spect2frames(bt_ctx* ctx, const float* spect_dev, const int64_t* frame_offsets_host,
                     int32_t n_clips, float* beat_dev, float* downbeat_dev, void* stream);
 
-/* BeatThis.forward (model/beat_tracker.py:188-192) on n_chunks spectrogram chunks of chunk_frames (<= 1500) frames
+/* BeatThis.forward (model/beat_tracker.py:188-192) on n_chunks spectrogram chunks of chunk_frames (<= bt_max_chunk) frames
  * each, chunks_dev = [n_chunks, chunk_frames, 128] fp32: no chunk planning, no borders cut -- the model call inside
  * split_predict_aggregate (inference.py:215), batched.  beat_dev / downbeat_dev: [n_chunks, chunk_frames] fp32. */
 int bt_forward_chunks(bt_ctx* ctx, const float* chunks_dev, int32_t n_chunks, int32_t chunk_frames,
@@ -277,7 +294,8 @@ int bt_audio2frames(bt_ctx* ctx, const float* audio_dev, const int64_t* sample_o
 /* bt_spect2frames / bt_audio2frames with the pieces cut and stitched by `ck` (see bt_plan_chunking) instead of
  * 1500 / 6 / keep_first: split_predict_aggregate (inference.py:188-230) with any valid chunk_size, border_size and
  * overlap_mode, every chunk of every clip batched into waves.  With { BT_CHUNK, BT_BORDER, BT_KEEP_FIRST } the results
- * are bitwise those of the plain entry points.  BT_ERR_ARG, before anything is enqueued, for an invalid ck. */
+ * are bitwise those of the plain entry points.  BT_ERR_ARG, before anything is enqueued, for an invalid ck; the
+ * maximum chunk_size is the ctx's bt_max_chunk. */
 int bt_spect2frames_chunked(bt_ctx* ctx, const float* spect_dev, const int64_t* frame_offsets_host, int32_t n_clips,
                             float* beat_dev, float* downbeat_dev, const bt_chunking* ck, void* stream);
 int bt_audio2frames_chunked(bt_ctx* ctx, const float* audio_dev, const int64_t* sample_offsets_host, int32_t n_clips,
@@ -400,9 +418,11 @@ int bt_beat_loss_backward(bt_ctx* ctx, const float* preds_dev, const float* targ
 
 /* ---- introspection / tuning ----------------------------------------------------------------- */
 
-/* Upper bound on the chunks processed per wave (default 128; one wave = one launch of every
- * kernel of the forward pass).  The workspace (~46 MB per 1500-frame chunk on the 16-bit path) grows on
- * demand up to this many chunks. */
+/* Upper bound on the chunks processed per wave (1..256, default 128; one wave = one launch of every kernel of the
+ * forward pass).  The workspace is budgeted in padded frames: max(chunks x BT_CHUNK, bt_max_chunk) frames (~46 MB per
+ * 1500 frames on the 16-bit path), allocated on first use.  Chunks run longest first; a wave is padded to its longest
+ * chunk and closes before it would exceed `chunks` chunks or the frame budget, so chunks of up to BT_CHUNK frames
+ * form the same waves whatever bt_max_chunk is, and one chunk of bt_max_chunk frames always fits. */
 int bt_set_wave_chunks(bt_ctx* ctx, int32_t chunks);
 
 /* Number of kernel launches issued by this ctx since creation (bench.py "gpu_launches"). */
