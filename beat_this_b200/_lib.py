@@ -102,6 +102,18 @@ class bt_loss_params(ctypes.Structure):
     ]
 
 
+class bt_debug_chunk(ctypes.Structure):
+    _fields_ = [
+        ("frame_base", c_int64),
+        ("T", c_int32),
+        ("start", c_int32),
+        ("out_base", c_int64),
+        ("write_lo", c_int32),
+        ("write_hi", c_int32),
+        ("len", c_int32),
+    ]
+
+
 BT_MEL_NORM_NONE = 0
 BT_MEL_NORM_FRAME_LENGTH = 1
 BT_MEL_NORM_WINDOW = 2
@@ -233,6 +245,19 @@ PROTOTYPES = {
         c_int,
         [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int32,
          c_void_p],
+    ),
+    "bt_debug_stem": (
+        c_int,
+        [c_void_p, c_void_p, c_int64, POINTER(bt_debug_chunk), c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p,
+         c_void_p, c_int64, c_void_p],
+    ),
+    "bt_debug_zero_tail": (
+        c_int, [c_void_p, c_void_p, c_int32, POINTER(bt_debug_chunk), c_int32, c_int32, c_int32, c_int32, c_int64, c_void_p],
+    ),
+    "bt_debug_head": (
+        c_int,
+        [c_void_p, c_void_p, c_int32, c_void_p, c_void_p, POINTER(bt_debug_chunk), c_int32, c_int32, c_int32, c_void_p,
+         c_void_p, c_int64, c_void_p],
     ),
 }
 

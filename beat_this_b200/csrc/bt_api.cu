@@ -692,7 +692,7 @@ cudaError_t to_h16_operand(DeviceBuffer<>& buf, const float* src, int64_t n, cud
 // ================================================================================== C ABI
 extern "C" {
 
-int bt_version(void) { return 207; }
+int bt_version(void) { return 208; }
 
 const char* bt_act_dtype(void) {
 #if defined(BT_ACT_BF16)
@@ -1721,6 +1721,117 @@ int bt_debug_fused_ff(bt_ctx* c, float* x_dev, const float* w1_dev, const float*
   const cudaError_t se = cudaStreamSynchronize(st);
   if (rc == BT_OK && se != cudaSuccess) rc = fail(c, BT_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(se));
   return rc;
+}
+
+}  // extern "C"
+
+namespace {
+
+// The public chunk entries as the kernels' ChunkSrc, field by field (the internal layout stays private).
+std::vector<ChunkSrc> chunk_table(const bt_debug_chunk* chunks, int32_t n) {
+  std::vector<ChunkSrc> v(n);
+  for (int32_t i = 0; i < n; ++i) {
+    ChunkSrc& s = v[i];
+    s.frame_base = chunks[i].frame_base;
+    s.T = chunks[i].T;
+    s.start = chunks[i].start;
+    s.out_base = chunks[i].out_base;
+    s.write_lo = chunks[i].write_lo;
+    s.write_hi = chunks[i].write_hi;
+    s.len = chunks[i].len;
+    s.pad_ = 0;
+  }
+  return v;
+}
+
+// Uploads the checked table through the staging ring, launches one kernel (launch(table_dev)) under the profile
+// name `what` and waits for it.
+template <class Launch>
+int run_chunk_hook(bt_ctx* c, const char* fn, const char* what, const bt_debug_chunk* chunks, int32_t n, void* stream,
+                   Launch launch) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  BT_CUDA(c, cudaSetDevice(c->device));
+  prof_mark(c, st);
+  const std::vector<ChunkSrc> table = chunk_table(chunks, n);
+  const ChunkSrc* dev = nullptr;
+  int rc = stage(c, st, {{table.data(), table.size()}}, &dev);
+  if (rc != BT_OK) return rc;
+  launch(dev, st);
+  rc = check_launch(c, what, st);
+  const cudaError_t se = cudaStreamSynchronize(st);
+  if (rc == BT_OK && se != cudaSuccess) rc = fail(c, BT_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(se));
+  return rc;
+}
+
+}  // namespace
+
+extern "C" {
+
+int bt_debug_stem(bt_ctx* c, const float* spect_dev, int64_t spect_frames, const bt_debug_chunk* chunks_host,
+                  int32_t n_chunks, int32_t L, const float* bn1_scale_dev, const float* bn1_shift_dev, const float* w_dev,
+                  const float* bias_dev, float* out_dev, int64_t out_count, void* stream) {
+  if (!c) return BT_ERR_ARG;
+  const char* fn = "bt_debug_stem";
+  if (!spect_dev || !chunks_host || !bn1_scale_dev || !bn1_shift_dev || !w_dev || !bias_dev || !out_dev ||
+      !aligned16(spect_dev) || !aligned16(out_dev))
+    return fail(c, BT_ERR_ARG, "%s: null argument, or spect / out not 16-byte aligned (float4 loads and stores)", fn);
+  if (n_chunks < 1 || n_chunks > 65535 || L < 1 || L > kMaxChunkCap)
+    return fail(c, BT_ERR_ARG, "%s: need 1 <= n_chunks <= 65535 and 1 <= L <= %lld", fn, (long long)kMaxChunkCap);
+  for (int32_t i = 0; i < n_chunks; ++i) {
+    const bt_debug_chunk& k = chunks_host[i];
+    if (k.T < 1 || k.len < 1 || k.len > L || k.frame_base < 0 || k.frame_base > spect_frames - k.T)
+      return fail(c, BT_ERR_ARG, "%s: chunk %d needs T >= 1, 1 <= len <= L and its clip inside the %lld spectrogram "
+                  "frames", fn, i, (long long)spect_frames);
+  }
+  if (out_count < static_cast<int64_t>(n_chunks) * 32 * L * 32)
+    return fail(c, BT_ERR_ARG, "%s: out holds %lld floats, fewer than n_chunks * 32 * L * 32", fn, (long long)out_count);
+  return run_chunk_hook(c, fn, "stem", chunks_host, n_chunks, stream, [&](const ChunkSrc* t, cudaStream_t st) {
+    launch_stem(spect_dev, t, n_chunks, L, bn1_scale_dev, bn1_shift_dev, w_dev, bias_dev, out_dev, st);
+  });
+}
+
+int bt_debug_zero_tail(bt_ctx* c, void* buf_dev, int32_t elem_bytes, const bt_debug_chunk* chunks_host,
+                       int32_t n_chunks, int32_t F, int32_t L, int32_t C, int64_t buf_bytes, void* stream) {
+  if (!c) return BT_ERR_ARG;
+  const char* fn = "bt_debug_zero_tail";
+  if (!buf_dev || !chunks_host || !aligned16(buf_dev))
+    return fail(c, BT_ERR_ARG, "%s: null argument, or buf not 16-byte aligned", fn);
+  if ((elem_bytes != 2 && elem_bytes != 4) || C < 1 || (static_cast<int64_t>(C) * elem_bytes) % 16 != 0 ||
+      n_chunks < 1 || F < 1 || static_cast<int64_t>(n_chunks) * F > INT32_MAX || L < 1 || L > kMaxChunkCap)
+    return fail(c, BT_ERR_ARG, "%s: need elem_bytes 2 or 4, C * elem_bytes a multiple of 16, n_chunks, F >= 1 with "
+                "n_chunks * F < 2^31 and 1 <= L <= %lld", fn, (long long)kMaxChunkCap);
+  for (int32_t i = 0; i < n_chunks; ++i)
+    if (chunks_host[i].len < 1 || chunks_host[i].len > L)
+      return fail(c, BT_ERR_ARG, "%s: chunk %d has len %d outside [1, L]", fn, i, chunks_host[i].len);
+  if (buf_bytes / elem_bytes / C / L / F < n_chunks)
+    return fail(c, BT_ERR_ARG, "%s: buf holds %lld bytes, fewer than n_chunks * F * L * C elements", fn,
+                (long long)buf_bytes);
+  return run_chunk_hook(c, fn, "zero_tail", chunks_host, n_chunks, stream, [&](const ChunkSrc* t, cudaStream_t st) {
+    launch_zero_tail(buf_dev, elem_bytes, t, n_chunks, F, L, C, st);
+  });
+}
+
+int bt_debug_head(bt_ctx* c, const float* x_dev, int32_t D, const float* w_dev, const float* b_dev,
+                  const bt_debug_chunk* chunks_host, int32_t n_chunks, int32_t L, int32_t sum_head, float* beat_dev,
+                  float* down_dev, int64_t out_count, void* stream) {
+  if (!c) return BT_ERR_ARG;
+  const char* fn = "bt_debug_head";
+  if (!x_dev || !w_dev || !b_dev || !chunks_host || !beat_dev || !down_dev)
+    return fail(c, BT_ERR_ARG, "%s: null argument", fn);
+  if (D < 64 || D > 1024 || D % 64 != 0 || n_chunks < 1 || L < 1 || static_cast<int64_t>(n_chunks) * L > INT32_MAX)
+    return fail(c, BT_ERR_ARG, "%s: need D a multiple of 64 in [64, 1024], n_chunks, L >= 1 and n_chunks * L < 2^31", fn);
+  for (int32_t i = 0; i < n_chunks; ++i) {
+    const bt_debug_chunk& k = chunks_host[i];
+    if (k.write_lo < 0 || k.write_lo > k.write_hi || k.write_hi > L)
+      return fail(c, BT_ERR_ARG, "%s: chunk %d owns [%d, %d), not inside [0, L]", fn, i, k.write_lo, k.write_hi);
+    const int64_t first = k.out_base + k.start + k.write_lo, last = k.out_base + k.start + k.write_hi - 1;
+    if (k.write_lo < k.write_hi && (first < 0 || last >= out_count))
+      return fail(c, BT_ERR_ARG, "%s: chunk %d writes frames [%lld, %lld], outside [0, %lld)", fn, i, (long long)first,
+                  (long long)last, (long long)out_count);
+  }
+  return run_chunk_hook(c, fn, "head", chunks_host, n_chunks, stream, [&](const ChunkSrc* t, cudaStream_t st) {
+    launch_head(x_dev, D, w_dev, b_dev, t, n_chunks, L, beat_dev, down_dev, sum_head ? 1 : 0, st);
+  });
 }
 
 }  // extern "C"

@@ -526,3 +526,33 @@ class Engine:
         code = self.lib.bt_debug_fused_ff(self.ctx, p(x, n * C), p(w1, 4 * C * C), p(b1, 4 * C), p(w2, 4 * C * C),
                                           p(b2, C), p(o, n * C), p(wout, C * C), p(xb_out, n * C), M, C, self._stream())
         _lib.check(self.lib, self.ctx, code)
+
+    # The chunk-table hooks take the table as a sequence of (frame_base, T, start, out_base, write_lo, write_hi, len)
+    # tuples (bt_debug_chunk); the library checks the table against the buffer lengths it is given.
+    @staticmethod
+    def _chunk_table(chunks):
+        return (_lib.bt_debug_chunk * max(len(chunks), 1))(*[_lib.bt_debug_chunk(*map(int, c)) for c in chunks])
+
+    def debug_stem(self, spect, chunks, L: int, bn1_scale, bn1_shift, w, bias, out):
+        """bt_debug_stem: out [len(chunks), 32, L, 32] (fp32, in place) from spect [frames, 128] through stem_kernel."""
+        p = self._dev_ptr
+        code = self.lib.bt_debug_stem(self.ctx, p(spect), spect.numel() // 128, self._chunk_table(chunks), len(chunks), L,
+                                      p(bn1_scale, 128), p(bn1_shift, 128), p(w, 32 * 12), p(bias, 32), p(out), out.numel(),
+                                      self._stream())
+        _lib.check(self.lib, self.ctx, code)
+
+    def debug_zero_tail(self, buf, chunks, F: int, L: int, C: int):
+        """bt_debug_zero_tail: rows [len, L) of every plane of buf [len(chunks), F, L, C] (fp32 or 16-bit, in place)
+        cleared through zero_tail_kernel."""
+        assert buf.is_cuda and buf.is_contiguous() and buf.element_size() in (2, 4)
+        code = self.lib.bt_debug_zero_tail(self.ctx, c_void_p(buf.data_ptr()), buf.element_size(), self._chunk_table(chunks),
+                                           len(chunks), F, L, C, buf.numel() * buf.element_size(), self._stream())
+        _lib.check(self.lib, self.ctx, code)
+
+    def debug_head(self, x, D: int, w, b, chunks, L: int, sum_head: bool, beat, down):
+        """bt_debug_head: the owned frames of beat / down (fp32, in place) from x [len(chunks), L, D] through head_kernel."""
+        p = self._dev_ptr
+        assert beat.numel() == down.numel()
+        code = self.lib.bt_debug_head(self.ctx, p(x, len(chunks) * L * D), D, p(w, 2 * D), p(b, 2), self._chunk_table(chunks),
+                                      len(chunks), L, int(bool(sum_head)), p(beat), p(down), beat.numel(), self._stream())
+        _lib.check(self.lib, self.ctx, code)

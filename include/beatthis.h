@@ -524,6 +524,44 @@ int bt_debug_fused_ff(bt_ctx* ctx, float* x_dev, const float* w1_dev, const floa
                       const float* b2_dev, const float* o_dev, const float* wout_dev, float* xb_dev, int64_t M, int32_t C,
                       void* stream);
 
+/* One entry of the chunk table the forward pass hands its stem, zero_tail and head kernels (one chunk of a wave):
+ * the clip is spectrogram frames [frame_base, frame_base + T) and output frames [out_base, out_base + T); the chunk
+ * starts at clip frame `start` (may be negative or run past T: those frames are zero before BN1d) and has `len`
+ * frames (rows [len, L) of its planes are padding); it owns chunk-local frames [write_lo, write_hi). */
+typedef struct bt_debug_chunk {
+  int64_t frame_base;
+  int32_t T, start;
+  int64_t out_base;
+  int32_t write_lo, write_hi, len;
+} bt_debug_chunk;
+
+/* Test hooks of the kernels that read the chunk table.  Parameters are fp32 device arrays, so a weight-less ctx will
+ * do; chunks_host is uploaded through the ctx's staging ring, as the forward pass uploads its table.  Each launches
+ * the kernel the forward pass launches, once, and synchronises the stream; each returns BT_ERR_ARG, before anything is
+ * enqueued, for a table or geometry that would take the kernel outside the buffers described.
+ *
+ * bt_debug_stem: stem_kernel over n_chunks chunks (1..65535) of padded length L (1..384000) gathered from spect_dev
+ * [spect_frames, 128]; bn1_scale / bn1_shift [128], w [32, 4, 3] (BN2d folded), bias [32]; out_dev [n_chunks, 32, L,
+ * 32] holds out_count >= n_chunks * 32 * L * 32 floats.  spect_dev and out_dev must be 16-byte aligned; every chunk
+ * needs T >= 1, 1 <= len <= L and its clip inside [0, spect_frames). */
+int bt_debug_stem(bt_ctx* ctx, const float* spect_dev, int64_t spect_frames, const bt_debug_chunk* chunks_host,
+                  int32_t n_chunks, int32_t L, const float* bn1_scale_dev, const float* bn1_shift_dev, const float* w_dev,
+                  const float* bias_dev, float* out_dev, int64_t out_count, void* stream);
+
+/* bt_debug_zero_tail: zero_tail_kernel: rows [len, L) of every plane of buf_dev [n_chunks, F, L, C] (elements of
+ * elem_bytes 2 or 4, buf_bytes bytes, 16-byte aligned) become 0.  Needs C * elem_bytes a multiple of 16, n_chunks,
+ * F >= 1 with n_chunks * F < 2^31, 1 <= len <= L <= 384000 for every chunk (only len is read). */
+int bt_debug_zero_tail(bt_ctx* ctx, void* buf_dev, int32_t elem_bytes, const bt_debug_chunk* chunks_host,
+                       int32_t n_chunks, int32_t F, int32_t L, int32_t C, int64_t buf_bytes, void* stream);
+
+/* bt_debug_head: head_kernel on x_dev [n_chunks, L, D] (D a multiple of 64 in [64, 1024], n_chunks * L < 2^31):
+ * o_j = (x . w_j) / max(||x||, 1e-12) + b_j with w [2, D], b [2]; beat = o0 + o1 (sum_head != 0) or o0, down = o1,
+ * stored at out_base + start + t for every owned frame t of a chunk.  Each owned range must lie in [0, L] and every
+ * owned frame's index in [0, out_count), the length of beat_dev and down_dev. */
+int bt_debug_head(bt_ctx* ctx, const float* x_dev, int32_t D, const float* w_dev, const float* b_dev,
+                  const bt_debug_chunk* chunks_host, int32_t n_chunks, int32_t L, int32_t sum_head, float* beat_dev,
+                  float* down_dev, int64_t out_count, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -45,17 +45,23 @@ def _check_bound(out, x, fb, c, what):
 
 
 def _run(mel, signals, fill=float("nan")):
-    """bt_logmel_config into an output pre-filled with `fill`, so that a missing store shows."""
+    """bt_logmel_config (bt_logmel for the defaults, whose LogMelSpect has no tables) into an output pre-filled with
+    `fill`, so that a missing store shows."""
     eng, t = mel.engine, mel.tables
     sigs = [torch.as_tensor(s, dtype=torch.float32, device=eng.device) for s in signals]
     so = np.concatenate([[0], np.cumsum([len(s) for s in sigs])]).tolist()
-    fo = eng.frame_offsets(so, t.hop_length)
-    spect = torch.full((fo[-1], t.n_mels), fill, dtype=torch.float32, device=eng.device)
-    d = mel.device_tables
-    code = eng.lib.bt_logmel_config(
-        eng.ctx, ctypes.byref(t.config), *(c_void_p(d[k].data_ptr()) for k in ("window", "twiddle", "fb_start", "fb_ptr", "fb_w")),
-        c_void_p(torch.cat(sigs).data_ptr()), (ctypes.c_int64 * len(so))(*so), len(sigs), c_void_p(spect.data_ptr()),
-        (ctypes.c_int64 * len(fo))(*fo), eng._stream())
+    hop, n_mels = (441, 128) if t is None else (t.hop_length, t.n_mels)
+    fo = eng.frame_offsets(so, hop)
+    spect = torch.full((fo[-1], n_mels), fill, dtype=torch.float32, device=eng.device)
+    audio, so_h, fo_h = torch.cat(sigs), (ctypes.c_int64 * len(so))(*so), (ctypes.c_int64 * len(fo))(*fo)
+    if t is None:
+        code = eng.lib.bt_logmel(eng.ctx, c_void_p(audio.data_ptr()), so_h, len(sigs), c_void_p(spect.data_ptr()), fo_h,
+                                 eng._stream())
+    else:
+        d = mel.device_tables
+        code = eng.lib.bt_logmel_config(
+            eng.ctx, ctypes.byref(t.config), *(c_void_p(d[k].data_ptr()) for k in ("window", "twiddle", "fb_start", "fb_ptr", "fb_w")),
+            c_void_p(audio.data_ptr()), so_h, len(sigs), c_void_p(spect.data_ptr()), fo_h, eng._stream())
     assert code == 0, eng.lib.bt_last_error(eng.ctx)
     torch.cuda.synchronize()
     return [spect[fo[i]:fo[i + 1]].cpu().numpy() for i in range(len(sigs))]
@@ -104,14 +110,19 @@ def test_issue_example_matches_reference(dev, fixture):
          normalized="window", power=0.5, log_multiplier=1000),
     dict(sample_rate=44100, n_fft=8192, hop_length=441, f_min=30, f_max=16000, n_mels=256, mel_scale="slaney",
          normalized="frame_length", power=1, log_multiplier=1000),
+    # the defaults: the model path's logmel_kernel (bt_logmel), every Audio2Frames call and the benchmark run it
+    dict(sample_rate=22050, n_fft=1024, hop_length=441, f_min=30, f_max=11000, n_mels=128, mel_scale="slaney",
+         normalized="frame_length", power=1, log_multiplier=1000),
 ])
 def test_ragged_batches_edges_and_repeatability(dev, cfg):
     """Batches of 1, 7 and 213 clips (enough frame groups for several grid-stride rounds at every n_fft), lengths of
     exactly n_fft // 2 + 1, = 0 and = hop - 1 (mod hop), and clips far longer than one CTA's span; outputs start as NaN
     and must match the float64 bound; a second run is bitwise the first."""
-    from beat_this_b200.preprocessing import LogMelSpect
+    from beat_this_b200.preprocessing import LogMelSpect, MelTables
 
     mel = LogMelSpect(**cfg, device=dev)
+    assert (mel.tables is None) == (tuple(cfg.values()) == LogMelSpect.DEFAULTS)
+    tables = mel.tables if mel.tables is not None else MelTables(*LogMelSpect.DEFAULTS)
     n, hop = cfg["n_fft"], cfg["hop_length"]
     rng = np.random.default_rng(n + hop)
     base = [n // 2 + 1, hop * (n // hop + 3), hop * (n // hop + 3) + hop - 1, 40 * n + 13]
@@ -122,7 +133,7 @@ def test_ragged_batches_edges_and_repeatability(dev, cfg):
         outs = _run(mel, sigs)
         for s, o in zip(sigs, outs):
             assert o.shape == (1 + len(s) // hop, cfg["n_mels"])
-        fb = mel.tables.fb.numpy()
+        fb = tables.fb.numpy()
         for i in sorted(set(rng.integers(0, n_clips, 6).tolist()) | {0, n_clips - 1}):
             _check_bound(outs[i], sigs[i], fb, cfg, f"{n_clips} clips, clip {i}")
         again = _run(mel, sigs, fill=0.0)
