@@ -210,6 +210,11 @@ PROTOTYPES = {
         c_int,
         [c_void_p, c_void_p, c_void_p, POINTER(c_int64), c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_void_p],
     ),
+    "bt_peakpick_fps": (
+        c_int,
+        [c_void_p, c_void_p, c_void_p, POINTER(c_int64), c_int32, c_double, c_void_p, c_void_p, c_void_p, c_void_p, c_int32,
+         c_void_p],
+    ),
     "bt_set_wave_chunks": (c_int, [c_void_p, c_int32]),
     "bt_launch_count": (c_int64, [c_void_p]),
     "bt_profile_enable": (c_int, [c_void_p, c_int]),

@@ -692,7 +692,7 @@ cudaError_t to_h16_operand(DeviceBuffer<>& buf, const float* src, int64_t n, cud
 // ================================================================================== C ABI
 extern "C" {
 
-int bt_version(void) { return 208; }
+int bt_version(void) { return 209; }
 
 const char* bt_act_dtype(void) {
 #if defined(BT_ACT_BF16)
@@ -1119,14 +1119,17 @@ int bt_audio2frames_chunked(bt_ctx* c, const float* audio_dev, const int64_t* sa
                       stream, "bt_audio2frames_chunked");
 }
 
-int bt_peakpick(bt_ctx* c, const float* beat_dev, const float* downbeat_dev, const int64_t* frame_offsets_host,
-                int32_t n_clips, double* beat_times_dev, int32_t* n_beats_dev, double* down_times_dev,
-                int32_t* n_down_dev, int32_t max_peaks, void* stream) {
+namespace {
+
+int peakpick(bt_ctx* c, const char* fn, const float* beat_dev, const float* downbeat_dev,
+             const int64_t* frame_offsets_host, int32_t n_clips, double* beat_times_dev, int32_t* n_beats_dev,
+             double* down_times_dev, int32_t* n_down_dev, int32_t max_peaks, double fps, void* stream) {
   if (!c) return BT_ERR_ARG;
+  if (!std::isfinite(fps) || !(fps > 0)) return fail(c, BT_ERR_ARG, "%s: fps must be finite and > 0", fn);
   if (n_clips <= 0) return BT_OK;
   if (!beat_dev || !downbeat_dev || !frame_offsets_host || !beat_times_dev || !n_beats_dev || !down_times_dev ||
       !n_down_dev || max_peaks < 1)
-    return fail(c, BT_ERR_ARG, "bt_peakpick: bad argument");
+    return fail(c, BT_ERR_ARG, "%s: bad argument", fn);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   BT_CUDA(c, cudaSetDevice(c->device));
   prof_mark(c, st);
@@ -1134,9 +1137,25 @@ int bt_peakpick(bt_ctx* c, const float* beat_dev, const float* downbeat_dev, con
   const int r = stage(c, st, {{frame_offsets_host, static_cast<size_t>(n_clips + 1)}}, &fo);
   if (r != BT_OK) return r;
   launch_peakpick(beat_dev, downbeat_dev, fo, n_clips, beat_times_dev,
-                  n_beats_dev, down_times_dev, n_down_dev, max_peaks, st);
+                  n_beats_dev, down_times_dev, n_down_dev, max_peaks, fps, st);
   BT_LAUNCHED(c, "peakpick", st);
   return BT_OK;
+}
+
+}  // namespace
+
+int bt_peakpick(bt_ctx* c, const float* beat_dev, const float* downbeat_dev, const int64_t* frame_offsets_host,
+                int32_t n_clips, double* beat_times_dev, int32_t* n_beats_dev, double* down_times_dev,
+                int32_t* n_down_dev, int32_t max_peaks, void* stream) {
+  return peakpick(c, "bt_peakpick", beat_dev, downbeat_dev, frame_offsets_host, n_clips, beat_times_dev, n_beats_dev,
+                  down_times_dev, n_down_dev, max_peaks, 50.0, stream);
+}
+
+int bt_peakpick_fps(bt_ctx* c, const float* beat_dev, const float* downbeat_dev, const int64_t* frame_offsets_host,
+                    int32_t n_clips, double fps, double* beat_times_dev, int32_t* n_beats_dev, double* down_times_dev,
+                    int32_t* n_down_dev, int32_t max_peaks, void* stream) {
+  return peakpick(c, "bt_peakpick_fps", beat_dev, downbeat_dev, frame_offsets_host, n_clips, beat_times_dev,
+                  n_beats_dev, down_times_dev, n_down_dev, max_peaks, fps, stream);
 }
 
 namespace {

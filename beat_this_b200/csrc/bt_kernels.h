@@ -106,7 +106,7 @@ cudaError_t launch_logmel_config(int log2n, const float* audio, const int64_t* s
                                  const MelConfigArgs& p, cudaStream_t st);
 void launch_peakpick(const float* beat, const float* down, const int64_t* frame_off_dev, int n_clips,
                      double* beat_t, int32_t* n_beat, double* down_t, int32_t* n_down,
-                     int max_peaks, cudaStream_t st);
+                     int max_peaks, double fps, cudaStream_t st);
 // ---- DBN post-processor on the device (kernels_dbn.cu) ---------------------------------------------------------
 // One bar model of the bar-pointer HMM (dbn_model.h BarModel), tables on the device.  State s = b * per_beat +
 // first[k] + p (beat b, tempo k, position p < intervals[k]); positions p < nrun[b * n_int + k] observe the (down)beat

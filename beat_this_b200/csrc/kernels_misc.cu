@@ -931,7 +931,8 @@ void launch_head(const float* x, int D, const float* w, const float* b, const Ch
 // minimal postprocessor (reference model/postprocessor.py:85-136, deduplicate_peaks
 // :176-197): peak <=> x[t] == max(x[t-3..t+3]) and x[t] > 0; runs of peaks at most one
 // frame from the running mean are merged into the running mean (float64, like the Python
-// loop); times = frame / 50; every downbeat snaps to the nearest beat (first argmin); unique.
+// loop); times = frame / fps, one correctly rounded float64 division as numpy's; every downbeat snaps to the
+// nearest beat (first argmin); unique.
 // One CTA per clip: ordered compaction by ballot/prefix, then the short sequential part.
 // ------------------------------------------------------------------------------------------
 __device__ int compact_peaks(const float* __restrict__ x, int T, double* __restrict__ frames, int cap,
@@ -972,7 +973,7 @@ __device__ int compact_peaks(const float* __restrict__ x, int T, double* __restr
   return *s_base;
 }
 
-__device__ int dedup_to_times(double* p, int n) {
+__device__ int dedup_to_times(double* p, int n, double fps) {
   // deduplicate_peaks(width=1) followed by / fps; in place (output index <= input index)
   if (n == 0) return 0;
   int out = 0;
@@ -984,19 +985,19 @@ __device__ int dedup_to_times(double* p, int n) {
       c += 1.0;
       cur += (p2 - cur) / c;
     } else {
-      p[out++] = cur / 50.0;
+      p[out++] = cur / fps;
       cur = p2;
       c = 1.0;
     }
   }
-  p[out++] = cur / 50.0;
+  p[out++] = cur / fps;
   return out;
 }
 
 __global__ void __launch_bounds__(256)
 peakpick_kernel(const float* __restrict__ beat, const float* __restrict__ down,
                 const int64_t* __restrict__ frame_off, double* __restrict__ beat_t, int32_t* __restrict__ n_beat,
-                double* __restrict__ down_t, int32_t* __restrict__ n_down, int max_peaks) {
+                double* __restrict__ down_t, int32_t* __restrict__ n_down, int max_peaks, double fps) {
   __shared__ int s_warp[8];
   __shared__ int s_base;
   const int clip = blockIdx.x;
@@ -1015,8 +1016,8 @@ peakpick_kernel(const float* __restrict__ beat, const float* __restrict__ down,
       n_down[clip] = nd_raw;
       s_nb = -1;
     } else {
-      s_nb = dedup_to_times(bt_, nb_raw);
-      s_nd = dedup_to_times(dt_, nd_raw);
+      s_nb = dedup_to_times(bt_, nb_raw, fps);
+      s_nd = dedup_to_times(dt_, nd_raw, fps);
     }
   }
   __syncthreads();
@@ -1056,10 +1057,10 @@ peakpick_kernel(const float* __restrict__ beat, const float* __restrict__ down,
 
 void launch_peakpick(const float* beat, const float* down, const int64_t* frame_off_dev, int n_clips,
                      double* beat_t, int32_t* n_beat, double* down_t, int32_t* n_down, int max_peaks,
-                     cudaStream_t st) {
+                     double fps, cudaStream_t st) {
   if (n_clips <= 0) return;
   peakpick_kernel<<<n_clips, 256, 0, st>>>(beat, down, frame_off_dev, beat_t, n_beat, down_t, n_down,
-                                           max_peaks);
+                                           max_peaks, fps);
 }
 
 // ------------------------------------------------------------------------------------------ utils

@@ -287,9 +287,9 @@ class Engine:
         _lib.check(self.lib, self.ctx, code)
         return beat, down, fo
 
-    def peakpick_cat(self, beat: torch.Tensor, down: torch.Tensor, frame_offsets):
-        """Minimal postprocessor on device; returns a list of (beat_times, downbeat_times)
-        float64 numpy arrays, one pair per clip."""
+    def peakpick_cat(self, beat: torch.Tensor, down: torch.Tensor, frame_offsets, fps: float = 50):
+        """Minimal postprocessor on device for logits at `fps` frames per second (bt_peakpick_fps); returns a list of
+        (beat_times, downbeat_times) float64 numpy arrays, one pair per clip."""
         n = len(frame_offsets) - 1
         if n == 0:
             return []
@@ -297,9 +297,9 @@ class Engine:
         bt_t = torch.empty((n, max_peaks), dtype=torch.float64, device=self.device)
         dn_t = torch.empty((n, max_peaks), dtype=torch.float64, device=self.device)
         cnt = torch.zeros((2, n), dtype=torch.int32, device=self.device)
-        code = self.lib.bt_peakpick(self.ctx, c_void_p(beat.data_ptr()), c_void_p(down.data_ptr()), i64_array(frame_offsets), n,
-                                    c_void_p(bt_t.data_ptr()), c_void_p(cnt[0].data_ptr()), c_void_p(dn_t.data_ptr()),
-                                    c_void_p(cnt[1].data_ptr()), max_peaks, self._stream())
+        code = self.lib.bt_peakpick_fps(self.ctx, c_void_p(beat.data_ptr()), c_void_p(down.data_ptr()), i64_array(frame_offsets),
+                                        n, float(fps), c_void_p(bt_t.data_ptr()), c_void_p(cnt[0].data_ptr()),
+                                        c_void_p(dn_t.data_ptr()), c_void_p(cnt[1].data_ptr()), max_peaks, self._stream())
         _lib.check(self.lib, self.ctx, code)
         cnt_h = cnt.cpu().numpy()
         width = int(cnt_h.max()) if cnt_h.size else 0
@@ -309,7 +309,8 @@ class Engine:
         dn_h = dn_t[:, :width].cpu().numpy()
         return [(bt_h[i, : cnt_h[0, i]].copy(), dn_h[i, : cnt_h[1, i]].copy()) for i in range(n)]
 
-    def peakpick_async(self, beat: torch.Tensor, down: torch.Tensor, frame_offsets, slot: dict | None = None):
+    def peakpick_async(self, beat: torch.Tensor, down: torch.Tensor, frame_offsets, slot: dict | None = None,
+                       fps: float = 50):
         """Like peakpick_cat but without a host synchronisation: the timestamp arrays are copied to
         pinned host memory asynchronously on the current stream; call ``.result()`` on the returned
         handle (it waits on a CUDA event) to get the per-clip numpy arrays."""
@@ -325,9 +326,9 @@ class Engine:
             slot["cnt_h"] = torch.empty((2, n), dtype=torch.int32).pin_memory()
             slot["event"] = torch.cuda.Event()
         t, cnt = slot["times"], slot["cnt"]
-        code = self.lib.bt_peakpick(self.ctx, c_void_p(beat.data_ptr()), c_void_p(down.data_ptr()), i64_array(frame_offsets), n,
-                                    c_void_p(t[0].data_ptr()), c_void_p(cnt[0].data_ptr()), c_void_p(t[1].data_ptr()),
-                                    c_void_p(cnt[1].data_ptr()), max_peaks, self._stream())
+        code = self.lib.bt_peakpick_fps(self.ctx, c_void_p(beat.data_ptr()), c_void_p(down.data_ptr()), i64_array(frame_offsets),
+                                        n, float(fps), c_void_p(t[0].data_ptr()), c_void_p(cnt[0].data_ptr()),
+                                        c_void_p(t[1].data_ptr()), c_void_p(cnt[1].data_ptr()), max_peaks, self._stream())
         _lib.check(self.lib, self.ctx, code)
         slot["times_h"].copy_(t, non_blocking=True)
         slot["cnt_h"].copy_(cnt, non_blocking=True)

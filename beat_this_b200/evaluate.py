@@ -7,6 +7,8 @@
   path, restricts the truth to the piece (``prepare_annotations``, dataset.py:536-547) and scores beats and downbeats
   in one metric launch.  Its summary keys are the reference's (``_compute_metrics_target``, pl_module.py:131-160).
   With ``losses=True`` (``--losses``) it adds the test losses of the checkpoint's loss pair (``piece_losses``).
+  Truth, losses and post-processing use the frame rate of the predictions: the checkpoint's ``fps`` hyper-parameter
+  (50 when absent, as the reference's ``PLBeatThis``), or ``fps=`` / ``--fps``.
 * ``python -m beat_this_b200.evaluate`` is the command line counterpart of compute_paper_metrics.py.
 
     python -m beat_this_b200.evaluate --models final0.ckpt --data data          # prepared dataset layout
@@ -128,10 +130,10 @@ class EvalResult:
         return {k: {d: float(np.mean(self.metrics[k][ds == d])) for d in np.unique(ds)} for k in SUMMARY_KEYS}
 
 
-def horizon(times: np.ndarray, T: int) -> np.ndarray:
-    """Annotations inside a piece of T spectrogram frames: times in [0, T / 50) (prepare_annotations with
-    start_frame = 0, dataset.py:536-547)."""
-    return times[(times >= 0) & (times < T / FPS)]
+def horizon(times: np.ndarray, T: int, fps: float = FPS) -> np.ndarray:
+    """Annotations inside a piece of T spectrogram frames at `fps` frames per second: times in [0, T / fps)
+    (prepare_annotations with start_frame = 0, dataset.py:536-547)."""
+    return times[(times >= 0) & (times < T / fps)]
 
 
 def _frames_of_audio(runner, path) -> int:
@@ -150,10 +152,12 @@ def _frames_of_audio(runner, path) -> int:
     return 1 + n // 441
 
 
-def _predict(runner, pieces, group=64, logits=False):
+def _predict(runner, pieces, group=64, logits=False, post=None):
     """(beats, downbeats) and spectrogram length of every piece through the batched inference path; with `logits`,
     also every piece's (beat, downbeat) logits on the device (audio then goes through the frames path and the
-    runner's post-processor, which gives the same beats), else None."""
+    runner's post-processor, which gives the same beats), else None.  post: the post-processor of the spectrogram
+    pieces' logits (default: the runner's)."""
+    post = runner.frames2beats if post is None else post
     preds, frames, frame_logits = [None] * len(pieces), [0] * len(pieces), [None] * len(pieces)
     audio = [i for i, p in enumerate(pieces) if p.audio is not None]
     if audio and logits:
@@ -177,26 +181,26 @@ def _predict(runner, pieces, group=64, logits=False):
             fo.append(fo[-1] + b.shape[0])
         beat = torch.cat([b for b, _ in out]).contiguous()
         down = torch.cat([d for _, d in out]).contiguous()
-        for i, r, a, b, o in zip(idx, runner.frames2beats.batch_cat(beat, down, fo), fo[:-1], fo[1:], out):
+        for i, r, a, b, o in zip(idx, post.batch_cat(beat, down, fo), fo[:-1], fo[1:], out):
             preds[i], frames[i] = r, b - a
             if logits:
                 frame_logits[i] = o
     return preds, frames, frame_logits
 
 
-def framewise_truth(times, T: int) -> np.ndarray:
-    """prepare_annotations(item, 0, T, 50)'s framewise truth (reference dataset.py:512-534) as fp32: 1 at the frames
-    np.round(time * 50) (half to even) inside [0, T), 0 elsewhere."""
-    f = np.round(np.asarray(times, dtype=np.float64) * FPS).astype(np.int64)
+def framewise_truth(times, T: int, fps: float = FPS) -> np.ndarray:
+    """prepare_annotations(item, 0, T, fps)'s framewise truth (reference dataset.py:512-534) as fp32: 1 at the frames
+    np.round(time * fps) (half to even) inside [0, T), 0 elsewhere."""
+    f = np.round(np.asarray(times, dtype=np.float64) * fps).astype(np.int64)
     out = np.zeros(T, dtype=np.float32)
     out[f[(f >= 0) & (f < T)]] = 1
     return out
 
 
-def piece_losses(runner, pieces, logits) -> dict:
+def piece_losses(runner, pieces, logits, fps: float = FPS) -> dict:
     """The reference's test losses (test_step, pl_module.py:99-114,224-229) of every piece: the checkpoint's loss pair
-    (loss_from_hparams) on the full-piece logits against the framewise truth, the downbeat mask 0 for pieces without
-    downbeat annotations.  All beat rows in one bt_beat_loss call, all downbeat rows in another."""
+    (loss_from_hparams) on the full-piece logits against the framewise truth at `fps`, the downbeat mask 0 for pieces
+    without downbeat annotations.  All beat rows in one bt_beat_loss call, all downbeat rows in another."""
     from .loss import beat_loss_rows, loss_from_hparams, loss_spec
 
     dev = runner.model.device
@@ -204,7 +208,7 @@ def piece_losses(runner, pieces, logits) -> dict:
     out = {}
     for t, (target, module) in enumerate(zip(("beat", "downbeat"), loss_from_hparams(runner.model.checkpoint_hparams))):
         x = torch.cat([lg[t] for lg in logits]).contiguous()
-        truth = [framewise_truth(p.beats if t == 0 else p.downbeats, len(lg[t])) for p, lg in zip(pieces, logits)]
+        truth = [framewise_truth(p.beats if t == 0 else p.downbeats, len(lg[t]), fps) for p, lg in zip(pieces, logits)]
         y = torch.from_numpy(np.concatenate(truth)).to(dev)
         keep = [1.0 if t == 0 or p.has_downbeats else 0.0 for p in pieces]
         m = torch.from_numpy(np.repeat(np.asarray(keep, np.float32), np.diff(fo))).to(dev)
@@ -224,24 +228,39 @@ def make_runner(model, device="cuda", float16=True, dbn=False, dbn_impl="auto"):
 
 
 def evaluate(model_or_runner, items, min_beat_time=5.0, device="cuda", float16=True, dbn=False, dbn_impl="auto",
-             losses=False):
+             losses=False, fps=None):
     """Predict every Piece of `items` with the model (a File2Beats / Audio2Beats runner, a BeatThisB200 or a checkpoint;
     float16 / dbn / dbn_impl apply when a runner has to be built) and score it against its annotations: truth cut to
-    [0, T / 50) for a spectrogram of T frames, beats and downbeats of all pieces in one bt_beat_metrics launch.
+    [0, T / fps) for a spectrogram of T frames, beats and downbeats of all pieces in one bt_beat_metrics launch.
+    fps: the frame rate of the model's predictions (None: the checkpoint's ``fps`` hyper-parameter, 50 when absent).
+    The logits of stored spectrograms are post-processed at that rate; audio files go through the inference
+    classes' 50 fps front end, so audio pieces with another fps are a ValueError.
     "Cemgil_<target>" is the reference's mean of mir_eval's (cemgil, cemgil_max) pair (pl_module.py:157-160); both
     parts stay available as cemgil_<target> and cemgil_max_<target>.  Pieces without downbeat annotations score 0 on
     the downbeat keys, as in the reference.  With `losses`, metrics also hold every piece's test_loss_beat,
     test_loss_downbeat and test_loss (piece_losses), and summary their means."""
+    from .postprocessor import Postprocessor, check_fps
+
     runner = model_or_runner
     if not hasattr(runner, "frames2beats"):
         runner = make_runner(runner, device, float16, dbn, dbn_impl)
+    if fps is None:
+        fps = runner.model.checkpoint_hparams.get("fps", FPS)
+    check_fps(fps)
     pieces = list(items)
-    preds, frames, logits = _predict(runner, pieces, logits=losses)
+    post = runner.frames2beats
+    if fps != post.fps:
+        audio = [p.name for p in pieces if p.audio is not None]
+        if audio:
+            raise ValueError(f"{audio[0]}: audio is analysed at {post.fps} fps by the inference front end, not at the "
+                             f"model's {fps}; evaluate stored spectrograms at that rate instead")
+        post = Postprocessor(post.type, fps, engine=runner.model.engine, dbn_impl=post.dbn_impl)
+    preds, frames, logits = _predict(runner, pieces, logits=losses, post=post)
     est, ref = [], []
     for target in (0, 1):
         for p, pr, T in zip(pieces, preds, frames):
             truth = check_times(p.beats if target == 0 else p.downbeats, f"{p.name}: truth")
-            ref.append(horizon(truth, T))
+            ref.append(horizon(truth, T, fps))
             est.append(pr[target])
     rows = beat_metrics(est, ref, min_beat_time=min_beat_time, device=runner.model.device)
     n = len(pieces)
@@ -259,7 +278,7 @@ def evaluate(model_or_runner, items, min_beat_time=5.0, device="cuda", float16=T
     metrics = {k: metrics[k] for k in (*SUMMARY_KEYS, *[k for k in metrics if k not in SUMMARY_KEYS])}
     keys = SUMMARY_KEYS
     if losses and n:
-        metrics.update(piece_losses(runner, pieces, logits))
+        metrics.update(piece_losses(runner, pieces, logits, fps))
         keys = (*SUMMARY_KEYS, *LOSS_KEYS)
     summary = {k: float(np.mean(metrics[k])) if n else float("nan") for k in keys}
     return EvalResult(pieces, metrics, preds, summary)
@@ -353,6 +372,9 @@ def build_parser() -> argparse.ArgumentParser:
     add("--dump-predictions", metavar="FILENAME", default=None, help="write the predictions to this .npz file")
     add("--losses", action="store_true",
         help="also report the test losses of the checkpoint's loss_type (test_loss_beat, test_loss_downbeat, test_loss)")
+    add("--fps", type=float, default=None,
+        help="frame rate of the model's predictions, for the truth and the post-processing (default: the checkpoint's "
+             "fps, else 50)")
     return ap
 
 
@@ -376,7 +398,7 @@ def _print_mean_std(summaries: list) -> None:
 
 
 def run(models, data=None, audio=None, annotations=None, items=None, gpu=0, eval_trim_beats=None, dbn=None,
-        dbn_impl="auto", float16=True, aggregation_type="mean-std", dump_predictions=None, losses=False) -> int:
+        dbn_impl="auto", float16=True, aggregation_type="mean-std", dump_predictions=None, losses=False, fps=None) -> int:
     from .inference import load_checkpoint
 
     if audio is not None and annotations is None:
@@ -393,8 +415,9 @@ def run(models, data=None, audio=None, annotations=None, items=None, gpu=0, eval
         hp = ckpt.get("hyper_parameters", {})
         trim = eval_trim_beats if eval_trim_beats is not None else float(hp.get("eval_trim_beats", 5))
         use_dbn = dbn if dbn is not None else bool(hp.get("use_dbn", False))
+        rate = fps if fps is not None else hp.get("fps", FPS)
         runner = make_runner(ckpt, f"cuda:{gpu}", float16, use_dbn, dbn_impl)
-        result = evaluate(runner, pieces, min_beat_time=trim, losses=losses)
+        result = evaluate(runner, pieces, min_beat_time=trim, losses=losses, fps=rate)
         summaries.append(result.summary)
         if len(models) == 1:
             _print_single(result)

@@ -1,31 +1,42 @@
 """Postprocessor mirror (reference beat_this/model/postprocessor.py:9-197).
 
 ``type="minimal"``: peak picking (max-pool 7 equality and logit > 0), adjacent-peak merging,
-downbeat snapping and ``np.unique`` all run in one device kernel (``bt_peakpick``); only the
+downbeat snapping and ``np.unique`` all run in one device kernel (``bt_peakpick_fps``); only the
 final timestamp arrays come back to the host.  ``type="dbn"``: the DBN stays on the host as in the
 reference (postprocessor.py:138-173): madmom's ``DBNDownBeatTrackingProcessor`` when madmom is
 installed (exactly the reference's object), otherwise the restatement of its published algorithm in
 ``beat_this_b200/dbn.py`` (parity with madmom unpinned); ``dbn_impl`` forces one of the two ("madmom", "native").
 ``dbn_impl="device"`` decodes on the GPU instead (``bt_dbn_track_device``: sigmoid, clamps, Viterbi and beat
 correction in three kernels, pinned to the host C++ tracker); only the beat times come back to the host.
+
+``fps`` is the frame rate of the predictions, as in the reference: any finite rate > 0, an integer or not (a model
+trained on another hop, madmom-style 100 fps activations).  The peak picker divides peak frames by it
+(``bt_peakpick_fps``) and every DBN is built at it.
 """
 from __future__ import annotations
 
+import math
+import numbers
 from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 import torch
 
 
+def check_fps(fps) -> None:
+    """ValueError unless `fps` is a finite real number > 0 (bools are not frame rates)."""
+    if isinstance(fps, bool) or not isinstance(fps, numbers.Real) or not math.isfinite(fps) or not fps > 0:
+        raise ValueError(f"fps must be a finite number > 0, got {fps!r}")
+
+
 class Postprocessor:
-    def __init__(self, type: str = "minimal", fps: int = 50, engine=None, device="cuda", dbn_impl: str = "auto"):
+    def __init__(self, type: str = "minimal", fps: float = 50, engine=None, device="cuda", dbn_impl: str = "auto"):
         assert type in ["minimal", "dbn"]
         assert dbn_impl in ["auto", "madmom", "native", "device"]
+        check_fps(fps)
         self.type = type
         self.dbn_impl = dbn_impl
         self.fps = fps
-        if fps != 50:
-            raise NotImplementedError("the device peak picker is built for the reference's 50 fps")
         if type == "dbn":
             kw = dict(beats_per_bar=[3, 4], min_bpm=55.0, max_bpm=215.0, fps=self.fps, transition_lambda=100)
             self.dbn = None
@@ -77,7 +88,7 @@ class Postprocessor:
     def batch_cat(self, beat: torch.Tensor, downbeat: torch.Tensor, frame_offsets):
         """Concatenated logits of many clips -> list of (beat_times, downbeat_times)."""
         if self.type == "minimal":
-            return self.engine.peakpick_cat(beat, downbeat, frame_offsets)
+            return self.engine.peakpick_cat(beat, downbeat, frame_offsets, self.fps)
         return self._postp_dbn(beat, downbeat, frame_offsets)
 
     @property

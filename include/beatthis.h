@@ -302,7 +302,8 @@ int bt_audio2frames_chunked(bt_ctx* ctx, const float* audio_dev, const int64_t* 
                             float* beat_dev, float* downbeat_dev, const int64_t* frame_offsets_host,
                             const bt_chunking* ck, void* stream);
 
-/* Postprocessor("minimal") (model/postprocessor.py:85-136,176-197) on device.
+/* Postprocessor("minimal") (model/postprocessor.py:85-136,176-197) on device, for predictions at 50 frames per
+ * second: bt_peakpick_fps with fps = 50.
  * Per clip i: beat_times_dev[i*max_peaks ..] (float64 seconds), n_beats_dev[i], same for
  * downbeats.  A clip with more than max_peaks peaks reports the true count (> max_peaks)
  * and stores the first max_peaks. */
@@ -310,6 +311,17 @@ int bt_peakpick(bt_ctx* ctx, const float* beat_dev, const float* downbeat_dev,
                 const int64_t* frame_offsets_host, int32_t n_clips, double* beat_times_dev,
                 int32_t* n_beats_dev, double* down_times_dev, int32_t* n_down_dev,
                 int32_t max_peaks, void* stream);
+
+/* Postprocessor("minimal", fps) for predictions at any frame rate (ABI 2.09).  Peaks, the merging of adjacent peaks
+ * (float64 running means) and the outputs are those of bt_peakpick; a merged peak frame f becomes the time f / fps,
+ * one correctly rounded float64 division, as numpy's beat_frame / fps.  Every downbeat time then moves to the nearest
+ * beat time (the first of equally near ones) and the downbeat times are sorted with duplicates removed (np.unique),
+ * both on those float64 times.  fps must be finite and > 0: anything else is BT_ERR_ARG before anything is
+ * enqueued.  With fps = 50 the outputs are bitwise bt_peakpick's; both launch the same kernel ("peakpick"). */
+int bt_peakpick_fps(bt_ctx* ctx, const float* beat_dev, const float* downbeat_dev,
+                    const int64_t* frame_offsets_host, int32_t n_clips, double fps, double* beat_times_dev,
+                    int32_t* n_beats_dev, double* down_times_dev, int32_t* n_down_dev,
+                    int32_t max_peaks, void* stream);
 
 /* Postprocessor("dbn") (model/postprocessor.py:138-173) on the device: the decoder of bt_dbn_track, pinned to it (the
  * same arithmetic, operation for operation, and the same tie-breaks), as three kernels (dbn_prep, dbn_viterbi,
