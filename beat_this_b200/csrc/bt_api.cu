@@ -87,6 +87,7 @@ struct bt_ctx {
   bool finalized = false;
   std::map<std::string, Param> params;
   mutable char err[1024] = "";
+  const char* call = "";  // the entry point that is launching (begin_call)
   int64_t launches = 0;
   bool sync_debug = false;
 
@@ -158,7 +159,10 @@ int prof_event(bt_ctx* c, cudaStream_t st) {
   return idx;
 }
 
-void prof_mark(bt_ctx* c, cudaStream_t st) {  // start of an API call: reference point for the first kernel
+// Start of an API call that launches: fn is the entry point its launch errors name, and the profile gets the reference
+// point of its first kernel.
+void begin_call(bt_ctx* c, const char* fn, cudaStream_t st) {
+  c->call = fn;
   if (c->prof) c->prof_prev = prof_event(c, st);
 }
 
@@ -177,18 +181,24 @@ void prof_launch(bt_ctx* c, const char* what, cudaStream_t st) {
   c->prof_prev = ev;
 }
 
-int check_launch(bt_ctx* c, const char* what, cudaStream_t st) {
-  c->launches++;
-  if (c->prof) prof_launch(c, what, st);
-  cudaError_t e = cudaGetLastError();
-  if (e == cudaSuccess && c->sync_debug) e = cudaStreamSynchronize(st);
-  if (e != cudaSuccess) return fail(c, BT_ERR_CUDA, "kernel %s failed: %s", what, cudaGetErrorString(e));
+// Follows every launcher call.  status: what the launcher returned; a failed host step launched nothing.  Otherwise the
+// launch is counted (bt_launch_count), profiled as `what`, checked, and under BT_SYNC_DEBUG waited for.
+int check_launch(bt_ctx* c, const char* what, cudaStream_t st, cudaError_t status = cudaSuccess) {
+  if (status == cudaSuccess) {
+    c->launches++;
+    if (c->prof) prof_launch(c, what, st);
+  }
+  cudaError_t e = cudaGetLastError();  // also clears the error a failed host step leaves behind
+  if (status != cudaSuccess) e = status;
+  else if (e == cudaSuccess && c->sync_debug) e = cudaStreamSynchronize(st);
+  if (e != cudaSuccess) return fail(c, BT_ERR_CUDA, "%s: kernel %s failed: %s", c->call, what, cudaGetErrorString(e));
   return BT_OK;
 }
-#define BT_LAUNCHED(c, what, st)                 \
-  do {                                           \
-    int _r = check_launch(c, what, st);          \
-    if (_r != BT_OK) return _r;                  \
+// check_launch(c, what, st[, status]), returning from the caller on failure
+#define BT_LAUNCHED(c, what, st, ...)                       \
+  do {                                                      \
+    int _r = check_launch(c, what, st, ##__VA_ARGS__);      \
+    if (_r != BT_OK) return _r;                             \
   } while (0)
 
 const Param* find_param(const bt_ctx* c, const std::string& name) {
@@ -351,13 +361,15 @@ GemmShape plain_shape(int planes, int L, int N, int K, int lda) {
   return g;
 }
 
-// Fills an empty plan slot of layer l: create(err, errlen) makes the plan from the operands of the launch that uses it.
+// Fills an empty plan slot: create(err, errlen) makes the plan from the operands of the launch that uses it.  label
+// (the layer, or the test hook) names it in the error; a refused plan returns `code`.
 template <class Plan, class Create>
-int make_plan(bt_ctx* c, const Layer& l, std::unique_ptr<Plan, CudaDestroy>& slot, Create create) {
+int make_plan(bt_ctx* c, const char* label, std::unique_ptr<Plan, CudaDestroy>& slot, Create create,
+              int code = BT_ERR_CUDA) {
   if (slot) return BT_OK;
   char err[512] = "";
   slot.reset(create(err, static_cast<int>(sizeof(err))));
-  if (!slot) return fail(c, BT_ERR_CUDA, "tensor-core plan creation failed (%s): %s", l.name.c_str(), err);
+  if (!slot) return fail(c, code, "tensor-core plan creation failed (%s): %s", label, err);
   return BT_OK;
 }
 
@@ -366,11 +378,11 @@ int make_plan(bt_ctx* c, const Layer& l, std::unique_ptr<Plan, CudaDestroy>& slo
 int run_gemm(bt_ctx* c, const Layer& l, int nb, GemmPlan& plan, const void* A, const Param* W, const GemmShape& g,
              const EpiParams& e, const char* what, cudaStream_t st) {
   if (c->dtype == BT_DTYPE_H16) {
-    const int r = make_plan(c, l, plan, [&](char* err, int errlen) {
+    const int r = make_plan(c, l.name.c_str(), plan, [&](char* err, int errlen) {
       return tc_gemm_plan_create(A, W->b16.get(), g, nb * l.F, e.resid != nullptr, e, err, errlen);
     });
     if (r != BT_OK) return r;
-    if (launch_gemm_tc(plan.get(), st) != 0) return fail(c, BT_ERR_CUDA, "tc gemm launch %s failed", what);
+    launch_gemm_tc(plan.get(), st);
   } else {
     launch_gemm_simt(reinterpret_cast<const float*>(A), W->f32.get(), g, e, st);
   }
@@ -417,7 +429,9 @@ int attention_block(bt_ctx* c, float* X, const Layer& l, LayerPlans& tp, int nb,
   const float qscale = tc && !freq ? inv_sqrt_d * 1.4426950408889634f : 1.0f;
   int r = BT_OK;
   if (tc && fused(l)) {  // norm + gates + QKV + RoPE in one kernel
-    r = make_plan(c, l, tp.fqkv, [&](char* err, int n) { return tc_qkv_plan_create(wqkv->b16.get(), C, M, err, n); });
+    r = make_plan(c, l.name.c_str(), tp.fqkv, [&](char* err, int n) {
+      return tc_qkv_plan_create(wqkv->b16.get(), C, M, err, n);
+    });
     if (r != BT_OK) return r;
     launch_fused_qkv(tp.fqkv.get(), X, wg->f32.get(), bg->f32.get(), c->rope_cos->f32.get(), c->rope_sin->f32.get(),
                      ws.QKV.get(), ws.GATES.get(), L, F, freq ? 1 : 0, qscale, st);
@@ -452,7 +466,7 @@ int attention_block(bt_ctx* c, float* X, const Layer& l, LayerPlans& tp, int nb,
   }
   if (freq) {
     if (tc) {
-      r = make_plan(c, l, tp.freq, [&](char* err, int n) {
+      r = make_plan(c, l.name.c_str(), tp.freq, [&](char* err, int n) {
         return tc_freq_plan_create(ws.QKV.get(), ws.O.get(), nb, F, L, heads, err, n);
       });
       if (r != BT_OK) return r;
@@ -463,7 +477,7 @@ int attention_block(bt_ctx* c, float* X, const Layer& l, LayerPlans& tp, int nb,
     }
     BT_LAUNCHED(c, "attn_freq", st);
   } else if (tc) {
-    r = make_plan(c, l, tp.attn, [&](char* err, int n) {
+    r = make_plan(c, l.name.c_str(), tp.attn, [&](char* err, int n) {
       return tc_attn_plan_create(ws.QKV.get(), planes, L, heads, err, n);
     });
     if (r != BT_OK) return r;
@@ -492,7 +506,7 @@ int ff_block(bt_ctx* c, float* X, const Layer& l, LayerPlans& tp, int nb, int L,
   const int64_t M = static_cast<int64_t>(planes) * L;
   if (tc && fused(l)) {
     FfPlan& plan = wout ? tp.ff_op : tp.ff;
-    const int r = make_plan(c, l, plan, [&](char* err, int n) {
+    const int r = make_plan(c, l.name.c_str(), plan, [&](char* err, int n) {
       return tc_ff_plan_create(w1->b16.get(), w2->b16.get(), C, M, wout ? ws.O.get() : nullptr,
                                wout ? wout->b16.get() : nullptr, err, n);
     });
@@ -679,12 +693,37 @@ std::vector<ParamSpec> layer_params(const Layer& l, int64_t D) {
 
 bool aligned16(const void* p) { return reinterpret_cast<uintptr_t>(p) % 16 == 0; }
 
-// A test hook's 16-bit operand: the fp32 device array src of n elements rounded into buf on st (nothing for null src).
-cudaError_t to_h16_operand(DeviceBuffer<>& buf, const float* src, int64_t n, cudaStream_t st) {
-  if (!src) return cudaSuccess;
-  const cudaError_t e = buf.alloc(n * 2);
-  if (e == cudaSuccess) launch_f32_to_h16(src, buf.get(), n, st);
-  return e;
+// A test hook's fp32 device array of n elements that its kernel reads in the activation type: the 16-bit context hands
+// the kernel h16, a rounded copy, and rounds an `out` array (an output the caller pre-filled, so that elements the
+// kernel does not store survive) back after the launch.  A null array stays null.
+struct HookArray {
+  float* f32;
+  int64_t n;
+  bool out;
+  DeviceBuffer<> h16;
+  HookArray(const float* p, int64_t n, bool out = false) : f32(const_cast<float*>(p)), n(n), out(out) {}
+};
+
+// Runs a test hook after its own argument checks: sets the device, takes the stream and begins the call; in the 16-bit
+// context rounds `arrays`; launch(st) makes its plans (make_plan) and launches the kernel(s) under test (check_launch:
+// only they are counted and profiled); then rounds the out arrays back and synchronises the stream.  Scratch that
+// launch uses must outlive the call.
+template <class Launch>
+int run_hook(bt_ctx* c, const char* fn, void* stream, std::initializer_list<HookArray*> arrays, Launch launch) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const bool tc = c->dtype == BT_DTYPE_H16;
+  cudaError_t e = cudaSetDevice(c->device);
+  if (e == cudaSuccess) begin_call(c, fn, st);
+  for (HookArray* a : arrays)
+    if (tc && a->f32 && e == cudaSuccess && (e = a->h16.alloc(a->n * 2)) == cudaSuccess)
+      launch_f32_to_h16(a->f32, a->h16.get(), a->n, st);
+  if (e != cudaSuccess) return fail(c, BT_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(e));
+  int rc = launch(st);
+  for (HookArray* a : arrays)
+    if (tc && a->f32 && a->out && rc == BT_OK) launch_h16_to_f32(a->h16.get(), a->f32, a->n, st);
+  e = cudaStreamSynchronize(st);
+  if (rc == BT_OK && e != cudaSuccess) rc = fail(c, BT_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(e));
+  return rc;
 }
 
 }  // namespace
@@ -915,7 +954,7 @@ int bt_logmel(bt_ctx* c, const float* audio_dev, const int64_t* sample_offsets_h
     return fail(c, BT_ERR_ARG, "bt_logmel: null argument");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   BT_CUDA(c, cudaSetDevice(c->device));
-  prof_mark(c, st);
+  begin_call(c, "bt_logmel", st);
   for (int i = 0; i < n_clips; ++i) {
     const int64_t len = sample_offsets_host[i + 1] - sample_offsets_host[i];
     if (len <= BT_N_FFT / 2)
@@ -972,15 +1011,15 @@ int bt_logmel_config(bt_ctx* c, const bt_mel_config* cfg, const float* window_de
   }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   BT_CUDA(c, cudaSetDevice(c->device));
-  prof_mark(c, st);
+  begin_call(c, fn, st);
   const size_t n = n_clips + 1;
   const int64_t* d[2];
   const int r = stage(c, st, {{sample_offsets_host, n}, {frame_offsets_host, n}}, d);
   if (r != BT_OK) return r;
   const MelConfigArgs args{window_dev, twiddle_dev, fb_start_dev, fb_ptr_dev, fb_w_dev, spect_dev,
                            cfg->hop_length, cfg->n_mels, cfg->norm_mode, cfg->power, cfg->log_multiplier};
-  BT_CUDA(c, launch_logmel_config(log2n, audio_dev, d[0], d[1], n_clips, frame_offsets_host[n_clips], args, st));
-  BT_LAUNCHED(c, "logmel_config", st);
+  BT_LAUNCHED(c, "logmel_config", st,
+              launch_logmel_config(log2n, audio_dev, d[0], d[1], n_clips, frame_offsets_host[n_clips], args, st));
   return BT_OK;
 }
 
@@ -994,20 +1033,21 @@ int bt_resample(bt_ctx* c, const float* audio_in_dev, const int64_t* in_offsets_
   if (L <= 0 || M <= 0 || K <= 0 || (K & 1)) return fail(c, BT_ERR_ARG, "bt_resample: need L, M > 0 and an even K > 0");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   BT_CUDA(c, cudaSetDevice(c->device));
-  prof_mark(c, st);
+  begin_call(c, "bt_resample", st);
   int64_t max_out = 0;
   for (int i = 0; i < n_clips; ++i) {
     if (in_offsets_host[i + 1] < in_offsets_host[i] || out_offsets_host[i + 1] < out_offsets_host[i])
       return fail(c, BT_ERR_ARG, "bt_resample: offsets must be non-decreasing");
     max_out = std::max(max_out, out_offsets_host[i + 1] - out_offsets_host[i]);
   }
+  if (max_out > 0 && resample_smem(L, M, K) > kResampleMaxSmem)
+    return fail(c, BT_ERR_ARG, "bt_resample: ratio %d/%d with %d taps needs too much shared memory", L, M, K);
   const size_t n = n_clips + 1;
   const int64_t* d[2];
   const int r = stage(c, st, {{in_offsets_host, n}, {out_offsets_host, n}}, d);
   if (r != BT_OK) return r;
-  if (launch_resample(audio_in_dev, d[0], audio_out_dev, d[1], n_clips, max_out, coef_dev, L, M, K, st) != 0)
-    return fail(c, BT_ERR_ARG, "bt_resample: ratio %d/%d with %d taps needs too much shared memory", L, M, K);
-  BT_LAUNCHED(c, "resample", st);
+  BT_LAUNCHED(c, "resample", st,
+              launch_resample(audio_in_dev, d[0], audio_out_dev, d[1], n_clips, max_out, coef_dev, L, M, K, st));
   return BT_OK;
 }
 
@@ -1018,7 +1058,7 @@ static int spect2frames(bt_ctx* c, const float* spect_dev, const int64_t* frame_
   if (!spect_dev || !frame_offsets_host || !beat_dev || !downbeat_dev) return fail(c, BT_ERR_ARG, "%s: null argument", fn);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   BT_CUDA(c, cudaSetDevice(c->device));
-  prof_mark(c, st);
+  begin_call(c, fn, st);
   // plan: all chunks of all clips; run_chunks groups them by chunk length
   std::vector<ChunkSrc> all;
   std::vector<int64_t> starts, lens, own_lo, own_hi;
@@ -1070,7 +1110,7 @@ int bt_forward_chunks(bt_ctx* c, const float* chunks_dev, int32_t n_chunks, int3
     return fail(c, BT_ERR_ARG, "bt_forward_chunks: chunk_frames must be in [1, %d] (bt_max_chunk)", c->max_chunk);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   BT_CUDA(c, cudaSetDevice(c->device));
-  prof_mark(c, st);
+  begin_call(c, "bt_forward_chunks", st);
   std::vector<ChunkSrc> all(n_chunks);
   for (int i = 0; i < n_chunks; ++i) {
     ChunkSrc& s = all[i];
@@ -1132,7 +1172,7 @@ int peakpick(bt_ctx* c, const char* fn, const float* beat_dev, const float* down
     return fail(c, BT_ERR_ARG, "%s: bad argument", fn);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   BT_CUDA(c, cudaSetDevice(c->device));
-  prof_mark(c, st);
+  begin_call(c, fn, st);
   const int64_t* fo = nullptr;
   const int r = stage(c, st, {{frame_offsets_host, static_cast<size_t>(n_clips + 1)}}, &fo);
   if (r != BT_OK) return r;
@@ -1326,7 +1366,7 @@ int bt_dbn_track_device(bt_ctx* c, const float* beat_logits_dev, const float* do
   const size_t bp_bytes = std::max<size_t>(bp_per_frame * total, 1);
   BT_CUDA(c, c->dbn_ws.reserve(ws_bytes, ws_bytes + ws_bytes / 4));
   BT_CUDA(c, c->dbn_bp.reserve(bp_bytes, bp_bytes + bp_bytes / 4));
-  prof_mark(c, st);
+  begin_call(c, fn, st);
   const DbnModelDev* md = nullptr;
   const int64_t* fo_dev = nullptr;
   const int r = dbn_stage(c, ms, frame_offsets_host, n_clips, total, nullptr, st, &md, &fo_dev, nullptr);
@@ -1342,10 +1382,8 @@ int bt_dbn_track_device(bt_ctx* c, const float* beat_logits_dev, const float* do
   launch_dbn_prep(beat_logits_dev, downbeat_logits_dev, activations_dev, fo_dev, n_clips, threshold, observation_lambda,
                   act, dens, win, st);
   BT_LAUNCHED(c, "dbn_prep", st);
-  if (const int e = launch_dbn_viterbi(md, n_bar_lengths, threads, smem, dens, fo_dev, win, n_clips, bp, res_logp,
-                                       res_state, st))
-    return fail(c, BT_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(static_cast<cudaError_t>(e)));
-  BT_LAUNCHED(c, "dbn_viterbi", st);
+  BT_LAUNCHED(c, "dbn_viterbi", st,
+              launch_dbn_viterbi(md, n_bar_lengths, threads, smem, dens, fo_dev, win, n_clips, bp, res_logp, res_state, st));
   launch_dbn_backtrace(md, n_bar_lengths, fo_dev, win, n_clips, bp, res_logp, res_state, act, codes, correct != 0, fps,
                        times_dev, numbers_dev, counts_dev, nullptr, nullptr, st);
   BT_LAUNCHED(c, "dbn_backtrace", st);
@@ -1365,26 +1403,24 @@ int bt_debug_dbn_viterbi(bt_ctx* c, const double* log_dens_dev, int64_t T, int32
   int threads;
   size_t smem, bp_per_frame;
   dbn_launch_shape(ms, &threads, &smem, &bp_per_frame);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  BT_CUDA(c, cudaSetDevice(c->device));
-  const size_t ws_bytes = 2 * sizeof(double), bp_bytes = bp_per_frame * T;
-  BT_CUDA(c, c->dbn_ws.reserve(ws_bytes, ws_bytes + ws_bytes / 4));
-  BT_CUDA(c, c->dbn_bp.reserve(bp_bytes, bp_bytes + bp_bytes / 4));
-  prof_mark(c, st);
-  const int64_t fo[2] = {0, T}, win_h[2] = {0, T};
-  const DbnModelDev* md = nullptr;
-  const int64_t *fo_dev = nullptr, *win = nullptr;
-  if ((r = dbn_stage(c, ms, fo, 1, T, win_h, st, &md, &fo_dev, &win)) != BT_OK) return r;
-  double* res_logp = reinterpret_cast<double*>(c->dbn_ws.get());
-  int64_t* res_state = reinterpret_cast<int64_t*>(res_logp + 1);
-  uint8_t* bp = c->dbn_bp.get();
-  if (const int e = launch_dbn_viterbi(md, 1, threads, smem, log_dens_dev, fo_dev, win, 1, bp, res_logp, res_state, st))
-    return fail(c, BT_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(static_cast<cudaError_t>(e)));
-  BT_LAUNCHED(c, "dbn_viterbi", st);
-  launch_dbn_backtrace(md, 1, fo_dev, win, 1, bp, res_logp, res_state, nullptr, nullptr, 0, 1.0, nullptr, nullptr, nullptr,
-                       path_dev, logp_dev, st);
-  BT_LAUNCHED(c, "dbn_backtrace", st);
-  return BT_OK;
+  return run_hook(c, fn, stream, {}, [&](cudaStream_t st) {
+    const size_t ws_bytes = 2 * sizeof(double), bp_bytes = bp_per_frame * T;
+    BT_CUDA(c, c->dbn_ws.reserve(ws_bytes, ws_bytes + ws_bytes / 4));
+    BT_CUDA(c, c->dbn_bp.reserve(bp_bytes, bp_bytes + bp_bytes / 4));
+    const int64_t fo[2] = {0, T}, win_h[2] = {0, T};
+    const DbnModelDev* md = nullptr;
+    const int64_t *fo_dev = nullptr, *win = nullptr;
+    const int rs = dbn_stage(c, ms, fo, 1, T, win_h, st, &md, &fo_dev, &win);
+    if (rs != BT_OK) return rs;
+    double* res_logp = reinterpret_cast<double*>(c->dbn_ws.get());
+    int64_t* res_state = reinterpret_cast<int64_t*>(res_logp + 1);
+    uint8_t* bp = c->dbn_bp.get();
+    BT_LAUNCHED(c, "dbn_viterbi", st,
+                launch_dbn_viterbi(md, 1, threads, smem, log_dens_dev, fo_dev, win, 1, bp, res_logp, res_state, st));
+    launch_dbn_backtrace(md, 1, fo_dev, win, 1, bp, res_logp, res_state, nullptr, nullptr, 0, 1.0, nullptr, nullptr,
+                         nullptr, path_dev, logp_dev, st);
+    return check_launch(c, "dbn_backtrace", st);
+  });
 }
 
 static_assert(BT_BEAT_METRIC_COLS == kBeatMetricCols, "bt_beat_metrics row width");
@@ -1410,13 +1446,12 @@ int bt_beat_metrics(bt_ctx* c, const double* est_dev, const int64_t* est_offsets
     return fail(c, BT_ERR_ARG, "%s: null device pointer", fn);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   BT_CUDA(c, cudaSetDevice(c->device));
-  prof_mark(c, st);
+  begin_call(c, fn, st);
   const size_t n = n_sets + 1;
   const int64_t* off_dev[2];
   const int r = stage(c, st, {{est_offsets_host, n}, {ref_offsets_host, n}}, off_dev);
   if (r != BT_OK) return r;
-  if (const int e = launch_beat_metrics(est_dev, off_dev[0], ref_dev, off_dev[1], n_sets, p, out_dev, st))
-    return fail(c, BT_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(static_cast<cudaError_t>(e)));
+  launch_beat_metrics(est_dev, off_dev[0], ref_dev, off_dev[1], n_sets, p, out_dev, st);
   BT_LAUNCHED(c, "beat_metrics", st);
   return BT_OK;
 }
@@ -1469,20 +1504,17 @@ int bt_beat_loss(bt_ctx* c, const float* preds_dev, const float* targets_dev, co
   if (!row_loss_dev || !mean_dev) return fail(c, BT_ERR_ARG, "%s: null output", fn);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   BT_CUDA(c, cudaSetDevice(c->device));
-  prof_mark(c, st);
+  begin_call(c, fn, st);
   const int64_t n_tiles = tiles.back();
   const size_t bytes = sizeof(double) * n_tiles;
   BT_CUDA(c, c->loss_partials.reserve(bytes, bytes + bytes / 4));
   const size_t n = static_cast<size_t>(n_rows) + 1;
   const int64_t* dev[2];
   if ((r = stage(c, st, {{row_offsets_host, n}, {tiles.data(), n}}, dev)) != BT_OK) return r;
-  if (const int e = launch_beat_loss(preds_dev, targets_dev, mask_dev, dev[0], dev[1], n_rows, n_tiles, p,
-                                     c->loss_partials.get(), st))
-    return fail(c, BT_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(static_cast<cudaError_t>(e)));
+  launch_beat_loss(preds_dev, targets_dev, mask_dev, dev[0], dev[1], n_rows, n_tiles, p, c->loss_partials.get(), st);
   BT_LAUNCHED(c, "beat_loss", st);
-  if (const int e = launch_beat_loss_reduce(c->loss_partials.get(), dev[0], dev[1], n_rows, n_tiles, n_scored, p,
-                                            row_loss_dev, mean_dev, st))
-    return fail(c, BT_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(static_cast<cudaError_t>(e)));
+  launch_beat_loss_reduce(c->loss_partials.get(), dev[0], dev[1], n_rows, n_tiles, n_scored, p, row_loss_dev, mean_dev,
+                          st);
   BT_LAUNCHED(c, "beat_loss_reduce", st);
   return BT_OK;
 }
@@ -1501,13 +1533,12 @@ int bt_beat_loss_backward(bt_ctx* c, const float* preds_dev, const float* target
   if (!grad_mean_dev || !grad_preds_dev) return fail(c, BT_ERR_ARG, "%s: null gradient pointer", fn);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   BT_CUDA(c, cudaSetDevice(c->device));
-  prof_mark(c, st);
+  begin_call(c, fn, st);
   const size_t n = static_cast<size_t>(n_rows) + 1;
   const int64_t* dev[2];
   if ((r = stage(c, st, {{row_offsets_host, n}, {tiles.data(), n}}, dev)) != BT_OK) return r;
-  if (const int e = launch_beat_loss_backward(preds_dev, targets_dev, mask_dev, dev[0], dev[1], n_rows, tiles.back(),
-                                              n_scored, p, grad_mean_dev, grad_preds_dev, st))
-    return fail(c, BT_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(static_cast<cudaError_t>(e)));
+  launch_beat_loss_backward(preds_dev, targets_dev, mask_dev, dev[0], dev[1], n_rows, tiles.back(), n_scored, p,
+                            grad_mean_dev, grad_preds_dev, st);
   BT_LAUNCHED(c, "beat_loss_backward", st);
   return BT_OK;
 }
@@ -1516,12 +1547,11 @@ int bt_debug_gemm(bt_ctx* c, const bt_debug_gemm_desc* d, const float* a_dev, co
                   const float* bias_dev, const float* resid_dev, float* out_f32_dev, float* out_act_dev,
                   int64_t out_act_count, const float* rope_cos_dev, const float* rope_sin_dev, int32_t* tile_out,
                   void* stream) {
-  if (!c || !d || !a_dev || !w_dev) return fail(c, BT_ERR_ARG, "bt_debug_gemm: null argument");
+  const char* fn = "bt_debug_gemm";
+  if (!c || !d || !a_dev || !w_dev) return fail(c, BT_ERR_ARG, "%s: null argument", fn);
   if (d->nslab < 1 || d->nslab > kMaxSlabs || d->planes_out < 1 || d->L < 1 || d->N % 4 != 0 || d->Kslab % 16 != 0 ||
       d->lda % 4 != 0 || (out_act_dev && out_act_count < static_cast<int64_t>(d->planes_out) * d->L * d->N))
-    return fail(c, BT_ERR_ARG, "bt_debug_gemm: unsupported shape");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  BT_CUDA(c, cudaSetDevice(c->device));
+    return fail(c, BT_ERR_ARG, "%s: unsupported shape", fn);
   GemmShape g{};
   g.planes_out = d->planes_out; g.L = d->L; g.N = d->N; g.Kslab = d->Kslab; g.nslab = d->nslab;
   g.plane_mul = d->plane_mul; g.lda = d->lda;
@@ -1534,127 +1564,97 @@ int bt_debug_gemm(bt_ctx* c, const bt_debug_gemm_desc* d, const float* a_dev, co
   e.rope_cos = rope_cos_dev; e.rope_sin = rope_sin_dev;
   e.C = d->C; e.heads = d->heads; e.posmode = d->posmode; e.F = d->F; e.qscale = d->qscale;
   if (tile_out) tile_out[0] = tile_out[1] = 0;
-  if (c->dtype != BT_DTYPE_H16) {
-    launch_gemm_simt(a_dev, w_dev, g, e, st);
-    BT_LAUNCHED(c, "debug_gemm", st);
-    BT_CUDA(c, cudaStreamSynchronize(st));
-    return BT_OK;
-  }
-  const int64_t a_n = static_cast<int64_t>(d->planes_in) * d->L * d->lda;
-  const int64_t w_n = static_cast<int64_t>(d->N) * d->Kslab * d->nslab;
-  DeviceBuffer<> ab, wb, ob;
-  if (ab.alloc(a_n * 2) != cudaSuccess || wb.alloc(w_n * 2) != cudaSuccess ||
-      (out_act_dev && ob.alloc(out_act_count * 2) != cudaSuccess))
-    return fail(c, BT_ERR_CUDA, "bt_debug_gemm: out of device memory");
-  launch_f32_to_h16(a_dev, ab.get(), a_n, st);
-  launch_f32_to_h16(w_dev, wb.get(), w_n, st);
-  if (out_act_dev) launch_f32_to_h16(out_act_dev, ob.get(), out_act_count, st);
-  e.out_act = ob.get();
-  char err[512] = "";
-  const GemmPlan p(tc_gemm_plan_create(ab.get(), wb.get(), g, d->planes_in, d->resid_epilogue != 0, e, err, sizeof(err)));
-  int rc = BT_OK;
-  if (!p) rc = fail(c, BT_ERR_CUDA, "%s", err);
-  else if (launch_gemm_tc(p.get(), st) != 0) rc = fail(c, BT_ERR_CUDA, "tc gemm launch failed");
-  else if (out_act_dev) launch_h16_to_f32(ob.get(), out_act_dev, out_act_count, st);
-  if (p && tile_out) tc_gemm_plan_tile(p.get(), &tile_out[0], &tile_out[1]);
-  const cudaError_t se = cudaStreamSynchronize(st);
-  if (rc == BT_OK && se != cudaSuccess) rc = fail(c, BT_ERR_CUDA, "tc gemm: %s", cudaGetErrorString(se));
-  c->launches++;
-  return rc;
+  HookArray a(a_dev, static_cast<int64_t>(d->planes_in) * d->L * d->lda);
+  HookArray w(w_dev, static_cast<int64_t>(d->N) * d->Kslab * d->nslab);
+  HookArray out_act(out_act_dev, out_act_count, true);
+  return run_hook(c, fn, stream, {&a, &w, &out_act}, [&](cudaStream_t st) {
+    if (c->dtype != BT_DTYPE_H16) {
+      launch_gemm_simt(a_dev, w_dev, g, e, st);
+      return check_launch(c, "debug_gemm", st);
+    }
+    e.out_act = out_act.h16.get();
+    GemmPlan p;
+    const int r = make_plan(c, fn, p, [&](char* err, int n) {
+      return tc_gemm_plan_create(a.h16.get(), w.h16.get(), g, d->planes_in, d->resid_epilogue != 0, e, err, n);
+    });
+    if (r != BT_OK) return r;
+    if (tile_out) tc_gemm_plan_tile(p.get(), &tile_out[0], &tile_out[1]);
+    launch_gemm_tc(p.get(), st);
+    return check_launch(c, "debug_gemm", st);
+  });
 }
 
 int bt_debug_attention(bt_ctx* c, const float* q_dev, const float* k_dev, const float* v_dev, const float* gates_dev,
                        float* o_dev, int64_t o_count, int32_t seqs, int32_t L, int32_t heads,
                        const int32_t* key_lens_host, int32_t seqs_per_chunk, void* stream) {
-  if (!c || !q_dev || !k_dev || !v_dev || !gates_dev || !o_dev) return fail(c, BT_ERR_ARG, "bt_debug_attention: null argument");
+  const char* fn = "bt_debug_attention";
+  if (!c || !q_dev || !k_dev || !v_dev || !gates_dev || !o_dev) return fail(c, BT_ERR_ARG, "%s: null argument", fn);
   if (seqs < 1 || L < 1 || heads < 1 || (key_lens_host && (seqs_per_chunk < 1 || seqs % seqs_per_chunk != 0)))
-    return fail(c, BT_ERR_ARG, "bt_debug_attention: bad geometry");
+    return fail(c, BT_ERR_ARG, "%s: bad geometry", fn);
   const int C = heads * 32;
   const int64_t M = static_cast<int64_t>(seqs) * L;
-  if (o_count < M * C) return fail(c, BT_ERR_ARG, "bt_debug_attention: o holds %lld elements, fewer than M * C",
-                                   static_cast<long long>(o_count));
+  if (o_count < M * C)
+    return fail(c, BT_ERR_ARG, "%s: o holds %lld elements, fewer than M * C", fn, static_cast<long long>(o_count));
   // per-chunk key counts travel in the ChunkSrc table the forward pass hands the kernels (only .len is read)
   std::vector<ChunkSrc> chunks;
   if (key_lens_host) {
     chunks.assign(seqs / seqs_per_chunk, ChunkSrc{});
     for (size_t i = 0; i < chunks.size(); ++i) {
-      if (key_lens_host[i] < 1 || key_lens_host[i] > L) return fail(c, BT_ERR_ARG, "bt_debug_attention: key length out of [1, L]");
+      if (key_lens_host[i] < 1 || key_lens_host[i] > L) return fail(c, BT_ERR_ARG, "%s: key length out of [1, L]", fn);
       chunks[i].len = key_lens_host[i];
     }
   }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  BT_CUDA(c, cudaSetDevice(c->device));
   const bool tc = c->dtype == BT_DTYPE_H16;
-  const size_t act = tc ? 2 : 4;
-  DeviceBuffer<> qkv, o;
-  DeviceBuffer<ChunkSrc> chunks_dev;
-  BT_CUDA(c, qkv.alloc(M * 3 * C * act));
-  if (tc) BT_CUDA(c, to_h16_operand(o, o_dev, o_count, st));  // elements the kernel does not store survive the round trip
-  if (key_lens_host) {
-    const size_t bytes = chunks.size() * sizeof(ChunkSrc);
-    BT_CUDA(c, chunks_dev.alloc(bytes));
-    BT_CUDA(c, cudaMemcpyAsync(chunks_dev.get(), chunks.data(), bytes, cudaMemcpyHostToDevice, st));
-  }
-  int rc = BT_OK;
-  if (tc) {
-    launch_pack_qkv_test(q_dev, k_dev, v_dev, qkv.get(), seqs, L, heads, 0.17677669529663687f * 1.4426950408889634f, 1, st);
-    char err[512] = "";
-    const AttnPlan p(tc_attn_plan_create(qkv.get(), seqs, L, heads, err, sizeof(err)));
-    if (!p) rc = fail(c, BT_ERR_CUDA, "%s", err);
-    else {
-      launch_attn_time_tc(p.get(), gates_dev, o.get(), st, chunks_dev.get(), seqs_per_chunk);
-      launch_h16_to_f32(o.get(), o_dev, o_count, st);
+  HookArray o(o_dev, o_count, true);
+  DeviceBuffer<> qkv;
+  return run_hook(c, fn, stream, {&o}, [&](cudaStream_t st) {
+    BT_CUDA(c, qkv.alloc(M * 3 * C * (tc ? 2 : 4)));
+    const ChunkSrc* chunks_dev = nullptr;
+    int r = chunks.empty() ? BT_OK : stage(c, st, {{chunks.data(), chunks.size()}}, &chunks_dev);
+    if (r != BT_OK) return r;
+    if (tc) {
+      launch_pack_qkv_test(q_dev, k_dev, v_dev, qkv.get(), seqs, L, heads, 0.17677669529663687f * 1.4426950408889634f, 1,
+                           st);
+      AttnPlan p;
+      r = make_plan(c, fn, p, [&](char* err, int n) { return tc_attn_plan_create(qkv.get(), seqs, L, heads, err, n); });
+      if (r != BT_OK) return r;
+      launch_attn_time_tc(p.get(), gates_dev, o.h16.get(), st, chunks_dev, seqs_per_chunk);
+    } else {
+      launch_pack_qkv_test(q_dev, k_dev, v_dev, qkv.get(), seqs, L, heads, 1.0f, 0, st);
+      launch_attn_time_simt(static_cast<const float*>(qkv.get()), gates_dev, o_dev, seqs, L, heads, st, chunks_dev,
+                            seqs_per_chunk);
     }
-    const cudaError_t se = cudaStreamSynchronize(st);
-    if (rc == BT_OK && se != cudaSuccess) rc = fail(c, BT_ERR_CUDA, "tc attention: %s", cudaGetErrorString(se));
-  } else {
-    launch_pack_qkv_test(q_dev, k_dev, v_dev, qkv.get(), seqs, L, heads, 1.0f, 0, st);
-    launch_attn_time_simt(static_cast<const float*>(qkv.get()), gates_dev, o_dev, seqs, L, heads, st, chunks_dev.get(),
-                          seqs_per_chunk);
-    const cudaError_t se = cudaStreamSynchronize(st);
-    if (se != cudaSuccess) rc = fail(c, BT_ERR_CUDA, "simt attention: %s", cudaGetErrorString(se));
-  }
-  c->launches += 2;
-  return rc;
+    return check_launch(c, "debug_attention", st);
+  });
 }
 
 int bt_debug_attention_freq(bt_ctx* c, const float* q_dev, const float* k_dev, const float* v_dev,
                             const float* gates_dev, float* o_dev, int64_t o_count, int32_t B, int32_t F, int32_t L,
                             int32_t heads, void* stream) {
-  if (!c || !q_dev || !k_dev || !v_dev || !gates_dev || !o_dev) return fail(c, BT_ERR_ARG, "bt_debug_attention_freq: null argument");
+  const char* fn = "bt_debug_attention_freq";
+  if (!c || !q_dev || !k_dev || !v_dev || !gates_dev || !o_dev) return fail(c, BT_ERR_ARG, "%s: null argument", fn);
   if (B < 1 || L < 1 || heads < 1 || (F != 8 && F != 16 && F != 32))
-    return fail(c, BT_ERR_ARG, "bt_debug_attention_freq: need B, L, heads >= 1 and F in {8, 16, 32}");
+    return fail(c, BT_ERR_ARG, "%s: need B, L, heads >= 1 and F in {8, 16, 32}", fn);
   const int C = heads * 32;
   const int64_t M = static_cast<int64_t>(B) * F * L;
-  if (o_count < M * C) return fail(c, BT_ERR_ARG, "bt_debug_attention_freq: o holds %lld elements, fewer than M * C",
-                                   static_cast<long long>(o_count));
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  BT_CUDA(c, cudaSetDevice(c->device));
+  if (o_count < M * C)
+    return fail(c, BT_ERR_ARG, "%s: o holds %lld elements, fewer than M * C", fn, static_cast<long long>(o_count));
   const bool tc = c->dtype == BT_DTYPE_H16;
-  const size_t act = tc ? 2 : 4;
   const float inv_sqrt_d = 0.17677669529663687f;
-  DeviceBuffer<> qkv, o;
-  FreqPlan p;
-  BT_CUDA(c, qkv.alloc(M * 3 * C * act));
-  if (tc) {
-    BT_CUDA(c, o.alloc(o_count * act));
-    char err[512] = "";
-    p.reset(tc_freq_plan_create(qkv.get(), o.get(), B, F, L, heads, err, sizeof(err)));
-    if (!p) return fail(c, BT_ERR_ARG, "bt_debug_attention_freq: %s", err);
-    launch_f32_to_h16(o_dev, o.get(), o_count, st);  // elements the kernel does not store survive the round trip
-  }
-  launch_pack_qkv_test(q_dev, k_dev, v_dev, qkv.get(), B * F, L, heads, 1.0f, tc ? 1 : 0, st);
-  if (tc) {
-    launch_attn_freq_tc(p.get(), gates_dev, inv_sqrt_d, st);
-    launch_h16_to_f32(o.get(), o_dev, o_count, st);
-  } else {
-    launch_attn_freq_simt(static_cast<const float*>(qkv.get()), gates_dev, o_dev, B, F, L, heads, inv_sqrt_d, st);
-  }
-  int rc = BT_OK;
-  cudaError_t se = cudaStreamSynchronize(st);
-  if (se != cudaSuccess) rc = fail(c, BT_ERR_CUDA, "frequency attention: %s", cudaGetErrorString(se));
-  c->launches += 2;
-  return rc;
+  HookArray o(o_dev, o_count, true);
+  DeviceBuffer<> qkv;
+  return run_hook(c, fn, stream, {&o}, [&](cudaStream_t st) {
+    BT_CUDA(c, qkv.alloc(M * 3 * C * (tc ? 2 : 4)));
+    FreqPlan p;
+    const int r = !tc ? BT_OK : make_plan(c, fn, p, [&](char* err, int n) {
+      return tc_freq_plan_create(qkv.get(), o.h16.get(), B, F, L, heads, err, n);
+    }, BT_ERR_ARG);
+    if (r != BT_OK) return r;
+    launch_pack_qkv_test(q_dev, k_dev, v_dev, qkv.get(), B * F, L, heads, 1.0f, tc ? 1 : 0, st);
+    if (tc) launch_attn_freq_tc(p.get(), gates_dev, inv_sqrt_d, st);
+    else launch_attn_freq_simt(static_cast<const float*>(qkv.get()), gates_dev, o_dev, B, F, L, heads, inv_sqrt_d, st);
+    return check_launch(c, "debug_attention_freq", st);
+  });
 }
 
 int bt_debug_norm(bt_ctx* c, const float* x_dev, float* xn_dev, int64_t M, int32_t C, const float* wg_dev,
@@ -1668,17 +1668,12 @@ int bt_debug_norm(bt_ctx* c, const float* x_dev, float* xn_dev, int64_t M, int32
     return fail(c, BT_ERR_ARG, "%s: need M >= 1 and C in {32, 64, 128, 256, 512, 1024}", fn);
   if (gates_dev ? (!wg_dev || !bg_dev || !aligned16(wg_dev) || heads < 1 || 32 * heads > C) : heads != 0)
     return fail(c, BT_ERR_ARG, "%s: gates need wg (16-byte aligned), bg and 1 <= heads <= C / 32; no gates, heads 0", fn);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  BT_CUDA(c, cudaSetDevice(c->device));
-  const int64_t n = M * C;
-  DeviceBuffer<> xb;
-  if (tc) BT_CUDA(c, to_h16_operand(xb, xn_dev, n, st));  // elements the kernel does not store survive the round trip
-  launch_norm(x_dev, tc ? xb.get() : static_cast<void*>(xn_dev), M, C, tc ? 1 : 0, st, gates_dev, wg_dev, bg_dev, heads);
-  int rc = check_launch(c, "debug_norm", st);
-  if (rc == BT_OK && tc) launch_h16_to_f32(xb.get(), xn_dev, n, st);
-  const cudaError_t se = cudaStreamSynchronize(st);
-  if (rc == BT_OK && se != cudaSuccess) rc = fail(c, BT_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(se));
-  return rc;
+  HookArray xn(xn_dev, M * C, true);
+  return run_hook(c, fn, stream, {&xn}, [&](cudaStream_t st) {
+    launch_norm(x_dev, tc ? xn.h16.get() : static_cast<void*>(xn_dev), M, C, tc ? 1 : 0, st, gates_dev, wg_dev, bg_dev,
+                heads);
+    return check_launch(c, "debug_norm", st);
+  });
 }
 
 int bt_debug_fused_qkv(bt_ctx* c, const float* x_dev, const float* wqkv_dev, const float* wg_dev, const float* bg_dev,
@@ -1694,22 +1689,15 @@ int bt_debug_fused_qkv(bt_ctx* c, const float* x_dev, const float* wqkv_dev, con
       (posmode == 1 && (F < 1 || F > BT_CHUNK)))
     return fail(c, BT_ERR_ARG, "%s: need M >= 1, C in {32, 64}, 1 <= L <= %d, posmode 0 or 1 (1: 1 <= F <= %d)", fn,
                 BT_CHUNK, BT_CHUNK);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  BT_CUDA(c, cudaSetDevice(c->device));
-  const int64_t n = M * 3 * C;
-  DeviceBuffer<> wb, ob;
-  BT_CUDA(c, to_h16_operand(wb, wqkv_dev, 3 * C * C, st));
-  BT_CUDA(c, to_h16_operand(ob, qkv_dev, n, st));
-  char err[512] = "";
-  const QkvPlan p(tc_qkv_plan_create(wb.get(), C, M, err, sizeof(err)));
-  if (!p) return fail(c, BT_ERR_CUDA, "%s: %s", fn, err);
-  launch_fused_qkv(p.get(), x_dev, wg_dev, bg_dev, rope_cos_dev, rope_sin_dev, ob.get(), gates_dev, L, F, posmode, qscale,
-                   st);
-  int rc = check_launch(c, "debug_fused_qkv", st);
-  if (rc == BT_OK) launch_h16_to_f32(ob.get(), qkv_dev, n, st);
-  const cudaError_t se = cudaStreamSynchronize(st);
-  if (rc == BT_OK && se != cudaSuccess) rc = fail(c, BT_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(se));
-  return rc;
+  HookArray wqkv(wqkv_dev, 3 * C * C), qkv(qkv_dev, M * 3 * C, true);
+  return run_hook(c, fn, stream, {&wqkv, &qkv}, [&](cudaStream_t st) {
+    QkvPlan p;
+    const int r = make_plan(c, fn, p, [&](char* err, int n) { return tc_qkv_plan_create(wqkv.h16.get(), C, M, err, n); });
+    if (r != BT_OK) return r;
+    launch_fused_qkv(p.get(), x_dev, wg_dev, bg_dev, rope_cos_dev, rope_sin_dev, qkv.h16.get(), gates_dev, L, F, posmode,
+                     qscale, st);
+    return check_launch(c, "debug_fused_qkv", st);
+  });
 }
 
 int bt_debug_fused_ff(bt_ctx* c, float* x_dev, const float* w1_dev, const float* b1_dev, const float* w2_dev,
@@ -1722,24 +1710,16 @@ int bt_debug_fused_ff(bt_ctx* c, float* x_dev, const float* w1_dev, const float*
       !aligned16(b2_dev) || !o_dev != !wout_dev)
     return fail(c, BT_ERR_ARG, "%s: null argument, x / b1 / b2 not 16-byte aligned, or only one of o and wout", fn);
   if (M < 1 || (C != 32 && C != 64)) return fail(c, BT_ERR_ARG, "%s: need M >= 1 and C in {32, 64}", fn);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  BT_CUDA(c, cudaSetDevice(c->device));
-  const int64_t n = M * C;
-  DeviceBuffer<> w1b, w2b, ob, woutb, xbb;
-  BT_CUDA(c, to_h16_operand(w1b, w1_dev, 4 * C * C, st));
-  BT_CUDA(c, to_h16_operand(w2b, w2_dev, 4 * C * C, st));
-  BT_CUDA(c, to_h16_operand(ob, o_dev, n, st));
-  BT_CUDA(c, to_h16_operand(woutb, wout_dev, C * C, st));
-  BT_CUDA(c, to_h16_operand(xbb, xb_dev, n, st));
-  char err[512] = "";
-  const FfPlan p(tc_ff_plan_create(w1b.get(), w2b.get(), C, M, ob.get(), woutb.get(), err, sizeof(err)));
-  if (!p) return fail(c, BT_ERR_CUDA, "%s: %s", fn, err);
-  launch_fused_ff(p.get(), x_dev, b1_dev, b2_dev, xbb.get(), st);
-  int rc = check_launch(c, "debug_fused_ff", st);
-  if (rc == BT_OK && xb_dev) launch_h16_to_f32(xbb.get(), xb_dev, n, st);
-  const cudaError_t se = cudaStreamSynchronize(st);
-  if (rc == BT_OK && se != cudaSuccess) rc = fail(c, BT_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(se));
-  return rc;
+  HookArray w1(w1_dev, 4 * C * C), w2(w2_dev, 4 * C * C), o(o_dev, M * C), wout(wout_dev, C * C), xb(xb_dev, M * C, true);
+  return run_hook(c, fn, stream, {&w1, &w2, &o, &wout, &xb}, [&](cudaStream_t st) {
+    FfPlan p;
+    const int r = make_plan(c, fn, p, [&](char* err, int n) {
+      return tc_ff_plan_create(w1.h16.get(), w2.h16.get(), C, M, o.h16.get(), wout.h16.get(), err, n);
+    });
+    if (r != BT_OK) return r;
+    launch_fused_ff(p.get(), x_dev, b1_dev, b2_dev, xb.h16.get(), st);
+    return check_launch(c, "debug_fused_ff", st);
+  });
 }
 
 }  // extern "C"
@@ -1763,23 +1743,19 @@ std::vector<ChunkSrc> chunk_table(const bt_debug_chunk* chunks, int32_t n) {
   return v;
 }
 
-// Uploads the checked table through the staging ring, launches one kernel (launch(table_dev)) under the profile
-// name `what` and waits for it.
+// A hook of a chunk-table kernel: uploads the checked table through the staging ring and launches the kernel
+// (launch(table_dev, st)) under the profile name `what`.
 template <class Launch>
 int run_chunk_hook(bt_ctx* c, const char* fn, const char* what, const bt_debug_chunk* chunks, int32_t n, void* stream,
                    Launch launch) {
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  BT_CUDA(c, cudaSetDevice(c->device));
-  prof_mark(c, st);
   const std::vector<ChunkSrc> table = chunk_table(chunks, n);
-  const ChunkSrc* dev = nullptr;
-  int rc = stage(c, st, {{table.data(), table.size()}}, &dev);
-  if (rc != BT_OK) return rc;
-  launch(dev, st);
-  rc = check_launch(c, what, st);
-  const cudaError_t se = cudaStreamSynchronize(st);
-  if (rc == BT_OK && se != cudaSuccess) rc = fail(c, BT_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(se));
-  return rc;
+  return run_hook(c, fn, stream, {}, [&](cudaStream_t st) {
+    const ChunkSrc* dev = nullptr;
+    const int r = stage(c, st, {{table.data(), table.size()}}, &dev);
+    if (r != BT_OK) return r;
+    launch(dev, st);
+    return check_launch(c, what, st);
+  });
 }
 
 }  // namespace

@@ -49,6 +49,9 @@ struct EpiParams {
 
 struct ChunkSrc;
 
+// Launchers enqueue their kernel(s) and return void, or, when a host step can fail (cudaFuncSetAttribute, an occupancy
+// query), that step's cudaError_t (cudaSuccess otherwise).  None checks the launch itself: the caller does.
+
 // ---- fp32 CUDA-core path -------------------------------------------------------------------
 void launch_gemm_simt(const float* A, const float* W, const GemmShape& g, const EpiParams& e,
                       cudaStream_t st);
@@ -84,8 +87,11 @@ void launch_stem(const float* spect, const ChunkSrc* chunks, int nchunks, int L,
                  cudaStream_t st);
 void launch_head(const float* x, int D, const float* w, const float* b, const ChunkSrc* chunks,
                  int nchunks, int L, float* beat, float* down, int sum_head, cudaStream_t st);
-int launch_resample(const float* in, const int64_t* in_off_dev, float* out, const int64_t* out_off_dev, int n_clips,
-                    int64_t max_out, const float* coef, int L, int M, int K, cudaStream_t st);
+// dynamic shared memory resample_kernel needs for the ratio L/M with K taps; the caller keeps it <= kResampleMaxSmem
+int64_t resample_smem(int L, int M, int K);
+constexpr int64_t kResampleMaxSmem = 200 * 1024;
+cudaError_t launch_resample(const float* in, const int64_t* in_off_dev, float* out, const int64_t* out_off_dev,
+                            int n_clips, int64_t max_out, const float* coef, int L, int M, int K, cudaStream_t st);
 void launch_logmel(const float* audio, const int64_t* sample_off_dev, const int64_t* frame_off_dev,
                    int n_clips, int64_t max_frames, const float* window, const float* twiddle,
                    const int32_t* fb_start, const int32_t* fb_ptr, const float* fb_w, float* spect,
@@ -130,10 +136,9 @@ void launch_dbn_prep(const float* beat, const float* down, const double* act_in,
 size_t dbn_viterbi_smem(int beats, int n_int, int per_beat);
 // Viterbi of every (clip, model): back pointers into bp, res_logp / res_state [clip * n_models + model] = log-probability
 // and final state of the best path.  threads >= max beats * n_int (multiple of 32), smem >= max dbn_viterbi_smem.
-// Returns a cudaError_t.
-int launch_dbn_viterbi(const DbnModelDev* models_dev, int n_models, int threads, size_t smem, const double* dens,
-                       const int64_t* fo_dev, const int64_t* win, int n_clips, uint8_t* bp, double* res_logp,
-                       int64_t* res_state, cudaStream_t st);
+cudaError_t launch_dbn_viterbi(const DbnModelDev* models_dev, int n_models, int threads, size_t smem, const double* dens,
+                               const int64_t* fo_dev, const int64_t* win, int n_clips, uint8_t* bp, double* res_logp,
+                               int64_t* res_state, cudaStream_t st);
 // Best model, backtrace and beats of every clip: (time, number) pairs at times / numbers + fo[clip], counts[clip]
 // (codes: one byte per frame of scratch).  With path_out non-null (one clip, one model) it writes the state path and
 // *logp_out instead.
@@ -149,9 +154,9 @@ struct BeatMetricParams {
 };
 constexpr int kBeatMetricCols = 12;
 // Every set s: estimates est[est_off[s], est_off[s+1]), references ref[ref_off[s], ref_off[s+1]) (sorted, finite,
-// non-negative) -> out[s * 12 ..].  Returns a cudaError_t.
-int launch_beat_metrics(const double* est, const int64_t* est_off_dev, const double* ref, const int64_t* ref_off_dev,
-                        int n_sets, const BeatMetricParams& p, double* out, cudaStream_t st);
+// non-negative) -> out[s * 12 ..].
+void launch_beat_metrics(const double* est, const int64_t* est_off_dev, const double* ref, const int64_t* ref_off_dev,
+                         int n_sets, const BeatMetricParams& p, double* out, cudaStream_t st);
 
 // ---- training losses (kernels_loss.cu) ----------------------------------------------------------------------------
 // The contract of bt_beat_loss (include/beatthis.h).  Rows are CSR over row_off_dev; tile_first_dev[i] is the first CTA
@@ -165,17 +170,17 @@ struct LossParams {
 // CTAs row i needs: scored frames (forward) or frames (backward) over kLossTile
 int64_t loss_tiles(int64_t len, const LossParams& p, bool backward);
 // forward: one float64 partial per CTA into partials, then one CTA reduces them in a fixed order into row_loss and
-// *mean (n_scored: scored frames of all rows).  Each returns a cudaError_t.
-int launch_beat_loss(const float* x, const float* y, const float* m, const int64_t* row_off_dev,
-                     const int64_t* tile_first_dev, int n_rows, int64_t n_tiles, const LossParams& p, double* partials,
-                     cudaStream_t st);
-int launch_beat_loss_reduce(const double* partials, const int64_t* row_off_dev, const int64_t* tile_first_dev, int n_rows,
-                            int64_t n_tiles, int64_t n_scored, const LossParams& p, double* row_loss, float* mean,
-                            cudaStream_t st);
-// backward: grad[j] for every frame (gather over the windows covering j).  One launch; returns a cudaError_t.
-int launch_beat_loss_backward(const float* x, const float* y, const float* m, const int64_t* row_off_dev,
-                              const int64_t* tile_first_dev, int n_rows, int64_t n_tiles, int64_t n_scored,
-                              const LossParams& p, const float* grad_mean, float* grad, cudaStream_t st);
+// *mean (n_scored: scored frames of all rows).
+void launch_beat_loss(const float* x, const float* y, const float* m, const int64_t* row_off_dev,
+                      const int64_t* tile_first_dev, int n_rows, int64_t n_tiles, const LossParams& p, double* partials,
+                      cudaStream_t st);
+void launch_beat_loss_reduce(const double* partials, const int64_t* row_off_dev, const int64_t* tile_first_dev,
+                             int n_rows, int64_t n_tiles, int64_t n_scored, const LossParams& p, double* row_loss,
+                             float* mean, cudaStream_t st);
+// backward: grad[j] for every frame (gather over the windows covering j).  One launch.
+void launch_beat_loss_backward(const float* x, const float* y, const float* m, const int64_t* row_off_dev,
+                               const int64_t* tile_first_dev, int n_rows, int64_t n_tiles, int64_t n_scored,
+                               const LossParams& p, const float* grad_mean, float* grad, cudaStream_t st);
 
 void launch_f32_to_h16(const float* in, void* out, int64_t n, cudaStream_t st);
 void launch_h16_to_f32(const void* in, float* out, int64_t n, cudaStream_t st);
@@ -193,7 +198,7 @@ TcGemmPlan* tc_gemm_plan_create(const void* A_h16, const void* W_h16, const Gemm
                                 bool resid_epilogue, const EpiParams& e, char* err, int errlen);
 void tc_gemm_plan_destroy(TcGemmPlan*);
 void tc_gemm_plan_tile(const TcGemmPlan*, int* bn, int* bk);  // the (BN, BK) tile the plan launches
-int launch_gemm_tc(const TcGemmPlan* plan, cudaStream_t st);  // 0, or -2 for a tile without a kernel
+void launch_gemm_tc(const TcGemmPlan* plan, cudaStream_t st);
 
 struct TcAttnPlan;
 TcAttnPlan* tc_attn_plan_create(const void* qkv_h16, int seqs, int L, int heads, char* err, int errlen);

@@ -259,15 +259,15 @@ void launch_dbn_prep(const float* beat, const float* down, const double* act_in,
   dbn_prep_kernel<<<n_clips, 256, 0, st>>>(beat, down, act_in, fo_dev, threshold, observation_lambda, act, dens, win);
 }
 
-int launch_dbn_viterbi(const DbnModelDev* models_dev, int n_models, int threads, size_t smem, const double* dens,
-                       const int64_t* fo_dev, const int64_t* win, int n_clips, uint8_t* bp, double* res_logp,
-                       int64_t* res_state, cudaStream_t st) {
-  if (n_clips <= 0) return 0;
+cudaError_t launch_dbn_viterbi(const DbnModelDev* models_dev, int n_models, int threads, size_t smem, const double* dens,
+                               const int64_t* fo_dev, const int64_t* win, int n_clips, uint8_t* bp, double* res_logp,
+                               int64_t* res_state, cudaStream_t st) {
+  if (n_clips <= 0) return cudaSuccess;
   cudaError_t e = cudaFuncSetAttribute(dbn_viterbi_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
-  if (e != cudaSuccess) return static_cast<int>(e);
+  if (e != cudaSuccess) return e;
   dbn_viterbi_kernel<<<dim3(n_clips, n_models), threads, smem, st>>>(models_dev, n_models, dens, fo_dev, win, bp, res_logp,
                                                                       res_state);
-  return 0;
+  return cudaSuccess;
 }
 
 void launch_dbn_backtrace(const DbnModelDev* models_dev, int n_models, const int64_t* fo_dev, const int64_t* win,

@@ -252,11 +252,10 @@ beat_metrics_kernel(const double* __restrict__ est, const int64_t* __restrict__ 
 
 }  // namespace
 
-int launch_beat_metrics(const double* est, const int64_t* est_off_dev, const double* ref, const int64_t* ref_off_dev,
-                        int n_sets, const BeatMetricParams& p, double* out, cudaStream_t st) {
+void launch_beat_metrics(const double* est, const int64_t* est_off_dev, const double* ref, const int64_t* ref_off_dev,
+                         int n_sets, const BeatMetricParams& p, double* out, cudaStream_t st) {
   const int blocks = static_cast<int>((static_cast<int64_t>(n_sets) + kWarpsPerBlock - 1) / kWarpsPerBlock);
   beat_metrics_kernel<<<blocks, kWarpsPerBlock * 32, 0, st>>>(est, est_off_dev, ref, ref_off_dev, n_sets, p, out);
-  return static_cast<int>(cudaGetLastError());
 }
 
 }  // namespace bt

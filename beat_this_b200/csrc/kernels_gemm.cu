@@ -350,6 +350,20 @@ static bool make_epi_tmap(CUtensorMap* tm, const void* base, int ld, int es, uin
                        base, 3, dims, strides, box, static_cast<int>(box_cols) * es, err, errlen);
 }
 
+// Every gemm_tc_kernel instantiation (BN, BK, epilogue kind): tc_init sets their shared-memory limits, plan creation
+// refuses any other tile and launch_gemm_tc dispatches over the same list.  The gates GEMM (kind 2) is N = 32 wide.
+#define BT_GEMM_TC_INSTANCES(X)                                                                                         \
+  X(256, 64, 0) X(256, 64, 1) X(192, 64, 0) X(192, 64, 1) X(128, 64, 0) X(128, 64, 1) X(64, 64, 0) X(64, 64, 1)       \
+  X(32, 64, 0) X(32, 64, 1) X(128, 32, 0) X(128, 32, 1) X(64, 32, 0) X(64, 32, 1) X(32, 32, 0) X(32, 32, 1)             \
+  X(32, 64, 2) X(32, 32, 2)
+
+static bool has_instance(const TcGemmPlan* p) {
+#define BT_TG_HAS(bn, bk, kd) if (p->BN == bn && p->BK == bk && p->kind == kd) return true;
+  BT_GEMM_TC_INSTANCES(BT_TG_HAS)
+#undef BT_TG_HAS
+  return false;
+}
+
 TcGemmPlan* tc_gemm_plan_create(const void* A, const void* W, const GemmShape& g, int planes_in, bool resid_epilogue,
                                 const EpiParams& e, char* err, int errlen) {
   TcGemmPlan* p = new TcGemmPlan();
@@ -360,6 +374,11 @@ TcGemmPlan* tc_gemm_plan_create(const void* A, const void* W, const GemmShape& g
   p->BN = pick_bn(g.N, p->BK == 32 || resid_epilogue ? 128 : 256);
   if (p->BN == 0 || g.Kslab % 32 != 0) {
     snprintf(err, errlen, "tc gemm: unsupported shape N=%d Kslab=%d", g.N, g.Kslab);
+    delete p;
+    return nullptr;
+  }
+  if (!has_instance(p)) {
+    snprintf(err, errlen, "tc gemm: no kernel for the tile BN=%d BK=%d of epilogue kind %d", p->BN, p->BK, p->kind);
     delete p;
     return nullptr;
   }
@@ -406,23 +425,15 @@ TcGemmPlan* tc_gemm_plan_create(const void* A, const void* W, const GemmShape& g
 void tc_gemm_plan_destroy(TcGemmPlan* p) { delete p; }
 void tc_gemm_plan_tile(const TcGemmPlan* p, int* bn, int* bk) { *bn = p->BN; *bk = p->BK; }
 
-// Every gemm_tc_kernel instantiation (BN, BK, epilogue kind): tc_init sets their shared-memory limits and
-// launch_gemm_tc dispatches over the same list.  The gates GEMM (kind 2) is N = 32 wide.
-#define BT_GEMM_TC_INSTANCES(X)                                                                                         \
-  X(256, 64, 0) X(256, 64, 1) X(192, 64, 0) X(192, 64, 1) X(128, 64, 0) X(128, 64, 1) X(64, 64, 0) X(64, 64, 1)       \
-  X(32, 64, 0) X(32, 64, 1) X(128, 32, 0) X(128, 32, 1) X(64, 32, 0) X(64, 32, 1) X(32, 32, 0) X(32, 32, 1)             \
-  X(32, 64, 2) X(32, 32, 2)
-
-int launch_gemm_tc(const TcGemmPlan* p, cudaStream_t st) {
+void launch_gemm_tc(const TcGemmPlan* p, cudaStream_t st) {
 #define BT_TG_LAUNCH(bn, bk, kd)                                                                                       \
   if (p->BN == bn && p->BK == bk && p->kind == kd) {                                                                   \
     gemm_tc_kernel<bn, bk, kd><<<p->grid, TG_THREADS, TgCfg<bn, bk>::SMEM, st>>>(                                     \
         p->tmA, p->tmW, p->tmR, p->tmF, p->tmH, p->g, p->e, p->num_tiles, p->t_tiles, p->n_tiles, p->m_tiles);        \
-    return 0;                                                                                                          \
+    return;                                                                                                            \
   }
   BT_GEMM_TC_INSTANCES(BT_TG_LAUNCH)
 #undef BT_TG_LAUNCH
-  return -2;
 }
 
 int tc_init(char* err, int errlen) {

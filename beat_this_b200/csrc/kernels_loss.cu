@@ -196,28 +196,25 @@ int64_t loss_tiles(int64_t len, const LossParams& p, bool backward) {
   return (n + kLossTile - 1) / kLossTile;
 }
 
-int launch_beat_loss(const float* x, const float* y, const float* m, const int64_t* row_off_dev,
-                     const int64_t* tile_first_dev, int n_rows, int64_t n_tiles, const LossParams& p, double* partials,
-                     cudaStream_t st) {
+void launch_beat_loss(const float* x, const float* y, const float* m, const int64_t* row_off_dev,
+                      const int64_t* tile_first_dev, int n_rows, int64_t n_tiles, const LossParams& p, double* partials,
+                      cudaStream_t st) {
   beat_loss_kernel<<<static_cast<unsigned>(n_tiles), kLossTile, 0, st>>>(x, y, m, row_off_dev, tile_first_dev, n_rows, p,
                                                                          partials);
-  return static_cast<int>(cudaGetLastError());
 }
 
-int launch_beat_loss_reduce(const double* partials, const int64_t* row_off_dev, const int64_t* tile_first_dev, int n_rows,
-                            int64_t n_tiles, int64_t n_scored, const LossParams& p, double* row_loss, float* mean,
-                            cudaStream_t st) {
+void launch_beat_loss_reduce(const double* partials, const int64_t* row_off_dev, const int64_t* tile_first_dev,
+                             int n_rows, int64_t n_tiles, int64_t n_scored, const LossParams& p, double* row_loss,
+                             float* mean, cudaStream_t st) {
   beat_loss_reduce_kernel<<<1, kReduceThreads, 0, st>>>(partials, row_off_dev, tile_first_dev, n_rows, n_tiles,
                                                         static_cast<double>(n_scored), p, row_loss, mean);
-  return static_cast<int>(cudaGetLastError());
 }
 
-int launch_beat_loss_backward(const float* x, const float* y, const float* m, const int64_t* row_off_dev,
-                              const int64_t* tile_first_dev, int n_rows, int64_t n_tiles, int64_t n_scored,
-                              const LossParams& p, const float* grad_mean, float* grad, cudaStream_t st) {
+void launch_beat_loss_backward(const float* x, const float* y, const float* m, const int64_t* row_off_dev,
+                               const int64_t* tile_first_dev, int n_rows, int64_t n_tiles, int64_t n_scored,
+                               const LossParams& p, const float* grad_mean, float* grad, cudaStream_t st) {
   beat_loss_backward_kernel<<<static_cast<unsigned>(n_tiles), kLossTile, 0, st>>>(
       x, y, m, row_off_dev, tile_first_dev, n_rows, static_cast<double>(n_scored), p, grad_mean, grad);
-  return static_cast<int>(cudaGetLastError());
 }
 
 }  // namespace bt

@@ -346,7 +346,7 @@ static cudaError_t launch_logmel_config_n(const float* audio, const int64_t* sam
   const unsigned grid = static_cast<unsigned>(std::min<int64_t>(groups, max_ctas));
   logmel_config_kernel<LOG2N><<<grid, G::THREADS, G::SMEM, st>>>(audio, sample_off_dev, frame_off_dev, n_clips,
                                                                   total_frames, p);
-  return cudaGetLastError();
+  return cudaSuccess;
 }
 
 cudaError_t launch_logmel_config(int log2n, const float* audio, const int64_t* sample_off_dev,
@@ -404,18 +404,18 @@ resample_kernel(const float* __restrict__ in, const int64_t* __restrict__ in_off
   out[o0 + n] = (a0 + a1) + (a2 + a3);
 }
 
-int launch_resample(const float* in, const int64_t* in_off_dev, float* out, const int64_t* out_off_dev, int n_clips,
-                    int64_t max_out, const float* coef, int L, int M, int K, cudaStream_t st) {
-  if (n_clips <= 0 || max_out <= 0) return 0;
-  const int64_t span = (255ll * M) / L + K + 2;
-  if (span * 4 > 200 * 1024) return -1;  // absurd ratio: the staged input span does not fit in shared memory
-  const int smem = static_cast<int>(span * 4);
-  if (smem > 48 * 1024 &&
-      cudaFuncSetAttribute(resample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess)
-    return -1;
+int64_t resample_smem(int L, int M, int K) { return ((255ll * M) / L + K + 2) * 4; }  // the staged input span
+
+cudaError_t launch_resample(const float* in, const int64_t* in_off_dev, float* out, const int64_t* out_off_dev,
+                            int n_clips, int64_t max_out, const float* coef, int L, int M, int K, cudaStream_t st) {
+  if (n_clips <= 0 || max_out <= 0) return cudaSuccess;
+  const int smem = static_cast<int>(resample_smem(L, M, K));
+  const cudaError_t e = smem > 48 * 1024
+      ? cudaFuncSetAttribute(resample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) : cudaSuccess;
+  if (e != cudaSuccess) return e;
   dim3 grid(static_cast<unsigned>((max_out + 255) / 256), static_cast<unsigned>(n_clips));
   resample_kernel<<<grid, 256, smem, st>>>(in, in_off_dev, out, out_off_dev, coef, L, M, K);
-  return 0;
+  return cudaSuccess;
 }
 
 // ------------------------------------------------------------------------------------------

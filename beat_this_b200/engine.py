@@ -446,12 +446,7 @@ class Engine:
         """One GEMM through bt_debug_gemm.  shape: the GemmShape fields (planes_out, planes_in, L, N, Kslab, nslab,
         plane_mul, lda, plane_add, t_shift); tensors are fp32 on this device and are passed through as they are (the
         outputs are written in place, resid may be out_f32).  Returns the (BN, BK) tile of the 16-bit plan."""
-        def ptr(t):
-            if t is None:
-                return None
-            assert t.is_cuda and t.dtype == torch.float32 and t.is_contiguous()
-            return c_void_p(t.data_ptr())
-
+        ptr = self._dev_ptr
         d = _lib.bt_debug_gemm_desc()
         for f in ("planes_out", "planes_in", "L", "N", "Kslab", "nslab", "plane_mul", "lda"):
             setattr(d, f, int(shape[f]))

@@ -338,9 +338,10 @@ int bt_dbn_track_device(bt_ctx* ctx, const float* beat_logits_dev, const float* 
                         double threshold, int32_t correct, double fps,
                         double* times_dev, int32_t* numbers_dev, int64_t* counts_dev, void* stream);
 
-/* Test hook: the device Viterbi alone, same arguments and meaning as bt_dbn_viterbi (log_dens and the outputs on the
- * device, the model tables on the host).  The pointer table must have the form BarModel builds: in every (beat, tempo)
- * a leading run of 2 (first beat of the bar) or 1 (other beats) followed by 0; anything else is BT_ERR_ARG. */
+/* Test hook (conventions with the others, below bt_debug_tap_count): the device Viterbi alone (dbn_viterbi, then
+ * dbn_backtrace for the path), same arguments and meaning as bt_dbn_viterbi (log_dens and the outputs on the device,
+ * the model tables on the host).  The pointer table must have the form BarModel builds: in every (beat, tempo) a
+ * leading run of 2 (first beat of the bar) or 1 (other beats) followed by 0; anything else is BT_ERR_ARG. */
 int bt_debug_dbn_viterbi(bt_ctx* ctx, const double* log_dens_dev, int64_t T, int32_t beats, int32_t n_int,
                          const int32_t* intervals, const double* log_tempo, const int32_t* pointers,
                          int64_t* path_dev, double* logp_dev, void* stream);
@@ -458,6 +459,21 @@ int bt_profile_get(const bt_ctx* ctx, int index, char* name, int name_cap, doubl
 int bt_debug_request_tap(bt_ctx* ctx, const char* tap, float* out_dev, int64_t cap);
 int64_t bt_debug_tap_count(const bt_ctx* ctx);
 
+/* Kernel test hooks: bt_debug_gemm, _attention, _attention_freq, _norm, _fused_qkv, _fused_ff, _stem, _zero_tail,
+ * _head (below) and bt_debug_dbn_viterbi (with the DBN entry points) each run the kernel the forward pass or
+ * post-processor runs, alone, on the ctx's device and the given stream.  Common to all of them:
+ *  - Arguments are checked before anything is enqueued; a bad one returns BT_ERR_ARG and launches nothing.
+ *  - Arrays are fp32 on the device unless stated.  The 16-bit context rounds the kernel's 16-bit operands to its
+ *    activation type, and runs each 16-bit output through that type: the whole buffer given, so that values the
+ *    kernel does not store survive.
+ *  - A tensor-core plan the geometry does not fit is refused with the plan's reason: BT_ERR_CUDA, except BT_ERR_ARG
+ *    for bt_debug_attention_freq.
+ *  - Only the kernel under test counts in bt_launch_count (+1 per call; +2 for bt_debug_dbn_viterbi) and in the
+ *    profile, under the name debug_gemm, debug_attention, debug_attention_freq, debug_norm, debug_fused_qkv,
+ *    debug_fused_ff, stem, zero_tail, head, or dbn_viterbi and dbn_backtrace.  Under BT_SYNC_DEBUG=1 it is checked as
+ *    every launch of the forward pass is.  Rounding and operand packing are neither counted nor profiled.
+ *  - Each synchronises the stream before it returns. */
+
 /* Shape and epilogue of one bt_debug_gemm call: the GEMM the forward pass runs for a linear layer, a k(2,3)
  * convolution or frontend.linear (csrc/bt_kernels.h GemmShape / EpiParams).  Output row m = p_out * L + t of N
  * columns; slab s reads plane p_out * plane_mul + plane_add[s] at time t + t_shift[s] (zeros outside [0, L)),
@@ -475,44 +491,36 @@ typedef struct bt_debug_gemm_desc {
   float qscale;
 } bt_debug_gemm_desc;
 
-/* Test hook: one GEMM of shape and epilogue `desc` through the ctx's GEMM kernel (16-bit: gemm_tc_kernel, fp32:
- * gemm_simt_kernel).  Every *_dev pointer is fp32 on the device (bias, resid, out_f32, out_act, rope tables may be
- * NULL) and is passed through unchanged, so resid may alias out_f32.  The 16-bit context rounds A and W to its
- * operand type and runs out_act (all out_act_count elements of the buffer, so values the kernel does not store
- * survive) through its activation type around the launch.  tile_out[2] (optional) receives the (BN, BK) tile of the
- * 16-bit plan, (0, 0) in the fp32 context.  Synchronises the stream. */
+/* One GEMM of shape and epilogue `desc` through the ctx's GEMM kernel (16-bit: gemm_tc_kernel, fp32:
+ * gemm_simt_kernel).  bias, resid, out_f32, out_act and the rope tables may be NULL; resid may alias out_f32.  The
+ * 16-bit operands are A and W; out_act (out_act_count elements) is the 16-bit output.  tile_out[2] (optional) receives
+ * the (BN, BK) tile of the 16-bit plan, (0, 0) in the fp32 context. */
 int bt_debug_gemm(bt_ctx* ctx, const bt_debug_gemm_desc* desc, const float* a_dev, const float* w_dev,
                   const float* bias_dev, const float* resid_dev, float* out_f32_dev, float* out_act_dev,
                   int64_t out_act_count, const float* rope_cos_dev, const float* rope_sin_dev, int32_t* tile_out,
                   void* stream);
 
-/* Test hook: gates * softmax(Q K^T / sqrt(32)) V for `seqs` sequences of length L and `heads` heads of dim 32
- * through the ctx's time-direction attention kernel.  q/k/v_dev are [seqs, L, heads*32] fp32, gates_dev
- * [seqs * L, heads] fp32.  o_dev holds o_count >= seqs * L * heads * 32 fp32 elements, the first seqs * L * heads * 32
- * of them the output; the 16-bit context runs all o_count elements through its activation type around the launch,
- * so values the kernel does not store survive.  key_lens_host (optional): sequence s belongs to chunk
- * s / seqs_per_chunk and attends to the first key_lens_host[chunk] keys only (1 <= len <= L), as in a wave of chunks
- * of different lengths.  Returns BT_ERR_ARG, before anything is enqueued, for a bad geometry or o_count.
- * Synchronises the stream. */
+/* gates * softmax(Q K^T / sqrt(32)) V for `seqs` sequences of length L and `heads` heads of dim 32 through the ctx's
+ * time-direction attention kernel.  q/k/v_dev are [seqs, L, heads*32], gates_dev [seqs * L, heads].  o_dev, the 16-bit
+ * output, holds o_count >= seqs * L * heads * 32 elements, the first seqs * L * heads * 32 of them the output.
+ * key_lens_host (optional): sequence s belongs to chunk s / seqs_per_chunk and attends to the first
+ * key_lens_host[chunk] keys only (1 <= len <= L), as in a wave of chunks of different lengths. */
 int bt_debug_attention(bt_ctx* ctx, const float* q_dev, const float* k_dev, const float* v_dev,
                        const float* gates_dev, float* o_dev, int64_t o_count, int32_t seqs, int32_t L, int32_t heads,
                        const int32_t* key_lens_host, int32_t seqs_per_chunk, void* stream);
 
-/* Test hook: the frequency-direction attention of B chunks of F planes of L frames: token m = (b * F + f) * L + t
- * attends over the F tokens of its (b, t), gates * softmax(q k^T / sqrt(32)) v per head.  q/k/v/o_dev are
- * [B * F * L, heads * 32] fp32, gates_dev [B * F * L, heads]; F in {8, 16, 32}.  o_dev holds o_count >= B * F * L *
- * heads * 32 elements, as for bt_debug_attention.  The 16-bit context runs the tensor-core kernel of the frontend
- * blocks and returns BT_ERR_ARG for any pair other than (F, heads) = (32, 1), (16, 2), (8, 4).  Synchronises the
- * stream. */
+/* The frequency-direction attention of B chunks of F planes of L frames: token m = (b * F + f) * L + t attends over
+ * the F tokens of its (b, t), gates * softmax(q k^T / sqrt(32)) v per head.  q/k/v/o_dev are [B * F * L, heads * 32],
+ * gates_dev [B * F * L, heads]; F in {8, 16, 32}.  o_dev holds o_count >= B * F * L * heads * 32 elements, as for
+ * bt_debug_attention.  The 16-bit context runs the tensor-core kernel of the frontend blocks, whose plan refuses any
+ * pair other than (F, heads) = (32, 1), (16, 2), (8, 4). */
 int bt_debug_attention_freq(bt_ctx* ctx, const float* q_dev, const float* k_dev, const float* v_dev,
                             const float* gates_dev, float* o_dev, int64_t o_count, int32_t B, int32_t F, int32_t L,
                             int32_t heads, void* stream);
 
-/* Test hooks of the frontend's row kernels.  Every *_dev pointer is fp32 on the device; x, wg, b1 and b2 must be
- * 16-byte aligned, and so must xn of bt_debug_norm in the fp32 context (the kernel stores it directly).  The 16-bit context rounds the 16-bit operands (wqkv, w1, w2, o, wout) to its activation type
- * around the launch, and runs each 16-bit output (the whole [M, ...] buffer, so values the kernel does not store
- * survive) through that type.  Each returns BT_ERR_ARG, before anything is enqueued, for a bad geometry or pointer,
- * and synchronises the stream. */
+/* The frontend's row kernels.  x, wg, b1 and b2 must be 16-byte aligned, and so must xn of bt_debug_norm in the fp32
+ * context (the kernel stores it directly).  The 16-bit operands are wqkv, w1, w2, o and wout; the 16-bit outputs are
+ * xn, qkv and xb. */
 
 /* RMSNorm xn = x / max(||x||, 1e-12) of M rows of C in {32, 64, 128, 256, 512, 1024} through norm_kernel, in the
  * ctx's activation type.  With gates_dev (then wg_dev [heads, C], bg_dev [heads], 1 <= heads <= C / 32) also
@@ -547,10 +555,9 @@ typedef struct bt_debug_chunk {
   int32_t write_lo, write_hi, len;
 } bt_debug_chunk;
 
-/* Test hooks of the kernels that read the chunk table.  Parameters are fp32 device arrays, so a weight-less ctx will
- * do; chunks_host is uploaded through the ctx's staging ring, as the forward pass uploads its table.  Each launches
- * the kernel the forward pass launches, once, and synchronises the stream; each returns BT_ERR_ARG, before anything is
- * enqueued, for a table or geometry that would take the kernel outside the buffers described.
+/* The kernels that read the chunk table.  Parameters are device arrays, so a weight-less ctx will do; chunks_host is
+ * uploaded through the ctx's staging ring, as the forward pass uploads its table.  A table or geometry that would
+ * take the kernel outside the buffers described is BT_ERR_ARG.
  *
  * bt_debug_stem: stem_kernel over n_chunks chunks (1..65535) of padded length L (1..384000) gathered from spect_dev
  * [spect_frames, 128]; bn1_scale / bn1_shift [128], w [32, 4, 3] (BN2d folded), bias [32]; out_dev [n_chunks, 32, L,
