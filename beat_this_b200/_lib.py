@@ -15,8 +15,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 # BT_LIB_PATH: an instrumented build of the same sources (e.g. build(extra_flags=("-DBT_FF_PROF",), out_path=...))
 LIB_PATH = os.environ.get("BT_LIB_PATH") or os.path.join(HERE, "libbeatthis_sm90.so")
-SOURCES = ["bt_api.cu", "kernels_simt.cu", "kernels_misc.cu", "kernels_gemm.cu", "kernels_attn.cu", "kernels_fused.cu", "kernels_dbn.cu", "kernels_eval.cu", "kernels_loss.cu", "dbn_host.cpp", "host_stage.cpp"]
-HEADERS = ["common.cuh", "epilogue.cuh", "tc_common.cuh", "bt_kernels.h", "cuda_owned.h", "dbn_model.h", os.path.join("..", "..", "include", "beatthis.h")]
+SOURCES = ["bt_api.cu", "kernels_simt.cu", "kernels_misc.cu", "kernels_gemm.cu", "kernels_attn.cu", "kernels_fused.cu", "kernels_dbn.cu", "kernels_eval.cu", "kernels_loss.cu", "kernels_augment.cu", "dbn_host.cpp", "host_stage.cpp"]
+HEADERS = ["common.cuh", "epilogue.cuh", "fft.cuh", "tc_common.cuh", "bt_kernels.h", "cuda_owned.h", "dbn_model.h", os.path.join("..", "..", "include", "beatthis.h")]
 
 BT_DTYPE_F32 = 0
 BT_DTYPE_H16 = 1
@@ -130,6 +130,16 @@ class bt_mel_config(ctypes.Structure):
     ]
 
 
+class bt_stft_config(ctypes.Structure):
+    _fields_ = [
+        ("n_fft", c_int32),
+        ("hop_length", c_int32),
+    ]
+
+
+VOCODER_RATE_RANGE = (0.25, 4.0)  # BT_VOCODER_MIN_RATE, BT_VOCODER_MAX_RATE
+
+
 # every symbol include/beatthis.h declares: name -> (restype, argtypes)
 PROTOTYPES = {
     "bt_version": (c_int, []),
@@ -192,6 +202,21 @@ PROTOTYPES = {
     "bt_beat_loss_backward": (
         c_int, [c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_int64), c_int32, POINTER(bt_loss_params), c_void_p,
                 c_void_p, c_void_p],
+    ),
+    "bt_stft": (
+        c_int,
+        [c_void_p, POINTER(bt_stft_config), c_void_p, c_void_p, c_void_p, POINTER(c_int64), c_int32, c_void_p,
+         POINTER(c_int64), c_void_p],
+    ),
+    "bt_phase_vocoder": (
+        c_int,
+        [c_void_p, c_int32, c_void_p, POINTER(c_int64), c_int32, POINTER(c_int32), POINTER(c_double), c_int32, c_void_p,
+         POINTER(c_int64), c_void_p],
+    ),
+    "bt_istft": (
+        c_int,
+        [c_void_p, POINTER(bt_stft_config), c_void_p, c_void_p, c_void_p, POINTER(c_int64), c_int32, c_void_p,
+         POINTER(c_int64), c_void_p],
     ),
     "bt_spect2frames": (c_int, [c_void_p, c_void_p, POINTER(c_int64), c_int32, c_void_p, c_void_p, c_void_p]),
     "bt_forward_chunks": (c_int, [c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_void_p]),

@@ -182,6 +182,26 @@ void launch_beat_loss_backward(const float* x, const float* y, const float* m, c
                                const int64_t* tile_first_dev, int n_rows, int64_t n_tiles, int64_t n_scored,
                                const LossParams& p, const float* grad_mean, float* grad, cudaStream_t st);
 
+// ---- tempo / pitch augmentation (kernels_augment.cu) -----------------------------------------------------------------
+// The contracts of bt_stft, bt_phase_vocoder and bt_istft (include/beatthis.h).  spec: interleaved complex fp32,
+// n_fft / 2 + 1 bins per frame; log2n: 6..13.
+cudaError_t launch_stft(int log2n, const float* audio, const int64_t* sample_off_dev, const int64_t* frame_off_dev,
+                        int n_clips, int64_t total_frames, const float* window, const float* twiddle, int hop, float* spec,
+                        cudaStream_t st);
+// One time-stretched variant: input frames [in_base, in_base + T) at `rate` -> output frames [out_base, out_base + T_out)
+struct VocoderVariant {
+  int64_t in_base, out_base, T, T_out;
+  double rate;
+};
+void launch_phase_vocoder(const float* spec, const VocoderVariant* variants_dev, int n_variants, int bins, float* out,
+                          cudaStream_t st);
+// frames: scratch of total_frames * n_fft floats (the windowed inverse transform of every frame), gathered by the second
+// launch into out (sequence s: frames frame_off[s].., samples out_off[s]..); n_seqs <= 65535.
+cudaError_t launch_istft_frames(int log2n, const float* spec, int64_t total_frames, const float* window,
+                                const float* twiddle, float* frames, cudaStream_t st);
+void launch_istft_ola(const float* frames, const int64_t* frame_off_dev, const int64_t* out_off_dev, int n_seqs,
+                      int64_t max_out, const float* window, int n_fft, int hop, float* out, cudaStream_t st);
+
 void launch_f32_to_h16(const float* in, void* out, int64_t n, cudaStream_t st);
 void launch_h16_to_f32(const void* in, float* out, int64_t n, cudaStream_t st);
 // [seqs, L, heads*32] fp32 q,k,v -> packed qkv buffer [seqs*L, 3C] of the activation dtype

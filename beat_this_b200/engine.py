@@ -3,6 +3,7 @@ device memory, streams and pinned host buffers; every FLOP runs in libbeatthis_s
 from __future__ import annotations
 
 import ctypes
+import math
 from ctypes import c_void_p
 
 import numpy as np
@@ -226,6 +227,51 @@ class Engine:
             so.append(so[-1] + s.numel())
         spect, fo = self.logmel_config_cat(torch.cat(sigs) if len(sigs) > 1 else sigs[0], so, tables, device_tables)
         return [spect[fo[i] : fo[i + 1]] for i in range(len(sigs))]
+
+    # ---- tempo / pitch augmentation (augment.py; contracts in include/beatthis.h) -------------
+    def stft_cat(self, audio: torch.Tensor, sample_offsets, tables):
+        """bt_stft on flat fp32 device audio for the analysis of ``tables`` (augment.StftTables on this device):
+        (complex64 spectrogram [total_frames, n_fft / 2 + 1], frame_offsets)."""
+        assert audio.is_cuda and audio.dtype == torch.float32 and audio.is_contiguous()
+        fo = self.frame_offsets(sample_offsets, tables.hop_length)
+        spec = torch.empty((fo[-1], tables.bins), dtype=torch.complex64, device=self.device)
+        code = self.lib.bt_stft(self.ctx, ctypes.byref(tables.config), c_void_p(tables.window.data_ptr()),
+                                c_void_p(tables.twiddle.data_ptr()), c_void_p(audio.data_ptr()), i64_array(sample_offsets),
+                                len(sample_offsets) - 1, c_void_p(spec.data_ptr()), i64_array(fo), self._stream())
+        _lib.check(self.lib, self.ctx, code)
+        return spec, fo
+
+    def phase_vocoder_cat(self, spec: torch.Tensor, frame_offsets, variant_clip, variant_rate):
+        """bt_phase_vocoder: variant v is clip variant_clip[v] of ``spec`` (complex64 [total_frames, bins]) at rate
+        variant_rate[v].  Returns (complex64 [total_out_frames, bins], out_frame_offsets)."""
+        assert spec.is_cuda and spec.dtype == torch.complex64 and spec.is_contiguous() and spec.ndim == 2
+        n_clips, nv = len(frame_offsets) - 1, len(variant_clip)
+        oo = [0]
+        for clip, rate in zip(variant_clip, variant_rate):
+            T = int(frame_offsets[clip + 1]) - int(frame_offsets[clip]) if 0 <= clip < n_clips else 0
+            oo.append(oo[-1] + (math.ceil(T / rate) if rate > 0 and math.isfinite(rate) else 0))
+        out = torch.empty((oo[-1], spec.shape[1]), dtype=torch.complex64, device=self.device)
+        code = self.lib.bt_phase_vocoder(
+            self.ctx, 2 * (spec.shape[1] - 1), c_void_p(spec.data_ptr()), i64_array(frame_offsets), n_clips,
+            (ctypes.c_int32 * max(nv, 1))(*[int(v) for v in variant_clip]),
+            (ctypes.c_double * max(nv, 1))(*[float(r) for r in variant_rate]), nv, c_void_p(out.data_ptr()), i64_array(oo),
+            self._stream())
+        _lib.check(self.lib, self.ctx, code)
+        return out, oo
+
+    def istft_cat(self, spec: torch.Tensor, frame_offsets, lengths, tables):
+        """bt_istft: sequence s (frames frame_offsets[s]..) -> lengths[s] samples.  Returns (flat fp32 audio, sample
+        offsets)."""
+        assert spec.is_cuda and spec.dtype == torch.complex64 and spec.is_contiguous()
+        so = [0]
+        for n in lengths:
+            so.append(so[-1] + int(n))
+        out = torch.empty(max(so[-1], 1), dtype=torch.float32, device=self.device)[: so[-1]]
+        code = self.lib.bt_istft(self.ctx, ctypes.byref(tables.config), c_void_p(tables.window.data_ptr()),
+                                 c_void_p(tables.twiddle.data_ptr()), c_void_p(spec.data_ptr()), i64_array(frame_offsets),
+                                 len(frame_offsets) - 1, c_void_p(out.data_ptr()), i64_array(so), self._stream())
+        _lib.check(self.lib, self.ctx, code)
+        return out, so
 
     def spect2frames_cat(self, spect: torch.Tensor, frame_offsets, chunking: tuple | None = None):
         """Concatenated [total, 128] spectrograms -> (beat, downbeat) logits.  chunking: (chunk_size, border_size,

@@ -429,6 +429,65 @@ int bt_beat_loss_backward(bt_ctx* ctx, const float* preds_dev, const float* targ
                           const int64_t* row_offsets_host, int32_t n_rows, const bt_loss_params* params,
                           const float* grad_mean_dev, float* grad_preds_dev, void* stream);
 
+/* ---- tempo and pitch augmentation: the time stretch and pitch shift of launch_scripts/preprocess_audio.py ---------
+ * The reference calls pedalboard (Rubber Band) for both; its arithmetic is not in the reference tree, so parity with it
+ * is unpinned.  The contract here is the classic phase vocoder as torch.stft -> torchaudio.functional.phase_vocoder ->
+ * torch.istft define it, in three calls that share one analysis among any number of variants.  Spectrograms are
+ * interleaved complex fp32, n_fft / 2 + 1 bins per frame, the frames of all clips concatenated under CSR frame offsets
+ * (host, int64, starting at 0).  window_dev: the periodic Hann window of n_fft fp32 values; twiddle_dev: e^{-2 pi i j /
+ * n_fft}, j < n_fft / 2, interleaved fp32.  All three work on a weight-less ctx and only enqueue. */
+
+typedef struct bt_stft_config {
+  int32_t n_fft;      /* a power of two in [64, 8192]; win_length = n_fft */
+  int32_t hop_length; /* >= 1 */
+} bt_stft_config;
+
+#define BT_VOCODER_MIN_RATE 0.25
+#define BT_VOCODER_MAX_RATE 4.0
+
+/* Analysis: torch.stft(center=True, pad_mode="reflect", onesided=True, normalized=False).  Clip i (samples
+ * [sample_offsets_host[i], sample_offsets_host[i+1]) of audio_dev) gives 1 + len_i / hop_length frames.
+ * BT_ERR_ARG, before anything is enqueued, for an unsupported n_fft, hop_length < 1, a negative clip count, a null
+ * pointer, frame offsets that do not start at 0 or do not match, or a clip of at most n_fft / 2 samples (reflect
+ * padding is undefined there). */
+int bt_stft(bt_ctx* ctx, const bt_stft_config* cfg, const float* window_dev, const float* twiddle_dev,
+            const float* audio_dev, const int64_t* sample_offsets_host, int32_t n_clips, float* spec_dev,
+            const int64_t* frame_offsets_host, void* stream);
+
+/* Phase vocoder: variant v reads the T frames X of clip variant_clip_host[v] at rate r = variant_rate_host[v] (finite,
+ * in [BT_VOCODER_MIN_RATE, BT_VOCODER_MAX_RATE]) and writes ceil(T / r) frames (the division and ceil in float64) at
+ * out_frame_offsets_host[v].  For output frame j: s_j = j r in float64, i = floor(s_j), alpha = s_j - i, and the frame
+ * paired with i is i' = floor(s_j + 1) with the sum rounded to float64 as torchaudio indexes it: i + 1, except where s_j
+ * lies within an ulp below an integer, where it is i + 2.  Frames T and T + 1 of X are zero;
+ *   magnitude  alpha |X[i']| + (1 - alpha) |X[i]|,
+ *   phase      phi_0 = angle X[0],  phi_{j+1} = phi_j + wrap(angle X[i'] - angle X[i] - omega_k) + omega_k,
+ * omega_k = pi hop k / (n_fft / 2), wrap(x) = x - 2 pi round(x / 2 pi), angle 0 = 0; output magnitude e^{i phi_j}.
+ * Since wrap(x - omega_k) + omega_k = x (mod 2 pi) and only e^{i phi} is written, the kernel accumulates angle X[i'] -
+ * angle X[i] in float64, reduced modulo 2 pi after every step, and needs no hop: |error of phi_j| <= (2 j + 1) 2^-21
+ * rad (two atan2f of 2 ulp each per step), whatever the size of the unreduced phase.
+ * Any number of variants may name the same clip; listing a clip's variants together lets them share its analysis in
+ * L2.  Each variant is computed from its own clip and rate alone: bitwise repeatable and independent of the batch.
+ * BT_ERR_ARG, before anything is enqueued, for an unsupported n_fft, a null pointer, n_clips or n_variants < 0 or
+ * n_variants > 65535, a clip index out of range, a clip without frames, a rate outside the range or not finite, or
+ * offsets that do not start at 0 or do not match. */
+int bt_phase_vocoder(bt_ctx* ctx, int32_t n_fft, const float* spec_dev, const int64_t* frame_offsets_host,
+                     int32_t n_clips, const int32_t* variant_clip_host, const double* variant_rate_host,
+                     int32_t n_variants, float* out_dev, const int64_t* out_frame_offsets_host, void* stream);
+
+/* Synthesis: torch.istft(center=True, length=len_s) of each of n_seqs sequences of frames: the inverse real FFT of
+ * every frame (the imaginary parts of bins 0 and n_fft / 2 ignored) times the window, overlap-added at p = f
+ * hop_length, divided by the envelope sum w^2 of the frames that cover p, the first n_fft / 2 samples removed, cut or
+ * zero-extended to len_s = out_sample_offsets_host[s+1] - out_sample_offsets_host[s].  Every output sample gathers its
+ * frames in ascending order (no atomics): bitwise repeatable and independent of the batch.  The windowed frames pass
+ * through ctx scratch of 4 n_fft bytes per frame, which grows on demand.
+ * BT_ERR_ARG, before anything is enqueued, for the bt_stft_config errors, a null pointer, n_seqs < 0 or > 65535,
+ * offsets that decrease or frame offsets that do not start at 0, a sequence without frames, or an envelope (of the
+ * periodic Hann window, evaluated in float64 on the host) below 1e-11 at a sample some frame covers, as torch.istft
+ * refuses it: hop_length >= n_fft, or a length that reaches the last samples of the last frame. */
+int bt_istft(bt_ctx* ctx, const bt_stft_config* cfg, const float* window_dev, const float* twiddle_dev,
+             const float* spec_dev, const int64_t* frame_offsets_host, int32_t n_seqs, float* audio_out_dev,
+             const int64_t* out_sample_offsets_host, void* stream);
+
 /* ---- introspection / tuning ----------------------------------------------------------------- */
 
 /* Upper bound on the chunks processed per wave (1..256, default 128; one wave = one launch of every kernel of the
