@@ -1,0 +1,320 @@
+// C ABI (include/beatthis.h): the kernel test hooks (bt_debug_*).  Each checks its own arguments, then runs the
+// kernel under test once through run_hook (api_internal.h).
+#include "api_internal.h"
+
+static bool aligned16(const void* p) { return reinterpret_cast<uintptr_t>(p) % 16 == 0; }
+
+// The public chunk entries as the kernels' ChunkSrc, field by field (the internal layout stays private).
+static std::vector<ChunkSrc> chunk_table(const bt_debug_chunk* chunks, int32_t n) {
+  std::vector<ChunkSrc> v(n);
+  for (int32_t i = 0; i < n; ++i) {
+    ChunkSrc& s = v[i];
+    s.frame_base = chunks[i].frame_base;
+    s.T = chunks[i].T;
+    s.start = chunks[i].start;
+    s.out_base = chunks[i].out_base;
+    s.write_lo = chunks[i].write_lo;
+    s.write_hi = chunks[i].write_hi;
+    s.len = chunks[i].len;
+    s.pad_ = 0;
+  }
+  return v;
+}
+
+// A hook of a chunk-table kernel: uploads the checked table through the staging ring and launches the kernel
+// (launch(table_dev, st)) under the profile name `what`.
+template <class Launch>
+static int run_chunk_hook(bt_ctx* c, const char* fn, const char* what, const bt_debug_chunk* chunks, int32_t n, void* stream,
+                   Launch launch) {
+  const std::vector<ChunkSrc> table = chunk_table(chunks, n);
+  return run_hook(c, fn, stream, {}, [&](cudaStream_t st) {
+    const ChunkSrc* dev = nullptr;
+    const int r = stage(c, st, {{table.data(), table.size()}}, &dev);
+    if (r != BT_OK) return r;
+    launch(dev, st);
+    return check_launch(c, what, st);
+  });
+}
+
+extern "C" {
+
+int bt_debug_dbn_viterbi(bt_ctx* c, const double* log_dens_dev, int64_t T, int32_t beats, int32_t n_int,
+                         const int32_t* intervals, const double* log_tempo, const int32_t* pointers, int64_t* path_dev,
+                         double* logp_dev, void* stream) {
+  if (!c) return BT_ERR_ARG;
+  const char* fn = "bt_debug_dbn_viterbi";
+  if (!log_dens_dev || !intervals || !log_tempo || !pointers || !path_dev || !logp_dev || T <= 0)
+    return fail(c, BT_ERR_ARG, "%s: null argument or T <= 0", fn);
+  std::vector<DbnHostModel> ms(1);
+  int r = dbn_host_model(c, fn, beats, n_int, intervals, log_tempo, pointers, ms[0]);
+  if (r != BT_OK) return r;
+  int threads;
+  size_t smem, bp_per_frame;
+  dbn_launch_shape(ms, &threads, &smem, &bp_per_frame);
+  return run_hook(c, fn, stream, {}, [&](cudaStream_t st) {
+    const size_t ws_bytes = 2 * sizeof(double), bp_bytes = bp_per_frame * T;
+    BT_CUDA(c, c->dbn_ws.reserve(ws_bytes, ws_bytes + ws_bytes / 4));
+    BT_CUDA(c, c->dbn_bp.reserve(bp_bytes, bp_bytes + bp_bytes / 4));
+    const int64_t fo[2] = {0, T}, win_h[2] = {0, T};
+    const DbnModelDev* md = nullptr;
+    const int64_t *fo_dev = nullptr, *win = nullptr;
+    const int rs = dbn_stage(c, ms, fo, 1, T, win_h, st, &md, &fo_dev, &win);
+    if (rs != BT_OK) return rs;
+    double* res_logp = reinterpret_cast<double*>(c->dbn_ws.get());
+    int64_t* res_state = reinterpret_cast<int64_t*>(res_logp + 1);
+    uint8_t* bp = c->dbn_bp.get();
+    BT_LAUNCHED(c, "dbn_viterbi", st,
+                launch_dbn_viterbi(md, 1, threads, smem, log_dens_dev, fo_dev, win, 1, bp, res_logp, res_state, st));
+    launch_dbn_backtrace(md, 1, fo_dev, win, 1, bp, res_logp, res_state, nullptr, nullptr, 0, 1.0, nullptr, nullptr,
+                         nullptr, path_dev, logp_dev, st);
+    return check_launch(c, "dbn_backtrace", st);
+  });
+}
+
+int bt_debug_gemm(bt_ctx* c, const bt_debug_gemm_desc* d, const float* a_dev, const float* w_dev,
+                  const float* bias_dev, const float* resid_dev, float* out_f32_dev, float* out_act_dev,
+                  int64_t out_act_count, const float* rope_cos_dev, const float* rope_sin_dev, int32_t* tile_out,
+                  void* stream) {
+  const char* fn = "bt_debug_gemm";
+  if (!c || !d || !a_dev || !w_dev) return fail(c, BT_ERR_ARG, "%s: null argument", fn);
+  if (d->nslab < 1 || d->nslab > kMaxSlabs || d->planes_out < 1 || d->L < 1 || d->N % 4 != 0 || d->Kslab % 16 != 0 ||
+      d->lda % 4 != 0 || (out_act_dev && out_act_count < static_cast<int64_t>(d->planes_out) * d->L * d->N))
+    return fail(c, BT_ERR_ARG, "%s: unsupported shape", fn);
+  GemmShape g{};
+  g.planes_out = d->planes_out; g.L = d->L; g.N = d->N; g.Kslab = d->Kslab; g.nslab = d->nslab;
+  g.plane_mul = d->plane_mul; g.lda = d->lda;
+  for (int s = 0; s < kMaxSlabs; ++s) { g.plane_add[s] = d->plane_add[s]; g.t_shift[s] = d->t_shift[s]; }
+  EpiParams e{};
+  e.kind = d->kind; e.bias = bias_dev; e.gelu = d->gelu;
+  e.resid = resid_dev; e.ldr = d->N;
+  e.out_f32 = out_f32_dev; e.ldo_f32 = d->N;
+  e.out_act = out_act_dev; e.ldo_act = d->N;
+  e.rope_cos = rope_cos_dev; e.rope_sin = rope_sin_dev;
+  e.C = d->C; e.heads = d->heads; e.posmode = d->posmode; e.F = d->F; e.qscale = d->qscale;
+  if (tile_out) tile_out[0] = tile_out[1] = 0;
+  HookArray a(a_dev, static_cast<int64_t>(d->planes_in) * d->L * d->lda);
+  HookArray w(w_dev, static_cast<int64_t>(d->N) * d->Kslab * d->nslab);
+  HookArray out_act(out_act_dev, out_act_count, true);
+  return run_hook(c, fn, stream, {&a, &w, &out_act}, [&](cudaStream_t st) {
+    if (c->dtype != BT_DTYPE_H16) {
+      launch_gemm_simt(a_dev, w_dev, g, e, st);
+      return check_launch(c, "debug_gemm", st);
+    }
+    e.out_act = out_act.h16.get();
+    GemmPlan p;
+    const int r = make_plan(c, fn, p, [&](char* err, int n) {
+      return tc_gemm_plan_create(a.h16.get(), w.h16.get(), g, d->planes_in, d->resid_epilogue != 0, e, err, n);
+    });
+    if (r != BT_OK) return r;
+    if (tile_out) tc_gemm_plan_tile(p.get(), &tile_out[0], &tile_out[1]);
+    launch_gemm_tc(p.get(), st);
+    return check_launch(c, "debug_gemm", st);
+  });
+}
+
+int bt_debug_attention(bt_ctx* c, const float* q_dev, const float* k_dev, const float* v_dev, const float* gates_dev,
+                       float* o_dev, int64_t o_count, int32_t seqs, int32_t L, int32_t heads,
+                       const int32_t* key_lens_host, int32_t seqs_per_chunk, void* stream) {
+  const char* fn = "bt_debug_attention";
+  if (!c || !q_dev || !k_dev || !v_dev || !gates_dev || !o_dev) return fail(c, BT_ERR_ARG, "%s: null argument", fn);
+  if (seqs < 1 || L < 1 || heads < 1 || (key_lens_host && (seqs_per_chunk < 1 || seqs % seqs_per_chunk != 0)))
+    return fail(c, BT_ERR_ARG, "%s: bad geometry", fn);
+  const int C = heads * 32;
+  const int64_t M = static_cast<int64_t>(seqs) * L;
+  if (o_count < M * C)
+    return fail(c, BT_ERR_ARG, "%s: o holds %lld elements, fewer than M * C", fn, static_cast<long long>(o_count));
+  // per-chunk key counts travel in the ChunkSrc table the forward pass hands the kernels (only .len is read)
+  std::vector<ChunkSrc> chunks;
+  if (key_lens_host) {
+    chunks.assign(seqs / seqs_per_chunk, ChunkSrc{});
+    for (size_t i = 0; i < chunks.size(); ++i) {
+      if (key_lens_host[i] < 1 || key_lens_host[i] > L) return fail(c, BT_ERR_ARG, "%s: key length out of [1, L]", fn);
+      chunks[i].len = key_lens_host[i];
+    }
+  }
+  const bool tc = c->dtype == BT_DTYPE_H16;
+  HookArray o(o_dev, o_count, true);
+  DeviceBuffer<> qkv;
+  return run_hook(c, fn, stream, {&o}, [&](cudaStream_t st) {
+    BT_CUDA(c, qkv.alloc(M * 3 * C * (tc ? 2 : 4)));
+    const ChunkSrc* chunks_dev = nullptr;
+    int r = chunks.empty() ? BT_OK : stage(c, st, {{chunks.data(), chunks.size()}}, &chunks_dev);
+    if (r != BT_OK) return r;
+    if (tc) {
+      launch_pack_qkv_test(q_dev, k_dev, v_dev, qkv.get(), seqs, L, heads, 0.17677669529663687f * 1.4426950408889634f, 1,
+                           st);
+      AttnPlan p;
+      r = make_plan(c, fn, p, [&](char* err, int n) { return tc_attn_plan_create(qkv.get(), seqs, L, heads, err, n); });
+      if (r != BT_OK) return r;
+      launch_attn_time_tc(p.get(), gates_dev, o.h16.get(), st, chunks_dev, seqs_per_chunk);
+    } else {
+      launch_pack_qkv_test(q_dev, k_dev, v_dev, qkv.get(), seqs, L, heads, 1.0f, 0, st);
+      launch_attn_time_simt(static_cast<const float*>(qkv.get()), gates_dev, o_dev, seqs, L, heads, st, chunks_dev,
+                            seqs_per_chunk);
+    }
+    return check_launch(c, "debug_attention", st);
+  });
+}
+
+int bt_debug_attention_freq(bt_ctx* c, const float* q_dev, const float* k_dev, const float* v_dev,
+                            const float* gates_dev, float* o_dev, int64_t o_count, int32_t B, int32_t F, int32_t L,
+                            int32_t heads, void* stream) {
+  const char* fn = "bt_debug_attention_freq";
+  if (!c || !q_dev || !k_dev || !v_dev || !gates_dev || !o_dev) return fail(c, BT_ERR_ARG, "%s: null argument", fn);
+  if (B < 1 || L < 1 || heads < 1 || (F != 8 && F != 16 && F != 32))
+    return fail(c, BT_ERR_ARG, "%s: need B, L, heads >= 1 and F in {8, 16, 32}", fn);
+  const int C = heads * 32;
+  const int64_t M = static_cast<int64_t>(B) * F * L;
+  if (o_count < M * C)
+    return fail(c, BT_ERR_ARG, "%s: o holds %lld elements, fewer than M * C", fn, static_cast<long long>(o_count));
+  const bool tc = c->dtype == BT_DTYPE_H16;
+  const float inv_sqrt_d = 0.17677669529663687f;
+  HookArray o(o_dev, o_count, true);
+  DeviceBuffer<> qkv;
+  return run_hook(c, fn, stream, {&o}, [&](cudaStream_t st) {
+    BT_CUDA(c, qkv.alloc(M * 3 * C * (tc ? 2 : 4)));
+    FreqPlan p;
+    const int r = !tc ? BT_OK : make_plan(c, fn, p, [&](char* err, int n) {
+      return tc_freq_plan_create(qkv.get(), o.h16.get(), B, F, L, heads, err, n);
+    }, BT_ERR_ARG);
+    if (r != BT_OK) return r;
+    launch_pack_qkv_test(q_dev, k_dev, v_dev, qkv.get(), B * F, L, heads, 1.0f, tc ? 1 : 0, st);
+    if (tc) launch_attn_freq_tc(p.get(), gates_dev, inv_sqrt_d, st);
+    else launch_attn_freq_simt(static_cast<const float*>(qkv.get()), gates_dev, o_dev, B, F, L, heads, inv_sqrt_d, st);
+    return check_launch(c, "debug_attention_freq", st);
+  });
+}
+
+int bt_debug_norm(bt_ctx* c, const float* x_dev, float* xn_dev, int64_t M, int32_t C, const float* wg_dev,
+                  const float* bg_dev, float* gates_dev, int32_t heads, void* stream) {
+  if (!c) return BT_ERR_ARG;
+  const char* fn = "bt_debug_norm";
+  const bool tc = c->dtype == BT_DTYPE_H16;
+  if (!x_dev || !xn_dev || !aligned16(x_dev) || (!tc && !aligned16(xn_dev)))  // the fp32 context stores xn directly
+    return fail(c, BT_ERR_ARG, "%s: need x and xn (16-byte aligned; xn only in the fp32 context)", fn);
+  if (M < 1 || (C != 32 && C != 64 && C != 128 && C != 256 && C != 512 && C != 1024))
+    return fail(c, BT_ERR_ARG, "%s: need M >= 1 and C in {32, 64, 128, 256, 512, 1024}", fn);
+  if (gates_dev ? (!wg_dev || !bg_dev || !aligned16(wg_dev) || heads < 1 || 32 * heads > C) : heads != 0)
+    return fail(c, BT_ERR_ARG, "%s: gates need wg (16-byte aligned), bg and 1 <= heads <= C / 32; no gates, heads 0", fn);
+  HookArray xn(xn_dev, M * C, true);
+  return run_hook(c, fn, stream, {&xn}, [&](cudaStream_t st) {
+    launch_norm(x_dev, tc ? xn.h16.get() : static_cast<void*>(xn_dev), M, C, tc ? 1 : 0, st, gates_dev, wg_dev, bg_dev,
+                heads);
+    return check_launch(c, "debug_norm", st);
+  });
+}
+
+int bt_debug_fused_qkv(bt_ctx* c, const float* x_dev, const float* wqkv_dev, const float* wg_dev, const float* bg_dev,
+                       const float* rope_cos_dev, const float* rope_sin_dev, float* qkv_dev, float* gates_dev, int64_t M,
+                       int32_t C, int32_t L, int32_t F, int32_t posmode, float qscale, void* stream) {
+  if (!c) return BT_ERR_ARG;
+  const char* fn = "bt_debug_fused_qkv";
+  if (c->dtype != BT_DTYPE_H16) return fail(c, BT_ERR_ARG, "%s: the fused kernel runs in the 16-bit context only", fn);
+  if (!x_dev || !wqkv_dev || !wg_dev || !bg_dev || !rope_cos_dev || !rope_sin_dev || !qkv_dev || !gates_dev ||
+      !aligned16(x_dev) || !aligned16(wg_dev))
+    return fail(c, BT_ERR_ARG, "%s: null argument, or x / wg not 16-byte aligned", fn);
+  if (M < 1 || (C != 32 && C != 64) || L < 1 || L > BT_CHUNK || (posmode != 0 && posmode != 1) ||
+      (posmode == 1 && (F < 1 || F > BT_CHUNK)))
+    return fail(c, BT_ERR_ARG, "%s: need M >= 1, C in {32, 64}, 1 <= L <= %d, posmode 0 or 1 (1: 1 <= F <= %d)", fn,
+                BT_CHUNK, BT_CHUNK);
+  HookArray wqkv(wqkv_dev, 3 * C * C), qkv(qkv_dev, M * 3 * C, true);
+  return run_hook(c, fn, stream, {&wqkv, &qkv}, [&](cudaStream_t st) {
+    QkvPlan p;
+    const int r = make_plan(c, fn, p, [&](char* err, int n) { return tc_qkv_plan_create(wqkv.h16.get(), C, M, err, n); });
+    if (r != BT_OK) return r;
+    launch_fused_qkv(p.get(), x_dev, wg_dev, bg_dev, rope_cos_dev, rope_sin_dev, qkv.h16.get(), gates_dev, L, F, posmode,
+                     qscale, st);
+    return check_launch(c, "debug_fused_qkv", st);
+  });
+}
+
+int bt_debug_fused_ff(bt_ctx* c, float* x_dev, const float* w1_dev, const float* b1_dev, const float* w2_dev,
+                      const float* b2_dev, const float* o_dev, const float* wout_dev, float* xb_dev, int64_t M, int32_t C,
+                      void* stream) {
+  if (!c) return BT_ERR_ARG;
+  const char* fn = "bt_debug_fused_ff";
+  if (c->dtype != BT_DTYPE_H16) return fail(c, BT_ERR_ARG, "%s: the fused kernel runs in the 16-bit context only", fn);
+  if (!x_dev || !w1_dev || !b1_dev || !w2_dev || !b2_dev || !aligned16(x_dev) || !aligned16(b1_dev) ||
+      !aligned16(b2_dev) || !o_dev != !wout_dev)
+    return fail(c, BT_ERR_ARG, "%s: null argument, x / b1 / b2 not 16-byte aligned, or only one of o and wout", fn);
+  if (M < 1 || (C != 32 && C != 64)) return fail(c, BT_ERR_ARG, "%s: need M >= 1 and C in {32, 64}", fn);
+  HookArray w1(w1_dev, 4 * C * C), w2(w2_dev, 4 * C * C), o(o_dev, M * C), wout(wout_dev, C * C), xb(xb_dev, M * C, true);
+  return run_hook(c, fn, stream, {&w1, &w2, &o, &wout, &xb}, [&](cudaStream_t st) {
+    FfPlan p;
+    const int r = make_plan(c, fn, p, [&](char* err, int n) {
+      return tc_ff_plan_create(w1.h16.get(), w2.h16.get(), C, M, o.h16.get(), wout.h16.get(), err, n);
+    });
+    if (r != BT_OK) return r;
+    launch_fused_ff(p.get(), x_dev, b1_dev, b2_dev, xb.h16.get(), st);
+    return check_launch(c, "debug_fused_ff", st);
+  });
+}
+
+int bt_debug_stem(bt_ctx* c, const float* spect_dev, int64_t spect_frames, const bt_debug_chunk* chunks_host,
+                  int32_t n_chunks, int32_t L, const float* bn1_scale_dev, const float* bn1_shift_dev, const float* w_dev,
+                  const float* bias_dev, float* out_dev, int64_t out_count, void* stream) {
+  if (!c) return BT_ERR_ARG;
+  const char* fn = "bt_debug_stem";
+  if (!spect_dev || !chunks_host || !bn1_scale_dev || !bn1_shift_dev || !w_dev || !bias_dev || !out_dev ||
+      !aligned16(spect_dev) || !aligned16(out_dev))
+    return fail(c, BT_ERR_ARG, "%s: null argument, or spect / out not 16-byte aligned (float4 loads and stores)", fn);
+  if (n_chunks < 1 || n_chunks > 65535 || L < 1 || L > kMaxChunkCap)
+    return fail(c, BT_ERR_ARG, "%s: need 1 <= n_chunks <= 65535 and 1 <= L <= %lld", fn, (long long)kMaxChunkCap);
+  for (int32_t i = 0; i < n_chunks; ++i) {
+    const bt_debug_chunk& k = chunks_host[i];
+    if (k.T < 1 || k.len < 1 || k.len > L || k.frame_base < 0 || k.frame_base > spect_frames - k.T)
+      return fail(c, BT_ERR_ARG, "%s: chunk %d needs T >= 1, 1 <= len <= L and its clip inside the %lld spectrogram "
+                  "frames", fn, i, (long long)spect_frames);
+  }
+  if (out_count < static_cast<int64_t>(n_chunks) * 32 * L * 32)
+    return fail(c, BT_ERR_ARG, "%s: out holds %lld floats, fewer than n_chunks * 32 * L * 32", fn, (long long)out_count);
+  return run_chunk_hook(c, fn, "stem", chunks_host, n_chunks, stream, [&](const ChunkSrc* t, cudaStream_t st) {
+    launch_stem(spect_dev, t, n_chunks, L, bn1_scale_dev, bn1_shift_dev, w_dev, bias_dev, out_dev, st);
+  });
+}
+
+int bt_debug_zero_tail(bt_ctx* c, void* buf_dev, int32_t elem_bytes, const bt_debug_chunk* chunks_host,
+                       int32_t n_chunks, int32_t F, int32_t L, int32_t C, int64_t buf_bytes, void* stream) {
+  if (!c) return BT_ERR_ARG;
+  const char* fn = "bt_debug_zero_tail";
+  if (!buf_dev || !chunks_host || !aligned16(buf_dev))
+    return fail(c, BT_ERR_ARG, "%s: null argument, or buf not 16-byte aligned", fn);
+  if ((elem_bytes != 2 && elem_bytes != 4) || C < 1 || (static_cast<int64_t>(C) * elem_bytes) % 16 != 0 ||
+      n_chunks < 1 || F < 1 || static_cast<int64_t>(n_chunks) * F > INT32_MAX || L < 1 || L > kMaxChunkCap)
+    return fail(c, BT_ERR_ARG, "%s: need elem_bytes 2 or 4, C * elem_bytes a multiple of 16, n_chunks, F >= 1 with "
+                "n_chunks * F < 2^31 and 1 <= L <= %lld", fn, (long long)kMaxChunkCap);
+  for (int32_t i = 0; i < n_chunks; ++i)
+    if (chunks_host[i].len < 1 || chunks_host[i].len > L)
+      return fail(c, BT_ERR_ARG, "%s: chunk %d has len %d outside [1, L]", fn, i, chunks_host[i].len);
+  if (buf_bytes / elem_bytes / C / L / F < n_chunks)
+    return fail(c, BT_ERR_ARG, "%s: buf holds %lld bytes, fewer than n_chunks * F * L * C elements", fn,
+                (long long)buf_bytes);
+  return run_chunk_hook(c, fn, "zero_tail", chunks_host, n_chunks, stream, [&](const ChunkSrc* t, cudaStream_t st) {
+    launch_zero_tail(buf_dev, elem_bytes, t, n_chunks, F, L, C, st);
+  });
+}
+
+int bt_debug_head(bt_ctx* c, const float* x_dev, int32_t D, const float* w_dev, const float* b_dev,
+                  const bt_debug_chunk* chunks_host, int32_t n_chunks, int32_t L, int32_t sum_head, float* beat_dev,
+                  float* down_dev, int64_t out_count, void* stream) {
+  if (!c) return BT_ERR_ARG;
+  const char* fn = "bt_debug_head";
+  if (!x_dev || !w_dev || !b_dev || !chunks_host || !beat_dev || !down_dev)
+    return fail(c, BT_ERR_ARG, "%s: null argument", fn);
+  if (D < 64 || D > 1024 || D % 64 != 0 || n_chunks < 1 || L < 1 || static_cast<int64_t>(n_chunks) * L > INT32_MAX)
+    return fail(c, BT_ERR_ARG, "%s: need D a multiple of 64 in [64, 1024], n_chunks, L >= 1 and n_chunks * L < 2^31", fn);
+  for (int32_t i = 0; i < n_chunks; ++i) {
+    const bt_debug_chunk& k = chunks_host[i];
+    if (k.write_lo < 0 || k.write_lo > k.write_hi || k.write_hi > L)
+      return fail(c, BT_ERR_ARG, "%s: chunk %d owns [%d, %d), not inside [0, L]", fn, i, k.write_lo, k.write_hi);
+    const int64_t first = k.out_base + k.start + k.write_lo, last = k.out_base + k.start + k.write_hi - 1;
+    if (k.write_lo < k.write_hi && (first < 0 || last >= out_count))
+      return fail(c, BT_ERR_ARG, "%s: chunk %d writes frames [%lld, %lld], outside [0, %lld)", fn, i, (long long)first,
+                  (long long)last, (long long)out_count);
+  }
+  return run_chunk_hook(c, fn, "head", chunks_host, n_chunks, stream, [&](const ChunkSrc* t, cudaStream_t st) {
+    launch_head(x_dev, D, w_dev, b_dev, t, n_chunks, L, beat_dev, down_dev, sum_head ? 1 : 0, st);
+  });
+}
+
+}  // extern "C"

@@ -1,4 +1,4 @@
-// Move-only owners of the CUDA resources bt_api.cu allocates: device and pinned host buffers, events and the
+// Move-only owners of the CUDA resources the C ABI allocates: device and pinned host buffers, events and the
 // tensor-core plans.  Each releases what it holds when it is destroyed or assigned over, so a bt_ctx that holds them
 // frees everything it allocated when it is deleted (with its device current).
 #pragma once

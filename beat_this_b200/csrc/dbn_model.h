@@ -1,5 +1,5 @@
 // Bar-pointer model of the DBN post-processor (beat_this_b200/dbn.py::_BarModel), shared by the host tracker
-// (dbn_host.cpp) and the device tracker (bt_dbn_track_device in bt_api.cu, kernels in kernels_dbn.cu): both decode
+// (dbn_host.cpp) and the device tracker (bt_dbn_track_device in api_post.cu, kernels in kernels_dbn.cu): both decode
 // exactly the tables built here.  Host code only.
 #pragma once
 #include <algorithm>

@@ -12,6 +12,9 @@
  *  - plain C types only; no torch / CUDA types in signatures (streams travel as void*).
  *  - `*_dev` pointers are device pointers on the context's GPU, `*_host` are host pointers.
  *  - ragged batches are CSR style: `offsets[n+1]` (host, int64) into a concatenated buffer.
+ *    Offsets never decrease, and offsets[0] is >= 0, or exactly 0 where an entry point says so.
+ *    Every ctx entry point checks this before anything is enqueued and returns BT_ERR_ARG
+ *    ("<entry point>: <offsets> must ...") otherwise.
  *  - all work is enqueued on the given CUDA stream (cudaStream_t as void*, NULL = default
  *    stream); no hidden device synchronisation except where stated.
  *  - return value: 0 = ok, negative = error (bt_last_error() gives the text).  Nothing
@@ -195,7 +198,8 @@ int bt_stage_wav_files(const char* const* paths, const bt_wav_info* infos, int32
 /* LogMelSpect.forward (preprocessing.py:56-59) for n_clips mono 22.05 kHz clips.
  * audio_dev: concatenated fp32 samples; sample_offsets_host[n_clips+1].
  * spect_dev: out, concatenated [T_i,128] fp32 with T_i = bt_num_frames(len_i), laid out
- * at frame_offsets_host[i] (frames; frame_offsets_host[n_clips+1]). */
+ * at frame_offsets_host[i] (frames; frame_offsets_host[n_clips+1], starting at 0).  Every clip needs more than
+ * BT_N_FFT/2 samples. */
 int bt_logmel(bt_ctx* ctx, const float* audio_dev, const int64_t* sample_offsets_host,
               int32_t n_clips, float* spect_dev, const int64_t* frame_offsets_host,
               void* stream);
