@@ -15,7 +15,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 # BT_LIB_PATH: an instrumented build of the same sources (e.g. build(extra_flags=("-DBT_FF_PROF",), out_path=...))
 LIB_PATH = os.environ.get("BT_LIB_PATH") or os.path.join(HERE, "libbeatthis_sm90.so")
-SOURCES = ["bt_api.cu", "api_signal.cu", "api_post.cu", "api_debug.cu", "kernels_simt.cu", "kernels_misc.cu", "kernels_gemm.cu", "kernels_attn.cu", "kernels_fused.cu", "kernels_dbn.cu", "kernels_eval.cu", "kernels_loss.cu", "kernels_augment.cu", "dbn_host.cpp", "host_stage.cpp"]
+SOURCES = ["bt_api.cu", "api_signal.cu", "api_post.cu", "api_data.cu", "api_debug.cu", "kernels_simt.cu", "kernels_misc.cu", "kernels_gemm.cu", "kernels_attn.cu", "kernels_fused.cu", "kernels_dbn.cu", "kernels_eval.cu", "kernels_loss.cu", "kernels_augment.cu", "kernels_data.cu", "dbn_host.cpp", "host_stage.cpp"]
 HEADERS = ["common.cuh", "epilogue.cuh", "fft.cuh", "tc_common.cuh", "bt_kernels.h", "cuda_owned.h", "dbn_model.h",
            "api_internal.h", os.path.join("..", "..", "include", "beatthis.h")]
 
@@ -218,6 +218,11 @@ PROTOTYPES = {
         c_int,
         [c_void_p, POINTER(bt_stft_config), c_void_p, c_void_p, c_void_p, POINTER(c_int64), c_int32, c_void_p,
          POINTER(c_int64), c_void_p],
+    ),
+    "bt_train_batch": (
+        c_int,
+        [c_void_p, c_void_p, POINTER(c_int64), c_int32, c_int32, POINTER(c_int32), POINTER(c_int32), POINTER(c_int64),
+         POINTER(c_int32), POINTER(c_int64), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
     ),
     "bt_spect2frames": (c_int, [c_void_p, c_void_p, POINTER(c_int64), c_int32, c_void_p, c_void_p, c_void_p]),
     "bt_forward_chunks": (c_int, [c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_void_p]),

@@ -1,4 +1,4 @@
-// Private to the C ABI's host files (bt_api.cu, api_signal.cu, api_post.cu, api_debug.cu): bt_ctx, the entry prologue
+// Private to the C ABI's host files (bt_api.cu, api_signal.cu, api_post.cu, api_data.cu, api_debug.cu): bt_ctx, the entry prologue
 // and argument checks, errors and launch checks, the staging ring, plan slots and the test-hook harness.
 #pragma once
 #include <algorithm>

@@ -202,6 +202,13 @@ cudaError_t launch_istft_frames(int log2n, const float* spec, int64_t total_fram
 void launch_istft_ola(const float* frames, const int64_t* frame_off_dev, const int64_t* out_off_dev, int n_seqs,
                       int64_t max_out, const float* window, int n_fft, int hop, float* out, cudaStream_t st);
 
+// ---- training batches (kernels_data.cu) -----------------------------------------------------------------------------
+// The contract of bt_train_batch (include/beatthis.h); all tables on the device, row_map may be null (identity).
+void launch_train_batch(const uint16_t* rows, const int64_t* row_off, int n_items, int length, const int32_t* row_map,
+                        const int32_t* beats, const int64_t* beat_off, const int32_t* downs, const int64_t* down_off,
+                        uint16_t* spect, uint8_t* truth_beat, uint8_t* truth_downbeat, uint8_t* padding_mask,
+                        cudaStream_t st);
+
 void launch_f32_to_h16(const float* in, void* out, int64_t n, cudaStream_t st);
 void launch_h16_to_f32(const void* in, float* out, int64_t n, cudaStream_t st);
 // [seqs, L, heads*32] fp32 q,k,v -> packed qkv buffer [seqs*L, 3C] of the activation dtype

@@ -13,6 +13,7 @@
 
     python -m beat_this_b200.evaluate --models final0.ckpt --data data          # prepared dataset layout
     python -m beat_this_b200.evaluate --models final0.ckpt --audio songs/ --annotations beats/
+    python -m beat_this_b200.evaluate --models fold*.ckpt --data data --datasplit val --aggregation-type k-fold
 """
 from __future__ import annotations
 
@@ -227,8 +228,8 @@ def make_runner(model, device="cuda", float16=True, dbn=False, dbn_impl="auto"):
     return File2Beats.from_model(model, dbn=dbn, dbn_impl=dbn_impl)
 
 
-def evaluate(model_or_runner, items, min_beat_time=5.0, device="cuda", float16=True, dbn=False, dbn_impl="auto",
-             losses=False, fps=None):
+def evaluate(model_or_runner, items=None, min_beat_time=5.0, device="cuda", float16=True, dbn=False, dbn_impl="auto",
+             losses=False, fps=None, data=None, datasplit=None, datamodule_hparams=None):
     """Predict every Piece of `items` with the model (a File2Beats / Audio2Beats runner, a BeatThisB200 or a checkpoint;
     float16 / dbn / dbn_impl apply when a runner has to be built) and score it against its annotations: truth cut to
     [0, T / fps) for a spectrogram of T frames, beats and downbeats of all pieces in one bt_beat_metrics launch.
@@ -238,9 +239,23 @@ def evaluate(model_or_runner, items, min_beat_time=5.0, device="cuda", float16=T
     "Cemgil_<target>" is the reference's mean of mir_eval's (cemgil, cemgil_max) pair (pl_module.py:157-160); both
     parts stay available as cemgil_<target> and cemgil_max_<target>.  Pieces without downbeat annotations score 0 on
     the downbeat keys, as in the reference.  With `losses`, metrics also hold every piece's test_loss_beat,
-    test_loss_downbeat and test_loss (piece_losses), and summary their means."""
+    test_loss_downbeat and test_loss (piece_losses), and summary their means.
+    datasplit ("train", "val" or "test"): instead of `items`, the full pieces of that split of the prepared dataset
+    `data` (split_pieces) under `datamodule_hparams`, by default the checkpoint's datamodule_hyper_parameters when
+    model_or_runner is a checkpoint (else BeatDataModule's defaults)."""
     from .postprocessor import Postprocessor, check_fps
 
+    if datasplit is not None:
+        if items is not None or data is None:
+            raise ValueError("datasplit selects the pieces of `data`: give data and no items")
+        if datamodule_hparams is None and isinstance(model_or_runner, (str, Path, dict)):
+            from .inference import load_checkpoint
+
+            ckpt = model_or_runner if isinstance(model_or_runner, dict) else load_checkpoint(model_or_runner, "cpu")
+            datamodule_hparams = ckpt.get("datamodule_hyper_parameters", {})
+        items = split_pieces(data, datasplit, datamodule_hparams)
+    elif items is None:
+        raise ValueError("evaluate needs items, or data and a datasplit")
     runner = model_or_runner
     if not hasattr(runner, "frames2beats"):
         runner = make_runner(runner, device, float16, dbn, dbn_impl)
@@ -290,15 +305,20 @@ def dataset_name(dataset: str, stem: str) -> str:
     return "rwc_" + stem.split("_", 2)[1] if dataset == "rwc" else dataset
 
 
-def discover_data(data_dir, items_file=None) -> list:
+def discover_data(data_dir, items_file=None, names=None) -> list:
     """Pieces of the reference's prepared layout: DIR/annotations/<dataset>/annotations/beats/<stem>.beats with the
     spectrogram in DIR/audio/spectrograms/<dataset>.npz (key <stem>/track) or .../<dataset>/<stem>/track.npy
     (float16 as stored, cast to fp32).  <dataset>/info.json's has_downbeats is honoured when present: false drops the
     downbeat truth, true skips a piece whose file has one column (as the reference's dataset does).  items_file:
-    lines "dataset/stem" restricting the set."""
+    lines "dataset/stem" restricting the set; names: the same as a list.  Bundles are read through
+    dataset.Bundle (memory-mapped, float16 members only)."""
+    from .dataset import Bundle
+
     root = Path(data_dir)
     ann = root / "annotations"
-    if items_file is not None:
+    if names is not None:
+        names = list(names)
+    elif items_file is not None:
         names = [ln.strip() for ln in Path(items_file).read_text().splitlines() if ln.strip()]
     else:
         names = [f"{d.name}/{f.stem}" for d in sorted(p for p in ann.iterdir() if p.is_dir())
@@ -310,7 +330,7 @@ def discover_data(data_dir, items_file=None) -> list:
             info = ann / dataset / "info.json"
             infos[dataset] = json.loads(info.read_text()) if info.exists() else {}
             npz = root / "audio" / "spectrograms" / f"{dataset}.npz"
-            bundles[dataset] = np.load(npz) if npz.exists() else None
+            bundles[dataset] = Bundle(npz) if npz.exists() else None
         beats, downbeats, has_down = load_beat_annotations(ann / dataset / "annotations" / "beats" / f"{stem}.beats")
         declared = infos[dataset].get("has_downbeats")
         if declared and not has_down:
@@ -319,13 +339,22 @@ def discover_data(data_dir, items_file=None) -> list:
         if declared is False:
             downbeats, has_down = np.zeros(0), False
         bundle = bundles[dataset]
-        if bundle is not None and f"{stem}/track" in bundle.files:
+        if bundle is not None and f"{stem}/track" in bundle:
             spect = bundle[f"{stem}/track"]
         else:
             spect = np.load(root / "audio" / "spectrograms" / dataset / stem / "track.npy")
         pieces.append(Piece(f"{name}/track.npy", beats, downbeats, has_down, dataset_name(dataset, stem),
                             spect=np.asarray(spect, dtype=np.float32)))
     return pieces
+
+
+def split_pieces(data_dir, datasplit, datamodule_hparams=None) -> list:
+    """discover_data's pieces for one split ("train", "val" or "test") of a prepared dataset under a checkpoint's
+    datamodule hyper-parameters (test_dataset, fold, hung_data, no_val; dataset.split_items), always full pieces, as
+    compute_paper_metrics.datamodule_setup selects them (:159-171)."""
+    from .dataset import split_items
+
+    return discover_data(data_dir, names=split_items(data_dir, datasplit, datamodule_hparams))
 
 
 def discover_audio(paths, annotations_dir) -> list:
@@ -358,7 +387,11 @@ def build_parser() -> argparse.ArgumentParser:
     src.add_argument("--data", help="prepared dataset directory (annotations/ and audio/spectrograms/)")
     src.add_argument("--audio", nargs="+", help="audio files or directories (with --annotations)")
     add("--annotations", help="directory of <stem>.beats files for --audio")
-    add("--items", help="file of 'dataset/stem' lines restricting --data")
+    pick = ap.add_mutually_exclusive_group()
+    pick.add_argument("--items", help="file of 'dataset/stem' lines restricting --data")
+    pick.add_argument("--datasplit", choices=["train", "val", "test"], default=None,
+                      help="score the pieces of this split of --data under each checkpoint's datamodule "
+                           "hyper-parameters (default: every annotated piece)")
     add("--gpu", type=int, default=0)
     add("--eval-trim-beats", metavar="SECONDS", type=float, default=None,
         help="skip beats before this time (default: the checkpoint's eval_trim_beats, else 5)")
@@ -367,8 +400,9 @@ def build_parser() -> argparse.ArgumentParser:
     add("--dbn-impl", default="auto", choices=["auto", "madmom", "native", "device"], help="DBN decoder [%(default)s]")
     add("--float16", default=True, action=argparse.BooleanOptionalAction,
         help="16-bit kernels, as the reference evaluates with precision='16-mixed' [on]")
-    add("--aggregation-type", default="mean-std", choices=["mean-std"],
-        help="summary over several models [%(default)s]")
+    add("--aggregation-type", default="mean-std", choices=["mean-std", "k-fold"],
+        help="summary over several models: mean and deviation of their summaries, or k-fold (each model on its own "
+             "split, per-piece metrics concatenated) [%(default)s]")
     add("--dump-predictions", metavar="FILENAME", default=None, help="write the predictions to this .npz file")
     add("--losses", action="store_true",
         help="also report the test losses of the checkpoint's loss_type (test_loss_beat, test_loss_downbeat, test_loss)")
@@ -397,21 +431,55 @@ def _print_mean_std(summaries: list) -> None:
         print(f"{k}: {round(float(np.mean(vals)), 3)} +- {round(float(np.std(vals)), 3)}")
 
 
+def _print_k_fold(result: EvalResult) -> None:
+    print("Dataset metrics")
+    for k, v in result.dataset_summary().items():
+        print(k)
+        for d, value in v.items():
+            print(f"{d}: {round(value, 3)}")
+        print("------")
+
+
+def concat_results(results: list) -> EvalResult:
+    """The k-fold aggregate of several results (compute_paper_metrics.py:127-137): pieces, per-piece metrics and
+    predictions concatenated in order; ValueError when a piece appears twice."""
+    pieces = [p for r in results for p in r.pieces]
+    names = [p.name for p in pieces]
+    if len(set(names)) != len(names):
+        raise ValueError("There are repeated pieces in the folds")
+    metrics = {k: np.concatenate([r.metrics[k] for r in results]) for k in results[0].metrics}
+    summary = {k: float(np.mean(metrics[k])) if pieces else float("nan") for k in results[0].summary}
+    return EvalResult(pieces, metrics, [p for r in results for p in r.predictions], summary)
+
+
 def run(models, data=None, audio=None, annotations=None, items=None, gpu=0, eval_trim_beats=None, dbn=None,
-        dbn_impl="auto", float16=True, aggregation_type="mean-std", dump_predictions=None, losses=False, fps=None) -> int:
+        dbn_impl="auto", float16=True, aggregation_type="mean-std", dump_predictions=None, losses=False, fps=None,
+        datasplit=None) -> int:
     from .inference import load_checkpoint
 
     if audio is not None and annotations is None:
         raise SystemExit("--audio needs --annotations")
-    if len(models) > 1 and dump_predictions:
+    if datasplit is not None and (data is None or items is not None):
+        raise SystemExit("--datasplit needs --data and excludes --items")
+    if aggregation_type not in ("mean-std", "k-fold"):
+        raise ValueError(f"Unknown aggregation type {aggregation_type}")
+    k_fold = len(models) > 1 and aggregation_type == "k-fold"
+    if len(models) > 1 and dump_predictions and not k_fold:
         print("cannot dump predictions when doing inference for multiple models")
         return 1
-    pieces = discover_data(data, items) if data is not None else discover_audio(audio, annotations)
-    summaries = []
-    for m in models:
+    pieces = None
+    if datasplit is None:
+        pieces = discover_data(data, items) if data is not None else discover_audio(audio, annotations)
+    summaries, results = [], []
+    for i, m in enumerate(models):
         if len(models) == 1:
             print("Single model prediction for", m)
+        elif k_fold:
+            print(f"Model {i + 1}/{len(models)}")
         ckpt = load_checkpoint(m, "cpu")
+        if datasplit is not None and (pieces is None or k_fold):
+            # k-fold: every checkpoint on its own split; otherwise the first checkpoint's split for all
+            pieces = split_pieces(data, datasplit, ckpt.get("datamodule_hyper_parameters", {}))
         hp = ckpt.get("hyper_parameters", {})
         trim = eval_trim_beats if eval_trim_beats is not None else float(hp.get("eval_trim_beats", 5))
         use_dbn = dbn if dbn is not None else bool(hp.get("use_dbn", False))
@@ -419,11 +487,17 @@ def run(models, data=None, audio=None, annotations=None, items=None, gpu=0, eval
         runner = make_runner(ckpt, f"cuda:{gpu}", float16, use_dbn, dbn_impl)
         result = evaluate(runner, pieces, min_beat_time=trim, losses=losses, fps=rate)
         summaries.append(result.summary)
+        results.append(result)
         if len(models) == 1:
             _print_single(result)
             if dump_predictions:
                 write_predictions(dump_predictions, result)
-    if len(models) > 1:
+    if k_fold:
+        result = concat_results(results)
+        _print_k_fold(result)
+        if dump_predictions:
+            write_predictions(dump_predictions, result)
+    elif len(models) > 1:
         _print_mean_std(summaries)
     return 0
 

@@ -492,6 +492,26 @@ int bt_istft(bt_ctx* ctx, const bt_stft_config* cfg, const float* window_dev, co
              const float* spec_dev, const int64_t* frame_offsets_host, int32_t n_seqs, float* audio_out_dev,
              const int64_t* out_sample_offsets_host, void* stream);
 
+/* ---- training batches: BeatTrackingDataset.__getitem__ + default_collate (dataset.py:169-241, augment.py:129-201) --
+ * Assembles n_items excerpts of `length` frames whose windows the caller has drawn and staged (ABI 2.11).  Item i owns
+ * rows [row_offsets_host[i], row_offsets_host[i+1]) of rows_dev (n_i of them, n_i <= length; a row is BT_N_MELS fp16
+ * values) and the same range of row_map_host: the window row each output row t < n_i copies, or -1 for a row a zero
+ * mask cleared (NULL: the identity map).  Beat and downbeat frames are CSR tables (beat_offsets_host[n_items + 1] into
+ * beat_frames_host, likewise for downbeats), each item's frames sorted, in [0, n_i), duplicates allowed.  Writes
+ *   out_spect_dev    [n_items, length, BT_N_MELS] fp16: the mapped row's bits (never converted), 0 for -1 rows and t >= n_i;
+ *   truth_beat_dev / truth_downbeat_dev [n_items, length] bytes: 1 where t is one of the item's frames, else 0;
+ *   padding_mask_dev [n_items, length] bytes: t < n_i.
+ * One launch: every output element is written once (a gather, a binary search per frame), so results are bitwise
+ * repeatable.  Works on a weight-less ctx; the tables travel through the ctx's staging ring.
+ * BT_ERR_ARG, before anything is enqueued, for n_items < 0, length < 1, a null pointer, offsets that do not start at 0
+ * or decrease, n_i > length, a map entry outside [-1, n_i), a frame outside [0, n_i), or an item's frames out of
+ * order. */
+int bt_train_batch(bt_ctx* ctx, const uint16_t* rows_dev, const int64_t* row_offsets_host, int32_t n_items,
+                   int32_t length, const int32_t* row_map_host, const int32_t* beat_frames_host,
+                   const int64_t* beat_offsets_host, const int32_t* downbeat_frames_host,
+                   const int64_t* downbeat_offsets_host, uint16_t* out_spect_dev, uint8_t* truth_beat_dev,
+                   uint8_t* truth_downbeat_dev, uint8_t* padding_mask_dev, void* stream);
+
 /* ---- introspection / tuning ----------------------------------------------------------------- */
 
 /* Upper bound on the chunks processed per wave (1..256, default 128; one wave = one launch of every kernel of the
