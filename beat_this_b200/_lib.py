@@ -11,6 +11,8 @@ import os
 import subprocess
 from ctypes import POINTER, c_char_p, c_double, c_float, c_int, c_int32, c_int64, c_void_p
 
+import numpy as np
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 # BT_LIB_PATH: an instrumented build of the same sources (e.g. build(extra_flags=("-DBT_FF_PROF",), out_path=...))
@@ -85,6 +87,7 @@ MAX_CHUNK_CAP = 256 * BT_CHUNK  # the longest maximum chunk bt_finalize accepts 
 BT_KEEP_FIRST = 0
 BT_KEEP_LAST = 1
 OVERLAP_MODES = {"keep_first": BT_KEEP_FIRST, "keep_last": BT_KEEP_LAST}
+DEFAULT_CHUNKING = (BT_CHUNK, 6, "keep_first")  # what Spect2Frames.spect2frames uses (reference inference.py:244-254)
 
 
 class bt_chunking(ctypes.Structure):
@@ -392,3 +395,99 @@ def check(lib, ctx, code: int):
 def i64_array(values):
     arr = (c_int64 * len(values))(*[int(v) for v in values])
     return arr
+
+
+def i32_array(values):
+    """An int32 host table as a C array argument: a pointer that keeps its contiguous copy alive.  It goes through
+    numpy because such tables can be long (a training batch's row maps have B * L entries)."""
+    return np.ascontiguousarray(values, dtype=np.int32).ctypes.data_as(POINTER(c_int32))
+
+
+def offsets(lengths) -> list:
+    """CSR offsets of consecutive lengths: [0, l0, l0 + l1, ...]."""
+    out = [0]
+    for n in lengths:
+        out.append(out[-1] + int(n))
+    return out
+
+
+# ---- entry points without a context --------------------------------------------------------------------------------
+SIG_F32, SIG_F64, SIG_I16 = 0, 1, 2
+SIGNAL_DTYPES = {np.dtype(np.float32): SIG_F32, np.dtype(np.float64): SIG_F64, np.dtype(np.int16): SIG_I16}
+
+
+def stage_audio(arrays, dst, threads: int) -> list:
+    """bt_stage_audio: mono mix + fp32 cast of C-contiguous ndarrays of SIGNAL_DTYPES (pipeline.as_signal_array) into
+    `dst` (host fp32 tensor) on `threads` host threads; returns the sample offsets."""
+    n = len(arrays)
+    so = offsets(a.shape[0] for a in arrays)
+    ptrs = (c_void_p * n)(*[a.ctypes.data for a in arrays])
+    dts = (c_int32 * n)(*[SIGNAL_DTYPES[a.dtype] for a in arrays])
+    frames = (c_int64 * n)(*[a.shape[0] for a in arrays])
+    chans = (c_int32 * n)(*[1 if a.ndim == 1 else a.shape[1] for a in arrays])
+    code = load().bt_stage_audio(ptrs, dts, frames, chans, n, c_void_p(dst.data_ptr()), i64_array(so), threads)
+    if code != 0:
+        raise BTError(f"bt_stage_audio failed ({code}): bad signal array")
+    return so
+
+
+def wav_probe(paths):
+    """bt_wav_probe on every path: (ctypes array of bt_wav_info, list of ok flags).  Files that are not plain WAV are
+    left to load_audio's backend chain."""
+    lib = load()
+    infos = (bt_wav_info * len(paths))()
+    ok = [lib.bt_wav_probe(str(p).encode(), ctypes.byref(infos[i])) == 0 and infos[i].frames > 0
+          for i, p in enumerate(paths)]
+    return infos, ok
+
+
+def stage_wav_files(paths, infos, dst, sample_offsets, threads: int):
+    """bt_stage_wav_files: file k (bt_wav_info infos[k] from wav_probe) read, mixed to mono and cast to fp32 into `dst`
+    (host fp32 tensor) from sample_offsets[k] on, on `threads` host threads.  RuntimeError names the files that
+    failed."""
+    n = len(paths)
+    cpaths = (c_char_p * n)(*[str(p).encode() for p in paths])
+    status = (c_int32 * n)()
+    code = load().bt_stage_wav_files(cpaths, (bt_wav_info * n)(*infos), n, c_void_p(dst.data_ptr()), i64_array(sample_offsets),
+                                     threads, status)
+    if code != 0:
+        bad = [str(paths[i]) for i in range(n) if status[i] != 0]
+        raise RuntimeError(f"Could not load audio from {bad}")
+
+
+def dbn_viterbi(log_densities, beats: int, intervals, log_tempo, pointers):
+    """bt_dbn_viterbi (host C++) of one bar model on float64 log densities [T, 3]: (state path, log-probability)."""
+    dens = np.ascontiguousarray(log_densities, dtype=np.float64)
+    T = len(dens)
+    path = np.empty(T, dtype=np.int64)
+    logp = c_double()
+    iv = np.ascontiguousarray(intervals, dtype=np.int32)
+    lt = np.ascontiguousarray(log_tempo, dtype=np.float64)
+    pt = np.ascontiguousarray(pointers, dtype=np.int32)
+    code = load().bt_dbn_viterbi(dens.ctypes.data, T, int(beats), len(iv), iv.ctypes.data, lt.ctypes.data, pt.ctypes.data,
+                                 path.ctypes.data, ctypes.byref(logp))
+    if code != 0:
+        raise RuntimeError(f"bt_dbn_viterbi failed ({code})")
+    return path, float(logp.value)
+
+
+def dbn_track(activations, frame_offsets, params: dict, n_threads: int = 0):
+    """bt_dbn_track (host C++, one thread per piece) on [total_frames, 2] float64 activations for the tracker
+    parameters `params` (dbn.DBNDownBeatTracker.track_params): (times, beat numbers, counts); piece i has counts[i]
+    pairs from frame_offsets[i] on."""
+    fo = np.ascontiguousarray(frame_offsets, dtype=np.int64)
+    n = len(fo) - 1
+    cat = np.ascontiguousarray(activations, dtype=np.float64).reshape(-1, 2)
+    total = max(int(fo[-1]), 1)
+    times = np.empty(total, dtype=np.float64)
+    numbers = np.empty(total, dtype=np.int32)
+    counts = np.zeros(max(n, 1), dtype=np.int64)
+    bpb = np.asarray(params["beats_per_bar"], dtype=np.int32)
+    p = params
+    code = load().bt_dbn_track(cat.ctypes.data, fo.ctypes.data, n, bpb.ctypes.data, len(bpb), p["min_bpm"], p["max_bpm"],
+                               p["num_tempi"], p["transition_lambda"], p["observation_lambda"], p["threshold"],
+                               int(p["correct"]), p["fps"], int(n_threads), times.ctypes.data, numbers.ctypes.data,
+                               counts.ctypes.data)
+    if code != 0:
+        raise RuntimeError(f"bt_dbn_track failed ({code})")
+    return times, numbers, counts

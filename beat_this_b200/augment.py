@@ -180,9 +180,7 @@ class Augmenter:
 
     def _group(self, sigs, variants, out):
         eng, nv = self.engine, len(variants)
-        so = [0]
-        for s in sigs:
-            so.append(so[-1] + s.numel())
+        so = _lib.offsets(s.numel() for s in sigs)
         spec, fo = eng.stft_cat(torch.cat(sigs) if len(sigs) > 1 else sigs[0], so, self.tables)
         # clip-major: the variants of a clip run together and share its analysis
         v_clip = [c for c in range(len(sigs)) for _ in variants]
@@ -198,9 +196,7 @@ class Augmenter:
                 for c, p in enumerate(parts):
                     out[c][name] = p
                 continue
-            po = [0]
-            for p in parts:
-                po.append(po[-1] + p.numel())
+            po = _lib.offsets(p.numel() for p in parts)
             res, ro = eng.resample_cat(torch.cat(parts) if len(parts) > 1 else parts[0].contiguous(), po, sr_from, self.sr)
             for c in range(len(sigs)):
                 n, y = sigs[c].numel(), res[ro[c] : ro[c + 1]]

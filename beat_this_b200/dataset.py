@@ -16,13 +16,11 @@ given): with ``np.random.seed(s)`` and the same index sequence, the batches equa
 """
 from __future__ import annotations
 
-import ctypes
 import io
 import json
 import re
 import zipfile
 from concurrent.futures import ThreadPoolExecutor
-from ctypes import c_void_p
 from dataclasses import dataclass
 from pathlib import Path
 
@@ -31,6 +29,7 @@ import torch
 
 from . import _lib
 from .augment import precomputed_augmentation_filenames, shift_filename, stretch_annotations, stretch_filename
+from .engine import Engine
 
 N_BINS = 128
 AUGMENTATIONS = ("mask", "pitch", "tempo")
@@ -347,14 +346,7 @@ class BeatTrackingDataset:
 
 
 # ---- batches ---------------------------------------------------------------------------------------------------------
-def _engine(device):
-    from .evaluate import _engine
-
-    return _engine(device)
-
-
-def _ptr(t):
-    return c_void_p(t.data_ptr())
+train_batch = Engine.train_batch  # train_batch(engine, rows, ...), the name earlier versions offered
 
 
 @dataclass
@@ -363,7 +355,7 @@ class _Staged:
     are being copied into by `copies`."""
     excerpts: list
     length: int
-    rows: np.ndarray
+    rows: list
     slot: int
     copies: list
 
@@ -394,7 +386,7 @@ class TrainingBatches:
             raise ValueError("a dataset of full pieces (train_length=None) needs batch_size=1")
         self.dataset, self.batch_size, self.shuffle, self.drop_last = dataset, batch_size, shuffle, drop_last
         self.rng = rng
-        self.engine = _engine(device)
+        self.engine = Engine.shared(device)
         self.device = self.engine.device
         if seed is None:
             seed = int(torch.empty((), dtype=torch.int64).random_().item())
@@ -433,17 +425,16 @@ class TrainingBatches:
     def _stage(self, indices) -> _Staged:
         ex = [self.dataset.draw(int(i), self.rng) for i in indices]
         length = self.dataset.train_length if self.dataset.train_length is not None else ex[0].n
-        rows = np.zeros(len(ex) + 1, np.int64)
-        rows[1:] = np.cumsum([e.n for e in ex])
+        rows = _lib.offsets(e.n for e in ex)
         slot = self._next
         self._next ^= 1
         if self._uploaded[slot] is not None:
             self._uploaded[slot].synchronize()  # the pinned buffer's previous upload has left it
-        need = max(int(rows[-1]), 1) * N_BINS
+        need = max(rows[-1], 1) * N_BINS
         if self._host[slot] is None or self._host[slot].numel() < need:
             self._host[slot] = torch.empty(need, dtype=torch.int16, pin_memory=True)
         host = self._host[slot].numpy().view(np.uint16)
-        copies = [self._pool.submit(self._copy_window, host, int(a), e) for a, e in zip(rows[:-1], ex)]
+        copies = [self._pool.submit(self._copy_window, host, a, e) for a, e in zip(rows[:-1], ex)]
         return _Staged(ex, length, rows, slot, copies)
 
     @staticmethod
@@ -456,7 +447,7 @@ class TrainingBatches:
             f.result()
         ex, rows, slot, L = s.excerpts, s.rows, s.slot, s.length
         B = len(ex)
-        total = int(rows[-1])
+        total = rows[-1]
         compute = torch.cuda.current_stream(self.device)
         need = max(total, 1) * N_BINS
         if self._dev[slot] is None or self._dev[slot].numel() < need:
@@ -473,13 +464,13 @@ class TrainingBatches:
         maps = None
         if any(e.row_map is not None for e in ex):
             maps = np.concatenate([e.row_map if e.row_map is not None else np.arange(e.n, dtype=np.int32) for e in ex])
-        beat_off = np.concatenate(([0], np.cumsum([len(e.beat_frames) for e in ex]))).astype(np.int64)
-        down_off = np.concatenate(([0], np.cumsum([len(e.downbeat_frames) for e in ex]))).astype(np.int64)
+        beat_off = _lib.offsets(len(e.beat_frames) for e in ex)
+        down_off = _lib.offsets(len(e.downbeat_frames) for e in ex)
         beats = np.concatenate([e.beat_frames for e in ex] + [np.zeros(1, np.int32)])
         downs = np.concatenate([e.downbeat_frames for e in ex] + [np.zeros(1, np.int32)])
         spect = torch.empty((B, L, N_BINS), dtype=torch.float16, device=self.device)
         tb, td, pm = (torch.empty((B, L), dtype=torch.bool, device=self.device) for _ in range(3))
-        train_batch(self.engine, dev, rows, L, maps, beats, beat_off, downs, down_off, spect, tb, td, pm)
+        self.engine.train_batch(dev, rows, L, maps, beats, beat_off, downs, down_off, spect, tb, td, pm)
         self._consumed[slot] = torch.cuda.Event()
         self._consumed[slot].record(compute)
         return {
@@ -494,27 +485,3 @@ class TrainingBatches:
             "truth_orig_beat": [e.truth_orig_beat for e in ex],
             "truth_orig_downbeat": [e.truth_orig_downbeat for e in ex],
         }
-
-
-def _i32(a):
-    a = np.ascontiguousarray(a, dtype=np.int32)
-    return a, a.ctypes.data_as(ctypes.POINTER(ctypes.c_int32))
-
-
-def _i64(a):
-    a = np.ascontiguousarray(a, dtype=np.int64)
-    return a, a.ctypes.data_as(ctypes.POINTER(ctypes.c_int64))
-
-
-def train_batch(engine, rows, row_offsets, length, row_map, beat_frames, beat_offsets, downbeat_frames,
-                downbeat_offsets, spect, truth_beat, truth_downbeat, padding_mask):
-    """One ``bt_train_batch`` launch on the current stream (contract in include/beatthis.h): rows, spect and the three
-    [B, L] outputs are device tensors (rows and spect of 16-bit elements, the others of bytes); the tables are host
-    arrays, row_map None for identity maps."""
-    n = len(row_offsets) - 1
-    keep = [_i64(row_offsets), _i64(beat_offsets), _i64(downbeat_offsets), _i32(beat_frames), _i32(downbeat_frames)]
-    m = _i32(row_map) if row_map is not None else (None, None)
-    code = engine.lib.bt_train_batch(engine.ctx, _ptr(rows), keep[0][1], n, int(length), m[1], keep[3][1], keep[1][1],
-                                     keep[4][1], keep[2][1], _ptr(spect), _ptr(truth_beat), _ptr(truth_downbeat),
-                                     _ptr(padding_mask), engine._stream())
-    _lib.check(engine.lib, engine.ctx, code)

@@ -19,18 +19,17 @@ from __future__ import annotations
 
 import numpy as np
 
+from . import _lib
 
 _LIB = False
 
 
 def _native():
-    """The shared library if it is built (the decoder itself needs no GPU)."""
+    """The shared library if it is built (the decoder itself needs no GPU): whether to use it or the numpy twins."""
     global _LIB
     if _LIB is False:
         try:
-            from . import _lib
-
-            _LIB = _lib.load() if hasattr(_lib, "load") else None
+            _LIB = _lib.load()
         except Exception:
             _LIB = None
     return _LIB
@@ -87,23 +86,9 @@ class _BarModel:
         """Most probable state path and its log-probability (uniform initial distribution): the C++ decoder of the
         shared library (bt_dbn_viterbi, csrc/dbn_host.cpp -- madmom's is Cython), or `viterbi_numpy` when the
         library has not been built (both are host code and are tested against each other)."""
-        lib = _native()
-        if lib is None:
+        if _native() is None:
             return self.viterbi_numpy(act)
-        import ctypes
-
-        dens = np.ascontiguousarray(self.log_densities(act))
-        T = len(act)
-        path = np.empty(T, dtype=np.int64)
-        logp = ctypes.c_double()
-        iv = np.ascontiguousarray(self.intervals, dtype=np.int32)
-        lt = np.ascontiguousarray(self.log_tempo, dtype=np.float64)
-        pt = np.ascontiguousarray(self.pointers, dtype=np.int32)
-        code = lib.bt_dbn_viterbi(dens.ctypes.data, T, self.beats, len(iv), iv.ctypes.data, lt.ctypes.data, pt.ctypes.data,
-                                  path.ctypes.data, ctypes.byref(logp))
-        if code != 0:
-            raise RuntimeError(f"bt_dbn_viterbi failed ({code})")
-        return path, float(logp.value)
+        return _lib.dbn_viterbi(self.log_densities(act), self.beats, self.intervals, self.log_tempo, self.pointers)
 
     def viterbi_numpy(self, act):
         T, S = len(act), self.num_states
@@ -167,32 +152,17 @@ class DBNDownBeatTracker:
         if _native() is None:
             return [self.track_numpy(a) for a in activations_list]
         acts = [np.ascontiguousarray(a, dtype=np.float64).reshape(-1, 2) for a in activations_list]
-        fo = np.zeros(len(acts) + 1, dtype=np.int64)
-        for i, a in enumerate(acts):
-            fo[i + 1] = fo[i] + len(a)
+        fo = _lib.offsets(len(a) for a in acts)
         cat = np.concatenate(acts) if acts else np.zeros((0, 2))
         return self.batch_cat(cat, fo, n_threads)
 
     def batch_cat(self, activations: np.ndarray, frame_offsets, n_threads: int = 0):
         """Same, for pieces that already sit back to back in one [total_frames, 2] float64 array."""
-        lib = _native()
         fo = np.ascontiguousarray(frame_offsets, dtype=np.int64)
         n = len(fo) - 1
-        if lib is None:
+        if _native() is None:
             return [self.track_numpy(activations[fo[i] : fo[i + 1]]) for i in range(n)]
-        cat = np.ascontiguousarray(activations, dtype=np.float64).reshape(-1, 2)
-        total = max(int(fo[-1]), 1)
-        times = np.empty(total, dtype=np.float64)
-        numbers = np.empty(total, dtype=np.int32)
-        counts = np.zeros(max(n, 1), dtype=np.int64)
-        bpb = np.asarray(self.params["beats_per_bar"], dtype=np.int32)
-        p = self.track_params
-        code = lib.bt_dbn_track(cat.ctypes.data, fo.ctypes.data, n, bpb.ctypes.data, len(bpb), p["min_bpm"], p["max_bpm"],
-                                p["num_tempi"], p["transition_lambda"], p["observation_lambda"], p["threshold"],
-                                int(p["correct"]), p["fps"], int(n_threads), times.ctypes.data, numbers.ctypes.data,
-                                counts.ctypes.data)
-        if code != 0:
-            raise RuntimeError(f"bt_dbn_track failed ({code})")
+        times, numbers, counts = _lib.dbn_track(activations, fo, self.track_params, n_threads)
         out = []
         for i in range(n):
             a, k = int(fo[i]), int(counts[i])

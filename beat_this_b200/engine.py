@@ -10,7 +10,9 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import BT_DTYPE_H16, BT_DTYPE_F32, bt_hparams, i64_array
+from ._lib import BT_DTYPE_H16, BT_DTYPE_F32, DEFAULT_CHUNKING, bt_hparams, i32_array, i64_array
+
+_SHARED = {}  # device -> the weight-less Engine of Engine.shared
 
 
 def _cuda_device(device) -> torch.device:
@@ -121,15 +123,22 @@ class Engine:
             eng._set_param(k, v)
         return eng
 
+    @classmethod
+    def shared(cls, device="cuda"):
+        """The weight-less engine of `device` that the beat metrics, the losses and the training batches share."""
+        dev = _cuda_device(device)
+        if dev not in _SHARED:
+            _SHARED[dev] = cls.mel_only(dev)
+        return _SHARED[dev]
+
     def _set_param(self, name: str, arr: np.ndarray):
         arr = np.ascontiguousarray(arr, dtype=np.float32).reshape(-1)
-        code = self.lib.bt_set_param(self.ctx, name.encode(), arr.ctypes.data_as(ctypes.POINTER(ctypes.c_float)), arr.size)
-        _lib.check(self.lib, self.ctx, code)
+        self._call("bt_set_param", name.encode(), arr.ctypes.data_as(ctypes.POINTER(ctypes.c_float)), arr.size, stream=False)
 
     def set_params(self, packed: dict):
         for k, v in packed.items():
             self._set_param(k, v)
-        _lib.check(self.lib, self.ctx, self.lib.bt_finalize(self.ctx))
+        self._call("bt_finalize", stream=False)
         self._model_ready = True
 
     @property
@@ -138,7 +147,7 @@ class Engine:
         return int(self.lib.bt_max_chunk(self.ctx))
 
     def set_wave_chunks(self, n: int):
-        _lib.check(self.lib, self.ctx, self.lib.bt_set_wave_chunks(self.ctx, int(n)))
+        self._call("bt_set_wave_chunks", int(n), stream=False)
 
     def close(self):
         if getattr(self, "ctx", None) is not None and self.ctx.value:
@@ -158,179 +167,149 @@ class Engine:
     def _stream(self):
         return c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
 
+    def _call(self, name: str, *args, stream: bool = True):
+        """The context entry point `name` on (ctx, *args), followed by the current stream of this device for the entry
+        points that enqueue work; a non-zero code raises BTError."""
+        _lib.check(self.lib, self.ctx, getattr(self.lib, name)(self.ctx, *args, *((self._stream(),) if stream else ())))
+
+    # The C library cannot see buffer sizes or types, so each tensor is checked here to be a contiguous device tensor
+    # of the dtype the entry point reads (one of them, for a tuple) holding at least the n elements it touches.
+    @staticmethod
+    def _dev_ptr(t, n: int = 0, dtype=torch.float32):
+        if t is None:
+            return None
+        assert t.is_cuda and t.is_contiguous() and t.dtype in (dtype if isinstance(dtype, tuple) else (dtype,)), \
+            f"expected a contiguous CUDA tensor of {dtype}, got {t.dtype} on {t.device}"
+        assert t.numel() >= n, f"tensor of {t.numel()} elements, the hook reads or writes {n}"
+        return c_void_p(t.data_ptr())
+
     # ---- hot path ---------------------------------------------------------------------------
     @staticmethod
     def frame_offsets(sample_offsets, hop: int = 441):
-        fo = [0]
-        for a, b in zip(sample_offsets[:-1], sample_offsets[1:]):
-            fo.append(fo[-1] + 1 + (int(b) - int(a)) // hop)
-        return fo
+        return _lib.offsets(1 + (int(b) - int(a)) // hop for a, b in zip(sample_offsets[:-1], sample_offsets[1:]))
 
     def resample_cat(self, audio: torch.Tensor, sample_offsets, sr: int, sr_out: int = 22050):
         """Concatenated fp32 device audio at `sr` Hz -> (audio at `sr_out` Hz, new sample offsets): the device
         stand-in for soxr.resample (reference inference.py:274-275), see preprocessing.resample_filter_bank."""
         from . import preprocessing as P
 
-        assert audio.is_cuda and audio.dtype == torch.float32 and audio.is_contiguous()
         key = (int(sr), int(sr_out))
         if key not in self._resample_banks:
             coef, L, M, K = P.resample_filter_bank(*key)
             self._resample_banks[key] = (torch.from_numpy(coef).to(self.device).contiguous(), L, M, K)
         coef, L, M, K = self._resample_banks[key]
         so = [int(v) for v in sample_offsets]
-        oo = [0]
-        for i in range(len(so) - 1):
-            oo.append(oo[-1] + P.resampled_length(so[i + 1] - so[i], L, M))
+        oo = _lib.offsets(P.resampled_length(so[i + 1] - so[i], L, M) for i in range(len(so) - 1))
         out = torch.empty(max(oo[-1], 1), dtype=torch.float32, device=self.device)[: oo[-1]]
-        code = self.lib.bt_resample(self.ctx, c_void_p(audio.data_ptr()), i64_array(so), len(so) - 1, c_void_p(coef.data_ptr()),
-                                    L, M, K, c_void_p(out.data_ptr()), i64_array(oo), self._stream())
-        _lib.check(self.lib, self.ctx, code)
+        p = self._dev_ptr
+        self._call("bt_resample", p(audio), i64_array(so), len(so) - 1, p(coef), L, M, K, p(out), i64_array(oo))
         return out, oo
 
     def logmel_cat(self, audio: torch.Tensor, sample_offsets):
         """audio: flat fp32 device tensor; returns (spect [total_frames,128], frame_offsets)."""
-        assert audio.is_cuda and audio.dtype == torch.float32 and audio.is_contiguous()
         fo = self.frame_offsets(sample_offsets)
         spect = torch.empty((fo[-1], 128), dtype=torch.float32, device=self.device)
-        code = self.lib.bt_logmel(self.ctx, c_void_p(audio.data_ptr()), i64_array(sample_offsets), len(sample_offsets) - 1,
-                                  c_void_p(spect.data_ptr()), i64_array(fo), self._stream())
-        _lib.check(self.lib, self.ctx, code)
+        self._call("bt_logmel", self._dev_ptr(audio), i64_array(sample_offsets), len(sample_offsets) - 1,
+                   self._dev_ptr(spect), i64_array(fo))
         return spect, fo
 
-    def logmel(self, signals):
+    def _per_clip(self, signals, cat):
+        """cat(flat fp32 device audio, sample offsets) -> (spect, frame offsets) for the clips `signals`: per clip spect."""
         sigs = [torch.as_tensor(s, dtype=torch.float32, device=self.device).contiguous() for s in signals]
-        so = [0]
-        for s in sigs:
-            so.append(so[-1] + s.numel())
-        spect, fo = self.logmel_cat(torch.cat(sigs) if len(sigs) > 1 else sigs[0], so)
+        spect, fo = cat(torch.cat(sigs) if len(sigs) > 1 else sigs[0], _lib.offsets(s.numel() for s in sigs))
         return [spect[fo[i] : fo[i + 1]] for i in range(len(sigs))]
+
+    def logmel(self, signals):
+        return self._per_clip(signals, self.logmel_cat)
 
     def logmel_config_cat(self, audio: torch.Tensor, sample_offsets, tables, device_tables: dict):
         """bt_logmel_config on flat fp32 device audio for the analysis of ``tables`` (preprocessing.MelTables, whose
         ``to(device)`` gave ``device_tables``): (spect [total_frames, n_mels], frame_offsets)."""
-        assert audio.is_cuda and audio.dtype == torch.float32 and audio.is_contiguous()
         fo = self.frame_offsets(sample_offsets, tables.hop_length)
         spect = torch.empty((fo[-1], tables.n_mels), dtype=torch.float32, device=self.device)
-        t = device_tables
-        code = self.lib.bt_logmel_config(
-            self.ctx, ctypes.byref(tables.config), c_void_p(t["window"].data_ptr()), c_void_p(t["twiddle"].data_ptr()),
-            c_void_p(t["fb_start"].data_ptr()), c_void_p(t["fb_ptr"].data_ptr()), c_void_p(t["fb_w"].data_ptr()),
-            c_void_p(audio.data_ptr()), i64_array(sample_offsets), len(sample_offsets) - 1, c_void_p(spect.data_ptr()),
-            i64_array(fo), self._stream())
-        _lib.check(self.lib, self.ctx, code)
+        t, p = device_tables, self._dev_ptr
+        self._call("bt_logmel_config", ctypes.byref(tables.config), p(t["window"]), p(t["twiddle"]),
+                   p(t["fb_start"], dtype=torch.int32), p(t["fb_ptr"], dtype=torch.int32), p(t["fb_w"]), p(audio),
+                   i64_array(sample_offsets), len(sample_offsets) - 1, p(spect), i64_array(fo))
         return spect, fo
 
     def logmel_config(self, signals, tables, device_tables: dict):
-        sigs = [torch.as_tensor(s, dtype=torch.float32, device=self.device).contiguous() for s in signals]
-        so = [0]
-        for s in sigs:
-            so.append(so[-1] + s.numel())
-        spect, fo = self.logmel_config_cat(torch.cat(sigs) if len(sigs) > 1 else sigs[0], so, tables, device_tables)
-        return [spect[fo[i] : fo[i + 1]] for i in range(len(sigs))]
+        return self._per_clip(signals, lambda audio, so: self.logmel_config_cat(audio, so, tables, device_tables))
 
     # ---- tempo / pitch augmentation (augment.py; contracts in include/beatthis.h) -------------
     def stft_cat(self, audio: torch.Tensor, sample_offsets, tables):
         """bt_stft on flat fp32 device audio for the analysis of ``tables`` (augment.StftTables on this device):
         (complex64 spectrogram [total_frames, n_fft / 2 + 1], frame_offsets)."""
-        assert audio.is_cuda and audio.dtype == torch.float32 and audio.is_contiguous()
         fo = self.frame_offsets(sample_offsets, tables.hop_length)
         spec = torch.empty((fo[-1], tables.bins), dtype=torch.complex64, device=self.device)
-        code = self.lib.bt_stft(self.ctx, ctypes.byref(tables.config), c_void_p(tables.window.data_ptr()),
-                                c_void_p(tables.twiddle.data_ptr()), c_void_p(audio.data_ptr()), i64_array(sample_offsets),
-                                len(sample_offsets) - 1, c_void_p(spec.data_ptr()), i64_array(fo), self._stream())
-        _lib.check(self.lib, self.ctx, code)
+        p = self._dev_ptr
+        self._call("bt_stft", ctypes.byref(tables.config), p(tables.window), p(tables.twiddle), p(audio),
+                   i64_array(sample_offsets), len(sample_offsets) - 1, p(spec, dtype=torch.complex64), i64_array(fo))
         return spec, fo
 
     def phase_vocoder_cat(self, spec: torch.Tensor, frame_offsets, variant_clip, variant_rate):
         """bt_phase_vocoder: variant v is clip variant_clip[v] of ``spec`` (complex64 [total_frames, bins]) at rate
         variant_rate[v].  Returns (complex64 [total_out_frames, bins], out_frame_offsets)."""
-        assert spec.is_cuda and spec.dtype == torch.complex64 and spec.is_contiguous() and spec.ndim == 2
+        assert spec.ndim == 2
         n_clips, nv = len(frame_offsets) - 1, len(variant_clip)
-        oo = [0]
-        for clip, rate in zip(variant_clip, variant_rate):
+
+        def frames(clip, rate):
             T = int(frame_offsets[clip + 1]) - int(frame_offsets[clip]) if 0 <= clip < n_clips else 0
-            oo.append(oo[-1] + (math.ceil(T / rate) if rate > 0 and math.isfinite(rate) else 0))
+            return math.ceil(T / rate) if rate > 0 and math.isfinite(rate) else 0
+
+        oo = _lib.offsets(frames(clip, rate) for clip, rate in zip(variant_clip, variant_rate))
         out = torch.empty((oo[-1], spec.shape[1]), dtype=torch.complex64, device=self.device)
-        code = self.lib.bt_phase_vocoder(
-            self.ctx, 2 * (spec.shape[1] - 1), c_void_p(spec.data_ptr()), i64_array(frame_offsets), n_clips,
-            (ctypes.c_int32 * max(nv, 1))(*[int(v) for v in variant_clip]),
-            (ctypes.c_double * max(nv, 1))(*[float(r) for r in variant_rate]), nv, c_void_p(out.data_ptr()), i64_array(oo),
-            self._stream())
-        _lib.check(self.lib, self.ctx, code)
+        p = self._dev_ptr
+        self._call("bt_phase_vocoder", 2 * (spec.shape[1] - 1), p(spec, dtype=torch.complex64), i64_array(frame_offsets),
+                   n_clips, (ctypes.c_int32 * max(nv, 1))(*[int(v) for v in variant_clip]),
+                   (ctypes.c_double * max(nv, 1))(*[float(r) for r in variant_rate]), nv, p(out, dtype=torch.complex64),
+                   i64_array(oo))
         return out, oo
 
     def istft_cat(self, spec: torch.Tensor, frame_offsets, lengths, tables):
         """bt_istft: sequence s (frames frame_offsets[s]..) -> lengths[s] samples.  Returns (flat fp32 audio, sample
         offsets)."""
-        assert spec.is_cuda and spec.dtype == torch.complex64 and spec.is_contiguous()
-        so = [0]
-        for n in lengths:
-            so.append(so[-1] + int(n))
+        so = _lib.offsets(lengths)
         out = torch.empty(max(so[-1], 1), dtype=torch.float32, device=self.device)[: so[-1]]
-        code = self.lib.bt_istft(self.ctx, ctypes.byref(tables.config), c_void_p(tables.window.data_ptr()),
-                                 c_void_p(tables.twiddle.data_ptr()), c_void_p(spec.data_ptr()), i64_array(frame_offsets),
-                                 len(frame_offsets) - 1, c_void_p(out.data_ptr()), i64_array(so), self._stream())
-        _lib.check(self.lib, self.ctx, code)
+        p = self._dev_ptr
+        self._call("bt_istft", ctypes.byref(tables.config), p(tables.window), p(tables.twiddle),
+                   p(spec, dtype=torch.complex64), i64_array(frame_offsets), len(frame_offsets) - 1, p(out), i64_array(so))
         return out, so
 
-    def spect2frames_cat(self, spect: torch.Tensor, frame_offsets, chunking: tuple | None = None):
+    def spect2frames_cat(self, spect: torch.Tensor, frame_offsets, chunking: tuple | None = DEFAULT_CHUNKING):
         """Concatenated [total, 128] spectrograms -> (beat, downbeat) logits.  chunking: (chunk_size, border_size,
-        overlap_mode) of split_predict_aggregate, checked by chunking_struct against max_chunk; None is 1500 / 6 /
-        keep_first."""
+        overlap_mode) of split_predict_aggregate, checked by chunking_struct against max_chunk; None, which earlier
+        versions took for the default, is DEFAULT_CHUNKING."""
         assert self._model_ready, "model parameters not loaded"
-        assert spect.is_cuda and spect.dtype == torch.float32 and spect.is_contiguous()
-        ck = None if chunking is None else chunking_struct(*chunking, self.max_chunk)
+        ck = chunking_struct(*(chunking or DEFAULT_CHUNKING), self.max_chunk)
         total = int(frame_offsets[-1])
         beat = torch.empty(total, dtype=torch.float32, device=self.device)
         down = torch.empty(total, dtype=torch.float32, device=self.device)
-        args = (self.ctx, c_void_p(spect.data_ptr()), i64_array(frame_offsets), len(frame_offsets) - 1,
-                c_void_p(beat.data_ptr()), c_void_p(down.data_ptr()))
-        if ck is None:
-            code = self.lib.bt_spect2frames(*args, self._stream())
-        else:
-            code = self.lib.bt_spect2frames_chunked(*args, ctypes.byref(ck), self._stream())
-        _lib.check(self.lib, self.ctx, code)
+        p = self._dev_ptr
+        self._call("bt_spect2frames_chunked", p(spect), i64_array(frame_offsets), len(frame_offsets) - 1, p(beat), p(down),
+                   ctypes.byref(ck))
         return beat, down
 
     def forward_chunks(self, chunks: torch.Tensor):
         """BeatThis.forward on [B, T<=max_chunk, 128] chunks (no chunk planning, no borders cut): flat (beat, downbeat)."""
         assert self._model_ready, "model parameters not loaded"
-        assert chunks.is_cuda and chunks.dtype == torch.float32 and chunks.is_contiguous() and chunks.ndim == 3
+        assert chunks.ndim == 3
         B, T, _ = chunks.shape
         beat = torch.empty(B * T, dtype=torch.float32, device=self.device)
         down = torch.empty(B * T, dtype=torch.float32, device=self.device)
-        code = self.lib.bt_forward_chunks(self.ctx, c_void_p(chunks.data_ptr()), B, T, c_void_p(beat.data_ptr()),
-                                          c_void_p(down.data_ptr()), self._stream())
-        _lib.check(self.lib, self.ctx, code)
+        self._call("bt_forward_chunks", self._dev_ptr(chunks), B, T, self._dev_ptr(beat), self._dev_ptr(down))
         return beat, down
 
-    def tap_chunks(self, name: str, chunks: torch.Tensor, capacity: int):
-        """Test hook: activation `name` of a forward_chunks call (single wave)."""
-        buf = torch.zeros(capacity, dtype=torch.float32, device=self.device)
-        _lib.check(self.lib, self.ctx, self.lib.bt_debug_request_tap(self.ctx, name.encode(), c_void_p(buf.data_ptr()), capacity))
-        try:
-            out = self.forward_chunks(chunks)
-            torch.cuda.synchronize(self.device)
-            n = int(self.lib.bt_debug_tap_count(self.ctx))
-        finally:
-            self.lib.bt_debug_request_tap(self.ctx, b"", None, 0)
-        return buf[:n], out
-
-    def audio2frames_cat(self, audio: torch.Tensor, sample_offsets, chunking: tuple | None = None):
+    def audio2frames_cat(self, audio: torch.Tensor, sample_offsets, chunking: tuple | None = DEFAULT_CHUNKING):
         """Concatenated mono 22.05 kHz audio -> (beat, downbeat, frame offsets); chunking as in spect2frames_cat."""
         assert self._model_ready, "model parameters not loaded"
-        assert audio.is_cuda and audio.dtype == torch.float32 and audio.is_contiguous()
-        ck = None if chunking is None else chunking_struct(*chunking, self.max_chunk)
+        ck = chunking_struct(*(chunking or DEFAULT_CHUNKING), self.max_chunk)
         fo = self.frame_offsets(sample_offsets)
         beat = torch.empty(fo[-1], dtype=torch.float32, device=self.device)
         down = torch.empty(fo[-1], dtype=torch.float32, device=self.device)
-        args = (self.ctx, c_void_p(audio.data_ptr()), i64_array(sample_offsets), len(sample_offsets) - 1,
-                c_void_p(beat.data_ptr()), c_void_p(down.data_ptr()), i64_array(fo))
-        if ck is None:
-            code = self.lib.bt_audio2frames(*args, self._stream())
-        else:
-            code = self.lib.bt_audio2frames_chunked(*args, ctypes.byref(ck), self._stream())
-        _lib.check(self.lib, self.ctx, code)
+        p = self._dev_ptr
+        self._call("bt_audio2frames_chunked", p(audio), i64_array(sample_offsets), len(sample_offsets) - 1, p(beat),
+                   p(down), i64_array(fo), ctypes.byref(ck))
         return beat, down, fo
 
     def peakpick_cat(self, beat: torch.Tensor, down: torch.Tensor, frame_offsets, fps: float = 50):
@@ -343,10 +322,7 @@ class Engine:
         bt_t = torch.empty((n, max_peaks), dtype=torch.float64, device=self.device)
         dn_t = torch.empty((n, max_peaks), dtype=torch.float64, device=self.device)
         cnt = torch.zeros((2, n), dtype=torch.int32, device=self.device)
-        code = self.lib.bt_peakpick_fps(self.ctx, c_void_p(beat.data_ptr()), c_void_p(down.data_ptr()), i64_array(frame_offsets),
-                                        n, float(fps), c_void_p(bt_t.data_ptr()), c_void_p(cnt[0].data_ptr()),
-                                        c_void_p(dn_t.data_ptr()), c_void_p(cnt[1].data_ptr()), max_peaks, self._stream())
-        _lib.check(self.lib, self.ctx, code)
+        self._peakpick(beat, down, frame_offsets, fps, bt_t, cnt[0], dn_t, cnt[1], max_peaks)
         cnt_h = cnt.cpu().numpy()
         width = int(cnt_h.max()) if cnt_h.size else 0
         if width > max_peaks:
@@ -372,25 +348,27 @@ class Engine:
             slot["cnt_h"] = torch.empty((2, n), dtype=torch.int32).pin_memory()
             slot["event"] = torch.cuda.Event()
         t, cnt = slot["times"], slot["cnt"]
-        code = self.lib.bt_peakpick_fps(self.ctx, c_void_p(beat.data_ptr()), c_void_p(down.data_ptr()), i64_array(frame_offsets),
-                                        n, float(fps), c_void_p(t[0].data_ptr()), c_void_p(cnt[0].data_ptr()),
-                                        c_void_p(t[1].data_ptr()), c_void_p(cnt[1].data_ptr()), max_peaks, self._stream())
-        _lib.check(self.lib, self.ctx, code)
+        self._peakpick(beat, down, frame_offsets, fps, t[0], cnt[0], t[1], cnt[1], max_peaks)
         slot["times_h"].copy_(t, non_blocking=True)
         slot["cnt_h"].copy_(cnt, non_blocking=True)
         slot["event"].record(torch.cuda.current_stream(self.device))
         slot["keep"] = (beat, down)  # keep the logits alive until the kernels have run
         return _PeakHandle(slot, n)
 
+    def _peakpick(self, beat, down, frame_offsets, fps, beat_times, beat_counts, down_times, down_counts, max_peaks):
+        p = self._dev_ptr
+        self._call("bt_peakpick_fps", p(beat), p(down), i64_array(frame_offsets), len(frame_offsets) - 1, float(fps),
+                   p(beat_times, dtype=torch.float64), p(beat_counts, dtype=torch.int32), p(down_times, dtype=torch.float64),
+                   p(down_counts, dtype=torch.int32), max_peaks)
+
     def _dbn_enqueue(self, beat, down, act, frame_offsets, params: dict, times, numbers, counts):
         bpb = np.ascontiguousarray(params["beats_per_bar"], dtype=np.int32)
-        ptr = lambda t: None if t is None else c_void_p(t.data_ptr())  # noqa: E731
-        code = self.lib.bt_dbn_track_device(
-            self.ctx, ptr(beat), ptr(down), ptr(act), i64_array(frame_offsets), len(frame_offsets) - 1,
-            c_void_p(bpb.ctypes.data), len(bpb), float(params["min_bpm"]), float(params["max_bpm"]), int(params["num_tempi"]),
-            float(params["transition_lambda"]), float(params["observation_lambda"]), float(params["threshold"]),
-            int(bool(params["correct"])), float(params["fps"]), ptr(times), ptr(numbers), ptr(counts), self._stream())
-        _lib.check(self.lib, self.ctx, code)
+        p = self._dev_ptr
+        self._call("bt_dbn_track_device", p(beat), p(down), p(act, dtype=torch.float64), i64_array(frame_offsets),
+                   len(frame_offsets) - 1, i32_array(bpb), len(bpb), float(params["min_bpm"]), float(params["max_bpm"]),
+                   int(params["num_tempi"]), float(params["transition_lambda"]), float(params["observation_lambda"]),
+                   float(params["threshold"]), int(bool(params["correct"])), float(params["fps"]),
+                   p(times, dtype=torch.float64), p(numbers, dtype=torch.int32), p(counts, dtype=torch.int64))
 
     def dbn_async(self, beat: torch.Tensor | None, down: torch.Tensor | None, frame_offsets, slot: dict | None = None,
                   params: dict | None = None, activations: torch.Tensor | None = None):
@@ -414,11 +392,8 @@ class Engine:
             slot["numbers_h"] = torch.empty(cap, dtype=torch.int32).pin_memory()
             slot["counts_h"] = torch.empty(nn, dtype=torch.int64).pin_memory()
             slot["event"] = torch.cuda.Event()
-        if activations is not None:
-            assert activations.is_cuda and activations.dtype == torch.float64 and activations.is_contiguous()
-        else:
-            assert beat.is_cuda and beat.dtype == torch.float32 and beat.is_contiguous()
-            assert down.is_cuda and down.dtype == torch.float32 and down.is_contiguous()
+        if activations is None:
+            assert beat is not None and down is not None, "logits or activations"
         self._dbn_enqueue(beat, down, activations, frame_offsets, params, slot["times"], slot["numbers"], slot["counts"])
         if n > 0:
             slot["times_h"][:total].copy_(slot["times"][:total], non_blocking=True)
@@ -435,29 +410,59 @@ class Engine:
     def debug_dbn_viterbi(self, log_dens: torch.Tensor, beats: int, intervals, log_tempo, pointers):
         """bt_debug_dbn_viterbi: the device Viterbi of one bar model on float64 log densities [T, 3] (device tensor);
         model tables as bt_dbn_viterbi takes them (host arrays).  Returns (path int64 numpy array, logp float)."""
-        assert log_dens.is_cuda and log_dens.dtype == torch.float64 and log_dens.is_contiguous()
         T = log_dens.shape[0]
-        iv = np.ascontiguousarray(intervals, dtype=np.int32)
         lt = np.ascontiguousarray(log_tempo, dtype=np.float64)
-        pt = np.ascontiguousarray(pointers, dtype=np.int32)
         path = torch.empty(max(T, 1), dtype=torch.int64, device=self.device)
         logp = torch.empty(1, dtype=torch.float64, device=self.device)
-        code = self.lib.bt_debug_dbn_viterbi(self.ctx, c_void_p(log_dens.data_ptr()), T, int(beats), len(iv),
-                                             c_void_p(iv.ctypes.data), c_void_p(lt.ctypes.data), c_void_p(pt.ctypes.data),
-                                             c_void_p(path.data_ptr()), c_void_p(logp.data_ptr()), self._stream())
-        _lib.check(self.lib, self.ctx, code)
+        p = self._dev_ptr
+        self._call("bt_debug_dbn_viterbi", p(log_dens, dtype=torch.float64), T, int(beats), len(intervals),
+                   i32_array(intervals), c_void_p(lt.ctypes.data), i32_array(pointers), p(path, dtype=torch.int64),
+                   p(logp, dtype=torch.float64))
         return path[:T].cpu().numpy(), float(logp.item())
+
+    # ---- scoring and training (evaluate.py, loss.py, dataset.py; contracts in include/beatthis.h) ----------------
+    def beat_metrics(self, times: torch.Tensor, offsets, params, out: torch.Tensor):
+        """bt_beat_metrics of n = out.shape[0] sets on one float64 device buffer of times: set i's estimates are
+        times[offsets[i]:offsets[i + 1]], its references times[offsets[n + i]:offsets[n + i + 1]]; out [n, 12] float64."""
+        n = out.shape[0]
+        base = self._dev_ptr(times, dtype=torch.float64)  # both offset arrays index the one buffer
+        self._call("bt_beat_metrics", base, i64_array(offsets[: n + 1]), base, i64_array(offsets[n:]), n,
+                   ctypes.byref(params), self._dev_ptr(out, dtype=torch.float64))
+
+    def beat_loss(self, preds, targets, mask, offsets, params, row_loss, mean):
+        """bt_beat_loss of the rows [offsets[i], offsets[i + 1]) of fp32 preds, targets and mask (None: no mask):
+        float64 row_loss per row and the fp32 mean over all rows."""
+        p = self._dev_ptr
+        self._call("bt_beat_loss", p(preds), p(targets), p(mask), i64_array(offsets), len(offsets) - 1,
+                   ctypes.byref(params), p(row_loss, dtype=torch.float64), p(mean))
+
+    def beat_loss_backward(self, preds, targets, mask, offsets, params, grad_mean, grad):
+        """bt_beat_loss_backward: grad (fp32, like preds) of the mean of beat_loss scaled by the fp32 grad_mean."""
+        p = self._dev_ptr
+        self._call("bt_beat_loss_backward", p(preds), p(targets), p(mask), i64_array(offsets), len(offsets) - 1,
+                   ctypes.byref(params), p(grad_mean), p(grad))
+
+    def train_batch(self, rows, row_offsets, length, row_map, beat_frames, beat_offsets, downbeat_frames,
+                    downbeat_offsets, spect, truth_beat, truth_downbeat, padding_mask):
+        """One ``bt_train_batch`` launch on the current stream: rows, spect and the three [B, L] outputs are device
+        tensors (rows and spect of 16-bit elements, the others of bytes); the tables are host arrays, row_map None for
+        identity maps."""
+        p, h16, byte = self._dev_ptr, (torch.int16, torch.float16), (torch.bool, torch.uint8)
+        self._call("bt_train_batch", p(rows, dtype=h16), i64_array(row_offsets), len(row_offsets) - 1, int(length),
+                   None if row_map is None else i32_array(row_map), i32_array(beat_frames), i64_array(beat_offsets),
+                   i32_array(downbeat_frames), i64_array(downbeat_offsets), p(spect, dtype=h16),
+                   p(truth_beat, dtype=byte), p(truth_downbeat, dtype=byte), p(padding_mask, dtype=byte))
 
     # ---- per-kernel-class timing (bench.py roofline) -------------------------------------------
     def profile_enable(self, on: bool = True):
-        _lib.check(self.lib, self.ctx, self.lib.bt_profile_enable(self.ctx, int(on)))
+        self._call("bt_profile_enable", int(on), stream=False)
 
     def profile_reset(self):
-        _lib.check(self.lib, self.ctx, self.lib.bt_profile_reset(self.ctx))
+        self._call("bt_profile_reset", stream=False)
 
     def profile_results(self) -> dict:
         """{kernel class: (total device ms, launches)} accumulated since the last reset."""
-        _lib.check(self.lib, self.ctx, self.lib.bt_profile_collect(self.ctx))
+        self._call("bt_profile_collect", stream=False)
         out = {}
         for i in range(int(self.lib.bt_profile_count(self.ctx))):
             name = ctypes.create_string_buffer(64)
@@ -468,10 +473,18 @@ class Engine:
 
     # ---- test hooks --------------------------------------------------------------------------
     def tap(self, name: str, spect: torch.Tensor, frame_offsets, capacity: int):
+        """Test hook: activation `name` of a spect2frames_cat call."""
+        return self._tap(name, capacity, lambda: self.spect2frames_cat(spect, frame_offsets))
+
+    def tap_chunks(self, name: str, chunks: torch.Tensor, capacity: int):
+        """Test hook: activation `name` of a forward_chunks call (single wave)."""
+        return self._tap(name, capacity, lambda: self.forward_chunks(chunks))
+
+    def _tap(self, name: str, capacity: int, forward):
         buf = torch.zeros(capacity, dtype=torch.float32, device=self.device)
-        _lib.check(self.lib, self.ctx, self.lib.bt_debug_request_tap(self.ctx, name.encode(), c_void_p(buf.data_ptr()), capacity))
+        self._call("bt_debug_request_tap", name.encode(), self._dev_ptr(buf), capacity, stream=False)
         try:
-            out = self.spect2frames_cat(spect, frame_offsets)
+            out = forward()
             torch.cuda.synchronize(self.device)
             n = int(self.lib.bt_debug_tap_count(self.ctx))
         finally:
@@ -502,10 +515,8 @@ class Engine:
         d.resid_epilogue, d.kind, d.gelu, d.C, d.heads, d.posmode, d.F = int(resid_epilogue), kind, int(gelu), C, heads, posmode, F
         d.qscale = float(qscale)
         tile = (ctypes.c_int32 * 2)()
-        code = self.lib.bt_debug_gemm(self.ctx, ctypes.byref(d), ptr(a), ptr(w), ptr(bias), ptr(resid), ptr(out_f32), ptr(out_act),
-                                      out_act.numel() if out_act is not None else 0, ptr(rope_cos), ptr(rope_sin), tile,
-                                      self._stream())
-        _lib.check(self.lib, self.ctx, code)
+        self._call("bt_debug_gemm", ctypes.byref(d), ptr(a), ptr(w), ptr(bias), ptr(resid), ptr(out_f32), ptr(out_act),
+                   out_act.numel() if out_act is not None else 0, ptr(rope_cos), ptr(rope_sin), tile)
         return int(tile[0]), int(tile[1])
 
     def debug_attention(self, q, k, v, gates=None, key_lens=None, seqs_per_chunk=1, out=None):
@@ -518,11 +529,9 @@ class Engine:
             gates = torch.ones(seqs * L, C // 32, dtype=torch.float32, device=self.device)
         o = torch.empty_like(q) if out is None else out
         p = self._dev_ptr
-        lens = (ctypes.c_int32 * len(key_lens))(*[int(x) for x in key_lens]) if key_lens is not None else None
-        code = self.lib.bt_debug_attention(self.ctx, p(q, q.numel()), p(k, q.numel()), p(v, q.numel()),
-                                           p(gates, seqs * L * (C // 32)), p(o, q.numel()), o.numel(), seqs, L, C // 32,
-                                           lens, seqs_per_chunk, self._stream())
-        _lib.check(self.lib, self.ctx, code)
+        lens = i32_array(key_lens) if key_lens is not None else None
+        self._call("bt_debug_attention", p(q, q.numel()), p(k, q.numel()), p(v, q.numel()), p(gates, seqs * L * (C // 32)),
+                   p(o, q.numel()), o.numel(), seqs, L, C // 32, lens, seqs_per_chunk)
         return o
 
     def debug_attention_freq(self, q, k, v, gates, B, F, out=None):
@@ -531,43 +540,32 @@ class Engine:
         M, C = q.shape
         o = torch.empty_like(q) if out is None else out
         p = self._dev_ptr
-        code = self.lib.bt_debug_attention_freq(self.ctx, p(q, M * C), p(k, M * C), p(v, M * C), p(gates, M * (C // 32)),
-                                                p(o, M * C), o.numel(), B, F, M // (B * F), C // 32, self._stream())
-        _lib.check(self.lib, self.ctx, code)
+        self._call("bt_debug_attention_freq", p(q, M * C), p(k, M * C), p(v, M * C), p(gates, M * (C // 32)), p(o, M * C),
+                   o.numel(), B, F, M // (B * F), C // 32)
         return o
 
     # The row-kernel hooks take fp32 device tensors and write their outputs in place, so a caller can surround the
     # M rows with sentinel values.  x and every output may have more than M rows; only the first M are the problem.
-    # The C hooks cannot see buffer sizes, so each tensor is checked here to hold at least the elements they touch.
-    def _dev_ptr(self, t, n: int = 0):
-        if t is None:
-            return None
-        assert t.is_cuda and t.dtype == torch.float32 and t.is_contiguous()
-        assert t.numel() >= n, f"tensor of {t.numel()} elements, the hook reads or writes {n}"
-        return c_void_p(t.data_ptr())
 
     def debug_norm(self, x, xn_out, M: int, C: int, wg=None, bg=None, gates_out=None, heads: int = 0):
         """bt_debug_norm: xn_out[:M] = rmsnorm(x[:M]) through norm_kernel (+ gates_out[:M] with heads > 0)."""
         p, n = self._dev_ptr, max(M, 0)
-        code = self.lib.bt_debug_norm(self.ctx, p(x, n * C), p(xn_out, n * C), M, C, p(wg, heads * C), p(bg, heads),
-                                      p(gates_out, n * heads), heads, self._stream())
-        _lib.check(self.lib, self.ctx, code)
+        self._call("bt_debug_norm", p(x, n * C), p(xn_out, n * C), M, C, p(wg, heads * C), p(bg, heads),
+                   p(gates_out, n * heads), heads)
 
     def debug_fused_qkv(self, x, wqkv, wg, bg, rope_cos, rope_sin, qkv_out, gates_out, M: int, C: int, L: int, F: int,
                         posmode: int, qscale: float):
         """bt_debug_fused_qkv: qkv_out[:M] (3C columns) and gates_out[:M] from x[:M] through fused_qkv_kernel<C>."""
         p, n, heads, rows = self._dev_ptr, max(M, 0), C // 32, 1500  # RoPE tables: [BT_CHUNK, 16]
-        code = self.lib.bt_debug_fused_qkv(self.ctx, p(x, n * C), p(wqkv, 3 * C * C), p(wg, heads * C), p(bg, heads),
-                                           p(rope_cos, rows * 16), p(rope_sin, rows * 16), p(qkv_out, n * 3 * C),
-                                           p(gates_out, n * heads), M, C, L, F, posmode, float(qscale), self._stream())
-        _lib.check(self.lib, self.ctx, code)
+        self._call("bt_debug_fused_qkv", p(x, n * C), p(wqkv, 3 * C * C), p(wg, heads * C), p(bg, heads),
+                   p(rope_cos, rows * 16), p(rope_sin, rows * 16), p(qkv_out, n * 3 * C), p(gates_out, n * heads), M, C, L,
+                   F, posmode, float(qscale))
 
     def debug_fused_ff(self, x, w1, b1, w2, b2, M: int, C: int, o=None, wout=None, xb_out=None):
         """bt_debug_fused_ff: x[:M] updated in place through fused_ff_kernel<C, o is not None> (+ xb_out[:M])."""
         p, n = self._dev_ptr, max(M, 0)
-        code = self.lib.bt_debug_fused_ff(self.ctx, p(x, n * C), p(w1, 4 * C * C), p(b1, 4 * C), p(w2, 4 * C * C),
-                                          p(b2, C), p(o, n * C), p(wout, C * C), p(xb_out, n * C), M, C, self._stream())
-        _lib.check(self.lib, self.ctx, code)
+        self._call("bt_debug_fused_ff", p(x, n * C), p(w1, 4 * C * C), p(b1, 4 * C), p(w2, 4 * C * C), p(b2, C),
+                   p(o, n * C), p(wout, C * C), p(xb_out, n * C), M, C)
 
     # The chunk-table hooks take the table as a sequence of (frame_base, T, start, out_base, write_lo, write_hi, len)
     # tuples (bt_debug_chunk); the library checks the table against the buffer lengths it is given.
@@ -578,23 +576,19 @@ class Engine:
     def debug_stem(self, spect, chunks, L: int, bn1_scale, bn1_shift, w, bias, out):
         """bt_debug_stem: out [len(chunks), 32, L, 32] (fp32, in place) from spect [frames, 128] through stem_kernel."""
         p = self._dev_ptr
-        code = self.lib.bt_debug_stem(self.ctx, p(spect), spect.numel() // 128, self._chunk_table(chunks), len(chunks), L,
-                                      p(bn1_scale, 128), p(bn1_shift, 128), p(w, 32 * 12), p(bias, 32), p(out), out.numel(),
-                                      self._stream())
-        _lib.check(self.lib, self.ctx, code)
+        self._call("bt_debug_stem", p(spect), spect.numel() // 128, self._chunk_table(chunks), len(chunks), L,
+                   p(bn1_scale, 128), p(bn1_shift, 128), p(w, 32 * 12), p(bias, 32), p(out), out.numel())
 
     def debug_zero_tail(self, buf, chunks, F: int, L: int, C: int):
         """bt_debug_zero_tail: rows [len, L) of every plane of buf [len(chunks), F, L, C] (fp32 or 16-bit, in place)
         cleared through zero_tail_kernel."""
-        assert buf.is_cuda and buf.is_contiguous() and buf.element_size() in (2, 4)
-        code = self.lib.bt_debug_zero_tail(self.ctx, c_void_p(buf.data_ptr()), buf.element_size(), self._chunk_table(chunks),
-                                           len(chunks), F, L, C, buf.numel() * buf.element_size(), self._stream())
-        _lib.check(self.lib, self.ctx, code)
+        assert buf.element_size() in (2, 4)
+        self._call("bt_debug_zero_tail", self._dev_ptr(buf, dtype=buf.dtype), buf.element_size(), self._chunk_table(chunks),
+                   len(chunks), F, L, C, buf.numel() * buf.element_size())
 
     def debug_head(self, x, D: int, w, b, chunks, L: int, sum_head: bool, beat, down):
         """bt_debug_head: the owned frames of beat / down (fp32, in place) from x [len(chunks), L, D] through head_kernel."""
         p = self._dev_ptr
         assert beat.numel() == down.numel()
-        code = self.lib.bt_debug_head(self.ctx, p(x, len(chunks) * L * D), D, p(w, 2 * D), p(b, 2), self._chunk_table(chunks),
-                                      len(chunks), L, int(bool(sum_head)), p(beat), p(down), beat.numel(), self._stream())
-        _lib.check(self.lib, self.ctx, code)
+        self._call("bt_debug_head", p(x, len(chunks) * L * D), D, p(w, 2 * D), p(b, 2), self._chunk_table(chunks),
+                   len(chunks), L, int(bool(sum_head)), p(beat), p(down), beat.numel())

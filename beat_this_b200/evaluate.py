@@ -18,10 +18,8 @@
 from __future__ import annotations
 
 import argparse
-import ctypes
 import json
 import sys
-from ctypes import c_void_p
 from dataclasses import dataclass, field
 from pathlib import Path
 
@@ -29,22 +27,14 @@ import numpy as np
 import torch
 
 from . import _lib
+from .engine import Engine
 
 FIELDS = ("n_ref", "n_est", "matches", "P", "R", "F", "cemgil", "cemgil_max", "CMLc", "CMLt", "AMLc", "AMLt")
 SUMMARY_KEYS = tuple(f"{k}_{t}" for t in ("beat", "downbeat") for k in ("F-measure", "Cemgil", "CMLt", "AMLt"))
 LOSS_KEYS = ("test_loss_beat", "test_loss_downbeat", "test_loss")
 FPS = 50
 
-_engines = {}
-
-
-def _engine(device):
-    from .engine import Engine, _cuda_device
-
-    dev = _cuda_device(device)
-    if dev not in _engines:
-        _engines[dev] = Engine.mel_only(dev)  # the metric kernel needs no weights
-    return _engines[dev]
+_engine = Engine.shared  # _engine(device), the name earlier versions offered
 
 
 def check_times(times, what="beat times") -> np.ndarray:
@@ -89,19 +79,15 @@ def beat_metrics(estimates, references, min_beat_time=5.0, f_window=0.07, cemgil
     n = len(est)
     if n == 0:
         return np.zeros((0, len(FIELDS)))
-    eng = _engine(device)
-    lens = [len(a) for a in est + ref]
-    offs = np.concatenate(([0], np.cumsum(lens))).astype(np.int64)
-    host = torch.empty(max(int(offs[-1]), 1), dtype=torch.float64).pin_memory()
+    eng = Engine.shared(device)
+    offs = _lib.offsets(len(a) for a in est + ref)
+    host = torch.empty(max(offs[-1], 1), dtype=torch.float64).pin_memory()
     if offs[-1]:
         host[: offs[-1]].numpy()[:] = np.concatenate(est + ref)
     packed = host.to(eng.device, non_blocking=True)  # estimates of every set, then references: one copy
     out = torch.empty((n, len(FIELDS)), dtype=torch.float64, device=eng.device)
     p = _lib.bt_beat_metric_params(min_beat_time, f_window, cemgil_sigma, phase_threshold, period_threshold)
-    base = c_void_p(packed.data_ptr())  # both offset arrays index the packed buffer
-    code = eng.lib.bt_beat_metrics(eng.ctx, base, _lib.i64_array(offs[: n + 1]), base, _lib.i64_array(offs[n:]), n,
-                                   ctypes.byref(p), c_void_p(out.data_ptr()), eng._stream())
-    _lib.check(eng.lib, eng.ctx, code)
+    eng.beat_metrics(packed, offs, p, out)
     return out.cpu().numpy()
 
 
@@ -142,7 +128,7 @@ def _frames_of_audio(runner, path) -> int:
     from . import preprocessing as P
     from .preprocessing import load_audio
 
-    infos, ok = runner.probe([path])
+    infos, ok = _lib.wav_probe([path])
     if ok[0]:
         n, sr = int(infos[0].frames), int(infos[0].sample_rate)
     else:
@@ -163,7 +149,7 @@ def _predict(runner, pieces, group=64, logits=False, post=None):
     audio = [i for i, p in enumerate(pieces) if p.audio is not None]
     if audio and logits:
         out = runner.frames_batch([pieces[i].audio for i in audio])
-        fo = np.cumsum([0] + [len(b) for b, _ in out]).tolist()
+        fo = _lib.offsets(len(b) for b, _ in out)
         beat = torch.cat([b for b, _ in out]).contiguous()
         down = torch.cat([d for _, d in out]).contiguous()
         for i, r, o in zip(audio, runner.frames2beats.batch_cat(beat, down, fo), out):
@@ -177,9 +163,7 @@ def _predict(runner, pieces, group=64, logits=False, post=None):
     for g in range(0, len(spect), group):
         idx = spect[g : g + group]
         out = runner.spects2frames([np.asarray(pieces[i].spect, dtype=np.float32) for i in idx])
-        fo = [0]
-        for b, _ in out:
-            fo.append(fo[-1] + b.shape[0])
+        fo = _lib.offsets(b.shape[0] for b, _ in out)
         beat = torch.cat([b for b, _ in out]).contiguous()
         down = torch.cat([d for _, d in out]).contiguous()
         for i, r, a, b, o in zip(idx, post.batch_cat(beat, down, fo), fo[:-1], fo[1:], out):
@@ -205,7 +189,7 @@ def piece_losses(runner, pieces, logits, fps: float = FPS) -> dict:
     from .loss import beat_loss_rows, loss_from_hparams, loss_spec
 
     dev = runner.model.device
-    fo = np.cumsum([0] + [len(b) for b, _ in logits]).tolist()
+    fo = _lib.offsets(len(b) for b, _ in logits)
     out = {}
     for t, (target, module) in enumerate(zip(("beat", "downbeat"), loss_from_hparams(runner.model.checkpoint_hparams))):
         x = torch.cat([lg[t] for lg in logits]).contiguous()

@@ -12,15 +12,15 @@ Differences a user can observe:
 """
 from __future__ import annotations
 
-import ctypes
 import math
 
 import numpy as np
 import torch
 
-from ._lib import BT_CHUNK, MAX_CHUNK_CAP, bt_wav_info
+from . import _lib
+from ._lib import BT_CHUNK, DEFAULT_CHUNKING, MAX_CHUNK_CAP
 from .engine import Engine, chunking_struct
-from .pipeline import BeatPipeline, as_signal_array, chunk_cost, padded_frames, plan_groups
+from .pipeline import BeatPipeline, as_signal_array, padded_frames, plan_groups
 from .postprocessor import Postprocessor
 from .preprocessing import LogMelSpect, load_audio
 from .utils import replace_state_dict_key, save_beat_tsv
@@ -187,24 +187,17 @@ def aggregate_prediction(pred_chunks: list, starts: list, full_size: int, chunk_
     return beat, downbeat
 
 
-DEFAULT_CHUNKING = (1500, 6, "keep_first")  # what Spect2Frames.spect2frames uses (reference inference.py:244-254)
-
-
-def engine_chunking(chunk_size: int, border_size: int, overlap_mode: str, max_chunk_size: int = BT_CHUNK
-                    ) -> tuple | None:
-    """The `chunking` argument of Engine.spect2frames_cat / audio2frames_cat for split_predict_aggregate's values:
-    None for 1500 / 6 / keep_first (the plain entry points), else the checked triple.  ``ValueError`` for values the
-    CUDA path cannot run (engine.chunking_struct; chunk_size up to the model's max_chunk_size)."""
+def engine_chunking(chunk_size: int, border_size: int, overlap_mode: str, max_chunk_size: int = BT_CHUNK) -> tuple:
+    """The `chunking` argument of Engine.spect2frames_cat / audio2frames_cat for split_predict_aggregate's values: the
+    checked triple.  ``ValueError`` for values the CUDA path cannot run (engine.chunking_struct; chunk_size up to the
+    model's max_chunk_size)."""
     chunking_struct(chunk_size, border_size, overlap_mode, max_chunk_size)
-    chunking = (int(chunk_size), int(border_size), overlap_mode)
-    return None if chunking == DEFAULT_CHUNKING else chunking
+    return int(chunk_size), int(border_size), overlap_mode
 
 
-def _plan_groups(n_samples, sr: int, chunking: tuple | None):
-    """Groups of consecutive clips for the pipeline: GROUP_CHUNKS 1500-frame chunks, or with a chunking the padded
-    frames of as many, so that a group of long chunks fits one wave's frame budget (bt_set_wave_chunks)."""
-    if chunking is None:
-        return plan_groups([chunk_cost(n, sr) for n in n_samples], GROUP_CHUNKS, GROUP_CLIPS)
+def _plan_groups(n_samples, sr: int, chunking: tuple):
+    """Groups of consecutive clips for the pipeline: the padded frames of GROUP_CHUNKS 1500-frame chunks each, so that
+    a group of long chunks fits one wave's frame budget (bt_set_wave_chunks)."""
     return plan_groups([padded_frames(n, sr, *chunking[:2]) for n in n_samples], GROUP_CHUNKS * BT_CHUNK, GROUP_CLIPS)
 
 
@@ -252,9 +245,7 @@ class Spect2Frames:
         split_predict_aggregate(spect, chunk_size, border_size, overlap_mode, model) does, all in one call."""
         chunking = engine_chunking(chunk_size, border_size, overlap_mode, self.model.max_chunk_size)
         spects = [torch.as_tensor(s, dtype=torch.float32, device=self.device) for s in spects]
-        fo = [0]
-        for s in spects:
-            fo.append(fo[-1] + s.shape[0])
+        fo = _lib.offsets(s.shape[0] for s in spects)
         beat, down = self.model.engine.spect2frames_cat(torch.cat(spects).contiguous(), fo, chunking)
         return [(beat[fo[i] : fo[i + 1]], down[fo[i] : fo[i + 1]]) for i in range(len(spects))]
 
@@ -334,7 +325,7 @@ class Audio2Frames(Spect2Frames):
         return beat, down
 
     # ---- many clips ---------------------------------------------------------------------------------------
-    def _run_groups(self, arrays, sr, want, chunking=None):
+    def _run_groups(self, arrays, sr, want, chunking=DEFAULT_CHUNKING):
         """Generator over groups: (first index, last index + 1, pipeline result)."""
         pipe = self.pipeline
         groups = _plan_groups([a.shape[0] for a in arrays], sr, chunking)
@@ -349,9 +340,9 @@ class Audio2Frames(Spect2Frames):
     def batch(self, signals, sr=22050):
         """list of signals (1-D or (time, channels) arrays, `sr` Hz) -> list of (beat_logits, downbeat_logits) device
         tensors; staging, copies and kernels of consecutive groups of clips overlap."""
-        return self._frames_batch(signals, sr, None)
+        return self._frames_batch(signals, sr)
 
-    def _frames_batch(self, signals, sr, chunking):
+    def _frames_batch(self, signals, sr, chunking=DEFAULT_CHUNKING):
         """batch() with the `chunking` argument of Engine.audio2frames_cat."""
         arrays, sr = self._prepare(signals, sr)
         out = [None] * len(arrays)
@@ -434,29 +425,16 @@ class File2Beats(Audio2Beats):
         signal, sr = load_audio(audio_path)
         return super().__call__(signal, sr)
 
-    def probe(self, audio_paths):
-        """bt_wav_probe on every path: (ctypes array of bt_wav_info, list of ok flags).  Files that are not plain
-        WAV are decoded by load_audio's backend chain instead."""
-        from ._lib import bt_wav_info
-
-        lib = self.model.engine.lib
-        infos = (bt_wav_info * len(audio_paths))()
-        ok = [lib.bt_wav_probe(str(p).encode(), ctypes.byref(infos[i])) == 0 and infos[i].frames > 0
-              for i, p in enumerate(audio_paths)]
-        return infos, ok
-
     def batch(self, audio_paths, on_error: str = "raise"):
         """Many files per call.  WAV files are read, mixed to mono and cast by the native host threads straight into
         the pinned staging ring (no numpy round trip); other containers go through load_audio.  Files of equal
         sample rate share groups.  on_error: "raise", or "skip" (a file that cannot be loaded or processed yields
         None instead of aborting the call -- the behaviour of the reference's per-file loop, cli.py:185-190)."""
-        from ._lib import bt_wav_info
-
         if on_error not in ("raise", "skip"):
             raise ValueError("on_error must be 'raise' or 'skip'")
         paths = [str(p) for p in audio_paths]
         out = [None] * len(paths)
-        infos, is_wav = self.probe(paths)
+        infos, is_wav = _lib.wav_probe(paths)
         for i in range(len(paths)):  # a clip needs more than 512 samples at 22.05 kHz (reflect padding of the STFT)
             if is_wav[i] and infos[i].frames * 22050 // max(1, infos[i].sample_rate) <= 512:
                 if on_error == "raise":
@@ -467,12 +445,11 @@ class File2Beats(Audio2Beats):
         want = self._want_beats
         for sr in sorted({infos[i].sample_rate for i in range(len(paths)) if is_wav[i]}):
             idx = [i for i in range(len(paths)) if is_wav[i] and infos[i].sample_rate == sr]
-            groups = plan_groups([chunk_cost(infos[i].frames, sr) for i in idx], GROUP_CHUNKS, GROUP_CLIPS)
+            groups = _plan_groups([infos[i].frames for i in idx], sr, DEFAULT_CHUNKING)
 
             def submit(g, idx=idx, groups=groups, sr=sr):
                 sel = idx[groups[g][0] : groups[g][1]]
-                sub = (bt_wav_info * len(sel))(*[infos[i] for i in sel])
-                pipe.submit_wavs([paths[i] for i in sel], sub, sr, want)
+                pipe.submit_wavs([paths[i] for i in sel], [infos[i] for i in sel], sr, want)
 
             try:
                 for (lo, hi), res in zip(groups, pipe.run(len(groups), submit)):
@@ -522,7 +499,7 @@ class File2Beats(Audio2Beats):
         chunking = engine_chunking(chunk_size, border_size, overlap_mode, self.model.max_chunk_size)
         paths = [str(p) for p in audio_paths]
         out = [None] * len(paths)
-        infos, is_wav = self.probe(paths)
+        infos, is_wav = _lib.wav_probe(paths)
         for i in range(len(paths)):
             if is_wav[i] and infos[i].frames * 22050 // max(1, infos[i].sample_rate) <= 512:
                 raise ValueError(f'"{paths[i]}" is too short ({infos[i].frames} samples)')
@@ -533,8 +510,7 @@ class File2Beats(Audio2Beats):
 
             def submit(g, idx=idx, groups=groups, sr=sr):
                 sel = idx[groups[g][0] : groups[g][1]]
-                pipe.submit_wavs([paths[i] for i in sel], (bt_wav_info * len(sel))(*[infos[i] for i in sel]), sr, "frames",
-                                 chunking)
+                pipe.submit_wavs([paths[i] for i in sel], [infos[i] for i in sel], sr, "frames", chunking)
 
             try:
                 for (lo, hi), (beat, down, fo) in zip(groups, pipe.run(len(groups), submit)):

@@ -10,34 +10,17 @@ There is no CPU path: CPU tensors raise.
 """
 from __future__ import annotations
 
-import ctypes
-from ctypes import c_void_p
-
 import numpy as np
 import torch
 
 from . import _lib
+from .engine import Engine
 
 MASKED_BCE, SHIFT_TOLERANT, SPLIT_SHIFT_TOLERANT = 0, 1, 2  # BT_LOSS_* (include/beatthis.h)
 
 
-def _engine(device):
-    from .evaluate import _engine
-
-    return _engine(device)
-
-
 def _flat(t, device):
     return t.to(device, torch.float32).contiguous().view(-1)
-
-
-def _call(entry, preds, targets, mask, offsets, params, *outs):
-    eng = _engine(preds.device)
-    offs = _lib.i64_array(offsets)
-    ptr = lambda t: c_void_p(t.data_ptr() if t is not None else None)  # noqa: E731
-    code = getattr(eng.lib, entry)(eng.ctx, ptr(preds), ptr(targets), ptr(mask), offs, len(offsets) - 1,
-                                   ctypes.byref(params), *[ptr(o) for o in outs], eng._stream())
-    _lib.check(eng.lib, eng.ctx, code)
 
 
 def _check_device(preds):
@@ -57,7 +40,7 @@ def beat_loss_rows(preds, targets, mask, offsets, kind, tolerance=3, pos_weight=
     row_loss = torch.empty(max(n, 1), dtype=torch.float64, device=dev)
     mean = torch.empty((), dtype=torch.float32, device=dev)
     params = _lib.bt_loss_params(int(kind), int(tolerance), float(pos_weight))
-    _call("bt_beat_loss", x, y, m, offsets, params, row_loss, mean)
+    Engine.shared(dev).beat_loss(x, y, m, offsets, params, row_loss, mean)
     return row_loss[:n], mean
 
 
@@ -75,7 +58,7 @@ class _BeatLoss(torch.autograd.Function):
         offsets, params = ctx.args
         grad = torch.empty_like(preds)
         g = grad_mean.to(preds.device, torch.float32).contiguous()
-        _call("bt_beat_loss_backward", preds, targets, mask, offsets, params, g, grad)
+        Engine.shared(preds.device).beat_loss_backward(preds, targets, mask, offsets, params, g, grad)
         return grad, None, None, None, None, None, None
 
 

@@ -16,18 +16,14 @@ stays one group ahead of the host.
 """
 from __future__ import annotations
 
-import ctypes
 import time
 from collections import deque
-from ctypes import c_void_p
 
 import numpy as np
 import torch
 
 from . import _lib
-
-SIG_F32, SIG_F64, SIG_I16 = 0, 1, 2
-_NP2SIG = {np.dtype(np.float32): SIG_F32, np.dtype(np.float64): SIG_F64, np.dtype(np.int16): SIG_I16}
+from ._lib import DEFAULT_CHUNKING
 
 
 def as_signal_array(signal) -> np.ndarray:
@@ -38,7 +34,7 @@ def as_signal_array(signal) -> np.ndarray:
     a = np.asarray(signal)
     if a.ndim not in (1, 2):
         raise ValueError(f"Expected 1D or 2D signal, got shape {a.shape}")
-    if a.dtype not in _NP2SIG:
+    if a.dtype not in _lib.SIGNAL_DTYPES:
         a = a.astype(np.float64)  # ints other than int16, float16, ...: the reference's mean(1) works in float64 too
     return np.ascontiguousarray(a)
 
@@ -57,12 +53,6 @@ def plan_groups(costs, max_cost: int, max_clips: int):
     return groups
 
 
-def chunk_cost(n_samples: int, sr: int = 22050) -> int:
-    """1500-frame model passes a clip of n_samples at `sr` Hz needs: ceil(frames / 1488) (split_piece, inference.py:119-125)."""
-    frames = 1 + (int(n_samples) * 22050 // max(1, int(sr))) // 441
-    return max(1, -(-frames // 1488))
-
-
 def padded_frames(n_samples: int, sr: int, chunk_size: int, border_size: int) -> int:
     """Frames a clip of n_samples at `sr` Hz occupies in the waves of the C library under a chunking: its chunks
     (split_piece, inference.py:119-125) times chunk_size, the most a chunk is padded to."""
@@ -73,7 +63,7 @@ def padded_frames(n_samples: int, sr: int, chunk_size: int, border_size: int) ->
 def _check_frames_route(want: str, chunking) -> None:
     """Only framewise logits take another chunking than 1500 / 6 / keep_first: the beat routes keep the reference's
     Audio2Beats, which always cuts that way (inference.py:244-254)."""
-    if chunking is not None and want != "frames":
+    if chunking != DEFAULT_CHUNKING and want != "frames":
         raise ValueError(f'a chunking applies to want="frames" only, not want="{want}"')
 
 
@@ -99,7 +89,6 @@ class BeatPipeline:
 
     def __init__(self, engine, depth: int = 3, host_threads: int | None = None):
         self.engine = engine
-        self.lib = engine.lib
         self.device = engine.device
         self.copy_stream = torch.cuda.Stream(self.device)
         self.compute_stream = torch.cuda.Stream(self.device)
@@ -137,21 +126,9 @@ class BeatPipeline:
     def stage_signals(self, arrays, dst: torch.Tensor):
         """Mono mix + fp32 cast of C-contiguous ndarrays (see as_signal_array) into `dst` (host fp32 tensor);
         returns the sample offsets."""
-        n = len(arrays)
-        so = [0]
-        for a in arrays:
-            so.append(so[-1] + a.shape[0])
-        ptrs = (c_void_p * n)(*[a.ctypes.data for a in arrays])
-        dts = (ctypes.c_int32 * n)(*[_NP2SIG[a.dtype] for a in arrays])
-        frames = (ctypes.c_int64 * n)(*[a.shape[0] for a in arrays])
-        chans = (ctypes.c_int32 * n)(*[1 if a.ndim == 1 else a.shape[1] for a in arrays])
-        offs = (ctypes.c_int64 * (n + 1))(*so)
-        code = self.lib.bt_stage_audio(ptrs, dts, frames, chans, n, c_void_p(dst.data_ptr()), offs, self.host_threads)
-        if code != 0:
-            raise _lib.BTError(f"bt_stage_audio failed ({code}): bad signal array")
-        return so
+        return _lib.stage_audio(arrays, dst, self.host_threads)
 
-    def _enqueue(self, idx, s, so, sr, want, chunking=None):
+    def _enqueue(self, idx, s, so, sr, want, chunking=DEFAULT_CHUNKING):
         n = so[-1]
         with torch.cuda.stream(self.copy_stream):
             s.dev[:n].copy_(s.host[:n], non_blocking=True)
@@ -194,7 +171,7 @@ class BeatPipeline:
             s.t1.record(self.compute_stream)
         self.inflight.append((idx, payload))
 
-    def submit_signals(self, arrays, sr: int = 22050, want: str = "beats", chunking: tuple | None = None):
+    def submit_signals(self, arrays, sr: int = 22050, want: str = "beats", chunking: tuple = DEFAULT_CHUNKING):
         """chunking (want="frames" only): (chunk_size, border_size, overlap_mode), see Engine.spect2frames_cat."""
         _check_frames_route(want, chunking)
         idx, s = self._slot(sum(a.shape[0] for a in arrays))
@@ -210,24 +187,15 @@ class BeatPipeline:
             self.free.append(idx)
             raise
 
-    def submit_wavs(self, paths, infos, sr: int, want: str = "beats", chunking: tuple | None = None):
-        """paths: list of str; infos: ctypes array of bt_wav_info (all `sr` Hz) from bt_wav_probe; chunking as in
+    def submit_wavs(self, paths, infos, sr: int, want: str = "beats", chunking: tuple = DEFAULT_CHUNKING):
+        """paths: list of str; infos: list of bt_wav_info (all `sr` Hz) from _lib.wav_probe; chunking as in
         submit_signals."""
         _check_frames_route(want, chunking)
-        n = len(paths)
-        so = [0]
-        for i in range(n):
-            so.append(so[-1] + int(infos[i].frames))
+        so = _lib.offsets(info.frames for info in infos)
         idx, s = self._slot(so[-1])
         try:
-            cpaths = (ctypes.c_char_p * n)(*[str(p).encode() for p in paths])
-            offs = (ctypes.c_int64 * (n + 1))(*so)
-            status = (ctypes.c_int32 * n)()
             t0 = time.perf_counter()
-            code = self.lib.bt_stage_wav_files(cpaths, infos, n, c_void_p(s.host.data_ptr()), offs, self.host_threads, status)
-            if code != 0:
-                bad = [str(paths[i]) for i in range(n) if status[i] != 0]
-                raise RuntimeError(f"Could not load audio from {bad}")
+            _lib.stage_wav_files(paths, infos, s.host, so, self.host_threads)
             t1 = time.perf_counter()
             self._enqueue(idx, s, so, int(sr), want, chunking)
             self.stats["stage_s"] += t1 - t0

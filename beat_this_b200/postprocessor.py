@@ -22,6 +22,8 @@ from concurrent.futures import ThreadPoolExecutor
 import numpy as np
 import torch
 
+from . import _lib
+
 
 def check_fps(fps) -> None:
     """ValueError unless `fps` is a finite real number > 0 (bools are not frame rates)."""
@@ -75,9 +77,7 @@ class Postprocessor:
             # the reference truncates each piece to its un-padded frames (postprocessor.py:116-117);
             # padding is trailing by construction
             lengths = [int(m.sum()) for m in padding_mask.to(torch.bool).cpu()]
-        fo = [0]
-        for n in lengths:
-            fo.append(fo[-1] + n)
+        fo = _lib.offsets(lengths)
         bcat = torch.cat([beat[i, :n] for i, n in enumerate(lengths)]).contiguous()
         dcat = torch.cat([downbeat[i, :n] for i, n in enumerate(lengths)]).contiguous()
         res = self.batch_cat(bcat, dcat, fo)

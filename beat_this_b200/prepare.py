@@ -16,7 +16,6 @@ does not quantise; and a piece that fails is reported and skipped, at its own co
 from __future__ import annotations
 
 import argparse
-import ctypes
 import os
 import shutil
 import sys
@@ -26,6 +25,7 @@ from pathlib import Path
 import numpy as np
 import torch
 
+from . import _lib
 from .augment import Augmenter, augmentation_dict, precomputed_augmentation_filenames
 from .preprocessing import SAMPLE_RATE, load_audio
 
@@ -69,45 +69,20 @@ def audio_files(paths) -> list:
     return sorted(files, key=lambda f: f.stem)
 
 
-class _Front:
-    """Files -> mono fp32 device audio: WAV files through the native reader (bt_wav_probe / bt_stage_wav_files, the
-    path of File2Beats.batch), anything else through load_audio."""
-
-    def __init__(self, engine, host_threads: int = 8):
-        self.engine, self.lib, self.host_threads = engine, engine.lib, host_threads
-
-    def probe(self, path):
-        from ._lib import bt_wav_info
-
-        info = bt_wav_info()
-        if self.lib.bt_wav_probe(str(path).encode(), ctypes.byref(info)) == 0 and info.frames > 0:
-            return info
-        return None
-
-    def load(self, paths, infos):
-        """One group of equal sample rate: (flat device audio, sample offsets).  infos[i] None: not a plain WAV."""
-        from ._lib import bt_wav_info
-
-        decoded = {i: load_audio(p, dtype="float32")[0] for i, p in enumerate(paths) if infos[i] is None}
-        lens = [int(infos[i].frames) if infos[i] is not None else len(decoded[i]) for i in range(len(paths))]
-        so = [0]
-        for n in lens:
-            so.append(so[-1] + n)
-        host = torch.empty(so[-1], dtype=torch.float32, pin_memory=True)
-        wav = [i for i in range(len(paths)) if infos[i] is not None]
-        if wav:  # file k of the call lands at its own slot so[wav[k]] of host
-            cpaths = (ctypes.c_char_p * len(wav))(*[str(paths[i]).encode() for i in wav])
-            sub = (bt_wav_info * len(wav))(*[infos[i] for i in wav])
-            offs = (ctypes.c_int64 * (len(wav) + 1))(*[so[i] for i in wav], so[-1])
-            status = (ctypes.c_int32 * len(wav))()
-            if self.lib.bt_stage_wav_files(cpaths, sub, len(wav), ctypes.c_void_p(host.data_ptr()), offs, self.host_threads,
-                                           status) != 0:
-                bad = [str(paths[i]) for k, i in enumerate(wav) if status[k] != 0]
-                raise RuntimeError(f"Could not load audio from {bad}")
-        for i, w in decoded.items():
-            w = np.asarray(w, dtype=np.float32)
-            host[so[i] : so[i + 1]] = torch.from_numpy(w if w.ndim == 1 else w.mean(axis=1))
-        return host.to(self.engine.device, non_blocking=True), so
+def _load_group(paths, infos, device, host_threads: int = 8):
+    """Files of one sample rate -> (flat mono fp32 device audio, sample offsets): WAV files through the native reader
+    (_lib.stage_wav_files, the path of File2Beats.batch), anything else (infos[i] None) through load_audio."""
+    decoded = {i: load_audio(p, dtype="float32")[0] for i, p in enumerate(paths) if infos[i] is None}
+    so = _lib.offsets(infos[i].frames if infos[i] is not None else len(decoded[i]) for i in range(len(paths)))
+    host = torch.empty(so[-1], dtype=torch.float32, pin_memory=True)
+    wav = [i for i in range(len(paths)) if infos[i] is not None]
+    if wav:  # file k of the call lands at its own slot so[wav[k]] of host
+        _lib.stage_wav_files([paths[i] for i in wav], [infos[i] for i in wav], host, [so[i] for i in wav] + [so[-1]],
+                             host_threads)
+    for i, w in decoded.items():
+        w = np.asarray(w, dtype=np.float32)
+        host[so[i] : so[i + 1]] = torch.from_numpy(w if w.ndim == 1 else w.mean(axis=1))
+    return host.to(device, non_blocking=True), so
 
 
 def prepare(audio, annotations, out, dataset, pitch_shift=(-5, 6), time_stretch=(20, 4), aug_sr=44100, augment=True,
@@ -126,7 +101,6 @@ def prepare(audio, annotations, out, dataset, pitch_shift=(-5, 6), time_stretch=
     engine = Engine.mel_only(device)
     logmel = LogMelSpect(_engine=engine)
     augmenter = Augmenter(aug_sr, pitch_shift, time_stretch, _engine=engine) if len(names) > 1 else None
-    front = _Front(engine)
     written, skipped = [], {}
 
     def skip(stem, reason):
@@ -142,7 +116,7 @@ def prepare(audio, annotations, out, dataset, pitch_shift=(-5, 6), time_stretch=
 
     def run_group(group, sr):
         """[(path, info)] of one sample rate -> per piece {name: float16 spectrogram}."""
-        audio_dev, so = front.load([p for p, _ in group], [i for _, i in group])
+        audio_dev, so = _load_group([p for p, _ in group], [i for _, i in group], engine.device)
         n = len(group)
         members = [{"track": s} for s in spectrograms(audio_dev, so, sr)]
         if augmenter is not None:
@@ -151,19 +125,19 @@ def prepare(audio, annotations, out, dataset, pitch_shift=(-5, 6), time_stretch=
             variants = augmenter.batch([audio_dev[so[i] : so[i + 1]] for i in range(n)])
             for name in names[1:]:
                 parts = [variants[i][name] for i in range(n)]
-                po = [0]
-                for p in parts:
-                    po.append(po[-1] + p.numel())
+                po = _lib.offsets(p.numel() for p in parts)
                 for i, s in enumerate(spectrograms(torch.cat(parts) if n > 1 else parts[0].contiguous(), po, aug_sr)):
                     members[i][name] = s
         return members
 
     todo = []
-    for f in audio_files(audio):
+    files = audio_files(audio)
+    infos, is_wav = _lib.wav_probe(files)
+    for f, info, ok in zip(files, infos, is_wav):
         if not (ann_in / f"{f.stem}.beats").exists():
             skip(f.stem, f"beat annotation {f.stem}.beats not found")
             continue
-        info = front.probe(f)
+        info = info if ok else None
         try:
             sr = int(info.sample_rate) if info is not None else int(load_audio(f)[1])
         except Exception as e:

@@ -77,17 +77,12 @@ def test_beats_writer_on_the_reference_cli_fixtures(tmp_path):
             assert path.read_bytes() == g[f"{model_name}_text{k}"].tobytes(), (model_name, k)
 
 
-def _stage(lib, arrays, threads=3):
-    from beat_this_b200.pipeline import BeatPipeline
+def _stage(arrays, threads=3):
+    from beat_this_b200 import _lib
 
-    class _E:  # the staging code only needs .lib / .device of an engine
-        pass
-
-    pipe = BeatPipeline.__new__(BeatPipeline)
-    pipe.lib, pipe.host_threads = lib, threads
     n = sum(a.shape[0] for a in arrays)
     dst = torch.zeros(n, dtype=torch.float32)
-    so = BeatPipeline.stage_signals(pipe, arrays, dst)
+    so = _lib.stage_audio(arrays, dst, threads)
     return dst.numpy(), so
 
 
@@ -102,7 +97,7 @@ def test_stage_audio_equals_numpy_mix(lib_built):
             (rng.standard_normal((2500, 2)) * 9000).astype(np.int16), (rng.standard_normal(100) * 9000).astype(np.int16),
             rng.standard_normal((50, 2))[:, ::-1], list(rng.standard_normal(20)), rng.standard_normal((64, 5)).astype(np.float32)]
     arrays = [as_signal_array(s) for s in sigs]
-    got, so = _stage(lib_built, arrays)
+    got, so = _stage(arrays)
     for i, s in enumerate(sigs):
         a = np.asarray(s)
         if a.dtype == np.int16:
@@ -173,14 +168,15 @@ def test_native_wav_front_door_equals_load_audio(lib_built, tmp_path):
     assert lib_built.bt_wav_probe(str(tmp_path / "missing.wav").encode(), ctypes.byref(info)) == -5
 
 
-def test_plan_groups():
+def test_plan_groups_and_padded_frames_known_answers():
     from beat_this_b200.pipeline import plan_groups
 
     assert plan_groups([10] * 5, 25, 64) == [(0, 2), (2, 4), (4, 5)]
     assert plan_groups([100, 1, 1], 25, 64) == [(0, 1), (1, 3)]
     assert plan_groups([1] * 10, 1000, 4) == [(0, 4), (4, 8), (8, 10)]
     assert plan_groups([], 10, 4) == []
-    from beat_this_b200.pipeline import chunk_cost
+    from beat_this_b200.pipeline import padded_frames
 
-    assert [chunk_cost(n) for n in (22050 * 5, 656082, 656083 + 441, 661500, 22050 * 300)] == [1, 1, 2, 2, 11]
-    assert chunk_cost(44100 * 30, 44100) == 2
+    lengths = (22050 * 5, 656082, 656083 + 441, 661500, 22050 * 300)
+    assert [padded_frames(n, 22050, 1500, 6) for n in lengths] == [1500 * k for k in (1, 1, 2, 2, 11)]
+    assert padded_frames(44100 * 30, 44100, 1500, 6) == 2 * 1500

@@ -104,7 +104,7 @@ def test_rope_tables_extend_the_default_bitwise():
 
 
 @pytest.mark.parametrize("chunk", [1501, 3000, 8000])
-def test_chunks_above_the_limit_raise(lib_built, chunk):
+def test_chunks_above_the_limit_raise_and_limits_give_triples(lib_built, chunk):
     """chunking_struct / engine_chunking refuse a chunk_size above the model's limit and name max_chunk_size; at the
     limit they accept it."""
     from beat_this_b200.engine import chunking_struct
@@ -118,7 +118,7 @@ def test_chunks_above_the_limit_raise(lib_built, chunk):
     ck = chunking_struct(chunk, 6, "keep_last", chunk)
     assert (ck.chunk_size, ck.border, ck.overlap_mode) == (chunk, 6, 1)
     assert engine_chunking(chunk, 0, "keep_first", chunk) == (chunk, 0, "keep_first")
-    assert engine_chunking(1500, 6, "keep_first", chunk) is None  # the default keeps the plain entry points
+    assert engine_chunking(1500, 6, "keep_first", chunk) == (1500, 6, "keep_first")
 
 
 @pytest.mark.parametrize("bad", [1499, 0, -1, 384001, 3000.0, "3000", True, None])
@@ -132,9 +132,9 @@ def test_bad_max_chunk_size_raises(bad):
     assert check_max_chunk_size(1500) == 1500 and check_max_chunk_size(np.int64(384000)) == 384000
 
 
-def test_padded_frames_counts_the_planned_chunks(lib_built):
+def test_padded_frames_counts_the_chunks_bt_plan_chunking_max_cuts(lib_built):
     """pipeline.padded_frames: the chunks bt_plan_chunking_max cuts times chunk_size, for clips at 22.05 and 44.1 kHz."""
-    from beat_this_b200.pipeline import chunk_cost, padded_frames
+    from beat_this_b200.pipeline import padded_frames
 
     for n in (441, 661500, 22050 * 61, 22050 * 150, 22050 * 600):
         for sr in (22050, 44100):
@@ -142,4 +142,3 @@ def test_padded_frames_counts_the_planned_chunks(lib_built):
             for c, b in ((3000, 6), (8000, 0), (30001, 0), (1500, 6)):
                 count = _plan(lib_built, T, c, b, 0, 384000)[0]
                 assert padded_frames(n, sr, c, b) == count * c, (n, sr, c, b)
-            assert padded_frames(n, sr, 1500, 6) == chunk_cost(n, sr) * 1500

@@ -96,9 +96,9 @@ def test_reference_logits(small0_ckpt, lib_built, float16):
 
 @pytest.mark.parametrize("float16", [False, True])
 def test_default_chunking_equals_plain_entry_points(small0_ckpt, lib_built, float16):
-    """{1500, 6, keep_first} through bt_spect2frames_chunked / bt_audio2frames_chunked == bt_spect2frames /
-    bt_audio2frames, bitwise, on a ragged batch of more than 128 chunks."""
-    from beat_this_b200 import synthetic
+    """{1500, 6, keep_first} through bt_spect2frames_chunked / bt_audio2frames_chunked (the Engine's route, by default
+    and given explicitly) == bt_spect2frames / bt_audio2frames, bitwise, on a ragged batch of more than 128 chunks."""
+    from beat_this_b200 import _lib, synthetic
     from beat_this_b200.engine import Engine
     from beat_this_b200.inference import Spect2Frames
 
@@ -110,13 +110,20 @@ def test_default_chunking_equals_plain_entry_points(small0_ckpt, lib_built, floa
     audio = torch.from_numpy(np.concatenate(clips)).cuda()
     fo = Engine.frame_offsets(so)
     assert sum(n_chunks(fo[i + 1] - fo[i], 1500, 6, "keep_first") for i in range(len(clips))) > 128
-    b0, d0, fo0 = eng.audio2frames_cat(audio, so)
+    p = eng._dev_ptr
+    b0, d0 = torch.empty(fo[-1], device="cuda:0"), torch.empty(fo[-1], device="cuda:0")
+    _lib.check(eng.lib, eng.ctx, eng.lib.bt_audio2frames(eng.ctx, p(audio), _lib.i64_array(so), len(clips), p(b0), p(d0),
+                                                         _lib.i64_array(fo), eng._stream()))
     b1, d1, fo1 = eng.audio2frames_cat(audio, so, (1500, 6, "keep_first"))
-    assert fo0 == fo1 and torch.equal(b0, b1) and torch.equal(d0, d1)
+    bd, dd, fod = eng.audio2frames_cat(audio, so)
+    assert fo == fo1 == fod and torch.equal(b0, b1) and torch.equal(d0, d1) and torch.equal(b0, bd) and torch.equal(d0, dd)
     spect, _ = eng.logmel_cat(audio, so)
-    b2, d2 = eng.spect2frames_cat(spect, fo)
+    b2, d2 = torch.empty_like(b0), torch.empty_like(d0)
+    _lib.check(eng.lib, eng.ctx, eng.lib.bt_spect2frames(eng.ctx, p(spect), _lib.i64_array(fo), len(clips), p(b2), p(d2),
+                                                         eng._stream()))
     b3, d3 = eng.spect2frames_cat(spect, fo, (1500, 6, "keep_first"))
     assert torch.equal(b2, b3) and torch.equal(d2, d3) and torch.equal(b0, b2) and torch.equal(d0, d2)
+    assert all(torch.equal(a, b) for a, b in zip((b2, d2), eng.spect2frames_cat(spect, fo)))
 
 
 def _write_wav(path, pcm):
@@ -129,8 +136,8 @@ def _write_wav(path, pcm):
 
 def test_frames_batch_equals_spects2frames(small0_ckpt, lib_built, tmp_path):
     """File2Beats.frames_batch with a chunking (native WAV decode, audio2frames route of the pipeline) == the same
-    chunking through spects2frames on the log-mel of the same samples, bitwise; the default keywords keep the plain
-    route."""
+    chunking through spects2frames on the log-mel of the same samples, bitwise; the default keywords are 1500 / 6 /
+    keep_first."""
     from beat_this_b200 import synthetic
     from beat_this_b200.inference import File2Beats
 

@@ -178,7 +178,7 @@ def _profiled(lib, ctx):
     return total
 
 
-def test_bad_tables_are_refused_before_any_launch(engine):
+def test_bad_train_batch_tables_are_refused_before_any_launch(engine):
     lib, ctx = engine.lib, engine.ctx
     rng = np.random.default_rng(3)
     L = 40
@@ -189,11 +189,12 @@ def test_bad_tables_are_refused_before_any_launch(engine):
     i0 = 0  # item 0 has n = L rows
 
     def call(rows=rows, L=L, maps=maps, beats=beats, boff=boff, downs=downs, doff=doff):
-        from beat_this_b200.dataset import _i32, _i64, _ptr
+        from beat_this_b200._lib import i32_array, i64_array
 
-        keep = [_i64(rows), _i64(boff), _i64(doff), _i32(beats), _i32(downs), _i32(maps)]
-        return lib.bt_train_batch(ctx, _ptr(src), keep[0][1], len(rows) - 1, L, keep[5][1], keep[3][1], keep[1][1],
-                                  keep[4][1], keep[2][1], *[_ptr(o) for o in outs], engine._stream())
+        ptr = lambda t: engine._dev_ptr(t, dtype=t.dtype)  # noqa: E731
+        return lib.bt_train_batch(ctx, ptr(src), i64_array(rows), len(rows) - 1, L, i32_array(maps), i32_array(beats),
+                                  i64_array(boff), i32_array(downs), i64_array(doff), *[ptr(o) for o in outs],
+                                  engine._stream())
 
     bad_map = maps.copy()
     bad_map[rows[i0] + 3] = n[i0]  # a source row past the window

@@ -136,7 +136,7 @@ def measure(ds, B, args):
     spect = torch.empty((B, L, 128), dtype=torch.float16, device="cuda:0")
     outs = [torch.empty((B, L), dtype=torch.bool, device="cuda:0") for _ in range(3)]
     eng = tb.engine
-    call = lambda: D.train_batch(eng, dst, s.rows, L, maps, beats, boff, downs, doff, spect, *outs)  # noqa: E731
+    call = lambda: eng.train_batch(dst, s.rows, L, maps, beats, boff, downs, doff, spect, *outs)  # noqa: E731
     for _ in range(20):
         call()
     torch.cuda.synchronize()

@@ -4,7 +4,6 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch
 from beat_this_b200 import _lib
 from beat_this_b200.dbn import DBNDownBeatTracker
-from beat_this_b200.pipeline import BeatPipeline
 
 d = DBNDownBeatTracker(beats_per_bar=[3, 4], min_bpm=55.0, max_bpm=215.0, fps=50, transition_lambda=100)
 acts = []
@@ -21,17 +20,14 @@ for nt in (8, 16, 32, 64, 128):
         t0 = time.perf_counter(); d.batch(acts, nt); ts.append(time.perf_counter() - t0)
     print("dbn 64 pieces, %3d threads: %.1f ms (best of 3)" % (nt, 1e3 * min(ts)))
 
-lib = _lib.load()
-pipe = BeatPipeline.__new__(BeatPipeline); pipe.lib = lib
 rng = np.random.default_rng(0)
 clips64 = [rng.standard_normal(661500) for _ in range(64)]
 clips32 = [c.astype(np.float32) for c in clips64]
 dst = torch.empty(64 * 661500, dtype=torch.float32, pin_memory=torch.cuda.is_available())
 for name, clips in (("float64", clips64), ("float32", clips32)):
     for nt in (4, 8, 16, 32, 64):
-        pipe.host_threads = nt
-        BeatPipeline.stage_signals(pipe, clips, dst)
+        _lib.stage_audio(clips, dst, nt)
         ts = []
         for _ in range(3):
-            t0 = time.perf_counter(); BeatPipeline.stage_signals(pipe, clips, dst); ts.append(time.perf_counter() - t0)
+            t0 = time.perf_counter(); _lib.stage_audio(clips, dst, nt); ts.append(time.perf_counter() - t0)
         print("stage 64 x 30 s %s, %2d threads: %.1f ms" % (name, nt, 1e3 * min(ts)))
