@@ -17,8 +17,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 # BT_LIB_PATH: an instrumented build of the same sources (e.g. build(extra_flags=("-DBT_FF_PROF",), out_path=...))
 LIB_PATH = os.environ.get("BT_LIB_PATH") or os.path.join(HERE, "libbeatthis_sm90.so")
-SOURCES = ["bt_api.cu", "api_signal.cu", "api_post.cu", "api_data.cu", "api_debug.cu", "kernels_simt.cu", "kernels_misc.cu", "kernels_gemm.cu", "kernels_attn.cu", "kernels_fused.cu", "kernels_dbn.cu", "kernels_eval.cu", "kernels_loss.cu", "kernels_augment.cu", "kernels_data.cu", "dbn_host.cpp", "host_stage.cpp"]
-HEADERS = ["common.cuh", "epilogue.cuh", "fft.cuh", "tc_common.cuh", "bt_kernels.h", "cuda_owned.h", "dbn_model.h",
+SOURCES = ["bt_api.cu", "api_signal.cu", "api_post.cu", "api_data.cu", "api_train.cu", "api_debug.cu", "kernels_simt.cu", "kernels_misc.cu", "kernels_gemm.cu", "kernels_attn.cu", "kernels_fused.cu", "kernels_dbn.cu", "kernels_eval.cu", "kernels_loss.cu", "kernels_augment.cu", "kernels_data.cu", "kernels_train.cu", "dbn_host.cpp", "host_stage.cpp"]
+HEADERS = ["common.cuh", "epilogue.cuh", "fft.cuh", "tc_common.cuh", "bt_kernels.h", "bt_train.h", "cuda_owned.h", "dbn_model.h",
            "api_internal.h", os.path.join("..", "..", "include", "beatthis.h")]
 
 BT_DTYPE_F32 = 0
@@ -227,6 +227,23 @@ PROTOTYPES = {
         [c_void_p, c_void_p, POINTER(c_int64), c_int32, c_int32, POINTER(c_int32), POINTER(c_int32), POINTER(c_int64),
          POINTER(c_int32), POINTER(c_int64), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p],
     ),
+    "bt_train_param_count": (c_int32, [POINTER(bt_hparams)]),
+    "bt_train_param_info": (
+        c_int, [POINTER(bt_hparams), c_int32, c_char_p, c_int32, POINTER(c_int64), POINTER(c_int32), POINTER(c_int32)],
+    ),
+    "bt_train_activation_bytes": (c_int64, [c_void_p, c_int32, c_int32]),
+    "bt_train_forward": (
+        c_int, [c_void_p, POINTER(c_void_p), c_int32, c_void_p, c_int32, c_int32, c_void_p, c_int64, c_void_p, c_void_p,
+                c_void_p],
+    ),
+    "bt_train_backward": (
+        c_int, [c_void_p, POINTER(c_void_p), c_int32, c_void_p, c_int64, c_int32, c_int32, c_void_p, c_void_p,
+                POINTER(c_void_p), c_void_p, c_void_p],
+    ),
+    "bt_debug_attention_backward": (
+        c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p,
+                c_void_p],
+    ),
     "bt_spect2frames": (c_int, [c_void_p, c_void_p, POINTER(c_int64), c_int32, c_void_p, c_void_p, c_void_p]),
     "bt_forward_chunks": (c_int, [c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_void_p]),
     "bt_audio2frames": (
@@ -306,6 +323,37 @@ _lib = None
 OBJ_DIR = os.path.join(CSRC, "_obj")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = [*ARCH, "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC"]
+
+
+def hparams_struct(hp: dict) -> bt_hparams:
+    """The bt_hparams of a BeatThis hyper-parameter dict (the reference's defaults for missing entries)."""
+    return bt_hparams(
+        int(hp.get("spect_dim", 128)),
+        int(hp.get("transformer_dim", 512)),
+        int(hp.get("ff_mult", 4)),
+        int(hp.get("n_layers", 6)),
+        int(hp.get("head_dim", 32)),
+        int(hp.get("stem_dim", 32)),
+        int(bool(hp.get("sum_head", True))),
+        int(bool(hp.get("partial_transformers", True))),
+    )
+
+
+def train_param_table(hp: dict) -> list[tuple[str, tuple, bool]]:
+    """bt_train_param_info of every entry: (state_dict name, shape, takes a gradient), in the table's order."""
+    lib = load()
+    chp = hparams_struct(hp)
+    n = lib.bt_train_param_count(ctypes.byref(chp))
+    if n < 0:
+        raise ValueError(f"bt_train_param_count refused {hp}")
+    name, shape, ndim, trainable = ctypes.create_string_buffer(256), (c_int64 * 4)(), c_int32(), c_int32()
+    table = []
+    for i in range(n):
+        code = lib.bt_train_param_info(ctypes.byref(chp), i, name, 256, shape, ctypes.byref(ndim), ctypes.byref(trainable))
+        if code != 0:
+            raise RuntimeError(f"bt_train_param_info({i}) returned {code}")
+        table.append((name.value.decode(), tuple(shape[: ndim.value]), bool(trainable.value)))
+    return table
 
 
 def _nvcc() -> str:

@@ -1,6 +1,7 @@
 // C ABI (include/beatthis.h): the kernel test hooks (bt_debug_*).  Each checks its own arguments, then runs the
 // kernel under test once through run_hook (api_internal.h).
 #include "api_internal.h"
+#include "bt_train.h"
 
 static bool aligned16(const void* p) { return reinterpret_cast<uintptr_t>(p) % 16 == 0; }
 
@@ -314,6 +315,46 @@ int bt_debug_head(bt_ctx* c, const float* x_dev, int32_t D, const float* w_dev, 
   }
   return run_chunk_hook(c, fn, "head", chunks_host, n_chunks, stream, [&](const ChunkSrc* t, cudaStream_t st) {
     launch_head(x_dev, D, w_dev, b_dev, t, n_chunks, L, beat_dev, down_dev, sum_head ? 1 : 0, st);
+  });
+}
+
+int bt_debug_attention_backward(bt_ctx* c, const float* qkv_dev, const float* gates_dev, const float* freqs_dev,
+                                const float* dy_dev, int32_t seqs, int32_t n, int32_t heads, float* y_dev,
+                                float* dqkv_dev, float* dgates_dev, void* stream) {
+  const char* fn = "bt_debug_attention_backward";
+  if (!c) return BT_ERR_ARG;
+  if (c->dtype != BT_DTYPE_F32) return fail(c, BT_ERR_ARG, "%s: the training kernels run on a BT_DTYPE_F32 context", fn);
+  if (!qkv_dev || !gates_dev || !freqs_dev || !dy_dev || !y_dev || !dqkv_dev || !dgates_dev)
+    return fail(c, BT_ERR_ARG, "%s: null argument", fn);
+  if (seqs < 1 || n < 1 || heads < 1 || heads > 32 || int64_t{seqs} * n > kMaxChunkCap)
+    return fail(c, BT_ERR_ARG, "%s: bad geometry", fn);
+  const int C = heads * 32;
+  const int64_t M = int64_t{seqs} * n;
+  const TrSeqs q{seqs, n, heads, 1, n, 0, 1};
+  DeviceBuffer<float> qkv, o, dg, lse, delta;
+  return run_hook(c, fn, stream, {}, [&](cudaStream_t st) {
+    BT_CUDA(c, qkv.alloc(M * 3 * C * sizeof(float)));
+    BT_CUDA(c, o.alloc(M * C * sizeof(float)));
+    BT_CUDA(c, dg.alloc(M * C * sizeof(float)));
+    BT_CUDA(c, lse.alloc(M * heads * sizeof(float)));
+    BT_CUDA(c, delta.alloc(M * heads * sizeof(float)));
+    BT_CUDA(c, cudaMemcpyAsync(qkv.get(), qkv_dev, M * 3 * C * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    BT_CUDA(c, cudaMemcpyAsync(dg.get(), dy_dev, M * C * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    launch_tr_rope(qkv.get(), freqs_dev, M, C, n, 1, 0, false, st);
+    BT_LAUNCHED(c, "train_rope", st);
+    launch_tr_attn_fwd(qkv.get(), q, o.get(), lse.get(), st);
+    BT_LAUNCHED(c, "train_attention", st);
+    launch_tr_gate_fwd(o.get(), gates_dev, M, C, y_dev, st);
+    BT_LAUNCHED(c, "train_gate", st);
+    launch_tr_gate_bwd(dg.get(), o.get(), gates_dev, M, C, dgates_dev, delta.get(), st);
+    BT_LAUNCHED(c, "train_gate_bwd", st);
+    launch_tr_attn_dq(qkv.get(), dg.get(), lse.get(), delta.get(), q, dqkv_dev, st);
+    BT_LAUNCHED(c, "train_attention_dq", st);
+    launch_tr_attn_dkv(qkv.get(), dg.get(), lse.get(), delta.get(), q, dqkv_dev, st);
+    BT_LAUNCHED(c, "train_attention_dkv", st);
+    launch_tr_rope(dqkv_dev, freqs_dev, M, C, n, 1, 0, true, st);
+    BT_LAUNCHED(c, "train_rope", st);
+    return BT_OK;
   });
 }
 

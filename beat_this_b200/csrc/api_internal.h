@@ -1,4 +1,4 @@
-// Private to the C ABI's host files (bt_api.cu, api_signal.cu, api_post.cu, api_data.cu, api_debug.cu): bt_ctx, the entry prologue
+// Private to the C ABI's host files (bt_api.cu, api_signal.cu, api_post.cu, api_data.cu, api_train.cu, api_debug.cu): bt_ctx, the entry prologue
 // and argument checks, errors and launch checks, the staging ring, plan slots and the test-hook harness.
 #pragma once
 #include <algorithm>
@@ -92,6 +92,8 @@ struct bt_ctx {
   DeviceBuffer<uint8_t> dbn_bp;
   // per-CTA partial sums of bt_beat_loss (grows on demand)
   DeviceBuffer<double> loss_partials;
+  // scratch of bt_train_forward / bt_train_backward (grows on demand)
+  DeviceBuffer<float> train_ws;
   // windowed inverse transforms of bt_istft's frames, n_fft floats each (grows on demand)
   DeviceBuffer<float> istft_frames;
   // pinned staging + device tables

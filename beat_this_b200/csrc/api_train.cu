@@ -1,0 +1,498 @@
+// The training entry points: bt_train_param_count / _info (the reference's state_dict as a table),
+// bt_train_activation_bytes, bt_train_forward and bt_train_backward.  Parameters are the caller's unfolded fp32 device
+// tensors; the forward pass saves what the backward pass reads in the caller's activation store.
+#include "api_internal.h"
+#include "bt_train.h"
+#include "common.cuh"
+
+namespace {
+
+struct TrParam {
+  std::string name;
+  int ndim;
+  int64_t shape[4];
+  bool trainable;
+};
+
+// One step of the model.  p: table index of the step's first parameter.  Offsets (in floats) into the activation
+// store; -1 where the step saves nothing there.
+enum TrKind { kStem, kAttnFreq, kAttnTime, kFfn, kConvBlock, kLinear, kHead };
+struct TrLayer {
+  TrKind kind;
+  int p;
+  int C, F, mult;  // channels, frequency planes, FFN multiplier
+  int64_t in = -1, xn = -1, inv = -1, qkv = -1, gate = -1, lse = -1, o = -1, h = -1, a = -1, z = -1, xl = -1;
+};
+
+struct TrModel {
+  std::vector<TrParam> table;
+  std::vector<TrLayer> layers;
+  int64_t floats = 0;  // activation store
+};
+
+void add(std::vector<TrParam>& t, const std::string& name, std::initializer_list<int64_t> shape, bool trainable = true) {
+  TrParam p{name, static_cast<int>(shape.size()), {1, 1, 1, 1}, trainable};
+  int i = 0;
+  for (int64_t s : shape) p.shape[i++] = s;
+  t.push_back(p);
+}
+void add_bn(std::vector<TrParam>& t, const std::string& p, int n) {
+  add(t, p + ".weight", {n});
+  add(t, p + ".bias", {n});
+  add(t, p + ".running_mean", {n}, false);
+  add(t, p + ".running_var", {n}, false);
+  add(t, p + ".num_batches_tracked", {}, false);
+}
+// table order of an attention: rotary_embed.freqs, norm.gamma, to_qkv.weight, to_gates.weight, to_gates.bias,
+// to_out.0.weight; of a feed-forward: net.0.gamma, net.1.weight, net.1.bias, net.4.weight, net.4.bias
+void add_attn(std::vector<TrParam>& t, const std::string& p, int C) {
+  add(t, p + ".rotary_embed.freqs", {16}, false);
+  add(t, p + ".norm.gamma", {C});
+  add(t, p + ".to_qkv.weight", {3 * C, C});
+  add(t, p + ".to_gates.weight", {C / 32, C});
+  add(t, p + ".to_gates.bias", {C / 32});
+  add(t, p + ".to_out.0.weight", {C, C});
+}
+void add_ffn(std::vector<TrParam>& t, const std::string& p, int C, int mult) {
+  add(t, p + ".net.0.gamma", {C});
+  add(t, p + ".net.1.weight", {mult * C, C});
+  add(t, p + ".net.1.bias", {mult * C});
+  add(t, p + ".net.4.weight", {C, mult * C});
+  add(t, p + ".net.4.bias", {C});
+}
+
+// The parameter table in BeatThis.state_dict() order and, for a batch of B x L frames (B = 0: table only), the steps
+// and their activation store.  Token rows of the frontend: ((b F + f) L + t), C channels.
+TrModel train_model(const bt_hparams& hp, int64_t B, int64_t L) {
+  TrModel m;
+  auto& t = m.table;
+  const int64_t BL = B * L;
+  auto alloc = [&](int64_t n) {
+    const int64_t off = m.floats;
+    m.floats += (n + 3) & ~int64_t{3};
+    return off;
+  };
+  auto attn = [&](TrKind kind, const std::string& p, int C, int F) {
+    TrLayer l{kind, static_cast<int>(t.size()), C, F, 0};
+    add_attn(t, p, C);
+    const int64_t M = BL * F;
+    l.in = alloc(M * C), l.xn = alloc(M * C), l.inv = alloc(M), l.qkv = alloc(3 * M * C), l.gate = alloc(M * C / 32);
+    l.lse = alloc(M * C / 32), l.o = alloc(M * C);
+    m.layers.push_back(l);
+  };
+  auto ffn = [&](const std::string& p, int C, int F, int mult) {
+    TrLayer l{kFfn, static_cast<int>(t.size()), C, F, mult};
+    add_ffn(t, p, C, mult);
+    const int64_t M = BL * F;
+    l.in = alloc(M * C), l.xn = alloc(M * C), l.inv = alloc(M), l.h = alloc(M * mult * C), l.a = alloc(M * mult * C);
+    m.layers.push_back(l);
+  };
+  {
+    TrLayer l{kStem, static_cast<int>(t.size()), hp.stem_dim, hp.spect_dim / 4, 0};
+    add_bn(t, "frontend.stem.bn1d", hp.spect_dim);
+    add(t, "frontend.stem.conv2d.weight", {hp.stem_dim, 1, 4, 3});
+    add_bn(t, "frontend.stem.bn2d", hp.stem_dim);
+    l.in = alloc(BL * hp.spect_dim), l.z = alloc(BL * l.F * l.C);
+    m.layers.push_back(l);
+  }
+  int C = hp.stem_dim, F = hp.spect_dim / 4;
+  for (int i = 0; i < 3; ++i) {
+    const std::string p = "frontend.blocks." + std::to_string(i);
+    if (hp.partial_transformers) {
+      attn(kAttnFreq, p + ".partial.attnF", C, F);
+      ffn(p + ".partial.ffF", C, F, 4);
+      attn(kAttnTime, p + ".partial.attnT", C, F);
+      ffn(p + ".partial.ffT", C, F, 4);
+    }
+    TrLayer l{kConvBlock, static_cast<int>(t.size()), C, F, 0};
+    add(t, p + ".conv2d.weight", {2 * C, C, 2, 3});
+    add_bn(t, p + ".norm", 2 * C);
+    l.in = alloc(BL * F * C), l.z = alloc(BL * F / 2 * 2 * C);
+    m.layers.push_back(l);
+    C *= 2;
+    F /= 2;
+  }
+  const int D = hp.transformer_dim;
+  {
+    TrLayer l{kLinear, static_cast<int>(t.size()), C, F, 0};
+    add(t, "frontend.linear.weight", {D, C * F});
+    add(t, "frontend.linear.bias", {D});
+    l.in = alloc(BL * F * C), l.xl = alloc(BL * F * C);
+    m.layers.push_back(l);
+  }
+  for (int i = 0; i < hp.n_layers; ++i) {
+    const std::string p = "transformer_blocks.layers." + std::to_string(i);
+    attn(kAttnTime, p + ".0", D, 1);
+    ffn(p + ".1", D, 1, hp.ff_mult);
+  }
+  {
+    TrLayer l{kHead, static_cast<int>(t.size()), D, 1, 0};
+    add(t, "transformer_blocks.norm.gamma", {D});
+    add(t, "task_heads.beat_downbeat_lin.weight", {2, D});
+    add(t, "task_heads.beat_downbeat_lin.bias", {2});
+    l.in = alloc(BL * D), l.xn = alloc(BL * D), l.inv = alloc(BL);
+    m.layers.push_back(l);
+  }
+  return m;
+}
+
+// Scratch of one call, in floats: the stream gradient, the im2col / FFN-hidden buffer, two [tokens, channels] buffers,
+// q/k/v gradients, per-head rows, and split-K / column-sum partials.
+constexpr int64_t kPartFloats = int64_t{8} << 20;
+struct TrScratch {
+  float *dcur, *big, *s1, *s2, *dqkv, *hd1, *hd2, *part;
+};
+int64_t scratch_floats(int64_t BL) {
+  // widest per frame: 1024 channels of tokens (every frontend stage: F C <= 32 * 32 ... 4 * 256; the main layers:
+  // D <= 1024), 4096 for the FFN hidden (4 * 32 * 32, or ff_mult D) and the convolutions' im2col (3 * 2 * C * F), 32
+  // per-head values (F heads <= 32 in the frontend, D / 32 in the main layers); and one value per channel, at least, for
+  // the column sums of the BatchNorm gradients
+  return BL * (3 * 1024 + 4096 + 3 * 1024 + 2 * 32) + 2 * 1024 + kPartFloats;
+}
+
+struct TrRun {
+  bt_ctx* c;
+  cudaStream_t st;
+  const float* const* P;  // parameters, table order
+  float* const* G;        // gradients, table order (backward)
+  float* act;
+  TrScratch s;
+  int B, L;
+  const float *dbeat, *ddown;  // backward: the gradient at the logits
+  const float* w(int i) const { return P[i]; }
+  float* at(int64_t off) const { return act + off; }
+  TrBn bn(int p) const { return TrBn{P[p], P[p + 1], P[p + 2], P[p + 3]}; }
+
+  // out[M, N] = X[M, K] W[N, K]^T (+ bias) (+ resid) (gelu_out: GELU of it as well)
+  int linear(const float* X, int64_t M, int K, const float* W, int N, const float* bias, float* out,
+             const float* resid = nullptr, float* gelu_out = nullptr) {
+    launch_tr_gemm({X, K, 1}, {W, K, 1}, {out, N, 0, bias, resid, N, gelu_out}, static_cast<int>(M), N, K, 1, st);
+    return check_launch(c, "train_gemm", st);
+  }
+  // dX[M, K] = dY[M, N] W[N, K] (+ resid)
+  int grad_input(const float* dY, int64_t M, int N, const float* W, int K, float* dX, const float* resid = nullptr) {
+    launch_tr_gemm({dY, N, 1}, {W, 1, K}, {dX, K, 0, nullptr, resid, K, nullptr}, static_cast<int>(M), K, N, 1, st);
+    return check_launch(c, "train_gemm_dx", st);
+  }
+  // dW[N, K] = dY[M, N]^T X[M, K], split over M with a fixed-order reduction; dW null: not wanted
+  int grad_weight(const float* dY, int64_t M, int N, const float* X, int K, float* dW) {
+    if (!dW) return BT_OK;
+    const int64_t tiles = int64_t{ceil_div(N, 64)} * ceil_div(K, 64);
+    int64_t splits = std::min<int64_t>(ceil_div64(2 * 132, tiles), std::max<int64_t>(1, M / 256));
+    splits = std::max<int64_t>(1, std::min<int64_t>(splits, kPartFloats / (int64_t{N} * K)));
+    const int parts = tr_gemm_parts(static_cast<int>(M), static_cast<int>(splits));
+    launch_tr_gemm({dY, 1, N}, {X, 1, K}, {parts > 1 ? s.part : dW, K, int64_t{N} * K, nullptr, nullptr, 0, nullptr}, N,
+                   K, static_cast<int>(M), static_cast<int>(splits), st);
+    if (const int r = check_launch(c, "train_gemm_dw", st)) return r;
+    if (parts == 1) return BT_OK;
+    launch_tr_reduce(s.part, parts, int64_t{N} * K, 1.f, dW, st);
+    return check_launch(c, "train_reduce", st);
+  }
+  // out[n] = scale sum_m A[m, n] (B[m, n]) (rs[m])
+  int colsum(const float* A, const float* Bm, const float* rs, int64_t M, int N, float scale, float* out) {
+    if (!out) return BT_OK;
+    const int parts = launch_tr_colsum(A, Bm, rs, M, N, static_cast<int>(std::min<int64_t>(
+                                                            ceil_div64(M, 512), kPartFloats / N)), s.part, st);
+    if (const int r = check_launch(c, "train_colsum", st)) return r;
+    launch_tr_reduce(s.part, parts, N, scale, out, st);
+    return check_launch(c, "train_reduce", st);
+  }
+  TrSeqs seqs(const TrLayer& l) const {
+    const int heads = l.C / 32;
+    if (l.kind == kAttnFreq) return {B * L, l.F, heads, L, int64_t{l.F} * L, 1, L};  // sequences (b, t) over f
+    return {B * l.F, L, heads, 1, L, 0, 1};                                       // sequences (b, f) over t
+  }
+  TrImg img(const TrLayer& l) const {
+    if (l.kind == kStem) return {B, l.F, 4, L, 1, int64_t{L} * 4 * l.F, 1, 4 * l.F, 0};  // the [B, L, 128] input
+    return {B, l.F / 2, 2, L, l.C, int64_t{l.F} * L * l.C, int64_t{L} * l.C, l.C, 1};
+  }
+};
+
+#define TR_OK(x)                 \
+  do {                           \
+    const int _r = (x);          \
+    if (_r != BT_OK) return _r;  \
+  } while (0)
+
+// Each step reads l.in and writes the next step's in (the head: the logits).
+int forward_layer(TrRun& R, const TrLayer& l, float* next, float* beat, float* down) {
+  const cudaStream_t st = R.st;
+  bt_ctx* c = R.c;
+  const int64_t M = int64_t{R.B} * R.L * l.F;
+  const int C = l.C, p = l.p;
+  switch (l.kind) {
+    case kStem: {
+      const TrImg g = R.img(l);
+      const TrBn bn1 = R.bn(p);
+      launch_tr_im2col(R.at(l.in), g, &bn1, R.s.big, st);
+      BT_LAUNCHED(c, "train_im2col", st);
+      TR_OK(R.linear(R.s.big, M, 12, R.w(p + 5), C, nullptr, R.at(l.z)));
+      launch_tr_bn_gelu_fwd(R.at(l.z), R.bn(p + 6), M * C, C, next, st);
+      BT_LAUNCHED(c, "train_bn_gelu", st);
+      return BT_OK;
+    }
+    case kAttnFreq:
+    case kAttnTime: {
+      const int heads = C / 32;
+      launch_tr_rms_fwd(R.at(l.in), R.w(p + 1), M, C, R.at(l.xn), R.at(l.inv), st);
+      BT_LAUNCHED(c, "train_rmsnorm", st);
+      TR_OK(R.linear(R.at(l.xn), M, C, R.w(p + 2), 3 * C, nullptr, R.at(l.qkv)));
+      TR_OK(R.linear(R.at(l.xn), M, C, R.w(p + 3), heads, R.w(p + 4), R.at(l.gate)));
+      launch_tr_rope(R.at(l.qkv), R.w(p), M, C, R.L, l.F, l.kind == kAttnFreq, false, st);
+      BT_LAUNCHED(c, "train_rope", st);
+      launch_tr_attn_fwd(R.at(l.qkv), R.seqs(l), R.at(l.o), R.at(l.lse), st);
+      BT_LAUNCHED(c, "train_attention", st);
+      launch_tr_gate_fwd(R.at(l.o), R.at(l.gate), M, C, R.s.s1, st);
+      BT_LAUNCHED(c, "train_gate", st);
+      return R.linear(R.s.s1, M, C, R.w(p + 5), C, nullptr, next, R.at(l.in));
+    }
+    case kFfn: {
+      launch_tr_rms_fwd(R.at(l.in), R.w(p), M, C, R.at(l.xn), R.at(l.inv), st);
+      BT_LAUNCHED(c, "train_rmsnorm", st);
+      TR_OK(R.linear(R.at(l.xn), M, C, R.w(p + 1), l.mult * C, R.w(p + 2), R.at(l.h), nullptr, R.at(l.a)));
+      return R.linear(R.at(l.a), M, l.mult * C, R.w(p + 3), C, R.w(p + 4), next, R.at(l.in));
+    }
+    case kConvBlock: {
+      const TrImg g = R.img(l);
+      const int64_t Mo = M / 2;
+      launch_tr_im2col(R.at(l.in), g, nullptr, R.s.big, st);
+      BT_LAUNCHED(c, "train_im2col", st);
+      TR_OK(R.linear(R.s.big, Mo, 6 * C, R.w(p), 2 * C, nullptr, R.at(l.z)));
+      launch_tr_bn_gelu_fwd(R.at(l.z), R.bn(p + 1), Mo * 2 * C, 2 * C, next, st);
+      BT_LAUNCHED(c, "train_bn_gelu", st);
+      return BT_OK;
+    }
+    case kLinear: {
+      launch_tr_concat(R.at(l.in), R.B, l.F, R.L, C, false, R.at(l.xl), st);
+      BT_LAUNCHED(c, "train_concat", st);
+      return R.linear(R.at(l.xl), int64_t{R.B} * R.L, C * l.F, R.w(p), c->hp.transformer_dim, R.w(p + 1), next);
+    }
+    case kHead: {
+      launch_tr_rms_fwd(R.at(l.in), R.w(p), M, C, R.at(l.xn), R.at(l.inv), st);
+      BT_LAUNCHED(c, "train_rmsnorm", st);
+      TR_OK(R.linear(R.at(l.xn), M, C, R.w(p + 1), 2, R.w(p + 2), R.s.s1));
+      launch_tr_head_fwd(R.s.s1, M, c->hp.sum_head, beat, down, st);
+      BT_LAUNCHED(c, "train_head", st);
+      return BT_OK;
+    }
+  }
+  return BT_OK;
+}
+
+// RMSNorm backward of a residual branch: dcur += d(branch)/d(input) from dxn; gamma's gradient.
+int rms_backward(TrRun& R, const TrLayer& l, int gamma, const float* dxn, int64_t M, bool add) {
+  launch_tr_rms_bwd(dxn, R.at(l.in), R.at(l.inv), R.w(gamma), M, l.C, add, R.s.dcur, R.st);
+  BT_LAUNCHED(R.c, "train_rmsnorm_bwd", R.st);
+  return R.colsum(dxn, R.at(l.in), R.at(l.inv), M, l.C, sqrtf(static_cast<float>(l.C)), R.G[gamma]);
+}
+
+// s.dcur holds the gradient at the step's output; on return, at its input.
+int backward_layer(TrRun& R, const TrLayer& l, float* dspect) {
+  const cudaStream_t st = R.st;
+  bt_ctx* c = R.c;
+  const int64_t M = int64_t{R.B} * R.L * l.F;
+  const int C = l.C, p = l.p;
+  float* const* G = R.G;
+  const TrScratch& s = R.s;
+  switch (l.kind) {
+    case kHead: {
+      launch_tr_head_bwd(R.dbeat, R.ddown, M, c->hp.sum_head, s.s1, st);
+      BT_LAUNCHED(c, "train_head", st);
+      TR_OK(R.grad_weight(s.s1, M, 2, R.at(l.xn), C, G[p + 1]));
+      TR_OK(R.colsum(s.s1, nullptr, nullptr, M, 2, 1.f, G[p + 2]));
+      TR_OK(R.grad_input(s.s1, M, 2, R.w(p + 1), C, s.s2));
+      return rms_backward(R, l, p, s.s2, M, false);
+    }
+    case kAttnFreq:
+    case kAttnTime: {
+      const int heads = C / 32;
+      launch_tr_gate_fwd(R.at(l.o), R.at(l.gate), M, C, s.s1, st);
+      BT_LAUNCHED(c, "train_gate", st);
+      TR_OK(R.grad_weight(s.dcur, M, C, s.s1, C, G[p + 5]));
+      TR_OK(R.grad_input(s.dcur, M, C, R.w(p + 5), C, s.s2));
+      launch_tr_gate_bwd(s.s2, R.at(l.o), R.at(l.gate), M, C, s.hd1, s.hd2, st);
+      BT_LAUNCHED(c, "train_gate_bwd", st);
+      const TrSeqs q = R.seqs(l);
+      launch_tr_attn_dq(R.at(l.qkv), s.s2, R.at(l.lse), s.hd2, q, s.dqkv, st);
+      BT_LAUNCHED(c, "train_attention_dq", st);
+      launch_tr_attn_dkv(R.at(l.qkv), s.s2, R.at(l.lse), s.hd2, q, s.dqkv, st);
+      BT_LAUNCHED(c, "train_attention_dkv", st);
+      launch_tr_rope(s.dqkv, R.w(p), M, C, R.L, l.F, l.kind == kAttnFreq, true, st);
+      BT_LAUNCHED(c, "train_rope", st);
+      TR_OK(R.grad_weight(s.dqkv, M, 3 * C, R.at(l.xn), C, G[p + 2]));
+      TR_OK(R.grad_weight(s.hd1, M, heads, R.at(l.xn), C, G[p + 3]));
+      TR_OK(R.colsum(s.hd1, nullptr, nullptr, M, heads, 1.f, G[p + 4]));
+      TR_OK(R.grad_input(s.dqkv, M, 3 * C, R.w(p + 2), C, s.s1));
+      TR_OK(R.grad_input(s.hd1, M, heads, R.w(p + 3), C, s.s1, s.s1));
+      return rms_backward(R, l, p + 1, s.s1, M, true);
+    }
+    case kFfn: {
+      const int H = l.mult * C;
+      TR_OK(R.grad_weight(s.dcur, M, C, R.at(l.a), H, G[p + 3]));
+      TR_OK(R.colsum(s.dcur, nullptr, nullptr, M, C, 1.f, G[p + 4]));
+      TR_OK(R.grad_input(s.dcur, M, C, R.w(p + 3), H, s.big));
+      launch_tr_gelu_bwd(s.big, R.at(l.h), M * H, s.big, st);
+      BT_LAUNCHED(c, "train_gelu_bwd", st);
+      TR_OK(R.grad_weight(s.big, M, H, R.at(l.xn), C, G[p + 1]));
+      TR_OK(R.colsum(s.big, nullptr, nullptr, M, H, 1.f, G[p + 2]));
+      TR_OK(R.grad_input(s.big, M, H, R.w(p + 1), C, s.s1));
+      return rms_backward(R, l, p, s.s1, M, true);
+    }
+    case kLinear: {
+      const int64_t BL = int64_t{R.B} * R.L;
+      const int D = c->hp.transformer_dim, K = C * l.F;
+      TR_OK(R.grad_weight(s.dcur, BL, D, R.at(l.xl), K, G[p]));
+      TR_OK(R.colsum(s.dcur, nullptr, nullptr, BL, D, 1.f, G[p + 1]));
+      TR_OK(R.grad_input(s.dcur, BL, D, R.w(p), K, s.s1));
+      launch_tr_concat(s.s1, R.B, l.F, R.L, C, true, s.dcur, st);
+      BT_LAUNCHED(c, "train_concat", st);
+      return BT_OK;
+    }
+    case kConvBlock:
+    case kStem: {
+      // the convolution's output: Mo rows of Co channels, K = Ci S 3 columns of im2col
+      const bool stem = l.kind == kStem;
+      const TrImg g = R.img(l);
+      const int Co = stem ? C : 2 * C, K = g.C * g.S * 3, bn2 = stem ? p + 6 : p + 1, wc = stem ? p + 5 : p;
+      const int64_t Mo = int64_t{g.B} * g.Fo * g.L;
+      const TrBn b2 = R.bn(bn2), b1 = R.bn(p);
+      launch_tr_bn_gelu_bwd(s.dcur, R.at(l.z), b2, Mo * Co, Co, s.s1, s.s2, st);  // s1: at the BatchNorm, s2: at z
+      BT_LAUNCHED(c, "train_bn_gelu_bwd", st);
+      TR_OK(R.colsum(s.s1, R.at(l.z), nullptr, Mo, Co, 1.f, s.hd1));
+      TR_OK(R.colsum(s.s1, nullptr, nullptr, Mo, Co, 1.f, s.hd2));
+      launch_tr_bn_grads(s.hd1, s.hd2, b2, Co, G[bn2], G[bn2 + 1], st);
+      BT_LAUNCHED(c, "train_bn_grads", st);
+      launch_tr_im2col(R.at(l.in), g, stem ? &b1 : nullptr, s.big, st);
+      BT_LAUNCHED(c, "train_im2col", st);
+      TR_OK(R.grad_weight(s.s2, Mo, Co, s.big, K, G[wc]));
+      if (stem && !dspect && !G[p] && !G[p + 1]) return BT_OK;
+      TR_OK(R.grad_input(s.s2, Mo, Co, R.w(wc), K, s.big));
+      launch_tr_col2im(s.big, g, stem ? s.s1 : s.dcur, st);  // the stem: the gradient at the 1-d BatchNorm's output
+      BT_LAUNCHED(c, "train_col2im", st);
+      if (!stem) return BT_OK;
+      const int64_t BL = int64_t{R.B} * R.L;
+      const int Fs = c->hp.spect_dim;
+      TR_OK(R.colsum(s.s1, R.at(l.in), nullptr, BL, Fs, 1.f, s.hd1));
+      TR_OK(R.colsum(s.s1, nullptr, nullptr, BL, Fs, 1.f, s.hd2));
+      launch_tr_bn_grads(s.hd1, s.hd2, b1, Fs, G[p], G[p + 1], st);
+      BT_LAUNCHED(c, "train_bn_grads", st);
+      if (!dspect) return BT_OK;
+      launch_tr_bn_scale(s.s1, b1, BL * Fs, Fs, dspect, st);
+      BT_LAUNCHED(c, "train_bn_scale", st);
+      return BT_OK;
+    }
+  }
+  return BT_OK;
+}
+
+// The checks both passes share, before anything is enqueued.
+int train_prepare(bt_ctx* c, const char* fn, const void* const* params, int32_t n_params, int32_t B, int32_t L,
+                  const void* act, int64_t act_bytes, TrModel* m) {
+  if (c->dtype != BT_DTYPE_F32)
+    return fail(c, BT_ERR_ARG, "%s: training runs on a BT_DTYPE_F32 context (fp32 CUDA cores)", fn);
+  if (B < 1 || L < 1) return fail(c, BT_ERR_ARG, "%s: need B >= 1 and L >= 1, got B=%d L=%d", fn, B, L);
+  if (int64_t{B} * L > kMaxChunkCap)
+    return fail(c, BT_ERR_ARG, "%s: B * L = %lld frames exceeds %lld", fn, static_cast<long long>(int64_t{B} * L),
+                static_cast<long long>(kMaxChunkCap));
+  *m = train_model(c->hp, B, L);
+  if (n_params != static_cast<int32_t>(m->table.size()))
+    return fail(c, BT_ERR_ARG, "%s: %d parameter pointers, the model has %zu (bt_train_param_count)", fn, n_params,
+                m->table.size());
+  if (!params || !act) return fail(c, BT_ERR_ARG, "%s: null parameter array or activation store", fn);
+  for (size_t i = 0; i < m->table.size(); ++i)
+    if (!params[i] && m->table[i].ndim > 0)
+      return fail(c, BT_ERR_ARG, "%s: parameter %zu (%s) is null", fn, i, m->table[i].name.c_str());
+  if (act_bytes < m->floats * static_cast<int64_t>(sizeof(float)))
+    return fail(c, BT_ERR_ARG, "%s: activation store of %lld bytes, B=%d L=%d needs %lld (bt_train_activation_bytes)",
+                fn, static_cast<long long>(act_bytes), B, L,
+                static_cast<long long>(m->floats * static_cast<int64_t>(sizeof(float))));
+  return BT_OK;
+}
+
+int train_scratch(bt_ctx* c, int64_t BL, TrScratch* s) {
+  const int64_t n = scratch_floats(BL);
+  BT_CUDA(c, c->train_ws.reserve(n * sizeof(float), n * sizeof(float)));
+  float* p = c->train_ws.get();
+  auto take = [&](int64_t k) {
+    float* r = p;
+    p += k;
+    return r;
+  };
+  s->dcur = take(BL * 1024), s->s1 = take(BL * 1024), s->s2 = take(BL * 1024), s->big = take(BL * 4096);
+  s->dqkv = take(BL * 3072), s->hd1 = take(BL * 32 + 1024), s->hd2 = take(BL * 32 + 1024);
+  s->part = take(kPartFloats);
+  return BT_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int32_t bt_train_param_count(const bt_hparams* hp) {
+  if (!hp) return BT_ERR_ARG;
+  return static_cast<int32_t>(train_model(*hp, 0, 0).table.size());
+}
+
+int bt_train_param_info(const bt_hparams* hp, int32_t i, char* name, int32_t cap, int64_t* shape, int32_t* ndim,
+                        int32_t* trainable) {
+  if (!hp || !name || cap < 1 || !shape || !ndim || !trainable) return BT_ERR_ARG;
+  const TrModel m = train_model(*hp, 0, 0);
+  if (i < 0 || i >= static_cast<int32_t>(m.table.size())) return BT_ERR_ARG;
+  const TrParam& p = m.table[i];
+  if (static_cast<int32_t>(p.name.size()) >= cap) return BT_ERR_ARG;
+  memcpy(name, p.name.c_str(), p.name.size() + 1);
+  for (int k = 0; k < 4; ++k) shape[k] = k < p.ndim ? p.shape[k] : 0;
+  *ndim = p.ndim;
+  *trainable = p.trainable;
+  return BT_OK;
+}
+
+int64_t bt_train_activation_bytes(const bt_ctx* c, int32_t B, int32_t L) {
+  if (!c || B < 1 || L < 1) return BT_ERR_ARG;
+  return train_model(c->hp, B, L).floats * static_cast<int64_t>(sizeof(float));
+}
+
+int bt_train_forward(bt_ctx* c, const float* const* params, int32_t n_params, const float* spect_dev, int32_t B,
+                     int32_t L, void* act_dev, int64_t act_bytes, float* beat_dev, float* down_dev, void* stream) {
+  if (!c) return BT_ERR_ARG;
+  const char* fn = "bt_train_forward";
+  TrModel m;
+  int r = train_prepare(c, fn, reinterpret_cast<const void* const*>(params), n_params, B, L, act_dev, act_bytes, &m);
+  if (r != BT_OK) return r;
+  if (!spect_dev || !beat_dev || !down_dev) return fail(c, BT_ERR_ARG, "%s: null spectrogram or logits pointer", fn);
+  cudaStream_t st;
+  if ((r = enter(c, fn, stream, &st)) != BT_OK) return r;
+  TrRun R{c, st, params, nullptr, static_cast<float*>(act_dev), {}, B, L, nullptr, nullptr};
+  if ((r = train_scratch(c, int64_t{B} * L, &R.s)) != BT_OK) return r;
+  BT_CUDA(c, cudaMemcpyAsync(R.at(m.layers[0].in), spect_dev, sizeof(float) * B * L * c->hp.spect_dim,
+                             cudaMemcpyDeviceToDevice, st));
+  for (size_t i = 0; i < m.layers.size(); ++i) {
+    float* next = i + 1 < m.layers.size() ? R.at(m.layers[i + 1].in) : nullptr;
+    if ((r = forward_layer(R, m.layers[i], next, beat_dev, down_dev)) != BT_OK) return r;
+  }
+  return BT_OK;
+}
+
+int bt_train_backward(bt_ctx* c, const float* const* params, int32_t n_params, const void* act_dev, int64_t act_bytes,
+                      int32_t B, int32_t L, const float* dbeat_dev, const float* ddown_dev, float* const* grads,
+                      float* dspect_dev, void* stream) {
+  if (!c) return BT_ERR_ARG;
+  const char* fn = "bt_train_backward";
+  TrModel m;
+  int r = train_prepare(c, fn, reinterpret_cast<const void* const*>(params), n_params, B, L, act_dev, act_bytes, &m);
+  if (r != BT_OK) return r;
+  if (!dbeat_dev || !ddown_dev || !grads) return fail(c, BT_ERR_ARG, "%s: null logit gradient or gradient array", fn);
+  // an entry that takes no gradient is never written, whatever it holds; every other null entry is skipped
+  std::vector<float*> g(grads, grads + m.table.size());
+  for (size_t i = 0; i < g.size(); ++i)
+    if (!m.table[i].trainable) g[i] = nullptr;
+  cudaStream_t st;
+  if ((r = enter(c, fn, stream, &st)) != BT_OK) return r;
+  TrRun R{c, st, params, g.data(), static_cast<float*>(const_cast<void*>(act_dev)), {}, B, L, dbeat_dev, ddown_dev};
+  if ((r = train_scratch(c, int64_t{B} * L, &R.s)) != BT_OK) return r;
+  for (size_t i = m.layers.size(); i-- > 0;)
+    if ((r = backward_layer(R, m.layers[i], dspect_dev)) != BT_OK) return r;
+  return BT_OK;
+}
+
+}  // extern "C"

@@ -10,7 +10,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import BT_DTYPE_H16, BT_DTYPE_F32, DEFAULT_CHUNKING, bt_hparams, i32_array, i64_array
+from ._lib import BT_DTYPE_H16, BT_DTYPE_F32, DEFAULT_CHUNKING, i32_array, i64_array
 
 _SHARED = {}  # device -> the weight-less Engine of Engine.shared
 
@@ -92,16 +92,7 @@ class Engine:
         self.act_dtype = self.lib.bt_act_dtype().decode() if half else "f32"
         hp = hparams or {}
         self.hparams = dict(hp)
-        chp = bt_hparams(
-            int(hp.get("spect_dim", 128)),
-            int(hp.get("transformer_dim", 512)),
-            int(hp.get("ff_mult", 4)),
-            int(hp.get("n_layers", 6)),
-            int(hp.get("head_dim", 32)),
-            int(hp.get("stem_dim", 32)),
-            int(bool(hp.get("sum_head", True))),
-            int(bool(hp.get("partial_transformers", True))),
-        )
+        chp = _lib.hparams_struct(hp)
         ctx = c_void_p()
         code = self.lib.bt_create(ctypes.byref(ctx), self.device.index, ctypes.byref(chp), BT_DTYPE_H16 if half else BT_DTYPE_F32)
         _lib.check(self.lib, None, code)
@@ -453,6 +444,44 @@ class Engine:
                    i32_array(downbeat_frames), i64_array(downbeat_offsets), p(spect, dtype=h16),
                    p(truth_beat, dtype=byte), p(truth_downbeat, dtype=byte), p(padding_mask, dtype=byte))
 
+    # ---- model gradients (bt_train_*) ----------------------------------------------------------------
+    def train_activation_bytes(self, B: int, L: int) -> int:
+        n = int(self.lib.bt_train_activation_bytes(self.ctx, int(B), int(L)))
+        if n < 0:
+            raise ValueError(f"bt_train_activation_bytes refused B={B}, L={L}")
+        return n
+
+    def _table_ptrs(self, tensors, what: str):
+        """Host array of device pointers (None: NULL) for a parameter or gradient table in bt_train_param_info order.
+        Every entry the kernels touch must be a contiguous fp32 tensor of its table shape on this engine's device: the
+        library sees only addresses, so a host, double or strided tensor would be read as other bytes."""
+        if getattr(self, "_param_table", None) is None:
+            self._param_table = _lib.train_param_table(self.hparams)
+        if len(tensors) != len(self._param_table):
+            raise ValueError(f"{what}: {len(tensors)} entries, the model has {len(self._param_table)}")
+        for t, (name, shape, _) in zip(tensors, self._param_table):
+            if t is None or not shape:  # ndim-0 entries (num_batches_tracked) are never read
+                continue
+            if t.device != self.device or t.dtype != torch.float32 or not t.is_contiguous() or tuple(t.shape) != shape:
+                raise RuntimeError(f"{what} {name}: need a contiguous float32 tensor of shape {shape} on {self.device}, "
+                                   f"got {t.dtype} {tuple(t.shape)} on {t.device}; there is no CPU fallback")
+        return (c_void_p * len(tensors))(*[None if t is None else t.data_ptr() for t in tensors])
+
+    def train_forward(self, params, spect, act, beat, down):
+        """bt_train_forward: params in bt_train_param_info order (device tensors), spect [B, L, 128] fp32, act a byte
+        tensor of train_activation_bytes(B, L), beat / down [B, L] fp32 outputs."""
+        B, L, _ = spect.shape
+        p = self._dev_ptr
+        self._call("bt_train_forward", self._table_ptrs(params, "parameter"), len(params), p(spect, B * L * 128), B, L,
+                   p(act, dtype=torch.uint8), act.numel(), p(beat, B * L), p(down, B * L))
+
+    def train_backward(self, params, act, B: int, L: int, dbeat, ddown, grads, dspect=None):
+        """bt_train_backward after train_forward with the same params and act: grads (None: not wanted) parallel to
+        params; dspect [B, L, 128] or None."""
+        p = self._dev_ptr
+        self._call("bt_train_backward", self._table_ptrs(params, "parameter"), len(params), p(act, dtype=torch.uint8), act.numel(),
+                   int(B), int(L), p(dbeat, B * L), p(ddown, B * L), self._table_ptrs(grads, "gradient"), p(dspect, B * L * 128))
+
     # ---- per-kernel-class timing (bench.py roofline) -------------------------------------------
     def profile_enable(self, on: bool = True):
         self._call("bt_profile_enable", int(on), stream=False)
@@ -533,6 +562,18 @@ class Engine:
         self._call("bt_debug_attention", p(q, q.numel()), p(k, q.numel()), p(v, q.numel()), p(gates, seqs * L * (C // 32)),
                    p(o, q.numel()), o.numel(), seqs, L, C // 32, lens, seqs_per_chunk)
         return o
+
+    def debug_attention_backward(self, qkv, gates, freqs, dy):
+        """bt_debug_attention_backward on qkv [seqs, n, 3 * heads * 32] (pre-RoPE), gates [seqs, n, heads] (logits),
+        freqs [16] and dy [seqs, n, heads * 32] -> (y, dqkv, dgates) shaped like dy, qkv and gates."""
+        seqs, n, C3 = qkv.shape
+        heads = C3 // 96
+        y, dqkv, dgates = torch.empty_like(dy), torch.empty_like(qkv), torch.empty_like(gates)
+        p = self._dev_ptr
+        self._call("bt_debug_attention_backward", p(qkv, qkv.numel()), p(gates, seqs * n * heads), p(freqs, 16),
+                   p(dy, seqs * n * heads * 32), seqs, n, heads, p(y, dy.numel()), p(dqkv, qkv.numel()),
+                   p(dgates, gates.numel()))
+        return y, dqkv, dgates
 
     def debug_attention_freq(self, q, k, v, gates, B, F, out=None):
         """gates * softmax over the F planes of each (chunk, frame, head); q/k/v [B*F*L, heads*32], gates [B*F*L, heads].

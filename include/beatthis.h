@@ -512,6 +512,53 @@ int bt_train_batch(bt_ctx* ctx, const uint16_t* rows_dev, const int64_t* row_off
                    const int64_t* downbeat_offsets_host, uint16_t* out_spect_dev, uint8_t* truth_beat_dev,
                    uint8_t* truth_downbeat_dev, uint8_t* padding_mask_dev, void* stream);
 
+/* ---- model gradients: loss.backward() through the reference's BeatThis in eval() mode ------------------------------
+ * The gradient of the function the inference path computes (BatchNorm on its running statistics, no dropout), in fp32
+ * on the CUDA cores (ABI 2.12).  The parameters are the caller's: unfolded fp32 device tensors, one per entry of
+ * BeatThis.state_dict(), in the order and shapes of bt_train_param_info, passed on every call as a host array of
+ * n_params device pointers.  The entries no kernel reads (the ndim-0 num_batches_tracked counters) may be NULL.  A ctx
+ * of any bt_hparams bt_create accepts serves, with BT_DTYPE_F32 and without bt_set_param / bt_finalize; a BT_DTYPE_H16
+ * ctx is refused with BT_ERR_ARG.  RoPE angles are computed from each attention's rotary_embed.freqs, so L is bounded
+ * only by the activation store (and B * L by 384000 frames). */
+
+/* Entries of the parameter table of a model of shape hp (pure host).  BT_ERR_ARG for a NULL hp. */
+int32_t bt_train_param_count(const bt_hparams* hp);
+/* Entry i: its state_dict name (NUL-terminated, cap bytes), shape[0 .. *ndim) (the rest 0) and whether it takes a
+ * gradient (0 for the BatchNorm running statistics and counters, and rotary_embed.freqs).  Pure host; BT_ERR_ARG for
+ * i out of range, a name longer than cap - 1 or a NULL pointer. */
+int bt_train_param_info(const bt_hparams* hp, int32_t i, char* name, int32_t cap, int64_t* shape, int32_t* ndim,
+                        int32_t* trainable);
+/* Bytes of the activation store of one forward pass over [B, L, 128]: what bt_train_backward reads.  BT_ERR_ARG for a
+ * NULL ctx or B, L < 1. */
+int64_t bt_train_activation_bytes(const bt_ctx* ctx, int32_t B, int32_t L);
+/* BeatThis.forward of a dense batch spect_dev [B, L, 128] (fp32; padded frames take part as they do in the reference)
+ * -> beat_dev, down_dev [B, L], saving its activations in act_dev (act_bytes >= bt_train_activation_bytes).  The
+ * logits equal those of the BT_DTYPE_F32 inference path within its fp32 tolerance. */
+int bt_train_forward(bt_ctx* ctx, const float* const* params, int32_t n_params, const float* spect_dev, int32_t B,
+                     int32_t L, void* act_dev, int64_t act_bytes, float* beat_dev, float* down_dev, void* stream);
+/* From the gradients at the logits (dbeat_dev, ddown_dev [B, L]) and the store of the bt_train_forward call with the
+ * same params, B and L: the gradient of every entry into grads[i] (a device buffer of the entry's shape, overwritten,
+ * never accumulated).  Entries that take no gradient are never written; a NULL grads[i] skips that gradient.
+ * dspect_dev: the gradient at the spectrogram [B, L, 128], or NULL.  Reductions run in a fixed order without atomics:
+ * two calls on the same inputs write the same bytes.
+ * Both passes: BT_ERR_ARG, before anything is enqueued, for a 16-bit ctx, B or L < 1, n_params other than
+ * bt_train_param_count, a NULL pointer, or a store smaller than the batch needs.  Enqueued on `stream` without
+ * synchronisation; the ctx's scratch grows on demand. */
+int bt_train_backward(bt_ctx* ctx, const float* const* params, int32_t n_params, const void* act_dev, int64_t act_bytes,
+                      int32_t B, int32_t L, const float* dbeat_dev, const float* ddown_dev, float* const* grads,
+                      float* dspect_dev, void* stream);
+
+/* Test hook (fp32 ctx only; BT_ERR_ARG for a 16-bit one): the attention core of one bt_train_forward /
+ * bt_train_backward layer alone, on `seqs` time-direction sequences of n positions and `heads` heads of 32.  qkv_dev
+ * [seqs * n, 3 * heads * 32] holds q | k | v before RoPE, gates_dev [seqs * n, heads] the gate logits, freqs_dev [16]
+ * the rotary frequencies.  Writes y_dev [seqs * n, heads * 32] = softmax(q k^T / sqrt 32) v * sigmoid(gate) (q, k
+ * rotated by position * freqs) and, from dy_dev (the gradient at y), the gradients at the pre-RoPE qkv (dqkv_dev) and
+ * at the gate logits (dgates_dev).  Seven kernels: RoPE, attention, gate, gate backward, dQ, dK/dV and the inverse
+ * RoPE, each counted and profiled under its train_* name.  Synchronises the stream before it returns. */
+int bt_debug_attention_backward(bt_ctx* ctx, const float* qkv_dev, const float* gates_dev, const float* freqs_dev,
+                                const float* dy_dev, int32_t seqs, int32_t n, int32_t heads, float* y_dev,
+                                float* dqkv_dev, float* dgates_dev, void* stream);
+
 /* ---- introspection / tuning ----------------------------------------------------------------- */
 
 /* Upper bound on the chunks processed per wave (1..256, default 128; one wave = one launch of every kernel of the
