@@ -17,7 +17,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 # BT_LIB_PATH: an instrumented build of the same sources (e.g. build(extra_flags=("-DBT_FF_PROF",), out_path=...))
 LIB_PATH = os.environ.get("BT_LIB_PATH") or os.path.join(HERE, "libbeatthis_sm90.so")
-SOURCES = ["bt_api.cu", "api_signal.cu", "api_post.cu", "api_data.cu", "api_train.cu", "api_debug.cu", "kernels_simt.cu", "kernels_misc.cu", "kernels_gemm.cu", "kernels_attn.cu", "kernels_fused.cu", "kernels_dbn.cu", "kernels_eval.cu", "kernels_loss.cu", "kernels_augment.cu", "kernels_data.cu", "kernels_train.cu", "dbn_host.cpp", "host_stage.cpp"]
+SOURCES = ["bt_api.cu", "api_signal.cu", "api_post.cu", "api_data.cu", "api_train.cu", "api_debug.cu", "kernels_simt.cu", "kernels_misc.cu", "kernels_signal.cu", "kernels_gemm.cu", "kernels_attn.cu", "kernels_fused.cu", "kernels_dbn.cu", "kernels_eval.cu", "kernels_loss.cu", "kernels_data.cu", "kernels_train.cu", "dbn_host.cpp", "host_stage.cpp"]
 HEADERS = ["common.cuh", "epilogue.cuh", "fft.cuh", "tc_common.cuh", "bt_kernels.h", "bt_train.h", "cuda_owned.h", "dbn_model.h",
            "api_internal.h", os.path.join("..", "..", "include", "beatthis.h")]
 

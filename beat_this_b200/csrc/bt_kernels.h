@@ -87,29 +87,6 @@ void launch_stem(const float* spect, const ChunkSrc* chunks, int nchunks, int L,
                  cudaStream_t st);
 void launch_head(const float* x, int D, const float* w, const float* b, const ChunkSrc* chunks,
                  int nchunks, int L, float* beat, float* down, int sum_head, cudaStream_t st);
-// dynamic shared memory resample_kernel needs for the ratio L/M with K taps; the caller keeps it <= kResampleMaxSmem
-int64_t resample_smem(int L, int M, int K);
-constexpr int64_t kResampleMaxSmem = 200 * 1024;
-cudaError_t launch_resample(const float* in, const int64_t* in_off_dev, float* out, const int64_t* out_off_dev,
-                            int n_clips, int64_t max_out, const float* coef, int L, int M, int K, cudaStream_t st);
-void launch_logmel(const float* audio, const int64_t* sample_off_dev, const int64_t* frame_off_dev,
-                   int n_clips, int64_t max_frames, const float* window, const float* twiddle,
-                   const int32_t* fb_start, const int32_t* fb_ptr, const float* fb_w, float* spect,
-                   cudaStream_t st);
-// bt_logmel_config's tables, output and scalars (kernels_misc.cu logmel_config_kernel); norm_mode as bt_mel_config
-struct MelConfigArgs {
-  const float* window;
-  const float* twiddle;
-  const int32_t* fb_start;
-  const int32_t* fb_ptr;
-  const float* fb_w;
-  float* spect;
-  int hop, n_mels, norm_mode;
-  float power, log_multiplier;
-};
-cudaError_t launch_logmel_config(int log2n, const float* audio, const int64_t* sample_off_dev,
-                                 const int64_t* frame_off_dev, int n_clips, int64_t total_frames,
-                                 const MelConfigArgs& p, cudaStream_t st);
 void launch_peakpick(const float* beat, const float* down, const int64_t* frame_off_dev, int n_clips,
                      double* beat_t, int32_t* n_beat, double* down_t, int32_t* n_down,
                      int max_peaks, double fps, cudaStream_t st);
@@ -182,9 +159,33 @@ void launch_beat_loss_backward(const float* x, const float* y, const float* m, c
                                const int64_t* tile_first_dev, int n_rows, int64_t n_tiles, int64_t n_scored,
                                const LossParams& p, const float* grad_mean, float* grad, cudaStream_t st);
 
-// ---- tempo / pitch augmentation (kernels_augment.cu) -----------------------------------------------------------------
-// The contracts of bt_stft, bt_phase_vocoder and bt_istft (include/beatthis.h).  spec: interleaved complex fp32,
-// n_fft / 2 + 1 bins per frame; log2n: 6..13.
+// ---- signal (kernels_signal.cu) ------------------------------------------------------------------------------------
+// The contracts of bt_logmel, bt_logmel_config, bt_resample, bt_stft, bt_phase_vocoder and bt_istft
+// (include/beatthis.h).  log2n: 6..13.
+void launch_logmel(const float* audio, const int64_t* sample_off_dev, const int64_t* frame_off_dev,
+                   int n_clips, int64_t max_frames, const float* window, const float* twiddle,
+                   const int32_t* fb_start, const int32_t* fb_ptr, const float* fb_w, float* spect,
+                   cudaStream_t st);
+// bt_logmel_config's tables, output and scalars (logmel_config_kernel); norm_mode as bt_mel_config
+struct MelConfigArgs {
+  const float* window;
+  const float* twiddle;
+  const int32_t* fb_start;
+  const int32_t* fb_ptr;
+  const float* fb_w;
+  float* spect;
+  int hop, n_mels, norm_mode;
+  float power, log_multiplier;
+};
+cudaError_t launch_logmel_config(int log2n, const float* audio, const int64_t* sample_off_dev,
+                                 const int64_t* frame_off_dev, int n_clips, int64_t total_frames,
+                                 const MelConfigArgs& p, cudaStream_t st);
+// dynamic shared memory resample_kernel needs for the ratio L/M with K taps; the caller keeps it <= kResampleMaxSmem
+int64_t resample_smem(int L, int M, int K);
+constexpr int64_t kResampleMaxSmem = 200 * 1024;
+cudaError_t launch_resample(const float* in, const int64_t* in_off_dev, float* out, const int64_t* out_off_dev,
+                            int n_clips, int64_t max_out, const float* coef, int L, int M, int K, cudaStream_t st);
+// spec: interleaved complex fp32, n_fft / 2 + 1 bins per frame.
 cudaError_t launch_stft(int log2n, const float* audio, const int64_t* sample_off_dev, const int64_t* frame_off_dev,
                         int n_clips, int64_t total_frames, const float* window, const float* twiddle, int hop, float* spec,
                         cudaStream_t st);

@@ -1,5 +1,5 @@
-// Device pieces of the shared-memory FFT that the log-mel kernels (kernels_misc.cu) and the STFT / inverse STFT kernels
-// (kernels_augment.cu) are built from: complex helpers, the register DFTs and the passes of the Stockham FFT.
+// Device pieces of the shared-memory FFT that the log-mel, STFT and inverse STFT kernels (kernels_signal.cu) are built
+// from: complex helpers, the register DFTs and the passes of the Stockham FFT.
 #pragma once
 #include <cuda_runtime.h>
 

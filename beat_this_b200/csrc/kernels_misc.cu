@@ -1,320 +1,14 @@
-// HBM-bound kernels of the path: log-mel frontend, stem conv, RMSNorm(+gates),
-// frequency-direction attention, head + aggregation scatter, peak picking.
+// The model's HBM-bound row kernels (stem conv, zero tail, RMSNorm(+gates)), both frequency-direction attentions,
+// head + aggregation scatter, peak picking, the f32 <-> 16-bit conversions and the QKV packing of the test hooks.
 #include <cuda_fp16.h>
-#include <algorithm>
 #include <cstdio>
 #include <cstdlib>
 
 #include "bt_kernels.h"
 #include "common.cuh"
-#include "fft.cuh"
 #include "tc_common.cuh"
 
 namespace bt {
-
-// ------------------------------------------------------------------------------------------
-// log-mel: reference LogMelSpect.forward (beat_this/preprocessing.py:56-59) =
-//   torch.stft(n_fft 1024, hop 441, periodic hann, center reflect, normalized) -> abs ->
-//   mel filterbank (slaney, 128 bins, 30..11000 Hz) -> log1p(1000 x).
-// Algorithmic HBM bytes: 441 new samples * 4 B read + 128 * 4 B written per frame.
-//
-// 64 threads per frame, two frames per CTA.  The real 1024-point transform is ONE complex 512-point FFT of
-// z[n] = x[2n] + i x[2n+1] followed by the usual untangling step, and 512 = 8 * 8 * 8: three radix-8 passes with the
-// eight points of a butterfly in registers,
-//   n = 64 n1 + 8 n2 + n3,  k = k1 + 8 k2 + 64 k3:
-//   A: thread (n2, n3)  DFT8 over n1, times e^{-2 pi i n2 k1 / 64}          -> T1[k1][n2][n3]
-//   B: thread (k1, n3)  DFT8 over n2, times e^{-2 pi i n3 (k1 + 8 k2) / 512} -> T2[n3][k2][k1]
-//   C: thread (k2, k1)  DFT8 over n3                                         -> Z[k1 + 8 k2 + 64 k3]
-// i.e. two exchanges through shared memory (8-byte accesses, padded pitches: at most the natural two wavefronts per
-// warp access) where the radix-2 version of round 1 made ten passes over separate re / im arrays -- that kernel was
-// bound by the shared-memory pipe (ncu: l1tex data-pipe wavefronts 97 %), not by HBM.
-// ------------------------------------------------------------------------------------------
-constexpr int LM_P1 = 72, LM_P2 = 68;  // pitches (float2) of the two exchange buffers
-
-__global__ void __launch_bounds__(128)
-logmel_kernel(const float* __restrict__ audio, const int64_t* __restrict__ sample_off,
-              const int64_t* __restrict__ frame_off, const float* __restrict__ window,
-              const float2* __restrict__ twiddle, const int32_t* __restrict__ fb_start,
-              const int32_t* __restrict__ fb_ptr, const float* __restrict__ fb_w,
-              float* __restrict__ spect) {
-  __shared__ float2 tw[512];                 // e^{-2 pi i j / 1024}, j < 512
-  __shared__ float2 t1[2][8 * LM_P1];        // per frame: T1, later Z (512 entries)
-  __shared__ float2 t2[2][8 * LM_P2];
-  __shared__ float mag[2][516];
-  const int clip = blockIdx.y;
-  const int64_t f0 = frame_off[clip];
-  const int T = static_cast<int>(frame_off[clip + 1] - f0);
-  const int tid = threadIdx.x, half = tid >> 6, lt = tid & 63;
-  const int t = 2 * blockIdx.x + half;
-  if (2 * static_cast<int>(blockIdx.x) >= T) return;  // whole CTA beyond the clip
-  const bool active = t < T;
-  const int64_t s0 = sample_off[clip];
-  const int64_t len = sample_off[clip + 1] - s0;
-  for (int i = tid; i < 512; i += 128) tw[i] = twiddle[i];
-  auto TW = [&](int j) -> float2 {  // e^{-2 pi i j / 1024}, 0 <= j < 1024
-    const float2 w = tw[j & 511];
-    return (j & 512) ? make_float2(-w.x, -w.y) : w;
-  };
-  float2 v[8];
-  float2* T1 = t1[half];
-  float2* T2 = t2[half];
-  {  // ---- pass A: thread (n2, n3) = lt, points z[64 n1 + lt] ----
-#pragma unroll
-    for (int n1 = 0; n1 < 8; ++n1) {
-      const int n = 2 * (64 * n1 + lt);
-      float xs[2];
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        int64_t i = 441ll * t + (n + e) - 512;
-        if (i < 0) i = -i;                      // reflect (no edge repeat), torch pad_mode="reflect"
-        if (i >= len) i = 2 * (len - 1) - i;
-        xs[e] = active ? audio[s0 + i] * __ldg(window + n + e) : 0.f;
-      }
-      v[n1] = make_float2(xs[0], xs[1]);
-    }
-  }
-  __syncthreads();  // twiddle table
-  {
-    dft8(v);
-    const int n2 = lt >> 3;
-#pragma unroll
-    for (int k1 = 0; k1 < 8; ++k1) T1[k1 * LM_P1 + lt] = k1 == 0 ? v[0] : cmul(v[k1], TW(16 * n2 * k1));
-  }
-  __syncthreads();
-  {  // ---- pass B: thread (k1, n3) = lt ----
-    const int k1 = lt >> 3, n3 = lt & 7;
-#pragma unroll
-    for (int n2 = 0; n2 < 8; ++n2) v[n2] = T1[k1 * LM_P1 + n2 * 8 + n3];
-    dft8(v);
-#pragma unroll
-    for (int k2 = 0; k2 < 8; ++k2) T2[n3 * LM_P2 + k2 * 8 + k1] = cmul(v[k2], TW(2 * n3 * (k1 + 8 * k2)));
-  }
-  __syncthreads();
-  {  // ---- pass C: thread (k2, k1) = lt -> Z[lt + 64 k3] (into T1's storage) ----
-#pragma unroll
-    for (int n3 = 0; n3 < 8; ++n3) v[n3] = T2[n3 * LM_P2 + lt];
-    dft8(v);
-#pragma unroll
-    for (int k3 = 0; k3 < 8; ++k3) T1[lt + 64 * k3] = v[k3];
-  }
-  __syncthreads();
-  // untangle: X[k] = E[k] + e^{-2 pi i k / 1024} O[k], E = (Z[k] + conj Z[512 - k]) / 2, O = -i (Z[k] - conj Z[512 - k]) / 2;
-  // magnitudes of bins 0..512 (normalized=True -> 1 / sqrt(1024))
-  for (int k = lt; k <= 512; k += 64) {
-    const float2 zk = T1[k & 511], zc = T1[(512 - k) & 511];
-    const float2 e = make_float2(0.5f * (zk.x + zc.x), 0.5f * (zk.y - zc.y));
-    const float2 o = make_float2(0.5f * (zk.y + zc.y), -0.5f * (zk.x - zc.x));
-    const float2 x = cadd(e, cmul(TW(k), o));
-    mag[half][k] = sqrtf(x.x * x.x + x.y * x.y) * 0.03125f;
-  }
-  __syncthreads();
-  if (active) {
-#pragma unroll
-    for (int mm = 0; mm < 2; ++mm) {
-      const int m = lt + 64 * mm;  // mel bin
-      const int p0 = fb_ptr[m], p1 = fb_ptr[m + 1];
-      const int k0 = fb_start[m];
-      float acc = 0.f;
-      for (int p = p0; p < p1; ++p) acc = fmaf(mag[half][k0 + (p - p0)], fb_w[p], acc);
-      spect[(f0 + t) * 128 + m] = log1pf(1000.0f * acc);
-    }
-  }
-}
-
-void launch_logmel(const float* audio, const int64_t* sample_off_dev, const int64_t* frame_off_dev,
-                   int n_clips, int64_t max_frames, const float* window, const float* twiddle,
-                   const int32_t* fb_start, const int32_t* fb_ptr, const float* fb_w, float* spect,
-                   cudaStream_t st) {
-  if (max_frames <= 0 || n_clips <= 0) return;
-  dim3 grid(static_cast<unsigned>((max_frames + 1) / 2), static_cast<unsigned>(n_clips));
-  logmel_kernel<<<grid, 128, 0, st>>>(audio, sample_off_dev, frame_off_dev, window,
-                                      reinterpret_cast<const float2*>(twiddle), fb_start, fb_ptr, fb_w, spect);
-}
-
-// ------------------------------------------------------------------------------------------
-// General log-mel (bt_logmel_config, contract in include/beatthis.h): STFT with any power-of-two n_fft = N in
-// [64, 8192] and any hop -> |.|^power -> CSR mel filterbank -> log1p(log_multiplier x).
-// Algorithmic HBM bytes: hop new samples * 4 B read + n_mels * 4 B written per frame.
-//
-// As in logmel_kernel, the real N-point transform is one complex H = N/2-point FFT of z[n] = x[2n] + i x[2n+1] and the
-// untangling step; the FFT (fft.cuh) takes TPF = H/8 threads per frame.  A CTA of max(256, TPF) threads transforms
-// FPC = threads / TPF consecutive frames of the batch's frames flattened over all clips (a frame finds its clip by
-// binary search of frame_off; a CTA may span clips) and loops over frame groups grid-stride.
-// ------------------------------------------------------------------------------------------
-template <int LOG2N>
-__global__ void __launch_bounds__(MelGeom<LOG2N>::THREADS)
-logmel_config_kernel(const float* __restrict__ audio, const int64_t* __restrict__ sample_off,
-                     const int64_t* __restrict__ frame_off, int n_clips, int64_t total_frames, MelConfigArgs p) {
-  using G = MelGeom<LOG2N>;
-  constexpr int N = G::N, H = G::H, TPF = G::TPF, FPC = G::FPC, THREADS = G::THREADS;
-  extern __shared__ float4 mel_smem4[];
-  unsigned char* const smem = reinterpret_cast<unsigned char*>(mel_smem4);
-  float2* const fft = reinterpret_cast<float2*>(smem);
-  float* const spec = reinterpret_cast<float*>(smem + G::SPEC_OFF);
-  double* const red = reinterpret_cast<double*>(smem + G::RED_OFF);
-  const float2* __restrict__ tw = reinterpret_cast<const float2*>(p.twiddle);
-  const int tid = threadIdx.x, fl = tid / TPF, lt = tid % TPF;
-
-  float scale = p.norm_mode == 1 ? rsqrtf(static_cast<float>(N)) : 1.f;
-  if (p.norm_mode == 2) {  // 1 / sqrt(sum window^2), summed in float64 in a fixed order
-    double s = 0.0;
-    for (int i = tid; i < N; i += THREADS) s += static_cast<double>(p.window[i]) * p.window[i];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    if ((tid & 31) == 0) red[tid >> 5] = s;
-    __syncthreads();
-    s = 0.0;
-    for (int w = 0; w < THREADS / 32; ++w) s += red[w];
-    scale = static_cast<float>(1.0 / sqrt(s));
-  }
-
-  float2* const a = fft + fl * G::PITCH;
-  float* const sp = spec + fl * (H + 1);
-  for (int64_t g0 = static_cast<int64_t>(blockIdx.x) * FPC; g0 < total_frames; g0 += static_cast<int64_t>(gridDim.x) * FPC) {
-    const int64_t g = g0 + fl;
-    float2 v[8];
-    if (g < total_frames) {
-      int lo = 0, hi = n_clips;  // frame_off[lo] <= g < frame_off[hi]
-      while (hi - lo > 1) {
-        const int mid = (lo + hi) >> 1;
-        if (__ldg(frame_off + mid) <= g) lo = mid; else hi = mid;
-      }
-      const int64_t s0 = __ldg(sample_off + lo), len = __ldg(sample_off + lo + 1) - s0;
-      const int64_t base = (g - __ldg(frame_off + lo)) * p.hop - N / 2;
-#pragma unroll
-      for (int r = 0; r < 8; ++r) {  // first radix-8 pass: points z[lt + r H/8] straight from the clip
-        const int n = 2 * (lt + r * (H / 8));
-        float xs[2];
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          int64_t i = base + n + e;
-          if (i < 0) i = -i;                    // reflect without repeating the edge, torch pad_mode="reflect";
-          if (i >= len) i = 2 * (len - 1) - i;  // len > N/2 makes one reflection enough
-          xs[e] = __ldg(audio + s0 + i) * __ldg(p.window + n + e);
-        }
-        v[r] = make_float2(xs[0], xs[1]);
-      }
-    } else {
-#pragma unroll
-      for (int r = 0; r < 8; ++r) v[r] = make_float2(0.f, 0.f);
-    }
-    mel_fft_from_registers<LOG2N>(a, v, lt, tw);
-    // untangle (as logmel_kernel): X[k] = E[k] + e^{-2 pi i k / N} O[k], bins 0..H, then (scale |X|)^power
-    for (int k = lt; k <= H; k += TPF) {
-      const float2 zk = a[mel_pad(k & (H - 1))], zc = a[mel_pad((H - k) & (H - 1))];
-      const float2 e = make_float2(0.5f * (zk.x + zc.x), 0.5f * (zk.y - zc.y));
-      const float2 o = make_float2(0.5f * (zk.y + zc.y), -0.5f * (zk.x - zc.x));
-      const float2 x = cadd(e, cmul(mel_tw<N>(tw, k), o));
-      const float m = sqrtf(x.x * x.x + x.y * x.y) * scale;
-      sp[k] = p.power == 1.f ? m : (p.power == 2.f ? m * m : powf(m, p.power));
-    }
-    __syncthreads();
-    // mel bands of the CTA's frames: consecutive threads write consecutive outputs
-    const int nm = p.n_mels;
-    for (int idx = tid; idx < FPC * nm; idx += THREADS) {
-      const int f = idx / nm, m = idx - f * nm;
-      if (g0 + f >= total_frames) break;
-      const int q0 = __ldg(p.fb_ptr + m), q1 = __ldg(p.fb_ptr + m + 1);
-      const float* s = spec + f * (H + 1) + __ldg(p.fb_start + m);
-      float acc = 0.f;
-      for (int q = q0; q < q1; ++q) acc = fmaf(s[q - q0], __ldg(p.fb_w + q), acc);
-      p.spect[(g0 + f) * nm + m] = log1pf(p.log_multiplier * acc);
-    }
-  }
-}
-
-template <int LOG2N>
-static cudaError_t launch_logmel_config_n(const float* audio, const int64_t* sample_off_dev, const int64_t* frame_off_dev,
-                                          int n_clips, int64_t total_frames, const MelConfigArgs& p, cudaStream_t st) {
-  using G = MelGeom<LOG2N>;
-  cudaError_t e = cudaFuncSetAttribute(logmel_config_kernel<LOG2N>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       static_cast<int>(G::SMEM));
-  if (e != cudaSuccess) return e;
-  static int max_ctas = 0;  // CTAs resident on the whole device at once: the grid-stride grid
-  if (max_ctas == 0) {
-    int dev = 0, sms = 0, per_sm = 0;
-    e = cudaGetDevice(&dev);
-    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (e == cudaSuccess)
-      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, logmel_config_kernel<LOG2N>, G::THREADS, G::SMEM);
-    if (e != cudaSuccess) return e;
-    max_ctas = std::max(1, sms * per_sm);
-  }
-  const int64_t groups = (total_frames + G::FPC - 1) / G::FPC;
-  const unsigned grid = static_cast<unsigned>(std::min<int64_t>(groups, max_ctas));
-  logmel_config_kernel<LOG2N><<<grid, G::THREADS, G::SMEM, st>>>(audio, sample_off_dev, frame_off_dev, n_clips,
-                                                                  total_frames, p);
-  return cudaSuccess;
-}
-
-cudaError_t launch_logmel_config(int log2n, const float* audio, const int64_t* sample_off_dev,
-                                 const int64_t* frame_off_dev, int n_clips, int64_t total_frames,
-                                 const MelConfigArgs& p, cudaStream_t st) {
-  if (n_clips <= 0 || total_frames <= 0) return cudaSuccess;
-  switch (log2n) {
-#define BT_MEL_CASE(L) \
-  case L: return launch_logmel_config_n<L>(audio, sample_off_dev, frame_off_dev, n_clips, total_frames, p, st);
-    BT_MEL_CASE(6) BT_MEL_CASE(7) BT_MEL_CASE(8) BT_MEL_CASE(9) BT_MEL_CASE(10) BT_MEL_CASE(11) BT_MEL_CASE(12)
-    BT_MEL_CASE(13)
-#undef BT_MEL_CASE
-    default: return cudaErrorInvalidValue;
-  }
-}
-
-// ------------------------------------------------------------------------------------------
-// Polyphase resampler to 22.05 kHz: device stand-in for soxr.resample (reference inference.py:274-275; method and
-// filter design in beat_this_b200/preprocessing.py, parity with soxr unpinned).
-//   y[n] = sum_k coef[(n M) mod L][k] * x[floor(n M / L) - K/2 + 1 + k],  zeros outside the clip.
-// One CTA = 256 consecutive output samples of one clip; the input span they read is staged in shared memory.
-// Algorithmic HBM bytes: 4 B per input sample + 4 B per output sample (the L x K bank stays in L1/L2).
-// ------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256)
-resample_kernel(const float* __restrict__ in, const int64_t* __restrict__ in_off, float* __restrict__ out,
-                const int64_t* __restrict__ out_off, const float* __restrict__ coef, int L, int M, int K) {
-  extern __shared__ float xs[];
-  const int clip = blockIdx.y;
-  const int64_t n0 = static_cast<int64_t>(blockIdx.x) * 256;
-  const int64_t s0 = in_off[clip], len = in_off[clip + 1] - s0;
-  const int64_t o0 = out_off[clip], nout = out_off[clip + 1] - o0;
-  if (n0 >= nout) return;
-  const int64_t n_last = min(n0 + 255, nout - 1);
-  const int64_t j_lo = (n0 * M) / L - K / 2 + 1;
-  const int span = static_cast<int>((n_last * M) / L - K / 2 + K - j_lo + 1);
-  for (int i = threadIdx.x; i < span; i += 256) {
-    const int64_t j = j_lo + i;
-    xs[i] = (j >= 0 && j < len) ? in[s0 + j] : 0.f;
-  }
-  __syncthreads();
-  const int64_t n = n0 + threadIdx.x;
-  if (n >= nout) return;
-  const int64_t nm = n * M;
-  const int base = static_cast<int>(nm / L - K / 2 + 1 - j_lo);
-  const float* c = coef + static_cast<int64_t>(nm % L) * K;
-  float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
-  int k = 0;
-  for (; k + 4 <= K; k += 4) {
-    a0 = fmaf(__ldg(c + k), xs[base + k], a0);
-    a1 = fmaf(__ldg(c + k + 1), xs[base + k + 1], a1);
-    a2 = fmaf(__ldg(c + k + 2), xs[base + k + 2], a2);
-    a3 = fmaf(__ldg(c + k + 3), xs[base + k + 3], a3);
-  }
-  for (; k < K; ++k) a0 = fmaf(__ldg(c + k), xs[base + k], a0);
-  out[o0 + n] = (a0 + a1) + (a2 + a3);
-}
-
-int64_t resample_smem(int L, int M, int K) { return ((255ll * M) / L + K + 2) * 4; }  // the staged input span
-
-cudaError_t launch_resample(const float* in, const int64_t* in_off_dev, float* out, const int64_t* out_off_dev,
-                            int n_clips, int64_t max_out, const float* coef, int L, int M, int K, cudaStream_t st) {
-  if (n_clips <= 0 || max_out <= 0) return cudaSuccess;
-  const int smem = static_cast<int>(resample_smem(L, M, K));
-  const cudaError_t e = smem > 48 * 1024
-      ? cudaFuncSetAttribute(resample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) : cudaSuccess;
-  if (e != cudaSuccess) return e;
-  dim3 grid(static_cast<unsigned>((max_out + 255) / 256), static_cast<unsigned>(n_clips));
-  resample_kernel<<<grid, 256, smem, st>>>(in, in_off_dev, out, out_off_dev, coef, L, M, K);
-  return cudaSuccess;
-}
 
 // ------------------------------------------------------------------------------------------
 // stem: BN1d(128) -> Conv2d(1->32, k(4,3), s(4,1), p(0,1), no bias) -> BN2d -> GELU
