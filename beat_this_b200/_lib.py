@@ -72,6 +72,48 @@ class bt_debug_gemm_desc(ctypes.Structure):
     ]
 
 
+class bt_debug_train_desc(ctypes.Structure):
+    _fields_ = [
+        ("op", c_int32),
+        ("splits", c_int32),
+        ("M", c_int64),
+        ("N", c_int32),
+        ("K", c_int32),
+        ("C", c_int32),
+        ("flag", c_int32),
+        ("scale", c_float),
+        ("a_rs", c_int64),
+        ("a_cs", c_int64),
+        ("b_rs", c_int64),
+        ("b_cs", c_int64),
+        ("ldc", c_int64),
+        ("ldr", c_int64),
+        ("B", c_int32),
+        ("F", c_int32),
+        ("L", c_int32),
+        ("S", c_int32),
+        ("posmode", c_int32),
+        ("heads", c_int32),
+        ("sb", c_int64),
+        ("sf", c_int64),
+        ("st", c_int64),
+        ("sc", c_int64),
+        ("seqs", c_int32),
+        ("n", c_int32),
+        ("seq_in", c_int32),
+        ("pad_", c_int32),
+        ("s_out", c_int64),
+        ("s_in", c_int64),
+        ("s_pos", c_int64),
+    ]
+
+
+# bt_debug_train_kernel's ops (BT_TRAIN_*), in the order of include/beatthis.h
+TRAIN_OPS = ("gemm", "reduce", "colsum", "rms_fwd", "rms_bwd", "bn_gelu_fwd", "bn_gelu_bwd", "bn_grads", "bn_scale",
+             "gelu_bwd", "im2col", "col2im", "concat", "rope", "gate_fwd", "gate_bwd", "head_fwd", "head_bwd", "attn_fwd",
+             "attn_dq", "attn_dkv")
+
+
 class bt_beat_metric_params(ctypes.Structure):
     _fields_ = [
         ("min_beat_time", c_double),
@@ -243,6 +285,9 @@ PROTOTYPES = {
     "bt_debug_attention_backward": (
         c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p,
                 c_void_p],
+    ),
+    "bt_debug_train_kernel": (
+        c_int, [c_void_p, POINTER(bt_debug_train_desc), POINTER(c_void_p), POINTER(c_int64), c_int32, c_void_p],
     ),
     "bt_spect2frames": (c_int, [c_void_p, c_void_p, POINTER(c_int64), c_int32, c_void_p, c_void_p, c_void_p]),
     "bt_forward_chunks": (c_int, [c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_void_p]),

@@ -359,3 +359,357 @@ int bt_debug_attention_backward(bt_ctx* c, const float* qkv_dev, const float* ga
 }
 
 }  // extern "C"
+
+namespace {
+
+// 1 + the largest offset sum_i (n_i - 1) stride_i of an array walked over dims n_i >= 1 with strides >= 0; -1 when it
+// does not fit in int64 (no array is that long)
+int64_t extent(std::initializer_list<std::pair<int64_t, int64_t>> dims) {
+  int64_t e = 1;
+  for (const auto& d : dims) {
+    int64_t t;
+    if (__builtin_mul_overflow(d.first - 1, d.second, &t) || __builtin_add_overflow(e, t, &e)) return -1;
+  }
+  return e;
+}
+
+// The slots of one bt_debug_train_kernel call.  need(i, n, ...) checks slot i against the n elements the op touches
+// there and returns its pointer; the first failure is kept in `err` for the caller to report.
+struct TrSlots {
+  float* const* p;
+  const int64_t* cnt;
+  int32_t n;
+  std::string err;
+  float* need(int i, int64_t elems, bool required = true, bool align = false) {
+    float* a = i < n ? p[i] : nullptr;
+    if (!err.empty()) return a;
+    if (!a) {
+      if (required) err = "slot " + std::to_string(i) + " is NULL";
+    } else if (elems < 0 || cnt[i] < elems) {
+      err = "slot " + std::to_string(i) + " holds " + std::to_string(cnt[i]) + " elements, the op touches " +
+            (elems < 0 ? std::string("more than 2^63") : std::to_string(elems));
+    } else if (align && reinterpret_cast<uintptr_t>(a) % 16 != 0) {
+      err = "slot " + std::to_string(i) + " is not 16-byte aligned (float4 access)";
+    }
+    return a;
+  }
+  bool present(int i) const { return i < n && p[i]; }
+};
+
+constexpr int64_t kMaxGrid1 = int64_t{INT32_MAX};  // gridDim.x
+constexpr int64_t kMaxElems = kMaxGrid1 * 256;     // elementwise launches of 256 threads per element block
+
+}  // namespace
+
+extern "C" {
+
+int bt_debug_train_kernel(bt_ctx* c, const bt_debug_train_desc* d, float* const* arrays_dev, const int64_t* counts,
+                          int32_t n_arrays, void* stream) {
+  if (!c) return BT_ERR_ARG;
+  const char* fn = "bt_debug_train_kernel";
+  if (c->dtype != BT_DTYPE_F32) return fail(c, BT_ERR_ARG, "%s: the training kernels run on a BT_DTYPE_F32 context", fn);
+  if (!d || n_arrays < 0 || (n_arrays > 0 && (!arrays_dev || !counts)))
+    return fail(c, BT_ERR_ARG, "%s: null descriptor or array table", fn);
+  TrSlots s{arrays_dev, counts, n_arrays, {}};
+  const int64_t M = d->M;
+  const int C = d->C;
+  const auto bad = [&](const char* what) { return fail(c, BT_ERR_ARG, "%s: op %d: %s", fn, d->op, what); };
+  const auto slots = [&]() { return s.err.empty() ? BT_OK : fail(c, BT_ERR_ARG, "%s: op %d: %s", fn, d->op, s.err.c_str()); };
+  const auto elementwise = [&](int64_t n) { return n >= 1 && n <= kMaxElems; };
+  // the BatchNorm of C channels in slots i .. i + 3
+  const auto bn_at = [&](int i, int64_t ch, bool required = true) {
+    return TrBn{s.need(i, ch, required), s.need(i + 1, ch, required), s.need(i + 2, ch, required),
+                s.need(i + 3, ch, required)};
+  };
+  const auto hook = [&](auto launch) { return run_hook(c, fn, stream, {}, launch); };
+
+  switch (d->op) {
+    case BT_TRAIN_GEMM: {
+      const int Mi = static_cast<int>(M), N = d->N, K = d->K;
+      if (M < 1 || M > INT32_MAX || N < 1 || K < 1 || d->a_rs < 0 || d->a_cs < 0 || d->b_rs < 0 || d->b_cs < 0 ||
+          d->ldc < N || d->splits < 0 || (N + 63) / 64 > 65535)
+        return bad("need 1 <= M < 2^31, N, K >= 1 (N <= 65535 * 64), strides >= 0, ldc >= N and splits >= 0");
+      const int splits = d->splits ? d->splits : tr_dw_splits(K, Mi, N);
+      const int parts = tr_gemm_parts(K, splits);
+      const TrMat A{s.need(0, extent({{M, d->a_rs}, {K, d->a_cs}})), d->a_rs, d->a_cs};
+      const TrMat Bm{s.need(1, extent({{N, d->b_rs}, {K, d->b_cs}})), d->b_rs, d->b_cs};
+      float* Cp = s.need(2, extent({{M, d->ldc}, {N, 1}}));
+      const float* bias = s.need(3, N, false);
+      if (s.present(4) && d->ldr < N) return bad("resid needs ldr >= N");
+      const float* resid = s.need(4, extent({{M, d->ldr}, {N, 1}}), false);
+      float* gelu = s.need(5, extent({{M, d->ldc}, {N, 1}}), false);
+      if (splits > 1 && (bias || resid || gelu)) return bad("a split GEMM takes no bias, resid or gelu_out");
+      if (parts > 65535) return bad("more than 65535 K parts");
+      if (parts > 1 && d->ldc != N) return bad("a GEMM of several K parts needs ldc = N (tr_reduce writes rows of N)");
+      int64_t part_n = 0;
+      if (parts > 1 && __builtin_mul_overflow(int64_t{parts} * N, M, &part_n)) part_n = -1;
+      float* part = s.need(6, part_n, parts > 1);
+      if (const int r = slots()) return r;
+      return hook([&](cudaStream_t st) {
+        const TrGemmOut o{parts > 1 ? part : Cp, d->ldc, M * N, bias, resid, d->ldr, gelu};
+        launch_tr_gemm(A, Bm, o, Mi, N, K, splits, st);
+        BT_LAUNCHED(c, "train_gemm", st);
+        if (parts == 1) return BT_OK;
+        launch_tr_reduce(part, parts, M * N, d->scale, Cp, st);
+        return check_launch(c, "train_reduce", st);
+      });
+    }
+    case BT_TRAIN_REDUCE: {
+      if (!elementwise(M) || d->splits < 1 || d->splits > 65535)
+        return bad("need 1 <= M <= 2^31 * 256 elements and 1 <= splits <= 65535 parts");
+      const float* part = s.need(0, d->splits * M);
+      float* out = s.need(1, M);
+      if (const int r = slots()) return r;
+      return hook([&](cudaStream_t st) {
+        launch_tr_reduce(part, d->splits, M, d->scale, out, st);
+        return check_launch(c, "train_reduce", st);
+      });
+    }
+    case BT_TRAIN_COLSUM: {
+      const int N = d->N;
+      if (M < 1 || N < 1 || d->splits < 0 || (N + 31) / 32 > kMaxGrid1)
+        return bad("need M, N >= 1 and splits >= 0");
+      const int splits = d->splits ? d->splits : tr_colsum_splits(M, N);
+      const int64_t rps = (M + std::max(splits, 1) - 1) / std::max(splits, 1), parts = (M + rps - 1) / rps;
+      if (splits < 1 || parts > 65535) return bad("the split gives no part or more than 65535 parts");
+      const float* A = s.need(0, M * N);
+      const float* Bm = s.need(1, M * N, false);
+      const float* rs = s.need(2, M, false);
+      float* part = s.need(3, parts * N);
+      float* out = s.need(4, N);
+      if (const int r = slots()) return r;
+      return hook([&](cudaStream_t st) {
+        const int z = launch_tr_colsum(A, Bm, rs, M, N, splits, part, st);
+        BT_LAUNCHED(c, "train_colsum", st);
+        launch_tr_reduce(part, z, N, d->scale, out, st);
+        return check_launch(c, "train_reduce", st);
+      });
+    }
+    case BT_TRAIN_RMS_FWD:
+    case BT_TRAIN_RMS_BWD: {
+      if (M < 1 || (M + 7) / 8 > kMaxGrid1 || C < 1) return bad("need M >= 1 rows (M / 8 < 2^31) and C >= 1");
+      if (d->op == BT_TRAIN_RMS_FWD) {
+        const float* x = s.need(0, M * C);
+        const float* gamma = s.need(1, C);
+        float* xn = s.need(2, M * C);
+        float* inv = s.need(3, M);
+        if (const int r = slots()) return r;
+        return hook([&](cudaStream_t st) {
+          launch_tr_rms_fwd(x, gamma, M, C, xn, inv, st);
+          return check_launch(c, "train_rmsnorm", st);
+        });
+      }
+      const float* dxn = s.need(0, M * C);
+      const float* x = s.need(1, M * C);
+      const float* inv = s.need(2, M);
+      const float* gamma = s.need(3, C);
+      float* dres = s.need(4, M * C);
+      if (const int r = slots()) return r;
+      return hook([&](cudaStream_t st) {
+        launch_tr_rms_bwd(dxn, x, inv, gamma, M, C, d->flag != 0, dres, st);
+        return check_launch(c, "train_rmsnorm_bwd", st);
+      });
+    }
+    case BT_TRAIN_BN_GELU_FWD:
+    case BT_TRAIN_BN_GELU_BWD:
+    case BT_TRAIN_BN_SCALE: {
+      if (!elementwise(M) || C < 1) return bad("need 1 <= M <= 2^31 * 256 elements and C >= 1 channels");
+      if (d->op == BT_TRAIN_BN_GELU_FWD) {
+        const float* z = s.need(0, M);
+        const TrBn b = bn_at(1, C);
+        float* y = s.need(5, M);
+        if (const int r = slots()) return r;
+        return hook([&](cudaStream_t st) {
+          launch_tr_bn_gelu_fwd(z, b, M, C, y, st);
+          return check_launch(c, "train_bn_gelu", st);
+        });
+      }
+      if (d->op == BT_TRAIN_BN_SCALE) {
+        const float* g = s.need(0, M);
+        const TrBn b = bn_at(1, C);
+        float* dx = s.need(5, M);
+        if (const int r = slots()) return r;
+        return hook([&](cudaStream_t st) {
+          launch_tr_bn_scale(g, b, M, C, dx, st);
+          return check_launch(c, "train_bn_scale", st);
+        });
+      }
+      const float* dy = s.need(0, M);
+      const float* z = s.need(1, M);
+      const TrBn b = bn_at(2, C);
+      float* dbn = s.need(6, M);
+      float* dz = s.need(7, M);
+      if (const int r = slots()) return r;
+      return hook([&](cudaStream_t st) {
+        launch_tr_bn_gelu_bwd(dy, z, b, M, C, dbn, dz, st);
+        return check_launch(c, "train_bn_gelu_bwd", st);
+      });
+    }
+    case BT_TRAIN_BN_GRADS: {
+      if (C < 1) return bad("need C >= 1");
+      const float* sgz = s.need(0, C);
+      const float* sg = s.need(1, C);
+      const TrBn b = bn_at(2, C);
+      float* dw = s.need(6, C, false);
+      float* db = s.need(7, C, false);
+      if (const int r = slots()) return r;
+      return hook([&](cudaStream_t st) {
+        launch_tr_bn_grads(sgz, sg, b, C, dw, db, st);
+        return check_launch(c, "train_bn_grads", st);
+      });
+    }
+    case BT_TRAIN_GELU_BWD: {
+      if (!elementwise(M)) return bad("need 1 <= M <= 2^31 * 256 elements");
+      const float* da = s.need(0, M);
+      const float* h = s.need(1, M);
+      float* dh = s.need(2, M);
+      if (const int r = slots()) return r;
+      return hook([&](cudaStream_t st) {
+        launch_tr_gelu_bwd(da, h, M, dh, st);
+        return check_launch(c, "train_gelu_bwd", st);
+      });
+    }
+    case BT_TRAIN_IM2COL:
+    case BT_TRAIN_COL2IM: {
+      if (d->B < 1 || d->F < 1 || d->S < 1 || d->L < 1 || C < 1 || d->sb < 0 || d->sf < 0 || d->st < 0 || d->sc < 0 ||
+          int64_t{C} * d->S * 3 > INT32_MAX || int64_t{d->F} * d->S > INT32_MAX)
+        return bad("need B, F, S, L, C >= 1, C S 3 and F S < 2^31, and strides >= 0");
+      const TrImg g{d->B, d->F, d->S, d->L, C, d->sb, d->sf, d->st, d->sc};
+      const int64_t in_n = extent({{d->B, d->sb}, {int64_t{d->F} * d->S, d->sf}, {d->L, d->st}, {C, d->sc}});
+      const int64_t col_n = int64_t{d->B} * d->F * d->L * C * d->S * 3;
+      if (!elementwise(col_n)) return bad("more than 2^31 * 256 im2col elements");
+      if (d->op == BT_TRAIN_IM2COL) {
+        const float* in = s.need(0, in_n);
+        float* col = s.need(1, col_n);
+        const TrBn b = bn_at(2, int64_t{d->F} * d->S, d->flag != 0);
+        if (const int r = slots()) return r;
+        return hook([&](cudaStream_t st) {
+          launch_tr_im2col(in, g, d->flag ? &b : nullptr, col, st);
+          return check_launch(c, "train_im2col", st);
+        });
+      }
+      const float* dcol = s.need(0, col_n);
+      float* din = s.need(1, in_n);
+      if (const int r = slots()) return r;
+      return hook([&](cudaStream_t st) {
+        launch_tr_col2im(dcol, g, din, st);
+        return check_launch(c, "train_col2im", st);
+      });
+    }
+    case BT_TRAIN_CONCAT: {
+      const int64_t n = int64_t{d->B} * d->F * d->L * C;
+      if (d->B < 1 || d->F < 1 || d->L < 1 || C < 1 || int64_t{C} * d->F > INT32_MAX || !elementwise(n))
+        return bad("need B, F, L, C >= 1, C F < 2^31 and B F L C <= 2^31 * 256");
+      const float* src = s.need(0, n);
+      float* dst = s.need(1, n);
+      if (const int r = slots()) return r;
+      return hook([&](cudaStream_t st) {
+        launch_tr_concat(src, d->B, d->F, d->L, C, d->flag != 0, dst, st);
+        return check_launch(c, "train_concat", st);
+      });
+    }
+    case BT_TRAIN_ROPE: {
+      if (M < 1 || C < 32 || C % 32 != 0 || !elementwise(M * C) || d->L < 1 || (d->posmode != 0 && d->posmode != 1) ||
+          (d->posmode == 1 && d->F < 1))
+        return bad("need M >= 1, C a multiple of 32, M C <= 2^31 * 256, L >= 1 and posmode 0 or 1 (1: F >= 1)");
+      float* qkv = s.need(0, M * 3 * C);
+      const float* freqs = s.need(1, 16);
+      if (const int r = slots()) return r;
+      return hook([&](cudaStream_t st) {
+        launch_tr_rope(qkv, freqs, M, C, d->L, d->F, d->posmode, d->flag != 0, st);
+        return check_launch(c, "train_rope", st);
+      });
+    }
+    case BT_TRAIN_GATE_FWD:
+    case BT_TRAIN_GATE_BWD: {
+      if (M < 1 || C < 32 || C % 32 != 0 || !elementwise(M * C))
+        return bad("need M >= 1, C a multiple of 32 and M C <= 2^31 * 256");
+      const int64_t heads = M * (C / 32);
+      if (d->op == BT_TRAIN_GATE_FWD) {
+        const float* O = s.need(0, M * C);
+        const float* g = s.need(1, heads);
+        float* G = s.need(2, M * C);
+        if (const int r = slots()) return r;
+        return hook([&](cudaStream_t st) {
+          launch_tr_gate_fwd(O, g, M, C, G, st);
+          return check_launch(c, "train_gate", st);
+        });
+      }
+      float* dG = s.need(0, M * C);
+      const float* O = s.need(1, M * C);
+      const float* g = s.need(2, heads);
+      float* dg = s.need(3, heads);
+      float* delta = s.need(4, heads);
+      if (const int r = slots()) return r;
+      return hook([&](cudaStream_t st) {
+        launch_tr_gate_bwd(dG, O, g, M, C, dg, delta, st);
+        return check_launch(c, "train_gate_bwd", st);
+      });
+    }
+    case BT_TRAIN_HEAD_FWD:
+    case BT_TRAIN_HEAD_BWD: {
+      if (!elementwise(M)) return bad("need 1 <= M <= 2^31 * 256 rows");
+      if (d->op == BT_TRAIN_HEAD_FWD) {
+        const float* o = s.need(0, 2 * M);
+        float* beat = s.need(1, M);
+        float* down = s.need(2, M);
+        if (const int r = slots()) return r;
+        return hook([&](cudaStream_t st) {
+          launch_tr_head_fwd(o, M, d->flag != 0, beat, down, st);
+          return check_launch(c, "train_head", st);
+        });
+      }
+      const float* dbeat = s.need(0, M);
+      const float* ddown = s.need(1, M);
+      float* dout = s.need(2, 2 * M);
+      if (const int r = slots()) return r;
+      return hook([&](cudaStream_t st) {
+        launch_tr_head_bwd(dbeat, ddown, M, d->flag != 0, dout, st);
+        return check_launch(c, "train_head", st);
+      });
+    }
+    case BT_TRAIN_ATTN_FWD:
+    case BT_TRAIN_ATTN_DQ:
+    case BT_TRAIN_ATTN_DKV: {
+      const TrSeqs q{d->seqs, d->n, d->heads, d->seq_in, d->s_out, d->s_in, d->s_pos};
+      if (q.seqs < 1 || q.n < 1 || q.heads < 1 || q.heads > 65535 || q.seq_in < 1 || q.s_out < 0 || q.s_in < 0 ||
+          q.s_pos < 0 || int64_t{q.seqs} * ((q.n + 63) / 64) > kMaxGrid1)
+        return bad("need seqs, n, seq_in >= 1, 1 <= heads <= 65535, strides >= 0 and seqs ceil(n / 64) < 2^31");
+      // the largest token row: the last sequence, or the last of the sequence block before it
+      const int64_t ql = (q.seqs - 1) / q.seq_in, rl = (q.seqs - 1) % q.seq_in;
+      int64_t r0 = extent({{ql + 1, q.s_out}, {rl + 1, q.s_in}});
+      if (ql > 0) r0 = std::max(r0, extent({{ql, q.s_out}, {q.seq_in, q.s_in}}));
+      const int64_t rows = r0 < 0 ? -1 : extent({{r0, 1}, {q.n, q.s_pos}});
+      const int64_t Cq = int64_t{q.heads} * 32;
+      const auto n_of = [&](int64_t per_row) {  // elements of an array of `rows` rows of per_row
+        int64_t e;
+        return rows < 0 || __builtin_mul_overflow(rows, per_row, &e) ? -1 : e;
+      };
+      const float* qkv = s.need(0, n_of(3 * Cq), true, true);
+      if (d->op == BT_TRAIN_ATTN_FWD) {
+        float* O = s.need(1, n_of(Cq), true, true);
+        float* lse = s.need(2, n_of(q.heads));
+        if (const int r = slots()) return r;
+        return hook([&](cudaStream_t st) {
+          launch_tr_attn_fwd(qkv, q, O, lse, st);
+          return check_launch(c, "train_attention", st);
+        });
+      }
+      const float* dO = s.need(1, n_of(Cq), true, true);
+      const float* lse = s.need(2, n_of(q.heads));
+      const float* delta = s.need(3, n_of(q.heads));
+      float* dqkv = s.need(4, n_of(3 * Cq), true, true);
+      if (const int r = slots()) return r;
+      const bool dq = d->op == BT_TRAIN_ATTN_DQ;
+      return hook([&](cudaStream_t st) {
+        if (dq) launch_tr_attn_dq(qkv, dO, lse, delta, q, dqkv, st);
+        else launch_tr_attn_dkv(qkv, dO, lse, delta, q, dqkv, st);
+        return check_launch(c, dq ? "train_attention_dq" : "train_attention_dkv", st);
+      });
+    }
+    default:
+      return bad("unknown op");
+  }
+}
+
+}  // extern "C"

@@ -138,7 +138,6 @@ TrModel train_model(const bt_hparams& hp, int64_t B, int64_t L) {
 
 // Scratch of one call, in floats: the stream gradient, the im2col / FFN-hidden buffer, two [tokens, channels] buffers,
 // q/k/v gradients, per-head rows, and split-K / column-sum partials.
-constexpr int64_t kPartFloats = int64_t{8} << 20;
 struct TrScratch {
   float *dcur, *big, *s1, *s2, *dqkv, *hd1, *hd2, *part;
 };
@@ -147,7 +146,7 @@ int64_t scratch_floats(int64_t BL) {
   // D <= 1024), 4096 for the FFN hidden (4 * 32 * 32, or ff_mult D) and the convolutions' im2col (3 * 2 * C * F), 32
   // per-head values (F heads <= 32 in the frontend, D / 32 in the main layers); and one value per channel, at least, for
   // the column sums of the BatchNorm gradients
-  return BL * (3 * 1024 + 4096 + 3 * 1024 + 2 * 32) + 2 * 1024 + kPartFloats;
+  return BL * (3 * 1024 + 4096 + 3 * 1024 + 2 * 32) + 2 * 1024 + kTrPartFloats;
 }
 
 struct TrRun {
@@ -177,12 +176,10 @@ struct TrRun {
   // dW[N, K] = dY[M, N]^T X[M, K], split over M with a fixed-order reduction; dW null: not wanted
   int grad_weight(const float* dY, int64_t M, int N, const float* X, int K, float* dW) {
     if (!dW) return BT_OK;
-    const int64_t tiles = int64_t{ceil_div(N, 64)} * ceil_div(K, 64);
-    int64_t splits = std::min<int64_t>(ceil_div64(2 * 132, tiles), std::max<int64_t>(1, M / 256));
-    splits = std::max<int64_t>(1, std::min<int64_t>(splits, kPartFloats / (int64_t{N} * K)));
-    const int parts = tr_gemm_parts(static_cast<int>(M), static_cast<int>(splits));
+    const int splits = tr_dw_splits(M, N, K);
+    const int parts = tr_gemm_parts(static_cast<int>(M), splits);
     launch_tr_gemm({dY, 1, N}, {X, 1, K}, {parts > 1 ? s.part : dW, K, int64_t{N} * K, nullptr, nullptr, 0, nullptr}, N,
-                   K, static_cast<int>(M), static_cast<int>(splits), st);
+                   K, static_cast<int>(M), splits, st);
     if (const int r = check_launch(c, "train_gemm_dw", st)) return r;
     if (parts == 1) return BT_OK;
     launch_tr_reduce(s.part, parts, int64_t{N} * K, 1.f, dW, st);
@@ -191,8 +188,7 @@ struct TrRun {
   // out[n] = scale sum_m A[m, n] (B[m, n]) (rs[m])
   int colsum(const float* A, const float* Bm, const float* rs, int64_t M, int N, float scale, float* out) {
     if (!out) return BT_OK;
-    const int parts = launch_tr_colsum(A, Bm, rs, M, N, static_cast<int>(std::min<int64_t>(
-                                                            ceil_div64(M, 512), kPartFloats / N)), s.part, st);
+    const int parts = launch_tr_colsum(A, Bm, rs, M, N, tr_colsum_splits(M, N), s.part, st);
     if (const int r = check_launch(c, "train_colsum", st)) return r;
     launch_tr_reduce(s.part, parts, N, scale, out, st);
     return check_launch(c, "train_reduce", st);
@@ -420,7 +416,7 @@ int train_scratch(bt_ctx* c, int64_t BL, TrScratch* s) {
   };
   s->dcur = take(BL * 1024), s->s1 = take(BL * 1024), s->s2 = take(BL * 1024), s->big = take(BL * 4096);
   s->dqkv = take(BL * 3072), s->hd1 = take(BL * 32 + 1024), s->hd2 = take(BL * 32 + 1024);
-  s->part = take(kPartFloats);
+  s->part = take(kTrPartFloats);
   return BT_OK;
 }
 

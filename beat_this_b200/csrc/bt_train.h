@@ -1,5 +1,7 @@
 // Launchers of kernels_train.cu, the fp32 training forward and backward (api_train.cu drives them).
 #pragma once
+#include <algorithm>
+
 #include "bt_kernels.h"
 
 namespace bt {
@@ -40,6 +42,20 @@ struct TrSeqs {
 // launch_tr_reduce
 inline int tr_gemm_kc(int K, int splits) { return ((K + splits - 1) / splits + 15) / 16 * 16; }
 inline int tr_gemm_parts(int K, int splits) { return (K + tr_gemm_kc(K, splits) - 1) / tr_gemm_kc(K, splits); }
+
+// Floats of the training pass's split-K / column-sum partials (its scratch holds one such block).
+constexpr int64_t kTrPartFloats = int64_t{8} << 20;
+// The split policy of a weight gradient dW[N, K] = dY[M, N]^T X[M, K] (a tr_gemm of N x K outputs over M): enough
+// parts to give two CTAs per SM of 132, at least 256 rows each, and all parts inside kTrPartFloats.
+inline int tr_dw_splits(int64_t M, int N, int K) {
+  const int64_t tiles = int64_t{(N + 63) / 64} * ((K + 63) / 64);
+  int64_t splits = std::min<int64_t>((2 * 132 + tiles - 1) / tiles, std::max<int64_t>(1, M / 256));
+  return static_cast<int>(std::max<int64_t>(1, std::min<int64_t>(splits, kTrPartFloats / (int64_t{N} * K))));
+}
+// The split policy of a column sum over M rows of N columns: 512 rows per part, all parts inside kTrPartFloats.
+inline int tr_colsum_splits(int64_t M, int N) {
+  return static_cast<int>(std::min<int64_t>((M + 511) / 512, kTrPartFloats / N));
+}
 void launch_tr_gemm(const TrMat& A, const TrMat& B, const TrGemmOut& o, int M, int N, int K, int splits, cudaStream_t st);
 void launch_tr_reduce(const float* part, int Z, int64_t n, float scale, float* out, cudaStream_t st);
 // column sums of [M, N] A (times B, times rs[m], where given) over up to `splits` row ranges: returns the parts written

@@ -575,6 +575,21 @@ class Engine:
                    p(dgates, gates.numel()))
         return y, dqkv, dgates
 
+    def debug_train_kernel(self, op: str, arrays, **desc):
+        """bt_debug_train_kernel: the training kernel(s) of `op` (one of _lib.TRAIN_OPS) on `arrays`, the op's slots in
+        the order include/beatthis.h lists them (None: absent), each a contiguous fp32 device tensor whose whole length
+        is its element count; outputs are written in place.  desc: the bt_debug_train_desc fields the op reads."""
+        d = _lib.bt_debug_train_desc()
+        d.op = _lib.TRAIN_OPS.index(op)
+        for k, v in desc.items():
+            if not hasattr(d, k):
+                raise TypeError(f"bt_debug_train_desc has no field {k}")
+            setattr(d, k, v)
+        n = len(arrays)
+        ptrs = (c_void_p * max(n, 1))(*[self._dev_ptr(a) for a in arrays])
+        counts = (ctypes.c_int64 * max(n, 1))(*[0 if a is None else a.numel() for a in arrays])
+        self._call("bt_debug_train_kernel", ctypes.byref(d), ptrs, counts, n)
+
     def debug_attention_freq(self, q, k, v, gates, B, F, out=None):
         """gates * softmax over the F planes of each (chunk, frame, head); q/k/v [B*F*L, heads*32], gates [B*F*L, heads].
         out as for debug_attention (None: a new tensor shaped like q).  Returns out."""

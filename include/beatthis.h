@@ -559,6 +559,64 @@ int bt_debug_attention_backward(bt_ctx* ctx, const float* qkv_dev, const float* 
                                 const float* dy_dev, int32_t seqs, int32_t n, int32_t heads, float* y_dev,
                                 float* dqkv_dev, float* dgates_dev, void* stream);
 
+/* Test hook (ABI 2.13; fp32 ctx only, BT_ERR_ARG for a 16-bit one): one training kernel alone, through the launcher
+ * bt_train_forward / bt_train_backward call, on the caller's fp32 device arrays.  arrays_dev[i] holds counts[i]
+ * elements (i < n_arrays; a missing or NULL slot is absent).  The slots of each op, in order (? optional, * written):
+ *   GEMM      A, B, C*, bias?, resid?, gelu_out?*, part?*   C[m, n] (ldc) = sum_k A(m, k) B(n, k) (+ bias[n])
+ *             (+ resid[m ldr + n]) over M x N x K, A(m, k) = A[m a_rs + k a_cs], B likewise; gelu_out (ldc) = GELU(C).
+ *             splits (0: the weight-gradient policy of the training pass) > 1 runs tr_gemm into part [parts, M, N] and
+ *             tr_reduce (scale) into C, which then needs ldc = N and no bias, resid or gelu_out.  resid may alias C.
+ *   REDUCE    part [splits, M], out* [M]           out = scale sum_z part[z]
+ *   COLSUM    A, B?, rs?, part*, out*              A, B [M, N], rs [M]: part [parts, N] of up to `splits` row ranges
+ *             (0: the training pass's policy) of A (* B) (* rs[m]), then out [N] = scale sum of the parts
+ *   RMS_FWD   x, gamma, xn*, inv*                  [M, C], gamma [C], inv [M]
+ *   RMS_BWD   dxn, x, inv, gamma, dres*            dres [M, C] = (flag ? dres : 0) + dx
+ *   BN_GELU_FWD  z, w, b, rm, rv, y*               [M] elements of C channels (index % C), BatchNorm arrays [C]
+ *   BN_GELU_BWD  dy, z, w, b, rm, rv, dbn*, dz*
+ *   BN_GRADS  s_gz, s_g, w, b, rm, rv, dw?*, db?*  [C]
+ *   BN_SCALE  g, w, b, rm, rv, dx*                 [M] elements of C channels
+ *   GELU_BWD  da, h, dh*                           [M]; dh may be da (in place)
+ *   IM2COL    in, col*, w?, b?, rm?, rv?           flag: through the 1-d BatchNorm of the input's F S frequencies;
+ *             input element (b, f, t, c) of B x (F S) x L x C at b sb + f sf + t st + c sc; col [B F L, C S 3]
+ *   COL2IM    dcol, din*                           the adjoint of IM2COL without BatchNorm
+ *   CONCAT    src, dst*                            [B F L C] tokens <-> [B L, C F] rows (flag: backward)
+ *   ROPE      qkv*, freqs                          qkv [M, 3C] in place, freqs [16]; posmode, L, F; flag: inverse
+ *   GATE_FWD  O, g, G*                             O, G [M, C], g [M, C / 32]
+ *   GATE_BWD  dG*, O, g, dg*, delta*               dG [M, C] becomes dO; dg, delta [M, C / 32]
+ *   HEAD_FWD  o, beat*, down*                      o [M, 2]; flag: sum head
+ *   HEAD_BWD  dbeat, ddown, dout*                  dout [M, 2]
+ *   ATTN_FWD  qkv, O*, lse*                        over the TrSeqs (seqs, n, heads, seq_in, s_out, s_in, s_pos): token
+ *             row r = (s / seq_in) s_out + (s % seq_in) s_in + i s_pos of qkv [*, 3C], O [*, C], lse [*, heads]
+ *   ATTN_DQ   qkv, dO, lse, delta, dqkv*           dO [*, C], delta [*, heads]; the q columns of dqkv [*, 3C]
+ *   ATTN_DKV  qkv, dO, lse, delta, dqkv*           the k and v columns of dqkv
+ * Beyond the hook rules below: a geometry or stride that would take a kernel outside an array's count, a negative
+ * stride, a launch grid out of range, or a misaligned pointer where the kernel moves float4 (qkv, O, dO and dqkv of
+ * the attention ops) is BT_ERR_ARG with nothing enqueued.  The kernels count and profile under the names the
+ * training pass gives them (train_gemm, train_reduce, train_colsum + train_reduce, train_rmsnorm, train_rmsnorm_bwd,
+ * train_bn_gelu, train_bn_gelu_bwd, train_bn_grads, train_bn_scale, train_gelu_bwd, train_im2col, train_col2im,
+ * train_concat, train_rope, train_gate, train_gate_bwd, train_head, train_attention, train_attention_dq,
+ * train_attention_dkv).  Synchronises the stream before it returns. */
+enum {
+  BT_TRAIN_GEMM, BT_TRAIN_REDUCE, BT_TRAIN_COLSUM, BT_TRAIN_RMS_FWD, BT_TRAIN_RMS_BWD, BT_TRAIN_BN_GELU_FWD,
+  BT_TRAIN_BN_GELU_BWD, BT_TRAIN_BN_GRADS, BT_TRAIN_BN_SCALE, BT_TRAIN_GELU_BWD, BT_TRAIN_IM2COL, BT_TRAIN_COL2IM,
+  BT_TRAIN_CONCAT, BT_TRAIN_ROPE, BT_TRAIN_GATE_FWD, BT_TRAIN_GATE_BWD, BT_TRAIN_HEAD_FWD, BT_TRAIN_HEAD_BWD,
+  BT_TRAIN_ATTN_FWD, BT_TRAIN_ATTN_DQ, BT_TRAIN_ATTN_DKV, BT_TRAIN_OPS
+};
+typedef struct bt_debug_train_desc {
+  int32_t op, splits;  /* BT_TRAIN_*; GEMM / COLSUM: parts (0: policy), REDUCE: parts */
+  int64_t M;           /* rows (GEMM, COLSUM, RMS_*, ROPE, GATE_*, HEAD_*), elements (REDUCE, BN_*, GELU_BWD) */
+  int32_t N, K, C;     /* GEMM: N x K; COLSUM: N columns; C: channels */
+  int32_t flag;        /* RMS_BWD add, IM2COL BatchNorm, CONCAT backward, ROPE inverse, HEAD_* sum head */
+  float scale;         /* REDUCE, COLSUM */
+  int64_t a_rs, a_cs, b_rs, b_cs, ldc, ldr;  /* GEMM */
+  int32_t B, F, L, S, posmode, heads;        /* IM2COL / COL2IM (F: output frequencies), CONCAT, ROPE; attention */
+  int64_t sb, sf, st, sc;                    /* IM2COL / COL2IM input strides */
+  int32_t seqs, n, seq_in, pad_;             /* attention sequences */
+  int64_t s_out, s_in, s_pos;
+} bt_debug_train_desc;
+int bt_debug_train_kernel(bt_ctx* ctx, const bt_debug_train_desc* desc, float* const* arrays_dev, const int64_t* counts,
+                          int32_t n_arrays, void* stream);
+
 /* ---- introspection / tuning ----------------------------------------------------------------- */
 
 /* Upper bound on the chunks processed per wave (1..256, default 128; one wave = one launch of every kernel of the
