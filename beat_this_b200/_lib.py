@@ -105,6 +105,21 @@ class bt_debug_train_desc(ctypes.Structure):
         ("s_out", c_int64),
         ("s_in", c_int64),
         ("s_pos", c_int64),
+        ("seed", ctypes.c_uint64),
+        ("p", c_float),
+        ("site", ctypes.c_uint32),
+        ("e0", c_int64),
+        ("beta", c_float),
+        ("pad2_", c_int32),
+        ("bn_n", c_int64),
+    ]
+
+
+class bt_train_mode(ctypes.Structure):
+    _fields_ = [
+        ("seed", ctypes.c_uint64),
+        ("dropout_frontend", c_float),
+        ("dropout_transformer", c_float),
     ]
 
 
@@ -281,6 +296,15 @@ PROTOTYPES = {
     "bt_train_backward": (
         c_int, [c_void_p, POINTER(c_void_p), c_int32, c_void_p, c_int64, c_int32, c_int32, c_void_p, c_void_p,
                 POINTER(c_void_p), c_void_p, c_void_p],
+    ),
+    "bt_train_activation_bytes_ex": (c_int64, [c_void_p, c_int32, c_int32, POINTER(bt_train_mode)]),
+    "bt_train_forward_ex": (
+        c_int, [c_void_p, POINTER(c_void_p), c_int32, POINTER(c_void_p), c_void_p, c_int32, c_int32,
+                POINTER(bt_train_mode), c_void_p, c_int64, c_void_p, c_void_p, c_void_p],
+    ),
+    "bt_train_backward_ex": (
+        c_int, [c_void_p, POINTER(c_void_p), c_int32, c_void_p, c_int64, c_int32, c_int32, POINTER(bt_train_mode),
+                c_void_p, c_void_p, POINTER(c_void_p), c_void_p, c_void_p],
     ),
     "bt_debug_attention_backward": (
         c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p,

@@ -422,6 +422,8 @@ int bt_debug_train_kernel(bt_ctx* c, const bt_debug_train_desc* d, float* const*
                 s.need(i + 3, ch, required)};
   };
   const auto hook = [&](auto launch) { return run_hook(c, fn, stream, {}, launch); };
+  if (!(d->p >= 0.f && d->p < 1.f) || d->e0 < 0) return bad("need a dropout rate in [0, 1) and e0 >= 0");
+  const TrDrop drop = tr_drop(d->seed, d->site, d->p, d->e0);
 
   switch (d->op) {
     case BT_TRAIN_GEMM: {
@@ -438,7 +440,8 @@ int bt_debug_train_kernel(bt_ctx* c, const bt_debug_train_desc* d, float* const*
       if (s.present(4) && d->ldr < N) return bad("resid needs ldr >= N");
       const float* resid = s.need(4, extent({{M, d->ldr}, {N, 1}}), false);
       float* gelu = s.need(5, extent({{M, d->ldc}, {N, 1}}), false);
-      if (splits > 1 && (bias || resid || gelu)) return bad("a split GEMM takes no bias, resid or gelu_out");
+      if (splits > 1 && (bias || resid || gelu || drop.thresh))
+        return bad("a split GEMM takes no bias, resid, gelu_out or dropout");
       if (parts > 65535) return bad("more than 65535 K parts");
       if (parts > 1 && d->ldc != N) return bad("a GEMM of several K parts needs ldc = N (tr_reduce writes rows of N)");
       int64_t part_n = 0;
@@ -446,7 +449,7 @@ int bt_debug_train_kernel(bt_ctx* c, const bt_debug_train_desc* d, float* const*
       float* part = s.need(6, part_n, parts > 1);
       if (const int r = slots()) return r;
       return hook([&](cudaStream_t st) {
-        const TrGemmOut o{parts > 1 ? part : Cp, d->ldc, M * N, bias, resid, d->ldr, gelu};
+        const TrGemmOut o{parts > 1 ? part : Cp, d->ldc, M * N, bias, resid, d->ldr, gelu, drop};
         launch_tr_gemm(A, Bm, o, Mi, N, K, splits, st);
         BT_LAUNCHED(c, "train_gemm", st);
         if (parts == 1) return BT_OK;
@@ -461,7 +464,7 @@ int bt_debug_train_kernel(bt_ctx* c, const bt_debug_train_desc* d, float* const*
       float* out = s.need(1, M);
       if (const int r = slots()) return r;
       return hook([&](cudaStream_t st) {
-        launch_tr_reduce(part, d->splits, M, d->scale, out, st);
+        launch_tr_reduce(part, d->splits, M, d->scale, out, st, d->beta, drop);
         return check_launch(c, "train_reduce", st);
       });
     }
@@ -477,9 +480,10 @@ int bt_debug_train_kernel(bt_ctx* c, const bt_debug_train_desc* d, float* const*
       const float* rs = s.need(2, M, false);
       float* part = s.need(3, parts * N);
       float* out = s.need(4, N);
+      const float* shift = s.need(5, N, false);
       if (const int r = slots()) return r;
       return hook([&](cudaStream_t st) {
-        const int z = launch_tr_colsum(A, Bm, rs, M, N, splits, part, st);
+        const int z = launch_tr_colsum(A, Bm, rs, M, N, splits, part, st, shift);
         BT_LAUNCHED(c, "train_colsum", st);
         launch_tr_reduce(part, z, N, d->scale, out, st);
         return check_launch(c, "train_reduce", st);
@@ -528,9 +532,13 @@ int bt_debug_train_kernel(bt_ctx* c, const bt_debug_train_desc* d, float* const*
         const float* g = s.need(0, M);
         const TrBn b = bn_at(1, C);
         float* dx = s.need(5, M);
+        const bool batch = s.present(6);
+        if (batch && d->bn_n < 1) return bad("batch statistics need bn_n >= 1 positions");
+        const TrBnBatch bb{s.need(6, M, false), s.need(7, C, batch), s.need(8, C, batch),
+                           static_cast<float>(1.0 / static_cast<double>(std::max<int64_t>(d->bn_n, 1)))};
         if (const int r = slots()) return r;
         return hook([&](cudaStream_t st) {
-          launch_tr_bn_scale(g, b, M, C, dx, st);
+          launch_tr_bn_scale(g, b, M, C, dx, st, batch ? &bb : nullptr);
           return check_launch(c, "train_bn_scale", st);
         });
       }
@@ -565,7 +573,7 @@ int bt_debug_train_kernel(bt_ctx* c, const bt_debug_train_desc* d, float* const*
       float* dh = s.need(2, M);
       if (const int r = slots()) return r;
       return hook([&](cudaStream_t st) {
-        launch_tr_gelu_bwd(da, h, M, dh, st);
+        launch_tr_gelu_bwd(da, h, M, dh, st, drop);
         return check_launch(c, "train_gelu_bwd", st);
       });
     }
@@ -691,7 +699,7 @@ int bt_debug_train_kernel(bt_ctx* c, const bt_debug_train_desc* d, float* const*
         float* lse = s.need(2, n_of(q.heads));
         if (const int r = slots()) return r;
         return hook([&](cudaStream_t st) {
-          launch_tr_attn_fwd(qkv, q, O, lse, st);
+          launch_tr_attn_fwd(qkv, q, O, lse, st, drop);
           return check_launch(c, "train_attention", st);
         });
       }
@@ -702,8 +710,8 @@ int bt_debug_train_kernel(bt_ctx* c, const bt_debug_train_desc* d, float* const*
       if (const int r = slots()) return r;
       const bool dq = d->op == BT_TRAIN_ATTN_DQ;
       return hook([&](cudaStream_t st) {
-        if (dq) launch_tr_attn_dq(qkv, dO, lse, delta, q, dqkv, st);
-        else launch_tr_attn_dkv(qkv, dO, lse, delta, q, dqkv, st);
+        if (dq) launch_tr_attn_dq(qkv, dO, lse, delta, q, dqkv, st, drop);
+        else launch_tr_attn_dkv(qkv, dO, lse, delta, q, dqkv, st, drop);
         return check_launch(c, dq ? "train_attention_dq" : "train_attention_dkv", st);
       });
     }

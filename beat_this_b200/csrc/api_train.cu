@@ -1,6 +1,7 @@
 // The training entry points: bt_train_param_count / _info (the reference's state_dict as a table),
-// bt_train_activation_bytes, bt_train_forward and bt_train_backward.  Parameters are the caller's unfolded fp32 device
-// tensors; the forward pass saves what the backward pass reads in the caller's activation store.
+// bt_train_activation_bytes(_ex), bt_train_forward(_ex) and bt_train_backward(_ex).  Parameters are the caller's
+// unfolded fp32 device tensors; the forward pass saves what the backward pass reads in the caller's activation store.
+// A bt_train_mode selects the reference's training-mode function: dropout and batch-statistics BatchNorm.
 #include "api_internal.h"
 #include "bt_train.h"
 #include "common.cuh"
@@ -15,14 +16,22 @@ struct TrParam {
 };
 
 // One step of the model.  p: table index of the step's first parameter.  Offsets (in floats) into the activation
-// store; -1 where the step saves nothing there.
+// store; -1 where the step saves nothing there.  bn1 / bn2 (training mode): the batch mean and, 4-float aligned after
+// it, the biased variance of the step's BatchNorms (the stem: bn1d, bn2d; a conv block: bn2 of its norm).
 enum TrKind { kStem, kAttnFreq, kAttnTime, kFfn, kConvBlock, kLinear, kHead };
 struct TrLayer {
   TrKind kind;
   int p;
   int C, F, mult;  // channels, frequency planes, FFN multiplier
   int64_t in = -1, xn = -1, inv = -1, qkv = -1, gate = -1, lse = -1, o = -1, h = -1, a = -1, z = -1, xl = -1;
+  int64_t bn1 = -1, bn2 = -1;
+  bool frontend = false;  // dropout at the frontend rate
 };
+
+// The dropout site numbering of include/beatthis.h: site k (0 or 1) of step `step` of the layer list.  An attention
+// step's site 0 is its probabilities and site 1 the output of to_out; a feed-forward step's site 0 is the GELU output
+// (net.3) and site 1 the output of net.4 (net.5).
+uint32_t dropout_site(size_t step, int k) { return static_cast<uint32_t>(2 * step + k); }
 
 struct TrModel {
   std::vector<TrParam> table;
@@ -62,8 +71,9 @@ void add_ffn(std::vector<TrParam>& t, const std::string& p, int C, int mult) {
 }
 
 // The parameter table in BeatThis.state_dict() order and, for a batch of B x L frames (B = 0: table only), the steps
-// and their activation store.  Token rows of the frontend: ((b F + f) L + t), C channels.
-TrModel train_model(const bt_hparams& hp, int64_t B, int64_t L) {
+// and their activation store (training mode: the BatchNorms' batch statistics appended).  Token rows of the frontend:
+// ((b F + f) L + t), C channels.
+TrModel train_model(const bt_hparams& hp, int64_t B, int64_t L, bool train = false) {
   TrModel m;
   auto& t = m.table;
   const int64_t BL = B * L;
@@ -72,19 +82,21 @@ TrModel train_model(const bt_hparams& hp, int64_t B, int64_t L) {
     m.floats += (n + 3) & ~int64_t{3};
     return off;
   };
-  auto attn = [&](TrKind kind, const std::string& p, int C, int F) {
+  auto attn = [&](TrKind kind, const std::string& p, int C, int F, bool frontend) {
     TrLayer l{kind, static_cast<int>(t.size()), C, F, 0};
     add_attn(t, p, C);
     const int64_t M = BL * F;
     l.in = alloc(M * C), l.xn = alloc(M * C), l.inv = alloc(M), l.qkv = alloc(3 * M * C), l.gate = alloc(M * C / 32);
     l.lse = alloc(M * C / 32), l.o = alloc(M * C);
+    l.frontend = frontend;
     m.layers.push_back(l);
   };
-  auto ffn = [&](const std::string& p, int C, int F, int mult) {
+  auto ffn = [&](const std::string& p, int C, int F, int mult, bool frontend) {
     TrLayer l{kFfn, static_cast<int>(t.size()), C, F, mult};
     add_ffn(t, p, C, mult);
     const int64_t M = BL * F;
     l.in = alloc(M * C), l.xn = alloc(M * C), l.inv = alloc(M), l.h = alloc(M * mult * C), l.a = alloc(M * mult * C);
+    l.frontend = frontend;
     m.layers.push_back(l);
   };
   {
@@ -99,10 +111,10 @@ TrModel train_model(const bt_hparams& hp, int64_t B, int64_t L) {
   for (int i = 0; i < 3; ++i) {
     const std::string p = "frontend.blocks." + std::to_string(i);
     if (hp.partial_transformers) {
-      attn(kAttnFreq, p + ".partial.attnF", C, F);
-      ffn(p + ".partial.ffF", C, F, 4);
-      attn(kAttnTime, p + ".partial.attnT", C, F);
-      ffn(p + ".partial.ffT", C, F, 4);
+      attn(kAttnFreq, p + ".partial.attnF", C, F, true);
+      ffn(p + ".partial.ffF", C, F, 4, true);
+      attn(kAttnTime, p + ".partial.attnT", C, F, true);
+      ffn(p + ".partial.ffT", C, F, 4, true);
     }
     TrLayer l{kConvBlock, static_cast<int>(t.size()), C, F, 0};
     add(t, p + ".conv2d.weight", {2 * C, C, 2, 3});
@@ -122,8 +134,8 @@ TrModel train_model(const bt_hparams& hp, int64_t B, int64_t L) {
   }
   for (int i = 0; i < hp.n_layers; ++i) {
     const std::string p = "transformer_blocks.layers." + std::to_string(i);
-    attn(kAttnTime, p + ".0", D, 1);
-    ffn(p + ".1", D, 1, hp.ff_mult);
+    attn(kAttnTime, p + ".0", D, 1, false);
+    ffn(p + ".1", D, 1, hp.ff_mult, false);
   }
   {
     TrLayer l{kHead, static_cast<int>(t.size()), D, 1, 0};
@@ -133,6 +145,12 @@ TrModel train_model(const bt_hparams& hp, int64_t B, int64_t L) {
     l.in = alloc(BL * D), l.xn = alloc(BL * D), l.inv = alloc(BL);
     m.layers.push_back(l);
   }
+  if (train)
+    for (TrLayer& l : m.layers) {
+      const auto stats = [&](int ch) { return alloc(2 * ((ch + 3) & ~3)); };
+      if (l.kind == kStem) l.bn1 = stats(hp.spect_dim), l.bn2 = stats(l.C);
+      if (l.kind == kConvBlock) l.bn2 = stats(2 * l.C);
+    }
   return m;
 }
 
@@ -158,14 +176,26 @@ struct TrRun {
   TrScratch s;
   int B, L;
   const float *dbeat, *ddown;  // backward: the gradient at the logits
+  const bt_train_mode* mode;   // null: eval mode
+  float* const* running;       // training-mode forward: the running statistics to update, table order
   const float* w(int i) const { return P[i]; }
   float* at(int64_t off) const { return act + off; }
-  TrBn bn(int p) const { return TrBn{P[p], P[p + 1], P[p + 2], P[p + 3]}; }
+  // the BatchNorm at table index p over ch channels: on its running statistics (eval mode) or on the batch statistics
+  // the forward pass keeps at store offset off
+  TrBn bn(int p, int64_t off, int ch) const {
+    if (!mode) return TrBn{P[p], P[p + 1], P[p + 2], P[p + 3]};
+    return TrBn{P[p], P[p + 1], at(off), at(off + ((ch + 3) & ~3))};
+  }
+  // dropout site k of step `step` (none in eval mode)
+  TrDrop drop(const TrLayer& l, size_t step, int k) const {
+    if (!mode) return TrDrop{};
+    return tr_drop(mode->seed, dropout_site(step, k), l.frontend ? mode->dropout_frontend : mode->dropout_transformer);
+  }
 
-  // out[M, N] = X[M, K] W[N, K]^T (+ bias) (+ resid) (gelu_out: GELU of it as well)
+  // out[M, N] = X[M, K] W[N, K]^T (+ bias) (+ resid) (gelu_out: GELU of it as well), dropout as TrGemmOut states
   int linear(const float* X, int64_t M, int K, const float* W, int N, const float* bias, float* out,
-             const float* resid = nullptr, float* gelu_out = nullptr) {
-    launch_tr_gemm({X, K, 1}, {W, K, 1}, {out, N, 0, bias, resid, N, gelu_out}, static_cast<int>(M), N, K, 1, st);
+             const float* resid = nullptr, float* gelu_out = nullptr, const TrDrop& drop = {}) {
+    launch_tr_gemm({X, K, 1}, {W, K, 1}, {out, N, 0, bias, resid, N, gelu_out, drop}, static_cast<int>(M), N, K, 1, st);
     return check_launch(c, "train_gemm", st);
   }
   // dX[M, K] = dY[M, N] W[N, K] (+ resid)
@@ -185,10 +215,11 @@ struct TrRun {
     launch_tr_reduce(s.part, parts, int64_t{N} * K, 1.f, dW, st);
     return check_launch(c, "train_reduce", st);
   }
-  // out[n] = scale sum_m A[m, n] (B[m, n]) (rs[m])
-  int colsum(const float* A, const float* Bm, const float* rs, int64_t M, int N, float scale, float* out) {
+  // out[n] = scale sum_m A[m, n] (B[m, n]) (rs[m]); with shift, A centred by shift[n] (squared without B)
+  int colsum(const float* A, const float* Bm, const float* rs, int64_t M, int N, float scale, float* out,
+             const float* shift = nullptr) {
     if (!out) return BT_OK;
-    const int parts = launch_tr_colsum(A, Bm, rs, M, N, tr_colsum_splits(M, N), s.part, st);
+    const int parts = launch_tr_colsum(A, Bm, rs, M, N, tr_colsum_splits(M, N), s.part, st, shift);
     if (const int r = check_launch(c, "train_colsum", st)) return r;
     launch_tr_reduce(s.part, parts, N, scale, out, st);
     return check_launch(c, "train_reduce", st);
@@ -197,6 +228,11 @@ struct TrRun {
     const int heads = l.C / 32;
     if (l.kind == kAttnFreq) return {B * L, l.F, heads, L, int64_t{l.F} * L, 1, L};  // sequences (b, t) over f
     return {B * l.F, L, heads, 1, L, 0, 1};                                       // sequences (b, f) over t
+  }
+  // mask and scale of a [M, N] gradient at a dropout site (the copy reads from, and writes to, other buffers)
+  int masked(const float* g, int64_t n, const TrDrop& d, float* out) {
+    launch_tr_reduce(g, 1, n, 1.f, out, st, 0.f, d);
+    return check_launch(c, "train_reduce", st);
   }
   TrImg img(const TrLayer& l) const {
     if (l.kind == kStem) return {B, l.F, 4, L, 1, int64_t{L} * 4 * l.F, 1, 4 * l.F, 0};  // the [B, L, 128] input
@@ -210,8 +246,24 @@ struct TrRun {
     if (_r != BT_OK) return _r;  \
   } while (0)
 
-// Each step reads l.in and writes the next step's in (the head: the logits).
-int forward_layer(TrRun& R, const TrLayer& l, float* next, float* beat, float* down) {
+// Training mode: the batch mean and biased variance (two passes: the mean, then centred squares) of x [N, ch] into the
+// store at off, and the running statistics of the BatchNorm at table index p moved towards them (momentum 0.1, the
+// unbiased variance N / (N - 1)).
+int bn_stats(TrRun& R, const float* x, int64_t N, int ch, int p, int64_t off) {
+  float* mean = R.at(off);
+  float* var = R.at(off + ((ch + 3) & ~3));
+  const float inv_n = static_cast<float>(1.0 / static_cast<double>(N));
+  TR_OK(R.colsum(x, nullptr, nullptr, N, ch, inv_n, mean));
+  TR_OK(R.colsum(x, nullptr, nullptr, N, ch, inv_n, var, mean));
+  launch_tr_reduce(mean, 1, ch, 0.1f, R.running[p + 2], R.st, 0.9f);
+  TR_OK(check_launch(R.c, "train_reduce", R.st));
+  launch_tr_reduce(var, 1, ch, static_cast<float>(0.1 * static_cast<double>(N) / static_cast<double>(N - 1)),
+                   R.running[p + 3], R.st, 0.9f);
+  return check_launch(R.c, "train_reduce", R.st);
+}
+
+// Each step reads l.in and writes the next step's in (the head: the logits).  step: its index in the layer list.
+int forward_layer(TrRun& R, const TrLayer& l, size_t step, float* next, float* beat, float* down) {
   const cudaStream_t st = R.st;
   bt_ctx* c = R.c;
   const int64_t M = int64_t{R.B} * R.L * l.F;
@@ -219,11 +271,14 @@ int forward_layer(TrRun& R, const TrLayer& l, float* next, float* beat, float* d
   switch (l.kind) {
     case kStem: {
       const TrImg g = R.img(l);
-      const TrBn bn1 = R.bn(p);
+      const int Fs = c->hp.spect_dim;
+      if (R.mode) TR_OK(bn_stats(R, R.at(l.in), int64_t{R.B} * R.L, Fs, p, l.bn1));
+      const TrBn bn1 = R.bn(p, l.bn1, Fs);
       launch_tr_im2col(R.at(l.in), g, &bn1, R.s.big, st);
       BT_LAUNCHED(c, "train_im2col", st);
       TR_OK(R.linear(R.s.big, M, 12, R.w(p + 5), C, nullptr, R.at(l.z)));
-      launch_tr_bn_gelu_fwd(R.at(l.z), R.bn(p + 6), M * C, C, next, st);
+      if (R.mode) TR_OK(bn_stats(R, R.at(l.z), M, C, p + 6, l.bn2));
+      launch_tr_bn_gelu_fwd(R.at(l.z), R.bn(p + 6, l.bn2, C), M * C, C, next, st);
       BT_LAUNCHED(c, "train_bn_gelu", st);
       return BT_OK;
     }
@@ -236,17 +291,19 @@ int forward_layer(TrRun& R, const TrLayer& l, float* next, float* beat, float* d
       TR_OK(R.linear(R.at(l.xn), M, C, R.w(p + 3), heads, R.w(p + 4), R.at(l.gate)));
       launch_tr_rope(R.at(l.qkv), R.w(p), M, C, R.L, l.F, l.kind == kAttnFreq, false, st);
       BT_LAUNCHED(c, "train_rope", st);
-      launch_tr_attn_fwd(R.at(l.qkv), R.seqs(l), R.at(l.o), R.at(l.lse), st);
+      launch_tr_attn_fwd(R.at(l.qkv), R.seqs(l), R.at(l.o), R.at(l.lse), st, R.drop(l, step, 0));
       BT_LAUNCHED(c, "train_attention", st);
       launch_tr_gate_fwd(R.at(l.o), R.at(l.gate), M, C, R.s.s1, st);
       BT_LAUNCHED(c, "train_gate", st);
-      return R.linear(R.s.s1, M, C, R.w(p + 5), C, nullptr, next, R.at(l.in));
+      return R.linear(R.s.s1, M, C, R.w(p + 5), C, nullptr, next, R.at(l.in), nullptr, R.drop(l, step, 1));
     }
     case kFfn: {
       launch_tr_rms_fwd(R.at(l.in), R.w(p), M, C, R.at(l.xn), R.at(l.inv), st);
       BT_LAUNCHED(c, "train_rmsnorm", st);
-      TR_OK(R.linear(R.at(l.xn), M, C, R.w(p + 1), l.mult * C, R.w(p + 2), R.at(l.h), nullptr, R.at(l.a)));
-      return R.linear(R.at(l.a), M, l.mult * C, R.w(p + 3), C, R.w(p + 4), next, R.at(l.in));
+      TR_OK(R.linear(R.at(l.xn), M, C, R.w(p + 1), l.mult * C, R.w(p + 2), R.at(l.h), nullptr, R.at(l.a),
+                     R.drop(l, step, 0)));
+      return R.linear(R.at(l.a), M, l.mult * C, R.w(p + 3), C, R.w(p + 4), next, R.at(l.in), nullptr,
+                      R.drop(l, step, 1));
     }
     case kConvBlock: {
       const TrImg g = R.img(l);
@@ -254,7 +311,8 @@ int forward_layer(TrRun& R, const TrLayer& l, float* next, float* beat, float* d
       launch_tr_im2col(R.at(l.in), g, nullptr, R.s.big, st);
       BT_LAUNCHED(c, "train_im2col", st);
       TR_OK(R.linear(R.s.big, Mo, 6 * C, R.w(p), 2 * C, nullptr, R.at(l.z)));
-      launch_tr_bn_gelu_fwd(R.at(l.z), R.bn(p + 1), Mo * 2 * C, 2 * C, next, st);
+      if (R.mode) TR_OK(bn_stats(R, R.at(l.z), Mo, 2 * C, p + 1, l.bn2));
+      launch_tr_bn_gelu_fwd(R.at(l.z), R.bn(p + 1, l.bn2, 2 * C), Mo * 2 * C, 2 * C, next, st);
       BT_LAUNCHED(c, "train_bn_gelu", st);
       return BT_OK;
     }
@@ -282,8 +340,9 @@ int rms_backward(TrRun& R, const TrLayer& l, int gamma, const float* dxn, int64_
   return R.colsum(dxn, R.at(l.in), R.at(l.inv), M, l.C, sqrtf(static_cast<float>(l.C)), R.G[gamma]);
 }
 
-// s.dcur holds the gradient at the step's output; on return, at its input.
-int backward_layer(TrRun& R, const TrLayer& l, float* dspect) {
+// s.dcur holds the gradient at the step's output; on return, at its input.  Dropout masks are regenerated from the
+// forward's sites; BatchNorms use the forward's batch statistics from the store.
+int backward_layer(TrRun& R, const TrLayer& l, size_t step, float* dspect) {
   const cudaStream_t st = R.st;
   bt_ctx* c = R.c;
   const int64_t M = int64_t{R.B} * R.L * l.F;
@@ -304,14 +363,22 @@ int backward_layer(TrRun& R, const TrLayer& l, float* dspect) {
       const int heads = C / 32;
       launch_tr_gate_fwd(R.at(l.o), R.at(l.gate), M, C, s.s1, st);
       BT_LAUNCHED(c, "train_gate", st);
-      TR_OK(R.grad_weight(s.dcur, M, C, s.s1, C, G[p + 5]));
-      TR_OK(R.grad_input(s.dcur, M, C, R.w(p + 5), C, s.s2));
+      // to_out's dropout: its GEMMs see the masked gradient (in dqkv, free until the attention passes), the residual
+      // path the plain one
+      const TrDrop d1 = R.drop(l, step, 1), d0 = R.drop(l, step, 0);
+      const float* dy = s.dcur;
+      if (d1.thresh) {
+        TR_OK(R.masked(s.dcur, M * C, d1, s.dqkv));
+        dy = s.dqkv;
+      }
+      TR_OK(R.grad_weight(dy, M, C, s.s1, C, G[p + 5]));
+      TR_OK(R.grad_input(dy, M, C, R.w(p + 5), C, s.s2));
       launch_tr_gate_bwd(s.s2, R.at(l.o), R.at(l.gate), M, C, s.hd1, s.hd2, st);
       BT_LAUNCHED(c, "train_gate_bwd", st);
       const TrSeqs q = R.seqs(l);
-      launch_tr_attn_dq(R.at(l.qkv), s.s2, R.at(l.lse), s.hd2, q, s.dqkv, st);
+      launch_tr_attn_dq(R.at(l.qkv), s.s2, R.at(l.lse), s.hd2, q, s.dqkv, st, d0);
       BT_LAUNCHED(c, "train_attention_dq", st);
-      launch_tr_attn_dkv(R.at(l.qkv), s.s2, R.at(l.lse), s.hd2, q, s.dqkv, st);
+      launch_tr_attn_dkv(R.at(l.qkv), s.s2, R.at(l.lse), s.hd2, q, s.dqkv, st, d0);
       BT_LAUNCHED(c, "train_attention_dkv", st);
       launch_tr_rope(s.dqkv, R.w(p), M, C, R.L, l.F, l.kind == kAttnFreq, true, st);
       BT_LAUNCHED(c, "train_rope", st);
@@ -324,10 +391,16 @@ int backward_layer(TrRun& R, const TrLayer& l, float* dspect) {
     }
     case kFfn: {
       const int H = l.mult * C;
-      TR_OK(R.grad_weight(s.dcur, M, C, R.at(l.a), H, G[p + 3]));
-      TR_OK(R.colsum(s.dcur, nullptr, nullptr, M, C, 1.f, G[p + 4]));
-      TR_OK(R.grad_input(s.dcur, M, C, R.w(p + 3), H, s.big));
-      launch_tr_gelu_bwd(s.big, R.at(l.h), M * H, s.big, st);
+      const TrDrop d1 = R.drop(l, step, 1);
+      const float* dy = s.dcur;  // net.5's dropout: the masked gradient to net.4, the plain one to the residual path
+      if (d1.thresh) {
+        TR_OK(R.masked(s.dcur, M * C, d1, s.s2));
+        dy = s.s2;
+      }
+      TR_OK(R.grad_weight(dy, M, C, R.at(l.a), H, G[p + 3]));
+      TR_OK(R.colsum(dy, nullptr, nullptr, M, C, 1.f, G[p + 4]));
+      TR_OK(R.grad_input(dy, M, C, R.w(p + 3), H, s.big));
+      launch_tr_gelu_bwd(s.big, R.at(l.h), M * H, s.big, st, R.drop(l, step, 0));
       BT_LAUNCHED(c, "train_gelu_bwd", st);
       TR_OK(R.grad_weight(s.big, M, H, R.at(l.xn), C, G[p + 1]));
       TR_OK(R.colsum(s.big, nullptr, nullptr, M, H, 1.f, G[p + 2]));
@@ -351,13 +424,20 @@ int backward_layer(TrRun& R, const TrLayer& l, float* dspect) {
       const TrImg g = R.img(l);
       const int Co = stem ? C : 2 * C, K = g.C * g.S * 3, bn2 = stem ? p + 6 : p + 1, wc = stem ? p + 5 : p;
       const int64_t Mo = int64_t{g.B} * g.Fo * g.L;
-      const TrBn b2 = R.bn(bn2), b1 = R.bn(p);
+      const int64_t BL = int64_t{R.B} * R.L;
+      const int Fs = c->hp.spect_dim;
+      const TrBn b2 = R.bn(bn2, l.bn2, Co), b1 = stem ? R.bn(p, l.bn1, Fs) : TrBn{};
       launch_tr_bn_gelu_bwd(s.dcur, R.at(l.z), b2, Mo * Co, Co, s.s1, s.s2, st);  // s1: at the BatchNorm, s2: at z
       BT_LAUNCHED(c, "train_bn_gelu_bwd", st);
       TR_OK(R.colsum(s.s1, R.at(l.z), nullptr, Mo, Co, 1.f, s.hd1));
       TR_OK(R.colsum(s.s1, nullptr, nullptr, Mo, Co, 1.f, s.hd2));
       launch_tr_bn_grads(s.hd1, s.hd2, b2, Co, G[bn2], G[bn2 + 1], st);
       BT_LAUNCHED(c, "train_bn_grads", st);
+      if (R.mode) {  // batch statistics: the gradient at z gains the terms through the mean and variance
+        const TrBnBatch bb{R.at(l.z), s.hd1, s.hd2, static_cast<float>(1.0 / static_cast<double>(Mo))};
+        launch_tr_bn_scale(s.s1, b2, Mo * Co, Co, s.s2, st, &bb);
+        BT_LAUNCHED(c, "train_bn_scale", st);
+      }
       launch_tr_im2col(R.at(l.in), g, stem ? &b1 : nullptr, s.big, st);
       BT_LAUNCHED(c, "train_im2col", st);
       TR_OK(R.grad_weight(s.s2, Mo, Co, s.big, K, G[wc]));
@@ -366,14 +446,13 @@ int backward_layer(TrRun& R, const TrLayer& l, float* dspect) {
       launch_tr_col2im(s.big, g, stem ? s.s1 : s.dcur, st);  // the stem: the gradient at the 1-d BatchNorm's output
       BT_LAUNCHED(c, "train_col2im", st);
       if (!stem) return BT_OK;
-      const int64_t BL = int64_t{R.B} * R.L;
-      const int Fs = c->hp.spect_dim;
       TR_OK(R.colsum(s.s1, R.at(l.in), nullptr, BL, Fs, 1.f, s.hd1));
       TR_OK(R.colsum(s.s1, nullptr, nullptr, BL, Fs, 1.f, s.hd2));
       launch_tr_bn_grads(s.hd1, s.hd2, b1, Fs, G[p], G[p + 1], st);
       BT_LAUNCHED(c, "train_bn_grads", st);
       if (!dspect) return BT_OK;
-      launch_tr_bn_scale(s.s1, b1, BL * Fs, Fs, dspect, st);
+      const TrBnBatch bb{R.at(l.in), s.hd1, s.hd2, static_cast<float>(1.0 / static_cast<double>(BL))};
+      launch_tr_bn_scale(s.s1, b1, BL * Fs, Fs, dspect, st, R.mode ? &bb : nullptr);
       BT_LAUNCHED(c, "train_bn_scale", st);
       return BT_OK;
     }
@@ -383,14 +462,22 @@ int backward_layer(TrRun& R, const TrLayer& l, float* dspect) {
 
 // The checks both passes share, before anything is enqueued.
 int train_prepare(bt_ctx* c, const char* fn, const void* const* params, int32_t n_params, int32_t B, int32_t L,
-                  const void* act, int64_t act_bytes, TrModel* m) {
+                  const bt_train_mode* mode, const void* act, int64_t act_bytes, TrModel* m) {
   if (c->dtype != BT_DTYPE_F32)
     return fail(c, BT_ERR_ARG, "%s: training runs on a BT_DTYPE_F32 context (fp32 CUDA cores)", fn);
   if (B < 1 || L < 1) return fail(c, BT_ERR_ARG, "%s: need B >= 1 and L >= 1, got B=%d L=%d", fn, B, L);
   if (int64_t{B} * L > kMaxChunkCap)
     return fail(c, BT_ERR_ARG, "%s: B * L = %lld frames exceeds %lld", fn, static_cast<long long>(int64_t{B} * L),
                 static_cast<long long>(kMaxChunkCap));
-  *m = train_model(c->hp, B, L);
+  if (mode) {
+    for (const float p : {mode->dropout_frontend, mode->dropout_transformer})
+      if (!(p >= 0.f && p < 1.f)) return fail(c, BT_ERR_ARG, "%s: dropout rate %g outside [0, 1)", fn, p);
+    // the fewest positions a BatchNorm sees is the stem's bn1d: B * L
+    if (int64_t{B} * L < 2)
+      return fail(c, BT_ERR_ARG, "%s: batch-statistics BatchNorm needs more than one value per channel, B * L = %lld",
+                  fn, static_cast<long long>(int64_t{B} * L));
+  }
+  *m = train_model(c->hp, B, L, mode != nullptr);
   if (n_params != static_cast<int32_t>(m->table.size()))
     return fail(c, BT_ERR_ARG, "%s: %d parameter pointers, the model has %zu (bt_train_param_count)", fn, n_params,
                 m->table.size());
@@ -399,8 +486,9 @@ int train_prepare(bt_ctx* c, const char* fn, const void* const* params, int32_t 
     if (!params[i] && m->table[i].ndim > 0)
       return fail(c, BT_ERR_ARG, "%s: parameter %zu (%s) is null", fn, i, m->table[i].name.c_str());
   if (act_bytes < m->floats * static_cast<int64_t>(sizeof(float)))
-    return fail(c, BT_ERR_ARG, "%s: activation store of %lld bytes, B=%d L=%d needs %lld (bt_train_activation_bytes)",
-                fn, static_cast<long long>(act_bytes), B, L,
+    return fail(c, BT_ERR_ARG,
+                "%s: activation store of %lld bytes, B=%d L=%d in %s mode needs %lld (bt_train_activation_bytes_ex)", fn,
+                static_cast<long long>(act_bytes), B, L, mode ? "training" : "eval",
                 static_cast<long long>(m->floats * static_cast<int64_t>(sizeof(float))));
   return BT_OK;
 }
@@ -443,39 +531,62 @@ int bt_train_param_info(const bt_hparams* hp, int32_t i, char* name, int32_t cap
   return BT_OK;
 }
 
-int64_t bt_train_activation_bytes(const bt_ctx* c, int32_t B, int32_t L) {
+int64_t bt_train_activation_bytes_ex(const bt_ctx* c, int32_t B, int32_t L, const bt_train_mode* mode) {
   if (!c || B < 1 || L < 1) return BT_ERR_ARG;
-  return train_model(c->hp, B, L).floats * static_cast<int64_t>(sizeof(float));
+  return train_model(c->hp, B, L, mode != nullptr).floats * static_cast<int64_t>(sizeof(float));
 }
 
-int bt_train_forward(bt_ctx* c, const float* const* params, int32_t n_params, const float* spect_dev, int32_t B,
-                     int32_t L, void* act_dev, int64_t act_bytes, float* beat_dev, float* down_dev, void* stream) {
+int64_t bt_train_activation_bytes(const bt_ctx* c, int32_t B, int32_t L) {
+  return bt_train_activation_bytes_ex(c, B, L, nullptr);
+}
+
+int bt_train_forward_ex(bt_ctx* c, const float* const* params, int32_t n_params, float* const* running,
+                        const float* spect_dev, int32_t B, int32_t L, const bt_train_mode* mode, void* act_dev,
+                        int64_t act_bytes, float* beat_dev, float* down_dev, void* stream) {
   if (!c) return BT_ERR_ARG;
-  const char* fn = "bt_train_forward";
+  const char* fn = "bt_train_forward_ex";
   TrModel m;
-  int r = train_prepare(c, fn, reinterpret_cast<const void* const*>(params), n_params, B, L, act_dev, act_bytes, &m);
+  int r = train_prepare(c, fn, reinterpret_cast<const void* const*>(params), n_params, B, L, mode, act_dev, act_bytes,
+                        &m);
   if (r != BT_OK) return r;
   if (!spect_dev || !beat_dev || !down_dev) return fail(c, BT_ERR_ARG, "%s: null spectrogram or logits pointer", fn);
+  if (mode) {  // the running statistics every BatchNorm updates
+    if (!running) return fail(c, BT_ERR_ARG, "%s: training mode needs the running-statistics table", fn);
+    for (size_t i = 0; i < m.table.size(); ++i) {
+      const std::string& n = m.table[i].name;
+      const bool stat = n.size() > 13 && (n.compare(n.size() - 13, 13, ".running_mean") == 0 ||
+                                          n.compare(n.size() - 12, 12, ".running_var") == 0);
+      if (stat && !running[i])
+        return fail(c, BT_ERR_ARG, "%s: running-statistics entry %zu (%s) is null", fn, i, n.c_str());
+    }
+  }
   cudaStream_t st;
   if ((r = enter(c, fn, stream, &st)) != BT_OK) return r;
-  TrRun R{c, st, params, nullptr, static_cast<float*>(act_dev), {}, B, L, nullptr, nullptr};
+  TrRun R{c, st, params, nullptr, static_cast<float*>(act_dev), {}, B, L, nullptr, nullptr, mode, running};
   if ((r = train_scratch(c, int64_t{B} * L, &R.s)) != BT_OK) return r;
   BT_CUDA(c, cudaMemcpyAsync(R.at(m.layers[0].in), spect_dev, sizeof(float) * B * L * c->hp.spect_dim,
                              cudaMemcpyDeviceToDevice, st));
   for (size_t i = 0; i < m.layers.size(); ++i) {
     float* next = i + 1 < m.layers.size() ? R.at(m.layers[i + 1].in) : nullptr;
-    if ((r = forward_layer(R, m.layers[i], next, beat_dev, down_dev)) != BT_OK) return r;
+    if ((r = forward_layer(R, m.layers[i], i, next, beat_dev, down_dev)) != BT_OK) return r;
   }
   return BT_OK;
 }
 
-int bt_train_backward(bt_ctx* c, const float* const* params, int32_t n_params, const void* act_dev, int64_t act_bytes,
-                      int32_t B, int32_t L, const float* dbeat_dev, const float* ddown_dev, float* const* grads,
-                      float* dspect_dev, void* stream) {
+int bt_train_forward(bt_ctx* c, const float* const* params, int32_t n_params, const float* spect_dev, int32_t B,
+                     int32_t L, void* act_dev, int64_t act_bytes, float* beat_dev, float* down_dev, void* stream) {
+  return bt_train_forward_ex(c, params, n_params, nullptr, spect_dev, B, L, nullptr, act_dev, act_bytes, beat_dev,
+                             down_dev, stream);
+}
+
+int bt_train_backward_ex(bt_ctx* c, const float* const* params, int32_t n_params, const void* act_dev,
+                         int64_t act_bytes, int32_t B, int32_t L, const bt_train_mode* mode, const float* dbeat_dev,
+                         const float* ddown_dev, float* const* grads, float* dspect_dev, void* stream) {
   if (!c) return BT_ERR_ARG;
-  const char* fn = "bt_train_backward";
+  const char* fn = "bt_train_backward_ex";
   TrModel m;
-  int r = train_prepare(c, fn, reinterpret_cast<const void* const*>(params), n_params, B, L, act_dev, act_bytes, &m);
+  int r = train_prepare(c, fn, reinterpret_cast<const void* const*>(params), n_params, B, L, mode, act_dev, act_bytes,
+                        &m);
   if (r != BT_OK) return r;
   if (!dbeat_dev || !ddown_dev || !grads) return fail(c, BT_ERR_ARG, "%s: null logit gradient or gradient array", fn);
   // an entry that takes no gradient is never written, whatever it holds; every other null entry is skipped
@@ -484,11 +595,19 @@ int bt_train_backward(bt_ctx* c, const float* const* params, int32_t n_params, c
     if (!m.table[i].trainable) g[i] = nullptr;
   cudaStream_t st;
   if ((r = enter(c, fn, stream, &st)) != BT_OK) return r;
-  TrRun R{c, st, params, g.data(), static_cast<float*>(const_cast<void*>(act_dev)), {}, B, L, dbeat_dev, ddown_dev};
+  TrRun R{c,    st, params, g.data(), static_cast<float*>(const_cast<void*>(act_dev)), {}, B, L, dbeat_dev, ddown_dev,
+          mode, nullptr};
   if ((r = train_scratch(c, int64_t{B} * L, &R.s)) != BT_OK) return r;
   for (size_t i = m.layers.size(); i-- > 0;)
-    if ((r = backward_layer(R, m.layers[i], dspect_dev)) != BT_OK) return r;
+    if ((r = backward_layer(R, m.layers[i], i, dspect_dev)) != BT_OK) return r;
   return BT_OK;
+}
+
+int bt_train_backward(bt_ctx* c, const float* const* params, int32_t n_params, const void* act_dev, int64_t act_bytes,
+                      int32_t B, int32_t L, const float* dbeat_dev, const float* ddown_dev, float* const* grads,
+                      float* dspect_dev, void* stream) {
+  return bt_train_backward_ex(c, params, n_params, act_dev, act_bytes, B, L, nullptr, dbeat_dev, ddown_dev, grads,
+                              dspect_dev, stream);
 }
 
 }  // extern "C"

@@ -554,7 +554,7 @@ std::vector<ParamSpec> layer_params(const Layer& l, int64_t D) {
 // ================================================================================== C ABI
 extern "C" {
 
-int bt_version(void) { return 213; }
+int bt_version(void) { return 214; }
 
 const char* bt_act_dtype(void) {
 #if defined(BT_ACT_BF16)

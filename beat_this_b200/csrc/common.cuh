@@ -54,6 +54,22 @@ __device__ __forceinline__ uint32_t pack_h16x2(float lo, float hi) {
 }
 #endif
 
+// Counter-based Philox4x32-10 (Salmon et al., SC'11; the rounds of curand's curand_Philox4x32_10): ten rounds of the
+// two 32 x 32 -> 64-bit products, the key bumped by the Weyl constants between rounds.  Dropout masks are regenerated
+// from it in every kernel that needs them (include/beatthis.h, "dropout masks").
+__host__ __device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    const uint64_t p0 = uint64_t{0xD2511F53u} * c.x, p1 = uint64_t{0xCD9E8D57u} * c.z;
+    const uint32_t hi0 = static_cast<uint32_t>(p0 >> 32), lo0 = static_cast<uint32_t>(p0);
+    const uint32_t hi1 = static_cast<uint32_t>(p1 >> 32), lo1 = static_cast<uint32_t>(p1);
+    c = make_uint4(hi1 ^ c.y ^ k.x, lo1, hi0 ^ c.w ^ k.y, lo0);
+    k.x += 0x9E3779B9u;
+    k.y += 0xBB67AE85u;
+  }
+  return c;
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

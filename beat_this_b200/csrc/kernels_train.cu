@@ -1,11 +1,47 @@
 // fp32 CUDA-core kernels of the training forward and backward (bt_train_forward / bt_train_backward): a strided GEMM
-// with split-K partials, fixed-order reductions, RMSNorm, eval-mode BatchNorm + GELU, the convolutions' im2col and
-// col2im, RoPE, and flash-style attention forward and backward over strided sequences (head_dim 32).  No kernel uses
-// atomics, so every result is bitwise repeatable.
+// with split-K partials, fixed-order reductions, RMSNorm, BatchNorm + GELU, the convolutions' im2col and col2im, RoPE,
+// and flash-style attention forward and backward over strided sequences (head_dim 32).  No kernel uses atomics, so
+// every result is bitwise repeatable.  Dropout masks (training mode) are regenerated from Philox4x32-10 wherever they
+// are needed and never stored.
+#include <cmath>
+
 #include "bt_train.h"
 #include "common.cuh"
 
 namespace bt {
+
+TrDrop tr_drop(uint64_t seed, uint32_t site, double p, int64_t e0) {
+  const uint32_t thresh = p > 0.0 ? static_cast<uint32_t>(std::floor(p * 4294967296.0)) : 0u;
+  return TrDrop{seed, site, thresh, thresh ? static_cast<float>(1.0 / (1.0 - p)) : 1.f, e0};
+}
+
+// ------------------------------------------------------------------------------------ dropout masks
+// the four Philox words of elements 4 g .. 4 g + 3 of a site
+__device__ __forceinline__ uint4 tr_drop_words(const TrDrop& d, int64_t g) {
+  const uint64_t u = static_cast<uint64_t>(g);
+  return philox4x32_10(make_uint4(static_cast<uint32_t>(u), static_cast<uint32_t>(u >> 32), d.site, 0u),
+                       make_uint2(static_cast<uint32_t>(d.seed), static_cast<uint32_t>(d.seed >> 32)));
+}
+// element e of the site kept
+__device__ __forceinline__ bool tr_keep(const TrDrop& d, int64_t e) {
+  const uint4 w = tr_drop_words(d, e >> 2);
+  const int k = static_cast<int>(e & 3);
+  return (k == 0 ? w.x : k == 1 ? w.y : k == 2 ? w.z : w.w) >= d.thresh;
+}
+// bit k (k < cnt <= 32): element e + k of the site kept; one Philox call per four elements
+__device__ __forceinline__ uint32_t tr_keep32(const TrDrop& d, int64_t e, int cnt) {
+  uint32_t bits = 0;
+  for (int64_t g = e >> 2; g <= (e + cnt - 1) >> 2; ++g) {
+    const uint4 w = tr_drop_words(d, g);
+    const uint32_t ws[4] = {w.x, w.y, w.z, w.w};
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const int64_t k = 4 * g + q - e;
+      if (k >= 0 && k < cnt && ws[q] >= d.thresh) bits |= 1u << k;
+    }
+  }
+  return bits;
+}
 
 // ------------------------------------------------------------------------------------ GEMM
 // C[z][m, n] = sum_{k in split z} A(m, k) B(n, k) (+ bias[n]) (+ resid[m, n]); with gelu_out also gelu_out = GELU(C).
@@ -55,12 +91,23 @@ tr_gemm_kernel(TrMat A, TrMat B, TrGemmOut o, int M, int N, int K, int kc) {
   for (int i = 0; i < 4; ++i) {
     const int m = m0 + ty * 4 + i;
     if (m >= M) continue;
+    const uint32_t keep =
+        o.drop.thresh ? tr_keep32(o.drop, o.drop.e0 + static_cast<int64_t>(m) * N + n0 + tx * 4, 4) : 0u;
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const int n = n0 + tx * 4 + j;
       if (n >= N) continue;
       float v = acc[i][j];
       if (o.bias) v += o.bias[n];
+      if (o.drop.thresh) {
+        const bool kept = (keep >> j) & 1u;
+        if (o.gelu_out) {  // the FFN hidden: C keeps the pre-GELU value, gelu_out the dropped GELU output
+          C[static_cast<int64_t>(m) * o.ldc + n] = v;
+          o.gelu_out[static_cast<int64_t>(m) * o.ldc + n] = kept ? gelu_erf(v) * o.drop.scale : 0.f;
+          continue;
+        }
+        v = kept ? v * o.drop.scale : 0.f;
+      }
       if (o.resid) v += o.resid[static_cast<int64_t>(m) * o.ldr + n];
       C[static_cast<int64_t>(m) * o.ldc + n] = v;
       if (o.gelu_out) o.gelu_out[static_cast<int64_t>(m) * o.ldc + n] = gelu_erf(v);
@@ -74,33 +121,42 @@ void launch_tr_gemm(const TrMat& A, const TrMat& B, const TrGemmOut& o, int M, i
   tr_gemm_kernel<<<grid, 256, 0, st>>>(A, B, o, M, N, K, kc);
 }
 
-// out[i] = scale * sum_{z < Z} part[z * n + i], z ascending
-__global__ void tr_reduce_kernel(const float* __restrict__ part, int Z, int64_t n, float scale, float* __restrict__ out) {
+// out[i] = scale * sum_{z < Z} part[z * n + i], z ascending; then masked (drop) and added to beta out[i] (beta != 0)
+__global__ void tr_reduce_kernel(const float* __restrict__ part, int Z, int64_t n, float scale, float* __restrict__ out,
+                                 float beta, TrDrop drop) {
   const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= n) return;
   float s = 0.f;
   for (int z = 0; z < Z; ++z) s += part[z * n + i];
-  out[i] = s * scale;
+  float v = s * scale;
+  if (drop.thresh) v = tr_keep(drop, drop.e0 + i) ? v * drop.scale : 0.f;
+  if (beta != 0.f) v = fmaf(beta, out[i], v);
+  out[i] = v;
 }
 
-void launch_tr_reduce(const float* part, int Z, int64_t n, float scale, float* out, cudaStream_t st) {
-  tr_reduce_kernel<<<static_cast<unsigned>(ceil_div64(n, 256)), 256, 0, st>>>(part, Z, n, scale, out);
+void launch_tr_reduce(const float* part, int Z, int64_t n, float scale, float* out, cudaStream_t st, float beta,
+                      const TrDrop& drop) {
+  tr_reduce_kernel<<<static_cast<unsigned>(ceil_div64(n, 256)), 256, 0, st>>>(part, Z, n, scale, out, beta, drop);
 }
 
-// part[z][n] = sum over rows m of split z of A[m, n] (* B[m, n]) (* rs[m]): 32 columns x 8 row lanes per CTA, the lanes
-// summed in a fixed order through shared memory.
+// part[z][n] = sum over rows m of split z of a (* B[m, n]) (* rs[m]), a = A[m, n] - shift[n] (SHIFT) or A[m, n], a * a
+// with SHIFT and no B: 32 columns x 8 row lanes per CTA, the lanes summed in a fixed order through shared memory.
+template <bool SHIFT>
 __global__ void __launch_bounds__(256)
 tr_colsum_kernel(const float* __restrict__ A, const float* __restrict__ B, const float* __restrict__ rs, int64_t M, int N,
-                 int64_t rows_per_split, float* __restrict__ part) {
+                 int64_t rows_per_split, float* __restrict__ part, const float* __restrict__ shift) {
   __shared__ float red[8][33];
   const int tx = threadIdx.x % 32, ty = threadIdx.x / 32;
   const int n = blockIdx.x * 32 + tx;
   const int64_t r0 = blockIdx.y * rows_per_split, r1 = min(M, r0 + rows_per_split);
+  const float sh = SHIFT && n < N ? shift[n] : 0.f;
   float s = 0.f;
   if (n < N)
     for (int64_t m = r0 + ty; m < r1; m += 8) {
       float v = A[m * N + n];
+      if (SHIFT) v -= sh;
       if (B) v *= B[m * N + n];
+      else if (SHIFT) v *= v;
       if (rs) v *= rs[m];
       s += v;
     }
@@ -115,10 +171,12 @@ tr_colsum_kernel(const float* __restrict__ A, const float* __restrict__ B, const
 }
 
 int launch_tr_colsum(const float* A, const float* B, const float* rs, int64_t M, int N, int splits, float* part,
-                     cudaStream_t st) {
+                     cudaStream_t st, const float* shift) {
   const int64_t rps = ceil_div64(M, splits);
   const int parts = static_cast<int>(ceil_div64(M, rps));
-  tr_colsum_kernel<<<dim3(ceil_div(N, 32), parts), 256, 0, st>>>(A, B, rs, M, N, rps, part);
+  const dim3 grid(ceil_div(N, 32), parts);
+  if (shift) tr_colsum_kernel<true><<<grid, 256, 0, st>>>(A, B, rs, M, N, rps, part, shift);
+  else tr_colsum_kernel<false><<<grid, 256, 0, st>>>(A, B, rs, M, N, rps, part, shift);
   return parts;
 }
 
@@ -174,7 +232,8 @@ void launch_tr_rms_bwd(const float* dxn, const float* x, const float* inv, const
   tr_rms_bwd_kernel<<<static_cast<unsigned>(ceil_div64(M, 8)), 256, 0, st>>>(dxn, x, inv, gamma, M, C, add, dres);
 }
 
-// ------------------------------------------------------------------------------------ BatchNorm (eval) + GELU
+// ------------------------------------------------------------------------------------ BatchNorm + GELU
+// rm / rv: the running statistics (eval mode) or the batch mean and biased variance (training mode)
 __device__ __forceinline__ float bn_scale(const TrBn& b, int c) { return b.w[c] / sqrtf(b.rv[c] + 1e-5f); }
 
 // y = GELU(z scale + shift), channel = index % C
@@ -213,10 +272,20 @@ __global__ void tr_bn_grads_kernel(const float* __restrict__ s_gz, const float* 
   if (db) db[c] = s_g[c];
 }
 
-// dx = g scale: the gradient at the 1-d BatchNorm's input
-__global__ void tr_bn_scale_kernel(const float* __restrict__ g, TrBn b, int64_t n, int C, float* __restrict__ dx) {
+// dx = g scale: the gradient at a BatchNorm's input in eval mode.  With batch statistics (bb.x set), xhat = (x - mean)
+// rstd: dx = scale (g - S_g / N - xhat sum(g xhat) / N), sum(g xhat) = rstd (S_gz - mean S_g).
+__global__ void tr_bn_scale_kernel(const float* __restrict__ g, TrBn b, int64_t n, int C, float* __restrict__ dx,
+                                   TrBnBatch bb) {
   const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i < n) dx[i] = g[i] * bn_scale(b, static_cast<int>(i % C));
+  if (i >= n) return;
+  const int c = static_cast<int>(i % C);
+  if (!bb.x) {
+    dx[i] = g[i] * bn_scale(b, c);
+    return;
+  }
+  const float mean = b.rm[c], ivar = 1.f / (b.rv[c] + 1e-5f);
+  const float t = (bb.s_gz[c] - mean * bb.s_g[c]) * ivar;
+  dx[i] = bn_scale(b, c) * (g[i] - bb.s_g[c] * bb.inv_n - (bb.x[i] - mean) * t * bb.inv_n);
 }
 
 void launch_tr_bn_gelu_fwd(const float* z, const TrBn& b, int64_t n, int C, float* y, cudaStream_t st) {
@@ -229,17 +298,22 @@ void launch_tr_bn_gelu_bwd(const float* dy, const float* z, const TrBn& b, int64
 void launch_tr_bn_grads(const float* s_gz, const float* s_g, const TrBn& b, int C, float* dw, float* db, cudaStream_t st) {
   tr_bn_grads_kernel<<<ceil_div(C, 128), 128, 0, st>>>(s_gz, s_g, b, C, dw, db);
 }
-void launch_tr_bn_scale(const float* g, const TrBn& b, int64_t n, int C, float* dx, cudaStream_t st) {
-  tr_bn_scale_kernel<<<static_cast<unsigned>(ceil_div64(n, 256)), 256, 0, st>>>(g, b, n, C, dx);
+void launch_tr_bn_scale(const float* g, const TrBn& b, int64_t n, int C, float* dx, cudaStream_t st,
+                        const TrBnBatch* batch) {
+  tr_bn_scale_kernel<<<static_cast<unsigned>(ceil_div64(n, 256)), 256, 0, st>>>(g, b, n, C, dx,
+                                                                                batch ? *batch : TrBnBatch{});
 }
 
-// dh = da GELU'(h), in place when dh == da
-__global__ void tr_gelu_bwd_kernel(const float* da, const float* __restrict__ h, int64_t n, float* dh) {
+// dh = da GELU'(h), da masked and scaled first under drop (element i); in place when dh == da
+__global__ void tr_gelu_bwd_kernel(const float* da, const float* __restrict__ h, int64_t n, float* dh, TrDrop drop) {
   const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i < n) dh[i] = da[i] * gelu_grad(h[i]);
+  if (i >= n) return;
+  float d = da[i];
+  if (drop.thresh) d = tr_keep(drop, drop.e0 + i) ? d * drop.scale : 0.f;
+  dh[i] = d * gelu_grad(h[i]);
 }
-void launch_tr_gelu_bwd(const float* da, const float* h, int64_t n, float* dh, cudaStream_t st) {
-  tr_gelu_bwd_kernel<<<static_cast<unsigned>(ceil_div64(n, 256)), 256, 0, st>>>(da, h, n, dh);
+void launch_tr_gelu_bwd(const float* da, const float* h, int64_t n, float* dh, cudaStream_t st, const TrDrop& drop) {
+  tr_gelu_bwd_kernel<<<static_cast<unsigned>(ceil_div64(n, 256)), 256, 0, st>>>(da, h, n, dh, drop);
 }
 
 // ------------------------------------------------------------------------------------ convolution slabs
@@ -446,9 +520,17 @@ __device__ __forceinline__ void ta_tile(float (*T)[32], const float* base, int64
   }
 }
 
-// O = softmax(q k^T / sqrt 32) v, lse = log-sum-exp of the scaled scores (natural log)
+// element ((s heads + h) n + i) n of the probability dropout site: the first of query row i
+__device__ __forceinline__ int64_t ta_drop_row(const TrSeqs& q, int s, int h, int i) {
+  return ((static_cast<int64_t>(s) * q.heads + h) * q.n + i) * q.n;
+}
+
+// O = softmax(q k^T / sqrt 32) v, lse = log-sum-exp of the scaled scores (natural log).  DROP: O = (mask P / (1 - p)) v
+// with the mask of drop (lse unchanged).
+template <bool DROP>
 __global__ void __launch_bounds__(TA_Q)
-tr_attn_fwd_kernel(const float* __restrict__ qkv, TrSeqs q, float* __restrict__ O, float* __restrict__ lse) {
+tr_attn_fwd_kernel(const float* __restrict__ qkv, TrSeqs q, float* __restrict__ O, float* __restrict__ lse,
+                   TrDrop drop) {
   __shared__ __align__(16) float Ks[TA_T][32];
   __shared__ __align__(16) float Vs[TA_T][32];
   const int C = q.heads * 32, h = blockIdx.y;
@@ -467,6 +549,7 @@ tr_attn_fwd_kernel(const float* __restrict__ qkv, TrSeqs q, float* __restrict__ 
     ta_tile(Vs, qkv, 3 * C, 2 * C + h * 32, q, s, j0);
     __syncthreads();
     const int kn = min(TA_T, q.n - j0);
+    const uint32_t keep = DROP ? tr_keep32(drop, drop.e0 + ta_drop_row(q, s, h, ok ? i : 0) + j0, kn) : 0u;
     for (int j = 0; j < kn; ++j) {
       float a = 0.f;
 #pragma unroll
@@ -474,22 +557,24 @@ tr_attn_fwd_kernel(const float* __restrict__ qkv, TrSeqs q, float* __restrict__ 
       const float mn = fmaxf(mx, a);
       const float corr = expf(mx - mn), p = expf(a - mn);
       l = l * corr + p;
+      const float pv = DROP && !((keep >> j) & 1u) ? 0.f : p;
 #pragma unroll
-      for (int d = 0; d < 32; ++d) o[d] = fmaf(p, Vs[j][d], o[d] * corr);
+      for (int d = 0; d < 32; ++d) o[d] = fmaf(pv, Vs[j][d], o[d] * corr);
       mx = mn;
     }
   }
   if (ok) {
-    ta_store32(O + row * C + h * 32, o, 1.f / l);
+    ta_store32(O + row * C + h * 32, o, DROP ? drop.scale / l : 1.f / l);
     lse[row * q.heads + h] = mx + logf(l);
   }
 }
 
 // dq = sum_j p_ij (dO_i . v_j - delta_i) k_j / sqrt 32, with p_ij = exp(q_i . k_j / sqrt 32 - lse_i); into the q columns
-// of dqkv
+// of dqkv.  DROP: dO_i . v_j is masked and scaled as the forward's P was.
+template <bool DROP>
 __global__ void __launch_bounds__(TA_Q)
 tr_attn_dq_kernel(const float* __restrict__ qkv, const float* __restrict__ dO, const float* __restrict__ lse,
-                  const float* __restrict__ delta, TrSeqs q, float* __restrict__ dqkv) {
+                  const float* __restrict__ delta, TrSeqs q, float* __restrict__ dqkv, TrDrop drop) {
   __shared__ __align__(16) float Ks[TA_T][32];
   __shared__ __align__(16) float Vs[TA_T][32];
   const int C = q.heads * 32, h = blockIdx.y;
@@ -510,6 +595,7 @@ tr_attn_dq_kernel(const float* __restrict__ qkv, const float* __restrict__ dO, c
     ta_tile(Vs, qkv, 3 * C, 2 * C + h * 32, q, s, j0);
     __syncthreads();
     const int kn = min(TA_T, q.n - j0);
+    const uint32_t keep = DROP ? tr_keep32(drop, drop.e0 + ta_drop_row(q, s, h, ok ? i : 0) + j0, kn) : 0u;
     for (int j = 0; j < kn; ++j) {
       float a = 0.f, dp = 0.f;
 #pragma unroll
@@ -517,6 +603,7 @@ tr_attn_dq_kernel(const float* __restrict__ qkv, const float* __restrict__ dO, c
         a = fmaf(qv[d], Ks[j][d], a);
         dp = fmaf(dov[d], Vs[j][d], dp);
       }
+      if (DROP) dp = (keep >> j) & 1u ? dp * drop.scale : 0.f;
       const float ds = expf(a - L_i) * (dp - D_i);
 #pragma unroll
       for (int d = 0; d < 32; ++d) dq[d] = fmaf(ds, Ks[j][d], dq[d]);
@@ -525,13 +612,18 @@ tr_attn_dq_kernel(const float* __restrict__ qkv, const float* __restrict__ dO, c
   if (ok) ta_store32(dqkv + row * 3 * C + h * 32, dq, sc);
 }
 
-// dk_j = sum_i ds_ij q_i / sqrt 32, dv_j = sum_i p_ij dO_i; into the k and v columns of dqkv
+// dk_j = sum_i ds_ij q_i / sqrt 32, dv_j = sum_i p_ij dO_i; into the k and v columns of dqkv.  DROP: dv takes the
+// masked, scaled p_ij and ds_ij the masked, scaled dO_i . v_j; each query tile's mask bits for the CTA's 64 keys are
+// expanded once into shared memory (two words per query row, one word per thread).
+template <bool DROP>
 __global__ void __launch_bounds__(TA_Q)
 tr_attn_dkv_kernel(const float* __restrict__ qkv, const float* __restrict__ dO, const float* __restrict__ lse,
-                   const float* __restrict__ delta, TrSeqs q, float* __restrict__ dqkv) {
+                   const float* __restrict__ delta, TrSeqs q, float* __restrict__ dqkv, TrDrop drop) {
+  static_assert(TA_Q == 2 * TA_T, "one mask word of 32 keys per thread and query row");
   __shared__ __align__(16) float Qs[TA_T][32];
   __shared__ __align__(16) float Ds[TA_T][32];
   __shared__ float Ls[TA_T], Dl[TA_T];
+  __shared__ uint32_t Ms[DROP ? TA_T : 1][2];
   const int C = q.heads * 32, h = blockIdx.y;
   const int kt = ceil_div(q.n, TA_Q);
   const int s = blockIdx.x / kt, j = (blockIdx.x % kt) * TA_Q + threadIdx.x;
@@ -553,6 +645,11 @@ tr_attn_dkv_kernel(const float* __restrict__ qkv, const float* __restrict__ dO, 
       Ls[threadIdx.x] = lse[r * q.heads + h];
       Dl[threadIdx.x] = delta[r * q.heads + h];
     }
+    if (DROP) {
+      const int i = i0 + threadIdx.x / 2, jb = (blockIdx.x % kt) * TA_Q + (threadIdx.x % 2) * 32;
+      Ms[threadIdx.x / 2][threadIdx.x % 2] =
+          i < q.n && jb < q.n ? tr_keep32(drop, drop.e0 + ta_drop_row(q, s, h, i) + jb, min(32, q.n - jb)) : 0u;
+    }
     __syncthreads();
     const int qn = min(TA_T, q.n - i0);
     for (int i = 0; i < qn; ++i) {
@@ -563,10 +660,16 @@ tr_attn_dkv_kernel(const float* __restrict__ qkv, const float* __restrict__ dO, 
         dp = fmaf(Ds[i][d], vv[d], dp);
       }
       const float p = expf(a * sc - Ls[i]);
+      float pv = p;
+      if (DROP) {
+        const bool kept = (Ms[i][threadIdx.x / 32] >> (threadIdx.x % 32)) & 1u;
+        pv = kept ? p * drop.scale : 0.f;
+        dp = kept ? dp * drop.scale : 0.f;
+      }
       const float ds = p * (dp - Dl[i]);
 #pragma unroll
       for (int d = 0; d < 32; ++d) {
-        dv[d] = fmaf(p, Ds[i][d], dv[d]);
+        dv[d] = fmaf(pv, Ds[i][d], dv[d]);
         dk[d] = fmaf(ds, Qs[i][d], dk[d]);
       }
     }
@@ -577,17 +680,23 @@ tr_attn_dkv_kernel(const float* __restrict__ qkv, const float* __restrict__ dO, 
   }
 }
 
-void launch_tr_attn_fwd(const float* qkv, const TrSeqs& q, float* O, float* lse, cudaStream_t st) {
+// a rate of 0 runs the eval-mode instantiation
+void launch_tr_attn_fwd(const float* qkv, const TrSeqs& q, float* O, float* lse, cudaStream_t st, const TrDrop& drop) {
   dim3 grid(q.seqs * ceil_div(q.n, TA_Q), q.heads);
-  tr_attn_fwd_kernel<<<grid, TA_Q, 0, st>>>(qkv, q, O, lse);
+  if (drop.thresh) tr_attn_fwd_kernel<true><<<grid, TA_Q, 0, st>>>(qkv, q, O, lse, drop);
+  else tr_attn_fwd_kernel<false><<<grid, TA_Q, 0, st>>>(qkv, q, O, lse, drop);
 }
 void launch_tr_attn_dq(const float* qkv, const float* dO, const float* lse, const float* delta, const TrSeqs& q,
-                       float* dqkv, cudaStream_t st) {
-  tr_attn_dq_kernel<<<dim3(q.seqs * ceil_div(q.n, TA_Q), q.heads), TA_Q, 0, st>>>(qkv, dO, lse, delta, q, dqkv);
+                       float* dqkv, cudaStream_t st, const TrDrop& drop) {
+  dim3 grid(q.seqs * ceil_div(q.n, TA_Q), q.heads);
+  if (drop.thresh) tr_attn_dq_kernel<true><<<grid, TA_Q, 0, st>>>(qkv, dO, lse, delta, q, dqkv, drop);
+  else tr_attn_dq_kernel<false><<<grid, TA_Q, 0, st>>>(qkv, dO, lse, delta, q, dqkv, drop);
 }
 void launch_tr_attn_dkv(const float* qkv, const float* dO, const float* lse, const float* delta, const TrSeqs& q,
-                        float* dqkv, cudaStream_t st) {
-  tr_attn_dkv_kernel<<<dim3(q.seqs * ceil_div(q.n, TA_Q), q.heads), TA_Q, 0, st>>>(qkv, dO, lse, delta, q, dqkv);
+                        float* dqkv, cudaStream_t st, const TrDrop& drop) {
+  dim3 grid(q.seqs * ceil_div(q.n, TA_Q), q.heads);
+  if (drop.thresh) tr_attn_dkv_kernel<true><<<grid, TA_Q, 0, st>>>(qkv, dO, lse, delta, q, dqkv, drop);
+  else tr_attn_dkv_kernel<false><<<grid, TA_Q, 0, st>>>(qkv, dO, lse, delta, q, dqkv, drop);
 }
 
 }  // namespace bt

@@ -445,10 +445,19 @@ class Engine:
                    p(truth_beat, dtype=byte), p(truth_downbeat, dtype=byte), p(padding_mask, dtype=byte))
 
     # ---- model gradients (bt_train_*) ----------------------------------------------------------------
-    def train_activation_bytes(self, B: int, L: int) -> int:
-        n = int(self.lib.bt_train_activation_bytes(self.ctx, int(B), int(L)))
+    @staticmethod
+    def _train_mode(mode):
+        """mode: None (eval mode) or (seed, dropout_frontend, dropout_transformer) -> a bt_train_mode or None."""
+        if mode is None:
+            return None
+        seed, p_front, p_trans = mode
+        return _lib.bt_train_mode(int(seed) & (2 ** 64 - 1), float(p_front), float(p_trans))
+
+    def train_activation_bytes(self, B: int, L: int, mode=None) -> int:
+        """Bytes of the activation store: mode None (eval mode) or (seed, dropout_frontend, dropout_transformer)."""
+        n = int(self.lib.bt_train_activation_bytes_ex(self.ctx, int(B), int(L), self._train_mode(mode)))
         if n < 0:
-            raise ValueError(f"bt_train_activation_bytes refused B={B}, L={L}")
+            raise ValueError(f"bt_train_activation_bytes_ex refused B={B}, L={L}")
         return n
 
     def _table_ptrs(self, tensors, what: str):
@@ -467,20 +476,26 @@ class Engine:
                                    f"got {t.dtype} {tuple(t.shape)} on {t.device}; there is no CPU fallback")
         return (c_void_p * len(tensors))(*[None if t is None else t.data_ptr() for t in tensors])
 
-    def train_forward(self, params, spect, act, beat, down):
-        """bt_train_forward: params in bt_train_param_info order (device tensors), spect [B, L, 128] fp32, act a byte
-        tensor of train_activation_bytes(B, L), beat / down [B, L] fp32 outputs."""
+    def train_forward(self, params, spect, act, beat, down, mode=None, running=None):
+        """bt_train_forward_ex: params in bt_train_param_info order (device tensors), spect [B, L, 128] fp32, act a byte
+        tensor of train_activation_bytes(B, L, mode), beat / down [B, L] fp32 outputs.  mode None: eval mode; else
+        (seed, dropout_frontend, dropout_transformer), and running (parallel to params; None: params itself) holds the
+        running statistics the pass updates in place."""
         B, L, _ = spect.shape
         p = self._dev_ptr
-        self._call("bt_train_forward", self._table_ptrs(params, "parameter"), len(params), p(spect, B * L * 128), B, L,
-                   p(act, dtype=torch.uint8), act.numel(), p(beat, B * L), p(down, B * L))
+        run = None
+        if mode is not None:
+            run = self._table_ptrs(params if running is None else running, "running statistic")
+        self._call("bt_train_forward_ex", self._table_ptrs(params, "parameter"), len(params), run, p(spect, B * L * 128),
+                   B, L, self._train_mode(mode), p(act, dtype=torch.uint8), act.numel(), p(beat, B * L), p(down, B * L))
 
-    def train_backward(self, params, act, B: int, L: int, dbeat, ddown, grads, dspect=None):
-        """bt_train_backward after train_forward with the same params and act: grads (None: not wanted) parallel to
-        params; dspect [B, L, 128] or None."""
+    def train_backward(self, params, act, B: int, L: int, dbeat, ddown, grads, dspect=None, mode=None):
+        """bt_train_backward_ex after train_forward with the same params, act and mode: grads (None: not wanted)
+        parallel to params; dspect [B, L, 128] or None."""
         p = self._dev_ptr
-        self._call("bt_train_backward", self._table_ptrs(params, "parameter"), len(params), p(act, dtype=torch.uint8), act.numel(),
-                   int(B), int(L), p(dbeat, B * L), p(ddown, B * L), self._table_ptrs(grads, "gradient"), p(dspect, B * L * 128))
+        self._call("bt_train_backward_ex", self._table_ptrs(params, "parameter"), len(params), p(act, dtype=torch.uint8),
+                   act.numel(), int(B), int(L), self._train_mode(mode), p(dbeat, B * L), p(ddown, B * L),
+                   self._table_ptrs(grads, "gradient"), p(dspect, B * L * 128))
 
     # ---- per-kernel-class timing (bench.py roofline) -------------------------------------------
     def profile_enable(self, on: bool = True):

@@ -512,7 +512,7 @@ int bt_train_batch(bt_ctx* ctx, const uint16_t* rows_dev, const int64_t* row_off
                    const int64_t* downbeat_offsets_host, uint16_t* out_spect_dev, uint8_t* truth_beat_dev,
                    uint8_t* truth_downbeat_dev, uint8_t* padding_mask_dev, void* stream);
 
-/* ---- model gradients: loss.backward() through the reference's BeatThis in eval() mode ------------------------------
+/* ---- model gradients: loss.backward() through the reference's BeatThis in eval() mode (train() mode: below) ---------
  * The gradient of the function the inference path computes (BatchNorm on its running statistics, no dropout), in fp32
  * on the CUDA cores (ABI 2.12).  The parameters are the caller's: unfolded fp32 device tensors, one per entry of
  * BeatThis.state_dict(), in the order and shapes of bt_train_param_info, passed on every call as a host array of
@@ -548,6 +548,48 @@ int bt_train_backward(bt_ctx* ctx, const float* const* params, int32_t n_params,
                       int32_t B, int32_t L, const float* dbeat_dev, const float* ddown_dev, float* const* grads,
                       float* dspect_dev, void* stream);
 
+/* ---- training mode (ABI 2.14): the reference's BeatThis in train() mode ---------------------------------------------
+ * The three calls above are the _ex calls below with mode NULL (eval mode).  With a bt_train_mode, the forward pass is
+ * that of the reference's model after .train():
+ *  - Dropout at rate dropout_frontend in the three frontend blocks' partial transformers and dropout_transformer in the
+ *    main transformer blocks, at four sites per residual branch: an attention's probabilities after the softmax (Attend's
+ *    dropout_p) and the output of to_out (to_out.1); a feed-forward's GELU output (net.3) and output (net.5).  Kept values
+ *    are scaled by 1 / (1 - p).  Valid rates are 0 <= p < 1; a rate of 0 is no dropout.
+ *  - BatchNorm (the stem's bn1d and bn2d, each frontend block's norm) on the batch mean and biased variance over every
+ *    position of the batch, zero padding included: B L positions for bn1d, B L F for the others.  The forward pass
+ *    updates running_mean and running_var in place, r = 0.9 r + 0.1 batch (the unbiased variance N / (N - 1) for
+ *    running_var), through `running`: a host array of device pointers parallel to params, whose running_mean and
+ *    running_var entries must be set (the others are not read; it may be params itself).  num_batches_tracked is the
+ *    caller's to increment.
+ * Dropout masks: element e of dropout site `site` under `seed` is kept iff 32-bit word e mod 4 of
+ * Philox4x32-10(counter (lo32(e / 4), hi32(e / 4), site, 0), key (lo32(seed), hi32(seed))) (the rounds of curand's
+ * curand_Philox4x32_10) is >= floor(p 2^32), and kept values are multiplied by 1 / (1 - p) rounded to float; p is the
+ * float rate as passed (0.9f, not 0.9).
+ *  - site: 2 s + k for step s of the model's layer list (stem, then per frontend block attnF, ffF, attnT, ffT and the
+ *    block's convolution (without partial transformers only the convolution), frontend.linear, per main block its
+ *    attention and feed-forward, the head), k = 0 for an attention's probabilities or a feed-forward's GELU output, 1 for
+ *    to_out's or the feed-forward's output.
+ *  - e, elementwise sites: row N + col of the step's [M, N] token rows (frontend token row ((b F + f) L + t), main
+ *    row b L + t; N = channels, or the FFN hidden width for net.3).
+ *  - e, attention probabilities: ((s heads + h) n + i) n + j for query i and key j of sequence s (frequency attention:
+ *    s = b L + t over n = F planes; time attention: s = b F + f, or b in the main blocks, over n = L frames).
+ * Masks are never stored: the backward pass regenerates them, so it must get the forward's mode (seed and rates), and
+ * uses the forward's batch statistics, kept in the store (bt_train_activation_bytes_ex with the same mode sizes it).
+ * BT_ERR_ARG before anything is enqueued, beyond the checks above: a rate outside [0, 1) or NaN, a store sized for eval
+ * mode, a NULL running table or running_mean / running_var entry (forward), and B L < 2 (a BatchNorm would see one value
+ * per channel, which torch refuses in training mode). */
+typedef struct bt_train_mode {
+  uint64_t seed;
+  float dropout_frontend, dropout_transformer;
+} bt_train_mode;
+int64_t bt_train_activation_bytes_ex(const bt_ctx* ctx, int32_t B, int32_t L, const bt_train_mode* mode);
+int bt_train_forward_ex(bt_ctx* ctx, const float* const* params, int32_t n_params, float* const* running,
+                        const float* spect_dev, int32_t B, int32_t L, const bt_train_mode* mode, void* act_dev,
+                        int64_t act_bytes, float* beat_dev, float* down_dev, void* stream);
+int bt_train_backward_ex(bt_ctx* ctx, const float* const* params, int32_t n_params, const void* act_dev,
+                         int64_t act_bytes, int32_t B, int32_t L, const bt_train_mode* mode, const float* dbeat_dev,
+                         const float* ddown_dev, float* const* grads, float* dspect_dev, void* stream);
+
 /* Test hook (fp32 ctx only; BT_ERR_ARG for a 16-bit one): the attention core of one bt_train_forward /
  * bt_train_backward layer alone, on `seqs` time-direction sequences of n positions and `heads` heads of 32.  qkv_dev
  * [seqs * n, 3 * heads * 32] holds q | k | v before RoPE, gates_dev [seqs * n, heads] the gate logits, freqs_dev [16]
@@ -566,16 +608,18 @@ int bt_debug_attention_backward(bt_ctx* ctx, const float* qkv_dev, const float* 
  *             (+ resid[m ldr + n]) over M x N x K, A(m, k) = A[m a_rs + k a_cs], B likewise; gelu_out (ldc) = GELU(C).
  *             splits (0: the weight-gradient policy of the training pass) > 1 runs tr_gemm into part [parts, M, N] and
  *             tr_reduce (scale) into C, which then needs ldc = N and no bias, resid or gelu_out.  resid may alias C.
- *   REDUCE    part [splits, M], out* [M]           out = scale sum_z part[z]
- *   COLSUM    A, B?, rs?, part*, out*              A, B [M, N], rs [M]: part [parts, N] of up to `splits` row ranges
- *             (0: the training pass's policy) of A (* B) (* rs[m]), then out [N] = scale sum of the parts
+ *   REDUCE    part [splits, M], out* [M]           out = scale sum_z part[z] (masked; + beta out when beta != 0)
+ *   COLSUM    A, B?, rs?, part*, out*, shift?      A, B [M, N], rs [M]: part [parts, N] of up to `splits` row ranges
+ *             (0: the training pass's policy) of A (* B) (* rs[m]), then out [N] = scale sum of the parts; shift [N]
+ *             centres A's columns (A - shift, squared without B)
  *   RMS_FWD   x, gamma, xn*, inv*                  [M, C], gamma [C], inv [M]
  *   RMS_BWD   dxn, x, inv, gamma, dres*            dres [M, C] = (flag ? dres : 0) + dx
  *   BN_GELU_FWD  z, w, b, rm, rv, y*               [M] elements of C channels (index % C), BatchNorm arrays [C]
  *   BN_GELU_BWD  dy, z, w, b, rm, rv, dbn*, dz*
  *   BN_GRADS  s_gz, s_g, w, b, rm, rv, dw?*, db?*  [C]
- *   BN_SCALE  g, w, b, rm, rv, dx*                 [M] elements of C channels
- *   GELU_BWD  da, h, dh*                           [M]; dh may be da (in place)
+ *   BN_SCALE  g, w, b, rm, rv, dx*, x?, s_gz?, s_g?  [M] elements of C channels; with x: the batch-statistics input
+ *             gradient, rm / rv the batch mean and biased variance over bn_n positions, s_gz / s_g [C] = sum g x, sum g
+ *   GELU_BWD  da, h, dh*                           [M]; dh may be da (in place); masked da
  *   IM2COL    in, col*, w?, b?, rm?, rv?           flag: through the 1-d BatchNorm of the input's F S frequencies;
  *             input element (b, f, t, c) of B x (F S) x L x C at b sb + f sf + t st + c sc; col [B F L, C S 3]
  *   COL2IM    dcol, din*                           the adjoint of IM2COL without BatchNorm
@@ -589,6 +633,10 @@ int bt_debug_attention_backward(bt_ctx* ctx, const float* qkv_dev, const float* 
  *             row r = (s / seq_in) s_out + (s % seq_in) s_in + i s_pos of qkv [*, 3C], O [*, C], lse [*, heads]
  *   ATTN_DQ   qkv, dO, lse, delta, dqkv*           dO [*, C], delta [*, heads]; the q columns of dqkv [*, 3C]
  *   ATTN_DKV  qkv, dO, lse, delta, dqkv*           the k and v columns of dqkv
+ * Dropout (p > 0; GEMM unsplit, REDUCE, GELU_BWD, ATTN_*): the mask of `site` under `seed` at element e0 + the op's own
+ * element index (GEMM m N + n, REDUCE and GELU_BWD i, attention ((s heads + h) n + i) n + j), as the training pass
+ * applies it; GEMM masks gelu_out when given, else the result before resid.  e0 lets a test reach element indices past
+ * 2^32 without an array that long.
  * Beyond the hook rules below: a geometry or stride that would take a kernel outside an array's count, a negative
  * stride, a launch grid out of range, or a misaligned pointer where the kernel moves float4 (qkv, O, dO and dqkv of
  * the attention ops) is BT_ERR_ARG with nothing enqueued.  The kernels count and profile under the names the
@@ -613,6 +661,14 @@ typedef struct bt_debug_train_desc {
   int64_t sb, sf, st, sc;                    /* IM2COL / COL2IM input strides */
   int32_t seqs, n, seq_in, pad_;             /* attention sequences */
   int64_t s_out, s_in, s_pos;
+  /* ABI 2.14; all zero: no dropout, no beta, eval-mode BN_SCALE */
+  uint64_t seed;                             /* dropout: the mask's seed */
+  float p;                                   /* dropout rate in [0, 1), 0: none */
+  uint32_t site;                             /* dropout site */
+  int64_t e0;                                /* element index of the op's first element */
+  float beta;                                /* REDUCE */
+  int32_t pad2_;
+  int64_t bn_n;                              /* BN_SCALE with batch statistics: positions per channel */
 } bt_debug_train_desc;
 int bt_debug_train_kernel(bt_ctx* ctx, const bt_debug_train_desc* desc, float* const* arrays_dev, const int64_t* counts,
                           int32_t n_arrays, void* stream);

@@ -1,0 +1,495 @@
+"""The training-mode function (bt_train_forward_ex / bt_train_backward_ex with a bt_train_mode, BeatThisModule with
+train_mode=True): dropout masks bit for bit from the documented Philox numbering, the model against a float64
+restatement of the reference's train() mode with the same masks (tests/train_mode_reference.py), the running
+statistics, the module's semantics and refusals, and a short training run from the reference's initialisation."""
+import ctypes
+import math
+import os
+
+import numpy as np
+import pytest
+import torch
+
+import train_mode_reference as TM
+from beat_this_b200 import _lib, synthetic
+from beat_this_b200.engine import Engine
+from beat_this_b200.loss import ShiftTolerantBCELoss
+from beat_this_b200.train import BeatThisModule
+from oracle import philox
+from test_gpu_train import GRAD_BOUND, LOGIT_TOL, _module, _rel, _spect
+
+pytestmark = [pytest.mark.gpu, pytest.mark.timeout(1800)]
+DEV = "cuda:0"
+RATES = (0.1, 0.2, 0.5, 0.9)
+BIG = 5 * 2 ** 32 + 3  # a starting element index past 2^32 (B = 64 at L = 1500 reaches such indices)
+# Batch-statistics BatchNorm makes each channel's input gradient sum to zero, so a bias gradient upstream of one is a
+# heavily cancelled fp32 sum: on an H100 the worst were 1.0e-4 (final0, rates 0), 2.1e-4 (small0, rates 0.5 / 0.9) and
+# 1.2e-3 (small0-nosum, rates 0.5 / 0.9, frontend.blocks.0.partial.attnT.to_gates.bias) while every other tensor
+# stayed within GRAD_BOUND.  torch's own fp32 autograd of the same restatement errs by 1.3e-3 on that tensor
+# (tests/test_cpu_train_mode.py measures it), so the bound is fp32's, not the kernels'.  Biases get this bound.
+BIAS_BOUND = 2e-3
+
+
+@pytest.fixture(scope="module")
+def eng(lib_built):
+    return Engine(None, synthetic.model_hparams("small0"), DEV)
+
+
+def _keep(seed, site, p, n, e0):
+    return torch.from_numpy(philox.keep(seed, site, p, n, e0))
+
+
+def _scale(p):
+    return np.float32(philox.scale(p))
+
+
+# ------------------------------------------------------------------------------------ masks, kernel by kernel
+@pytest.mark.parametrize("p", RATES)
+@pytest.mark.parametrize("seed,site,e0", [(0, 0, 0), (0x0123456789ABCDEF, 7, 13), (2 ** 64 - 1, 70, BIG)])
+def test_reduce_and_gemm_masks_are_bitwise(eng, p, seed, site, e0):
+    drop = dict(p=p, seed=seed, site=site, e0=e0)
+    n = 4099
+    out = torch.full((n,), math.nan, device=DEV)
+    eng.debug_train_kernel("reduce", [torch.ones(n, device=DEV), out], M=n, splits=1, scale=1.0, **drop)
+    want = torch.where(_keep(seed, site, p, n, e0), torch.tensor(_scale(p)), torch.tensor(0.0))
+    assert torch.equal(out.cpu(), want)
+    # GEMM epilogue: all-ones operands of K = 1 give 1 at every (m, n); element e0 + m N + n
+    M, N = 5, 70
+    A, B = torch.ones(M, device=DEV), torch.ones(N, device=DEV)
+    keep = _keep(seed, site, p, M * N, e0).view(M, N)
+    C = torch.full((M * N,), math.nan, device=DEV)
+    eng.debug_train_kernel("gemm", [A, B, C], M=M, N=N, K=1, a_rs=1, a_cs=1, b_rs=1, b_cs=1, ldc=N, splits=1, **drop)
+    assert torch.equal(C.view(M, N).cpu(), torch.where(keep, torch.tensor(_scale(p)), torch.tensor(0.0)))
+    # with gelu_out: C keeps the pre-GELU value, gelu_out is masked
+    g0 = torch.full((M * N,), math.nan, device=DEV)
+    eng.debug_train_kernel("gemm", [A, B, C, None, None, g0], M=M, N=N, K=1, a_rs=1, a_cs=1, b_rs=1, b_cs=1, ldc=N,
+                           splits=1)
+    g = torch.full((M * N,), math.nan, device=DEV)
+    eng.debug_train_kernel("gemm", [A, B, C, None, None, g], M=M, N=N, K=1, a_rs=1, a_cs=1, b_rs=1, b_cs=1, ldc=N,
+                           splits=1, **drop)
+    assert torch.equal(C.cpu(), torch.ones(M * N))
+    want = torch.where(keep.reshape(-1), g0.cpu() * torch.tensor(_scale(p)), torch.tensor(0.0))
+    assert torch.equal(g.cpu(), want)
+
+
+@pytest.mark.parametrize("p", RATES)
+@pytest.mark.parametrize("seed,site,e0", [(3, 1, 0), (2 ** 63 + 5, 33, BIG)])
+def test_gelu_backward_mask(eng, p, seed, site, e0):
+    n = 3001
+    h = torch.randn(n, generator=torch.Generator().manual_seed(seed % 1000)).to(DEV)
+    da = torch.ones(n, device=DEV)
+    d0, d = torch.full((n,), math.nan, device=DEV), torch.full((n,), math.nan, device=DEV)
+    eng.debug_train_kernel("gelu_bwd", [da, h, d0], M=n)
+    eng.debug_train_kernel("gelu_bwd", [da, h, d], M=n, p=p, seed=seed, site=site, e0=e0)
+    keep = _keep(seed, site, p, n, e0)
+    d, ref = d.cpu().double(), d0.cpu().double() * float(_scale(p))
+    assert torch.equal(d == 0, ~keep | (ref == 0))
+    assert ((d - ref).abs() <= 2 ** -23 * ref.abs() * 2)[keep].all()
+
+
+def _attn_inputs(seqs, n, heads):
+    """q = 0 (uniform probabilities), k_j and v_j one-hot at dimension j of every head, lse = log n"""
+    C = heads * 32
+    qkv = torch.zeros(seqs * n, 3 * C)
+    for j in range(n):
+        for h in range(heads):
+            qkv[j::n, C + h * 32 + j] = 1.0
+            qkv[j::n, 2 * C + h * 32 + j] = 1.0
+    lse = torch.full((seqs * n, heads), math.log(n))
+    return qkv.to(DEV), lse.to(DEV)
+
+
+@pytest.mark.parametrize("p", RATES)
+@pytest.mark.parametrize("seed,site,e0", [(11, 0, 0), (2 ** 40 + 1, 9, BIG)])
+def test_attention_masks_are_where_the_outputs_vanish(eng, p, seed, site, e0):
+    seqs, n, heads = 3, 29, 2
+    C = heads * 32
+    geo = dict(seqs=seqs, n=n, heads=heads, seq_in=1, s_out=n, s_in=0, s_pos=1)
+    drop = dict(p=p, seed=seed, site=site, e0=e0)
+    keep = _keep(seed, site, p, seqs * heads * n * n, e0).view(seqs, heads, n, n)  # [s, h, i, j]
+    qkv, lse = _attn_inputs(seqs, n, heads)
+    O = torch.full((seqs * n, C), math.nan, device=DEV)
+    L_ = torch.full((seqs * n, heads), math.nan, device=DEV)
+    eng.debug_train_kernel("attn_fwd", [qkv, O, L_], **geo, **drop)
+    o = O.cpu().view(seqs, n, heads, 32)[..., :n].permute(0, 2, 1, 3)  # [s, h, i, j]: m_ij s / n
+    assert torch.equal(o != 0, keep)
+    assert torch.allclose(L_.cpu(), torch.full_like(L_.cpu(), math.log(n)))
+    # dq_i[j] = p_ij (m_ij s dO_i . v_j - delta_i) / sqrt 32 with dO = 1, delta = 0
+    delta = torch.zeros(seqs * n, heads, device=DEV)
+    dqkv = torch.full((seqs * n, 3 * C), math.nan, device=DEV)
+    eng.debug_train_kernel("attn_dq", [qkv, torch.ones(seqs * n, C, device=DEV), lse, delta, dqkv], **geo, **drop)
+    dq = dqkv.cpu().view(seqs, n, 3, heads, 32)[:, :, 0, :, :n].permute(0, 2, 1, 3)
+    assert torch.equal(dq != 0, keep)
+    # dv_j[i] = sum_i' m_i'j s p_i'j dO_i'[i] with dO_i one-hot at dimension i
+    dO = torch.zeros(seqs * n, C)
+    for i in range(n):
+        for h in range(heads):
+            dO[i::n, h * 32 + i] = 1.0
+    eng.debug_train_kernel("attn_dkv", [qkv, dO.to(DEV), lse, delta, dqkv], **geo, **drop)
+    dv = dqkv.cpu().view(seqs, n, 3, heads, 32)[:, :, 2, :, :n].permute(0, 2, 3, 1)  # [s, h, i, j]
+    assert torch.equal(dv != 0, keep)
+
+
+def test_kept_fractions_and_independence(eng):
+    n = 10 ** 7
+    ones = torch.ones(n, device=DEV)
+    for p in (0.1, 0.5):
+        masks = []
+        for seed, site in ((1, 0), (1, 1), (2, 0)):
+            out = torch.empty(n, device=DEV)
+            eng.debug_train_kernel("reduce", [ones, out], M=n, splits=1, scale=1.0, p=p, seed=seed, site=site)
+            masks.append(out != 0)
+        for m in masks:
+            assert abs(m.float().mean().item() - (1 - p)) <= 6 * math.sqrt(p * (1 - p) / n)
+        q = (1 - p) ** 2  # two independent masks keep an element together at this rate
+        for a, b in ((0, 1), (0, 2)):
+            both = (masks[a] & masks[b]).float().mean().item()
+            assert abs(both - q) <= 6 * math.sqrt(q * (1 - q) / n)
+
+
+def test_colsum_shift_and_reduce_beta(eng):
+    g = torch.Generator().manual_seed(4)
+    M, N = 1000, 37
+    A = torch.randn(M, N, generator=g, dtype=torch.float64) * 0.5 + 3.0
+    Bm = torch.randn(M, N, generator=g, dtype=torch.float64)
+    mean = A.mean(0)
+    part = torch.empty(64 * N, device=DEV)
+    for B_, want in ((None, ((A - mean) ** 2).sum(0)), (Bm, ((A - mean) * Bm).sum(0))):
+        out = torch.full((N,), math.nan, device=DEV)
+        eng.debug_train_kernel("colsum", [A.float().to(DEV).reshape(-1), None if B_ is None else B_.float().to(DEV).reshape(-1),
+                                          None, part, out, mean.float().to(DEV)], M=M, N=N, splits=3, scale=1.0)
+        assert _rel(out, want) < 1e-5
+    r = torch.randn(N, generator=g)
+    x = torch.randn(N, generator=g)
+    out = r.to(DEV)
+    eng.debug_train_kernel("reduce", [x.to(DEV), out], M=N, splits=1, scale=0.1, beta=0.9)
+    assert _rel(out, 0.9 * r.double() + 0.1 * x.double()) < 1e-6
+
+
+def test_bn_scale_batch_statistics_terms(eng):
+    """dx of a training-mode BatchNorm against float64 autograd"""
+    g = torch.Generator().manual_seed(5)
+    M, C = 700, 24
+    x = torch.randn(M, C, generator=g, dtype=torch.float64) * 2 + 1
+    w, b = torch.rand(C, generator=g, dtype=torch.float64) + 0.5, torch.randn(C, generator=g, dtype=torch.float64)
+    dy = torch.randn(M, C, generator=g, dtype=torch.float64)
+    xr = x.clone().requires_grad_(True)
+    mean, var = xr.mean(0), xr.var(0, unbiased=False)
+    ((xr - mean) / torch.sqrt(var + 1e-5) * w + b).backward(dy)
+    f = lambda t: t.float().contiguous().to(DEV).reshape(-1)  # noqa: E731
+    dx = torch.full((M * C,), math.nan, device=DEV)
+    sgz, sg = (dy * x).sum(0), dy.sum(0)
+    eng.debug_train_kernel("bn_scale", [f(dy), f(w), f(b), f(mean.detach()), f(var.detach()), dx, f(x), f(sgz), f(sg)],
+                           M=M * C, C=C, bn_n=M)
+    assert _rel(dx, xr.grad.reshape(-1)) < 1e-4
+
+
+# ------------------------------------------------------------------------------------ the model end to end
+def _tables(module):
+    return module._tables()
+
+
+def _run(module, x, mode, dbeat, ddown):
+    """forward + backward through the engine: (beat, down, dspect, {trainable name: grad})"""
+    eng = module.engine
+    params = _tables(module)
+    B, L, _ = x.shape
+    act = torch.empty(eng.train_activation_bytes(B, L, mode), dtype=torch.uint8, device=DEV)
+    beat, down = torch.empty(B, L, device=DEV), torch.empty(B, L, device=DEV)
+    xs = x.to(DEV).contiguous()
+    eng.train_forward(params, xs, act, beat, down, mode=mode)
+    grads = [torch.empty_like(p) if t else None for p, t in zip(params, module._trainable)]
+    dspect = torch.empty(B, L, 128, device=DEV)
+    eng.train_backward(params, act, B, L, dbeat.to(DEV), ddown.to(DEV), grads, dspect, mode=mode)
+    named = {n: g for n, g in zip(module._names, grads) if g is not None}
+    return beat, down, dspect, named
+
+
+E2E = [  # family, B, L, lengths, overrides
+    ("small0", 3, 17, None, {}),
+    ("small0", 8, 17, None, {}),
+    ("small0-nosum", 3, 17, None, {}),
+    ("small0-nopartial", 3, 17, None, {}),
+    ("1024", 3, 17, None, {"ff_mult": 2}),
+    ("small0", 3, 400, (400, 251, 90), {}),
+]
+
+
+def _check_e2e(family, B, L, lengths, overrides, rates, seed=1234567):
+    module, _ = _module(family, **overrides)
+    sum_head = synthetic.model_hparams(family)["sum_head"]
+    x = _spect(B, L, 1, lengths)
+    g = torch.Generator().manual_seed(2)
+    dbeat, ddown = torch.randn(B, L, generator=g), torch.randn(B, L, generator=g)
+    running0 = {k: v.detach().clone().cpu().double() for k, v in module.state_dict().items() if "running" in k}
+    beat, down, dspect, grads = _run(module, x, (seed,) + rates, dbeat, ddown)
+    sd = {k: (v.detach().cpu().double().requires_grad_(v.requires_grad) if v.is_floating_point() else v.cpu())
+          for k, v in module.state_dict(keep_vars=True).items()}
+    x64 = x.double().requires_grad_(True)
+    ob, od, stats = TM.forward_train(sd, x64, seed, *rates, sum_head=sum_head)
+    names = list(grads)
+    ref = torch.autograd.grad((ob, od), [x64] + [sd[n] for n in names], (dbeat.double(), ddown.double()))
+    assert (beat.cpu().double() - ob.detach()).abs().max() < LOGIT_TOL
+    assert (down.cpu().double() - od.detach()).abs().max() < LOGIT_TOL
+    errs = {"spect": _rel(dspect, ref[0])}
+    errs.update({n: _rel(grads[n], r) for n, r in zip(names, ref[1:])})
+    for name, e in errs.items():
+        assert e <= (BIAS_BOUND if name.endswith(".bias") else GRAD_BOUND), f"{name}: {e:.3e}"
+    now = module.state_dict()
+    for p, (mean, var, N) in stats.items():
+        want_m = 0.9 * running0[p + ".running_mean"] + 0.1 * mean
+        want_v = 0.9 * running0[p + ".running_var"] + 0.1 * var * N / (N - 1)
+        assert _rel(now[p + ".running_mean"], want_m) < 1e-4, p
+        assert _rel(now[p + ".running_var"], want_v) < 1e-4, p
+
+
+@pytest.mark.parametrize("rates", [(0.0, 0.0), (0.1, 0.2), (0.5, 0.9)])
+@pytest.mark.parametrize("family,B,L,lengths,overrides", E2E)
+def test_training_mode_matches_float64_autograd(family, B, L, lengths, overrides, rates):
+    _check_e2e(family, B, L, lengths, overrides, rates)
+
+
+def test_training_mode_final0_batch_statistics():
+    """final0 at the reference's training batch (8, 1500) with batch-statistics BatchNorm; the float64 restatement of
+    its dropout masks (explicit probabilities of 8 x 16 x 1500^2 per layer) does not fit a test's memory."""
+    _check_e2e("final0", 8, 1500, None, {}, (0.0, 0.0))
+
+
+def test_activation_store_counted_independently(eng):
+    for family in ("small0", "small0-nopartial", "final0"):
+        hp = synthetic.model_hparams(family)
+        e = Engine(None, hp, DEV)
+        for B, L in ((2, 10), (3, 17)):
+            assert e.train_activation_bytes(B, L, (0, 0.1, 0.2)) == 4 * TM.activation_floats(hp, B, L)
+
+
+# ------------------------------------------------------------------------------------ semantics
+def test_reference_fixture_is_reproduced():
+    """The unmodified reference's BeatThis in train() mode with the library's masks patched into its nn.Dropout and
+    Attend (tests/golden/train_mode.npz, oracle/make_golden_train_mode.py): logits, loss, the spectrogram's gradient,
+    every parameter's fingerprint, the updated running statistics and num_batches_tracked."""
+    from oracle.train_fingerprint import bounds, fingerprint
+
+    z = np.load(os.path.join(os.path.dirname(__file__), "golden", "train_mode.npz"))
+    k = 0
+    while f"family{k}" in z:
+        family, seed = str(z[f"family{k}"]), int(z[f"seed{k}"])
+        mode = (int(z[f"mode_seed{k}"]), *map(float, z[f"rates{k}"]))
+        module = BeatThisModule.from_checkpoint(synthetic.make_checkpoint(family, seed), DEV, train_mode=True)
+        x = torch.tensor(z[f"spect{k}"])
+        beat, down, dspect, grads = _run(module, x, mode, torch.tensor(z[f"dbeat{k}"]).float(),
+                                         torch.tensor(z[f"ddown{k}"]).float())
+        assert np.abs(beat.cpu().numpy() - z[f"beat{k}"]).max() < LOGIT_TOL
+        assert np.abs(down.cpu().numpy() - z[f"downbeat{k}"]).max() < LOGIT_TOL
+        t = lambda a: torch.tensor(a, device=DEV, dtype=torch.float32)  # noqa: E731
+        mask = t(z[f"padding_mask{k}"])
+        loss = ShiftTolerantBCELoss()(beat, t(z[f"truth_beat{k}"]), mask) + ShiftTolerantBCELoss()(
+            down, t(z[f"truth_downbeat{k}"]), mask * t(z[f"downbeat_mask{k}"])[:, None])
+        assert abs(loss.item() - float(z[f"loss{k}"])) <= 1e-3 * abs(float(z[f"loss{k}"]))
+        ref = z[f"dspect{k}"].astype(np.float64)
+        assert np.linalg.norm(dspect.cpu().numpy() - ref) <= GRAD_BOUND * np.linalg.norm(ref)
+        index = {n: i for i, n in enumerate(module.state_dict())}
+        for name, fp in zip(z[f"names{k}"], z[f"fp{k}"]):
+            name = str(name)
+            g = grads[name].double().cpu().numpy()
+            rel = BIAS_BOUND if name.endswith(".bias") else GRAD_BOUND
+            assert (np.abs(fingerprint(g, index[name]) - fp) <= bounds(fp, g.size, index[name], rel)).all(), name
+        sd = module.state_dict()
+        got = np.concatenate([sd[str(n)].cpu().double().numpy().reshape(-1) for n in z[f"running_names{k}"]])
+        want = z[f"running{k}"]
+        assert np.linalg.norm(got - want) <= GRAD_BOUND * np.linalg.norm(want)
+        # num_batches_tracked: the module's counter after one training-mode forward
+        module.train()
+        with torch.no_grad():
+            module(x.to(DEV))
+        tracked = [int(v) for n, v in module.state_dict().items() if n.endswith(".num_batches_tracked")]
+        assert tracked == [int(v) for v in z[f"tracked{k}"]]
+        k += 1
+    assert k == 4
+
+
+def test_two_forwards_then_one_backward():
+    """A training-mode forward updates the running statistics and num_batches_tracked in place; a second forward
+    before the first one's backward is allowed, as with torch's BatchNorm, and gives each its own gradient."""
+    ckpt = synthetic.make_checkpoint("small0", 5)
+    module = BeatThisModule.from_checkpoint(ckpt, DEV, train_mode=True).train()
+    x1, x2 = _spect(2, 30, 1).to(DEV), _spect(2, 30, 2).to(DEV)
+    torch.manual_seed(3)
+    o1 = module(x1)
+    o2 = module(x2)
+    (o1["beat"].sum() + o2["downbeat"].square().sum()).backward()
+    both = {n: p.grad.clone() for n, p in module.named_parameters() if p.grad is not None}
+    # the same two passes, each with its own backward
+    module = BeatThisModule.from_checkpoint(ckpt, DEV, train_mode=True).train()
+    torch.manual_seed(3)
+    module(x1)["beat"].sum().backward()
+    module(x2)["downbeat"].square().sum().backward()
+    for n, p in module.named_parameters():
+        if p.grad is not None:
+            assert torch.allclose(both[n], p.grad, rtol=1e-5, atol=1e-6 * p.grad.abs().max().item()), n
+    assert module.state_dict()["frontend.stem.bn1d.num_batches_tracked"].item() == \
+        int(ckpt["state_dict"]["model.frontend.stem.bn1d.num_batches_tracked"]) + 2
+
+
+def test_seeds_determine_the_result():
+    module, _ = _module("small0", 3)
+    x = _spect(2, 40, 7)
+    g = torch.Generator().manual_seed(8)
+    db, dd = torch.randn(2, 40, generator=g), torch.randn(2, 40, generator=g)
+    state = {k: v.clone() for k, v in module.state_dict().items()}
+
+    def run(seed):
+        module.load_state_dict(state)
+        b, d, ds, gr = _run(module, x, (seed, 0.1, 0.2), db, dd)
+        return [b, d, ds] + [gr[k] for k in sorted(gr)]
+
+    a, b, c = run(5), run(5), run(6)
+    assert all(torch.equal(u, v) for u, v in zip(a, b))
+    assert not torch.equal(a[0], c[0]) and not torch.equal(a[3], c[3])
+
+
+def test_module_train_mode_semantics():
+    ckpt = synthetic.make_checkpoint("small0", 4)
+    default = BeatThisModule.from_checkpoint(ckpt, DEV)
+    with pytest.raises(NotImplementedError, match="dropout"):
+        default.train()
+    module = BeatThisModule.from_checkpoint(ckpt, DEV, train_mode=True)
+    assert not module.training
+    x = _spect(2, 30, 9).to(DEV)
+
+    def step(m, seed=None):
+        if seed is not None:
+            torch.manual_seed(seed)
+        m.zero_grad(set_to_none=True)
+        xs = x.clone().requires_grad_(True)
+        out = m(xs)
+        (out["beat"].square().sum() + out["downbeat"].sum()).backward()
+        return [out["beat"].detach(), xs.grad] + [p.grad for p in m.parameters() if p.grad is not None]
+
+    state = {k: v.clone() for k, v in module.state_dict().items()}
+    module.train()
+    r1 = step(module, 17)
+    n1 = module.state_dict()["frontend.stem.bn1d.num_batches_tracked"].item()
+    moved = not torch.equal(module.state_dict()["frontend.stem.bn1d.running_mean"], state["frontend.stem.bn1d.running_mean"])
+    module.load_state_dict(state)
+    r2 = step(module, 17)
+    assert all(torch.equal(a, b) for a, b in zip(r1, r2))  # torch.manual_seed makes a run repeatable
+    assert n1 == state["frontend.stem.bn1d.num_batches_tracked"].item() + 1 and moved
+    module.load_state_dict(state)
+    with torch.no_grad():  # still updates the running statistics, as torch's BatchNorm does
+        module(x)
+    sd = module.state_dict()
+    assert sd["frontend.blocks.2.norm.num_batches_tracked"].item() == state["frontend.blocks.2.norm.num_batches_tracked"].item() + 1
+    assert not torch.equal(sd["frontend.blocks.2.norm.running_var"], state["frontend.blocks.2.norm.running_var"])
+    # back in eval mode: bitwise the default module
+    module.load_state_dict(state)
+    module.eval()
+    assert all(torch.equal(a, b) for a, b in zip(step(module), step(default)))
+
+
+def test_reset_parameters_is_the_reference_initialisation():
+    module = BeatThisModule(synthetic.model_hparams("final0"), DEV, train_mode=True)
+    module.reset_parameters(torch.Generator().manual_seed(0))
+    freqs = 1.0 / (10000 ** (torch.arange(0, 32, 2).float() / 32))
+    for name, t in module.state_dict().items():
+        t = t.cpu()
+        leaf = name.rsplit(".", 1)[1]
+        bn = any(s in name for s in ("bn1d", "bn2d", ".norm.")) and "gamma" not in name
+        if leaf == "freqs":
+            assert torch.equal(t, freqs), name
+        elif leaf == "gamma" or (bn and leaf in ("weight", "running_var")):
+            assert torch.equal(t, torch.ones_like(t)), name
+        elif leaf in ("bias", "running_mean", "num_batches_tracked"):
+            assert torch.equal(t, torch.zeros_like(t)), name
+        else:
+            assert leaf == "weight" and t.ndim in (2, 4), name
+            std = 0.02 if t.ndim == 2 else math.sqrt(2.0 / (t.shape[0] * t.shape[2] * t.shape[3]))
+            n = t.numel()
+            # mean ~ N(0, std^2 / n); sample variance ~ std^2 (1 +- sqrt(2 / n)): 6 sigma each
+            assert abs(t.double().mean().item()) <= 6 * std / math.sqrt(n), name
+            assert abs(t.double().var().item() / std ** 2 - 1) <= 6 * math.sqrt(2.0 / n) + 1e-3, name
+
+
+def test_training_mode_refusals_before_any_launch():
+    module, _ = _module("small0")
+    eng = module.engine
+    params = module._tables()
+    lib = eng.lib
+    ptrs = eng._table_ptrs(params, "parameter")
+    p = lambda t: ctypes.c_void_p(t.data_ptr())  # noqa: E731
+    stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+    B, L = 2, 10
+    spect = torch.zeros(B, L, 128, device=DEV)
+    beat, down = torch.zeros(B, L, device=DEV), torch.zeros(B, L, device=DEV)
+    ok = _lib.bt_train_mode(1, 0.1, 0.2)
+    act = torch.empty(eng.train_activation_bytes(B, L, (1, 0.1, 0.2)), dtype=torch.uint8, device=DEV)
+    eval_bytes = eng.train_activation_bytes(B, L)
+    assert eval_bytes < act.numel()
+    grads = eng._table_ptrs([None] * len(params), "gradient")
+    before = eng.launches
+
+    def fwd(mode, running=ptrs, nbytes=act.numel(), B_=B, L_=L):
+        return lib.bt_train_forward_ex(eng.ctx, ptrs, len(params), running, p(spect), B_, L_, mode, p(act), nbytes,
+                                       p(beat), p(down), stream)
+
+    for bad in (-0.1, 1.0, math.nan, math.inf):
+        assert fwd(_lib.bt_train_mode(1, bad, 0.2)) == -1
+        assert fwd(_lib.bt_train_mode(1, 0.1, bad)) == -1
+        assert lib.bt_train_backward_ex(eng.ctx, ptrs, len(params), p(act), act.numel(), B, L,
+                                        _lib.bt_train_mode(1, 0.1, bad), p(beat), p(down), grads, None, stream) == -1
+    assert fwd(ok, nbytes=eval_bytes) == -1  # a store sized for eval mode
+    assert lib.bt_train_backward_ex(eng.ctx, ptrs, len(params), p(act), eval_bytes, B, L, ok, p(beat), p(down), grads,
+                                    None, stream) == -1
+    assert fwd(ok, running=None) == -1
+    names = [n for n, _, _ in _lib.train_param_table(module.hparams)]
+    for stat in ("frontend.stem.bn1d.running_mean", "frontend.blocks.1.norm.running_var"):
+        run = (ctypes.c_void_p * len(params))(*[None if n == stat else t.data_ptr() for n, t in zip(names, params)])
+        assert fwd(ok, running=run) == -1
+        assert stat.encode() in lib.bt_last_error(eng.ctx)
+    assert fwd(ok, B_=1, L_=1) == -1  # a BatchNorm of one value per channel
+    assert eng.launches == before
+    with pytest.raises(Exception):
+        BeatThisModule.from_checkpoint(synthetic.make_checkpoint("small0"), DEV, train_mode=True).train()(
+            torch.zeros(1, 1, 128, device=DEV))
+    assert fwd(ok) == 0  # the same call with valid arguments runs
+    torch.cuda.synchronize()
+
+
+# ------------------------------------------------------------------------------------ training from scratch
+def test_training_from_scratch_lowers_the_loss_and_reloads(tmp_path):
+    from beat_this_b200.inference import load_model
+
+    torch.manual_seed(0)
+    module = BeatThisModule(synthetic.model_hparams("small0"), DEV, train_mode=True)
+    module.reset_parameters(torch.Generator().manual_seed(1))
+    module.train()
+    g = torch.Generator().manual_seed(8)
+    B, L = 4, 256
+    x = (torch.rand(B, L, 128, generator=g) * 4).to(DEV)
+    beats = torch.zeros(B, L, device=DEV)
+    beats[:, ::25] = 1
+    downs = torch.zeros(B, L, device=DEV)
+    downs[:, ::100] = 1
+    mask = torch.ones(B, L, device=DEV)
+    mask[1, 200:] = 0
+    x[1, 200:] = 0
+    loss_b, loss_d = ShiftTolerantBCELoss(), ShiftTolerantBCELoss()
+    opt = torch.optim.AdamW([q for q in module.parameters() if q.requires_grad], lr=1e-3)
+    losses = []
+    for _ in range(30):
+        opt.zero_grad()
+        out = module(x)
+        loss = loss_b(out["beat"], beats, mask) + loss_d(out["downbeat"], downs, mask)
+        loss.backward()
+        opt.step()
+        losses.append(loss.item())
+    assert np.isfinite(losses).all()
+    assert np.mean(losses[-5:]) < 0.8 * np.mean(losses[:5]), losses
+    assert module.state_dict()["frontend.stem.bn1d.num_batches_tracked"].item() == 30
+    module.eval()
+    path = module.save_checkpoint(os.path.join(tmp_path, "scratch.ckpt"))
+    with torch.no_grad():
+        out = module(x)
+    ref = load_model(path, DEV, float16=False)(x)
+    for k in ("beat", "downbeat"):
+        assert (out[k] - ref[k]).abs().max().item() < LOGIT_TOL
