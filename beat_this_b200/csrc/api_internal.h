@@ -21,16 +21,23 @@ struct Param {
   int64_t n = 0;
 };
 
-// One layer of the forward pass between the stem and the head.  bt_finalize builds the list from bt_hparams, in schedule
-// order: b{i}.attnF, b{i}.ffF, b{i}.attnT, b{i}.ffT (with partial transformers), b{i}.conv for i < 3, lin, then
-// l{l}.attn, l{l}.ff for every main layer.
-enum LayerKind { kAttnF, kAttnT, kAttn, kFf, kConv, kLin };  // kAttnF / kAttnT: frequency / time attention of a frontend block
-struct Layer {
-  LayerKind kind;
-  std::string name;  // parameter prefix, and the tap name of the layer's output (frontend.linear: "frontend")
-  int C, F;          // channels; frequency planes per chunk (1 in the main layers)
-  int mult;          // FFN hidden width multiplier
-  const Param* w[4]; // resolved weights, in the order of layer_params
+// One step of the model.  model_steps lists them in the order BeatThis.forward runs them: the stem; per frontend block
+// i < 3 attnF, ffF, attnT, ffT (with partial transformers) and the convolution; frontend.linear; per main layer its
+// attention and FFN; the head.  The inference pass (bt_ctx::layers) and the training passes (api_train.cu) both walk
+// this one list, and a step's index in it numbers its dropout sites (include/beatthis.h).
+enum StepKind { kStem, kAttnFreq, kAttnTime, kFfn, kConv, kLinear, kHead };
+struct Step {
+  StepKind kind;
+  int C, F;            // channels; frequency planes per chunk (F > 1: a frontend step)
+  int mult;            // FFN hidden width multiplier
+  std::string name;    // packed-parameter prefix, and the tap name of the step's output (frontend.linear's: "frontend")
+  std::string module;  // state_dict prefix (the head has none: its entries sit under two modules)
+};
+std::vector<Step> model_steps(const bt_hparams& hp);
+
+// A step of the inference pass with its packed weights, resolved by bt_finalize in the order of layer_params.
+struct Layer : Step {
+  const Param* w[4] = {};
 };
 
 // small host -> device tables (offsets, chunk descriptors) travel through a ring of pinned slots: a slot is only
@@ -99,10 +106,9 @@ struct bt_ctx {
   // pinned staging + device tables
   StageSlot stage[kStageSlots];
   int stage_next = 0;
-  std::vector<Layer> layers;  // built by bt_finalize
-  // parameters outside the layer list, resolved in bt_finalize
-  const Param *rope_cos = nullptr, *rope_sin = nullptr, *bn1_scale = nullptr, *bn1_shift = nullptr, *stem_w = nullptr,
-              *stem_b = nullptr, *head_w = nullptr, *head_b = nullptr;
+  std::vector<Layer> layers;  // model_steps, built by bt_finalize: the stem first, the head last
+  // the RoPE tables, resolved in bt_finalize
+  const Param *rope_cos = nullptr, *rope_sin = nullptr;
 
   // per-kernel-class device timing (bt_profile_*): one event after every launch; the
   // duration of a launch is the gap to the previous event on the same stream

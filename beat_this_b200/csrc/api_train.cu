@@ -15,20 +15,17 @@ struct TrParam {
   bool trainable;
 };
 
-// One step of the model.  p: table index of the step's first parameter.  Offsets (in floats) into the activation
-// store; -1 where the step saves nothing there.  bn1 / bn2 (training mode): the batch mean and, 4-float aligned after
-// it, the biased variance of the step's BatchNorms (the stem: bn1d, bn2d; a conv block: bn2 of its norm).
-enum TrKind { kStem, kAttnFreq, kAttnTime, kFfn, kConvBlock, kLinear, kHead };
-struct TrLayer {
-  TrKind kind;
+// A step of model_steps as the training passes run it.  p: table index of the step's first parameter.  Offsets (in
+// floats) into the activation store; -1 where the step saves nothing there.  bn1 / bn2 (training mode): the batch mean
+// and, 4-float aligned after it, the biased variance of the step's BatchNorms (the stem: bn1d, bn2d; a convolution: bn2
+// of its block's norm).
+struct TrLayer : Step {
   int p;
-  int C, F, mult;  // channels, frequency planes, FFN multiplier
   int64_t in = -1, xn = -1, inv = -1, qkv = -1, gate = -1, lse = -1, o = -1, h = -1, a = -1, z = -1, xl = -1;
   int64_t bn1 = -1, bn2 = -1;
-  bool frontend = false;  // dropout at the frontend rate
 };
 
-// The dropout site numbering of include/beatthis.h: site k (0 or 1) of step `step` of the layer list.  An attention
+// The dropout site numbering of include/beatthis.h: site k (0 or 1) of step `step` of model_steps.  An attention
 // step's site 0 is its probabilities and site 1 the output of to_out; a feed-forward step's site 0 is the GELU output
 // (net.3) and site 1 the output of net.4 (net.5).
 uint32_t dropout_site(size_t step, int k) { return static_cast<uint32_t>(2 * step + k); }
@@ -82,74 +79,51 @@ TrModel train_model(const bt_hparams& hp, int64_t B, int64_t L, bool train = fal
     m.floats += (n + 3) & ~int64_t{3};
     return off;
   };
-  auto attn = [&](TrKind kind, const std::string& p, int C, int F, bool frontend) {
-    TrLayer l{kind, static_cast<int>(t.size()), C, F, 0};
-    add_attn(t, p, C);
-    const int64_t M = BL * F;
-    l.in = alloc(M * C), l.xn = alloc(M * C), l.inv = alloc(M), l.qkv = alloc(3 * M * C), l.gate = alloc(M * C / 32);
-    l.lse = alloc(M * C / 32), l.o = alloc(M * C);
-    l.frontend = frontend;
-    m.layers.push_back(l);
-  };
-  auto ffn = [&](const std::string& p, int C, int F, int mult, bool frontend) {
-    TrLayer l{kFfn, static_cast<int>(t.size()), C, F, mult};
-    add_ffn(t, p, C, mult);
-    const int64_t M = BL * F;
-    l.in = alloc(M * C), l.xn = alloc(M * C), l.inv = alloc(M), l.h = alloc(M * mult * C), l.a = alloc(M * mult * C);
-    l.frontend = frontend;
-    m.layers.push_back(l);
-  };
-  {
-    TrLayer l{kStem, static_cast<int>(t.size()), hp.stem_dim, hp.spect_dim / 4, 0};
-    add_bn(t, "frontend.stem.bn1d", hp.spect_dim);
-    add(t, "frontend.stem.conv2d.weight", {hp.stem_dim, 1, 4, 3});
-    add_bn(t, "frontend.stem.bn2d", hp.stem_dim);
-    l.in = alloc(BL * hp.spect_dim), l.z = alloc(BL * l.F * l.C);
-    m.layers.push_back(l);
-  }
-  int C = hp.stem_dim, F = hp.spect_dim / 4;
-  for (int i = 0; i < 3; ++i) {
-    const std::string p = "frontend.blocks." + std::to_string(i);
-    if (hp.partial_transformers) {
-      attn(kAttnFreq, p + ".partial.attnF", C, F, true);
-      ffn(p + ".partial.ffF", C, F, 4, true);
-      attn(kAttnTime, p + ".partial.attnT", C, F, true);
-      ffn(p + ".partial.ffT", C, F, 4, true);
+  for (const Step& s : model_steps(hp)) {
+    TrLayer l{s, static_cast<int>(t.size())};
+    const int C = s.C, H = s.mult * C;
+    const int64_t M = BL * s.F;
+    switch (s.kind) {
+      case kStem:
+        add_bn(t, s.module + ".bn1d", hp.spect_dim);
+        add(t, s.module + ".conv2d.weight", {C, 1, 4, 3});
+        add_bn(t, s.module + ".bn2d", C);
+        l.in = alloc(BL * hp.spect_dim), l.z = alloc(M * C);
+        break;
+      case kAttnFreq:
+      case kAttnTime:
+        add_attn(t, s.module, C);
+        l.in = alloc(M * C), l.xn = alloc(M * C), l.inv = alloc(M), l.qkv = alloc(3 * M * C), l.gate = alloc(M * C / 32);
+        l.lse = alloc(M * C / 32), l.o = alloc(M * C);
+        break;
+      case kFfn:
+        add_ffn(t, s.module, C, s.mult);
+        l.in = alloc(M * C), l.xn = alloc(M * C), l.inv = alloc(M), l.h = alloc(M * H), l.a = alloc(M * H);
+        break;
+      case kConv:
+        add(t, s.module + ".conv2d.weight", {2 * C, C, 2, 3});
+        add_bn(t, s.module + ".norm", 2 * C);
+        l.in = alloc(M * C), l.z = alloc(M / 2 * 2 * C);
+        break;
+      case kLinear:
+        add(t, s.module + ".weight", {hp.transformer_dim, C * s.F});
+        add(t, s.module + ".bias", {hp.transformer_dim});
+        l.in = alloc(M * C), l.xl = alloc(M * C);
+        break;
+      case kHead:
+        add(t, "transformer_blocks.norm.gamma", {C});
+        add(t, "task_heads.beat_downbeat_lin.weight", {2, C});
+        add(t, "task_heads.beat_downbeat_lin.bias", {2});
+        l.in = alloc(M * C), l.xn = alloc(M * C), l.inv = alloc(M);
+        break;
     }
-    TrLayer l{kConvBlock, static_cast<int>(t.size()), C, F, 0};
-    add(t, p + ".conv2d.weight", {2 * C, C, 2, 3});
-    add_bn(t, p + ".norm", 2 * C);
-    l.in = alloc(BL * F * C), l.z = alloc(BL * F / 2 * 2 * C);
-    m.layers.push_back(l);
-    C *= 2;
-    F /= 2;
-  }
-  const int D = hp.transformer_dim;
-  {
-    TrLayer l{kLinear, static_cast<int>(t.size()), C, F, 0};
-    add(t, "frontend.linear.weight", {D, C * F});
-    add(t, "frontend.linear.bias", {D});
-    l.in = alloc(BL * F * C), l.xl = alloc(BL * F * C);
-    m.layers.push_back(l);
-  }
-  for (int i = 0; i < hp.n_layers; ++i) {
-    const std::string p = "transformer_blocks.layers." + std::to_string(i);
-    attn(kAttnTime, p + ".0", D, 1, false);
-    ffn(p + ".1", D, 1, hp.ff_mult, false);
-  }
-  {
-    TrLayer l{kHead, static_cast<int>(t.size()), D, 1, 0};
-    add(t, "transformer_blocks.norm.gamma", {D});
-    add(t, "task_heads.beat_downbeat_lin.weight", {2, D});
-    add(t, "task_heads.beat_downbeat_lin.bias", {2});
-    l.in = alloc(BL * D), l.xn = alloc(BL * D), l.inv = alloc(BL);
     m.layers.push_back(l);
   }
   if (train)
     for (TrLayer& l : m.layers) {
       const auto stats = [&](int ch) { return alloc(2 * ((ch + 3) & ~3)); };
       if (l.kind == kStem) l.bn1 = stats(hp.spect_dim), l.bn2 = stats(l.C);
-      if (l.kind == kConvBlock) l.bn2 = stats(2 * l.C);
+      if (l.kind == kConv) l.bn2 = stats(2 * l.C);
     }
   return m;
 }
@@ -186,10 +160,10 @@ struct TrRun {
     if (!mode) return TrBn{P[p], P[p + 1], P[p + 2], P[p + 3]};
     return TrBn{P[p], P[p + 1], at(off), at(off + ((ch + 3) & ~3))};
   }
-  // dropout site k of step `step` (none in eval mode)
+  // dropout site k of step `step` (none in eval mode), at the frontend rate in a frontend step (F > 1)
   TrDrop drop(const TrLayer& l, size_t step, int k) const {
     if (!mode) return TrDrop{};
-    return tr_drop(mode->seed, dropout_site(step, k), l.frontend ? mode->dropout_frontend : mode->dropout_transformer);
+    return tr_drop(mode->seed, dropout_site(step, k), l.F > 1 ? mode->dropout_frontend : mode->dropout_transformer);
   }
 
   // out[M, N] = X[M, K] W[N, K]^T (+ bias) (+ resid) (gelu_out: GELU of it as well), dropout as TrGemmOut states
@@ -305,7 +279,7 @@ int forward_layer(TrRun& R, const TrLayer& l, size_t step, float* next, float* b
       return R.linear(R.at(l.a), M, l.mult * C, R.w(p + 3), C, R.w(p + 4), next, R.at(l.in), nullptr,
                       R.drop(l, step, 1));
     }
-    case kConvBlock: {
+    case kConv: {
       const TrImg g = R.img(l);
       const int64_t Mo = M / 2;
       launch_tr_im2col(R.at(l.in), g, nullptr, R.s.big, st);
@@ -417,7 +391,7 @@ int backward_layer(TrRun& R, const TrLayer& l, size_t step, float* dspect) {
       BT_LAUNCHED(c, "train_concat", st);
       return BT_OK;
     }
-    case kConvBlock:
+    case kConv:
     case kStem: {
       // the convolution's output: Mo rows of Co channels, K = Ci S 3 columns of im2col
       const bool stem = l.kind == kStem;

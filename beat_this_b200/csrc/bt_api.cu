@@ -119,6 +119,33 @@ int bt::upload_stage(bt_ctx* c, StageSlot* sl, size_t bytes, cudaStream_t st) {
   return BT_OK;
 }
 
+std::vector<Step> bt::model_steps(const bt_hparams& hp) {
+  std::vector<Step> v;
+  int C = hp.stem_dim, F = hp.spect_dim / 4;
+  v.push_back({kStem, C, F, 0, "stem", "frontend.stem"});
+  for (int i = 0; i < 3; ++i) {
+    const std::string b = "b" + std::to_string(i), m = "frontend.blocks." + std::to_string(i);
+    if (hp.partial_transformers) {
+      v.push_back({kAttnFreq, C, F, 0, b + ".attnF", m + ".partial.attnF"});
+      v.push_back({kFfn, C, F, 4, b + ".ffF", m + ".partial.ffF"});
+      v.push_back({kAttnTime, C, F, 0, b + ".attnT", m + ".partial.attnT"});
+      v.push_back({kFfn, C, F, 4, b + ".ffT", m + ".partial.ffT"});
+    }
+    v.push_back({kConv, C, F, 0, b + ".conv", m});
+    C *= 2;
+    F /= 2;
+  }
+  v.push_back({kLinear, C, F, 0, "lin", "frontend.linear"});
+  const int D = hp.transformer_dim;
+  for (int i = 0; i < hp.n_layers; ++i) {
+    const std::string b = "l" + std::to_string(i), m = "transformer_blocks.layers." + std::to_string(i);
+    v.push_back({kAttnTime, D, 1, 0, b + ".attn", m + ".0"});
+    v.push_back({kFfn, D, 1, hp.ff_mult, b + ".ff", m + ".1"});
+  }
+  v.push_back({kHead, D, 1, 0, "head", ""});
+  return v;
+}
+
 namespace {
 
 constexpr bt_chunking kDefaultChunking{BT_CHUNK, BT_BORDER, BT_KEEP_FIRST};
@@ -260,26 +287,27 @@ EpiParams epi_generic(const Param* bias, int gelu, const float* resid, int ldr, 
   return e;
 }
 
-bool is_attention(const Layer& l) { return l.kind == kAttnF || l.kind == kAttnT || l.kind == kAttn; }
+bool is_attention(const Layer& l) { return l.kind == kAttnFreq || l.kind == kAttnTime; }
 
 // sub-blocks of width C = 32 / 64 (the first two frontend blocks) run as one fused kernel each on the 16-bit path
-bool fused(const Layer& l) { return (l.C == 32 || l.C == 64) && (l.kind != kFf || l.mult == 4); }
+bool fused(const Layer& l) { return (l.C == 32 || l.C == 64) && (l.kind != kFfn || l.mult == 4); }
 
-// The out-projection + residual of attention layer i run inside the fused FFN after it (fused_ff_kernel<C, true>) on
-// the 16-bit path when the attention is a frontend one, unless a tap asks to see the residual stream between the two.
+// The out-projection + residual of attention layer i (before the head) run inside the fused FFN after it
+// (fused_ff_kernel<C, true>) on the 16-bit path when the attention is a frontend one, unless a tap asks to see the
+// residual stream between the two.
 bool outproj_in_ff(const bt_ctx* c, size_t i) {
   const Layer& l = c->layers[i];
-  return c->dtype == BT_DTYPE_H16 && (l.kind == kAttnF || l.kind == kAttnT) && i + 1 < c->layers.size() &&
-         c->layers[i + 1].kind == kFf && fused(c->layers[i + 1]) && c->tap_name != l.name;
+  return c->dtype == BT_DTYPE_H16 && is_attention(l) && l.F > 1 && c->layers[i + 1].kind == kFfn &&
+         fused(c->layers[i + 1]) && c->tap_name != l.name;
 }
 
 // x += attention(x) over nb * F planes of L tokens with dim C (reference roformer.py:114-132).
-// kAttnF: sequences run over the F planes of each chunk (PartialFTTransformer attnF).
+// kAttnFreq: sequences run over the F planes of each chunk (PartialFTTransformer attnF).
 int attention_block(bt_ctx* c, float* X, const Layer& l, LayerPlans& tp, int nb, int L, bool out_in_ff,
                     const ChunkSrc* vl_chunks, cudaStream_t st) {
   const Workspace& ws = c->ws;
   const bool tc = c->dtype == BT_DTYPE_H16;
-  const bool freq = l.kind == kAttnF, front = l.F > 1;
+  const bool freq = l.kind == kAttnFreq, front = l.F > 1;
   const int C = l.C, F = l.F, heads = C / kHeadDim, planes = nb * F;
   const Param *wqkv = l.w[0], *wg = l.w[1], *bg = l.w[2], *wout = l.w[3];
   const int64_t M = static_cast<int64_t>(planes) * L;
@@ -431,13 +459,13 @@ int run_wave(bt_ctx* c, const float* spect, const Wave& wv, float* beat, float* 
   const ChunkSrc* vl = wv.varlen ? wv.chunks_dev : nullptr;
   // the fp32 residual stream: the stem writes X0, and every convolution but the last writes Xalt, which then carries it
   float *X = ws.X0.get(), *Xalt = ws.X1.get();
-  launch_stem(spect, wv.chunks_dev, nb, L, c->bn1_scale->f32.get(), c->bn1_shift->f32.get(), c->stem_w->f32.get(),
-              c->stem_b->f32.get(), X, st);
-  BT_LAUNCHED(c, "stem", st);
-  if ((r = do_tap(c, "stem", X, static_cast<int64_t>(nb) * (c->hp.spect_dim / 4) * L * c->hp.stem_dim, false, st)) != BT_OK)
-    return r;
   const std::vector<Layer>& layers = c->layers;
-  for (size_t i = 0; i < layers.size(); ++i) {
+  const Layer &stem = layers.front(), &head = layers.back();
+  launch_stem(spect, wv.chunks_dev, nb, L, stem.w[0]->f32.get(), stem.w[1]->f32.get(), stem.w[2]->f32.get(),
+              stem.w[3]->f32.get(), X, st);
+  BT_LAUNCHED(c, "stem", st);
+  if ((r = do_tap(c, "stem", X, static_cast<int64_t>(nb) * stem.F * L * stem.C, false, st)) != BT_OK) return r;
+  for (size_t i = 1; i + 1 < layers.size(); ++i) {
     const Layer& l = layers[i];
     LayerPlans& tp = plans[i];
     const char* tap = l.name.c_str();
@@ -445,13 +473,13 @@ int run_wave(bt_ctx* c, const float* spect, const Wave& wv, float* beat, float* 
     bool out_act = false;
     int64_t elems = static_cast<int64_t>(nb) * l.F * L * l.C;
     if (is_attention(l)) {
-      r = attention_block(c, X, l, tp, nb, L, outproj_in_ff(c, i), l.kind == kAttnF ? nullptr : vl, st);
-    } else if (l.kind == kFf) {
+      r = attention_block(c, X, l, tp, nb, L, outproj_in_ff(c, i), l.kind == kAttnFreq ? nullptr : vl, st);
+    } else if (l.kind == kFfn) {
       // the FFN in front of a convolution also writes the 16-bit copy the convolution reads (16-bit path)
-      void* copy_act = tc && i + 1 < layers.size() && layers[i + 1].kind == kConv ? ws.XB.get() : nullptr;
-      r = ff_block(c, X, l, tp, nb, L, i > 0 && outproj_in_ff(c, i - 1) ? layers[i - 1].w[3] : nullptr, copy_act, st);
+      void* copy_act = tc && layers[i + 1].kind == kConv ? ws.XB.get() : nullptr;
+      r = ff_block(c, X, l, tp, nb, L, outproj_in_ff(c, i - 1) ? layers[i - 1].w[3] : nullptr, copy_act, st);
     } else if (l.kind == kConv) {
-      if (tc && (i == 0 || layers[i - 1].kind != kFf)) {  // no FFN in front (no partial transformers)
+      if (tc && layers[i - 1].kind != kFfn) {  // no FFN in front (no partial transformers)
         launch_f32_to_h16(X, ws.XB.get(), elems, st);
         BT_LAUNCHED(c, "f32_to_h16", st);
       }
@@ -460,7 +488,7 @@ int run_wave(bt_ctx* c, const float* spect, const Wave& wv, float* beat, float* 
         BT_LAUNCHED(c, "zero_tail", st);
       }
       // conv C -> 2C (+ folded BN2d + GELU); the last one feeds frontend.linear in the activation dtype (XN) instead
-      const bool last = i + 1 < layers.size() && layers[i + 1].kind == kLin;
+      const bool last = layers[i + 1].kind == kLinear;
       void* act_out = last ? ws.XN.get() : nullptr;
       EpiParams e = epi_generic(l.w[1], 1, nullptr, 0, last ? nullptr : Xalt, 2 * l.C, act_out, 2 * l.C);
       r = run_gemm(c, l, nb, tp.gemm, tc ? ws.XB.get() : static_cast<const void*>(X), l.w[0],
@@ -472,7 +500,7 @@ int run_wave(bt_ctx* c, const float* spect, const Wave& wv, float* beat, float* 
         out = Xalt;
         std::swap(X, Xalt);
       }
-    } else {  // kLin
+    } else {  // kLinear
       const int D = c->hp.transformer_dim;
       EpiParams e = epi_generic(l.w[1], 0, nullptr, 0, X, D, nullptr, 0);
       r = run_gemm(c, l, nb, tp.gemm, ws.XN.get(), l.w[0], lin_shape(nb, L, D, l.F, l.C), e, "gemm_frontend_linear",
@@ -482,7 +510,7 @@ int run_wave(bt_ctx* c, const float* spect, const Wave& wv, float* beat, float* 
     }
     if (r != BT_OK || (r = do_tap(c, tap, out, elems, out_act, st)) != BT_OK) return r;
   }
-  launch_head(X, c->hp.transformer_dim, c->head_w->f32.get(), c->head_b->f32.get(), wv.chunks_dev, nb, L, beat, down,
+  launch_head(X, head.C, head.w[0]->f32.get(), head.w[1]->f32.get(), wv.chunks_dev, nb, L, beat, down,
               c->hp.sum_head ? 1 : 0, st);
   BT_LAUNCHED(c, "head", st);
   return BT_OK;
@@ -514,37 +542,19 @@ int run_chunks(bt_ctx* c, const float* spect_dev, std::vector<ChunkSrc>& all, fl
   return BT_OK;
 }
 
-std::vector<Layer> layer_list(const bt_hparams& hp) {
-  std::vector<Layer> v;
-  int C = hp.stem_dim, F = hp.spect_dim / 4;
-  for (int i = 0; i < 3; ++i) {
-    const std::string b = "b" + std::to_string(i);
-    if (hp.partial_transformers) {
-      v.push_back({kAttnF, b + ".attnF", C, F, 0, {}});
-      v.push_back({kFf, b + ".ffF", C, F, 4, {}});
-      v.push_back({kAttnT, b + ".attnT", C, F, 0, {}});
-      v.push_back({kFf, b + ".ffT", C, F, 4, {}});
-    }
-    v.push_back({kConv, b + ".conv", C, F, 0, {}});
-    C *= 2; F /= 2;
-  }
-  v.push_back({kLin, "lin", C, F, 0, {}});
-  for (int l = 0; l < hp.n_layers; ++l) {
-    v.push_back({kAttn, "l" + std::to_string(l) + ".attn", hp.transformer_dim, 1, 0, {}});
-    v.push_back({kFf, "l" + std::to_string(l) + ".ff", hp.transformer_dim, 1, hp.ff_mult, {}});
-  }
-  return v;
-}
-
 // the parameters of a layer in the order of Layer::w: name suffix, element count, and whether a GEMM reads it as
 // a 16-bit operand
 struct ParamSpec { const char* suffix; int64_t count; bool gemm; };
-std::vector<ParamSpec> layer_params(const Layer& l, int64_t D) {
-  const int64_t C = l.C, m = l.mult;
+std::vector<ParamSpec> layer_params(const Layer& l, const bt_hparams& hp) {
+  const int64_t C = l.C, m = l.mult, D = hp.transformer_dim;
   switch (l.kind) {
-    case kFf: return {{".w1", m * C * C, true}, {".b1", m * C, false}, {".w2", m * C * C, true}, {".b2", C, false}};
+    case kStem:
+      return {{".bn1_scale", hp.spect_dim, false}, {".bn1_shift", hp.spect_dim, false}, {".w", C * 12, false},
+              {".bias", C, false}};
+    case kFfn: return {{".w1", m * C * C, true}, {".b1", m * C, false}, {".w2", m * C * C, true}, {".b2", C, false}};
     case kConv: return {{".w", 2 * C * 6 * C, true}, {".bias", 2 * C, false}};
-    case kLin: return {{".w", D * C * l.F, true}, {".b", D, false}};
+    case kLinear: return {{".w", D * C * l.F, true}, {".b", D, false}};
+    case kHead: return {{".w", 2 * C, false}, {".b", 2, false}};
     default: return {{".wqkv", 3 * C * C, true}, {".wg", 32 * C, true}, {".bg", 32, false}, {".wout", C * C, true}};
   }
 }
@@ -649,20 +659,17 @@ int bt_finalize(bt_ctx* c) {
   if (!c) return BT_ERR_ARG;
   if (c->finalized) return BT_OK;
   BT_CUDA(c, cudaSetDevice(c->device));
-  const int64_t D = c->hp.transformer_dim;
   // every parameter the forward pass reads, with its element count (-1: not checked), resolved once here (no name
   // lookups per launch)
   struct Need { std::string name; int64_t count; const Param** dst; bool gemm; };
   std::vector<Need> need = {
       {"mel.window", 1024, nullptr, false}, {"mel.twiddle", 1024, nullptr, false}, {"mel.fb_start", 128, nullptr, false},
       {"mel.fb_ptr", 129, nullptr, false}, {"mel.fb_w", -1, nullptr, false},
-      {"rope.cos", -1, &c->rope_cos, false}, {"rope.sin", -1, &c->rope_sin, false},  // checked below
-      {"stem.bn1_scale", -1, &c->bn1_scale, false}, {"stem.bn1_shift", -1, &c->bn1_shift, false},
-      {"stem.w", 32 * 12, &c->stem_w, false}, {"stem.bias", -1, &c->stem_b, false},
-      {"head.w", 2 * D, &c->head_w, false}, {"head.b", 2, &c->head_b, false}};
-  c->layers = layer_list(c->hp);
+      {"rope.cos", -1, &c->rope_cos, false}, {"rope.sin", -1, &c->rope_sin, false}};  // checked below
+  c->layers.clear();
+  for (const Step& s : model_steps(c->hp)) c->layers.push_back({s});
   for (Layer& l : c->layers) {
-    const std::vector<ParamSpec> specs = layer_params(l, D);
+    const std::vector<ParamSpec> specs = layer_params(l, c->hp);
     for (size_t k = 0; k < specs.size(); ++k) need.push_back({l.name + specs[k].suffix, specs[k].count, &l.w[k], specs[k].gemm});
   }
   for (const Need& n : need)
