@@ -17,7 +17,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 # BT_LIB_PATH: an instrumented build of the same sources (e.g. build(extra_flags=("-DBT_FF_PROF",), out_path=...))
 LIB_PATH = os.environ.get("BT_LIB_PATH") or os.path.join(HERE, "libbeatthis_sm90.so")
-SOURCES = ["bt_api.cu", "api_signal.cu", "api_post.cu", "api_data.cu", "api_train.cu", "api_debug.cu", "kernels_simt.cu", "kernels_misc.cu", "kernels_signal.cu", "kernels_gemm.cu", "kernels_attn.cu", "kernels_fused.cu", "kernels_dbn.cu", "kernels_eval.cu", "kernels_loss.cu", "kernels_data.cu", "kernels_train.cu", "dbn_host.cpp", "host_stage.cpp"]
+SOURCES = ["bt_api.cu", "api_signal.cu", "api_post.cu", "api_data.cu", "api_train.cu", "api_debug.cu", "kernels_simt.cu", "kernels_misc.cu", "kernels_signal.cu", "kernels_gemm.cu", "kernels_attn.cu", "kernels_fused.cu", "kernels_dbn.cu", "kernels_eval.cu", "kernels_loss.cu", "kernels_data.cu", "kernels_train.cu", "kernels_optim.cu", "dbn_host.cpp", "host_stage.cpp"]
 HEADERS = ["common.cuh", "epilogue.cuh", "fft.cuh", "tc_common.cuh", "bt_kernels.h", "bt_train.h", "cuda_owned.h", "dbn_model.h",
            "api_internal.h", os.path.join("..", "..", "include", "beatthis.h")]
 
@@ -120,6 +120,22 @@ class bt_train_mode(ctypes.Structure):
         ("seed", ctypes.c_uint64),
         ("dropout_frontend", c_float),
         ("dropout_transformer", c_float),
+    ]
+
+
+class bt_adamw_entry(ctypes.Structure):
+    _fields_ = [
+        ("param", c_void_p),
+        ("grad", c_void_p),
+        ("exp_avg", c_void_p),
+        ("exp_avg_sq", c_void_p),
+        ("numel", c_int64),
+        ("lr", c_double),
+        ("beta1", c_double),
+        ("beta2", c_double),
+        ("eps", c_double),
+        ("weight_decay", c_double),
+        ("step", c_int64),
     ]
 
 
@@ -306,6 +322,7 @@ PROTOTYPES = {
         c_int, [c_void_p, POINTER(c_void_p), c_int32, c_void_p, c_int64, c_int32, c_int32, POINTER(bt_train_mode),
                 c_void_p, c_void_p, POINTER(c_void_p), c_void_p, c_void_p],
     ),
+    "bt_adamw_step": (c_int, [c_void_p, POINTER(bt_adamw_entry), c_int32, c_void_p]),
     "bt_debug_attention_backward": (
         c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p,
                 c_void_p],

@@ -2,6 +2,7 @@
 // bt_train_activation_bytes(_ex), bt_train_forward(_ex) and bt_train_backward(_ex).  Parameters are the caller's
 // unfolded fp32 device tensors; the forward pass saves what the backward pass reads in the caller's activation store.
 // A bt_train_mode selects the reference's training-mode function: dropout and batch-statistics BatchNorm.
+// bt_adamw_step: the AdamW update of a parameter table in one launch (csrc/kernels_optim.cu).
 #include "api_internal.h"
 #include "bt_train.h"
 #include "common.cuh"
@@ -582,6 +583,45 @@ int bt_train_backward(bt_ctx* c, const float* const* params, int32_t n_params, c
                       float* dspect_dev, void* stream) {
   return bt_train_backward_ex(c, params, n_params, act_dev, act_bytes, B, L, nullptr, dbeat_dev, ddown_dev, grads,
                               dspect_dev, stream);
+}
+
+int bt_adamw_step(bt_ctx* c, const bt_adamw_entry* entries, int32_t n, void* stream) {
+  if (!c) return BT_ERR_ARG;
+  const char* fn = "bt_adamw_step";
+  if (n < 0 || (n > 0 && !entries)) return fail(c, BT_ERR_ARG, "%s: need n >= 0 entries, got %d", fn, n);
+  std::vector<AdamwEntry> dev;
+  int64_t chunks = 0;
+  for (int32_t i = 0; i < n; ++i) {
+    const bt_adamw_entry& e = entries[i];
+    if (!e.param || !e.exp_avg || !e.exp_avg_sq) return fail(c, BT_ERR_ARG, "%s: entry %d has a null pointer", fn, i);
+    if (e.numel < 0) return fail(c, BT_ERR_ARG, "%s: entry %d has numel %lld", fn, i, static_cast<long long>(e.numel));
+    for (const double h : {e.lr, e.beta1, e.beta2, e.eps, e.weight_decay})
+      if (!std::isfinite(h)) return fail(c, BT_ERR_ARG, "%s: entry %d has a non-finite hyperparameter", fn, i);
+    if (e.lr < 0 || e.eps < 0 || !(e.beta1 >= 0 && e.beta1 < 1) || !(e.beta2 >= 0 && e.beta2 < 1) || e.step < 1)
+      return fail(c, BT_ERR_ARG, "%s: entry %d needs lr >= 0, eps >= 0, betas in [0, 1) and step >= 1", fn, i);
+    if (!e.grad || e.numel == 0) continue;  // torch's rule: a parameter without a gradient is not updated
+    // the scalars as torch's foreach path derives them in Python (double), then rounded to fp32
+    const double t = static_cast<double>(e.step);
+    const double bc1 = 1.0 - std::pow(e.beta1, t), bc2 = 1.0 - std::pow(e.beta2, t);
+    const auto aligned = [](const void* q) { return reinterpret_cast<uintptr_t>(q) % 16 == 0; };
+    AdamwEntry d{e.param, e.grad, e.exp_avg, e.exp_avg_sq, e.numel, chunks,
+                 static_cast<float>(1.0 - e.lr * e.weight_decay), static_cast<float>(1.0 - e.beta1),
+                 static_cast<float>(e.beta2), static_cast<float>(1.0 - e.beta2), static_cast<float>(std::pow(bc2, 0.5)),
+                 static_cast<float>(e.eps), static_cast<float>(e.lr / bc1 * -1.0), e.weight_decay != 0.0,
+                 aligned(e.param) && aligned(e.grad) && aligned(e.exp_avg) && aligned(e.exp_avg_sq)};
+    chunks += adamw_chunks(e.numel);
+    dev.push_back(d);
+  }
+  if (chunks > 0x7fffffff) return fail(c, BT_ERR_ARG, "%s: %lld blocks exceed the grid", fn, static_cast<long long>(chunks));
+  if (dev.empty()) return BT_OK;
+  cudaStream_t st;
+  int r;
+  if ((r = enter(c, fn, stream, &st)) != BT_OK) return r;
+  const AdamwEntry* table = nullptr;
+  if ((r = stage(c, st, {{dev.data(), dev.size()}}, &table)) != BT_OK) return r;
+  launch_adamw(table, static_cast<int>(dev.size()), chunks, st);
+  BT_LAUNCHED(c, "adamw", st);
+  return BT_OK;
 }
 
 }  // extern "C"

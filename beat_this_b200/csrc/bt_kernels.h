@@ -210,6 +210,23 @@ void launch_train_batch(const uint16_t* rows, const int64_t* row_off, int n_item
                         uint16_t* spect, uint8_t* truth_beat, uint8_t* truth_downbeat, uint8_t* padding_mask,
                         cudaStream_t st);
 
+// ---- optimizer (kernels_optim.cu) -------------------------------------------------------------------------------------
+// One entry of bt_adamw_step's device table: n > 0 elements from p, g, m, v; chunk0, its first chunk of the launch
+// (prefix sums of adamw_chunks over the entries before it); vec: all four pointers 16-byte aligned.  The scalars are
+// the fp32 values of what the host derived in double: decay = 1 - lr wd (applied when decay_on), w1 = 1 - beta1,
+// beta2, w2 = 1 - beta2, bc2_sqrt = (1 - beta2^t)^0.5, eps and step_size = -lr / (1 - beta1^t).
+struct AdamwEntry {
+  float* p;
+  const float* g;
+  float* m;
+  float* v;
+  int64_t n, chunk0;
+  float decay, w1, beta2, w2, bc2_sqrt, eps, step_size;
+  int32_t decay_on, vec;
+};
+int64_t adamw_chunks(int64_t n);  // blocks of one entry of n elements
+void launch_adamw(const AdamwEntry* entries_dev, int n_entries, int64_t chunks, cudaStream_t st);
+
 void launch_f32_to_h16(const float* in, void* out, int64_t n, cudaStream_t st);
 void launch_h16_to_f32(const void* in, float* out, int64_t n, cudaStream_t st);
 // [seqs, L, heads*32] fp32 q,k,v -> packed qkv buffer [seqs*L, 3C] of the activation dtype

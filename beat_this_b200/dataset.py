@@ -85,6 +85,7 @@ def split_items(data_dir, datasplit, hparams=None) -> list:
     ``datamodule_hyper_parameters``; missing keys take BeatDataModule's defaults), as the reference's predict stage
     selects them (dataset.py:426-446)."""
     hp = dict(hparams or {})
+    hp.pop("data_dir", None)  # a Lightning checkpoint records the directory it was trained from; data_dir wins
     if datasplit == "test":
         return test_items(data_dir, **hp)
     if datasplit not in ("train", "val"):

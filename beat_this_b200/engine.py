@@ -497,6 +497,12 @@ class Engine:
                    act.numel(), int(B), int(L), self._train_mode(mode), p(dbeat, B * L), p(ddown, B * L),
                    self._table_ptrs(grads, "gradient"), p(dspect, B * L * 128))
 
+    def adamw_step(self, entries):
+        """One ``bt_adamw_step`` call on the current stream: entries is a sequence of _lib.bt_adamw_entry whose device
+        pointers the caller has checked and keeps alive until the update has run."""
+        n = len(entries)
+        self._call("bt_adamw_step", (_lib.bt_adamw_entry * max(n, 1))(*entries), n)
+
     # ---- per-kernel-class timing (bench.py roofline) -------------------------------------------
     def profile_enable(self, on: bool = True):
         self._call("bt_profile_enable", int(on), stream=False)

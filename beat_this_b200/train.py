@@ -1,5 +1,7 @@
 """The reference's ``BeatThis`` as a trainable module on the GPU: parameters named and shaped as its ``state_dict``,
-forward and backward through ``bt_train_forward_ex`` / ``bt_train_backward_ex`` (fp32 CUDA cores).
+forward and backward through ``bt_train_forward_ex`` / ``bt_train_backward_ex`` (fp32 CUDA cores); and ``fit`` /
+``python -m beat_this_b200.train``, the reference's training run (launch_scripts/train.py with PLBeatThis) without
+Lightning.
 
 By default the gradient is that of the eval-mode function the inference path computes: BatchNorm on its running
 statistics and no dropout, and ``.train(True)`` raises rather than train with other semantics than asked for.  A module
@@ -9,8 +11,14 @@ path.
 """
 from __future__ import annotations
 
+import argparse
+import json
 import math
+import os
+import random
+import sys
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -160,3 +168,305 @@ class BeatThisModule(torch.nn.Module):
             "hyper_parameters": dict(hparams if hparams is not None else self.checkpoint_hparams),
         }, path)
         return path
+
+
+# ---- the training run (reference launch_scripts/train.py, PLBeatThis) ---------------------------------------------
+# The loop follows Lightning's rules as the reference's Trainer applies them, in fp32 without a GradScaler (the
+# reference trains at precision="16-mixed"), so no step is ever skipped:
+# * every micro-batch runs backward() on (beat_loss + downbeat_loss) / accumulate_grad_batches;
+# * the optimizer steps after every accumulate-th micro-batch and after the last one of an epoch, then the scheduler
+#   steps and the gradients are set to None; global_step counts optimizer steps;
+# * estimated_stepping_batches = ceil(batches per epoch / accumulate) * max_epochs sets the schedule's length.
+# Lightning's one-batch sanity validation before training is left out: it changes no training state.
+
+def step_plan(n_batches: int, accumulate: int) -> list:
+    """Indices of the micro-batches of an epoch of `n_batches` after which the optimizer steps."""
+    return [i for i in range(n_batches) if (i + 1) % accumulate == 0 or i + 1 == n_batches]
+
+
+def estimated_stepping_batches(n_batches: int, accumulate: int, max_epochs: int) -> int:
+    return math.ceil(n_batches / accumulate) * max_epochs
+
+
+def augmentations(tempo: bool, pitch: bool, mask: bool) -> dict:
+    """The reference's augmentation settings for --tempo/pitch/mask-augmentation."""
+    aug = {}
+    if tempo:
+        aug["tempo"] = {"min": -20, "max": 20, "stride": 4}
+    if pitch:
+        aug["pitch"] = {"min": -5, "max": 6}
+    if mask:
+        aug["mask"] = {"kind": "permute", "min_count": 1, "max_count": 6, "min_len": 0.1, "max_len": 2,
+                       "min_parts": 5, "max_parts": 9}
+    return aug
+
+
+def params_str(val=True, hung_data=False, fold=None, loss="shift_tolerant_weighted_bce", transformer_dim=512,
+               tempo_augmentation=True, pitch_augmentation=True, mask_augmentation=True, sum_head=True,
+               partial_transformers=True, **_) -> str:
+    """The run description the reference puts into its checkpoint's file name."""
+    head = ("" if val else "noval ") + ("hung " if hung_data else "") + ("" if fold is None else f"fold{fold} ")
+    tail = ("" if sum_head else " nosumH ") + ("" if partial_transformers else " nopartialT ")
+    return (f"{head}{loss}-h{transformer_dim}-aug{tempo_augmentation}{pitch_augmentation}{mask_augmentation}"
+            f"{tail}")
+
+
+def checkpoint_path(checkpoint_dir, name="", seed=0, **run) -> str:
+    """<checkpoint_dir>/<name> S<seed> <params_str>.ckpt, the reference's ModelCheckpoint file name."""
+    return os.path.join(str(checkpoint_dir), f"{name} S{seed} {params_str(**run)}".strip() + ".ckpt")
+
+
+def _rng_state(batches) -> dict:
+    """The random states the next epoch draws from, in types torch.load(weights_only=True) reads."""
+    version, mt, gauss = random.getstate()
+    kind, keys, pos, has_gauss, cached = np.random.get_state()
+    return {"python": [version, list(mt), gauss], "numpy": [kind, torch.from_numpy(keys.astype(np.int64)), int(pos),
+                                                            int(has_gauss), float(cached)],
+            "torch": torch.get_rng_state(), "batches": batches.generator.get_state()}
+
+
+def _set_rng_state(state: dict, batches) -> None:
+    version, mt, gauss = state["python"]
+    random.setstate((version, tuple(mt), gauss))
+    kind, keys, pos, has_gauss, cached = state["numpy"]
+    np.random.set_state((kind, keys.numpy().astype(np.uint32), pos, has_gauss, cached))
+    torch.set_rng_state(state["torch"])
+    batches.generator.set_state(state["batches"])
+
+
+def _losses(loss_pair, out, batch):
+    """PLBeatThis._compute_loss: the beat loss under the padding mask, the downbeat loss under the padding mask times
+    each item's downbeat mask."""
+    beat_loss, downbeat_loss = loss_pair
+    mask = batch["padding_mask"]
+    down_mask = mask.float() * batch["downbeat_mask"].to(mask.device).float()[:, None]
+    lb = beat_loss(out["beat"], batch["truth_beat"].float(), mask)
+    ld = downbeat_loss(out["downbeat"], batch["truth_downbeat"].float(), down_mask)
+    return lb, ld
+
+
+def _validate(module, batches, loss_pair, post, eval_trim_beats) -> dict:
+    """validation_step over every batch: the loss pair (means over batches weighted by batch size), then the
+    post-processed beats under the padding mask scored against truth_orig_* (F-measure and Cemgil, means over
+    pieces)."""
+    from .evaluate import beat_metrics
+
+    module.eval()
+    sums, n = torch.zeros(2, dtype=torch.float64, device=module.engine.device), 0
+    est, ref = {"beat": [], "downbeat": []}, {"beat": [], "downbeat": []}
+    with torch.no_grad():
+        for batch in batches:
+            out = module(batch["spect"])
+            B = len(batch["spect"])
+            lb, ld = _losses(loss_pair, out, batch)
+            sums += torch.stack([lb, ld]).double() * B
+            n += B
+            beats, downs = post(out["beat"], out["downbeat"], batch["padding_mask"])
+            for target, times in (("beat", beats), ("downbeat", downs)):
+                est[target] += list(times)
+                ref[target] += [np.frombuffer(b, dtype=np.float64) for b in batch[f"truth_orig_{target}"]]
+    module.train()
+    lb, ld = (sums / max(n, 1)).tolist()
+    rec = {"val_loss_beat": lb, "val_loss_downbeat": ld, "val_loss": lb + ld}
+    for target in ("beat", "downbeat"):
+        rows = beat_metrics(est[target], ref[target], min_beat_time=eval_trim_beats, device=module.engine.device)
+        rec[f"val_F-measure_{target}"] = float(np.mean(rows[:, 5])) if len(rows) else float("nan")
+        rec[f"val_Cemgil_{target}"] = float(np.mean((rows[:, 6] + rows[:, 7]) / 2)) if len(rows) else float("nan")
+    return rec
+
+
+def fit(data="data", checkpoint_dir="checkpoints", *, name="", gpu=0, n_layers=6, transformer_dim=512,
+        frontend_dropout=0.1, transformer_dropout=0.2, lr=0.0008, weight_decay=0.01, fps=50,
+        loss="shift_tolerant_weighted_bce", warmup_steps=1000, max_epochs=100, batch_size=8,
+        accumulate_grad_batches=8, train_length=1500, dbn=False, eval_trim_beats=5, val_frequency=5,
+        tempo_augmentation=True, pitch_augmentation=True, mask_augmentation=True, sum_head=True,
+        partial_transformers=True, length_based_oversampling_factor=0.65, val=True, hung_data=False, fold=None,
+        seed=0, resume_checkpoint=None, test=True, epochs=None) -> list:
+    """Train a BeatThis model from scratch (or resume) as the reference's train.py does, on CUDA device `gpu`; the
+    keyword arguments are the reference's command-line flags.  Returns one record per epoch run (each also printed
+    as a JSON line): epoch, global_step, lr (after the epoch), step_lr (the rate of each optimizer step, as
+    LearningRateMonitor logs it), the train losses' means over micro-batches weighted by batch size and, after a
+    validation, the val losses, F-measure and Cemgil.  The checkpoint <checkpoint_dir>/<name> S<seed>
+    <params_str>.ckpt is written at the end of every epoch (through a temporary file, so an interrupted save leaves
+    the last one).  After the last epoch, unless `test` is off, the checkpoint is scored on the test split by
+    ``evaluate`` (the reference's trainer.test); its summary goes into the last record under "test".
+    epochs: run at most this many epochs in this call (None: up to max_epochs); the schedule still spans max_epochs,
+    and `resume_checkpoint` continues the run later."""
+    from . import dataset as D
+    from .loss import loss_from_hparams
+    from .optim import AdamW, CosineWarmupScheduler, param_groups
+    from .postprocessor import Postprocessor
+
+    device = torch.device("cuda", gpu)
+    torch.cuda.set_device(device)
+    random.seed(seed)  # seed_everything
+    np.random.seed(seed)
+    torch.manual_seed(seed)
+
+    run = dict(val=val, hung_data=hung_data, fold=fold, loss=loss, transformer_dim=transformer_dim,
+               tempo_augmentation=tempo_augmentation, pitch_augmentation=pitch_augmentation,
+               mask_augmentation=mask_augmentation, sum_head=sum_head, partial_transformers=partial_transformers)
+    aug = augmentations(tempo_augmentation, pitch_augmentation, mask_augmentation)
+    dm_hparams = dict(data_dir=str(data), batch_size=batch_size, train_length=train_length, num_workers=0,
+                      augmentations=aug, test_dataset="gtzan", hung_data=hung_data, no_val=not val, spect_fps=fps,
+                      length_based_oversampling_factor=length_based_oversampling_factor, fold=fold,
+                      predict_datasplit="test")
+    train_items, val_items = D.train_val_items(data, "gtzan", fold, hung_data, not val)
+    train_set = D.BeatTrackingDataset(train_items, data, fps, train_length, deterministic=False, augmentations=aug,
+                                      length_based_oversampling_factor=length_based_oversampling_factor)
+    val_set = D.BeatTrackingDataset(val_items, data, fps, train_length, deterministic=True, augmentations={})
+    train_batches = D.TrainingBatches(train_set, batch_size, shuffle=True, drop_last=True, device=device)
+    val_batches = D.TrainingBatches(val_set, batch_size, shuffle=False, drop_last=False, seed=0, device=device)
+    if len(train_batches) == 0:
+        raise ValueError(f"{len(train_set)} training items make no batch of {batch_size}")
+    pos_weights = train_set.positive_weights(widen_target_mask=3)
+    print("Using positive weights: ", pos_weights)
+
+    hparams = dict(spect_dim=128, fps=50, transformer_dim=transformer_dim, ff_mult=4, n_layers=n_layers, stem_dim=32,
+                   dropout={"frontend": frontend_dropout, "transformer": transformer_dropout}, lr=lr,
+                   weight_decay=weight_decay, pos_weights=pos_weights, head_dim=32, loss_type=loss,
+                   warmup_steps=warmup_steps, max_epochs=max_epochs, use_dbn=dbn, eval_trim_beats=eval_trim_beats,
+                   sum_head=sum_head, partial_transformers=partial_transformers)
+    if loss == "fast_shift_tolerant_weighted_bce":
+        raise ValueError("loss_type must be one of 'shift_tolerant_weighted_bce', 'weighted_bce', 'bce'")
+    loss_pair = loss_from_hparams(hparams)
+    module = BeatThisModule(hparams, device, train_mode=True).reset_parameters()
+    opt = AdamW(param_groups(module, weight_decay), lr=lr)
+    total_steps = estimated_stepping_batches(len(train_batches), accumulate_grad_batches, max_epochs)
+    sched = CosineWarmupScheduler(opt, warmup_steps, total_steps)
+    post = Postprocessor("dbn" if dbn else "minimal", 50, engine=module.engine)
+
+    first_epoch, global_step = 0, 0
+    if resume_checkpoint is not None:
+        # a checkpoint the user names: a Lightning one holds numpy scalars, so it is unpickled in full
+        ckpt = torch.load(resume_checkpoint, map_location="cpu", weights_only=False)
+        module.load_state_dict(strip_prefixes(ckpt["state_dict"]))
+        opt.load_state_dict(ckpt["optimizer_states"][0])
+        sched.load_state_dict(ckpt["lr_schedulers"][0])
+        first_epoch, global_step = int(ckpt["epoch"]) + 1, int(ckpt["global_step"])
+        if "beat_this_b200" in ckpt:
+            _set_rng_state(ckpt["beat_this_b200"], train_batches)
+        else:
+            print(f"{resume_checkpoint} holds no random states: the data order and dropout masks of the resumed "
+                  f"epochs differ from those of an uninterrupted run")
+
+    path = checkpoint_path(checkpoint_dir, name, seed, **run)
+    os.makedirs(str(checkpoint_dir), exist_ok=True)
+    last_epoch = max_epochs if epochs is None else min(max_epochs, first_epoch + epochs)
+    plan = set(step_plan(len(train_batches), accumulate_grad_batches))
+    records = []
+    module.train()
+    for epoch in range(first_epoch, last_epoch):
+        sums, n, step_lr = torch.zeros(2, dtype=torch.float64, device=device), 0, []
+        for i, batch in enumerate(train_batches):
+            out = module(batch["spect"])
+            lb, ld = _losses(loss_pair, out, batch)
+            ((lb + ld) / accumulate_grad_batches).backward()
+            B = len(batch["spect"])
+            sums += torch.stack([lb.detach(), ld.detach()]).double() * B
+            n += B
+            if i in plan:
+                step_lr.append(opt.param_groups[0]["lr"])
+                opt.step()
+                sched.step()
+                opt.zero_grad(set_to_none=True)
+                global_step += 1
+        lb, ld = (sums / n).tolist()
+        rec = {"epoch": epoch, "global_step": global_step, "lr": opt.param_groups[0]["lr"], "step_lr": step_lr,
+               "train_loss_beat": lb, "train_loss_downbeat": ld, "train_loss": lb + ld}
+        if (epoch + 1) % val_frequency == 0:
+            rec.update(_validate(module, val_batches, loss_pair, post, eval_trim_beats))
+        ckpt = {"epoch": epoch, "global_step": global_step,
+                "state_dict": {"model." + k: v.detach().cpu() for k, v in module.state_dict().items()},
+                "hyper_parameters": hparams, "datamodule_hyper_parameters": dm_hparams,
+                "optimizer_states": [opt.state_dict()], "lr_schedulers": [sched.state_dict()],
+                "beat_this_b200": _rng_state(train_batches)}
+        torch.save(ckpt, path + ".tmp")
+        os.replace(path + ".tmp", path)
+        print(json.dumps(rec), flush=True)
+        records.append(rec)
+    if test and last_epoch == max_epochs and first_epoch < max_epochs:
+        from .evaluate import evaluate
+
+        result = evaluate(path, data=data, datasplit="test", min_beat_time=eval_trim_beats, device=device, dbn=dbn,
+                          losses=True)
+        records[-1]["test"] = result.summary
+        print(json.dumps({"test": result.summary}), flush=True)
+    return records
+
+
+def build_parser() -> argparse.ArgumentParser:
+    """The reference's train.py flags, names and defaults; --data and --checkpoint-dir stand for its fixed paths."""
+    ap = argparse.ArgumentParser(prog="python -m beat_this_b200.train",
+                                 description="Train a BeatThis model on a prepared dataset on one GPU.")
+    add = ap.add_argument
+    flag = argparse.BooleanOptionalAction
+    add("--data", default="data", help="prepared dataset directory (annotations/ and audio/spectrograms/) [%(default)s]")
+    add("--checkpoint-dir", default="checkpoints", help="where the checkpoint goes [%(default)s]")
+    add("--name", type=str, default="")
+    add("--gpu", type=int, default=0)
+    add("--force-flash-attention", default=False, action=flag, help="accepted, no effect")
+    add("--compile", action="store", nargs="*", type=str, default=["frontend", "transformer_blocks", "task_heads"],
+        help="accepted, no effect")
+    add("--n-layers", type=int, default=6)
+    add("--transformer-dim", type=int, default=512)
+    add("--frontend-dropout", type=float, default=0.1, help="dropout rate to apply in the frontend")
+    add("--transformer-dropout", type=float, default=0.2, help="dropout rate to apply in the main transformer blocks")
+    add("--lr", type=float, default=0.0008)
+    add("--weight-decay", type=float, default=0.01)
+    add("--logger", type=str, choices=["wandb", "none"], default="none", help="only none: there is no wandb")
+    add("--num-workers", type=int, default=8, help="accepted, no effect")
+    add("--n-heads", type=int, default=16, help="accepted, no effect (the reference does not use it either)")
+    add("--fps", type=int, default=50, help="The spectrograms fps.")
+    add("--loss", type=str, default="shift_tolerant_weighted_bce",
+        choices=["shift_tolerant_weighted_bce", "fast_shift_tolerant_weighted_bce", "weighted_bce", "bce"])
+    add("--warmup-steps", type=int, default=1000, help="warmup steps for optimizer")
+    add("--max-epochs", type=int, default=100, help="max epochs for training")
+    add("--batch-size", type=int, default=8, help="batch size for training")
+    add("--accumulate-grad-batches", type=int, default=8)
+    add("--train-length", type=int, default=1500, help="maximum seq length for training in frames")
+    add("--dbn", default=False, action=flag, help="use the DBN post-processor in validation")
+    add("--eval-trim-beats", metavar="SECONDS", type=float, default=5,
+        help="Skip the first given seconds per piece in evaluating (default: %(default)s)")
+    add("--val-frequency", metavar="N", type=int, default=5, help="validate every N epochs (default: %(default)s)")
+    add("--tempo-augmentation", default=True, action=flag, help="Use precomputed tempo augmentation")
+    add("--pitch-augmentation", default=True, action=flag, help="Use precomputed pitch augmentation")
+    add("--mask-augmentation", default=True, action=flag, help="Use online mask augmentation")
+    add("--sum-head", default=True, action=flag, help="Use SumHead instead of two separate Linear heads")
+    add("--partial-transformers", default=True, action=flag, help="Use Partial transformers in the frontend")
+    add("--length-based-oversampling-factor", type=float, default=0.65,
+        help="The factor to oversample the long pieces in the dataset. Set to 0 to only take one excerpt for each "
+             "piece.")
+    add("--val", default=True, action=flag, help="Train on all data, including validation data, excluding test data "
+                                                 "(--no-val); the validation metrics are still computed.")
+    add("--hung-data", default=False, action=flag, help="Limit the training to Hung et al. data.")
+    add("--fold", type=int, default=None, help="If given, the CV fold number to *not* train on (0-based).")
+    add("--seed", type=int, default=0, help="Seed for the random number generators.")
+    add("--resume-checkpoint", type=str, default=None, help="Resume training from a local checkpoint.")
+    add("--resume-id", type=str, default=None, help="refused: a wandb run id, and there is no wandb")
+    add("--test", default=True, action=flag, help="score the final checkpoint on the test split (--no-test: skip)")
+    return ap
+
+
+def parse_args(argv=None) -> dict:
+    """fit's keyword arguments from a command line; --logger wandb and --resume-id are refused."""
+    ap = build_parser()
+    args = ap.parse_args(argv)
+    if args.logger == "wandb" or args.resume_id is not None:
+        ap.error("--logger wandb and --resume-id need wandb, which this command does not use")
+    kw = vars(args)
+    for k in ("force_flash_attention", "compile", "logger", "num_workers", "n_heads", "resume_id"):
+        del kw[k]
+    return kw
+
+
+def main(argv=None) -> int:
+    kw = parse_args(argv)
+    print("Starting a new run with the following parameters:")
+    print(kw)
+    fit(**kw)
+    return 0
+
+
+if __name__ == "__main__":
+    sys.exit(main())

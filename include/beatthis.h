@@ -590,6 +590,35 @@ int bt_train_backward_ex(bt_ctx* ctx, const float* const* params, int32_t n_para
                          int64_t act_bytes, int32_t B, int32_t L, const bt_train_mode* mode, const float* dbeat_dev,
                          const float* ddown_dev, float* const* grads, float* dspect_dev, void* stream);
 
+/* ---- optimizer (ABI 2.15): AdamW over a parameter table -------------------------------------------------------------
+ * bt_adamw_step updates every entry of `entries_host` (n entries, a host array) in one kernel launch, as
+ * torch.optim.AdamW(amsgrad=False, maximize=False) does one step: per element of an entry with t = step,
+ *   p <- p (1 - lr wd)                                  (only if wd != 0)
+ *   m <- m + (1 - beta1)(g - m)                          (torch's lerp: g - (g - m) beta1 when 1 - beta1 >= 0.5)
+ *   v <- beta2 v + (1 - beta2) g g
+ *   p <- p - (lr / (1 - beta1^t)) m / (sqrt(v) / sqrt(1 - beta2^t) + eps)
+ * op by op in the order of torch's foreach path, each op rounded to fp32 (multiply-adds may be fused).  The scalars
+ * 1 - lr wd, 1 - beta1, beta2, 1 - beta2, (1 - beta2^t)^0.5, eps and -lr / (1 - beta1^t) are derived on the host in
+ * double, as torch derives them in Python, and rounded to fp32.  `step` is t, the entry's step count after this
+ * update (torch increments its state step first).  param, grad, exp_avg and exp_avg_sq are fp32 device arrays of numel
+ * elements; grad is read, the other three are updated in place.  An entry whose grad is NULL, or with numel 0, is left
+ * untouched (torch skips a parameter without a gradient); when no entry is left, nothing is launched.  Each element
+ * is read and written by one thread, without atomics: two calls on the same inputs write the same bytes.
+ * BT_ERR_ARG before anything is enqueued: n < 0 (or entries_host NULL with n > 0), a NULL param, exp_avg or exp_avg_sq,
+ * numel < 0, a non-finite hyperparameter, lr < 0, eps < 0, a beta outside [0, 1) or step < 1.  The table goes to the
+ * device through the ctx's staging ring; the launch is counted and profiled as "adamw".  Any ctx will do (a
+ * weight-less one too); enqueued on `stream` without synchronisation. */
+typedef struct bt_adamw_entry {
+  float* param;
+  const float* grad;
+  float* exp_avg;
+  float* exp_avg_sq;
+  int64_t numel;
+  double lr, beta1, beta2, eps, weight_decay;
+  int64_t step;
+} bt_adamw_entry;
+int bt_adamw_step(bt_ctx* ctx, const bt_adamw_entry* entries_host, int32_t n, void* stream);
+
 /* Test hook (fp32 ctx only; BT_ERR_ARG for a 16-bit one): the attention core of one bt_train_forward /
  * bt_train_backward layer alone, on `seqs` time-direction sequences of n positions and `heads` heads of 32.  qkv_dev
  * [seqs * n, 3 * heads * 32] holds q | k | v before RoPE, gates_dev [seqs * n, heads] the gate logits, freqs_dev [16]
