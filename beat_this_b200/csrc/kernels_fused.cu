@@ -3,11 +3,12 @@
 // roformer.py:38-61,114-128 as called by PartialFTTransformer, beat_tracker.py:290-301.
 //
 // Every weight matrix of the block is staged once per CTA into shared memory (rows padded by 16 bytes, so that the
-// B-fragment reads of a warp hit 32 different banks).  A warp then owns 16 token rows at a time and does the whole
-// block in registers with mma.sync m16n8k16 (16-bit operands, fp32 accumulate): each thread loads the fp32 values of
-// its two rows in the order of the MMA fragments, so the row it normalises is also the A operand, and for C <= 64 the
-// accumulator of an N = C product holds exactly the columns the thread loaded.  Unfused, the FFN streams 32 bytes per
-// element through HBM (norm 6 + ff1 10 + ff2 16); fused it is 8 (+2 for the out-projection input, +2 for the 16-bit copy).
+// eight row addresses of each ldmatrix hit different bank groups).  A warp then owns 16 token rows at a time and does
+// the whole block in registers with mma.sync m16n8k16 (16-bit operands, fp32 accumulate): each thread reads the fp32
+// values of its two rows in the order of the MMA fragments, so the row it normalises is also the A operand, and for
+// C <= 64 the accumulator of an N = C product holds exactly the columns the thread read.  The rows come from a
+// per-warp stage in shared memory that cp.async fills with the warp's next 16 rows while it computes the current ones.
+// Unfused, the FFN streams 32 bytes per element through HBM (norm 6 + ff1 10 + ff2 16); fused it is 8 (+2 for the out-projection input, +2 for the 16-bit copy).
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -27,13 +28,61 @@ __device__ __forceinline__ void stage_weight(h16* dst, const h16* __restrict__ s
     *reinterpret_cast<uint4*>(dst + r * (cols + 8) + v * 8) = __ldg(reinterpret_cast<const uint4*>(src + static_cast<int64_t>(r) * cols) + v);
   }
 }
-__device__ __forceinline__ uint32_t lds32(const h16* p) { return *reinterpret_cast<const uint32_t*>(p); }
-// B fragment of out = A W^T for output columns [8 nb, 8 nb + 8) and K [16 ks, 16 ks + 16): W staged with row stride LD
+// B fragments of out = A W^T, W staged at shared address sW with row stride LD elements.  b_frag_k2: output columns
+// [8 nb, 8 nb + 8) at the k-steps ks (b[0], b[1]) and ks + 1 (b[2], b[3]); b_frag_n2: the column blocks nb (b[0], b[1])
+// and nb + 1 (b[2], b[3]) at the k-step ks.  Lanes 8 i .. 8 i + 7 address the rows of 8 x 8 matrix i.
 template <int LD>
-__device__ __forceinline__ void b_frag(const h16* sW, int nb, int ks, int lane, uint32_t& b0, uint32_t& b1) {
-  const h16* p = sW + (nb * 8 + (lane >> 2)) * LD + ks * 16 + 2 * (lane & 3);
-  b0 = lds32(p);
-  b1 = lds32(p + 8);
+__device__ __forceinline__ void b_frag_k2(uint32_t sW, int nb, int ks, int lane, uint32_t (&b)[4]) {
+  ldmatrix_x4(sW + 2 * ((nb * 8 + (lane & 7)) * LD + ks * 16 + 8 * (lane >> 3)), b);
+}
+template <int LD>
+__device__ __forceinline__ void b_frag_n2(uint32_t sW, int nb, int ks, int lane, uint32_t (&b)[4]) {
+  ldmatrix_x4(sW + 2 * ((nb * 8 + (lane & 7) + 8 * (lane >> 4)) * LD + ks * 16 + 8 * ((lane >> 3) & 1)), b);
+}
+
+// Two 16-bit pairs of one row, lo at columns 8 nb + 2 q (+1) and hi at 8 (nb + 1) + 2 q (+1), spread over the lanes
+// q = 0..3 of a quad: after one exchange with lane q ^ 1, lane q holds the 4 consecutive columns from
+// 8 nb + quad_col(q), so the quad writes the row's 32 bytes of both blocks as one whole 32-byte sector, 8 bytes per
+// lane.  Stored block by block, each warp store covered half of every sector it touched, and the QKV kernels ran at
+// under half the HBM rate of the FFN kernels, whose fp32 stores cover whole sectors.
+__device__ __forceinline__ int quad_col(int q) { return 8 * (q & 1) + 2 * (q & 2); }
+__device__ __forceinline__ uint2 quad_pair(uint32_t lo, uint32_t hi, int q) {
+  const uint32_t other = __shfl_xor_sync(0xffffffffu, (q & 1) ? lo : hi, 1);
+  return (q & 1) ? make_uint2(other, hi) : make_uint2(lo, other);
+}
+
+// ---------------------------------------------------------------- per-warp row stage
+// The 16 fp32 rows [16 g, 16 g + 16) of X [M][C], 8 floats of padding after every row but each fourth: the 4 rows of
+// a half warp's float2 fragment read (8 consecutive floats each) start 8 banks apart, so the read hits 32 different
+// banks.  Every index is the lane's own offset plus a constant, and the stage is 384 bytes smaller than with 8 floats
+// after every row, which is what lets two CTAs of fused_ff_kernel<64, true> fit on an SM.
+template <int C> __host__ __device__ constexpr int stage_floats() { return 16 * C + 96; }
+template <int C>
+__device__ __forceinline__ int stage_idx(int r, int col) { return r * C + 8 * (r & 3) + 24 * (r >> 2) + col; }
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, bool ok) {  // !ok: 16 zero bytes, src unread
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(ok ? 16 : 0) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
+// Start loading group g into the stage at shared address st (rows >= M zero-filled; nothing for g past the last group).
+// One commit group per call, so cp_async_wait_all waits for exactly this load.
+template <int C>
+__device__ __forceinline__ void stage_rows(uint32_t st, const float* __restrict__ X, int64_t g, int64_t ngroups,
+                                           int64_t M, int lane) {
+  constexpr int CPR = C / 4;  // 16-byte chunks per row
+  if (g < ngroups) {
+#pragma unroll
+    for (int t = 0; t < 16 * CPR / 32; ++t) {
+      const int r = (lane >> 3) + 4 * (t / (CPR / 8)), k = (lane & 7) + 8 * (t % (CPR / 8));
+      cp_async16(st + 4 * stage_idx<C>(r, 4 * k), X + (g * 16 + r) * C + 4 * k, g * 16 + r < M);  // M <= row: no read
+    }
+  }
+  cp_async_commit();
+}
+// the fragment-order float2 of row r (0..15) at column col (even) from the stage at shared address st
+template <int C>
+__device__ __forceinline__ float2 stage_f2(uint32_t st, int r, int col) {
+  return ld_shared_v2_f32(st + 4 * stage_idx<C>(r, col));
 }
 
 // ==================================================================== fused frontend QKV projection
@@ -44,25 +93,29 @@ __global__ void __launch_bounds__(FU_THREADS, C == 32 ? 4 : 2)
 fused_qkv_kernel(const h16* __restrict__ wqkv, const float* __restrict__ X, const float* __restrict__ wg,
                  const float* __restrict__ bg, const float* __restrict__ rope_cos, const float* __restrict__ rope_sin,
                  h16* __restrict__ qkv, float* __restrict__ gates, int64_t M, int L, int F, int posmode, float qscale) {
-  constexpr int LD = C + 8, KS = C / 16, NB = 3 * C / 8, heads = C / 32;
+  constexpr int LD = C + 8, KS = C / 16, heads = C / 32;
   extern __shared__ uint4 fu_smem[];
   h16* sW = reinterpret_cast<h16*>(fu_smem);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, q = lane & 3;
+  const uint32_t sw = smem_u32(sW), st = sw + 2 * 3 * C * LD + 4 * warp * stage_floats<C>();  // st: this warp's row stage
+  const int64_t ngroups = (M + 15) / 16;
+  int64_t g = static_cast<int64_t>(blockIdx.x) * FU_WARPS + warp;
+  stage_rows<C>(st, X, g, ngroups, M, lane);
   stage_weight(sW, wqkv, 3 * C, C);
   __syncthreads();
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, q = lane & 3;
-  const int64_t ngroups = (M + 15) / 16;
-  for (int64_t g = static_cast<int64_t>(blockIdx.x) * FU_WARPS + warp; g < ngroups; g += static_cast<int64_t>(gridDim.x) * FU_WARPS) {
+  for (; g < ngroups; g += static_cast<int64_t>(gridDim.x) * FU_WARPS) {
     int64_t m[2];
     bool ok[2];
     float xs[2][C / 4];  // xs[r][4 ks + 2 h + e] = x[row r][16 ks + 8 h + 2 q + e]
+    cp_async_wait_all();
+    __syncwarp();
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
       m[r] = g * 16 + (lane >> 2) + 8 * r;
       ok[r] = m[r] < M;
 #pragma unroll
       for (int j = 0; j < C / 4; j += 2) {
-        const float2 v = ok[r] ? *reinterpret_cast<const float2*>(X + m[r] * C + 16 * (j >> 2) + 8 * ((j >> 1) & 1) + 2 * q)
-                               : make_float2(0.f, 0.f);
+        const float2 v = stage_f2<C>(st, (lane >> 2) + 8 * r, 16 * (j >> 2) + 8 * ((j >> 1) & 1) + 2 * q);
         xs[r][j] = v.x;
         xs[r][j + 1] = v.y;
       }
@@ -101,6 +154,8 @@ fused_qkv_kernel(const h16* __restrict__ wqkv, const float* __restrict__ X, cons
       a[ks][2] = pack_h16x2(xs[0][4 * ks + 2], xs[0][4 * ks + 3]);
       a[ks][3] = pack_h16x2(xs[1][4 * ks + 2], xs[1][4 * ks + 3]);
     }
+    __syncwarp();  // every lane has read the stage: refill it with the next group while this one computes
+    stage_rows<C>(st, X, g + static_cast<int64_t>(gridDim.x) * FU_WARPS, ngroups, M, lane);
     const float* cs[2];
     const float* sn[2];
 #pragma unroll
@@ -109,29 +164,41 @@ fused_qkv_kernel(const h16* __restrict__ wqkv, const float* __restrict__ X, cons
       cs[r] = rope_cos + pos * 16;
       sn[r] = rope_sin + pos * 16;
     }
+    // 0 q, 1 k, 2 v, C / 8 column blocks each, two at a time; not unrolled, so that the B fragments of all 3 C columns
+    // are not loaded ahead at once (at C = 64 that spilled at the 128 registers of 2 CTAs per SM)
+#pragma unroll 1
+    for (int which = 0; which < 3; ++which)
 #pragma unroll
-    for (int nb = 0; nb < NB; ++nb) {
-      float acc[4] = {0.f, 0.f, 0.f, 0.f};
+    for (int nb = which * (C / 8); nb < (which + 1) * (C / 8); nb += 2) {
+      float acc[2][4] = {};
 #pragma unroll
-      for (int ks = 0; ks < KS; ++ks) {
-        uint32_t b0, b1;
-        b_frag<LD>(sW, nb, ks, lane, b0, b1);
-        mma_16816(acc, a[ks], b0, b1);
-      }
-      const int n = nb * 8 + 2 * q;
-      const int which = (nb * 8) / C;  // 0 q, 1 k, 2 v (a block of 8 columns never straddles them)
+      for (int u = 0; u < 2; ++u)
+#pragma unroll
+        for (int ks = 0; ks < KS; ks += 2) {
+          uint32_t b[4];
+          b_frag_k2<LD>(sw, nb + u, ks, lane, b);
+          mma_16816(acc[u], a[ks], b[0], b[1]);
+          mma_16816(acc[u], a[ks + 1], b[2], b[3]);
+        }
 #pragma unroll
       for (int r = 0; r < 2; ++r) {
-        float v0 = acc[2 * r], v1 = acc[2 * r + 1];
-        if (which < 2) {
-          const float sc = which == 0 ? qscale : 1.0f;
-          const int i = ((n - which * C) & 31) >> 1;
-          const float co = __ldg(cs[r] + i), si = __ldg(sn[r] + i);
-          const float x0 = v0, x1 = v1;
-          v0 = (x0 * co - x1 * si) * sc;
-          v1 = (x1 * co + x0 * si) * sc;
+        uint32_t p[2];
+#pragma unroll
+        for (int u = 0; u < 2; ++u) {
+          const int n = (nb + u) * 8 + 2 * q;
+          float v0 = acc[u][2 * r], v1 = acc[u][2 * r + 1];
+          if (which < 2) {
+            const float sc = which == 0 ? qscale : 1.0f;
+            const int i = ((n - which * C) & 31) >> 1;
+            const float co = __ldg(cs[r] + i), si = __ldg(sn[r] + i);
+            const float x0 = v0, x1 = v1;
+            v0 = (x0 * co - x1 * si) * sc;
+            v1 = (x1 * co + x0 * si) * sc;
+          }
+          p[u] = pack_h16x2(v0, v1);
         }
-        if (ok[r]) *reinterpret_cast<uint32_t*>(qkv + m[r] * (3 * C) + n) = pack_h16x2(v0, v1);
+        const uint2 w = quad_pair(p[0], p[1], q);
+        if (ok[r]) *reinterpret_cast<uint2*>(qkv + m[r] * (3 * C) + nb * 8 + quad_col(q)) = w;
       }
     }
   }
@@ -153,13 +220,26 @@ fused_ff_kernel(const h16* __restrict__ w1, const h16* __restrict__ w2, const h1
   h16* sW1 = reinterpret_cast<h16*>(fu_smem);  // [4C][C + 8]
   h16* sW2 = sW1 + HID * LD1;                   // [C][4C + 8]
   h16* sWo = sW2 + C * LD2;                     // [C][C + 8] (OP)
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, q = lane & 3;
+  const uint32_t sw1 = smem_u32(sW1), sw2 = smem_u32(sW2), swo = smem_u32(sWo);
+  const uint32_t st = swo + 2 * (OP ? C * LD1 : 0) + 4 * warp * stage_floats<C>();  // this warp's row stage
+  const int64_t ngroups = (M + 15) / 16;
+  int64_t g = static_cast<int64_t>(blockIdx.x) * FU_WARPS + warp;
+  // O is not staged (at C = 64 the weights and the X stages leave no room for it): its rows go to L2 one group ahead
+  auto prefetch_o = [&](int64_t gg) {
+    if (OP && lane == 0 && gg < ngroups) {
+      const int64_t rows = M - gg * 16 < 16 ? M - gg * 16 : 16;
+      asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(O + gg * 16 * C), "r"(static_cast<uint32_t>(rows * C * 2))
+                   : "memory");
+    }
+  };
+  stage_rows<C>(st, X, g, ngroups, M, lane);
+  prefetch_o(g);
   stage_weight(sW1, w1, HID, C);
   stage_weight(sW2, w2, C, HID);
   if constexpr (OP) stage_weight(sWo, wo, C, C);
   __syncthreads();
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, q = lane & 3;
-  const int64_t ngroups = (M + 15) / 16;
-  for (int64_t g = static_cast<int64_t>(blockIdx.x) * FU_WARPS + warp; g < ngroups; g += static_cast<int64_t>(gridDim.x) * FU_WARPS) {
+  for (; g < ngroups; g += static_cast<int64_t>(gridDim.x) * FU_WARPS) {
     int64_t m[2];
     bool ok[2];
 #pragma unroll
@@ -168,14 +248,19 @@ fused_ff_kernel(const h16* __restrict__ w1, const h16* __restrict__ w2, const h1
       ok[r] = m[r] < M;
     }
     float acc[NB][4];  // columns 8 nb + 2 q + {0, 1} of rows r0 (acc[nb][0..1]) and r0 + 8 (acc[nb][2..3])
+    cp_async_wait_all();
+    __syncwarp();
 #pragma unroll
     for (int nb = 0; nb < NB; ++nb)
 #pragma unroll
       for (int r = 0; r < 2; ++r) {
-        const float2 v = ok[r] ? *reinterpret_cast<const float2*>(X + m[r] * C + nb * 8 + 2 * q) : make_float2(0.f, 0.f);
+        const float2 v = stage_f2<C>(st, (lane >> 2) + 8 * r, nb * 8 + 2 * q);
         acc[nb][2 * r] = v.x;
         acc[nb][2 * r + 1] = v.y;
       }
+    __syncwarp();  // every lane has read the stage: refill it with the next group while this one computes
+    stage_rows<C>(st, X, g + static_cast<int64_t>(gridDim.x) * FU_WARPS, ngroups, M, lane);
+    prefetch_o(g + static_cast<int64_t>(gridDim.x) * FU_WARPS);
     if constexpr (OP) {  // x' = x + O Wo^T, O (gated attention output, 16-bit) loaded in A-fragment order
       uint32_t ao[KS][4];
 #pragma unroll
@@ -188,10 +273,11 @@ fused_ff_kernel(const h16* __restrict__ w1, const h16* __restrict__ w2, const h1
 #pragma unroll
       for (int nb = 0; nb < NB; ++nb)
 #pragma unroll
-        for (int ks = 0; ks < KS; ++ks) {
-          uint32_t b0, b1;
-          b_frag<LD1>(sWo, nb, ks, lane, b0, b1);
-          mma_16816(acc[nb], ao[ks], b0, b1);
+        for (int ks = 0; ks < KS; ks += 2) {
+          uint32_t b[4];
+          b_frag_k2<LD1>(swo, nb, ks, lane, b);
+          mma_16816(acc[nb], ao[ks], b[0], b[1]);
+          mma_16816(acc[nb], ao[ks + 1], b[2], b[3]);
         }
     }
     float inv[2];
@@ -225,10 +311,11 @@ fused_ff_kernel(const h16* __restrict__ w1, const h16* __restrict__ w2, const h1
       for (int t = 0; t < 2; ++t) {
         hh[t][0] = hh[t][1] = hh[t][2] = hh[t][3] = 0.f;
 #pragma unroll
-        for (int ks = 0; ks < KS; ++ks) {
-          uint32_t b0, b1;
-          b_frag<LD1>(sW1, 2 * j + t, ks, lane, b0, b1);
-          mma_16816(hh[t], a[ks], b0, b1);
+        for (int ks = 0; ks < KS; ks += 2) {
+          uint32_t b[4];
+          b_frag_k2<LD1>(sw1, 2 * j + t, ks, lane, b);
+          mma_16816(hh[t], a[ks], b[0], b[1]);
+          mma_16816(hh[t], a[ks + 1], b[2], b[3]);
         }
         const float2 b = __ldg(reinterpret_cast<const float2*>(b1 + (2 * j + t) * 8 + 2 * q));
         hh[t][0] = gelu_tanh_fast(hh[t][0] + b.x); hh[t][1] = gelu_tanh_fast(hh[t][1] + b.y);
@@ -237,10 +324,11 @@ fused_ff_kernel(const h16* __restrict__ w1, const h16* __restrict__ w2, const h1
       const uint32_t ah[4] = {pack_h16x2(hh[0][0], hh[0][1]), pack_h16x2(hh[0][2], hh[0][3]), pack_h16x2(hh[1][0], hh[1][1]),
                               pack_h16x2(hh[1][2], hh[1][3])};
 #pragma unroll
-      for (int nb = 0; nb < NB; ++nb) {
-        uint32_t b0, b1;
-        b_frag<LD2>(sW2, nb, j, lane, b0, b1);
-        mma_16816(acc[nb], ah, b0, b1);
+      for (int nb = 0; nb < NB; nb += 2) {
+        uint32_t b[4];
+        b_frag_n2<LD2>(sw2, nb, j, lane, b);
+        mma_16816(acc[nb], ah, b[0], b[1]);
+        mma_16816(acc[nb + 1], ah, b[2], b[3]);
       }
     }
 #pragma unroll
@@ -255,8 +343,11 @@ fused_ff_kernel(const h16* __restrict__ w1, const h16* __restrict__ w2, const h1
   }
 }
 
-template <int C> constexpr int ff_smem(bool op) { return (4 * C * (C + 8) + C * (4 * C + 8) + (op ? C * (C + 8) : 0)) * 2; }
-template <int C> constexpr int qkv_smem() { return 3 * C * (C + 8) * 2; }
+// weights, then one 16-row fp32 stage per warp
+template <int C> constexpr int ff_smem(bool op) {
+  return (4 * C * (C + 8) + C * (4 * C + 8) + (op ? C * (C + 8) : 0)) * 2 + FU_WARPS * stage_floats<C>() * 4;
+}
+template <int C> constexpr int qkv_smem() { return 3 * C * (C + 8) * 2 + FU_WARPS * stage_floats<C>() * 4; }
 template <int C> constexpr int ff_ctas() { return C == 32 ? 3 : 2; }
 template <int C> constexpr int qkv_ctas() { return C == 32 ? 4 : 2; }
 
@@ -324,13 +415,23 @@ void launch_fused_qkv(const TcQkvPlan* p, const float* X, const float* wg, const
                                                                                              gates, p->M, L, F, posmode, qscale);
 }
 
+// fused_ff_kernel<64, OP> needs the largest shared-memory carveout for its 2 CTAs per SM (2 x 113 KB + 1 KB reserved
+// per CTA = 228 KB with OP); the others keep the default, which leaves L1 room for the RoPE tables and biases.
+template <typename K>
+static cudaError_t fused_attrs(K* kernel, int smem, bool max_carveout = false) {
+  cudaError_t r = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  if (r == cudaSuccess && max_carveout)
+    r = cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  return r;
+}
+
 int tc_init_fused(char* err, int errlen) {
-  cudaError_t r = cudaFuncSetAttribute(fused_ff_kernel<32, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, ff_smem<32>(false));
-  if (r == cudaSuccess) r = cudaFuncSetAttribute(fused_ff_kernel<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, ff_smem<64>(false));
-  if (r == cudaSuccess) r = cudaFuncSetAttribute(fused_ff_kernel<32, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, ff_smem<32>(true));
-  if (r == cudaSuccess) r = cudaFuncSetAttribute(fused_ff_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, ff_smem<64>(true));
-  if (r == cudaSuccess) r = cudaFuncSetAttribute(fused_qkv_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, qkv_smem<32>());
-  if (r == cudaSuccess) r = cudaFuncSetAttribute(fused_qkv_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, qkv_smem<64>());
+  cudaError_t r = fused_attrs(fused_ff_kernel<32, false>, ff_smem<32>(false));
+  if (r == cudaSuccess) r = fused_attrs(fused_ff_kernel<64, false>, ff_smem<64>(false), true);
+  if (r == cudaSuccess) r = fused_attrs(fused_ff_kernel<32, true>, ff_smem<32>(true));
+  if (r == cudaSuccess) r = fused_attrs(fused_ff_kernel<64, true>, ff_smem<64>(true), true);
+  if (r == cudaSuccess) r = fused_attrs(fused_qkv_kernel<32>, qkv_smem<32>());
+  if (r == cudaSuccess) r = fused_attrs(fused_qkv_kernel<64>, qkv_smem<64>());
   if (r != cudaSuccess) {
     snprintf(err, errlen, "cudaFuncSetAttribute(fused_ff_kernel / fused_qkv_kernel) failed: %s", cudaGetErrorString(r));
     return -1;

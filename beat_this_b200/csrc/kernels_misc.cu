@@ -27,11 +27,10 @@ stem_kernel(const float* __restrict__ spect, const ChunkSrc* __restrict__ chunks
   for (int i = threadIdx.x; i < 32 * 12; i += 128) ws[i] = w[i];
   if (threadIdx.x < 32) bs[threadIdx.x] = bias[threadIdx.x];
   __syncthreads();
-  const int t = blockIdx.x * 128 + threadIdx.x;
+  const int t = blockIdx.x * 128 + threadIdx.x;  // frames t and t ^ 1 are neighbouring lanes
   const int f = blockIdx.y;
   const int b = blockIdx.z;
-  if (t >= L) return;
-  const ChunkSrc cs = chunks[b];
+  const ChunkSrc cs = chunks[b];  // t >= L: computed (its loads stay inside the clip) but not stored
   float in[4][3];
 #pragma unroll
   for (int dt = 0; dt < 3; ++dt) {
@@ -47,13 +46,18 @@ stem_kernel(const float* __restrict__ spect, const ChunkSrc* __restrict__ chunks
     for (int df = 0; df < 4; ++df)
       in[df][dt] = conv_ok ? fmaf(vv[df], bn1_scale[4 * f + df], bn1_shift[4 * f + df]) : 0.f;
   }
-  float* op = out + ((static_cast<int64_t>(b) * 32 + f) * L + t) * 32;
+  // Channels go 8 at a time, one 32-byte sector of the frame's row.  The lanes of frames t and t ^ 1 swap half of their
+  // 8 values, then each store of the pair writes one whole sector: first frame t & ~1's, then frame t | 1's, the even
+  // lane channels 8 c8 .. + 3 and the odd lane 8 c8 + 4 .. + 7.  (A lane's own 16-byte stores would cover half of
+  // every sector they touch, which makes L2 read the sector from HBM before it merges the write.)
+  const bool odd = t & 1;
+  float* op = out + ((static_cast<int64_t>(b) * 32 + f) * L + (t & ~1)) * 32 + (odd ? 4 : 0);
 #pragma unroll
-  for (int c4 = 0; c4 < 8; ++c4) {
-    float r[4];
+  for (int c8 = 0; c8 < 4; ++c8) {
+    float r[8];
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int co = c4 * 4 + i;
+    for (int i = 0; i < 8; ++i) {
+      const int co = c8 * 8 + i;
       float a = bs[co];
 #pragma unroll
       for (int df = 0; df < 4; ++df)
@@ -61,7 +65,14 @@ stem_kernel(const float* __restrict__ spect, const ChunkSrc* __restrict__ chunks
         for (int dt = 0; dt < 3; ++dt) a = fmaf(in[df][dt], ws[co * 12 + df * 3 + dt], a);
       r[i] = gelu_fast(a);  // erf to 1.5e-7 on rcp + ex2 (erff: ~35 instructions, 32 of them per thread here)
     }
-    reinterpret_cast<float4*>(op)[c4] = make_float4(r[0], r[1], r[2], r[3]);
+    float x[4];  // the partner's values: the even lane gets channels 8 c8 .. + 3 of frame t | 1, the odd lane
+                 // 8 c8 + 4 .. + 7 of frame t & ~1
+#pragma unroll
+    for (int i = 0; i < 4; ++i) x[i] = __shfl_xor_sync(0xffffffffu, odd ? r[i] : r[4 + i], 1);
+    const float4 lo = odd ? make_float4(x[0], x[1], x[2], x[3]) : make_float4(r[0], r[1], r[2], r[3]);
+    const float4 hi = odd ? make_float4(r[4], r[5], r[6], r[7]) : make_float4(x[0], x[1], x[2], x[3]);
+    if ((t & ~1) < L) reinterpret_cast<float4*>(op + 8 * c8)[0] = lo;
+    if ((t | 1) < L) reinterpret_cast<float4*>(op + 32 + 8 * c8)[0] = hi;
   }
 }
 
