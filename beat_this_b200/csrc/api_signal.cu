@@ -33,7 +33,8 @@ int bt_logmel(bt_ctx* c, const float* audio_dev, const int64_t* sample_offsets_h
   if (!c) return BT_ERR_ARG;
   for (const char* n : {"mel.window", "mel.twiddle", "mel.fb_start", "mel.fb_ptr", "mel.fb_w"})
     if (!find_param(c, n)) return fail(c, BT_ERR_STATE, "bt_logmel: parameter '%s' not set", n);
-  if (n_clips <= 0) return BT_OK;
+  if (n_clips < 0) return fail(c, BT_ERR_ARG, "bt_logmel: negative clip count");
+  if (n_clips == 0) return BT_OK;
   if (!audio_dev || !sample_offsets_host || !spect_dev || !frame_offsets_host)
     return fail(c, BT_ERR_ARG, "bt_logmel: null argument");
   int r = check_stft_frames(c, "bt_logmel", sample_offsets_host, frame_offsets_host, n_clips, BT_N_FFT, BT_HOP);
@@ -88,7 +89,8 @@ int bt_resample(bt_ctx* c, const float* audio_in_dev, const int64_t* in_offsets_
                 const float* coef_dev, int32_t L, int32_t M, int32_t K, float* audio_out_dev,
                 const int64_t* out_offsets_host, void* stream) {
   if (!c) return BT_ERR_ARG;
-  if (n_clips <= 0) return BT_OK;
+  if (n_clips < 0) return fail(c, BT_ERR_ARG, "bt_resample: negative clip count");
+  if (n_clips == 0) return BT_OK;
   if (!audio_in_dev || !in_offsets_host || !coef_dev || !audio_out_dev || !out_offsets_host)
     return fail(c, BT_ERR_ARG, "bt_resample: null argument");
   if (L <= 0 || M <= 0 || K <= 0 || (K & 1)) return fail(c, BT_ERR_ARG, "bt_resample: need L, M > 0 and an even K > 0");

@@ -13,6 +13,8 @@ namespace bt {
 
 namespace {
 
+constexpr int kMaxGridY = 65535;  // gridDim.y limit: logmel_kernel and resample_kernel loop over the clips beyond it
+
 template <int LOG2N>
 constexpr size_t fft_smem() { return MelGeom<LOG2N>::SPEC_OFF; }  // the FFT buffer of the CTA's FPC frames
 
@@ -126,87 +128,90 @@ logmel_kernel(const float* __restrict__ audio, const int64_t* __restrict__ sampl
               const int64_t* __restrict__ frame_off, const float* __restrict__ window,
               const float2* __restrict__ twiddle, const int32_t* __restrict__ fb_start,
               const int32_t* __restrict__ fb_ptr, const float* __restrict__ fb_w,
-              float* __restrict__ spect) {
+              float* __restrict__ spect, int n_clips) {
   __shared__ float2 tw[512];                 // e^{-2 pi i j / 1024}, j < 512
   __shared__ float2 t1[2][8 * LM_P1];        // per frame: T1, later Z (512 entries)
   __shared__ float2 t2[2][8 * LM_P2];
   __shared__ float mag[2][516];
-  const int clip = blockIdx.y;
-  const int64_t f0 = frame_off[clip];
-  const int T = static_cast<int>(frame_off[clip + 1] - f0);
   const int tid = threadIdx.x, half = tid >> 6, lt = tid & 63;
   const int t = 2 * blockIdx.x + half;
-  if (2 * static_cast<int>(blockIdx.x) >= T) return;  // whole CTA beyond the clip
-  const bool active = t < T;
-  const int64_t s0 = sample_off[clip];
-  const int64_t len = sample_off[clip + 1] - s0;
-  for (int i = tid; i < 512; i += 128) tw[i] = twiddle[i];
-  auto TW = [&](int j) -> float2 {  // e^{-2 pi i j / 1024}, 0 <= j < 1024
-    const float2 w = tw[j & 511];
-    return (j & 512) ? make_float2(-w.x, -w.y) : w;
-  };
-  float2 v[8];
-  float2* T1 = t1[half];
-  float2* T2 = t2[half];
-  {  // ---- pass A: thread (n2, n3) = lt, points z[64 n1 + lt] ----
+  // clips blockIdx.y, blockIdx.y + gridDim.y, ...: a grid holds at most kMaxGridY clips, a call any number.  Each shared
+  // array is rewritten for the next clip only after a barrier that follows this clip's last read of it.
+  for (int clip = blockIdx.y; clip < n_clips; clip += gridDim.y) {
+    const int64_t f0 = frame_off[clip];
+    const int T = static_cast<int>(frame_off[clip + 1] - f0);
+    if (2 * static_cast<int>(blockIdx.x) >= T) continue;  // whole CTA beyond the clip
+    const bool active = t < T;
+    const int64_t s0 = sample_off[clip];
+    const int64_t len = sample_off[clip + 1] - s0;
+    for (int i = tid; i < 512; i += 128) tw[i] = twiddle[i];
+    auto TW = [&](int j) -> float2 {  // e^{-2 pi i j / 1024}, 0 <= j < 1024
+      const float2 w = tw[j & 511];
+      return (j & 512) ? make_float2(-w.x, -w.y) : w;
+    };
+    float2 v[8];
+    float2* T1 = t1[half];
+    float2* T2 = t2[half];
+    {  // ---- pass A: thread (n2, n3) = lt, points z[64 n1 + lt] ----
 #pragma unroll
-    for (int n1 = 0; n1 < 8; ++n1) {
-      const int n = 2 * (64 * n1 + lt);
-      float xs[2];
+      for (int n1 = 0; n1 < 8; ++n1) {
+        const int n = 2 * (64 * n1 + lt);
+        float xs[2];
 #pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        int64_t i = 441ll * t + (n + e) - 512;
-        if (i < 0) i = -i;                      // reflect (no edge repeat), torch pad_mode="reflect"
-        if (i >= len) i = 2 * (len - 1) - i;
-        xs[e] = active ? audio[s0 + i] * __ldg(window + n + e) : 0.f;
+        for (int e = 0; e < 2; ++e) {
+          int64_t i = 441ll * t + (n + e) - 512;
+          if (i < 0) i = -i;                      // reflect (no edge repeat), torch pad_mode="reflect"
+          if (i >= len) i = 2 * (len - 1) - i;
+          xs[e] = active ? audio[s0 + i] * __ldg(window + n + e) : 0.f;
+        }
+        v[n1] = make_float2(xs[0], xs[1]);
       }
-      v[n1] = make_float2(xs[0], xs[1]);
     }
-  }
-  __syncthreads();  // twiddle table
-  {
-    dft8(v);
-    const int n2 = lt >> 3;
+    __syncthreads();  // twiddle table
+    {
+      dft8(v);
+      const int n2 = lt >> 3;
 #pragma unroll
-    for (int k1 = 0; k1 < 8; ++k1) T1[k1 * LM_P1 + lt] = k1 == 0 ? v[0] : cmul(v[k1], TW(16 * n2 * k1));
-  }
-  __syncthreads();
-  {  // ---- pass B: thread (k1, n3) = lt ----
-    const int k1 = lt >> 3, n3 = lt & 7;
+      for (int k1 = 0; k1 < 8; ++k1) T1[k1 * LM_P1 + lt] = k1 == 0 ? v[0] : cmul(v[k1], TW(16 * n2 * k1));
+    }
+    __syncthreads();
+    {  // ---- pass B: thread (k1, n3) = lt ----
+      const int k1 = lt >> 3, n3 = lt & 7;
 #pragma unroll
-    for (int n2 = 0; n2 < 8; ++n2) v[n2] = T1[k1 * LM_P1 + n2 * 8 + n3];
-    dft8(v);
+      for (int n2 = 0; n2 < 8; ++n2) v[n2] = T1[k1 * LM_P1 + n2 * 8 + n3];
+      dft8(v);
 #pragma unroll
-    for (int k2 = 0; k2 < 8; ++k2) T2[n3 * LM_P2 + k2 * 8 + k1] = cmul(v[k2], TW(2 * n3 * (k1 + 8 * k2)));
-  }
-  __syncthreads();
-  {  // ---- pass C: thread (k2, k1) = lt -> Z[lt + 64 k3] (into T1's storage) ----
+      for (int k2 = 0; k2 < 8; ++k2) T2[n3 * LM_P2 + k2 * 8 + k1] = cmul(v[k2], TW(2 * n3 * (k1 + 8 * k2)));
+    }
+    __syncthreads();
+    {  // ---- pass C: thread (k2, k1) = lt -> Z[lt + 64 k3] (into T1's storage) ----
 #pragma unroll
-    for (int n3 = 0; n3 < 8; ++n3) v[n3] = T2[n3 * LM_P2 + lt];
-    dft8(v);
+      for (int n3 = 0; n3 < 8; ++n3) v[n3] = T2[n3 * LM_P2 + lt];
+      dft8(v);
 #pragma unroll
-    for (int k3 = 0; k3 < 8; ++k3) T1[lt + 64 * k3] = v[k3];
-  }
-  __syncthreads();
-  // untangle: X[k] = E[k] + e^{-2 pi i k / 1024} O[k], E = (Z[k] + conj Z[512 - k]) / 2, O = -i (Z[k] - conj Z[512 - k]) / 2;
-  // magnitudes of bins 0..512 (normalized=True -> 1 / sqrt(1024))
-  for (int k = lt; k <= 512; k += 64) {
-    const float2 zk = T1[k & 511], zc = T1[(512 - k) & 511];
-    const float2 e = make_float2(0.5f * (zk.x + zc.x), 0.5f * (zk.y - zc.y));
-    const float2 o = make_float2(0.5f * (zk.y + zc.y), -0.5f * (zk.x - zc.x));
-    const float2 x = cadd(e, cmul(TW(k), o));
-    mag[half][k] = sqrtf(x.x * x.x + x.y * x.y) * 0.03125f;
-  }
-  __syncthreads();
-  if (active) {
+      for (int k3 = 0; k3 < 8; ++k3) T1[lt + 64 * k3] = v[k3];
+    }
+    __syncthreads();
+    // untangle: X[k] = E[k] + e^{-2 pi i k / 1024} O[k], E = (Z[k] + conj Z[512 - k]) / 2, O = -i (Z[k] - conj Z[512 - k]) / 2;
+    // magnitudes of bins 0..512 (normalized=True -> 1 / sqrt(1024))
+    for (int k = lt; k <= 512; k += 64) {
+      const float2 zk = T1[k & 511], zc = T1[(512 - k) & 511];
+      const float2 e = make_float2(0.5f * (zk.x + zc.x), 0.5f * (zk.y - zc.y));
+      const float2 o = make_float2(0.5f * (zk.y + zc.y), -0.5f * (zk.x - zc.x));
+      const float2 x = cadd(e, cmul(TW(k), o));
+      mag[half][k] = sqrtf(x.x * x.x + x.y * x.y) * 0.03125f;
+    }
+    __syncthreads();
+    if (active) {
 #pragma unroll
-    for (int mm = 0; mm < 2; ++mm) {
-      const int m = lt + 64 * mm;  // mel bin
-      const int p0 = fb_ptr[m], p1 = fb_ptr[m + 1];
-      const int k0 = fb_start[m];
-      float acc = 0.f;
-      for (int p = p0; p < p1; ++p) acc = fmaf(mag[half][k0 + (p - p0)], fb_w[p], acc);
-      spect[(f0 + t) * 128 + m] = log1pf(1000.0f * acc);
+      for (int mm = 0; mm < 2; ++mm) {
+        const int m = lt + 64 * mm;  // mel bin
+        const int p0 = fb_ptr[m], p1 = fb_ptr[m + 1];
+        const int k0 = fb_start[m];
+        float acc = 0.f;
+        for (int p = p0; p < p1; ++p) acc = fmaf(mag[half][k0 + (p - p0)], fb_w[p], acc);
+        spect[(f0 + t) * 128 + m] = log1pf(1000.0f * acc);
+      }
     }
   }
 }
@@ -216,9 +221,9 @@ void launch_logmel(const float* audio, const int64_t* sample_off_dev, const int6
                    const int32_t* fb_start, const int32_t* fb_ptr, const float* fb_w, float* spect,
                    cudaStream_t st) {
   if (max_frames <= 0 || n_clips <= 0) return;
-  dim3 grid(static_cast<unsigned>((max_frames + 1) / 2), static_cast<unsigned>(n_clips));
+  dim3 grid(static_cast<unsigned>((max_frames + 1) / 2), static_cast<unsigned>(std::min(n_clips, kMaxGridY)));
   logmel_kernel<<<grid, 128, 0, st>>>(audio, sample_off_dev, frame_off_dev, window,
-                                      reinterpret_cast<const float2*>(twiddle), fb_start, fb_ptr, fb_w, spect);
+                                      reinterpret_cast<const float2*>(twiddle), fb_start, fb_ptr, fb_w, spect, n_clips);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -306,36 +311,40 @@ cudaError_t launch_logmel_config(int log2n, const float* audio, const int64_t* s
 // ------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
 resample_kernel(const float* __restrict__ in, const int64_t* __restrict__ in_off, float* __restrict__ out,
-                const int64_t* __restrict__ out_off, const float* __restrict__ coef, int L, int M, int K) {
+                const int64_t* __restrict__ out_off, int n_clips, const float* __restrict__ coef, int L, int M, int K) {
   extern __shared__ float xs[];
-  const int clip = blockIdx.y;
   const int64_t n0 = static_cast<int64_t>(blockIdx.x) * 256;
-  const int64_t s0 = in_off[clip], len = in_off[clip + 1] - s0;
-  const int64_t o0 = out_off[clip], nout = out_off[clip + 1] - o0;
-  if (n0 >= nout) return;
-  const int64_t n_last = min(n0 + 255, nout - 1);
-  const int64_t j_lo = (n0 * M) / L - K / 2 + 1;
-  const int span = static_cast<int>((n_last * M) / L - K / 2 + K - j_lo + 1);
-  for (int i = threadIdx.x; i < span; i += 256) {
-    const int64_t j = j_lo + i;
-    xs[i] = (j >= 0 && j < len) ? in[s0 + j] : 0.f;
+  // clips blockIdx.y, blockIdx.y + gridDim.y, ...: a grid holds at most kMaxGridY clips, a call any number
+  for (int clip = blockIdx.y; clip < n_clips; clip += gridDim.y) {
+    const int64_t s0 = in_off[clip], len = in_off[clip + 1] - s0;
+    const int64_t o0 = out_off[clip], nout = out_off[clip + 1] - o0;
+    if (n0 >= nout) continue;
+    const int64_t n_last = min(n0 + 255, nout - 1);
+    const int64_t j_lo = (n0 * M) / L - K / 2 + 1;
+    const int span = static_cast<int>((n_last * M) / L - K / 2 + K - j_lo + 1);
+    for (int i = threadIdx.x; i < span; i += 256) {
+      const int64_t j = j_lo + i;
+      xs[i] = (j >= 0 && j < len) ? in[s0 + j] : 0.f;
+    }
+    __syncthreads();
+    const int64_t n = n0 + threadIdx.x;
+    if (n < nout) {
+      const int64_t nm = n * M;
+      const int base = static_cast<int>(nm / L - K / 2 + 1 - j_lo);
+      const float* c = coef + static_cast<int64_t>(nm % L) * K;
+      float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
+      int k = 0;
+      for (; k + 4 <= K; k += 4) {
+        a0 = fmaf(__ldg(c + k), xs[base + k], a0);
+        a1 = fmaf(__ldg(c + k + 1), xs[base + k + 1], a1);
+        a2 = fmaf(__ldg(c + k + 2), xs[base + k + 2], a2);
+        a3 = fmaf(__ldg(c + k + 3), xs[base + k + 3], a3);
+      }
+      for (; k < K; ++k) a0 = fmaf(__ldg(c + k), xs[base + k], a0);
+      out[o0 + n] = (a0 + a1) + (a2 + a3);
+    }
+    __syncthreads();  // the next clip's span overwrites xs
   }
-  __syncthreads();
-  const int64_t n = n0 + threadIdx.x;
-  if (n >= nout) return;
-  const int64_t nm = n * M;
-  const int base = static_cast<int>(nm / L - K / 2 + 1 - j_lo);
-  const float* c = coef + static_cast<int64_t>(nm % L) * K;
-  float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
-  int k = 0;
-  for (; k + 4 <= K; k += 4) {
-    a0 = fmaf(__ldg(c + k), xs[base + k], a0);
-    a1 = fmaf(__ldg(c + k + 1), xs[base + k + 1], a1);
-    a2 = fmaf(__ldg(c + k + 2), xs[base + k + 2], a2);
-    a3 = fmaf(__ldg(c + k + 3), xs[base + k + 3], a3);
-  }
-  for (; k < K; ++k) a0 = fmaf(__ldg(c + k), xs[base + k], a0);
-  out[o0 + n] = (a0 + a1) + (a2 + a3);
 }
 
 int64_t resample_smem(int L, int M, int K) { return ((255ll * M) / L + K + 2) * 4; }  // the staged input span
@@ -347,8 +356,8 @@ cudaError_t launch_resample(const float* in, const int64_t* in_off_dev, float* o
   const cudaError_t e = smem > 48 * 1024
       ? cudaFuncSetAttribute(resample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) : cudaSuccess;
   if (e != cudaSuccess) return e;
-  dim3 grid(static_cast<unsigned>((max_out + 255) / 256), static_cast<unsigned>(n_clips));
-  resample_kernel<<<grid, 256, smem, st>>>(in, in_off_dev, out, out_off_dev, coef, L, M, K);
+  dim3 grid(static_cast<unsigned>((max_out + 255) / 256), static_cast<unsigned>(std::min(n_clips, kMaxGridY)));
+  resample_kernel<<<grid, 256, smem, st>>>(in, in_off_dev, out, out_off_dev, n_clips, coef, L, M, K);
   return cudaSuccess;
 }
 

@@ -199,7 +199,8 @@ int bt_stage_wav_files(const char* const* paths, const bt_wav_info* infos, int32
  * audio_dev: concatenated fp32 samples; sample_offsets_host[n_clips+1].
  * spect_dev: out, concatenated [T_i,128] fp32 with T_i = bt_num_frames(len_i), laid out
  * at frame_offsets_host[i] (frames; frame_offsets_host[n_clips+1], starting at 0).  Every clip needs more than
- * BT_N_FFT/2 samples. */
+ * BT_N_FFT/2 samples.  Any n_clips >= 0 runs in one launch (no limit of the grid applies); n_clips < 0 is BT_ERR_ARG
+ * before anything is enqueued, n_clips == 0 does nothing. */
 int bt_logmel(bt_ctx* ctx, const float* audio_dev, const int64_t* sample_offsets_host,
               int32_t n_clips, float* spect_dev, const int64_t* frame_offsets_host,
               void* stream);
@@ -249,7 +250,10 @@ int bt_logmel_config(bt_ctx* ctx, const bt_mel_config* cfg, const float* window_
  * with sr_out/sr_in = L/M in lowest terms.  coef_dev: [L][K] fp32 bank (the host side designs it,
  * beat_this_b200/preprocessing.py: Kaiser-windowed sinc to soxr-HQ-like targets; parity with
  * soxr itself is unpinned).  in/out: concatenated fp32 clips with host offset arrays
- * [n_clips+1]; out lengths are the caller's (normally round(len*L/M)). */
+ * [n_clips+1]; out lengths are the caller's (normally round(len*L/M)).  Any n_clips >= 0 runs in one launch (no
+ * limit of the grid applies); n_clips < 0, a null pointer, L, M < 1, an odd K or K < 1, bad offsets, or (when any
+ * clip has outputs) a ratio whose staged input span of (255*M)/L + K + 2 floats exceeds 200 KB of shared memory is
+ * BT_ERR_ARG before anything is enqueued. */
 int bt_resample(bt_ctx* ctx, const float* audio_in_dev, const int64_t* in_offsets_host,
                 int32_t n_clips, const float* coef_dev, int32_t L, int32_t M, int32_t K,
                 float* audio_out_dev, const int64_t* out_offsets_host, void* stream);

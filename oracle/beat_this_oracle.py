@@ -326,11 +326,11 @@ def audio2beats(sd: dict, signal: np.ndarray, sr: int = SR):
     return postp_minimal(b, d)
 
 
-def resample_direct(x, sr_in: int, sr_out: int = 22050):
-    """Float64 direct-form evaluation of the resampler DEFINITION in beat_this_b200/preprocessing.py
-    (stand-in for soxr.resample, reference inference.py:274-275; parity with soxr unpinned): every output
-    sample sums the continuous Kaiser-windowed sinc over the input samples in its support -- no polyphase
-    bank, so the bank construction and the kernel indexing are checked independently."""
+def resample_direct_terms(x, sr_in: int, sr_out: int, n):
+    """The terms of the direct form at the output indices n: (samples [len(n), 2 half + 1], weights [len(n), 2 half + 1])
+    with y[n] = sum(samples * weights, 1) -- the input samples j = floor(n M / L) - half .. floor(n M / L) + half
+    (zeros outside the clip) and their weights s h(s (n M / L - j)), half = ceil(Z / s) + 1.  The phase n M / L - j
+    is an exact integer plus (n M mod L) / L, so it is rounded once however long the clip is."""
     import math
 
     import numpy as np
@@ -341,14 +341,30 @@ def resample_direct(x, sr_in: int, sr_out: int = 22050):
     g = math.gcd(int(sr_in), int(sr_out))
     L, M = sr_out // g, sr_in // g
     s = min(1.0, L / M)
-    n_out = (2 * len(x) * L + M) // (2 * M)
     half = int(math.ceil(P.RESAMPLE_ZERO_CROSSINGS / s)) + 1
+    q, r = np.divmod(np.asarray(n, dtype=np.int64) * M, L)
+    off = np.arange(-half, half + 1)
+    j = q[:, None] + off[None, :]
+    ok = (j >= 0) & (j < len(x))
+    xv = np.where(ok, x[np.clip(j, 0, max(len(x) - 1, 0))] if len(x) else 0.0, 0.0)
+    t = (r / L)[:, None] - off[None, :]
+    return xv, s * P.resample_kernel(s * t)
+
+
+def resample_direct(x, sr_in: int, sr_out: int = 22050):
+    """Float64 direct-form evaluation of the resampler DEFINITION in beat_this_b200/preprocessing.py
+    (stand-in for soxr.resample, reference inference.py:274-275; parity with soxr unpinned): every output
+    sample sums the continuous Kaiser-windowed sinc over the input samples in its support -- no polyphase
+    bank, so the bank construction and the kernel indexing are checked independently."""
+    import math
+
+    import numpy as np
+
+    g = math.gcd(int(sr_in), int(sr_out))
+    L, M = sr_out // g, sr_in // g
+    n_out = (2 * len(x) * L + M) // (2 * M)
     y = np.zeros(n_out)
     for n0 in range(0, n_out, 4096):
-        n = np.arange(n0, min(n_out, n0 + 4096))
-        pos = n * (M / L)
-        j = np.floor(pos)[:, None].astype(np.int64) + np.arange(-half, half + 1)[None, :]
-        ok = (j >= 0) & (j < len(x))
-        xv = np.where(ok, x[np.clip(j, 0, len(x) - 1)], 0.0)
-        y[n0 : n0 + len(n)] = (xv * (s * P.resample_kernel(s * (pos[:, None] - j)))).sum(1)
+        xv, w = resample_direct_terms(x, sr_in, sr_out, np.arange(n0, min(n_out, n0 + 4096)))
+        y[n0 : n0 + len(xv)] = (xv * w).sum(1)
     return y
