@@ -93,9 +93,10 @@ def rope_tables(freqs: torch.Tensor, positions: int = ROPE_POSITIONS):
     return ang.cos(), ang.sin()
 
 
-def pack_parameters(state_dict: dict, hparams: dict, rope_positions: int = ROPE_POSITIONS) -> dict:
+def pack_parameters(state_dict: dict, hparams: dict, rope_positions: int = ROPE_POSITIONS, dtype=np.float32) -> dict:
     """rope_positions: rows of the RoPE tables, the longest chunk the loaded model will run (bt_max_chunk).  Rows
-    below 1500 do not depend on it."""
+    below 1500 do not depend on it.  dtype: of the arrays; the library takes float32, and float64 keeps the folds
+    exact for float64 references of the packed layout (the RoPE tables stay the fp32 values either way)."""
     sd = strip_prefixes(state_dict)
     hp = filter_hparams(hparams)
     out: dict = {}
@@ -141,7 +142,7 @@ def pack_parameters(state_dict: dict, hparams: dict, rope_positions: int = ROPE_
     out["head.w"] = _f64(sd["task_heads.beat_downbeat_lin.weight"]) * g[None, :]
     out["head.b"] = _f64(sd["task_heads.beat_downbeat_lin.bias"])
     return {
-        k: np.ascontiguousarray((v.numpy() if isinstance(v, torch.Tensor) else np.asarray(v)).astype(np.float32).reshape(-1))
+        k: np.ascontiguousarray((v.numpy() if isinstance(v, torch.Tensor) else np.asarray(v)).astype(dtype).reshape(-1))
         for k, v in out.items()
     }
 
