@@ -5,10 +5,10 @@ tests/test_gpu_attention.py (runs the cases) and tests/test_cpu_attention_refere
 the bounds to a CPU emulation of the kernels, and the cases to the instantiations in the library).
 
 Operands, as the hooks pack them (round16: the activation type; the fp32 context does not round):
-  time, tensor cores : q^ = round16(fp32(q * QSCALE_F32)), QSCALE_F32 = fp32(s * log2 e), s = fp32(1 / sqrt(32));
+  time, tensor cores : q^ = round16(fp32(q * QSCALE_H16)), QSCALE_H16 = fp32(s * log2 e), s = fp32(1 / sqrt(32));
                        k^ = round16(k), v^ = round16(v); scores in base-2 units: t_ij = q^_i . k^_j
   time, SIMT         : qs = fp32(q * s); t_ij = log2 e * (qs_i . k_j)      (the kernel takes expf of qs . k)
-  frequency, TC      : q^, k^, v^ = round16(q, k, v); t = SL2 * (q^ . k^), SL2 = fp32(s * log2 e) = QSCALE_F32
+  frequency, TC      : q^, k^, v^ = round16(q, k, v); t = SL2 * (q^ . k^), SL2 = fp32(s * log2 e) = QSCALE_H16
   frequency, SIMT    : as the SIMT time path (__expf)
 Restatement, per (sequence or group, head, query row i), over the keys j a row may see (the first len of its chunk in
 time; the F planes of its (chunk, frame, head) in frequency):
@@ -19,7 +19,7 @@ time; the F planes of its (chunk, frame, head) in frequency):
   o_i = g_i sum_j Wn_j v^_j / sum_j W_j     (the denominator l sums the UNROUNDED p); 16-bit paths store round16(o)
 
 Bound per output element, first order in each term, in float64 from the data (all exponents base 2):
-  scores     e_j = mma_error(32, sum_d |q^_d k^_jd|) on tensor cores (fused_reference.mma_error: products of 16-bit
+  scores     e_j = mma_error(32, sum_d |q^_d k^_jd|) on tensor cores (numerics.mma_error: products of 16-bit
              operands are exact in fp32, each of the K + K/16 additions of an m16n8k16 chain loses <= 2^-23 of the
              sum of magnitudes); SIMT: a 32-term fmaf chain, 32 2^-24 sum_d |qs_d k_jd| (times log2 e).  SL2 e_j on
              the frequency tensor-core path.  The row maximum of step k is off by at most Ek_j = max e over the keys of
@@ -54,18 +54,11 @@ With A_j, B_j the absolute errors of the numerator and denominator weights (rela
 import math
 from dataclasses import dataclass
 
-import numpy as np
 import torch
 
-from fused_reference import mma_error, rnd, rounding_error
+from numerics import EX2_APPROX_REL, EXPF_REL, LOG2E, QSCALE_H16, S_F32, U, mma_error, rnd, rounding_error
 
-U = 2.0**-24
-LOG2E = 1.4426950408889634
-S_F32 = float(np.float32(0.17677669529663687))  # the kernels' fp32 1 / sqrt(32)
-QSCALE_F32 = float(np.float32(np.float32(S_F32) * np.float32(LOG2E)))  # tensor-core q scale = the frequency SL2
-EX2_APPROX_REL = 2.0**-22
 EX2_POLY_REL = 8e-5
-EXPF_REL = 2.0**-22
 TINY = 2.0**-119
 AT_TILE = 64  # keys per step of attn_time_kernel (AT_BKV)
 AT_POLY_MASK = 0x52  # score pairs nb of a tile (keys 8 nb .. 8 nb + 7) that take ex2_poly (kernels_attn.cu)
@@ -160,7 +153,7 @@ def time_ref(q, k, v, gates, lens, path, dt, exact=False):
     if exact:
         qh, kh, vh, sc = hv(q), hv(k), hv(v), LOG2E / math.sqrt(32)
     elif path == "tc":
-        qh, kh, vh, sc = hv(rnd(_f32mul(q, QSCALE_F32), dt)), hv(rnd(k, dt)), hv(rnd(v, dt)), 1.0
+        qh, kh, vh, sc = hv(rnd(_f32mul(q, QSCALE_H16), dt)), hv(rnd(k, dt)), hv(rnd(v, dt)), 1.0
     else:
         qh, kh, vh, sc = hv(_f32mul(q, S_F32)), hv(k), hv(v), LOG2E
     g = gates.reshape(seqs, L, H).permute(0, 2, 1).reshape(seqs * H, L)
@@ -203,7 +196,7 @@ def freq_ref(q, k, v, gates, B, F, path, dt, exact=False):
     if exact:
         qh, kh, vh, sc = grp(q), grp(k), grp(v), LOG2E / math.sqrt(32)
     elif path == "tc":
-        qh, kh, vh, sc = grp(rnd(q, dt)), grp(rnd(k, dt)), grp(rnd(v, dt)), QSCALE_F32
+        qh, kh, vh, sc = grp(rnd(q, dt)), grp(rnd(k, dt)), grp(rnd(v, dt)), QSCALE_H16
     else:
         qh, kh, vh, sc = grp(_f32mul(q, S_F32)), grp(k), grp(v), LOG2E
     g = grp(gates)[..., 0]
@@ -219,7 +212,7 @@ def freq_ref(q, k, v, gates, B, F, path, dt, exact=False):
         if path == "tc":
             NT = 4 if F == 32 else 2
             ones = torch.ones(G, dtype=torch.float64, device=q.device)
-            res = softmax_ref(T2, QSCALE_F32 * mma_error(32, S), valid, vh, g, step=F, alpha_rel=0.0,
+            res = softmax_ref(T2, QSCALE_H16 * mma_error(32, S), valid, vh, g, step=F, alpha_rel=0.0,
                                      sub_ops=2, p_dt=dt, n_sum=(2 * NT + 2) * ones,
                                      pv_error=lambda s, nnz: mma_error(nnz, s), out_dt=dt, n_pad=0,
                                      exp_rel=lambda x, e: torch.full_like(x, EXPF_REL))
@@ -312,7 +305,7 @@ def _unit(*shape, g, device):
 
 
 def _dominant_q(k, kappa, exclude, g):
-    """q [.., R, 32] (fp32) whose score QSCALE_F32 q_i . k_kappa(i) beats every rival key of its row by >= 32 base-2
+    """q [.., R, 32] (fp32) whose score QSCALE_H16 q_i . k_kappa(i) beats every rival key of its row by >= 32 base-2
     units: q_i = c_i k_kappa(i).  k [.., K, 32] unit rows; kappa [.., R]; exclude [.., R, K]: keys that are no
     rivals (kappa itself, keys the row does not see)."""
     kk = torch.gather(k, -2, kappa[..., None].expand(*kappa.shape, 32))  # [.., R, 32]
@@ -320,7 +313,7 @@ def _dominant_q(k, kappa, exclude, g):
     rival = cos.masked_fill(exclude, -1.0)
     gap = 1 - rival.amax(-1)
     assert gap.min().item() > 0.05, f"dominant-key family: gap {gap.min().item():.3f}"
-    c = 32 / (QSCALE_F32 * gap)
+    c = 32 / (QSCALE_H16 * gap)
     return kk * c[..., None]
 
 
@@ -363,7 +356,7 @@ def time_inputs(case, family, g, device):
     else:
         # one direction u carries the score: q_i = c u + noise, k_j = beta_j u + noise; beta ~ 1 in the last (late_max)
         # or first (early_max) tile of each chunk, <= 0.85 elsewhere (>= 20 base-2 units lower), down to 0 (< -120)
-        c = 200 / QSCALE_F32
+        c = 200 / QSCALE_H16
         ntile = (lens + AT_TILE - 1) // AT_TILE
         tile = j[None, :] // AT_TILE
         top = tile == (ntile[:, None] - 1) if family == "late_max" else tile == 0
@@ -404,7 +397,7 @@ def freq_inputs(case, family, g, device):
     rival = (target @ k.transpose(-1, -2)).masked_fill(exclude, -1.0)
     gap = 1 - rival.amax(-1)
     assert gap.min().item() > 0.05, f"{family} family: gap {gap.min().item():.3f}"
-    q = target * (32 / (QSCALE_F32 * gap))[..., None]
+    q = target * (32 / (QSCALE_H16 * gap))[..., None]
     to_tok = lambda t: t.permute(0, 3, 1, 2, 4).reshape(M, C)  # [B, L, H, F, 32] -> token-major
     return to_tok(q).contiguous(), to_tok(k).contiguous(), v, gates
 

@@ -7,7 +7,8 @@ import math
 
 import numpy as np
 
-U32 = 2.0 ** -24  # unit round-off of fp32
+from numerics import U
+
 ATAN2F_ERR = 2.0 ** -21  # 2 ulp of a value <= pi (CUDA math API: atan2f max error 2 ulp)
 
 
@@ -110,7 +111,7 @@ def fft_delta(n_fft: int, l2_norm):
     """Per-output error of an n_fft-point fp32 transform of data with that l2 norm per unit of output scale: the
     derivation of logmel_reference.device_bound (Higham thm. 24.2 per radix-2 stage, two stages for the untangling and
     window, the rms share of the norm-wise bound times a safety factor 8)."""
-    return 8 * (math.log2(n_fft) + 2) * 8 * U32 * math.sqrt(2.0) * np.asarray(l2_norm)
+    return 8 * (math.log2(n_fft) + 2) * 8 * U * math.sqrt(2.0) * np.asarray(l2_norm)
 
 
 def stft_bound(x, n_fft: int, hop: int) -> np.ndarray:
@@ -136,7 +137,7 @@ def vocoder_bound(X, rate: float) -> np.ndarray:
     i1 = next_index(s)
     mag = alpha * Xp[i1] + (1 - alpha) * Xp[i]
     phase_err = (2 * np.arange(n)[:, None] + 2) * ATAN2F_ERR
-    return mag * phase_err + 8 * U32 * (Xp[i] + Xp[i1]) + 1e-30
+    return mag * phase_err + 8 * U * (Xp[i] + Xp[i1]) + 1e-30
 
 
 def istft_bound(Y, n_fft: int, hop: int, length: int) -> np.ndarray:
@@ -160,4 +161,4 @@ def istft_bound(Y, n_fft: int, hop: int, length: int) -> np.ndarray:
     sl = slice(n_fft // 2, n_fft // 2 + length)
     c = math.ceil(n_fft / hop)
     envs = np.where(env[sl] > 0, env[sl], 1.0)
-    return (err[sl] + (2 * c + 6) * U32 * mod[sl]) / envs + 1e-30
+    return (err[sl] + (2 * c + 6) * U * mod[sl]) / envs + 1e-30

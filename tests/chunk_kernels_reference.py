@@ -45,20 +45,12 @@ import math
 import numpy as np
 import torch
 
-from attention_reference import EX2_APPROX_REL
+from numerics import EX2_APPROX_REL, GELU_SLOPE, LOG2E, RCP_APPROX_REL, U, f32, fma_f32, gelu_erf
 
-U = 2.0**-24
-RCP_APPROX_REL = 2.0**-23
 AS_ERF = 1.5e-7
-GELU_SLOPE = 1.13
 AS_P = 0.3275911
 AS_A = (0.254829592, -0.284496736, 1.421413741, -1.453152027, 1.061405429)  # a1 .. a5 of A&S 7.1.26
-LOG2E = 1.4426950408889634
 FIELDS = ("frame_base", "T", "start", "out_base", "write_lo", "write_hi", "len")
-
-
-def f32(v):
-    return float(np.float32(v))
 
 
 def erf_error_bound(n=200001, z_max=10.0):
@@ -83,10 +75,6 @@ def erf_error_bound(n=200001, z_max=10.0):
 
 
 E_ERF = erf_error_bound()
-
-
-def gelu_erf(a):
-    return 0.5 * a * (1.0 + torch.erf(a / math.sqrt(2.0)))
 
 
 # ------------------------------------------------------------------------------------------ restatements and bounds
@@ -176,13 +164,6 @@ def sweep_lengths(chunk_size, border):
 
 
 # ------------------------------------------------------------------------------------------ fp32 emulations (numpy)
-def _fma(a, b, c):
-    """fmaf on float32 arrays: the product of two fp32 values is exact in float64, then one rounding to fp32 (a double
-    rounding through float64 can differ from fmaf by 2^-53 relative, well inside every bound here)."""
-    return (np.float64(a) * np.float64(b) + np.float64(c)).astype(np.float32) if np.isscalar(a) else \
-        (a.astype(np.float64) * np.asarray(b, np.float64) + np.asarray(c, np.float64)).astype(np.float32)
-
-
 def _approx(exact, rel, sign):
     """An fp32 result within `rel` (relative) of the float64 `exact`, off by about `rel` in direction `sign`."""
     y = exact * (1.0 + sign * rel)
@@ -197,18 +178,18 @@ def gelu_fast_np(x, sign=1.0, p_const=AS_P):
     Returns (gelu, erf_abs)."""
     x = np.asarray(x, np.float32)
     z = (np.abs(x) * np.float32(0.70710678118654752440)).astype(np.float32)
-    d = _fma(np.float32(p_const), z, np.float32(1.0))
+    d = fma_f32(np.float32(p_const), z, np.float32(1.0))
     t = _approx(1.0 / d.astype(np.float64), RCP_APPROX_REL, sign)
-    p = _fma(np.float32(AS_A[4]), t, np.float32(AS_A[3]))
+    p = fma_f32(np.float32(AS_A[4]), t, np.float32(AS_A[3]))
     for c in AS_A[2::-1]:
-        p = _fma(p, t, np.float32(c))
+        p = fma_f32(p, t, np.float32(c))
     p = (p * t).astype(np.float32)
     arg = ((z * z).astype(np.float32) * np.float32(-LOG2E)).astype(np.float32)
     exact = np.exp2(arg.astype(np.float64))
     e = np.where(exact < 2.0**-126, np.float32(0), _approx(exact, EX2_APPROX_REL, sign)).astype(np.float32)
-    erf_abs = _fma(-p, e, np.float32(1.0))
+    erf_abs = fma_f32(-p, e, np.float32(1.0))
     half = (np.float32(0.5) * x).astype(np.float32)
-    return _fma((np.float32(0.5) * np.abs(x)).astype(np.float32), erf_abs, half), erf_abs
+    return fma_f32((np.float32(0.5) * np.abs(x)).astype(np.float32), erf_abs, half), erf_abs
 
 
 STEM_MISTAKES = ("conv_by_clip", "bn_on_chunk_pad", "clip_pad_after_bn", "gelu_const")
@@ -229,7 +210,7 @@ def stem_np(spect, chunks, L, bn1_scale, bn1_shift, w, bias, sign=1.0, mistake=N
             clip_ok = (fr >= 0) & (fr < T)
             conv_ok = (tl >= 0) & ((fr < T) if mistake == "conv_by_clip" else (tl < ln))
             v = np.where((conv_ok & clip_ok)[:, None], spect[fb + np.clip(fr, 0, T - 1)], np.float32(0)).astype(np.float32)
-            x = _fma(v, bn1_scale[None, :], bn1_shift[None, :])  # [L, 128]
+            x = fma_f32(v, bn1_scale[None, :], bn1_shift[None, :])  # [L, 128]
             if mistake == "clip_pad_after_bn":
                 x = np.where(clip_ok[:, None], x, np.float32(0))
             pad = np.broadcast_to(bn1_shift, x.shape) if mistake == "bn_on_chunk_pad" else np.float32(0)
@@ -239,7 +220,7 @@ def stem_np(spect, chunks, L, bn1_scale, bn1_shift, w, bias, sign=1.0, mistake=N
             a = np.broadcast_to(np.float32(bias[co]), (32, L)).astype(np.float32)
             for df in range(4):
                 for dt in range(3):
-                    a = _fma(ins[:, df, dt, :], w[co, df * 3 + dt], a)
+                    a = fma_f32(ins[:, df, dt, :], w[co, df * 3 + dt], a)
             out[b, :, :, co] = gelu_fast_np(a, sign, 0.3275 if mistake == "gelu_const" else AS_P)[0]
     return out
 
@@ -254,17 +235,17 @@ def head_np(x, w, bias, chunks, L, sum_head, out_count, mistake=None):
     a0, a1 = ss.copy(), ss.copy()
     for i in range(D // 32):  # lane chains over i = lane, lane + 32, ...
         v = xl[:, :, i, :]
-        ss = _fma(v, v, ss)
-        a0 = _fma(v, wl[0, i], a0)
-        a1 = _fma(v, wl[1, i], a1)
+        ss = fma_f32(v, v, ss)
+        a0 = fma_f32(v, wl[0, i], a0)
+        a1 = fma_f32(v, wl[1, i], a1)
     for o in (16, 8, 4, 2, 1):  # warp_sum: lane l adds lane l ^ o
         idx = np.arange(32) ^ o
         ss, a0, a1 = [(s + s[..., idx]).astype(np.float32) for s in (ss, a0, a1)]
     ss, a0, a1 = ss[..., 0], a0[..., 0], a1[..., 0]
     nrm = ss if mistake == "ss_no_sqrt" else np.sqrt(ss).astype(np.float32)
     inv = (np.float32(1.0) / np.maximum(nrm, np.float32(1e-12))).astype(np.float32)
-    o0 = _fma(a0, inv, np.float32(bias[0]))
-    o1 = _fma(a1, inv, np.float32(bias[1]))
+    o0 = fma_f32(a0, inv, np.float32(bias[0]))
+    o1 = fma_f32(a1, inv, np.float32(bias[1]))
     beat_v = (o0 + o1).astype(np.float32) if (sum_head or mistake == "ignore_sum_head") else o0
     beat = np.full(out_count, np.nan, np.float32)
     down = beat.copy()

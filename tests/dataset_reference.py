@@ -9,6 +9,8 @@ both split files.  The same seed writes the same bytes.
 """
 from __future__ import annotations
 
+import contextlib
+import io
 import json
 from pathlib import Path
 
@@ -145,3 +147,25 @@ def apply_mask_reference(spect, mask, fps, rng):
         else:
             ex[:] = 0
     return spect
+
+
+# ---- the fixture's draws: the seed, the items and the datasets the dataset tests build
+SEED = 4000  # oracle/make_golden_train_batches.py
+
+
+def _items():
+    return sorted(f"{d}/{p[0]}" for d, (_, _, ps) in DATASETS.items() if d != "gtzan" for p in ps)
+
+
+def _tests():
+    return sorted(f"gtzan/{p[0]}" for p in DATASETS["gtzan"][2])
+
+
+def _dataset(tree, cfg):
+    from beat_this_b200.dataset import BeatTrackingDataset
+
+    kw = {"train_length": TRAIN_LENGTH, **CONFIGS[cfg][0]}
+    log = io.StringIO()
+    with contextlib.redirect_stdout(log):
+        ds = BeatTrackingDataset(_tests() if cfg == "full" else _items(), tree, spect_fps=FPS, **kw)
+    return ds, log.getvalue()

@@ -36,13 +36,11 @@ from __future__ import annotations
 import math
 from dataclasses import dataclass, field
 
-import numpy as np
 import torch
 
 from gemm_reference import QSCALE_TIME, conv_shape, lin_shape, plain_shape
+from numerics import normalize
 
-# the q scale bt_debug_attention applies in the 16-bit context (api_debug.cu: inv_sqrt_d * log2 e in fp32)
-HOOK_QSCALE_H16 = float(np.float32(np.float32(0.17677669529663687) * np.float32(1.4426950408889634)))
 FUSED_WIDTHS = (32, 64)
 HOOK_ROPE_ROWS = 1500  # bt_debug_fused_qkv takes L <= BT_CHUNK: longer planes run as pieces of at most this many rows
 
@@ -224,10 +222,6 @@ def production_taps(hp: dict, half: bool) -> list:
 # position modes, q scales, key lengths, zero_tail -- to the reference model independently of the library, and the GPU
 # test ties the forward pass to the chains bit for bit.  Rounding points (round16, the 16-bit operands) are identities
 # here.
-def _norm64(x):
-    return x / x.norm(dim=-1, keepdim=True).clamp_min(1e-12)
-
-
 def _attend(q, k, v, mask=None):
     """softmax(q k^T / sqrt(32)) v over the last two dims of [..., n, 32] (mask [.., n]: keys kept)."""
     s = q @ k.transpose(-1, -2) / math.sqrt(32)
@@ -275,7 +269,7 @@ class Eval64:
         self.regs["x"] = ref.reshape(-1, 32)
 
     def _norm(self, C, heads, wg, bg):
-        xn = _norm64(self.regs["x"])
+        xn = normalize(self.regs["x"])
         self.regs["xn"] = xn
         if heads:
             self.regs["gates"] = torch.sigmoid(xn @ self.P[wg].view(32, C)[:heads].T + self.P[bg][:heads])
@@ -327,7 +321,7 @@ class Eval64:
         x = self.regs["x"]
         if wout:
             x = x + self.regs["o"] @ self.P[wout].view(C, C).T
-        h = torch.nn.functional.gelu(_norm64(x) @ self.P[w1].view(4 * C, C).T + self.P[b1])
+        h = torch.nn.functional.gelu(normalize(x) @ self.P[w1].view(4 * C, C).T + self.P[b1])
         x = x + h @ self.P[w2].view(C, 4 * C).T + self.P[b2]
         self.regs["x"] = x
         if xb:

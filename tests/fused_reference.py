@@ -11,17 +11,13 @@ round16 is the activation type (rnd(t, None): no rounding, the reference block i
   ff   : x' = x (+ round16(O) round16(Wo)^T), u16 = round16(normalize(x')), h16 = round16(gelu_tanh(u16 W1^T + b1)),
          y = x' + b2 + h16 round16(W2)^T; the 16-bit copy is round16(y)
 
-Bounds, elementwise and in float64 from the data.  The kernels compute in fp32, so the value a kernel rounds to 16
-bits differs from its float64 value v by up to some d, and the rounded value can land on the other neighbour of
-round16(v).  Rounding is monotonic, so the kernel's rounded value lies in [round16(v - d), round16(v + d)]:
-  rounding_error(v, d) = max |round16(v +- d) - round16(v)|
-is 0 where v is farther than d from a rounding midpoint, one ulp near one (d below half an ulp), and stays sound for
-any d.  Each rounded intermediate carries that error to first order into the products after it.
+Bounds, elementwise and in float64 from the data, with the error model of tests/numerics.py.  A value the kernel
+rounds to 16 bits is off by rounding_error(v, d) of round16(v) when its fp32 value is within d of v; each rounded
+intermediate carries that error to first order into the products after it.
 ACC = GEMM_ACC_TOL_H16 x (1 + |value|) is the stated fp32 accumulation error of one tensor-core product
-(test_gpu_kernels.py).  The fused FFN, whose output is fp32 and whose products are short, uses the derived form
-mma_error(K, s) = 2 K 2^-23 s, s = |c| + sum_k |a_k b_k|: the products of 16-bit operands are exact in fp32, and each
-of the K + K/16 additions of an m16n8k16 chain (aligned to its largest term, rounded or truncated) loses at most
-2^-23 of s.  An fp32 addition outside the MMA adds 2^-24 of its result.
+(numerics.py).  The fused FFN, whose output is fp32 and whose products are short, uses the derived form
+mma_error(K, s) = 2 K 2^-23 s, s = |c| + sum_k |a_k b_k| (numerics.mma_error).  An fp32 addition outside the MMA adds
+2^-24 of its result (F32_ADD).
   u    : d_u = norm_rel(C) |u| (the fp32 normalisation, see norm); with the out-projection in front, x' is off by
          e_x and d_u = norm_rel(C) |u| + (e_x + |u| ||e_x||) / ||x'|| (first order);  e_u = rounding_error(u, d_u)
   ff   : e_x = mma_error(C, |x| + |O16| |Wo16|^T)                              (out-projection, x' = x + O16 Wo16^T)
@@ -43,28 +39,11 @@ import math
 
 import torch
 
-from gemm_reference import gelu_erf, gelu_tanh, rope_ref  # noqa: F401  (gelu_erf: the reference block's GELU)
-from test_gpu_kernels import GATES_TOL, GEMM_ACC_TOL_H16, TANH_APPROX_TOL, _ulp
+from numerics import (F32_ADD, GATES_TOL, GELU_SLOPE, GEMM_ACC_TOL_H16, TANH_APPROX_TOL, U, gelu_tanh, mma_error,
+                      normalize, rnd, rope_positions, rope_ref, rounding_error, ulp16)
 
 ACC = GEMM_ACC_TOL_H16
-GELU_SLOPE = 1.13  # max |d gelu_tanh / dx| = 1.1290 (at x ~ 2.4)
 NORM_CS = (32, 64, 128, 256, 512, 1024)  # the BT_NORM_CASE widths of norm_kernel
-
-
-def rnd(t, dt):
-    """t rounded to the 16-bit type dt, back in float64; dt None: t unchanged."""
-    return t if dt is None else t.to(dt).double()
-
-
-def rounding_error(v, d, dt):
-    """max |round16(v +- d) - round16(v)|: how far the 16-bit rounding of a value within d of float64 v can land from
-    round16(v) (round to nearest is monotonic)."""
-    r = rnd(v, dt)
-    return torch.maximum((rnd(v + d, dt) - r).abs(), (rnd(v - d, dt) - r).abs())
-
-
-def normalize(x):
-    return x / x.norm(dim=-1, keepdim=True).clamp_min(1e-12)
 
 
 def norm_error(x, e_x=None):
@@ -77,28 +56,15 @@ def norm_error(x, e_x=None):
     return d
 
 
-F32_ADD = 2.0**-24
-
-
-def mma_error(K, s):
-    """Error bound of an fp32 mma.sync accumulation of K products of 16-bit operands onto c: s = |c| + sum |a_k b_k|."""
-    return 2 * K * 2.0**-23 * s
-
-
 def norm_rel(C):
-    return (C / 2 + 3) * 2.0**-24
-
-
-def rope_positions(M, L, F, posmode, device=None):
-    m = torch.arange(M, device=device)
-    return m % L if posmode == 0 else (m // L) % F
+    return (C / 2 + 3) * U
 
 
 def gates_ref(u, wg, bg, heads):
     """(gates [M, heads], bound) from the unrounded float64 u."""
     C = u.shape[1]
     g = torch.sigmoid(u @ wg[:heads].T + bg[:heads])
-    bound = GATES_TOL + 0.25 * (C + 4) * 2.0**-24 * (u.abs() @ wg[:heads].abs().T)
+    bound = GATES_TOL + 0.25 * (C + 4) * U * (u.abs() @ wg[:heads].abs().T)
     return g, bound
 
 
@@ -109,7 +75,7 @@ def norm_ref(x, dt):
     if dt is None:
         return u, bound
     u16 = rnd(u, dt)
-    return u16, bound + _ulp(u16, dt)
+    return u16, bound + ulp16(u16, dt)
 
 
 def qkv_ref(x, wqkv, wg, bg, cos, sin, L, F, posmode, qscale, dt):
@@ -133,7 +99,7 @@ def qkv_ref(x, wqkv, wg, bg, cos, sin, L, F, posmode, qscale, dt):
     e[:, :C] = math.sqrt(2) * pair[:, :C] * abs(qscale)
     e[:, C : 2 * C] = math.sqrt(2) * pair[:, C:]
     out16 = rnd(out, dt)
-    return out16, e + _ulp(out16, dt), g, gb
+    return out16, e + ulp16(out16, dt), g, gb
 
 
 def ff_ref(x, w1, b1, w2, b2, o=None, wout=None, dt=None, gelu=gelu_tanh):

@@ -1,11 +1,20 @@
 """Cases and float64 references for the unit tests of the 16-bit GEMM (gemm_tc_kernel<BN, BK, KIND>) and the fp32
-GEMM (gemm_simt_kernel) through bt_debug_gemm.  Shared by tests/test_gpu_kernels.py (runs the cases) and
-tests/test_cpu_gemm_sass.py (ties GEMM_TILES to the instantiations in the built library)."""
+GEMM (gemm_simt_kernel) through bt_debug_gemm, and the check of one case on the device.  Shared by
+tests/test_gpu_kernels.py and tests/test_gpu_gemm_epilogue.py (run the cases) and tests/test_cpu_gemm_sass.py (ties
+GEMM_TILES to the instantiations in the built library)."""
 import math
+import re
+import zlib
 from dataclasses import dataclass, field
 
 import torch
 
+from numerics import (GATES_TOL, GEMM_ACC_TOL_F32, GEMM_ACC_TOL_H16, TANH_APPROX_TOL, gelu_erf, gelu_tanh, rnd,
+                      rope_positions, rope_ref, ulp16)
+from support import act_dtype, bits
+
+# gemm_tc_kernel<BN, BK, KIND> in the SASS; KIND 2 (the N = 32 attention gates) keeps the IEEE-division sigmoid
+GEMM_TC_KERNEL = re.compile(r"_ZN2bt14gemm_tc_kernelILi(\d+)ELi(\d+)E(?:Li(\d+)E)?E")
 # every (BN, BK, KIND) instantiation of gemm_tc_kernel in the library; the GPU matrix runs each at least once
 GEMM_TILES = sorted(
     [(bn, 64, k) for k in (0, 1) for bn in (256, 192, 128, 64, 32)]
@@ -174,31 +183,13 @@ def gemm_ref(shape, a, w):
     return (x @ wref.T).reshape(nb * L, N)
 
 
-def gelu_erf(x):
-    return 0.5 * x * (1.0 + torch.erf(x / math.sqrt(2.0)))
-
-
-def gelu_tanh(x):
-    return 0.5 * x * (1.0 + torch.tanh(math.sqrt(2.0 / math.pi) * (x + 0.044715 * x**3)))
-
-
-def rope_ref(x, cos, sin):
-    """Interleaved-pair rotation (oracle.rope / rotary_embedding_torch) of x [M, heads * 32] by per-row tables
-    cos, sin [M, 16]: out[2i] = x[2i] cos_i - x[2i+1] sin_i, out[2i+1] = x[2i+1] cos_i + x[2i] sin_i."""
-    M = x.shape[0]
-    p = x.reshape(M, -1, 16, 2)
-    c, s = cos[:, None, :], sin[:, None, :]
-    return torch.stack((p[..., 0] * c - p[..., 1] * s, p[..., 1] * c + p[..., 0] * s), dim=-1).reshape(x.shape)
-
-
 def epilogue_ref(case, acc, bias, resid, half, rope_cos=None, rope_sin=None):
     """(out [M, ldo], pre-GELU value or None) in float64 for the case's epilogue on acc [M, N]."""
     if case.kind == 2:
         return torch.sigmoid(acc[:, : case.heads] + bias[: case.heads]), None
     if case.kind == 1:
         L, C = case.shape["L"], case.C
-        m = torch.arange(acc.shape[0], device=acc.device)
-        pos = m % L if case.posmode == 0 else (m // L) % case.F
+        pos = rope_positions(acc.shape[0], L, case.F, case.posmode, acc.device)
         out = acc.clone()
         out[:, :C] = rope_ref(acc[:, :C], rope_cos[pos], rope_sin[pos]) * case.qscale
         out[:, C : 2 * C] = rope_ref(acc[:, C : 2 * C], rope_cos[pos], rope_sin[pos])
@@ -211,3 +202,76 @@ def epilogue_ref(case, acc, bias, resid, half, rope_cos=None, rope_sin=None):
     if case.resid:
         y = y + resid
     return y, pre
+
+
+# ---- one case on the device: bt_debug_gemm against the float64 references above, at the tolerances of numerics.py
+def _run_gemm(eng, case, a, w, bias, resid, rope):
+    """One bt_debug_gemm call on fresh output buffers of M + 1 rows: the last row is a NaN sentinel, and every other
+    element starts as NaN too (or as the residual where out_f32 doubles as it), so a missing store shows up."""
+    M, N = case.M, case.shape["N"]
+    ldo = case.heads if case.kind == 2 else N
+    nan = float("nan")
+    o32 = torch.full(((M + 1) * ldo,), nan, device=a.device) if case.out_f32 else None
+    if case.resid:
+        o32[: M * N] = resid.flatten()
+    oa = torch.full(((M + 1) * N,), nan, device=a.device) if case.out_act else None
+    tile = eng.debug_gemm_full(case.shape, a, w, bias=bias if (case.bias or case.kind == 2) else None,
+                               resid=o32 if case.resid else None, out_f32=o32, out_act=oa, rope_cos=rope[0],
+                               rope_sin=rope[1], resid_epilogue=case.resid_epilogue, kind=case.kind, gelu=case.gelu,
+                               C=case.C, heads=case.heads, posmode=case.posmode, F=case.F, qscale=case.qscale)
+    return tile, o32, oa
+
+
+def _check_gemm_case(eng, half, case):
+    from beat_this_b200.weights import rope_tables
+
+    dev = eng.device
+    sh, M, N = case.shape, case.M, case.shape["N"]
+    Ktot = sh["Kslab"] * sh["nslab"]
+    g = torch.Generator(device=dev).manual_seed(zlib.crc32(case.id.encode()))
+    a = torch.randn(sh["planes_in"] * sh["L"], sh["lda"], generator=g, device=dev)
+    w = torch.randn(N, Ktot, generator=g, device=dev) / math.sqrt(Ktot)
+    bias = torch.randn(N, generator=g, device=dev) * 0.5
+    resid = torch.randn(M, N, generator=g, device=dev) if case.resid else None
+    freqs = 1.0 / (10000 ** (torch.arange(0, 32, 2).float() / 32))
+    rope = tuple(t.contiguous().to(dev) for t in rope_tables(freqs)) if case.kind == 1 else (None, None)
+
+    tile, o32, oa = _run_gemm(eng, case, a, w, bias, resid, rope)
+    if half:
+        assert tile == case.tile, f"plan tile {tile}, policy {case.tile}"
+        again = _run_gemm(eng, case, a, w, bias, resid, rope)  # the same launch twice: bitwise equal
+        for x, y in zip((o32, oa), again[1:]):
+            assert x is None or torch.equal(bits(x), bits(y)), "16-bit GEMM is not deterministic"
+    else:
+        assert tile == (0, 0)
+
+    adt = act_dtype(eng)
+    dt = adt if half else None
+    acc = gemm_ref(sh, rnd(a.double(), dt), rnd(w.double(), dt))
+    ref, pre = epilogue_ref(case, acc, bias.double(), resid.double() if resid is not None else None, half,
+                            *(t.double() if t is not None else None for t in rope))
+    tol = (GEMM_ACC_TOL_H16 if half else GEMM_ACC_TOL_F32) * (1 + ref.abs())
+    if case.kind == 2:
+        tol = torch.full_like(ref, GATES_TOL)
+    if pre is not None and half:
+        tol = tol + 0.5 * pre.abs() * TANH_APPROX_TOL
+    ldo = ref.shape[1]
+    line = f"gemm {'h16' if half else 'f32'} {case.id}: tile {tile[0]}x{tile[1]} kind {case.kind} M={M} N={N} K={Ktot}"
+
+    def check(name, got, ref, bound):
+        err = (got - ref).abs().nan_to_num(float("inf"))  # an unwritten (NaN) element fails
+        worst, ratio = err.max().item(), (err / bound).max().item()
+        print(f"{line} | {name} max abs err {worst:.3e} = {ratio:.2f} of its bound")
+        assert ratio <= 1, f"{name} off by up to {worst:.3e}, {ratio:.2f} x its bound"
+
+    if o32 is not None:
+        assert torch.isnan(o32[M * ldo :]).all(), "fp32 store past the last row"
+        check("f32 out", o32[: M * ldo].view(M, ldo).double(), ref, tol)
+    if oa is not None:
+        assert torch.isnan(oa[M * N :]).all(), "activation store past the last row"
+        got = oa[: M * N].view(M, N).double()
+        if half:
+            ref16 = ref.to(adt).double()
+            check(f"{eng.act_dtype} out", got, ref16, ulp16(ref16, adt) + tol)
+        else:
+            check("act out (fp32)", got, ref, tol)

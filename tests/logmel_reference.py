@@ -13,7 +13,7 @@ import math
 import numpy as np
 import torch
 
-U32 = 2.0 ** -24  # unit round-off of fp32
+from numerics import U
 
 
 def pcm_signal(seed: int, n: int) -> np.ndarray:
@@ -75,13 +75,13 @@ def device_bound(x, fb, n_fft: int, hop_length: int, normalized, power: float, l
     """
     mag, xw_norm = spectrum(x, n_fft, hop_length, normalized)
     fb = np.asarray(fb, np.float64)
-    delta = 8 * (math.log2(n_fft) + 2) * 8 * U32 * math.sqrt(2.0) * xw_norm[:, None]
-    s_lo = np.clip(mag - delta, 0.0, None) ** power * (1 - 4 * U32)
-    s_hi = (mag + delta) ** power * (1 + 4 * U32)
+    delta = 8 * (math.log2(n_fft) + 2) * 8 * U * math.sqrt(2.0) * xw_norm[:, None]
+    s_lo = np.clip(mag - delta, 0.0, None) ** power * (1 - 4 * U)
+    s_hi = (mag + delta) ** power * (1 + 4 * U)
     terms = (fb != 0).sum(0)[None, :]
     mel_lo, mel_hi = s_lo @ fb, s_hi @ fb
-    mel_lo = np.clip(mel_lo * (1 - (terms + 2) * U32), 0.0, None)
-    mel_hi = mel_hi * (1 + (terms + 2) * U32)
+    mel_lo = np.clip(mel_lo * (1 - (terms + 2) * U), 0.0, None)
+    mel_hi = mel_hi * (1 + (terms + 2) * U)
     lo = np.log1p(log_multiplier * mel_lo)
     hi = np.log1p(log_multiplier * mel_hi)
-    return lo - 4 * U32 * np.abs(lo) - 1e-7, hi + 4 * U32 * np.abs(hi) + 1e-7
+    return lo - 4 * U * np.abs(lo) - 1e-7, hi + 4 * U * np.abs(hi) + 1e-7

@@ -1,6 +1,11 @@
 """Float64 numpy restatement of the loss contract of include/beatthis.h (bt_beat_loss, bt_beat_loss_backward): what the
-kernels in csrc/kernels_loss.cu and the reference's beat_this/model/loss.py compute, written out frame by frame."""
+kernels in csrc/kernels_loss.cu and the reference's beat_this/model/loss.py compute, written out frame by frame; and
+the cases of the reference's outputs the CPU and GPU loss tests share."""
+import os
+
 import numpy as np
+
+from conftest import GOLDEN
 
 MASKED_BCE, SHIFT_TOLERANT, SPLIT_SHIFT_TOLERANT = 0, 1, 2
 FPS = 50
@@ -73,3 +78,25 @@ def framewise_truth(times, T, fps=FPS):
     out = np.zeros(T, np.float32)
     out[f] = 1
     return out
+
+
+# ---- the cases of the unmodified reference's outputs (tests/golden/loss.npz, oracle/make_golden_loss.py)
+GOLD = np.load(os.path.join(GOLDEN, "loss.npz"))
+CASES = range(int(GOLD["n"]))
+
+
+def fixture_case(k):
+    """(preds, targets, mask or None, row offsets, kind, tolerance, pos_weight, reference loss, reference grad), the
+    mask broadcast to the predictions' shape and every array flattened into rows of T frames."""
+    kind, t, pw, has_mask = GOLD[f"spec{k}"]
+    x = GOLD[f"preds{k}"]
+    m = np.broadcast_to(GOLD[f"mask{k}"], x.shape).astype(np.float32).ravel() if has_mask else None
+    T = x.shape[-1]
+    off = (np.arange(x.size // T + 1) * T).tolist()
+    return (x.ravel(), GOLD[f"targets{k}"].ravel(), m, off, int(kind), int(t), float(pw), float(GOLD[f"loss{k}"]),
+            GOLD[f"grad{k}"].ravel())
+
+
+# torch's fp32 gradient form cancels when p y is close to (p y + 1 - y) sigmoid(x) (soft targets, p = 4.5): the fixture
+# itself is then off by up to ~2e-6 of max |g| (1.7e-6 in case 61)
+GRAD_TOL = 2e-6

@@ -12,17 +12,17 @@ from __future__ import annotations
 
 import numpy as np
 
-U = 2.0 ** -24
+from numerics import U, f32
+
 TINY = float(np.finfo(np.float32).tiny)
 
 
 def scalars(lr, beta1, beta2, eps, weight_decay, step) -> dict:
     """The fp32 scalars of one entry, derived in double as torch's foreach path does in Python."""
-    f = lambda x: float(np.float32(x))  # noqa: E731
     bc1 = 1.0 - beta1 ** float(step)
     bc2 = 1.0 - beta2 ** float(step)
-    return dict(decay=f(1.0 - lr * weight_decay), decay_on=weight_decay != 0, w1=f(1.0 - beta1), beta2=f(beta2),
-                w2=f(1.0 - beta2), c2=f(bc2 ** 0.5), eps=f(eps), s=f(lr / bc1 * -1.0))
+    return dict(decay=f32(1.0 - lr * weight_decay), decay_on=weight_decay != 0, w1=f32(1.0 - beta1),
+                beta2=f32(beta2), w2=f32(1.0 - beta2), c2=f32(bc2 ** 0.5), eps=f32(eps), s=f32(lr / bc1 * -1.0))
 
 
 def adamw(p, g, m, v, **hp):

@@ -37,9 +37,9 @@ import numpy as np
 
 from beat_this_b200 import augment as A
 from beat_this_b200 import preprocessing as P
+from numerics import U
 from oracle import beat_this_oracle as O
 
-U = 2.0**-24
 E64 = 2.0**-36
 H_SLOPE = 4.0  # max |d/dt h(t)|, t in output-band zero crossings (test_cpu_resample_reference checks it)
 SR = P.SAMPLE_RATE

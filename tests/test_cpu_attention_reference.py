@@ -13,29 +13,13 @@ import pytest
 import torch
 
 import attention_reference as R
-from test_cpu_gemm_sass import _sass
+from numerics import EX2_APPROX_REL, EXPF_REL, QSCALE_H16, fma_f32, worst
+from support import sass
 
 H16 = torch.float16
 
 
 # ---- fp32 building blocks, as the kernels compute them
-def fma_f32(a, b, c):
-    """fmaf on float32 numpy arrays, correctly rounded: the float64 sum of the exact product and c, with the one case
-    where rounding twice differs from rounding once (a float64 result exactly between two floats) resolved by the
-    exact remainder of the float64 addition."""
-    p = a.astype(np.float64) * b.astype(np.float64)  # exact: 24 + 24 bits
-    c64 = c.astype(np.float64)
-    s = p + c64
-    bb = s - p
-    err = (p - (s - bb)) + (c64 - bb)  # s + err == p + c exactly
-    f = s.astype(np.float32)
-    r = f.astype(np.float64)
-    nb = np.nextafter(f, np.where(s > r, np.float32(np.inf), np.float32(-np.inf)))
-    tie = (s != r) & (s == (r + nb.astype(np.float64)) / 2) & (err != 0)
-    past = np.sign(err) == np.sign(s - r)  # the exact value lies beyond the midpoint: the far neighbour
-    return np.where(tie & past, nb, f).astype(np.float32)
-
-
 def ex2_poly_np(x, c0=0.99992895):
     """tc_common.cuh ex2_poly, bit for bit (float32 numpy in and out)."""
     x = np.maximum(x.astype(np.float32), np.float32(-120.0))
@@ -49,7 +33,7 @@ def ex2_poly_np(x, c0=0.99992895):
     return y.astype(np.uint32).view(np.int32).view(np.float32)
 
 
-def ex2_mufu(x, rel=R.EX2_APPROX_REL):
+def ex2_mufu(x, rel=EX2_APPROX_REL):
     """ex2.approx.ftz.f32 as the exact 2^x off by its stated relative error, with alternating sign; ftz below 2^-126."""
     xd = x.double()
     sign = 1 - 2 * (torch.arange(x.numel()).view(x.shape) % 2).double()
@@ -68,7 +52,7 @@ def emulate_time_tc(q, k, v, gates, lens, mistake=None):
     constant 0.9995), "gate_head" (the gate of head h + 1), "v_prev" (key 0 of a tile takes the previous tile's V)."""
     seqs, L, C = q.shape
     H = C // 32
-    qh = (q.float() * torch.tensor(R.QSCALE_F32, dtype=torch.float32)).to(H16).float()
+    qh = (q.float() * torch.tensor(QSCALE_H16, dtype=torch.float32)).to(H16).float()
     kh, vh = k.float().to(H16).float(), v.float().to(H16).float()
     poly = R.poly_keys(R.AT_TILE)
     c0 = 0.9995 if mistake == "poly_c0" else 0.99992895
@@ -126,22 +110,17 @@ def emulate_freq_tc(q, k, v, gates, B, F, cross_mask=True):
         V = torch.cat([V, pad(V)[:, partner]], 3)
     S = Q @ K.transpose(-1, -2)
     mx = S.amax(-1, keepdim=True)
-    x = ((S - mx) * torch.tensor(R.QSCALE_F32, dtype=torch.float32)).float()
-    p = ex2_mufu(x, R.EXPF_REL)
+    x = ((S - mx) * torch.tensor(QSCALE_H16, dtype=torch.float32)).float()
+    p = ex2_mufu(x, EXPF_REL)
     l = p.sum(-1)
     o = p.to(H16).float() @ V
     out = (o * (G / l)[..., None]).to(H16).double()
     return out.permute(0, 3, 1, 2, 4).reshape(M, C)
 
 
-def _ratio(got, ref, bound):
-    err = (got - ref).abs()
-    return torch.where(err == 0, 0.0, err / bound).max().item()
-
-
 def _report(got, ref, bound):
     """(ratio, max abs error): a ratio of inf is an error where the bound asks for the exact value."""
-    return _ratio(got, ref, bound), (got - ref).abs().max().item()
+    return worst(got, ref, bound), (got - ref).abs().max().item()
 
 
 # ---- the restatement is the reference operation
@@ -172,29 +151,29 @@ EMU_CASES = [R.TimeCase(2, 150, 2, (150, 97), 1), R.TimeCase(3, 129, 1), R.TimeC
 
 
 def test_time_bound_holds_the_emulation_and_catches_mistakes():
-    worst = {None: 0.0, **{m: {} for m in MISTAKES}}
+    peak = {None: 0.0, **{m: {} for m in MISTAKES}}
     for ci, case in enumerate(EMU_CASES):
         for fam in R.time_families(case):
             g = torch.Generator().manual_seed(100 + ci)
             q, k, v, gates = R.time_inputs(case, fam, g, "cpu")
             lens = torch.tensor(case.lens())
             ref, bound, _, _ = R.time_ref(q.double(), k.double(), v.double(), gates.double(), lens, "tc", H16)
-            good = _ratio(emulate_time_tc(q, k, v, gates, lens), ref, bound)
+            good = worst(emulate_time_tc(q, k, v, gates, lens), ref, bound)
             print(f"{case.id} {fam}: emulation at {good:.3f} of the bound")
             assert good <= 1, (case.id, fam, good)
-            worst[None] = max(worst[None], good)
+            peak[None] = max(peak[None], good)
             if fam in ("random", "dominant", "late_max", "flat_split"):
                 for m in MISTAKES:
                     r, e = _report(emulate_time_tc(q, k, v, gates, lens, m), ref, bound)
-                    w = worst[m].get(fam, (0.0, 0.0))
-                    worst[m][fam] = (max(w[0], r), max(w[1], e))
+                    w = peak[m].get(fam, (0.0, 0.0))
+                    peak[m][fam] = (max(w[0], r), max(w[1], e))
     for m in MISTAKES:
-        print(f"mistake {m}: " + ", ".join(f"{f} {r:.3g} x the bound (max error {e:.2e})" for f, (r, e) in worst[m].items()))
-        assert max(r for r, _ in worst[m].values()) > 1, m
+        print(f"mistake {m}: " + ", ".join(f"{f} {r:.3g} x the bound (max error {e:.2e})" for f, (r, e) in peak[m].items()))
+        assert max(r for r, _ in peak[m].values()) > 1, m
     for m in ("drop_last", "v_prev"):  # one misindexed key or value row: an O(1) error where it is the dominant key
-        assert worst[m]["dominant"][0] > 100, (m, worst[m])
+        assert peak[m]["dominant"][0] > 100, (m, peak[m])
     # ex2_poly's constant at 0.9995: a bias of 4.9e-4 on 3 of 8 weights, the output itself on the flat_split rows
-    assert worst["poly_c0"]["flat_split"][0] > 4 and worst["poly_c0"]["flat_split"][1] > 1e-4, worst["poly_c0"]
+    assert peak["poly_c0"]["flat_split"][0] > 4 and peak["poly_c0"]["flat_split"][1] > 1e-4, peak["poly_c0"]
 
 
 def test_freq_bound_holds_the_emulation_and_catches_the_cross_group_mask():
@@ -205,7 +184,7 @@ def test_freq_bound_holds_the_emulation_and_catches_the_cross_group_mask():
                 g = torch.Generator().manual_seed(F * 100 + L)
                 q, k, v, gates = R.freq_inputs(case, fam, g, "cpu")
                 ref, bound, _, _ = R.freq_ref(q.double(), k.double(), v.double(), gates.double(), case.B, F, "tc", H16)
-                good = _ratio(emulate_freq_tc(q, k, v, gates, case.B, F), ref, bound)
+                good = worst(emulate_freq_tc(q, k, v, gates, case.B, F), ref, bound)
                 msg = f"{case.id} {fam}: emulation at {good:.3f} of the bound"
                 if F == 8:
                     bad, e = _report(emulate_freq_tc(q, k, v, gates, case.B, F, cross_mask=False), ref, bound)
@@ -225,9 +204,9 @@ def test_ex2_poly_meets_its_stated_error():
     y = ex2_poly_np(x).astype(np.float64)
     inside = x >= -120
     rel = np.abs(y[inside] / np.exp2(x[inside].astype(np.float64)) - 1)
-    worst = rel.max()
-    print(f"ex2_poly: max relative error {worst:.3e} at x = {x[inside][rel.argmax()]} over {inside.sum()} points")
-    assert worst <= R.EX2_POLY_REL
+    rel_max = rel.max()
+    print(f"ex2_poly: max relative error {rel_max:.3e} at x = {x[inside][rel.argmax()]} over {inside.sum()} points")
+    assert rel_max <= R.EX2_POLY_REL
     clamp = ex2_poly_np(np.float32([-120.0]))[0]
     assert np.all(y[~inside] == clamp) and clamp <= 2.0**-119
     neg_inf = ex2_poly_np(np.float32([-np.inf]))
@@ -255,7 +234,7 @@ KERNEL = re.compile(r"_ZN2bt\d+(attn_time_kernel|attn_time_simt_kernel|attn_freq
 
 def test_every_attention_instantiation_has_a_case(lib_built):
     found = set()
-    for line in _sass(lib_built).splitlines():
+    for line in sass(lib_built).splitlines():
         if "Function :" in line and (m := KERNEL.search(line)):
             found.add((m.group(1), int(m.group(2) or 0)))
     launched = R.launched_kernels("tc") | R.launched_kernels("simt")

@@ -2,14 +2,14 @@
 whole key loop in registers.  A spill puts local-memory loads and stores into the loop that every key tile runs."""
 import re
 
-from test_cpu_gemm_sass import _sass
+from support import sass
 
 KERNEL = re.compile(r"_ZN2bt16attn_time_kernelE")
 
 
 def test_attn_time_kernel_has_no_local_memory_access(lib_built):
     local, fn, found = [], False, False
-    for line in _sass(lib_built).splitlines():
+    for line in sass(lib_built).splitlines():
         if "Function :" in line:
             fn = bool(KERNEL.search(line))
             found |= fn

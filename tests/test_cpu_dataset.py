@@ -11,8 +11,7 @@ import pytest
 
 import dataset_reference as R
 from conftest import GOLDEN
-
-SEED = 4000  # oracle/make_golden_train_batches.py
+from dataset_reference import SEED, _dataset, _items, _tests
 
 
 @pytest.fixture(scope="module")
@@ -23,24 +22,6 @@ def gold():
 @pytest.fixture(scope="module")
 def tree(tmp_path_factory):
     return R.write_tree(tmp_path_factory.mktemp("train_tree") / "data")
-
-
-def _items():
-    return sorted(f"{d}/{p[0]}" for d, (_, _, ps) in R.DATASETS.items() if d != "gtzan" for p in ps)
-
-
-def _tests():
-    return sorted(f"gtzan/{p[0]}" for p in R.DATASETS["gtzan"][2])
-
-
-def _dataset(tree, cfg):
-    from beat_this_b200.dataset import BeatTrackingDataset
-
-    kw = {"train_length": R.TRAIN_LENGTH, **R.CONFIGS[cfg][0]}
-    log = io.StringIO()
-    with contextlib.redirect_stdout(log):
-        ds = BeatTrackingDataset(_tests() if cfg == "full" else _items(), tree, spect_fps=R.FPS, **kw)
-    return ds, log.getvalue()
 
 
 @pytest.mark.parametrize("name", list(R.SPLITS))

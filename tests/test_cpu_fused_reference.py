@@ -13,10 +13,11 @@ import numpy as np
 import pytest
 import torch
 
-from fused_reference import (FF_CTAS, NORM_CS, QKV_CTAS, ff_cases, ff_ref, gates_ref, gelu_erf, gelu_tanh, norm_cases,
-                             norm_ref, normalize, qkv_cases, qkv_ref, random_weights, rope_positions, special_rows)
+from fused_reference import (FF_CTAS, NORM_CS, QKV_CTAS, ff_cases, ff_ref, gates_ref, norm_cases, norm_ref, qkv_cases,
+                             qkv_ref, random_weights, special_rows)
 from gemm_reference import QSCALE_TIME
-from test_cpu_gemm_sass import _sass
+from numerics import gelu_erf, gelu_tanh, normalize, rope_positions, worst
+from support import sass
 
 H16 = torch.float16
 
@@ -123,10 +124,6 @@ def emulate_qkv(x, wqkv, wg, bg, cos, sin, L, F, posmode, qscale, pos_mod_f=Fals
     return _r16(out).double(), gates.double()
 
 
-def _ratio(got, ref, bound):
-    return ((got - ref).abs() / bound).max().item()
-
-
 @pytest.mark.parametrize("C", [32, 64])
 def test_bounds_hold_the_emulation_and_catch_a_mistake(C):
     from beat_this_b200.weights import rope_tables
@@ -139,11 +136,11 @@ def test_bounds_hold_the_emulation_and_catch_a_mistake(C):
     for op in (False, True):
         oo, wo = (o, w["wout"]) if op else (None, None)
         ref, bound = ff_ref(x, w["w1"], w["b1"], w["w2"], w["b2"], oo, wo, H16)
-        good = _ratio(emulate_ff(x, w["w1"], w["b1"], w["w2"], w["b2"], oo, wo), ref, bound)
-        bad = _ratio(emulate_ff(x, w["w1"], w["b1"], w["w2"], w["b2"], oo, wo, drop_b2_block=True), ref, bound)
+        good = worst(emulate_ff(x, w["w1"], w["b1"], w["w2"], w["b2"], oo, wo), ref, bound)
+        bad = worst(emulate_ff(x, w["w1"], w["b1"], w["w2"], w["b2"], oo, wo, drop_b2_block=True), ref, bound)
         # an error of 1e-2 in one column: the size the stage taps (0.03 absolute) cannot see
-        shift = _ratio(emulate_ff(x, w["w1"], w["b1"], w["w2"], w["b2"], oo, wo, b2_shift=1e-2), ref, bound)
-        bf16 = _ratio(emulate_ff(x, w["w1"], w["b1"], w["w2"], w["b2"], oo, wo, hidden=torch.bfloat16), ref, bound)
+        shift = worst(emulate_ff(x, w["w1"], w["b1"], w["w2"], w["b2"], oo, wo, b2_shift=1e-2), ref, bound)
+        bf16 = worst(emulate_ff(x, w["w1"], w["b1"], w["w2"], w["b2"], oo, wo, hidden=torch.bfloat16), ref, bound)
         print(f"ff C={C} outproj={op}: emulation at {good:.3f} of the bound; with b2 dropped from a block at {bad:.1f}, "
               f"one column off by 1e-2 at {shift:.2f}, hidden units in bf16 at {bf16:.2f}")
         assert good <= 1 and bad > 1 and shift > 1
@@ -151,13 +148,13 @@ def test_bounds_hold_the_emulation_and_catch_a_mistake(C):
     for posmode, L, F, qscale in ((0, 150, 1, QSCALE_TIME), (1, 150, 32 // (C // 32), 1.0)):
         ref, bound, gref, gbound = qkv_ref(x, w["wqkv"], w["wg"], w["bg"], cos, sin, L, F, posmode, qscale, H16)
         got, gates = emulate_qkv(x, w["wqkv"], w["wg"], w["bg"], cos, sin, L, F, posmode, qscale)
-        good, gr = _ratio(got, ref, bound), _ratio(gates, gref, gbound)
+        good, gr = worst(got, ref, bound), worst(gates, gref, gbound)
         print(f"qkv C={C} posmode={posmode}: emulation at {good:.3f} of the bound, gates at {gr:.3f}")
         assert good <= 1 and gr <= 1
         if posmode == 1:
             bad, _ = emulate_qkv(x, w["wqkv"], w["wg"], w["bg"], cos, sin, L, F, posmode, qscale, pos_mod_f=True)
-            print(f"qkv C={C} posmode=1 with position m % F: {_ratio(bad, ref, bound):.1f} of the bound")
-            assert _ratio(bad, ref, bound) > 1
+            print(f"qkv C={C} posmode=1 with position m % F: {worst(bad, ref, bound):.1f} of the bound")
+            assert worst(bad, ref, bound) > 1
 
 
 @pytest.mark.parametrize("C", NORM_CS)
@@ -168,14 +165,14 @@ def test_norm_bound_holds_the_emulation(C):
         ref, bound = norm_ref(x, dt)
         u = _emu_norm(x.float())
         got = (u if dt is None else _r16(u)).double()
-        print(f"norm C={C} {'fp32' if dt is None else 'fp16'}: emulation at {_ratio(got, ref, bound):.3f} of the bound")
-        assert _ratio(got, ref, bound) <= 1
+        print(f"norm C={C} {'fp32' if dt is None else 'fp16'}: emulation at {worst(got, ref, bound):.3f} of the bound")
+        assert worst(got, ref, bound) <= 1
     wg = torch.randn(4, C, generator=g, dtype=torch.float64) / math.sqrt(C)
     bg = torch.randn(4, generator=g, dtype=torch.float64)
     u = _emu_norm(x.float())
     gates = torch.sigmoid(u @ wg.float().T + bg.float()).double()
     gref, gbound = gates_ref(normalize(x), wg, bg, min(4, C // 32))
-    assert _ratio(gates[:, : gref.shape[1]], gref, gbound) <= 1
+    assert worst(gates[:, : gref.shape[1]], gref, gbound) <= 1
 
 
 def test_every_instantiation_has_a_unit_test(lib_built):
@@ -185,7 +182,7 @@ def test_every_instantiation_has_a_unit_test(lib_built):
     qkv = re.compile(r"_ZN2bt16fused_qkv_kernelILi(\d+)EE")
     norm = re.compile(r"_ZN2bt11norm_kernelI(f|6__half|13__nv_bfloat16)Li(\d+)EE")
     found = {"ff": set(), "qkv": set(), "norm": set()}
-    for line in _sass(lib_built).splitlines():
+    for line in sass(lib_built).splitlines():
         if "Function :" not in line:
             continue
         if m := ff.search(line):

@@ -4,7 +4,7 @@ take every B fragment from the staged weights with ldmatrix.x4 (LDSM) rather tha
 per MMA, and read their rows from the per-warp stage that cp.async (LDGSTS) fills, with 64-bit shared loads."""
 import re
 
-from test_cpu_gemm_sass import _sass
+from support import sass
 
 KERNEL = re.compile(r"_ZN2bt(?:15fused_ff_kernelILi(32|64)ELb([01])EE|16fused_qkv_kernelILi(32|64)EE)")
 # "@!PT" never executes: ptxas places such dummy shared loads next to LDGSTS
@@ -14,7 +14,7 @@ OPCODE = re.compile(r"/\*[0-9a-f]{4,}\*/\s+(@!?U?P[T0-9]+\s+)?([A-Z][A-Z0-9_.]*)
 def _opcodes(lib_built):
     """{kernel name: {opcode: count}} over the six fused instantiations, never-executed instructions left out."""
     ops, fn = {}, None
-    for line in _sass(lib_built).splitlines():
+    for line in sass(lib_built).splitlines():
         if "Function :" in line:
             m = KERNEL.search(line)
             fn = (f"fused_ff_kernel<{m.group(1)}, {'true' if m.group(2) == '1' else 'false'}>" if m.group(1)

@@ -6,12 +6,13 @@ residual arrives by TMA as well, so a residual read in registers (a load after t
 round trip each) cannot come back unnoticed.  The gates GEMM (kind 2) keeps its register epilogue."""
 import re
 
-from test_cpu_gemm_sass import KERNEL, _sass
+from gemm_reference import GEMM_TC_KERNEL as KERNEL
+from support import sass
 
 
-def _counts(sass):
+def _counts(listing):
     counts, fn = {}, None
-    for line in sass.splitlines():
+    for line in listing.splitlines():
         if "Function :" in line:
             m = KERNEL.search(line)
             fn = (int(m.group(1)), int(m.group(2)), int(m.group(3) or 0)) if m else None
@@ -28,7 +29,7 @@ def _counts(sass):
 
 
 def test_staged_gemm_epilogues_store_by_tma(lib_built):
-    counts = _counts(_sass(lib_built))
+    counts = _counts(sass(lib_built))
     assert len(counts) == 16, f"kind-0/1 instantiations found: {sorted(counts)}"
     bad = {k: c for k, c in counts.items() if c["UTMASTG"] == 0 or c["STG"] or c["LDG"]}
     for k in sorted(counts):

@@ -4,27 +4,18 @@ The GEMM kernels of epilogue kinds 0 and 1 (every linear layer and convolution o
 call: a call anywhere in a kernel that issues wgmma makes ptxas serialise all of its wgmma instructions (warning
 C7510), each MMA waiting for the previous one.  Every instantiation of the kernel in the library has a case in the GPU
 unit tests (tests/gemm_reference.py), so a new tile or epilogue cannot ship untested."""
-import os
 import re
-import subprocess
 
 import torch
 
-from beat_this_b200 import _lib
-from gemm_reference import GEMM_CASES, GEMM_TILES, gelu_erf, gelu_tanh, rope_ref
-
-# gemm_tc_kernel<BN, BK, KIND>; KIND 2 (the N = 32 attention gates) keeps the IEEE-division sigmoid
-KERNEL = re.compile(r"_ZN2bt14gemm_tc_kernelILi(\d+)ELi(\d+)E(?:Li(\d+)E)?E")
-
-
-def _sass(lib_built):
-    cuobjdump = os.path.join(os.path.dirname(_lib._nvcc()), "cuobjdump")
-    return subprocess.run([cuobjdump, "-sass", _lib.LIB_PATH], capture_output=True, text=True, check=True).stdout
+from gemm_reference import GEMM_CASES, GEMM_TC_KERNEL as KERNEL, GEMM_TILES
+from numerics import gelu_erf, gelu_tanh, rope_ref
+from support import sass
 
 
 def test_gemm_kernels_have_no_call(lib_built):
     calls, checked, fn = {}, set(), None
-    for line in _sass(lib_built).splitlines():
+    for line in sass(lib_built).splitlines():
         if "Function :" in line:
             m = KERNEL.search(line)
             fn = m.group(0) if m and m.group(3) != "2" else None
@@ -40,7 +31,7 @@ def test_every_gemm_instantiation_has_a_unit_test(lib_built):
     """The (BN, BK, KIND) instantiations in the SASS are exactly GEMM_TILES, and the GPU cases reach each of them
     (the GPU test asserts that the plan of every case picks the tile expected_tile names)."""
     found = set()
-    for line in _sass(lib_built).splitlines():
+    for line in sass(lib_built).splitlines():
         if "Function :" in line:
             m = KERNEL.search(line)
             if m:

@@ -1,32 +1,10 @@
 """The loss restatement (tests/loss_reference.py) against the unmodified reference's outputs (tests/golden/loss.npz,
 oracle/make_golden_loss.py), the framewise truth builder of beat_this_b200.evaluate, loss_from_hparams and --losses."""
-import os
-
 import numpy as np
 import pytest
 
 import loss_reference as R
-from conftest import GOLDEN
-
-GOLD = np.load(os.path.join(GOLDEN, "loss.npz"))
-CASES = range(int(GOLD["n"]))
-
-
-def fixture_case(k):
-    """(preds, targets, mask or None, row offsets, kind, tolerance, pos_weight, reference loss, reference grad), the
-    mask broadcast to the predictions' shape and every array flattened into rows of T frames."""
-    kind, t, pw, has_mask = GOLD[f"spec{k}"]
-    x = GOLD[f"preds{k}"]
-    m = np.broadcast_to(GOLD[f"mask{k}"], x.shape).astype(np.float32).ravel() if has_mask else None
-    T = x.shape[-1]
-    off = (np.arange(x.size // T + 1) * T).tolist()
-    return (x.ravel(), GOLD[f"targets{k}"].ravel(), m, off, int(kind), int(t), float(pw), float(GOLD[f"loss{k}"]),
-            GOLD[f"grad{k}"].ravel())
-
-
-# torch's fp32 gradient form cancels when p y is close to (p y + 1 - y) sigmoid(x) (soft targets, p = 4.5): the fixture
-# itself is then off by up to ~2e-6 of max |g| (1.7e-6 in case 61)
-GRAD_TOL = 2e-6
+from loss_reference import CASES, GOLD, GRAD_TOL, fixture_case
 
 
 @pytest.mark.parametrize("k", CASES)

@@ -13,7 +13,7 @@ from beat_this_b200 import _lib
 from beat_this_b200 import train as T
 from beat_this_b200.optim import CosineWarmupScheduler
 from conftest import GOLDEN
-from test_cpu_gemm_sass import _sass
+from support import sass
 
 
 @pytest.fixture(scope="module")
@@ -80,7 +80,7 @@ def test_command_line_takes_the_reference_flags():
 
 def test_adamw_kernel_has_no_local_memory(lib_built):
     fn, found, local = None, set(), []
-    for line in _sass(lib_built).splitlines():
+    for line in sass(lib_built).splitlines():
         if "Function :" in line:
             fn = line.split("Function :")[1].strip()
             if "adamw" in fn:

@@ -9,15 +9,13 @@ import torch
 import torch.nn.functional as Fn
 
 import train_kernels_reference as R
+from numerics import worst
 from oracle import beat_this_oracle as O
+from support import rnd
 
 
 def _g(seed):
     return torch.Generator().manual_seed(seed)
-
-
-def rnd(*shape, g, scale=1.0):
-    return (torch.randn(*shape, generator=g) * scale).float()
 
 
 def _bn(C, g):  # running variances 0.5 .. 1.5, as the synthetic checkpoints have them
@@ -142,26 +140,26 @@ def _cases():
     for m in ("bn_eps", "gelu_tanh"):
         clean = R.emu_bn_gelu_bwd(dy.numpy(), z.numpy(), bn, C)
         bad = R.emu_bn_gelu_bwd(dy.numpy(), z.numpy(), bn, C, m)
-        out[m] = (max(R.worst(torch.tensor(clean[0]), dbn, e1), R.worst(torch.tensor(clean[1]), dz, e2)),
-                  max(R.worst(torch.tensor(bad[0]), dbn, e1), R.worst(torch.tensor(bad[1]), dz, e2)), "bn_gelu_bwd C32")
+        out[m] = (max(worst(torch.tensor(clean[0]), dbn, e1), worst(torch.tensor(clean[1]), dz, e2)),
+                  max(worst(torch.tensor(bad[0]), dbn, e1), worst(torch.tensor(bad[1]), dz, e2)), "bn_gelu_bwd C32")
     ref, e = R.bn_scale_ref(dy, bn, C)
-    out["bn_eps (bn_scale)"] = (R.worst(torch.tensor(R.emu_bn_scale_op(dy.numpy(), bn, C)), ref, e),
-                                R.worst(torch.tensor(R.emu_bn_scale_op(dy.numpy(), bn, C, "bn_eps")), ref, e),
+    out["bn_eps (bn_scale)"] = (worst(torch.tensor(R.emu_bn_scale_op(dy.numpy(), bn, C)), ref, e),
+                                worst(torch.tensor(R.emu_bn_scale_op(dy.numpy(), bn, C, "bn_eps")), ref, e),
                                 "bn_scale C32")
     # 3, 4: tr_reduce over Z - 1 parts; the last K tile masked at K (dY^T X over 4099 rows, 7 parts)
     A, B = rnd(9, 4099, g=g), rnd(7, 4099, g=g)
     ref, e, _, _ = R.gemm_ref(A, B, splits=7)
-    out["reduce_z_minus_1"] = (R.worst(torch.tensor(R.emu_gemm(A.numpy(), B.numpy(), 7)), ref, e),
-                               R.worst(torch.tensor(R.emu_gemm(A.numpy(), B.numpy(), 7, "reduce_z_minus_1")), ref, e),
+    out["reduce_z_minus_1"] = (worst(torch.tensor(R.emu_gemm(A.numpy(), B.numpy(), 7)), ref, e),
+                               worst(torch.tensor(R.emu_gemm(A.numpy(), B.numpy(), 7, "reduce_z_minus_1")), ref, e),
                                "gemm M9 N7 K4099 splits 7")
     out["gemm_mask_at_K"] = (out["reduce_z_minus_1"][0],
-                             R.worst(torch.tensor(R.emu_gemm(A.numpy(), B.numpy(), 7, "gemm_mask_at_K")), ref, e),
+                             worst(torch.tensor(R.emu_gemm(A.numpy(), B.numpy(), 7, "gemm_mask_at_K")), ref, e),
                              "gemm M9 N7 K4099 splits 7")
     # 5: colsum lanes all from the part's first row
     A = rnd(1025, 33, g=g)
     ref, e, _, _ = R.colsum_ref(A, splits=3, scale=0.5)
-    out["colsum_lane_start"] = (R.worst(torch.tensor(R.emu_colsum(A.numpy(), 3, 0.5)[0]), ref, e),
-                                R.worst(torch.tensor(R.emu_colsum(A.numpy(), 3, 0.5, "colsum_lane_start")[0]), ref, e),
+    out["colsum_lane_start"] = (worst(torch.tensor(R.emu_colsum(A.numpy(), 3, 0.5)[0]), ref, e),
+                                worst(torch.tensor(R.emu_colsum(A.numpy(), 3, 0.5, "colsum_lane_start")[0]), ref, e),
                                 "colsum M1025 N33 splits 3")
     # 6: rms_bwd without its clamped branch (a row of norm 1e-13)
     x = rnd(8, 64, g=g)
@@ -173,16 +171,16 @@ def _cases():
     inv32 = inv.float()
     ref, e = R.rms_bwd_ref(dxn, x, inv32, gamma)
     args = (dxn.numpy(), x.numpy(), inv32.numpy(), gamma.numpy())
-    out["rms_no_clamp"] = (R.worst(torch.tensor(R.emu_rms_bwd(*args)), ref, e),
-                           R.worst(torch.tensor(R.emu_rms_bwd(*args, "rms_no_clamp")), ref, e), "rms_bwd C64, norm 1e-13")
+    out["rms_no_clamp"] = (worst(torch.tensor(R.emu_rms_bwd(*args)), ref, e),
+                           worst(torch.tensor(R.emu_rms_bwd(*args, "rms_no_clamp")), ref, e), "rms_bwd C64, norm 1e-13")
     # 7, 8: inverse RoPE with +sin; posmode 1 with m % F
     fr = (1.0 / 10000 ** (torch.arange(0, 32, 2).float() / 32)).float()
     for m, (pm, L, F, inv_, M) in (("rope_inverse_plus_sin", (0, 1500, 1, 1, 1600)),
                                    ("rope_pos_mod_F", (1, 17, 16, 0, 16 * 17))):
         qkv = rnd(M, 192, g=g)
         ref, e = R.rope_ref(qkv, fr, L, F, pm, inv_)
-        out[m] = (R.worst(torch.tensor(R.emu_rope(qkv.numpy(), fr.numpy(), L, F, pm, inv_)), ref, e),
-                  R.worst(torch.tensor(R.emu_rope(qkv.numpy(), fr.numpy(), L, F, pm, inv_, m)), ref, e),
+        out[m] = (worst(torch.tensor(R.emu_rope(qkv.numpy(), fr.numpy(), L, F, pm, inv_)), ref, e),
+                  worst(torch.tensor(R.emu_rope(qkv.numpy(), fr.numpy(), L, F, pm, inv_, m)), ref, e),
                   f"rope posmode {pm} M{M}")
     # 9: dkv without delta
     H, n = 1, 65
@@ -195,16 +193,16 @@ def _cases():
     args = (qkv, dO, lse_t.float(), delta.float(), rows, H)
     ck, cv = R.emu_attn_dkv(*args)
     bk, _ = R.emu_attn_dkv(*args, mistake="dkv_no_delta")
-    out["dkv_no_delta"] = (max(R.worst(ck, dk, edk), R.worst(cv, dv, edv)), R.worst(bk, dk, edk), "attn_dkv time n65")
+    out["dkv_no_delta"] = (max(worst(ck, dk, edk), worst(cv, dv, edv)), worst(bk, dk, edk), "attn_dkv time n65")
     # 10: lse in log2
     _, _, l2, _ = R.attn_fwd_ref(qkv, rows, H, lse_log2=True)
-    out["lse_log2"] = (0.0, R.worst(l2, lse, el), "attn_fwd time n65")
+    out["lse_log2"] = (0.0, worst(l2, lse, el), "attn_fwd time n65")
     # 11: im2col tap t + dt
     gm = (2, 16, 2, 17, 32, 16 * 2 * 17 * 32, 17 * 32, 32, 1)
     x = rnd(2 * 32 * 17 * 32, g=g)
     ref, e = R.im2col_ref(x, gm)
-    out["im2col_tap"] = (R.worst(torch.tensor(R.emu_im2col(x.numpy(), gm)).reshape(ref.shape), ref, e + 0),
-                         R.worst(torch.tensor(R.emu_im2col(x.numpy(), gm, "im2col_tap")).reshape(ref.shape), ref,
+    out["im2col_tap"] = (worst(torch.tensor(R.emu_im2col(x.numpy(), gm)).reshape(ref.shape), ref, e + 0),
+                         worst(torch.tensor(R.emu_im2col(x.numpy(), gm, "im2col_tap")).reshape(ref.shape), ref,
                                  e + 0), "im2col conv0 L17 (exact: any difference)")
     # 12: dg without (1 - sg)
     Og, dG = rnd(40, 64, g=g), rnd(40, 64, g=g)
@@ -212,8 +210,8 @@ def _cases():
     dOr, e0, dg, eg, de, ed = R.gate_bwd_ref(dG, Og, gl)
     c = R.emu_gate_bwd(dG.numpy(), Og.numpy(), gl.numpy())
     b = R.emu_gate_bwd(dG.numpy(), Og.numpy(), gl.numpy(), "dg_no_one_minus")
-    out["dg_no_one_minus"] = (max(R.worst(torch.tensor(c[0]), dOr, e0), R.worst(torch.tensor(c[1]), dg, eg),
-                                  R.worst(torch.tensor(c[2]), de, ed)), R.worst(torch.tensor(b[1]), dg, eg),
+    out["dg_no_one_minus"] = (max(worst(torch.tensor(c[0]), dOr, e0), worst(torch.tensor(c[1]), dg, eg),
+                                  worst(torch.tensor(c[2]), de, ed)), worst(torch.tensor(b[1]), dg, eg),
                               "gate_bwd M40 C64")
     return out
 

@@ -16,18 +16,10 @@ import pytest
 import torch
 
 import attention_reference as R
+from numerics import ulp16
+from support import act_dtype, dev, launch_twice  # noqa: F401  (fixture)
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(3000)]
-
-NAN = float("nan")
-
-
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.fail("GPU tests need a CUDA device")
-    return torch.device("cuda:0")
-
 
 @pytest.fixture(scope="module")
 def engines(lib_built, dev):
@@ -35,16 +27,6 @@ def engines(lib_built, dev):
     from beat_this_b200.engine import Engine
 
     return {half: Engine(None, None, dev, half=half) for half in (False, True)}
-
-
-def _act_dtype(eng):
-    return torch.float16 if eng.act_dtype == "f16" else torch.bfloat16
-
-
-def _ulp(x, dt):
-    """Spacing of the 16-bit type dt at its representable values x (float64)."""
-    mant, emin = (10, -14) if dt == torch.float16 else (7, -126)
-    return torch.exp2(torch.floor(torch.log2(x.abs().clamp_min(2.0**emin))) - mant)
 
 
 class Family:
@@ -66,7 +48,7 @@ class Family:
         assert torch.isfinite(got).all(), "non-finite values in rows < M"
         err = (got - ref).abs()
         ratio = torch.where(err == 0, 0.0, err / bound).max().item()  # a bound of 0 asks for the exact value
-        half_ulp = 0.0 if dt is None else _ulp(got, dt) / 2
+        half_ulp = 0.0 if dt is None else ulp16(got, dt) / 2
         r32 = ((got - o).abs() / (e32 + half_ulp)).max().item()
         print(f"{self.name} {case_id}: max {err.max().item():.3e} = {ratio:.3f} of its bound; fp32 level {r32:.3f}")
         self.worst, self.worst32 = max(self.worst, ratio), max(self.worst32, r32)
@@ -82,24 +64,12 @@ def _finish(families):
     assert not failures, f"{len(failures)} of {total} attention cases failed:\n" + "\n".join(failures)
 
 
-def _launch_twice(call, M, C, dev):
-    """Two launches on fresh NaN buffers of M + 1 rows; returns the first after checking the sentinel row and bits."""
-    outs = []
-    for _ in range(2):
-        out = torch.full(((M + 1) * C,), NAN, device=dev)
-        call(out)
-        outs.append(out)
-    assert torch.equal(outs[0].view(torch.int32), outs[1].view(torch.int32)), "a second launch gives other bits"
-    assert torch.isnan(outs[0][M * C :]).all(), "store past the last row"
-    return outs[0][: M * C].view(M, C).double()
-
-
 def _time_case(fam, case_id, eng, case, q, k, v, gates):
     half = eng.half
     M, C = case.seqs * case.L, 32 * case.heads
-    got = _launch_twice(lambda out: eng.debug_attention(q, k, v, gates, case.key_lens, case.spc, out=out), M, C, q.device)
+    got = launch_twice(lambda out: eng.debug_attention(q, k, v, gates, case.key_lens, case.spc, out=out), M, C, q.device)
     lens = torch.tensor(case.lens(), device=q.device)
-    dt = _act_dtype(eng) if half else None
+    dt = act_dtype(eng) if half else None
     res = R.time_ref(q.double(), k.double(), v.double(), gates.double(), lens, "tc" if half else "simt", dt)
     fam.check(case_id, got, [t.reshape(M, C) for t in res], dt)
 
@@ -107,8 +77,8 @@ def _time_case(fam, case_id, eng, case, q, k, v, gates):
 def _freq_case(fam, case_id, eng, case, q, k, v, gates):
     half = eng.half
     M, C = case.B * case.F * case.L, 32 * case.heads
-    got = _launch_twice(lambda out: eng.debug_attention_freq(q, k, v, gates, case.B, case.F, out=out), M, C, q.device)
-    dt = _act_dtype(eng) if half else None
+    got = launch_twice(lambda out: eng.debug_attention_freq(q, k, v, gates, case.B, case.F, out=out), M, C, q.device)
+    dt = act_dtype(eng) if half else None
     res = R.freq_ref(q.double(), k.double(), v.double(), gates.double(), case.B, case.F, "tc" if half else "simt", dt)
     fam.check(case_id, got, res, dt)
 

@@ -17,6 +17,7 @@ import pytest
 import torch
 
 import chunk_kernels_reference as R
+from support import bits, dev  # noqa: F401  (fixture)
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(1800)]
 
@@ -25,22 +26,11 @@ TAIL = 1024  # guard elements after every output
 
 
 @pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.fail("GPU tests need a CUDA device")
-    return torch.device("cuda:0")
-
-
-@pytest.fixture(scope="module")
 def engines(lib_built, dev):
     """Weight-less contexts: {False: fp32, True: 16-bit}."""
     from beat_this_b200.engine import Engine
 
     return {half: Engine(None, None, dev, half=half) for half in (False, True)}
-
-
-def _bits(t):
-    return t.contiguous().view(torch.int32 if t.element_size() == 4 else torch.int16)
 
 
 class Family:
@@ -134,7 +124,7 @@ def _stem_case(fam, case_id, eng, spect, chunks, L, params):
         out = torch.full((size + TAIL,), NAN, device=spect.device)
         eng.debug_stem(spect, chunks, L, *params, out)
         runs.append(out)
-    assert torch.equal(_bits(runs[0]), _bits(runs[1])), "not deterministic"
+    assert torch.equal(bits(runs[0]), bits(runs[1])), "not deterministic"
     out = runs[0]
     assert torch.isnan(out[size:]).all(), "stored past n_chunks * 32 * L * 32"
     ref, bound = R.stem_ref(spect.double(), chunks, L, *(p.double() for p in params))
@@ -192,14 +182,14 @@ def _head_case(fam, case_id, eng, x, w, b, chunks, L, sum_head, frames, planner)
         eng.debug_head(x, D, w, b, chunks, L, sum_head, beat, down)
         runs.append((beat, down))
     (beat, down), (beat2, down2) = runs
-    assert torch.equal(_bits(beat), _bits(beat2)) and torch.equal(_bits(down), _bits(down2)), "not deterministic"
+    assert torch.equal(bits(beat), bits(beat2)) and torch.equal(bits(down), bits(down2)), "not deterministic"
     rb, rd, eb, ed = R.head_ref(x.double(), w.double(), b.double(), sum_head)
     owned = R.head_scatter(chunks, L, rb, frames)[1]
     if planner:  # the planner's ranges tile every clip
         assert torch.equal(owned > 0, _clip_mask(chunks, frames, x.device)) and owned.max() <= 1, "not owned exactly once"
-    nan_bits = _bits(torch.full((1,), NAN, device=x.device))
+    nan_bits = bits(torch.full((1,), NAN, device=x.device))
     for name, got, ref, bnd in (("beat", beat, rb, eb), ("down", down, rd, ed)):
-        assert (_bits(got)[owned == 0] == nan_bits).all(), f"{name}: a frame no chunk owns was written"
+        assert (bits(got)[owned == 0] == nan_bits).all(), f"{name}: a frame no chunk owns was written"
         fam.check(case_id, name, got[owned > 0], R.head_scatter(chunks, L, ref, frames)[0][owned > 0],
                   R.head_scatter(chunks, L, bnd, frames)[0][owned > 0])
     zero = x.view(-1, D).abs().amax(-1) == 0  # zero rows: exactly the bias
@@ -255,18 +245,18 @@ def test_head(engines, dev, lib_built):
 def _zero_tail_case(fam, case_id, eng, chunks, F, L, C, dtype, g):
     n = len(chunks)
     size = n * F * L * C
-    bits = torch.randint(1, 2**15 - 1, (size + TAIL,), generator=g, device=g.device, dtype=torch.int32)
-    base = (bits if dtype == torch.float32 else bits.to(torch.int16)).view(dtype)
+    raw = torch.randint(1, 2**15 - 1, (size + TAIL,), generator=g, device=g.device, dtype=torch.int32)
+    base = (raw if dtype == torch.float32 else raw.to(torch.int16)).view(dtype)
     runs = []
     for _ in range(2):
         buf = base.clone()
         eng.debug_zero_tail(buf, chunks, F, L, C)
         runs.append(buf)
-    assert torch.equal(_bits(runs[0]), _bits(runs[1])), "not deterministic"
+    assert torch.equal(bits(runs[0]), bits(runs[1])), "not deterministic"
     buf = runs[0]
-    assert torch.equal(_bits(buf[size:]), _bits(base[size:])), "changed past n_chunks * F * L * C"
+    assert torch.equal(bits(buf[size:]), bits(base[size:])), "changed past n_chunks * F * L * C"
     ref = R.zero_tail_ref(base[:size].view(n, F, L, C), chunks, F, L, C)
-    bad = int((_bits(buf[:size]) != _bits(ref.reshape(-1))).sum())
+    bad = int((bits(buf[:size]) != bits(ref.reshape(-1))).sum())
     assert bad == 0, f"{bad} elements differ from the exact result"
 
 
@@ -307,12 +297,12 @@ def test_hooks_reproduce_the_forward_pass(dev, lib_built, half):
     stem_tap, (beat, down) = eng.tap("stem", spect, fo, n * 32 * L * 32)
     out = torch.full((n * 32 * L * 32,), NAN, device=dev)
     eng.debug_stem(spect, chunks, L, P["stem.bn1_scale"], P["stem.bn1_shift"], P["stem.w"], P["stem.bias"], out)
-    assert stem_tap.numel() == out.numel() and torch.equal(_bits(stem_tap), _bits(out)), "stem tap != bt_debug_stem"
+    assert stem_tap.numel() == out.numel() and torch.equal(bits(stem_tap), bits(out)), "stem tap != bt_debug_stem"
     x, (beat2, down2) = eng.tap(f"l{hp['n_layers'] - 1}.ff", spect, fo, n * L * D)
-    assert torch.equal(_bits(beat), _bits(beat2)) and torch.equal(_bits(down), _bits(down2))
+    assert torch.equal(bits(beat), bits(beat2)) and torch.equal(bits(down), bits(down2))
     hb, hd = torch.full_like(beat, NAN), torch.full_like(down, NAN)
     eng.debug_head(x.contiguous(), D, P["head.w"], P["head.b"], chunks, L, hp["sum_head"], hb, hd)
-    assert torch.equal(_bits(hb), _bits(beat)) and torch.equal(_bits(hd), _bits(down)), "logits != bt_debug_head"
+    assert torch.equal(bits(hb), bits(beat)) and torch.equal(bits(hd), bits(down)), "logits != bt_debug_head"
 
 
 # ------------------------------------------------------------------------------ launches and refusals

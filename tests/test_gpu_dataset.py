@@ -10,7 +10,7 @@ import torch
 
 import dataset_reference as R
 import loss_reference as LR
-from test_cpu_dataset import SEED, _dataset, _items
+from dataset_reference import SEED, _dataset, _items
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(1800)]
 DEV = "cuda:0"

@@ -7,7 +7,7 @@ import pytest
 import torch
 
 from conftest import GOLDEN
-from test_gpu_kernels import F32_TOL, H16_TOL
+from numerics import F32_TOL, H16_TOL
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(900)]
 

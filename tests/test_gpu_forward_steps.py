@@ -29,22 +29,13 @@ import pytest
 import torch
 
 import forward_steps_reference as R
+from numerics import QSCALE_H16
+from support import bits, dev  # noqa: F401  (fixture)
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(1800)]
 
 NAN = float("nan")
 LONG = 3000  # frames of the long chunks, and the maximum chunk length of their context
-
-
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.fail("GPU tests need a CUDA device")
-    return torch.device("cuda:0")
-
-
-def _bits(t):
-    return t.contiguous().view(torch.int32)
 
 
 def _planner(lib):
@@ -216,7 +207,7 @@ class Chain:
             # or GEMM epilogue's 16-bit q, already scaled by `qscale`.  Dividing by the hook's scale in fp32 gives a
             # value whose fp32 product with that scale rounds back to q (2 fp32 roundings, far inside half a 16-bit
             # ulp), which is checked here before it is relied on
-            s = torch.tensor(R.HOOK_QSCALE_H16, dtype=torch.float32, device=q.device)
+            s = torch.tensor(QSCALE_H16, dtype=torch.float32, device=q.device)
             q = (q / s).contiguous()
             assert torch.equal((q * s).to(self.ps.adt).float(), self.regs["qkv"][:, :C]), "q does not survive the hook's scale"
         o = self._nan(q.shape[0], C, q.device)
@@ -271,7 +262,7 @@ def test_steps_tie_to_hooks(dev, lib_built, model, half, wave_kind):
     b1, d1 = ps.forward()
     b2, d2 = ps.forward()
     torch.cuda.synchronize()
-    if not (torch.equal(_bits(b1), _bits(b2)) and torch.equal(_bits(d1), _bits(d2))):
+    if not (torch.equal(bits(b1), bits(b2)) and torch.equal(bits(d1), bits(d2))):
         failures.append("two forward calls give different logits")
 
     # coverage: the production chains, by the launch each call stands for, are the launch profile of one call
@@ -341,4 +332,4 @@ def _run_chain(ps, step, regs):
 def _differ(got, want):
     """(elements whose bits differ, max abs difference) of two fp32 tensors of the same size."""
     got, want = got.contiguous().view(-1), want.contiguous().view(-1)
-    return int((_bits(got) != _bits(want)).sum()), (got.double() - want.double()).abs().max().item()
+    return int((bits(got) != bits(want)).sum()), (got.double() - want.double()).abs().max().item()

@@ -13,20 +13,15 @@ import zlib
 import pytest
 import torch
 
-from fused_reference import (ff_cases, ff_ref, gates_ref, norm_cases, norm_ref, normalize, qkv_cases, qkv_ref,
-                             random_weights, special_rows)
+from fused_reference import (ff_cases, ff_ref, gates_ref, norm_cases, norm_ref, qkv_cases, qkv_ref, random_weights,
+                             special_rows)
 from gemm_reference import QSCALE_TIME
+from numerics import normalize
+from support import act_dtype, bits, dev  # noqa: F401  (fixture)
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(1200)]
 
 NAN = float("nan")
-
-
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.fail("GPU tests need a CUDA device")
-    return torch.device("cuda:0")
 
 
 @pytest.fixture(scope="module")
@@ -35,10 +30,6 @@ def engines(lib_built, dev):
     from beat_this_b200.engine import Engine
 
     return {half: Engine(None, None, dev, half=half) for half in (False, True)}
-
-
-def _act_dtype(eng):
-    return torch.float16 if eng.act_dtype == "f16" else torch.bfloat16
 
 
 def _rope(dev):
@@ -54,10 +45,6 @@ def _f32(t):
 def _with_row(x, row):
     """x [M, n] fp32 with one more row appended."""
     return torch.cat([_f32(x), row.reshape(1, -1).to(x.device, torch.float32)]).contiguous()
-
-
-def _bits(t):
-    return t.contiguous().view(torch.int32)
 
 
 class Family:
@@ -88,7 +75,7 @@ class Family:
 # ------------------------------------------------------------------------------ fused FFN
 def _ff_case(fam, case_id, eng, C, op, xb, M, x, w, o):
     """x [M, C], o [M + 1, C] (its last row NaN) float64 on the device; w: float64 weights."""
-    dt = _act_dtype(eng)
+    dt = act_dtype(eng)
     sentinel = torch.full((C,), 7.0)
     X0 = _with_row(x, sentinel)
     runs = []
@@ -99,13 +86,13 @@ def _ff_case(fam, case_id, eng, C, op, xb, M, x, w, o):
                            o=_f32(o) if op else None, wout=_f32(w["wout"]) if op else None, xb_out=XB)
         runs.append((X, XB))
     (X, XB), (X2, XB2) = runs
-    assert torch.equal(_bits(X), _bits(X2)) and (not xb or torch.equal(_bits(XB), _bits(XB2))), "not deterministic"
-    assert torch.equal(_bits(X[M]), _bits(X0[M])), "X changed past row M"
+    assert torch.equal(bits(X), bits(X2)) and (not xb or torch.equal(bits(XB), bits(XB2))), "not deterministic"
+    assert torch.equal(bits(X[M]), bits(X0[M])), "X changed past row M"
     ref, bound = ff_ref(x, w["w1"], w["b1"], w["w2"], w["b2"], o[:M] if op else None, w["wout"] if op else None, dt)
     fam.check(case_id, "x", X[:M].double(), ref, bound)
     if xb:
         assert torch.isnan(XB[M]).all(), "16-bit copy written past row M"
-        assert torch.equal(_bits(XB[:M]), _bits(X[:M].to(dt).float())), "16-bit copy is not round16 of the fp32 result"
+        assert torch.equal(bits(XB[:M]), bits(X[:M].to(dt).float())), "16-bit copy is not round16 of the fp32 result"
 
 
 def test_fused_ff(engines, dev):
@@ -124,7 +111,7 @@ def test_fused_ff(engines, dev):
 
 # ------------------------------------------------------------------------------ fused QKV
 def _qkv_case(fam, case_id, eng, C, posmode, L, F, qscale, M, x, w, rope):
-    dt = _act_dtype(eng)
+    dt = act_dtype(eng)
     heads = C // 32
     X = _with_row(x, torch.randn(C) * 3)
     runs = []
@@ -135,7 +122,7 @@ def _qkv_case(fam, case_id, eng, C, posmode, L, F, qscale, M, x, w, rope):
                             posmode, qscale)
         runs.append((QKV, G))
     (QKV, G), (QKV2, G2) = runs
-    assert torch.equal(_bits(QKV), _bits(QKV2)) and torch.equal(_bits(G), _bits(G2)), "not deterministic"
+    assert torch.equal(bits(QKV), bits(QKV2)) and torch.equal(bits(G), bits(G2)), "not deterministic"
     assert torch.isnan(QKV[M]).all() and torch.isnan(G[M]).all(), "store past row M"
     cos, sin = (t.double() for t in rope)
     ref, bound, gref, gbound = qkv_ref(x, w["wqkv"], w["wg"], w["bg"], cos, sin, L, F, posmode, qscale, dt)
@@ -159,7 +146,7 @@ def test_fused_qkv(engines, dev):
 
 # ------------------------------------------------------------------------------ norm
 def _norm_case(fam, case_id, eng, C, heads, M, x, wg, bg):
-    dt = _act_dtype(eng) if eng.half else None
+    dt = act_dtype(eng) if eng.half else None
     X = _with_row(x, torch.randn(C) * 3)
     runs = []
     for _ in range(2):
@@ -168,7 +155,7 @@ def _norm_case(fam, case_id, eng, C, heads, M, x, wg, bg):
         eng.debug_norm(X, XN, M, C, _f32(wg) if heads else None, _f32(bg) if heads else None, G if heads else None, heads)
         runs.append((XN, G))
     (XN, G), (XN2, G2) = runs
-    assert torch.equal(_bits(XN), _bits(XN2)) and torch.equal(_bits(G), _bits(G2)), "not deterministic"
+    assert torch.equal(bits(XN), bits(XN2)) and torch.equal(bits(G), bits(G2)), "not deterministic"
     assert torch.isnan(XN[M]).all() and torch.isnan(G[M]).all(), "store past row M"
     ref, bound = norm_ref(x, dt)
     fam.check(case_id, "xn", XN[:M].double(), ref, bound)

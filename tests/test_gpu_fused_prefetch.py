@@ -11,18 +11,12 @@ import torch
 
 from fused_reference import FF_CTAS, FUSED_WARPS, QKV_CTAS, WARP_ROWS, random_weights
 from gemm_reference import QSCALE_TIME
+from support import bits, dev  # noqa: F401  (fixture)
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(1200)]
 
 NAN = float("nan")
 TAIL = 2 * WARP_ROWS  # rows past M in every buffer
-
-
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.fail("GPU tests need a CUDA device")
-    return torch.device("cuda:0")
 
 
 @pytest.fixture(scope="module")
@@ -37,10 +31,6 @@ def _ms(ctas, sms):
     full (-1), a single row (-15) or a single row of one more group (+1)."""
     wave = WARP_ROWS * FUSED_WARPS * ctas * sms  # rows of one step of the whole persistent grid
     return sorted({5, WARP_ROWS} | {k * wave + d for k in (1, 2, 3) for d in (-15, -1, 0, 1)})
-
-
-def _bits(t):
-    return t.contiguous().view(torch.int32)
 
 
 def _padded(x, M, fill):
@@ -69,12 +59,12 @@ def test_fused_ff_prefetch_past_m(eng, dev, op):
             X_in = X.clone()
             eng.debug_fused_ff(X, w["w1"], w["b1"], w["w2"], w["b2"], M, C, o=O if op else None,
                                wout=w["wout"] if op else None, xb_out=XB)
-            assert torch.equal(_bits(X[M:]), _bits(X_in[M:])), f"C={C} M={M} fill={fill}: X changed past row M"
+            assert torch.equal(bits(X[M:]), bits(X_in[M:])), f"C={C} M={M} fill={fill}: X changed past row M"
             assert (XB[M:] == 7.0).all(), f"C={C} M={M} fill={fill}: 16-bit copy written past row M"
             assert torch.isfinite(X[:M]).all(), f"C={C} M={M} fill={fill}: non-finite rows < M"
             runs[fill == 0.0] = (X[:M], XB[:M])
-        assert torch.equal(_bits(runs[False][0]), _bits(runs[True][0])), f"C={C} M={M}: rows past M reached X"
-        assert torch.equal(_bits(runs[False][1]), _bits(runs[True][1])), f"C={C} M={M}: rows past M reached the copy"
+        assert torch.equal(bits(runs[False][0]), bits(runs[True][0])), f"C={C} M={M}: rows past M reached X"
+        assert torch.equal(bits(runs[False][1]), bits(runs[True][1])), f"C={C} M={M}: rows past M reached the copy"
 
 
 def test_fused_qkv_prefetch_past_m(eng, dev):
@@ -97,4 +87,4 @@ def test_fused_qkv_prefetch_past_m(eng, dev):
             assert torch.isfinite(QKV[:M]).all() and torch.isfinite(G[:M]).all(), f"C={C} M={M}: non-finite rows < M"
             runs[fill == 0.0] = (QKV[:M], G[:M])
         for i, what in enumerate(("qkv", "gates")):
-            assert torch.equal(_bits(runs[False][i]), _bits(runs[True][i])), f"C={C} M={M}: rows past M reached {what}"
+            assert torch.equal(bits(runs[False][i]), bits(runs[True][i])), f"C={C} M={M}: rows past M reached {what}"

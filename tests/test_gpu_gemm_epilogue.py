@@ -1,15 +1,15 @@
 """GPU tests of the staged epilogue of the 16-bit GEMM (gemm_tc_kernel kinds 0 and 1, csrc/kernels_gemm.cu): results
 go through shared-memory staging units and TMA stores, the fp32 residual arrives by TMA into the units the result then
 overwrites.  Checked against the float64 references of tests/gemm_reference.py at the tolerances of
-tests/test_gpu_kernels.py, twice each (bitwise equal), with NaN sentinel rows around the output."""
+tests/numerics.py, twice each (bitwise equal), with NaN sentinel rows around the output."""
 import math
 import zlib
 
 import pytest
 import torch
 
-from gemm_reference import GemmCase, _kind1, plain_shape
-from test_gpu_kernels import _check_gemm_case, _run_gemm, dev, small_h16  # noqa: F401  (fixtures)
+from gemm_reference import GemmCase, _check_gemm_case, _kind1, _run_gemm, plain_shape
+from support import bits, dev, small_h16  # noqa: F401  (fixtures)
 
 pytestmark = pytest.mark.gpu
 
@@ -88,5 +88,5 @@ def test_staged_epilogue_leaves_neighbouring_rows(small_h16, L):
     oa = torch.full(((M + 1) * N,), float("nan"), device=eng.device)
     eng.debug_gemm_full(case.shape, a, w, bias=bias, resid=o32, out_f32=o32, out_act=oa, resid_epilogue=True)
     assert torch.isnan(buf[: guard * N]).all() and torch.isnan(buf[(guard + M) * N :]).all(), "store outside the output"
-    assert torch.equal(o32.view(torch.int32), want32[: M * N].view(torch.int32))
-    assert torch.equal(oa.view(torch.int32), want_act.view(torch.int32))
+    assert torch.equal(bits(o32), bits(want32[: M * N]))
+    assert torch.equal(bits(oa), bits(want_act))

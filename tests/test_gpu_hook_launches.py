@@ -7,16 +7,11 @@ import numpy as np
 import pytest
 import torch
 
+from support import dev  # noqa: F401  (fixture)
+
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(600)]
 
 H16_ONLY = {"fused_qkv", "fused_ff"}
-
-
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.fail("GPU tests need a CUDA device")
-    return torch.device("cuda:0")
 
 
 def _engines(dev):

@@ -10,27 +10,19 @@ Tolerances (stated):
 """
 import math
 import os
-import zlib
 
 import numpy as np
 import pytest
 import torch
 
 from conftest import GOLDEN
-from gemm_reference import GEMM_CASES, epilogue_ref, gemm_ref
+from gemm_reference import GEMM_CASES, _check_gemm_case
+from numerics import H16_TOL
+from support import dev, small_h16  # noqa: F401  (fixtures)
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(600)]
 
-F32_TOL = 1e-3
-H16_TOL = 0.05
 H16_STAGE_TOL = 0.03
-
-
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.fail("GPU tests need a CUDA device")
-    return torch.device("cuda:0")
 
 
 def _engine(ckpt, half):
@@ -42,11 +34,6 @@ def _engine(ckpt, half):
 @pytest.fixture(scope="module")
 def small_f32(small0_ckpt, lib_built, dev):
     return _engine(small0_ckpt, False)
-
-
-@pytest.fixture(scope="module")
-def small_h16(small0_ckpt, lib_built, dev):
-    return _engine(small0_ckpt, True)
 
 
 @pytest.fixture(scope="module")
@@ -126,52 +113,6 @@ def test_peakpick_golden_bit_exact(lib_built, dev):
 
 # ------------------------------------------------------------------------------ GEMM units
 # (the attention kernels: tests/test_gpu_attention.py)
-# GEMM unit tolerances (bt_debug_gemm against the float64 reference of tests/gemm_reference.py, on the operands the
-# kernel multiplies: rounded to the 16-bit type in the 16-bit context):
-#   fp32 outputs  : fp32 accumulation over K <= 2048 of unit-scale products, |ref| ~ 1:
-#                   GEMM_ACC_TOL_H16 (wgmma) / GEMM_ACC_TOL_F32 (CUDA-core fmaf chain) x (1 + |ref|)
-#   16-bit outputs: 1 ulp of the 16-bit-rounded float64 value (the fp32 result may sit on the other side of a rounding
-#                   boundary) + the fp32 bound above, which only matters near zero where the ulp is tiny
-#   GELU          : the 16-bit path evaluates the tanh form with tanh.approx.f32, |error| <= 2^-10.987 (PTX ISA), so
-#                   0.5 |x| 2^-10 on top; the fp32 path the exact erf form (erff)
-#   gates         : GATES_TOL absolute on sigmoid values (slope <= 1/4 of the fp32 accumulation error)
-GEMM_ACC_TOL_H16 = 1e-4
-GEMM_ACC_TOL_F32 = 3e-5
-TANH_APPROX_TOL = 2.0**-10
-GATES_TOL = 1e-6
-
-
-def _act_dtype(eng):
-    return torch.float16 if eng.act_dtype == "f16" else torch.bfloat16
-
-
-def _ulp(x, dt):
-    """Spacing of the 16-bit floating-point type dt at its representable values x (float64)."""
-    mant, emin = (10, -14) if dt == torch.float16 else (7, -126)
-    return torch.exp2(torch.floor(torch.log2(x.abs().clamp_min(2.0**emin))) - mant)
-
-
-def _run_gemm(eng, case, a, w, bias, resid, rope):
-    """One bt_debug_gemm call on fresh output buffers of M + 1 rows: the last row is a NaN sentinel, and every other
-    element starts as NaN too (or as the residual where out_f32 doubles as it), so a missing store shows up."""
-    M, N = case.M, case.shape["N"]
-    ldo = case.heads if case.kind == 2 else N
-    nan = float("nan")
-    o32 = torch.full(((M + 1) * ldo,), nan, device=a.device) if case.out_f32 else None
-    if case.resid:
-        o32[: M * N] = resid.flatten()
-    oa = torch.full(((M + 1) * N,), nan, device=a.device) if case.out_act else None
-    tile = eng.debug_gemm_full(case.shape, a, w, bias=bias if (case.bias or case.kind == 2) else None,
-                               resid=o32 if case.resid else None, out_f32=o32, out_act=oa, rope_cos=rope[0],
-                               rope_sin=rope[1], resid_epilogue=case.resid_epilogue, kind=case.kind, gelu=case.gelu,
-                               C=case.C, heads=case.heads, posmode=case.posmode, F=case.F, qscale=case.qscale)
-    return tile, o32, oa
-
-
-def _bits(t):
-    return None if t is None else t.view(torch.int32)
-
-
 # plain D = A W^T through Engine.debug_gemm, no epilogue (M, N, K)
 GEMM_SHAPES = [(300, 96, 32), (1500, 32, 128), (1000, 64, 64), (700, 192, 64), (1500, 1536, 512), (520, 512, 2048), (257, 128, 256)]
 
@@ -199,61 +140,6 @@ def test_debug_gemm(small_f32, small_h16, half):
         except AssertionError as e:
             failures.append(f"{case.id}: {str(e).splitlines()[0]}")
     assert not failures, f"{len(failures)} of {len(GEMM_CASES)} GEMM cases failed:\n" + "\n".join(failures)
-
-
-def _check_gemm_case(eng, half, case):
-    from beat_this_b200.weights import rope_tables
-
-    dev = eng.device
-    sh, M, N = case.shape, case.M, case.shape["N"]
-    Ktot = sh["Kslab"] * sh["nslab"]
-    g = torch.Generator(device=dev).manual_seed(zlib.crc32(case.id.encode()))
-    a = torch.randn(sh["planes_in"] * sh["L"], sh["lda"], generator=g, device=dev)
-    w = torch.randn(N, Ktot, generator=g, device=dev) / math.sqrt(Ktot)
-    bias = torch.randn(N, generator=g, device=dev) * 0.5
-    resid = torch.randn(M, N, generator=g, device=dev) if case.resid else None
-    freqs = 1.0 / (10000 ** (torch.arange(0, 32, 2).float() / 32))
-    rope = tuple(t.contiguous().to(dev) for t in rope_tables(freqs)) if case.kind == 1 else (None, None)
-
-    tile, o32, oa = _run_gemm(eng, case, a, w, bias, resid, rope)
-    if half:
-        assert tile == case.tile, f"plan tile {tile}, policy {case.tile}"
-        again = _run_gemm(eng, case, a, w, bias, resid, rope)  # the same launch twice: bitwise equal
-        for x, y in zip((o32, oa), again[1:]):
-            assert x is None or torch.equal(_bits(x), _bits(y)), "16-bit GEMM is not deterministic"
-    else:
-        assert tile == (0, 0)
-
-    adt = _act_dtype(eng)
-    rnd = (lambda t: t.to(adt).double()) if half else (lambda t: t.double())
-    acc = gemm_ref(sh, rnd(a), rnd(w))
-    ref, pre = epilogue_ref(case, acc, bias.double(), resid.double() if resid is not None else None, half,
-                            *(t.double() if t is not None else None for t in rope))
-    tol = (GEMM_ACC_TOL_H16 if half else GEMM_ACC_TOL_F32) * (1 + ref.abs())
-    if case.kind == 2:
-        tol = torch.full_like(ref, GATES_TOL)
-    if pre is not None and half:
-        tol = tol + 0.5 * pre.abs() * TANH_APPROX_TOL
-    ldo = ref.shape[1]
-    line = f"gemm {'h16' if half else 'f32'} {case.id}: tile {tile[0]}x{tile[1]} kind {case.kind} M={M} N={N} K={Ktot}"
-
-    def check(name, got, ref, bound):
-        err = (got - ref).abs().nan_to_num(float("inf"))  # an unwritten (NaN) element fails
-        worst, ratio = err.max().item(), (err / bound).max().item()
-        print(f"{line} | {name} max abs err {worst:.3e} = {ratio:.2f} of its bound")
-        assert ratio <= 1, f"{name} off by up to {worst:.3e}, {ratio:.2f} x its bound"
-
-    if o32 is not None:
-        assert torch.isnan(o32[M * ldo :]).all(), "fp32 store past the last row"
-        check("f32 out", o32[: M * ldo].view(M, ldo).double(), ref, tol)
-    if oa is not None:
-        assert torch.isnan(oa[M * N :]).all(), "activation store past the last row"
-        got = oa[: M * N].view(M, N).double()
-        if half:
-            ref16 = ref.to(adt).double()
-            check(f"{eng.act_dtype} out", got, ref16, _ulp(ref16, adt) + tol)
-        else:
-            check("act out (fp32)", got, ref, tol)
 
 
 @pytest.mark.parametrize("sr", [44100, 48000, 16000, 96000])

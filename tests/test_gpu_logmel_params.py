@@ -19,17 +19,11 @@ import torch
 
 import logmel_reference as R
 from conftest import GOLDEN
+from support import dev  # noqa: F401  (fixture)
 
-pytestmark = [pytest.mark.gpu, pytest.mark.timeout(900)]
+pytestmark = [pytest.mark.gpu, pytest.mark.timeout(900), pytest.mark.usefixtures("lib_built")]
 
 REF_TOL = 2e-3
-
-
-@pytest.fixture(scope="module")
-def dev(lib_built):
-    if not torch.cuda.is_available():
-        pytest.fail("GPU tests need a CUDA device")
-    return torch.device("cuda:0")
 
 
 @pytest.fixture(scope="module")

@@ -15,9 +15,10 @@ import torch
 
 import attention_reference as R
 from conftest import GOLDEN, ckpt_path
-from gemm_reference import _kind1, epilogue_ref, gemm_ref
-from test_gpu_attention import _act_dtype, _launch_twice, _ulp
-from test_gpu_kernels import F32_TOL, GEMM_ACC_TOL_F32, GEMM_ACC_TOL_H16, H16_TOL, _run_gemm
+from gemm_reference import _kind1, _run_gemm, epilogue_ref, gemm_ref
+from numerics import (EX2_APPROX_REL, EXPF_REL, F32_TOL, GEMM_ACC_TOL_F32, GEMM_ACC_TOL_H16, H16_TOL, LOG2E, QSCALE_H16,
+                      S_F32, U, mma_error, rnd, ulp16)
+from support import act_dtype, launch_twice
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(1800)]
 
@@ -198,9 +199,9 @@ def time_ref_rows(q, k, v, gates, lens, path, dt, r0, r1):
     H = C // 32
     hv = lambda t: t.reshape(seqs, L, H, 32).permute(0, 2, 1, 3).reshape(seqs * H, L, 32)  # noqa: E731
     if path == "tc":
-        qh, kh, vh, sc = hv(R.rnd(R._f32mul(q, R.QSCALE_F32), dt)), hv(R.rnd(k, dt)), hv(R.rnd(v, dt)), 1.0
+        qh, kh, vh, sc = hv(rnd(R._f32mul(q, QSCALE_H16), dt)), hv(rnd(k, dt)), hv(rnd(v, dt)), 1.0
     else:
-        qh, kh, vh, sc = hv(R._f32mul(q, R.S_F32)), hv(k), hv(v), R.LOG2E
+        qh, kh, vh, sc = hv(R._f32mul(q, S_F32)), hv(k), hv(v), LOG2E
     g = gates.reshape(seqs, L, H).permute(0, 2, 1).reshape(seqs * H, L)[:, r0:r1]
     qh = qh[:, r0:r1]
     lens_g = torch.as_tensor(lens, device=q.device).repeat_interleave(H)
@@ -214,16 +215,16 @@ def time_ref_rows(q, k, v, gates, lens, path, dt, r0, r1):
         nkv = (vm.sum(-1) + R.AT_TILE - 1) // R.AT_TILE
         if path == "tc":
             pk = R.poly_keys(L, q.device)
-            kw = dict(step=R.AT_TILE, alpha_rel=R.EX2_APPROX_REL + R.U, sub_ops=1, p_dt=dt, n_sum=16 * nkv + 2,
-                      pv_error=lambda s, nnz: R.mma_error(nnz, s), out_dt=dt, n_pad=R.AT_TILE,
-                      exp_rel=lambda x, e: torch.where(pk, R.EX2_POLY_REL, R.EX2_APPROX_REL).expand_as(x))
-            E2 = R.mma_error(32, S)
+            kw = dict(step=R.AT_TILE, alpha_rel=EX2_APPROX_REL + U, sub_ops=1, p_dt=dt, n_sum=16 * nkv + 2,
+                      pv_error=lambda s, nnz: mma_error(nnz, s), out_dt=dt, n_pad=R.AT_TILE,
+                      exp_rel=lambda x, e: torch.where(pk, R.EX2_POLY_REL, EX2_APPROX_REL).expand_as(x))
+            E2 = mma_error(32, S)
         else:
             nk = R.SA_BLOCK * ((vm.sum(-1) + R.SA_BLOCK - 1) // R.SA_BLOCK)
-            kw = dict(step=R.SA_BLOCK, alpha_rel=R.EXPF_REL + R.U, sub_ops=1, p_dt=None, n_sum=nk,
-                      pv_error=lambda s, nnz: nk[:, None, None] * R.U * s, out_dt=None, n_pad=0,
-                      exp_rel=lambda x, e: torch.full_like(x, R.EXPF_REL))
-            E2 = 32 * R.U * S * R.LOG2E
+            kw = dict(step=R.SA_BLOCK, alpha_rel=EXPF_REL + U, sub_ops=1, p_dt=None, n_sum=nk,
+                      pv_error=lambda s, nnz: nk[:, None, None] * U * s, out_dt=None, n_pad=0,
+                      exp_rel=lambda x, e: torch.full_like(x, EXPF_REL))
+            E2 = 32 * U * S * LOG2E
         for o, r in zip(out, R.softmax_ref(T2, E2, vm, vh[a:b], g[a:b], **kw)):
             o[a:b] = r
     n = r1 - r0
@@ -247,7 +248,7 @@ def test_row_slices_are_the_reference(engines, half):
     g = torch.Generator(device=dev).manual_seed(5)
     q, k, v, gates = (t.double() for t in R.time_inputs(case, "random", g, dev))
     lens = torch.tensor(case.lens(), device=dev)
-    path, dt = ("tc", _act_dtype(engines[True])) if half else ("simt", None)
+    path, dt = ("tc", act_dtype(engines[True])) if half else ("simt", None)
     full = R.time_ref(q, k, v, gates, lens, path, dt)
     for r0, r1 in ((0, 512), (512, 1024), (1024, 1501)):
         for f, s in zip(full, time_ref_rows(q, k, v, gates, lens, path, dt, r0, r1)):
@@ -261,7 +262,7 @@ def test_attention_at_long_L(engines, half):
     row): every element within the derived bound of attention_reference, finite, no store past M, repeatable."""
     eng = engines[half]
     dev = torch.device("cuda:0")
-    path, dt = ("tc", _act_dtype(eng)) if half else ("simt", None)
+    path, dt = ("tc", act_dtype(eng)) if half else ("simt", None)
     failures, worst = [], {}
     for case in LONG_TIME_CASES:
         families = ["random", "late_max"] + (["masked_garbage"] if case.key_lens is not None else [])
@@ -269,7 +270,7 @@ def test_attention_at_long_L(engines, half):
             g = torch.Generator(device=dev).manual_seed(zlib.crc32(f"{case.id} {family}".encode()))
             q, k, v, gates = R.time_inputs(case, family, g, dev)
             M, C = case.seqs * case.L, 32 * case.heads
-            got = _launch_twice(lambda out: eng.debug_attention(q, k, v, gates, case.key_lens, case.spc, out=out),
+            got = launch_twice(lambda out: eng.debug_attention(q, k, v, gates, case.key_lens, case.spc, out=out),
                                 M, C, dev).view(case.seqs, case.L, C)
             lens = torch.tensor(case.lens(), device=dev)
             ratio = 0.0
@@ -293,7 +294,7 @@ def test_attention_at_long_L(engines, half):
 @pytest.mark.parametrize("half", [False, True])
 def test_rope_gemm_past_1500(engines, half):
     """The RoPE epilogue (kind 1) of gemm_tc_kernel / gemm_simt_kernel at positions up to 8000 and 24000, with tables of
-    that many rows, against gemm_reference (the tolerances of test_gpu_kernels' GEMM cases)."""
+    that many rows, against gemm_reference (the GEMM tolerances of numerics.py)."""
     from beat_this_b200.weights import rope_tables
 
     eng = engines[half]
@@ -308,14 +309,15 @@ def test_rope_gemm_past_1500(engines, half):
         rope = tuple(t.contiguous().to(dev) for t in rope_tables(freqs, P))
         _, _, oa = _run_gemm(eng, case, a, w, None, None, rope)
         assert torch.isnan(oa[M * N :]).all(), "activation store past the last row"
-        adt = _act_dtype(eng)
-        rnd = (lambda t: t.to(adt).double()) if half else (lambda t: t.double())  # noqa: E731
-        ref, _ = epilogue_ref(case, gemm_ref(sh, rnd(a), rnd(w)), None, None, half, *(t.double() for t in rope))
+        adt = act_dtype(eng)
+        dt = adt if half else None
+        ref, _ = epilogue_ref(case, gemm_ref(sh, rnd(a.double(), dt), rnd(w.double(), dt)), None, None, half,
+                              *(t.double() for t in rope))
         tol = (GEMM_ACC_TOL_H16 if half else GEMM_ACC_TOL_F32) * (1 + ref.abs())
         got = oa[: M * N].view(M, N).double()
         if half:
             ref = ref.to(adt).double()
-            tol = _ulp(ref, adt) + tol
+            tol = ulp16(ref, adt) + tol
         err = (got - ref).abs().nan_to_num(float("inf"))
         ratio = (err / tol).max().item()
         print(f"gemm {'h16' if half else 'f32'} {case.id}, table of {P} rows: max abs err {err.max().item():.3e} = "

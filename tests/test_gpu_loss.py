@@ -8,7 +8,7 @@ import pytest
 import torch
 
 import loss_reference as R
-from test_cpu_loss import CASES, GRAD_TOL, fixture_case
+from loss_reference import CASES, GOLD, GRAD_TOL, fixture_case
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(1800)]
 DEV = "cuda:0"
@@ -86,7 +86,6 @@ def test_kernel_equals_restatement(lib_built, kind, t, pw):
 @pytest.mark.parametrize("k", CASES)
 def test_modules_against_reference_fixture(lib_built, k):
     from beat_this_b200 import loss as L
-    from test_cpu_loss import GOLD
 
     kind, t, pw, has_mask = GOLD[f"spec{k}"]
     kind, t = int(kind), int(t)

@@ -12,30 +12,9 @@ from beat_this_b200.engine import Engine
 from beat_this_b200.loss import ShiftTolerantBCELoss
 from beat_this_b200.train import BeatThisModule
 from oracle import beat_this_oracle as O
+from support import DEV, GRAD_BOUND, LOGIT_TOL, _module, _rel, _spect
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-GRAD_BOUND = 1e-4  # per tensor: ||g - g64|| / ||g64||
-LOGIT_TOL = 1e-3   # the fp32 inference path's bound against the oracle (tests/test_gpu_kernels.py, smoke())
-
-
-def _module(family, seed=0, **overrides):
-    """A module on a seeded synthetic checkpoint of `family`, with hyper-parameters overridden as given."""
-    ckpt = synthetic.make_checkpoint(family, seed)
-    if overrides:
-        hp = dict(ckpt["hyper_parameters"], **overrides)
-        ckpt = dict(ckpt, hyper_parameters=hp,
-                    state_dict={"model." + k: v for k, v in synthetic.make_state_dict(hp, seed).items()})
-    return BeatThisModule.from_checkpoint(ckpt, DEV), ckpt
-
-
-def _spect(B, L, seed, lengths=None):
-    g = torch.Generator().manual_seed(seed)
-    x = torch.rand(B, L, 128, generator=g) * 4.0
-    if lengths is not None:  # zero-padded as TrainingBatches yields a batch of shorter pieces
-        for b, n in enumerate(lengths):
-            x[b, n:] = 0
-    return x
 
 
 def _oracle(module, x, dbeat, ddown, sum_head):
@@ -47,11 +26,6 @@ def _oracle(module, x, dbeat, ddown, sum_head):
     names = [k for k, v in sd.items() if v.is_floating_point() and v.requires_grad]
     grads = torch.autograd.grad((beat, down), [x64] + [sd[k] for k in names], (dbeat.double(), ddown.double()))
     return beat.detach(), down.detach(), grads[0], dict(zip(names, grads[1:]))
-
-
-def _rel(g, ref):
-    g = g.detach().double().cpu()
-    return float((g - ref).norm() / ref.norm().clamp_min(1e-300))
 
 
 CASES = [  # family, B, L, lengths of a zero-padded batch (None: dense), hyper-parameter overrides

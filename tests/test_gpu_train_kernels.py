@@ -11,6 +11,8 @@ import torch
 import train_kernels_reference as R
 from beat_this_b200 import _lib
 from beat_this_b200.engine import Engine
+from numerics import REL_2ULP, worst
+from support import rnd
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(1800)]
 DEV = "cuda:0"
@@ -18,17 +20,6 @@ PAD = 37           # sentinel elements after every output
 SENTINEL = 1234.5
 RATIOS = {}
 COVERED = set()    # kernels the cases launch (tests/test_cpu_train_sass.py lists the library's)
-
-KERNELS = {  # op -> the kernels it launches
-    "gemm": ("tr_gemm_kernel", "tr_reduce_kernel"), "reduce": ("tr_reduce_kernel",),
-    "colsum": ("tr_colsum_kernel", "tr_reduce_kernel"), "rms_fwd": ("tr_rms_fwd_kernel",),
-    "rms_bwd": ("tr_rms_bwd_kernel",), "bn_gelu_fwd": ("tr_bn_gelu_fwd_kernel",),
-    "bn_gelu_bwd": ("tr_bn_gelu_bwd_kernel",), "bn_grads": ("tr_bn_grads_kernel",), "bn_scale": ("tr_bn_scale_kernel",),
-    "gelu_bwd": ("tr_gelu_bwd_kernel",), "im2col": ("tr_im2col_kernel",), "col2im": ("tr_col2im_kernel",),
-    "concat": ("tr_concat_kernel",), "rope": ("tr_rope_kernel",), "gate_fwd": ("tr_gate_fwd_kernel",),
-    "gate_bwd": ("tr_gate_bwd_kernel",), "head_fwd": ("tr_head_fwd_kernel",), "head_bwd": ("tr_head_bwd_kernel",),
-    "attn_fwd": ("tr_attn_fwd_kernel",), "attn_dq": ("tr_attn_dq_kernel",), "attn_dkv": ("tr_attn_dkv_kernel",),
-}
 
 
 @pytest.fixture(scope="module")
@@ -38,10 +29,6 @@ def eng(lib_built):
 
 def _g(seed):
     return torch.Generator().manual_seed(seed)
-
-
-def rnd(*shape, g, scale=1.0):
-    return (torch.randn(*shape, generator=g) * scale).float()
 
 
 def out(n):
@@ -79,13 +66,13 @@ def run(eng, op, arrays, **desc):
         assert torch.equal(x.view(torch.int32), y.view(torch.int32)), f"{op}: not bitwise repeatable"
         if isinstance(a, tuple):
             assert (x[x.numel() - PAD:] == SENTINEL).all(), f"{op}: wrote past its output"
-    COVERED.update(KERNELS[op])
+    COVERED.update(R.KERNELS[op])
     return [None if b is None else (b[: b.numel() - PAD] if isinstance(a, tuple) else b).cpu()
             for a, b in zip(arrays, results[0])]
 
 
 def check(op, case, got, ref, bound):
-    r = R.worst(got, ref, bound)
+    r = worst(got, ref, bound)
     RATIOS[op] = max(RATIOS.get(op, 0.0), r)
     assert r <= 1.0, f"{op} {case}: {r:.3g} x the bound"
 
@@ -145,7 +132,7 @@ def _run_alias(eng, arrays, **desc):
         results.append([cb[: cb.numel() - PAD].cpu()] + [None if b is None else b[: b.numel() - PAD].cpu()
                                                            for b in bufs[5:]])
     assert torch.equal(results[0][0], results[1][0])
-    COVERED.update(KERNELS["gemm"])
+    COVERED.update(R.KERNELS["gemm"])
     return [None, None, results[0][0], None, None, results[0][1], results[0][2]]
 
 
@@ -355,7 +342,7 @@ def test_rope(eng, posmode, F, L, M, C):
         assert torch.equal(got[:, 2 * C:], qkv[:, 2 * C:]), "v columns changed"
     fwd = run(eng, "rope", [padded(qkv), dev(fr)], M=M, C=C, L=L, F=F, posmode=posmode, flag=0)[0]
     back = run(eng, "rope", [padded(fwd), dev(fr)], M=M, C=C, L=L, F=F, posmode=posmode, flag=1)[0]
-    ident = (R.ULP2 + 3 * R.U) * 4 * (qkv.abs().reshape(M, 3 * C) + qkv.abs().reshape(M, 3 * C).roll(1, 1)
+    ident = (REL_2ULP + 3 * R.U) * 4 * (qkv.abs().reshape(M, 3 * C) + qkv.abs().reshape(M, 3 * C).roll(1, 1)
                                       + qkv.abs().reshape(M, 3 * C).roll(-1, 1)).double() + 1e-37
     check("rope", f"pm{posmode} identity", back.reshape(M, 3 * C), qkv.double(), ident)
 
@@ -482,7 +469,7 @@ def test_refused_geometries(eng):
 
 def test_zz_every_kernel_covered_and_report():
     """Runs last: every training kernel was launched by some case, and the worst ratios are printed."""
-    want = {k for ks in KERNELS.values() for k in ks}
+    want = {k for ks in R.KERNELS.values() for k in ks}
     assert want <= COVERED, f"not launched: {sorted(want - COVERED)}"
     for op in sorted(RATIOS):
         print(f"train kernel {op:12s} worst |err| / bound = {RATIOS[op]:.3g}")

@@ -16,10 +16,9 @@ from beat_this_b200.engine import Engine
 from beat_this_b200.loss import ShiftTolerantBCELoss
 from beat_this_b200.train import BeatThisModule
 from oracle import philox
-from test_gpu_train import GRAD_BOUND, LOGIT_TOL, _module, _rel, _spect
+from support import DEV, GRAD_BOUND, LOGIT_TOL, _module, _rel, _spect
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(1800)]
-DEV = "cuda:0"
 RATES = (0.1, 0.2, 0.5, 0.9)
 BIG = 5 * 2 ** 32 + 3  # a starting element index past 2^32 (B = 64 at L = 1500 reaches such indices)
 # Batch-statistics BatchNorm makes each channel's input gradient sum to zero, so a bias gradient upstream of one is a

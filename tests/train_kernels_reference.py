@@ -57,29 +57,25 @@ import math
 import numpy as np
 import torch
 
-U = 2.0**-24
+from numerics import (EXPF_REL, GELU2_SLOPE, GELU_SLOPE, LOG2E, REL_2ULP, S_F32, U, f32, f64, fma_f32, gelu_erf,
+                      rope_positions)
+
 SAFE = 1.0 + 2.0**-10
 TINY = 2.0**-140
-ULP2 = 2.0**-22  # 2 ulp, relative
-GELU_SLOPE = 1.13  # max |GELU'| = 1.1290 at sqrt 2
-GELU2_SLOPE = 0.8  # max |GELU''| = 0.7979 at 0
 BN_EPS = 1e-5
-S_F32 = float(np.float32(0.17677669529663687))
-
-
-def f64(t):
-    return torch.as_tensor(t).double()
-
-
-def f32(v):
-    return float(np.float32(v))
+KERNELS = {  # op -> the kernels it launches
+    "gemm": ("tr_gemm_kernel", "tr_reduce_kernel"), "reduce": ("tr_reduce_kernel",),
+    "colsum": ("tr_colsum_kernel", "tr_reduce_kernel"), "rms_fwd": ("tr_rms_fwd_kernel",),
+    "rms_bwd": ("tr_rms_bwd_kernel",), "bn_gelu_fwd": ("tr_bn_gelu_fwd_kernel",),
+    "bn_gelu_bwd": ("tr_bn_gelu_bwd_kernel",), "bn_grads": ("tr_bn_grads_kernel",), "bn_scale": ("tr_bn_scale_kernel",),
+    "gelu_bwd": ("tr_gelu_bwd_kernel",), "im2col": ("tr_im2col_kernel",), "col2im": ("tr_col2im_kernel",),
+    "concat": ("tr_concat_kernel",), "rope": ("tr_rope_kernel",), "gate_fwd": ("tr_gate_fwd_kernel",),
+    "gate_bwd": ("tr_gate_bwd_kernel",), "head_fwd": ("tr_head_fwd_kernel",), "head_bwd": ("tr_head_bwd_kernel",),
+    "attn_fwd": ("tr_attn_fwd_kernel",), "attn_dq": ("tr_attn_dq_kernel",), "attn_dkv": ("tr_attn_dkv_kernel",),
+}
 
 
 # ------------------------------------------------------------------------------------ restatements and bounds
-def gelu(x):
-    return 0.5 * x * (1 + torch.erf(x / math.sqrt(2)))
-
-
 def gelu_grad(x):
     return 0.5 * (1 + torch.erf(x / math.sqrt(2))) + x * torch.exp(-0.5 * x * x) / math.sqrt(2 * math.pi)
 
@@ -91,8 +87,8 @@ def gelu_grad_err(x, ex):
     ax = x.abs()
     cdf = 0.5 * (1 + torch.erf(x / math.sqrt(2)))
     pdf = torch.exp(-0.5 * x * x) / math.sqrt(2 * math.pi)
-    e_cdf = 0.5 * (ULP2 + U * ax * 2 / math.sqrt(math.pi) * torch.exp(-0.5 * x * x) / math.sqrt(2) + U * (1 + cdf))
-    e_pdf = pdf * (ULP2 + 4 * U + U * x * x)  # expf 2 ulp; the argument's 2 products (u x^2 absolute); k, the product
+    e_cdf = 0.5 * (REL_2ULP + U * ax * 2 / math.sqrt(math.pi) * torch.exp(-0.5 * x * x) / math.sqrt(2) + U * (1 + cdf))
+    e_pdf = pdf * (REL_2ULP + 4 * U + U * x * x)  # expf 2 ulp; the argument's 2 products (u x^2 absolute); k, the product
     xp = ax * pdf
     return GELU2_SLOPE * ex + e_cdf + ax * e_pdf + U * xp + U * (cdf + xp) + U * (cdf + xp).abs()
 
@@ -114,7 +110,7 @@ def gemm_ref(A, B, bias=None, resid=None, splits=1, scale=1.0):
     if resid is not None:
         C, S = C + f64(resid), S + f64(resid).abs()
     e = SAFE * ((kc + (Z if Z > 1 else 0) + 3) * U * S + U * C.abs()) + TINY
-    g = gelu(C)
+    g = gelu_erf(C)
     eg = SAFE * (GELU_SLOPE * e + 2.0**-21 * C.abs() + U * g.abs()) + TINY
     return C, e, g, eg
 
@@ -211,7 +207,7 @@ def bn_apply(z, bn, c):
 def bn_gelu_fwd_ref(z, bn, C):
     z = f64(z)
     x, ex = bn_apply(z, bn, torch.arange(z.numel()) % C)
-    y = gelu(x)
+    y = gelu_erf(x)
     return y, SAFE * (GELU_SLOPE * ex + 2.0**-21 * x.abs() + U * y.abs()) + TINY
 
 
@@ -309,11 +305,6 @@ def concat_ref(src, B, F, L, C, backward):
     return s.reshape(B, F, L, C).permute(0, 2, 3, 1).reshape(-1)
 
 
-def rope_positions(M, L, F, posmode):
-    m = torch.arange(M)
-    return m % L if posmode == 0 else (m // L) % F
-
-
 def rope_ref(qkv, freqs, L, F, posmode, inverse):
     """(qkv', bound) of rotary_embedding_torch's rotation (angle fl32(pos fl32(freq))) of the q and k columns of qkv
     [M, 3C] by +angle (inverse: -angle); v is untouched."""
@@ -332,15 +323,15 @@ def rope_ref(qkv, freqs, L, F, posmode, inverse):
     t0, t1 = (x0 * co).abs() + (x1 * si).abs(), (x1 * co).abs() + (x0 * si).abs()
     e = torch.zeros_like(x)
     x[:, 0:2 * C:2], x[:, 1:2 * C:2] = y0, y1
-    e[:, 0:2 * C:2] = SAFE * ((ULP2 + 3 * U) * t0) + 2.0**-148 * (x0.abs() + x1.abs())
-    e[:, 1:2 * C:2] = SAFE * ((ULP2 + 3 * U) * t1) + 2.0**-148 * (x0.abs() + x1.abs())
+    e[:, 0:2 * C:2] = SAFE * ((REL_2ULP + 3 * U) * t0) + 2.0**-148 * (x0.abs() + x1.abs())
+    e[:, 1:2 * C:2] = SAFE * ((REL_2ULP + 3 * U) * t1) + 2.0**-148 * (x0.abs() + x1.abs())
     return x, e
 
 
 def sigmoid_err(g):
     sg = torch.sigmoid(g)
     # expf(-g) 2 ulp relative, 1 + e and the division: the relative error of 1 / (1 + e) is (e / (1 + e)) 2^-22 + 2 u
-    return sg, sg * ((1 - sg) * ULP2 + 2 * U)
+    return sg, sg * ((1 - sg) * REL_2ULP + 2 * U)
 
 
 def gate_fwd_ref(O, g):
@@ -403,7 +394,7 @@ def _heads(t, rows, H, off, width):
 
 def attn_fwd_ref(qkv, rows, H, lse_log2=False):
     """(O, bound, lse, lse bound) [seqs * H, n, 32] / [seqs * H, n] of the forward over sequences `rows` [seqs, n]."""
-    from attention_reference import EXPF_REL, LOG2E, softmax_ref
+    from attention_reference import softmax_ref
 
     C = 32 * H
     t = f64(qkv)
@@ -447,7 +438,7 @@ def attn_bwd_ref(qkv, dO, lse, delta, rows, H):
     e_a = (32 + 2) * U * S_F32 * (q.abs() @ k.abs().transpose(1, 2))
     x = a - L_[..., None]
     p = torch.exp(x)
-    e_p = p * (e_a + U * x.abs() + ULP2)
+    e_p = p * (e_a + U * x.abs() + REL_2ULP)
     dp = do @ v.transpose(1, 2)
     e_dp = 32 * U * (do.abs() @ v.abs().transpose(1, 2))
     diff = dp - D_[..., None]
@@ -471,24 +462,9 @@ def heads_back(x, rows, H, n_rows, off, width, base=None):
     return out
 
 
-def worst(got, ref, bound):
-    """max |got - ref| / bound (NaN in got or a non-finite difference: inf)."""
-    got, ref, bound = f64(got), f64(ref), f64(bound)
-    d = (got - ref).abs()
-    if not torch.isfinite(d).all():
-        return math.inf
-    r = torch.where(d == 0, torch.zeros_like(d), d / bound)
-    return float(r.max()) if d.numel() else 0.0
-
-
 # ------------------------------------------------------------------------------------ fp32 emulations
-# numpy fp32 in the kernels' operation order.  fmaf is an exact float64 product plus one rounded add (two roundings:
-# off by one ulp in rare cases, so these are not bitwise oracles).  `mistake` plants one single-line error.
+# numpy fp32 in the kernels' operation order (fmaf: numerics.fma_f32).  `mistake` plants one single-line error.
 F = np.float32
-
-
-def _fma(a, b, c):
-    return (a.astype(np.float64) * b + c).astype(F)
 
 
 def emu_bn_scale(w, rv, mistake=None):
@@ -539,7 +515,7 @@ def emu_gemm(A, B, splits=1, mistake=None):
             for k in range(k0, k0 + 16):
                 lim = K if mistake == "gemm_mask_at_K" else ke
                 if k < lim:
-                    acc = _fma(A[:, k:k + 1], B[:, k][None, :], acc)
+                    acc = fma_f32(A[:, k:k + 1], B[:, k][None, :], acc)
         parts.append(acc)
     return emu_reduce(np.stack(parts), 1.0, mistake) if Z > 1 else parts[0]
 
