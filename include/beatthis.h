@@ -586,6 +586,18 @@ typedef struct bt_train_mode {
   uint64_t seed;
   float dropout_frontend, dropout_transformer;
 } bt_train_mode;
+/* The activation store's layout (fp32, offsets in floats; each region rounded up to 4 floats, pads never written).
+ * Per step of the layer list, in order, with M = B L F token rows of the step's C channels (frontend row
+ * ((b F + f) L + t), main row b L + t):
+ *   stem       in [B L, 128] (the spectrogram), z [M, C] (the convolution before bn2d)
+ *   attention  in [M, C], xn [M, C], inv [M] (1 / ||in||), qkv [M, 3C] (q and k after RoPE), gate logits [M, C/32],
+ *              lse [M, C/32] (natural log), o [M, C] (attention output before the gates)
+ *   FFN        in [M, C], xn [M, C], inv [M], h [M, mult C] (before GELU), a [M, mult C] (after GELU and dropout)
+ *   conv       in [M, C], z [M / 2, 2C] (the convolution before the norm)
+ *   linear     in [M, C], xl [B L, C F] (the gathered rows)
+ *   head       in [B L, D], xn [B L, D], inv [B L]
+ * A step's input is the previous step's output.  Training mode appends, per BatchNorm in layer order (the stem's bn1d
+ * then bn2d, each convolution's norm), its batch mean then its biased variance, ch floats each. */
 int64_t bt_train_activation_bytes_ex(const bt_ctx* ctx, int32_t B, int32_t L, const bt_train_mode* mode);
 int bt_train_forward_ex(bt_ctx* ctx, const float* const* params, int32_t n_params, float* const* running,
                         const float* spect_dev, int32_t B, int32_t L, const bt_train_mode* mode, void* act_dev,
