@@ -17,8 +17,9 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 # BT_LIB_PATH: an instrumented build of the same sources (e.g. build(extra_flags=("-DBT_FF_PROF",), out_path=...))
 LIB_PATH = os.environ.get("BT_LIB_PATH") or os.path.join(HERE, "libbeatthis_sm90.so")
-SOURCES = ["bt_api.cu", "api_signal.cu", "api_post.cu", "api_data.cu", "api_train.cu", "api_debug.cu", "kernels_simt.cu", "kernels_misc.cu", "kernels_signal.cu", "kernels_gemm.cu", "kernels_attn.cu", "kernels_fused.cu", "kernels_dbn.cu", "kernels_eval.cu", "kernels_loss.cu", "kernels_data.cu", "kernels_train.cu", "kernels_optim.cu", "dbn_host.cpp", "host_stage.cpp"]
-HEADERS = ["common.cuh", "epilogue.cuh", "fft.cuh", "tc_common.cuh", "bt_kernels.h", "bt_train.h", "cuda_owned.h", "dbn_model.h",
+SOURCES = ["bt_api.cu", "api_signal.cu", "api_post.cu", "api_data.cu", "api_train.cu", "api_debug.cu", "kernels_simt.cu", "kernels_misc.cu", "kernels_signal.cu", "kernels_gemm.cu", "kernels_attn.cu", "kernels_fused.cu", "kernels_dbn.cu", "kernels_eval.cu", "kernels_loss.cu", "kernels_data.cu", "kernels_train.cu", "kernels_optim.cu", "kernels_dp.cu", "dbn_host.cpp", "host_stage.cpp"]
+HEADERS = ["common.cuh", "epilogue.cuh", "fft.cuh", "tc_common.cuh", "chunk_table.cuh", "bt_kernels.h", "bt_train.h", "cuda_owned.h",
+           "dbn_model.h",
            "api_internal.h", os.path.join("..", "..", "include", "beatthis.h")]
 
 BT_DTYPE_F32 = 0
@@ -136,6 +137,13 @@ class bt_adamw_entry(ctypes.Structure):
         ("eps", c_double),
         ("weight_decay", c_double),
         ("step", c_int64),
+    ]
+
+
+class bt_grad_entry(ctypes.Structure):
+    _fields_ = [
+        ("grad", c_void_p),
+        ("numel", c_int64),
     ]
 
 
@@ -323,6 +331,11 @@ PROTOTYPES = {
                 c_void_p, c_void_p, POINTER(c_void_p), c_void_p, c_void_p],
     ),
     "bt_adamw_step": (c_int, [c_void_p, POINTER(bt_adamw_entry), c_int32, c_void_p]),
+    "bt_grad_pack": (c_int, [c_void_p, POINTER(bt_grad_entry), c_int32, c_void_p, c_void_p]),
+    "bt_grad_ordered_sum": (c_int, [c_void_p, POINTER(bt_grad_entry), c_int32, POINTER(c_void_p), c_int32, c_void_p]),
+    "bt_train_running_replay": (
+        c_int, [c_void_p, POINTER(c_void_p), c_int32, POINTER(c_void_p), c_int32, c_int32, c_int32, c_void_p],
+    ),
     "bt_debug_attention_backward": (
         c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p,
                 c_void_p],

@@ -3,6 +3,8 @@
 // unfolded fp32 device tensors; the forward pass saves what the backward pass reads in the caller's activation store.
 // A bt_train_mode selects the reference's training-mode function: dropout and batch-statistics BatchNorm.
 // bt_adamw_step: the AdamW update of a parameter table in one launch (csrc/kernels_optim.cu).
+// Data-parallel training: bt_grad_pack and bt_grad_ordered_sum (csrc/kernels_dp.cu) move a gradient table into and out
+// of packed rows, and bt_train_running_replay applies captured batch statistics to the running statistics.
 #include "api_internal.h"
 #include "bt_train.h"
 #include "common.cuh"
@@ -221,20 +223,46 @@ struct TrRun {
     if (_r != BT_OK) return _r;  \
   } while (0)
 
+// The running statistics rm, rv of a BatchNorm of ch channels moved towards a batch mean and biased variance over N
+// positions (momentum 0.1, the unbiased variance N / (N - 1)).  The training-mode forward pass and
+// bt_train_running_replay make the same launches.
+int running_update(bt_ctx* c, cudaStream_t st, const float* mean, const float* var, int64_t N, int ch, float* rm,
+                   float* rv) {
+  launch_tr_reduce(mean, 1, ch, 0.1f, rm, st, 0.9f);
+  TR_OK(check_launch(c, "train_reduce", st));
+  launch_tr_reduce(var, 1, ch, static_cast<float>(0.1 * static_cast<double>(N) / static_cast<double>(N - 1)), rv, st,
+                   0.9f);
+  return check_launch(c, "train_reduce", st);
+}
+
 // Training mode: the batch mean and biased variance (two passes: the mean, then centred squares) of x [N, ch] into the
-// store at off, and the running statistics of the BatchNorm at table index p moved towards them (momentum 0.1, the
-// unbiased variance N / (N - 1)).
+// store at off, and the running statistics of the BatchNorm at table index p moved towards them.
 int bn_stats(TrRun& R, const float* x, int64_t N, int ch, int p, int64_t off) {
   float* mean = R.at(off);
   float* var = R.at(off + ((ch + 3) & ~3));
   const float inv_n = static_cast<float>(1.0 / static_cast<double>(N));
   TR_OK(R.colsum(x, nullptr, nullptr, N, ch, inv_n, mean));
   TR_OK(R.colsum(x, nullptr, nullptr, N, ch, inv_n, var, mean));
-  launch_tr_reduce(mean, 1, ch, 0.1f, R.running[p + 2], R.st, 0.9f);
-  TR_OK(check_launch(R.c, "train_reduce", R.st));
-  launch_tr_reduce(var, 1, ch, static_cast<float>(0.1 * static_cast<double>(N) / static_cast<double>(N - 1)),
-                   R.running[p + 3], R.st, 0.9f);
-  return check_launch(R.c, "train_reduce", R.st);
+  return running_update(R.c, R.st, mean, var, N, ch, R.running[p + 2], R.running[p + 3]);
+}
+
+// The BatchNorms of a training-mode pass over B x L frames in the order the forward pass updates them: table index p of
+// the BatchNorm's weight, offset of its batch mean in the store (its variance follows, 4-float aligned), channels and
+// positions N.
+struct TrBnStat {
+  int p;
+  int64_t off;
+  int ch;
+  int64_t N;
+};
+std::vector<TrBnStat> bn_stat_list(const TrModel& m, const bt_hparams& hp, int64_t B, int64_t L) {
+  std::vector<TrBnStat> out;
+  for (const TrLayer& l : m.layers) {
+    const int64_t M = B * L * l.F;
+    if (l.kind == kStem) out.push_back({l.p, l.bn1, hp.spect_dim, B * L}), out.push_back({l.p + 6, l.bn2, l.C, M});
+    if (l.kind == kConv) out.push_back({l.p + 1, l.bn2, 2 * l.C, M / 2});
+  }
+  return out;
 }
 
 // Each step reads l.in and writes the next step's in (the head: the logits).  step: its index in the layer list.
@@ -468,6 +496,39 @@ int train_prepare(bt_ctx* c, const char* fn, const void* const* params, int32_t 
   return BT_OK;
 }
 
+// The running statistics every BatchNorm updates: the table and its running_mean / running_var entries must be set.
+int check_running(bt_ctx* c, const char* fn, const TrModel& m, float* const* running) {
+  if (!running) return fail(c, BT_ERR_ARG, "%s: training mode needs the running-statistics table", fn);
+  for (size_t i = 0; i < m.table.size(); ++i) {
+    const std::string& n = m.table[i].name;
+    const bool stat = n.size() > 13 && (n.compare(n.size() - 13, 13, ".running_mean") == 0 ||
+                                        n.compare(n.size() - 12, 12, ".running_var") == 0);
+    if (stat && !running[i])
+      return fail(c, BT_ERR_ARG, "%s: running-statistics entry %zu (%s) is null", fn, i, n.c_str());
+  }
+  return BT_OK;
+}
+
+// bt_grad_pack's and bt_grad_ordered_sum's device table: the entries with elements, packed densely in table order.
+int grad_table(bt_ctx* c, const char* fn, const bt_grad_entry* entries, int32_t n, std::vector<GradEntry>* dev,
+               int64_t* chunks) {
+  if (n < 0 || (n > 0 && !entries)) return fail(c, BT_ERR_ARG, "%s: need n >= 0 entries, got %d", fn, n);
+  int64_t off = 0;
+  *chunks = 0;
+  for (int32_t i = 0; i < n; ++i) {
+    const bt_grad_entry& e = entries[i];
+    if (e.numel < 0) return fail(c, BT_ERR_ARG, "%s: entry %d has numel %lld", fn, i, static_cast<long long>(e.numel));
+    if (e.numel == 0) continue;
+    if (!e.grad) return fail(c, BT_ERR_ARG, "%s: entry %d has a null pointer", fn, i);
+    dev->push_back(GradEntry{e.grad, e.numel, off, *chunks});
+    off += e.numel;
+    *chunks += grad_chunks(e.numel);
+  }
+  if (*chunks > 0x7fffffff)
+    return fail(c, BT_ERR_ARG, "%s: %lld blocks exceed the grid", fn, static_cast<long long>(*chunks));
+  return BT_OK;
+}
+
 int train_scratch(bt_ctx* c, int64_t BL, TrScratch* s) {
   const int64_t n = scratch_floats(BL);
   BT_CUDA(c, c->train_ws.reserve(n * sizeof(float), n * sizeof(float)));
@@ -525,16 +586,7 @@ int bt_train_forward_ex(bt_ctx* c, const float* const* params, int32_t n_params,
                         &m);
   if (r != BT_OK) return r;
   if (!spect_dev || !beat_dev || !down_dev) return fail(c, BT_ERR_ARG, "%s: null spectrogram or logits pointer", fn);
-  if (mode) {  // the running statistics every BatchNorm updates
-    if (!running) return fail(c, BT_ERR_ARG, "%s: training mode needs the running-statistics table", fn);
-    for (size_t i = 0; i < m.table.size(); ++i) {
-      const std::string& n = m.table[i].name;
-      const bool stat = n.size() > 13 && (n.compare(n.size() - 13, 13, ".running_mean") == 0 ||
-                                          n.compare(n.size() - 12, 12, ".running_var") == 0);
-      if (stat && !running[i])
-        return fail(c, BT_ERR_ARG, "%s: running-statistics entry %zu (%s) is null", fn, i, n.c_str());
-    }
-  }
+  if (mode && (r = check_running(c, fn, m, running)) != BT_OK) return r;
   cudaStream_t st;
   if ((r = enter(c, fn, stream, &st)) != BT_OK) return r;
   TrRun R{c, st, params, nullptr, static_cast<float*>(act_dev), {}, B, L, nullptr, nullptr, mode, running};
@@ -621,6 +673,75 @@ int bt_adamw_step(bt_ctx* c, const bt_adamw_entry* entries, int32_t n, void* str
   if ((r = stage(c, st, {{dev.data(), dev.size()}}, &table)) != BT_OK) return r;
   launch_adamw(table, static_cast<int>(dev.size()), chunks, st);
   BT_LAUNCHED(c, "adamw", st);
+  return BT_OK;
+}
+
+int bt_grad_pack(bt_ctx* c, const bt_grad_entry* entries, int32_t n, float* row_dev, void* stream) {
+  if (!c) return BT_ERR_ARG;
+  const char* fn = "bt_grad_pack";
+  std::vector<GradEntry> dev;
+  int64_t chunks = 0;
+  int r = grad_table(c, fn, entries, n, &dev, &chunks);
+  if (r != BT_OK) return r;
+  if (!row_dev) return fail(c, BT_ERR_ARG, "%s: null row", fn);
+  if (dev.empty()) return BT_OK;
+  cudaStream_t st;
+  if ((r = enter(c, fn, stream, &st)) != BT_OK) return r;
+  const GradEntry* table = nullptr;
+  if ((r = stage(c, st, {{dev.data(), dev.size()}}, &table)) != BT_OK) return r;
+  launch_grad_pack(table, static_cast<int>(dev.size()), chunks, row_dev, st);
+  BT_LAUNCHED(c, "grad_pack", st);
+  return BT_OK;
+}
+
+int bt_grad_ordered_sum(bt_ctx* c, const bt_grad_entry* entries, int32_t n, const float* const* rows_host, int32_t k,
+                        void* stream) {
+  if (!c) return BT_ERR_ARG;
+  const char* fn = "bt_grad_ordered_sum";
+  std::vector<GradEntry> dev;
+  int64_t chunks = 0;
+  int r = grad_table(c, fn, entries, n, &dev, &chunks);
+  if (r != BT_OK) return r;
+  if (k < 1 || !rows_host) return fail(c, BT_ERR_ARG, "%s: need k >= 1 rows, got %d", fn, k);
+  for (int32_t j = 0; j < k; ++j)
+    if (!rows_host[j]) return fail(c, BT_ERR_ARG, "%s: row %d is null", fn, j);
+  if (dev.empty()) return BT_OK;
+  cudaStream_t st;
+  if ((r = enter(c, fn, stream, &st)) != BT_OK) return r;
+  const GradEntry* table = nullptr;
+  const float* const* rows = nullptr;
+  if ((r = stage(c, st, {{dev.data(), dev.size()}}, &table)) != BT_OK) return r;
+  if ((r = stage(c, st, {{rows_host, static_cast<size_t>(k)}}, &rows)) != BT_OK) return r;
+  launch_grad_ordered_sum(table, static_cast<int>(dev.size()), chunks, rows, k, st);
+  BT_LAUNCHED(c, "grad_ordered_sum", st);
+  return BT_OK;
+}
+
+int bt_train_running_replay(bt_ctx* c, float* const* running, int32_t n_params, const float* const* stats_host,
+                            int32_t k, int32_t B, int32_t L, void* stream) {
+  if (!c) return BT_ERR_ARG;
+  const char* fn = "bt_train_running_replay";
+  if (B < 1 || L < 1 || int64_t{B} * L < 2)
+    return fail(c, BT_ERR_ARG, "%s: need B >= 1, L >= 1 and B * L >= 2, got B=%d L=%d", fn, B, L);
+  const TrModel m = train_model(c->hp, B, L, true);
+  if (n_params != static_cast<int32_t>(m.table.size()))
+    return fail(c, BT_ERR_ARG, "%s: %d running-statistics pointers, the model has %zu (bt_train_param_count)", fn,
+                n_params, m.table.size());
+  int r = check_running(c, fn, m, running);
+  if (r != BT_OK) return r;
+  if (k < 0 || (k > 0 && !stats_host)) return fail(c, BT_ERR_ARG, "%s: need k >= 0 micro-batches, got %d", fn, k);
+  for (int32_t j = 0; j < k; ++j)
+    if (!stats_host[j]) return fail(c, BT_ERR_ARG, "%s: statistics of micro-batch %d are null", fn, j);
+  if (k == 0) return BT_OK;
+  const int64_t tail = train_model(c->hp, B, L, false).floats;  // the statistics follow the eval-mode layout
+  cudaStream_t st;
+  if ((r = enter(c, fn, stream, &st)) != BT_OK) return r;
+  const std::vector<TrBnStat> bns = bn_stat_list(m, c->hp, B, L);
+  for (int32_t j = 0; j < k; ++j)
+    for (const TrBnStat& b : bns) {
+      const float* mean = stats_host[j] + (b.off - tail);
+      TR_OK(running_update(c, st, mean, mean + ((b.ch + 3) & ~3), b.N, b.ch, running[b.p + 2], running[b.p + 3]));
+    }
   return BT_OK;
 }
 

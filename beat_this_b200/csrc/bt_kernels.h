@@ -227,6 +227,21 @@ struct AdamwEntry {
 int64_t adamw_chunks(int64_t n);  // blocks of one entry of n elements
 void launch_adamw(const AdamwEntry* entries_dev, int n_entries, int64_t chunks, cudaStream_t st);
 
+// ---- data-parallel gradient exchange (kernels_dp.cu) ----------------------------------------------------------------
+// One entry of bt_grad_pack's and bt_grad_ordered_sum's device table: n > 0 elements of grad, at element off of a
+// packed row; chunk0, its first chunk of the launch (prefix sums of grad_chunks over the entries before it).
+struct GradEntry {
+  float* grad;
+  int64_t n, off, chunk0;
+};
+int64_t grad_chunks(int64_t n);  // blocks of one entry of n elements
+// row[off + i] = grad[i] for every entry
+void launch_grad_pack(const GradEntry* entries_dev, int n_entries, int64_t chunks, float* row, cudaStream_t st);
+// grad[i] = ((rows[0][off + i] + rows[1][off + i]) + ...) + rows[k - 1][off + i], fp32 adds in row order; rows_dev: k
+// device pointers on the device
+void launch_grad_ordered_sum(const GradEntry* entries_dev, int n_entries, int64_t chunks, const float* const* rows_dev,
+                             int k, cudaStream_t st);
+
 void launch_f32_to_h16(const float* in, void* out, int64_t n, cudaStream_t st);
 void launch_h16_to_f32(const void* in, float* out, int64_t n, cudaStream_t st);
 // [seqs, L, heads*32] fp32 q,k,v -> packed qkv buffer [seqs*L, 3C] of the activation dtype

@@ -15,6 +15,7 @@
 #include <cstdint>
 
 #include "bt_kernels.h"
+#include "chunk_table.cuh"
 
 namespace bt {
 
@@ -35,15 +36,8 @@ __device__ __forceinline__ void adamw_element(float& p, float g, float& m, float
 }
 
 __global__ void __launch_bounds__(kThreads) adamw_kernel(const AdamwEntry* __restrict__ entries, int n_entries) {
-  // the entry of this block: the last one whose first chunk is <= blockIdx.x
   const int64_t chunk = blockIdx.x;
-  int lo = 0, hi = n_entries - 1;
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) >> 1;
-    if (entries[mid].chunk0 <= chunk) lo = mid;
-    else hi = mid - 1;
-  }
-  const AdamwEntry e = entries[lo];
+  const AdamwEntry e = entries[entry_of_chunk(entries, n_entries, chunk)];
   const int64_t begin = (chunk - e.chunk0) * kChunk;
   const int64_t end = min(begin + kChunk, e.n);
   if (e.vec) {

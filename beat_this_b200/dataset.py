@@ -377,16 +377,20 @@ class TrainingBatches:
     pinned buffer, which goes to the device in one copy on a copy stream; one ``bt_train_batch`` launch on the current
     stream then gathers the rows through the mask row maps and writes the targets.  While a batch is consumed, the
     next one's draws are taken and its windows copied and uploaded (two pinned buffers and two device buffers
-    alternate)."""
+    alternate).
+
+    ``shard`` (data-parallel training; None: every batch): a function of the batch index that says whether this rank
+    assembles the batch.  Iteration then yields None for the batches it does not, after taking their items' draws all
+    the same, in order, so that every rank's random state follows the one-process run's."""
 
     def __init__(self, dataset: BeatTrackingDataset, batch_size=8, shuffle=True, drop_last=True, seed=None,
-                 device="cuda", rng=None, threads=8):
+                 device="cuda", rng=None, threads=8, shard=None):
         if batch_size < 1:
             raise ValueError("batch_size must be positive")
         if dataset.train_length is None and batch_size != 1:
             raise ValueError("a dataset of full pieces (train_length=None) needs batch_size=1")
         self.dataset, self.batch_size, self.shuffle, self.drop_last = dataset, batch_size, shuffle, drop_last
-        self.rng = rng
+        self.rng, self.shard = rng, shard
         self.engine = Engine.shared(device)
         self.device = self.engine.device
         if seed is None:
@@ -413,18 +417,21 @@ class TrainingBatches:
         chunks = [order[i : i + self.batch_size] for i in range(0, len(order), self.batch_size)]
         if self.drop_last and chunks and len(chunks[-1]) < self.batch_size:
             chunks.pop()
-        staged = self._stage(chunks[0]) if chunks else None
+        own = self.shard or (lambda k: True)
+        staged = self._stage(chunks[0], own(0)) if chunks else None
         for k in range(len(chunks)):
-            out = self._launch(staged)
-            staged = self._stage(chunks[k + 1]) if k + 1 < len(chunks) else None
+            out = None if staged is None else self._launch(staged)
+            staged = self._stage(chunks[k + 1], own(k + 1)) if k + 1 < len(chunks) else None
             yield out
 
     def batch(self, indices) -> dict:
         return self._launch(self._stage(list(indices)))
 
     # -- staging
-    def _stage(self, indices) -> _Staged:
+    def _stage(self, indices, own: bool = True) -> _Staged | None:
         ex = [self.dataset.draw(int(i), self.rng) for i in indices]
+        if not own:  # drawn for the random state; another rank assembles the batch
+            return None
         length = self.dataset.train_length if self.dataset.train_length is not None else ex[0].n
         rows = _lib.offsets(e.n for e in ex)
         slot = self._next

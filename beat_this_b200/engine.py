@@ -503,6 +503,50 @@ class Engine:
         n = len(entries)
         self._call("bt_adamw_step", (_lib.bt_adamw_entry * max(n, 1))(*entries), n)
 
+    # ---- data-parallel training (bt_grad_pack, bt_grad_ordered_sum, bt_train_running_replay) -------------------------
+    def _grad_table(self, grads, rows):
+        """The bt_grad_entry table of `grads` (contiguous fp32 tensors on this device), after checking that every packed
+        row (fp32 device tensors) holds their total numel."""
+        total = 0
+        for g in grads:
+            if g.device != self.device or g.dtype != torch.float32 or not g.is_contiguous():
+                raise RuntimeError(f"gradient: need a contiguous float32 tensor on {self.device}, got {g.dtype} "
+                                   f"{tuple(g.shape)} on {g.device}; there is no CPU fallback")
+            total += g.numel()
+        for r in rows:
+            if r.device != self.device or r.dtype != torch.float32 or not r.is_contiguous() or r.numel() < total:
+                raise RuntimeError(f"packed row: need a contiguous float32 tensor of at least {total} elements on "
+                                   f"{self.device}, got {r.dtype} {tuple(r.shape)} on {r.device}")
+        return (_lib.bt_grad_entry * max(len(grads), 1))(*[_lib.bt_grad_entry(g.data_ptr(), g.numel()) for g in grads])
+
+    def grad_pack(self, grads, row):
+        """One ``bt_grad_pack`` launch on the current stream: the tensors of `grads` copied into `row`, densely in
+        order."""
+        self._call("bt_grad_pack", self._grad_table(grads, [row]), len(grads), row.data_ptr())
+
+    def grad_ordered_sum(self, grads, rows):
+        """One ``bt_grad_ordered_sum`` launch on the current stream: each tensor of `grads` becomes the sum, in the order
+        of `rows`, of its elements in the packed rows (((r0 + r1) + r2) + ..., one fp32 add at a time)."""
+        ptrs = (c_void_p * max(len(rows), 1))(*[r.data_ptr() for r in rows])
+        self._call("bt_grad_ordered_sum", self._grad_table(grads, rows), len(grads), ptrs, len(rows))
+
+    def train_batch_stat_floats(self, B: int, L: int) -> int:
+        """Floats of the batch statistics a training-mode activation store keeps after the eval-mode layout."""
+        return (self.train_activation_bytes(B, L, (0, 0.0, 0.0)) - self.train_activation_bytes(B, L)) // 4
+
+    def train_running_replay(self, running, stats, B: int, L: int):
+        """``bt_train_running_replay`` on the current stream: the batch statistics of the micro-batches in `stats` (fp32
+        device tensors of train_batch_stat_floats(B, L) elements each, in micro-batch order) applied to the running
+        statistics of `running` (a table parallel to the parameters, as train_forward takes it)."""
+        need = self.train_batch_stat_floats(B, L)
+        for s in stats:
+            if s.device != self.device or s.dtype != torch.float32 or not s.is_contiguous() or s.numel() < need:
+                raise RuntimeError(f"batch statistics: need a contiguous float32 tensor of at least {need} elements on "
+                                   f"{self.device}, got {s.dtype} {tuple(s.shape)} on {s.device}")
+        ptrs = (c_void_p * max(len(stats), 1))(*[s.data_ptr() for s in stats])
+        self._call("bt_train_running_replay", self._table_ptrs(running, "running statistic"), len(running), ptrs,
+                   len(stats), int(B), int(L))
+
     # ---- per-kernel-class timing (bench.py roofline) -------------------------------------------
     def profile_enable(self, on: bool = True):
         self._call("bt_profile_enable", int(on), stream=False)

@@ -1,7 +1,7 @@
 """The reference's ``BeatThis`` as a trainable module on the GPU: parameters named and shaped as its ``state_dict``,
 forward and backward through ``bt_train_forward_ex`` / ``bt_train_backward_ex`` (fp32 CUDA cores); and ``fit`` /
 ``python -m beat_this_b200.train``, the reference's training run (launch_scripts/train.py with PLBeatThis) without
-Lightning.
+Lightning, on one GPU or data-parallel on several (``torchrun --nproc-per-node N -m beat_this_b200.train``).
 
 By default the gradient is that of the eval-mode function the inference path computes: BatchNorm on its running
 statistics and no dropout, and ``.train(True)`` raises rather than train with other semantics than asked for.  A module
@@ -12,14 +12,17 @@ path.
 from __future__ import annotations
 
 import argparse
+import hashlib
 import json
 import math
 import os
 import random
 import sys
+from datetime import timedelta
 
 import numpy as np
 import torch
+import torch.distributed as dist
 
 from . import _lib
 from .engine import Engine
@@ -29,15 +32,20 @@ from .weights import filter_hparams, strip_prefixes
 
 class _BeatThisFunction(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, module, mode, spect, *params):
+    def forward(ctx, module, mode, capture, spect, *params):
         # mode: None (eval mode) or (seed, dropout_frontend, dropout_transformer); the running statistics in params
-        # are updated in place by a training-mode pass and never read by its backward
+        # are updated in place by a training-mode pass and never read by its backward.  capture: None, or (running,
+        # batch_stats): the pass updates the running table `running` instead and its batch statistics are copied into
+        # batch_stats
         B, L, _ = spect.shape
         eng = module.engine
         act = torch.empty(eng.train_activation_bytes(B, L, mode), dtype=torch.uint8, device=spect.device)
         beat = torch.empty(B, L, device=spect.device)
         down = torch.empty(B, L, device=spect.device)
-        eng.train_forward(params, spect, act, beat, down, mode=mode)
+        eng.train_forward(params, spect, act, beat, down, mode=mode, running=None if capture is None else capture[0])
+        if capture is not None:  # the store keeps them after the eval-mode layout
+            stats = capture[1]
+            stats.copy_(act.view(torch.float32)[act.numel() // 4 - stats.numel():])
         ctx.module, ctx.act, ctx.shape, ctx.mode = module, act, (B, L), mode
         # autograd tracks the trainable entries; the buffers (running statistics, num_batches_tracked) and freqs are
         # held as they are, so a second training-mode forward before this backward may update them in place, as with
@@ -54,11 +62,11 @@ class _BeatThisFunction(torch.autograd.Function):
         dev = ctx.act.device
         dbeat = torch.zeros(B, L, device=dev) if dbeat is None else dbeat.to(torch.float32).contiguous()
         ddown = torch.zeros(B, L, device=dev) if ddown is None else ddown.to(torch.float32).contiguous()
-        grads = [torch.empty_like(p) if trainable and ctx.needs_input_grad[3 + i] else None
+        grads = [torch.empty_like(p) if trainable and ctx.needs_input_grad[4 + i] else None
                  for i, (p, trainable) in enumerate(zip(params, ctx.module._trainable))]
-        dspect = torch.empty(B, L, 128, device=dev) if ctx.needs_input_grad[2] else None
+        dspect = torch.empty(B, L, 128, device=dev) if ctx.needs_input_grad[3] else None
         ctx.module.engine.train_backward(params, ctx.act, B, L, dbeat, ddown, grads, dspect, mode=ctx.mode)
-        return (None, None, dspect, *grads)
+        return (None, None, None, dspect, *grads)
 
 
 class BeatThisModule(torch.nn.Module):
@@ -69,7 +77,9 @@ class BeatThisModule(torch.nn.Module):
     A default module is always in eval mode.  With ``train_mode=True``, ``.train()`` selects the reference's
     training-mode function: each forward draws a 64-bit dropout seed from torch's default generator (so
     ``torch.manual_seed`` makes runs repeatable), uses batch statistics in every BatchNorm and updates its running
-    statistics and ``num_batches_tracked``, also under ``torch.no_grad()``."""
+    statistics and ``num_batches_tracked``, also under ``torch.no_grad()``.  A training-mode forward given
+    ``batch_stats`` leaves the running statistics and counters as they are and writes its batch statistics there
+    instead; ``replay_batch_stats`` applies them later, bitwise as the forward passes would have."""
 
     def __init__(self, hparams: dict, device="cuda", *, train_mode: bool = False):
         super().__init__()
@@ -132,24 +142,68 @@ class BeatThisModule(torch.nn.Module):
         named.update(self.named_buffers())
         return [named[n] for n in self._names]
 
-    def forward(self, spect: torch.Tensor) -> dict:
+    def dropout_mode(self) -> tuple:
+        """The mode of one training-mode forward pass, (seed, dropout_frontend, dropout_transformer): a 64-bit seed drawn
+        from torch's default generator and the model's rates.  Each training-mode forward calls it once; a rank of a
+        data-parallel run calls it for every micro-batch another rank runs, so that all ranks draw the same seeds."""
+        seed = int(torch.randint(-2 ** 63, 2 ** 63 - 1, (), dtype=torch.int64).item()) & (2 ** 64 - 1)
+        rates = self.hparams["dropout"]
+        return (seed, float(rates["frontend"]), float(rates["transformer"]))
+
+    def batch_stat_floats(self, B: int, L: int) -> int:
+        """The length of the ``batch_stats`` tensor a training-mode forward over [B, L, 128] fills."""
+        return self.engine.train_batch_stat_floats(B, L)
+
+    def _counters(self):
+        return [t for name, t in zip(self._names, self._tables()) if name.endswith(".num_batches_tracked")]
+
+    def _running(self, scratch: bool = False):
+        """The running-statistics table parallel to the parameter table: this module's running statistics, or scratch
+        tensors of their shapes (allocated once) that a forward with batch_stats updates instead."""
+        if not scratch:
+            return self._tables()
+        if getattr(self, "_scratch_running", None) is None:
+            self._scratch_running = [torch.empty_like(t) if name.endswith((".running_mean", ".running_var")) else None
+                                     for name, t in zip(self._names, self._tables())]
+        return self._scratch_running
+
+    def forward(self, spect: torch.Tensor, batch_stats: torch.Tensor | None = None) -> dict:
+        """batch_stats (training mode only): a contiguous fp32 tensor of batch_stat_floats(B, L) elements on the
+        module's device that receives the pass's BatchNorm batch statistics; the running statistics and
+        ``num_batches_tracked`` are then left as they are."""
         if not spect.is_cuda:
             raise RuntimeError("BeatThisModule runs on a CUDA device; there is no CPU fallback")
         if spect.ndim != 3 or spect.shape[2] != 128:
             raise ValueError(f"expected spectrograms [B, L, 128], got {tuple(spect.shape)}")
         spect = spect.to(self.engine.device, torch.float32).contiguous()
-        mode = None
+        mode, capture = None, None
         if self.training:
-            seed = int(torch.randint(-2 ** 63, 2 ** 63 - 1, (), dtype=torch.int64).item()) & (2 ** 64 - 1)
-            rates = self.hparams["dropout"]
-            mode = (seed, float(rates["frontend"]), float(rates["transformer"]))
-            # before the function saves its inputs: an in-place bump after would fail autograd's version check
-            with torch.no_grad():
-                for name, t in zip(self._names, self._tables()):
-                    if name.endswith(".num_batches_tracked"):
+            mode = self.dropout_mode()
+            if batch_stats is not None:
+                need = self.batch_stat_floats(*spect.shape[:2])
+                if (batch_stats.device != self.engine.device or batch_stats.dtype != torch.float32
+                        or not batch_stats.is_contiguous() or batch_stats.numel() != need):
+                    raise ValueError(f"batch_stats: need a contiguous float32 tensor of {need} elements on "
+                                     f"{self.engine.device}")
+                capture = (self._running(scratch=True), batch_stats)
+            else:
+                # before the function saves its inputs: an in-place bump after would fail autograd's version check
+                with torch.no_grad():
+                    for t in self._counters():
                         t.add_(1)
-        beat, down = _BeatThisFunction.apply(self, mode, spect, *self._tables())
+        elif batch_stats is not None:
+            raise ValueError("batch_stats is for training-mode forward passes")
+        beat, down = _BeatThisFunction.apply(self, mode, capture, spect, *self._tables())
         return {"beat": beat, "downbeat": down}
+
+    @torch.no_grad()
+    def replay_batch_stats(self, stats, B: int, L: int) -> None:
+        """Applies the batch statistics of training-mode forward passes over [B, L, 128] (``batch_stats`` tensors, in
+        the order of the passes) to the running statistics and adds their number to ``num_batches_tracked``: bitwise
+        what the passes would have done without ``batch_stats``."""
+        self.engine.train_running_replay(self._running(), list(stats), B, L)
+        for t in self._counters():
+            t.add_(len(stats))
 
     @classmethod
     def from_checkpoint(cls, checkpoint_path, device="cuda", *, train_mode: bool = False) -> "BeatThisModule":
@@ -182,6 +236,23 @@ class BeatThisModule(torch.nn.Module):
 def step_plan(n_batches: int, accumulate: int) -> list:
     """Indices of the micro-batches of an epoch of `n_batches` after which the optimizer steps."""
     return [i for i in range(n_batches) if (i + 1) % accumulate == 0 or i + 1 == n_batches]
+
+
+def micro_batch_owners(n_batches: int, accumulate: int, world: int) -> list:
+    """Who runs what in a data-parallel epoch of `n_batches` micro-batches on `world` ranks: per optimizer-step group of
+    step_plan (the consecutive micro-batches up to each step point; the last group may be short), the (rank, slot) of
+    each of its micro-batches.  Micro-batch j of a group (0-based) belongs to rank j mod world, in slot j div world, so
+    a short group leaves the last ranks idle.  world > accumulate raises ValueError: a rank would never train."""
+    if world < 1:
+        raise ValueError(f"need at least one rank, got {world}")
+    if world > accumulate:
+        raise ValueError(f"{world} ranks for {accumulate} micro-batches per optimizer step (accumulate_grad_batches): "
+                         f"ranks {accumulate} and up would never train")
+    groups, start = [], 0
+    for end in step_plan(n_batches, accumulate):
+        groups.append([(j % world, j // world) for j in range(end + 1 - start)])
+        start = end + 1
+    return groups
 
 
 def estimated_stepping_batches(n_batches: int, accumulate: int, max_epochs: int) -> int:
@@ -245,27 +316,40 @@ def _losses(loss_pair, out, batch):
     return lb, ld
 
 
-def _validate(module, batches, loss_pair, post, eval_trim_beats) -> dict:
+def _validate(module, batches, loss_pair, post, eval_trim_beats, world: int = 1) -> dict:
     """validation_step over every batch: the loss pair (means over batches weighted by batch size), then the
     post-processed beats under the padding mask scored against truth_orig_* (F-measure and Cemgil, means over
-    pieces)."""
+    pieces).  With world > 1, `batches` yields None for the batches other ranks run, and the ranks' results are
+    gathered and combined in batch order."""
     from .evaluate import beat_metrics
 
     module.eval()
-    sums, n = torch.zeros(2, dtype=torch.float64, device=module.engine.device), 0
-    est, ref = {"beat": [], "downbeat": []}, {"beat": [], "downbeat": []}
+    device = module.engine.device
+    local = []  # per batch run here: (batch index, fp32 loss pair, size, beats, downbeats, truth beats, truth downbeats)
     with torch.no_grad():
-        for batch in batches:
+        for b, batch in enumerate(batches):
+            if batch is None:
+                continue
             out = module(batch["spect"])
-            B = len(batch["spect"])
             lb, ld = _losses(loss_pair, out, batch)
-            sums += torch.stack([lb, ld]).double() * B
-            n += B
             beats, downs = post(out["beat"], out["downbeat"], batch["padding_mask"])
-            for target, times in (("beat", beats), ("downbeat", downs)):
-                est[target] += list(times)
-                ref[target] += [np.frombuffer(b, dtype=np.float64) for b in batch[f"truth_orig_{target}"]]
+            local.append((b, torch.stack([lb, ld]), len(batch["spect"]), list(beats), list(downs),
+                          *[[np.frombuffer(t, dtype=np.float64) for t in batch[f"truth_orig_{k}"]]
+                            for k in ("beat", "downbeat")]))
     module.train()
+    if world > 1:
+        parts = [None] * world
+        dist.all_gather_object(parts, [(r[0], r[1].cpu(), *r[2:]) for r in local])
+        local = sorted((r for part in parts for r in part), key=lambda r: r[0])
+    sums, n = torch.zeros(2, dtype=torch.float64, device=device), 0
+    est, ref = {"beat": [], "downbeat": []}, {"beat": [], "downbeat": []}
+    for _, pair, B, beats, downs, ref_beats, ref_downs in local:
+        sums += pair.to(device).double() * B
+        n += B
+        est["beat"] += beats
+        est["downbeat"] += downs
+        ref["beat"] += ref_beats
+        ref["downbeat"] += ref_downs
     lb, ld = (sums / max(n, 1)).tolist()
     rec = {"val_loss_beat": lb, "val_loss_downbeat": ld, "val_loss": lb + ld}
     for target in ("beat", "downbeat"):
@@ -291,14 +375,32 @@ def fit(data="data", checkpoint_dir="checkpoints", *, name="", gpu=0, n_layers=6
     the last one).  After the last epoch, unless `test` is off, the checkpoint is scored on the test split by
     ``evaluate`` (the reference's trainer.test); its summary goes into the last record under "test".
     epochs: run at most this many epochs in this call (None: up to max_epochs); the schedule still spans max_epochs,
-    and `resume_checkpoint` continues the run later."""
+    and `resume_checkpoint` continues the run later.
+
+    Data-parallel: when the default process group is initialised with more than one rank, every rank calls fit with
+    the same flags (`gpu` aside: each rank's own device) and the micro-batches of each optimizer step are spread over
+    the ranks (micro_batch_owners).  Every rank draws every random number a one-process run draws, in its order, the
+    gradients are summed in micro-batch order and the BatchNorm running statistics replayed in it, so the run writes the
+    checkpoint and returns the records of the one-process run with the same flags, bitwise; checkpoints pass between
+    world sizes.  Rank 0 writes the checkpoint and runs the final test; every rank returns the records."""
+    flags = {k: v for k, v in locals().items() if k != "gpu"}
     from . import dataset as D
     from .loss import loss_from_hparams
     from .optim import AdamW, CosineWarmupScheduler, param_groups
     from .postprocessor import Postprocessor
 
+    world = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
+    rank = dist.get_rank() if world > 1 else 0
     device = torch.device("cuda", gpu)
     torch.cuda.set_device(device)
+    if world > 1:
+        # the digests first: every rank then refuses what follows alike, whatever flags it was given
+        digest = hashlib.sha256(repr(sorted(flags.items())).encode()).hexdigest()
+        digests = [None] * world
+        dist.all_gather_object(digests, digest)
+        if len(set(digests)) > 1:
+            raise ValueError(f"the ranks of a data-parallel run were given different flags (digests {digests})")
+        micro_batch_owners(0, accumulate_grad_batches, world)  # refuses more ranks than micro-batches per step
     random.seed(seed)  # seed_everything
     np.random.seed(seed)
     torch.manual_seed(seed)
@@ -319,8 +421,14 @@ def fit(data="data", checkpoint_dir="checkpoints", *, name="", gpu=0, n_layers=6
     val_batches = D.TrainingBatches(val_set, batch_size, shuffle=False, drop_last=False, seed=0, device=device)
     if len(train_batches) == 0:
         raise ValueError(f"{len(train_set)} training items make no batch of {batch_size}")
+    groups = micro_batch_owners(len(train_batches), accumulate_grad_batches, world)
+    if world > 1:
+        owners = [r for group in groups for r, _ in group]
+        train_batches.shard = lambda k: owners[k] == rank
+        val_batches.shard = lambda k: k % world == rank
     pos_weights = train_set.positive_weights(widen_target_mask=3)
-    print("Using positive weights: ", pos_weights)
+    if rank == 0:
+        print("Using positive weights: ", pos_weights)
 
     hparams = dict(spect_dim=128, fps=50, transformer_dim=transformer_dim, ff_mult=4, n_layers=n_layers, stem_dim=32,
                    dropout={"frontend": frontend_dropout, "transformer": transformer_dropout}, lr=lr,
@@ -354,18 +462,40 @@ def fit(data="data", checkpoint_dir="checkpoints", *, name="", gpu=0, n_layers=6
     os.makedirs(str(checkpoint_dir), exist_ok=True)
     last_epoch = max_epochs if epochs is None else min(max_epochs, first_epoch + epochs)
     plan = set(step_plan(len(train_batches), accumulate_grad_batches))
+    exchange = _GradientExchange(module, opt, world, accumulate_grad_batches) if world > 1 else None
     records = []
     module.train()
     for epoch in range(first_epoch, last_epoch):
         sums, n, step_lr = torch.zeros(2, dtype=torch.float64, device=device), 0, []
-        for i, batch in enumerate(train_batches):
-            out = module(batch["spect"])
-            lb, ld = _losses(loss_pair, out, batch)
-            ((lb + ld) / accumulate_grad_batches).backward()
-            B = len(batch["spect"])
-            sums += torch.stack([lb.detach(), ld.detach()]).double() * B
-            n += B
-            if i in plan:
+        if exchange is None:
+            for i, batch in enumerate(train_batches):
+                out = module(batch["spect"])
+                lb, ld = _losses(loss_pair, out, batch)
+                ((lb + ld) / accumulate_grad_batches).backward()
+                B = len(batch["spect"])
+                sums += torch.stack([lb.detach(), ld.detach()]).double() * B
+                n += B
+                if i in plan:
+                    step_lr.append(opt.param_groups[0]["lr"])
+                    opt.step()
+                    sched.step()
+                    opt.zero_grad(set_to_none=True)
+                    global_step += 1
+        else:
+            batches = iter(train_batches)
+            for group in groups:
+                for owner, slot in group:
+                    batch = next(batches)
+                    if owner != rank:
+                        module.dropout_mode()  # the seed of a micro-batch another rank runs
+                        continue
+                    out = module(batch["spect"], batch_stats=exchange.stats(slot))
+                    lb, ld = _losses(loss_pair, out, batch)
+                    ((lb + ld) / accumulate_grad_batches).backward()
+                    exchange.pack(slot, lb, ld, batch["spect"].shape)
+                for lb_ld, B in exchange.reduce(len(group)):
+                    sums += lb_ld.double() * B
+                    n += B
                 step_lr.append(opt.param_groups[0]["lr"])
                 opt.step()
                 sched.step()
@@ -375,36 +505,104 @@ def fit(data="data", checkpoint_dir="checkpoints", *, name="", gpu=0, n_layers=6
         rec = {"epoch": epoch, "global_step": global_step, "lr": opt.param_groups[0]["lr"], "step_lr": step_lr,
                "train_loss_beat": lb, "train_loss_downbeat": ld, "train_loss": lb + ld}
         if (epoch + 1) % val_frequency == 0:
-            rec.update(_validate(module, val_batches, loss_pair, post, eval_trim_beats))
-        ckpt = {"epoch": epoch, "global_step": global_step,
-                "state_dict": {"model." + k: v.detach().cpu() for k, v in module.state_dict().items()},
-                "hyper_parameters": hparams, "datamodule_hyper_parameters": dm_hparams,
-                "optimizer_states": [opt.state_dict()], "lr_schedulers": [sched.state_dict()],
-                "beat_this_b200": _rng_state(train_batches)}
-        torch.save(ckpt, path + ".tmp")
-        os.replace(path + ".tmp", path)
-        print(json.dumps(rec), flush=True)
+            rec.update(_validate(module, val_batches, loss_pair, post, eval_trim_beats, world))
+        if rank == 0:
+            ckpt = {"epoch": epoch, "global_step": global_step,
+                    "state_dict": {"model." + k: v.detach().cpu() for k, v in module.state_dict().items()},
+                    "hyper_parameters": hparams, "datamodule_hyper_parameters": dm_hparams,
+                    "optimizer_states": [opt.state_dict()], "lr_schedulers": [sched.state_dict()],
+                    "beat_this_b200": _rng_state(train_batches)}
+            torch.save(ckpt, path + ".tmp")
+            os.replace(path + ".tmp", path)
+            print(json.dumps(rec), flush=True)
         records.append(rec)
     if test and last_epoch == max_epochs and first_epoch < max_epochs:
         from .evaluate import evaluate
 
-        result = evaluate(path, data=data, datasplit="test", min_beat_time=eval_trim_beats, device=device, dbn=dbn,
-                          losses=True)
-        records[-1]["test"] = result.summary
-        print(json.dumps({"test": result.summary}), flush=True)
+        summary = [None]
+        # the others wait for rank 0's test on the host, over gloo with a deadline of days: the test split's length
+        # (and the DBN) set how long the test takes, and the default group's watchdog could abort a device wait
+        waiting = dist.new_group(backend="gloo", timeout=timedelta(days=7)) if world > 1 else None
+        if rank == 0:
+            summary[0] = evaluate(path, data=data, datasplit="test", min_beat_time=eval_trim_beats, device=device,
+                                  dbn=dbn, losses=True).summary
+            print(json.dumps({"test": summary[0]}), flush=True)
+        if world > 1:  # the others wait here for rank 0's test
+            dist.broadcast_object_list(summary, src=0, group=waiting)
+            dist.destroy_process_group(waiting)
+        records[-1]["test"] = summary[0]
+    if world > 1:
+        dist.barrier()  # the checkpoint is written when fit returns on any rank
     return records
+
+
+class _GradientExchange:
+    """The gradient exchange of a data-parallel optimizer step of up to `accumulate` micro-batches on `world` ranks.
+
+    Each rank keeps a send buffer of S = ceil(accumulate / world) slots, one per micro-batch it runs in a step.  A
+    slot is a row [P | Q | 4]: the P gradient elements of every trainable parameter in the optimizer's order
+    (bt_grad_pack), the Q floats of the micro-batch's BatchNorm batch statistics (captured by its forward pass), and
+    its fp32 beat and downbeat losses, batch size and frame length; rows are rounded up to 4 floats.  At the step, one
+    all_gather brings every rank's slots to every rank ([world, S, row]), and micro-batch j of the step is read from
+    rank j mod world, slot j div world: bt_grad_ordered_sum writes each .grad as the fp32 sum over the micro-batches in
+    index order, and bt_train_running_replay applies their batch statistics in that order."""
+
+    def __init__(self, module, opt, world: int, accumulate: int):
+        self.module, self.world = module, world
+        self.params = [p for group in opt.param_groups for p in group["params"]]
+        self.P = sum(p.numel() for p in self.params)
+        self.Q = module.batch_stat_floats(1, 1)  # one mean and variance per BatchNorm channel, whatever B and L
+        row = (self.P + self.Q + 4 + 3) // 4 * 4
+        S = -(-accumulate // world)
+        self.send = torch.zeros(S, row, device=module.engine.device)
+        self.recv = torch.empty(world, S, row, device=module.engine.device)
+        self.grads = [torch.empty_like(p) for p in self.params]  # every step's .grad tensors, allocated once
+
+    def stats(self, slot: int) -> torch.Tensor:
+        """Where the forward pass of the micro-batch in `slot` writes its batch statistics."""
+        return self.send[slot, self.P : self.P + self.Q]
+
+    def pack(self, slot: int, lb, ld, shape) -> None:
+        """After the backward pass of the micro-batch in `slot`: its gradients and losses into the slot, and the
+        gradients set to None for the next micro-batch."""
+        B, L = shape[0], shape[1]
+        self.send[slot, self.P + self.Q : self.P + self.Q + 4] = torch.stack(
+            [lb.detach(), ld.detach(), lb.new_tensor(float(B)), lb.new_tensor(float(L))])
+        self.module.engine.grad_pack([p.grad for p in self.params], self.send[slot])
+        for p in self.params:
+            p.grad = None
+
+    def reduce(self, k: int) -> list:
+        """At the step of a group of k micro-batches: the gather, every .grad as the ordered sum, the running
+        statistics replayed; returns each micro-batch's fp32 (beat, downbeat) losses and batch size, in order."""
+        dist.all_gather(list(self.recv.unbind(0)), self.send)
+        rows = [self.recv[j % self.world, j // self.world] for j in range(k)]
+        for p, g in zip(self.params, self.grads):
+            p.grad = g
+        self.module.engine.grad_ordered_sum(self.grads, rows)
+        tails = [row[self.P + self.Q : self.P + self.Q + 4] for row in rows]
+        shapes = [tuple(int(v) for v in t[2:].tolist()) for t in tails]
+        start = 0  # one replay per run of micro-batches of one shape
+        for j in range(1, k + 1):
+            if j == k or shapes[j] != shapes[start]:
+                self.module.replay_batch_stats([row[self.P : self.P + self.Q] for row in rows[start:j]],
+                                               *shapes[start])
+                start = j
+        return [(t[:2], B) for t, (B, _) in zip(tails, shapes)]
 
 
 def build_parser() -> argparse.ArgumentParser:
     """The reference's train.py flags, names and defaults; --data and --checkpoint-dir stand for its fixed paths."""
     ap = argparse.ArgumentParser(prog="python -m beat_this_b200.train",
-                                 description="Train a BeatThis model on a prepared dataset on one GPU.")
+                                 description="Train a BeatThis model on a prepared dataset on one GPU, or "
+                                             "data-parallel on several under torchrun.")
     add = ap.add_argument
     flag = argparse.BooleanOptionalAction
     add("--data", default="data", help="prepared dataset directory (annotations/ and audio/spectrograms/) [%(default)s]")
     add("--checkpoint-dir", default="checkpoints", help="where the checkpoint goes [%(default)s]")
     add("--name", type=str, default="")
-    add("--gpu", type=int, default=0)
+    add("--gpu", type=int, default=int(os.environ.get("LOCAL_RANK", "0")),
+        help="CUDA device (default: LOCAL_RANK under torchrun, else 0)")
     add("--force-flash-attention", default=False, action=flag, help="accepted, no effect")
     add("--compile", action="store", nargs="*", type=str, default=["frontend", "transformer_blocks", "task_heads"],
         help="accepted, no effect")
@@ -461,10 +659,18 @@ def parse_args(argv=None) -> dict:
 
 
 def main(argv=None) -> int:
+    from .distributed import init_from_env
+
+    rank, world, _ = init_from_env()  # NCCL under torchrun with more than one process
     kw = parse_args(argv)
-    print("Starting a new run with the following parameters:")
-    print(kw)
-    fit(**kw)
+    if rank == 0:
+        print("Starting a new run with the following parameters:")
+        print(kw)
+    try:
+        fit(**kw)
+    finally:
+        if world > 1 and dist.is_initialized():
+            dist.destroy_process_group()
     return 0
 
 

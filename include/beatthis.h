@@ -635,6 +635,49 @@ typedef struct bt_adamw_entry {
 } bt_adamw_entry;
 int bt_adamw_step(bt_ctx* ctx, const bt_adamw_entry* entries_host, int32_t n, void* stream);
 
+/* ---- data-parallel training (ABI 2.16): the gradient exchange and the running statistics -----------------------------
+ * An optimizer step of k micro-batches on W ranks: each rank runs the micro-batches it owns, packs each one's gradients
+ * into a row with bt_grad_pack, the rows travel by all_gather, and every rank sums the k rows in micro-batch order into
+ * its gradients with bt_grad_ordered_sum and replays the k micro-batches' BatchNorm statistics with
+ * bt_train_running_replay, so every rank holds what one process running the k micro-batches in order would hold.
+ *
+ * A gradient table: entries_host (n entries, a host array) of fp32 device arrays of numel elements.  Its packed row
+ * holds entry i's elements at the sum of the numel of the entries before it, densely in table order (no padding).
+ * bt_grad_pack copies every entry's grad into row_dev (the table's total numel floats; nothing else is written).
+ * bt_grad_ordered_sum writes every entry's grad as ((r_0 + r_1) + r_2) + ... + r_{k-1} elementwise over the k packed
+ * rows rows_host[0 .. k) (a host array of device pointers), in that order: each step one fp32 add rounded to nearest,
+ * never fused or reassociated, and r_0 stored as it is (k = 1: a copy).  That is what autograd's AccumulateGrad makes
+ * of the same gradients (the first stored, each later one added in place), so the results are bitwise equal to it,
+ * signed zeros, infinities, NaNs and subnormals included.  The rows may not overlap the grads.  Each element is read
+ * and written by one thread without atomics: two calls on the same inputs write the same bytes.
+ * Both: one launch over the whole table (entries with numel 0 are skipped; when no element is left, nothing is
+ * launched), counted and profiled as "grad_pack" / "grad_ordered_sum"; the tables go to the device through the ctx's
+ * staging ring; any ctx will do (a weight-less one too); enqueued on `stream` without synchronisation.  BT_ERR_ARG
+ * before anything is enqueued: n < 0 (or entries_host NULL with n > 0), numel < 0, a NULL grad with numel > 0, a NULL
+ * row_dev (pack), k < 1, a NULL rows_host or row (sum), or more than 2^31 - 1 blocks of 2048 elements. */
+typedef struct bt_grad_entry {
+  float* grad;
+  int64_t numel;
+} bt_grad_entry;
+int bt_grad_pack(bt_ctx* ctx, const bt_grad_entry* entries_host, int32_t n, float* row_dev, void* stream);
+int bt_grad_ordered_sum(bt_ctx* ctx, const bt_grad_entry* entries_host, int32_t n, const float* const* rows_host,
+                        int32_t k, void* stream);
+/* The BatchNorm statistics of k training-mode micro-batches of B x L frames applied to the running statistics in
+ * micro-batch order, as k bt_train_forward_ex calls in training mode would have updated them: per micro-batch and per
+ * BatchNorm in layer order, r = 0.9 r + 0.1 mean for running_mean and r = 0.9 r + (0.1 N / (N - 1)) var for
+ * running_var (N positions), by the same launches the forward pass makes, so the results are bitwise those of the
+ * forward passes.  stats_host[j] (a host array of k device pointers) holds micro-batch j's batch statistics: the
+ * floats its activation store keeps after the eval-mode layout, (bt_train_activation_bytes_ex with a mode - without) / 4
+ * of them, per BatchNorm its batch mean then its biased variance (bt_train_activation_bytes_ex).  running: a host array
+ * of device pointers parallel to the parameter table (n_params entries), as bt_train_forward_ex takes it; only its
+ * running_mean and running_var entries are read and updated.  num_batches_tracked is the caller's to increment by k.
+ * Two launches per BatchNorm and micro-batch, each counted and profiled as "train_reduce" (k = 0: none); any ctx of
+ * the model's shape; enqueued on `stream` without synchronisation.  BT_ERR_ARG before anything is enqueued: B or L < 1,
+ * B L < 2, n_params other than bt_train_param_count, a NULL running table or running_mean / running_var entry, k < 0,
+ * or a NULL stats_host (k > 0) or entry. */
+int bt_train_running_replay(bt_ctx* ctx, float* const* running, int32_t n_params, const float* const* stats_host,
+                            int32_t k, int32_t B, int32_t L, void* stream);
+
 /* Test hook (fp32 ctx only; BT_ERR_ARG for a 16-bit one): the attention core of one bt_train_forward /
  * bt_train_backward layer alone, on `seqs` time-direction sequences of n positions and `heads` heads of 32.  qkv_dev
  * [seqs * n, 3 * heads * 32] holds q | k | v before RoPE, gates_dev [seqs * n, heads] the gate logits, freqs_dev [16]
