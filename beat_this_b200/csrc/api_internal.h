@@ -103,6 +103,8 @@ struct bt_ctx {
   DeviceBuffer<float> train_ws;
   // windowed inverse transforms of bt_istft's frames, n_fft floats each (grows on demand)
   DeviceBuffer<float> istft_frames;
+  // decoded samples of bt_flac_decode, [channels][n_samples] int64 per stream (grows on demand)
+  DeviceBuffer<int64_t> flac_ws;
   // pinned staging + device tables
   StageSlot stage[kStageSlots];
   int stage_next = 0;

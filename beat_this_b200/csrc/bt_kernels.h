@@ -242,6 +242,25 @@ void launch_grad_pack(const GradEntry* entries_dev, int n_entries, int64_t chunk
 void launch_grad_ordered_sum(const GradEntry* entries_dev, int n_entries, int64_t chunks, const float* const* rows_dev,
                              int k, cudaStream_t st);
 
+// ---- FLAC decoding (kernels_flac.cu, flac.cuh) ------------------------------------------------------------------------
+// One stream of a bt_flac_decode call on the device: its frame bytes and frame table (entries of 24 bytes: offset,
+// first sample, bytes, block size, as bt_flac_frame), its int64 scratch [channels][n_samples] and its first output
+// element.
+struct FlacStreamDev {
+  const uint8_t* bytes;
+  const void* frames;
+  int64_t* scratch;
+  int64_t byte_count, n_frames, n_samples, out_off;
+  int32_t channels, bits;
+};
+// one thread per frame: CRC-16, subframes and decorrelation into the scratch; a malformed frame stores BT_ERR_IO in
+// status[stream].  Streams whose status is not BT_OK are skipped.
+void launch_flac_frames(const FlacStreamDev* streams_dev, int n_streams, int64_t max_frames, int32_t* status,
+                        cudaStream_t st);
+// one thread per sample: mode 0 mono fp32, mode 1 float64 [time, channels]; zeros for a stream whose status is not BT_OK
+void launch_flac_output(const FlacStreamDev* streams_dev, int n_streams, int64_t max_samples, int mode, void* out,
+                        const int32_t* status, cudaStream_t st);
+
 void launch_f32_to_h16(const float* in, void* out, int64_t n, cudaStream_t st);
 void launch_h16_to_f32(const void* in, float* out, int64_t n, cudaStream_t st);
 // [seqs, L, heads*32] fp32 q,k,v -> packed qkv buffer [seqs*L, 3C] of the activation dtype

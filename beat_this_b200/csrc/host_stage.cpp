@@ -15,6 +15,7 @@
 #include <vector>
 
 #include "../../include/beatthis.h"
+#include "host_pool.h"
 
 namespace {
 
@@ -27,25 +28,7 @@ std::vector<Piece> split_pieces(const int64_t* frames, int32_t n, int64_t grain)
   return v;
 }
 
-template <typename F>
-void run_pool(size_t n_tasks, int n_threads, F&& fn) {
-  if (n_threads <= 0) n_threads = static_cast<int>(std::thread::hardware_concurrency());
-  n_threads = std::max(1, std::min<int>(n_threads, static_cast<int>(n_tasks)));
-  std::atomic<size_t> next{0};
-  auto worker = [&]() {
-    for (;;) {
-      const size_t i = next.fetch_add(1, std::memory_order_relaxed);
-      if (i >= n_tasks) break;
-      fn(i);
-    }
-  };
-  if (n_threads == 1) { worker(); return; }
-  std::vector<std::thread> th;
-  th.reserve(n_threads - 1);
-  for (int t = 1; t < n_threads; ++t) th.emplace_back(worker);
-  worker();
-  for (auto& t : th) t.join();
-}
+using bt::run_pool;
 
 // mean over channels exactly as numpy's signal.mean(1) computes it for `ch` < 8 channels (sequential sum in the
 // array's own floating type, one division), then the fp32 cast of torch.tensor(signal, dtype=float32)

@@ -427,33 +427,34 @@ class File2Beats(Audio2Beats):
 
     def batch(self, audio_paths, on_error: str = "raise"):
         """Many files per call.  WAV files are read, mixed to mono and cast by the native host threads straight into
-        the pinned staging ring (no numpy round trip); other containers go through load_audio.  Files of equal
-        sample rate share groups.  on_error: "raise", or "skip" (a file that cannot be loaded or processed yields
-        None instead of aborting the call -- the behaviour of the reference's per-file loop, cli.py:185-190)."""
+        the pinned staging ring (no numpy round trip); FLAC files (with a known length) are staged as frame bytes and
+        decoded and mixed on the device (bt_flac_decode); other containers go through load_audio.  Files of equal
+        container and sample rate share groups.  on_error: "raise", or "skip" (a file that cannot be loaded or processed
+        yields None instead of aborting the call -- the behaviour of the reference's per-file loop, cli.py:185-190); a
+        FLAC file with a malformed frame raises RuntimeError naming it, or yields None."""
         if on_error not in ("raise", "skip"):
             raise ValueError("on_error must be 'raise' or 'skip'")
         paths = [str(p) for p in audio_paths]
         out = [None] * len(paths)
-        infos, is_wav = _lib.wav_probe(paths)
-        for i in range(len(paths)):  # a clip needs more than 512 samples at 22.05 kHz (reflect padding of the STFT)
-            if is_wav[i] and infos[i].frames * 22050 // max(1, infos[i].sample_rate) <= 512:
-                if on_error == "raise":
-                    raise ValueError(f'"{paths[i]}" is too short ({infos[i].frames} samples)')
-                is_wav[i] = False
-                infos[i].frames = -1  # marks "known bad": not retried through load_audio either
+        kinds, bad = _native_groups(paths, raise_short=on_error == "raise")
         pipe = self.pipeline
         want = self._want_beats
-        for sr in sorted({infos[i].sample_rate for i in range(len(paths)) if is_wav[i]}):
-            idx = [i for i in range(len(paths)) if is_wav[i] and infos[i].sample_rate == sr]
-            groups = _plan_groups([infos[i].frames for i in idx], sr, DEFAULT_CHUNKING)
+        for (kind, sr), (idx, infos) in kinds.items():
+            groups = _plan_groups([_n_samples(info) for info in infos], sr, DEFAULT_CHUNKING)
 
-            def submit(g, idx=idx, groups=groups, sr=sr):
-                sel = idx[groups[g][0] : groups[g][1]]
-                pipe.submit_wavs([paths[i] for i in sel], [infos[i] for i in sel], sr, want)
+            def submit(g, idx=idx, infos=infos, groups=groups, sr=sr, kind=kind):
+                lo, hi = groups[g]
+                (pipe.submit_wavs if kind == "wav" else pipe.submit_flacs)(
+                    [paths[i] for i in idx[lo:hi]], infos[lo:hi], sr, want)
 
             try:
                 for (lo, hi), res in zip(groups, pipe.run(len(groups), submit)):
-                    for k, r in zip(idx[lo:hi], self._finish(res)):
+                    status = pipe.last_status
+                    for j, (k, r) in enumerate(zip(idx[lo:hi], self._finish(res))):
+                        if status is not None and status[j] != 0:
+                            if on_error == "raise":
+                                raise RuntimeError(f'Could not decode "{paths[k]}": malformed FLAC frames')
+                            r = None
                         out[k] = r
             except Exception:
                 pipe.drain()
@@ -465,7 +466,8 @@ class File2Beats(Audio2Beats):
                             out[i] = File2Beats.__call__(self, paths[i])
                         except Exception:
                             out[i] = None
-        rest = [i for i in range(len(paths)) if not is_wav[i] and infos[i].frames >= 0]
+        native = bad.union(*(idx for idx, _ in kinds.values()))
+        rest = [i for i in range(len(paths)) if i not in native]
         loaded = {}
         for i in rest:
             try:
@@ -499,31 +501,57 @@ class File2Beats(Audio2Beats):
         chunking = engine_chunking(chunk_size, border_size, overlap_mode, self.model.max_chunk_size)
         paths = [str(p) for p in audio_paths]
         out = [None] * len(paths)
-        infos, is_wav = _lib.wav_probe(paths)
-        for i in range(len(paths)):
-            if is_wav[i] and infos[i].frames * 22050 // max(1, infos[i].sample_rate) <= 512:
-                raise ValueError(f'"{paths[i]}" is too short ({infos[i].frames} samples)')
+        kinds, _ = _native_groups(paths, raise_short=True)
         pipe = self.pipeline
-        for sr in sorted({infos[i].sample_rate for i in range(len(paths)) if is_wav[i]}):
-            idx = [i for i in range(len(paths)) if is_wav[i] and infos[i].sample_rate == sr]
-            groups = _plan_groups([infos[i].frames for i in idx], sr, chunking)
+        for (kind, sr), (idx, infos) in kinds.items():
+            groups = _plan_groups([_n_samples(info) for info in infos], sr, chunking)
 
-            def submit(g, idx=idx, groups=groups, sr=sr):
-                sel = idx[groups[g][0] : groups[g][1]]
-                pipe.submit_wavs([paths[i] for i in sel], [infos[i] for i in sel], sr, "frames", chunking)
+            def submit(g, idx=idx, infos=infos, groups=groups, sr=sr, kind=kind):
+                lo, hi = groups[g]
+                (pipe.submit_wavs if kind == "wav" else pipe.submit_flacs)(
+                    [paths[i] for i in idx[lo:hi]], infos[lo:hi], sr, "frames", chunking)
 
             try:
                 for (lo, hi), (beat, down, fo) in zip(groups, pipe.run(len(groups), submit)):
+                    status = pipe.last_status
                     for j, k in enumerate(idx[lo:hi]):
+                        if status is not None and status[j] != 0:
+                            raise RuntimeError(f'Could not decode "{paths[k]}": malformed FLAC frames')
                         out[k] = (beat[fo[j] : fo[j + 1]], down[fo[j] : fo[j + 1]])
             finally:
                 pipe.drain()
-        loaded = {i: load_audio(paths[i]) for i in range(len(paths)) if not is_wav[i]}
+        native = set().union(*(idx for idx, _ in kinds.values()))
+        loaded = {i: load_audio(paths[i]) for i in range(len(paths)) if i not in native}
         for sr in sorted({s for _, s in loaded.values()}):
             idx = [i for i in loaded if loaded[i][1] == sr]
             for i, r in zip(idx, Audio2Frames._frames_batch(self, [loaded[i][0] for i in idx], sr, chunking)):
                 out[i] = r
         return out
+
+
+def _n_samples(info) -> int:
+    return int(info.frames) if isinstance(info, _lib.bt_wav_info) else int(info.total_samples)
+
+
+def _native_groups(paths, raise_short: bool):
+    """The files the native readers take, by (container, sample rate) in sorted order: ({("wav" | "flac", sr):
+    ([index, ...], [probe info, ...])}, set of indices of files too short to run).  A clip needs more than 512 samples at 22.05 kHz (reflect padding
+    of the STFT): a shorter one raises ValueError under raise_short, else it is marked bad (not retried through
+    load_audio).  A FLAC file whose STREAMINFO leaves the length unknown goes to load_audio."""
+    kinds, bad = {}, set()
+    for i, (kind, info) in enumerate(_lib.probe_audio(paths)):
+        if kind is None or (kind == "flac" and info.total_samples == 0):
+            continue
+        n = _n_samples(info)
+        if n * 22050 // max(1, info.sample_rate) <= 512:
+            if raise_short:
+                raise ValueError(f'"{paths[i]}" is too short ({n} samples)')
+            bad.add(i)
+            continue
+        idx, infos = kinds.setdefault((kind, int(info.sample_rate)), ([], []))
+        idx.append(i)
+        infos.append(info)
+    return dict(sorted(kinds.items())), bad
 
 
 class File2File(File2Beats):

@@ -5,10 +5,11 @@ The reference handles one clip at a time on one stream (reference beat_this/infe
 one pass of every kernel); for every group
 
   host threads   mono mix + fp32 cast of all clips straight into a pinned ring slot (``bt_stage_audio`` /
-                 ``bt_stage_wav_files``: C++, GIL released)
+                 ``bt_stage_wav_files``: C++, GIL released); for FLAC files, their frame bytes and frame tables
+                 (``bt_stage_flac_files``)
   copy stream    one H2D copy of the slot
-  compute stream log-mel -> BeatThis forward -> (peak picking | device DBN -> D2H of the timestamps
-                 | D2H of the logits for the host DBN)
+  compute stream [FLAC: decode and mono mix (``bt_flac_decode``)] -> log-mel -> BeatThis forward -> (peak picking
+                 | device DBN -> D2H of the timestamps | D2H of the logits for the host DBN)
 
 and group g+1 is staged and copied while the kernels of group g run; results are collected in order.  Nothing in the
 enqueue path waits for the GPU (the C library keeps its small tables in a ring of pinned slots), so the device queue
@@ -78,6 +79,10 @@ class _Slot:
         self.done = None
         self.t0 = None        # events around the group's kernels (stats: GPU busy time)
         self.t1 = None
+        self.flac_host = None  # pinned bytes of a FLAC group (_lib.flac_layout), its device copy and the D2H
+        self.flac_dev = None   # copy of its files' statuses
+        self.flac_status = None
+        self.flac_files = 0    # FLAC files of the group in flight (0: not a FLAC group)
 
 
 class BeatPipeline:
@@ -107,6 +112,7 @@ class BeatPipeline:
         self.h2d_bytes = 0
         self.d2h_bytes = 0
         self.dbn_params = None  # tracker parameters of want="dbn_device" (Postprocessor.dbn_params)
+        self.last_status = None  # per-file statuses of the last collected FLAC group (collect)
         # host seconds spent staging (mono mix / decode into pinned memory), enqueueing and waiting for results
         self.stats = {"stage_s": 0.0, "enqueue_s": 0.0, "collect_wait_s": 0.0, "gpu_busy_s": 0.0, "groups": 0}
 
@@ -128,18 +134,30 @@ class BeatPipeline:
         returns the sample offsets."""
         return _lib.stage_audio(arrays, dst, self.host_threads)
 
-    def _enqueue(self, idx, s, so, sr, want, chunking=DEFAULT_CHUNKING):
+    def _enqueue(self, idx, s, so, sr, want, chunking=DEFAULT_CHUNKING, flac=None):
+        """flac: (streams, status offset, bytes) of a FLAC group staged in s.flac_host, decoded into s.dev on the
+        compute stream; otherwise s.host holds the group's mono fp32 samples."""
         n = so[-1]
         with torch.cuda.stream(self.copy_stream):
-            s.dev[:n].copy_(s.host[:n], non_blocking=True)
+            if flac is None:
+                s.dev[:n].copy_(s.host[:n], non_blocking=True)
+            else:
+                s.flac_dev[: flac[2]].copy_(s.flac_host[: flac[2]], non_blocking=True)
             s.copied.record(self.copy_stream)
-        self.h2d_bytes += n * 4
+        self.h2d_bytes += n * 4 if flac is None else flac[2]
         eng = self.engine
         if s.t0 is None:
             s.t0, s.t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         with torch.cuda.stream(self.compute_stream):
             self.compute_stream.wait_event(s.copied)
             s.t0.record(self.compute_stream)
+            s.flac_files = 0
+            if flac is not None:
+                streams, status_at, _ = flac
+                eng.flac_decode(s.flac_dev, streams, _lib.BT_FLAC_MONO_F32, s.dev, status_at)
+                s.flac_files = len(streams)
+                s.flac_status[: len(streams)].copy_(s.flac_dev[status_at : status_at + 4 * len(streams)].view(torch.int32),
+                                                    non_blocking=True)
             audio, offs = s.dev[:n], so
             if sr != 22050:
                 audio, offs = eng.resample_cat(audio, so, sr)
@@ -205,6 +223,39 @@ class BeatPipeline:
             self.free.append(idx)
             raise
 
+    def submit_flacs(self, paths, infos, sr: int, want: str = "beats", chunking: tuple = DEFAULT_CHUNKING):
+        """paths: list of str; infos: list of bt_flac_info (all `sr` Hz, total_samples known) from _lib.probe_audio;
+        chunking as in submit_signals.  Host threads stage the frame bytes and tables, the device decodes them and mixes
+        to mono (bt_flac_decode), and the group runs on as submit_wavs's.  A file that fails to stage or decode runs as
+        zeros of its STREAMINFO length; `last_status` gives every file's status when the group is collected."""
+        _check_frames_route(want, chunking)
+        so = _lib.offsets(info.total_samples for info in infos)
+        fo, status_at, bo, total = _lib.flac_layout(infos)
+        idx, s = self._slot(so[-1])
+        try:
+            t0 = time.perf_counter()
+            if s.flac_host is None or s.flac_host.numel() < total:
+                cap = max(int(total * 1.25), 1 << 20)
+                s.flac_host = torch.empty(cap, dtype=torch.uint8, pin_memory=True)
+                s.flac_dev = torch.empty(cap, dtype=torch.uint8, device=self.device)
+            if s.flac_status is None or s.flac_status.numel() < len(paths):
+                s.flac_status = torch.empty(max(len(paths), 64), dtype=torch.int32, pin_memory=True)
+            nf, ns, status = _lib.stage_flac_files(paths, infos, s.flac_host.data_ptr(), self.host_threads)
+            # staging checks the block sizes against STREAMINFO's total, so a staged file has its so length; one that
+            # failed is not decoded and runs as zeros of that length
+            streams = _lib.flac_streams(infos, nf, [info.total_samples for info in infos], so[:-1])
+            for i, st in enumerate(status):
+                if st != 0:
+                    streams[i].n_frames = 0
+            t1 = time.perf_counter()
+            self._enqueue(idx, s, so, int(sr), want, chunking, (streams, status_at, total))
+            self.stats["stage_s"] += t1 - t0
+            self.stats["enqueue_s"] += time.perf_counter() - t1
+            self.stats["groups"] += 1
+        except Exception:
+            self.free.append(idx)
+            raise
+
     def submit_pinned(self, audio_host: torch.Tensor, sample_offsets, sr: int = 22050, want: str = "beats"):
         """Mono fp32 audio already in one pinned host tensor (clips back to back)."""
         so = [int(v) for v in sample_offsets]
@@ -215,20 +266,27 @@ class BeatPipeline:
     # ---- results ----------------------------------------------------------------------------------
     def collect(self):
         """Oldest group: list of (beat_times, downbeat_times) ["beats", "dbn_device"], (beat, down, fo) host arrays
-        ["logits_host"] or device tensors ["frames"]."""
+        ["logits_host"] or device tensors ["frames"].  After it, last_status lists the status (BT_OK or BT_ERR_IO) of
+        every file of a FLAC group, and is None for other groups."""
         idx, (kind, p) = self.inflight.popleft()
         t0 = time.perf_counter()
+        self.last_status = None
         try:
             if kind == "beats":
-                return p.result()
-            if kind == "logits_host":
+                out = p.result()
+            elif kind == "logits_host":
                 s, fo, _keep = p
                 s.done.synchronize()
                 total = fo[-1]
-                return s.logits_h[0, :total].numpy().copy(), s.logits_h[1, :total].numpy().copy(), fo
-            s, beat, down, fo = p
-            s.done.synchronize()
-            return beat, down, fo
+                out = s.logits_h[0, :total].numpy().copy(), s.logits_h[1, :total].numpy().copy(), fo
+            else:
+                s, beat, down, fo = p
+                s.done.synchronize()
+                out = beat, down, fo
+            s = self.slots[idx]
+            if s.flac_files:  # the status copy precedes the group's last event on the compute stream
+                self.last_status = s.flac_status[: s.flac_files].tolist()
+            return out
         finally:
             self.stats["collect_wait_s"] += time.perf_counter() - t0
             try:

@@ -38,7 +38,8 @@ extern "C" {
 #define BT_ERR_STATE (-3)
 #define BT_ERR_PARAM (-4)
 #define BT_ERR_IO (-5)     /* file could not be opened / read */
-#define BT_ERR_FORMAT (-6) /* not a RIFF/WAVE file this library decodes (caller falls back to another decoder) */
+#define BT_ERR_FORMAT (-6) /* not a file of the container the probe reads (RIFF/WAVE, FLAC) that this library decodes
+                            * (caller falls back to another decoder) */
 
 #define BT_DTYPE_F32 0  /* fp32 CUDA-core kernels: the reference's float16=False numerics   */
 #define BT_DTYPE_H16 1 /* 16-bit tensor-core kernels (wgmma GEMMs, mma.sync attention), fp32 accumulate + fp32 residual stream.  Operand type
@@ -192,6 +193,101 @@ int bt_wav_probe(const char* path, bt_wav_info* info);
  * BT_OK / BT_ERR_IO per file; files that fail are zero-filled and the call returns BT_ERR_IO. */
 int bt_stage_wav_files(const char* const* paths, const bt_wav_info* infos, int32_t n_files, float* dst,
                        const int64_t* dst_offsets, int32_t n_threads, int32_t* status);
+
+/* ---- FLAC (ABI 2.17): native decoding of FLAC files (RFC 9639), on the device -------------------------------------
+ * The front door of load_audio for FLAC files, and of the batched File2Beats path.  Three steps: bt_flac_probe reads
+ * the metadata (host), bt_stage_flac_files reads the frame bytes and finds the frames (host threads), bt_flac_decode
+ * decodes every frame of many files in one call (device).  Native FLAC streams only (no Ogg); 1..8 channels, 4..32 bits
+ * per sample. */
+typedef struct bt_flac_info {
+  int32_t sample_rate;
+  int32_t channels;        /* 1..8 */
+  int32_t bits_per_sample; /* 4..32 */
+  int32_t min_block;       /* STREAMINFO's block-size limits */
+  int32_t max_block;
+  int32_t reserved_;
+  int64_t total_samples;   /* samples per channel; 0: unknown (the frames define the length) */
+  int64_t frames_offset;   /* byte offset of the first frame in the file */
+  int64_t frames_bytes;    /* bytes from there to the end of the file */
+  int64_t max_frames;      /* frame-table entries bt_stage_flac_files may need for this file */
+  uint8_t md5[16];         /* STREAMINFO's MD5 of the samples (all zero: not given) */
+} bt_flac_info;
+
+/* Parse the metadata of a FLAC file: an optional leading ID3v2 tag, the "fLaC" marker, STREAMINFO as the first metadata
+ * block, every other block skipped.  max_frames is ceil(total / max(min_block, 16)) + 1 when the total is known, else
+ * frames_bytes / 10 + 1 (the shortest frame has 10 bytes).  Host only: no ctx, no GPU.  BT_ERR_IO: cannot open or read;
+ * BT_ERR_FORMAT: not a FLAC stream this library decodes (no marker, no or a malformed STREAMINFO, channels or bits per
+ * sample outside the limits above, metadata running past the end). */
+int bt_flac_probe(const char* path, bt_flac_info* info);
+
+/* One frame of a FLAC file: `offset` bytes from the start of its frame bytes, `bytes` long, holding samples
+ * [first_sample, first_sample + block_size) of every channel. */
+typedef struct bt_flac_frame {
+  int64_t offset;
+  int64_t first_sample;
+  int32_t bytes;
+  int32_t block_size;
+} bt_flac_frame;
+
+/* Read n_files probed FLAC files on n_threads host threads (<= 0: all): file i's infos[i].frames_bytes frame bytes go to
+ * bytes_dst + byte_offsets[i] (normally pinned memory, the source of one H2D copy), its frame table to frames_dst +
+ * frame_offsets[i] (room for infos[i].max_frames entries), its frame count to n_frames[i] and its samples per channel
+ * to n_samples[i].  Frames are found by a scan for the sync code; a candidate is a frame only when its header passes
+ * CRC-8, its reserved bits and values are valid, its frame number (fixed block size) or sample number (variable)
+ * continues the previous frame, and its channels, bits per sample, sample rate and block size agree with STREAMINFO
+ * (block size <= max_block).  The first frame starts at the first byte, the last runs to the end of the file.  When
+ * STREAMINFO's total is not 0 the block sizes must add up to it.  status[i]: BT_OK, or BT_ERR_IO (cannot read, no valid
+ * first frame, a total that disagrees, more frames than max_frames), which leaves n_frames[i] = n_samples[i] = 0; the
+ * call returns BT_ERR_IO when a file failed.  No CUDA, no ctx. */
+int bt_stage_flac_files(const char* const* paths, const bt_flac_info* infos, int32_t n_files, uint8_t* bytes_dst,
+                        const int64_t* byte_offsets, bt_flac_frame* frames_dst, const int64_t* frame_offsets,
+                        int64_t* n_frames, int64_t* n_samples, int32_t n_threads, int32_t* status);
+
+/* One stream of a bt_flac_decode call (host table). */
+typedef struct bt_flac_stream {
+  int64_t byte_offset;  /* its frame bytes start at bytes_dev + byte_offset ... */
+  int64_t byte_count;   /* ... and have this many bytes                        */
+  int64_t frame_offset; /* its frame table starts at frames_dev + frame_offset  */
+  int64_t n_frames;
+  int64_t n_samples;    /* per channel                                          */
+  int64_t out_offset;   /* element of out_dev where its output starts           */
+  int32_t channels;     /* 1..8                                                 */
+  int32_t bits_per_sample; /* 4..32                                             */
+} bt_flac_stream;
+
+#define BT_FLAC_MONO_F32 0     /* n_samples fp32: the mono mix of bt_stage_wav_files               */
+#define BT_FLAC_CHANNELS_F64 1 /* n_samples x channels float64 [time, ch]: what soundfile returns  */
+
+/* Decode n_streams FLAC streams on the device.  For every frame: CRC-16, each subframe (CONSTANT, VERBATIM, FIXED
+ * orders 0..4, LPC orders 1..32 with up to 15-bit coefficients and a shift >= 0; wasted bits; Rice residuals with 4- and
+ * 5-bit parameters, any partition order, escaped partitions), accumulated in int64; then the channel decorrelation
+ * (independent, left/side, side/right, mid/side).  Outputs, per sample t and with v * 2^-(bits-1) taken in float64:
+ *  - BT_FLAC_MONO_F32: out_dev (float*)[out_offset + t] = fp32(sum over channels in order / channels), the arithmetic of
+ *    bt_stage_wav_files, so a FLAC file and a WAV file of the same samples give the same bits (one channel: one multiply
+ *    and one rounding);
+ *  - BT_FLAC_CHANNELS_F64: out_dev (double*)[out_offset + t * channels + c].
+ * status_dev (n_streams int32, device) is read and written: a stream whose entry is not BT_OK is not decoded and its
+ * output is zero-filled; a malformed frame (CRC mismatch, reserved or refused coding, a read past the frame's end, a
+ * partition order the block size does not allow, a header that disagrees with the table or the stream, a frame outside
+ * the stream's bytes or samples) stores BT_ERR_IO there and zero-fills that stream's output; the other streams still
+ * decode.  Every read of a frame is bounded by its own span.  The frame table must cover each stream's samples (what
+ * bt_stage_flac_files writes); samples no frame covers are undefined.
+ * Needs an int64 scratch of sum(n_samples * channels) values, kept by the ctx and grown on demand (8 bytes per
+ * sample and channel: a group of 64 stereo clips of 30 s at 44.1 kHz needs 1.35 GB).  Any ctx will do (a weight-less
+ * one too).  Two launches at most, counted and profiled as "flac_frames" (when there is a frame) and "flac_output" (when
+ * there is a sample), enqueued on `stream` without synchronisation; the stream table goes through the staging ring.
+ * BT_ERR_ARG before anything is enqueued: n_streams < 0 or > 65535, an unknown mode, a NULL pointer (n_streams > 0),
+ * a negative count or offset, channels or bits per sample outside the limits. */
+int bt_flac_decode(bt_ctx* ctx, const uint8_t* bytes_dev, const bt_flac_frame* frames_dev,
+                   const bt_flac_stream* streams_host, int32_t n_streams, int32_t mode, void* out_dev, int32_t* status_dev,
+                   void* stream);
+
+/* Test hook: bt_flac_decode's arithmetic on the host, through the same frame decoder (bytes_host, frames_host, out_host
+ * and status_host in host memory; the same contract otherwise).  It is a check of the device code on machines without
+ * a GPU, not a decoder for the library's callers. */
+int bt_debug_flac_decode_host(const uint8_t* bytes_host, const bt_flac_frame* frames_host,
+                              const bt_flac_stream* streams_host, int32_t n_streams, int32_t mode, void* out_host,
+                              int32_t* status_host);
 
 /* ---- the hot path ------------------------------------------------------------------------- */
 
