@@ -17,8 +17,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 # BT_LIB_PATH: an instrumented build of the same sources (e.g. build(extra_flags=("-DBT_FF_PROF",), out_path=...))
 LIB_PATH = os.environ.get("BT_LIB_PATH") or os.path.join(HERE, "libbeatthis_sm90.so")
-SOURCES = ["bt_api.cu", "api_signal.cu", "api_post.cu", "api_data.cu", "api_train.cu", "api_debug.cu", "kernels_simt.cu", "kernels_misc.cu", "kernels_signal.cu", "kernels_gemm.cu", "kernels_attn.cu", "kernels_fused.cu", "kernels_dbn.cu", "kernels_eval.cu", "kernels_loss.cu", "kernels_data.cu", "kernels_train.cu", "kernels_optim.cu", "kernels_dp.cu", "kernels_flac.cu", "api_flac.cu", "dbn_host.cpp", "host_stage.cpp"]
-HEADERS = ["common.cuh", "epilogue.cuh", "fft.cuh", "tc_common.cuh", "chunk_table.cuh", "flac.cuh", "host_pool.h", "bt_kernels.h", "bt_train.h", "cuda_owned.h",
+SOURCES = ["bt_api.cu", "api_signal.cu", "api_post.cu", "api_data.cu", "api_train.cu", "api_debug.cu", "kernels_simt.cu", "kernels_misc.cu", "kernels_signal.cu", "kernels_gemm.cu", "kernels_attn.cu", "kernels_fused.cu", "kernels_dbn.cu", "kernels_eval.cu", "kernels_loss.cu", "kernels_data.cu", "kernels_train.cu", "kernels_optim.cu", "kernels_dp.cu", "kernels_flac.cu", "api_flac.cu", "kernels_mp3.cu", "api_mp3.cu", "dbn_host.cpp", "host_stage.cpp"]
+HEADERS = ["common.cuh", "epilogue.cuh", "fft.cuh", "tc_common.cuh", "chunk_table.cuh", "flac.cuh", "mp3.cuh", "host_pool.h", "bt_kernels.h", "bt_train.h", "cuda_owned.h",
            "dbn_model.h",
            "api_internal.h", os.path.join("..", "..", "include", "beatthis.h")]
 
@@ -77,6 +77,52 @@ class bt_flac_stream(ctypes.Structure):
 
 BT_FLAC_MONO_F32 = 0
 BT_FLAC_CHANNELS_F64 = 1
+
+
+class bt_mp3_info(ctypes.Structure):
+    _fields_ = [
+        ("sample_rate", c_int32),
+        ("channels", c_int32),
+        ("n_frames", c_int64),
+        ("n_samples", c_int64),
+        ("skip", c_int64),
+        ("padding", c_int64),
+        ("frames_offset", c_int64),
+        ("frames_bytes", c_int64),
+        ("max_frames", c_int64),
+        ("main_bytes", c_int64),
+        ("gapless", c_int32),
+        ("reserved_", c_int32),
+    ]
+
+
+class bt_mp3_frame(ctypes.Structure):
+    _fields_ = [
+        ("main_start", c_int64),
+        ("first_sample", c_int64),
+        ("header", ctypes.c_uint32),
+        ("main_bytes", c_int32),
+        ("side_info", ctypes.c_uint8 * 32),
+    ]
+
+
+class bt_mp3_stream(ctypes.Structure):
+    _fields_ = [
+        ("byte_offset", c_int64),
+        ("byte_count", c_int64),
+        ("frame_offset", c_int64),
+        ("n_frames", c_int64),
+        ("skip", c_int64),
+        ("n_samples", c_int64),
+        ("out_offset", c_int64),
+        ("channels", c_int32),
+        ("sample_rate", c_int32),
+    ]
+
+
+# the MP3 output modes are FLAC's
+BT_MP3_MONO_F32 = BT_FLAC_MONO_F32
+BT_MP3_CHANNELS_F64 = BT_FLAC_CHANNELS_F64
 
 
 class bt_hparams(ctypes.Structure):
@@ -305,6 +351,16 @@ PROTOTYPES = {
     ),
     "bt_debug_flac_decode_host": (
         c_int, [c_void_p, c_void_p, POINTER(bt_flac_stream), c_int32, c_int32, c_void_p, c_void_p],
+    ),
+    "bt_mp3_probe": (c_int, [c_char_p, POINTER(bt_mp3_info)]),
+    "bt_stage_mp3_files": (
+        c_int, [c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_void_p],
+    ),
+    "bt_mp3_decode": (
+        c_int, [c_void_p, c_void_p, c_void_p, POINTER(bt_mp3_stream), c_int32, c_int32, c_void_p, c_void_p, c_void_p],
+    ),
+    "bt_debug_mp3_decode_host": (
+        c_int, [c_void_p, c_void_p, POINTER(bt_mp3_stream), c_int32, c_int32, c_void_p, c_void_p],
     ),
     "bt_resample": (
         c_int,
@@ -656,16 +712,19 @@ def stage_wav_files(paths, infos, dst, sample_offsets, threads: int):
 
 def probe_audio(paths):
     """The container of every path as the native readers see it: a list of ("wav", bt_wav_info) (bt_wav_probe, with
-    samples), ("flac", bt_flac_info) (bt_flac_probe, with frame bytes) or (None, None) for anything else, which
-    load_audio's backend chain takes."""
+    samples), ("flac", bt_flac_info) (bt_flac_probe, with frame bytes), ("mp3", bt_mp3_info) (bt_mp3_probe, with
+    output samples) or (None, None) for anything else, which load_audio's backend chain takes.  WAV is tried first, then
+    FLAC, then MP3."""
     lib = load()
     out = []
     for p in paths:
-        w, f = bt_wav_info(), bt_flac_info()
+        w, f, m = bt_wav_info(), bt_flac_info(), bt_mp3_info()
         if lib.bt_wav_probe(str(p).encode(), ctypes.byref(w)) == 0 and w.frames > 0:
             out.append(("wav", w))
         elif lib.bt_flac_probe(str(p).encode(), ctypes.byref(f)) == 0 and f.frames_bytes > 0:
             out.append(("flac", f))
+        elif lib.bt_mp3_probe(str(p).encode(), ctypes.byref(m)) == 0 and m.n_samples > 0:
+            out.append(("mp3", m))
         else:
             out.append((None, None))
     return out
@@ -674,15 +733,22 @@ def probe_audio(paths):
 FLAC_FRAME_BYTES = ctypes.sizeof(bt_flac_frame)
 
 
+def _compressed_layout(entries, entry_bytes: int, byte_counts):
+    """Frame tables first (entry k at byte entry_bytes * k; entries[i] per file), then one int32 status per file, then
+    each file's bytes (byte_counts[i]): (frame-table entry offsets, status offset, byte offsets, total bytes)."""
+    fo = offsets(entries)
+    status_at = entry_bytes * fo[-1]
+    bytes_at = status_at + 4 * (len(fo) - 1)
+    bo = [bytes_at + v for v in offsets(byte_counts)]
+    return fo, status_at, bo, bo[-1]
+
+
 def flac_layout(infos):
     """Where bt_stage_flac_files puts the files `infos` in one byte buffer: (frame-table entry offsets, status offset,
     frame-byte offsets, total bytes).  The frame tables come first (entry k at byte FLAC_FRAME_BYTES * k), then one
     int32 status per file, then each file's frame bytes."""
-    fo = offsets(info.max_frames for info in infos)
-    status_at = FLAC_FRAME_BYTES * fo[-1]
-    bytes_at = status_at + 4 * len(infos)
-    bo = [bytes_at + v for v in offsets(info.frames_bytes for info in infos)]
-    return fo, status_at, bo, bo[-1]
+    return _compressed_layout([info.max_frames for info in infos], FLAC_FRAME_BYTES,
+                              [info.frames_bytes for info in infos])
 
 
 def stage_flac_files(paths, infos, buf_ptr: int, threads: int):
@@ -706,6 +772,38 @@ def flac_streams(infos, n_frames, n_samples, out_offsets):
     return (bt_flac_stream * n)(*[
         bt_flac_stream(bo[i], infos[i].frames_bytes, fo[i], n_frames[i], n_samples[i], out_offsets[i],
                        infos[i].channels, infos[i].bits_per_sample) for i in range(n)])
+
+
+MP3_FRAME_BYTES = ctypes.sizeof(bt_mp3_frame)
+
+
+def mp3_layout(infos):
+    """Where bt_stage_mp3_files puts the files `infos` in one byte buffer, as flac_layout does: frame tables
+    (MP3_FRAME_BYTES per entry), one int32 status per file, then each file's compacted main data."""
+    return _compressed_layout([info.max_frames for info in infos], MP3_FRAME_BYTES, [info.main_bytes for info in infos])
+
+
+def stage_mp3_files(paths, infos, buf_ptr: int, threads: int):
+    """bt_stage_mp3_files into the byte buffer at host address buf_ptr, laid out as mp3_layout(infos) says, each file's
+    status stored at its slot of the buffer: (n_frames, main_bytes, status) lists."""
+    n = len(paths)
+    fo, status_at, bo, _ = mp3_layout(infos)
+    cpaths = (c_char_p * n)(*[str(p).encode() for p in paths])
+    nf, mb = (c_int64 * n)(), (c_int64 * n)()
+    status = (c_int32 * n).from_address(buf_ptr + status_at)
+    load().bt_stage_mp3_files(cpaths, (bt_mp3_info * n)(*infos), n, c_void_p(buf_ptr), i64_array(bo[:-1]),
+                              c_void_p(buf_ptr), i64_array(fo[:-1]), mb, nf, threads, status)
+    return list(nf), list(mb), list(status)
+
+
+def mp3_streams(infos, n_frames, main_bytes, out_offsets):
+    """The bt_mp3_stream table of files staged by stage_mp3_files (offsets relative to the same buffer), file i's
+    output (infos[i].n_samples samples per channel) from out_offsets[i] on."""
+    fo, _, bo, _ = mp3_layout(infos)
+    n = len(infos)
+    return (bt_mp3_stream * n)(*[
+        bt_mp3_stream(bo[i], main_bytes[i], fo[i], n_frames[i], infos[i].skip, infos[i].n_samples, out_offsets[i],
+                      infos[i].channels, infos[i].sample_rate) for i in range(n)])
 
 
 def dbn_viterbi(log_densities, beats: int, intervals, log_tempo, pointers):

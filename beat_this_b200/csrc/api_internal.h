@@ -105,6 +105,8 @@ struct bt_ctx {
   DeviceBuffer<float> istft_frames;
   // decoded samples of bt_flac_decode, [channels][n_samples] int64 per stream (grows on demand)
   DeviceBuffer<int64_t> flac_ws;
+  // granule records and IMDCT blocks of bt_mp3_decode (grows on demand)
+  DeviceBuffer<char> mp3_ws;
   // pinned staging + device tables
   StageSlot stage[kStageSlots];
   int stage_next = 0;

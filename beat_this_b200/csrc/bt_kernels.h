@@ -261,6 +261,30 @@ void launch_flac_frames(const FlacStreamDev* streams_dev, int n_streams, int64_t
 void launch_flac_output(const FlacStreamDev* streams_dev, int n_streams, int64_t max_samples, int mode, void* out,
                         const int32_t* status, cudaStream_t st);
 
+// ---- MP3 decoding (kernels_mp3.cu, mp3.cuh) --------------------------------------------------------------------------
+// One stream of a bt_mp3_decode call on the device: its compacted main data and frame table (bt_mp3_frame entries),
+// its scratch (one granule record per frame, granule and channel; 2 x channels x 32 x 36 fp32 IMDCT values per frame)
+// and its output window.
+struct Mp3StreamDev {
+  const uint8_t* bytes;
+  const void* frames;
+  void* recs;
+  float* blocks;
+  int64_t byte_count, n_frames, skip, n_samples, out_off;
+  int32_t channels, rate_index;
+};
+// one thread per (frame, channel): scalefactors and Huffman lines of both granules (lut: mp3.cuh's lookup tables)
+void launch_mp3_granules(const Mp3StreamDev* streams_dev, int n_streams, int64_t max_frames, const uint32_t* lut,
+                         int32_t* status, cudaStream_t st);
+// one CTA per (frame, granule): requantisation, stereo, reorder, alias reduction, IMDCT of both channels (tables:
+// mp3.cuh's kFloatTables floats)
+void launch_mp3_hybrid(const Mp3StreamDev* streams_dev, int n_streams, int64_t max_frames, const float* tables,
+                       const int32_t* status, cudaStream_t st);
+// one CTA per granule of output, max_granules covering every stream's skip + n_samples: overlap-add, polyphase
+// synthesis, trim, output mode (0 mono fp32, 1 float64 [time, ch]); zeros where a stream is not decoded
+void launch_mp3_synth(const Mp3StreamDev* streams_dev, int n_streams, int64_t max_granules, const float* tables,
+                      int mode, void* out, const int32_t* status, cudaStream_t st);
+
 void launch_f32_to_h16(const float* in, void* out, int64_t n, cudaStream_t st);
 void launch_h16_to_f32(const void* in, float* out, int64_t n, cudaStream_t st);
 // [seqs, L, heads*32] fp32 q,k,v -> packed qkv buffer [seqs*L, 3C] of the activation dtype

@@ -5,10 +5,10 @@ The reference handles one clip at a time on one stream (reference beat_this/infe
 one pass of every kernel); for every group
 
   host threads   mono mix + fp32 cast of all clips straight into a pinned ring slot (``bt_stage_audio`` /
-                 ``bt_stage_wav_files``: C++, GIL released); for FLAC files, their frame bytes and frame tables
-                 (``bt_stage_flac_files``)
+                 ``bt_stage_wav_files``: C++, GIL released); for FLAC and MP3 files, their frame bytes and frame
+                 tables (``bt_stage_flac_files``, ``bt_stage_mp3_files``)
   copy stream    one H2D copy of the slot
-  compute stream [FLAC: decode and mono mix (``bt_flac_decode``)] -> log-mel -> BeatThis forward -> (peak picking
+  compute stream [FLAC / MP3: decode and mono mix (``bt_flac_decode``, ``bt_mp3_decode``)] -> log-mel -> BeatThis forward -> (peak picking
                  | device DBN -> D2H of the timestamps | D2H of the logits for the host DBN)
 
 and group g+1 is staged and copied while the kernels of group g run; results are collected in order.  Nothing in the
@@ -79,10 +79,10 @@ class _Slot:
         self.done = None
         self.t0 = None        # events around the group's kernels (stats: GPU busy time)
         self.t1 = None
-        self.flac_host = None  # pinned bytes of a FLAC group (_lib.flac_layout), its device copy and the D2H
-        self.flac_dev = None   # copy of its files' statuses
+        self.flac_host = None  # pinned bytes of a FLAC or MP3 group (_lib.flac_layout, _lib.mp3_layout), its device
+        self.flac_dev = None   # copy and the D2H copy of its files' statuses
         self.flac_status = None
-        self.flac_files = 0    # FLAC files of the group in flight (0: not a FLAC group)
+        self.flac_files = 0    # FLAC or MP3 files of the group in flight (0: not a compressed group)
 
 
 class BeatPipeline:
@@ -112,7 +112,7 @@ class BeatPipeline:
         self.h2d_bytes = 0
         self.d2h_bytes = 0
         self.dbn_params = None  # tracker parameters of want="dbn_device" (Postprocessor.dbn_params)
-        self.last_status = None  # per-file statuses of the last collected FLAC group (collect)
+        self.last_status = None  # per-file statuses of the last collected FLAC or MP3 group (collect)
         # host seconds spent staging (mono mix / decode into pinned memory), enqueueing and waiting for results
         self.stats = {"stage_s": 0.0, "enqueue_s": 0.0, "collect_wait_s": 0.0, "gpu_busy_s": 0.0, "groups": 0}
 
@@ -135,16 +135,17 @@ class BeatPipeline:
         return _lib.stage_audio(arrays, dst, self.host_threads)
 
     def _enqueue(self, idx, s, so, sr, want, chunking=DEFAULT_CHUNKING, flac=None):
-        """flac: (streams, status offset, bytes) of a FLAC group staged in s.flac_host, decoded into s.dev on the
-        compute stream; otherwise s.host holds the group's mono fp32 samples."""
+        """flac: (decode, streams, status offset, bytes) of a compressed (FLAC or MP3) group staged in s.flac_host,
+        decoded into s.dev on the compute stream by decode(buf, streams, mode, out, status offset) (an Engine
+        method); otherwise s.host holds the group's mono fp32 samples."""
         n = so[-1]
         with torch.cuda.stream(self.copy_stream):
             if flac is None:
                 s.dev[:n].copy_(s.host[:n], non_blocking=True)
             else:
-                s.flac_dev[: flac[2]].copy_(s.flac_host[: flac[2]], non_blocking=True)
+                s.flac_dev[: flac[3]].copy_(s.flac_host[: flac[3]], non_blocking=True)
             s.copied.record(self.copy_stream)
-        self.h2d_bytes += n * 4 if flac is None else flac[2]
+        self.h2d_bytes += n * 4 if flac is None else flac[3]
         eng = self.engine
         if s.t0 is None:
             s.t0, s.t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -153,8 +154,8 @@ class BeatPipeline:
             s.t0.record(self.compute_stream)
             s.flac_files = 0
             if flac is not None:
-                streams, status_at, _ = flac
-                eng.flac_decode(s.flac_dev, streams, _lib.BT_FLAC_MONO_F32, s.dev, status_at)
+                decode, streams, status_at, _ = flac
+                decode(s.flac_dev, streams, _lib.BT_FLAC_MONO_F32, s.dev, status_at)
                 s.flac_files = len(streams)
                 s.flac_status[: len(streams)].copy_(s.flac_dev[status_at : status_at + 4 * len(streams)].view(torch.int32),
                                                     non_blocking=True)
@@ -228,9 +229,38 @@ class BeatPipeline:
         chunking as in submit_signals.  Host threads stage the frame bytes and tables, the device decodes them and mixes
         to mono (bt_flac_decode), and the group runs on as submit_wavs's.  A file that fails to stage or decode runs as
         zeros of its STREAMINFO length; `last_status` gives every file's status when the group is collected."""
-        _check_frames_route(want, chunking)
+
+        def stage(buf_ptr):
+            nf, ns, status = _lib.stage_flac_files(paths, infos, buf_ptr, self.host_threads)
+            # staging checks the block sizes against STREAMINFO's total, so a staged file has its so length; one that
+            # failed is not decoded and runs as zeros of that length
+            return _lib.flac_streams(infos, nf, [info.total_samples for info in infos], so[:-1]), status
+
         so = _lib.offsets(info.total_samples for info in infos)
-        fo, status_at, bo, total = _lib.flac_layout(infos)
+        self._submit_compressed(so, _lib.flac_layout(infos), stage, self.engine.flac_decode, len(paths), sr, want,
+                                chunking)
+
+    def submit_mp3s(self, paths, infos, sr: int, want: str = "beats", chunking: tuple = DEFAULT_CHUNKING):
+        """paths: list of str; infos: list of bt_mp3_info (all `sr` Hz) from _lib.probe_audio; chunking as in
+        submit_signals.  Host threads stage the main data and frame tables, the device decodes them and mixes to mono
+        (bt_mp3_decode), and the group runs on as submit_wavs's.  A file that fails to stage or decode runs as zeros of
+        its probed length; `last_status` gives every file's status when the group is collected."""
+
+        def stage(buf_ptr):
+            nf, mb, status = _lib.stage_mp3_files(paths, infos, buf_ptr, self.host_threads)
+            return _lib.mp3_streams(infos, nf, mb, so[:-1]), status
+
+        so = _lib.offsets(info.n_samples for info in infos)
+        self._submit_compressed(so, _lib.mp3_layout(infos), stage, self.engine.mp3_decode, len(paths), sr, want,
+                                chunking)
+
+    def _submit_compressed(self, so, layout, stage, decode, n_files, sr, want, chunking):
+        """One group of compressed files: so, their sample offsets; layout, where the staged frame tables, statuses and
+        frame data sit (_lib.flac_layout, _lib.mp3_layout); stage(host address) fills a pinned buffer and returns (streams,
+        statuses); decode is the Engine method that decodes the streams on the compute stream.  A file whose staging
+        failed is not decoded (no frames) and runs as zeros."""
+        _check_frames_route(want, chunking)
+        _, status_at, _, total = layout
         idx, s = self._slot(so[-1])
         try:
             t0 = time.perf_counter()
@@ -238,17 +268,14 @@ class BeatPipeline:
                 cap = max(int(total * 1.25), 1 << 20)
                 s.flac_host = torch.empty(cap, dtype=torch.uint8, pin_memory=True)
                 s.flac_dev = torch.empty(cap, dtype=torch.uint8, device=self.device)
-            if s.flac_status is None or s.flac_status.numel() < len(paths):
-                s.flac_status = torch.empty(max(len(paths), 64), dtype=torch.int32, pin_memory=True)
-            nf, ns, status = _lib.stage_flac_files(paths, infos, s.flac_host.data_ptr(), self.host_threads)
-            # staging checks the block sizes against STREAMINFO's total, so a staged file has its so length; one that
-            # failed is not decoded and runs as zeros of that length
-            streams = _lib.flac_streams(infos, nf, [info.total_samples for info in infos], so[:-1])
+            if s.flac_status is None or s.flac_status.numel() < n_files:
+                s.flac_status = torch.empty(max(n_files, 64), dtype=torch.int32, pin_memory=True)
+            streams, status = stage(s.flac_host.data_ptr())
             for i, st in enumerate(status):
                 if st != 0:
                     streams[i].n_frames = 0
             t1 = time.perf_counter()
-            self._enqueue(idx, s, so, int(sr), want, chunking, (streams, status_at, total))
+            self._enqueue(idx, s, so, int(sr), want, chunking, (decode, streams, status_at, total))
             self.stats["stage_s"] += t1 - t0
             self.stats["enqueue_s"] += time.perf_counter() - t1
             self.stats["groups"] += 1
@@ -267,7 +294,7 @@ class BeatPipeline:
     def collect(self):
         """Oldest group: list of (beat_times, downbeat_times) ["beats", "dbn_device"], (beat, down, fo) host arrays
         ["logits_host"] or device tensors ["frames"].  After it, last_status lists the status (BT_OK or BT_ERR_IO) of
-        every file of a FLAC group, and is None for other groups."""
+        every file of a FLAC or MP3 group, and is None for other groups."""
         idx, (kind, p) = self.inflight.popleft()
         t0 = time.perf_counter()
         self.last_status = None

@@ -5,9 +5,10 @@ reference defaults it runs the model path's fused sm_90a kernel (frame -> Hann -
 128-band slaney mel -> log1p(1000 x)) through ``bt_logmel``; any other analysis parameters run the general kernel
 through ``bt_logmel_config`` on the tables ``MelTables`` builds.
 ``load_audio`` (preprocessing.py:6-24) walks the reference's decoder chain (torchaudio, soundfile, madmom -- whichever
-is installed), then the native FLAC decoder (``bt_flac_decode`` on the current CUDA device) and then two
-dependency-free WAV readers; the batched File2Beats path reads WAV and FLAC files natively (``bt_stage_wav_files``,
-``bt_flac_decode``) and only falls back to this function for other containers.
+is installed), then the native FLAC and MP3 decoders (``bt_flac_decode``, ``bt_mp3_decode`` on the current CUDA device)
+and then two dependency-free WAV readers; the batched File2Beats path reads WAV, FLAC and MP3 files natively
+(``bt_stage_wav_files``, ``bt_flac_decode``, ``bt_mp3_decode``) and only falls back to this function for other
+containers.
 """
 from __future__ import annotations
 
@@ -107,11 +108,43 @@ def _decode_flac_native(path, dtype):
     return (wav.reshape(n, ch) if ch > 1 else wav).astype(dtype, copy=False), int(info.sample_rate)
 
 
+def _decode_mp3_native(path, dtype):
+    """An MPEG-1 Layer III file decoded on the current CUDA device (bt_mp3_decode): float64 samples, [time] or
+    [time, channels], as torchaudio returns them cast to float64."""
+    import ctypes
+
+    from . import _lib
+
+    info = _lib.bt_mp3_info()
+    code = _lib.load().bt_mp3_probe(str(path).encode(), ctypes.byref(info))
+    if code != 0:
+        raise ValueError("not an MPEG-1 Layer III stream" if code == -6 else "cannot read the file")
+    if not torch.cuda.is_available():
+        raise RuntimeError("no CUDA device to decode MP3 on")
+    from .engine import Engine
+
+    fo, status_at, bo, total = _lib.mp3_layout([info])
+    host = np.zeros(max(total, 1), dtype=np.uint8)
+    nf, mb, status = _lib.stage_mp3_files([path], [info], host.ctypes.data, 1)
+    if status[0] != 0:
+        raise RuntimeError("malformed MP3 frames")
+    n, ch = info.n_samples, info.channels
+    dev = torch.device("cuda", torch.cuda.current_device())
+    buf = torch.from_numpy(host).to(dev)
+    out = torch.empty(max(n * ch, 1), dtype=torch.float64, device=dev)
+    Engine.shared(dev).mp3_decode(buf, _lib.mp3_streams([info], nf, mb, [0]), _lib.BT_MP3_CHANNELS_F64, out, status_at)
+    if int(buf[status_at : status_at + 4].view(torch.int32).item()) != 0:
+        raise RuntimeError("malformed MP3 frames")
+    wav = out[: n * ch].cpu().numpy()
+    return (wav.reshape(n, ch) if ch > 1 else wav).astype(dtype, copy=False), int(info.sample_rate)
+
+
 # tried in this order; the first three are the reference's chain (preprocessing.py:6-24), the rest need nothing beyond
 # this package, scipy and the standard library and keep FLAC and WAV input working where none of those packages has a
 # decoder
 AUDIO_BACKENDS = (("torchaudio", _decode_torchaudio), ("soundfile", _decode_soundfile), ("madmom", _decode_madmom),
-                  ("native FLAC", _decode_flac_native), ("scipy.io.wavfile", _decode_wav_scipy),
+                  ("native FLAC", _decode_flac_native), ("native MP3", _decode_mp3_native),
+                  ("scipy.io.wavfile", _decode_wav_scipy),
                   ("wave", _decode_wav_stdlib))
 
 
@@ -123,9 +156,10 @@ def load_audio(path, dtype="float64"):
         try:
             return decode(path, dtype)
         except Exception as e:  # missing package, missing codec, unreadable file: next backend
-            tried.append(f"{name}: {type(e).__name__}" + (f" ({e})" if name == "native FLAC" else ""))
-    raise RuntimeError(f'Could not load audio from "{path}". Without torchaudio, soundfile or madmom, FLAC (on a CUDA '
-                       "device) and WAV are the formats read. (" + "; ".join(tried) + ")")
+            tried.append(f"{name}: {type(e).__name__}" + (f" ({e})" if name.startswith("native") else ""))
+    raise RuntimeError(f'Could not load audio from "{path}". Without torchaudio, soundfile or madmom, FLAC and MP3 '
+                       "(MPEG-1 Layer III; both on a CUDA device) and WAV are the formats read. (" + "; ".join(tried)
+                       + ")")
 
 
 # ------------------------------------------------------------------------------------------

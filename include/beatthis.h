@@ -38,7 +38,7 @@ extern "C" {
 #define BT_ERR_STATE (-3)
 #define BT_ERR_PARAM (-4)
 #define BT_ERR_IO (-5)     /* file could not be opened / read */
-#define BT_ERR_FORMAT (-6) /* not a file of the container the probe reads (RIFF/WAVE, FLAC) that this library decodes
+#define BT_ERR_FORMAT (-6) /* not a file of the container the probe reads (RIFF/WAVE, FLAC, MP3) that this library decodes
                             * (caller falls back to another decoder) */
 
 #define BT_DTYPE_F32 0  /* fp32 CUDA-core kernels: the reference's float16=False numerics   */
@@ -288,6 +288,94 @@ int bt_flac_decode(bt_ctx* ctx, const uint8_t* bytes_dev, const bt_flac_frame* f
 int bt_debug_flac_decode_host(const uint8_t* bytes_host, const bt_flac_frame* frames_host,
                               const bt_flac_stream* streams_host, int32_t n_streams, int32_t mode, void* out_host,
                               int32_t* status_host);
+
+/* ---- MP3 (ABI 2.18): native decoding of MPEG-1 Layer III files (ISO/IEC 11172-3), on the device --------------------
+ * The same three steps as FLAC's: bt_mp3_probe walks the frame headers (host), bt_stage_mp3_files reads each file's
+ * frames and lays out their main data (host threads), bt_mp3_decode decodes every frame of many files in one call
+ * (device).  32, 44.1 and 48 kHz, mono and stereo; every bitrate, CBR or VBR.  MPEG-2 / 2.5 (LSF), Layers I and II, free
+ * format, reserved header values and streams whose rate or channel count changes are refused (BT_ERR_FORMAT). */
+typedef struct bt_mp3_info {
+  int32_t sample_rate;
+  int32_t channels;        /* 1 or 2 */
+  int64_t n_frames;        /* audio frames (a Xing / Info frame is not one) */
+  int64_t n_samples;       /* output samples per channel, after the gapless trim */
+  int64_t skip;            /* decoded samples dropped at the start (encoder delay + 529 when tagged, else 0) */
+  int64_t padding;         /* encoder padding of a gapless tag (0: none) */
+  int64_t frames_offset;   /* byte range of the audio frames in the file */
+  int64_t frames_bytes;
+  int64_t max_frames;      /* frame-table entries bt_stage_mp3_files writes for this file */
+  int64_t main_bytes;      /* bound on the file's compacted main-data bytes */
+  int32_t gapless;         /* 1: a Xing / Info frame with a LAME-style tag whose frame count matches */
+  int32_t reserved_;
+} bt_mp3_info;
+
+/* Walk the headers of an MP3 file: an optional leading ID3v2 tag (with or without footer), then junk or false syncs
+ * until the first header that is followed by two more consistent headers, each at the length the one before gives (or
+ * by the end of the file, after a trailing ID3v1 or APEv2 tag); then frame after frame.  Bytes after the last frame with no further frame in
+ * them are ignored, and a truncated last frame is dropped.  Host only.  BT_ERR_IO: cannot open or read;
+ * BT_ERR_FORMAT: no MPEG-1 Layer III stream as above, or one whose rate or channel count changes.  A stream that loses
+ * sync in the middle is probed (n_frames counts the frames before the loss) and refused by bt_stage_mp3_files. */
+int bt_mp3_probe(const char* path, bt_mp3_info* info);
+
+/* One frame of a staged MP3 stream. */
+typedef struct bt_mp3_frame {
+  int64_t main_start;      /* its main data starts at this byte of the stream's compacted main data (may be < 0) */
+  int64_t first_sample;    /* its first decoded sample: 1152 x frame index */
+  uint32_t header;         /* the 4 header bytes, big-endian */
+  int32_t main_bytes;      /* main-data bytes the frame itself carries */
+  uint8_t side_info[32];   /* its side info (17 bytes for mono) */
+} bt_mp3_frame;
+
+/* Read n_files probed MP3 files on n_threads host threads (<= 0: all): file i's compacted main data (each frame's
+ * bytes after header, CRC and side info, back to back; at most infos[i].main_bytes) goes to bytes_dst + byte_offsets[i],
+ * its frame table to frames_dst + frame_offsets[i] (infos[i].max_frames entries), the main-data bytes to main_bytes[i]
+ * and the frame count to n_frames[i].  status[i]: BT_OK, or BT_ERR_IO (cannot read, lost sync in the middle, a walk
+ * that disagrees with the probe), which leaves n_frames[i] = 0; the call returns BT_ERR_IO when a file failed. */
+int bt_stage_mp3_files(const char* const* paths, const bt_mp3_info* infos, int32_t n_files, uint8_t* bytes_dst,
+                       const int64_t* byte_offsets, bt_mp3_frame* frames_dst, const int64_t* frame_offsets,
+                       int64_t* main_bytes, int64_t* n_frames, int32_t n_threads, int32_t* status);
+
+/* One stream of a bt_mp3_decode call (host table). */
+typedef struct bt_mp3_stream {
+  int64_t byte_offset;  /* its compacted main data starts at bytes_dev + byte_offset ... */
+  int64_t byte_count;   /* ... and has this many bytes                                 */
+  int64_t frame_offset; /* its frame table starts at frames_dev + frame_offset          */
+  int64_t n_frames;
+  int64_t skip;         /* decoded samples dropped at the start                          */
+  int64_t n_samples;    /* output samples per channel from there                         */
+  int64_t out_offset;   /* element of out_dev where its output starts                    */
+  int32_t channels;     /* 1 or 2                                                        */
+  int32_t sample_rate;  /* 32000, 44100 or 48000                                         */
+} bt_mp3_stream;
+
+#define BT_MP3_MONO_F32 BT_FLAC_MONO_F32         /* fp32((sum over channels of double(s_c)) / channels)         */
+#define BT_MP3_CHANNELS_F64 BT_FLAC_CHANNELS_F64 /* double(s_c) [time, ch], what torchaudio returns as float64 */
+
+/* Decode n_streams MP3 streams on the device in fp32 (no clipping, no rounding to integers): scalefactors with scfsi,
+ * Huffman big-values and count1 regions, requantisation, M/S and intensity stereo, short-block reordering, alias
+ * reduction, IMDCT of every block type including mixed blocks, overlap-add and the polyphase synthesis; then decoded
+ * samples [skip, skip + n_samples) in the mode's output.  status_dev (n_streams int32, device) is read and written as
+ * bt_flac_decode's: a stream whose entry is not BT_OK is not decoded and is zero-filled; a malformed granule
+ * (scalefactors or big values past part2_3_length, big_values > 288, table 4 or 14, block type 0 with window switching,
+ * main data past the stream's end, a frame entry outside its stream) stores BT_ERR_IO and zero-fills the stream.  A
+ * count1 quadruple that overshoots part2_3_length is dropped, and a granule whose main data begins before the stream
+ * decodes as zeros (a main-data start more than 511 bytes before the stream is outside it: BT_ERR_IO).  Needs a
+ * scratch of 5820 bytes per granule and channel (a 1212-byte granule record and 32 x 36 fp32 IMDCT values), about
+ * 20 bytes per output sample of a stereo stream (2.2 GB for 64 stereo clips of 30 s at 44.1 kHz, 14 GB for 64 of four
+ * minutes), kept by the ctx and grown on demand.  Three launches at most, counted and profiled as "mp3_granules" and
+ * "mp3_hybrid" (when a stream has a frame) and "mp3_synth" (when a stream has an output sample: streams that are not
+ * decoded, having no frames or a status that is not BT_OK, are zero-filled by it), enqueued on `stream`.
+ * BT_ERR_ARG before anything is enqueued: n_streams < 0 or > 65535, an unknown mode, a NULL pointer (n_streams > 0),
+ * a negative count or offset, channels outside 1..2, a sample rate MPEG-1 does not have. */
+int bt_mp3_decode(bt_ctx* ctx, const uint8_t* bytes_dev, const bt_mp3_frame* frames_dev,
+                  const bt_mp3_stream* streams_host, int32_t n_streams, int32_t mode, void* out_dev, int32_t* status_dev,
+                  void* stream);
+
+/* Test hook: bt_mp3_decode's arithmetic on the host, through the same per-lane functions (mp3.cuh); host memory, the
+ * same contract otherwise. */
+int bt_debug_mp3_decode_host(const uint8_t* bytes_host, const bt_mp3_frame* frames_host,
+                             const bt_mp3_stream* streams_host, int32_t n_streams, int32_t mode, void* out_host,
+                             int32_t* status_host);
 
 /* ---- the hot path ------------------------------------------------------------------------- */
 
