@@ -17,8 +17,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 # BT_LIB_PATH: an instrumented build of the same sources (e.g. build(extra_flags=("-DBT_FF_PROF",), out_path=...))
 LIB_PATH = os.environ.get("BT_LIB_PATH") or os.path.join(HERE, "libbeatthis_sm90.so")
-SOURCES = ["bt_api.cu", "api_signal.cu", "api_post.cu", "api_data.cu", "api_train.cu", "api_debug.cu", "kernels_simt.cu", "kernels_misc.cu", "kernels_signal.cu", "kernels_gemm.cu", "kernels_attn.cu", "kernels_fused.cu", "kernels_dbn.cu", "kernels_eval.cu", "kernels_loss.cu", "kernels_data.cu", "kernels_train.cu", "kernels_optim.cu", "kernels_dp.cu", "kernels_flac.cu", "api_flac.cu", "kernels_mp3.cu", "api_mp3.cu", "dbn_host.cpp", "host_stage.cpp"]
-HEADERS = ["common.cuh", "epilogue.cuh", "fft.cuh", "tc_common.cuh", "chunk_table.cuh", "flac.cuh", "mp3.cuh", "host_pool.h", "bt_kernels.h", "bt_train.h", "cuda_owned.h",
+SOURCES = ["bt_api.cu", "api_signal.cu", "api_post.cu", "api_data.cu", "api_train.cu", "api_debug.cu", "kernels_simt.cu", "kernels_misc.cu", "kernels_signal.cu", "kernels_gemm.cu", "kernels_attn.cu", "kernels_fused.cu", "kernels_dbn.cu", "kernels_eval.cu", "kernels_loss.cu", "kernels_data.cu", "kernels_train.cu", "kernels_optim.cu", "kernels_dp.cu", "kernels_flac.cu", "api_flac.cu", "kernels_mp3.cu", "api_mp3.cu", "kernels_vorbis.cu", "api_vorbis.cu", "dbn_host.cpp", "host_stage.cpp"]
+HEADERS = ["common.cuh", "epilogue.cuh", "fft.cuh", "tc_common.cuh", "chunk_table.cuh", "flac.cuh", "mp3.cuh", "vorbis.cuh", "host_pool.h", "bt_kernels.h", "bt_train.h", "cuda_owned.h",
            "dbn_model.h",
            "api_internal.h", os.path.join("..", "..", "include", "beatthis.h")]
 
@@ -123,6 +123,55 @@ class bt_mp3_stream(ctypes.Structure):
 # the MP3 output modes are FLAC's
 BT_MP3_MONO_F32 = BT_FLAC_MONO_F32
 BT_MP3_CHANNELS_F64 = BT_FLAC_CHANNELS_F64
+
+
+class bt_vorbis_info(ctypes.Structure):
+    _fields_ = [
+        ("sample_rate", c_int32),
+        ("channels", c_int32),
+        ("blocksize0", c_int32),
+        ("blocksize1", c_int32),
+        ("n_packets", c_int64),
+        ("packet_bytes", c_int64),
+        ("table_bytes", c_int64),
+        ("skip", c_int64),
+        ("n_samples", c_int64),
+    ]
+
+
+class bt_vorbis_packet(ctypes.Structure):
+    _fields_ = [
+        ("byte_offset", c_int64),
+        ("end_sample", c_int64),
+        ("block_offset", c_int64),
+        ("bytes", c_int32),
+        ("mode", ctypes.c_uint8),
+        ("blockflag", ctypes.c_uint8),
+        ("prev_long", ctypes.c_uint8),
+        ("next_long", ctypes.c_uint8),
+    ]
+
+
+class bt_vorbis_stream(ctypes.Structure):
+    _fields_ = [
+        ("byte_offset", c_int64),
+        ("byte_count", c_int64),
+        ("table_offset", c_int64),
+        ("table_bytes", c_int64),
+        ("packet_offset", c_int64),
+        ("n_packets", c_int64),
+        ("block_samples", c_int64),
+        ("skip", c_int64),
+        ("n_samples", c_int64),
+        ("out_offset", c_int64),
+        ("channels", c_int32),
+        ("sample_rate", c_int32),
+    ]
+
+
+# the Vorbis output modes are FLAC's
+BT_VORBIS_MONO_F32 = BT_FLAC_MONO_F32
+BT_VORBIS_CHANNELS_F64 = BT_FLAC_CHANNELS_F64
 
 
 class bt_hparams(ctypes.Structure):
@@ -361,6 +410,17 @@ PROTOTYPES = {
     ),
     "bt_debug_mp3_decode_host": (
         c_int, [c_void_p, c_void_p, POINTER(bt_mp3_stream), c_int32, c_int32, c_void_p, c_void_p],
+    ),
+    "bt_vorbis_probe": (c_int, [c_char_p, POINTER(bt_vorbis_info)]),
+    "bt_stage_vorbis_files": (
+        c_int, [c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                c_int32, c_void_p],
+    ),
+    "bt_vorbis_decode": (
+        c_int, [c_void_p, c_void_p, c_void_p, POINTER(bt_vorbis_stream), c_int32, c_int32, c_void_p, c_void_p, c_void_p],
+    ),
+    "bt_debug_vorbis_decode_host": (
+        c_int, [c_void_p, c_void_p, POINTER(bt_vorbis_stream), c_int32, c_int32, c_void_p, c_void_p],
     ),
     "bt_resample": (
         c_int,
@@ -713,18 +773,20 @@ def stage_wav_files(paths, infos, dst, sample_offsets, threads: int):
 def probe_audio(paths):
     """The container of every path as the native readers see it: a list of ("wav", bt_wav_info) (bt_wav_probe, with
     samples), ("flac", bt_flac_info) (bt_flac_probe, with frame bytes), ("mp3", bt_mp3_info) (bt_mp3_probe, with
-    output samples) or (None, None) for anything else, which load_audio's backend chain takes.  WAV is tried first, then
-    FLAC, then MP3."""
+    output samples), ("vorbis", bt_vorbis_info) (bt_vorbis_probe, with output samples) or (None, None) for anything
+    else, which load_audio's backend chain takes.  WAV is tried first, then FLAC, then MP3, then Ogg Vorbis."""
     lib = load()
     out = []
     for p in paths:
-        w, f, m = bt_wav_info(), bt_flac_info(), bt_mp3_info()
+        w, f, m, v = bt_wav_info(), bt_flac_info(), bt_mp3_info(), bt_vorbis_info()
         if lib.bt_wav_probe(str(p).encode(), ctypes.byref(w)) == 0 and w.frames > 0:
             out.append(("wav", w))
         elif lib.bt_flac_probe(str(p).encode(), ctypes.byref(f)) == 0 and f.frames_bytes > 0:
             out.append(("flac", f))
         elif lib.bt_mp3_probe(str(p).encode(), ctypes.byref(m)) == 0 and m.n_samples > 0:
             out.append(("mp3", m))
+        elif lib.bt_vorbis_probe(str(p).encode(), ctypes.byref(v)) == 0 and v.n_samples > 0:
+            out.append(("vorbis", v))
         else:
             out.append((None, None))
     return out
@@ -804,6 +866,46 @@ def mp3_streams(infos, n_frames, main_bytes, out_offsets):
     return (bt_mp3_stream * n)(*[
         bt_mp3_stream(bo[i], main_bytes[i], fo[i], n_frames[i], infos[i].skip, infos[i].n_samples, out_offsets[i],
                       infos[i].channels, infos[i].sample_rate) for i in range(n)])
+
+
+VORBIS_PACKET_BYTES = ctypes.sizeof(bt_vorbis_packet)
+
+
+def _vorbis_tables_at(info) -> int:
+    """Where a staged Vorbis file's decode tables start after its packet bytes."""
+    return (int(info.packet_bytes) + 3) // 4 * 4
+
+
+def vorbis_layout(infos):
+    """Where bt_stage_vorbis_files puts the files `infos` in one byte buffer, as flac_layout does: packet tables
+    (VORBIS_PACKET_BYTES per entry), one int32 status per file, then each file's packet bytes followed by its decode
+    tables."""
+    return _compressed_layout([info.n_packets for info in infos], VORBIS_PACKET_BYTES,
+                              [_vorbis_tables_at(info) + info.table_bytes for info in infos])
+
+
+def stage_vorbis_files(paths, infos, buf_ptr: int, threads: int):
+    """bt_stage_vorbis_files into the byte buffer at host address buf_ptr, laid out as vorbis_layout(infos) says, each
+    file's status stored at its slot of the buffer: (n_packets, packet_bytes, block_samples, status) lists."""
+    n = len(paths)
+    fo, status_at, bo, _ = vorbis_layout(infos)
+    cpaths = (c_char_p * n)(*[str(p).encode() for p in paths])
+    npk, pb, bs = (c_int64 * n)(), (c_int64 * n)(), (c_int64 * n)()
+    status = (c_int32 * n).from_address(buf_ptr + status_at)
+    load().bt_stage_vorbis_files(cpaths, (bt_vorbis_info * n)(*infos), n, c_void_p(buf_ptr), i64_array(bo[:-1]),
+                                 c_void_p(buf_ptr), i64_array(fo[:-1]), pb, npk, bs, threads, status)
+    return list(npk), list(pb), list(bs), list(status)
+
+
+def vorbis_streams(infos, n_packets, packet_bytes, block_samples, out_offsets):
+    """The bt_vorbis_stream table of files staged by stage_vorbis_files (offsets relative to the same buffer), file i's
+    output (infos[i].n_samples samples per channel) from out_offsets[i] on."""
+    fo, _, bo, _ = vorbis_layout(infos)
+    n = len(infos)
+    return (bt_vorbis_stream * n)(*[
+        bt_vorbis_stream(bo[i], packet_bytes[i], bo[i] + _vorbis_tables_at(infos[i]), infos[i].table_bytes, fo[i],
+                         n_packets[i], block_samples[i], infos[i].skip, infos[i].n_samples, out_offsets[i],
+                         infos[i].channels, infos[i].sample_rate) for i in range(n)])
 
 
 def dbn_viterbi(log_densities, beats: int, intervals, log_tempo, pointers):

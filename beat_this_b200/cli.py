@@ -1,8 +1,8 @@
 #!/usr/bin/env python3
 """``beat_this`` command line tool on the H100 engine (reference beat_this/cli.py:22-191: same options, same
 output naming, same ``.beats`` / ``.npy`` files), re-organised around the batched device path: the work list is
-built first, then ``--batch`` files at a time are claimed and handed to ``File2Beats.batch`` (native WAV, FLAC and MP3
-decode: host threads -> pinned ring -> device, groups of one sample rate share launches, decode of the next group overlaps
+built first, then ``--batch`` files at a time are claimed and handed to ``File2Beats.batch`` (native WAV, FLAC, MP3 and Ogg
+Vorbis decode: host threads -> pinned ring -> device, groups of one sample rate share launches, decode of the next group overlaps
 the kernels of the current one); under ``torchrun`` every rank takes every WORLD_SIZE-th task (tasks are
 independent: no collective).  A file that fails costs only itself, and its --touch-first placeholder is removed.
 

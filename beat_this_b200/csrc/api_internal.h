@@ -107,6 +107,8 @@ struct bt_ctx {
   DeviceBuffer<int64_t> flac_ws;
   // granule records and IMDCT blocks of bt_mp3_decode (grows on demand)
   DeviceBuffer<char> mp3_ws;
+  // packet spectra and blocks, floor posts and residue classifications of bt_vorbis_decode (grows on demand)
+  DeviceBuffer<char> vorbis_ws;
   // pinned staging + device tables
   StageSlot stage[kStageSlots];
   int stage_next = 0;

@@ -1,10 +1,6 @@
 // C ABI (include/beatthis.h): native MP3 input -- bt_mp3_probe and bt_stage_mp3_files on the host, bt_mp3_decode on
 // the device (kernels_mp3.cu), and the host test hook bt_debug_mp3_decode_host.  Header parsing, the Huffman walk and
 // the filter banks are mp3.cuh's, shared by all of them.
-#include <fcntl.h>
-#include <sys/stat.h>
-#include <unistd.h>
-
 #include <algorithm>
 #include <atomic>
 #include <cmath>
@@ -219,24 +215,6 @@ Walk walk(const uint8_t* b, int64_t n) {
   return w;
 }
 
-bool read_file(const char* path, std::vector<uint8_t>* out) {
-  const int fd = open(path, O_RDONLY);
-  if (fd < 0) return false;
-  struct stat sb;
-  bool ok = fstat(fd, &sb) == 0;
-  if (ok) {
-    out->resize(static_cast<size_t>(sb.st_size));
-    int64_t got = 0;
-    while (ok && got < sb.st_size) {
-      const ssize_t r = pread(fd, out->data() + got, static_cast<size_t>(sb.st_size - got), got);
-      ok = r > 0;
-      got += r > 0 ? r : 0;
-    }
-  }
-  close(fd);
-  return ok;
-}
-
 void fill_info(const Walk& w, bt_mp3_info* info) {
   const int64_t N = static_cast<int64_t>(w.offsets.size());
   info->sample_rate = w.sample_rate;
@@ -270,7 +248,7 @@ int bt_mp3_probe(const char* path, bt_mp3_info* info) {
   if (!path || !info) return BT_ERR_ARG;
   memset(info, 0, sizeof(*info));
   std::vector<uint8_t> b;
-  if (!read_file(path, &b)) return BT_ERR_IO;
+  if (!bt::read_whole_file(path, &b)) return BT_ERR_IO;
   const Walk w = walk(b.data(), static_cast<int64_t>(b.size()));
   if (w.rc != BT_OK) return w.rc;
   fill_info(w, info);
@@ -289,7 +267,7 @@ int bt_stage_mp3_files(const char* const* paths, const bt_mp3_info* infos, int32
     n_frames[i] = main_bytes[i] = 0;
     int rc = BT_ERR_IO;
     std::vector<uint8_t> b;
-    if (read_file(paths[i], &b)) {
+    if (bt::read_whole_file(paths[i], &b)) {
       const Walk w = walk(b.data(), static_cast<int64_t>(b.size()));
       const int64_t N = static_cast<int64_t>(w.offsets.size());
       if (w.rc == BT_OK && !w.lost_sync && N == in.n_frames && N <= in.max_frames && w.first == in.frames_offset) {

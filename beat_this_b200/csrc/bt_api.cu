@@ -564,7 +564,7 @@ std::vector<ParamSpec> layer_params(const Layer& l, const bt_hparams& hp) {
 // ================================================================================== C ABI
 extern "C" {
 
-int bt_version(void) { return 218; }
+int bt_version(void) { return 219; }
 
 const char* bt_act_dtype(void) {
 #if defined(BT_ACT_BF16)

@@ -285,6 +285,22 @@ void launch_mp3_hybrid(const Mp3StreamDev* streams_dev, int n_streams, int64_t m
 void launch_mp3_synth(const Mp3StreamDev* streams_dev, int n_streams, int64_t max_granules, const float* tables,
                       int mode, void* out, const int32_t* status, cudaStream_t st);
 
+// ---- Ogg Vorbis decoding (kernels_vorbis.cu, vorbis.cuh) -------------------------------------------------------------
+namespace vorbis {
+struct StreamDev;
+}
+// one thread per packet: floors and residues into the packet's scratch
+void launch_vorbis_packets(const vorbis::StreamDev* streams_dev, int n_streams, int64_t max_packets, int32_t* status,
+                           cudaStream_t st);
+// one CTA per packet: floor curves, inverse coupling, floor x residue, IMDCT and window (tables: vorbis.cuh's signal
+// tables)
+void launch_vorbis_blocks(const vorbis::StreamDev* streams_dev, int n_streams, int64_t max_packets, const float* tables,
+                          const int32_t* status, cudaStream_t st);
+// one thread per output sample, max_samples covering every stream's n_samples: overlap-add, trim, output mode (0 mono
+// fp32, 1 float64 [time, ch]); zeros where a stream is not decoded
+void launch_vorbis_output(const vorbis::StreamDev* streams_dev, int n_streams, int64_t max_samples, int mode, void* out,
+                          const int32_t* status, cudaStream_t st);
+
 void launch_f32_to_h16(const float* in, void* out, int64_t n, cudaStream_t st);
 void launch_h16_to_f32(const void* in, float* out, int64_t n, cudaStream_t st);
 // [seqs, L, heads*32] fp32 q,k,v -> packed qkv buffer [seqs*L, 3C] of the activation dtype

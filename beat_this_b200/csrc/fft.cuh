@@ -5,13 +5,13 @@
 
 namespace bt {
 
-__device__ __forceinline__ float2 cmul(float2 a, float2 b) { return make_float2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }
-__device__ __forceinline__ float2 cadd(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }
-__device__ __forceinline__ float2 csub(float2 a, float2 b) { return make_float2(a.x - b.x, a.y - b.y); }
-__device__ __forceinline__ float2 cmul_mi(float2 a) { return make_float2(a.y, -a.x); }  // a * (-i)
+__host__ __device__ __forceinline__ float2 cmul(float2 a, float2 b) { return make_float2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }
+__host__ __device__ __forceinline__ float2 cadd(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }
+__host__ __device__ __forceinline__ float2 csub(float2 a, float2 b) { return make_float2(a.x - b.x, a.y - b.y); }
+__host__ __device__ __forceinline__ float2 cmul_mi(float2 a) { return make_float2(a.y, -a.x); }  // a * (-i)
 
 // in-place 8-point DFT (e^{-2 pi i nk/8}), natural order in and out
-__device__ __forceinline__ void dft8(float2 (&v)[8]) {
+__host__ __device__ __forceinline__ void dft8(float2 (&v)[8]) {
   constexpr float R = 0.70710678118654752f;
   float2 a[4], b[4];
 #pragma unroll
@@ -57,7 +57,7 @@ __device__ __forceinline__ float2 mel_tw(const float2* __restrict__ tw, int j) {
   return (j & (N / 2)) ? make_float2(-w.x, -w.y) : w;
 }
 
-__device__ __forceinline__ void dft4(float2& a0, float2& a1, float2& a2, float2& a3) {
+__host__ __device__ __forceinline__ void dft4(float2& a0, float2& a1, float2& a2, float2& a3) {
   const float2 s0 = cadd(a0, a2), s1 = csub(a0, a2), s2 = cadd(a1, a3), s3 = cmul_mi(csub(a1, a3));
   a0 = cadd(s0, s2); a2 = csub(s0, s2); a1 = cadd(s1, s3); a3 = csub(s1, s3);
 }

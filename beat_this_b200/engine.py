@@ -218,6 +218,17 @@ class Engine:
         self._call("bt_mp3_decode", base, base, streams, len(streams), int(mode), self._dev_ptr(out, need, dtype),
                    c_void_p(buf.data_ptr() + int(status_at)))
 
+    def vorbis_decode(self, buf: torch.Tensor, streams, mode: int, out: torch.Tensor, status_at: int):
+        """bt_vorbis_decode of the Ogg Vorbis files staged in the uint8 device tensor `buf` as _lib.vorbis_layout lays
+        them out (streams: _lib.vorbis_streams); their statuses, read and written, sit at byte status_at of buf.  out:
+        fp32 (BT_VORBIS_MONO_F32) or float64 (BT_VORBIS_CHANNELS_F64) device tensor."""
+        dtype = torch.float32 if mode == _lib.BT_VORBIS_MONO_F32 else torch.float64
+        base = self._dev_ptr(buf, dtype=torch.uint8)
+        need = max((s.out_offset + s.n_samples * (1 if mode == _lib.BT_VORBIS_MONO_F32 else s.channels)
+                    for s in streams), default=0)
+        self._call("bt_vorbis_decode", base, base, streams, len(streams), int(mode), self._dev_ptr(out, need, dtype),
+                   c_void_p(buf.data_ptr() + int(status_at)))
+
     def logmel_cat(self, audio: torch.Tensor, sample_offsets):
         """audio: flat fp32 device tensor; returns (spect [total_frames,128], frame_offsets)."""
         fo = self.frame_offsets(sample_offsets)

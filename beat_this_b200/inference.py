@@ -428,11 +428,11 @@ class File2Beats(Audio2Beats):
     def batch(self, audio_paths, on_error: str = "raise"):
         """Many files per call.  WAV files are read, mixed to mono and cast by the native host threads straight into
         the pinned staging ring (no numpy round trip); FLAC files (with a known length) are staged as frame bytes and
-        decoded and mixed on the device (bt_flac_decode), and so are MP3 files (bt_mp3_decode); other containers go
-        through load_audio.  Files of equal container and sample rate share groups.  on_error: "raise", or "skip" (a
-        file that cannot be loaded or processed yields None instead of aborting the call -- the behaviour of the
-        reference's per-file loop, cli.py:185-190); a FLAC or MP3 file with a malformed frame raises RuntimeError naming
-        it, or yields None."""
+        decoded and mixed on the device (bt_flac_decode), and so are MP3 files (bt_mp3_decode) and Ogg Vorbis files
+        (bt_vorbis_decode); other containers go through load_audio.  Files of equal container and sample rate share
+        groups.  on_error: "raise", or "skip" (a file that cannot be loaded or processed yields None instead of
+        aborting the call -- the behaviour of the reference's per-file loop, cli.py:185-190); a FLAC, MP3 or Ogg Vorbis
+        file with a malformed frame or packet raises RuntimeError naming it, or yields None."""
         if on_error not in ("raise", "skip"):
             raise ValueError("on_error must be 'raise' or 'skip'")
         paths = [str(p) for p in audio_paths]
@@ -453,7 +453,7 @@ class File2Beats(Audio2Beats):
                     for j, (k, r) in enumerate(zip(idx[lo:hi], self._finish(res))):
                         if status is not None and status[j] != 0:
                             if on_error == "raise":
-                                raise RuntimeError(f'Could not decode "{paths[k]}": malformed {_NAME[kind]} frames')
+                                raise RuntimeError(f'Could not decode "{paths[k]}": malformed {_NAME[kind]}')
                             r = None
                         out[k] = r
             except Exception:
@@ -515,7 +515,7 @@ class File2Beats(Audio2Beats):
                     status = pipe.last_status
                     for j, k in enumerate(idx[lo:hi]):
                         if status is not None and status[j] != 0:
-                            raise RuntimeError(f'Could not decode "{paths[k]}": malformed {_NAME[kind]} frames')
+                            raise RuntimeError(f'Could not decode "{paths[k]}": malformed {_NAME[kind]}')
                         out[k] = (beat[fo[j] : fo[j + 1]], down[fo[j] : fo[j + 1]])
             finally:
                 pipe.drain()
@@ -531,16 +531,17 @@ class File2Beats(Audio2Beats):
 def _n_samples(info) -> int:
     if isinstance(info, _lib.bt_wav_info):
         return int(info.frames)
-    return int(info.n_samples) if isinstance(info, _lib.bt_mp3_info) else int(info.total_samples)
+    return int(info.n_samples) if isinstance(info, (_lib.bt_mp3_info, _lib.bt_vorbis_info)) else int(info.total_samples)
 
 
 # the BeatPipeline route and the error-message name of each native container
-_SUBMIT = {"wav": lambda p: p.submit_wavs, "flac": lambda p: p.submit_flacs, "mp3": lambda p: p.submit_mp3s}
-_NAME = {"flac": "FLAC", "mp3": "MP3"}
+_SUBMIT = {"wav": lambda p: p.submit_wavs, "flac": lambda p: p.submit_flacs, "mp3": lambda p: p.submit_mp3s,
+           "vorbis": lambda p: p.submit_vorbis}
+_NAME = {"flac": "FLAC frames", "mp3": "MP3 frames", "vorbis": "Ogg Vorbis packets"}
 
 
 def _native_groups(paths, raise_short: bool):
-    """The files the native readers take, by (container, sample rate) in sorted order: ({("wav" | "flac" | "mp3", sr):
+    """The files the native readers take, by (container, sample rate) in sorted order: ({("wav" | "flac" | "mp3" | "vorbis", sr):
     ([index, ...], [probe info, ...])}, set of indices of files too short to run).  A clip needs more than 512 samples at 22.05 kHz (reflect padding
     of the STFT): a shorter one raises ValueError under raise_short, else it is marked bad (not retried through
     load_audio).  A FLAC file whose STREAMINFO leaves the length unknown goes to load_audio."""

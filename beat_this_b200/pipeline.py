@@ -254,6 +254,21 @@ class BeatPipeline:
         self._submit_compressed(so, _lib.mp3_layout(infos), stage, self.engine.mp3_decode, len(paths), sr, want,
                                 chunking)
 
+    def submit_vorbis(self, paths, infos, sr: int, want: str = "beats", chunking: tuple = DEFAULT_CHUNKING):
+        """paths: list of str; infos: list of bt_vorbis_info (all `sr` Hz) from _lib.probe_audio; chunking as in
+        submit_signals.  Host threads stage the audio packets, packet tables and decode tables, the device decodes them
+        and mixes to mono (bt_vorbis_decode), and the group runs on as submit_wavs's.  A file that fails to stage or
+        decode runs as zeros of its probed length; `last_status` gives every file's status when the group is
+        collected."""
+
+        def stage(buf_ptr):
+            npk, pb, bs, status = _lib.stage_vorbis_files(paths, infos, buf_ptr, self.host_threads)
+            return _lib.vorbis_streams(infos, npk, pb, bs, so[:-1]), status
+
+        so = _lib.offsets(info.n_samples for info in infos)
+        self._submit_compressed(so, _lib.vorbis_layout(infos), stage, self.engine.vorbis_decode, len(paths), sr, want,
+                                chunking)
+
     def _submit_compressed(self, so, layout, stage, decode, n_files, sr, want, chunking):
         """One group of compressed files: so, their sample offsets; layout, where the staged frame tables, statuses and
         frame data sit (_lib.flac_layout, _lib.mp3_layout); stage(host address) fills a pinned buffer and returns (streams,
@@ -273,7 +288,10 @@ class BeatPipeline:
             streams, status = stage(s.flac_host.data_ptr())
             for i, st in enumerate(status):
                 if st != 0:
-                    streams[i].n_frames = 0
+                    if hasattr(streams[i], "n_packets"):
+                        streams[i].n_packets = 0
+                    else:
+                        streams[i].n_frames = 0
             t1 = time.perf_counter()
             self._enqueue(idx, s, so, int(sr), want, chunking, (decode, streams, status_at, total))
             self.stats["stage_s"] += t1 - t0

@@ -5,10 +5,10 @@ reference defaults it runs the model path's fused sm_90a kernel (frame -> Hann -
 128-band slaney mel -> log1p(1000 x)) through ``bt_logmel``; any other analysis parameters run the general kernel
 through ``bt_logmel_config`` on the tables ``MelTables`` builds.
 ``load_audio`` (preprocessing.py:6-24) walks the reference's decoder chain (torchaudio, soundfile, madmom -- whichever
-is installed), then the native FLAC and MP3 decoders (``bt_flac_decode``, ``bt_mp3_decode`` on the current CUDA device)
-and then two dependency-free WAV readers; the batched File2Beats path reads WAV, FLAC and MP3 files natively
-(``bt_stage_wav_files``, ``bt_flac_decode``, ``bt_mp3_decode``) and only falls back to this function for other
-containers.
+is installed), then the native FLAC, MP3 and Ogg Vorbis decoders (``bt_flac_decode``, ``bt_mp3_decode``,
+``bt_vorbis_decode`` on the current CUDA device) and then two dependency-free WAV readers; the batched File2Beats path
+reads WAV, FLAC, MP3 and Ogg Vorbis files natively (``bt_stage_wav_files``, ``bt_flac_decode``, ``bt_mp3_decode``,
+``bt_vorbis_decode``) and only falls back to this function for other containers.
 """
 from __future__ import annotations
 
@@ -139,11 +139,44 @@ def _decode_mp3_native(path, dtype):
     return (wav.reshape(n, ch) if ch > 1 else wav).astype(dtype, copy=False), int(info.sample_rate)
 
 
+def _decode_vorbis_native(path, dtype):
+    """An Ogg Vorbis file decoded on the current CUDA device (bt_vorbis_decode): float64 samples, [time] or
+    [time, channels]."""
+    import ctypes
+
+    from . import _lib
+
+    info = _lib.bt_vorbis_info()
+    code = _lib.load().bt_vorbis_probe(str(path).encode(), ctypes.byref(info))
+    if code != 0:
+        raise ValueError("not an Ogg Vorbis stream" if code == -6 else "cannot read the file")
+    if not torch.cuda.is_available():
+        raise RuntimeError("no CUDA device to decode Ogg Vorbis on")
+    from .engine import Engine
+
+    fo, status_at, bo, total = _lib.vorbis_layout([info])
+    host = np.zeros(max(total, 1), dtype=np.uint8)
+    npk, pb, bs, status = _lib.stage_vorbis_files([path], [info], host.ctypes.data, 1)
+    if status[0] != 0:
+        raise RuntimeError("malformed Ogg Vorbis packets")
+    n, ch = info.n_samples, info.channels
+    dev = torch.device("cuda", torch.cuda.current_device())
+    buf = torch.from_numpy(host).to(dev)
+    out = torch.empty(max(n * ch, 1), dtype=torch.float64, device=dev)
+    Engine.shared(dev).vorbis_decode(buf, _lib.vorbis_streams([info], npk, pb, bs, [0]), _lib.BT_VORBIS_CHANNELS_F64,
+                                     out, status_at)
+    if int(buf[status_at : status_at + 4].view(torch.int32).item()) != 0:
+        raise RuntimeError("malformed Ogg Vorbis packets")
+    wav = out[: n * ch].cpu().numpy()
+    return (wav.reshape(n, ch) if ch > 1 else wav).astype(dtype, copy=False), int(info.sample_rate)
+
+
 # tried in this order; the first three are the reference's chain (preprocessing.py:6-24), the rest need nothing beyond
 # this package, scipy and the standard library and keep FLAC and WAV input working where none of those packages has a
 # decoder
 AUDIO_BACKENDS = (("torchaudio", _decode_torchaudio), ("soundfile", _decode_soundfile), ("madmom", _decode_madmom),
                   ("native FLAC", _decode_flac_native), ("native MP3", _decode_mp3_native),
+                  ("native Ogg Vorbis", _decode_vorbis_native),
                   ("scipy.io.wavfile", _decode_wav_scipy),
                   ("wave", _decode_wav_stdlib))
 
@@ -157,8 +190,8 @@ def load_audio(path, dtype="float64"):
             return decode(path, dtype)
         except Exception as e:  # missing package, missing codec, unreadable file: next backend
             tried.append(f"{name}: {type(e).__name__}" + (f" ({e})" if name.startswith("native") else ""))
-    raise RuntimeError(f'Could not load audio from "{path}". Without torchaudio, soundfile or madmom, FLAC and MP3 '
-                       "(MPEG-1 Layer III; both on a CUDA device) and WAV are the formats read. (" + "; ".join(tried)
+    raise RuntimeError(f'Could not load audio from "{path}". Without torchaudio, soundfile or madmom, FLAC, MP3 '
+                       "(MPEG-1 Layer III) and Ogg Vorbis (all on a CUDA device) and WAV are the formats read. (" + "; ".join(tried)
                        + ")")
 
 

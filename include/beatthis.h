@@ -38,7 +38,7 @@ extern "C" {
 #define BT_ERR_STATE (-3)
 #define BT_ERR_PARAM (-4)
 #define BT_ERR_IO (-5)     /* file could not be opened / read */
-#define BT_ERR_FORMAT (-6) /* not a file of the container the probe reads (RIFF/WAVE, FLAC, MP3) that this library decodes
+#define BT_ERR_FORMAT (-6) /* not a file of the container the probe reads (RIFF/WAVE, FLAC, MP3, Ogg Vorbis) that this library decodes
                             * (caller falls back to another decoder) */
 
 #define BT_DTYPE_F32 0  /* fp32 CUDA-core kernels: the reference's float16=False numerics   */
@@ -376,6 +376,96 @@ int bt_mp3_decode(bt_ctx* ctx, const uint8_t* bytes_dev, const bt_mp3_frame* fra
 int bt_debug_mp3_decode_host(const uint8_t* bytes_host, const bt_mp3_frame* frames_host,
                              const bt_mp3_stream* streams_host, int32_t n_streams, int32_t mode, void* out_host,
                              int32_t* status_host);
+
+/* ---- Ogg Vorbis (ABI 2.19): native decoding of Vorbis I audio in an Ogg stream, on the device -------------------------
+ * The same three steps: bt_vorbis_probe reads the pages and the three Vorbis headers (host), bt_stage_vorbis_files
+ * reassembles each file's audio packets and builds its decode tables (host threads), bt_vorbis_decode decodes every
+ * packet of many files in one call (device).  1 to 8 channels, block sizes 64 .. 8192, floor type 1, residue types 0, 1
+ * and 2.  Floor type 0, more than one logical stream (multiplexed or chained files), a first stream that is not Vorbis
+ * (Opus, Ogg FLAC, Speex) and invalid header values are refused (BT_ERR_FORMAT). */
+typedef struct bt_vorbis_info {
+  int32_t sample_rate;
+  int32_t channels;        /* 1 .. 8 */
+  int32_t blocksize0;      /* short and long block sizes */
+  int32_t blocksize1;
+  int64_t n_packets;       /* audio packets: the packet-table entries bt_stage_vorbis_files writes at most */
+  int64_t packet_bytes;    /* bound on the audio packets' bytes */
+  int64_t table_bytes;     /* the decode tables' bytes */
+  int64_t skip;            /* decoded samples dropped at the start (front trim by the first audio page's granule) */
+  int64_t n_samples;       /* output samples per channel, after both trims */
+} bt_vorbis_info;
+
+/* Read the Ogg pages of a file from byte 0 (capture pattern, version 0, CRC-32 of the header pages, lacing, packets
+ * spanning pages) and its identification, comment and setup headers, validating the setup completely; then walk the
+ * page headers to the end.  A partial last page is dropped, and the output ends at the granule position of the last
+ * whole page.  Host only.  BT_ERR_IO: cannot open or read; BT_ERR_FORMAT: as above. */
+int bt_vorbis_probe(const char* path, bt_vorbis_info* info);
+
+/* One audio packet of a staged Vorbis stream. */
+typedef struct bt_vorbis_packet {
+  int64_t byte_offset;     /* its bytes in the stream's packet bytes */
+  int64_t end_sample;      /* decoded samples complete once it is decoded: its own are [the previous one's, this) */
+  int64_t block_offset;    /* the block sizes of the stream's packets before it (its scratch) */
+  int32_t bytes;
+  uint8_t mode;            /* its mode number (as read; the decode refuses one >= the mode count) */
+  uint8_t blockflag;       /* 1: a long block */
+  uint8_t prev_long;       /* window flags of a long block (0 for a short one) */
+  uint8_t next_long;
+} bt_vorbis_packet;
+
+/* Read n_files probed Vorbis files on n_threads host threads (<= 0: all), checking every page's CRC and sequence number:
+ * file i's audio packets, back to back (at most infos[i].packet_bytes), go to bytes_dst + byte_offsets[i], its decode
+ * tables (infos[i].table_bytes) right after them at the next multiple of 4 bytes, its packet table to packets_dst +
+ * packet_offsets[i] (infos[i].n_packets entries); the packet bytes to packet_bytes[i], the packet count to n_packets[i]
+ * and the sum of the packets' block sizes to block_samples[i].  status[i]: BT_OK, or BT_ERR_IO (cannot read, a CRC or
+ * sequence mismatch, a walk that disagrees with the probe), which leaves n_packets[i] = 0; the call returns BT_ERR_IO
+ * when a file failed. */
+int bt_stage_vorbis_files(const char* const* paths, const bt_vorbis_info* infos, int32_t n_files, uint8_t* bytes_dst,
+                          const int64_t* byte_offsets, bt_vorbis_packet* packets_dst, const int64_t* packet_offsets,
+                          int64_t* packet_bytes, int64_t* n_packets, int64_t* block_samples, int32_t n_threads,
+                          int32_t* status);
+
+/* One stream of a bt_vorbis_decode call (host table). */
+typedef struct bt_vorbis_stream {
+  int64_t byte_offset;    /* its packet bytes start at bytes_dev + byte_offset ...                  */
+  int64_t byte_count;     /* ... and have this many bytes                                           */
+  int64_t table_offset;   /* its decode tables start at bytes_dev + table_offset (a multiple of 4)  */
+  int64_t table_bytes;
+  int64_t packet_offset;  /* its packet table starts at packets_dev + packet_offset                  */
+  int64_t n_packets;
+  int64_t block_samples;  /* the sum of its packets' block sizes                                    */
+  int64_t skip;           /* decoded samples dropped at the start                                   */
+  int64_t n_samples;      /* output samples per channel from there                                  */
+  int64_t out_offset;     /* element of out_dev where its output starts                             */
+  int32_t channels;       /* 1 .. 8                                                                 */
+  int32_t sample_rate;
+} bt_vorbis_stream;
+
+#define BT_VORBIS_MONO_F32 BT_FLAC_MONO_F32         /* fp32((sum over channels of double(s_c)) / channels)        */
+#define BT_VORBIS_CHANNELS_F64 BT_FLAC_CHANNELS_F64 /* double(s_c) [time, ch]                                     */
+
+/* Decode n_streams Vorbis streams on the device in fp32 (no clipping, no rounding to integers): floor1 and residue
+ * decode, inverse coupling, floor x residue, IMDCT, window and overlap-add; then decoded samples [skip, skip +
+ * n_samples) in the mode's output.  status_dev (n_streams int32, device) is read and written as bt_flac_decode's: a
+ * stream whose entry is not BT_OK is not decoded and is zero-filled.  A packet cut short follows the specification's
+ * end-of-packet rules (every floor unused when it ends in the floors, the rest of the residue zero when it ends in the
+ * residue).  A mode number >= the mode count, a codeword a book does not have and a packet entry outside its stream
+ * or out of step with the one before store BT_ERR_IO and zero-fill the stream.  Needs a scratch of 4.5 n + 264 bytes
+ * per packet of block size n and channel (about 9.3 bytes per output sample and channel at blocks 256 / 2048: 1.6 GB
+ * for 64 stereo clips of 30 s at 44.1 kHz), kept by the ctx and grown on demand.  Three launches at most, counted and
+ * profiled as "vorbis_packets" and "vorbis_blocks" (when a stream has a packet) and "vorbis_output" (when a stream has
+ * an output sample; streams that are not decoded are zero-filled by it), enqueued on `stream`.  BT_ERR_ARG before
+ * anything is enqueued: n_streams < 0 or > 65535, an unknown mode, a NULL pointer (n_streams > 0), a negative count or
+ * offset, a table offset that is not a multiple of 4, channels outside 1..8, a sample rate <= 0. */
+int bt_vorbis_decode(bt_ctx* ctx, const uint8_t* bytes_dev, const bt_vorbis_packet* packets_dev,
+                     const bt_vorbis_stream* streams_host, int32_t n_streams, int32_t mode, void* out_dev,
+                     int32_t* status_dev, void* stream);
+
+/* Test hook: bt_vorbis_decode's arithmetic on the host, through the same per-lane functions (vorbis.cuh); host memory,
+ * the same contract otherwise. */
+int bt_debug_vorbis_decode_host(const uint8_t* bytes_host, const bt_vorbis_packet* packets_host,
+                                const bt_vorbis_stream* streams_host, int32_t n_streams, int32_t mode, void* out_host,
+                                int32_t* status_host);
 
 /* ---- the hot path ------------------------------------------------------------------------- */
 
